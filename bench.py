@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- queries/s of the brute-force cosine hot path on B200 (BASELINE.json configs[1]).
+"""bench.py -- queries/s of the brute-force cosine hot path on H100 (BASELINE.json configs[1]).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port)
+    python bench.py --steps K --dump-outputs DIR             # + the last timed step's results as DIR/<name>.npy
 
 A "step" is one batch search of B=1024 queries over the whole resident corpus
 (10M x 768 fp32 at N=1).  `value` is measured with every input already in HBM
@@ -31,6 +32,35 @@ sys.path.insert(0, ROOT)
 
 SEED_CORPUS = 0xC05DA7A + 2
 SEED_QUERY = 0xC05DA7A + 102
+# NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth and dense f16/bf16 tensor rate -- roofline denominators when no
+# measured peak is at hand; never reported as reached
+H100_HBM_GBS = 3350.0
+H100_F16_TFLOPS = 989.0
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, **arrays):
+    """arrays -> out_dir/<name>.npy, float32 / float64 only, at most DUMP_LIMIT_BYTES in all (checked before anything is
+    written).  The callers pass what the timed path returned in its last step: ids and counts as float64 (exact for u32),
+    scores as float32."""
+    for name, a in arrays.items():
+        if a.dtype not in (np.float32, np.float64):
+            raise ValueError(f"dump_outputs: {name} is {a.dtype}, not float32 / float64")
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise ValueError(f"dump_outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
+def dump_device_results(args, d_ids, d_scores, d_counts):
+    """--dump-outputs: the device result buffers of the last timed step (ids [B][k] u32 as float64, scores f32, counts)"""
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ids=d_ids.cpu().numpy().view(np.uint32).astype(np.float64),
+                     scores=d_scores.cpu().numpy().astype(np.float32), counts=d_counts.cpu().numpy().astype(np.float64))
 
 
 def parse_args():
@@ -59,12 +89,16 @@ def parse_args():
     ap.add_argument("--hnsw-variants", action="store_true", help="c3: time every kernel variant (cdb_debug_set_hnsw_flags) on the same graph")
     ap.add_argument("--dump-ids", default=None, help="c3: write the result ids/scores of the batch to this .npz (A/B runs)")
     ap.add_argument("--graph", default=os.path.join(ROOT, "bench_data", "hnsw_100k_128_f16.npz"))
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned (ids, scores and, on the GPU paths, counts of the whole batch) as "
+                         "DIR/<name>.npy (float64 / float32, <= 64 MB); every workload and --impl reference honour it; the inputs "
+                         "are seeded, so two builds can be compared output for output")
     return ap.parse_args()
 
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """samples nvidia-smi during the timed region (B200_PROFILING.md recipe)"""
+    """samples nvidia-smi (read-only queries) during the timed region"""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -177,8 +211,11 @@ def run_reference(args, rank, world):
     times = []
     for _ in range(args.steps):
         t0 = time.perf_counter()
-        orc.brute_topk_f32(corpus, queries, args.k, threads=threads)
+        r_ids, r_scores = orc.brute_topk_f32(corpus, queries, args.k, threads=threads)
         times.append(time.perf_counter() - t0)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ids=np.asarray(r_ids).view(np.uint32).astype(np.float64),
+                     scores=np.asarray(r_scores).astype(np.float32))
     dt = float(np.sum(times))
     qps = args.steps * nqs / dt * (sample_rows / args.rows)
     busy = min(threads, nqs)
@@ -199,7 +236,7 @@ def workload_config(args, world):
     return {"workload": f"brute-force cosine top-{args.k}, {args.rows}x{args.dim} fp32 corpus, batch={args.batch} queries "
                         f"(BASELINE.json configs[1])",
             "rows": args.rows, "dim": args.dim, "batch": args.batch, "k": args.k,
-            "sharding": f"rows/{world}" if world > 1 else "none", "l2": "inputs_exceed_l2 (corpus >> 126 MB)",
+            "sharding": f"rows/{world}" if world > 1 else "none", "l2": "inputs_exceed_l2 (corpus >> 50 MB)",
             "synthetic": "uniform[-1,1) counter RNG, include/cosdata_b200.h"}
 
 
@@ -324,6 +361,8 @@ def run_ours(args, rank, world, local_rank):
 
     t_from = time.perf_counter()
     total_ms, launches_timed = timed(step_device, args.steps, max(args.warmup, 3))
+    if rank == 0:    # the results of the last timed step, before anything else touches the buffers
+        dump_device_results(args, d_ids, d_scores, d_counts)
     # nvidia-smi delivers a sample every 20 ms: a timed region shorter than ~0.2 s is followed by UNTIMED repeats of the
     # same step so that the clock record still comes from this load (the timing above is not affected)
     # (the number of repeats is derived from the max-reduced step time, so every rank issues the same number of collectives)
@@ -341,31 +380,24 @@ def run_ours(args, rank, world, local_rank):
     e2e_value = args.steps * B / (e2e_ms / 1000.0)
 
     # roofline of the dominant kernel (DESIGN.md section 6).  Algorithmic work per launch:
-    #   flops = 2*rows*D*B ; bytes = rows*(D*4+4) + B*D*4 (fp32 corpus) -- the tcgen05 prefilter reads the
+    #   flops = 2*rows*D*B ; bytes = rows*(D*4+4) + B*D*4 (fp32 corpus) -- the wgmma prefilter reads the
     #   fp16 shadow instead (rows*D*2 bytes), reported as shadow_bytes.
     stats = ix.stats()
     tensor_path = stats["tensor_searches"] > 0 and stats["fallback_queries"] == 0
     alg_bytes = rows_local * (D * 4 + 4) + B * D * 4
     alg_flops = 2.0 * rows_local * D * B
     peaks = _peaks()
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    tc_peak = float(peaks.get("bf16_tflops", 1590.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else f"H100 SXM data sheet ({H100_HBM_GBS:.0f} GB/s, {H100_F16_TFLOPS:.0f} TFLOP/s dense f16)"
+    hbm_peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
+    tc_peak = float(peaks.get("bf16_tflops", H100_F16_TFLOPS))
     scan_avg_ms = float(np.mean(scan_ms)) if len(scan_ms) else float("nan")
     traffic, traffic_src = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        ent = tj.get("tensor_scan_kernel" if tensor_path else "scan_f32_kernel", {})
-        if ent.get("rows") == rows_local and ent.get("batch") == B:      # only a capture of THIS launch shape counts
-            traffic, traffic_src = ent.get("dram_bytes_per_launch"), ent.get("source")
-    except Exception:
-        pass
     if tensor_path:
         achieved = alg_flops / (scan_avg_ms / 1000.0) / 1e12
         cand = ix.last_candidate_counts(B)
         roofline = {"bound": "tensor", "achieved": achieved, "peak": tc_peak, "unit": "TFLOP/s", "frac": achieved / tc_peak,
                     "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src + ", dense bf16/fp16 burst",
-                    "kernel": "tensor_scan_kernel (tcgen05 fp16 prefilter, threshold epilogue)", "kernel_ms": scan_avg_ms,
+                    "kernel": "tensor_scan_kernel (wgmma fp16 prefilter, threshold epilogue)", "kernel_ms": scan_avg_ms,
                     "alg_flops_per_launch": alg_flops, "shadow_bytes_per_launch": rows_local * D * 2,
                     "hbm_gbs_on_shadow": rows_local * D * 2 / (scan_avg_ms / 1000.0) / 1e9,
                     "candidates_per_query": {"mean": float(cand.mean()), "max": int(cand.max())},
@@ -424,7 +456,7 @@ def secondary_records(args, ix, cdb, torch, stream, dev, q_host):
     separately, with their own rooflines and clock samples"""
     out = []
     pk = _peaks()
-    hbm = float(pk.get("hbm_gbs", 6650.0))
+    hbm = float(pk.get("hbm_gbs", H100_HBM_GBS))
     B, D, k, rows = args.batch, args.dim, args.k, ix.size
 
     def run(fn, n, flush=None):
@@ -495,7 +527,7 @@ def secondary_records(args, ix, cdb, torch, stream, dev, q_host):
                              "frac": c1_bytes / (cold_ms / 1000.0) / 1e9 / hbm, "alg_bytes_per_launch": c1_bytes,
                              "note": "51 MB per query: warm = L2-resident + launch latency bound; cold = L2 flushed (256 MB write) before every launch, "
                                      "whole step timed (quantize + scan + merge launches), so the HBM fraction is a latency figure"}})
-    # ---- BASELINE.json configs[3] on a 5M shard: quaternary inner product, batch 4096, exact integer scores on tcgen05 kind::i8
+    # ---- BASELINE.json configs[3] on a 5M shard: quaternary inner product, batch 4096, exact integer scores on wgmma u8
     try:
         i8_tops, _ = cdb.tensor_peak(True, dev.index)
         f16_tops, _ = cdb.tensor_peak(False, dev.index)
@@ -521,10 +553,10 @@ def secondary_records(args, ix, cdb, torch, stream, dev, q_host):
                     "value": B4 / (ms4 / 1000.0), "unit": "queries/s", "ms_per_step": ms4, "clocks": clk4,
                     "roofline": {"bound": "tensor", "achieved": ops4 / (kms4 / 1000.0) / 1e12, "peak": i8_tops, "unit": "TOP/s",
                                  "frac": ops4 / (kms4 / 1000.0) / 1e12 / i8_tops, "kernel_ms": kms4, "alg_ops_per_launch": ops4,
-                                 "peak_source": "measured in this run: dense tcgen05 kind::i8 issue-rate probe (csrc/tc_probe.cu); "
-                                                f"the same probe with kind::f16 gives {f16_tops:.0f} TFLOP/s next to the cuBLAS bf16 "
+                                 "peak_source": "measured in this run: dense wgmma u8 issue-rate probe (csrc/tc_probe.cu); "
+                                                f"the same probe with f16 gives {f16_tops:.0f} TFLOP/s next to the cuBLAS bf16 "
                                                 f"{float(pk.get('bf16_tflops', 0)):.0f}",
-                                 "kernel": "tensor_scan_kernel<KIND=1> (tcgen05 kind::i8, exact)", "tensor_path": st4}})
+                                 "kernel": "tensor_scan_kernel<KIND=1> (wgmma u8, exact)", "tensor_path": st4}})
     except Exception as e:
         out.append({"name": "quaternary-quantized inner product (configs[3] shard)", "error": repr(e)})
     # ---- BASELINE.json configs[2] at 1/10 size: HNSW f16, ef_search 128, batch 1024; graph built on the GPU (reference defaults)
@@ -651,6 +683,7 @@ def run_c4(args):
     sampler.start()
     l0 = cdb.kernel_launch_count()
     ms = _timed_single(step, args.steps, max(args.warmup, 3), stream)
+    dump_device_results(args, d_ids, d_scores, d_counts)
     clocks = sampler.stop()
     launches = (cdb.kernel_launch_count() - l0) * args.steps // (args.steps + max(args.warmup, 3))
     nchunks = (B + 2047) // 2048
@@ -660,7 +693,7 @@ def run_c4(args):
     kernel_ms = float(np.sum(scan_ms)) / args.steps
     ops = 2.0 * rows * D * B
     pk = _peaks()
-    peak, _ = cdb.tensor_peak(True, 0)     # dense tcgen05 kind::i8 issue-rate probe, measured in this run (csrc/tc_probe.cu)
+    peak, _ = cdb.tensor_peak(True, 0)     # dense wgmma u8 issue-rate probe, measured in this run (csrc/tc_probe.cu)
     achieved = ops / (kernel_ms / 1000.0) / 1e12
     line = {
         "metric": "queries/sec, quaternary inner product top-10", "value": args.steps * B / (ms / 1000.0), "unit": "queries/s",
@@ -672,9 +705,9 @@ def run_c4(args):
         "e2e": {"value": args.steps * B / (e2e_ms / 1000.0), "unit": "queries/s", "h2d_bytes_per_step": B * D * 4,
                 "d2h_bytes_per_step": B * k * 8 + B * 5, "ms_per_step": e2e_ms / args.steps},
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TOP/s", "frac": achieved / peak, "traffic": None,
-                     "peak_source": "measured in this run: dense tcgen05 kind::i8 issue-rate probe (cdb_debug_tensor_peak); cuBLAS bf16 in "
+                     "peak_source": "measured in this run: dense wgmma u8 issue-rate probe (cdb_debug_tensor_peak); cuBLAS bf16 in "
                                     f"MEASURED_PEAKS.json: {float(pk.get('bf16_tflops', 0)):.0f} TFLOP/s",
-                     "kernel": "tensor_scan_kernel<KIND=1> (tcgen05 kind::i8, exact)", "kernel_ms": kernel_ms,
+                     "kernel": "tensor_scan_kernel<KIND=1> (wgmma u8, exact)", "kernel_ms": kernel_ms,
                      "alg_ops_per_launch": ops, "digit_bytes": rows * D, "tensor_path": st},
         "recall_at_10": 1.0, "recall_note": "exact integer scores; ids identical to the CPU oracle (tests/test_gpu_tensor_u8.py)",
     }
@@ -748,6 +781,7 @@ def run_hnsw(args):
     t_from = time.perf_counter()
     l0 = cdb.kernel_launch_count()
     ms = _timed_single(step, args.steps, max(args.warmup, 3), stream)
+    dump_device_results(args, d_ids, d_scores, d_counts)
     launches = (cdb.kernel_launch_count() - l0) * args.steps // (args.steps + max(args.warmup, 3))
     scan_ms = ix.scan_ms_history(args.steps)
     while time.perf_counter() - t_from < 0.3:      # untimed repeats of the same step: the clock record needs ~0.2 s of this load
@@ -776,7 +810,7 @@ def run_hnsw(args):
     kernel_ms = float(np.mean(scan_ms))
     alg_bytes = evals * (D * 2 + 4) + pops * 64 * 4          # SURVEY 8d: evals*(D*s+4) + pops*(nbrs*4), counted on this graph
     pk = _peaks()
-    hbm = float(pk.get("hbm_gbs", 6650.0))
+    hbm = float(pk.get("hbm_gbs", H100_HBM_GBS))
     ach = alg_bytes / (kernel_ms / 1000.0) / 1e9
     line = {
         "metric": "queries/sec + recall@10, HNSW f16", "value": args.steps * B / (ms / 1000.0), "unit": "queries/s", "n_gpus": 1,
@@ -856,6 +890,7 @@ def run_c3(args):
     t_from = time.perf_counter()
     l0 = cdb.kernel_launch_count()
     ms = _timed_single(step, args.steps, max(args.warmup, 3), stream)
+    dump_device_results(args, d_ids, d_scores, d_counts)
     launches = (cdb.kernel_launch_count() - l0) * args.steps // (args.steps + max(args.warmup, 3))
     scan_ms = ix.scan_ms_history(args.steps)
     while time.perf_counter() - t_from < 0.3:      # untimed repeats of the same step: the clock record needs ~0.2 s of this load
@@ -874,7 +909,7 @@ def run_c3(args):
     kernel_ms = float(np.mean(scan_ms))
     alg_bytes = evals * (D * 2 + 4) + pops * 64 * 4
     pk = _peaks()
-    hbm = float(pk.get("hbm_gbs", 6650.0))
+    hbm = float(pk.get("hbm_gbs", H100_HBM_GBS))
     ach = alg_bytes / (kernel_ms / 1000.0) / 1e9
     prof = None
     if args.hnsw_prof:
@@ -939,7 +974,7 @@ def run_c3(args):
 
 
 def run_c5(args, rank, world, local_rank):
-    """BASELINE.json configs[4]: sharded HNSW, 100M x 768 fp32, batch 4096, 8 x B200 with an NCCL top-k merge.
+    """BASELINE.json configs[4]: sharded HNSW, 100M x 768 fp32, batch 4096, 8 GPUs with an NCCL top-k merge.
     One independent HNSW per shard (12.5M rows per GPU by default), built on the GPU; every rank searches the same
     queries on its shard; one all-gather of the per-shard top-k; merge with the common ordering rule."""
     import torch
@@ -1019,6 +1054,8 @@ def run_c5(args, rank, world, local_rank):
         m_ids, m_scores = step()
     e1.record(stream)
     barrier()
+    if rank == 0:
+        dump_device_results(args, d_ids, d_scores, d_counts)
     clocks = sampler.stop()
     launches = cdb.kernel_launch_count() - l0
     ms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
@@ -1053,7 +1090,7 @@ def run_c5(args, rank, world, local_rank):
     evals, pops = (ev1 - ev0) / max(args.warmup, 3), (pp1 - pp0) / max(args.warmup, 3)
     kernel_ms = float(np.sum(scan_ms)) / args.steps
     alg_bytes = evals * (D * 4 + 4) + pops * 64 * 4
-    hbm = float(_peaks().get("hbm_gbs", 6650.0))
+    hbm = float(_peaks().get("hbm_gbs", H100_HBM_GBS))
     ach = alg_bytes / (kernel_ms / 1000.0) / 1e9
     tb = torch.tensor([t_build], dtype=torch.float64, device=dev)
     if world > 1:

@@ -1,4 +1,4 @@
-"""cosdata_b200 -- B200-native (sm_100a) implementation of cosdata's ANN distance hot path.
+"""cosdata_b200 -- H100-native (sm_90a) implementation of cosdata's ANN distance hot path.
 
 The package is a thin host mirror of the reference's operator surface over the
 C ABI in include/cosdata_b200.h; all compute lives in csrc/*.cu.

@@ -187,7 +187,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} is missing: run `python -m cosdata_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: run `python -m cosdata_b200.build` (nvcc, sm_90a). "
             "There is no CPU fallback for this path.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in PROTOTYPES.items():

@@ -96,7 +96,7 @@ def debug_set_hnsw_flags(flags=0xFFFFFFFF):
 
 
 def tensor_peak(kind_i8=True, device=0, iters=0):
-    """dense tcgen05 issue-rate probe -> (TOP/s or TFLOP/s, ms); the measured peak of kind::i8 / kind::f16 MMAs"""
+    """dense wgmma issue-rate probe -> (TOP/s or TFLOP/s, ms); the measured peak of u8 / f16 MMAs"""
     tops, ms = C.c_double(0), C.c_float(0)
     _check(_lib.load().cdb_debug_tensor_peak(device, 1 if kind_i8 else 0, iters, C.byref(tops), C.byref(ms)))
     return tops.value, ms.value

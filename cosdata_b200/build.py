@@ -1,11 +1,10 @@
-"""Builds libcosdata_b200.so (sm_100a only) in-tree with nvcc.
+"""Builds libcosdata_b200.so (sm_90a, H100) in-tree with nvcc.
 
     python -m cosdata_b200.build [--force] [--verbose]
 
-The shared object is git-ignored but travels to the GPU box with the gpurun
-snapshot.  cudart is linked statically (nvcc default), so the library shares
-the primary CUDA context with any torch in the same process without sharing a
-runtime instance.
+The shared object and the object files are git-ignored build products.  cudart
+is linked statically (nvcc default), so the library shares the primary CUDA
+context with any torch in the same process without sharing a runtime instance.
 """
 import concurrent.futures
 import os
@@ -19,8 +18,9 @@ LIB = os.path.join(HERE, "libcosdata_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]   # wgmma, TMA and setmaxnreg: Hopper-only, no other target
 FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", *GENCODE, "-lineinfo",
     "-ccbin", HOST_CXX, "-Xcompiler", "-fPIC,-O2,-Wall", "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
@@ -38,6 +38,11 @@ def _headers_mtime():
 
 def build(force=False, verbose=False):
     os.makedirs(OBJ, exist_ok=True)
+    # objects compiled with other flags (another architecture) are never reused
+    stamp = os.path.join(OBJ, "flags.txt")
+    want = " ".join([NVCC] + FLAGS)
+    if not os.path.exists(stamp) or open(stamp).read() != want:
+        force = True
     hm = _headers_mtime()
     jobs = []
     for src in _sources():
@@ -67,12 +72,13 @@ def build(force=False, verbose=False):
         raise RuntimeError("nvcc failed")
     objs = [os.path.join(OBJ, src[:-3] + ".o") for src in _sources()]
     if jobs or force or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-ccbin", HOST_CXX, "-gencode", "arch=compute_100a,code=sm_100a",
-               "-o", LIB] + objs
+        cmd = [NVCC, "-shared", "-ccbin", HOST_CXX, *GENCODE, "-o", LIB] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError("link failed")
+    with open(stamp, "w") as f:
+        f.write(want)
     return LIB
 
 

@@ -154,9 +154,9 @@ struct cdb_index {
     float *d_raw = nullptr;       // raw f32 rows (may alias d_codes)
     float *d_raw_mags = nullptr;  // |raw row| (may alias d_mags)
     bool raw_owned = false, raw_mags_owned = false;
-    uint8_t *d_digits = nullptr;   // sub-byte storage unpacked to u8 digits for tcgen05 kind::i8 (tensor_scan_u8.cu)
+    uint8_t *d_digits = nullptr;   // sub-byte storage unpacked to u8 digits for the u8 wgmma (tensor_scan_u8.cu)
     uint32_t digit_pitch = 0;
-    void *d_xh = nullptr;          // fp16 L2-normalised rows for the tcgen05 prefilter (tensor_scan.cu)
+    void *d_xh = nullptr;          // fp16 L2-normalised rows for the wgmma prefilter (tensor_scan.cu)
     uint32_t xh_pitch = 0;         // halfs per shadow row
     uint64_t n_allzero_rows = 0;   // degenerate rows (tensor_scan.cu): all-zero rows score NaN against every query = last
     uint64_t n_odd_rows = 0;       // other degenerate rows (norm 0/inf/NaN/out of range): ride on every candidate list
@@ -860,7 +860,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         return rc;
     }
     const uint32_t pitch = raw ? ix->raw_pitch_elems * 4 : ix->row_pitch;
-    // ---- tcgen05 prefilter + exact re-rank: identical results, far fewer exact dot products.
+    // ---- wgmma prefilter + exact re-rank: identical results, far fewer exact dot products.
     // Needs k proper (non-degenerate) rows for the bound to exist, and few enough odd degenerate rows to carry them on
     // every candidate list (tensor_scan.cu).
     const bool tensor_ok = raw && ix->d_xh && !p->exact_only && nq >= 4 && ix->size >= 16384 && p->k <= 64 &&
@@ -910,7 +910,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         ix->stat_tensor_searches++;
         qsel = sc->qsel.as<uint32_t>();  // the exact scan below only runs (on the device's own decision) for the queries listed there
     }
-    // ---- exact integer scoring on tcgen05 kind::i8: u8 codes in place, sub-byte codes through the digit copy
+    // ---- exact integer scoring on wgmma u8: u8 codes in place, sub-byte codes through the digit copy
     const uint8_t *u8_rows = !raw ? (st == CDB_ST_U8 ? ix->d_codes : ix->d_digits) : nullptr;
     const bool u8_ok = u8_rows && !p->exact_only && (metric == CDB_METRIC_COSINE || metric == CDB_METRIC_DOT_PRODUCT) &&
                        ix->size >= 16384 && p->k <= 64 && tensor_u8_smem_bytes(p->k) <= 227 * 1024 &&
@@ -960,8 +960,8 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
     return CDB_OK;
 }
 
-// Batches are processed in chunks of <= 2048 queries (16 query tiles of 128): 148 SMs then split into 9 whole
-// CTA groups (144 CTAs) for the tensor-core kernels, and per-chunk scratch stays bounded.
+// Batches are processed in chunks of <= 2048 queries (16 query tiles of 128): 132 SMs then split into 8 whole
+// CTA groups (128 CTAs) for the tensor-core kernels, and per-chunk scratch stays bounded.
 static cdb_status search_device_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
                                        uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s) {
     // the handle's scratch arena is reused by every search: a search enqueued on a different stream than the previous

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libcosdata_b200 (sm_100a only).
+// common.cuh -- shared device/host helpers for libcosdata_b200 (sm_90a only).
 #pragma once
 
 #include <cuda_fp16.h>

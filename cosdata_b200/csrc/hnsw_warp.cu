@@ -18,9 +18,8 @@
 //
 // f16 chain.  dot_product_f16 = sum_i f32(x_i) * f32(y_i), sequential, no FMA in the reference.  The product of two
 // halfs is exact in f32 (11 + 11 significand bits, exponent range far inside f32), so fma(x, y, s) rounds exactly once
-// at the same place as s + (x * y): one fused multiply-add per element instead of FMUL + FADD, bit-identical.  On sm_100
-// that FMA is FHFMA (fma.rn.f32.f16: 16-bit operands read from packed registers, widened exactly, one f32 rounding), so the
-// chain costs 1 instruction per element (+ 2 LDS.128 per 8 elements) and needs neither conversions nor an f32 query copy.
+// at the same place as s + (x * y): one fused multiply-add per element instead of FMUL + FADD, bit-identical.  The 16-bit
+// operands are widened exactly from the packed registers (scorers.cuh, widen16), so no f32 query copy is needed.
 #include <cstdlib>
 
 #include "hnsw_traverse.cuh"
@@ -53,7 +52,7 @@ __host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, ui
     uint32_t r = (spec ? HW_STAGE_BYTES_SPEC : HW_STAGE_BYTES) / c.stage_pitch;
     c.stage_rows = r > 32 ? 32 : (r ? r : 1u);      // one lane scores one staged row
     uint32_t o = round_up(row_pitch, 16);
-    c.off_q32 = o;            // (the f32 copy of the query is gone: FHFMA reads the f16 / bf16 code directly)
+    c.off_q32 = o;            // (no f32 copy of the query: the chain widens the f16 / bf16 code directly)
     c.off_qkeys = o;          o += 2 * c.EFP * 8;
     c.off_rkeys = o;          o += c.EFP * 8;
     c.off_nkeys = o;          o += HN_MAX_TAKE * 8;
@@ -115,19 +114,14 @@ __device__ __forceinline__ void hw_mbar_wait(uint32_t bar, uint32_t parity) {
     } while (!ok);
 }
 
-// sum_i f32(q_i) * f32(row_i), sequential, on FHFMA: sm_100's mixed-precision FMA (PTX fma.rn.f32.f16 / .bf16) takes the two
-// 16-bit operands straight out of the packed registers (.H0/.H1 selectors), widens them exactly and rounds a*b + c once in
-// f32 -- the same single rounding as the FFMA of the converted values, and (the product of two halfs / two bf16 values being
-// exact in f32) the same result as the reference's multiply-then-add.  No conversion instructions, no f32 copy of the query:
-// 8 FHFMA + 2 LDS.128 per 8 elements instead of 8 FFMA + 8 conversions + 3 LDS.128.
+// sum_i f32(q_i) * f32(row_i), sequential: both 16-bit operands widened exactly, then one FFMA rounding a*b + c once in
+// f32 -- (the product of two halfs / two bf16 values being exact in f32) the same result as the reference's
+// multiply-then-add.  No f32 copy of the query: 8 FFMA + their conversions + 2 LDS.128 per 8 elements.
 // The chain is latency bound (one dependent FMA per element), so the shared-memory operands of the NEXT 16 elements are
 // loaded before the current 16 FMAs issue (explicit double buffering: ptxas does not pipeline this loop itself).
 template <int FAST>
 __device__ __forceinline__ float hw_fhfma(float s, uint32_t q, uint32_t r, bool hi) {
-    const unsigned short a = (unsigned short)(hi ? q >> 16 : q & 0xFFFFu), b = (unsigned short)(hi ? r >> 16 : r & 0xFFFFu);
-    if (FAST == 1) asm("fma.rn.f32.f16 %0, %1, %2, %0;" : "+f"(s) : "h"(a), "h"(b));
-    else asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(s) : "h"(a), "h"(b));
-    return s;
+    return FAST == 1 ? fhfma16<false>(s, q, r, hi) : fhfma16<true>(s, q, r, hi);
 }
 template <int FAST>
 __device__ __forceinline__ float hw_chain8(float s, const uint4 &q, const uint4 &r) {

@@ -185,7 +185,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
                                       std::vector<const uint32_t *> *out_ch, ReplicaGraphDev *out_md, std::vector<uint8_t> *out_failed,
                                       cudaStream_t s);
 
-// ---- tensor_scan.cu (tcgen05 prefilter)
+// ---- tensor_scan.cu (wgmma prefilter)
 constexpr uint32_t TS_MAX_ODD = 64;   // degenerate rows that are not all-zero ride on every candidate list; more -> no prefilter
 constexpr uint32_t TS_DEG_WORDS = 2 + TS_MAX_ODD;
 cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t n, uint32_t dim,
@@ -210,7 +210,7 @@ cdb_status tensor_scan_i8_device(const uint8_t *d_x, const uint8_t *d_q, uint32_
 cdb_status select_fallback_device(const uint32_t *d_cnt, uint32_t cap, const float *d_qmags, uint32_t n, uint32_t *d_qsel,
                                   uint32_t *d_flags, cudaStream_t s);
 
-// ---- tensor_scan_u8.cu (exact integer scoring on tcgen05 kind::i8)
+// ---- tensor_scan_u8.cu (exact integer scoring on wgmma u8)
 size_t tensor_u8_smem_bytes(uint32_t k);
 cdb_status unpack_digits_device(const uint8_t *d_codes, uint32_t row_pitch, uint64_t n, uint32_t dim, int res, uint8_t *d_out,
                                 uint32_t out_pitch, cudaStream_t s);

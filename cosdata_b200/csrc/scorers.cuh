@@ -91,17 +91,18 @@ __device__ inline float mag_f32_seq(const float *__restrict__ v, uint32_t n) {
 
 // ------------------------------------------------------------------ f16 / bf16 dot products
 // The reference's `.sum()` is a sequential left fold of f32(x_i) * f32(y_i).  The product of two halfs (11 + 11 significand
-// bits) or two bf16 values (8 + 8) is exact in f32, so s + x*y rounds once -- exactly what a fused multiply-add does.  sm_100
-// has that FMA with 16-bit operands: FHFMA (PTX fma.rn.f32.f16 / fma.rn.f32.bf16) reads the halves straight out of the packed
-// registers (.H0/.H1), widens them exactly (subnormals included) and rounds a*b + c once in f32.  One instruction per element
-// instead of two conversions + FMUL + FADD; bit-identical (tests: every f16 / bf16 arm against the oracle).
+// bits) or two bf16 values (8 + 8) is exact in f32, so s + x*y rounds once -- exactly what a fused multiply-add does: both
+// operands are widened exactly (subnormals included; bf16 is the upper half of an f32) and folded with one FFMA per element
+// instead of FMUL + FADD; bit-identical (tests: every f16 / bf16 arm against the oracle).
 // Rows are 16-byte pitched, so the operands are walked with 128-bit loads; the additions stay strictly in element order.
 template <bool BF16>
+__device__ __forceinline__ float widen16(uint32_t x, bool hi) {
+    if (BF16) return __uint_as_float(hi ? (x & 0xFFFF0000u) : (x << 16));
+    return __half2float(__ushort_as_half((unsigned short)(hi ? x >> 16 : x & 0xFFFFu)));
+}
+template <bool BF16>
 __device__ __forceinline__ float fhfma16(float s, uint32_t x, uint32_t y, bool hi) {
-    const unsigned short a = (unsigned short)(hi ? x >> 16 : x & 0xFFFFu), b = (unsigned short)(hi ? y >> 16 : y & 0xFFFFu);
-    if (BF16) asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(s) : "h"(a), "h"(b));
-    else asm("fma.rn.f32.f16 %0, %1, %2, %0;" : "+f"(s) : "h"(a), "h"(b));
-    return s;
+    return __fmaf_rn(widen16<BF16>(x, hi), widen16<BF16>(y, hi), s);
 }
 template <bool BF16>
 __device__ __forceinline__ float fhfma16x8(float s, const uint4 &x, const uint4 &y) {

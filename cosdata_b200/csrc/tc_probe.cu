@@ -1,11 +1,12 @@
-// tc_probe.cu -- dense tcgen05 issue-rate probe: the roofline denominator of the integer tensor path.
+// tc_probe.cu -- dense wgmma issue-rate probe: the roofline denominator of the integer tensor path.
 //
-// MEASURED_PEAKS.json holds a cuBLAS bf16 figure only; tensor_scan_u8.cu computes on tcgen05.mma.kind::i8, whose peak
-// has no library yardstick in this image.  This kernel measures it directly: every SM keeps one CTA that issues
-// back-to-back M128 x N256 MMAs (K = 32 bytes for kind::i8, 16 halfs for kind::f16) on operand tiles that stay resident
-// in shared memory, alternating two TMEM accumulators, with no loads, no epilogue, no global traffic.  What it reports is
-// the rate the tensor pipe sustains when nothing else limits it -- an upper bound for any real kernel, like the cuBLAS
-// number is for bf16 (the f16 variant of the probe is printed next to the cuBLAS figure as a sanity check).
+// tensor_scan_u8.cu computes on wgmma .s32.u8.u8, whose peak has no library yardstick.  This kernel measures it directly:
+// every SM keeps one CTA of two warpgroups, each issuing back-to-back M64 x N256 MMAs (K = 32 bytes for u8, 16 halfs for
+// f16) on operand tiles that stay resident in shared memory, into its own register accumulator, with no loads, no epilogue,
+// no global traffic.  What it reports is the rate the tensor pipe sustains when nothing else limits it -- an upper bound
+// for any real kernel (the f16 variant of the probe is printed next to it as a sanity check).
+#include <type_traits>
+
 #include "kernels.h"
 #include "tc_common.cuh"
 
@@ -14,74 +15,60 @@ namespace cdb {
 constexpr uint32_t PR_M = 128, PR_N = 256;
 constexpr uint32_t PR_A_BYTES = PR_M * 128, PR_B_BYTES = PR_N * 128;   // one 128-byte swizzle row per matrix row
 
-__device__ __forceinline__ void probe_mma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-
 template <bool I8>
-__global__ void __launch_bounds__(128, 1) tc_probe_kernel(uint32_t iters) {
+__global__ void __launch_bounds__(256, 1) tc_probe_kernel(uint32_t iters, uint32_t *sink) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + PR_A_BYTES + PR_B_BYTES);
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(bar + 1);
     for (uint32_t i = threadIdx.x; i < (PR_A_BYTES + PR_B_BYTES) / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem)[i] = 0x01010101u;
-    const int warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) {
-        mbar_init(smem_u32(bar), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes of the tiles -> visible to the MMA's async proxy
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    if (threadIdx.x == 0) {
-        const uint32_t sa = smem_u32(smem);
-        const uint64_t adesc = make_smem_desc(sa), bdesc = make_smem_desc(sa + PR_A_BYTES);
-        // instruction descriptors as in tensor_scan.cu / tensor_scan_u8.cu
-        const uint32_t idesc = I8 ? ((2u << 4) | ((PR_N >> 3) << 17) | ((PR_M >> 4) << 24))
-                                  : ((1u << 4) | ((PR_N >> 3) << 17) | ((PR_M >> 4) << 24));
-        for (uint32_t it = 0; it < iters; ++it) {
+    const uint32_t wg = threadIdx.x >> 7;
+    const uint32_t sa = smem_u32(smem);
+    const uint64_t adesc = make_smem_desc(sa + wg * (PR_A_BYTES / 2)), bdesc = make_smem_desc(sa + PR_A_BYTES);
+    using Acc = typename std::conditional<I8, uint32_t, float>::type;
+    Acc d[128];
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {   // 4 K-steps of one 128-byte swizzle row, two accumulators alternating
-                if (I8) probe_mma_i8(tmem_base + (it & 1u) * PR_N, adesc + 2 * kk, bdesc + 2 * kk, idesc, 1u);
-                else tcgen05_mma_f16(tmem_base + (it & 1u) * PR_N, adesc + 2 * kk, bdesc + 2 * kk, idesc, 1u);
-            }
+    for (int i = 0; i < 128; ++i) d[i] = 0;
+    for (uint32_t it = 0; it < iters; ++it) {
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {   // 4 K-steps of one 128-byte swizzle row
+            if constexpr (I8) wgmma_u8(d, adesc + 2 * kk, bdesc + 2 * kk);
+            else wgmma_f16(d, adesc + 2 * kk, bdesc + 2 * kk);
         }
-        tcgen05_commit(smem_u32(bar));
-        mbar_wait(smem_u32(bar), 0);
+        wgmma_commit();
+        wgmma_wait<1>();
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+    wgmma_wait<0>();
+    uint32_t x = 0;
+#pragma unroll
+    for (int i = 0; i < 128; ++i) {
+        if constexpr (I8) x ^= d[i]; else x ^= __float_as_uint(d[i]);
     }
+    if (x == 0x9E3779B9u) sink[0] = x;   // keeps the accumulators (and so the MMAs) observable
 }
 
 template <bool I8>
 static cdb_status run_probe(int sm_count, uint32_t iters, float *ms) {
     auto kern = tc_probe_kernel<I8>;
-    const size_t smem = 1024 + PR_A_BYTES + PR_B_BYTES + 64;
+    const size_t smem = 1024 + PR_A_BYTES + PR_B_BYTES;
     CDB_ALLOW_SMEM(kern, smem);
     cudaEvent_t e0, e1;
     CDB_CUDA_TRY(cudaEventCreate(&e0));
     CDB_CUDA_TRY(cudaEventCreate(&e1));
-    kern<<<sm_count, 128, smem, 0>>>(iters / 8 + 1);   // warm-up
+    uint32_t *sink = nullptr;
+    CDB_CUDA_TRY(cudaMalloc(&sink, 4));
+    kern<<<sm_count, 256, smem, 0>>>(iters / 8 + 1, sink);   // warm-up
     CDB_LAUNCH_CHECK();
     CDB_CUDA_TRY(cudaEventRecord(e0, 0));
-    kern<<<sm_count, 128, smem, 0>>>(iters);
+    kern<<<sm_count, 256, smem, 0>>>(iters, sink);
     CDB_LAUNCH_CHECK();
     CDB_CUDA_TRY(cudaEventRecord(e1, 0));
     CDB_CUDA_TRY(cudaEventSynchronize(e1));
     CDB_CUDA_TRY(cudaEventElapsedTime(ms, e0, e1));
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
+    cudaFree(sink);
     return CDB_OK;
 }
 

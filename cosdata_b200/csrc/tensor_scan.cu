@@ -1,25 +1,26 @@
-// tensor_scan.cu -- tcgen05 prefilter for the batched brute-force cosine scan (S1, large B).
+// tensor_scan.cu -- wgmma prefilter for the batched brute-force cosine scan (S1, large B).
 //
 // The dense query x corpus product of configs C2/C5 genuinely is a contraction, so it runs
-// on the 5th-gen tensor cores: fp16 copies of the L2-normalised rows ("shadow", built at
-// append time) and of the normalised queries are multiplied with tcgen05.mma.kind::f16
-// (fp32 accumulators in TMEM).  The result is an APPROXIMATE cosine a(q,x) with a rigorous
-// error bound eps (DESIGN.md section 5); it is used only to discard rows that provably
-// cannot be in the exact top-k:
-//     every epilogue thread owns one query (one TMEM lane) and keeps, in shared memory,
-//     the k best approximate scores it has seen (A_k = the k-th).  k rows with a >= A_k
-//     exist, so the exact k-th best score is >= A_k - eps, so a row can be in the exact
-//     top-k only if a >= A_k - 2*eps.  Rows passing that test are appended to the query's
-//     candidate list; A_k is shared between CTAs through a global atomicMax.
+// on the tensor cores: fp16 copies of the L2-normalised rows ("shadow", built at append time)
+// and of the normalised queries are multiplied with wgmma .f32.f16.f16 (fp32 accumulators in
+// registers).  The result is an APPROXIMATE cosine a(q,x) with a rigorous error bound eps
+// (DESIGN.md section 5); it is used only to discard rows that provably cannot be in the exact top-k:
+//     every query keeps the maximum approximate score of each of NG disjoint row classes; the k-th
+//     largest class maximum A_k is a lower bound of the k-th best approximate score, so the exact
+//     k-th best score is >= A_k - eps, and a row can be in the exact top-k only if a >= A_k - 2*eps.
+//     Rows passing that test are appended to the query's candidate list; the class maxima are
+//     shared between CTAs through global atomicMax.
 // The candidates are then re-scored by rerank_f32_kernel with the reference's exact
 // arithmetic, so the final ids/scores are bit-identical to the exact scan.
 //
-// Kernel anatomy (one CTA per SM, 192 threads):
-//   warp 0      TMA producer   cp.async.bulk.tensor.2d, SWIZZLE_128B, 4-stage mbarrier ring
-//   warp 1      MMA issuer     tcgen05.mma cta_group::1 M128 x N256 x K16, commit -> mbarrier
-//   warps 2..5  epilogue       tcgen05.ld 32x32b.x32 from a double-buffered TMEM accumulator
+// Kernel anatomy (one CTA per SM, 384 threads):
+//   warps 0..7   two consumer warpgroups: wgmma M64 x N256 x K16 on their half of the query tile, accumulators in
+//                registers, then the threshold epilogue straight from those registers (setmaxnreg: 232 registers)
+//   warps 8..11  producer warpgroup (setmaxnreg: 40 registers), one thread issues the TMA loads:
+//                cp.async.bulk.tensor.2d, SWIZZLE_128B, 4-stage mbarrier ring
 // Tile: 128 queries (A, K-major) x 256 corpus rows (B, K-major), K block = 64 halfs (128 B).
 #include <cstdlib>
+#include <type_traits>
 
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -30,14 +31,11 @@ constexpr int TS_BLOCK_M = 128;
 constexpr int TS_BLOCK_N = 256;
 constexpr int TS_BLOCK_K = 64;  // fp16 elements = one 128-byte swizzle row
 constexpr int TS_STAGES = 4;
-constexpr int TS_THREADS = 192;
+constexpr int TS_CONSUMERS = 256;                  // two warpgroups of 64 query rows each
+constexpr int TS_THREADS = TS_CONSUMERS + 128;     // + the producer warpgroup
 constexpr uint32_t TS_A_BYTES = TS_BLOCK_M * TS_BLOCK_K * 2;  // 16 KB
 constexpr uint32_t TS_B_BYTES = TS_BLOCK_N * TS_BLOCK_K * 2;  // 32 KB
 constexpr uint32_t TS_STAGE_BYTES = TS_A_BYTES + TS_B_BYTES;
-constexpr uint32_t TS_TMEM_COLS = 512;  // 2 accumulator stages x 256 fp32 columns
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = F16, both K-major, N >> 3, M >> 4
-constexpr uint32_t TS_IDESC = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(TS_BLOCK_N >> 3) << 17) | ((uint32_t)(TS_BLOCK_M >> 4) << 24);
 
 struct TensorScanArgs {
     uint64_t n_rows;     // rows visible to this launch (the seeding pass sees a prefix)
@@ -47,7 +45,7 @@ struct TensorScanArgs {
     float two_eps;
     uint32_t id_base;
     uint32_t emit;       // 0: seeding pass (only tightens gthr), 1: emit candidates
-    int *ggm;            // [mtiles][64][128] shared class maxima (ordered int, class-major so a warp's 32 queries are
+    int *ggm;            // [mtiles][64][128] shared class maxima (ordered int, class-major so a tile's queries are
                          // contiguous), init f2ord(-inf)
     uint32_t *cand;      // [n_queries][cand_cap] global ids
     uint32_t *cand_cnt;  // [n_queries]
@@ -56,7 +54,7 @@ struct TensorScanArgs {
     uint32_t window;     // a CTA may run at most `window` tiles ahead of the slowest CTA of its group
     uint32_t refresh_mask;  // the shared bound is refreshed when (tile & mask) == mask (and for the first tiles)
     uint32_t has_deg;       // the corpus holds degenerate rows: kernel variant that keeps zero accumulators out of the bound
-    // ---- integer form (KIND 1: exact scoring of u8 codes / sub-byte digits on kind::i8, tensor_scan_u8.cu)
+    // ---- integer form (KIND 1: exact scoring of u8 codes / sub-byte digits on wgmma .s32.u8.u8, tensor_scan_u8.cu)
     int metric;             // CDB_METRIC_COSINE or CDB_METRIC_DOT_PRODUCT
     const float *mags;      // [n_rows] stored magnitudes (cosine)
     const float *qmags;     // [n_queries]
@@ -65,10 +63,14 @@ struct TensorScanArgs {
     float rel;              // threshold = bound * rel - two_eps (1 for the f16 form and for the dot product; 1 - 2^-18 for cosine)
 };
 
-constexpr uint32_t TS_LSTAGE = 32;  // thread-private candidate staging slots (shared memory), slot 0 = count
+// Candidate staging in shared memory: 40 bytes per (consumer thread, query row): slot 0 = count, then 9 row ids (f16 form)
+// resp. 4 selection keys (integer form)
+constexpr uint32_t TS_STAGE_SLOT_BYTES = 40;
+constexpr uint32_t TS_LSTAGE = 9;
+constexpr uint32_t TS_KSTAGE = 4;
 constexpr int TS_GROUPS = 64;       // at most 64 class maxima per query; the filter supports k <= TS_GROUPS
 
-// rare path: one approximate score passed the threshold -> stage the row id, flush 32 at a time
+// rare path: one approximate score passed the threshold -> stage the row id, flush TS_LSTAGE at a time
 __device__ __noinline__ void epi_emit(const TensorScanArgs &a, uint32_t qi, uint32_t *stage, uint32_t id) {
     uint32_t c = stage[0];
     stage[1 + c] = id;
@@ -82,8 +84,7 @@ __device__ __noinline__ void epi_emit(const TensorScanArgs &a, uint32_t qi, uint
 }
 
 // integer form: a value passed the filter -> its EXACT score (dp as f32, or dp / (|q| * |row|), cosine.rs:120, 223-235) becomes
-// a selection key; 16 keys are staged per thread, slot 0 of the stage = count
-constexpr uint32_t TS_KSTAGE = 16;
+// a selection key
 __device__ __noinline__ void epi_emit_key(const TensorScanArgs &a, uint32_t qi, uint64_t *stage, int dp, uint64_t row, float qmag) {
     float score = __int2float_rn(dp);   // u64 -> f32 of the reference; dp < 2^31 so the conversion is the same RNE
     if (a.metric == CDB_METRIC_COSINE) {
@@ -122,320 +123,278 @@ __device__ __forceinline__ void sort_desc(float (&v)[NG]) {
     }
 }
 
+// k-th largest of the NG class maxima of one query (volatile: other CTAs raise them concurrently)
+template <int NG>
+__device__ __forceinline__ float class_bound(const int *ggm_q, uint32_t k) {
+    float g2[NG];
+#pragma unroll
+    for (int i = 0; i < NG; ++i) g2[i] = ord2f(*reinterpret_cast<const volatile int *>(ggm_q + (size_t)i * TS_BLOCK_M));
+    sort_desc<NG>(g2);
+    float b = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < NG; ++i) if ((uint32_t)i == k - 1) b = g2[i];
+    return b;
+}
+
+// accumulator value -> filter value.  f16 form: the f32 accumulator.  Integer form, dot product: u8 x u8 sums are >= 0, and
+// non-negative s32 bit patterns order like non-negative floats (FMNMX and the compare keep denormals), so the raw accumulator
+// IS the filter value -- no I2F.  Integer form, cosine: f32(dp) / |row| through the staged reciprocal.
+template <int KIND>
+__device__ __forceinline__ float acc_value(float x, bool, float) { return x; }
+template <int KIND>
+__device__ __forceinline__ float acc_value(uint32_t x, bool cosine, float rinv) {
+    return cosine ? __int2float_rn((int)x) * rinv : __uint_as_float(x);
+}
+__device__ __forceinline__ uint32_t acc_bits(float x) { return __float_as_uint(x); }
+__device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
+
 // HAS_DEG: the corpus holds degenerate rows (zero / non-finite / out-of-range norm).  Their shadow rows are all zero, so
 // they score a == 0.0f exactly, but their exact score is NaN (worst) or +-inf -- the error bound does not cover them.
 // They must not tighten the bound: accumulators that are exactly 0.0f are left out of the class maxima (dropping values
 // from a maximum only loosens a lower bound, so a proper row that happens to score 0.0f is harmless).  Degenerate rows
 // that are not all-zero are put on every candidate list by the host side (api.cu), all-zero rows are provably worst.
-// CTAS = 2: two CTAs of a cluster (one TPC) work as a pair on query tiles 2p and 2p+1 against the same corpus tile:
-// tcgen05.mma.cta_group::2 with M = 256 (each CTA's 128 queries stay in its own shared memory and TMEM) and N = 256 corpus
-// rows of which each CTA stages only HALF (128 rows).  Per SM and k-block the shared-memory traffic drops from 96 KB
-// (fill 48 + operand reads 48) to 64 KB (fill 32 + reads 32) against 542 tensor-pipe cycles of work -- the single-CTA form
-// is bound by the 128 B/clk shared-memory port (DESIGN.md section 5).  Barriers of the pair live in the leader (even) CTA:
-// both CTAs' TMA loads complete on its full barrier, its MMA thread issues for both, commits multicast to both CTAs'
-// empty / accumulator-full barriers, and both epilogues release the accumulator stage on its accumulator-empty barrier.
-// KIND = 1: the same pipeline on tcgen05.mma.kind::i8 (u8 x u8 -> s32, exact): operand rows are 128 BYTES of K per stage
-// (128 u8 elements instead of 64 halfs -- identical tile bytes, descriptors and swizzle), and the epilogue's values are
-// exact integer dot products: the class-maximum bound works on f32(dp) (dot product) or on f32(dp) / |row| (cosine, the
-// per-row reciprocals staged in shared memory per tile), the filter keeps a 2^-18 relative margin for the cosine form and
-// none for the dot product, and whatever passes is scored EXACTLY (epi_emit_key) -- final selection keys, not candidates.
-template <int STAGES, int NG, bool HAS_DEG, int CTAS, int KIND>
+// KIND = 1: the same pipeline on wgmma .s32.u8.u8 (exact): operand rows are 128 BYTES of K per stage (128 u8 elements
+// instead of 64 halfs -- identical tile bytes, descriptors and swizzle), and the epilogue's values are exact integer dot
+// products: the class-maximum bound works on f32(dp) (dot product) or on f32(dp) / |row| (cosine, the per-row reciprocals
+// staged in shared memory per tile), the filter keeps a 2^-18 relative margin for the cosine form and none for the dot
+// product, and whatever passes is scored EXACTLY (epi_emit_key) -- final selection keys, not candidates.
+//
+// Register layout of the epilogue: a consumer thread holds two query rows (r and r + 8 of its warpgroup's 64) and, of each,
+// the 64 columns 8j + 2(lane%4) + {0,1}.  Classes are column mod NG, so the thread owns NG/4 classes of each of its queries
+// (those = 2(lane%4) or 2(lane%4)+1 mod 8); the four threads of a quad together cover all NG classes of their two queries.
+template <int STAGES, int NG, bool HAS_DEG, int KIND>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x, TensorScanArgs a) {
-    constexpr uint32_t B_ROWS = TS_BLOCK_N / CTAS;                          // corpus rows staged by this CTA
-    constexpr uint32_t B_BYTES = B_ROWS * TS_BLOCK_K * 2;                   // 128 bytes of K per row in either form
-    constexpr uint32_t STAGE_BYTES = TS_A_BYTES + B_BYTES;                  // 48 KB, resp. 32 KB per CTA of a pair
     constexpr uint32_t K_ELEMS = KIND == 1 ? 2 * TS_BLOCK_K : TS_BLOCK_K;   // elements per 128-byte row: 128 u8 / 64 halfs
-    // instruction descriptor: D format (1 = F32, 2 = S32) | A/B formats (0 = F16 resp. UINT8) | N >> 3 | M >> 4
-    constexpr uint32_t IDESC = ((KIND == 1 ? 2u : 1u) << 4) | ((uint32_t)(TS_BLOCK_N >> 3) << 17) | ((uint32_t)((TS_BLOCK_M * CTAS) >> 4) << 24);
+    constexpr int NL = NG / 4;                                              // classes a thread owns per query
+    using Acc = typename std::conditional<KIND == 1, uint32_t, float>::type;
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t *tiles = smem;
-    uint32_t *lstage = reinterpret_cast<uint32_t *>(tiles + STAGES * STAGE_BYTES);           // [128][TS_LSTAGE+1]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(lstage + TS_BLOCK_M * (TS_LSTAGE + 2));     // 8-byte aligned
-    uint64_t *full_bar = bars, *empty_bar = bars + STAGES, *tfull_bar = bars + 2 * STAGES, *tempty_bar = bars + 2 * STAGES + 2;
-    uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(bars + 2 * STAGES + 4);
-    float *rinv_s = reinterpret_cast<float *>(tmem_ptr_smem + 4);           // KIND 1 cosine: [2][256] reciprocal row magnitudes
+    uint8_t *lstage = tiles + STAGES * TS_STAGE_BYTES;                                      // [256][2] x 40 bytes
+    uint64_t *bars = reinterpret_cast<uint64_t *>(lstage + TS_CONSUMERS * 2 * TS_STAGE_SLOT_BYTES);
+    uint64_t *full_bar = bars, *empty_bar = bars + STAGES;
+    float *rinv_s = reinterpret_cast<float *>(bars + 2 * STAGES);          // KIND 1 cosine: [2][256] reciprocal row magnitudes
     uint32_t *zflag_s = reinterpret_cast<uint32_t *>(rinv_s + 2 * TS_BLOCK_N);   // [2] a valid row of the tile has |row| = 0
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t crank = CTAS == 2 ? cluster_ctarank() : 0u;              // 0 = leader of the pair
-    const bool leader = crank == 0;
+    const int lane = threadIdx.x & 31;
 
     // work assignment: CTA c owns query tile c % mtiles and every G-th corpus tile
     // gridDim.x is a multiple of mtiles: the mtiles CTAs of group g walk the same corpus tiles g, g+G, ...
     // and are kept within `window` tiles of each other, so a corpus tile is fetched from HBM once and
-    // served to the other query tiles from L2.  (Pairs: mtiles is even, CTAs 2j and 2j+1 of a group are one cluster.)
+    // served to the other query tiles from L2.
     const uint32_t mt = blockIdx.x % a.mtiles;
     const uint32_t g = blockIdx.x / a.mtiles;
     const uint32_t G = gridDim.x / a.mtiles;
-    const uint32_t issuers = a.mtiles / CTAS;                               // MMA issuers per group (progress counter units)
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == TS_CONSUMERS) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-        for (int s = 0; s < STAGES; ++s) { mbar_init(smem_u32(&full_bar[s]), 1); mbar_init(smem_u32(&empty_bar[s]), 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(smem_u32(&tfull_bar[s]), 1); mbar_init(smem_u32(&tempty_bar[s]), 128 * CTAS); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(smem_u32(&full_bar[s]), 1); mbar_init(smem_u32(&empty_bar[s]), TS_CONSUMERS / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        if (CTAS == 2) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TS_TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TS_TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tcgen05_fence_before();
-    if (CTAS == 2) cluster_sync_all(); else __syncthreads();               // barriers of both CTAs initialised before any remote arrive
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
+    __syncthreads();
 
-    if (warp == 0) {
-        // ===================== TMA producer (one per CTA) =====================
-        if (lane == 0) {
+    if (threadIdx.x >= TS_CONSUMERS) {
+        // ===================== TMA producer =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (threadIdx.x == TS_CONSUMERS) {
             uint32_t s = 0, phase = 0, t = 0;
             for (uint32_t nt = g; nt < a.ntiles; nt += G, ++t) {
                 if (a.mtiles > 1 && t >= a.window) {
-                    // bounded drift: every issuer of the group must have issued tile t - window
-                    const uint32_t need = (t - a.window + 1) * issuers;
+                    // bounded drift: every CTA of the group must have consumed tile t - window
+                    const uint32_t need = (t - a.window + 1) * a.mtiles;
                     // bounded spin: if a peer CTA is not resident (GPU shared with another stream) we only lose locality
                     for (int spin = 0; spin < 20000 && *reinterpret_cast<volatile uint32_t *>(a.progress + g) < need; ++spin) __nanosleep(64);
                 }
                 for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
-                    mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);          // own stage free (commit multicast reaches both CTAs)
+                    mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
                     const uint32_t fb = smem_u32(&full_bar[s]);
-                    const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
-                    if (CTAS == 2) {
-                        if (leader) mbar_expect_tx(fb, 2 * STAGE_BYTES);     // the leader's barrier counts both CTAs' bytes
-                        tma_load_2d_pair(sa, &map_q, fb, (int)(kb * K_ELEMS), (int)(mt * TS_BLOCK_M));
-                        tma_load_2d_pair(sa + TS_A_BYTES, &map_x, fb, (int)(kb * K_ELEMS), (int)(nt * TS_BLOCK_N + crank * B_ROWS));
-                    } else {
-                        mbar_expect_tx(fb, STAGE_BYTES);
-                        tma_load_2d(sa, &map_q, fb, (int)(kb * K_ELEMS), (int)(mt * TS_BLOCK_M));
-                        tma_load_2d(sa + TS_A_BYTES, &map_x, fb, (int)(kb * K_ELEMS), (int)(nt * TS_BLOCK_N));
-                    }
+                    const uint32_t sa = smem_u32(tiles + (size_t)s * TS_STAGE_BYTES);
+                    mbar_expect_tx(fb, TS_STAGE_BYTES);
+                    tma_load_2d(sa, &map_q, fb, (int)(kb * K_ELEMS), (int)(mt * TS_BLOCK_M));
+                    tma_load_2d(sa + TS_A_BYTES, &map_x, fb, (int)(kb * K_ELEMS), (int)(nt * TS_BLOCK_N));
                     if (++s == STAGES) { s = 0; phase ^= 1; }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (the leader issues for the pair) =====================
-        if (lane == 0 && leader) {
-            uint32_t s = 0, phase = 0, as = 0, aphase = 0;
-            for (uint32_t nt = g; nt < a.ntiles; nt += G) {
-                mbar_wait(smem_u32(&tempty_bar[as]), aphase ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + as * TS_BLOCK_N;
-                for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
-                    mbar_wait(smem_u32(&full_bar[s]), phase);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE_BYTES);
-                    const uint64_t adesc = make_smem_desc(sa), bdesc = make_smem_desc(sa + TS_A_BYTES);
-#pragma unroll
-                    for (int kk = 0; kk < TS_BLOCK_K / 16; ++kk) {  // +32 bytes along K = +2 in the encoded start address
-                        if (KIND == 1) {
-                            if (CTAS == 2) tcgen05_mma_i8_pair(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, IDESC, (kb | kk) != 0);
-                            else tcgen05_mma_i8(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, IDESC, (kb | kk) != 0);
-                        } else {
-                            if (CTAS == 2) tcgen05_mma_f16_pair(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, IDESC, (kb | kk) != 0);
-                            else tcgen05_mma_f16(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, IDESC, (kb | kk) != 0);
-                        }
-                    }
-                    // frees the smem stage (of both CTAs) when these MMAs retire
-                    if (CTAS == 2) tcgen05_commit_pair(smem_u32(&empty_bar[s])); else tcgen05_commit(smem_u32(&empty_bar[s]));
-                    if (++s == STAGES) { s = 0; phase ^= 1; }
-                }
-                // accumulator complete (in both CTAs' TMEM)
-                if (CTAS == 2) tcgen05_commit_pair(smem_u32(&tfull_bar[as])); else tcgen05_commit(smem_u32(&tfull_bar[as]));
-                if (a.mtiles > 1) atomicAdd(a.progress + g, 1u);  // all loads of this tile have landed in smem
-                if (++as == 2) { as = 0; aphase ^= 1; }
             }
         }
     } else {
-        // ===================== epilogue: threshold filter =====================
-        const uint32_t lane_base = (uint32_t)(warp & 3) * 32;  // a warp may only touch TMEM lanes 32*(warp%4)..+31
-        const uint32_t ql = lane_base + lane;                  // query within the tile == TMEM lane
-        const uint32_t qi = mt * TS_BLOCK_M + ql;
-        const bool qvalid = qi < a.n_queries;
-        // Bound maintenance without a heap and without divergence: the thread keeps the maximum of each of NG
-        // row classes (class = row mod NG; NG = 16/32/64 chosen from k).  The classes are disjoint row sets, so "the k-th largest class
-        // maximum" is a valid lower bound of A_k; the maxima are shared between CTAs through atomicMax on
-        // ggm[query][64] (class sets of different CTAs are disjoint too), which makes the bound GLOBAL: about as
-        // tight as the exact running k-th best, at one FMNMX per value.
-        uint32_t *stage = lstage + (size_t)ql * (TS_LSTAGE + 1);
-        uint64_t *kstage = reinterpret_cast<uint64_t *>(lstage) + (size_t)ql * (TS_KSTAGE + 1);   // KIND 1: same bytes, 16 keys
-        if (KIND == 1) kstage[0] = 0ull; else stage[0] = 0;
+        // ===================== consumers: MMA + threshold filter =====================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+        const uint32_t ct = threadIdx.x;                       // 0..255
+        const uint32_t wg = ct >> 7, wl = (ct >> 5) & 3, qd = (uint32_t)lane & 3;
+        const uint32_t qrow0 = wg * 64 + wl * 16 + ((uint32_t)lane >> 2);   // its two query rows: qrow0, qrow0 + 8
         const bool cosine = KIND == 1 && a.metric == CDB_METRIC_COSINE;
-        const float qmag = (KIND == 1 && qvalid) ? a.qmags[qi] : 0.0f;
-        uint32_t err = (cosine && qvalid && qmag == 0.0f && a.n_rows > 0) ? (uint32_t)CDB_ERRFLAG_CALCULATION : 0u;
-        const uint32_t et = threadIdx.x - 64;                  // 0..127 within the epilogue warps
-        float gm[NG];
+        uint32_t qi[2];
+        bool qvalid[2];
+        float qmag[2], bound[2], thr[2];
+        uint32_t err[2];
+        int *ggm_q[2];
+        uint32_t *stage[2];
+        uint64_t *kstage[2];
+        float gm[2][NL];
 #pragma unroll
-        for (int i = 0; i < NG; ++i) gm[i] = -INFINITY;
-        float bound = -INFINITY, thr = -INFINITY;
-        int *ggm_q = a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql;  // + class * 128
-        if (qvalid) {  // what earlier launches (the seeding pass) and other CTAs already know
-            float g2[NG];
+        for (int i = 0; i < 2; ++i) {
+            const uint32_t ql = qrow0 + 8 * i;
+            qi[i] = mt * TS_BLOCK_M + ql;
+            qvalid[i] = qi[i] < a.n_queries;
+            qmag[i] = (KIND == 1 && qvalid[i]) ? a.qmags[qi[i]] : 0.0f;
+            err[i] = (cosine && qvalid[i] && qmag[i] == 0.0f && a.n_rows > 0) ? (uint32_t)CDB_ERRFLAG_CALCULATION : 0u;
+            ggm_q[i] = a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql;  // + class * 128
+            stage[i] = reinterpret_cast<uint32_t *>(lstage + (size_t)(ct * 2 + i) * TS_STAGE_SLOT_BYTES);
+            kstage[i] = reinterpret_cast<uint64_t *>(stage[i]);
+            if (KIND == 1) kstage[i][0] = 0ull; else stage[i][0] = 0;
 #pragma unroll
-            for (int i = 0; i < NG; ++i) g2[i] = ord2f(*reinterpret_cast<volatile int *>(ggm_q + (size_t)i * TS_BLOCK_M));
-            sort_desc<NG>(g2);
-#pragma unroll
-            for (int i = 0; i < NG; ++i) if ((uint32_t)i == a.k - 1) bound = g2[i];
-            thr = KIND == 1 ? (cosine ? bound * a.rel : bound) : bound - a.two_eps;
+            for (int l = 0; l < NL; ++l) gm[i][l] = -INFINITY;
+            bound[i] = thr[i] = -INFINITY;
+            if (qvalid[i]) {  // what earlier launches (the seeding pass) and other CTAs already know
+                bound[i] = class_bound<NG>(ggm_q[i], a.k);
+                thr[i] = KIND == 1 ? (cosine ? bound[i] * a.rel : bound[i]) : bound[i] - a.two_eps;
+            }
         }
-        uint32_t as = 0, aphase = 0, t = 0;
+        const uint32_t sa0 = smem_u32(tiles);
+        uint32_t s = 0, phase = 0, t = 0;
         for (uint32_t nt = g; nt < a.ntiles; nt += G, ++t) {
             const uint64_t row0 = (uint64_t)nt * TS_BLOCK_N;
-            const float *rs = rinv_s + as * TS_BLOCK_N;
+            const float *rs = rinv_s + (t & 1) * TS_BLOCK_N;
             if (cosine) {
-                // reciprocal magnitudes of this tile's rows -> shared memory (double buffered by accumulator stage); a zero
+                // reciprocal magnitudes of this tile's rows -> shared memory (double buffered by tile parity); a zero
                 // magnitude is an Err for every query that meets the row (cosine.rs:230-231)
-                if (et == 0) zflag_s[as] = 0u;
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (uint32_t c = et; c < (uint32_t)TS_BLOCK_N; c += 128) {
-                    const bool valid = row0 + c < a.n_rows;
-                    const float mg = valid ? a.mags[row0 + c] : 0.0f;
-                    rinv_s[as * TS_BLOCK_N + c] = mg > 0.0f ? __frcp_rn(mg) : 0.0f;
-                    if (valid && mg == 0.0f) zflag_s[as] = 1u;
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                if (qvalid && zflag_s[as]) err |= (uint32_t)CDB_ERRFLAG_CALCULATION;
-            }
-            mbar_wait(smem_u32(&tfull_bar[as]), aphase);
-            tcgen05_fence_after();
-            const bool full_tile = row0 + TS_BLOCK_N <= a.n_rows;  // only the corpus' last tile can be partial (TMA zero fill)
-#pragma unroll 1
-            for (int c = 0; c < TS_BLOCK_N / 64; ++c) {
-                uint32_t r0[32], r1[32];
-                const uint32_t taddr = tmem_base + (lane_base << 16) + as * TS_BLOCK_N + c * 64;
-                tmem_ld_32x32(taddr, r0);
-                tmem_ld_32x32(taddr + 32, r1);
-                tmem_ld_wait();
-                uint32_t m0 = 0, m1 = 0;
-                if (full_tile) {
-                    // common case: fold the 64 values into the class maxima (max trees, FMNMX/FMNMX3) and test only the
-                    // chunk maximum against the threshold; the per-value masks are built on the rare hit
-                    float cm[NG];
+                if (ct == 0) zflag_s[t & 1] = 0u;
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                const bool valid = row0 + ct < a.n_rows;
+                const float mg = valid ? a.mags[row0 + ct] : 0.0f;
+                rinv_s[(t & 1) * TS_BLOCK_N + ct] = mg > 0.0f ? __frcp_rn(mg) : 0.0f;
+                if (valid && mg == 0.0f) zflag_s[t & 1] = 1u;
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                if (zflag_s[t & 1]) {
 #pragma unroll
-                    for (int i = 0; i < NG; ++i) cm[i] = -INFINITY;
-                    float zmax = -INFINITY;   // HAS_DEG: 0.0f if some accumulator of the chunk is exactly zero
+                    for (int i = 0; i < 2; ++i) if (qvalid[i]) err[i] |= (uint32_t)CDB_ERRFLAG_CALCULATION;
+                }
+            }
+            // ---- the tile's product: kblocks x 4 wgmma into registers; a stage is released when its MMAs have retired
+            Acc acc[128];
+#pragma unroll
+            for (int i = 0; i < 128; ++i) acc[i] = 0;
+            uint32_t prev = 0;
+            for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
+                mbar_wait(smem_u32(&full_bar[s]), phase);
+                const uint32_t sa = sa0 + s * TS_STAGE_BYTES;
+                const uint64_t adesc = make_smem_desc(sa + wg * (TS_A_BYTES / 2)), bdesc = make_smem_desc(sa + TS_A_BYTES);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {  // +32 bytes along K = +2 in the encoded start address
+                    if constexpr (KIND == 1) wgmma_u8(acc, adesc + 2 * kk, bdesc + 2 * kk);
+                    else wgmma_f16(acc, adesc + 2 * kk, bdesc + 2 * kk);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                                   // the previous k-block's MMAs have retired
+                if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+                prev = s;
+                if (++s == STAGES) { s = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            if (a.kblocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+            if (ct == 0 && a.mtiles > 1) atomicAdd(a.progress + g, 1u);   // all loads of this tile have landed in smem
+
+            // ---- epilogue: fold the values into the class maxima, test the tile maximum against the threshold,
+            //      build the per-value tests only on a hit
+            const bool full_tile = row0 + TS_BLOCK_N <= a.n_rows;   // only the corpus' last tile can be partial (TMA zero fill)
+            const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;   // valid columns of this tile
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                bool hit;
+                if (full_tile) {
+                    float cm[NL];
+#pragma unroll
+                    for (int l = 0; l < NL; ++l) cm[l] = -INFINITY;
+                    float zmax = -INFINITY;   // HAS_DEG: 0.0f if some accumulator of the tile is exactly zero
 #pragma unroll
                     for (int j = 0; j < 32; ++j) {
-                        float v0, v1;
-                        if (KIND == 1) {
-                            // dot product: u8 x u8 sums are >= 0, and non-negative s32 bit patterns order like non-negative floats
-                            // (FMNMX and the compare keep denormals), so the raw accumulator IS the filter value -- no I2F.
-                            // cosine: f32(dp) / |row| through the staged reciprocals
-                            if (cosine) {
-                                v0 = __int2float_rn((int)r0[j]) * rs[c * 64 + j]; v1 = __int2float_rn((int)r1[j]) * rs[c * 64 + 32 + j];
-                            } else {
-                                v0 = __uint_as_float(r0[j]); v1 = __uint_as_float(r1[j]);
+#pragma unroll
+                        for (int b = 0; b < 2; ++b) {
+                            const uint32_t col = 8 * j + 2 * qd + b;
+                            float v = acc_value<KIND>(acc[4 * j + 2 * i + b], cosine, cosine ? rs[col] : 0.0f);
+                            if (HAS_DEG) {
+                                zmax = v == 0.0f ? 0.0f : zmax;
+                                v = v == 0.0f ? -INFINITY : v;
                             }
-                        } else {
-                            v0 = __uint_as_float(r0[j]); v1 = __uint_as_float(r1[j]);
+                            const int l = (j & (NG / 8 - 1)) * 2 + b;
+                            cm[l] = fmaxf(cm[l], v);
                         }
-                        if (HAS_DEG) {
-                            zmax = (v0 == 0.0f || v1 == 0.0f) ? 0.0f : zmax;
-                            v0 = v0 == 0.0f ? -INFINITY : v0;
-                            v1 = v1 == 0.0f ? -INFINITY : v1;
-                        }
-                        cm[j & (NG - 1)] = fmaxf(cm[j & (NG - 1)], v0);
-                        cm[(32 + j) & (NG - 1)] = fmaxf(cm[(32 + j) & (NG - 1)], v1);
                     }
                     float cmax = zmax;   // the emission test sees every value, the bound only the non-zero ones
 #pragma unroll
-                    for (int i = 0; i < NG; ++i) { cmax = fmaxf(cmax, cm[i]); gm[i] = fmaxf(gm[i], cm[i]); }
-                    if (cmax >= thr) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            float v0, v1;
-                            if (KIND == 1 && cosine) {
-                                v0 = __int2float_rn((int)r0[j]) * rs[c * 64 + j]; v1 = __int2float_rn((int)r1[j]) * rs[c * 64 + 32 + j];
-                            } else {
-                                v0 = __uint_as_float(r0[j]); v1 = __uint_as_float(r1[j]);
-                            }
-                            m0 |= (v0 >= thr ? 1u : 0u) << j;
-                            m1 |= (v1 >= thr ? 1u : 0u) << j;
-                        }
-                    }
+                    for (int l = 0; l < NL; ++l) { cmax = fmaxf(cmax, cm[l]); gm[i][l] = fmaxf(gm[i][l], cm[l]); }
+                    hit = cmax >= thr[i];
                 } else {
-                    const uint64_t left = a.n_rows > row0 + c * 64 ? a.n_rows - (row0 + c * 64) : 0;  // valid columns in this chunk
 #pragma unroll
                     for (int j = 0; j < 32; ++j) {
-                        float v0, v1;
-                        if (KIND == 1 && cosine) {
-                            v0 = __int2float_rn((int)r0[j]) * rs[c * 64 + j]; v1 = __int2float_rn((int)r1[j]) * rs[c * 64 + 32 + j];
-                        } else {
-                            v0 = __uint_as_float(r0[j]); v1 = __uint_as_float(r1[j]);
+#pragma unroll
+                        for (int b = 0; b < 2; ++b) {
+                            const uint32_t col = 8 * j + 2 * qd + b;
+                            const float v = acc_value<KIND>(acc[4 * j + 2 * i + b], cosine, cosine ? rs[col] : 0.0f);
+                            const int l = (j & (NG / 8 - 1)) * 2 + b;
+                            if ((uint64_t)col < left && !(HAS_DEG && v == 0.0f)) gm[i][l] = fmaxf(gm[i][l], v);
                         }
-                        const bool ok0 = (uint64_t)j < left, ok1 = (uint64_t)(32 + j) < left;
-                        m0 |= ((ok0 && v0 >= thr) ? 1u : 0u) << j;
-                        m1 |= ((ok1 && v1 >= thr) ? 1u : 0u) << j;
-                        if (ok0 && !(HAS_DEG && v0 == 0.0f)) gm[j & (NG - 1)] = fmaxf(gm[j & (NG - 1)], v0);
-                        if (ok1 && !(HAS_DEG && v1 == 0.0f)) gm[(32 + j) & (NG - 1)] = fmaxf(gm[(32 + j) & (NG - 1)], v1);
+                    }
+                    hit = true;
+                }
+                if (qvalid[i] && a.emit && hit) {
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) {
+#pragma unroll
+                        for (int b = 0; b < 2; ++b) {
+                            const uint32_t col = 8 * j + 2 * qd + b;
+                            const float v = acc_value<KIND>(acc[4 * j + 2 * i + b], cosine, cosine ? rs[col] : 0.0f);
+                            if ((uint64_t)col < left && v >= thr[i]) {
+                                if (KIND == 1) epi_emit_key(a, qi[i], kstage[i], (int)acc_bits(acc[4 * j + 2 * i + b]), row0 + col, qmag[i]);
+                                else epi_emit(a, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
+                            }
+                        }
                     }
                 }
-                if (qvalid && a.emit && (m0 | m1)) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if ((m0 >> j) & 1u) {
-                            if (KIND == 1) epi_emit_key(a, qi, kstage, (int)r0[j], row0 + c * 64 + j, qmag);
-                            else epi_emit(a, qi, stage, a.id_base + (uint32_t)(row0 + c * 64 + j));
-                        }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if ((m1 >> j) & 1u) {
-                            if (KIND == 1) epi_emit_key(a, qi, kstage, (int)r1[j], row0 + c * 64 + 32 + j, qmag);
-                            else epi_emit(a, qi, stage, a.id_base + (uint32_t)(row0 + c * 64 + 32 + j));
-                        }
-                }
             }
-            tcgen05_fence_before();
-            // the accumulator stage is free: the MMA warp can run ahead (pairs: both CTAs' epilogues report to the leader)
-            if (CTAS == 2) mbar_arrive_leader(smem_u32(&tempty_bar[as])); else mbar_arrive(smem_u32(&tempty_bar[as]));
-            if (++as == 2) { as = 0; aphase ^= 1; }
-            // refresh the shared bound: every tile early on (and in the seeding pass), then every 8th tile
-            if (qvalid && (t < 8 || (t & a.refresh_mask) == a.refresh_mask || !a.emit)) {
-                float g2[NG];
+            // refresh the shared bound: every tile early on (and in the seeding pass), then every 16th tile.  The quad's
+            // classes are published before any of its threads reads the maxima back.
+            if (t < 8 || (t & a.refresh_mask) == a.refresh_mask || !a.emit) {
 #pragma unroll
-                for (int i = 0; i < NG; ++i) {
-                    int *p = ggm_q + (size_t)i * TS_BLOCK_M;
-                    const int mine = f2ord(gm[i]);
-                    const int seen = *reinterpret_cast<volatile int *>(p);
-                    if (mine > seen) atomicMax(p, mine);
-                    g2[i] = ord2f(mine > seen ? mine : seen);
+                for (int i = 0; i < 2; ++i) {
+                    if (!qvalid[i]) continue;
+#pragma unroll
+                    for (int l = 0; l < NL; ++l) {
+                        int *p = ggm_q[i] + (size_t)(8 * (l >> 1) + 2 * qd + (l & 1)) * TS_BLOCK_M;
+                        const int mine = f2ord(gm[i][l]);
+                        if (mine > *reinterpret_cast<volatile int *>(p)) atomicMax(p, mine);
+                    }
                 }
-                sort_desc<NG>(g2);
-                float nb = -INFINITY;
+                __syncwarp();
 #pragma unroll
-                for (int i = 0; i < NG; ++i) if ((uint32_t)i == a.k - 1) nb = g2[i];
-                if (nb > bound) { bound = nb; thr = KIND == 1 ? (cosine ? bound * a.rel : bound) : bound - a.two_eps; }
+                for (int i = 0; i < 2; ++i) {
+                    if (!qvalid[i]) continue;
+                    const float nb = class_bound<NG>(ggm_q[i], a.k);
+                    if (nb > bound[i]) { bound[i] = nb; thr[i] = KIND == 1 ? (cosine ? bound[i] * a.rel : bound[i]) : bound[i] - a.two_eps; }
+                }
             }
         }
-        if (qvalid) {  // final publish + flush of the staged candidates
 #pragma unroll
-            for (int i = 0; i < NG; ++i) atomicMax(ggm_q + (size_t)i * TS_BLOCK_M, f2ord(gm[i]));
-            const uint32_t c = KIND == 1 ? (uint32_t)kstage[0] : stage[0];
+        for (int i = 0; i < 2; ++i) {
+            if (!qvalid[i]) continue;
+            // final publish + flush of the staged candidates
+#pragma unroll
+            for (int l = 0; l < NL; ++l) atomicMax(ggm_q[i] + (size_t)(8 * (l >> 1) + 2 * qd + (l & 1)) * TS_BLOCK_M, f2ord(gm[i][l]));
+            const uint32_t c = KIND == 1 ? (uint32_t)kstage[i][0] : stage[i][0];
             if (a.emit && c) {
-                const uint32_t pos = atomicAdd(a.cand_cnt + qi, c);
-                for (uint32_t i = 0; i < c; ++i)
-                    if (pos + i < a.cand_cap) {
-                        if (KIND == 1) a.cand64[(size_t)qi * a.cand_cap + pos + i] = kstage[1 + i];
-                        else a.cand[(size_t)qi * a.cand_cap + pos + i] = stage[1 + i];
+                const uint32_t pos = atomicAdd(a.cand_cnt + qi[i], c);
+                for (uint32_t x = 0; x < c; ++x)
+                    if (pos + x < a.cand_cap) {
+                        if (KIND == 1) a.cand64[(size_t)qi[i] * a.cand_cap + pos + x] = kstage[i][1 + x];
+                        else a.cand[(size_t)qi[i] * a.cand_cap + pos + x] = stage[i][1 + x];
                     }
             }
-            if (KIND == 1 && err) atomicOr(a.err32 + qi, err);
+            if (KIND == 1 && err[i]) atomicOr(a.err32 + qi[i], err[i]);
         }
-    }
-    tcgen05_fence_before();
-    if (CTAS == 2) cluster_sync_all(); else __syncthreads();   // pairs: no CTA leaves while its peer may still touch its barriers / smem
-    if (warp == 1) {
-        tcgen05_fence_after();
-        if (CTAS == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TS_TMEM_COLS) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TS_TMEM_COLS) : "memory");
     }
 }
 
@@ -626,62 +585,46 @@ static int tensor_scan_stages(uint32_t k) {
     if (k > (uint32_t)TS_GROUPS) return 0;  // the class-maximum bound needs k <= 64 disjoint classes
     return TS_STAGES;
 }
-constexpr int TS_STAGES_PAIR = 6;   // 32 KB per stage and CTA in the pair form: a deeper ring fits
-static size_t tensor_scan_smem(int stages, uint32_t stage_bytes) {
-    // tiles + per-thread staging + barriers + tmem pointer + (integer form) reciprocal magnitudes of two tiles + flags
-    return 1024 + (size_t)stages * stage_bytes + (size_t)TS_BLOCK_M * (TS_LSTAGE + 2) * 4 + (2 * stages + 4) * 8 + 16 +
+static size_t tensor_scan_smem(int stages) {
+    // tiles + candidate staging + barriers + (integer form) reciprocal magnitudes of two tiles + flags
+    return 1024 + (size_t)stages * TS_STAGE_BYTES + (size_t)TS_CONSUMERS * 2 * TS_STAGE_SLOT_BYTES + 2 * stages * 8 +
            2 * TS_BLOCK_N * 4 + 16;
 }
 size_t tensor_scan_smem_bytes(uint32_t k) {
     if (!tensor_scan_stages(k)) return (size_t)1 << 30;
-    return tensor_scan_smem(TS_STAGES, TS_STAGE_BYTES);
+    return tensor_scan_smem(TS_STAGES);
 }
 
-template <int STAGES, int NG, bool HAS_DEG, int CTAS, int KIND>
-static cdb_status launch_tensor_scan_gdc(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid,
-                                         cudaStream_t s) {
-    auto kern = tensor_scan_kernel<STAGES, NG, HAS_DEG, CTAS, KIND>;
-    const size_t smem = tensor_scan_smem(STAGES, TS_A_BYTES + TS_B_BYTES / CTAS);
+template <int NG, bool HAS_DEG, int KIND>
+static cdb_status launch_tensor_scan_gd(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid,
+                                        cudaStream_t s) {
+    auto kern = tensor_scan_kernel<TS_STAGES, NG, HAS_DEG, KIND>;
+    const size_t smem = tensor_scan_smem(TS_STAGES);
     CDB_ALLOW_SMEM(kern, smem);
-    if (CTAS == 1) {
-        kern<<<grid, TS_THREADS, smem, s>>>(mq, mx, a);
-    } else {
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(grid);
-        cfg.blockDim = dim3(TS_THREADS);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = s;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at;
-        cfg.numAttrs = 1;
-        CDB_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, mq, mx, a));
-    }
+    kern<<<grid, TS_THREADS, smem, s>>>(mq, mx, a);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }
 
-template <int NG, int CTAS, int KIND>
+template <int NG, int KIND>
 static cdb_status launch_tensor_scan_g(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid, cudaStream_t s) {
-    constexpr int ST = CTAS == 2 ? TS_STAGES_PAIR : TS_STAGES;
-    if (KIND == 1) return launch_tensor_scan_gdc<ST, NG, false, CTAS, KIND>(mq, mx, a, grid, s);   // exact scores: no degenerate-row variant
-    return a.has_deg ? launch_tensor_scan_gdc<ST, NG, true, CTAS, 0>(mq, mx, a, grid, s)
-                     : launch_tensor_scan_gdc<ST, NG, false, CTAS, 0>(mq, mx, a, grid, s);
+    if (KIND == 1) return launch_tensor_scan_gd<NG, false, KIND>(mq, mx, a, grid, s);   // exact scores: no degenerate-row variant
+    return a.has_deg ? launch_tensor_scan_gd<NG, true, 0>(mq, mx, a, grid, s)
+                     : launch_tensor_scan_gd<NG, false, 0>(mq, mx, a, grid, s);
 }
 
 // fewer classes = cheaper bound refresh (the sort network grows as NG log^2 NG); the bound stays within ~1.5x of the
 // exact k-th best as long as k is well below NG
-template <int CTAS, int KIND>
+template <int KIND>
 static cdb_status launch_tensor_scan(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid, cudaStream_t s) {
-    if (a.k <= 12) return launch_tensor_scan_g<16, CTAS, KIND>(mq, mx, a, grid, s);
-    if (a.k <= 28) return launch_tensor_scan_g<32, CTAS, KIND>(mq, mx, a, grid, s);
-    return launch_tensor_scan_g<64, CTAS, KIND>(mq, mx, a, grid, s);
+    if (a.k <= 12) return launch_tensor_scan_g<16, KIND>(mq, mx, a, grid, s);
+    if (a.k <= 28) return launch_tensor_scan_g<32, KIND>(mq, mx, a, grid, s);
+    return launch_tensor_scan_g<64, KIND>(mq, mx, a, grid, s);
 }
 
 // seeding pass over a prefix of the corpus, then the main pass (both forms)
 template <int KIND>
-static cdb_status run_tensor_scan(const CUtensorMap &mq, const CUtensorMap &mx, TensorScanArgs a, bool pair, uint64_t n_rows,
+static cdb_status run_tensor_scan(const CUtensorMap &mq, const CUtensorMap &mx, TensorScanArgs a, uint64_t n_rows,
                                   uint32_t *d_progress, int sm_count, cudaStream_t s) {
     cdb_status rc;
     // 1. seeding pass over a prefix of the corpus: a few CTAs per query tile, no emission, only the class maxima.
@@ -698,23 +641,16 @@ static cdb_status run_tensor_scan(const CUtensorMap &mq, const CUtensorMap &mx, 
         uint32_t per_m = std::max<uint32_t>(1, (uint32_t)sm_count / a.mtiles);
         per_m = std::min<uint32_t>(per_m, std::max<uint32_t>(1, seed_tiles / 2));
         const uint32_t sgrid = a.mtiles * per_m;
-        rc = pair ? launch_tensor_scan<2, KIND>(mq, mx, sa, sgrid, s) : launch_tensor_scan<1, KIND>(mq, mx, sa, sgrid, s);
-        if (rc) return rc;
+        if ((rc = launch_tensor_scan<KIND>(mq, mx, sa, sgrid, s))) return rc;
     }
     // 2. main pass.  Every CTA should own several corpus tiles, so tiny corpora are not shredded over all SMs.
     a.emit = 1;
     uint64_t total_tiles = (uint64_t)a.mtiles * a.ntiles;
     uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sm_count, std::max<uint64_t>(1, total_tiles / 4));
-    grid = std::max<uint32_t>(1, grid / a.mtiles) * a.mtiles;  // whole groups only (148 SMs, 8 query tiles -> 144 CTAs)
+    grid = std::max<uint32_t>(1, grid / a.mtiles) * a.mtiles;  // whole groups only (132 SMs, 16 query tiles -> 128 CTAs)
     if (grid > (uint32_t)sm_count) { set_error("tensor scan: more query tiles than SMs"); return CDB_INVALID_PARAMS; }
     a.progress = d_progress + 1024;   // the seeding pass used the first 1024 counters
-    return pair ? launch_tensor_scan<2, KIND>(mq, mx, a, grid, s) : launch_tensor_scan<1, KIND>(mq, mx, a, grid, s);
-}
-
-static bool tensor_scan_pair_ok(uint32_t mtiles) {
-    // CTA pairs (cta_group::2) need an even number of query tiles; CDB_TS_PAIR=0 forces the single-CTA form (A/B runs)
-    static const bool pair_allowed = !(getenv("CDB_TS_PAIR") && atoi(getenv("CDB_TS_PAIR")) == 0);
-    return pair_allowed && mtiles % 2 == 0;
+    return launch_tensor_scan<KIND>(mq, mx, a, grid, s);
 }
 
 // d_xh: fp16 normalised corpus [n_rows][pitch_halfs]; d_qh: fp16 normalised queries, padded with zero
@@ -744,11 +680,10 @@ cdb_status tensor_scan_device(const void *d_xh, const void *d_qh, uint32_t pitch
     a.cand_cap = cand_cap;
     const int stages = tensor_scan_stages(k);
     if (!stages) { set_error("tensor scan: k too large for shared memory"); return CDB_INVALID_PARAMS; }
-    const bool pair = tensor_scan_pair_ok(a.mtiles);
     CUtensorMap mq, mx;
     cdb_status rc;
     if ((rc = make_map_f16(&mq, d_qh, (uint64_t)a.mtiles * TS_BLOCK_M, dim, pitch_halfs, TS_BLOCK_M))) return rc;
-    if ((rc = make_map_f16(&mx, d_xh, n_rows, dim, pitch_halfs, pair ? TS_BLOCK_N / 2 : TS_BLOCK_N))) return rc;
+    if ((rc = make_map_f16(&mx, d_xh, n_rows, dim, pitch_halfs, TS_BLOCK_N))) return rc;
     if (!prepared) {   // prep_queries_kernel did all of this already
         fill_i32_kernel<<<(a.mtiles * TS_BLOCK_M * TS_GROUPS + 255) / 256, 256, 0, s>>>(d_ggm, (int)0x807FFFFF /* f2ord(-inf) */, a.mtiles * TS_BLOCK_M * TS_GROUPS);
         CDB_LAUNCH_CHECK();
@@ -762,7 +697,7 @@ cdb_status tensor_scan_device(const void *d_xh, const void *d_qh, uint32_t pitch
     }
 
     a.rel = 1.0f;
-    return run_tensor_scan<0>(mq, mx, a, pair, n_rows, d_progress, sm_count, s);
+    return run_tensor_scan<0>(mq, mx, a, n_rows, d_progress, sm_count, s);
 }
 
 // Integer form (tensor_scan_u8.cu): d_x u8 operand rows [n_rows][pitch] (u8 codes or unpacked digits), d_q the query operand
@@ -793,16 +728,15 @@ cdb_status tensor_scan_i8_device(const uint8_t *d_x, const uint8_t *d_q, uint32_
     a.err32 = d_err32;
     if (!tensor_scan_stages(k)) { set_error("u8 tensor scan: k too large (class-maximum bound needs k <= 64)"); return CDB_INVALID_PARAMS; }
     if ((uint32_t)sm_count < a.mtiles) { set_error("u8 tensor scan: more query tiles than SMs"); return CDB_INVALID_PARAMS; }
-    const bool pair = tensor_scan_pair_ok(a.mtiles);
     CUtensorMap mq, mx;
     cdb_status rc;
     if ((rc = make_tensor_map_2d(&mq, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_q, (uint64_t)a.mtiles * TS_BLOCK_M, dim, pitch, TS_BLOCK_M))) return rc;
-    if ((rc = make_tensor_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_x, n_rows, dim, pitch, pair ? TS_BLOCK_N / 2 : TS_BLOCK_N))) return rc;
+    if ((rc = make_tensor_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_x, n_rows, dim, pitch, TS_BLOCK_N))) return rc;
     fill_i32_kernel<<<(a.mtiles * TS_BLOCK_M * TS_GROUPS + 255) / 256, 256, 0, s>>>(d_ggm, (int)0x807FFFFF /* f2ord(-inf) */, a.mtiles * TS_BLOCK_M * TS_GROUPS);
     CDB_LAUNCH_CHECK();
     CDB_CUDA_TRY(cudaMemsetAsync(d_cand_cnt, 0, (size_t)nq * 4, s));
     CDB_CUDA_TRY(cudaMemsetAsync(d_progress, 0, 8192, s));
-    return run_tensor_scan<1>(mq, mx, a, pair, n_rows, d_progress, sm_count, s);
+    return run_tensor_scan<1>(mq, mx, a, n_rows, d_progress, sm_count, s);
 }
 
 cdb_status select_fallback_device(const uint32_t *d_cnt, uint32_t cap, const float *d_qmags, uint32_t n, uint32_t *d_qsel,

@@ -4,19 +4,17 @@
 // dot_product_u8 (src/models/dot_product/x86_64.rs:22-66) and the bit-plane products
 // dot_product_binary/quaternary/octal (src/models/dot_product.rs:21-90) are integer contractions
 //   sum_i a_i * b_i   with a_i, b_i in 0..255 (u8) or the sub-byte digits 0..1 / 0..3 / 0..7,
-// so tcgen05.mma.kind::i8 (u8 x u8 -> s32 in TMEM) computes them bit-exactly: max 255*255*D < 2^31.
+// so wgmma .s32.u8.u8 (u8 x u8 -> s32 in registers) computes them bit-exactly: max 255*255*D < 2^31.
 // u8 storage is consumed in place; sub-byte storage through an unpacked digit copy (digit =
 // plane0 + 2*plane1 + 4*plane2, exactly the weights the reference kernels apply).
 //
-// The kernel is the KIND = 1 instantiation of tensor_scan_kernel (tensor_scan.cu): same TMA / MMA / epilogue warp roles, CTA
-// pairs (cta_group::2), bounded-drift CTA groups and the same heap-free class-maximum bound, but on kind::i8 and with
-// FINAL scores:
+// The kernel is the KIND = 1 instantiation of tensor_scan_kernel (tensor_scan.cu): same TMA producer, consumer warpgroups,
+// bounded-drift CTA groups and the same heap-free class-maximum bound, but on u8 operands and with FINAL scores:
 //   DotProduct:  score = dp as f32                       (dotproduct.rs:28,55-60)
 //   Cosine:      score = (dp as f32) / (|q| * |row|)     (cosine.rs:120,223-235), 0 denominator -> Err
-// Each epilogue thread owns one query; per value one int->float convert (+ one multiply by the row's reciprocal magnitude for
-// cosine) and one FMNMX into the class maxima; rows passing the bound are scored exactly and emitted as 64-bit selection
-// keys; select_keys_kernel below sorts them and picks the top-k.  (Round 1 kept a per-thread heap here: its divergent slow
-// path held the tensor pipe at 54 %.)
+// Per value one int->float convert (+ one multiply by the row's reciprocal magnitude for cosine) and one FMNMX into the
+// class maxima; rows passing the bound are scored exactly and emitted as 64-bit selection keys; select_keys_kernel below
+// sorts them and picks the top-k.
 #include "kernels.h"
 #include "tc_common.cuh"
 

@@ -1,6 +1,6 @@
 """Row-sharding of a corpus over the GPUs of one node (SURVEY.md 8e).
 
-The reference is single-process; the natural B200 form is one index shard per GPU (contiguous id ranges), the same
+The reference is single-process; the natural multi-GPU form is one index shard per GPU (contiguous id ranges), the same
 query batch on every shard, a local search, ONE all-gather of the per-shard top-k as packed 64-bit keys
 (order_key(score) << 32 | ~global_id; B*k*8 bytes per rank, latency bound on NVLink) and a k-way merge with the common
 ordering rule (better score, then smaller id).  On GPUs all of that lives behind the C ABI (`ShardGroup` ->

@@ -1,5 +1,5 @@
 /*
- * cosdata_b200.h -- C ABI of libcosdata_b200.so, the B200 (sm_100a) replacement
+ * cosdata_b200.h -- C ABI of libcosdata_b200.so, the H100 (sm_90a) replacement
  * for cosdata's ANN-search distance hot path.
  *
  * The reference (cosdata/cosdata, Rust) has no FFI layer; its operator surface
@@ -109,7 +109,7 @@ typedef struct {
                                (Collection.internal_to_external_map, collection.rs:110) */
     uint32_t id_base;       /* global id of local row 0 (corpus shard offset) */
     uint32_t tensor_prefilter; /* 1: also keep an fp16 copy of the L2-normalised raw rows so that large
-                                  batches use the tcgen05 prefilter + exact re-rank (results identical) */
+                                  batches use the wgmma prefilter + exact re-rank (results identical) */
 } cdb_index_desc;
 
 typedef struct {
@@ -374,8 +374,8 @@ cdb_status cdb_index_hnsw_counters(const cdb_index *index, uint64_t *out2);
  * unused slots get CDB_INVALID_ID / 0.  out_counts[q] = valid slots.
  * err_flags may be NULL.  k <= 1024.
  * Execution paths (same results, chosen by shape): BRUTE_RAW with an fp16 shadow, >= 4 queries, >= 16384 rows and
- * k <= 64 -> tcgen05 fp16 prefilter + exact re-rank; BRUTE_CODES over u8 / sub-byte codes with cosine or dot product,
- * >= 16384 rows and k <= 64 -> exact tcgen05 kind::i8 scoring; everything else -> exact SIMT scan. */
+ * k <= 64 -> wgmma fp16 prefilter + exact re-rank; BRUTE_CODES over u8 / sub-byte codes with cosine or dot product,
+ * >= 16384 rows and k <= 64 -> exact wgmma u8 scoring; everything else -> exact SIMT scan. */
 cdb_status cdb_search_batch(cdb_index *index, const float *queries, uint32_t n_queries,
                             const cdb_search_params *params,
                             uint32_t *out_ids, float *out_scores, uint32_t *out_counts,
@@ -452,8 +452,8 @@ cdb_status cdb_merge_topk_device(int32_t device, int32_t metric, const uint32_t 
  * CDB_HNSW_PROF_SLOTS entries) receives the sums accumulated so far.  Synchronizes the device. */
 #define CDB_HNSW_PROF_SLOTS 16
 cdb_status cdb_index_hnsw_profile(cdb_index *index, int32_t enable, uint64_t *out);
-/* dense tcgen05 issue-rate probe (csrc/tc_probe.cu): every SM issues M128 x N256 MMAs on shared-memory-resident operands,
- * no loads, no epilogue.  kind_i8 != 0: kind::i8 (u8 x u8 -> s32), else kind::f16.  out_tops = 2*M*N*K*count / time in
+/* dense wgmma issue-rate probe (csrc/tc_probe.cu): every SM issues M128 x N256 MMAs on shared-memory-resident operands,
+ * no loads, no epilogue.  kind_i8 != 0: u8 x u8 -> s32, else f16 x f16 -> f32.  out_tops = 2*M*N*K*count / time in
  * TOP/s resp. TFLOP/s: the measured roofline denominator of the integer tensor path (MEASURED_PEAKS.json only has bf16).
  * iters = 0 -> default length (~10 ms). */
 cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters, double *out_tops, float *out_ms);

@@ -170,7 +170,7 @@ float orc_bf16_to_f32(uint16_t h) {
     memcpy(&f, &x, 4);
     return f;
 }
-/* The extension DEFINES its fold step as a fused multiply-add (one rounding): that is what the sm_100 FHFMA.BF16 computes, and
+/* The extension DEFINES its fold step as a fused multiply-add (one rounding): that is what the CUDA kernels compute, and
  * it equals the f16 arm's multiply-then-add whenever the product is a normal f32 -- always for operands quantized from
  * [-1,1] above 1e-19, since two 8-bit significands multiply exactly.  Only f32-subnormal or overflowing products (operands
  * below 1e-19 / above 1e19, which bf16 unlike f16 can hold) would round differently in the two-step form. */

@@ -133,7 +133,7 @@ def test_gpu_quantize_and_pair_distances_match_golden(gold, dim):
 def test_gpu_brute_force_topk_matches_golden(gold, dim):
     cdb = _cdb()
     m, q = gold[f"d{dim}/corpus"], gold[f"d{dim}/queries"]
-    for tensor in (False, True):                                     # exact FFMA scan and tcgen05 prefilter + re-rank
+    for tensor in (False, True):                                     # exact FFMA scan and wgmma prefilter + re-rank
         ix = cdb.DenseIndex(dim=dim, storage_type=cdb.StorageType.FullPrecisionFP, capacity=m.shape[0], tensor_prefilter=tensor)
         ix.append(m)
         ids, scores, counts, err = ix.batch_search(q, mg.K)

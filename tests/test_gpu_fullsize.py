@@ -40,7 +40,7 @@ def host_rows(ids):
 def test_full_size_tensor_path_equals_exact_scan_and_oracle_formula(index):
     rows = np.array([0, 1, 4_999_999, 9_999_999, 1234567], dtype=np.int64)
     q = np.concatenate([host_rows(rows), orc.synth_matrix(SEED + 100, 27, D)])        # 5 stored rows + 27 random queries
-    ids_t, sc_t, cnt_t, _ = index.batch_search(q, K)                                    # tcgen05 prefilter + exact re-rank
+    ids_t, sc_t, cnt_t, _ = index.batch_search(q, K)                                    # wgmma prefilter + exact re-rank
     st = index.stats()
     assert st["tensor_searches"] >= 1 and st["fallbacks"] == 0
     ids_e, sc_e, cnt_e, _ = index.batch_search(q, K, exact_only=True)                   # pure FFMA scan

@@ -50,7 +50,7 @@ def test_sharded_brute_raw_equals_single_index(nshards, n, nq):
     assert np.array_equal(ids, want_ids) and np.array_equal(bits(scores), bits(want_scores))
     assert (counts == k).all() and not err.any()
     if n >= 2 * 16384:
-        assert all(p.stats()["tensor_searches"] == 1 for p in parts)      # the tcgen05 path ran on every shard
+        assert all(p.stats()["tensor_searches"] == 1 for p in parts)      # the tensor-core path ran on every shard
     ids2, scores2, _, _ = g.search(q, k, exact_only=True)
     assert np.array_equal(ids2, ids) and np.array_equal(bits(scores2), bits(scores))
     g.close()

@@ -1,4 +1,4 @@
-"""tcgen05 prefilter + exact re-rank must return exactly what the exact scan / CPU oracle
+"""wgmma prefilter + exact re-rank must return exactly what the exact scan / CPU oracle
 return (bit-identical ids and scores), for every shape, and must actually have run."""
 import numpy as np
 import pytest
@@ -20,7 +20,7 @@ def run_case(corpus, queries, k, expect_fallback=False, **kw):
     assert ix.stats()["has_shadow"]
     ids, scores, counts, err = ix.batch_search(queries, k, **kw)
     st = ix.stats()
-    assert st["tensor_searches"] == 1, "the tcgen05 path did not run"
+    assert st["tensor_searches"] == 1, "the tensor-core path did not run"
     assert (st["fallbacks"] == 1) == expect_fallback, st
     want_ids, want_scores = orc.brute_topk_f32(corpus, queries, k)
     assert np.array_equal(ids, want_ids)

@@ -1,4 +1,4 @@
-"""tcgen05 kind::i8 path (tensor_scan_u8.cu): exact integer scoring of u8 / sub-byte codes must equal the
+"""wgmma u8 path (tensor_scan_u8.cu): exact integer scoring of u8 / sub-byte codes must equal the
 CPU oracle bit for bit -- scores, ids (ties broken by smaller id: quantized scores tie often), error flags."""
 import numpy as np
 import pytest
@@ -23,7 +23,7 @@ def run_case(st, metric, n, dim, nq, k=10, zero_row=None, expect_fallback=None, 
     ix.append(corpus)
     ids, scores, counts, err = ix.batch_search(q, k, cdb.SearchMode.BRUTE_CODES, **kw)
     stt = ix.stats()
-    assert stt["tensor_searches"] == (1 if expect_tensor else 0), "tcgen05 i8 path: ran / did not run against expectation"
+    assert stt["tensor_searches"] == (1 if expect_tensor else 0), "u8 tensor-core path: ran / did not run against expectation"
     if expect_fallback is not None:
         assert (stt["fallbacks"] == 1) == expect_fallback, stt
     codes, mags = orc.quantize_batch(int(st), corpus)

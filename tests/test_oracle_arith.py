@@ -384,8 +384,8 @@ def test_bf16_extension_conversion_and_dot_against_independent_restatements():
 
 
 def test_fused_multiply_add_of_16_bit_operands_equals_the_reference_fold():
-    """The CUDA kernels fold f16 / bf16 dot products with ONE fused multiply-add per element (sm_100 FHFMA, PTX fma.rn.f32.f16 /
-    .bf16: operands widened exactly, a*b + c rounded once).  The reference rounds twice (f32 multiply, then f32 add).  Both
+    """The CUDA kernels fold f16 / bf16 dot products with ONE fused multiply-add per element (operands widened exactly to
+    f32, a*b + c rounded once).  The reference rounds twice (f32 multiply, then f32 add).  Both
     agree because the product of two halfs (11-bit significands) or two bf16 values (8-bit) is exact in f32 -- checked here
     with the exact-integer binary32 emulation over operands that include subnormals, the largest finite values and sign
     mixes, against the oracle's dot_product_f16 / bf16 arm."""

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Summarise an .ncu-rep (read with `ncu -i ... --page raw --csv`) into the handful of numbers the
-roofline discussion needs.  Usage: python tools/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/x.txt"""
+roofline discussion needs.  Usage: python tools/ncu_summary.py prof.ncu-rep"""
 import csv
 import subprocess
 import sys
