@@ -562,6 +562,35 @@ class DenseIndex:
         bp = BuildParams(num_levels, neighbors_count, level0_neighbors_count, ef_construction, shortlist_size, max_batch, seed)
         _check(self._lib.cdb_index_build_graph(self._h, C.byref(bp)))
 
+    def insert_graph(self, ef_construction=128, shortlist_size=64, max_batch=4096, seed=1, max_level=None):
+        """GPU-side index_embeddings on the live graph (cdb_index_insert_graph): inserts every row appended since the graph was
+        built or uploaded.  num_levels and the neighbour counts are the graph's.  max_level: the caller's
+        get_max_insert_level draws (u8 per new row) or None for the seeded counter RNG.  -> failed u8[n_new]"""
+        check_insert_args(ef_construction, shortlist_size, max_batch)
+        info = np.zeros(5, dtype=np.uint32)
+        counts = np.zeros(32, dtype=np.uint32)
+        _check(self._lib.cdb_index_graph_info(self._h, _ptr(info), _ptr(counts)))
+        n_new = self.size - int(counts[0])
+        lv = check_insert_args(ef_construction, shortlist_size, max_batch, max_level, n_new)
+        failed = np.zeros(max(n_new, 1), dtype=np.uint8)
+        done = C.c_uint64(0)
+        bp = BuildParams(int(info[0]), int(info[1]), int(info[2]), ef_construction, shortlist_size, max_batch, seed)
+        _check(self._lib.cdb_index_insert_graph(self._h, C.byref(bp), _ptr(lv) if lv is not None else None, _ptr(failed),
+                                                C.byref(done)))
+        return failed[: done.value]
+
+    def read_graph_slot_scores(self):
+        """-> [f32[level_counts[L] * neighbours]] per level: the similarity stored with each neighbour slot (0 = empty slot)"""
+        info = np.zeros(5, dtype=np.uint32)
+        counts = np.zeros(32, dtype=np.uint32)
+        _check(self._lib.cdb_index_graph_info(self._h, _ptr(info), _ptr(counts)))
+        out = []
+        for lv in range(int(info[0]) + 1):
+            a = np.zeros(int(counts[lv]) * int(info[2] if lv == 0 else info[1]), dtype=np.float32)
+            _check(self._lib.cdb_index_read_graph_slot_scores(self._h, lv, _ptr(a)))
+            out.append(a)
+        return out
+
     def build_graph_replicas(self, row, node_id, base_id, md_row, max_level, md_bits, md_mags, main_root_md, pseudo_root_md,
                              num_levels=9, neighbors_count=32, level0_neighbors_count=64, ef_construction=128, shortlist_size=64,
                              max_batch=4096, seed=1):
@@ -613,6 +642,24 @@ class DenseIndex:
     def append_device(self, d_ptr, n):
         """rows already on the index's device: d_ptr = address of n*dim contiguous f32"""
         _check(self._lib.cdb_index_append_f32_device(self._h, d_ptr, n))
+
+
+def check_insert_args(ef_construction, shortlist_size, max_batch, max_level=None, n_new=None):
+    """argument checks of DenseIndex.insert_graph (the ranges cdb_index_insert_graph accepts) -> max_level as u8 or None"""
+    if not 1 <= int(ef_construction) <= 4096:
+        raise ValueError(f"ef_construction must be in 1..4096, got {ef_construction}")
+    if not 1 <= int(shortlist_size) <= 64:
+        raise ValueError(f"shortlist_size must be in 1..64, got {shortlist_size}")
+    if not 0 <= int(max_batch) <= 0xFFFFFFFF:
+        raise ValueError(f"max_batch must be a u32 (0 = 4096), got {max_batch}")
+    if max_level is None:
+        return None
+    lv = np.asarray(max_level)
+    if lv.ndim != 1 or (n_new is not None and lv.size != n_new):
+        raise ValueError(f"max_level needs one draw per new row ({n_new}), got shape {lv.shape}")
+    if lv.size and (lv.min() < 0 or lv.max() > 255):
+        raise ValueError("max_level draws must fit in u8")
+    return np.ascontiguousarray(lv, dtype=np.uint8)
 
 
 # ----------------------------------------------------------------------------- level draws (host side of the builders)

@@ -183,6 +183,7 @@ struct cdb_index {
     bool has_graph = false;
     GraphDev graph{};
     std::vector<void *> graph_allocs;
+    HnswBuildState *bstate = nullptr;   // the builder's slot state of the graph (kept by a build, derived for an upload)
     // replica ids / metadata of the graph nodes (cdb_index_set_graph_metadata)
     bool has_md = false;
     std::vector<void *> md_allocs;
@@ -486,6 +487,7 @@ cdb_status cdb_index_destroy(cdb_index *ix) {
     if (ix->raw_mags_owned && ix->d_raw_mags) cudaFree(ix->d_raw_mags);
     if (ix->d_xh) cudaFree(ix->d_xh);
     if (ix->d_digits) cudaFree(ix->d_digits);
+    hnsw_state_free(ix->bstate);
     for (void *g : ix->graph_allocs) cudaFree(g);
     for (void *g : ix->md_allocs) cudaFree(g);
     if (ix->h_flags) cudaFreeHost(ix->h_flags);
@@ -1232,6 +1234,8 @@ cdb_status cdb_index_set_graph(cdb_index *ix, const cdb_graph_desc *gd) {
             CDB_REQUIRE(gd->adjacency[L][t] == CDB_INVALID_ID || gd->adjacency[L][t] < cnt, "adjacency entry out of range");
     }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    hnsw_state_free(ix->bstate);
+    ix->bstate = nullptr;
     for (void *g : ix->graph_allocs) cudaFree(g);
     ix->graph_allocs.clear();
     for (void *g : ix->md_allocs) cudaFree(g);
@@ -1331,6 +1335,10 @@ cdb_status cdb_index_set_graph_metadata(cdb_index *ix, const cdb_graph_metadata 
     return CDB_OK;
 }
 
+static GraphHost graph_host(cdb_index *ix) {
+    return GraphHost{&ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr, &ix->g_ad, &ix->g_ch};
+}
+
 cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
     CDB_REQUIRE(ix && bp, "null argument");
     CDB_REQUIRE(bp->neighbors_count >= 1 && bp->neighbors_count <= 64 && bp->level0_neighbors_count >= 1 &&
@@ -1354,13 +1362,14 @@ cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
     for (void *g : ix->md_allocs) cudaFree(g);
     ix->md_allocs.clear();
     ix->has_md = false;
+    hnsw_state_free(ix->bstate);
+    ix->bstate = nullptr;
     for (void *g : ix->graph_allocs) cudaFree(g);
     ix->graph_allocs.clear();
     ix->has_graph = false;
     HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, n};
     rc = hnsw_build_device(sc, n, bp->num_levels, bp->neighbors_count, bp->level0_neighbors_count, bp->ef_construction,
-                           bp->shortlist_size, bp->max_batch, bp->seed, &ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr,
-                           &ix->g_ad, &ix->g_ch, ix->stream);
+                           bp->shortlist_size, bp->max_batch, bp->seed, graph_host(ix), &ix->bstate, ix->stream);
     if (rc) return rc;
     ix->has_graph = true;
     return CDB_OK;
@@ -1398,6 +1407,8 @@ cdb_status cdb_index_build_graph_replicas(cdb_index *ix, const cdb_build_params 
     for (void *g : ix->md_allocs) cudaFree(g);
     ix->md_allocs.clear();
     ix->has_md = false;
+    hnsw_state_free(ix->bstate);
+    ix->bstate = nullptr;
     for (void *g : ix->graph_allocs) cudaFree(g);
     ix->graph_allocs.clear();
     ix->has_graph = false;
@@ -1446,6 +1457,79 @@ cdb_status cdb_index_read_graph_level(const cdb_index *ix, uint32_t level, uint3
     if (node_row) CDB_CUDA_TRY(cudaMemcpy(node_row, ix->g_nr[level], (size_t)cnt * 4, cudaMemcpyDeviceToHost));
     if (adjacency) CDB_CUDA_TRY(cudaMemcpy(adjacency, ix->g_ad[level], (size_t)cnt * nb * 4, cudaMemcpyDeviceToHost));
     if (child && level > 0) CDB_CUDA_TRY(cudaMemcpy(child, ix->g_ch[level], (size_t)cnt * 4, cudaMemcpyDeviceToHost));
+    return CDB_OK;
+}
+
+// the builder's slot state of the current graph, derived on first use for a graph that came through cdb_index_set_graph
+static cdb_status ensure_build_state(cdb_index *ix) {
+    if (ix->bstate) return CDB_OK;
+    HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
+    return hnsw_slot_state_device(sc, graph_host(ix), &ix->bstate, ix->stream);
+}
+
+cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, const uint8_t *max_level, uint8_t *out_failed,
+                                  uint64_t *out_inserted) {
+    CDB_REQUIRE(ix && bp, "null argument");
+    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64,
+                "bad build parameters");
+    if (out_inserted) *out_inserted = 0;
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph, "no graph: cdb_index_build_graph or cdb_index_set_graph first");
+    if (ix->has_md) { set_error("insert into a graph with metadata is not supported"); return CDB_UNSUPPORTED; }
+    CDB_REQUIRE(bp->num_levels == ix->graph.num_levels && bp->neighbors_count == ix->graph.nbrs &&
+                    bp->level0_neighbors_count == ix->graph.nbrs0,
+                "params num_levels / neighbors_count / level0_neighbors_count differ from the graph's");
+    CDB_REQUIRE((ix->graph.identity_mask & 1u) && ix->g_cnt[0] <= ix->size, "level 0 of the graph must list rows 0..level_counts[0]-1");
+    cdb_status rc;
+    if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
+        set_error("metric/storage arm is an Err in the reference");
+        return rc;
+    }
+    const uint64_t n_new = ix->size - ix->g_cnt[0];
+    if (!n_new) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    {   // searches already enqueued on their callers' streams finish on the old graph before it changes
+        std::lock_guard<std::mutex> g(ix->pool_mu);
+        for (auto &u : ix->pool)
+            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
+    }
+    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    if ((rc = ensure_build_state(ix))) return rc;
+    HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
+    bool changed = false;
+    if ((rc = hnsw_insert_device(sc, graph_host(ix), ix->bstate, (uint32_t)n_new, max_level, bp->seed, bp->ef_construction,
+                                 bp->shortlist_size, bp->max_batch, ix->desc.capacity, out_failed, &changed, ix->stream))) {
+        if (changed) {   // a half-inserted graph is not the reference's graph: the index has none until a build / upload
+            const std::string why = cdb_last_error_string();
+            hnsw_state_free(ix->bstate);
+            ix->bstate = nullptr;
+            for (void *g : ix->graph_allocs) cudaFree(g);
+            ix->graph_allocs.clear();
+            ix->has_graph = false;
+            set_error(why + " (the insert had started: the graph was dropped)");
+        }
+        return rc;
+    }
+    if (out_inserted) *out_inserted = n_new;
+    return CDB_OK;
+}
+
+cdb_status cdb_index_read_graph_slot_scores(cdb_index *ix, uint32_t level, float *out_scores) {
+    CDB_REQUIRE(ix && out_scores, "null argument");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph && level <= ix->graph.num_levels, "no graph / bad level");
+    if (ix->has_md) { set_error("slot scores of a graph with metadata are not supported"); return CDB_UNSUPPORTED; }
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    cdb_status rc;
+    if ((rc = ensure_build_state(ix))) return rc;
+    const size_t slots = (size_t)ix->g_cnt[level] * (level == 0 ? ix->graph.nbrs0 : ix->graph.nbrs);
+    std::vector<uint32_t> adj(slots), keys(slots);
+    CDB_CUDA_TRY(cudaMemcpy(adj.data(), ix->g_ad[level], slots * 4, cudaMemcpyDeviceToHost));
+    CDB_CUDA_TRY(cudaMemcpy(keys.data(), hnsw_state_slot_keys(ix->bstate, level), slots * 4, cudaMemcpyDeviceToHost));
+    for (size_t t = 0; t < slots; ++t) {
+        const uint32_t b = adj[t] == CDB_INVALID_ID ? 0u : key_to_bits(ix->desc.metric, keys[t]);
+        std::memcpy(out_scores + t, &b, 4);
+    }
     return CDB_OK;
 }
 

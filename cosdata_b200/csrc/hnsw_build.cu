@@ -12,10 +12,14 @@
 //   phase B (hnsw_build_link_kernel): create_node_edges for levels 0..max_level with the reference's add_neighbor
 //     (lowest-similarity slot, strict improvement, stale lowest_index, back-link removal of the evicted neighbour,
 //     remove_neighbor_by_index_and_id on a failed reverse edge) under a per-node spin lock.
+// A build is the root on every level followed by an insert of every row; cdb_index_insert_graph runs the same insert on
+// rows appended later, against the slot state the build kept (or, for an uploaded graph, hnsw_slot_state_kernel derived).
 // Batches grow geometrically from 1 so the upper structure is built almost sequentially.
-// Level membership is decided up front from a counter RNG, so node_row / child are static and only the adjacency
-// (plus each slot's similarity and the node's lowest slot) evolves.
+// Level membership is decided up front (counter RNG or the caller's draws), so node_row / child are static during a call
+// and only the adjacency (plus each slot's similarity and the node's lowest slot) evolves.
 #include <algorithm>
+#include <array>
+#include <memory>
 #include <vector>
 
 #include "hnsw_traverse.cuh"
@@ -24,7 +28,8 @@ namespace cdb {
 
 struct BuildLevel {
     uint32_t cnt, nb;
-    uint32_t *node_row;    // [cnt] (level >= 1: [0] = root row, then ascending rows)
+    uint32_t app;          // first node appended by the current call: level >= 1 lists its new rows ascending from here
+    uint32_t *node_row;    // [cnt] (level >= 1: the root, then each call's rows ascending)
     uint32_t *child;       // [cnt] level-local index one level down
     uint32_t *adj;         // [cnt*nb]
     uint32_t *simkey;      // [cnt*nb] order key of the slot's similarity
@@ -56,7 +61,8 @@ struct ReplicaDev {
 struct BuildArgs {
     BuildGraph g;
     HnScoreCtx sc;
-    const uint8_t *levels;  // [n] max insert level of each row
+    const uint8_t *levels;  // [count of the call] max insert level of row lv_first + i
+    uint32_t lv_first;
     uint32_t first, count;  // rows [first, first+count) form this batch
     uint32_t ef, shortlist;
     uint32_t *z_nodes;      // [count][num_levels+1][64]
@@ -67,7 +73,8 @@ struct BuildArgs {
     ReplicaDev rl;
 };
 
-// local index of `row` at `level` (level 0: the row itself; level >= 1: binary search in the sorted node_row)
+// local index of `row` at `level` (level 0: the row itself; level >= 1: binary search in the part of node_row the current
+// call appended -- an uploaded level need not be sorted before it)
 __device__ inline uint32_t build_local(const BuildLevel &l, uint32_t level, uint32_t row, bool replicas = false) {
     if (replicas) {   // every level lists the created nodes in list order behind the two roots
         uint32_t lo = 2, hi = l.cnt;
@@ -75,7 +82,7 @@ __device__ inline uint32_t build_local(const BuildLevel &l, uint32_t level, uint
         return lo;
     }
     if (level == 0) return row;
-    uint32_t lo = 1, hi = l.cnt;
+    uint32_t lo = l.app, hi = l.cnt;
     while (lo < hi) { const uint32_t md = (lo + hi) >> 1; if (l.node_row[md] < row) lo = md + 1; else hi = md; }
     return lo;
 }
@@ -90,7 +97,7 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs
     for (uint32_t i = tid; i < a.sc.row_pitch / 4; i += HN_THREADS)
         reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(a.sc.rows + (size_t)vrow * a.sc.row_pitch)[i];
     const float qmag = a.sc.mags[vrow];
-    const uint32_t max_level = a.levels[r];
+    const uint32_t max_level = a.levels[r - a.lv_first];
     const uint32_t L1 = a.g.num_levels + 1;
     // replica builds: the traversal carries the embedding's metadata and prop_value.id (vector_store.rs:809-821); nodes whose
     // metadata has mag != 0 (Pseudo / Metadata kinds) start at the pseudo root (:461-483, 755-758)
@@ -184,7 +191,7 @@ __global__ void __launch_bounds__(128) hnsw_build_link_kernel(BuildArgs a) {
     if ((threadIdx.x & 31) != 0 || b >= a.count || a.failed[b]) return;
     const uint32_t r = a.first + b;
     const uint32_t L1 = a.g.num_levels + 1;
-    const uint32_t top = min((uint32_t)a.levels[r], a.g.num_levels);
+    const uint32_t top = min((uint32_t)a.levels[r - a.lv_first], a.g.num_levels);
     for (uint32_t level = 0; level <= top; ++level) {  // edges are created bottom-up as the recursion unwinds
         const BuildLevel &l = a.g.lv[level];
         const uint32_t node = build_local(l, level, r, a.replicas);
@@ -221,12 +228,86 @@ __global__ void fill_u32_kernel(uint32_t *p, uint32_t v, uint64_t n) {
     if (i < n) p[i] = v;
 }
 
+// ------------------------------------------------------------------ slot state of an uploaded graph
+// ProbNode::new_with_neighbors_and_versions (prob_node.rs:145-181): every slot's similarity is recomputed and lowest_index is
+// the first empty slot (MetricResult::min) or else the first slot with a strictly lower similarity, scanning from
+// MetricResult::max.  The builder stores the similarity of the NEW node (x) against the neighbour (y) on both ends of an
+// edge; recomputing it from the node's side gives the same bits because every plain arm is symmetric.  A slot whose pair
+// is an Err (a zero-norm row under cosine) cannot come from the reference's build: it gets MetricResult::min, so it is the
+// first slot add_neighbor replaces.
+// One warp per node: lane 0 stages the node's row, every lane with a filled slot stages that neighbour's row (TMA bulk
+// copies completing on the warp's mbarrier, as hnsw_warp.cu stages rows), then lane s scores slot s with the same
+// pair_distance every other scorer uses.  Slots go in rounds of `group` lanes when the rows of all 32 do not fit.
+constexpr int SS_WARPS = 4;
+constexpr uint32_t SS_STAGE_BYTES = 24 * 1024;   // shared memory per warp (node row + one round of neighbour rows)
+
+__global__ void __launch_bounds__(SS_WARPS * 32) hnsw_slot_state_kernel(BuildLevel l, HnScoreCtx sc, uint32_t min_key, uint32_t max_key,
+                                                                        uint32_t group) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ __align__(8) uint64_t bars[SS_WARPS];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint8_t *own = smem + (size_t)warp * (group + 1) * sc.row_pitch;
+    uint8_t *mine_row = own + (size_t)(lane + 1) * sc.row_pitch;
+    const uint32_t bar = hw_smem_u32(&bars[warp]);
+    if (lane == 0) hw_mbar_init(bar, 1);
+    __syncwarp();
+    const uint32_t pp = plane_pitch(sc.dim);
+    uint32_t parity = 0;
+    for (uint32_t node = blockIdx.x * SS_WARPS + warp; node < l.cnt; node += gridDim.x * SS_WARPS) {
+        const uint32_t row = l.node_row[node];
+        uint32_t first_empty = HN_EMPTY;
+        uint64_t best = ~0ull;   // (key << 32 | slot): lowest filled slot strictly below MetricResult::max
+        for (uint32_t base = 0; base < l.nb; base += group) {
+            const uint32_t s = base + lane;
+            const bool in_round = lane < group && s < l.nb;
+            const uint32_t nbr = in_round ? l.adj[(size_t)node * l.nb + s] : HN_EMPTY;
+            const uint32_t filled = __ballot_sync(0xFFFFFFFFu, nbr != HN_EMPTY);
+            const uint32_t empties = __ballot_sync(0xFFFFFFFFu, in_round && nbr == HN_EMPTY);
+            if (first_empty == HN_EMPTY && empties) first_empty = base + __ffs(empties) - 1;
+            const uint32_t nrow = nbr != HN_EMPTY ? l.node_row[nbr] : 0;
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the previous round's reads before the copies below
+            __syncwarp();
+            if (lane == 0) {
+                hw_mbar_expect(bar, (uint32_t)(__popc(filled) + (base == 0)) * sc.row_pitch);
+                if (base == 0) hw_bulk_g2s(hw_smem_u32(own), sc.rows + (size_t)row * sc.row_pitch, sc.row_pitch, bar);
+            }
+            __syncwarp();
+            if (nbr != HN_EMPTY) hw_bulk_g2s(hw_smem_u32(mine_row), sc.rows + (size_t)nrow * sc.row_pitch, sc.row_pitch, bar);
+            hw_mbar_wait(bar, parity);
+            parity ^= 1u;
+            if (nbr != HN_EMPTY) {
+                float d = 0.f;
+                const int rc = pair_distance(sc.metric, sc.st, sc.dim, own, sc.mags[row], pp, mine_row, sc.mags[nrow], pp, &d);
+                const uint32_t key = rc == CDB_OK ? order_key(sc.metric, __float_as_uint(d)) : min_key;
+                l.simkey[(size_t)node * l.nb + s] = key;
+                if (key < max_key) best = min(best, ((uint64_t)key << 32) | s);
+            }
+        }
+        for (int o = 16; o; o >>= 1) best = min(best, (uint64_t)__shfl_xor_sync(0xFFFFFFFFu, best, o));
+        if (lane == 0) {
+            uint32_t li = 0, lk = max_key;
+            if (first_empty != HN_EMPTY) { li = first_empty; lk = min_key; }
+            else if (best != ~0ull) { li = (uint32_t)best; lk = (uint32_t)(best >> 32); }
+            l.lowest_idx[node] = li;
+            l.lowest_key[node] = lk;
+        }
+    }
+}
+
 // ------------------------------------------------------------------ host
-struct BuiltGraph {
-    BuildGraph g{};
-    std::vector<void *> allocs;
-    uint8_t *d_levels = nullptr;
+struct HnswBuildState {
+    BuildGraph g{};                          // level arrays (owned by the graph's allocations) and the slot state
+    uint64_t cap[BUILD_MAX_LEVELS] = {};     // nodes each level's arrays hold
 };
+void hnsw_state_free(HnswBuildState *st) { delete st; }
+const uint32_t *hnsw_state_slot_keys(const HnswBuildState *st, uint32_t level) { return st->g.lv[level].simkey; }
+
+static void metric_key_range(int metric, uint32_t *min_key, uint32_t *max_key) {   // MetricResult::min / ::max (types.rs:435-457)
+    switch (metric) {
+    case CDB_METRIC_COSINE: *min_key = order_key(metric, 0xBF800000u /* -1.0 */); *max_key = order_key(metric, 0x40000000u /* 2.0 */); break;
+    default: *min_key = order_key(metric, 0xFF800000u /* -inf */); *max_key = order_key(metric, 0x7F800000u /* +inf */); break;
+    }
+}
 
 static float unit_rng(uint64_t seed, uint64_t i) {  // stands in for rand::random::<f32>() (vector_store.rs:750-753)
     uint64_t z = seed + (i + 1) * 0x9E3779B97F4A7C15ull;
@@ -235,104 +316,180 @@ static float unit_rng(uint64_t seed, uint64_t i) {  // stands in for rand::rando
     z = z ^ (z >> 31);
     return (float)(z >> 40) * (1.0f / 16777216.0f);
 }
+// get_max_insert_level with probabilities 1 - 4^-n: x >= 1 - 4^-lv is monotone in lv, so the largest satisfied lv is the
+// first hit of the reference's top-down scan
+static uint8_t draw_level(uint64_t seed, uint32_t row, uint32_t num_levels) {
+    const double x = (double)unit_rng(seed, row);
+    uint32_t ml = 0;
+    double p4 = 1.0;
+    for (uint32_t lv = 1; lv <= num_levels; ++lv) { p4 *= 4.0; if (x >= 1.0 - 1.0 / p4) ml = lv; else break; }
+    return (uint8_t)ml;
+}
 
-cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root is row n */, uint32_t num_levels, uint32_t nbrs,
-                             uint32_t nbrs0, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed,
-                             GraphDev *out_graph, std::vector<void *> *out_allocs, std::vector<uint32_t> *out_counts,
-                             std::vector<const uint32_t *> *out_nr, std::vector<const uint32_t *> *out_ad,
-                             std::vector<const uint32_t *> *out_ch, cudaStream_t s) {
-    if (num_levels + 1 > BUILD_MAX_LEVELS) { set_error("build: too many levels"); return CDB_INVALID_PARAMS; }
-    const uint32_t L1 = num_levels + 1;
-    // ---- level membership (get_max_insert_level with probabilities 1 - 4^-n)
-    std::vector<uint8_t> levels(n);
-    std::vector<std::vector<uint32_t>> rows(L1);
-    for (uint32_t L = 1; L < L1; ++L) rows[L].push_back(n);  // root is local 0 on every upper level
-    for (uint32_t r = 0; r < n; ++r) {
-        const double x = (double)unit_rng(seed, r);
-        uint32_t ml = 0;
-        double p4 = 1.0;
-        for (uint32_t lv = 1; lv <= num_levels; ++lv) { p4 *= 4.0; if (x >= 1.0 - 1.0 / p4) ml = lv; else break; }
-        // x >= 1 - 4^-lv is monotone in lv, so the largest satisfied lv is the first hit of the reference's top-down scan
-        levels[r] = (uint8_t)ml;
-        for (uint32_t L = 1; L <= ml; ++L) rows[L].push_back(r);
-    }
-    BuiltGraph bg;
-    bg.g.num_levels = num_levels;
-    bg.g.root_row = n;
-    bg.g.entry = num_levels == 0 ? n : 0;
-    switch (sc.metric) {
-    case CDB_METRIC_COSINE: bg.g.min_key = order_key(sc.metric, 0xBF800000u /* -1.0 */); bg.g.max_key = order_key(sc.metric, 0x40000000u /* 2.0 */); break;
-    default: bg.g.min_key = order_key(sc.metric, 0xFF800000u /* -inf */); bg.g.max_key = order_key(sc.metric, 0x7F800000u /* +inf */); break;
-    }
-    auto dalloc = [&](void **p, size_t bytes) -> cdb_status {
-        CDB_CUDA_TRY(cudaMalloc(p, bytes ? bytes : 4));
-        out_allocs->push_back(*p);
+static cdb_status publish(const HnswBuildState &st, const GraphHost &gh);
+
+// device allocations freed when the owner goes out of scope (release() hands them over)
+struct DevAllocs {
+    std::vector<void *> p;
+    ~DevAllocs() { for (void *q : p) cudaFree(q); }
+    cdb_status get(void **out, size_t bytes) {
+        CDB_CUDA_TRY(cudaMalloc(out, bytes ? bytes : 4));
+        p.push_back(*out);
         return CDB_OK;
-    };
-    cdb_status rc;
-    std::vector<const uint32_t *> t_nr(L1), t_ad(L1), t_ch(L1);
-    for (uint32_t L = 0; L < L1; ++L) {
-        BuildLevel &l = bg.g.lv[L];
-        l.nb = L == 0 ? nbrs0 : nbrs;
-        l.cnt = L == 0 ? n + 1 : (uint32_t)rows[L].size();
-        if ((rc = dalloc((void **)&l.node_row, (size_t)l.cnt * 4)) || (rc = dalloc((void **)&l.child, (size_t)l.cnt * 4)) ||
-            (rc = dalloc((void **)&l.adj, (size_t)l.cnt * l.nb * 4)) || (rc = dalloc((void **)&l.simkey, (size_t)l.cnt * l.nb * 4)) ||
-            (rc = dalloc((void **)&l.lowest_idx, (size_t)l.cnt * 4)) || (rc = dalloc((void **)&l.lowest_key, (size_t)l.cnt * 4)) ||
-            (rc = dalloc((void **)&l.lock, (size_t)l.cnt * 4)))
-            return rc;
-        std::vector<uint32_t> nr(l.cnt), ch(l.cnt, HN_EMPTY);
-        if (L == 0) for (uint32_t i = 0; i <= n; ++i) nr[i] = i;
-        else {
-            nr = rows[L];
-            // child = position of the same row one level down (both lists: root first, then ascending rows)
-            if (L == 1) for (uint32_t i = 0; i < l.cnt; ++i) ch[i] = nr[i];
-            else {
-                const std::vector<uint32_t> &below = rows[L - 1];
-                uint32_t j = 1;
-                ch[0] = 0;
-                for (uint32_t i = 1; i < l.cnt; ++i) { while (below[j] != nr[i]) ++j; ch[i] = j; }
-            }
-        }
-        CDB_CUDA_TRY(cudaMemcpyAsync(l.node_row, nr.data(), (size_t)l.cnt * 4, cudaMemcpyHostToDevice, s));
-        CDB_CUDA_TRY(cudaMemcpyAsync(l.child, ch.data(), (size_t)l.cnt * 4, cudaMemcpyHostToDevice, s));
-        CDB_CUDA_TRY(cudaStreamSynchronize(s));  // nr/ch are stack-owned
-        const uint64_t slots = (uint64_t)l.cnt * l.nb;
-        fill_u32_kernel<<<(uint32_t)((slots + 255) / 256), 256, 0, s>>>(l.adj, HN_EMPTY, slots);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemsetAsync(l.simkey, 0, slots * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(l.lowest_idx, 0, (size_t)l.cnt * 4, s));  // ProbNode::new: (0, MetricResult::min)
-        fill_u32_kernel<<<(l.cnt + 255) / 256, 256, 0, s>>>(l.lowest_key, bg.g.min_key, l.cnt);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemsetAsync(l.lock, 0, (size_t)l.cnt * 4, s));
-        t_nr[L] = l.node_row; t_ad[L] = l.adj; t_ch[L] = l.child;
     }
-    uint8_t *d_levels = nullptr;
-    if ((rc = dalloc((void **)&d_levels, n))) return rc;
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_levels, levels.data(), n, cudaMemcpyHostToDevice, s));
-    // ---- batches
+    void release() { p.clear(); }
+};
+
+// the arrays of one level: per node (node_row, lowest_idx, lowest_key, lock, child) and per slot (adj, simkey)
+constexpr int LEVEL_ARRAYS = 7;
+static uint32_t *&level_array(BuildLevel &l, int t) {
+    switch (t) {
+    case 0: return l.node_row;
+    case 1: return l.lowest_idx;
+    case 2: return l.lowest_key;
+    case 3: return reinterpret_cast<uint32_t *&>(l.lock);
+    case 4: return l.child;
+    case 5: return l.adj;
+    default: return l.simkey;
+    }
+}
+static size_t level_words(const BuildLevel &l, int t, uint64_t nodes) { return t >= 5 ? nodes * l.nb : nodes; }
+
+// Appends nodes (vector rows rows[L], level-local children child[L] on levels >= 1) to every level.  Arrays that must
+// grow are allocated first (by half their size at least; level 0 never beyond rows_cap nodes): if one allocation fails,
+// nothing has changed.  After that *changed is set; the old arrays are copied, the new nodes start as ProbNode::new (no
+// neighbours, lowest_index (0, MetricResult::min)), the search layout is re-published and the old arrays are freed.
+static cdb_status append_levels(HnswBuildState &st, const GraphHost &gh, const std::vector<std::vector<uint32_t>> &rows,
+                                const std::vector<std::vector<uint32_t>> &child, uint64_t rows_cap, bool *changed, cudaStream_t s) {
+    const uint32_t L1 = st.g.num_levels + 1;
+    cdb_status rc;
+    std::vector<uint64_t> cap(L1, 0);
+    std::vector<std::array<uint32_t *, LEVEL_ARRAYS>> fresh(L1);
+    DevAllocs grown;
+    for (uint32_t L = 0; L < L1; ++L) {
+        const BuildLevel &l = st.g.lv[L];
+        fresh[L].fill(nullptr);
+        const uint64_t need = (uint64_t)l.cnt + rows[L].size();
+        if (need <= st.cap[L]) continue;
+        cap[L] = std::max<uint64_t>(need, st.cap[L] + st.cap[L] / 2);
+        if (L == 0) cap[L] = std::max<uint64_t>(need, std::min<uint64_t>(cap[L], rows_cap));
+        for (int t = 0; t < LEVEL_ARRAYS; ++t)
+            if ((t != 4 || L > 0) && (rc = grown.get((void **)&fresh[L][t], level_words(l, t, cap[L]) * 4))) return rc;
+    }
+    // ---- commit: every new array joins the graph's allocations, the old ones leave them once the tables moved on
+    *changed = true;
+    gh.allocs->insert(gh.allocs->end(), grown.p.begin(), grown.p.end());
+    grown.release();
+    std::vector<void *> retired;
+    for (uint32_t L = 0; L < L1; ++L) {
+        BuildLevel &l = st.g.lv[L];
+        if (cap[L]) {
+            for (int t = 0; t < LEVEL_ARRAYS; ++t) {
+                if (!fresh[L][t]) continue;
+                uint32_t *&arr = level_array(l, t);
+                const size_t used = level_words(l, t, l.cnt);
+                if (arr && used) CDB_CUDA_TRY(cudaMemcpyAsync(fresh[L][t], arr, used * 4, cudaMemcpyDeviceToDevice, s));
+                if (arr) retired.push_back(arr);
+                arr = fresh[L][t];
+            }
+            st.cap[L] = cap[L];
+        }
+        l.app = l.cnt;
+        const uint32_t add = (uint32_t)rows[L].size();
+        if (!add) continue;
+        for (uint32_t i = 0; L > 0 && i < add; ++i)   // an uploaded level that listed node i as row i may stop doing so
+            if (rows[L][i] != l.cnt + i) { gh.dev->identity_mask &= ~(1u << L); break; }
+        CDB_CUDA_TRY(cudaMemcpyAsync(l.node_row + l.cnt, rows[L].data(), (size_t)add * 4, cudaMemcpyHostToDevice, s));
+        if (L > 0) CDB_CUDA_TRY(cudaMemcpyAsync(l.child + l.cnt, child[L].data(), (size_t)add * 4, cudaMemcpyHostToDevice, s));
+        const uint64_t slots = (uint64_t)add * l.nb;
+        fill_u32_kernel<<<(uint32_t)((slots + 255) / 256), 256, 0, s>>>(l.adj + (size_t)l.cnt * l.nb, HN_EMPTY, slots);
+        CDB_LAUNCH_CHECK();
+        CDB_CUDA_TRY(cudaMemsetAsync(l.simkey + (size_t)l.cnt * l.nb, 0, slots * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(l.lowest_idx + l.cnt, 0, (size_t)add * 4, s));
+        fill_u32_kernel<<<(add + 255) / 256, 256, 0, s>>>(l.lowest_key + l.cnt, st.g.min_key, add);
+        CDB_LAUNCH_CHECK();
+        CDB_CUDA_TRY(cudaMemsetAsync(l.lock + l.cnt, 0, (size_t)add * 4, s));
+        l.cnt += add;
+    }
+    CDB_CUDA_TRY(cudaStreamSynchronize(s));   // the copies are done (host vectors, old arrays)
+    if ((rc = publish(st, gh))) return rc;
+    for (void *p : retired) {
+        gh.allocs->erase(std::find(gh.allocs->begin(), gh.allocs->end(), p));
+        cudaFree(p);
+    }
+    return CDB_OK;
+}
+
+// points the search layout (pointer tables, counts, host copies) at the level arrays of `st`
+static cdb_status publish(const HnswBuildState &st, const GraphHost &gh) {
+    const uint32_t L1 = st.g.num_levels + 1;
+    gh.cnt->assign(L1, 0);
+    gh.nr->assign(L1, nullptr); gh.ad->assign(L1, nullptr); gh.ch->assign(L1, nullptr);
+    for (uint32_t L = 0; L < L1; ++L) {
+        (*gh.cnt)[L] = st.g.lv[L].cnt;
+        (*gh.nr)[L] = st.g.lv[L].node_row;
+        (*gh.ad)[L] = st.g.lv[L].adj;
+        (*gh.ch)[L] = L ? st.g.lv[L].child : nullptr;
+    }
+    CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->node_row, gh.nr->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+    CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->adj, gh.ad->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+    CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->child, gh.ch->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+    return CDB_OK;
+}
+
+// index_embeddings for rows [first, first+count) (levels[i] = max insert level of row first+i), the one batch loop of both
+// the build and the insert.  Nodes for every level the rows reach are appended up front (level 0: node = row; levels >= 1:
+// ascending rows after the existing nodes, child pointing into the appended part of the level below), so node_row / child
+// are static while the adjacency evolves.  Batches hold max(1, min(max_batch, linked / 8)) rows, linked = data rows already
+// in the graph: a fresh build starts almost sequentially, a small transaction into a large graph runs as one batch.
+// Every allocation happens before the graph changes; *changed tells the caller whether an error left it half-inserted.
+static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState &st, uint32_t first, uint32_t count,
+                              const std::vector<uint8_t> &levels, uint32_t linked, uint32_t ef_construction, uint32_t shortlist,
+                              uint32_t max_batch, uint64_t rows_cap, uint8_t *out_failed, bool *changed, cudaStream_t s) {
+    const uint32_t L1 = st.g.num_levels + 1;
+    cdb_status rc;
+    std::vector<std::vector<uint32_t>> rows(L1), child(L1);
+    for (uint32_t r = std::max(first, st.g.lv[0].cnt); r < first + count; ++r) rows[0].push_back(r);
+    for (uint32_t i = 0; i < count; ++i)
+        for (uint32_t L = 1; L <= levels[i]; ++L) rows[L].push_back(first + i);
+    for (uint32_t L = 1; L < L1; ++L) {
+        uint32_t j = 0;   // position in the rows appended one level down (both lists ascend)
+        for (uint32_t r : rows[L]) {
+            if (L == 1) { child[L].push_back(r); continue; }
+            while (rows[L - 1][j] != r) ++j;
+            child[L].push_back(st.g.lv[L - 1].cnt + j);
+        }
+    }
     if (max_batch == 0) max_batch = 4096;
+    max_batch = std::max<uint32_t>(1, std::min(max_batch, count));
+    DevAllocs tmp;
+    uint8_t *d_levels = nullptr, *failed = nullptr;
     uint32_t *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
-    uint8_t *failed = nullptr;
-    CDB_CUDA_TRY(cudaMalloc(&z_nodes, (size_t)max_batch * L1 * 64 * 4));
-    CDB_CUDA_TRY(cudaMalloc(&z_keys, (size_t)max_batch * L1 * 64 * 4));
-    CDB_CUDA_TRY(cudaMalloc(&z_n, (size_t)max_batch * L1 * 4));
-    CDB_CUDA_TRY(cudaMalloc(&failed, max_batch));
+    if ((rc = tmp.get((void **)&d_levels, count)) || (rc = tmp.get((void **)&failed, count)) ||
+        (rc = tmp.get((void **)&z_nodes, (size_t)max_batch * L1 * 64 * 4)) || (rc = tmp.get((void **)&z_keys, (size_t)max_batch * L1 * 64 * 4)) ||
+        (rc = tmp.get((void **)&z_n, (size_t)max_batch * L1 * 4)))
+        return rc;
     const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
     CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    if ((rc = append_levels(st, gh, rows, child, rows_cap, changed, s))) return rc;
+    if (!count) return CDB_OK;
+    // ---- batches
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_levels, levels.data(), count, cudaMemcpyHostToDevice, s));
     BuildArgs a{};
-    a.g = bg.g;
+    a.g = st.g;
     a.sc = sc;
-    a.sc.root_row = n;
+    a.sc.root_row = st.g.root_row;
     a.levels = d_levels;
+    a.lv_first = first;
     a.ef = ef_construction;
     a.shortlist = shortlist;
-    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n; a.failed = failed;
-    cdb_status result = CDB_OK;
-    for (uint32_t done = 0; done < n && result == CDB_OK;) {
-        uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, done / 8));
-        batch = std::min<uint32_t>(batch, n - done);
-        a.first = done;
+    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
+    for (uint32_t done = 0; done < count;) {
+        uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, (uint32_t)(((uint64_t)linked + done) / 8)));
+        batch = std::min<uint32_t>(batch, count - done);
+        a.first = first + done;
         a.count = batch;
+        a.failed = failed + done;
         hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         hnsw_build_link_kernel<<<(batch * 32 + 127) / 128, 128, 0, s>>>(a);
@@ -341,29 +498,109 @@ cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root
     }
     cudaError_t e = cudaStreamSynchronize(s);
     if (e == cudaSuccess) e = cudaGetLastError();
-    cudaFree(z_nodes); cudaFree(z_keys); cudaFree(z_n); cudaFree(failed);
+    if (e == cudaSuccess && out_failed) e = cudaMemcpy(out_failed, failed, count, cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) { set_error(std::string("hnsw build: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
-    // ---- publish as a search graph
-    const std::vector<const uint32_t *> *src[3] = {&t_nr, &t_ad, &t_ch};
+    return CDB_OK;
+}
+
+cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root is row n */, uint32_t num_levels, uint32_t nbrs,
+                             uint32_t nbrs0, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed,
+                             const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s) {
+    if (num_levels + 1 > BUILD_MAX_LEVELS) { set_error("build: too many levels"); return CDB_INVALID_PARAMS; }
+    const uint32_t L1 = num_levels + 1;
+    std::unique_ptr<HnswBuildState> st(new HnswBuildState());
+    st->g.num_levels = num_levels;
+    st->g.root_row = n;
+    st->g.entry = num_levels == 0 ? n : 0;
+    metric_key_range(sc.metric, &st->g.min_key, &st->g.max_key);
     const uint32_t *tbl[3];
     for (int t = 0; t < 3; ++t) {
         void *p = nullptr;
-        if ((rc = dalloc(&p, L1 * sizeof(void *)))) return rc;
-        CDB_CUDA_TRY(cudaMemcpy(p, src[t]->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+        CDB_CUDA_TRY(cudaMalloc(&p, L1 * sizeof(void *)));
+        gh.allocs->push_back(p);
         tbl[t] = (const uint32_t *)p;
     }
-    out_counts->clear();
-    for (uint32_t L = 0; L < L1; ++L) out_counts->push_back(bg.g.lv[L].cnt);
-    *out_nr = t_nr; *out_ad = t_ad; *out_ch = t_ch;
-    out_graph->num_levels = num_levels;
-    out_graph->nbrs = nbrs;
-    out_graph->nbrs0 = nbrs0;
-    out_graph->entry = bg.g.entry;
-    out_graph->root_row = n;
-    out_graph->identity_mask = 1u;   // level 0: node i is row i (lv_local), the search skips the node_row lookup there
-    out_graph->node_row = reinterpret_cast<const uint32_t *const *>(tbl[0]);
-    out_graph->adj = reinterpret_cast<const uint32_t *const *>(tbl[1]);
-    out_graph->child = reinterpret_cast<const uint32_t *const *>(tbl[2]);
+    gh.dev->num_levels = num_levels;
+    gh.dev->nbrs = nbrs;
+    gh.dev->nbrs0 = nbrs0;
+    gh.dev->entry = st->g.entry;
+    gh.dev->root_row = n;
+    gh.dev->identity_mask = 1u;   // level 0: node i is row i (lv_local), the search skips the node_row lookup there
+    gh.dev->node_row = reinterpret_cast<const uint32_t *const *>(tbl[0]);
+    gh.dev->adj = reinterpret_cast<const uint32_t *const *>(tbl[1]);
+    gh.dev->child = reinterpret_cast<const uint32_t *const *>(tbl[2]);
+    // ---- the root on every level (vector_store.rs:44-140); level 0 holds a node for every row, linked once inserted
+    cdb_status rc;
+    bool changed = false;
+    std::vector<std::vector<uint32_t>> rows(L1), child(L1);
+    for (uint32_t i = 0; i <= n; ++i) rows[0].push_back(i);
+    for (uint32_t L = 0; L < L1; ++L) {
+        st->g.lv[L].nb = L == 0 ? nbrs0 : nbrs;
+        if (L) { rows[L] = {n}; child[L] = {L == 1 ? n : 0u}; }
+    }
+    if ((rc = append_levels(*st, gh, rows, child, n + 1, &changed, s))) return rc;
+    // ---- then every data row through the insert path
+    std::vector<uint8_t> levels(n);
+    for (uint32_t r = 0; r < n; ++r) levels[r] = draw_level(seed, r, num_levels);
+    if ((rc = insert_rows(sc, gh, *st, 0, n, levels, 0, ef_construction, shortlist, max_batch, n + 1, nullptr, &changed, s))) return rc;
+    *out_state = st.release();
+    return CDB_OK;
+}
+
+cdb_status hnsw_insert_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, uint32_t n_new, const uint8_t *max_level,
+                              uint64_t seed, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t rows_cap,
+                              uint8_t *out_failed, bool *changed, cudaStream_t s) {
+    const uint32_t first = (*gh.cnt)[0], num_levels = st->g.num_levels;   // the published graph
+    std::vector<uint8_t> levels(n_new);
+    for (uint32_t i = 0; i < n_new; ++i)
+        levels[i] = max_level ? (uint8_t)std::min<uint32_t>(max_level[i], num_levels) : draw_level(seed, first + i, num_levels);
+    return insert_rows(sc, gh, *st, first, n_new, levels, first - 1, ef_construction, shortlist, max_batch, rows_cap, out_failed, changed, s);
+}
+
+cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s) {
+    const GraphDev &d = *gh.dev;
+    const uint32_t L1 = d.num_levels + 1;
+    if (L1 > BUILD_MAX_LEVELS) { set_error("the graph has more levels than the builder supports"); return CDB_UNSUPPORTED; }
+    const uint32_t rows_fit = SS_STAGE_BYTES / sc.row_pitch;   // node row + `group` neighbour rows per warp
+    const uint32_t group = rows_fit >= 2 ? std::min<uint32_t>(32, rows_fit - 1) : 1u;
+    const size_t smem = (size_t)SS_WARPS * (group + 1) * sc.row_pitch;
+    int dev = 0, optin = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    if (smem + SS_WARPS * 8 > (size_t)optin) { set_error("slot state: rows too wide for shared memory"); return CDB_UNSUPPORTED; }
+    CDB_ALLOW_SMEM(hnsw_slot_state_kernel, smem);
+    std::unique_ptr<HnswBuildState> st(new HnswBuildState());
+    st->g.num_levels = d.num_levels;
+    st->g.entry = d.entry;
+    st->g.root_row = d.root_row;
+    metric_key_range(sc.metric, &st->g.min_key, &st->g.max_key);
+    HnScoreCtx c = sc;
+    c.root_row = d.root_row;
+    for (uint32_t L = 0; L < L1; ++L) {
+        BuildLevel &l = st->g.lv[L];
+        l.cnt = l.app = (*gh.cnt)[L];
+        l.nb = L == 0 ? d.nbrs0 : d.nbrs;
+        l.node_row = const_cast<uint32_t *>((*gh.nr)[L]);
+        l.adj = const_cast<uint32_t *>((*gh.ad)[L]);
+        l.child = L ? const_cast<uint32_t *>((*gh.ch)[L]) : nullptr;
+        st->cap[L] = l.cnt;
+        void *p[4];
+        const size_t words[4] = {(size_t)l.cnt * l.nb, l.cnt, l.cnt, l.cnt};
+        for (int t = 0; t < 4; ++t) {
+            CDB_CUDA_TRY(cudaMalloc(&p[t], std::max<size_t>(words[t], 1) * 4));
+            gh.allocs->push_back(p[t]);
+        }
+        l.simkey = (uint32_t *)p[0]; l.lowest_idx = (uint32_t *)p[1]; l.lowest_key = (uint32_t *)p[2]; l.lock = (int *)p[3];
+        CDB_CUDA_TRY(cudaMemsetAsync(l.simkey, 0, words[0] * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(l.lock, 0, (size_t)l.cnt * 4, s));
+        if (!l.cnt) continue;
+        const uint32_t grid = (l.cnt + SS_WARPS - 1) / SS_WARPS;
+        hnsw_slot_state_kernel<<<grid, SS_WARPS * 32, smem, s>>>(l, c, st->g.min_key, st->g.max_key, group);
+        CDB_LAUNCH_CHECK();
+    }
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error(std::string("hnsw slot state: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    *out_state = st.release();
     return CDB_OK;
 }
 
@@ -385,15 +622,12 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
         levels[t] = (uint8_t)std::min<uint32_t>(rh.max_level[t], num_levels);
         for (uint32_t L = 0; L <= levels[t]; ++L) members[L].push_back(t);
     }
-    BuiltGraph bg;
-    bg.g.num_levels = num_levels;
-    bg.g.root_row = rh.main_root_row;
-    bg.g.entry = 0;
-    bg.g.pseudo_entry = 1;
-    switch (sc.metric) {
-    case CDB_METRIC_COSINE: bg.g.min_key = order_key(sc.metric, 0xBF800000u); bg.g.max_key = order_key(sc.metric, 0x40000000u); break;
-    default: bg.g.min_key = order_key(sc.metric, 0xFF800000u); bg.g.max_key = order_key(sc.metric, 0x7F800000u); break;
-    }
+    BuildGraph bg{};
+    bg.num_levels = num_levels;
+    bg.root_row = rh.main_root_row;
+    bg.entry = 0;
+    bg.pseudo_entry = 1;
+    metric_key_range(sc.metric, &bg.min_key, &bg.max_key);
     auto dalloc = [&](void **p, size_t bytes) -> cdb_status {
         CDB_CUDA_TRY(cudaMalloc(p, bytes ? bytes : 4));
         out_allocs->push_back(*p);
@@ -425,7 +659,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
     rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
     std::vector<const uint32_t *> t_nr(L1), t_ad(L1), t_ch(L1), t_id(L1), t_md(L1);
     for (uint32_t L = 0; L < L1; ++L) {
-        BuildLevel &l = bg.g.lv[L];
+        BuildLevel &l = bg.lv[L];
         const std::vector<uint32_t> &mem = members[L];
         l.nb = L == 0 ? nbrs0 : nbrs;
         l.cnt = 2 + (uint32_t)mem.size();
@@ -455,7 +689,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
         CDB_LAUNCH_CHECK();
         CDB_CUDA_TRY(cudaMemsetAsync(l.simkey, 0, slots * 4, s));
         CDB_CUDA_TRY(cudaMemsetAsync(l.lowest_idx, 0, (size_t)l.cnt * 4, s));
-        fill_u32_kernel<<<(l.cnt + 255) / 256, 256, 0, s>>>(l.lowest_key, bg.g.min_key, l.cnt);
+        fill_u32_kernel<<<(l.cnt + 255) / 256, 256, 0, s>>>(l.lowest_key, bg.min_key, l.cnt);
         CDB_LAUNCH_CHECK();
         CDB_CUDA_TRY(cudaMemsetAsync(l.lock, 0, (size_t)l.cnt * 4, s));
         t_nr[L] = l.node_row; t_ad[L] = l.adj; t_ch[L] = l.child; t_id[L] = l.node_id; t_md[L] = l.node_md;
@@ -473,7 +707,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
     const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
     CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
     BuildArgs a{};
-    a.g = bg.g;
+    a.g = bg;
     a.sc = sc;
     a.sc.root_row = rh.main_root_row;
     a.levels = d_levels;
@@ -510,7 +744,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
         tbl[t] = (const uint32_t *)q;
     }
     out_counts->clear();
-    for (uint32_t L = 0; L < L1; ++L) out_counts->push_back(bg.g.lv[L].cnt);
+    for (uint32_t L = 0; L < L1; ++L) out_counts->push_back(bg.lv[L].cnt);
     *out_nr = t_nr; *out_ad = t_ad; *out_ch = t_ch;
     out_graph->num_levels = num_levels;
     out_graph->nbrs = nbrs;

@@ -155,11 +155,32 @@ cdb_status hnsw_dedup_md_device(const uint32_t *d_ids, const uint32_t *d_rows, c
 
 // ---- hnsw_build.cu
 struct HnScoreCtx;
+// the index's graph as the builder sees it: the search layout, the allocations that own every level array (per-level
+// arrays are replaced when a level grows) and host copies of the per-level device pointers
+struct GraphHost {
+    GraphDev *dev;
+    std::vector<void *> *allocs;
+    std::vector<uint32_t> *cnt;
+    std::vector<const uint32_t *> *nr, *ad, *ch;
+};
+// the builder's per-slot state (similarity keys, stale lowest_index, node locks), kept next to the graph it belongs to
+struct HnswBuildState;
+void hnsw_state_free(HnswBuildState *st);
+// cdb_index_build_graph: root row n on every level, then rows [0, n) inserted
 cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
-                             uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed, GraphDev *out_graph,
-                             std::vector<void *> *out_allocs, std::vector<uint32_t> *out_counts,
-                             std::vector<const uint32_t *> *out_nr, std::vector<const uint32_t *> *out_ad,
-                             std::vector<const uint32_t *> *out_ch, cudaStream_t s);
+                             uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed, const GraphHost &gh,
+                             HnswBuildState **out_state, cudaStream_t s);
+// slot state of a graph that came from elsewhere (cdb_index_set_graph), under the reload semantics of
+// ProbNode::new_with_neighbors_and_versions; sc.root_row = the graph's root row
+cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s);
+// cdb_index_insert_graph: rows [cnt[0], cnt[0] + n_new) inserted into the graph; max_level = NULL draws from `seed`;
+// rows_cap bounds level 0; out_failed[n_new] may be NULL.  Every allocation precedes the first change: an error with
+// *changed == false left the graph as it was, with *changed == true the graph is half-inserted and must be dropped.
+cdb_status hnsw_insert_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, uint32_t n_new, const uint8_t *max_level,
+                              uint64_t seed, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t rows_cap,
+                              uint8_t *out_failed, bool *changed, cudaStream_t s);
+// similarity keys of every slot of `level` ([cnt*nb], device)
+const uint32_t *hnsw_state_slot_keys(const HnswBuildState *st, uint32_t level);
 
 // replica lists: one entry per graph node to create, host arrays (cdb_replica_build)
 struct ReplicaHost {

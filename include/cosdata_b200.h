@@ -365,6 +365,32 @@ cdb_status cdb_index_read_graph_metadata_level(const cdb_index *index, uint32_t 
 /* read the current graph back: info5 = {num_levels, neighbors_count, level0_neighbors_count, entry, root_row} */
 cdb_status cdb_index_graph_info(const cdb_index *index, uint32_t *info5, uint32_t *level_counts /* [num_levels+1] or NULL */);
 cdb_status cdb_index_read_graph_level(const cdb_index *index, uint32_t level, uint32_t *node_row, uint32_t *adjacency, uint32_t *child);
+/* GPU-side index_embeddings on the current graph (src/vector_store.rs:714-940): inserts every row appended since the graph
+ * was built / uploaded, i.e. rows [level_counts[0], cdb_index_size()), in ascending row order, with the same traversal and
+ * create_node_edges / add_neighbor as cdb_index_build_graph (which is this insert applied to a graph holding only the root).
+ * params->num_levels / neighbors_count / level0_neighbors_count must equal the graph's (else CDB_INVALID_PARAMS);
+ * ef_construction, shortlist_size, max_batch as for the build, batches of max(1, min(max_batch, rows already linked / 8));
+ * max_batch = 1 inserts one row at a time (deterministic).  max_level[n_new] (may be NULL): the caller's
+ * get_max_insert_level draws, clamped to num_levels; NULL = the build's counter RNG on the row index with params->seed.
+ * out_failed[n_new] (may be NULL): 1 where the reference's insert returns Err (the node stays unlinked).
+ * Each node keeps the add_neighbor state of the reference: a similarity per slot and a lowest_index that eviction leaves
+ * stale.  A graph built on this handle keeps its state in memory; a graph from cdb_index_set_graph gets it derived on the
+ * first insert as the reference derives it when it loads nodes from storage (ProbNode::new_with_neighbors_and_versions,
+ * prob_node.rs:145-181: every slot's similarity recomputed, lowest_index = the first empty slot, else the first slot with
+ * the strictly lowest similarity).  A slot whose pair is an Err (e.g. a zero-norm row under cosine) gets MetricResult::min
+ * and is the first slot replaced.  Graphs with metadata (cdb_index_set_graph_metadata, *_replicas, *_from_files):
+ * CDB_UNSUPPORTED.  No new rows: CDB_OK, *out_inserted = 0.  The level-0 list must be rows 0..level_counts[0]-1.
+ * Takes the writer lock; searches enqueued (cdb_search_batch_device) before the call see the old graph, searches after it
+ * the new one; the call returns once the graph is complete.  Failure: every device allocation happens before the graph
+ * changes, so an error there (e.g. CDB_CUDA_ERROR on out-of-memory) leaves the graph and its rows as they were and the call
+ * can be repeated.  An error after the graph started changing (a failed kernel or copy) drops the graph: the index has none
+ * until cdb_index_build_graph / cdb_index_set_graph, and cdb_last_error_string says so. */
+cdb_status cdb_index_insert_graph(cdb_index *index, const cdb_build_params *params, const uint8_t *max_level, uint8_t *out_failed,
+                                  uint64_t *out_inserted);
+/* similarity stored with each neighbour slot of `level` (level_counts[level] x neighbours f32, the MetricResult value; 0 for
+ * empty slots): what the reference's serializer writes next to each link (serializer/hnsw/neighbors.rs:53-57).  Derived
+ * as above for an uploaded graph.  Graphs with metadata: CDB_UNSUPPORTED. */
+cdb_status cdb_index_read_graph_slot_scores(cdb_index *index, uint32_t level, float *out_scores);
 /* cumulative {distance evaluations, pops} of CDB_MODE_HNSW searches (roofline accounting) */
 cdb_status cdb_index_hnsw_counters(const cdb_index *index, uint64_t *out2);
 

@@ -166,6 +166,23 @@ class DenseIndex {
         failed.resize(rb.n_nodes);
         return failed;
     }
+    // index_embeddings on the live graph: inserts the rows appended since it was built / uploaded; max_level = the caller's
+    // get_max_insert_level draws (empty: the seeded counter RNG); returns the per-row "insert failed" flags
+    std::vector<uint8_t> insert_graph(const cdb_build_params &bp, const std::vector<uint8_t> &max_level = {}) {
+        std::vector<uint8_t> failed(std::max<uint64_t>(cdb_index_size(h_), 1));
+        uint64_t n = 0;
+        check(cdb_index_insert_graph(h_, &bp, max_level.empty() ? nullptr : max_level.data(), failed.data(), &n));
+        failed.resize(n);
+        return failed;
+    }
+    // similarity of every neighbour slot of `level` (0 for empty slots), as the reference's serializer stores it
+    std::vector<float> read_graph_slot_scores(uint32_t level) {
+        uint32_t info[5], counts[32];
+        check(cdb_index_graph_info(h_, info, counts));
+        std::vector<float> out((size_t)counts[level] * (level == 0 ? info[2] : info[1]));
+        check(cdb_index_read_graph_slot_scores(h_, level, out.data()));
+        return out;
+    }
     // raw f32 rows for rows appended as codes (cold start of a quantized index)
     void set_raw(uint64_t first_row, const float *vecs, uint64_t n) { check(cdb_index_set_raw_f32(h_, first_row, vecs, n)); }
     uint64_t raw_missing() const { return cdb_index_raw_missing(h_); }
