@@ -425,6 +425,8 @@ cdb_status cdb_index_create(const cdb_index_desc *d, cdb_index **out) {
     CDB_REQUIRE(d->dim > 0 && d->storage_type >= CDB_ST_U8 && d->storage_type <= CDB_ST_LAST, "bad dim/storage type");
     CDB_REQUIRE(d->metric >= CDB_METRIC_COSINE && d->metric <= CDB_METRIC_DOT_PRODUCT, "bad metric");
     CDB_REQUIRE(d->capacity > 0 && d->capacity < 0xFFFFFFFFull, "capacity must be in 1..2^32-2");
+    // 0xFFFFFFFF is CDB_INVALID_ID (an empty result slot): no row may carry it
+    CDB_REQUIRE((uint64_t)d->id_base + d->capacity <= 0xFFFFFFFFull, "id_base + capacity must not exceed 2^32-1");
     CDB_CUDA_TRY(cudaSetDevice(d->device));
     int sms = 0;
     CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d->device));
@@ -625,20 +627,26 @@ cdb_status cdb_index_set_raw_f32(cdb_index *ix, uint64_t first_row, const float 
         if (ix->raw_mags_owned &&
             (rc = raw_mags_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, m, dim, ix->d_raw_mags + first, ix->stream)))
             return rc;
-        if (ix->d_xh) {
-            if ((rc = normalize_f16_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, m, dim,
-                                           (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->stream)) ||
-                (rc = classify_rows_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, m, dim,
-                                           (uint32_t)first, ix->deg.as<uint32_t>(), ix->stream)))
-                return rc;
-            CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 4, ix->deg.p, 8, cudaMemcpyDeviceToHost, ix->stream));
-        }
+        if (ix->d_xh &&
+            (rc = normalize_f16_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, m, dim,
+                                       (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->stream)))
+            return rc;
         CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
-        if (ix->d_xh) { ix->n_allzero_rows = ix->h_flags[4]; ix->n_odd_rows = ix->h_flags[5]; }
     }
     if (ix->raw_have.size() < ix->size) ix->raw_have.resize(ix->size, true);
     for (uint64_t r = first_row; r < first_row + n; ++r)
         if (!ix->raw_have[r]) { ix->raw_have[r] = true; --ix->raw_missing; }
+    // The rows may have been classified before (set twice, or appended as f32): classifying only this range would count
+    // its degenerate rows again.  Once every raw row is present, recount the whole index instead.
+    if (ix->d_xh && ix->raw_missing == 0) {
+        CDB_CUDA_TRY(cudaMemsetAsync(ix->deg.p, 0, 8, ix->stream));
+        cdb_status rc = classify_rows_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, dim, 0, ix->deg.as<uint32_t>(), ix->stream);
+        if (rc) return rc;
+        CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 4, ix->deg.p, 8, cudaMemcpyDeviceToHost, ix->stream));
+        CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+        ix->n_allzero_rows = ix->h_flags[4];
+        ix->n_odd_rows = ix->h_flags[5];
+    }
     return CDB_OK;
 }
 
@@ -865,7 +873,9 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
     // ---- wgmma prefilter + exact re-rank: identical results, far fewer exact dot products.
     // Needs k proper (non-degenerate) rows for the bound to exist, and few enough odd degenerate rows to carry them on
     // every candidate list (tensor_scan.cu).
+    // The exact re-rank holds the query in shared memory, which bounds the dimension.
     const bool tensor_ok = raw && ix->d_xh && !p->exact_only && nq >= 4 && ix->size >= 16384 && p->k <= 64 &&
+                           d.dim <= rerank_f32_max_dim() &&
                            ix->n_odd_rows <= TS_MAX_ODD && ix->size - ix->n_allzero_rows - ix->n_odd_rows >= p->k &&
                            tensor_scan_smem_bytes(p->k) <= 227 * 1024 && (nq + 127) / 128 <= (uint32_t)ix->sm_count;
     // search_internal: quantize the query with the index's storage type and range (hnsw/mod.rs:399-403);
@@ -913,8 +923,12 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         qsel = sc->qsel.as<uint32_t>();  // the exact scan below only runs (on the device's own decision) for the queries listed there
     }
     // ---- exact integer scoring on wgmma u8: u8 codes in place, sub-byte codes through the digit copy
+    // The s32 accumulator holds at most max_digit^2 * D, and the dot-product filter reads its bits as a float: both are
+    // exact only while that bound is a finite float bit pattern (u8 codes: D <= 32896); above it the exact scan answers.
     const uint8_t *u8_rows = !raw ? (st == CDB_ST_U8 ? ix->d_codes : ix->d_digits) : nullptr;
+    const uint64_t max_digit = st == CDB_ST_U8 ? 255u : (1u << st) - 1u;
     const bool u8_ok = u8_rows && !p->exact_only && (metric == CDB_METRIC_COSINE || metric == CDB_METRIC_DOT_PRODUCT) &&
+                       max_digit * max_digit * d.dim <= 0x7F7FFFFFull &&
                        ix->size >= 16384 && p->k <= 64 && tensor_u8_smem_bytes(p->k) <= 227 * 1024 &&
                        (nq + 127) / 128 <= (uint32_t)ix->sm_count;
     if (u8_ok) {

@@ -187,6 +187,8 @@ __global__ void __launch_bounds__(RERANK_THREADS) rerank_f32_kernel(
     if (threadIdx.x == 0 && out_counts) out_counts[b] = nout;
 }
 
+uint32_t rerank_f32_max_dim() { return (200 * 1024 - RERANK_BUF * 8) / 4; }
+
 cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const float *d_raw_mags, uint64_t n_rows,
                              uint32_t dim, const float *d_q, uint32_t q_pitch_elems, const float *d_qmags, uint32_t nq,
                              const uint32_t *d_cand, const uint32_t *d_cand_counts, uint32_t ncand, uint32_t k, uint32_t id_base,

@@ -511,6 +511,8 @@ cdb_status prep_queries_device(const float *d_q, uint32_t nq, uint32_t dim, floa
                                uint32_t *d_cand, uint32_t cand_cap, uint32_t *d_cand_cnt, uint32_t *d_err32, uint8_t *d_err8,
                                uint32_t *d_progress, cudaStream_t s) {
     const uint32_t mtiles = (nq + TS_BLOCK_M - 1) / TS_BLOCK_M;
+    // dim*4 bytes of squares: above 12287 dims that exceeds the 48 KB a launch gets without the opt-in
+    CDB_ALLOW_SMEM(prep_queries_kernel, (size_t)dim * 4);
     prep_queries_kernel<<<mtiles * TS_BLOCK_M, 128, (size_t)dim * 4, s>>>(d_q, nq, dim, d_q_raw, raw_pitch_elems, d_q_mags,
                                                                           reinterpret_cast<__half *>(d_qh), qh_pitch_halfs, d_ggm, d_deg,
                                                                           has_deg ? 1u : 0u, id_base, d_cand, cand_cap, d_cand_cnt, d_err32,

@@ -4,7 +4,9 @@
 // dot_product_u8 (src/models/dot_product/x86_64.rs:22-66) and the bit-plane products
 // dot_product_binary/quaternary/octal (src/models/dot_product.rs:21-90) are integer contractions
 //   sum_i a_i * b_i   with a_i, b_i in 0..255 (u8) or the sub-byte digits 0..1 / 0..3 / 0..7,
-// so wgmma .s32.u8.u8 (u8 x u8 -> s32 in registers) computes them bit-exactly: max 255*255*D < 2^31.
+// so wgmma .s32.u8.u8 (u8 x u8 -> s32 in registers) computes them bit-exactly as long as max_digit^2 * D stays below 2^31.
+// The dot-product filter also reads the s32 bits as a float, which is only finite up to 0x7F7FFFFF: search_chunk_locked
+// (api.cu) sends a shard to the exact scan unless max_digit^2 * D <= 0x7F7FFFFF (u8 codes: D <= 32896).
 // u8 storage is consumed in place; sub-byte storage through an unpacked digit copy (digit =
 // plane0 + 2*plane1 + 4*plane2, exactly the weights the reference kernels apply).
 //

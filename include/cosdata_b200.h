@@ -107,7 +107,7 @@ typedef struct {
     int32_t device;         /* CUDA ordinal */
     int32_t keep_raw_f32;   /* keep raw f32 rows for the exact re-rank
                                (Collection.internal_to_external_map, collection.rs:110) */
-    uint32_t id_base;       /* global id of local row 0 (corpus shard offset) */
+    uint32_t id_base;       /* global id of local row 0 (corpus shard offset); id_base + capacity <= 2^32-1 */
     uint32_t tensor_prefilter; /* 1: also keep an fp16 copy of the L2-normalised raw rows so that large
                                   batches use the wgmma prefilter + exact re-rank (results identical) */
 } cdb_index_desc;
