@@ -579,6 +579,26 @@ class DenseIndex:
                                                 C.byref(done)))
         return failed[: done.value]
 
+    def delete_rows(self, rows, shortlist_size=64, max_batch=0):
+        """delete_embedding on the GPU (cdb_index_delete_rows) for local row numbers -> status u8[len(rows)]: 0 deleted,
+        1 already deleted, 2 deleted but an Err stopped some relinks"""
+        r = np.asarray(rows)
+        if r.ndim != 1:
+            raise ValueError(f"rows must be one-dimensional, got shape {r.shape}")
+        if r.size and (r.min() < 0 or r.max() >= self.size):
+            raise ValueError(f"rows must be in 0..{self.size - 1}")
+        check_insert_args(1, shortlist_size, max_batch)
+        r = np.ascontiguousarray(r, dtype=np.uint32)
+        status = np.zeros(max(r.size, 1), dtype=np.uint8)
+        _check(self._lib.cdb_index_delete_rows(self._h, _ptr(r), r.size, shortlist_size, max_batch, _ptr(status), None))
+        return status[: r.size]
+
+    def deleted_rows(self):
+        """-> bool[size]: True where the row is deleted"""
+        out = np.zeros(max(self.size, 1), dtype=np.uint8)
+        _check(self._lib.cdb_index_deleted_rows(self._h, 0, self.size, _ptr(out), None))
+        return out[: self.size].astype(bool)
+
     def read_graph_slot_scores(self):
         """-> [f32[level_counts[L] * neighbours]] per level: the similarity stored with each neighbour slot (0 = empty slot)"""
         info = np.zeros(5, dtype=np.uint32)

@@ -7,6 +7,7 @@
 #include <memory>
 #include <mutex>
 #include <shared_mutex>
+#include <unordered_set>
 #include <vector>
 
 #include "kernels.h"
@@ -196,6 +197,14 @@ struct cdb_index {
     std::vector<const uint32_t *> g_id, g_md;        // same for node_id / node_md when has_md
     DevBuf hn_counters, hn_prof;   // cumulative device counters (atomics: shared by concurrent searches)
     bool hn_prof_on = false;
+    // deleted rows (cdb_index_delete_rows): bitmap over the capacity, allocated on the first delete; kernels get nullptr
+    // while no row is deleted
+    uint32_t *d_deleted = nullptr;
+    std::vector<uint32_t> h_deleted;
+    uint64_t n_deleted = 0;
+    const uint32_t *del_dev() const { return n_deleted ? d_deleted : nullptr; }
+    const uint32_t *del_host() const { return n_deleted ? h_deleted.data() : nullptr; }
+    bool is_deleted(uint64_t row) const { return n_deleted && ((h_deleted[row >> 5] >> (row & 31)) & 1u); }
 };
 
 // a leased scratch set; returned to the pool (and remembered as "last") on destruction
@@ -489,6 +498,7 @@ cdb_status cdb_index_destroy(cdb_index *ix) {
     if (ix->raw_mags_owned && ix->d_raw_mags) cudaFree(ix->d_raw_mags);
     if (ix->d_xh) cudaFree(ix->d_xh);
     if (ix->d_digits) cudaFree(ix->d_digits);
+    if (ix->d_deleted) cudaFree(ix->d_deleted);
     hnsw_state_free(ix->bstate);
     for (void *g : ix->graph_allocs) cudaFree(g);
     for (void *g : ix->md_allocs) cudaFree(g);
@@ -713,6 +723,7 @@ static cdb_status exact_scan_locked(cdb_index *ix, Scratch *sc, bool raw, int st
     if ((rc = sc->partial.ensure(std::max(part_full, part_sel))) || (rc = sc->err32.ensure((size_t)nq * 4))) return rc;
     a.partial = sc->partial.as<uint64_t>();
     a.err32 = sc->err32.as<uint32_t>();
+    a.deleted = ix->del_dev();
     if (!qsel) CDB_CUDA_TRY(cudaMemsetAsync(a.err32, 0, (size_t)nq * 4, s));   // the tensor-core path prepared it otherwise
     if (qsel) {
         a.sel_mode = 1;
@@ -874,7 +885,8 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
     // Needs k proper (non-degenerate) rows for the bound to exist, and few enough odd degenerate rows to carry them on
     // every candidate list (tensor_scan.cu).
     // The exact re-rank holds the query in shared memory, which bounds the dimension.
-    const bool tensor_ok = raw && ix->d_xh && !p->exact_only && nq >= 4 && ix->size >= 16384 && p->k <= 64 &&
+    // The tensor-core paths know nothing of deleted rows: once a row is deleted the exact scan answers.
+    const bool tensor_ok = raw && ix->d_xh && !p->exact_only && ix->n_deleted == 0 && nq >= 4 && ix->size >= 16384 && p->k <= 64 &&
                            d.dim <= rerank_f32_max_dim() &&
                            ix->n_odd_rows <= TS_MAX_ODD && ix->size - ix->n_allzero_rows - ix->n_odd_rows >= p->k &&
                            tensor_scan_smem_bytes(p->k) <= 227 * 1024 && (nq + 127) / 128 <= (uint32_t)ix->sm_count;
@@ -927,7 +939,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
     // exact only while that bound is a finite float bit pattern (u8 codes: D <= 32896); above it the exact scan answers.
     const uint8_t *u8_rows = !raw ? (st == CDB_ST_U8 ? ix->d_codes : ix->d_digits) : nullptr;
     const uint64_t max_digit = st == CDB_ST_U8 ? 255u : (1u << st) - 1u;
-    const bool u8_ok = u8_rows && !p->exact_only && (metric == CDB_METRIC_COSINE || metric == CDB_METRIC_DOT_PRODUCT) &&
+    const bool u8_ok = u8_rows && !p->exact_only && ix->n_deleted == 0 && (metric == CDB_METRIC_COSINE || metric == CDB_METRIC_DOT_PRODUCT) &&
                        max_digit * max_digit * d.dim <= 0x7F7FFFFFull &&
                        ix->size >= 16384 && p->k <= 64 && tensor_u8_smem_bytes(p->k) <= 227 * 1024 &&
                        (nq + 127) / 128 <= (uint32_t)ix->sm_count;
@@ -1246,6 +1258,9 @@ cdb_status cdb_index_set_graph(cdb_index *ix, const cdb_graph_desc *gd) {
         }
         for (size_t t = 0; t < (size_t)cnt * nb; ++t)
             CDB_REQUIRE(gd->adjacency[L][t] == CDB_INVALID_ID || gd->adjacency[L][t] < cnt, "adjacency entry out of range");
+        for (size_t t = 0; ix->n_deleted && t < (size_t)cnt * nb; ++t)   // no live link to a deleted row
+            CDB_REQUIRE(gd->adjacency[L][t] == CDB_INVALID_ID || !ix->is_deleted(gd->node_row[L][gd->adjacency[L][t]]),
+                        "an adjacency entry names a deleted row");
     }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     hnsw_state_free(ix->bstate);
@@ -1383,7 +1398,8 @@ cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
     ix->has_graph = false;
     HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, n};
     rc = hnsw_build_device(sc, n, bp->num_levels, bp->neighbors_count, bp->level0_neighbors_count, bp->ef_construction,
-                           bp->shortlist_size, bp->max_batch, bp->seed, graph_host(ix), &ix->bstate, ix->stream);
+                           bp->shortlist_size, bp->max_batch, bp->seed, graph_host(ix), &ix->bstate, ix->stream, ix->del_dev(),
+                           ix->del_host());
     if (rc) return rc;
     ix->has_graph = true;
     return CDB_OK;
@@ -1406,6 +1422,7 @@ cdb_status cdb_index_build_graph_replicas(cdb_index *ix, const cdb_build_params 
     for (uint32_t t = 0; t < rb->n_nodes; ++t) {
         CDB_REQUIRE(rb->row[t] == CDB_INVALID_ID || rb->row[t] < n, "replica row out of range");
         CDB_REQUIRE(rb->md_row[t] == CDB_INVALID_ID || rb->md_row[t] < rb->n_md, "replica md_row out of range");
+        CDB_REQUIRE(rb->row[t] == CDB_INVALID_ID || !ix->is_deleted(rb->row[t]), "replica row is deleted");
     }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     cdb_status rc;
@@ -1512,7 +1529,8 @@ cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, con
     HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
     bool changed = false;
     if ((rc = hnsw_insert_device(sc, graph_host(ix), ix->bstate, (uint32_t)n_new, max_level, bp->seed, bp->ef_construction,
-                                 bp->shortlist_size, bp->max_batch, ix->desc.capacity, out_failed, &changed, ix->stream))) {
+                                 bp->shortlist_size, bp->max_batch, ix->desc.capacity, out_failed, &changed, ix->stream, ix->del_dev(),
+                                 ix->del_host()))) {
         if (changed) {   // a half-inserted graph is not the reference's graph: the index has none until a build / upload
             const std::string why = cdb_last_error_string();
             hnsw_state_free(ix->bstate);
@@ -1525,6 +1543,89 @@ cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, con
         return rc;
     }
     if (out_inserted) *out_inserted = n_new;
+    return CDB_OK;
+}
+
+cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
+                                 uint8_t *out_status, uint64_t *out_deleted) {
+    CDB_REQUIRE(ix && (rows || !n), "null argument");
+    CDB_REQUIRE(shortlist_size >= 1 && shortlist_size <= 64, "shortlist_size must be in 1..64");
+    if (out_deleted) *out_deleted = 0;
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    for (uint64_t i = 0; i < n; ++i) {
+        CDB_REQUIRE(rows[i] < ix->size, "row out of range");
+        CDB_REQUIRE(!ix->has_graph || rows[i] != ix->graph.root_row, "the graph's root row cannot be deleted");
+    }
+    if (ix->has_graph && ix->has_md) { set_error("delete from a graph with metadata is not supported"); return CDB_UNSUPPORTED; }
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    // status 1 for rows deleted before or earlier in the list
+    std::vector<uint8_t> status(n, 1);
+    std::vector<uint32_t> fresh;
+    std::unordered_set<uint32_t> seen;
+    for (uint64_t i = 0; i < n; ++i)
+        if (!ix->is_deleted(rows[i]) && seen.insert(rows[i]).second) { status[i] = 0; fresh.push_back(rows[i]); }
+    cdb_status rc;
+    if (!fresh.empty()) {
+        const size_t words = ix->desc.capacity / 32 + 1;
+        if (!ix->d_deleted) {   // allocated before anything changes; kernels see it only once a row is deleted
+            void *p = nullptr;
+            CDB_CUDA_TRY(cudaMalloc(&p, words * 4));
+            ix->d_deleted = (uint32_t *)p;
+            ix->h_deleted.assign(words, 0u);
+            CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
+        }
+        {   // searches already enqueued on their callers' streams finish on the old graph and the old marks
+            std::lock_guard<std::mutex> g(ix->pool_mu);
+            for (auto &u : ix->pool)
+                if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
+        }
+        CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+        std::vector<uint8_t> fst(fresh.size(), 0);
+        if (ix->has_graph) {
+            if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
+                set_error("metric/storage arm is an Err in the reference");
+                return rc;
+            }
+            if ((rc = ensure_build_state(ix))) return rc;
+            HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
+            bool changed = false;
+            if ((rc = hnsw_delete_device(sc, graph_host(ix), ix->bstate, fresh.data(), (uint32_t)fresh.size(), shortlist_size, max_batch,
+                                         fst.data(), &changed, ix->stream))) {
+                if (changed) {   // a half-repaired graph links deleted rows: the index has none until a build / upload
+                    const std::string why = cdb_last_error_string();
+                    hnsw_state_free(ix->bstate);
+                    ix->bstate = nullptr;
+                    for (void *g : ix->graph_allocs) cudaFree(g);
+                    ix->graph_allocs.clear();
+                    ix->has_graph = false;
+                    set_error(why + " (the delete had started: the graph was dropped)");
+                }
+                return rc;
+            }
+        }
+        // the marks, once the repair succeeded
+        uint32_t lo = 0xFFFFFFFFu, hi = 0;
+        for (uint32_t r : fresh) {
+            ix->h_deleted[r >> 5] |= 1u << (r & 31);
+            lo = std::min(lo, r >> 5);
+            hi = std::max(hi, r >> 5);
+        }
+        CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted + lo, ix->h_deleted.data() + lo, (size_t)(hi - lo + 1) * 4, cudaMemcpyHostToDevice));
+        ix->n_deleted += fresh.size();
+        size_t j = 0;
+        for (uint64_t i = 0; i < n; ++i)
+            if (status[i] == 0) status[i] = fst[j++];
+        if (out_deleted) *out_deleted = fresh.size();
+    }
+    if (out_status) std::copy(status.begin(), status.end(), out_status);
+    return CDB_OK;
+}
+
+cdb_status cdb_index_deleted_rows(const cdb_index *ix, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total) {
+    CDB_REQUIRE(ix && (out || !n), "null argument");
+    CDB_REQUIRE(first + n <= ix->desc.capacity, "rows out of range");
+    for (uint64_t i = 0; i < n; ++i) out[i] = ix->is_deleted(first + i) ? 1 : 0;
+    if (out_total) *out_total = ix->n_deleted;
     return CDB_OK;
 }
 

@@ -20,6 +20,7 @@
 #include <algorithm>
 #include <array>
 #include <memory>
+#include <unordered_map>
 #include <vector>
 
 #include "hnsw_traverse.cuh"
@@ -65,13 +66,18 @@ struct BuildArgs {
     uint32_t lv_first;
     uint32_t first, count;  // rows [first, first+count) form this batch
     uint32_t ef, shortlist;
-    uint32_t *z_nodes;      // [count][num_levels+1][64]
-    uint32_t *z_keys;       // [count][num_levels+1][64] order keys
-    uint32_t *z_n;          // [count][num_levels+1]
-    uint8_t *failed;        // [count]
+    uint32_t zcap;          // results kept per level: 64 (is_indexing) or 100 (delete_embedding)
+    uint32_t *z_nodes;      // [count][num_levels+1][zcap]
+    uint32_t *z_keys;       // [count][num_levels+1][zcap] order keys
+    uint32_t *z_n;          // [count][num_levels+1] (delete: HN_EMPTY on the level whose traversal failed and below)
+    uint8_t *failed;        // [count] 1: the traversal returned Err, 2: the row is deleted (not inserted)
     bool replicas;          // rows of the batch are positions of the replica list `rl`
     ReplicaDev rl;
+    const uint32_t *deleted;   // deleted-row bitmap of the index (insert: such rows are skipped) or null
+    const uint32_t *rowlist;   // delete: the batch is rows rowlist[first .. first+count), traversed on every level
 };
+
+__device__ __forceinline__ bool bit_set(const uint32_t *bits, uint32_t i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
 
 // local index of `row` at `level` (level 0: the row itself; level >= 1: binary search in the part of node_row the current
 // call appended -- an uploaded level need not be sorted before it)
@@ -91,13 +97,18 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs
     extern __shared__ __align__(16) uint8_t smem[];
     const HnSmem m = hn_carve(smem, a.sc.row_pitch, a.ef);
     __shared__ HnShared sh;
-    const uint32_t b = blockIdx.x, r = a.first + b;
+    const uint32_t b = blockIdx.x, r = a.rowlist ? a.rowlist[a.first + b] : a.first + b;
     const int tid = threadIdx.x;
+    const bool del = a.rowlist != nullptr;
+    if (!del && !a.replicas && a.deleted && bit_set(a.deleted, r)) {   // a deleted row is not inserted
+        if (tid == 0) a.failed[b] = 2;
+        return;
+    }
     const uint32_t vrow = a.replicas ? a.rl.row[r] : r;
     for (uint32_t i = tid; i < a.sc.row_pitch / 4; i += HN_THREADS)
         reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(a.sc.rows + (size_t)vrow * a.sc.row_pitch)[i];
     const float qmag = a.sc.mags[vrow];
-    const uint32_t max_level = a.levels[r - a.lv_first];
+    const uint32_t max_level = del ? a.g.num_levels : a.levels[r - a.lv_first];
     const uint32_t L1 = a.g.num_levels + 1;
     // replica builds: the traversal carries the embedding's metadata and prop_value.id (vector_store.rs:809-821); nodes whose
     // metadata has mag != 0 (Pseudo / Metadata kinds) start at the pseudo root (:461-483, 755-758)
@@ -120,11 +131,16 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs
         const BuildLevel &l = a.g.lv[level];
         const uint32_t take = min(min(a.shortlist, l.nb), HN_MAX_TAKE);
         if (a.replicas) { md.node_id = l.node_id; md.node_md = l.node_md; }
-        hn_traverse_level(l.node_row, l.adj, l.nb, take, a.sc, m, sh, qmag, self_id, a.ef, evals, pops, a.replicas ? &md : nullptr);
-        if (sh.err) break;
-        const uint32_t keep = min(sh.rlen, 64u);  // is_indexing: final_len = 64 (vector_store.rs:1194)
+        hn_traverse_level(l.node_row, l.adj, l.nb, take, a.sc, m, sh, qmag, self_id, a.ef, evals, pops, a.replicas ? &md : nullptr,
+                          nullptr, !del);
+        if (sh.err) {
+            if (del && tid == 0)   // D3: no relinks on this level or below
+                for (int lv = level; lv >= 0; --lv) a.z_n[(size_t)b * L1 + lv] = HN_EMPTY;
+            break;
+        }
+        const uint32_t keep = min(sh.rlen, a.zcap);  // final_len: 64 while indexing, 100 otherwise (vector_store.rs:1194)
         if ((uint32_t)level <= max_level) {
-            const size_t base = ((size_t)b * L1 + level) * 64;
+            const size_t base = ((size_t)b * L1 + level) * a.zcap;
             for (uint32_t i = tid; i < keep; i += HN_THREADS) {
                 a.z_nodes[base + i] = m.rnodes[i];
                 a.z_keys[base + i] = (uint32_t)(m.rkeys[i] >> 32);
@@ -195,7 +211,7 @@ __global__ void __launch_bounds__(128) hnsw_build_link_kernel(BuildArgs a) {
     for (uint32_t level = 0; level <= top; ++level) {  // edges are created bottom-up as the recursion unwinds
         const BuildLevel &l = a.g.lv[level];
         const uint32_t node = build_local(l, level, r, a.replicas);
-        const size_t base = ((size_t)b * L1 + level) * 64;
+        const size_t base = ((size_t)b * L1 + level) * a.zcap;
         const uint32_t zn = a.z_n[(size_t)b * L1 + level];
         const bool rules = a.replicas && a.sc.metric == CDB_METRIC_COSINE;   // the rules match MetricResult::CosineSimilarity only
         const int nk = rules ? build_node_kind(a.rl, l, node) : MD_KIND_BASE;
@@ -444,11 +460,15 @@ static cdb_status publish(const HnswBuildState &st, const GraphHost &gh) {
 // in the graph: a fresh build starts almost sequentially, a small transaction into a large graph runs as one batch.
 // Every allocation happens before the graph changes; *changed tells the caller whether an error left it half-inserted.
 static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState &st, uint32_t first, uint32_t count,
-                              const std::vector<uint8_t> &levels, uint32_t linked, uint32_t ef_construction, uint32_t shortlist,
-                              uint32_t max_batch, uint64_t rows_cap, uint8_t *out_failed, bool *changed, cudaStream_t s) {
+                              const std::vector<uint8_t> &levels_in, uint32_t linked, uint32_t ef_construction, uint32_t shortlist,
+                              uint32_t max_batch, uint64_t rows_cap, uint8_t *out_failed, bool *changed, cudaStream_t s,
+                              const uint32_t *d_deleted, const uint32_t *h_deleted) {
     const uint32_t L1 = st.g.num_levels + 1;
     cdb_status rc;
     std::vector<std::vector<uint32_t>> rows(L1), child(L1);
+    std::vector<uint8_t> levels = levels_in;
+    for (uint32_t i = 0; h_deleted && i < count; ++i)   // a deleted row gets no upper-level nodes (and is not linked)
+        if ((h_deleted[(first + i) >> 5] >> ((first + i) & 31)) & 1u) levels[i] = 0;
     for (uint32_t r = std::max(first, st.g.lv[0].cnt); r < first + count; ++r) rows[0].push_back(r);
     for (uint32_t i = 0; i < count; ++i)
         for (uint32_t L = 1; L <= levels[i]; ++L) rows[L].push_back(first + i);
@@ -483,7 +503,9 @@ static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
     a.lv_first = first;
     a.ef = ef_construction;
     a.shortlist = shortlist;
+    a.zcap = 64;
     a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
+    a.deleted = d_deleted;
     for (uint32_t done = 0; done < count;) {
         uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, (uint32_t)(((uint64_t)linked + done) / 8)));
         batch = std::min<uint32_t>(batch, count - done);
@@ -505,7 +527,8 @@ static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
 
 cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root is row n */, uint32_t num_levels, uint32_t nbrs,
                              uint32_t nbrs0, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed,
-                             const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s) {
+                             const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s, const uint32_t *d_deleted,
+                             const uint32_t *h_deleted) {
     if (num_levels + 1 > BUILD_MAX_LEVELS) { set_error("build: too many levels"); return CDB_INVALID_PARAMS; }
     const uint32_t L1 = num_levels + 1;
     std::unique_ptr<HnswBuildState> st(new HnswBuildState());
@@ -542,19 +565,22 @@ cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root
     // ---- then every data row through the insert path
     std::vector<uint8_t> levels(n);
     for (uint32_t r = 0; r < n; ++r) levels[r] = draw_level(seed, r, num_levels);
-    if ((rc = insert_rows(sc, gh, *st, 0, n, levels, 0, ef_construction, shortlist, max_batch, n + 1, nullptr, &changed, s))) return rc;
+    if ((rc = insert_rows(sc, gh, *st, 0, n, levels, 0, ef_construction, shortlist, max_batch, n + 1, nullptr, &changed, s,
+                          d_deleted, h_deleted)))
+        return rc;
     *out_state = st.release();
     return CDB_OK;
 }
 
 cdb_status hnsw_insert_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, uint32_t n_new, const uint8_t *max_level,
                               uint64_t seed, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t rows_cap,
-                              uint8_t *out_failed, bool *changed, cudaStream_t s) {
+                              uint8_t *out_failed, bool *changed, cudaStream_t s, const uint32_t *d_deleted, const uint32_t *h_deleted) {
     const uint32_t first = (*gh.cnt)[0], num_levels = st->g.num_levels;   // the published graph
     std::vector<uint8_t> levels(n_new);
     for (uint32_t i = 0; i < n_new; ++i)
         levels[i] = max_level ? (uint8_t)std::min<uint32_t>(max_level[i], num_levels) : draw_level(seed, first + i, num_levels);
-    return insert_rows(sc, gh, *st, first, n_new, levels, first - 1, ef_construction, shortlist, max_batch, rows_cap, out_failed, changed, s);
+    return insert_rows(sc, gh, *st, first, n_new, levels, first - 1, ef_construction, shortlist, max_batch, rows_cap, out_failed, changed, s,
+                       d_deleted, h_deleted);
 }
 
 cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s) {
@@ -601,6 +627,343 @@ cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, Hns
     cudaError_t e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) { set_error(std::string("hnsw slot state: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
     *out_state = st.release();
+    return CDB_OK;
+}
+
+// ------------------------------------------------------------------ delete_embedding (vector_store.rs:1206-1371)
+// Phase A is hnsw_build_search_kernel in delete mode (rowlist set: nothing pre-seeded, ef 512, best 100 kept).  Phase B runs
+// one warp per (delete, level): remove_neighbor_by_id on each neighbour in D's slot order, relink a neighbour that emptied
+// (create_node_edges over the results, rescored against it), then clear D's slots.  The sweep then clears every remaining
+// slot that names a node deleted in the batch (D2), and the nodes it touched are relinked if empty at their turn, in
+// ascending level-local index when deletes run one at a time.  A level's repair never reads or writes another level.
+struct DelArgs {
+    BuildGraph g;
+    HnScoreCtx sc;
+    const uint32_t *loc;    // [n][num_levels+1] level-local index of each deleted row (HN_EMPTY: not on that level)
+    uint32_t first, count, zcap;
+    const uint32_t *z_nodes, *z_n;
+    uint8_t *status;        // [n] 2 where a rescoring Err stopped a relink
+    uint32_t *dead[BUILD_MAX_LEVELS];      // [cnt/32+1] nodes deleted by this call
+    uint32_t *dead_of[BUILD_MAX_LEVELS];   // [cnt] batch position of a deleted node
+    uint32_t *touched[BUILD_MAX_LEVELS];   // [cnt/32+1] nodes the sweep cleared a slot of
+    uint2 *list[BUILD_MAX_LEVELS];         // [cnt] (node, batch position) of each touched node
+    uint32_t *list_n;                      // [num_levels+1]
+};
+
+__global__ void hnsw_delete_mark_kernel(DelArgs a) {
+    const uint32_t L1 = a.g.num_levels + 1;
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < L1) a.list_n[t] = 0;
+    if (t >= a.count * L1) return;
+    const uint32_t b = t / L1, L = t % L1, D = a.loc[(size_t)(a.first + b) * L1 + L];
+    if (D == HN_EMPTY) return;
+    atomicOr(a.dead[L] + (D >> 5), 1u << (D & 31));
+    a.dead_of[L][D] = b;
+}
+
+// remove_neighbor_by_id (prob_node.rs:285-306): the first slot naming `id` is cleared, lowest_index is left stale
+__device__ bool build_remove_by_id(const BuildLevel &l, uint32_t node, uint32_t id) {
+    volatile uint32_t *na = l.adj + (size_t)node * l.nb;
+    bool found = false;
+    node_lock(l.lock + node);
+    for (uint32_t s = 0; s < l.nb && !found; ++s)
+        if (na[s] == id) { na[s] = HN_EMPTY; found = true; }
+    node_unlock(l.lock + node);
+    return found;
+}
+__device__ bool build_is_empty(const BuildLevel &l, uint32_t node) {
+    const volatile uint32_t *na = l.adj + (size_t)node * l.nb;
+    for (uint32_t s = 0; s < l.nb; ++s)
+        if (na[s] != HN_EMPTY) return false;
+    return true;
+}
+
+struct DelSmem {
+    uint64_t keys[2][128];
+    uint32_t nodes[2][128];
+    uint64_t bar;
+};
+
+// The relink of an emptied node N (vector_store.rs:1306-1357), whole warp: the results minus D, N and the nodes this call
+// deletes are rescored against N (N's row staged by one bulk copy, candidates scored one per lane with pair_distance), sorted
+// best first (ties: smaller id), then lane 0 runs create_node_edges with N's stale lowest_index.  false: a rescoring Err.
+__device__ bool del_relink(const DelArgs &a, uint32_t level, uint32_t N, uint32_t D, const uint32_t *cand, uint32_t zn, uint8_t *row,
+                           DelSmem &sm, uint32_t &parity) {
+    const BuildLevel &l = a.g.lv[level];
+    const HnScoreCtx &sc = a.sc;
+    const uint32_t lane = threadIdx.x & 31, bar = hw_smem_u32(&sm.bar);
+    const uint32_t nrow = l.node_row[N];
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+    if (lane == 0) {
+        hw_mbar_expect(bar, sc.row_pitch);
+        hw_bulk_g2s(hw_smem_u32(row), sc.rows + (size_t)nrow * sc.row_pitch, sc.row_pitch, bar);
+    }
+    hw_mbar_wait(bar, parity);
+    parity ^= 1u;
+    const uint32_t pp = plane_pitch(sc.dim);
+    uint32_t m = 0;
+    bool bad = false;
+    for (uint32_t base = 0; base < zn; base += 32) {
+        const uint32_t i = base + lane;
+        const uint32_t c = i < zn ? cand[i] : HN_EMPTY;
+        const bool keep = c != HN_EMPTY && c != D && c != N && !bit_set(a.dead[level], c);
+        const uint32_t ball = __ballot_sync(0xFFFFFFFFu, keep);
+        if (keep) {
+            const uint32_t crow = l.node_row[c], pos = m + __popc(ball & ((1u << lane) - 1u));
+            float d = 0.f;
+            const int rc = pair_distance(sc.metric, sc.st, sc.dim, row, sc.mags[nrow], pp, sc.rows + (size_t)crow * sc.row_pitch,
+                                         sc.mags[crow], pp, &d);
+            if (rc != CDB_OK) bad = true;
+            sm.keys[0][pos] = make_key64(order_key(sc.metric, __float_as_uint(d)), hn_id(sc.root_row, crow));
+            sm.nodes[0][pos] = c;
+        }
+        m += __popc(ball);
+    }
+    if (__any_sync(0xFFFFFFFFu, bad)) return false;
+    __syncwarp();
+    for (uint32_t i = lane; i < m; i += 32) {   // rank sort, best first (keys are unique: one per node)
+        const uint64_t k = sm.keys[0][i];
+        uint32_t r = 0;
+        for (uint32_t j = 0; j < m; ++j) r += sm.keys[0][j] > k;
+        sm.keys[1][r] = k;
+        sm.nodes[1][r] = sm.nodes[0][i];
+    }
+    __syncwarp();
+    if (lane == 0) {   // create_node_edges (vector_store.rs:976-1070), Base nodes
+        uint32_t successful = 0;
+        for (uint32_t i = 0; i < m; ++i) {
+            if (successful >= l.nb) break;
+            const uint32_t nbr = sm.nodes[1][i], dkey = (uint32_t)(sm.keys[1][i] >> 32);
+            const int idx = build_add_neighbor(a.g, l, N, nbr, dkey);
+            if (idx < 0) continue;
+            if (build_add_neighbor(a.g, l, nbr, N, dkey) >= 0) { successful++; continue; }
+            volatile uint32_t *na = l.adj + (size_t)N * l.nb;
+            node_lock(l.lock + N);
+            if (na[idx] == nbr) na[idx] = HN_EMPTY;
+            node_unlock(l.lock + N);
+        }
+    }
+    __syncwarp();
+    return true;
+}
+
+__device__ inline void del_smem_init(DelSmem &sm) {
+    if ((threadIdx.x & 31) == 0) hw_mbar_init(hw_smem_u32(&sm.bar), 1);
+    __syncwarp();
+}
+
+// phase B: one warp (one block) per (delete, level)
+__global__ void __launch_bounds__(32) hnsw_delete_repair_kernel(DelArgs a) {
+    extern __shared__ __align__(128) uint8_t row[];
+    __shared__ DelSmem sm;
+    const uint32_t L1 = a.g.num_levels + 1, b = blockIdx.x / L1, level = blockIdx.x % L1, lane = threadIdx.x & 31;
+    const uint32_t D = a.loc[(size_t)(a.first + b) * L1 + level];
+    if (D == HN_EMPTY) return;
+    del_smem_init(sm);
+    const BuildLevel &l = a.g.lv[level];
+    const uint32_t zn = a.z_n[(size_t)b * L1 + level];
+    const uint32_t *cand = a.z_nodes + ((size_t)b * L1 + level) * a.zcap;
+    uint32_t parity = 0;
+    bool err = false;
+    volatile uint32_t *da = l.adj + (size_t)D * l.nb;
+    for (uint32_t s = 0; s < l.nb; ++s) {
+        uint32_t N = lane == 0 ? da[s] : 0u;
+        N = __shfl_sync(0xFFFFFFFFu, N, 0);
+        if (N == HN_EMPTY) continue;
+        int go = 0;
+        if (lane == 0) go = build_remove_by_id(l, N, D) && !bit_set(a.dead[level], N) && build_is_empty(l, N);
+        go = __shfl_sync(0xFFFFFFFFu, go, 0);
+        if (go && zn != HN_EMPTY && !del_relink(a, level, N, D, cand, zn, row, sm, parity)) err = true;
+    }
+    if (lane == 0) {   // D4: the node stays, isolated
+        node_lock(l.lock + D);
+        for (uint32_t s = 0; s < l.nb; ++s) da[s] = HN_EMPTY;
+        ((volatile uint32_t *)l.lowest_idx)[D] = 0;
+        ((volatile uint32_t *)l.lowest_key)[D] = a.g.min_key;
+        node_unlock(l.lock + D);
+        if (err) a.status[a.first + b] = 2;
+    }
+}
+
+// D2: one pass over the level's adjacency (128-bit loads, grid-stride) clears every slot naming a node deleted by this call
+// and lists each node it cleared a slot of once, with the batch position of (one of) the deleted nodes it named
+__device__ __forceinline__ bool del_sweep_slot(const DelArgs &a, uint32_t level, uint64_t t, uint32_t &v) {
+    if (v == HN_EMPTY || !bit_set(a.dead[level], v)) return false;
+    const uint32_t node = (uint32_t)(t / a.g.lv[level].nb), bit = 1u << (node & 31);
+    if (!(atomicOr(a.touched[level] + (node >> 5), bit) & bit))
+        a.list[level][atomicAdd(a.list_n + level, 1u)] = make_uint2(node, a.dead_of[level][v]);
+    v = HN_EMPTY;
+    return true;
+}
+__global__ void hnsw_delete_sweep_kernel(DelArgs a, uint32_t level) {
+    const BuildLevel &l = a.g.lv[level];
+    const uint64_t slots = (uint64_t)l.cnt * l.nb, vecs = slots / 4;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    uint4 *adj4 = reinterpret_cast<uint4 *>(l.adj);
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < vecs; i += stride) {
+        uint4 v = adj4[i];
+        bool ch = del_sweep_slot(a, level, 4 * i, v.x);
+        ch |= del_sweep_slot(a, level, 4 * i + 1, v.y);
+        ch |= del_sweep_slot(a, level, 4 * i + 2, v.z);
+        ch |= del_sweep_slot(a, level, 4 * i + 3, v.w);
+        if (ch) adj4[i] = v;
+    }
+    const uint64_t t = vecs * 4 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < slots) {
+        uint32_t v = l.adj[t];
+        if (del_sweep_slot(a, level, t, v)) l.adj[t] = v;
+    }
+}
+
+// relink of the nodes the sweep touched: one warp per list entry, or (ordered, deletes one at a time) a single warp taking
+// the entries in ascending node index.  A node is relinked if it is empty at its turn and not deleted itself.
+__global__ void __launch_bounds__(32) hnsw_delete_relink_kernel(DelArgs a, uint32_t level, bool ordered) {
+    extern __shared__ __align__(128) uint8_t row[];
+    __shared__ DelSmem sm;
+    const uint32_t L1 = a.g.num_levels + 1, lane = threadIdx.x & 31, n = a.list_n[level];
+    if (!n) return;
+    del_smem_init(sm);
+    const BuildLevel &l = a.g.lv[level];
+    const uint2 *list = a.list[level];
+    uint32_t parity = 0;
+    auto process = [&](uint2 e) {
+        const uint32_t X = e.x, b = e.y;
+        const uint32_t zn = a.z_n[(size_t)b * L1 + level];
+        int go = 0;
+        if (lane == 0) go = zn != HN_EMPTY && !bit_set(a.dead[level], X) && build_is_empty(l, X);
+        if (!__shfl_sync(0xFFFFFFFFu, go, 0)) return;
+        const uint32_t D = a.loc[(size_t)(a.first + b) * L1 + level];
+        if (!del_relink(a, level, X, D, a.z_nodes + ((size_t)b * L1 + level) * a.zcap, zn, row, sm, parity) && lane == 0)
+            a.status[a.first + b] = 2;
+    };
+    if (!ordered) {
+        for (uint32_t e = blockIdx.x; e < n; e += gridDim.x) {
+            process(list[e]);
+            if (lane == 0) atomicAnd(a.touched[level] + (list[e].x >> 5), ~(1u << (list[e].x & 31)));
+        }
+        return;
+    }
+    if (blockIdx.x) return;
+    int64_t last = -1;
+    for (;;) {
+        uint64_t best = ~0ull;   // (node << 32 | entry) of the smallest node above `last`
+        for (uint32_t e = lane; e < n; e += 32)
+            if ((int64_t)list[e].x > last) best = min(best, ((uint64_t)list[e].x << 32) | e);
+        for (int o = 16; o; o >>= 1) best = min(best, (uint64_t)__shfl_xor_sync(0xFFFFFFFFu, best, o));
+        if (best == ~0ull) break;
+        last = (int64_t)(best >> 32);
+        process(list[(uint32_t)best]);
+    }
+    for (uint32_t e = lane; e < n; e += 32) atomicAnd(a.touched[level] + (list[e].x >> 5), ~(1u << (list[e].x & 31)));
+}
+
+cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
+                              uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s) {
+    const GraphDev &gd = *gh.dev;
+    const uint32_t L1 = st->g.num_levels + 1;
+    constexpr uint32_t DEL_EF = 512, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
+    // level-local index of every row on every level (level 0 is the row when the level lists rows in order)
+    std::vector<uint32_t> loc((size_t)n * L1, HN_EMPTY);
+    std::unordered_map<uint32_t, uint32_t> pos;
+    for (uint32_t i = 0; i < n; ++i) pos.emplace(rows[i], i);
+    for (uint32_t L = 0; L < L1; ++L) {
+        const uint32_t cnt = (*gh.cnt)[L];
+        if (L == 0 && (gd.identity_mask & 1u)) {
+            for (uint32_t i = 0; i < n; ++i) if (rows[i] < cnt) loc[(size_t)i * L1] = rows[i];
+            continue;
+        }
+        std::vector<uint32_t> nr(cnt);
+        if (cnt) CDB_CUDA_TRY(cudaMemcpy(nr.data(), (*gh.nr)[L], (size_t)cnt * 4, cudaMemcpyDeviceToHost));
+        for (uint32_t j = 0; j < cnt; ++j) {
+            auto it = pos.find(nr[j]);
+            if (it != pos.end() && loc[(size_t)it->second * L1 + L] == HN_EMPTY) loc[(size_t)it->second * L1 + L] = j;
+        }
+    }
+    // only rows with a level-0 node take part in the repair (a row appended after the graph was built is not in it)
+    std::vector<uint32_t> grows, gidx, gloc;
+    for (uint32_t i = 0; i < n; ++i) {
+        out_status[i] = 0;
+        if (loc[(size_t)i * L1] == HN_EMPTY) continue;
+        gidx.push_back(i);
+        grows.push_back(rows[i]);
+        gloc.insert(gloc.end(), loc.begin() + (size_t)i * L1, loc.begin() + (size_t)(i + 1) * L1);
+    }
+    const uint32_t ng = (uint32_t)grows.size();
+    if (!ng) return CDB_OK;
+    if (max_batch == 0) max_batch = 4096;
+    max_batch = std::max<uint32_t>(1, std::min(max_batch, ng));
+    // ---- every allocation before the graph changes
+    cdb_status rc;
+    DevAllocs tmp;
+    DelArgs d{};
+    uint32_t *d_rows = nullptr, *d_loc = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
+    uint8_t *failed = nullptr;
+    if ((rc = tmp.get((void **)&d_rows, (size_t)ng * 4)) || (rc = tmp.get((void **)&d_loc, (size_t)ng * L1 * 4)) ||
+        (rc = tmp.get((void **)&z_nodes, (size_t)max_batch * L1 * DEL_KEEP * 4)) ||
+        (rc = tmp.get((void **)&z_keys, (size_t)max_batch * L1 * DEL_KEEP * 4)) || (rc = tmp.get((void **)&z_n, (size_t)max_batch * L1 * 4)) ||
+        (rc = tmp.get((void **)&failed, ng)) || (rc = tmp.get((void **)&d.status, ng)) || (rc = tmp.get((void **)&d.list_n, L1 * 4)))
+        return rc;
+    for (uint32_t L = 0; L < L1; ++L) {
+        const uint32_t cnt = (*gh.cnt)[L], words = cnt / 32 + 1;
+        if ((rc = tmp.get((void **)&d.dead[L], (size_t)words * 4)) || (rc = tmp.get((void **)&d.touched[L], (size_t)words * 4)) ||
+            (rc = tmp.get((void **)&d.dead_of[L], (size_t)cnt * 4)) || (rc = tmp.get((void **)&d.list[L], (size_t)cnt * 8)))
+            return rc;
+        CDB_CUDA_TRY(cudaMemsetAsync(d.dead[L], 0, (size_t)words * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d.touched[L], 0, (size_t)words * 4, s));
+    }
+    const size_t smem = hn_smem_bytes(sc.row_pitch, DEL_EF);
+    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    CDB_ALLOW_SMEM(hnsw_delete_repair_kernel, sc.row_pitch);
+    CDB_ALLOW_SMEM(hnsw_delete_relink_kernel, sc.row_pitch);
+    CDB_CUDA_TRY(cudaMemsetAsync(d.status, 0, ng, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_rows, grows.data(), (size_t)ng * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_loc, gloc.data(), (size_t)ng * L1 * 4, cudaMemcpyHostToDevice, s));
+    // ---- batches
+    *changed = true;
+    BuildArgs a{};
+    a.g = st->g;
+    a.sc = sc;
+    a.sc.root_row = st->g.root_row;
+    a.ef = DEL_EF;
+    a.shortlist = shortlist;
+    a.zcap = DEL_KEEP;
+    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
+    a.rowlist = d_rows;
+    d.g = st->g;
+    d.sc = a.sc;
+    d.loc = d_loc;
+    d.zcap = DEL_KEEP;
+    d.z_nodes = z_nodes; d.z_n = z_n;
+    int dev = 0, sms = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const bool ordered = max_batch == 1;
+    for (uint32_t done = 0; done < ng;) {
+        const uint32_t batch = std::min(max_batch, ng - done);
+        a.first = d.first = done;
+        a.count = d.count = batch;
+        a.failed = failed + done;
+        hnsw_delete_mark_kernel<<<(batch * L1 + 127) / 128, 128, 0, s>>>(d);
+        hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
+        hnsw_delete_repair_kernel<<<batch * L1, 32, sc.row_pitch, s>>>(d);
+        g_launch_count.fetch_add(3, std::memory_order_relaxed);
+        for (uint32_t L = 0; L < L1; ++L) {
+            const uint64_t vecs = (uint64_t)(*gh.cnt)[L] * a.g.lv[L].nb / 4 + 1;
+            const uint32_t grid = (uint32_t)std::min<uint64_t>((vecs + 255) / 256, (uint64_t)sms * 8);
+            hnsw_delete_sweep_kernel<<<grid, 256, 0, s>>>(d, L);
+            hnsw_delete_relink_kernel<<<ordered ? 1 : 1024, 32, sc.row_pitch, s>>>(d, L, ordered);
+            g_launch_count.fetch_add(2, std::memory_order_relaxed);
+        }
+        done += batch;
+    }
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    std::vector<uint8_t> hf(ng), hs(ng);
+    if (e == cudaSuccess) e = cudaMemcpy(hf.data(), failed, ng, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(hs.data(), d.status, ng, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error(std::string("hnsw delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    for (uint32_t j = 0; j < ng; ++j) out_status[gidx[j]] = (hf[j] || hs[j]) ? 2 : 0;
     return CDB_OK;
 }
 
@@ -713,6 +1076,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
     a.levels = d_levels;
     a.ef = ef_construction;
     a.shortlist = shortlist;
+    a.zcap = 64;
     a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
     a.replicas = true;
     a.rl = rl;

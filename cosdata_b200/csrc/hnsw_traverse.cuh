@@ -170,8 +170,9 @@ __device__ __forceinline__ int hn_score_node(const uint32_t *__restrict__ node_r
 __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, const uint32_t *__restrict__ adj, uint32_t nb,
                                          uint32_t take, const HnScoreCtx &sc, const HnSmem &m, HnShared &sh, float qmag,
                                          uint32_t self_id, uint32_t ef, unsigned long long &evals, unsigned long long &pops,
-                                         const HnMdCtx *md = nullptr, long long *prof = nullptr) {
+                                         const HnMdCtx *md = nullptr, long long *prof = nullptr, bool seed_self = true) {
     // prof (thread 0 only, may be null): clock64 sums with the slot meaning of hnsw_warp.cu's HW_PROF_SLOTS
+    // seed_self = false: nothing is pre-inserted into the fixed set (delete_embedding, vector_store.rs:1231-1235)
     const int tid = threadIdx.x;
     long long pt0 = 0, pt1 = 0, pt2 = 0, pt3 = 0, pts = 0, ptg = 0, ptw = 0;
     if (prof && tid == 0) pt0 = clock64();
@@ -182,7 +183,7 @@ __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, 
     __syncthreads();
     if (tid == 0) {
         const uint32_t mask = nb - 1u;
-        m.fs[(self_id >> 6) & mask] |= 1ull << (self_id & 0x3f);
+        if (seed_self) m.fs[(self_id >> 6) & mask] |= 1ull << (self_id & 0x3f);
         const uint32_t entry = sh.entry;
         float d = 0.f;
         uint32_t eid;

@@ -69,6 +69,7 @@ struct ScanArgs {
     uint64_t *partial;     // [nq][nsplit][k] selection keys
     uint32_t nsplit;
     uint32_t *err32;       // [nq] error bits (atomicOr) or null
+    const uint32_t *deleted;   // deleted-row bitmap (bit r = row r) or null: such rows are neither offered nor flag errors
     // Device-side fallback decision of the tensor-core paths (no host sync).  qsel = {n_sel, query indices...} is written by
     // select_fallback_kernel.  Two launches share it:
     //   selective (sel_mode = 1): 1-D grid; runs only if 0 < n_sel <= sel_cap, over the selected queries only -- the CTAs
@@ -171,7 +172,8 @@ void hnsw_state_free(HnswBuildState *st);
 // cdb_index_build_graph: root row n on every level, then rows [0, n) inserted
 cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
                              uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed, const GraphHost &gh,
-                             HnswBuildState **out_state, cudaStream_t s);
+                             HnswBuildState **out_state, cudaStream_t s, const uint32_t *d_deleted = nullptr,
+                             const uint32_t *h_deleted = nullptr);
 // slot state of a graph that came from elsewhere (cdb_index_set_graph), under the reload semantics of
 // ProbNode::new_with_neighbors_and_versions; sc.root_row = the graph's root row
 cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s);
@@ -180,7 +182,14 @@ cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, Hns
 // *changed == false left the graph as it was, with *changed == true the graph is half-inserted and must be dropped.
 cdb_status hnsw_insert_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, uint32_t n_new, const uint8_t *max_level,
                               uint64_t seed, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t rows_cap,
-                              uint8_t *out_failed, bool *changed, cudaStream_t s);
+                              uint8_t *out_failed, bool *changed, cudaStream_t s, const uint32_t *d_deleted = nullptr,
+                              const uint32_t *h_deleted = nullptr);
+// deleted-row bitmaps (d_deleted device, h_deleted host, bit r = row r; null = none): build and insert skip those rows
+// (no upper-level nodes, not linked, out_failed 2)
+// cdb_index_delete_rows: delete_embedding for the distinct rows rows[0..n) with the deviations D1-D4 (DESIGN.md section 4);
+// out_status[i] = 0, or 2 where an Err stopped relinks.  *changed as for the insert.
+cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
+                              uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s);
 // similarity keys of every slot of `level` ([cnt*nb], device)
 const uint32_t *hnsw_state_slot_keys(const HnswBuildState *st, uint32_t level);
 

@@ -52,8 +52,12 @@ __device__ inline TopK topk_carve(uint8_t *p, uint32_t qb, uint32_t k) {
 __device__ inline void topk_init(const TopK &t, uint32_t qb) {
     for (uint32_t i = threadIdx.x; i < qb; i += blockDim.x) { t.thr[i] = 0; t.cnt[i] = 0; t.err[i] = 0; }
 }
-__device__ inline void topk_offer(const TopK &t, int b, uint64_t key) {
-    if (key > t.thr[b]) {
+__device__ __forceinline__ bool row_deleted(const uint32_t *deleted, uint64_t row) {
+    return deleted && ((deleted[row >> 5] >> (row & 31)) & 1u);
+}
+// a deleted row is never offered: the bitmap is read only for keys that pass the threshold, so the per-row cost stays one compare
+__device__ inline void topk_offer(const TopK &t, int b, uint64_t key, const uint32_t *deleted, uint64_t row) {
+    if (key > t.thr[b] && !row_deleted(deleted, row)) {
         int pos = atomicAdd(&t.cnt[b], 1);
         t.buf[(size_t)b * t.cap + pos] = key;
     }
@@ -227,10 +231,11 @@ __global__ void __launch_bounds__(SCAN_THREADS, 2) scan_f32_kernel(ScanArgs a) {
                 if (valid && (uint32_t)b < nqv && (b & 1) == t) {
                     const float denom = __fmul_rn(qmag[b], rmag);
                     if (!a.raw_mode && denom == 0.0f) {
-                        atomicOr(&tk.err[b], CDB_ERRFLAG_CALCULATION);
+                        if (!row_deleted(a.deleted, row[rr])) atomicOr(&tk.err[b], CDB_ERRFLAG_CALCULATION);
                     } else {
                         const float v = canon_nan(__fdiv_rn(tot, denom));
-                        topk_offer(tk, b, make_key64(order_key(CDB_METRIC_COSINE, __float_as_uint(v)), a.id_base + (uint32_t)row[rr]));
+                        topk_offer(tk, b, make_key64(order_key(CDB_METRIC_COSINE, __float_as_uint(v)), a.id_base + (uint32_t)row[rr]),
+                                   a.deleted, row[rr]);
                     }
                 }
             }
@@ -270,8 +275,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 2) scan_generic_kernel(ScanArgs 
                 float v;
                 int rc = pair_distance(a.metric, a.st, a.dim, qs + (size_t)b * a.row_pitch, qmag[b], pp, xr, rmag, pp, &v);
                 if (rc == CDB_OK)
-                    topk_offer(tk, b, make_key64(order_key(a.metric, __float_as_uint(v)), a.id_base + (uint32_t)row));
-                else if (rc == CDB_CALCULATION_ERROR)
+                    topk_offer(tk, b, make_key64(order_key(a.metric, __float_as_uint(v)), a.id_base + (uint32_t)row), a.deleted, row);
+                else if (rc == CDB_CALCULATION_ERROR && !row_deleted(a.deleted, row))
                     atomicOr(&tk.err[b], CDB_ERRFLAG_CALCULATION);
             }
         }

@@ -391,6 +391,36 @@ cdb_status cdb_index_insert_graph(cdb_index *index, const cdb_build_params *para
  * empty slots): what the reference's serializer writes next to each link (serializer/hnsw/neighbors.rs:53-57).  Derived
  * as above for an uploaded graph.  Graphs with metadata: CDB_UNSUPPORTED. */
 cdb_status cdb_index_read_graph_slot_scores(cdb_index *index, uint32_t level, float *out_scores);
+/* delete_embedding (src/vector_store.rs:1206-1371) for local rows rows[0..n) (row numbers as cdb_score_ids takes them: a shard
+ * caller subtracts id_base).  A row out of range or the graph's root_row: CDB_INVALID_PARAMS, nothing changed.
+ * out_status[n] (may be NULL): 0 deleted; 1 already deleted (by an earlier call or earlier in this list), nothing happened;
+ * 2 deleted and unlinked, but a traversal or rescoring Err stopped some relinks (D3).  *out_deleted (may be NULL) = rows
+ * newly deleted.  Per level, top-down: the deleted node D's stored codes traverse from the root with nothing pre-inserted
+ * in the fixed set, ef = 512 (the reference's literal) and the best 100 kept; remove_neighbor_by_id(D) on each of D's
+ * neighbours in slot order (lowest_index left stale); a neighbour whose list emptied is relinked: the results minus D and
+ * itself, rescored against it, sorted best first (ties: smaller id), through create_node_edges / add_neighbor with its
+ * stale lowest_index.  shortlist_size = config.search.shortlist_size; max_batch (0 = 4096) deletes in flight, each batch
+ * traversing the graph as of its start; 1 deletes one row at a time in list order (deterministic).  Deviations:
+ *   D1 D is unlinked on every level it is on, whether or not the traversal found it (a deleted row never comes back from a
+ *      search); where it was not found there is nothing to take out of the results.
+ *   D2 links to D from nodes outside D's list are cleared too (the reference leaves them dangling): after D's own slots,
+ *      one pass clears every slot naming D, then each node it cleared a slot of is relinked, in ascending level-local
+ *      index, if its list is empty at its turn.  In batched mode relink candidates exclude rows deleted in the batch.
+ *   D3 an Err stops relinks, not unlinking: a failed traversal stops the relinks of that level and the levels below, a
+ *      rescoring Err that one relink; D is unlinked everywhere and gets status 2.
+ *   D4 D keeps its node entries with an empty adjacency on every level (an isolated node); rows are never reused.
+ * Deleted rows: the exact scans never return them nor flag their errors; the tensor-core brute-force paths are bypassed
+ * while any row is deleted (the exact scan answers); cdb_index_build_graph / cdb_index_insert_graph skip them (out_failed
+ * 2, no nodes above level 0), cdb_index_build_graph_replicas refuses a list naming one, cdb_index_set_graph refuses a
+ * graph linking one.  cdb_score_ids, cdb_rerank_f32 and cdb_distance_pairs take explicit ids and are unchanged.  Without
+ * a graph the call only marks the rows.  Graphs with metadata: CDB_UNSUPPORTED, nothing changed.  Locking, the order
+ * against enqueued searches and the failure contract are those of cdb_index_insert_graph; the marks are set only once the
+ * repair has succeeded. */
+cdb_status cdb_index_delete_rows(cdb_index *index, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
+                                 uint8_t *out_status, uint64_t *out_deleted);
+/* out[i] = 1 if row first+i is deleted (first + n <= capacity); *out_total = deleted rows of the index (either pointer may be
+ * NULL when unused) */
+cdb_status cdb_index_deleted_rows(const cdb_index *index, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total);
 /* cumulative {distance evaluations, pops} of CDB_MODE_HNSW searches (roofline accounting) */
 cdb_status cdb_index_hnsw_counters(const cdb_index *index, uint64_t *out2);
 

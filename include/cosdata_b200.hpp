@@ -175,6 +175,20 @@ class DenseIndex {
         failed.resize(n);
         return failed;
     }
+    // delete_embedding for local rows; returns the per-row status (0 deleted, 1 already deleted, 2 an Err stopped relinks)
+    std::vector<uint8_t> delete_rows(const std::vector<uint32_t> &rows, uint32_t shortlist_size = 64, uint32_t max_batch = 0) {
+        std::vector<uint8_t> status(std::max<size_t>(rows.size(), 1));
+        check(cdb_index_delete_rows(h_, rows.data(), rows.size(), shortlist_size, max_batch, status.data(), nullptr));
+        status.resize(rows.size());
+        return status;
+    }
+    // deleted flag of every row
+    std::vector<uint8_t> deleted_rows() const {
+        std::vector<uint8_t> out(std::max<uint64_t>(cdb_index_size(h_), 1));
+        check(cdb_index_deleted_rows(h_, 0, cdb_index_size(h_), out.data(), nullptr));
+        out.resize(cdb_index_size(h_));
+        return out;
+    }
     // similarity of every neighbour slot of `level` (0 for empty slots), as the reference's serializer stores it
     std::vector<float> read_graph_slot_scores(uint32_t level) {
         uint32_t info[5], counts[32];
