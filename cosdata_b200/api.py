@@ -488,10 +488,10 @@ class DenseIndex:
         return {n: int(v) for n, v in zip(names, out)}
 
     def stats(self):
-        out = np.zeros(6, dtype=np.uint64)
-        _check(self._lib.cdb_index_stats_ex(self._h, _ptr(out), 6))
+        out = np.zeros(7, dtype=np.uint64)
+        _check(self._lib.cdb_index_stats_ex(self._h, _ptr(out), 7))
         return {"tensor_searches": int(out[0]), "fallbacks": int(out[1]), "zero_rows": int(out[2]), "odd_rows": int(out[3]),
-                "has_shadow": bool(out[4]), "fallback_queries": int(out[5])}
+                "has_shadow": bool(out[4]), "fallback_queries": int(out[5]), "s8_searches": int(out[6])}
 
     def last_candidate_counts(self, n):
         out = np.zeros(n, dtype=np.uint32)

@@ -115,7 +115,7 @@ using namespace cdb;
 // single arena -- the index data itself is read-only during a search (SURVEY 8b: the ABI is re-entrant per handle).
 struct Scratch {
     DevBuf q_codes, q_mags, partial, err32, io_ids, io_scores, io_counts, io_err, io_q, misc;
-    DevBuf qh, gthr, cand, cand_cnt, flags, progress, qsel;
+    DevBuf qh, gthr, cand, cand_cnt, flags, progress, qsel, qse;
     DevBuf hn_rows, hn_scores, hn_n, qraw, qraw_mags, hn_ids, hn_labels, flt_off, flt_dims, flt_has;
     cudaStream_t stream = nullptr;         // used by the host-buffer entry points
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
@@ -137,7 +137,7 @@ struct Scratch {
         if (stream) cudaStreamSynchronize(stream);
         for (DevBuf *b : {&q_codes, &q_mags, &partial, &err32, &io_ids, &io_scores, &io_counts, &io_err, &io_q, &misc, &qh, &gthr, &cand,
                           &cand_cnt, &flags, &progress, &qsel, &hn_rows, &hn_scores, &hn_n, &qraw, &qraw_mags, &hn_ids, &hn_labels,
-                          &flt_off, &flt_dims, &flt_has})
+                          &flt_off, &flt_dims, &flt_has, &qse})
             b->release();
         for (auto &e : ev) if (e) cudaEventDestroy(e);
         if (stream) cudaStreamDestroy(stream);
@@ -159,10 +159,16 @@ struct cdb_index {
     uint32_t digit_pitch = 0;
     void *d_xh = nullptr;          // fp16 L2-normalised rows for the wgmma prefilter (tensor_scan.cu)
     uint32_t xh_pitch = 0;         // halfs per shadow row
+    void *d_xs8 = nullptr;         // s8 shadow for the s8 form of the prefilter (tensor_scan.cu KIND 2, DESIGN.md section 5c)
+    uint32_t xs8_pitch = 0;        // bytes per s8 shadow row
+    float2 *d_s8se = nullptr;      // [corpus tiles] {s_T, E_T}, then one float: E_max
+    uint32_t s8_tiles = 0;         // corpus tiles of the capacity
+    float s8_emax = 0.0f;          // max E_T of the stored rows (host copy, read by the gate)
     uint64_t n_allzero_rows = 0;   // degenerate rows (tensor_scan.cu): all-zero rows score NaN against every query = last
     uint64_t n_odd_rows = 0;       // other degenerate rows (norm 0/inf/NaN/out of range): ride on every candidate list
     uint32_t *h_flags = nullptr;   // pinned host staging (16 words)
     std::atomic<uint64_t> stat_tensor_searches{0};
+    std::atomic<uint64_t> stat_s8_searches{0};   // of those, answered by the s8 form
     cudaStream_t stream = nullptr; // ingest / build stream (exclusive operations)
     static constexpr int EV_RING = 64;
     cudaEvent_t ring0[EV_RING] = {}, ring1[EV_RING] = {};  // per-search (before scan, after scan)
@@ -474,6 +480,12 @@ cdb_status cdb_index_create(const cdb_index_desc *d, cdb_index **out) {
         ix->xh_pitch = round_up(d->dim * 2, 16) / 2;
         if ((e = cudaMalloc(&ix->d_xh, (size_t)d->capacity * ix->xh_pitch * 2)) != cudaSuccess) return fail(e, "cudaMalloc(fp16 shadow)");
         if ((e = cudaMemsetAsync(ix->d_xh, 0, (size_t)d->capacity * ix->xh_pitch * 2, ix->stream)) != cudaSuccess) return fail(e, "memset");
+        ix->xs8_pitch = round_up(d->dim, 16);
+        ix->s8_tiles = (uint32_t)((d->capacity + 255) / 256);
+        if ((e = cudaMalloc(&ix->d_xs8, (size_t)d->capacity * ix->xs8_pitch)) != cudaSuccess) return fail(e, "cudaMalloc(s8 shadow)");
+        if ((e = cudaMemsetAsync(ix->d_xs8, 0, (size_t)d->capacity * ix->xs8_pitch, ix->stream)) != cudaSuccess) return fail(e, "memset");
+        if ((e = cudaMalloc(&ix->d_s8se, ((size_t)ix->s8_tiles + 1) * 8)) != cudaSuccess) return fail(e, "cudaMalloc(s8 scales)");
+        if ((e = cudaMemsetAsync(ix->d_s8se, 0, ((size_t)ix->s8_tiles + 1) * 8, ix->stream)) != cudaSuccess) return fail(e, "memset");
     }
     if (d->tensor_prefilter && d->storage_type >= CDB_ST_SUB1 && d->storage_type <= CDB_ST_SUB3) {
         ix->digit_pitch = round_up(d->dim, 16);
@@ -497,6 +509,8 @@ cdb_status cdb_index_destroy(cdb_index *ix) {
     if (ix->raw_owned && ix->d_raw) cudaFree(ix->d_raw);
     if (ix->raw_mags_owned && ix->d_raw_mags) cudaFree(ix->d_raw_mags);
     if (ix->d_xh) cudaFree(ix->d_xh);
+    if (ix->d_xs8) cudaFree(ix->d_xs8);
+    if (ix->d_s8se) cudaFree(ix->d_s8se);
     if (ix->d_digits) cudaFree(ix->d_digits);
     if (ix->d_deleted) cudaFree(ix->d_deleted);
     hnsw_state_free(ix->bstate);
@@ -541,10 +555,16 @@ static cdb_status index_after_append(cdb_index *ix, uint64_t first, uint64_t n) 
         if ((rc = classify_rows_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, n,
                                        ix->desc.dim, (uint32_t)first, ix->deg.as<uint32_t>(), ix->stream)))
             return rc;
+        // s8 shadow: every tile the range touches, the open tile's earlier rows included (its scale can change)
+        if ((rc = quantize_s8_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, first, n, first + n, ix->desc.dim, ix->d_xs8,
+                                     ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->stream)))
+            return rc;
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 4, ix->deg.p, 8, cudaMemcpyDeviceToHost, ix->stream));
+        CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
         CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
         ix->n_allzero_rows = ix->h_flags[4];
         ix->n_odd_rows = ix->h_flags[5];
+        std::memcpy(&ix->s8_emax, ix->h_flags + 6, 4);
     }
     return CDB_OK;
 }
@@ -642,6 +662,14 @@ cdb_status cdb_index_set_raw_f32(cdb_index *ix, uint64_t first_row, const float 
                                        (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->stream)))
             return rc;
         CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    }
+    if (ix->d_xs8) {
+        cdb_status rc = quantize_s8_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, first_row, n, ix->size, dim, ix->d_xs8,
+                                           ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->stream);
+        if (rc) return rc;
+        CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
+        CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+        std::memcpy(&ix->s8_emax, ix->h_flags + 6, 4);
     }
     if (ix->raw_have.size() < ix->size) ix->raw_have.resize(ix->size, true);
     for (uint64_t r = first_row; r < first_row + n; ++r)
@@ -860,6 +888,16 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
 // (two fp16 roundings, fp32 tensor accumulation, f32 norms; DESIGN.md section 5)
 static float prefilter_eps(uint32_t dim) { return 1.0e-3f + 8.0e-7f * (float)dim; }
 
+// The s8 form of the prefilter (DESIGN.md section 5c) halves the tensor work; its error bound grows with the shard's
+// residual bound E_max = max_T E_T, and with it the candidate lists.  It is taken for compute-bound shapes whose E_max is
+// at most TS_S8_TAU; CDB_TS_S8=0|1 (read per search) forces either form wherever the prefilter runs.
+constexpr float TS_S8_TAU = 1.5e-2f;
+static bool use_s8_form(const cdb_index *ix, uint32_t nq) {
+    if (!ix->d_xs8) return false;
+    if (const char *e = getenv("CDB_TS_S8")) return atoi(e) != 0;
+    return nq >= 512 && ix->desc.dim >= 256 && ix->s8_emax <= TS_S8_TAU;
+}
+
 static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
                                       uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s) {
     const cdb_index_desc &d = ix->desc;
@@ -914,16 +952,26 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
             return rc;
         uint32_t *flags = sc->flags.as<uint32_t>();  // [0] queries of the last search that needed the exact scan, [3] searches with a fallback
         const bool has_deg = ix->n_allzero_rows + ix->n_odd_rows > 0;
+        const bool s8 = use_s8_form(ix, nq);
+        if (s8 && (rc = sc->qse.ensure((size_t)nq * 8))) return rc;
         if ((rc = prep_queries_device(d_queries, nq, d.dim, sc->q_codes.as<float>(), pitch / 4, sc->q_mags.as<float>(), sc->qh.p,
-                                      ix->xh_pitch, sc->gthr.as<int>(), ix->deg.as<uint32_t>(), has_deg, d.id_base,
+                                      s8 ? ix->xs8_pitch : ix->xh_pitch, sc->gthr.as<int>(), ix->deg.as<uint32_t>(), has_deg, d.id_base,
                                       sc->cand.as<uint32_t>(), cap, sc->cand_cnt.as<uint32_t>(), sc->err32.as<uint32_t>(), d_err,
-                                      sc->progress.as<uint32_t>(), s)))
+                                      sc->progress.as<uint32_t>(), s8 ? sc->qse.as<float2>() : nullptr, s)))
             return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring0[slot], s));
-        if ((rc = tensor_scan_device(ix->d_xh, sc->qh.p, ix->xh_pitch, ix->size, nq, d.dim, p->k, 2.0f * prefilter_eps(d.dim),
-                                     d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), cap,
-                                     sc->progress.as<uint32_t>(), ix->deg.as<uint32_t>(), has_deg, ix->sm_count, s, /*prepared=*/true)))
+        if (s8) {
+            if ((rc = tensor_scan_s8_device(ix->d_xs8, sc->qh.p, ix->xs8_pitch, ix->size, nq, d.dim, p->k, ix->d_s8se,
+                                            sc->qse.as<float2>(), d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(),
+                                            sc->cand_cnt.as<uint32_t>(), cap, sc->progress.as<uint32_t>(), has_deg, ix->sm_count, s)))
+                return rc;
+            ix->stat_s8_searches++;
+        } else if ((rc = tensor_scan_device(ix->d_xh, sc->qh.p, ix->xh_pitch, ix->size, nq, d.dim, p->k, 2.0f * prefilter_eps(d.dim),
+                                            d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), cap,
+                                            sc->progress.as<uint32_t>(), ix->deg.as<uint32_t>(), has_deg, ix->sm_count, s,
+                                            /*prepared=*/true))) {
             return rc;
+        }
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
         if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->q_codes.as<float>(),
                                     pitch / 4, sc->q_mags.as<float>(), nq, sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(),
@@ -1712,7 +1760,7 @@ cdb_status cdb_index_stats_ex(const cdb_index *ix, uint64_t *out, uint32_t n) {
     cdb_status rc = read_pool_flags(ix, &fb, &lq);
     if (rc) return rc;
     const uint64_t v[CDB_STATS_FIELDS] = {ix->stat_tensor_searches.load(), fb, ix->n_allzero_rows, ix->n_odd_rows,
-                                          ix->d_xh ? 1ull : 0ull, lq};
+                                          ix->d_xh ? 1ull : 0ull, lq, ix->stat_s8_searches.load()};
     for (uint32_t i = 0; i < n && i < CDB_STATS_FIELDS; ++i) out[i] = v[i];
     return CDB_OK;
 }

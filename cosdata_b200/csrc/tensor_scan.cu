@@ -19,6 +19,8 @@
 //   warps 8..11  producer warpgroup (setmaxnreg: 40 registers), one thread issues the TMA loads:
 //                cp.async.bulk.tensor.2d, SWIZZLE_128B, 4-stage mbarrier ring
 // Tile: 128 queries (A, K-major) x 256 corpus rows (B, K-major), K block = 64 halfs (128 B).
+#include <climits>
+#include <cmath>
 #include <cstdlib>
 #include <type_traits>
 
@@ -61,6 +63,11 @@ struct TensorScanArgs {
     uint64_t *cand64;       // [n_queries][cand_cap] emitted selection keys (exact scores)
     uint32_t *err32;        // [n_queries] error bits
     float rel;              // threshold = bound * rel - two_eps (1 for the f16 form and for the dot product; 1 - 2^-18 for cosine)
+    // ---- s8 form (KIND 2: the prefilter on wgmma .s32.s8.s8 against the s8 shadow, DESIGN.md section 5c)
+    const float2 *tile_se;  // [ntiles] {s_T, E_T} of each corpus tile
+    const float2 *q_se;     // [n_queries] {s_q, e_q}
+    float dn1;              // 1 + delta_n, rounded up: bound on |x_hat| and |q_hat|
+    float dref;             // delta_ref(D), rounded up: the reference's f32 cosine against the exact q_hat . x_hat
 };
 
 // Candidate staging in shared memory: 40 bytes per (consumer thread, query row): slot 0 = count, then 9 row ids (f16 form)
@@ -159,15 +166,23 @@ __device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
 // staged in shared memory per tile), the filter keeps a 2^-18 relative margin for the cosine form and none for the dot
 // product, and whatever passes is scored EXACTLY (epi_emit_key) -- final selection keys, not candidates.
 //
+// KIND = 2: the prefilter of KIND 0 on wgmma .s32.s8.s8 (twice the f16 rate, half the operand bytes): s8 codes of the
+// normalised rows / queries with one scale per corpus tile (s_T) and per query (s_q), 128 bytes of K per stage like KIND 1.
+// An s32 accumulator dp scores s_T*s_q*dp with |s_T*s_q*dp - cos_ref| <= eps(q,T) (DESIGN.md section 5c).  Per value the
+// epilogue keeps integer class maxima; once per tile and query it folds their rigorous lower bounds
+// fl_down(cm*s_T*s_q) - eps(q,T) into the float class maxima and turns the threshold A into the integer
+// thrI = floor((A - eps(q,T)) / (s_T*s_q)) (directed rounding throughout): a row is emitted iff dp >= thrI, i.e. iff its
+// upper bound reaches A.
+//
 // Register layout of the epilogue: a consumer thread holds two query rows (r and r + 8 of its warpgroup's 64) and, of each,
 // the 64 columns 8j + 2(lane%4) + {0,1}.  Classes are column mod NG, so the thread owns NG/4 classes of each of its queries
 // (those = 2(lane%4) or 2(lane%4)+1 mod 8); the four threads of a quad together cover all NG classes of their two queries.
 template <int STAGES, int NG, bool HAS_DEG, int KIND>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x, TensorScanArgs a) {
-    constexpr uint32_t K_ELEMS = KIND == 1 ? 2 * TS_BLOCK_K : TS_BLOCK_K;   // elements per 128-byte row: 128 u8 / 64 halfs
+    constexpr uint32_t K_ELEMS = KIND != 0 ? 2 * TS_BLOCK_K : TS_BLOCK_K;   // elements per 128-byte row: 128 u8/s8 / 64 halfs
     constexpr int NL = NG / 4;                                              // classes a thread owns per query
-    using Acc = typename std::conditional<KIND == 1, uint32_t, float>::type;
+    using Acc = typename std::conditional<KIND != 0, uint32_t, float>::type;
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -234,12 +249,14 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         uint32_t *stage[2];
         uint64_t *kstage[2];
         float gm[2][NL];
+        float2 qse[2];   // KIND 2: {s_q, e_q}
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const uint32_t ql = qrow0 + 8 * i;
             qi[i] = mt * TS_BLOCK_M + ql;
             qvalid[i] = qi[i] < a.n_queries;
             qmag[i] = (KIND == 1 && qvalid[i]) ? a.qmags[qi[i]] : 0.0f;
+            if (KIND == 2) qse[i] = qvalid[i] ? a.q_se[qi[i]] : make_float2(0.0f, 0.0f);
             err[i] = (cosine && qvalid[i] && qmag[i] == 0.0f && a.n_rows > 0) ? (uint32_t)CDB_ERRFLAG_CALCULATION : 0u;
             ggm_q[i] = a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql;  // + class * 128
             stage[i] = reinterpret_cast<uint32_t *>(lstage + (size_t)(ct * 2 + i) * TS_STAGE_SLOT_BYTES);
@@ -286,6 +303,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk) {  // +32 bytes along K = +2 in the encoded start address
                     if constexpr (KIND == 1) wgmma_u8(acc, adesc + 2 * kk, bdesc + 2 * kk);
+                    else if constexpr (KIND == 2) wgmma_s8(acc, adesc + 2 * kk, bdesc + 2 * kk);
                     else wgmma_f16(acc, adesc + 2 * kk, bdesc + 2 * kk);
                 }
                 wgmma_commit();
@@ -302,6 +320,69 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             //      build the per-value tests only on a hit
             const bool full_tile = row0 + TS_BLOCK_N <= a.n_rows;   // only the corpus' last tile can be partial (TMA zero fill)
             const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;   // valid columns of this tile
+            if constexpr (KIND == 2) {
+                const float2 se = __ldg(a.tile_se + nt);   // {s_T, E_T}
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    // s_T*s_q rounded down and up, eps(q,T) rounded up, thrI <= (A - eps) / (s_T*s_q)
+                    const float slo = __fmul_rd(se.x, qse[i].x), shi = __fmul_ru(se.x, qse[i].x);
+                    const float eps = __fmaf_ru(__fadd_ru(a.dn1, qse[i].y), se.y, __fmaf_ru(qse[i].y, a.dn1, a.dref));
+                    const float num = __fsub_rd(bound[i], eps);
+                    const int thrI = __float2int_rd(__fdiv_rd(num, num >= 0.0f ? shi : slo));
+                    int cm[NL];
+#pragma unroll
+                    for (int l = 0; l < NL; ++l) cm[l] = INT_MIN;
+                    bool hit;
+                    if (full_tile) {
+                        int zmax = INT_MIN;   // HAS_DEG: 0 if some accumulator of the tile is exactly zero
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) {
+#pragma unroll
+                            for (int b = 0; b < 2; ++b) {
+                                int v = (int)acc[4 * j + 2 * i + b];
+                                if (HAS_DEG) {
+                                    zmax = v == 0 ? 0 : zmax;
+                                    v = v == 0 ? INT_MIN : v;
+                                }
+                                const int l = (j & (NG / 8 - 1)) * 2 + b;
+                                cm[l] = max(cm[l], v);
+                            }
+                        }
+                        int cmax = zmax;
+#pragma unroll
+                        for (int l = 0; l < NL; ++l) cmax = max(cmax, cm[l]);
+                        hit = cmax >= thrI;
+                    } else {
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) {
+#pragma unroll
+                            for (int b = 0; b < 2; ++b) {
+                                const uint32_t col = 8 * j + 2 * qd + b;
+                                const int v = (int)acc[4 * j + 2 * i + b];
+                                const int l = (j & (NG / 8 - 1)) * 2 + b;
+                                if ((uint64_t)col < left && !(HAS_DEG && v == 0)) cm[l] = max(cm[l], v);
+                            }
+                        }
+                        hit = true;
+                    }
+                    // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class
+#pragma unroll
+                    for (int l = 0; l < NL; ++l)
+                        if (cm[l] != INT_MIN)
+                            gm[i][l] = fmaxf(gm[i][l], __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo : shi), eps));
+                    if (qvalid[i] && a.emit && hit) {
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) {
+#pragma unroll
+                            for (int b = 0; b < 2; ++b) {
+                                const uint32_t col = 8 * j + 2 * qd + b;
+                                if ((uint64_t)col < left && (int)acc[4 * j + 2 * i + b] >= thrI)
+                                    epi_emit(a, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
+                            }
+                        }
+                    }
+                }
+            } else {
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 bool hit;
@@ -355,6 +436,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                         }
                     }
                 }
+            }
             }
             // refresh the shared bound: every tile early on (and in the seeding pass), then every 16th tile.  The quad's
             // classes are published before any of its threads reads the maxima back.
@@ -428,6 +510,97 @@ cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const 
     return CDB_OK;
 }
 
+// ------------------------------------------------------------------ s8 shadow (KIND 2, DESIGN.md section 5c)
+__device__ __forceinline__ float warp_max_f(float v) {
+    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ double warp_sum_d(double v) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+// code of one normalised entry v under scale sc (sc = 0: every v of the row set is 0)
+__device__ __forceinline__ int s8_code(float v, float sc) {
+    return sc > 0.0f ? max(-127, min(127, __float2int_rn(__fdiv_rn(v, sc)))) : 0;
+}
+// upper bound of sqrt(e2), e2 a sum of at most 2^17 f64 squares (relative rounding error < 2^-35, covered by 2^-30)
+__device__ __forceinline__ float residual_norm_up(double e2) {
+    return __double2float_ru(__dsqrt_ru(__dmul_ru(e2, 1.0 + 0x1p-30)));
+}
+
+// One CTA (8 warps, a warp per row) per corpus tile t = tile0 + blockIdx.x, rows [256t, min(256t + 256, row_end)):
+// x_hat = x / |x| exactly as normalize_f16_kernel computes it, s_T = max |x_hat_i| / 127 over the tile's proper rows,
+// codes rint(x_hat / s_T), E_T >= max over proper rows of |x_hat - s_T * codes| (f64, rounded up).  Degenerate rows get
+// zero codes and no say in s_T or E_T.
+__global__ void __launch_bounds__(256) quantize_s8_tiles_kernel(const float *__restrict__ raw, uint32_t pitch_elems,
+                                                                const float *__restrict__ mags, uint32_t tile0, uint64_t row_end,
+                                                                uint32_t dim, int8_t *__restrict__ xs8, uint32_t pitch8,
+                                                                float2 *__restrict__ tile_se) {
+    __shared__ float s_max[8];
+    __shared__ double s_e2[8];
+    const uint32_t t = tile0 + blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t r0 = (uint64_t)t * TS_BLOCK_N, r1 = min(r0 + TS_BLOCK_N, row_end);
+    float mx = 0.0f;
+    for (uint64_t r = r0 + warp; r < r1; r += 8) {
+        const float m = mags[r];
+        if (!norm_is_proper(m)) continue;
+        for (uint32_t c = lane; c < dim; c += 32) mx = fmaxf(mx, fabsf(__fdiv_rn(raw[r * pitch_elems + c], m)));
+    }
+    mx = warp_max_f(mx);
+    if (lane == 0) s_max[warp] = mx;
+    __syncthreads();
+    mx = s_max[0];
+    for (int w = 1; w < 8; ++w) mx = fmaxf(mx, s_max[w]);
+    const float st = mx > 0.0f ? __fdiv_rn(mx, 127.0f) : 0.0f;
+    double e2 = 0.0;
+    for (uint64_t r = r0 + warp; r < r1; r += 8) {
+        const float m = mags[r];
+        const bool ok = norm_is_proper(m);
+        double rr = 0.0;
+        for (uint32_t c = lane; c < dim; c += 32) {
+            const float v = ok ? __fdiv_rn(raw[r * pitch_elems + c], m) : 0.0f;
+            const int code = s8_code(v, st);
+            xs8[r * pitch8 + c] = (int8_t)code;
+            const double d = (double)v - (double)st * (double)code;
+            rr += d * d;
+        }
+        e2 = fmax(e2, warp_sum_d(rr));
+    }
+    if (lane == 0) s_e2[warp] = e2;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < 8; ++w) e2 = fmax(e2, s_e2[w]);
+        tile_se[t] = make_float2(st, residual_norm_up(e2));
+    }
+}
+
+// *out = max over the first ntiles tiles of E_T (the shard's E_max, read by the s8 gate)
+__global__ void __launch_bounds__(1024) s8_emax_kernel(const float2 *__restrict__ tile_se, uint32_t ntiles, float *out) {
+    __shared__ float s_max[32];
+    float mx = 0.0f;
+    for (uint32_t t = threadIdx.x; t < ntiles; t += 1024) mx = fmaxf(mx, tile_se[t].y);
+    mx = warp_max_f(mx);
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        mx = warp_max_f(s_max[threadIdx.x]);
+        if (threadIdx.x == 0) *out = mx;
+    }
+}
+
+cdb_status quantize_s8_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
+                              uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
+                              cudaStream_t s) {
+    if (!n) return CDB_OK;
+    const uint32_t t0 = (uint32_t)(first / TS_BLOCK_N), t1 = (uint32_t)((first + n + TS_BLOCK_N - 1) / TS_BLOCK_N);
+    quantize_s8_tiles_kernel<<<t1 - t0, 256, 0, s>>>(d_raw, pitch_elems, d_mags, t0, row_end, dim,
+                                                     reinterpret_cast<int8_t *>(d_xs8), pitch8, d_tile_se);
+    CDB_LAUNCH_CHECK();
+    s8_emax_kernel<<<1, 1024, 0, s>>>(d_tile_se, (uint32_t)((row_end + TS_BLOCK_N - 1) / TS_BLOCK_N), d_emax);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
 // Degenerate rows of an appended range.  deg = {all-zero rows, other degenerate rows, ids of the first TS_MAX_ODD of those}.
 // An all-zero row scores 0/0 = NaN against every finite query: provably last.  Any other degenerate row (norm underflowed
 // to 0 with non-zero elements -> +-inf, overflowed norm -> 0 or NaN, inf/NaN elements) can land anywhere in the exact
@@ -455,7 +628,9 @@ cdb_status classify_rows_device(const float *d_raw, uint32_t pitch_elems, const 
 // kernels whose launch gaps were a fixed ~0.1 ms per batch -- the limiter of strong scaling once the scan itself takes 1.6 ms):
 //   q_raw   f32 copy in the index's pitched layout (operand of the exact re-rank), zero padded
 //   q_mags  |q| = sqrt of the SEQUENTIAL fold of x*x (vector_store.rs:412), one thread, squares staged in shared memory
-//   qh      fp16 copy of q / |q| (zero row for a degenerate norm and for the padding rows up to mtiles*128)
+//   qh      fp16 copy of q / |q| (zero row for a degenerate norm and for the padding rows up to mtiles*128), or with q_se
+//           (s8 form, KIND 2) s8 codes rint(q_hat / s_q) with s_q = max |q_hat_i| / 127 (qh_pitch then counts bytes) and
+//           q_se = {s_q, e_q >= |q_hat - s_q * codes|}
 //   ggm     class maxima of the query := -inf;  cand_cnt := number of pre-seeded odd rows (+ their ids);  err := 0
 //   progress counters of the seeding and of the main pass := 0
 // One CTA of 128 threads per query slot (mtiles*128 slots).
@@ -464,16 +639,21 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const float *__restri
                                                            uint32_t qh_pitch, int *__restrict__ ggm, const uint32_t *__restrict__ deg,
                                                            uint32_t has_deg, uint32_t id_base, uint32_t *__restrict__ cand,
                                                            uint32_t cand_cap, uint32_t *__restrict__ cand_cnt, uint32_t *__restrict__ err32,
-                                                           uint8_t *__restrict__ err8, uint32_t *__restrict__ progress) {
-    extern __shared__ float sq[];     // [dim] squares
+                                                           uint8_t *__restrict__ err8, uint32_t *__restrict__ progress,
+                                                           float2 *__restrict__ q_se) {
+    extern __shared__ float sq[];     // [dim] squares, then (s8 form) q_hat
     __shared__ float s_mag;
+    __shared__ float s_max[4];
+    __shared__ double s_e2[4];
     const uint32_t slot = blockIdx.x, tid = threadIdx.x;
     if (slot == 0) for (uint32_t i = tid; i < 2048; i += 128) progress[i] = 0u;
     // class maxima: layout [tile][class][128]
     if (tid < (uint32_t)TS_GROUPS) ggm[((size_t)(slot >> 7) * TS_GROUPS + tid) * TS_BLOCK_M + (slot & 127u)] = (int)0x807FFFFF;   // f2ord(-inf)
     __half *hrow = qh + (size_t)slot * qh_pitch;
+    int8_t *crow = reinterpret_cast<int8_t *>(qh) + (size_t)slot * qh_pitch;
     if (slot >= nq) {
-        for (uint32_t c = tid; c < qh_pitch; c += 128) hrow[c] = __float2half_rn(0.0f);
+        if (q_se) for (uint32_t c = tid; c < qh_pitch; c += 128) crow[c] = 0;
+        else for (uint32_t c = tid; c < qh_pitch; c += 128) hrow[c] = __float2half_rn(0.0f);
         return;
     }
     const float *src = q + (size_t)slot * dim;
@@ -502,21 +682,51 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const float *__restri
     __syncthreads();
     const float m = s_mag;
     const bool ok = norm_is_proper(m);
-    for (uint32_t c = tid; c < qh_pitch; c += 128)
-        hrow[c] = __float2half_rn((ok && c < dim) ? __fdiv_rn(src[c], m) : 0.0f);
+    if (!q_se) {
+        for (uint32_t c = tid; c < qh_pitch; c += 128)
+            hrow[c] = __float2half_rn((ok && c < dim) ? __fdiv_rn(src[c], m) : 0.0f);
+        return;
+    }
+    const uint32_t warp = tid >> 5, lane = tid & 31;
+    float mx = 0.0f;
+    for (uint32_t c = tid; c < dim; c += 128) {
+        const float v = ok ? __fdiv_rn(src[c], m) : 0.0f;
+        sq[c] = v;
+        mx = fmaxf(mx, fabsf(v));
+    }
+    mx = warp_max_f(mx);
+    if (lane == 0) s_max[warp] = mx;
+    __syncthreads();
+    mx = fmaxf(fmaxf(s_max[0], s_max[1]), fmaxf(s_max[2], s_max[3]));
+    const float sc = mx > 0.0f ? __fdiv_rn(mx, 127.0f) : 0.0f;
+    double e2 = 0.0;
+    for (uint32_t c = tid; c < qh_pitch; c += 128) {
+        int code = 0;
+        if (c < dim) {
+            const float v = sq[c];
+            code = s8_code(v, sc);
+            const double d = (double)v - (double)sc * (double)code;
+            e2 += d * d;
+        }
+        crow[c] = (int8_t)code;
+    }
+    e2 = warp_sum_d(e2);
+    if (lane == 0) s_e2[warp] = e2;
+    __syncthreads();
+    if (tid == 0) q_se[slot] = make_float2(sc, residual_norm_up((s_e2[0] + s_e2[1]) + (s_e2[2] + s_e2[3])));
 }
 
 cdb_status prep_queries_device(const float *d_q, uint32_t nq, uint32_t dim, float *d_q_raw, uint32_t raw_pitch_elems, float *d_q_mags,
                                void *d_qh, uint32_t qh_pitch_halfs, int *d_ggm, const uint32_t *d_deg, bool has_deg, uint32_t id_base,
                                uint32_t *d_cand, uint32_t cand_cap, uint32_t *d_cand_cnt, uint32_t *d_err32, uint8_t *d_err8,
-                               uint32_t *d_progress, cudaStream_t s) {
+                               uint32_t *d_progress, float2 *d_q_se, cudaStream_t s) {
     const uint32_t mtiles = (nq + TS_BLOCK_M - 1) / TS_BLOCK_M;
     // dim*4 bytes of squares: above 12287 dims that exceeds the 48 KB a launch gets without the opt-in
     CDB_ALLOW_SMEM(prep_queries_kernel, (size_t)dim * 4);
     prep_queries_kernel<<<mtiles * TS_BLOCK_M, 128, (size_t)dim * 4, s>>>(d_q, nq, dim, d_q_raw, raw_pitch_elems, d_q_mags,
                                                                           reinterpret_cast<__half *>(d_qh), qh_pitch_halfs, d_ggm, d_deg,
                                                                           has_deg ? 1u : 0u, id_base, d_cand, cand_cap, d_cand_cnt, d_err32,
-                                                                          d_err8, d_progress);
+                                                                          d_err8, d_progress, d_q_se);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }
@@ -610,9 +820,9 @@ static cdb_status launch_tensor_scan_gd(const CUtensorMap &mq, const CUtensorMap
 
 template <int NG, int KIND>
 static cdb_status launch_tensor_scan_g(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid, cudaStream_t s) {
-    if (KIND == 1) return launch_tensor_scan_gd<NG, false, KIND>(mq, mx, a, grid, s);   // exact scores: no degenerate-row variant
-    return a.has_deg ? launch_tensor_scan_gd<NG, true, 0>(mq, mx, a, grid, s)
-                     : launch_tensor_scan_gd<NG, false, 0>(mq, mx, a, grid, s);
+    if constexpr (KIND == 1) return launch_tensor_scan_gd<NG, false, KIND>(mq, mx, a, grid, s);   // exact scores: no degenerate-row variant
+    else return a.has_deg ? launch_tensor_scan_gd<NG, true, KIND>(mq, mx, a, grid, s)
+                     : launch_tensor_scan_gd<NG, false, KIND>(mq, mx, a, grid, s);
 }
 
 // fewer classes = cheaper bound refresh (the sort network grows as NG log^2 NG); the bound stays within ~1.5x of the
@@ -700,6 +910,52 @@ cdb_status tensor_scan_device(const void *d_xh, const void *d_qh, uint32_t pitch
 
     a.rel = 1.0f;
     return run_tensor_scan<0>(mq, mx, a, n_rows, d_progress, sm_count, s);
+}
+
+// smallest float >= x
+static float f32_up(double x) {
+    float f = (float)x;
+    return (double)f < x ? std::nextafter(f, INFINITY) : f;
+}
+
+// s8 form (KIND 2, DESIGN.md section 5c): d_xs8 s8 shadow [n_rows][pitch8], d_qs8 query codes padded with zero rows to a
+// multiple of 128, d_tile_se / d_q_se their {scale, residual bound}.  Same candidates / class maxima contract as
+// tensor_scan_device; prep_queries_device (s8 mode) has reset them.
+cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t pitch8, uint64_t n_rows, uint32_t nq, uint32_t dim,
+                                 uint32_t k, const float2 *d_tile_se, const float2 *d_q_se, uint32_t id_base, int *d_ggm,
+                                 uint32_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_progress, bool has_deg,
+                                 int sm_count, cudaStream_t s) {
+    TensorScanArgs a{};
+    a.has_deg = has_deg ? 1u : 0u;
+    a.window = 3;
+    a.refresh_mask = 15;
+    if (const char *e = getenv("CDB_TS_WINDOW")) a.window = (uint32_t)atoi(e);
+    if (const char *e = getenv("CDB_TS_REFRESH")) a.refresh_mask = (uint32_t)atoi(e);
+    a.n_rows = n_rows;
+    a.n_queries = nq;
+    a.k = k;
+    a.kblocks = (dim + 2 * TS_BLOCK_K - 1) / (2 * TS_BLOCK_K);   // 128 s8 elements per 128-byte row
+    a.mtiles = (nq + TS_BLOCK_M - 1) / TS_BLOCK_M;
+    a.ntiles = (uint32_t)((n_rows + TS_BLOCK_N - 1) / TS_BLOCK_N);
+    a.id_base = id_base;
+    a.ggm = d_ggm;
+    a.cand = d_cand;
+    a.cand_cnt = d_cand_cnt;
+    a.cand_cap = cand_cap;
+    a.tile_se = d_tile_se;
+    a.q_se = d_q_se;
+    // u = 2^-24.  |x_hat|, |q_hat| <= 1 + (D/2 + 2) u + O(D^2 u^2) (sequential f32 norm, one division per entry);
+    // |cos_ref - q_hat . x_hat| <= (D + 4) u + O(D^2 u^2) (FMA dot product, norm product, division).  Both are taken
+    // twice over, which covers the second-order terms for every D <= rerank_f32_max_dim().
+    a.dn1 = f32_up(1.0 + ((double)dim + 8.0) * 0x1p-24);
+    a.dref = f32_up((2.0 * dim + 16.0) * 0x1p-24);
+    a.rel = 1.0f;
+    if (!tensor_scan_stages(k)) { set_error("s8 tensor scan: k too large (class-maximum bound needs k <= 64)"); return CDB_INVALID_PARAMS; }
+    CUtensorMap mq, mx;
+    cdb_status rc;
+    if ((rc = make_tensor_map_2d(&mq, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_qs8, (uint64_t)a.mtiles * TS_BLOCK_M, dim, pitch8, TS_BLOCK_M))) return rc;
+    if ((rc = make_tensor_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_xs8, n_rows, dim, pitch8, TS_BLOCK_N))) return rc;
+    return run_tensor_scan<2>(mq, mx, a, n_rows, d_progress, sm_count, s);
 }
 
 // Integer form (tensor_scan_u8.cu): d_x u8 operand rows [n_rows][pitch] (u8 codes or unpacked digits), d_q the query operand

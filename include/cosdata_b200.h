@@ -533,8 +533,9 @@ cdb_status cdb_index_scan_ms_history(const cdb_index *index, uint32_t n, float *
 cdb_status cdb_index_stats(const cdb_index *index, uint64_t *out4);
 /* the first n of: {tensor-core searches, searches where some query needed the exact scan, all-zero rows, other degenerate rows
  * (norm outside [1e-15, 1e15]: they ride on every prefilter candidate list), fp16 shadow present, queries of the LAST
- * tensor-core search that were re-done by the exact scan (candidate overflow or degenerate query norm)} */
-#define CDB_STATS_FIELDS 6
+ * tensor-core search that were re-done by the exact scan (candidate overflow or degenerate query norm), tensor-core
+ * searches whose prefilter ran in the s8 form (also counted in the first field)} */
+#define CDB_STATS_FIELDS 7
 cdb_status cdb_index_stats_ex(const cdb_index *index, uint64_t *out, uint32_t n);
 /* candidates the prefilter emitted for each of the first n queries of the last prefilter search */
 cdb_status cdb_index_last_candidate_counts(const cdb_index *index, uint32_t n, uint32_t *out);
