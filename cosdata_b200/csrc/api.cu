@@ -1430,6 +1430,7 @@ cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
         set_error("metric/storage arm is an Err in the reference");
         return rc;
     }
+    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
     const uint32_t n = (uint32_t)ix->size;
     // root vector: uniform in [range_lo, range_hi) (vector_store.rs:57-64)
     std::vector<float> root(ix->desc.dim);
@@ -1478,6 +1479,7 @@ cdb_status cdb_index_build_graph_replicas(cdb_index *ix, const cdb_build_params 
         set_error("metric/storage arm is an Err in the reference");
         return rc;
     }
+    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
     // main root: uniform in [range_lo, range_hi) (vector_store.rs:57-64); pseudo root: pseudo_node_vector = zeros (metadata/mod.rs:214-216)
     std::vector<float> roots(2 * (size_t)ix->desc.dim, 0.0f);
     for (uint32_t c = 0; c < ix->desc.dim; ++c)
@@ -1567,6 +1569,7 @@ cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, con
     const uint64_t n_new = ix->size - ix->g_cnt[0];
     if (!n_new) return CDB_OK;
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
     {   // searches already enqueued on their callers' streams finish on the old graph before it changes
         std::lock_guard<std::mutex> g(ix->pool_mu);
         for (auto &u : ix->pool)
@@ -1614,6 +1617,7 @@ cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n
         if (!ix->is_deleted(rows[i]) && seen.insert(rows[i]).second) { status[i] = 0; fresh.push_back(rows[i]); }
     cdb_status rc;
     if (!fresh.empty()) {
+        if (ix->has_graph && (rc = hnsw_build_smem_check(ix->row_pitch, HNSW_DELETE_EF))) return rc;
         const size_t words = ix->desc.capacity / 32 + 1;
         if (!ix->d_deleted) {   // allocated before anything changes; kernels see it only once a row is deleted
             void *p = nullptr;

@@ -453,6 +453,21 @@ static cdb_status publish(const HnswBuildState &st, const GraphHost &gh) {
     return CDB_OK;
 }
 
+cdb_status hnsw_build_smem_check(uint32_t row_pitch, uint32_t ef) {
+    int dev = 0, optin = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa;
+    CDB_CUDA_TRY(cudaFuncGetAttributes(&fa, reinterpret_cast<const void *>(hnsw_build_search_kernel)));
+    const size_t need = hn_smem_bytes(row_pitch, ef) + fa.sharedSizeBytes;
+    if (need > (size_t)optin) {
+        set_error("hnsw build: ef " + std::to_string(ef) + " with " + std::to_string(row_pitch) + "-byte rows needs " +
+                  std::to_string(need) + " bytes of shared memory per block, the device allows " + std::to_string(optin));
+        return CDB_INVALID_PARAMS;
+    }
+    return CDB_OK;
+}
+
 // index_embeddings for rows [first, first+count) (levels[i] = max insert level of row first+i), the one batch loop of both
 // the build and the insert.  Nodes for every level the rows reach are appended up front (level 0: node = row; levels >= 1:
 // ascending rows after the existing nodes, child pointing into the appended part of the level below), so node_row / child
@@ -862,7 +877,7 @@ cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
                               uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s) {
     const GraphDev &gd = *gh.dev;
     const uint32_t L1 = st->g.num_levels + 1;
-    constexpr uint32_t DEL_EF = 512, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
+    constexpr uint32_t DEL_EF = HNSW_DELETE_EF, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
     // level-local index of every row on every level (level 0 is the row when the level lists rows in order)
     std::vector<uint32_t> loc((size_t)n * L1, HN_EMPTY);
     std::unordered_map<uint32_t, uint32_t> pos;

@@ -192,6 +192,11 @@ cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
                               uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s);
 // similarity keys of every slot of `level` ([cnt*nb], device)
 const uint32_t *hnsw_state_slot_keys(const HnswBuildState *st, uint32_t level);
+constexpr uint32_t HNSW_DELETE_EF = 512;   // the ef of a delete's traversal (vector_store.rs:1247)
+// CDB_INVALID_PARAMS (with a message) when the graph writers' traversal kernel cannot run at this row pitch and ef: its
+// dynamic shared memory (hn_smem_bytes) plus its static shared memory exceed the current device's opt-in limit per block.
+// The build, replica build, insert and delete entry points call it before they change anything.
+cdb_status hnsw_build_smem_check(uint32_t row_pitch, uint32_t ef);
 
 // replica lists: one entry per graph node to create, host arrays (cdb_replica_build)
 struct ReplicaHost {

@@ -166,7 +166,9 @@ static cdb_status run_quantize(Src src, uint64_t n, uint32_t dim, int st, float 
     uint32_t blocks = (uint32_t)((total + 255) / 256);
     quantize_codes_kernel<Src><<<blocks, 256, 0, s>>>(src, n, dim, st, lo, hi, codes, row_pitch, raw, raw_pitch_elems);
     CDB_LAUNCH_CHECK();
-    if (n <= 8192 && (size_t)dim * 4 <= 48 * 1024)
+    // the squares share the 48 KB default with the kernel's static word (16 bytes with the dynamic area's alignment): at
+    // D = 12288 they alone fill it and the launch would fail
+    if (n <= 8192 && (size_t)dim * 4 + 16 <= 48 * 1024)
         mags_cta_kernel<Src><<<(uint32_t)n, 128, (size_t)dim * 4, s>>>(src, n, dim, st, lo, hi, mags);
     else
         mags_kernel<Src><<<(uint32_t)((n + 127) / 128), 128, 0, s>>>(src, n, dim, st, lo, hi, mags);

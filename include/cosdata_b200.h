@@ -324,7 +324,10 @@ cdb_status cdb_index_set_graph_from_files(cdb_index *index, const cdb_hnsw_files
  * values_range, id u32::MAX; vector_store.rs:57-67) as the last row and builds the HNSW graph over all rows with the
  * reference's algorithm (traverse with ef_construction per level, create_node_edges / add_neighbor with
  * lowest-similarity eviction), batches of up to max_batch vectors in flight like the reference's concurrent build.
- * The index needs capacity for one more row.  The result replaces any uploaded graph and can be read back. */
+ * The index needs capacity for one more row.  The result replaces any uploaded graph and can be read back.
+ * The traversal keeps a row and ef_construction queue entries in shared memory: a row size / ef_construction pair above the
+ * device's per-block limit (on an H100, f32 rows at ef_construction 4096 fit up to about D = 10.4K) is refused with CDB_INVALID_PARAMS
+ * before anything changes; the same check guards the replica build, the insert and the delete (at ef 512). */
 typedef struct {
     uint32_t num_levels;              /* hnsw.default_num_layer = 9 (config.toml:19-25) */
     uint32_t neighbors_count;         /* 32 */
