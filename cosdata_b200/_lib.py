@@ -91,6 +91,15 @@ class ReplicaBuild(C.Structure):
     ]
 
 
+class ReplicaInsert(C.Structure):
+    _fields_ = [
+        ("n_nodes", C.c_uint32),
+        ("row", C.c_void_p), ("node_id", C.c_void_p), ("base_id", C.c_void_p), ("md_row", C.c_void_p), ("max_level", C.c_void_p),
+        ("md_dims", C.c_uint32), ("n_md_new", C.c_uint32),
+        ("md_bits_new", C.c_void_p), ("md_mags_new", C.c_void_p),
+    ]
+
+
 class SearchParams(C.Structure):
     _fields_ = [
         ("k", C.c_uint32),
@@ -150,6 +159,8 @@ PROTOTYPES = {
     "cdb_index_graph_info": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "cdb_index_read_graph_level": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cdb_index_insert_graph": (C.c_int32, [C.c_void_p, C.POINTER(BuildParams), c_vp, c_vp, C.POINTER(C.c_uint64)]),
+    "cdb_index_insert_graph_replicas": (C.c_int32, [C.c_void_p, C.POINTER(BuildParams), C.POINTER(ReplicaInsert), c_vp,
+                                                    C.POINTER(C.c_uint64)]),
     "cdb_index_read_graph_slot_scores": (C.c_int32, [C.c_void_p, C.c_uint32, c_vp]),
     "cdb_index_delete_rows": (C.c_int32, [C.c_void_p, c_vp, C.c_uint64, C.c_uint32, C.c_uint32, c_vp, C.POINTER(C.c_uint64)]),
     "cdb_index_deleted_rows": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, c_vp, C.POINTER(C.c_uint64)]),

@@ -631,6 +631,36 @@ class DenseIndex:
         self.md_dims = bits.shape[1]
         return failed[:n]
 
+    def insert_graph_replicas(self, row, node_id, base_id, md_row, max_level, md_bits_new=None, md_mags_new=None,
+                              ef_construction=128, shortlist_size=64, max_batch=4096):
+        """GPU-side index_embeddings on a graph that build_graph_replicas built (cdb_index_insert_graph_replicas): one entry per
+        graph node to create, rows already appended; row 0xFFFFFFFF = the pseudo root's vector.  md_bits_new / md_mags_new:
+        rows appended to the graph's metadata table (md_row may name them).  num_levels and the neighbour counts are the
+        graph's.  -> failed u8[n_nodes]"""
+        from ._lib import ReplicaInsert
+        check_insert_args(ef_construction, shortlist_size, max_batch)
+        # without a graph with metadata there is no md_dims: the library refuses the call (CDB_INVALID_PARAMS)
+        md_dims = getattr(self, "md_dims", None) or (np.asarray(md_bits_new).shape[-1] if md_bits_new is not None else 1)
+        arrs = [np.ascontiguousarray(a, dtype=np.uint32) for a in (row, node_id, base_id, md_row)]
+        n = arrs[0].size
+        if max_level is None:
+            raise ValueError("max_level (the caller's get_max_insert_level draws) is required")
+        lv = check_insert_args(ef_construction, shortlist_size, max_batch, max_level, n)
+        if any(a.ndim != 1 or a.size != n for a in arrs):
+            raise ValueError("row, node_id, base_id, md_row and max_level need one entry per node")
+        bits = np.zeros((0, md_dims), np.int32) if md_bits_new is None else np.ascontiguousarray(md_bits_new, dtype=np.int32)
+        mags = np.zeros(0, np.float32) if md_mags_new is None else np.ascontiguousarray(md_mags_new, dtype=np.float32)
+        if bits.ndim != 2 or bits.shape[1] != md_dims or mags.shape != (bits.shape[0],):
+            raise ValueError(f"md_bits_new must be [n, {md_dims}] with one md_mags_new entry per row")
+        info = np.zeros(5, dtype=np.uint32)
+        _check(self._lib.cdb_index_graph_info(self._h, _ptr(info), None))
+        ri = ReplicaInsert(n, *[a.ctypes.data for a in arrs], lv.ctypes.data, md_dims, bits.shape[0], bits.ctypes.data, mags.ctypes.data)
+        bp = BuildParams(int(info[0]), int(info[1]), int(info[2]), ef_construction, shortlist_size, max_batch, 0)
+        failed = np.zeros(max(n, 1), dtype=np.uint8)
+        done = C.c_uint64(0)
+        _check(self._lib.cdb_index_insert_graph_replicas(self._h, C.byref(bp), C.byref(ri), _ptr(failed), C.byref(done)))
+        return failed[: done.value]
+
     def read_graph_metadata(self):
         """-> (node_id[], node_md[]) per level of a graph with replica nodes"""
         info = np.zeros(5, dtype=np.uint32)

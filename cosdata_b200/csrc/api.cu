@@ -1383,6 +1383,11 @@ cdb_status cdb_index_set_graph_metadata(cdb_index *ix, const cdb_graph_metadata 
     for (void *g : ix->md_allocs) cudaFree(g);
     ix->md_allocs.clear();
     ix->has_md = false;
+    uint32_t pseudo_row, n_md;
+    if (hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {   // a replica build's state does not describe uploaded metadata
+        hnsw_state_free(ix->bstate);
+        ix->bstate = nullptr;
+    }
     auto upload = [&](const void *src, size_t bytes, const void **dst) -> cdb_status {
         void *p = nullptr;
         CDB_CUDA_TRY(cudaMalloc(&p, bytes ? bytes : 4));
@@ -1413,7 +1418,9 @@ cdb_status cdb_index_set_graph_metadata(cdb_index *ix, const cdb_graph_metadata 
 }
 
 static GraphHost graph_host(cdb_index *ix) {
-    return GraphHost{&ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr, &ix->g_ad, &ix->g_ch};
+    GraphHost gh{&ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr, &ix->g_ad, &ix->g_ch};
+    if (ix->has_md) { gh.id = &ix->g_id; gh.md = &ix->g_md; gh.id_tbl = ix->md_node_id; gh.md_tbl = ix->md_node_md; }
+    return gh;
 }
 
 cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
@@ -1502,7 +1509,7 @@ cdb_status cdb_index_build_graph_replicas(cdb_index *ix, const cdb_build_params 
     std::vector<uint8_t> failed;
     rc = hnsw_build_replicas_device(sc, rh, bp->num_levels, bp->neighbors_count, bp->level0_neighbors_count, bp->ef_construction,
                                     bp->shortlist_size, bp->max_batch, &ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr,
-                                    &ix->g_ad, &ix->g_ch, &mdv, &failed, ix->stream);
+                                    &ix->g_ad, &ix->g_ch, &mdv, &failed, &ix->bstate, ix->stream);
     if (rc) return rc;
     ix->has_graph = true;
     ix->md_node_id = mdv.node_id; ix->md_node_md = mdv.node_md;
@@ -1594,6 +1601,75 @@ cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, con
         return rc;
     }
     if (out_inserted) *out_inserted = n_new;
+    return CDB_OK;
+}
+
+cdb_status cdb_index_insert_graph_replicas(cdb_index *ix, const cdb_build_params *bp, const cdb_replica_insert *ri, uint8_t *out_failed,
+                                           uint64_t *out_inserted) {
+    CDB_REQUIRE(ix && bp && ri, "null argument");
+    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64,
+                "bad build parameters");
+    if (out_inserted) *out_inserted = 0;
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph && ix->has_md,
+                "no graph with metadata: cdb_index_build_graph_replicas first (a graph without metadata grows through cdb_index_insert_graph)");
+    uint32_t pseudo_row = 0, n_md = 0;
+    if (!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {
+        set_error("insert into a graph whose metadata was uploaded is not supported (its slot similarities cannot be derived)");
+        return CDB_UNSUPPORTED;
+    }
+    CDB_REQUIRE(bp->num_levels == ix->graph.num_levels && bp->neighbors_count == ix->graph.nbrs &&
+                    bp->level0_neighbors_count == ix->graph.nbrs0,
+                "params num_levels / neighbors_count / level0_neighbors_count differ from the graph's");
+    CDB_REQUIRE(ri->md_dims == ix->md_dims, "md_dims differs from the graph's");
+    CDB_REQUIRE((ri->row && ri->node_id && ri->base_id && ri->md_row && ri->max_level) || !ri->n_nodes, "null replica list");
+    CDB_REQUIRE((ri->md_bits_new && ri->md_mags_new) || !ri->n_md_new, "null metadata table rows");
+    CDB_REQUIRE((uint64_t)n_md + ri->n_md_new < CDB_INVALID_ID, "metadata table too large");
+    const uint64_t n_md_all = (uint64_t)n_md + ri->n_md_new;
+    for (uint32_t t = 0; t < ri->n_nodes; ++t) {
+        const uint32_t r = ri->row[t];
+        CDB_REQUIRE(r == CDB_INVALID_ID || r < ix->size, "replica row out of range");
+        CDB_REQUIRE(r != ix->graph.root_row && r != pseudo_row, "replica row is one of the graph's root rows");
+        CDB_REQUIRE(r == CDB_INVALID_ID || !ix->is_deleted(r), "replica row is deleted");
+        CDB_REQUIRE(ri->md_row[t] == CDB_INVALID_ID || ri->md_row[t] < n_md_all, "replica md_row out of range");
+    }
+    cdb_status rc;
+    if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
+        set_error("metric/storage arm is an Err in the reference");
+        return rc;
+    }
+    if (!ri->n_nodes) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
+    {   // searches already enqueued on their callers' streams finish on the old graph before it changes
+        std::lock_guard<std::mutex> g(ix->pool_mu);
+        for (auto &u : ix->pool)
+            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
+    }
+    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    std::vector<uint32_t> rows(ri->row, ri->row + ri->n_nodes);
+    for (auto &r : rows) if (r == CDB_INVALID_ID) r = pseudo_row;   // pseudo replicas reuse the pseudo root's prop_value (vector_store.rs:661)
+    ReplicaHost rh{ri->n_nodes, rows.data(), ri->node_id, ri->base_id, ri->md_row, ri->max_level, ri->md_dims, ri->n_md_new,
+                   ri->md_bits_new, ri->md_mags_new, ix->graph.root_row, CDB_INVALID_ID, pseudo_row, CDB_INVALID_ID};
+    HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
+    bool changed = false;
+    if ((rc = hnsw_insert_replicas_device(sc, graph_host(ix), ix->bstate, rh, bp->ef_construction, bp->shortlist_size, bp->max_batch,
+                                          out_failed, &ix->md_bits, &ix->md_mags, &changed, ix->stream))) {
+        if (changed) {   // a half-inserted graph is not the reference's graph: the index has none until a build / upload
+            const std::string why = cdb_last_error_string();
+            hnsw_state_free(ix->bstate);
+            ix->bstate = nullptr;
+            for (void *g : ix->graph_allocs) cudaFree(g);
+            ix->graph_allocs.clear();
+            for (void *g : ix->md_allocs) cudaFree(g);
+            ix->md_allocs.clear();
+            ix->has_md = false;
+            ix->has_graph = false;
+            set_error(why + " (the insert had started: the graph and its metadata were dropped)");
+        }
+        return rc;
+    }
+    if (out_inserted) *out_inserted = ri->n_nodes;
     return CDB_OK;
 }
 

@@ -314,9 +314,22 @@ __global__ void __launch_bounds__(SS_WARPS * 32) hnsw_slot_state_kernel(BuildLev
 struct HnswBuildState {
     BuildGraph g{};                          // level arrays (owned by the graph's allocations) and the slot state
     uint64_t cap[BUILD_MAX_LEVELS] = {};     // nodes each level's arrays hold
+    // replica graphs (cdb_index_build_graph_replicas): levels also carry node_id / node_md / node_ins
+    bool replicas = false;
+    uint32_t n_list = 0;                     // replica list positions created so far (the next node's node_ins)
+    uint32_t pseudo_root_row = 0;            // g.root_row is the main root's row
+    uint32_t n_md = 0, md_dims = 0;          // the Metadata table (owned by the graph's allocations)
+    const int32_t *md_bits = nullptr;
+    const float *md_mags = nullptr;
 };
 void hnsw_state_free(HnswBuildState *st) { delete st; }
 const uint32_t *hnsw_state_slot_keys(const HnswBuildState *st, uint32_t level) { return st->g.lv[level].simkey; }
+bool hnsw_state_replica_info(const HnswBuildState *st, uint32_t *pseudo_root_row, uint32_t *n_md) {
+    if (!st || !st->replicas) return false;
+    *pseudo_root_row = st->pseudo_root_row;
+    *n_md = st->n_md;
+    return true;
+}
 
 static void metric_key_range(int metric, uint32_t *min_key, uint32_t *max_key) {   // MetricResult::min / ::max (types.rs:435-457)
     switch (metric) {
@@ -356,8 +369,9 @@ struct DevAllocs {
     void release() { p.clear(); }
 };
 
-// the arrays of one level: per node (node_row, lowest_idx, lowest_key, lock, child) and per slot (adj, simkey)
-constexpr int LEVEL_ARRAYS = 7;
+// the arrays of one level: per node (node_row, lowest_idx, lowest_key, lock, child), per slot (adj, simkey), and on replica
+// graphs per node (node_id, node_md, node_ins)
+constexpr int LEVEL_ARRAYS = 10, PLAIN_LEVEL_ARRAYS = 7;
 static uint32_t *&level_array(BuildLevel &l, int t) {
     switch (t) {
     case 0: return l.node_row;
@@ -366,17 +380,28 @@ static uint32_t *&level_array(BuildLevel &l, int t) {
     case 3: return reinterpret_cast<uint32_t *&>(l.lock);
     case 4: return l.child;
     case 5: return l.adj;
-    default: return l.simkey;
+    case 6: return l.simkey;
+    case 7: return const_cast<uint32_t *&>(l.node_id);
+    case 8: return const_cast<uint32_t *&>(l.node_md);
+    default: return const_cast<uint32_t *&>(l.node_ins);
     }
 }
-static size_t level_words(const BuildLevel &l, int t, uint64_t nodes) { return t >= 5 ? nodes * l.nb : nodes; }
+static size_t level_words(const BuildLevel &l, int t, uint64_t nodes) { return t == 5 || t == 6 ? nodes * l.nb : nodes; }
 
-// Appends nodes (vector rows rows[L], level-local children child[L] on levels >= 1) to every level.  Arrays that must
-// grow are allocated first (by half their size at least; level 0 never beyond rows_cap nodes): if one allocation fails,
-// nothing has changed.  After that *changed is set; the old arrays are copied, the new nodes start as ProbNode::new (no
-// neighbours, lowest_index (0, MetricResult::min)), the search layout is re-published and the old arrays are freed.
+// the per-level columns of nodes appended to a replica graph, parallel to append_levels' rows
+struct ReplicaCols {
+    std::vector<std::vector<uint32_t>> id, md, ins;
+};
+
+// Appends nodes (vector rows rows[L], level-local children child[L] on levels >= 1; on replica graphs also rc->id / md / ins)
+// to every level.  Arrays that must grow are allocated first (by half their size at least; level 0 never beyond rows_cap
+// nodes): if one allocation fails, nothing has changed.  After that *changed is set; the old arrays are copied, the new
+// nodes start as ProbNode::new (no neighbours, lowest_index (0, MetricResult::min)), the search layout is re-published and
+// the old arrays are freed.
 static cdb_status append_levels(HnswBuildState &st, const GraphHost &gh, const std::vector<std::vector<uint32_t>> &rows,
-                                const std::vector<std::vector<uint32_t>> &child, uint64_t rows_cap, bool *changed, cudaStream_t s) {
+                                const std::vector<std::vector<uint32_t>> &child, uint64_t rows_cap, bool *changed, cudaStream_t s,
+                                const ReplicaCols *rcols = nullptr) {
+    const int n_arrays = st.replicas ? LEVEL_ARRAYS : PLAIN_LEVEL_ARRAYS;
     const uint32_t L1 = st.g.num_levels + 1;
     cdb_status rc;
     std::vector<uint64_t> cap(L1, 0);
@@ -389,7 +414,7 @@ static cdb_status append_levels(HnswBuildState &st, const GraphHost &gh, const s
         if (need <= st.cap[L]) continue;
         cap[L] = std::max<uint64_t>(need, st.cap[L] + st.cap[L] / 2);
         if (L == 0) cap[L] = std::max<uint64_t>(need, std::min<uint64_t>(cap[L], rows_cap));
-        for (int t = 0; t < LEVEL_ARRAYS; ++t)
+        for (int t = 0; t < n_arrays; ++t)
             if ((t != 4 || L > 0) && (rc = grown.get((void **)&fresh[L][t], level_words(l, t, cap[L]) * 4))) return rc;
     }
     // ---- commit: every new array joins the graph's allocations, the old ones leave them once the tables moved on
@@ -400,7 +425,7 @@ static cdb_status append_levels(HnswBuildState &st, const GraphHost &gh, const s
     for (uint32_t L = 0; L < L1; ++L) {
         BuildLevel &l = st.g.lv[L];
         if (cap[L]) {
-            for (int t = 0; t < LEVEL_ARRAYS; ++t) {
+            for (int t = 0; t < n_arrays; ++t) {
                 if (!fresh[L][t]) continue;
                 uint32_t *&arr = level_array(l, t);
                 const size_t used = level_words(l, t, l.cnt);
@@ -417,6 +442,11 @@ static cdb_status append_levels(HnswBuildState &st, const GraphHost &gh, const s
             if (rows[L][i] != l.cnt + i) { gh.dev->identity_mask &= ~(1u << L); break; }
         CDB_CUDA_TRY(cudaMemcpyAsync(l.node_row + l.cnt, rows[L].data(), (size_t)add * 4, cudaMemcpyHostToDevice, s));
         if (L > 0) CDB_CUDA_TRY(cudaMemcpyAsync(l.child + l.cnt, child[L].data(), (size_t)add * 4, cudaMemcpyHostToDevice, s));
+        if (rcols) {
+            const std::vector<uint32_t> *col[3] = {&rcols->id[L], &rcols->md[L], &rcols->ins[L]};
+            for (int c = 0; c < 3; ++c)
+                CDB_CUDA_TRY(cudaMemcpyAsync(level_array(l, 7 + c) + l.cnt, col[c]->data(), (size_t)add * 4, cudaMemcpyHostToDevice, s));
+        }
         const uint64_t slots = (uint64_t)add * l.nb;
         fill_u32_kernel<<<(uint32_t)((slots + 255) / 256), 256, 0, s>>>(l.adj + (size_t)l.cnt * l.nb, HN_EMPTY, slots);
         CDB_LAUNCH_CHECK();
@@ -450,6 +480,12 @@ static cdb_status publish(const HnswBuildState &st, const GraphHost &gh) {
     CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->node_row, gh.nr->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
     CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->adj, gh.ad->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
     CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->child, gh.ch->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+    if (gh.id) {   // replica graphs: the tables the filtered search (hnsw_md.cu) reads
+        gh.id->assign(L1, nullptr); gh.md->assign(L1, nullptr);
+        for (uint32_t L = 0; L < L1; ++L) { (*gh.id)[L] = st.g.lv[L].node_id; (*gh.md)[L] = st.g.lv[L].node_md; }
+        CDB_CUDA_TRY(cudaMemcpy((void *)gh.id_tbl, gh.id->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+        CDB_CUDA_TRY(cudaMemcpy((void *)gh.md_tbl, gh.md->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
+    }
     return CDB_OK;
 }
 
@@ -991,7 +1027,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
                                       std::vector<void *> *out_allocs, std::vector<uint32_t> *out_counts,
                                       std::vector<const uint32_t *> *out_nr, std::vector<const uint32_t *> *out_ad,
                                       std::vector<const uint32_t *> *out_ch, ReplicaGraphDev *out_md, std::vector<uint8_t> *out_failed,
-                                      cudaStream_t s) {
+                                      HnswBuildState **out_state, cudaStream_t s) {
     if (num_levels + 1 > BUILD_MAX_LEVELS) { set_error("build: too many levels"); return CDB_INVALID_PARAMS; }
     const uint32_t L1 = num_levels + 1, n = rh.n_nodes;
     std::vector<uint8_t> levels(n);
@@ -1142,6 +1178,132 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
     out_md->md_mags = rl.md_mags;
     out_md->md_dims = rh.md_dims;
     out_md->pseudo_entry = 1;
+    // the builder's state stays with the graph, so hnsw_insert_replicas_device can continue where this build stopped
+    std::unique_ptr<HnswBuildState> st(new HnswBuildState());
+    st->g = bg;
+    for (uint32_t L = 0; L < L1; ++L) st->cap[L] = bg.lv[L].cnt;
+    st->replicas = true;
+    st->n_list = n;
+    st->pseudo_root_row = rh.pseudo_root_row;
+    st->n_md = rh.n_md;
+    st->md_dims = rh.md_dims;
+    st->md_bits = rl.md_bits;
+    st->md_mags = rl.md_mags;
+    *out_state = st.release();
+    return CDB_OK;
+}
+
+// index_embeddings over more IndexableEmbeddings of a collection with a metadata schema, into the graph a replica build made
+// (and earlier calls grew).  New nodes are appended to every level they reach, behind the existing ones in list order, with
+// node_ins continuing the list positions, so build_local's binary search and both kernels run unchanged; ReplicaDev is
+// offset so that it is indexed by those global positions.  Batches hold max(1, min(max_batch, nodes already linked / 8)).
+// Every allocation (the list, the batch buffers, the grown Metadata table, the grown level arrays) happens before the graph
+// changes; the table replaces the old one only once the insert has succeeded.
+cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const ReplicaHost &rh,
+                                       uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed,
+                                       const int32_t **md_bits, const float **md_mags, bool *changed, cudaStream_t s) {
+    const uint32_t L1 = st->g.num_levels + 1, n = rh.n_nodes, first = st->n_list, M = st->md_dims;
+    std::vector<uint8_t> levels(n);
+    std::vector<std::vector<uint32_t>> rows(L1), child(L1);
+    ReplicaCols cols;
+    cols.id.resize(L1); cols.md.resize(L1); cols.ins.resize(L1);
+    std::vector<std::vector<uint32_t>> members(L1);   // new list indices present on each level
+    for (uint32_t t = 0; t < n; ++t) {
+        levels[t] = (uint8_t)std::min<uint32_t>(rh.max_level[t], st->g.num_levels);
+        for (uint32_t L = 0; L <= levels[t]; ++L) {
+            members[L].push_back(t);
+            rows[L].push_back(rh.row[t]);
+            cols.id[L].push_back(rh.node_id[t]);
+            cols.md[L].push_back(rh.md_row[t]);
+            cols.ins[L].push_back(first + t);
+        }
+    }
+    for (uint32_t L = 1; L < L1; ++L) {
+        uint32_t j = 0;   // position among the nodes appended one level down (both lists ascend)
+        for (uint32_t t : members[L]) {
+            while (members[L - 1][j] != t) ++j;
+            child[L].push_back(st->g.lv[L - 1].cnt + j);
+        }
+    }
+    if (max_batch == 0) max_batch = 4096;
+    max_batch = std::max<uint32_t>(1, std::min(max_batch, n));
+    // ---- every allocation before the graph changes
+    cdb_status rc;
+    DevAllocs tmp, table;
+    uint32_t *d_list = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
+    uint8_t *d_levels = nullptr, *failed = nullptr;
+    if ((rc = tmp.get((void **)&d_list, (size_t)n * 4 * 4)) || (rc = tmp.get((void **)&d_levels, n)) || (rc = tmp.get((void **)&failed, n)) ||
+        (rc = tmp.get((void **)&z_nodes, (size_t)max_batch * L1 * 64 * 4)) || (rc = tmp.get((void **)&z_keys, (size_t)max_batch * L1 * 64 * 4)) ||
+        (rc = tmp.get((void **)&z_n, (size_t)max_batch * L1 * 4)))
+        return rc;
+    const uint32_t n_md = st->n_md + rh.n_md;
+    int32_t *new_bits = nullptr;
+    float *new_mags = nullptr;
+    if (rh.n_md) {   // the grown table: the old rows, then the new ones
+        if ((rc = table.get((void **)&new_bits, (size_t)n_md * M * 4)) || (rc = table.get((void **)&new_mags, (size_t)n_md * 4))) return rc;
+        CDB_CUDA_TRY(cudaMemcpyAsync(new_bits, st->md_bits, (size_t)st->n_md * M * 4, cudaMemcpyDeviceToDevice, s));
+        CDB_CUDA_TRY(cudaMemcpyAsync(new_bits + (size_t)st->n_md * M, rh.md_bits, (size_t)rh.n_md * M * 4, cudaMemcpyHostToDevice, s));
+        CDB_CUDA_TRY(cudaMemcpyAsync(new_mags, st->md_mags, (size_t)st->n_md * 4, cudaMemcpyDeviceToDevice, s));
+        CDB_CUDA_TRY(cudaMemcpyAsync(new_mags + st->n_md, rh.md_mags, (size_t)rh.n_md * 4, cudaMemcpyHostToDevice, s));
+    }
+    const uint32_t *src[4] = {rh.row, rh.node_id, rh.base_id, rh.md_row};
+    for (int c = 0; c < 4; ++c) CDB_CUDA_TRY(cudaMemcpyAsync(d_list + (size_t)c * n, src[c], (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_levels, levels.data(), n, cudaMemcpyHostToDevice, s));
+    const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
+    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    if ((rc = append_levels(*st, gh, rows, child, ~0ull, changed, s, &cols))) return rc;
+    // ---- batches
+    BuildArgs a{};
+    a.g = st->g;
+    a.sc = sc;
+    a.sc.root_row = st->g.root_row;
+    a.levels = d_levels;
+    a.lv_first = first;
+    a.ef = ef_construction;
+    a.shortlist = shortlist;
+    a.zcap = 64;
+    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
+    a.replicas = true;
+    a.rl.row = d_list - first;   // indexed by global list position: entry t of this call is position first + t
+    a.rl.id = d_list + n - first;
+    a.rl.base_id = d_list + 2 * (size_t)n - first;
+    a.rl.md = d_list + 3 * (size_t)n - first;
+    a.rl.md_bits = rh.n_md ? new_bits : st->md_bits;
+    a.rl.md_mags = rh.n_md ? new_mags : st->md_mags;
+    a.rl.M = M;
+    a.rl.key_one = order_key(CDB_METRIC_COSINE, 0x3F800000u);
+    a.rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
+    for (uint32_t done = 0; done < n;) {
+        uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, (uint32_t)(((uint64_t)first + done) / 8)));
+        batch = std::min<uint32_t>(batch, n - done);
+        a.first = first + done;
+        a.count = batch;
+        a.failed = failed + done;
+        hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        hnsw_build_link_kernel<<<(batch * 32 + 127) / 128, 128, 0, s>>>(a);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        done += batch;
+    }
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e == cudaSuccess && out_failed) e = cudaMemcpy(out_failed, failed, n, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error(std::string("hnsw replica insert: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    // ---- the grown table replaces the old one
+    if (rh.n_md) {
+        for (const void *old : {(const void *)st->md_bits, (const void *)st->md_mags}) {
+            auto it = std::find(gh.allocs->begin(), gh.allocs->end(), old);
+            if (it != gh.allocs->end()) { gh.allocs->erase(it); cudaFree(const_cast<void *>(old)); }
+        }
+        gh.allocs->insert(gh.allocs->end(), table.p.begin(), table.p.end());
+        table.release();
+        st->md_bits = new_bits;
+        st->md_mags = new_mags;
+        st->n_md = n_md;
+    }
+    st->n_list += n;
+    *md_bits = st->md_bits;
+    *md_mags = st->md_mags;
     return CDB_OK;
 }
 

@@ -165,6 +165,9 @@ struct GraphHost {
     std::vector<void *> *allocs;
     std::vector<uint32_t> *cnt;
     std::vector<const uint32_t *> *nr, *ad, *ch;
+    // graphs with replica nodes (null otherwise): host copies and device tables of the per-level node_id / node_md arrays
+    std::vector<const uint32_t *> *id = nullptr, *md = nullptr;
+    const uint32_t *const *id_tbl = nullptr, *const *md_tbl = nullptr;
 };
 // the builder's per-slot state (similarity keys, stale lowest_index, node locks), kept next to the graph it belongs to
 struct HnswBuildState;
@@ -215,12 +218,22 @@ struct ReplicaGraphDev {
     const float *md_mags;
     uint32_t md_dims, pseudo_entry;
 };
+// out_state: the builder's state of the replica graph, which hnsw_insert_replicas_device continues from
 cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &rh, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
                                       uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, GraphDev *out_graph,
                                       std::vector<void *> *out_allocs, std::vector<uint32_t> *out_counts,
                                       std::vector<const uint32_t *> *out_nr, std::vector<const uint32_t *> *out_ad,
                                       std::vector<const uint32_t *> *out_ch, ReplicaGraphDev *out_md, std::vector<uint8_t> *out_failed,
-                                      cudaStream_t s);
+                                      HnswBuildState **out_state, cudaStream_t s);
+// true (and the pseudo root's row, the Metadata table's row count) when `st` is the state of a replica build
+bool hnsw_state_replica_info(const HnswBuildState *st, uint32_t *pseudo_root_row, uint32_t *n_md);
+// cdb_index_insert_graph_replicas: the nodes of `rh` (n_nodes entries; row already mapped to the pseudo root's row where the
+// caller passed CDB_INVALID_ID; md_bits / md_mags / n_md = the table rows to append) inserted into the replica graph of
+// `st`, continuing its list positions.  On success *md_bits / *md_mags point at the grown Metadata table.  *changed as for
+// hnsw_insert_device.
+cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const ReplicaHost &rh,
+                                       uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed,
+                                       const int32_t **md_bits, const float **md_mags, bool *changed, cudaStream_t s);
 
 // ---- tensor_scan.cu (wgmma prefilter)
 constexpr uint32_t TS_MAX_ODD = 64;   // degenerate rows that are not all-zero ride on every candidate list; more -> no prefilter

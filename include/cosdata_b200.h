@@ -351,7 +351,8 @@ cdb_status cdb_index_build_graph(cdb_index *index, const cdb_build_params *param
  * main_root_md; pseudo root: zeros, id u32::MAX - 257, metadata pseudo_root_md).  Every level lists [0] main root,
  * [1] pseudo root, then the created nodes in list order.  out_failed[n_nodes] (optional): 1 where the reference's insert
  * would have returned Err / panicked (the node stays unlinked).  The graph and its metadata replace any uploaded ones;
- * searches then go through cdb_search_batch_filtered / CDB_MODE_HNSW as after cdb_index_set_graph_metadata. */
+ * searches then go through cdb_search_batch_filtered / CDB_MODE_HNSW as after cdb_index_set_graph_metadata.  The handle
+ * keeps the builder's state, so cdb_index_insert_graph_replicas can grow the graph later. */
 typedef struct {
     uint32_t n_nodes;
     const uint32_t *row, *node_id, *base_id, *md_row;
@@ -382,7 +383,7 @@ cdb_status cdb_index_read_graph_level(const cdb_index *index, uint32_t level, ui
  * prob_node.rs:145-181: every slot's similarity recomputed, lowest_index = the first empty slot, else the first slot with
  * the strictly lowest similarity).  A slot whose pair is an Err (e.g. a zero-norm row under cosine) gets MetricResult::min
  * and is the first slot replaced.  Graphs with metadata (cdb_index_set_graph_metadata, *_replicas, *_from_files):
- * CDB_UNSUPPORTED.  No new rows: CDB_OK, *out_inserted = 0.  The level-0 list must be rows 0..level_counts[0]-1.
+ * CDB_UNSUPPORTED (a graph that cdb_index_build_graph_replicas built grows through cdb_index_insert_graph_replicas).  No new rows: CDB_OK, *out_inserted = 0.  The level-0 list must be rows 0..level_counts[0]-1.
  * Takes the writer lock; searches enqueued (cdb_search_batch_device) before the call see the old graph, searches after it
  * the new one; the call returns once the graph is complete.  Failure: every device allocation happens before the graph
  * changes, so an error there (e.g. CDB_CUDA_ERROR on out-of-memory) leaves the graph and its rows as they were and the call
@@ -390,6 +391,41 @@ cdb_status cdb_index_read_graph_level(const cdb_index *index, uint32_t level, ui
  * until cdb_index_build_graph / cdb_index_set_graph, and cdb_last_error_string says so. */
 cdb_status cdb_index_insert_graph(cdb_index *index, const cdb_build_params *params, const uint8_t *max_level, uint8_t *out_failed,
                                   uint64_t *out_inserted);
+/* index_embeddings on a graph with metadata (src/vector_store.rs:714-780): creates more nodes of preprocess_embedding's
+ * flattened IndexableEmbeddings (:629-712) in a graph that cdb_index_build_graph_replicas built on this handle and that
+ * earlier calls of this function may have grown.  The replica build, continued:
+ *   row        a row < cdb_index_size() the caller has already appended, or CDB_INVALID_ID for the pseudo root's row (pseudo
+ *              replicas, :655-667); a row out of range, one of the graph's two root rows or a deleted row: CDB_INVALID_PARAMS
+ *   node_id, base_id, md_row, max_level   as in cdb_replica_build; md_row is CDB_INVALID_ID or below the table's rows plus
+ *              n_md_new; max_level is required when n_nodes > 0 (clamped to num_levels)
+ *   md_dims    must equal the graph's
+ *   n_md_new, md_bits_new, md_mags_new   rows appended to the graph's Metadata table, only when the call returns CDB_OK
+ * A node whose metadata has mag != 0 descends from the pseudo root, every other node from the main root; edges follow
+ * create_node_edges with the replica rules (:1014-1040), and every node keeps its add_neighbor state (slot similarities,
+ * stale lowest_index) from the build and earlier inserts.  New nodes are appended to every level they reach, behind the
+ * existing ones, in list order.  out_failed[n_nodes] (may be NULL): 1 where the reference's insert returns Err (the node
+ * stays unlinked).  *out_inserted (may be NULL) = n_nodes.
+ * params: num_levels / neighbors_count / level0_neighbors_count must equal the graph's; ef_construction, shortlist_size and
+ * max_batch as for the build (batches of max(1, min(max_batch, nodes already linked / 8)); 1 inserts one node at a time,
+ * deterministically); seed is unused (level draws come from the caller).
+ * No graph, or a graph without metadata (those grow through cdb_index_insert_graph): CDB_INVALID_PARAMS.  A graph whose
+ * metadata came from cdb_index_set_graph_metadata / cdb_index_set_graph_from_files: CDB_UNSUPPORTED (its slot similarities
+ * cannot be derived).  n_nodes == 0: CDB_OK, *out_inserted = 0, nothing changes (no table rows are appended either).
+ * Locking, the order against enqueued searches and the failure contract are those of cdb_index_insert_graph: every
+ * allocation comes before the graph changes, so an allocation failure leaves the graph, its metadata and its table as they
+ * were; an error after the graph started changing drops the graph and its metadata, and cdb_last_error_string says so.
+ * cdb_index_insert_graph, cdb_index_delete_rows and cdb_index_read_graph_slot_scores stay CDB_UNSUPPORTED on these graphs. */
+typedef struct {
+    uint32_t n_nodes;                           /* graph nodes to create, in insertion order */
+    const uint32_t *row, *node_id, *base_id, *md_row;   /* as in cdb_replica_build */
+    const uint8_t *max_level;                   /* the caller's get_max_insert_level draws */
+    uint32_t md_dims;                           /* must equal the graph's */
+    uint32_t n_md_new;                          /* rows appended to the graph's Metadata table */
+    const int32_t *md_bits_new;                 /* [n_md_new x md_dims] */
+    const float *md_mags_new;                   /* [n_md_new] */
+} cdb_replica_insert;
+cdb_status cdb_index_insert_graph_replicas(cdb_index *index, const cdb_build_params *params, const cdb_replica_insert *nodes,
+                                           uint8_t *out_failed, uint64_t *out_inserted);
 /* similarity stored with each neighbour slot of `level` (level_counts[level] x neighbours f32, the MetricResult value; 0 for
  * empty slots): what the reference's serializer writes next to each link (serializer/hnsw/neighbors.rs:53-57).  Derived
  * as above for an uploaded graph.  Graphs with metadata: CDB_UNSUPPORTED. */

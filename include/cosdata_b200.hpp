@@ -175,6 +175,15 @@ class DenseIndex {
         failed.resize(n);
         return failed;
     }
+    // index_embeddings on a graph that build_graph_replicas built: more flattened IndexableEmbeddings (rows already appended);
+    // returns the per-entry "insert failed" flags
+    std::vector<uint8_t> insert_graph_replicas(const cdb_replica_insert &ri, const cdb_build_params &bp) {
+        std::vector<uint8_t> failed(ri.n_nodes ? ri.n_nodes : 1);
+        uint64_t n = 0;
+        check(cdb_index_insert_graph_replicas(h_, &bp, &ri, failed.data(), &n));
+        failed.resize(n);
+        return failed;
+    }
     // delete_embedding for local rows; returns the per-row status (0 deleted, 1 already deleted, 2 an Err stopped relinks)
     std::vector<uint8_t> delete_rows(const std::vector<uint32_t> &rows, uint32_t shortlist_size = 64, uint32_t max_batch = 0) {
         std::vector<uint8_t> status(std::max<size_t>(rows.size(), 1));
