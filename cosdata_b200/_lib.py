@@ -163,6 +163,8 @@ PROTOTYPES = {
                                                     C.POINTER(C.c_uint64)]),
     "cdb_index_read_graph_slot_scores": (C.c_int32, [C.c_void_p, C.c_uint32, c_vp]),
     "cdb_index_delete_rows": (C.c_int32, [C.c_void_p, c_vp, C.c_uint64, C.c_uint32, C.c_uint32, c_vp, C.POINTER(C.c_uint64)]),
+    "cdb_index_delete_rows_replicas": (C.c_int32, [C.c_void_p, c_vp, C.c_uint64, C.c_uint32, C.c_uint32, c_vp, C.POINTER(C.c_uint64)]),
+    "cdb_index_read_replica_slot_scores": (C.c_int32, [C.c_void_p, C.c_uint32, c_vp]),
     "cdb_index_deleted_rows": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, c_vp, C.POINTER(C.c_uint64)]),
     "cdb_index_hnsw_counters": (C.c_int32, [C.c_void_p, C.c_void_p]),
     "cdb_search_batch": (C.c_int32, [C.c_void_p, c_f32p, C.c_uint32, C.POINTER(SearchParams), c_u32p, c_f32p, c_u32p, c_u8p]),

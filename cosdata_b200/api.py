@@ -593,6 +593,34 @@ class DenseIndex:
         _check(self._lib.cdb_index_delete_rows(self._h, _ptr(r), r.size, shortlist_size, max_batch, _ptr(status), None))
         return status[: r.size]
 
+    def delete_rows_replicas(self, rows, shortlist_size=64, max_batch=0):
+        """delete_embedding on a graph that build_graph_replicas built (cdb_index_delete_rows_replicas): every node of each
+        row, its base replica and its Metadata replicas, is deleted -> status u8[len(rows)]: 0 deleted, 1 already deleted,
+        2 deleted but an Err hit one of the row's nodes"""
+        r = np.asarray(rows)
+        if r.ndim != 1:
+            raise ValueError(f"rows must be one-dimensional, got shape {r.shape}")
+        if r.size and (r.min() < 0 or r.max() >= self.size):
+            raise ValueError(f"rows must be in 0..{self.size - 1}")
+        check_insert_args(1, shortlist_size, max_batch)
+        r = np.ascontiguousarray(r, dtype=np.uint32)
+        status = np.zeros(max(r.size, 1), dtype=np.uint8)
+        _check(self._lib.cdb_index_delete_rows_replicas(self._h, _ptr(r), r.size, shortlist_size, max_batch, _ptr(status), None))
+        return status[: r.size]
+
+    def read_replica_slot_scores(self):
+        """-> [f32[level_counts[L] * neighbours]] per level of a graph that build_graph_replicas built: the similarity its
+        builder keeps with each neighbour slot (0 = empty slot)"""
+        info = np.zeros(5, dtype=np.uint32)
+        counts = np.zeros(32, dtype=np.uint32)
+        _check(self._lib.cdb_index_graph_info(self._h, _ptr(info), _ptr(counts)))
+        out = []
+        for lv in range(int(info[0]) + 1):
+            a = np.zeros(int(counts[lv]) * int(info[2] if lv == 0 else info[1]), dtype=np.float32)
+            _check(self._lib.cdb_index_read_replica_slot_scores(self._h, lv, _ptr(a)))
+            out.append(a)
+        return out
+
     def deleted_rows(self):
         """-> bool[size]: True where the row is deleted"""
         out = np.zeros(max(self.size, 1), dtype=np.uint8)

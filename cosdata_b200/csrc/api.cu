@@ -1749,6 +1749,110 @@ cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n
     return CDB_OK;
 }
 
+cdb_status cdb_index_delete_rows_replicas(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
+                                          uint8_t *out_status, uint64_t *out_deleted) {
+    CDB_REQUIRE(ix && (rows || !n), "null argument");
+    CDB_REQUIRE(shortlist_size >= 1 && shortlist_size <= 64, "shortlist_size must be in 1..64");
+    if (out_deleted) *out_deleted = 0;
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph && ix->has_md,
+                "no graph with metadata: cdb_index_build_graph_replicas first (a graph without metadata deletes through cdb_index_delete_rows)");
+    uint32_t pseudo_row = 0, n_md = 0;
+    if (!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {
+        set_error("delete from a graph whose metadata was uploaded is not supported (its slot similarities cannot be derived)");
+        return CDB_UNSUPPORTED;
+    }
+    for (uint64_t i = 0; i < n; ++i) {
+        CDB_REQUIRE(rows[i] < ix->size, "row out of range");
+        CDB_REQUIRE(rows[i] != ix->graph.root_row && rows[i] != pseudo_row, "the graph's root rows cannot be deleted");
+    }
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    // status 1 for rows deleted before or earlier in the list
+    std::vector<uint8_t> status(n, 1);
+    std::vector<uint32_t> fresh;
+    std::unordered_set<uint32_t> seen;
+    for (uint64_t i = 0; i < n; ++i)
+        if (!ix->is_deleted(rows[i]) && seen.insert(rows[i]).second) { status[i] = 0; fresh.push_back(rows[i]); }
+    cdb_status rc;
+    if (!fresh.empty()) {
+        if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
+            set_error("metric/storage arm is an Err in the reference");
+            return rc;
+        }
+        if ((rc = hnsw_build_smem_check(ix->row_pitch, HNSW_DELETE_EF))) return rc;
+        const size_t words = ix->desc.capacity / 32 + 1;
+        if (!ix->d_deleted) {   // allocated before anything changes; kernels see it only once a row is deleted
+            void *p = nullptr;
+            CDB_CUDA_TRY(cudaMalloc(&p, words * 4));
+            ix->d_deleted = (uint32_t *)p;
+            ix->h_deleted.assign(words, 0u);
+            CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
+        }
+        {   // searches already enqueued on their callers' streams finish on the old graph and the old marks
+            std::lock_guard<std::mutex> g(ix->pool_mu);
+            for (auto &u : ix->pool)
+                if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
+        }
+        CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+        std::vector<uint8_t> fst(fresh.size(), 0);
+        HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
+        bool changed = false;
+        if ((rc = hnsw_delete_replicas_device(sc, graph_host(ix), ix->bstate, fresh.data(), (uint32_t)fresh.size(), shortlist_size,
+                                              max_batch, fst.data(), &changed, ix->stream))) {
+            if (changed) {   // a half-repaired graph links deleted rows: the index has no graph until a build / upload
+                const std::string why = cdb_last_error_string();
+                hnsw_state_free(ix->bstate);
+                ix->bstate = nullptr;
+                for (void *g : ix->graph_allocs) cudaFree(g);
+                ix->graph_allocs.clear();
+                for (void *g : ix->md_allocs) cudaFree(g);
+                ix->md_allocs.clear();
+                ix->has_md = false;
+                ix->has_graph = false;
+                set_error(why + " (the delete had started: the graph and its metadata were dropped)");
+            }
+            return rc;
+        }
+        // the marks, once the repair succeeded
+        uint32_t lo = 0xFFFFFFFFu, hi = 0;
+        for (uint32_t r : fresh) {
+            ix->h_deleted[r >> 5] |= 1u << (r & 31);
+            lo = std::min(lo, r >> 5);
+            hi = std::max(hi, r >> 5);
+        }
+        CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted + lo, ix->h_deleted.data() + lo, (size_t)(hi - lo + 1) * 4, cudaMemcpyHostToDevice));
+        ix->n_deleted += fresh.size();
+        size_t j = 0;
+        for (uint64_t i = 0; i < n; ++i)
+            if (status[i] == 0) status[i] = fst[j++];
+        if (out_deleted) *out_deleted = fresh.size();
+    }
+    if (out_status) std::copy(status.begin(), status.end(), out_status);
+    return CDB_OK;
+}
+
+cdb_status cdb_index_read_replica_slot_scores(cdb_index *ix, uint32_t level, float *out_scores) {
+    CDB_REQUIRE(ix && out_scores, "null argument");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph && level <= ix->graph.num_levels, "no graph / bad level");
+    CDB_REQUIRE(ix->has_md, "the graph has no metadata: cdb_index_read_graph_slot_scores reads its slot scores");
+    uint32_t pseudo_row = 0, n_md = 0;
+    if (!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {
+        set_error("slot scores of a graph whose metadata was uploaded are not supported (they cannot be derived)");
+        return CDB_UNSUPPORTED;
+    }
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    const size_t slots = (size_t)ix->g_cnt[level] * (level == 0 ? ix->graph.nbrs0 : ix->graph.nbrs);
+    std::vector<uint32_t> adj(slots), keys(slots);
+    CDB_CUDA_TRY(cudaMemcpy(adj.data(), ix->g_ad[level], slots * 4, cudaMemcpyDeviceToHost));
+    CDB_CUDA_TRY(cudaMemcpy(keys.data(), hnsw_state_slot_keys(ix->bstate, level), slots * 4, cudaMemcpyDeviceToHost));
+    for (size_t t = 0; t < slots; ++t) {
+        const uint32_t b = adj[t] == CDB_INVALID_ID ? 0u : key_to_bits(ix->desc.metric, keys[t]);
+        std::memcpy(out_scores + t, &b, 4);
+    }
+    return CDB_OK;
+}
+
 cdb_status cdb_index_deleted_rows(const cdb_index *ix, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total) {
     CDB_REQUIRE(ix && (out || !n), "null argument");
     CDB_REQUIRE(first + n <= ix->desc.capacity, "rows out of range");

@@ -699,6 +699,14 @@ struct DelArgs {
     uint32_t *touched[BUILD_MAX_LEVELS];   // [cnt/32+1] nodes the sweep cleared a slot of
     uint2 *list[BUILD_MAX_LEVELS];         // [cnt] (node, batch position) of each touched node
     uint32_t *list_n;                      // [num_levels+1]
+    // replica graphs (hnsw_delete_replicas_device): the batch positions are replica-list items (every node of a deleted row),
+    // the batch's rows own items [row_items[j], row_items[j+1]) for j from rfirst, relinks rescore with the replica arms
+    // and apply the edge rules, and a touched node takes the candidates of the smallest batch position it named (tmin)
+    bool replicas;
+    ReplicaDev rl;                         // the Metadata table and the edge rules' keys
+    const uint32_t *row_items;
+    uint32_t rfirst;
+    uint32_t *tmin[BUILD_MAX_LEVELS];      // [cnt] HN_EMPTY between calls; null on plain graphs
 };
 
 __global__ void hnsw_delete_mark_kernel(DelArgs a) {
@@ -729,6 +737,14 @@ __device__ bool build_is_empty(const BuildLevel &l, uint32_t node) {
     return true;
 }
 
+// one side of calculate() for a node of a replica graph: VectorData { Some(get_id()), vector, metadata }
+__device__ __forceinline__ MdSide del_md_side(const ReplicaDev &rl, const BuildLevel &l, uint32_t node, const void *code, float mag,
+                                              uint32_t pp) {
+    const uint32_t mrow = l.node_md[node];
+    return MdSide{code, mag, pp, true, l.node_id[node], mrow == HN_EMPTY ? nullptr : rl.md_bits + (size_t)mrow * rl.M,
+                  mrow == HN_EMPTY ? 0.0f : rl.md_mags[mrow]};
+}
+
 struct DelSmem {
     uint64_t keys[2][128];
     uint32_t nodes[2][128];
@@ -744,6 +760,7 @@ __device__ bool del_relink(const DelArgs &a, uint32_t level, uint32_t N, uint32_
     const HnScoreCtx &sc = a.sc;
     const uint32_t lane = threadIdx.x & 31, bar = hw_smem_u32(&sm.bar);
     const uint32_t nrow = l.node_row[N];
+    const bool rules = a.replicas && sc.metric == CDB_METRIC_COSINE;   // the rules match MetricResult::CosineSimilarity only
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncwarp();
     if (lane == 0) {
@@ -762,11 +779,20 @@ __device__ bool del_relink(const DelArgs &a, uint32_t level, uint32_t N, uint32_
         const uint32_t ball = __ballot_sync(0xFFFFFFFFu, keep);
         if (keep) {
             const uint32_t crow = l.node_row[c], pos = m + __popc(ball & ((1u << lane) - 1u));
+            const uint8_t *ccode = sc.rows + (size_t)crow * sc.row_pitch;
             float d = 0.f;
-            const int rc = pair_distance(sc.metric, sc.st, sc.dim, row, sc.mags[nrow], pp, sc.rows + (size_t)crow * sc.row_pitch,
-                                         sc.mags[crow], pp, &d);
+            int rc;
+            uint32_t cid;
+            if (a.replicas) {   // calculate(N, cand) with the replica arms: N's id and metadata are x
+                rc = md_pair_distance(sc.metric, sc.st, sc.dim, a.rl.M, del_md_side(a.rl, l, N, row, sc.mags[nrow], pp),
+                                      del_md_side(a.rl, l, c, ccode, sc.mags[crow], pp), &d);
+                cid = l.node_id[c];
+            } else {
+                rc = pair_distance(sc.metric, sc.st, sc.dim, row, sc.mags[nrow], pp, ccode, sc.mags[crow], pp, &d);
+                cid = hn_id(sc.root_row, crow);
+            }
             if (rc != CDB_OK) bad = true;
-            sm.keys[0][pos] = make_key64(order_key(sc.metric, __float_as_uint(d)), hn_id(sc.root_row, crow));
+            sm.keys[0][pos] = make_key64(order_key(sc.metric, __float_as_uint(d)), cid);
             sm.nodes[0][pos] = c;
         }
         m += __popc(ball);
@@ -781,11 +807,17 @@ __device__ bool del_relink(const DelArgs &a, uint32_t level, uint32_t N, uint32_
         sm.nodes[1][r] = sm.nodes[0][i];
     }
     __syncwarp();
-    if (lane == 0) {   // create_node_edges (vector_store.rs:976-1070), Base nodes
+    if (lane == 0) {   // create_node_edges (vector_store.rs:976-1070); on replica graphs with the rules of :1014-1040
+        const int nk = rules ? build_node_kind(a.rl, l, N) : MD_KIND_BASE;
         uint32_t successful = 0;
         for (uint32_t i = 0; i < m; ++i) {
             if (successful >= l.nb) break;
             const uint32_t nbr = sm.nodes[1][i], dkey = (uint32_t)(sm.keys[1][i] >> 32);
+            if (nk == MD_KIND_METADATA) {   // as hnsw_build_link_kernel
+                const int bk = build_node_kind(a.rl, l, nbr);
+                if (bk == MD_KIND_PSEUDO && dkey != a.rl.key_one) continue;
+                if (bk == MD_KIND_METADATA && dkey == a.rl.key_minus_one) continue;
+            }
             const int idx = build_add_neighbor(a.g, l, N, nbr, dkey);
             if (idx < 0) continue;
             if (build_add_neighbor(a.g, l, nbr, N, dkey) >= 0) { successful++; continue; }
@@ -804,18 +836,12 @@ __device__ inline void del_smem_init(DelSmem &sm) {
     __syncwarp();
 }
 
-// phase B: one warp (one block) per (delete, level)
-__global__ void __launch_bounds__(32) hnsw_delete_repair_kernel(DelArgs a) {
-    extern __shared__ __align__(128) uint8_t row[];
-    __shared__ DelSmem sm;
-    const uint32_t L1 = a.g.num_levels + 1, b = blockIdx.x / L1, level = blockIdx.x % L1, lane = threadIdx.x & 31;
-    const uint32_t D = a.loc[(size_t)(a.first + b) * L1 + level];
-    if (D == HN_EMPTY) return;
-    del_smem_init(sm);
+// phase B for the node D of batch position b on `level` (whole warp): D's own slots, then D isolated
+__device__ void del_repair_node(const DelArgs &a, uint32_t level, uint32_t b, uint32_t D, uint8_t *row, DelSmem &sm, uint32_t &parity) {
+    const uint32_t L1 = a.g.num_levels + 1, lane = threadIdx.x & 31;
     const BuildLevel &l = a.g.lv[level];
     const uint32_t zn = a.z_n[(size_t)b * L1 + level];
     const uint32_t *cand = a.z_nodes + ((size_t)b * L1 + level) * a.zcap;
-    uint32_t parity = 0;
     bool err = false;
     volatile uint32_t *da = l.adj + (size_t)D * l.nb;
     for (uint32_t s = 0; s < l.nb; ++s) {
@@ -835,6 +861,33 @@ __global__ void __launch_bounds__(32) hnsw_delete_repair_kernel(DelArgs a) {
         node_unlock(l.lock + D);
         if (err) a.status[a.first + b] = 2;
     }
+    __syncwarp();
+}
+
+// phase B: one warp (one block) per (delete, level)
+__global__ void __launch_bounds__(32) hnsw_delete_repair_kernel(DelArgs a) {
+    extern __shared__ __align__(128) uint8_t row[];
+    __shared__ DelSmem sm;
+    const uint32_t L1 = a.g.num_levels + 1, b = blockIdx.x / L1, level = blockIdx.x % L1;
+    const uint32_t D = a.loc[(size_t)(a.first + b) * L1 + level];
+    if (D == HN_EMPTY) return;
+    del_smem_init(sm);
+    uint32_t parity = 0;
+    del_repair_node(a, level, b, D, row, sm, parity);
+}
+
+// phase B on a replica graph: one warp (one block) per (deleted row, level) repairs the row's nodes on that level in list
+// order -- two replicas of a row can share neighbours, so one after the other keeps the result deterministic
+__global__ void __launch_bounds__(32) hnsw_delete_repair_replicas_kernel(DelArgs a) {
+    extern __shared__ __align__(128) uint8_t row[];
+    __shared__ DelSmem sm;
+    const uint32_t L1 = a.g.num_levels + 1, j = a.rfirst + blockIdx.x / L1, level = blockIdx.x % L1;
+    del_smem_init(sm);
+    uint32_t parity = 0;
+    for (uint32_t k = a.row_items[j]; k < a.row_items[j + 1]; ++k) {
+        const uint32_t D = a.loc[(size_t)k * L1 + level];
+        if (D != HN_EMPTY) del_repair_node(a, level, k - a.first, D, row, sm, parity);
+    }
 }
 
 // D2: one pass over the level's adjacency (128-bit loads, grid-stride) clears every slot naming a node deleted by this call
@@ -844,6 +897,7 @@ __device__ __forceinline__ bool del_sweep_slot(const DelArgs &a, uint32_t level,
     const uint32_t node = (uint32_t)(t / a.g.lv[level].nb), bit = 1u << (node & 31);
     if (!(atomicOr(a.touched[level] + (node >> 5), bit) & bit))
         a.list[level][atomicAdd(a.list_n + level, 1u)] = make_uint2(node, a.dead_of[level][v]);
+    if (a.tmin[level]) atomicMin(a.tmin[level] + node, a.dead_of[level][v]);   // replica graphs: the smallest position named
     v = HN_EMPTY;
     return true;
 }
@@ -878,8 +932,9 @@ __global__ void __launch_bounds__(32) hnsw_delete_relink_kernel(DelArgs a, uint3
     const BuildLevel &l = a.g.lv[level];
     const uint2 *list = a.list[level];
     uint32_t parity = 0;
+    uint32_t *tmin = a.tmin[level];
     auto process = [&](uint2 e) {
-        const uint32_t X = e.x, b = e.y;
+        const uint32_t X = e.x, b = tmin ? tmin[X] : e.y;
         const uint32_t zn = a.z_n[(size_t)b * L1 + level];
         int go = 0;
         if (lane == 0) go = zn != HN_EMPTY && !bit_set(a.dead[level], X) && build_is_empty(l, X);
@@ -892,6 +947,7 @@ __global__ void __launch_bounds__(32) hnsw_delete_relink_kernel(DelArgs a, uint3
         for (uint32_t e = blockIdx.x; e < n; e += gridDim.x) {
             process(list[e]);
             if (lane == 0) atomicAnd(a.touched[level] + (list[e].x >> 5), ~(1u << (list[e].x & 31)));
+            if (lane == 0 && tmin) tmin[list[e].x] = HN_EMPTY;
         }
         return;
     }
@@ -906,7 +962,10 @@ __global__ void __launch_bounds__(32) hnsw_delete_relink_kernel(DelArgs a, uint3
         last = (int64_t)(best >> 32);
         process(list[(uint32_t)best]);
     }
-    for (uint32_t e = lane; e < n; e += 32) atomicAnd(a.touched[level] + (list[e].x >> 5), ~(1u << (list[e].x & 31)));
+    for (uint32_t e = lane; e < n; e += 32) {
+        atomicAnd(a.touched[level] + (list[e].x >> 5), ~(1u << (list[e].x & 31)));
+        if (tmin) tmin[list[e].x] = HN_EMPTY;
+    }
 }
 
 cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
@@ -1304,6 +1363,188 @@ cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh
     st->n_list += n;
     *md_bits = st->md_bits;
     *md_mags = st->md_mags;
+    return CDB_OK;
+}
+
+// ------------------------------------------------------------------ delete_embedding on a replica graph (D5)
+// The unit is a vector row: every node whose node_row is the row (its base replica and its Metadata replicas, on every level)
+// is deleted.  Each such node is an item: it traverses as the graph sees it (hnsw_build_search_kernel in delete mode over
+// per-item arrays), then one warp per (row, level) repairs the row's nodes in list order, the sweep clears the remaining links
+// to them, and the touched nodes are relinked from the candidates of the smallest item position they named.
+struct DelHit { uint32_t level, node, ins, row, id, md; };
+
+__global__ void hnsw_delete_rowset_kernel(const uint32_t *rows, uint32_t n, uint32_t *bits) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) atomicOr(bits + (rows[i] >> 5), 1u << (rows[i] & 31));
+}
+
+// one grid-stride pass over a level's node_row behind the two roots: each node whose row is in `bits` is counted, and with
+// `out` set emitted (the order of the hits is the host's to fix)
+__global__ void hnsw_delete_find_kernel(BuildLevel l, uint32_t level, const uint32_t *bits, uint32_t n_rows, uint32_t *n_hits,
+                                        DelHit *out) {
+    for (uint32_t j = 2 + blockIdx.x * blockDim.x + threadIdx.x; j < l.cnt; j += gridDim.x * blockDim.x) {
+        const uint32_t r = l.node_row[j];
+        if (r >= n_rows || !bit_set(bits, r)) continue;
+        const uint32_t k = atomicAdd(n_hits, 1u);
+        if (out) out[k] = DelHit{level, j, l.node_ins[j], r, l.node_id[j], l.node_md[j]};
+    }
+}
+
+cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
+                                       uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s) {
+    const uint32_t L1 = st->g.num_levels + 1;
+    constexpr uint32_t DEL_EF = HNSW_DELETE_EF, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
+    for (uint32_t i = 0; i < n; ++i) out_status[i] = 0;
+    if (!n) return CDB_OK;
+    cdb_status rc;
+    int dev = 0, sms = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    // ---- the rows' nodes, found on the device (a replica graph has no level that lists rows in order)
+    const uint32_t n_rows = *std::max_element(rows, rows + n) + 1;
+    DevAllocs look;
+    uint32_t *d_rows = nullptr, *d_bits = nullptr, *d_nhits = nullptr;
+    DelHit *d_hits = nullptr;
+    if ((rc = look.get((void **)&d_rows, (size_t)n * 4)) || (rc = look.get((void **)&d_bits, (size_t)(n_rows / 32 + 1) * 4)) ||
+        (rc = look.get((void **)&d_nhits, 4)))
+        return rc;
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_rows, rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemsetAsync(d_bits, 0, (size_t)(n_rows / 32 + 1) * 4, s));
+    hnsw_delete_rowset_kernel<<<(n + 255) / 256, 256, 0, s>>>(d_rows, n, d_bits);
+    CDB_LAUNCH_CHECK();
+    uint32_t nh = 0;
+    for (int pass = 0; pass < 2; ++pass) {   // count, then emit into an array of that size
+        CDB_CUDA_TRY(cudaMemsetAsync(d_nhits, 0, 4, s));
+        for (uint32_t L = 0; L < L1; ++L) {
+            const BuildLevel &l = st->g.lv[L];
+            if (l.cnt <= 2) continue;
+            const uint32_t grid = std::min<uint32_t>((l.cnt + 255) / 256, (uint32_t)sms * 8);
+            hnsw_delete_find_kernel<<<grid, 256, 0, s>>>(l, L, d_bits, n_rows, d_nhits, d_hits);
+            CDB_LAUNCH_CHECK();
+        }
+        CDB_CUDA_TRY(cudaMemcpyAsync(&nh, d_nhits, 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaStreamSynchronize(s));
+        if (pass == 0 && !nh) return CDB_OK;   // no row of the call has a node: they are only marked
+        if (pass == 0 && (rc = look.get((void **)&d_hits, (size_t)nh * sizeof(DelHit)))) return rc;
+    }
+    std::vector<DelHit> hits(nh);
+    CDB_CUDA_TRY(cudaMemcpy(hits.data(), d_hits, (size_t)nh * sizeof(DelHit), cudaMemcpyDeviceToHost));
+    // items: the level-0 nodes (every node of the list has one), by the row's position in the call, then by list position
+    std::unordered_map<uint32_t, uint32_t> pos;
+    for (uint32_t i = 0; i < n; ++i) pos.emplace(rows[i], i);
+    std::vector<DelHit> items;
+    for (const DelHit &h : hits) if (h.level == 0) items.push_back(h);
+    std::sort(items.begin(), items.end(), [&](const DelHit &x, const DelHit &y) {
+        const uint32_t px = pos[x.row], py = pos[y.row];
+        return px != py ? px < py : x.ins < y.ins;
+    });
+    const uint32_t ni = (uint32_t)items.size();
+    std::unordered_map<uint32_t, uint32_t> item_of;   // list position -> item
+    std::vector<uint32_t> loc((size_t)ni * L1, HN_EMPTY), cols((size_t)ni * 3), iota(ni), item_pos(ni), row_items;
+    for (uint32_t k = 0; k < ni; ++k) {
+        item_of.emplace(items[k].ins, k);
+        cols[k] = items[k].row; cols[ni + k] = items[k].id; cols[2 * (size_t)ni + k] = items[k].md;
+        iota[k] = k;
+        item_pos[k] = pos[items[k].row];
+        if (!k || item_pos[k] != item_pos[k - 1]) row_items.push_back(k);
+    }
+    for (const DelHit &h : hits) loc[(size_t)item_of.at(h.ins) * L1 + h.level] = h.node;
+    const uint32_t ng = (uint32_t)row_items.size();   // rows with nodes; the others are only marked
+    row_items.push_back(ni);
+    if (max_batch == 0) max_batch = 4096;
+    max_batch = std::max<uint32_t>(1, std::min(max_batch, ng));
+    uint32_t max_items = 0;
+    for (uint32_t j = 0; j < ng; j += max_batch)
+        max_items = std::max(max_items, row_items[std::min(ng, j + max_batch)] - row_items[j]);
+    // ---- every allocation before the graph changes
+    DevAllocs tmp;
+    DelArgs d{};
+    uint32_t *d_cols = nullptr, *d_iota = nullptr, *d_loc = nullptr, *d_ri = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
+    uint8_t *failed = nullptr;
+    if ((rc = tmp.get((void **)&d_cols, cols.size() * 4)) || (rc = tmp.get((void **)&d_iota, (size_t)ni * 4)) ||
+        (rc = tmp.get((void **)&d_loc, loc.size() * 4)) || (rc = tmp.get((void **)&d_ri, row_items.size() * 4)) ||
+        (rc = tmp.get((void **)&z_nodes, (size_t)max_items * L1 * DEL_KEEP * 4)) ||
+        (rc = tmp.get((void **)&z_keys, (size_t)max_items * L1 * DEL_KEEP * 4)) || (rc = tmp.get((void **)&z_n, (size_t)max_items * L1 * 4)) ||
+        (rc = tmp.get((void **)&failed, ni)) || (rc = tmp.get((void **)&d.status, ni)) || (rc = tmp.get((void **)&d.list_n, L1 * 4)))
+        return rc;
+    for (uint32_t L = 0; L < L1; ++L) {
+        const uint32_t cnt = st->g.lv[L].cnt, words = cnt / 32 + 1;
+        if ((rc = tmp.get((void **)&d.dead[L], (size_t)words * 4)) || (rc = tmp.get((void **)&d.touched[L], (size_t)words * 4)) ||
+            (rc = tmp.get((void **)&d.dead_of[L], (size_t)cnt * 4)) || (rc = tmp.get((void **)&d.list[L], (size_t)cnt * 8)) ||
+            (rc = tmp.get((void **)&d.tmin[L], (size_t)cnt * 4)))
+            return rc;
+        CDB_CUDA_TRY(cudaMemsetAsync(d.dead[L], 0, (size_t)words * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d.touched[L], 0, (size_t)words * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d.tmin[L], 0xFF, (size_t)cnt * 4, s));
+    }
+    const size_t smem = hn_smem_bytes(sc.row_pitch, DEL_EF);
+    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    CDB_ALLOW_SMEM(hnsw_delete_repair_replicas_kernel, sc.row_pitch);
+    CDB_ALLOW_SMEM(hnsw_delete_relink_kernel, sc.row_pitch);
+    CDB_CUDA_TRY(cudaMemsetAsync(d.status, 0, ni, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_cols, cols.data(), cols.size() * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_iota, iota.data(), (size_t)ni * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_loc, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_ri, row_items.data(), row_items.size() * 4, cudaMemcpyHostToDevice, s));
+    // ---- batches of rows
+    *changed = true;
+    BuildArgs a{};
+    a.g = st->g;
+    a.sc = sc;
+    a.sc.root_row = st->g.root_row;
+    a.ef = DEL_EF;
+    a.shortlist = shortlist;
+    a.zcap = DEL_KEEP;
+    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
+    a.rowlist = d_iota;
+    a.replicas = true;
+    // the traversal of an item carries Some(its node_id) as the query id; that id only decides the Pseudo kind (types.rs:232),
+    // which a data row's replicas never have (the pseudo root's row cannot be deleted)
+    a.rl.row = d_cols;
+    a.rl.id = d_cols + ni;
+    a.rl.base_id = d_cols + ni;
+    a.rl.md = d_cols + 2 * (size_t)ni;
+    a.rl.md_bits = st->md_bits;
+    a.rl.md_mags = st->md_mags;
+    a.rl.M = st->md_dims;
+    a.rl.key_one = order_key(CDB_METRIC_COSINE, 0x3F800000u);
+    a.rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
+    d.g = st->g;
+    d.sc = a.sc;
+    d.loc = d_loc;
+    d.zcap = DEL_KEEP;
+    d.z_nodes = z_nodes; d.z_n = z_n;
+    d.replicas = true;
+    d.rl = a.rl;
+    d.row_items = d_ri;
+    const bool ordered = max_batch == 1;
+    for (uint32_t rdone = 0; rdone < ng;) {
+        const uint32_t rb = std::min(max_batch, ng - rdone), first = row_items[rdone], count = row_items[rdone + rb] - first;
+        a.first = d.first = first;
+        a.count = d.count = count;
+        a.failed = failed + first;
+        d.rfirst = rdone;
+        hnsw_delete_mark_kernel<<<(count * L1 + 127) / 128, 128, 0, s>>>(d);
+        hnsw_build_search_kernel<<<count, HN_THREADS, smem, s>>>(a);
+        hnsw_delete_repair_replicas_kernel<<<rb * L1, 32, sc.row_pitch, s>>>(d);
+        g_launch_count.fetch_add(3, std::memory_order_relaxed);
+        for (uint32_t L = 0; L < L1; ++L) {
+            const uint64_t vecs = (uint64_t)a.g.lv[L].cnt * a.g.lv[L].nb / 4 + 1;
+            const uint32_t grid = (uint32_t)std::min<uint64_t>((vecs + 255) / 256, (uint64_t)sms * 8);
+            hnsw_delete_sweep_kernel<<<grid, 256, 0, s>>>(d, L);
+            hnsw_delete_relink_kernel<<<ordered ? 1 : 1024, 32, sc.row_pitch, s>>>(d, L, ordered);
+            g_launch_count.fetch_add(2, std::memory_order_relaxed);
+        }
+        rdone += rb;
+    }
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    std::vector<uint8_t> hf(ni), hs(ni);
+    if (e == cudaSuccess) e = cudaMemcpy(hf.data(), failed, ni, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(hs.data(), d.status, ni, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error(std::string("hnsw replica delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    for (uint32_t k = 0; k < ni; ++k)
+        if (hf[k] || hs[k]) out_status[item_pos[k]] = 2;
     return CDB_OK;
 }
 

@@ -234,6 +234,11 @@ bool hnsw_state_replica_info(const HnswBuildState *st, uint32_t *pseudo_root_row
 cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const ReplicaHost &rh,
                                        uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed,
                                        const int32_t **md_bits, const float **md_mags, bool *changed, cudaStream_t s);
+// cdb_index_delete_rows_replicas: every node of each of the distinct rows rows[0..n) (none a root row) deleted from the replica
+// graph of `st` with D1-D5 (DESIGN.md section 4); out_status[i] = 0, or 2 where an Err hit one of the row's nodes.  A row
+// without a node is left alone.  *changed as for hnsw_insert_device.
+cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
+                                       uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s);
 
 // ---- tensor_scan.cu (wgmma prefilter)
 constexpr uint32_t TS_MAX_ODD = 64;   // degenerate rows that are not all-zero ride on every candidate list; more -> no prefilter

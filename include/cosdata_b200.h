@@ -414,7 +414,8 @@ cdb_status cdb_index_insert_graph(cdb_index *index, const cdb_build_params *para
  * Locking, the order against enqueued searches and the failure contract are those of cdb_index_insert_graph: every
  * allocation comes before the graph changes, so an allocation failure leaves the graph, its metadata and its table as they
  * were; an error after the graph started changing drops the graph and its metadata, and cdb_last_error_string says so.
- * cdb_index_insert_graph, cdb_index_delete_rows and cdb_index_read_graph_slot_scores stay CDB_UNSUPPORTED on these graphs. */
+ * cdb_index_insert_graph, cdb_index_delete_rows and cdb_index_read_graph_slot_scores stay CDB_UNSUPPORTED on these graphs;
+ * they delete through cdb_index_delete_rows_replicas and read slot scores through cdb_index_read_replica_slot_scores. */
 typedef struct {
     uint32_t n_nodes;                           /* graph nodes to create, in insertion order */
     const uint32_t *row, *node_id, *base_id, *md_row;   /* as in cdb_replica_build */
@@ -457,6 +458,35 @@ cdb_status cdb_index_read_graph_slot_scores(cdb_index *index, uint32_t level, fl
  * repair has succeeded. */
 cdb_status cdb_index_delete_rows(cdb_index *index, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
                                  uint8_t *out_status, uint64_t *out_deleted);
+/* delete_embedding on a graph that cdb_index_build_graph_replicas built (and cdb_index_insert_graph_replicas may have grown).
+ * The unit is a vector row (one embedding): deleting row r deletes every graph node whose node_row is r -- its base replica
+ * and all of its Metadata replicas, on every level.  Arguments, out_status, *out_deleted, the marks and the deleted rows'
+ * treatment elsewhere are those of cdb_index_delete_rows; a status is per row (2 if an Err hit any of its nodes).  A row
+ * with no graph node (appended after the build, or never listed) is only marked; a row whose insert failed has isolated
+ * nodes and is traversed and marked like any other.  D1-D4 apply to each node R of the row, with
+ *   D5 replica rules.  R traverses as the graph sees it: R's vector row, R's Metadata row and Some(R's node_id) (that id only
+ *      decides the Pseudo kind, which a data row's replicas never have), from the pseudo root when its metadata has
+ *      mag != 0, else from the main root, nothing pre-inserted, ef 512, best 100 kept.  A base replica's traversal is the
+ *      reference's own (a Base-kind query from the main root).  An emptied neighbour N is relinked from R's results minus R,
+ *      N and every node of a row deleted in the batch, rescored with the replica arms (calculate(N, candidate), N's id and
+ *      metadata as x), sorted best first (ties: smaller id), then create_node_edges with the replica edge rules (cosine: a
+ *      Metadata N takes a Pseudo neighbour only at cs == 1.0, two Metadata nodes never link at cs == -1.0).  A rescoring Err,
+ *      CDB_UNREACHABLE_ARM included (a Pseudo N rescoring a Metadata candidate), stops that relink (D3).  Order: all nodes of
+ *      a batch traverse the graph as of the batch's start; per level, a row's nodes repair their own slots in list order;
+ *      then the D2 sweep over all of the batch's nodes, after which each touched node is relinked from the candidates of
+ *      the first deleted node (in list order) it named.  max_batch = 1 deletes one row at a time in list order
+ *      (deterministic); larger batches guarantee the invariants only.
+ * Refusals (nothing changes, no marks): a row out of range, the main root's or the pseudo root's row (pseudo replicas share
+ * it), shortlist_size outside 1..64, no graph or a graph without metadata (cdb_index_delete_rows): CDB_INVALID_PARAMS; a
+ * graph whose metadata came from cdb_index_set_graph_metadata / cdb_index_set_graph_from_files: CDB_UNSUPPORTED.  Locking,
+ * the order against enqueued searches and the failure contract are those of cdb_index_insert_graph_replicas: an error after
+ * the graph started changing drops the graph and its metadata. */
+cdb_status cdb_index_delete_rows_replicas(cdb_index *index, const uint32_t *rows, uint64_t n, uint32_t shortlist_size,
+                                          uint32_t max_batch, uint8_t *out_status, uint64_t *out_deleted);
+/* the slot similarities a replica build, insert or delete keeps for `level` (layout and values as in
+ * cdb_index_read_graph_slot_scores; on a Pseudo-Metadata edge both slots hold calculate(Metadata end, Pseudo end)).  A graph
+ * without metadata: CDB_INVALID_PARAMS; uploaded metadata: CDB_UNSUPPORTED. */
+cdb_status cdb_index_read_replica_slot_scores(cdb_index *index, uint32_t level, float *out_scores);
 /* out[i] = 1 if row first+i is deleted (first + n <= capacity); *out_total = deleted rows of the index (either pointer may be
  * NULL when unused) */
 cdb_status cdb_index_deleted_rows(const cdb_index *index, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total);

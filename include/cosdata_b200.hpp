@@ -206,6 +206,21 @@ class DenseIndex {
         check(cdb_index_read_graph_slot_scores(h_, level, out.data()));
         return out;
     }
+    // delete_embedding on a graph with metadata: every node of each row (its base and Metadata replicas); per-row status
+    std::vector<uint8_t> delete_rows_replicas(const std::vector<uint32_t> &rows, uint32_t shortlist_size = 64, uint32_t max_batch = 0) {
+        std::vector<uint8_t> status(std::max<size_t>(rows.size(), 1));
+        check(cdb_index_delete_rows_replicas(h_, rows.data(), rows.size(), shortlist_size, max_batch, status.data(), nullptr));
+        status.resize(rows.size());
+        return status;
+    }
+    // slot similarities of `level` of a graph that build_graph_replicas built
+    std::vector<float> read_replica_slot_scores(uint32_t level) {
+        uint32_t info[5], counts[32];
+        check(cdb_index_graph_info(h_, info, counts));
+        std::vector<float> out((size_t)counts[level] * (level == 0 ? info[2] : info[1]));
+        check(cdb_index_read_replica_slot_scores(h_, level, out.data()));
+        return out;
+    }
     // raw f32 rows for rows appended as codes (cold start of a quantized index)
     void set_raw(uint64_t first_row, const float *vecs, uint64_t n) { check(cdb_index_set_raw_f32(h_, first_row, vecs, n)); }
     uint64_t raw_missing() const { return cdb_index_raw_missing(h_); }
