@@ -108,7 +108,7 @@ class SearchParams(C.Structure):
         ("shortlist_size", C.c_uint32),
         ("exact_only", C.c_int32),
         ("prefilter_k", C.c_uint32),
-        ("reserved0", C.c_uint32),
+        ("flags", C.c_uint32),            # CDB_SEARCH_* bits
         ("reserved1", C.c_uint32),
     ]
 

@@ -22,6 +22,7 @@ from . import _lib
 from ._lib import BuildParams, GraphDesc, GraphMetadata, IndexDesc, SearchParams, VectorDataBatch
 
 INVALID_ID = 0xFFFFFFFF
+SEARCH_TENSOR_WITH_DELETED = 1      # cdb_search_params.flags bit CDB_SEARCH_TENSOR_WITH_DELETED
 
 
 class Status(enum.IntEnum):
@@ -423,8 +424,12 @@ class DenseIndex:
     def size(self):
         return int(self._lib.cdb_index_size(self._h))
 
-    def params(self, k, mode=SearchMode.BRUTE_RAW, ef_search=256, shortlist_size=64, exact_only=False, prefilter_k=0):
-        return SearchParams(k, int(mode), ef_search, shortlist_size, 1 if exact_only else 0, prefilter_k, 0, 0)
+    def params(self, k, mode=SearchMode.BRUTE_RAW, ef_search=256, shortlist_size=64, exact_only=False, prefilter_k=0,
+               tensor_with_deleted=False):
+        """tensor_with_deleted: brute-force searches may take the tensor-core paths while rows are deleted (the kernels skip
+        them; results are identical, CDB_SEARCH_TENSOR_WITH_DELETED)"""
+        flags = SEARCH_TENSOR_WITH_DELETED if tensor_with_deleted else 0
+        return SearchParams(k, int(mode), ef_search, shortlist_size, 1 if exact_only else 0, prefilter_k, flags, 0)
 
     def batch_search(self, queries, k, mode=SearchMode.BRUTE_RAW, **kw):
         """IndexOps::batch_search -> (ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B])"""
@@ -488,10 +493,11 @@ class DenseIndex:
         return {n: int(v) for n, v in zip(names, out)}
 
     def stats(self):
-        out = np.zeros(7, dtype=np.uint64)
-        _check(self._lib.cdb_index_stats_ex(self._h, _ptr(out), 7))
+        out = np.zeros(8, dtype=np.uint64)
+        _check(self._lib.cdb_index_stats_ex(self._h, _ptr(out), 8))
         return {"tensor_searches": int(out[0]), "fallbacks": int(out[1]), "zero_rows": int(out[2]), "odd_rows": int(out[3]),
-                "has_shadow": bool(out[4]), "fallback_queries": int(out[5]), "s8_searches": int(out[6])}
+                "has_shadow": bool(out[4]), "fallback_queries": int(out[5]), "s8_searches": int(out[6]),
+                "tensor_deleted_searches": int(out[7])}
 
     def last_candidate_counts(self, n):
         out = np.zeros(n, dtype=np.uint32)

@@ -1,6 +1,7 @@
 // api.cu -- the extern "C" boundary declared in include/cosdata_b200.h.
 // Host-side orchestration only: device buffers, streams, launch order.  No torch,
 // no CPU compute path -- without a CUDA device every entry point fails.
+#include <algorithm>
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
@@ -169,6 +170,7 @@ struct cdb_index {
     uint32_t *h_flags = nullptr;   // pinned host staging (16 words)
     std::atomic<uint64_t> stat_tensor_searches{0};
     std::atomic<uint64_t> stat_s8_searches{0};   // of those, answered by the s8 form
+    std::atomic<uint64_t> stat_tensor_deleted_searches{0};   // of those, run while the shard had deleted rows
     cudaStream_t stream = nullptr; // ingest / build stream (exclusive operations)
     static constexpr int EV_RING = 64;
     cudaEvent_t ring0[EV_RING] = {}, ring1[EV_RING] = {};  // per-search (before scan, after scan)
@@ -548,16 +550,18 @@ static cdb_status index_after_append(cdb_index *ix, uint64_t first, uint64_t n) 
                                    ix->d_digits + first * ix->digit_pitch, ix->digit_pitch, ix->stream)))
         return rc;
     if (ix->d_xh) {
-        if ((rc = normalize_f16_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, n,
-                                       ix->desc.dim, (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->stream)))
+        if ((rc = normalize_f16_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, first,
+                                       n, ix->desc.dim, (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->del_dev(),
+                                       ix->stream)))
             return rc;
         // deg[0], deg[1] accumulate the all-zero / other degenerate rows, deg[2..] lists the first of the latter
         if ((rc = classify_rows_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, n,
                                        ix->desc.dim, (uint32_t)first, ix->deg.as<uint32_t>(), ix->stream)))
             return rc;
-        // s8 shadow: every tile the range touches, the open tile's earlier rows included (its scale can change)
+        // s8 shadow: every tile the range touches, the open tile's earlier rows included (its scale can change; deleted rows
+        // among them keep zero codes)
         if ((rc = quantize_s8_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, first, n, first + n, ix->desc.dim, ix->d_xs8,
-                                     ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->stream)))
+                                     ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->del_dev(), ix->stream)))
             return rc;
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 4, ix->deg.p, 8, cudaMemcpyDeviceToHost, ix->stream));
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
@@ -658,14 +662,14 @@ cdb_status cdb_index_set_raw_f32(cdb_index *ix, uint64_t first_row, const float 
             (rc = raw_mags_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, m, dim, ix->d_raw_mags + first, ix->stream)))
             return rc;
         if (ix->d_xh &&
-            (rc = normalize_f16_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, m, dim,
-                                       (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->stream)))
+            (rc = normalize_f16_device(ix->d_raw + first * ix->raw_pitch_elems, ix->raw_pitch_elems, ix->d_raw_mags + first, first, m,
+                                       dim, (uint8_t *)ix->d_xh + first * ix->xh_pitch * 2, ix->xh_pitch, ix->del_dev(), ix->stream)))
             return rc;
         CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
     }
     if (ix->d_xs8) {
         cdb_status rc = quantize_s8_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, first_row, n, ix->size, dim, ix->d_xs8,
-                                           ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->stream);
+                                           ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->del_dev(), ix->stream);
         if (rc) return rc;
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
         CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
@@ -923,10 +927,13 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
     // Needs k proper (non-degenerate) rows for the bound to exist, and few enough odd degenerate rows to carry them on
     // every candidate list (tensor_scan.cu).
     // The exact re-rank holds the query in shared memory, which bounds the dimension.
-    // The tensor-core paths know nothing of deleted rows: once a row is deleted the exact scan answers.
-    const bool tensor_ok = raw && ix->d_xh && !p->exact_only && ix->n_deleted == 0 && nq >= 4 && ix->size >= 16384 && p->k <= 64 &&
-                           d.dim <= rerank_f32_max_dim() &&
-                           ix->n_odd_rows <= TS_MAX_ODD && ix->size - ix->n_allzero_rows - ix->n_odd_rows >= p->k &&
+    // Deleted rows: without CDB_SEARCH_TENSOR_WITH_DELETED the exact scan answers.  With it, a deleted row has a zero shadow
+    // row (it stays out of the bound like a degenerate row) and the re-rank drops it; the k proper rows must be live ones
+    // (a deleted degenerate row is subtracted twice: conservative).
+    const bool del_ok = ix->n_deleted == 0 || (p->flags & CDB_SEARCH_TENSOR_WITH_DELETED);
+    const bool tensor_ok = raw && ix->d_xh && !p->exact_only && del_ok && nq >= 4 && ix->size >= 16384 && p->k <= 64 &&
+                           d.dim <= rerank_f32_max_dim() && ix->n_odd_rows <= TS_MAX_ODD &&
+                           ix->size - ix->n_allzero_rows - ix->n_odd_rows >= p->k + ix->n_deleted &&
                            tensor_scan_smem_bytes(p->k) <= 227 * 1024 && (nq + 127) / 128 <= (uint32_t)ix->sm_count;
     // search_internal: quantize the query with the index's storage type and range (hnsw/mod.rs:399-403);
     // raw mode keeps f32 and |q| = sequential fold (vector_store.rs:412)
@@ -951,7 +958,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
             (rc = sc->progress.ensure(8192)) || (rc = sc->qsel.ensure((size_t)(nq + 1) * 4)) || (rc = sc->err32.ensure((size_t)nq * 4)))
             return rc;
         uint32_t *flags = sc->flags.as<uint32_t>();  // [0] queries of the last search that needed the exact scan, [3] searches with a fallback
-        const bool has_deg = ix->n_allzero_rows + ix->n_odd_rows > 0;
+        const bool has_deg = ix->n_allzero_rows + ix->n_odd_rows + ix->n_deleted > 0;
         const bool s8 = use_s8_form(ix, nq);
         if (s8 && (rc = sc->qse.ensure((size_t)nq * 8))) return rc;
         if ((rc = prep_queries_device(d_queries, nq, d.dim, sc->q_codes.as<float>(), pitch / 4, sc->q_mags.as<float>(), sc->qh.p,
@@ -975,11 +982,12 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
         if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->q_codes.as<float>(),
                                     pitch / 4, sc->q_mags.as<float>(), nq, sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(),
-                                    cap, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr, sc->cur_keys)))
+                                    cap, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr, sc->cur_keys, ix->del_dev())))
             return rc;
         if ((rc = select_fallback_device(sc->cand_cnt.as<uint32_t>(), cap, sc->q_mags.as<float>(), nq, sc->qsel.as<uint32_t>(), flags, s)))
             return rc;
         ix->stat_tensor_searches++;
+        if (ix->n_deleted) ix->stat_tensor_deleted_searches++;
         qsel = sc->qsel.as<uint32_t>();  // the exact scan below only runs (on the device's own decision) for the queries listed there
     }
     // ---- exact integer scoring on wgmma u8: u8 codes in place, sub-byte codes through the digit copy
@@ -987,7 +995,8 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
     // exact only while that bound is a finite float bit pattern (u8 codes: D <= 32896); above it the exact scan answers.
     const uint8_t *u8_rows = !raw ? (st == CDB_ST_U8 ? ix->d_codes : ix->d_digits) : nullptr;
     const uint64_t max_digit = st == CDB_ST_U8 ? 255u : (1u << st) - 1u;
-    const bool u8_ok = u8_rows && !p->exact_only && ix->n_deleted == 0 && (metric == CDB_METRIC_COSINE || metric == CDB_METRIC_DOT_PRODUCT) &&
+    // (deleted rows: the kernel masks them out of every tile that holds one, see tensor_scan.cu)
+    const bool u8_ok = u8_rows && !p->exact_only && del_ok && (metric == CDB_METRIC_COSINE || metric == CDB_METRIC_DOT_PRODUCT) &&
                        max_digit * max_digit * d.dim <= 0x7F7FFFFFull &&
                        ix->size >= 16384 && p->k <= 64 && tensor_u8_smem_bytes(p->k) <= 227 * 1024 &&
                        (nq + 127) / 128 <= (uint32_t)ix->sm_count;
@@ -1011,7 +1020,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         if ((rc = tensor_u8_scan_device(u8_rows, sc->qh.as<uint8_t>(), upitch, ix->size, nq, d.dim, p->k, metric, ix->d_mags,
                                         sc->q_mags.as<float>(), d.id_base, sc->gthr.as<int>(), sc->cand.as<uint64_t>(),
                                         sc->cand_cnt.as<uint32_t>(), cap, sc->err32.as<uint32_t>(), sc->progress.as<uint32_t>(),
-                                        d_ids, d_scores, d_counts, ix->sm_count, s, sc->cur_keys)))
+                                        d_ids, d_scores, d_counts, ix->del_dev(), ix->sm_count, s, sc->cur_keys)))
             return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
         if ((rc = select_fallback_device(sc->cand_cnt.as<uint32_t>(), cap, nullptr, nq, sc->qsel.as<uint32_t>(), flags, s))) return rc;
@@ -1020,6 +1029,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
             CDB_LAUNCH_CHECK();
         }
         ix->stat_tensor_searches++;
+        if (ix->n_deleted) ix->stat_tensor_deleted_searches++;
         qsel = sc->qsel.as<uint32_t>();
     }
     {
@@ -1673,6 +1683,30 @@ cdb_status cdb_index_insert_graph_replicas(cdb_index *ix, const cdb_build_params
     return CDB_OK;
 }
 
+// the prefilter shadows of newly deleted rows (marks already on the device): fp16 rows := 0, and the s8 tiles holding them
+// re-quantized without them, so that they score exactly 0 and stay out of the class-maximum bound (tensor_scan.cu)
+static cdb_status drop_from_shadows(cdb_index *ix, const std::vector<uint32_t> &rows) {
+    if (!ix->d_xh || rows.empty()) return CDB_OK;
+    std::vector<uint32_t> list(rows);
+    const size_t n_rows = list.size();
+    for (size_t i = 0; i < n_rows; ++i) list.push_back(rows[i] / 256);   // corpus tiles of 256 rows
+    std::sort(list.begin() + n_rows, list.end());
+    list.erase(std::unique(list.begin() + n_rows, list.end()), list.end());
+    const size_t n_tiles = list.size() - n_rows;
+    cdb_status rc;
+    if ((rc = ix->stage.ensure(list.size() * 4))) return rc;
+    CDB_CUDA_TRY(cudaMemcpyAsync(ix->stage.p, list.data(), list.size() * 4, cudaMemcpyHostToDevice, ix->stream));
+    const uint32_t *d_list = ix->stage.as<uint32_t>();
+    if ((rc = shadow_drop_rows_device(d_list, (uint32_t)n_rows, d_list + n_rows, (uint32_t)n_tiles, ix->d_xh, ix->xh_pitch, ix->d_raw,
+                                      ix->raw_pitch_elems, ix->d_raw_mags, ix->size, ix->desc.dim, ix->d_xs8, ix->xs8_pitch, ix->d_s8se,
+                                      ix->d_xs8 ? &ix->d_s8se[ix->s8_tiles].x : nullptr, ix->d_deleted, ix->stream)))
+        return rc;
+    if (ix->d_xs8) CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
+    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    if (ix->d_xs8) std::memcpy(&ix->s8_emax, ix->h_flags + 6, 4);
+    return CDB_OK;
+}
+
 cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
                                  uint8_t *out_status, uint64_t *out_deleted) {
     CDB_REQUIRE(ix && (rows || !n), "null argument");
@@ -1740,6 +1774,7 @@ cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n
         }
         CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted + lo, ix->h_deleted.data() + lo, (size_t)(hi - lo + 1) * 4, cudaMemcpyHostToDevice));
         ix->n_deleted += fresh.size();
+        if ((rc = drop_from_shadows(ix, fresh))) return rc;
         size_t j = 0;
         for (uint64_t i = 0; i < n; ++i)
             if (status[i] == 0) status[i] = fst[j++];
@@ -1822,6 +1857,7 @@ cdb_status cdb_index_delete_rows_replicas(cdb_index *ix, const uint32_t *rows, u
         }
         CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted + lo, ix->h_deleted.data() + lo, (size_t)(hi - lo + 1) * 4, cudaMemcpyHostToDevice));
         ix->n_deleted += fresh.size();
+        if ((rc = drop_from_shadows(ix, fresh))) return rc;
         size_t j = 0;
         for (uint64_t i = 0; i < n; ++i)
             if (status[i] == 0) status[i] = fst[j++];
@@ -1944,7 +1980,8 @@ cdb_status cdb_index_stats_ex(const cdb_index *ix, uint64_t *out, uint32_t n) {
     cdb_status rc = read_pool_flags(ix, &fb, &lq);
     if (rc) return rc;
     const uint64_t v[CDB_STATS_FIELDS] = {ix->stat_tensor_searches.load(), fb, ix->n_allzero_rows, ix->n_odd_rows,
-                                          ix->d_xh ? 1ull : 0ull, lq, ix->stat_s8_searches.load()};
+                                          ix->d_xh ? 1ull : 0ull, lq, ix->stat_s8_searches.load(),
+                                          ix->stat_tensor_deleted_searches.load()};
     for (uint32_t i = 0; i < n && i < CDB_STATS_FIELDS; ++i) out[i] = v[i];
     return CDB_OK;
 }

@@ -47,7 +47,8 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
                              const uint32_t *d_cand, const uint32_t *d_cand_counts, uint32_t ncand, uint32_t k, uint32_t id_base,
                              uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s,
                              const uint32_t *d_labels = nullptr,    // labels: ids reported instead of the candidate ids (replica ids)
-                             uint64_t *d_out_keys = nullptr);       // [nq][k] packed selection keys as well (shard merge)
+                             uint64_t *d_out_keys = nullptr,        // [nq][k] packed selection keys as well (shard merge)
+                             const uint32_t *d_deleted = nullptr);  // deleted-row bitmap: such candidates are dropped
 // largest dimension rerank_f32_device accepts for any candidate count (its query and key buffer share 200 KB of smem)
 uint32_t rerank_f32_max_dim();
 
@@ -243,8 +244,15 @@ cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh
 // ---- tensor_scan.cu (wgmma prefilter)
 constexpr uint32_t TS_MAX_ODD = 64;   // degenerate rows that are not all-zero ride on every candidate list; more -> no prefilter
 constexpr uint32_t TS_DEG_WORDS = 2 + TS_MAX_ODD;
-cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t n, uint32_t dim,
-                                void *d_out, uint32_t out_pitch_halfs, cudaStream_t s);
+// rows [first, first + n): d_raw / d_mags / d_out point at row `first`; rows set in d_deleted (may be null) get zero rows
+cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
+                                uint32_t dim, void *d_out, uint32_t out_pitch_halfs, const uint32_t *d_deleted, cudaStream_t s);
+// deleted rows: fp16 shadow rows d_rows[0..n_rows) := 0; the s8 shadow tiles d_tiles[0..n_tiles) re-quantized without the rows
+// set in d_deleted (d_xs8 may be null: no s8 shadow), then *d_emax refreshed
+cdb_status shadow_drop_rows_device(const uint32_t *d_rows, uint32_t n_rows, const uint32_t *d_tiles, uint32_t n_tiles, void *d_xh,
+                                   uint32_t xh_pitch_halfs, const float *d_raw, uint32_t pitch_elems, const float *d_mags,
+                                   uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
+                                   const uint32_t *d_deleted, cudaStream_t s);
 cdb_status classify_rows_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t n, uint32_t dim,
                                 uint32_t first_row, uint32_t *d_deg, cudaStream_t s);
 size_t tensor_scan_smem_bytes(uint32_t k);
@@ -258,10 +266,10 @@ cdb_status prep_queries_device(const float *d_q, uint32_t nq, uint32_t dim, floa
                                uint32_t *d_cand, uint32_t cand_cap, uint32_t *d_cand_cnt, uint32_t *d_err32, uint8_t *d_err8,
                                uint32_t *d_progress, float2 *d_q_se, cudaStream_t s);
 // s8 form of the prefilter (DESIGN.md section 5c): shadow of the tiles touching rows [first, first + n) of rows < row_end,
-// then *d_emax = max E_T over all tiles below row_end
+// then *d_emax = max E_T over all tiles below row_end; rows set in d_deleted (may be null) are treated as degenerate
 cdb_status quantize_s8_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
                               uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
-                              cudaStream_t s);
+                              const uint32_t *d_deleted, cudaStream_t s);
 cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t pitch8, uint64_t n_rows, uint32_t nq, uint32_t dim,
                                  uint32_t k, const float2 *d_tile_se, const float2 *d_q_se, uint32_t id_base, int *d_ggm,
                                  uint32_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_progress, bool has_deg,
@@ -269,7 +277,7 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
 cdb_status tensor_scan_i8_device(const uint8_t *d_x, const uint8_t *d_q, uint32_t pitch, uint64_t n_rows, uint32_t nq, uint32_t dim,
                                  uint32_t k, int metric, const float *d_mags, const float *d_qmags, uint32_t id_base, int *d_ggm,
                                  uint64_t *d_cand64, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_err32,
-                                 uint32_t *d_progress /* 2048 words */, int sm_count, cudaStream_t s);
+                                 uint32_t *d_progress /* 2048 words */, const uint32_t *d_deleted, int sm_count, cudaStream_t s);
 // queries whose candidate list overflowed (or whose norm is degenerate, d_qmags may be null) -> d_qsel = {n, indices...}
 cdb_status select_fallback_device(const uint32_t *d_cnt, uint32_t cap, const float *d_qmags, uint32_t n, uint32_t *d_qsel,
                                   uint32_t *d_flags, cudaStream_t s);
@@ -281,7 +289,7 @@ cdb_status unpack_digits_device(const uint8_t *d_codes, uint32_t row_pitch, uint
 cdb_status tensor_u8_scan_device(const uint8_t *d_x, const uint8_t *d_q, uint32_t pitch, uint64_t n_rows, uint32_t nq, uint32_t dim,
                                  uint32_t k, int metric, const float *d_mags, const float *d_qmags, uint32_t id_base, int *d_gthr,
                                  uint64_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_err32, uint32_t *d_progress,
-                                 uint32_t *d_ids, float *d_scores, uint32_t *d_counts, int sm_count, cudaStream_t s,
-                                 uint64_t *d_out_keys = nullptr);
+                                 uint32_t *d_ids, float *d_scores, uint32_t *d_counts, const uint32_t *d_deleted, int sm_count,
+                                 cudaStream_t s, uint64_t *d_out_keys = nullptr);
 
 }  // namespace cdb

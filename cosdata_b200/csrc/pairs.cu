@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(RERANK_THREADS) rerank_f32_kernel(
     uint32_t dim, const float *__restrict__ q, uint32_t q_pitch_elems, const float *__restrict__ qmags,
     const uint32_t *__restrict__ cand, const uint32_t *__restrict__ cand_counts, uint32_t cand_stride, uint32_t k, uint32_t id_base,
     uint32_t *__restrict__ out_ids, float *__restrict__ out_scores, uint32_t *__restrict__ out_counts,
-    const uint32_t *__restrict__ labels, uint64_t *__restrict__ out_keys) {
+    const uint32_t *__restrict__ labels, uint64_t *__restrict__ out_keys, const uint32_t *__restrict__ deleted) {
     extern __shared__ __align__(16) uint8_t smem[];
     float *qs = reinterpret_cast<float *>(smem);
     uint64_t *keys = reinterpret_cast<uint64_t *>(qs + round_up(dim, 4));
@@ -141,7 +141,9 @@ __global__ void __launch_bounds__(RERANK_THREADS) rerank_f32_kernel(
         for (uint32_t r = 0; r < rounds; ++r) {
             const uint32_t ci = r * (RERANK_THREADS / 8) + grp;   // within this chunk
             uint32_t id = ci < take ? cand[(size_t)b * cand_stride + pos + ci] : CDB_INVALID_ID;
-            const bool ok = id != CDB_INVALID_ID && id >= id_base && (uint64_t)(id - id_base) < n_rows;
+            // deleted rows reach the list through a zero shadow row emitted at a threshold <= 0, or as pre-seeded odd rows
+            bool ok = id != CDB_INVALID_ID && id >= id_base && (uint64_t)(id - id_base) < n_rows;
+            if (ok && deleted) ok = !((deleted[(id - id_base) >> 5] >> ((id - id_base) & 31)) & 1u);
             const uint64_t rowi = ok ? (uint64_t)(id - id_base) : 0;
             float dp = dot_f32_avx_order_8t(qs, raw + rowi * pitch_elems, dim, j);  // all lanes participate in the shuffles
             if (j == 0 && ci < take) {
@@ -193,7 +195,7 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
                              uint32_t dim, const float *d_q, uint32_t q_pitch_elems, const float *d_qmags, uint32_t nq,
                              const uint32_t *d_cand, const uint32_t *d_cand_counts, uint32_t ncand, uint32_t k, uint32_t id_base,
                              uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s,
-                             const uint32_t *d_labels, uint64_t *d_out_keys) {
+                             const uint32_t *d_labels, uint64_t *d_out_keys, const uint32_t *d_deleted) {
     if (!nq) return CDB_OK;
     if (k == 0 || k > 1024) { set_error("rerank: k must be in 1..1024"); return CDB_INVALID_PARAMS; }
     uint32_t pcap = 64;
@@ -203,7 +205,8 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
     if (smem > 200 * 1024) { set_error("rerank: dimension too large"); return CDB_INVALID_PARAMS; }
     CDB_ALLOW_SMEM(rerank_f32_kernel, smem);
     rerank_f32_kernel<<<nq, RERANK_THREADS, smem, s>>>(d_raw, pitch_elems, d_raw_mags, n_rows, dim, d_q, q_pitch_elems,
-                                                        d_qmags, d_cand, d_cand_counts, ncand, k, id_base, d_out_ids, d_out_scores, d_out_counts, d_labels, d_out_keys);
+                                                        d_qmags, d_cand, d_cand_counts, ncand, k, id_base, d_out_ids, d_out_scores, d_out_counts, d_labels, d_out_keys,
+                                                        d_deleted);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }

@@ -63,6 +63,7 @@ struct TensorScanArgs {
     uint64_t *cand64;       // [n_queries][cand_cap] emitted selection keys (exact scores)
     uint32_t *err32;        // [n_queries] error bits
     float rel;              // threshold = bound * rel - two_eps (1 for the f16 form and for the dot product; 1 - 2^-18 for cosine)
+    const uint32_t *deleted;   // deleted-row bitmap (bit r = row r), null while no row is deleted: a corpus tile is 8 words
     // ---- s8 form (KIND 2: the prefilter on wgmma .s32.s8.s8 against the s8 shadow, DESIGN.md section 5c)
     const float2 *tile_se;  // [ntiles] {s_T, E_T} of each corpus tile
     const float2 *q_se;     // [n_queries] {s_q, e_q}
@@ -76,6 +77,9 @@ constexpr uint32_t TS_STAGE_SLOT_BYTES = 40;
 constexpr uint32_t TS_LSTAGE = 9;
 constexpr uint32_t TS_KSTAGE = 4;
 constexpr int TS_GROUPS = 64;       // at most 64 class maxima per query; the filter supports k <= TS_GROUPS
+
+// bit r of a row bitmap (null: no bit is set)
+__device__ __forceinline__ bool bit_is_set(const uint32_t *bits, uint64_t r) { return bits && ((bits[r >> 5] >> (r & 31)) & 1u); }
 
 // rare path: one approximate score passed the threshold -> stage the row id, flush TS_LSTAGE at a time
 __device__ __noinline__ void epi_emit(const TensorScanArgs &a, uint32_t qi, uint32_t *stage, uint32_t id) {
@@ -108,6 +112,21 @@ __device__ __noinline__ void epi_emit_key(const TensorScanArgs &a, uint32_t qi, 
         c = 0;
     }
     stage[0] = c;
+}
+
+// word x (0..7) of the deleted-row bitmap over the corpus tile starting at row0 (rows past the corpus: 0)
+__device__ __forceinline__ uint32_t tile_word(const TensorScanArgs &a, uint64_t row0, int x) {
+    return row0 + 32 * x < a.n_rows ? __ldg(a.deleted + (row0 >> 5) + x) : 0u;
+}
+// the deleted bits of a consumer thread's 64 columns 8j + 2qd + b, as bit 2j + b
+__device__ __forceinline__ uint64_t tile_dead(const TensorScanArgs &a, uint64_t row0, uint32_t qd) {
+    uint64_t dead = 0;
+#pragma unroll
+    for (int x = 0; x < 8; ++x) {
+        const uint32_t sw = tile_word(a, row0, x) >> (2 * qd);   // bits 8m + {0,1}: columns 32x + 8m + 2qd + {0,1}
+        dead |= (uint64_t)((sw & 0x3u) | ((sw >> 6) & 0xCu) | ((sw >> 12) & 0x30u) | ((sw >> 18) & 0xC0u)) << (8 * x);
+    }
+    return dead;
 }
 
 // bitonic sort of NG register values, descending (fully unrolled: all indices are compile-time)
@@ -283,7 +302,8 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                 const bool valid = row0 + ct < a.n_rows;
                 const float mg = valid ? a.mags[row0 + ct] : 0.0f;
                 rinv_s[(t & 1) * TS_BLOCK_N + ct] = mg > 0.0f ? __frcp_rn(mg) : 0.0f;
-                if (valid && mg == 0.0f) zflag_s[t & 1] = 1u;
+                // a deleted row raises no Err (as in the exact scan)
+                if (valid && mg == 0.0f && !bit_is_set(a.deleted, row0 + ct)) zflag_s[t & 1] = 1u;
                 asm volatile("bar.sync 1, 256;" ::: "memory");
                 if (zflag_s[t & 1]) {
 #pragma unroll
@@ -318,6 +338,16 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 
             // ---- epilogue: fold the values into the class maxima, test the tile maximum against the threshold,
             //      build the per-value tests only on a hit
+            // KIND 1 (its operands are the stored codes, so deleted rows cannot be zeroed like the shadows of KIND 0 / 2):
+            // every thread reads the tile's 8 bitmap words, so `dirty` is uniform; a dirty tile takes the masked epilogue
+            bool dirty = false;
+            if constexpr (KIND == 1) {
+                if (a.deleted) {
+#pragma unroll
+                    for (int x = 0; x < 8; ++x) dirty |= tile_word(a, row0, x) != 0u;
+                }
+            }
+            const uint64_t dead = dirty ? tile_dead(a, row0, qd) : 0ull;   // bit 2j+b: column 8j + 2qd + b is a deleted row
             const bool full_tile = row0 + TS_BLOCK_N <= a.n_rows;   // only the corpus' last tile can be partial (TMA zero fill)
             const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;   // valid columns of this tile
             if constexpr (KIND == 2) {
@@ -386,7 +416,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 bool hit;
-                if (full_tile) {
+                if (full_tile && !dirty) {
                     float cm[NL];
 #pragma unroll
                     for (int l = 0; l < NL; ++l) cm[l] = -INFINITY;
@@ -409,7 +439,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 #pragma unroll
                     for (int l = 0; l < NL; ++l) { cmax = fmaxf(cmax, cm[l]); gm[i][l] = fmaxf(gm[i][l], cm[l]); }
                     hit = cmax >= thr[i];
-                } else {
+                } else {   // the corpus' partial last tile, or (KIND 1) a tile with deleted rows: they stay out of the bound
 #pragma unroll
                     for (int j = 0; j < 32; ++j) {
 #pragma unroll
@@ -417,7 +447,8 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                             const uint32_t col = 8 * j + 2 * qd + b;
                             const float v = acc_value<KIND>(acc[4 * j + 2 * i + b], cosine, cosine ? rs[col] : 0.0f);
                             const int l = (j & (NG / 8 - 1)) * 2 + b;
-                            if ((uint64_t)col < left && !(HAS_DEG && v == 0.0f)) gm[i][l] = fmaxf(gm[i][l], v);
+                            if ((uint64_t)col < left && !(HAS_DEG && v == 0.0f) && !((dead >> (2 * j + b)) & 1u))
+                                gm[i][l] = fmaxf(gm[i][l], v);
                         }
                     }
                     hit = true;
@@ -429,7 +460,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                         for (int b = 0; b < 2; ++b) {
                             const uint32_t col = 8 * j + 2 * qd + b;
                             const float v = acc_value<KIND>(acc[4 * j + 2 * i + b], cosine, cosine ? rs[col] : 0.0f);
-                            if ((uint64_t)col < left && v >= thr[i]) {
+                            if ((uint64_t)col < left && !((dead >> (2 * j + b)) & 1u) && v >= thr[i]) {
                                 if (KIND == 1) epi_emit_key(a, qi[i], kstage[i], (int)acc_bits(acc[4 * j + 2 * i + b]), row0 + col, qmag[i]);
                                 else epi_emit(a, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
                             }
@@ -483,29 +514,33 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 // ------------------------------------------------------------------ fp16 normalised copies
 // x_hat = x / |x| (IEEE), rounded to fp16.  Rows whose norm is outside [1e-15, 1e15] (zero, underflowed, overflowed,
 // inf/NaN) are DEGENERATE: the error bound of the prefilter does not cover them, their shadow row is all zero.
+// Deleted rows get an all-zero shadow row as well: like a degenerate row they then stay out of the class maxima (HAS_DEG),
+// and the re-rank drops them if they are emitted.
 __host__ __device__ inline bool norm_is_proper(float m) { return m >= 1.0e-15f && m <= 1.0e15f; }
 
+// rows [first, first + n); raw / mags / out point at row `first`, `deleted` (may be null) is indexed by absolute row
 __global__ void normalize_f16_kernel(const float *__restrict__ raw, uint32_t pitch_elems, const float *__restrict__ mags,
-                                     uint64_t n, uint32_t dim, __half *__restrict__ out, uint32_t out_pitch) {
+                                     uint64_t first, uint64_t n, uint32_t dim, __half *__restrict__ out, uint32_t out_pitch,
+                                     const uint32_t *__restrict__ deleted) {
     const uint32_t groups = (dim + 7) / 8;
     uint64_t gid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= n * groups) return;
     uint64_t row = gid / groups;
     uint32_t c0 = (uint32_t)(gid % groups) * 8;
     const float m = mags[row];
-    const bool ok = norm_is_proper(m);
+    const bool ok = norm_is_proper(m) && !bit_is_set(deleted, first + row);
     for (uint32_t e = 0; e < 8 && c0 + e < dim; ++e) {
         float v = raw[row * pitch_elems + c0 + e];
         out[row * out_pitch + c0 + e] = __float2half_rn(ok ? __fdiv_rn(v, m) : 0.0f);
     }
 }
 
-cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t n, uint32_t dim,
-                                void *d_out, uint32_t out_pitch_halfs, cudaStream_t s) {
+cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
+                                uint32_t dim, void *d_out, uint32_t out_pitch_halfs, const uint32_t *d_deleted, cudaStream_t s) {
     if (!n) return CDB_OK;
     uint64_t total = n * ((dim + 7) / 8);
-    normalize_f16_kernel<<<(uint32_t)((total + 255) / 256), 256, 0, s>>>(d_raw, pitch_elems, d_mags, n, dim,
-                                                                          reinterpret_cast<__half *>(d_out), out_pitch_halfs);
+    normalize_f16_kernel<<<(uint32_t)((total + 255) / 256), 256, 0, s>>>(d_raw, pitch_elems, d_mags, first, n, dim,
+                                                                          reinterpret_cast<__half *>(d_out), out_pitch_halfs, d_deleted);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }
@@ -530,20 +565,21 @@ __device__ __forceinline__ float residual_norm_up(double e2) {
 
 // One CTA (8 warps, a warp per row) per corpus tile t = tile0 + blockIdx.x, rows [256t, min(256t + 256, row_end)):
 // x_hat = x / |x| exactly as normalize_f16_kernel computes it, s_T = max |x_hat_i| / 127 over the tile's proper rows,
-// codes rint(x_hat / s_T), E_T >= max over proper rows of |x_hat - s_T * codes| (f64, rounded up).  Degenerate rows get
-// zero codes and no say in s_T or E_T.
+// codes rint(x_hat / s_T), E_T >= max over proper rows of |x_hat - s_T * codes| (f64, rounded up).  Degenerate and
+// deleted rows get zero codes and no say in s_T or E_T.  tiles (may be null): the CTA's tile is tiles[blockIdx.x].
 __global__ void __launch_bounds__(256) quantize_s8_tiles_kernel(const float *__restrict__ raw, uint32_t pitch_elems,
                                                                 const float *__restrict__ mags, uint32_t tile0, uint64_t row_end,
                                                                 uint32_t dim, int8_t *__restrict__ xs8, uint32_t pitch8,
-                                                                float2 *__restrict__ tile_se) {
+                                                                float2 *__restrict__ tile_se, const uint32_t *__restrict__ tiles,
+                                                                const uint32_t *__restrict__ deleted) {
     __shared__ float s_max[8];
     __shared__ double s_e2[8];
-    const uint32_t t = tile0 + blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t t = tiles ? tiles[blockIdx.x] : tile0 + blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint64_t r0 = (uint64_t)t * TS_BLOCK_N, r1 = min(r0 + TS_BLOCK_N, row_end);
     float mx = 0.0f;
     for (uint64_t r = r0 + warp; r < r1; r += 8) {
         const float m = mags[r];
-        if (!norm_is_proper(m)) continue;
+        if (!norm_is_proper(m) || bit_is_set(deleted, r)) continue;
         for (uint32_t c = lane; c < dim; c += 32) mx = fmaxf(mx, fabsf(__fdiv_rn(raw[r * pitch_elems + c], m)));
     }
     mx = warp_max_f(mx);
@@ -555,7 +591,7 @@ __global__ void __launch_bounds__(256) quantize_s8_tiles_kernel(const float *__r
     double e2 = 0.0;
     for (uint64_t r = r0 + warp; r < r1; r += 8) {
         const float m = mags[r];
-        const bool ok = norm_is_proper(m);
+        const bool ok = norm_is_proper(m) && !bit_is_set(deleted, r);
         double rr = 0.0;
         for (uint32_t c = lane; c < dim; c += 32) {
             const float v = ok ? __fdiv_rn(raw[r * pitch_elems + c], m) : 0.0f;
@@ -590,14 +626,38 @@ __global__ void __launch_bounds__(1024) s8_emax_kernel(const float2 *__restrict_
 
 cdb_status quantize_s8_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
                               uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
-                              cudaStream_t s) {
+                              const uint32_t *d_deleted, cudaStream_t s) {
     if (!n) return CDB_OK;
     const uint32_t t0 = (uint32_t)(first / TS_BLOCK_N), t1 = (uint32_t)((first + n + TS_BLOCK_N - 1) / TS_BLOCK_N);
     quantize_s8_tiles_kernel<<<t1 - t0, 256, 0, s>>>(d_raw, pitch_elems, d_mags, t0, row_end, dim,
-                                                     reinterpret_cast<int8_t *>(d_xs8), pitch8, d_tile_se);
+                                                     reinterpret_cast<int8_t *>(d_xs8), pitch8, d_tile_se, nullptr, d_deleted);
     CDB_LAUNCH_CHECK();
     s8_emax_kernel<<<1, 1024, 0, s>>>(d_tile_se, (uint32_t)((row_end + TS_BLOCK_N - 1) / TS_BLOCK_N), d_emax);
     CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
+// one CTA per listed row: the row's bytes := 0
+__global__ void zero_rows_kernel(const uint32_t *__restrict__ rows, uint8_t *base, uint32_t pitch_bytes) {
+    uint8_t *p = base + (size_t)rows[blockIdx.x] * pitch_bytes;
+    for (uint32_t c = threadIdx.x; c < pitch_bytes; c += blockDim.x) p[c] = 0;
+}
+
+cdb_status shadow_drop_rows_device(const uint32_t *d_rows, uint32_t n_rows, const uint32_t *d_tiles, uint32_t n_tiles, void *d_xh,
+                                   uint32_t xh_pitch_halfs, const float *d_raw, uint32_t pitch_elems, const float *d_mags,
+                                   uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
+                                   const uint32_t *d_deleted, cudaStream_t s) {
+    if (n_rows) {
+        zero_rows_kernel<<<n_rows, 128, 0, s>>>(d_rows, reinterpret_cast<uint8_t *>(d_xh), xh_pitch_halfs * 2);
+        CDB_LAUNCH_CHECK();
+    }
+    if (d_xs8 && n_tiles) {
+        quantize_s8_tiles_kernel<<<n_tiles, 256, 0, s>>>(d_raw, pitch_elems, d_mags, 0, row_end, dim, reinterpret_cast<int8_t *>(d_xs8),
+                                                         pitch8, d_tile_se, d_tiles, d_deleted);
+        CDB_LAUNCH_CHECK();
+        s8_emax_kernel<<<1, 1024, 0, s>>>(d_tile_se, (uint32_t)((row_end + TS_BLOCK_N - 1) / TS_BLOCK_N), d_emax);
+        CDB_LAUNCH_CHECK();
+    }
     return CDB_OK;
 }
 
@@ -963,8 +1023,9 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
 cdb_status tensor_scan_i8_device(const uint8_t *d_x, const uint8_t *d_q, uint32_t pitch, uint64_t n_rows, uint32_t nq, uint32_t dim,
                                  uint32_t k, int metric, const float *d_mags, const float *d_qmags, uint32_t id_base, int *d_ggm,
                                  uint64_t *d_cand64, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_err32, uint32_t *d_progress,
-                                 int sm_count, cudaStream_t s) {
+                                 const uint32_t *d_deleted, int sm_count, cudaStream_t s) {
     TensorScanArgs a{};
+    a.deleted = d_deleted;
     a.window = 3;
     a.refresh_mask = 15;
     a.n_rows = n_rows;

@@ -89,14 +89,15 @@ cdb_status unpack_digits_device(const uint8_t *d_codes, uint32_t row_pitch, uint
 size_t tensor_u8_smem_bytes(uint32_t k) { return tensor_scan_smem_bytes(k); }
 
 // d_x: u8 operand rows [n_rows][pitch] (u8 codes or unpacked digits); d_q: query operand rows padded with zero
-// rows to a multiple of 128.  Writes ids/scores/counts (and the packed keys when d_out_keys is given).
+// rows to a multiple of 128.  Writes ids/scores/counts (and the packed keys when d_out_keys is given).  d_deleted (null while
+// no row is deleted): rows whose bit is set are kept out of the bound, the output and the zero-magnitude Err.
 cdb_status tensor_u8_scan_device(const uint8_t *d_x, const uint8_t *d_q, uint32_t pitch, uint64_t n_rows, uint32_t nq, uint32_t dim,
                                  uint32_t k, int metric, const float *d_mags, const float *d_qmags, uint32_t id_base, int *d_gthr,
                                  uint64_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_err32, uint32_t *d_progress,
-                                 uint32_t *d_ids, float *d_scores, uint32_t *d_counts, int sm_count, cudaStream_t s,
-                                 uint64_t *d_out_keys) {
+                                 uint32_t *d_ids, float *d_scores, uint32_t *d_counts, const uint32_t *d_deleted, int sm_count,
+                                 cudaStream_t s, uint64_t *d_out_keys) {
     cdb_status rc = tensor_scan_i8_device(d_x, d_q, pitch, n_rows, nq, dim, k, metric, d_mags, d_qmags, id_base, d_gthr, d_cand,
-                                          d_cand_cnt, cand_cap, d_err32, d_progress, sm_count, s);
+                                          d_cand_cnt, cand_cap, d_err32, d_progress, d_deleted, sm_count, s);
     if (rc) return rc;
     uint32_t P = 1;
     while (P < cand_cap) P <<= 1;

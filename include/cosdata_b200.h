@@ -120,9 +120,14 @@ typedef struct {
     int32_t exact_only;      /* 1: never take a tensor-core path (pure SIMT scan); results are identical either way */
     uint32_t prefilter_k;    /* candidate slots per query of the tensor-core paths (0 = default); a query whose list
                                 overflows is re-done by the exact scan on the device (alone if <= 64 queries overflow) */
-    uint32_t reserved0;
+    uint32_t flags;          /* CDB_SEARCH_* bits; unknown bits are ignored */
     uint32_t reserved1;
 } cdb_search_params;
+/* Brute-force modes may take the tensor-core paths while the shard has deleted rows; the kernels skip those rows (the
+ * fp16 / s8 prefilter shadows of a deleted row are zero and its candidates are dropped by the re-rank, the u8 wgmma masks
+ * its tiles' epilogue).  Results are bit-identical with and without the flag, as with exact_only, which still wins.
+ * Without it a shard with deleted rows is answered by the exact scan.  HNSW mode ignores it. */
+#define CDB_SEARCH_TENSOR_WITH_DELETED 1u
 
 /* ---------------------------------------------------------------- misc */
 int32_t cdb_abi_version(void);
@@ -450,7 +455,10 @@ cdb_status cdb_index_read_graph_slot_scores(cdb_index *index, uint32_t level, fl
  *      rescoring Err that one relink; D is unlinked everywhere and gets status 2.
  *   D4 D keeps its node entries with an empty adjacency on every level (an isolated node); rows are never reused.
  * Deleted rows: the exact scans never return them nor flag their errors; the tensor-core brute-force paths are bypassed
- * while any row is deleted (the exact scan answers); cdb_index_build_graph / cdb_index_insert_graph skip them (out_failed
+ * while any row is deleted (the exact scan answers) unless the search sets CDB_SEARCH_TENSOR_WITH_DELETED, which lets them
+ * run and skip the deleted rows (same results; making that the default is a later behaviour change).  The
+ * call zeroes the deleted rows' fp16 shadow rows and re-quantizes the s8 shadow tiles they are in, without them;
+ * cdb_index_build_graph / cdb_index_insert_graph skip them (out_failed
  * 2, no nodes above level 0), cdb_index_build_graph_replicas refuses a list naming one, cdb_index_set_graph refuses a
  * graph linking one.  cdb_score_ids, cdb_rerank_f32 and cdb_distance_pairs take explicit ids and are unchanged.  Without
  * a graph the call only marks the rows.  Graphs with metadata: CDB_UNSUPPORTED, nothing changed.  Locking, the order
@@ -603,8 +611,9 @@ cdb_status cdb_index_stats(const cdb_index *index, uint64_t *out4);
 /* the first n of: {tensor-core searches, searches where some query needed the exact scan, all-zero rows, other degenerate rows
  * (norm outside [1e-15, 1e15]: they ride on every prefilter candidate list), fp16 shadow present, queries of the LAST
  * tensor-core search that were re-done by the exact scan (candidate overflow or degenerate query norm), tensor-core
- * searches whose prefilter ran in the s8 form (also counted in the first field)} */
-#define CDB_STATS_FIELDS 7
+ * searches whose prefilter ran in the s8 form (also counted in the first field), tensor-core searches that ran while the
+ * shard had deleted rows (CDB_SEARCH_TENSOR_WITH_DELETED; also counted in the first field)} */
+#define CDB_STATS_FIELDS 8
 cdb_status cdb_index_stats_ex(const cdb_index *index, uint64_t *out, uint32_t n);
 /* candidates the prefilter emitted for each of the first n queries of the last prefilter search */
 cdb_status cdb_index_last_candidate_counts(const cdb_index *index, uint32_t n, uint32_t *out);
