@@ -141,6 +141,8 @@ PROTOTYPES = {
     "cdb_hnsw_files_info": (C.c_int32, [c_vp, c_vp, c_vp]),
     "cdb_hnsw_files_level": (C.c_int32, [c_vp, C.c_uint32, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cdb_hnsw_files_metadata": (C.c_int32, [c_vp, c_vp, c_f32p]),
+    "cdb_hnsw_files_slot_scores": (C.c_int32, [c_vp, C.c_uint32, c_vp, c_vp]),
+    "cdb_index_set_graph_slot_scores": (C.c_int32, [C.c_void_p, c_vp, c_vp]),
     "cdb_index_set_graph_from_files": (C.c_int32, [c_vp, c_vp]),
     "cdb_quantize_batch": (C.c_int32, [C.c_int32, C.c_int32, C.c_float, C.c_float, c_f32p, C.c_uint64, C.c_uint32, c_vp, c_f32p]),
     "cdb_distance_pairs": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_uint32, c_vp, c_f32p, c_vp, c_f32p, C.c_uint64, c_f32p, c_i32p]),

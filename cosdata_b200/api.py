@@ -245,11 +245,21 @@ class HnswFiles:
         self.md_bits = np.zeros((self.n_md, max(self.md_dims, 1)), dtype=np.int32)
         self.md_mags = np.zeros(self.n_md, dtype=np.float32)
         _check(self._lib.cdb_hnsw_files_metadata(self._h, _ptr(self.md_bits), _ptr(self.md_mags)))
+        # the MetricResult stored with each slot, parallel to adj: value (empty slot 0) and tag (empty slot 0xFF)
+        self.slot_scores, self.slot_tags = [], []
+        for lv in range(self.num_levels + 1):
+            sc, tg = np.zeros(self.adj[lv].size, np.float32), np.zeros(self.adj[lv].size, np.uint8)
+            _check(self._lib.cdb_hnsw_files_slot_scores(self._h, lv, _ptr(sc), _ptr(tg)))
+            self.slot_scores.append(sc)
+            self.slot_tags.append(tg)
 
-    def apply(self, index):
-        """cdb_index_set_graph_from_files"""
+    def apply(self, index, slot_scores=False):
+        """cdb_index_set_graph_from_files; slot_scores=True also attaches the stored slot similarities
+        (cdb_index_set_graph_slot_scores), so the graph takes insert_graph_replicas / delete_rows_replicas"""
         _check(self._lib.cdb_index_set_graph_from_files(index._h, self._h))
         index.md_dims = max(self.md_dims, 1)
+        if slot_scores:
+            index.set_graph_slot_scores(self.slot_scores, self.slot_tags)
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -531,6 +541,28 @@ class DenseIndex:
                            C.cast(t_nm, C.c_void_p), int(pseudo_entry))
         _check(self._lib.cdb_index_set_graph_metadata(self._h, C.byref(md)))
         self.md_dims = bits.shape[1]
+
+    def set_graph_slot_scores(self, scores, tags=None):
+        """cdb_index_set_graph_slot_scores: the similarity stored with every slot of a graph with uploaded metadata (one f32
+        array of level_counts[L] * neighbours per level, the graph's upload order) and optionally the MetricResult tags
+        (u8, same shape; checked against the index's metric).  The graph then takes insert_graph_replicas /
+        delete_rows_replicas."""
+        info = np.zeros(5, dtype=np.uint32)
+        counts = np.zeros(32, dtype=np.uint32)
+        _check(self._lib.cdb_index_graph_info(self._h, _ptr(info), _ptr(counts)))
+        L1 = int(info[0]) + 1
+        shapes = [int(counts[lv]) * int(info[2] if lv == 0 else info[1]) for lv in range(L1)]
+        sc = [np.ascontiguousarray(a, dtype=np.float32).ravel() for a in scores]
+        tg = None if tags is None else [np.ascontiguousarray(a, dtype=np.uint8).ravel() for a in tags]
+        if len(sc) != L1 or (tg is not None and len(tg) != L1):
+            raise ValueError(f"need one array per level ({L1})")
+        for lv in range(L1):
+            if sc[lv].size != shapes[lv] or (tg is not None and tg[lv].size != shapes[lv]):
+                raise ValueError(f"level {lv} needs {shapes[lv]} slot values")
+        t_sc = (C.c_void_p * L1)(*[a.ctypes.data for a in sc])
+        t_tg = None if tg is None else (C.c_void_p * L1)(*[a.ctypes.data for a in tg])
+        _check(self._lib.cdb_index_set_graph_slot_scores(self._h, C.cast(t_sc, C.c_void_p),
+                                                         None if t_tg is None else C.cast(t_tg, C.c_void_p)))
 
     def batch_search_filtered(self, queries, filters, k, **kw):
         """search_internal with per-query metadata filters: filters[q] is None or a list of int8[md_dims] (QueryFilterDimensions)

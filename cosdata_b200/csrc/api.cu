@@ -199,7 +199,7 @@ struct cdb_index {
     const uint32_t *const *md_node_id = nullptr, *const *md_node_md = nullptr;
     const int32_t *md_bits = nullptr;
     const float *md_mags = nullptr;
-    uint32_t md_dims = 0, md_pseudo_entry = 0;
+    uint32_t md_dims = 0, md_pseudo_entry = 0, md_rows = 0;
     std::vector<uint32_t> g_cnt;
     std::vector<const uint32_t *> g_nr, g_ad, g_ch;  // host copies of the per-level device pointers
     std::vector<const uint32_t *> g_id, g_md;        // same for node_id / node_md when has_md
@@ -1394,8 +1394,8 @@ cdb_status cdb_index_set_graph_metadata(cdb_index *ix, const cdb_graph_metadata 
     ix->md_allocs.clear();
     ix->has_md = false;
     uint32_t pseudo_row, n_md;
-    if (hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {   // a replica build's state does not describe uploaded metadata
-        hnsw_state_free(ix->bstate);
+    if (hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {   // a replica builder's state does not describe uploaded metadata
+        hnsw_state_release(ix->bstate, &ix->graph_allocs);
         ix->bstate = nullptr;
     }
     auto upload = [&](const void *src, size_t bytes, const void **dst) -> cdb_status {
@@ -1423,6 +1423,7 @@ cdb_status cdb_index_set_graph_metadata(cdb_index *ix, const cdb_graph_metadata 
     ix->md_mags = reinterpret_cast<const float *>(mags);
     ix->md_dims = md->md_dims;
     ix->md_pseudo_entry = md->pseudo_entry;
+    ix->md_rows = md->n_md;
     ix->has_md = true;
     return CDB_OK;
 }
@@ -1431,6 +1432,38 @@ static GraphHost graph_host(cdb_index *ix) {
     GraphHost gh{&ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr, &ix->g_ad, &ix->g_ch};
     if (ix->has_md) { gh.id = &ix->g_id; gh.md = &ix->g_md; gh.id_tbl = ix->md_node_id; gh.md_tbl = ix->md_node_md; }
     return gh;
+}
+
+cdb_status cdb_index_set_graph_slot_scores(cdb_index *ix, const float *const *scores, const uint8_t *const *tags) {
+    CDB_REQUIRE(ix && scores, "null argument");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph && ix->has_md,
+                "no graph with metadata: cdb_index_set_graph_from_files or cdb_index_set_graph_metadata first (a graph without "
+                "metadata derives its slot state itself)");
+    uint32_t pseudo_row = 0, n_md = 0;
+    CDB_REQUIRE(!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md),
+                "the graph already has its builder state (a replica build, or an earlier cdb_index_set_graph_slot_scores)");
+    const uint32_t L1 = ix->graph.num_levels + 1;
+    for (uint32_t L = 0; L < L1; ++L) CDB_REQUIRE(scores[L] && (!tags || tags[L]), "null level array");
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    {   // searches already enqueued on their callers' streams finish before the graph's state changes
+        std::lock_guard<std::mutex> g(ix->pool_mu);
+        for (auto &u : ix->pool)
+            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
+    }
+    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    HnswBuildState *st = nullptr;
+    cdb_status rc = hnsw_attach_replica_state_device(ix->desc.metric, graph_host(ix), scores, tags, ix->md_pseudo_entry, ix->md_rows,
+                                                     ix->md_dims, ix->md_bits, ix->md_mags, &st, ix->stream);
+    if (rc) return rc;
+    hnsw_state_release(ix->bstate, &ix->graph_allocs);   // a plain slot state derived before the metadata was uploaded
+    ix->bstate = st;
+    // as after a replica build: the uploaded node_id / node_md arrays and the Metadata table are the builder's now, which
+    // replaces them when a level or the table grows
+    ix->graph_allocs.insert(ix->graph_allocs.end(), ix->md_allocs.begin(), ix->md_allocs.end());
+    ix->md_allocs.clear();
+    ix->graph.identity_mask = 0u;   // inserted level-0 nodes do not list rows in order
+    return CDB_OK;
 }
 
 cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
@@ -1625,7 +1658,7 @@ cdb_status cdb_index_insert_graph_replicas(cdb_index *ix, const cdb_build_params
                 "no graph with metadata: cdb_index_build_graph_replicas first (a graph without metadata grows through cdb_index_insert_graph)");
     uint32_t pseudo_row = 0, n_md = 0;
     if (!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {
-        set_error("insert into a graph whose metadata was uploaded is not supported (its slot similarities cannot be derived)");
+        set_error("insert into a graph whose metadata was uploaded needs its stored slot similarities (cdb_index_set_graph_slot_scores)");
         return CDB_UNSUPPORTED;
     }
     CDB_REQUIRE(bp->num_levels == ix->graph.num_levels && bp->neighbors_count == ix->graph.nbrs &&
@@ -1636,6 +1669,16 @@ cdb_status cdb_index_insert_graph_replicas(cdb_index *ix, const cdb_build_params
     CDB_REQUIRE((ri->md_bits_new && ri->md_mags_new) || !ri->n_md_new, "null metadata table rows");
     CDB_REQUIRE((uint64_t)n_md + ri->n_md_new < CDB_INVALID_ID, "metadata table too large");
     const uint64_t n_md_all = (uint64_t)n_md + ri->n_md_new;
+    if (pseudo_row == CDB_INVALID_ID && ri->n_nodes) {   // a graph without a pseudo root (a collection without a metadata schema)
+        std::vector<float> mags(n_md);
+        if (n_md) CDB_CUDA_TRY(cudaMemcpy(mags.data(), ix->md_mags, (size_t)n_md * 4, cudaMemcpyDeviceToHost));
+        for (uint32_t t = 0; t < ri->n_nodes; ++t) {
+            CDB_REQUIRE(ri->row[t] != CDB_INVALID_ID, "the graph has no pseudo root: a pseudo replica (row CDB_INVALID_ID) cannot be inserted");
+            const uint32_t m = ri->md_row[t];
+            CDB_REQUIRE(m == CDB_INVALID_ID || m >= n_md_all || (m < n_md ? mags[m] : ri->md_mags_new[m - n_md]) == 0.0f,
+                        "the graph has no pseudo root: a node whose Metadata has mag != 0 cannot be inserted");
+        }
+    }
     for (uint32_t t = 0; t < ri->n_nodes; ++t) {
         const uint32_t r = ri->row[t];
         CDB_REQUIRE(r == CDB_INVALID_ID || r < ix->size, "replica row out of range");
@@ -1794,7 +1837,7 @@ cdb_status cdb_index_delete_rows_replicas(cdb_index *ix, const uint32_t *rows, u
                 "no graph with metadata: cdb_index_build_graph_replicas first (a graph without metadata deletes through cdb_index_delete_rows)");
     uint32_t pseudo_row = 0, n_md = 0;
     if (!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {
-        set_error("delete from a graph whose metadata was uploaded is not supported (its slot similarities cannot be derived)");
+        set_error("delete from a graph whose metadata was uploaded needs its stored slot similarities (cdb_index_set_graph_slot_scores)");
         return CDB_UNSUPPORTED;
     }
     for (uint64_t i = 0; i < n; ++i) {
@@ -1874,7 +1917,7 @@ cdb_status cdb_index_read_replica_slot_scores(cdb_index *ix, uint32_t level, flo
     CDB_REQUIRE(ix->has_md, "the graph has no metadata: cdb_index_read_graph_slot_scores reads its slot scores");
     uint32_t pseudo_row = 0, n_md = 0;
     if (!hnsw_state_replica_info(ix->bstate, &pseudo_row, &n_md)) {
-        set_error("slot scores of a graph whose metadata was uploaded are not supported (they cannot be derived)");
+        set_error("slot scores of a graph whose metadata was uploaded need cdb_index_set_graph_slot_scores first");
         return CDB_UNSUPPORTED;
     }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));

@@ -37,10 +37,11 @@ struct BuildLevel {
     uint32_t *lowest_idx;  // [cnt]
     uint32_t *lowest_key;  // [cnt]
     int *lock;             // [cnt]
-    // replica builds (collections with a metadata schema): [0] main root, [1] pseudo root, then created nodes in list order
+    // replica builds (collections with a metadata schema): [0] main root, [1] pseudo root, then created nodes in list order;
+    // a graph attached by cdb_index_set_graph_slot_scores keeps its uploaded order, and the nodes each call appends follow
     const uint32_t *node_id;   // [cnt] ProbNode::get_id()
     const uint32_t *node_md;   // [cnt] metadata table row or HN_EMPTY
-    const uint32_t *node_ins;  // [cnt] position in the replica list (ascending from local 2; roots HN_EMPTY)
+    const uint32_t *node_ins;  // [cnt] position in the replica list (roots HN_EMPTY); the current call's nodes ascend from `app`
 };
 constexpr int BUILD_MAX_LEVELS = 16;
 struct BuildGraph {
@@ -80,10 +81,11 @@ struct BuildArgs {
 __device__ __forceinline__ bool bit_set(const uint32_t *bits, uint32_t i) { return (bits[i >> 5] >> (i & 31)) & 1u; }
 
 // local index of `row` at `level` (level 0: the row itself; level >= 1: binary search in the part of node_row the current
-// call appended -- an uploaded level need not be sorted before it)
+// call appended -- an uploaded level need not be sorted before it).  Replica graphs: `row` is a list position, searched among
+// the nodes the current call created (they follow in list order from `app`)
 __device__ inline uint32_t build_local(const BuildLevel &l, uint32_t level, uint32_t row, bool replicas = false) {
-    if (replicas) {   // every level lists the created nodes in list order behind the two roots
-        uint32_t lo = 2, hi = l.cnt;
+    if (replicas) {
+        uint32_t lo = l.app, hi = l.cnt;
         while (lo < hi) { const uint32_t md = (lo + hi) >> 1; if (l.node_ins[md] < row) lo = md + 1; else hi = md; }
         return lo;
     }
@@ -244,6 +246,28 @@ __global__ void fill_u32_kernel(uint32_t *p, uint32_t v, uint64_t n) {
     if (i < n) p[i] = v;
 }
 
+// ------------------------------------------------------------------ lowest_index of a loaded node
+// ProbNode::new_with_neighbors_and_versions (prob_node.rs:155-169), over one node's slots held by a whole warp: each lane
+// notes the slots it holds, finish() reduces.  The first empty slot gives MetricResult::min; otherwise, scanning from
+// MetricResult::max, the first slot with a strictly lower key.
+struct SlotLowest {
+    uint32_t first_empty = HN_EMPTY;
+    uint64_t best = ~0ull;   // (key << 32 | slot): lowest filled slot strictly below MetricResult::max
+    __device__ void note(uint32_t s, bool empty, uint32_t key, uint32_t max_key) {
+        if (empty) first_empty = min(first_empty, s);
+        else if (key < max_key) best = min(best, ((uint64_t)key << 32) | s);
+    }
+    __device__ void finish(uint32_t min_key, uint32_t max_key, uint32_t &li, uint32_t &lk) {   // whole warp, every lane gets it
+        for (int o = 16; o; o >>= 1) {
+            best = min(best, (uint64_t)__shfl_xor_sync(0xFFFFFFFFu, best, o));
+            first_empty = min(first_empty, __shfl_xor_sync(0xFFFFFFFFu, first_empty, o));
+        }
+        li = 0; lk = max_key;
+        if (first_empty != HN_EMPTY) { li = first_empty; lk = min_key; }
+        else if (best != ~0ull) { li = (uint32_t)best; lk = (uint32_t)(best >> 32); }
+    }
+};
+
 // ------------------------------------------------------------------ slot state of an uploaded graph
 // ProbNode::new_with_neighbors_and_versions (prob_node.rs:145-181): every slot's similarity is recomputed and lowest_index is
 // the first empty slot (MetricResult::min) or else the first slot with a strictly lower similarity, scanning from
@@ -271,15 +295,13 @@ __global__ void __launch_bounds__(SS_WARPS * 32) hnsw_slot_state_kernel(BuildLev
     uint32_t parity = 0;
     for (uint32_t node = blockIdx.x * SS_WARPS + warp; node < l.cnt; node += gridDim.x * SS_WARPS) {
         const uint32_t row = l.node_row[node];
-        uint32_t first_empty = HN_EMPTY;
-        uint64_t best = ~0ull;   // (key << 32 | slot): lowest filled slot strictly below MetricResult::max
+        SlotLowest lo;
         for (uint32_t base = 0; base < l.nb; base += group) {
             const uint32_t s = base + lane;
             const bool in_round = lane < group && s < l.nb;
             const uint32_t nbr = in_round ? l.adj[(size_t)node * l.nb + s] : HN_EMPTY;
             const uint32_t filled = __ballot_sync(0xFFFFFFFFu, nbr != HN_EMPTY);
-            const uint32_t empties = __ballot_sync(0xFFFFFFFFu, in_round && nbr == HN_EMPTY);
-            if (first_empty == HN_EMPTY && empties) first_empty = base + __ffs(empties) - 1;
+            if (in_round && nbr == HN_EMPTY) lo.note(s, true, 0, max_key);
             const uint32_t nrow = nbr != HN_EMPTY ? l.node_row[nbr] : 0;
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the previous round's reads before the copies below
             __syncwarp();
@@ -296,14 +318,12 @@ __global__ void __launch_bounds__(SS_WARPS * 32) hnsw_slot_state_kernel(BuildLev
                 const int rc = pair_distance(sc.metric, sc.st, sc.dim, own, sc.mags[row], pp, mine_row, sc.mags[nrow], pp, &d);
                 const uint32_t key = rc == CDB_OK ? order_key(sc.metric, __float_as_uint(d)) : min_key;
                 l.simkey[(size_t)node * l.nb + s] = key;
-                if (key < max_key) best = min(best, ((uint64_t)key << 32) | s);
+                lo.note(s, false, key, max_key);
             }
         }
-        for (int o = 16; o; o >>= 1) best = min(best, (uint64_t)__shfl_xor_sync(0xFFFFFFFFu, best, o));
+        uint32_t li, lk;
+        lo.finish(min_key, max_key, li, lk);
         if (lane == 0) {
-            uint32_t li = 0, lk = max_key;
-            if (first_empty != HN_EMPTY) { li = first_empty; lk = min_key; }
-            else if (best != ~0ull) { li = (uint32_t)best; lk = (uint32_t)(best >> 32); }
             l.lowest_idx[node] = li;
             l.lowest_key[node] = lk;
         }
@@ -387,6 +407,21 @@ static uint32_t *&level_array(BuildLevel &l, int t) {
     }
 }
 static size_t level_words(const BuildLevel &l, int t, uint64_t nodes) { return t == 5 || t == 6 ? nodes * l.nb : nodes; }
+
+void hnsw_state_release(HnswBuildState *st, std::vector<void *> *allocs) {
+    if (!st) return;
+    auto drop = [&](const void *p) {
+        auto it = p ? std::find(allocs->begin(), allocs->end(), p) : allocs->end();
+        if (it == allocs->end()) return;
+        allocs->erase(it);
+        cudaFree(const_cast<void *>(p));
+    };
+    for (uint32_t L = 0; L <= st->g.num_levels && L < (uint32_t)BUILD_MAX_LEVELS; ++L)
+        for (int t : {1, 2, 3, 6, 7, 8, 9}) drop(level_array(st->g.lv[L], t));   // not node_row / child / adj: the graph's
+    drop(st->md_bits);
+    drop(st->md_mags);
+    delete st;
+}
 
 // the per-level columns of nodes appended to a replica graph, parallel to append_levels' rows
 struct ReplicaCols {
@@ -1136,6 +1171,7 @@ cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &r
         const std::vector<uint32_t> &mem = members[L];
         l.nb = L == 0 ? nbrs0 : nbrs;
         l.cnt = 2 + (uint32_t)mem.size();
+        l.app = 2;
         std::vector<uint32_t> nr(l.cnt), ch(l.cnt, HN_EMPTY), ni(l.cnt), nm(l.cnt), ins(l.cnt, HN_EMPTY);
         nr[0] = rh.main_root_row; ni[0] = 0xFFFFFFFFu; nm[0] = rh.main_root_md;
         nr[1] = rh.pseudo_root_row; ni[1] = MD_PSEUDO_ID_LO; nm[1] = rh.pseudo_root_md;
@@ -1378,13 +1414,13 @@ __global__ void hnsw_delete_rowset_kernel(const uint32_t *rows, uint32_t n, uint
     if (i < n) atomicOr(bits + (rows[i] >> 5), 1u << (rows[i] & 31));
 }
 
-// one grid-stride pass over a level's node_row behind the two roots: each node whose row is in `bits` is counted, and with
-// `out` set emitted (the order of the hits is the host's to fix)
+// one grid-stride pass over a level's node_row: each node with a list position (not a root) whose row is in `bits` is
+// counted, and with `out` set emitted (the order of the hits is the host's to fix)
 __global__ void hnsw_delete_find_kernel(BuildLevel l, uint32_t level, const uint32_t *bits, uint32_t n_rows, uint32_t *n_hits,
                                         DelHit *out) {
-    for (uint32_t j = 2 + blockIdx.x * blockDim.x + threadIdx.x; j < l.cnt; j += gridDim.x * blockDim.x) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < l.cnt; j += gridDim.x * blockDim.x) {
         const uint32_t r = l.node_row[j];
-        if (r >= n_rows || !bit_set(bits, r)) continue;
+        if (r >= n_rows || !bit_set(bits, r) || l.node_ins[j] == HN_EMPTY) continue;
         const uint32_t k = atomicAdd(n_hits, 1u);
         if (out) out[k] = DelHit{level, j, l.node_ins[j], r, l.node_id[j], l.node_md[j]};
     }
@@ -1417,7 +1453,7 @@ cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh
         CDB_CUDA_TRY(cudaMemsetAsync(d_nhits, 0, 4, s));
         for (uint32_t L = 0; L < L1; ++L) {
             const BuildLevel &l = st->g.lv[L];
-            if (l.cnt <= 2) continue;
+            if (!l.cnt) continue;
             const uint32_t grid = std::min<uint32_t>((l.cnt + 255) / 256, (uint32_t)sms * 8);
             hnsw_delete_find_kernel<<<grid, 256, 0, s>>>(l, L, d_bits, n_rows, d_nhits, d_hits);
             CDB_LAUNCH_CHECK();
@@ -1545,6 +1581,167 @@ cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh
     if (e != cudaSuccess) { set_error(std::string("hnsw replica delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
     for (uint32_t k = 0; k < ni; ++k)
         if (hf[k] || hs[k]) out_status[item_pos[k]] = 2;
+    return CDB_OK;
+}
+
+// ------------------------------------------------------------------ builder state of a loaded replica graph
+// cdb_index_set_graph_slot_scores: the state the reference holds after a restart (ProbNode::new_with_neighbors_and_versions,
+// prob_node.rs:145-181) -- every filled slot keeps the similarity stored with it on disk and lowest_index is derived afresh.
+// The uploaded order stays (nothing is renumbered; searches and read_graph see the same arrays): the roots keep their local
+// indices, and a loaded node's list position is the level-0 index of its node, carried up the child links (the roots have
+// none).  build_local only ever searches the nodes of the current call, and the delete finds a row's nodes by a pass over
+// node_row, so neither needs the loaded nodes in any order.  Inserted nodes take positions from level_counts[0] on.
+
+// one warp per node: simkey arrives holding the stored f32 bits and becomes their order keys; a filled slot whose tag is not
+// want_tag sets bit 0 of *bad
+__global__ void __launch_bounds__(SS_WARPS * 32) hnsw_attach_slots_kernel(BuildLevel l, uint32_t level, const uint32_t *below_ins,
+                                                                          const uint8_t *tags, uint32_t want_tag, int metric,
+                                                                          uint32_t min_key, uint32_t max_key, uint32_t root0,
+                                                                          uint32_t root1, uint32_t *bad) {
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (uint32_t node = blockIdx.x * SS_WARPS + warp; node < l.cnt; node += gridDim.x * SS_WARPS) {
+        SlotLowest lo;
+        bool mismatch = false;
+        for (uint32_t s = lane; s < l.nb; s += 32) {
+            const size_t t = (size_t)node * l.nb + s;
+            const bool empty = l.adj[t] == HN_EMPTY;
+            const uint32_t key = empty ? 0u : order_key(metric, l.simkey[t]);
+            if (!empty && tags && tags[t] != want_tag) mismatch = true;
+            l.simkey[t] = key;
+            lo.note(s, empty, key, max_key);
+        }
+        uint32_t li, lk;
+        lo.finish(min_key, max_key, li, lk);
+        if (mismatch) atomicOr(bad, 1u);
+        if (lane == 0) {
+            l.lowest_idx[node] = li;
+            l.lowest_key[node] = lk;
+            l.lock[node] = 0;
+            const_cast<uint32_t *>(l.node_ins)[node] =
+                level == 0 ? (node == root0 || node == root1 ? HN_EMPTY : node) : below_ins[l.child[node]];
+        }
+    }
+}
+
+// duplicate node ids on a level: open addressing over id + 1 (0 = free); an id met twice sets bit 1 of *bad
+__global__ void hnsw_attach_ids_kernel(const uint32_t *ids, uint32_t cnt, unsigned long long *table, uint64_t mask, uint32_t *bad) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) {
+        const unsigned long long v = (unsigned long long)ids[i] + 1ull;
+        uint64_t h = ((uint64_t)ids[i] * 0x9E3779B97F4A7C15ull >> 24) & mask;
+        for (;;) {
+            const unsigned long long old = atomicCAS(table + h, 0ull, v);
+            if (old == 0ull) break;
+            if (old == v) { atomicOr(bad, 2u); break; }
+            h = (h + 1) & mask;
+        }
+    }
+}
+
+// MetricResult's tag byte for the index's metric (types.rs:425-431)
+static uint32_t metric_result_tag(int metric) {
+    switch (metric) {
+    case CDB_METRIC_COSINE: return 0;        // CosineSimilarity
+    case CDB_METRIC_EUCLIDEAN: return 2;     // EuclideanDistance
+    case CDB_METRIC_HAMMING: return 3;       // HammingDistance
+    default: return 4;                       // DotProductDistance
+    }
+}
+
+cdb_status hnsw_attach_replica_state_device(int metric, const GraphHost &gh, const float *const *scores, const uint8_t *const *tags,
+                                            uint32_t pseudo_entry, uint32_t n_md, uint32_t md_dims, const int32_t *md_bits,
+                                            const float *md_mags, HnswBuildState **out_state, cudaStream_t s) {
+    const GraphDev &d = *gh.dev;
+    const uint32_t L1 = d.num_levels + 1;
+    if (L1 > BUILD_MAX_LEVELS) { set_error("the graph has more levels than the builder supports"); return CDB_UNSUPPORTED; }
+    const bool has_pseudo = pseudo_entry != d.entry;
+    // the roots' level-local indices, down their child links from the top level
+    std::vector<uint32_t> root0(L1), root1(L1, HN_EMPTY);
+    root0[L1 - 1] = d.entry;
+    if (has_pseudo) root1[L1 - 1] = pseudo_entry;
+    for (uint32_t L = L1 - 1; L > 0; --L) {
+        CDB_CUDA_TRY(cudaMemcpy(&root0[L - 1], (*gh.ch)[L] + root0[L], 4, cudaMemcpyDeviceToHost));
+        if (has_pseudo) CDB_CUDA_TRY(cudaMemcpy(&root1[L - 1], (*gh.ch)[L] + root1[L], 4, cudaMemcpyDeviceToHost));
+    }
+    uint32_t pseudo_row = CDB_INVALID_ID;
+    if (has_pseudo) CDB_CUDA_TRY(cudaMemcpy(&pseudo_row, (*gh.nr)[L1 - 1] + pseudo_entry, 4, cudaMemcpyDeviceToHost));
+    // ---- every allocation before anything changes
+    std::unique_ptr<HnswBuildState> st(new HnswBuildState());
+    st->g.num_levels = d.num_levels;
+    st->g.entry = d.entry;
+    st->g.root_row = d.root_row;
+    st->g.pseudo_entry = pseudo_entry;
+    metric_key_range(metric, &st->g.min_key, &st->g.max_key);
+    cdb_status rc;
+    DevAllocs kept, tmp;
+    size_t max_slots = 0;
+    uint32_t max_cnt = 0;
+    for (uint32_t L = 0; L < L1; ++L) {
+        BuildLevel &l = st->g.lv[L];
+        l.cnt = l.app = (*gh.cnt)[L];
+        l.nb = L == 0 ? d.nbrs0 : d.nbrs;
+        l.node_row = const_cast<uint32_t *>((*gh.nr)[L]);
+        l.adj = const_cast<uint32_t *>((*gh.ad)[L]);
+        l.child = L ? const_cast<uint32_t *>((*gh.ch)[L]) : nullptr;
+        l.node_id = (*gh.id)[L];
+        l.node_md = (*gh.md)[L];
+        st->cap[L] = l.cnt;
+        const size_t slots = (size_t)l.cnt * l.nb;
+        if ((rc = kept.get((void **)&l.simkey, slots * 4)) || (rc = kept.get((void **)&l.lowest_idx, (size_t)l.cnt * 4)) ||
+            (rc = kept.get((void **)&l.lowest_key, (size_t)l.cnt * 4)) || (rc = kept.get((void **)&l.lock, (size_t)l.cnt * 4)) ||
+            (rc = kept.get((void **)&level_array(l, 9), (size_t)l.cnt * 4)))
+            return rc;
+        max_slots = std::max(max_slots, slots);
+        max_cnt = std::max(max_cnt, l.cnt);
+    }
+    uint64_t table_n = 2;
+    while (table_n < 2ull * max_cnt) table_n <<= 1;
+    uint8_t *d_tags = nullptr;
+    unsigned long long *table = nullptr;
+    uint32_t *d_bad = nullptr;
+    if ((tags && (rc = tmp.get((void **)&d_tags, max_slots))) || (rc = tmp.get((void **)&table, table_n * 8)) ||
+        (rc = tmp.get((void **)&d_bad, 4)))
+        return rc;
+    int dev = 0, sms = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    // ---- per level: the stored values in, the ids checked, keys / lowest_index / list positions derived
+    CDB_CUDA_TRY(cudaMemsetAsync(d_bad, 0, 4, s));
+    const uint32_t want_tag = metric_result_tag(metric);
+    for (uint32_t L = 0; L < L1; ++L) {
+        const BuildLevel &l = st->g.lv[L];
+        const size_t slots = (size_t)l.cnt * l.nb;
+        if (!l.cnt) continue;
+        CDB_CUDA_TRY(cudaMemcpyAsync(l.simkey, scores[L], slots * 4, cudaMemcpyHostToDevice, s));
+        if (tags) CDB_CUDA_TRY(cudaMemcpyAsync(d_tags, tags[L], slots, cudaMemcpyHostToDevice, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(table, 0, table_n * 8, s));
+        const uint32_t id_grid = std::min<uint32_t>((l.cnt + 255) / 256, (uint32_t)sms * 8);
+        hnsw_attach_ids_kernel<<<id_grid, 256, 0, s>>>(l.node_id, l.cnt, table, table_n - 1, d_bad);
+        CDB_LAUNCH_CHECK();
+        const uint32_t grid = std::min<uint32_t>((l.cnt + SS_WARPS - 1) / SS_WARPS, (uint32_t)sms * 16);
+        hnsw_attach_slots_kernel<<<grid, SS_WARPS * 32, 0, s>>>(l, L, L ? st->g.lv[L - 1].node_ins : nullptr, tags ? d_tags : nullptr,
+                                                               want_tag, metric, st->g.min_key, st->g.max_key, root0[L], root1[L], d_bad);
+        CDB_LAUNCH_CHECK();
+    }
+    uint32_t bad = 0;
+    CDB_CUDA_TRY(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error(std::string("hnsw slot scores: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    if (bad & 1u) {
+        set_error("a stored slot's MetricResult tag is not the index metric's (" + std::to_string(want_tag) + ")");
+        return CDB_STORAGE_MISMATCH;
+    }
+    if (bad & 2u) { set_error("a level of the graph lists a node id twice"); return CDB_INVALID_PARAMS; }
+    // ---- the state joins the graph
+    st->replicas = true;
+    st->n_list = (*gh.cnt)[0];
+    st->pseudo_root_row = pseudo_row;
+    st->n_md = n_md;
+    st->md_dims = md_dims;
+    st->md_bits = md_bits;
+    st->md_mags = md_mags;
+    gh.allocs->insert(gh.allocs->end(), kept.p.begin(), kept.p.end());
+    kept.release();
+    *out_state = st.release();
     return CDB_OK;
 }
 

@@ -9,7 +9,9 @@
 //                   u8 level | u32 version | u32 prop offset | u32 prop length | u32 metadata offset (u32::MAX = none) | u32 length |
 //                   u32 parent link | u32 child link | u16 n | n x (u32 neighbour id, u32 neighbour link, u8 tag, f32 similarity)
 //                 every "link" is a byte offset into nodes.ptr (u32::MAX = null); an empty neighbour slot is 13 x 0xFF
-//                 (serializer/hnsw/neighbors.rs:21-60).
+//                 (serializer/hnsw/neighbors.rs:21-60); (tag, similarity) is the MetricResult add_neighbor kept for the slot
+//                 (types.rs:425-431), kept as read (slot_tag / slot_score) for cdb_index_set_graph_slot_scores: the reader does
+//                 not know the index's metric, so tags are not checked here.
 // The two entry links (root_vec_ptr_offset / pseudo_root_vec_ptr_offset) live in LMDB next to the index parameters
 // (types.rs:899-945) and are passed in by the caller.  With enable_context_history the link image is not one file: every
 // flush writes each dirty 8192-byte region in full to "<region>-<version>.ptr" (cache_loader.rs:91-113,
@@ -35,6 +37,8 @@ struct cdb_hnsw_files {
     uint32_t num_levels = 0, nbrs = 0, nbrs0 = 0, entry = 0, pseudo_entry = CDB_INVALID_ID, root_row = 0, md_dims = 0;
     bool has_md = false;
     std::vector<std::vector<uint32_t>> node_row, node_id, node_md, adj, child;
+    std::vector<std::vector<float>> slot_score;     // per level, parallel to adj (empty slot: 0)
+    std::vector<std::vector<uint8_t>> slot_tag;     // per level, parallel to adj (empty slot: 0xFF)
     std::vector<int32_t> md_bits;
     std::vector<float> md_mags;
 };
@@ -76,6 +80,8 @@ struct NodeRec {
     uint8_t level;
     uint32_t prop_off, md_off, parent, child;
     std::vector<uint32_t> nbr_link;   // CDB_INVALID_ID = empty slot
+    std::vector<uint8_t> tag;         // MetricResult of each slot as stored
+    std::vector<float> score;
 };
 
 struct Reader {
@@ -147,8 +153,13 @@ struct Reader {
         n.prop_off = u32(p + 5); n.md_off = u32(p + 13); n.parent = u32(p + 21); n.child = u32(p + 25);
         uint16_t cnt; memcpy(&cnt, p + 29, 2);
         if ((uint64_t)off + 31 + (uint64_t)cnt * 13 > f->len) return fail("neighbour list outside " + std::to_string(fid) + ".index");
-        n.nbr_link.resize(cnt);
-        for (uint32_t s = 0; s < cnt; ++s) n.nbr_link[s] = u32(p + 31 + s * 13 + 4);   // 0xFFFFFFFF for an empty slot
+        n.nbr_link.resize(cnt); n.tag.resize(cnt); n.score.resize(cnt);
+        for (uint32_t s = 0; s < cnt; ++s) {
+            const uint8_t *e = p + 31 + s * 13;
+            n.nbr_link[s] = u32(e + 4);   // 0xFFFFFFFF for an empty slot
+            n.tag[s] = e[8];
+            memcpy(&n.score[s], e + 9, 4);
+        }
         return true;
     }
 };
@@ -198,6 +209,7 @@ cdb_status flatten(const char *index_dir, uint32_t root_link, uint32_t pseudo_li
     out.entry = rw.second;
     out.pseudo_entry = pseudo_link == CDB_INVALID_ID ? CDB_INVALID_ID : where[pseudo_link].second;
     out.node_row.assign(L1, {}); out.node_id.assign(L1, {}); out.node_md.assign(L1, {}); out.adj.assign(L1, {}); out.child.assign(L1, {});
+    out.slot_score.assign(L1, {}); out.slot_tag.assign(L1, {});
     out.nbrs = out.nbrs0 = 0;
     for (uint32_t L = 0; L < L1; ++L) {
         const uint32_t cnt = (uint32_t)order[L].size();
@@ -209,6 +221,8 @@ cdb_status flatten(const char *index_dir, uint32_t root_link, uint32_t pseudo_li
         else if (out.nbrs != nb) return bad("levels >= 1 differ in neighbour count");
         out.node_row[L].resize(cnt); out.node_id[L].resize(cnt); out.node_md[L].resize(cnt); out.child[L].assign(cnt, 0);
         out.adj[L].assign((size_t)cnt * nb, CDB_INVALID_ID);
+        out.slot_score[L].assign((size_t)cnt * nb, 0.0f);
+        out.slot_tag[L].assign((size_t)cnt * nb, 0xFF);
         for (uint32_t i = 0; i < cnt; ++i) {
             const NodeRec &n = recs[L][i];
             if (n.nbr_link.size() != nb) return bad("nodes of one level differ in neighbour count");
@@ -224,8 +238,12 @@ cdb_status flatten(const char *index_dir, uint32_t root_link, uint32_t pseudo_li
                 out.node_id[L][i] = pm->second.second;   // ProbNode::get_id(): the replica id
                 out.has_md = true;
             }
-            for (uint32_t s = 0; s < nb; ++s)
-                if (n.nbr_link[s] != CDB_INVALID_ID) out.adj[L][(size_t)i * nb + s] = where[n.nbr_link[s]].second;
+            for (uint32_t s = 0; s < nb; ++s) {
+                if (n.nbr_link[s] == CDB_INVALID_ID) continue;
+                out.adj[L][(size_t)i * nb + s] = where[n.nbr_link[s]].second;
+                out.slot_score[L][(size_t)i * nb + s] = n.score[s];
+                out.slot_tag[L][(size_t)i * nb + s] = n.tag[s];
+            }
             if (L > 0) {
                 if (n.child == CDB_INVALID_ID) return bad("a node above level 0 has no child");
                 out.child[L][i] = where[n.child].second;
@@ -282,6 +300,14 @@ cdb_status cdb_hnsw_files_level(const cdb_hnsw_files *h, uint32_t level, uint32_
     if (node_md) memcpy(node_md, h->node_md[level].data(), cnt * 4);
     if (adjacency) memcpy(adjacency, h->adj[level].data(), h->adj[level].size() * 4);
     if (child) memcpy(child, h->child[level].data(), cnt * 4);
+    return CDB_OK;
+}
+
+cdb_status cdb_hnsw_files_slot_scores(const cdb_hnsw_files *h, uint32_t level, float *out_scores, uint8_t *out_tags) {
+    if (!h || level > h->num_levels) { set_error("bad argument"); return CDB_INVALID_PARAMS; }
+    const size_t slots = h->adj[level].size();
+    if (out_scores) memcpy(out_scores, h->slot_score[level].data(), slots * 4);
+    if (out_tags) memcpy(out_tags, h->slot_tag[level].data(), slots);
     return CDB_OK;
 }
 

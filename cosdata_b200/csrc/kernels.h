@@ -173,6 +173,9 @@ struct GraphHost {
 // the builder's per-slot state (similarity keys, stale lowest_index, node locks), kept next to the graph it belongs to
 struct HnswBuildState;
 void hnsw_state_free(HnswBuildState *st);
+// frees the state and the arrays that only it uses (slot keys, lowest_index, locks, list positions, and on replica graphs the
+// node_id / node_md arrays and the Metadata table it grew) when `allocs` owns them; the graph's node_row / adj / child stay
+void hnsw_state_release(HnswBuildState *st, std::vector<void *> *allocs);
 // cdb_index_build_graph: root row n on every level, then rows [0, n) inserted
 cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
                              uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed, const GraphHost &gh,
@@ -235,6 +238,15 @@ bool hnsw_state_replica_info(const HnswBuildState *st, uint32_t *pseudo_root_row
 cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const ReplicaHost &rh,
                                        uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed,
                                        const int32_t **md_bits, const float **md_mags, bool *changed, cudaStream_t s);
+// cdb_index_set_graph_slot_scores: the builder's state of an uploaded graph with metadata from the similarities stored with its
+// slots (scores[L] / tags[L]: host, level_counts[L] x nbrs(L); tags may be NULL), as a reference restart holds it.  The graph is
+// not renumbered.  pseudo_entry == the graph's entry: no pseudo root (the state's pseudo root row is CDB_INVALID_ID).  The
+// Metadata table (n_md rows) becomes the builder's.  CDB_STORAGE_MISMATCH when a filled slot's tag is not the metric's,
+// CDB_INVALID_PARAMS when a level lists a node id twice; on any error nothing changed.  On success the new arrays have
+// joined gh.allocs.
+cdb_status hnsw_attach_replica_state_device(int metric, const GraphHost &gh, const float *const *scores, const uint8_t *const *tags,
+                                            uint32_t pseudo_entry, uint32_t n_md, uint32_t md_dims, const int32_t *md_bits,
+                                            const float *md_mags, HnswBuildState **out_state, cudaStream_t s);
 // cdb_index_delete_rows_replicas: every node of each of the distinct rows rows[0..n) (none a root row) deleted from the replica
 // graph of `st` with D1-D5 (DESIGN.md section 4); out_status[i] = 0, or 2 where an Err hit one of the row's nodes.  A row
 // without a node is left alone.  *changed as for hnsw_insert_device.

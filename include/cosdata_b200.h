@@ -305,6 +305,12 @@ cdb_status cdb_hnsw_files_info(const cdb_hnsw_files *files, uint32_t *info8, uin
 cdb_status cdb_hnsw_files_level(const cdb_hnsw_files *files, uint32_t level, uint32_t *node_row, uint32_t *node_id, uint32_t *node_md,
                                 uint32_t *adjacency, uint32_t *child);
 cdb_status cdb_hnsw_files_metadata(const cdb_hnsw_files *files, int32_t *md_bits, float *md_mags);
+/* the MetricResult stored with each neighbour slot of `level` (serializer/hnsw/neighbors.rs:52-57, types.rs:425-431), in the
+ * layout of cdb_hnsw_files_level's adjacency: out_scores[level_counts[level] x neighbours] the f32 value, out_tags the tag
+ * byte (0 CosineSimilarity, 2 EuclideanDistance, 3 HammingDistance, 4 DotProductDistance); an empty slot gives 0 and 0xFF.
+ * Either pointer may be NULL.  The reader does not know the index's metric, so tags are returned as stored, unchecked
+ * (cdb_index_set_graph_slot_scores checks them). */
+cdb_status cdb_hnsw_files_slot_scores(const cdb_hnsw_files *files, uint32_t level, float *out_scores, uint8_t *out_tags);
 
 /* Replica nodes and metadata of a graph uploaded with cdb_index_set_graph (collections with a metadata schema:
  * src/vector_store.rs:57-250, 485-712).  One embedding may own several graph nodes (its base replica and one per
@@ -325,6 +331,25 @@ typedef struct {
 } cdb_graph_metadata;
 cdb_status cdb_index_set_graph_metadata(cdb_index *index, const cdb_graph_metadata *md);
 cdb_status cdb_index_set_graph_from_files(cdb_index *index, const cdb_hnsw_files *files);
+/* stored similarities per slot of the current graph, [num_levels+1] arrays of level_counts[L] x nbrs(L), in the level-local
+ * order the graph was uploaded with; tags (may be NULL) are MetricResult tags and must match the index's metric.
+ * Makes a graph whose metadata came from cdb_index_set_graph_metadata / cdb_index_set_graph_from_files writable: afterwards
+ * cdb_index_insert_graph_replicas, cdb_index_delete_rows_replicas and cdb_index_read_replica_slot_scores accept it.  The
+ * builder's state is the one the reference holds after a restart (ProbNode::new_with_neighbors_and_versions,
+ * prob_node.rs:145-181): every filled slot keeps its stored similarity, lowest_index is derived afresh (the first empty slot,
+ * else the first slot with the strictly lowest similarity).  The graph is not renumbered: searches and
+ * cdb_index_read_graph_level see the same arrays before and after.  The roots keep their indices; a loaded node's list
+ * position (the order in which a deleted row's nodes repair, D5) is the level-0 index of its node in the uploaded order, and
+ * nodes inserted later follow every loaded node.  The graph's Metadata table becomes the builder's (md_bits_new appends to it).
+ * A graph whose pseudo_entry is its entry has no pseudo root (a collection without a metadata schema, as
+ * cdb_index_set_graph_from_files uploads it): its inserts refuse pseudo replicas (row CDB_INVALID_ID) and nodes whose
+ * Metadata has mag != 0, and its deletes refuse only the main root's row.
+ * Refusals, nothing changed and the graph stays searchable: a filled slot whose tag is not the metric's MetricResult variant
+ * (cosine 0, dot product 4, Euclidean 2, Hamming 3): CDB_STORAGE_MISMATCH; no graph, a graph without metadata (a
+ * cdb_index_set_graph graph derives its state itself), a graph that already has its builder state (a replica build or an
+ * earlier call), a null level array, or a level listing a node id twice: CDB_INVALID_PARAMS.  Takes the writer lock;
+ * searches enqueued before the call finish first.  Every device allocation happens before anything changes. */
+cdb_status cdb_index_set_graph_slot_scores(cdb_index *index, const float *const *scores, const uint8_t *const *tags);
 /* GPU-side index build (index_embeddings, src/vector_store.rs:714-940): appends the root vector (random in
  * values_range, id u32::MAX; vector_store.rs:57-67) as the last row and builds the HNSW graph over all rows with the
  * reference's algorithm (traverse with ef_construction per level, create_node_edges / add_neighbor with
@@ -415,7 +440,9 @@ cdb_status cdb_index_insert_graph(cdb_index *index, const cdb_build_params *para
  * deterministically); seed is unused (level draws come from the caller).
  * No graph, or a graph without metadata (those grow through cdb_index_insert_graph): CDB_INVALID_PARAMS.  A graph whose
  * metadata came from cdb_index_set_graph_metadata / cdb_index_set_graph_from_files: CDB_UNSUPPORTED (its slot similarities
- * cannot be derived).  n_nodes == 0: CDB_OK, *out_inserted = 0, nothing changes (no table rows are appended either).
+ * cannot be derived) until cdb_index_set_graph_slot_scores attached the stored ones; from then on it grows like a graph
+ * built here.  A graph without a pseudo root refuses pseudo replicas and nodes whose Metadata has mag != 0
+ * (CDB_INVALID_PARAMS).  n_nodes == 0: CDB_OK, *out_inserted = 0, nothing changes (no table rows are appended either).
  * Locking, the order against enqueued searches and the failure contract are those of cdb_index_insert_graph: every
  * allocation comes before the graph changes, so an allocation failure leaves the graph, its metadata and its table as they
  * were; an error after the graph started changing drops the graph and its metadata, and cdb_last_error_string says so.
@@ -466,7 +493,8 @@ cdb_status cdb_index_read_graph_slot_scores(cdb_index *index, uint32_t level, fl
  * repair has succeeded. */
 cdb_status cdb_index_delete_rows(cdb_index *index, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
                                  uint8_t *out_status, uint64_t *out_deleted);
-/* delete_embedding on a graph that cdb_index_build_graph_replicas built (and cdb_index_insert_graph_replicas may have grown).
+/* delete_embedding on a graph that cdb_index_build_graph_replicas built, or whose stored slot similarities
+ * cdb_index_set_graph_slot_scores attached (and cdb_index_insert_graph_replicas may have grown).
  * The unit is a vector row (one embedding): deleting row r deletes every graph node whose node_row is r -- its base replica
  * and all of its Metadata replicas, on every level.  Arguments, out_status, *out_deleted, the marks and the deleted rows'
  * treatment elsewhere are those of cdb_index_delete_rows; a status is per row (2 if an Err hit any of its nodes).  A row
@@ -486,14 +514,14 @@ cdb_status cdb_index_delete_rows(cdb_index *index, const uint32_t *rows, uint64_
  *      (deterministic); larger batches guarantee the invariants only.
  * Refusals (nothing changes, no marks): a row out of range, the main root's or the pseudo root's row (pseudo replicas share
  * it), shortlist_size outside 1..64, no graph or a graph without metadata (cdb_index_delete_rows): CDB_INVALID_PARAMS; a
- * graph whose metadata came from cdb_index_set_graph_metadata / cdb_index_set_graph_from_files: CDB_UNSUPPORTED.  Locking,
- * the order against enqueued searches and the failure contract are those of cdb_index_insert_graph_replicas: an error after
+ * graph whose metadata came from cdb_index_set_graph_metadata / cdb_index_set_graph_from_files without
+ * cdb_index_set_graph_slot_scores: CDB_UNSUPPORTED.  Locking, the order against enqueued searches and the failure contract are those of cdb_index_insert_graph_replicas: an error after
  * the graph started changing drops the graph and its metadata. */
 cdb_status cdb_index_delete_rows_replicas(cdb_index *index, const uint32_t *rows, uint64_t n, uint32_t shortlist_size,
                                           uint32_t max_batch, uint8_t *out_status, uint64_t *out_deleted);
 /* the slot similarities a replica build, insert or delete keeps for `level` (layout and values as in
  * cdb_index_read_graph_slot_scores; on a Pseudo-Metadata edge both slots hold calculate(Metadata end, Pseudo end)).  A graph
- * without metadata: CDB_INVALID_PARAMS; uploaded metadata: CDB_UNSUPPORTED. */
+ * without metadata: CDB_INVALID_PARAMS; uploaded metadata without cdb_index_set_graph_slot_scores: CDB_UNSUPPORTED. */
 cdb_status cdb_index_read_replica_slot_scores(cdb_index *index, uint32_t level, float *out_scores);
 /* out[i] = 1 if row first+i is deleted (first + n <= capacity); *out_total = deleted rows of the index (either pointer may be
  * NULL when unused) */
