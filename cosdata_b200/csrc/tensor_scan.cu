@@ -19,6 +19,7 @@
 //   warps 8..11  producer warpgroup (setmaxnreg: 40 registers), one thread issues the TMA loads:
 //                cp.async.bulk.tensor.2d, SWIZZLE_128B, 4-stage mbarrier ring
 // Tile: 128 queries (A, K-major) x 256 corpus rows (B, K-major), K block = 64 halfs (128 B).
+#include <atomic>
 #include <climits>
 #include <cmath>
 #include <cstdlib>
@@ -38,6 +39,21 @@ constexpr int TS_THREADS = TS_CONSUMERS + 128;     // + the producer warpgroup
 constexpr uint32_t TS_A_BYTES = TS_BLOCK_M * TS_BLOCK_K * 2;  // 16 KB
 constexpr uint32_t TS_B_BYTES = TS_BLOCK_N * TS_BLOCK_K * 2;  // 32 KB
 constexpr uint32_t TS_STAGE_BYTES = TS_A_BYTES + TS_B_BYTES;
+// clock64 sums of the instrumented instantiation (PROF): consumer slots summed over both warpgroups (thread 0 of each),
+// producer slots over the issuing thread, all over every CTA of every launch since the sums were last read
+enum : int {
+    TS_PROF_FULL_WAIT,   // consumers waiting on a full barrier (starved of operands)
+    TS_PROF_MMA,         // consumers issuing the k-blocks' wgmma and waiting for them to retire
+    TS_PROF_EPILOGUE,    // class maxima, threshold test, emission (and the KIND 1 cosine staging) up to the bound refresh
+    TS_PROF_REFRESH,     // the bound refresh
+    TS_PROF_EMPTY_WAIT,  // producer waiting on an empty barrier (ring full)
+    TS_PROF_DRIFT,       // producer in the bounded-drift spin
+    TS_PROF_TILES,       // tiles processed (per warpgroup)
+    TS_PROF_CONSUMER,    // consumers: whole tile loop
+    TS_PROF_PRODUCER,    // producer: whole issue loop
+    TS_PROF_CTAS,        // CTAs
+    TS_PROF_SLOTS
+};
 
 struct TensorScanArgs {
     uint64_t n_rows;     // rows visible to this launch (the seeding pass sees a prefix)
@@ -56,6 +72,7 @@ struct TensorScanArgs {
     uint32_t window;     // a CTA may run at most `window` tiles ahead of the slowest CTA of its group
     uint32_t refresh_mask;  // the shared bound is refreshed when (tile & mask) == mask (and for the first tiles)
     uint32_t has_deg;       // the corpus holds degenerate rows: kernel variant that keeps zero accumulators out of the bound
+    unsigned long long *prof;   // [TS_PROF_SLOTS] clock64 sums of the instrumented instantiation, null otherwise
     // ---- integer form (KIND 1: exact scoring of u8 codes / sub-byte digits on wgmma .s32.u8.u8, tensor_scan_u8.cu)
     int metric;             // CDB_METRIC_COSINE or CDB_METRIC_DOT_PRODUCT
     const float *mags;      // [n_rows] stored magnitudes (cosine)
@@ -196,7 +213,9 @@ __device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
 // Register layout of the epilogue: a consumer thread holds two query rows (r and r + 8 of its warpgroup's 64) and, of each,
 // the 64 columns 8j + 2(lane%4) + {0,1}.  Classes are column mod NG, so the thread owns NG/4 classes of each of its queries
 // (those = 2(lane%4) or 2(lane%4)+1 mod 8); the four threads of a quad together cover all NG classes of their two queries.
-template <int STAGES, int NG, bool HAS_DEG, int KIND>
+//
+// PROF: the instrumented instantiation (a.prof): clock64 sums per phase, see TS_PROF_*.
+template <int STAGES, int NG, bool HAS_DEG, int KIND, bool PROF>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x, TensorScanArgs a) {
     constexpr uint32_t K_ELEMS = KIND != 0 ? 2 * TS_BLOCK_K : TS_BLOCK_K;   // elements per 128-byte row: 128 u8/s8 / 64 halfs
@@ -234,16 +253,21 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         // ===================== TMA producer =====================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
         if (threadIdx.x == TS_CONSUMERS) {
+            unsigned long long p_empty = 0, p_drift = 0, p_t0 = PROF ? clock64() : 0;
             uint32_t s = 0, phase = 0, t = 0;
             for (uint32_t nt = g; nt < a.ntiles; nt += G, ++t) {
                 if (a.mtiles > 1 && t >= a.window) {
+                    const unsigned long long c0 = PROF ? clock64() : 0;
                     // bounded drift: every CTA of the group must have consumed tile t - window
                     const uint32_t need = (t - a.window + 1) * a.mtiles;
                     // bounded spin: if a peer CTA is not resident (GPU shared with another stream) we only lose locality
                     for (int spin = 0; spin < 20000 && *reinterpret_cast<volatile uint32_t *>(a.progress + g) < need; ++spin) __nanosleep(64);
+                    if (PROF) p_drift += clock64() - c0;
                 }
                 for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
+                    const unsigned long long c0 = PROF ? clock64() : 0;
                     mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+                    if (PROF) p_empty += clock64() - c0;
                     const uint32_t fb = smem_u32(&full_bar[s]);
                     const uint32_t sa = smem_u32(tiles + (size_t)s * TS_STAGE_BYTES);
                     mbar_expect_tx(fb, TS_STAGE_BYTES);
@@ -251,6 +275,12 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                     tma_load_2d(sa + TS_A_BYTES, &map_x, fb, (int)(kb * K_ELEMS), (int)(nt * TS_BLOCK_N));
                     if (++s == STAGES) { s = 0; phase ^= 1; }
                 }
+            }
+            if (PROF) {
+                atomicAdd(a.prof + TS_PROF_EMPTY_WAIT, p_empty);
+                atomicAdd(a.prof + TS_PROF_DRIFT, p_drift);
+                atomicAdd(a.prof + TS_PROF_PRODUCER, clock64() - p_t0);
+                atomicAdd(a.prof + TS_PROF_CTAS, 1ull);
             }
         }
     } else {
@@ -290,10 +320,14 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             }
         }
         const uint32_t sa0 = smem_u32(tiles);
+        unsigned long long p_full = 0, p_mma = 0, p_epi = 0, p_ref = 0, p_c = PROF ? clock64() : 0;
         uint32_t s = 0, phase = 0, t = 0;
         for (uint32_t nt = g; nt < a.ntiles; nt += G, ++t) {
             const uint64_t row0 = (uint64_t)nt * TS_BLOCK_N;
             const float *rs = rinv_s + (t & 1) * TS_BLOCK_N;
+            unsigned long long c_tile = PROF ? clock64() : 0, c_full = 0;
+            // KIND 2: {s_T, E_T}, loaded before the MMAs so that its L2 round trip hides under them
+            const float2 se = KIND == 2 ? __ldg(a.tile_se + nt) : make_float2(0.0f, 0.0f);
             if (cosine) {
                 // reciprocal magnitudes of this tile's rows -> shared memory (double buffered by tile parity); a zero
                 // magnitude is an Err for every query that meets the row (cosine.rs:230-231)
@@ -310,13 +344,19 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                     for (int i = 0; i < 2; ++i) if (qvalid[i]) err[i] |= (uint32_t)CDB_ERRFLAG_CALCULATION;
                 }
             }
-            // ---- the tile's product: kblocks x 4 wgmma into registers; a stage is released when its MMAs have retired
+            // ---- the tile's product: kblocks x 4 wgmma into registers; a stage is released when its MMAs have retired.
+            //      The zeroing costs 128 moves per thread and tile, but it is what ends the accumulators' live range for
+            //      ptxas: a wgmma with scale-d 0 still reads them, so without it they stay live through the epilogue and
+            //      the NG = 64 instantiations spill.
+            const unsigned long long c_main = PROF ? clock64() : 0;
             Acc acc[128];
 #pragma unroll
             for (int i = 0; i < 128; ++i) acc[i] = 0;
             uint32_t prev = 0;
             for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
+                const unsigned long long c0 = PROF ? clock64() : 0;
                 mbar_wait(smem_u32(&full_bar[s]), phase);
+                if (PROF) c_full += clock64() - c0;
                 const uint32_t sa = sa0 + s * TS_STAGE_BYTES;
                 const uint64_t adesc = make_smem_desc(sa + wg * (TS_A_BYTES / 2)), bdesc = make_smem_desc(sa + TS_A_BYTES);
                 wgmma_fence();
@@ -335,6 +375,13 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             wgmma_wait<0>();
             if (a.kblocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
             if (ct == 0 && a.mtiles > 1) atomicAdd(a.progress + g, 1u);   // all loads of this tile have landed in smem
+            unsigned long long c_epi = 0;
+            if (PROF) {
+                c_epi = clock64();
+                p_full += c_full;
+                p_mma += c_epi - c_main - c_full;
+                p_epi += c_main - c_tile;   // KIND 1 cosine: the per-tile reciprocal staging
+            }
 
             // ---- epilogue: fold the values into the class maxima, test the tile maximum against the threshold,
             //      build the per-value tests only on a hit
@@ -351,7 +398,6 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             const bool full_tile = row0 + TS_BLOCK_N <= a.n_rows;   // only the corpus' last tile can be partial (TMA zero fill)
             const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;   // valid columns of this tile
             if constexpr (KIND == 2) {
-                const float2 se = __ldg(a.tile_se + nt);   // {s_T, E_T}
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
                     // s_T*s_q rounded down and up, eps(q,T) rounded up, thrI <= (A - eps) / (s_T*s_q)
@@ -469,6 +515,11 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                 }
             }
             }
+            unsigned long long c_ref = 0;
+            if (PROF) {
+                c_ref = clock64();
+                p_epi += c_ref - c_epi;
+            }
             // refresh the shared bound: every tile early on (and in the seeding pass), then every 16th tile.  The quad's
             // classes are published before any of its threads reads the maxima back.
             if (t < 8 || (t & a.refresh_mask) == a.refresh_mask || !a.emit) {
@@ -490,6 +541,15 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                     if (nb > bound[i]) { bound[i] = nb; thr[i] = KIND == 1 ? (cosine ? bound[i] * a.rel : bound[i]) : bound[i] - a.two_eps; }
                 }
             }
+            if (PROF) p_ref += clock64() - c_ref;
+        }
+        if (PROF && (ct & 127) == 0) {
+            atomicAdd(a.prof + TS_PROF_FULL_WAIT, p_full);
+            atomicAdd(a.prof + TS_PROF_MMA, p_mma);
+            atomicAdd(a.prof + TS_PROF_EPILOGUE, p_epi);
+            atomicAdd(a.prof + TS_PROF_REFRESH, p_ref);
+            atomicAdd(a.prof + TS_PROF_TILES, (unsigned long long)t);
+            atomicAdd(a.prof + TS_PROF_CONSUMER, clock64() - p_c);
         }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -867,10 +927,18 @@ size_t tensor_scan_smem_bytes(uint32_t k) {
     return tensor_scan_smem(TS_STAGES);
 }
 
+// cdb_debug_scan_profile: launches use the instrumented instantiation while g_scan_prof_on is set
+static std::atomic<bool> g_scan_prof_on{false};
+static unsigned long long *g_scan_prof = nullptr;   // [TS_PROF_SLOTS] on the device that enabled profiling
+
 template <int NG, bool HAS_DEG, int KIND>
 static cdb_status launch_tensor_scan_gd(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid,
                                         cudaStream_t s) {
-    auto kern = tensor_scan_kernel<TS_STAGES, NG, HAS_DEG, KIND>;
+    auto kern = tensor_scan_kernel<TS_STAGES, NG, HAS_DEG, KIND, false>;
+    if (a.prof) {   // the instrumented instantiation exists for the headline's k <= 12 without degenerate rows
+        if constexpr (NG == 16 && !HAS_DEG) kern = tensor_scan_kernel<TS_STAGES, NG, HAS_DEG, KIND, true>;
+        else { set_error("tensor scan profile: only for k <= 12 on shards without degenerate or deleted rows"); return CDB_INVALID_PARAMS; }
+    }
     const size_t smem = tensor_scan_smem(TS_STAGES);
     CDB_ALLOW_SMEM(kern, smem);
     kern<<<grid, TS_THREADS, smem, s>>>(mq, mx, a);
@@ -899,6 +967,7 @@ template <int KIND>
 static cdb_status run_tensor_scan(const CUtensorMap &mq, const CUtensorMap &mx, TensorScanArgs a, uint64_t n_rows,
                                   uint32_t *d_progress, int sm_count, cudaStream_t s) {
     cdb_status rc;
+    if (g_scan_prof_on.load()) a.prof = g_scan_prof;
     // 1. seeding pass over a prefix of the corpus: a few CTAs per query tile, no emission, only the class maxima.
     //    Afterwards every CTA of the main pass starts from the k-th best of ~16K rows instead of from
     //    -inf, which removes the per-CTA warm-up bursts from the candidate lists.
@@ -1066,3 +1135,21 @@ cdb_status select_fallback_device(const uint32_t *d_cnt, uint32_t cap, const flo
 }
 
 }  // namespace cdb
+
+// Measurement switch of the prefilter scan (tools/bench_prefilter_resident.py; not part of the public header).  enable != 0
+// runs the clock64-instrumented instantiation (k <= 12, no degenerate or deleted rows) from now on, 0 the default one;
+// results are the same either way.  out (may be null, TS_PROF_SLOTS entries, see the TS_PROF_* enum) receives the sums
+// accumulated since the previous call, which zeroes them.  Process-wide; synchronizes the current device, whose searches
+// the profile then covers.
+extern "C" cdb_status cdb_debug_scan_profile(int32_t enable, uint64_t *out) {
+    using namespace cdb;
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    if (out) {
+        for (int i = 0; i < TS_PROF_SLOTS; ++i) out[i] = 0;
+        if (g_scan_prof) CDB_CUDA_TRY(cudaMemcpy(out, g_scan_prof, TS_PROF_SLOTS * 8, cudaMemcpyDeviceToHost));
+    }
+    if (enable && !g_scan_prof) CDB_CUDA_TRY(cudaMalloc(&g_scan_prof, TS_PROF_SLOTS * 8));
+    if (g_scan_prof) CDB_CUDA_TRY(cudaMemset(g_scan_prof, 0, TS_PROF_SLOTS * 8));
+    g_scan_prof_on.store(enable != 0);
+    return CDB_OK;
+}
