@@ -113,6 +113,26 @@ class SearchParams(C.Structure):
     ]
 
 
+class SparseIndexDesc(C.Structure):
+    _fields_ = [
+        ("device", C.c_int32),
+        ("quantization_bits", C.c_uint32),
+        ("values_upper_bound", C.c_float),
+        ("capacity_rows", C.c_uint64),
+        ("capacity_pairs", C.c_uint64),
+        ("id_base", C.c_uint32),
+    ]
+
+
+class SparseSearchParams(C.Structure):
+    _fields_ = [
+        ("k", C.c_uint32),
+        ("early_terminate_threshold", C.c_float),
+        ("rerank", C.c_int32),
+        ("reranking_factor", C.c_uint32),
+    ]
+
+
 # symbol -> (restype, argtypes); must list every function of include/cosdata_b200.h
 PROTOTYPES = {
     "cdb_abi_version": (C.c_int32, []),
@@ -194,6 +214,22 @@ PROTOTYPES = {
     "cdb_index_stats_ex": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32]),
     "cdb_index_last_candidate_counts": (C.c_int32, [C.c_void_p, C.c_uint32, c_u32p]),
     "cdb_index_scan_ms_history": (C.c_int32, [C.c_void_p, C.c_uint32, c_f32p, C.POINTER(C.c_uint32)]),
+    "cdb_sparse_index_create": (C.c_int32, [C.POINTER(SparseIndexDesc), C.POINTER(C.c_void_p)]),
+    "cdb_sparse_index_destroy": (C.c_int32, [C.c_void_p]),
+    "cdb_sparse_index_size": (C.c_uint64, [C.c_void_p]),
+    "cdb_sparse_index_append": (C.c_int32, [C.c_void_p, c_vp, c_u32p, c_f32p, C.c_uint64]),
+    "cdb_sparse_index_delete_rows": (C.c_int32, [C.c_void_p, c_u32p, C.c_uint64]),
+    "cdb_sparse_index_deleted_rows": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, c_u8p, C.POINTER(C.c_uint64)]),
+    "cdb_sparse_search_batch": (C.c_int32, [C.c_void_p, c_vp, c_u32p, c_f32p, C.c_uint32, C.POINTER(SparseSearchParams),
+                                            c_u32p, c_f32p, c_u32p]),
+    "cdb_sparse_search_batch_device": (C.c_int32, [C.c_void_p, c_vp, c_u32p, c_f32p, C.c_uint32, C.POINTER(SparseSearchParams),
+                                                   c_u32p, c_f32p, c_u32p, C.c_void_p]),
+    "cdb_sparse_sample_upper_bound": (C.c_int32, [C.c_int32, c_f32p, C.c_uint64, C.c_float, c_vp, C.c_uint64, c_vp,
+                                                  C.POINTER(C.c_float)]),
+    "cdb_itoe_scan_sparse": (C.c_int32, [C.c_char_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "cdb_itoe_load_sparse": (C.c_int32, [C.c_char_p, C.c_uint64, C.c_uint64, C.c_uint64, c_u32p, c_vp, c_u32p, c_f32p,
+                                         C.POINTER(C.c_uint64)]),
+    "cdb_sparse_index_append_itoe": (C.c_int32, [C.c_void_p, C.c_char_p, c_u32p, C.c_uint64, C.POINTER(C.c_uint64)]),
 }
 
 _lib = None

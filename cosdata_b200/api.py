@@ -801,3 +801,150 @@ def max_insert_level(x, probs):
         if x >= p:
             return lv
     raise ValueError("No matching element found")
+
+
+# ---------------------------------------------------------------- sparse inverted index (InvertedIndex)
+def sparse_csr(rows):
+    """list of [(dim, value), ...] per row -> (offsets u64[n+1], dims u32, values f32)"""
+    off = np.zeros(len(rows) + 1, np.uint64)
+    if rows:
+        off[1:] = np.cumsum([len(r) for r in rows])
+    dims = np.array([d for r in rows for d, _ in r], np.uint32)
+    vals = np.array([v for r in rows for _, v in r], np.float32)
+    return off, dims, vals
+
+
+def _as_csr(x):
+    if isinstance(x, tuple) and len(x) == 3:
+        o, d, v = x
+        return (np.ascontiguousarray(o, dtype=np.uint64), np.ascontiguousarray(d, dtype=np.uint32),
+                np.ascontiguousarray(v, dtype=np.float32))
+    return sparse_csr(x)
+
+
+class SparseSearchOptions:
+    """SparseSearchOptions (inverted/mod.rs:29-32) plus the config values search_internal reads: top_k (required here),
+    early_terminate_threshold (None = config.search.early_terminate_threshold, 0.0), rerank_sparse_with_raw_values and
+    sparse_raw_values_reranking_factor (config.toml:5-6)"""
+
+    def __init__(self, top_k, early_terminate_threshold=None, rerank=False, reranking_factor=5, config_threshold=0.0):
+        self.top_k = top_k
+        self.early_terminate_threshold = early_terminate_threshold
+        self.rerank = rerank
+        self.reranking_factor = reranking_factor
+        self.config_threshold = config_threshold
+
+    def params(self):
+        thr = self.config_threshold if self.early_terminate_threshold is None else self.early_terminate_threshold
+        return _lib.SparseSearchParams(int(self.top_k or 0), float(thr), 1 if self.rerank else 0, int(self.reranking_factor))
+
+
+class SparseIndex:
+    """InvertedIndex's IndexOps surface on one GPU (cdb_sparse_index).  Row r has id id_base + r."""
+
+    def __init__(self, quantization_bits=4, values_upper_bound=1.0, capacity_rows=1 << 20, capacity_pairs=1 << 27, id_base=0,
+                 device=0):
+        L = _lib.load()
+        d = _lib.SparseIndexDesc(device, quantization_bits, values_upper_bound, capacity_rows, capacity_pairs, id_base)
+        h = C.c_void_p()
+        _check(L.cdb_sparse_index_create(C.byref(d), C.byref(h)))
+        self.h, self.desc = h, d
+        self.sampling_counts, self.values_collected = np.zeros(9, np.uint64), 0
+
+    def close(self):
+        if getattr(self, "h", None):
+            _lib.load().cdb_sparse_index_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def __len__(self):
+        return int(_lib.load().cdb_sparse_index_size(self.h))
+
+    def append(self, rows):
+        """rows: list of pair lists, or a CSR triple (offsets, dims, values)"""
+        o, d, v = _as_csr(rows)
+        _check(_lib.load().cdb_sparse_index_append(self.h, _ptr(o), _ptr(d), _ptr(v), len(o) - 1))
+
+    index_embeddings = append
+
+    def delete_embedding(self, rows):
+        """tombstones local rows (delete_embedding with the inserted pairs removes the row from every list)"""
+        r = np.ascontiguousarray(np.atleast_1d(rows), dtype=np.uint32)
+        _check(_lib.load().cdb_sparse_index_delete_rows(self.h, _ptr(r), r.size))
+
+    def deleted_rows(self, first=0, n=None):
+        n = len(self) - first if n is None else n
+        out = np.zeros(max(n, 1), np.uint8)
+        tot = C.c_uint64(0)
+        _check(_lib.load().cdb_sparse_index_deleted_rows(self.h, first, n, _ptr(out), C.byref(tot)))
+        return out[:n], tot.value
+
+    def batch_search(self, queries, options):
+        """-> ids u32[B, k], scores f32[B, k], counts u32[B]"""
+        o, d, v = _as_csr(queries)
+        nq, k = len(o) - 1, int(options.top_k or 0)
+        ids = np.zeros((nq, max(k, 1)), np.uint32)
+        scores = np.zeros((nq, max(k, 1)), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        p = options.params()
+        _check(_lib.load().cdb_sparse_search_batch(self.h, _ptr(o), _ptr(d), _ptr(v), nq, C.byref(p), _ptr(ids), _ptr(scores),
+                                                   _ptr(counts)))
+        return ids[:, :k], scores[:, :k], counts[:nq]
+
+    def search(self, query, options):
+        ids, scores, counts = self.batch_search([list(query)], options)
+        c = int(counts[0])
+        return list(zip(ids[0, :c].tolist(), scores[0, :c].tolist()))
+
+    def sample_embedding(self, pairs, device=None):
+        """accumulates the sampling counters over the pair values (sample_embedding)"""
+        v = np.ascontiguousarray([x for _, x in pairs], dtype=np.float32)
+        self.sampling_counts, _ = sparse_sample_upper_bound(v, 1.0, self.sampling_counts, self.values_collected,
+                                                            self.desc.device if device is None else device)
+        self.values_collected += v.size
+
+    def finalize_sampling(self, clamp_margin_percent=1.0):
+        """-> values_upper_bound (for an index created after sampling, as the reference's is_configured gate orders it)"""
+        _, ub = sparse_sample_upper_bound(np.zeros(0, np.float32), clamp_margin_percent, self.sampling_counts, self.values_collected,
+                                          self.desc.device)
+        return ub
+
+    def append_itoe(self, collection_dir):
+        """cdb_sparse_index_append_itoe -> internal ids of the appended rows"""
+        n, _, _ = itoe_scan_sparse(collection_dir)
+        ids = np.zeros(max(n, 1), np.uint32)
+        got = C.c_uint64(0)
+        _check(_lib.load().cdb_sparse_index_append_itoe(self.h, os.fsencode(collection_dir), _ptr(ids), n, C.byref(got)))
+        return ids[: got.value]
+
+
+def sparse_sample_upper_bound(values, clamp_margin_percent=1.0, prior_counts=None, prior_values=0, device=0):
+    """-> (counts u64[9] of values > 1..9, values_upper_bound)"""
+    v = np.ascontiguousarray(values, dtype=np.float32)
+    out = np.zeros(9, np.uint64)
+    pr = None if prior_counts is None else np.ascontiguousarray(prior_counts, dtype=np.uint64)
+    ub = C.c_float(0)
+    _check(_lib.load().cdb_sparse_sample_upper_bound(device, _ptr(v), v.size, float(clamp_margin_percent), _ptr(pr), prior_values,
+                                                     _ptr(out), C.byref(ub)))
+    return out, ub.value
+
+
+def itoe_scan_sparse(collection_dir):
+    """-> (live embeddings with sparse values, their pairs, max internal id)"""
+    n, p, mx = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+    _check(_lib.load().cdb_itoe_scan_sparse(os.fsencode(collection_dir), C.byref(n), C.byref(p), C.byref(mx)))
+    return n.value, p.value, mx.value
+
+
+def itoe_load_sparse(collection_dir):
+    """-> (internal ids u32[n] ascending, (offsets u64[n+1], dims u32, values f32))"""
+    n, p, _ = itoe_scan_sparse(collection_dir)
+    ids = np.zeros(max(n, 1), np.uint32)
+    off = np.zeros(n + 1, np.uint64)
+    dims = np.zeros(max(p, 1), np.uint32)
+    vals = np.zeros(max(p, 1), np.float32)
+    got = C.c_uint64(0)
+    _check(_lib.load().cdb_itoe_load_sparse(os.fsencode(collection_dir), 0, n, p, _ptr(ids), _ptr(off), _ptr(dims), _ptr(vals),
+                                            C.byref(got)))
+    return ids[:n], (off, dims[:p], vals[:p])

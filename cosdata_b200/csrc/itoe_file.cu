@@ -57,13 +57,15 @@ struct MappedFile {
     uint64_t u64(uint64_t o) const { uint64_t v; memcpy(&v, p + o, 8); return v; }
 };
 
-struct Entry { uint64_t key; uint32_t version; uint64_t dense_off; uint32_t dense_len; };   // dense values inside itoe.<version>.data
+// dense values (and, when the store reads sparse values, the (u32 dim, f32 value) pairs) inside itoe.<version>.data
+struct Entry { uint64_t key; uint32_t version; uint64_t dense_off; uint32_t dense_len; uint64_t sparse_off = 0; uint32_t sparse_len = 0; };
 
 struct ItoeStore {
     std::string dir;
     MappedFile dim;
     std::map<uint32_t, std::unique_ptr<MappedFile>> data;
     std::string err;
+    bool sparse = false;   // parse past the metadata to the sparse pairs; enumerate embeddings that have them
 
     bool fail(const std::string &m) { if (err.empty()) err = m; return false; }
 
@@ -114,6 +116,27 @@ struct ItoeStore {
         o += n;
         if (!read_len(*f, o, n) || !f->has(o, (uint64_t)n * 4)) return fail("truncated RawVectorEmbedding dense values");
         e.dense_off = o; e.dense_len = n;
+        if (!sparse) return true;
+        o += (uint64_t)n * 4;
+        uint32_t n_md;                                                   // raw_vector_embedding.rs:91-116
+        if (!read_len(*f, o, n_md)) return fail("truncated RawVectorEmbedding metadata");
+        for (uint32_t i = 0; i < n_md; ++i) {
+            if (!read_len(*f, o, n) || !f->has(o, n)) return fail("truncated RawVectorEmbedding metadata field");
+            o += n;
+            if (!f->has(o, 1)) return fail("truncated RawVectorEmbedding metadata value");
+            const uint8_t variant = f->p[o++];
+            if (variant == 0) {
+                if (!f->has(o, 4)) return fail("truncated RawVectorEmbedding metadata value");
+                o += 4;
+            } else if (variant == 1) {
+                if (!read_len(*f, o, n) || !f->has(o, n)) return fail("truncated RawVectorEmbedding metadata value");
+                o += n;
+            } else {
+                return fail("invalid FieldValue variant " + std::to_string(variant));
+            }
+        }
+        if (!read_len(*f, o, n) || !f->has(o, (uint64_t)n * 8)) return fail("truncated RawVectorEmbedding sparse values");
+        e.sparse_off = o; e.sparse_len = n;                             // raw_vector_embedding.rs:118-132
         return true;
     }
 
@@ -132,7 +155,7 @@ struct ItoeStore {
                 Entry e; e.key = key;
                 if (!latest(ioff, iver, e)) return false;
                 if (want_key) { *found = e; *hit = true; return true; }
-                if (e.dense_len) out->push_back(e);
+                if (sparse ? e.sparse_len : e.dense_len) out->push_back(e);
             }
             const uint32_t next = dim.u32(o + 64);
             if (next == UINT32_MAX) break;
@@ -187,6 +210,10 @@ struct ItoeStore {
         return quotients(dim.u32((uint64_t)node + 34), nullptr, &key, &e, &hit);
     }
     void copy_dense(const Entry &e, float *dst) { memcpy(dst, data_file(e.version)->p + e.dense_off, (size_t)e.dense_len * 4); }
+    void copy_sparse(const Entry &e, uint32_t *dims, float *vals) {
+        const uint8_t *p = data_file(e.version)->p + e.sparse_off;
+        for (uint32_t i = 0; i < e.sparse_len; ++i) { memcpy(dims + i, p + 8 * i, 4); memcpy(vals + i, p + 8 * i + 4, 4); }
+    }
 };
 
 cdb_status store_error(const ItoeStore &s) {
@@ -314,6 +341,90 @@ cdb_status cdb_index_fill_raw_from_itoe(cdb_index *index, const char *collection
     if (out_filled) *out_filled = filled;
     if (out_missing) *out_missing = missing;
     if (missing) { set_error(std::to_string(missing) + " rows have no embedding in the itoe store (their raw rows are zero)"); return CDB_INVALID_PARAMS; }
+    return CDB_OK;
+}
+
+// ---- the sparse pairs (InvertedIndex's rows): live embeddings with sparse values, ascending internal id
+static bool sparse_entries(ItoeStore &s, const char *dir, std::vector<Entry> &es) {
+    s.sparse = true;
+    return s.open(dir) && s.enumerate(es);
+}
+
+cdb_status cdb_itoe_scan_sparse(const char *collection_dir, uint64_t *out_entries, uint64_t *out_pairs, uint64_t *out_max_internal_id) {
+    if (!collection_dir) { set_error("null path"); return CDB_INVALID_PARAMS; }
+    ItoeStore s;
+    std::vector<Entry> es;
+    if (!sparse_entries(s, collection_dir, es)) return store_error(s);
+    uint64_t pairs = 0;
+    for (const Entry &e : es) pairs += e.sparse_len;
+    if (out_entries) *out_entries = es.size();
+    if (out_pairs) *out_pairs = pairs;
+    if (out_max_internal_id) *out_max_internal_id = es.empty() ? 0 : es.back().key;
+    return CDB_OK;
+}
+
+cdb_status cdb_itoe_load_sparse(const char *collection_dir, uint64_t first_entry, uint64_t max_entries, uint64_t max_pairs,
+                                uint32_t *out_internal_ids, uint64_t *out_row_offsets, uint32_t *out_dims, float *out_values,
+                                uint64_t *out_read) {
+    if (!collection_dir || !out_read || !out_row_offsets) { set_error("null argument"); return CDB_INVALID_PARAMS; }
+    ItoeStore s;
+    std::vector<Entry> es;
+    if (!sparse_entries(s, collection_dir, es)) return store_error(s);
+    uint64_t got = 0, pairs = 0;
+    out_row_offsets[0] = 0;
+    for (uint64_t i = first_entry; i < es.size() && got < max_entries; ++i, ++got) {
+        if (pairs + es[i].sparse_len > max_pairs) { set_error("itoe store: more sparse pairs than max_pairs"); return CDB_INVALID_PARAMS; }
+        if (!out_dims || !out_values) { set_error("null pair buffers"); return CDB_INVALID_PARAMS; }
+        if (out_internal_ids) out_internal_ids[got] = (uint32_t)es[i].key;
+        s.copy_sparse(es[i], out_dims + pairs, out_values + pairs);
+        pairs += es[i].sparse_len;
+        out_row_offsets[got + 1] = pairs;
+    }
+    *out_read = got;
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_index_append_itoe(cdb_sparse_index *index, const char *collection_dir, uint32_t *out_internal_ids, uint64_t max_ids,
+                                        uint64_t *out_appended) {
+    if (!index || !collection_dir) { set_error("null argument"); return CDB_INVALID_PARAMS; }
+    ItoeStore s;
+    std::vector<Entry> es;
+    if (!sparse_entries(s, collection_dir, es)) return store_error(s);
+    uint64_t rows0 = 0, rows_left = 0, pairs_left = 0, pairs = 0;
+    cdb_status rc = sparse_index_room(index, &rows0, &rows_left, &pairs_left);
+    if (rc) return rc;
+    for (const Entry &e : es) pairs += e.sparse_len;
+    if (es.size() > rows_left || pairs > pairs_left) { set_error("itoe store: the embeddings exceed the index's capacity"); return CDB_INVALID_PARAMS; }
+    const uint64_t CH = 16ull << 20;   // pairs per staged append
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> dims;
+    std::vector<float> vals;
+    uint64_t done = 0;
+    while (done < es.size()) {
+        off.assign(1, 0);
+        dims.clear();
+        vals.clear();
+        uint64_t m = 0;
+        while (done + m < es.size() && (m == 0 || off.back() + es[done + m].sparse_len <= CH)) {
+            const Entry &e = es[done + m];
+            dims.resize(off.back() + e.sparse_len);
+            vals.resize(off.back() + e.sparse_len);
+            s.copy_sparse(e, dims.data() + off.back(), vals.data() + off.back());
+            off.push_back(off.back() + e.sparse_len);
+            if (out_internal_ids && done + m < max_ids) out_internal_ids[done + m] = (uint32_t)e.key;
+            ++m;
+        }
+        if ((rc = cdb_sparse_index_append(index, off.data(), dims.data(), vals.data(), m))) {
+            if (done) {                                   // the earlier chunks go too: all or nothing
+                const std::string msg = cdb_last_error_string();
+                sparse_index_truncate(index, rows0);
+                set_error(msg);
+            }
+            return rc;
+        }
+        done += m;
+    }
+    if (out_appended) *out_appended = done;
     return CDB_OK;
 }
 

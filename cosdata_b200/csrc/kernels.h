@@ -20,6 +20,12 @@ cdb_status raw_mags_device(const float *d_raw, uint32_t pitch_elems, uint64_t n,
 cdb_status sample_counts_device(const float *d_vecs, uint64_t n_values, unsigned long long *d_counts, int sm_count, cudaStream_t s);
 void values_range_from_counts(const uint64_t *counts, uint64_t n_values, float clamp_margin_percent, float *range);
 
+// ---- sparse.cu
+// rows held, rows and pairs that still fit
+cdb_status sparse_index_room(cdb_sparse_index *ix, uint64_t *rows, uint64_t *rows_left, uint64_t *pairs_left);
+// drops the rows from `rows` on (their tombstones too): an append of several calls undone after a later call failed
+cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows);
+
 // ---- pairs.cu
 cdb_status distance_pairs_device(int metric, int st, uint32_t dim, const uint8_t *d_x, const float *d_xm,
                                  const uint8_t *d_y, const float *d_ym, uint32_t row_pitch, uint64_t n,

@@ -1,0 +1,845 @@
+// sparse.cu -- the sparse inverted index (InvertedIndex, src/indexes/inverted/mod.rs) on the GPU: ingest, deletes, scoring
+// of posting lists (SparseAnnQueryBasic::sequential_search, src/models/sparse_ann_query.rs:68-147), the raw-value re-rank
+// (finalize_sparse_ann_results, inverted/mod.rs:331-381) and the values_upper_bound sampler (inverted/mod.rs:148-247).
+//
+// Layout (DESIGN.md section 8c).  Rows are kept as raw CSR on the device (dims u32, values f32, u64 row offsets).  Posting
+// lists are split into row tiles of 2^15 rows; a tile holds its distinct dims (ascending), one segment per dim and packed
+// u32 entries row_in_tile << 8 | key, sorted by key descending inside a segment.  An append rebuilds the last partial tile
+// and builds the new ones (CUB radix sort).  A search scores one (query, tile) per CTA into shared-memory u32 accumulators
+// plus a touched flag per row, selects the tile's top k*f touched rows exactly (radix select on (sim << 32) | ~id), merges
+// the tile lists, then sorts (and re-ranks) the survivors.
+#include <algorithm>
+#include <cmath>
+#include <mutex>
+#include <shared_mutex>
+#include <vector>
+
+#include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include "kernels.h"
+
+namespace cdb {
+namespace {
+
+constexpr uint32_t SP_TILE_SHIFT = 15;
+constexpr uint32_t SP_TILE = 1u << SP_TILE_SHIFT;
+constexpr int SP_THREADS = 512;
+constexpr uint32_t SP_QCHUNK = SP_THREADS;       // query pairs resolved per pass of the scoring kernel
+constexpr uint32_t SP_MAX_K = 1024;
+constexpr uint32_t SP_MAX_CAND = 5120;       // k * reranking_factor
+constexpr uint32_t SP_MERGE_KEYS = 25600;    // keys a merge CTA holds in shared memory (200 KB)
+constexpr uint32_t SP_MERGE_MAX_LISTS = 63;  // lists a merge CTA takes at once
+
+struct SpTile {
+    uint64_t entry_base;   // first entry of the tile in d_entries
+    uint64_t dim_base;     // first distinct dim in d_tdims; its segment starts are d_tseg[dim_base + tile ..]
+    uint32_t n_dims;
+    uint32_t pad;
+};
+
+// InvertedIndexNode::quantize (src/models/inverted_index.rs:168-172): an f32 divide then an f32 multiply (no FMA), clamp
+// keeps NaN, the saturating `as u8` sends NaN to 0
+__device__ inline uint32_t sparse_quantize(float v, float ub, uint32_t maxq) {
+    float x = __fmul_rn(__fdiv_rn(v, ub), (float)maxq);
+    const float m = (float)maxq;
+    if (x < 0.0f) x = 0.0f;
+    if (x > m) x = m;
+    const uint32_t q = (x != x) ? 0u : (uint32_t)x;
+    return q < maxq ? q : maxq;
+}
+
+// ---------------------------------------------------------------- build side
+__global__ void sp_tile_keys_kernel(const uint64_t *__restrict__ row_off, uint64_t r0, uint32_t nr, uint64_t p0,
+                                    const uint32_t *__restrict__ dims, const float *__restrict__ vals, float ub, uint32_t maxq,
+                                    uint64_t *__restrict__ sort_keys, uint32_t *__restrict__ sort_vals) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= nr) return;
+    const uint64_t b = row_off[r0 + warp], e = row_off[r0 + warp + 1];
+    for (uint64_t p = b + lane; p < e; p += 32) {
+        const uint32_t key = sparse_quantize(vals[p], ub, maxq);
+        sort_keys[p - p0] = ((uint64_t)dims[p] << 8) | (255u - key);
+        sort_vals[p - p0] = (warp << 8) | key;
+    }
+}
+
+__global__ void sp_seg_flags_kernel(const uint64_t *__restrict__ keys, uint32_t n, uint32_t *__restrict__ flags) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) flags[i] = (i == 0 || (keys[i] >> 8) != (keys[i - 1] >> 8)) ? 1u : 0u;
+}
+
+__global__ void sp_seg_scatter_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ flags,
+                                      const uint32_t *__restrict__ pos, uint32_t n, uint32_t *__restrict__ tdims,
+                                      uint32_t *__restrict__ tseg) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (flags[i]) {
+        tdims[pos[i] - 1] = (uint32_t)(keys[i] >> 8);
+        tseg[pos[i] - 1] = i;
+    }
+    if (i == n - 1) tseg[pos[i]] = n;
+}
+
+// ---------------------------------------------------------------- search side
+// Exact threshold of the top `need` keys among the non-zero keys key_at(0..n) (unique; more than `need` of them):
+// keys >= the result are exactly the top `need`.  8-bit radix passes from the top, stopping once a bucket is taken whole.
+template <class KeyAt>
+__device__ uint64_t sp_select_threshold(uint32_t n, uint32_t need, KeyAt key_at, uint32_t *hist, uint32_t *state) {
+    uint64_t prefix = 0;
+    const uint32_t tid = threadIdx.x, lane = tid & 31;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        for (uint32_t i = tid; i < 256; i += blockDim.x) hist[i] = 0;
+        __syncthreads();
+        const uint64_t hmask = shift == 56 ? 0ull : (~0ull << (shift + 8));
+        for (uint32_t i = tid; i < n; i += blockDim.x) {
+            const uint64_t k = key_at(i);
+            if (k && (k & hmask) == prefix) atomicAdd(&hist[(uint32_t)(k >> shift) & 255u], 1u);
+        }
+        __syncthreads();
+        if (tid < 32) {
+            uint32_t c[8], sum = 0;
+#pragma unroll
+            for (int s = 0; s < 8; ++s) { c[s] = hist[255 - 8 * lane - s]; sum += c[s]; }
+            uint32_t incl = sum;
+#pragma unroll
+            for (int off = 1; off < 32; off <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+                if (lane >= (uint32_t)off) incl += t;
+            }
+            const uint32_t excl = incl - sum;
+            if (excl < need && need <= incl) {
+                uint32_t acc = excl;
+                for (int s = 0; s < 8; ++s) {
+                    if (acc + c[s] >= need) { state[0] = 255 - 8 * lane - s; state[1] = need - acc; state[2] = c[s]; break; }
+                    acc += c[s];
+                }
+            }
+        }
+        __syncthreads();
+        const uint32_t d = state[0], rem = state[1], bc = state[2];
+        __syncthreads();
+        prefix |= (uint64_t)d << shift;
+        need = rem;
+        if (rem == bc) break;
+    }
+    return prefix;
+}
+
+struct SpSearch {
+    const uint32_t *entries, *tdims, *tseg, *deleted;
+    const SpTile *tiles;
+    uint64_t n_rows;
+    uint32_t id_base, maxq, etv, low;
+    float ub;
+    const uint64_t *q_off;
+    const uint32_t *q_dims;
+    const float *q_vals;
+    uint32_t q0;            // first query of the chunk
+    uint32_t m;             // candidates kept per query (k * factor)
+    uint32_t n_tiles;
+    uint64_t *out_keys;     // [chunk][n_tiles][m]
+    uint32_t *out_cnt;      // [chunk][n_tiles]
+};
+
+constexpr size_t SP_SCORE_SMEM = (size_t)SP_TILE * 4 + SP_TILE + SP_QCHUNK * 8 + (SP_QCHUNK + 1) * 8 + SP_QCHUNK * 4 + 260 * 4;
+
+__global__ void __launch_bounds__(SP_THREADS, 1) sp_score_tile_kernel(SpSearch a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint32_t *acc = reinterpret_cast<uint32_t *>(smem);
+    uint8_t *touched = smem + (size_t)SP_TILE * 4;
+    uint64_t *c_beg = reinterpret_cast<uint64_t *>(touched + SP_TILE);
+    uint64_t *c_pre = c_beg + SP_QCHUNK;
+    uint32_t *c_qv = reinterpret_cast<uint32_t *>(c_pre + SP_QCHUNK + 1);
+    uint32_t *hist = c_qv + SP_QCHUNK;   // 256 + state[4]
+    using Scan = cub::BlockScan<unsigned long long, SP_THREADS>;
+    __shared__ typename Scan::TempStorage scan_tmp;
+    __shared__ uint32_t s_cnt;
+
+    const uint32_t t = blockIdx.x, qi = blockIdx.y, q = a.q0 + qi, tid = threadIdx.x;
+    const SpTile tile = a.tiles[t];
+    const uint64_t row0 = (uint64_t)t << SP_TILE_SHIFT;
+    const uint32_t nr = (uint32_t)std::min<uint64_t>(SP_TILE, a.n_rows - row0);
+    uint4 *a4 = reinterpret_cast<uint4 *>(acc);
+    for (uint32_t i = tid; i < SP_TILE / 4; i += SP_THREADS) a4[i] = make_uint4(0, 0, 0, 0);
+    uint4 *t4 = reinterpret_cast<uint4 *>(touched);
+    for (uint32_t i = tid; i < SP_TILE / 16; i += SP_THREADS) t4[i] = make_uint4(0, 0, 0, 0);
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();   // an empty query reaches the touched scan below without passing another barrier
+
+    const uint32_t *tdims = a.tdims + tile.dim_base;
+    const uint32_t *tseg = a.tseg + tile.dim_base + t;
+    const uint32_t *ent = a.entries + tile.entry_base;
+    const uint64_t qb = a.q_off[q], qe = a.q_off[q + 1];
+    for (uint64_t j0 = qb; j0 < qe; j0 += SP_QCHUNK) {
+        const uint32_t nj = (uint32_t)std::min<uint64_t>(SP_QCHUNK, qe - j0);
+        unsigned long long len = 0;
+        if (tid < nj) {
+            const uint32_t d = a.q_dims[j0 + tid];
+            const uint32_t qv = sparse_quantize(a.q_vals[j0 + tid], a.ub, a.maxq);
+            uint32_t lo = 0, hi = tile.n_dims;        // first tile dim >= d
+            while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (tdims[mid] < d) lo = mid + 1; else hi = mid; }
+            uint32_t s = 0, e = 0;
+            if (lo < tile.n_dims && tdims[lo] == d) {
+                s = tseg[lo]; e = tseg[lo + 1];
+                if (!(qv > a.low)) {                  // keys etv..=max only: a prefix of the key-descending segment
+                    uint32_t l2 = s, h2 = e;
+                    while (l2 < h2) { const uint32_t mid = (l2 + h2) >> 1; if ((ent[mid] & 255u) >= a.etv) l2 = mid + 1; else h2 = mid; }
+                    e = l2;
+                }
+            }
+            c_beg[tid] = s;
+            c_qv[tid] = qv;
+            len = e - s;
+        }
+        unsigned long long pre;
+        Scan(scan_tmp).ExclusiveSum(len, pre);
+        if (tid < nj) c_pre[tid] = pre;
+        if (tid == nj - 1) c_pre[nj] = pre + len;
+        __syncthreads();
+        const unsigned long long total = c_pre[nj];
+        uint32_t j = 0;
+        for (unsigned long long i = tid; i < total; i += SP_THREADS) {
+            while (c_pre[j + 1] <= i) ++j;
+            const uint32_t e = __ldg(ent + c_beg[j] + (i - c_pre[j]));
+            const uint32_t r = e >> 8;
+            atomicAdd(&acc[r], c_qv[j] * (e & 255u));
+            touched[r] = 1;
+        }
+        __syncthreads();
+    }
+    // deleted rows are never candidates; count the rest
+    uint32_t mine = 0;
+    for (uint32_t r = tid; r < nr; r += SP_THREADS) {
+        if (!touched[r]) continue;
+        const uint64_t g = row0 + r;
+        if (a.deleted && (a.deleted[g >> 5] >> (g & 31)) & 1u) touched[r] = 0;
+        else ++mine;
+    }
+    mine = __reduce_add_sync(0xFFFFFFFFu, mine);
+    if ((tid & 31) == 0 && mine) atomicAdd(&s_cnt, mine);
+    __syncthreads();
+    const uint32_t nnz = s_cnt;
+    const uint32_t id0 = a.id_base + (uint32_t)row0;
+    auto key_at = [&](uint32_t r) -> uint64_t {
+        return touched[r] ? (((uint64_t)acc[r] << 32) | (uint64_t)(~(id0 + r))) : 0ull;
+    };
+    const uint64_t thr = nnz > a.m ? sp_select_threshold(nr, a.m, key_at, hist, hist + 256) : 1ull;
+    __syncthreads();
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    uint64_t *out = a.out_keys + ((size_t)qi * a.n_tiles + t) * a.m;
+    for (uint32_t r = tid; r < nr; r += SP_THREADS) {
+        const uint64_t k = key_at(r);
+        if (k && k >= thr) out[atomicAdd(&s_cnt, 1u)] = k;
+    }
+    __syncthreads();
+    if (tid == 0) a.out_cnt[(size_t)qi * a.n_tiles + t] = s_cnt;
+}
+
+// lists [q][n_in][m] -> [q][ceil(n_in / g)][m]: the top m of every group of g lists
+__global__ void __launch_bounds__(SP_THREADS, 1) sp_merge_kernel(const uint64_t *__restrict__ in_keys, const uint32_t *__restrict__ in_cnt,
+                                                                  uint32_t n_in, uint32_t g, uint32_t m, uint64_t *__restrict__ out_keys,
+                                                                  uint32_t *__restrict__ out_cnt) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint64_t *keys = reinterpret_cast<uint64_t *>(smem);
+    __shared__ uint32_t hist[260], s_off[SP_MERGE_MAX_LISTS + 1], s_cnt;
+    const uint32_t grp = blockIdx.x, qi = blockIdx.y, tid = threadIdx.x, n_out = gridDim.x;
+    const uint32_t l0 = grp * g, nl = min(g, n_in - l0);
+    if (tid == 0) {
+        uint32_t o = 0;
+        for (uint32_t l = 0; l < nl; ++l) { s_off[l] = o; o += in_cnt[(size_t)qi * n_in + l0 + l]; }
+        s_off[nl] = o;
+        s_cnt = 0;
+    }
+    __syncthreads();
+    for (uint32_t l = 0; l < nl; ++l) {
+        const uint64_t *src = in_keys + ((size_t)qi * n_in + l0 + l) * m;
+        for (uint32_t i = tid; i < s_off[l + 1] - s_off[l]; i += SP_THREADS) keys[s_off[l] + i] = src[i];
+    }
+    __syncthreads();
+    const uint32_t n = s_off[nl];
+    auto key_at = [&](uint32_t i) -> uint64_t { return keys[i]; };
+    const uint64_t thr = n > m ? sp_select_threshold(n, m, key_at, hist, hist + 256) : 1ull;
+    uint64_t *out = out_keys + ((size_t)qi * n_out + grp) * m;
+    for (uint32_t i = tid; i < n; i += SP_THREADS) {
+        const uint64_t k = keys[i];
+        if (k >= thr) out[atomicAdd(&s_cnt, 1u)] = k;
+    }
+    __syncthreads();
+    if (tid == 0) out_cnt[(size_t)qi * n_out + grp] = s_cnt;
+}
+
+// one list of <= m candidates per query -> the best k, best first.  rerank: finalize_sparse_ann_results -- for every
+// candidate dp = 0f32, dp += doc_val * q_val over the query pairs in the caller's order (a row's last pair of a dim wins),
+// then total_cmp order (NaN canonicalised), ties to the smaller id.  Otherwise the score is the u32 similarity as f32.
+__global__ void __launch_bounds__(SP_THREADS, 1) sp_finalize_kernel(const uint64_t *__restrict__ in_keys, const uint32_t *__restrict__ in_cnt,
+                                                                     uint32_t m, uint32_t k, int rerank, uint32_t q0,
+                                                                     const uint64_t *__restrict__ q_off, const uint32_t *__restrict__ q_dims,
+                                                                     const float *__restrict__ q_vals, const uint64_t *__restrict__ row_off,
+                                                                     const uint32_t *__restrict__ dims, const float *__restrict__ vals,
+                                                                     uint32_t id_base, uint32_t *__restrict__ out_ids,
+                                                                     float *__restrict__ out_scores, uint32_t *__restrict__ out_counts) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint64_t *keys = reinterpret_cast<uint64_t *>(smem);   // pow2ceil(m) keys
+    const uint32_t qi = blockIdx.x, q = q0 + qi, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t n = in_cnt[qi];
+    const uint64_t *src = in_keys + (size_t)qi * m;
+    uint32_t P = 1;
+    while (P < n) P <<= 1;
+    for (uint32_t i = tid; i < P; i += SP_THREADS) keys[i] = i < n ? src[i] : 0ull;
+    __syncthreads();
+    if (rerank) {
+        const uint64_t qb = q_off[q], qe = q_off[q + 1];
+        for (uint32_t c = warp; c < n; c += SP_THREADS / 32) {
+            const uint32_t id = ~(uint32_t)keys[c];
+            const uint64_t rb = row_off[id - id_base], re = row_off[id - id_base + 1];
+            float dp = 0.0f;
+            for (uint64_t j0 = qb; j0 < qe; j0 += 32) {
+                const uint32_t nj = (uint32_t)std::min<uint64_t>(32, qe - j0);
+                uint32_t qd = 0xFFFFFFFFu;
+                float qv = 0.0f, val = 0.0f;
+                bool found = false;
+                if (lane < nj) { qd = q_dims[j0 + lane]; qv = q_vals[j0 + lane]; }
+                for (uint64_t p0 = rb; p0 < re; p0 += 32) {
+                    const uint32_t np = (uint32_t)std::min<uint64_t>(32, re - p0);
+                    uint32_t rd = 0;
+                    float rv = 0.0f;
+                    if (lane < np) { rd = dims[p0 + lane]; rv = vals[p0 + lane]; }
+                    for (uint32_t l = 0; l < np; ++l) {
+                        const uint32_t d = __shfl_sync(0xFFFFFFFFu, rd, l);
+                        const float v = __shfl_sync(0xFFFFFFFFu, rv, l);
+                        if (lane < nj && d == qd) { val = v; found = true; }
+                    }
+                }
+                for (uint32_t l = 0; l < nj; ++l) {
+                    const bool f = __shfl_sync(0xFFFFFFFFu, found, l);
+                    const float x = __shfl_sync(0xFFFFFFFFu, val, l), y = __shfl_sync(0xFFFFFFFFu, qv, l);
+                    if (f) dp = __fadd_rn(dp, __fmul_rn(x, y));
+                }
+            }
+            if (lane == 0) keys[c] = ((uint64_t)order_key(CDB_METRIC_DOT_PRODUCT, __float_as_uint(canon_nan(dp))) << 32) | (uint64_t)(~id);
+        }
+        __syncthreads();
+    }
+    // bitonic sort, descending
+    for (uint32_t size = 2; size <= P; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            for (uint32_t i = tid; i < P / 2; i += SP_THREADS) {
+                const uint32_t lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+                const bool desc = (lo & size) == 0;
+                const uint64_t x = keys[lo], y = keys[hi];
+                if ((x < y) == desc) { keys[lo] = y; keys[hi] = x; }
+            }
+            __syncthreads();
+        }
+    }
+    const uint32_t cnt = min(n, k);
+    for (uint32_t i = tid; i < k; i += SP_THREADS) {
+        uint32_t id = CDB_INVALID_ID;
+        float s = 0.0f;
+        if (i < cnt) {
+            const uint64_t key = keys[i];
+            id = ~(uint32_t)key;
+            const uint32_t hi = (uint32_t)(key >> 32);
+            s = rerank ? __uint_as_float(key_to_bits(CDB_METRIC_DOT_PRODUCT, hi)) : __uint2float_rn(hi);
+        }
+        out_ids[(size_t)qi * k + i] = id;
+        out_scores[(size_t)qi * k + i] = s;
+    }
+    if (tid == 0) out_counts[qi] = cnt;
+}
+
+// sample_embedding: values > 1.0 ... > 9.0 (inverted/mod.rs:148-192)
+__global__ void sp_sample_kernel(const float *__restrict__ v, uint64_t n, unsigned long long *__restrict__ counts) {
+    uint32_t c[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const float x = __ldcs(v + i);
+#pragma unroll
+        for (int t = 0; t < 9; ++t) c[t] += x > (float)(t + 1);
+    }
+#pragma unroll
+    for (int t = 0; t < 9; ++t) {
+        const uint32_t s = __reduce_add_sync(0xFFFFFFFFu, c[t]);
+        if ((threadIdx.x & 31) == 0 && s) atomicAdd(&counts[t], (unsigned long long)s);
+    }
+}
+
+// Rust's `f32 as u32` / `as u8`: saturating, NaN -> 0
+uint32_t sat_u32(float x, uint32_t hi) {
+    if (!(x > 0.0f)) return 0;
+    if (x >= (float)hi) return hi;
+    return (uint32_t)x;
+}
+
+}  // namespace
+}  // namespace cdb
+
+using namespace cdb;
+
+struct cdb_sparse_index {
+    cdb_sparse_index_desc desc;
+    std::shared_mutex rw;
+    uint32_t maxq = 15;
+    uint64_t n_rows = 0, n_pairs = 0, n_deleted = 0;
+    std::vector<uint64_t> h_row_off{0};
+    std::vector<SpTile> h_tiles;
+    std::vector<uint32_t> h_deleted;
+    uint64_t *d_row_off = nullptr;
+    uint32_t *d_dims = nullptr, *d_entries = nullptr, *d_tdims = nullptr, *d_tseg = nullptr, *d_deleted = nullptr;
+    float *d_vals = nullptr;
+    SpTile *d_tiles = nullptr;
+    uint64_t max_tiles = 0;
+    int sms = 0;
+    ~cdb_sparse_index() {
+        for (void *p : {(void *)d_row_off, (void *)d_dims, (void *)d_entries, (void *)d_tdims, (void *)d_tseg, (void *)d_deleted,
+                        (void *)d_vals, (void *)d_tiles})
+            if (p) cudaFree(p);
+    }
+};
+
+#define SP_REQUIRE(cond, msg)                                              \
+    do {                                                                   \
+        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; }        \
+    } while (0)
+
+namespace {
+
+// CUB temp storage + sort buffers of one append, sized for its largest tile
+struct BuildBufs {
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    uint64_t *keys_in = nullptr, *keys_out = nullptr;
+    uint32_t *vals_in = nullptr, *flags = nullptr, *pos = nullptr;
+    ~BuildBufs() {
+        for (void *p : {tmp, (void *)keys_in, (void *)keys_out, (void *)vals_in, (void *)flags, (void *)pos})
+            if (p) cudaFree(p);
+    }
+};
+
+// posting lists of tile t (rows [t*TILE, min(n_rows, (t+1)*TILE))) appended after the tiles below it
+cdb_status build_tile(cdb_sparse_index *ix, uint64_t t, BuildBufs &b, cudaStream_t s) {
+    const uint64_t r0 = t << SP_TILE_SHIFT, r1 = std::min<uint64_t>(ix->n_rows, r0 + SP_TILE);
+    const uint64_t p0 = ix->h_row_off[r0], p1 = ix->h_row_off[r1];
+    const uint32_t np = (uint32_t)(p1 - p0);
+    SpTile tile;
+    tile.entry_base = p0;   // a tile's entries are its rows' pairs, re-ordered
+    tile.dim_base = t ? ix->h_tiles[t - 1].dim_base + ix->h_tiles[t - 1].n_dims : 0;
+    tile.n_dims = 0;
+    tile.pad = 0;
+    uint32_t *tseg = ix->d_tseg + tile.dim_base + t;
+    if (np == 0) {
+        CDB_CUDA_TRY(cudaMemsetAsync(tseg, 0, 4, s));
+    } else {
+        const uint32_t nr = (uint32_t)(r1 - r0);
+        sp_tile_keys_kernel<<<(nr * 32 + 255) / 256, 256, 0, s>>>(ix->d_row_off, r0, nr, p0, ix->d_dims, ix->d_vals,
+                                                                   ix->desc.values_upper_bound, ix->maxq, b.keys_in, b.vals_in);
+        CDB_LAUNCH_CHECK();
+        size_t tb = b.tmp_bytes;
+        CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tb, b.keys_in, b.keys_out, b.vals_in, ix->d_entries + tile.entry_base,
+                                                     (int)np, 0, 40, s));
+        sp_seg_flags_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, np, b.flags);
+        CDB_LAUNCH_CHECK();
+        tb = b.tmp_bytes;
+        CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(b.tmp, tb, b.flags, b.pos, (int)np, s));
+        sp_seg_scatter_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, b.flags, b.pos, np, ix->d_tdims + tile.dim_base, tseg);
+        CDB_LAUNCH_CHECK();
+        CDB_CUDA_TRY(cudaMemcpyAsync(&tile.n_dims, b.pos + np - 1, 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaStreamSynchronize(s));
+    }
+    ix->h_tiles.push_back(tile);
+    return CDB_OK;
+}
+
+cdb_status alloc_build_bufs(BuildBufs &b, uint64_t max_np, cudaStream_t s) {
+    if (!max_np) return CDB_OK;
+    CDB_CUDA_TRY(cudaMalloc(&b.keys_in, max_np * 8));
+    CDB_CUDA_TRY(cudaMalloc(&b.keys_out, max_np * 8));
+    CDB_CUDA_TRY(cudaMalloc(&b.vals_in, max_np * 4));
+    CDB_CUDA_TRY(cudaMalloc(&b.flags, max_np * 4));
+    CDB_CUDA_TRY(cudaMalloc(&b.pos, max_np * 4));
+    size_t t_sort = 0, t_scan = 0;
+    CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, b.keys_in, b.keys_out, b.vals_in, b.vals_in, (int)max_np, 0, 40, s));
+    CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, t_scan, b.flags, b.pos, (int)max_np, s));
+    b.tmp_bytes = std::max(t_sort, t_scan);
+    CDB_CUDA_TRY(cudaMalloc(&b.tmp, b.tmp_bytes));
+    return CDB_OK;
+}
+
+// tiles [t0, t1) of the current rows, host and device tables
+cdb_status build_tiles(cdb_sparse_index *ix, uint64_t t0, uint64_t t1, BuildBufs &b, cudaStream_t s) {
+    ix->h_tiles.resize(t0);
+    cdb_status rc;
+    for (uint64_t t = t0; t < t1; ++t)
+        if ((rc = build_tile(ix, t, b, s))) return rc;
+    if (t1 > t0)
+        CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_tiles + t0, ix->h_tiles.data() + t0, (t1 - t0) * sizeof(SpTile), cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaStreamSynchronize(s));
+    return CDB_OK;
+}
+
+// back to the first `rows` rows (rows <= n_rows): their pairs are still in place, the tile holding row `rows` is rebuilt and
+// tombstones of the dropped rows are cleared.  b must fit that tile.  Device work is ordered by the caller.
+cdb_status restore_rows(cdb_sparse_index *ix, uint64_t rows, BuildBufs &b, cudaStream_t s) {
+    ix->h_row_off.resize(rows + 1);
+    ix->n_rows = rows;
+    ix->n_pairs = ix->h_row_off[rows];
+    for (uint64_t w = rows >> 5; w < ix->h_deleted.size(); ++w) {
+        const uint32_t keep = w == (rows >> 5) ? (uint32_t)((1ull << (rows & 31)) - 1) : 0u;
+        ix->n_deleted -= __builtin_popcount(ix->h_deleted[w] & ~keep);
+        ix->h_deleted[w] &= keep;
+    }
+    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_deleted, ix->h_deleted.data(), ix->h_deleted.size() * 4, cudaMemcpyHostToDevice, s));
+    return build_tiles(ix, rows >> SP_TILE_SHIFT, (rows + SP_TILE - 1) >> SP_TILE_SHIFT, b, s);
+}
+
+struct StreamGuard {
+    cudaStream_t s = nullptr;
+    ~StreamGuard() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
+};
+
+cdb_status check_search_params(const cdb_sparse_search_params *p, uint32_t *m) {
+    SP_REQUIRE(p, "null params");
+    SP_REQUIRE(p->k >= 1 && p->k <= SP_MAX_K, "k must be in 1..1024");
+    const uint64_t f = p->rerank ? p->reranking_factor : 1;
+    SP_REQUIRE(f >= 1 && (uint64_t)p->k * f <= SP_MAX_CAND, "k * reranking_factor must be in 1..5120");
+    *m = (uint32_t)(p->k * f);
+    return CDB_OK;
+}
+
+// the search on device buffers, under the reader lock
+cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
+                         const cdb_sparse_search_params *p, uint32_t m, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                         cudaStream_t s) {
+    if (!nq) return CDB_OK;
+    const uint32_t k = p->k;
+    const uint32_t n_tiles = (uint32_t)ix->h_tiles.size();
+    const uint32_t bits = ix->desc.quantization_bits;
+    // sequential_search, sparse_ann_query.rs:80-83
+    const float thr = p->early_terminate_threshold;
+    const float prod = (float)(1u << bits) * thr;
+    const float etv_f = std::isnan(prod) ? 255.0f : std::min(prod, 255.0f);
+    const uint32_t etv = sat_u32(etv_f, 255), low = sat_u32(thr * (float)(1u << bits), 0xFFFFFFFFu);
+    if (n_tiles == 0) {
+        CDB_CUDA_TRY(cudaMemsetAsync(d_ids, 0xFF, (size_t)nq * k * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d_scores, 0, (size_t)nq * k * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
+        return CDB_OK;
+    }
+    const uint32_t g = std::min<uint32_t>(SP_MERGE_MAX_LISTS, std::max<uint32_t>(2, SP_MERGE_KEYS / m));
+    const uint32_t n_lvl1 = (n_tiles + g - 1) / g;
+    uint32_t sort_cap = 1;
+    while (sort_cap < m) sort_cap <<= 1;
+    const size_t per_q = ((size_t)n_tiles + n_lvl1) * m * 8 + ((size_t)n_tiles + n_lvl1) * 4;
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, (512ull << 20) / per_q}));
+    uint64_t *ka = nullptr, *kb = nullptr;
+    uint32_t *ca = nullptr, *cb = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&ka, (size_t)chunk * n_tiles * m * 8, s));
+    cudaError_t e = cudaMallocAsync(&kb, (size_t)chunk * n_lvl1 * m * 8, s);
+    if (e == cudaSuccess) e = cudaMallocAsync(&ca, (size_t)chunk * n_tiles * 4, s);
+    if (e == cudaSuccess) e = cudaMallocAsync(&cb, (size_t)chunk * n_lvl1 * 4, s);
+    cdb_status rc = CDB_OK;
+    if (e != cudaSuccess) { set_error(std::string("cudaMallocAsync: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    if (!rc) {
+        if ((e = allow_max_dynamic_smem((const void *)sp_score_tile_kernel)) != cudaSuccess ||
+            (e = allow_max_dynamic_smem((const void *)sp_merge_kernel)) != cudaSuccess ||
+            (e = allow_max_dynamic_smem((const void *)sp_finalize_kernel)) != cudaSuccess) {
+            set_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e));
+            rc = CDB_CUDA_ERROR;
+        }
+    }
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        SpSearch a;
+        a.entries = ix->d_entries; a.tdims = ix->d_tdims; a.tseg = ix->d_tseg; a.deleted = ix->n_deleted ? ix->d_deleted : nullptr;
+        a.tiles = ix->d_tiles; a.n_rows = ix->n_rows; a.id_base = ix->desc.id_base; a.maxq = ix->maxq; a.etv = etv; a.low = low;
+        a.ub = ix->desc.values_upper_bound; a.q_off = d_qoff; a.q_dims = d_qdims; a.q_vals = d_qvals; a.q0 = q0; a.m = m;
+        a.n_tiles = n_tiles; a.out_keys = ka; a.out_cnt = ca;
+        sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(a);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
+        uint64_t *cur = ka, *nxt = kb;
+        uint32_t *ccur = ca, *cnxt = cb, n_lists = n_tiles;
+        while (n_lists > 1) {
+            const uint32_t n_out = (n_lists + g - 1) / g;
+            const uint32_t held = std::min<uint32_t>(g, n_lists) * m;
+            sp_merge_kernel<<<dim3(n_out, c), SP_THREADS, (size_t)held * 8, s>>>(cur, ccur, n_lists, g, m, nxt, cnxt);
+            g_launch_count.fetch_add(1, std::memory_order_relaxed);
+            if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
+            std::swap(cur, nxt);
+            std::swap(ccur, cnxt);
+            n_lists = n_out;
+        }
+        if (rc) break;
+        sp_finalize_kernel<<<c, SP_THREADS, (size_t)sort_cap * 8, s>>>(cur, ccur, m, k, p->rerank ? 1 : 0, q0, d_qoff, d_qdims, d_qvals, ix->d_row_off,
+                                                    ix->d_dims, ix->d_vals, ix->desc.id_base, d_ids + (size_t)q0 * k,
+                                                    d_scores + (size_t)q0 * k, d_counts + q0);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    for (void *ptr : {(void *)ka, (void *)kb, (void *)ca, (void *)cb})
+        if (ptr) cudaFreeAsync(ptr, s);
+    return rc;
+}
+
+// the query CSR the caller passed (host): offsets start at 0 and never decrease
+cdb_status check_csr(const uint64_t *off, uint64_t n, const char *what) {
+    SP_REQUIRE(off, "null offsets");
+    if (off[0] != 0) { set_error(std::string(what) + ": offsets[0] must be 0"); return CDB_INVALID_PARAMS; }
+    for (uint64_t i = 0; i < n; ++i)
+        if (off[i + 1] < off[i]) { set_error(std::string(what) + ": offsets decrease"); return CDB_INVALID_PARAMS; }
+    return CDB_OK;
+}
+
+}  // namespace
+
+namespace cdb {
+cdb_status sparse_index_room(cdb_sparse_index *ix, uint64_t *rows, uint64_t *rows_left, uint64_t *pairs_left) {
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    *rows = ix->n_rows;
+    *rows_left = ix->desc.capacity_rows - ix->n_rows;
+    *pairs_left = ix->desc.capacity_pairs - ix->n_pairs;
+    return CDB_OK;
+}
+
+cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows) {
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    SP_REQUIRE(rows <= ix->n_rows, "truncate beyond the index");
+    if (rows == ix->n_rows) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    const uint64_t r0 = rows & ~(uint64_t)(SP_TILE - 1);
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    BuildBufs b;
+    cdb_status rc = alloc_build_bufs(b, ix->h_row_off[rows] - ix->h_row_off[r0], sg.s);
+    if (rc) return rc;
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    return restore_rows(ix, rows, b, sg.s);
+}
+}  // namespace cdb
+
+extern "C" {
+
+cdb_status cdb_sparse_index_create(const cdb_sparse_index_desc *desc, cdb_sparse_index **out) {
+    SP_REQUIRE(desc && out, "null argument");
+    SP_REQUIRE(desc->quantization_bits >= 4 && desc->quantization_bits <= 8, "quantization_bits must be in 4..8");
+    SP_REQUIRE(desc->capacity_rows >= 1 && (uint64_t)desc->id_base + desc->capacity_rows <= 0xFFFFFFFFull,
+               "capacity_rows must be >= 1 and id_base + capacity_rows <= 2^32 - 1");
+    SP_REQUIRE(desc->capacity_pairs < (1ull << 40), "capacity_pairs too large");
+    *out = nullptr;
+    CDB_CUDA_TRY(cudaSetDevice(desc->device));
+    std::unique_ptr<cdb_sparse_index> ix(new cdb_sparse_index());
+    ix->desc = *desc;
+    ix->maxq = (1u << desc->quantization_bits) - 1;
+    ix->max_tiles = (desc->capacity_rows + SP_TILE - 1) / SP_TILE;
+    const size_t pairs = std::max<uint64_t>(1, desc->capacity_pairs);
+    const size_t words = (desc->capacity_rows + 31) / 32;
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&ix->sms, cudaDevAttrMultiProcessorCount, desc->device));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_row_off, (desc->capacity_rows + 1) * 8));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_dims, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_vals, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_entries, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_tdims, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_tseg, (pairs + ix->max_tiles) * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_deleted, words * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_tiles, ix->max_tiles * sizeof(SpTile)));
+    CDB_CUDA_TRY(cudaMemset(ix->d_row_off, 0, 8));
+    CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
+    ix->h_deleted.assign(words, 0u);
+    *out = ix.release();
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_index_destroy(cdb_sparse_index *ix) {
+    if (!ix) return CDB_OK;
+    cudaSetDevice(ix->desc.device);
+    cudaDeviceSynchronize();
+    delete ix;
+    return CDB_OK;
+}
+
+uint64_t cdb_sparse_index_size(const cdb_sparse_index *ix) { return ix ? ix->n_rows : 0; }
+
+cdb_status cdb_sparse_index_append(cdb_sparse_index *ix, const uint64_t *row_offsets, const uint32_t *dims, const float *values,
+                                   uint64_t n) {
+    SP_REQUIRE(ix, "null index");
+    if (!n) return CDB_OK;
+    cdb_status rc = check_csr(row_offsets, n, "row_offsets");
+    if (rc) return rc;
+    const uint64_t np = row_offsets[n];
+    SP_REQUIRE((dims && values) || !np, "null pairs");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    SP_REQUIRE(ix->n_rows + n <= ix->desc.capacity_rows, "append exceeds capacity_rows");
+    SP_REQUIRE(ix->n_pairs + np <= ix->desc.capacity_pairs, "append exceeds capacity_pairs");
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    // every check and allocation precedes the first change
+    const uint64_t r_old = ix->n_rows, p_old = ix->n_pairs, r_new = r_old + n;
+    std::vector<uint64_t> off(n);
+    for (uint64_t i = 0; i < n; ++i) off[i] = p_old + row_offsets[i + 1];
+    auto row_off = [&](uint64_t r) { return r <= r_old ? ix->h_row_off[r] : off[r - r_old - 1]; };
+    const uint64_t t0 = r_old >> SP_TILE_SHIFT, t1 = (r_new + SP_TILE - 1) >> SP_TILE_SHIFT;
+    uint64_t max_np = 0;
+    for (uint64_t t = t0; t < t1; ++t)
+        max_np = std::max(max_np, row_off(std::min<uint64_t>(r_new, (t + 1) << SP_TILE_SHIFT)) - row_off(t << SP_TILE_SHIFT));
+    SP_REQUIRE(max_np < (1ull << 31), "a row tile holds 2^31 pairs or more");
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    BuildBufs b;
+    if ((rc = alloc_build_bufs(b, max_np, s))) return rc;
+    // searches already enqueued on other streams (cdb_sparse_search_batch_device) read the tile this call rebuilds
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    cudaError_t e = cudaSuccess;
+    if (np) {
+        e = cudaMemcpyAsync(ix->d_dims + p_old, dims, np * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_vals + p_old, values, np * 4, cudaMemcpyHostToDevice, s);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_row_off + r_old + 1, off.data(), n * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error(std::string("sparse append: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    ix->h_row_off.insert(ix->h_row_off.end(), off.begin(), off.end());
+    ix->n_rows = r_new;
+    ix->n_pairs += np;
+    // rebuild the last partial tile, build the new ones; on failure the index goes back to its r_old rows
+    if ((rc = build_tiles(ix, t0, t1, b, s))) {
+        const std::string msg = cdb_last_error_string();
+        restore_rows(ix, r_old, b, s);
+        set_error(msg);
+    }
+    return rc;
+}
+
+cdb_status cdb_sparse_index_delete_rows(cdb_sparse_index *ix, const uint32_t *rows, uint64_t n) {
+    SP_REQUIRE(ix && (rows || !n), "null argument");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    for (uint64_t i = 0; i < n; ++i) SP_REQUIRE(rows[i] < ix->n_rows, "row out of range");
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    if (!n) return CDB_OK;
+    std::vector<uint32_t> w = ix->h_deleted;
+    uint64_t added = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        uint32_t &x = w[rows[i] >> 5];
+        const uint32_t bit = 1u << (rows[i] & 31);
+        if (!(x & bit)) { x |= bit; ++added; }
+    }
+    // searches enqueued before this call finish first (they read the bitmap)
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
+    ix->h_deleted.swap(w);
+    ix->n_deleted += added;
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_index_deleted_rows(const cdb_sparse_index *ix, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total) {
+    SP_REQUIRE(ix && (out || !n), "null argument");
+    SP_REQUIRE(first + n <= ix->desc.capacity_rows, "first + n exceeds capacity_rows");
+    std::shared_lock<std::shared_mutex> lock(const_cast<cdb_sparse_index *>(ix)->rw);
+    for (uint64_t i = 0; i < n; ++i) out[i] = (ix->h_deleted[(first + i) >> 5] >> ((first + i) & 31)) & 1u;
+    if (out_total) *out_total = ix->n_deleted;
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_search_batch_device(cdb_sparse_index *ix, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
+                                          const float *d_q_values, uint32_t nq, const cdb_sparse_search_params *p,
+                                          uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream) {
+    SP_REQUIRE(ix && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
+    uint32_t m = 0;
+    cdb_status rc = check_search_params(p, &m);
+    if (rc) return rc;
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    return search_locked(ix, d_q_offsets, d_q_dims, d_q_values, nq, p, m, d_ids, d_scores, d_counts, (cudaStream_t)stream);
+}
+
+cdb_status cdb_sparse_search_batch(cdb_sparse_index *ix, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
+                                   uint32_t nq, const cdb_sparse_search_params *p, uint32_t *out_ids, float *out_scores,
+                                   uint32_t *out_counts) {
+    SP_REQUIRE(ix && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    uint32_t m = 0;
+    cdb_status rc = check_search_params(p, &m);
+    if (rc) return rc;
+    if (!nq) return CDB_OK;
+    if ((rc = check_csr(q_offsets, nq, "q_offsets"))) return rc;
+    const uint64_t nqp = q_offsets[nq];
+    SP_REQUIRE((q_dims && q_values) || !nqp, "null query pairs");
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    const size_t k = p->k;
+    const size_t bytes = (nq + 1) * 8 + nqp * 8 + (size_t)nq * k * 8 + (size_t)nq * 4;
+    uint8_t *buf = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
+    uint64_t *d_off = reinterpret_cast<uint64_t *>(buf);
+    uint32_t *d_ids = reinterpret_cast<uint32_t *>(d_off + nq + 1);
+    float *d_scores = reinterpret_cast<float *>(d_ids + (size_t)nq * k);
+    uint32_t *d_counts = reinterpret_cast<uint32_t *>(d_scores + (size_t)nq * k);
+    uint32_t *d_qd = d_counts + nq;
+    float *d_qv = reinterpret_cast<float *>(d_qd + nqp);
+    cudaError_t e = cudaMemcpyAsync(d_off, q_offsets, (nq + 1) * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && nqp) e = cudaMemcpyAsync(d_qd, q_dims, nqp * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && nqp) e = cudaMemcpyAsync(d_qv, q_values, nqp * 4, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) { set_error(std::string("cudaMemcpyAsync: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    if (!rc) rc = search_locked(ix, d_off, d_qd, d_qv, nq, p, m, d_ids, d_scores, d_counts, s);
+    if (!rc) {
+        e = cudaMemcpyAsync(out_ids, d_ids, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, d_scores, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out_counts, d_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) { set_error(std::string("sparse search: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    cudaFreeAsync(buf, s);
+    return rc;
+}
+
+cdb_status cdb_sparse_sample_upper_bound(int32_t device, const float *values, uint64_t n, float clamp_margin_percent,
+                                         const uint64_t *prior_counts, uint64_t prior_values, uint64_t *out_counts, float *out_ub) {
+    SP_REQUIRE((values || !n) && (out_counts || out_ub), "bad arguments");
+    CDB_CUDA_TRY(cudaSetDevice(device));
+    int sms = 0;
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    const uint64_t chunk = 16ull << 20;
+    float *d_in = nullptr;
+    unsigned long long *d_c = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&d_c, 9 * 8, s));
+    cdb_status rc = CDB_OK;
+    cudaError_t e = cudaMemsetAsync(d_c, 0, 9 * 8, s);
+    if (e == cudaSuccess) e = cudaMallocAsync(&d_in, std::min(std::max<uint64_t>(n, 1), chunk) * 4, s);
+    for (uint64_t off = 0; off < n && e == cudaSuccess; off += chunk) {
+        const uint64_t m = std::min(chunk, n - off);
+        e = cudaMemcpyAsync(d_in, values + off, m * 4, cudaMemcpyHostToDevice, s);
+        if (e != cudaSuccess) break;
+        const uint32_t grid = (uint32_t)std::min<uint64_t>((m + 255) / 256, (uint64_t)sms * 8);
+        sp_sample_kernel<<<grid, 256, 0, s>>>(d_in, m, d_c);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        e = cudaGetLastError();
+    }
+    uint64_t c[9];
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c, d_c, sizeof(c), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (d_in) cudaFreeAsync(d_in, s);
+    cudaFreeAsync(d_c, s);
+    if (e != cudaSuccess) { set_error(std::string("sparse sampling: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    for (int i = 0; i < 9; ++i) {
+        if (prior_counts) c[i] += prior_counts[i];
+        if (out_counts) out_counts[i] = c[i];
+    }
+    // finalize_sampling (inverted/mod.rs:194-247): (count as f32 / values_collected as f32) * 100.0, first t with
+    // pct <= clamp_margin_percent, else 10.0 (also when no value was sampled: 0/0 is NaN)
+    if (out_ub) {
+        const float vc = (float)(n + (prior_counts ? prior_values : 0));
+        float ub = 10.0f;
+        for (int i = 0; i < 9; ++i) {
+            volatile float r = (float)c[i] / vc;
+            if (r * 100.0f <= clamp_margin_percent) { ub = (float)(i + 1); break; }
+        }
+        *out_ub = ub;
+    }
+    return rc;
+}
+
+}  // extern "C"

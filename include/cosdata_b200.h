@@ -646,6 +646,79 @@ cdb_status cdb_index_stats_ex(const cdb_index *index, uint64_t *out, uint32_t n)
 /* candidates the prefilter emitted for each of the first n queries of the last prefilter search */
 cdb_status cdb_index_last_candidate_counts(const cdb_index *index, uint32_t n, uint32_t *out);
 
+/* ------------------------------------------------ sparse inverted index
+ * InvertedIndex (src/indexes/inverted/mod.rs): SPLADE-style sparse vectors, a list of (dim u32, value f32) pairs per row.
+ * Rows are CSR: row r holds pairs [row_offsets[r], row_offsets[r+1]) and has id id_base + r.  Every pair is indexed under
+ * key = quantize(value) = (((value / values_upper_bound) * max).clamp(0, max) as u8).min(max), max = 2^bits - 1, zero and
+ * duplicate pairs included (inverted_index.rs:168-172).  Empty rows are allowed and never candidates.
+ * A search is SparseAnnQueryBasic::sequential_search (sparse_ann_query.rs:68-147): every query pair whose dim has a list
+ * adds qv * key (u32, wrapping) to each live row of the visited keys (all keys when qv > low, else keys >= etv, with
+ * etv = ((2^bits * thr).min(255.0)) as u8 and low = (thr * 2^bits) as u32); a row is a candidate once any visited list holds
+ * it.  The best k * f candidates are kept (higher similarity, then smaller id; f = reranking_factor when rerank, else 1).
+ *   rerank = 0: out_scores = similarity as f32, best first.
+ *   rerank = 1: finalize_sparse_ann_results (inverted/mod.rs:331-381) -- dp = 0f32; dp += row_value * query_value over the
+ *               query pairs in the caller's order (a row's last pair of a dim wins, dims the row lacks are skipped), sorted
+ *               by total_cmp (NaN canonicalised to the sign-set quiet NaN), ties to the smaller id, truncated to k.
+ * out_counts[q] = min(k, candidates); unused slots hold CDB_INVALID_ID / 0.  k must be 1..1024 and k * f <= 5120
+ * (CDB_INVALID_PARAMS otherwise, nothing truncated).  Searches on one handle are re-entrant; append and delete take the
+ * handle exclusively and first wait for the searches already enqueued on the device.  An append that fails changes nothing.  Deleted rows (a tombstone per row, as mark_embedding_as_deleted with the inserted pairs leaves it)
+ * are never candidates; rows are not reused.  Without a CUDA device every compute entry point returns CDB_CUDA_ERROR. */
+typedef struct cdb_sparse_index cdb_sparse_index; /* opaque */
+
+typedef struct {
+    int32_t device;
+    uint32_t quantization_bits;   /* 4..8 (QuantizationBits, src/api/vectordb/indexes/dtos.rs:18-25; default 4) */
+    float values_upper_bound;     /* InvertedIndex.values_upper_bound (1.0 before sampling) */
+    uint64_t capacity_rows;       /* id_base + capacity_rows <= 2^32 - 1 */
+    uint64_t capacity_pairs;      /* (dim, value) pairs over all rows */
+    uint32_t id_base;
+} cdb_sparse_index_desc;
+
+typedef struct {
+    uint32_t k;                        /* top_k (Some); the reference's None is not supported */
+    float early_terminate_threshold;   /* the request's value, else config.search.early_terminate_threshold (0.0) */
+    int32_t rerank;                    /* config.rerank_sparse_with_raw_values (default 0) */
+    uint32_t reranking_factor;         /* config.sparse_raw_values_reranking_factor (default 5), used when rerank */
+} cdb_sparse_search_params;
+
+cdb_status cdb_sparse_index_create(const cdb_sparse_index_desc *desc, cdb_sparse_index **out);
+cdb_status cdb_sparse_index_destroy(cdb_sparse_index *index);
+uint64_t cdb_sparse_index_size(const cdb_sparse_index *index);
+/* n rows; row_offsets[n+1] (row_offsets[0] = 0), dims / values [row_offsets[n]] */
+cdb_status cdb_sparse_index_append(cdb_sparse_index *index, const uint64_t *row_offsets, const uint32_t *dims, const float *values,
+                                   uint64_t n);
+/* tombstones rows[0..n) (local rows < cdb_sparse_index_size; deleting a row twice is a no-op) */
+cdb_status cdb_sparse_index_delete_rows(cdb_sparse_index *index, const uint32_t *rows, uint64_t n);
+/* out[i] = 1 if row first+i is deleted (first + n <= capacity_rows); *out_total = deleted rows (either may be NULL) */
+cdb_status cdb_sparse_index_deleted_rows(const cdb_sparse_index *index, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total);
+/* B queries as CSR (q_offsets[B+1]); out_ids / out_scores [B][k], out_counts [B] */
+cdb_status cdb_sparse_search_batch(cdb_sparse_index *index, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
+                                   uint32_t n_queries, const cdb_sparse_search_params *params, uint32_t *out_ids, float *out_scores,
+                                   uint32_t *out_counts);
+/* same with every array in DEVICE memory on the index's device, asynchronous on `stream` (NULL = the legacy default stream) */
+cdb_status cdb_sparse_search_batch_device(cdb_sparse_index *index, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
+                                          const float *d_q_values, uint32_t n_queries, const cdb_sparse_search_params *params,
+                                          uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream);
+/* InvertedIndex::sample_embedding + finalize_sampling (inverted/mod.rs:148-247) over n pair values:
+ *   out_counts[t-1] = #values > t for t = 1..9 (prior_counts, may be NULL, added first; prior_values = values they cover)
+ *   out_ub = first t with (count as f32 / values as f32) * 100.0 <= clamp_margin_percent, else 10.0 (also with no values) */
+cdb_status cdb_sparse_sample_upper_bound(int32_t device, const float *values, uint64_t n, float clamp_margin_percent,
+                                         const uint64_t *prior_counts, uint64_t prior_values, uint64_t *out_counts, float *out_ub);
+/* the itoe store's live embeddings that have sparse values, in ascending internal-id order (metadata fields are parsed past,
+ * raw_vector_embedding.rs:34-64, 91-132).  Host-side readers, no GPU work.
+ *   scan -> number of such embeddings, their pairs in total, the largest internal id
+ *   load -> entries [first_entry, first_entry + max_entries): internal ids, row_offsets[read+1] (starting at 0), dims and
+ *           values (at most max_pairs pairs, else CDB_INVALID_PARAMS)
+ *   cdb_sparse_index_append_itoe -> cdb_sparse_index_append of every such embedding; out_internal_ids[r] = the internal id of
+ *           appended row r (the first max_ids of them).  The cold start of a collection's sparse index: the caller sets
+ *           values_upper_bound to what LMDB holds. */
+cdb_status cdb_itoe_scan_sparse(const char *collection_dir, uint64_t *out_entries, uint64_t *out_pairs, uint64_t *out_max_internal_id);
+cdb_status cdb_itoe_load_sparse(const char *collection_dir, uint64_t first_entry, uint64_t max_entries, uint64_t max_pairs,
+                                uint32_t *out_internal_ids, uint64_t *out_row_offsets, uint32_t *out_dims, float *out_values,
+                                uint64_t *out_read);
+cdb_status cdb_sparse_index_append_itoe(cdb_sparse_index *index, const char *collection_dir, uint32_t *out_internal_ids,
+                                        uint64_t max_ids, uint64_t *out_appended);
+
 #ifdef __cplusplus
 }
 #endif
