@@ -133,6 +133,15 @@ class SparseSearchParams(C.Structure):
     ]
 
 
+class TfIdfIndexDesc(C.Structure):
+    _fields_ = [
+        ("device", C.c_int32),
+        ("capacity_rows", C.c_uint64),
+        ("capacity_pairs", C.c_uint64),
+        ("id_base", C.c_uint32),
+    ]
+
+
 # symbol -> (restype, argtypes); must list every function of include/cosdata_b200.h
 PROTOTYPES = {
     "cdb_abi_version": (C.c_int32, []),
@@ -230,6 +239,16 @@ PROTOTYPES = {
     "cdb_itoe_load_sparse": (C.c_int32, [C.c_char_p, C.c_uint64, C.c_uint64, C.c_uint64, c_u32p, c_vp, c_u32p, c_f32p,
                                          C.POINTER(C.c_uint64)]),
     "cdb_sparse_index_append_itoe": (C.c_int32, [C.c_void_p, C.c_char_p, c_u32p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "cdb_tfidf_index_create": (C.c_int32, [C.POINTER(TfIdfIndexDesc), C.POINTER(C.c_void_p)]),
+    "cdb_tfidf_index_destroy": (C.c_int32, [C.c_void_p]),
+    "cdb_tfidf_index_size": (C.c_uint64, [C.c_void_p]),
+    "cdb_tfidf_index_append": (C.c_int32, [C.c_void_p, c_vp, c_u32p, c_f32p, c_u8p, C.c_uint64, C.c_uint32]),
+    "cdb_tfidf_index_delete_rows": (C.c_int32, [C.c_void_p, c_u32p, C.c_uint64, C.c_uint32]),
+    "cdb_tfidf_index_deleted_rows": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, c_u8p, C.POINTER(C.c_uint64)]),
+    "cdb_tfidf_index_term_stats": (C.c_int32, [C.c_void_p, c_u32p, C.c_uint64, c_u32p, c_f32p, C.POINTER(C.c_uint32)]),
+    "cdb_tfidf_search_batch": (C.c_int32, [C.c_void_p, c_vp, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p]),
+    "cdb_tfidf_search_batch_device": (C.c_int32, [C.c_void_p, c_vp, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p,
+                                                  C.c_void_p]),
 }
 
 _lib = None

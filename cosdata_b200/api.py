@@ -948,3 +948,126 @@ def itoe_load_sparse(collection_dir):
     _check(_lib.load().cdb_itoe_load_sparse(os.fsencode(collection_dir), 0, n, p, _ptr(ids), _ptr(off), _ptr(dims), _ptr(vals),
                                             C.byref(got)))
     return ids[:n], (off, dims[:p], vals[:p])
+
+
+# ---------------------------------------------------------------- TF-IDF / BM25 index (TFIDFIndex)
+def _u_to_f32(x):
+    """Rust's `u32 as f32` / `u64 as f32` on an array: round to nearest, ties to even (exact for every u64)"""
+    x = np.asarray(x, dtype=np.uint64)
+    small = x < np.uint64(1 << 53)          # exact in f64, so one rounding to f32
+    out = x.astype(np.float64).astype(np.float32)
+    for i in np.flatnonzero(~small):
+        v = int(x.flat[i])
+        shift = v.bit_length() - 24
+        m, rem = v >> shift, v & ((1 << shift) - 1)
+        half = 1 << (shift - 1)
+        if rem > half or (rem == half and m & 1):
+            m += 1
+        out.flat[i] = np.float32(m * 2.0 ** shift)
+    return out
+
+
+def bm25_term_frequency(count, doc_len, avgdl, k1, b):
+    """compute_bm25_term_frequency (tf_idf/mod.rs:362-371) in f32, one rounding per operation, no FMA:
+    count as f32 * (k1 + 1.0) / (count as f32 + k1 * (1.0 - b + b * (document_length as f32 / average_document_length)))"""
+    f32 = np.float32
+    c = _u_to_f32(np.asarray(count, dtype=np.uint32))
+    dl = _u_to_f32(np.asarray(doc_len, dtype=np.uint32))
+    k1, b, avgdl = f32(k1), f32(b), f32(avgdl)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        num = c * (k1 + f32(1.0))
+        den = c + k1 * ((f32(1.0) - b) + b * (dl / avgdl))
+        return (num / den).astype(np.float32)
+
+
+def average_document_length(total_len, count):
+    """finalize_sampling (tf_idf/mod.rs:187-207): total_documents_length (u64) as f32 / total_documents_count (u32) as f32"""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.float32(_u_to_f32(np.uint64(total_len)) / _u_to_f32(np.uint32(count)))
+
+
+def _tfidf_csr(rows):
+    """list of [(hash, tf), ...] per row, or (offsets, hashes, tfs) -> CSR triple"""
+    if isinstance(rows, tuple) and len(rows) == 3:
+        o, h, v = rows
+        return (np.ascontiguousarray(o, dtype=np.uint64), np.ascontiguousarray(h, dtype=np.uint32),
+                np.ascontiguousarray(v, dtype=np.float32))
+    return sparse_csr(rows)
+
+
+def _query_csr(queries):
+    """list of hash lists, or (offsets, hashes) -> (offsets u64, hashes u32)"""
+    if isinstance(queries, tuple) and len(queries) == 2:
+        return np.ascontiguousarray(queries[0], dtype=np.uint64), np.ascontiguousarray(queries[1], dtype=np.uint32)
+    off = np.zeros(len(queries) + 1, np.uint64)
+    if queries:
+        off[1:] = np.cumsum([len(q) for q in queries])
+    return off, np.array([h for q in queries for h in q], np.uint32)
+
+
+class TfIdfIndex:
+    """TFIDFIndex's IndexOps surface on one GPU (cdb_tfidf_index) from (term_hash, tf) pairs.  Row r has id id_base + r."""
+
+    def __init__(self, capacity_rows=1 << 20, capacity_pairs=1 << 26, id_base=0, device=0):
+        L = _lib.load()
+        d = _lib.TfIdfIndexDesc(device, capacity_rows, capacity_pairs, id_base)
+        h = C.c_void_p()
+        _check(L.cdb_tfidf_index_create(C.byref(d), C.byref(h)))
+        self.h, self.desc = h, d
+
+    def close(self):
+        if getattr(self, "h", None):
+            _lib.load().cdb_tfidf_index_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def __len__(self):
+        return int(_lib.load().cdb_tfidf_index_size(self.h))
+
+    def append(self, rows, version=0, counted=None):
+        """rows: list of (hash, tf) lists or a CSR triple; counted: per-row flags (False = an id without text, empty row)"""
+        o, h, v = _tfidf_csr(rows)
+        c = None if counted is None else np.ascontiguousarray(counted, dtype=np.uint8)
+        _check(_lib.load().cdb_tfidf_index_append(self.h, _ptr(o), _ptr(h), _ptr(v), _ptr(c), len(o) - 1, version))
+
+    index_embeddings = append
+
+    def delete_embedding(self, rows, version=0):
+        """deletes local rows at `version` (mark_embedding_as_deleted)"""
+        r = np.ascontiguousarray(np.atleast_1d(rows), dtype=np.uint32)
+        _check(_lib.load().cdb_tfidf_index_delete_rows(self.h, _ptr(r), r.size, version))
+
+    def deleted_rows(self, first=0, n=None):
+        n = len(self) - first if n is None else n
+        out = np.zeros(max(n, 1), np.uint8)
+        tot = C.c_uint64(0)
+        _check(_lib.load().cdb_tfidf_index_deleted_rows(self.h, first, n, _ptr(out), C.byref(tot)))
+        return out[:n], tot.value
+
+    def term_stats(self, hashes):
+        """-> (df u32[n], idf f32[n] as the device holds it, N); unseen hashes get df 0 and idf NaN"""
+        hs = np.ascontiguousarray(np.atleast_1d(hashes), dtype=np.uint32)
+        df = np.zeros(max(hs.size, 1), np.uint32)
+        idf = np.zeros(max(hs.size, 1), np.float32)
+        n = C.c_uint32(0)
+        _check(_lib.load().cdb_tfidf_index_term_stats(self.h, _ptr(hs), hs.size, _ptr(df), _ptr(idf), C.byref(n)))
+        return df[:hs.size], idf[:hs.size], n.value
+
+    def batch_search(self, queries, top_k=None):
+        """queries: list of hash lists or (offsets, hashes); top_k None = all bucket winners (up to 512)
+        -> ids u32[B, kout], scores f32[B, kout], counts u32[B] with kout = min(top_k, 512) (512 for None)"""
+        o, h = _query_csr(queries)
+        nq, k = len(o) - 1, int(top_k or 0)
+        kout = 512 if k == 0 or k > 512 else k
+        ids = np.zeros((max(nq, 1), kout), np.uint32)
+        scores = np.zeros((max(nq, 1), kout), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        _check(_lib.load().cdb_tfidf_search_batch(self.h, _ptr(o), _ptr(h), nq, k, _ptr(ids), _ptr(scores), _ptr(counts)))
+        return ids[:nq], scores[:nq], counts[:nq]
+
+    def search(self, query, top_k=None):
+        """-> [(id, score)] best first (search_internal's result order)"""
+        ids, scores, counts = self.batch_search([list(query)], top_k)
+        c = int(counts[0])
+        return list(zip(ids[0, :c].tolist(), scores[0, :c].tolist()))

@@ -1,0 +1,731 @@
+// tfidf.cu -- the TF-IDF / BM25 index (TFIDFIndex, src/indexes/tf_idf/mod.rs) on the GPU: ingest and versioned deletes of
+// (term_hash, tf) documents (TFIDFIndexRoot::insert / delete, src/models/tf_idf_index.rs:315-352, on the VersionedVec of
+// src/models/versioned_vec.rs) and SparseAnnQueryBasic::search_bm25 (src/models/sparse_ann_query.rs:149-233) with get_idf
+// (sparse_ann_query.rs:298-302).  The contract is the header comment of cdb_tfidf_index_create.
+//
+// Layout (DESIGN.md section 8d).  Rows are kept as raw CSR on the device (hashes u32, tf f32, u64 row offsets).  Posting
+// lists are split into row tiles of 2^15 rows; a tile holds its distinct hashes (ascending), one segment per hash and
+// entries (row_in_tile, tf bits), ascending by row inside a segment.  The host keeps the sorted table of every hash the
+// index has seen with its df (VersionedVec::len) and uploads the table and its idf (log1pf on the host) after every append
+// and delete.  An append rebuilds the last partial tile and builds the new ones (CUB radix sort).  A search scores one
+// (query, tile) per CTA into shared-memory f32 accumulators plus a touched flag per row, query terms strictly in the
+// caller's order, reduces the tile to its 512 bucket winners, then merges the tiles per bucket and sorts the winners.
+#include <algorithm>
+#include <cmath>
+#include <mutex>
+#include <shared_mutex>
+#include <vector>
+
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_run_length_encode.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include "kernels.h"
+
+namespace cdb {
+namespace {
+
+constexpr uint32_t TF_TILE_SHIFT = 15;
+constexpr uint32_t TF_TILE = 1u << TF_TILE_SHIFT;
+constexpr int TF_THREADS = 512;
+constexpr uint32_t TF_BUCKETS = 512;       // search_bm25's BUCKETS
+constexpr uint32_t TF_QCHUNK = TF_THREADS; // query terms resolved per pass of the scoring kernel
+static_assert(TF_THREADS == (int)TF_BUCKETS, "one thread per bucket in the tile reduction and the final sort");
+
+struct TfTile {
+    uint64_t entry_base;   // first entry of the tile in d_entries
+    uint64_t hash_base;    // first distinct hash in d_thash; its segment starts are d_tseg[hash_base + tile ..]
+    uint32_t n_hashes;
+    uint32_t pad;
+};
+
+// ---------------------------------------------------------------- build side
+// key = hash << 15 | row_in_tile (47 bits), value = tf bits
+__global__ void tf_tile_keys_kernel(const uint64_t *__restrict__ row_off, uint64_t r0, uint32_t nr, uint64_t p0,
+                                    const uint32_t *__restrict__ hashes, const float *__restrict__ tfs,
+                                    uint64_t *__restrict__ sort_keys, uint32_t *__restrict__ sort_vals) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= nr) return;
+    const uint64_t b = row_off[r0 + warp], e = row_off[r0 + warp + 1];
+    for (uint64_t p = b + lane; p < e; p += 32) {
+        sort_keys[p - p0] = ((uint64_t)hashes[p] << TF_TILE_SHIFT) | warp;
+        sort_vals[p - p0] = __float_as_uint(tfs[p]);
+    }
+}
+
+// entries from the sorted keys, segment flags, and a duplicate (hash, row) flag
+__global__ void tf_entries_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ vals, uint32_t n,
+                                  uint2 *__restrict__ entries, uint32_t *__restrict__ flags, uint32_t *__restrict__ dup) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t k = keys[i];
+    entries[i] = make_uint2((uint32_t)(k & (TF_TILE - 1)), vals[i]);
+    flags[i] = (i == 0 || (k >> TF_TILE_SHIFT) != (keys[i - 1] >> TF_TILE_SHIFT)) ? 1u : 0u;
+    if (i > 0 && k == keys[i - 1]) *dup = 1u;
+}
+
+__global__ void tf_seg_scatter_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ flags,
+                                      const uint32_t *__restrict__ pos, uint32_t n, uint32_t *__restrict__ thash,
+                                      uint32_t *__restrict__ tseg) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (flags[i]) {
+        thash[pos[i] - 1] = (uint32_t)(keys[i] >> TF_TILE_SHIFT);
+        tseg[pos[i] - 1] = i;
+    }
+    if (i == n - 1) tseg[pos[i]] = n;
+}
+
+// the hashes of rows[0..n) packed at out[off[i] ..] (one warp per row)
+__global__ void tf_gather_rows_kernel(const uint64_t *__restrict__ row_off, const uint32_t *__restrict__ hashes,
+                                      const uint32_t *__restrict__ rows, const uint64_t *__restrict__ off, uint32_t n,
+                                      uint32_t *__restrict__ out) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= n) return;
+    const uint64_t b = row_off[rows[warp]], e = row_off[rows[warp] + 1];
+    for (uint64_t p = b + lane; p < e; p += 32) out[off[warp] + (p - b)] = hashes[p];
+}
+
+// ---------------------------------------------------------------- search side
+struct TfSearch {
+    const uint2 *entries;
+    const uint32_t *thash, *tseg, *deleted;
+    const TfTile *tiles;
+    const uint32_t *terms;   // every hash the index has seen, ascending
+    const float *idf;        // idf of terms[i]
+    uint32_t n_terms;
+    uint64_t n_rows;
+    uint32_t id_base;
+    const uint64_t *q_off;
+    const uint32_t *q_hash;
+    uint32_t q0;             // first query of the chunk
+    uint32_t n_tiles;
+    uint2 *out;              // [chunk][n_tiles][512] bucket winners (id, score bits); id CDB_INVALID_ID = empty
+};
+
+constexpr size_t TF_SCORE_SMEM = (size_t)TF_TILE * 4 + TF_TILE + (size_t)TF_QCHUNK * 12;
+
+__device__ inline uint32_t lower_bound_u32(const uint32_t *a, uint32_t n, uint32_t x) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < x) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+__global__ void __launch_bounds__(TF_THREADS, 1) tf_score_tile_kernel(TfSearch a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    float *acc = reinterpret_cast<float *>(smem);
+    uint8_t *touched = smem + (size_t)TF_TILE * 4;
+    uint32_t *c_beg = reinterpret_cast<uint32_t *>(touched + TF_TILE);   // segment of each resolved term (tile-relative)
+    uint32_t *c_len = c_beg + TF_QCHUNK;
+    float *c_idf = reinterpret_cast<float *>(c_len + TF_QCHUNK);
+
+    const uint32_t t = blockIdx.x, qi = blockIdx.y, q = a.q0 + qi, tid = threadIdx.x;
+    const TfTile tile = a.tiles[t];
+    const uint64_t row0 = (uint64_t)t << TF_TILE_SHIFT;
+    const uint32_t nr = (uint32_t)std::min<uint64_t>(TF_TILE, a.n_rows - row0);
+    uint4 *t4 = reinterpret_cast<uint4 *>(touched);
+    for (uint32_t i = tid; i < TF_TILE / 16; i += TF_THREADS) t4[i] = make_uint4(0, 0, 0, 0);
+    __syncthreads();
+
+    const uint32_t *thash = a.thash + tile.hash_base;
+    const uint32_t *tseg = a.tseg + tile.hash_base + t;
+    const uint2 *ent = a.entries + tile.entry_base;
+    const uint64_t qb = a.q_off[q], qe = a.q_off[q + 1];
+    for (uint64_t j0 = qb; j0 < qe; j0 += TF_QCHUNK) {
+        const uint32_t nj = (uint32_t)std::min<uint64_t>(TF_QCHUNK, qe - j0);
+        if (tid < nj) {
+            // search_bm25's head for this term: absent terms are skipped, a present one carries get_idf of its list
+            const uint32_t h = a.q_hash[j0 + tid];
+            const uint32_t g = lower_bound_u32(a.terms, a.n_terms, h);
+            uint32_t s = 0, e = 0;
+            float idf = 0.0f;
+            if (g < a.n_terms && a.terms[g] == h) {
+                idf = a.idf[g];
+                const uint32_t l = lower_bound_u32(thash, tile.n_hashes, h);
+                if (l < tile.n_hashes && thash[l] == h) { s = tseg[l]; e = tseg[l + 1]; }
+            }
+            c_beg[tid] = s;
+            c_len[tid] = e - s;
+            c_idf[tid] = idf;
+        }
+        __syncthreads();
+        // the terms in the caller's order; inside one segment every row appears once, so each thread owns its rows
+        for (uint32_t j = 0; j < nj; ++j) {
+            const uint32_t beg = c_beg[j], len = c_len[j];
+            const float idf = c_idf[j];
+            for (uint32_t i = tid; i < len; i += TF_THREADS) {
+                const uint2 e = __ldg(ent + beg + i);
+                const float p = __fmul_rn(__uint_as_float(e.y), idf);
+                if (touched[e.x]) {
+                    acc[e.x] = __fadd_rn(acc[e.x], p);
+                } else {
+                    acc[e.x] = p;   // the first product, not 0 + product: a -0 score keeps its sign
+                    touched[e.x] = 1;
+                }
+            }
+            __syncthreads();
+        }
+    }
+    // bucket id % 512: the rows of one bucket, visited in ascending id; `score > best` from -inf keeps the first of equal
+    // scores and never admits NaN or -inf.  Deleted rows are skipped.
+    const uint32_t id0 = a.id_base + (uint32_t)row0;
+    float best = -INFINITY;
+    uint32_t bid = CDB_INVALID_ID;
+    for (uint32_t r = (tid - id0) & (TF_BUCKETS - 1); r < nr; r += TF_BUCKETS) {
+        if (!touched[r]) continue;
+        const uint64_t g = row0 + r;
+        if (a.deleted && (a.deleted[g >> 5] >> (g & 31)) & 1u) continue;
+        const float s = acc[r];
+        if (s > best) { best = s; bid = id0 + r; }
+    }
+    a.out[((size_t)qi * a.n_tiles + t) * TF_BUCKETS + tid] = make_uint2(bid, __float_as_uint(best));
+}
+
+// per query: the tiles' winners of each bucket merged in ascending tile order (ascending ids, so `>` keeps the reference's
+// winner), then the <= 512 winners sorted by total_cmp descending, ties to the smaller id, truncated to kout
+__global__ void __launch_bounds__(TF_THREADS, 1) tf_finalize_kernel(const uint2 *__restrict__ in, uint32_t n_tiles, uint32_t kout,
+                                                                     uint32_t *__restrict__ out_ids, float *__restrict__ out_scores,
+                                                                     uint32_t *__restrict__ out_counts) {
+    __shared__ uint64_t keys[TF_BUCKETS];
+    __shared__ uint32_t s_cnt;
+    const uint32_t qi = blockIdx.x, tid = threadIdx.x;
+    if (tid == 0) s_cnt = 0;
+    const uint2 *src = in + (size_t)qi * n_tiles * TF_BUCKETS + tid;
+    float best = -INFINITY;
+    uint32_t bid = CDB_INVALID_ID;
+    for (uint32_t t = 0; t < n_tiles; ++t) {
+        const uint2 w = src[(size_t)t * TF_BUCKETS];
+        const float s = __uint_as_float(w.y);
+        if (w.x != CDB_INVALID_ID && s > best) { best = s; bid = w.x; }
+    }
+    __syncthreads();
+    // order_key of a non-NaN score is non-zero above -inf's; 0 marks an empty bucket
+    keys[tid] = bid == CDB_INVALID_ID ? 0ull
+                                      : ((uint64_t)order_key(CDB_METRIC_DOT_PRODUCT, __float_as_uint(best)) << 32) | (uint64_t)(~bid);
+    if (bid != CDB_INVALID_ID) atomicAdd(&s_cnt, 1u);
+    __syncthreads();
+    for (uint32_t size = 2; size <= TF_BUCKETS; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            if (tid < TF_BUCKETS / 2) {
+                const uint32_t lo = 2 * tid - (tid & (stride - 1)), hi = lo + stride;
+                const bool desc = (lo & size) == 0;
+                const uint64_t x = keys[lo], y = keys[hi];
+                if ((x < y) == desc) { keys[lo] = y; keys[hi] = x; }
+            }
+            __syncthreads();
+        }
+    }
+    const uint32_t cnt = min(s_cnt, kout);
+    if (tid < kout) {
+        uint32_t id = CDB_INVALID_ID;
+        float s = 0.0f;
+        if (tid < cnt) {
+            const uint64_t key = keys[tid];
+            id = ~(uint32_t)key;
+            s = __uint_as_float(key_to_bits(CDB_METRIC_DOT_PRODUCT, (uint32_t)(key >> 32)));
+        }
+        out_ids[(size_t)qi * kout + tid] = id;
+        out_scores[(size_t)qi * kout + tid] = s;
+    }
+    if (tid == 0) out_counts[qi] = cnt;
+}
+
+}  // namespace
+}  // namespace cdb
+
+using namespace cdb;
+
+struct cdb_tfidf_index {
+    cdb_tfidf_index_desc desc;
+    std::shared_mutex rw;
+    uint64_t n_rows = 0, n_pairs = 0, n_deleted = 0;
+    uint32_t documents = 0;          // total_documents_count
+    uint32_t version = 0;            // the latest version passed to append / delete_rows
+    std::vector<uint64_t> h_row_off{0};
+    std::vector<uint8_t> h_counted;
+    std::vector<uint32_t> h_version; // insert version per row
+    std::vector<uint32_t> h_deleted;
+    std::vector<uint32_t> h_terms;   // every hash seen, ascending
+    std::vector<uint32_t> h_df;      // VersionedVec::len of each
+    std::vector<TfTile> h_tiles;
+    uint64_t *d_row_off = nullptr;
+    uint32_t *d_hashes = nullptr, *d_thash = nullptr, *d_tseg = nullptr, *d_deleted = nullptr, *d_terms = nullptr;
+    float *d_tfs = nullptr, *d_idf = nullptr;
+    uint2 *d_entries = nullptr;
+    TfTile *d_tiles = nullptr;
+    uint64_t max_tiles = 0, terms_cap = 0;
+    ~cdb_tfidf_index() {
+        for (void *p : {(void *)d_row_off, (void *)d_hashes, (void *)d_thash, (void *)d_tseg, (void *)d_deleted, (void *)d_terms,
+                        (void *)d_tfs, (void *)d_idf, (void *)d_entries, (void *)d_tiles})
+            if (p) cudaFree(p);
+    }
+};
+
+#define TF_REQUIRE(cond, msg)                                              \
+    do {                                                                   \
+        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; }        \
+    } while (0)
+
+namespace {
+
+// get_idf (sparse_ann_query.rs:298-302): u32 wrapping N - df, round-to-nearest u32 -> f32, f32 add / divide, and Rust's
+// f32::ln_1p, which is the platform libm's log1pf
+float tf_idf(uint32_t n_docs, uint32_t df) {
+    const float num = (float)(uint32_t)(n_docs - df) + 0.5f;
+    const float den = (float)df + 0.5f;
+    return log1pf(num / den);
+}
+
+struct BuildBufs {
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    uint64_t *keys_in = nullptr, *keys_out = nullptr;
+    uint32_t *vals_in = nullptr, *vals_out = nullptr, *flags = nullptr, *pos = nullptr, *dup = nullptr;
+    ~BuildBufs() {
+        for (void *p : {tmp, (void *)keys_in, (void *)keys_out, (void *)vals_in, (void *)vals_out, (void *)flags, (void *)pos, (void *)dup})
+            if (p) cudaFree(p);
+    }
+};
+
+cdb_status alloc_build_bufs(BuildBufs &b, uint64_t max_np, cudaStream_t s) {
+    CDB_CUDA_TRY(cudaMalloc(&b.dup, 4));
+    if (!max_np) return CDB_OK;
+    CDB_CUDA_TRY(cudaMalloc(&b.keys_in, max_np * 8));
+    CDB_CUDA_TRY(cudaMalloc(&b.keys_out, max_np * 8));
+    CDB_CUDA_TRY(cudaMalloc(&b.vals_in, max_np * 4));
+    CDB_CUDA_TRY(cudaMalloc(&b.vals_out, max_np * 4));
+    CDB_CUDA_TRY(cudaMalloc(&b.flags, max_np * 4));
+    CDB_CUDA_TRY(cudaMalloc(&b.pos, max_np * 4));
+    size_t t_sort = 0, t_scan = 0;
+    CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, b.keys_in, b.keys_out, b.vals_in, b.vals_out, (int)max_np, 0,
+                                                 32 + TF_TILE_SHIFT, s));
+    CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, t_scan, b.flags, b.pos, (int)max_np, s));
+    b.tmp_bytes = std::max(t_sort, t_scan);
+    CDB_CUDA_TRY(cudaMalloc(&b.tmp, b.tmp_bytes));
+    return CDB_OK;
+}
+
+// posting lists of tile t appended after the tiles below it; CDB_INVALID_PARAMS if a row of it repeats a hash
+cdb_status build_tile(cdb_tfidf_index *ix, uint64_t t, BuildBufs &b, cudaStream_t s) {
+    const uint64_t r0 = t << TF_TILE_SHIFT, r1 = std::min<uint64_t>(ix->n_rows, r0 + TF_TILE);
+    const uint64_t p0 = ix->h_row_off[r0], p1 = ix->h_row_off[r1];
+    const uint32_t np = (uint32_t)(p1 - p0);
+    TfTile tile;
+    tile.entry_base = p0;
+    tile.hash_base = t ? ix->h_tiles[t - 1].hash_base + ix->h_tiles[t - 1].n_hashes : 0;
+    tile.n_hashes = 0;
+    tile.pad = 0;
+    uint32_t *tseg = ix->d_tseg + tile.hash_base + t;
+    if (np == 0) {
+        CDB_CUDA_TRY(cudaMemsetAsync(tseg, 0, 4, s));
+    } else {
+        const uint32_t nr = (uint32_t)(r1 - r0);
+        tf_tile_keys_kernel<<<(nr * 32 + 255) / 256, 256, 0, s>>>(ix->d_row_off, r0, nr, p0, ix->d_hashes, ix->d_tfs, b.keys_in, b.vals_in);
+        CDB_LAUNCH_CHECK();
+        size_t tb = b.tmp_bytes;
+        CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tb, b.keys_in, b.keys_out, b.vals_in, b.vals_out, (int)np, 0,
+                                                     32 + TF_TILE_SHIFT, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(b.dup, 0, 4, s));
+        tf_entries_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, b.vals_out, np, ix->d_entries + p0, b.flags, b.dup);
+        CDB_LAUNCH_CHECK();
+        tb = b.tmp_bytes;
+        CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(b.tmp, tb, b.flags, b.pos, (int)np, s));
+        tf_seg_scatter_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, b.flags, b.pos, np, ix->d_thash + tile.hash_base, tseg);
+        CDB_LAUNCH_CHECK();
+        uint32_t dup = 0;
+        CDB_CUDA_TRY(cudaMemcpyAsync(&tile.n_hashes, b.pos + np - 1, 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaMemcpyAsync(&dup, b.dup, 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaStreamSynchronize(s));
+        if (dup) { set_error("a row repeats a term hash"); return CDB_INVALID_PARAMS; }
+    }
+    ix->h_tiles.push_back(tile);
+    return CDB_OK;
+}
+
+cdb_status build_tiles(cdb_tfidf_index *ix, uint64_t t0, uint64_t t1, BuildBufs &b, cudaStream_t s) {
+    ix->h_tiles.resize(t0);
+    cdb_status rc;
+    for (uint64_t t = t0; t < t1; ++t)
+        if ((rc = build_tile(ix, t, b, s))) return rc;
+    if (t1 > t0)
+        CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_tiles + t0, ix->h_tiles.data() + t0, (t1 - t0) * sizeof(TfTile), cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaStreamSynchronize(s));
+    return CDB_OK;
+}
+
+// back to the first `rows` rows (their pairs are still in place; nothing was deleted among the dropped ones)
+cdb_status restore_rows(cdb_tfidf_index *ix, uint64_t rows, BuildBufs &b, cudaStream_t s) {
+    ix->h_row_off.resize(rows + 1);
+    ix->n_rows = rows;
+    ix->n_pairs = ix->h_row_off[rows];
+    return build_tiles(ix, rows >> TF_TILE_SHIFT, (rows + TF_TILE - 1) >> TF_TILE_SHIFT, b, s);
+}
+
+// the term table and its idf under `n_docs` to the device (the device is idle: the caller holds the handle exclusively
+// and has drained queued searches)
+cdb_status upload_terms(cdb_tfidf_index *ix, const std::vector<uint32_t> &terms, const std::vector<uint32_t> &df, uint32_t n_docs,
+                        bool terms_changed, cudaStream_t s) {
+    const size_t n = terms.size();
+    if (n > ix->terms_cap) {
+        const uint64_t cap = std::max<uint64_t>(n, 2 * ix->terms_cap);
+        uint32_t *t = nullptr;
+        float *f = nullptr;
+        CDB_CUDA_TRY(cudaMalloc(&t, cap * 4));
+        cudaError_t e = cudaMalloc(&f, cap * 4);
+        if (e != cudaSuccess) { cudaFree(t); set_error(std::string("cudaMalloc: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+        if (ix->d_terms) cudaFree(ix->d_terms);
+        if (ix->d_idf) cudaFree(ix->d_idf);
+        ix->d_terms = t;
+        ix->d_idf = f;
+        ix->terms_cap = cap;
+        terms_changed = true;
+    }
+    if (!n) return CDB_OK;
+    std::vector<float> idf(n);
+    for (size_t i = 0; i < n; ++i) idf[i] = tf_idf(n_docs, df[i]);
+    if (terms_changed) CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_terms, terms.data(), n * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_idf, idf.data(), n * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaStreamSynchronize(s));
+    return CDB_OK;
+}
+
+struct StreamGuard {
+    cudaStream_t s = nullptr;
+    ~StreamGuard() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
+};
+
+cdb_status check_csr(const uint64_t *off, uint64_t n, const char *what) {
+    TF_REQUIRE(off, "null offsets");
+    if (off[0] != 0) { set_error(std::string(what) + ": offsets[0] must be 0"); return CDB_INVALID_PARAMS; }
+    for (uint64_t i = 0; i < n; ++i)
+        if (off[i + 1] < off[i]) { set_error(std::string(what) + ": offsets decrease"); return CDB_INVALID_PARAMS; }
+    return CDB_OK;
+}
+
+uint32_t out_cols(uint32_t k) { return (k == 0 || k > TF_BUCKETS) ? TF_BUCKETS : k; }
+
+cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint32_t nq, uint32_t k,
+                         uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t s) {
+    if (!nq) return CDB_OK;
+    const uint32_t kout = out_cols(k);
+    const uint32_t n_tiles = (uint32_t)ix->h_tiles.size();
+    if (n_tiles == 0) {
+        CDB_CUDA_TRY(cudaMemsetAsync(d_ids, 0xFF, (size_t)nq * kout * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d_scores, 0, (size_t)nq * kout * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
+        return CDB_OK;
+    }
+    const size_t per_q = (size_t)n_tiles * TF_BUCKETS * sizeof(uint2);
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, (512ull << 20) / per_q}));
+    uint2 *win = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&win, (size_t)chunk * per_q, s));
+    cdb_status rc = CDB_OK;
+    cudaError_t e = allow_max_dynamic_smem((const void *)tf_score_tile_kernel);
+    if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        TfSearch a;
+        a.entries = ix->d_entries; a.thash = ix->d_thash; a.tseg = ix->d_tseg; a.deleted = ix->n_deleted ? ix->d_deleted : nullptr;
+        a.tiles = ix->d_tiles; a.terms = ix->d_terms; a.idf = ix->d_idf; a.n_terms = (uint32_t)ix->h_terms.size();
+        a.n_rows = ix->n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q0 = q0; a.n_tiles = n_tiles;
+        a.out = win;
+        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(a);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
+        tf_finalize_kernel<<<c, TF_THREADS, 0, s>>>(win, n_tiles, kout, d_ids + (size_t)q0 * kout, d_scores + (size_t)q0 * kout,
+                                                     d_counts + q0);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    cudaFreeAsync(win, s);
+    return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+cdb_status cdb_tfidf_index_create(const cdb_tfidf_index_desc *desc, cdb_tfidf_index **out) {
+    TF_REQUIRE(desc && out, "null argument");
+    TF_REQUIRE(desc->capacity_rows >= 1 && (uint64_t)desc->id_base + desc->capacity_rows <= 0xFFFFFFFFull,
+               "capacity_rows must be >= 1 and id_base + capacity_rows <= 2^32 - 1");
+    TF_REQUIRE(desc->capacity_pairs < (1ull << 40), "capacity_pairs too large");
+    *out = nullptr;
+    CDB_CUDA_TRY(cudaSetDevice(desc->device));
+    std::unique_ptr<cdb_tfidf_index> ix(new cdb_tfidf_index());
+    ix->desc = *desc;
+    ix->max_tiles = (desc->capacity_rows + TF_TILE - 1) / TF_TILE;
+    const size_t pairs = std::max<uint64_t>(1, desc->capacity_pairs);
+    const size_t words = (desc->capacity_rows + 31) / 32;
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_row_off, (desc->capacity_rows + 1) * 8));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_hashes, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_tfs, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_entries, pairs * 8));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_thash, pairs * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_tseg, (pairs + ix->max_tiles) * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_deleted, words * 4));
+    CDB_CUDA_TRY(cudaMalloc(&ix->d_tiles, ix->max_tiles * sizeof(TfTile)));
+    CDB_CUDA_TRY(cudaMemset(ix->d_row_off, 0, 8));
+    CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
+    ix->h_deleted.assign(words, 0u);
+    *out = ix.release();
+    return CDB_OK;
+}
+
+cdb_status cdb_tfidf_index_destroy(cdb_tfidf_index *ix) {
+    if (!ix) return CDB_OK;
+    cudaSetDevice(ix->desc.device);
+    cudaDeviceSynchronize();
+    delete ix;
+    return CDB_OK;
+}
+
+uint64_t cdb_tfidf_index_size(const cdb_tfidf_index *ix) { return ix ? ix->n_rows : 0; }
+
+cdb_status cdb_tfidf_index_append(cdb_tfidf_index *ix, const uint64_t *row_offsets, const uint32_t *hashes, const float *tfs,
+                                  const uint8_t *counted, uint64_t n, uint32_t version) {
+    TF_REQUIRE(ix, "null index");
+    if (!n) return CDB_OK;
+    cdb_status rc = check_csr(row_offsets, n, "row_offsets");
+    if (rc) return rc;
+    const uint64_t np = row_offsets[n];
+    TF_REQUIRE((hashes && tfs) || !np, "null pairs");
+    uint32_t n_counted = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        if (!counted || counted[i]) ++n_counted;
+        else TF_REQUIRE(row_offsets[i + 1] == row_offsets[i], "an uncounted row must be empty");
+    }
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    TF_REQUIRE(ix->n_rows + n <= ix->desc.capacity_rows, "append exceeds capacity_rows");
+    TF_REQUIRE(ix->n_pairs + np <= ix->desc.capacity_pairs, "append exceeds capacity_pairs");
+    TF_REQUIRE(version >= ix->version, "version is older than the index's latest");
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    // every check and allocation precedes the first change
+    const uint64_t r_old = ix->n_rows, p_old = ix->n_pairs, r_new = r_old + n;
+    std::vector<uint64_t> off(n);
+    for (uint64_t i = 0; i < n; ++i) off[i] = p_old + row_offsets[i + 1];
+    auto row_off = [&](uint64_t r) { return r <= r_old ? ix->h_row_off[r] : off[r - r_old - 1]; };
+    const uint64_t t0 = r_old >> TF_TILE_SHIFT, t1 = (r_new + TF_TILE - 1) >> TF_TILE_SHIFT;
+    uint64_t max_np = 0;
+    for (uint64_t t = t0; t < t1; ++t)
+        max_np = std::max(max_np, row_off(std::min<uint64_t>(r_new, (t + 1) << TF_TILE_SHIFT)) - row_off(t << TF_TILE_SHIFT));
+    TF_REQUIRE(max_np < (1ull << 31) && np < (1ull << 31), "a row tile or an append holds 2^31 pairs or more");
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    BuildBufs b;
+    if ((rc = alloc_build_bufs(b, std::max(max_np, np), s))) return rc;
+    // searches already enqueued on other streams (cdb_tfidf_search_batch_device) read the tile and the idf this call rewrites
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    cudaError_t e = cudaSuccess;
+    if (np) {
+        e = cudaMemcpyAsync(ix->d_hashes + p_old, hashes, np * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_tfs + p_old, tfs, np * 4, cudaMemcpyHostToDevice, s);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_row_off + r_old + 1, off.data(), n * 8, cudaMemcpyHostToDevice, s);
+    // df increments: the distinct hashes of the appended pairs and how many rows hold each (rows never repeat a hash)
+    std::vector<uint32_t> uniq, cnt;
+    if (e == cudaSuccess && np) {
+        uint32_t *runs = b.pos;   // scratch: sorted hashes -> b.vals_out, unique -> b.flags, counts -> b.vals_in, runs -> pos
+        size_t t_sort = 0, t_rle = 0;
+        e = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, ix->d_hashes + p_old, b.vals_out, (int)np, 0, 32, s);
+        if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
+        const size_t need = std::max(t_sort, t_rle);
+        void *tmp = b.tmp;
+        if (e == cudaSuccess && need > b.tmp_bytes) e = cudaMallocAsync(&tmp, need, s);
+        size_t tb = need;
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp, tb, ix->d_hashes + p_old, b.vals_out, (int)np, 0, 32, s);
+        tb = need;
+        if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(tmp, tb, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
+        uint32_t n_runs = 0;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&n_runs, runs, 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) {
+            uniq.resize(n_runs);
+            cnt.resize(n_runs);
+            e = cudaMemcpyAsync(uniq.data(), b.flags, n_runs * 4ull, cudaMemcpyDeviceToHost, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(cnt.data(), b.vals_in, n_runs * 4ull, cudaMemcpyDeviceToHost, s);
+        }
+        if (tmp != b.tmp) cudaFreeAsync(tmp, s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error(std::string("tf-idf append: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    // the merged term table
+    std::vector<uint32_t> terms, df;
+    terms.reserve(ix->h_terms.size() + uniq.size());
+    df.reserve(ix->h_terms.size() + uniq.size());
+    size_t i = 0, j = 0;
+    while (i < ix->h_terms.size() || j < uniq.size()) {
+        if (j == uniq.size() || (i < ix->h_terms.size() && ix->h_terms[i] < uniq[j])) { terms.push_back(ix->h_terms[i]); df.push_back(ix->h_df[i]); ++i; }
+        else if (i == ix->h_terms.size() || uniq[j] < ix->h_terms[i]) { terms.push_back(uniq[j]); df.push_back(cnt[j]); ++j; }
+        else { terms.push_back(ix->h_terms[i]); df.push_back(ix->h_df[i] + cnt[j]); ++i; ++j; }
+    }
+    const bool new_terms = terms.size() != ix->h_terms.size();
+    ix->h_row_off.insert(ix->h_row_off.end(), off.begin(), off.end());
+    ix->n_rows = r_new;
+    ix->n_pairs += np;
+    // rebuild the last partial tile, build the new ones, then the idf of every term under the new N; on failure the index
+    // goes back to its r_old rows
+    const uint32_t docs = ix->documents + n_counted;
+    if (!(rc = build_tiles(ix, t0, t1, b, s))) rc = upload_terms(ix, terms, df, docs, new_terms, s);
+    if (rc) {
+        const std::string msg = cdb_last_error_string();
+        restore_rows(ix, r_old, b, s);
+        upload_terms(ix, ix->h_terms, ix->h_df, ix->documents, true, s);
+        set_error(msg);
+        return rc;
+    }
+    ix->h_terms.swap(terms);
+    ix->h_df.swap(df);
+    ix->documents = docs;
+    ix->version = version;
+    for (uint64_t r = 0; r < n; ++r) ix->h_counted.push_back(!counted || counted[r] ? 1 : 0);
+    ix->h_version.resize(r_new, version);
+    return CDB_OK;
+}
+
+cdb_status cdb_tfidf_index_delete_rows(cdb_tfidf_index *ix, const uint32_t *rows, uint64_t n, uint32_t version) {
+    TF_REQUIRE(ix && (rows || !n), "null argument");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    for (uint64_t i = 0; i < n; ++i) TF_REQUIRE(rows[i] < ix->n_rows, "row out of range");
+    TF_REQUIRE(version >= ix->version, "version is older than the index's latest");
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    if (!n) return CDB_OK;
+    std::vector<uint32_t> w = ix->h_deleted;
+    std::vector<uint32_t> fresh;      // rows this call deletes (already deleted rows are left alone)
+    for (uint64_t i = 0; i < n; ++i) {
+        uint32_t &x = w[rows[i] >> 5];
+        const uint32_t bit = 1u << (rows[i] & 31);
+        if (!(x & bit)) { x |= bit; fresh.push_back(rows[i]); }
+    }
+    // VersionedVec::delete of each of their terms: a delete in the insert's version removes the entry (df - 1), a later one
+    // marks it and pushes a tombstone word (df + 1)
+    std::vector<uint64_t> goff(fresh.size() + 1, 0);
+    for (size_t i = 0; i < fresh.size(); ++i) goff[i + 1] = goff[i] + ix->h_row_off[fresh[i] + 1] - ix->h_row_off[fresh[i]];
+    const uint64_t ng = goff.back();
+    std::vector<uint32_t> gh(ng);
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    if (ng) {
+        uint8_t *buf = nullptr;
+        const size_t bytes = fresh.size() * 4 + goff.size() * 8 + ng * 4;
+        CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
+        uint64_t *d_off = reinterpret_cast<uint64_t *>(buf);
+        uint32_t *d_rows = reinterpret_cast<uint32_t *>(d_off + goff.size());
+        uint32_t *d_out = d_rows + fresh.size();
+        cudaError_t e = cudaMemcpyAsync(d_off, goff.data(), goff.size() * 8, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_rows, fresh.data(), fresh.size() * 4, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) {
+            tf_gather_rows_kernel<<<(uint32_t)((fresh.size() * 32 + 255) / 256), 256, 0, s>>>(ix->d_row_off, ix->d_hashes, d_rows, d_off,
+                                                                                          (uint32_t)fresh.size(), d_out);
+            g_launch_count.fetch_add(1, std::memory_order_relaxed);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(gh.data(), d_out, ng * 4, cudaMemcpyDeviceToHost, s);
+        cudaFreeAsync(buf, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) { set_error(std::string("tf-idf delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    }
+    std::vector<uint32_t> df = ix->h_df;
+    uint32_t docs = ix->documents;
+    for (size_t i = 0; i < fresh.size(); ++i) {
+        const uint32_t r = fresh[i];
+        if (!ix->h_counted[r]) continue;     // delete_embedding returns early for an embedding without text
+        --docs;
+        const uint32_t delta = ix->h_version[r] == version ? 0xFFFFFFFFu : 1u;
+        for (uint64_t p = goff[i]; p < goff[i + 1]; ++p) {
+            const size_t g = std::lower_bound(ix->h_terms.begin(), ix->h_terms.end(), gh[p]) - ix->h_terms.begin();
+            df[g] += delta;
+        }
+    }
+    // searches enqueued before this call finish first (they read the bitmap and the idf)
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_deleted, w.data(), w.size() * 4, cudaMemcpyHostToDevice, s));
+    cdb_status rc = upload_terms(ix, ix->h_terms, df, docs, false, s);
+    if (rc) {
+        cudaMemcpyAsync(ix->d_deleted, ix->h_deleted.data(), w.size() * 4, cudaMemcpyHostToDevice, s);
+        return rc;
+    }
+    ix->h_deleted.swap(w);
+    ix->n_deleted += fresh.size();
+    ix->h_df.swap(df);
+    ix->documents = docs;
+    ix->version = version;
+    return CDB_OK;
+}
+
+cdb_status cdb_tfidf_index_deleted_rows(const cdb_tfidf_index *ix, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total) {
+    TF_REQUIRE(ix && (out || !n), "null argument");
+    TF_REQUIRE(first + n <= ix->desc.capacity_rows, "first + n exceeds capacity_rows");
+    std::shared_lock<std::shared_mutex> lock(const_cast<cdb_tfidf_index *>(ix)->rw);
+    for (uint64_t i = 0; i < n; ++i) out[i] = (ix->h_deleted[(first + i) >> 5] >> ((first + i) & 31)) & 1u;
+    if (out_total) *out_total = ix->n_deleted;
+    return CDB_OK;
+}
+
+cdb_status cdb_tfidf_index_term_stats(cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *out_df, float *out_idf,
+                                      uint32_t *out_documents_count) {
+    TF_REQUIRE(ix && (hashes || !n), "null argument");
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    if (out_documents_count) *out_documents_count = ix->documents;
+    if (!n) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    // the idf as the device holds it
+    std::vector<float> idf(ix->h_terms.size());
+    if (!idf.empty()) CDB_CUDA_TRY(cudaMemcpy(idf.data(), ix->d_idf, idf.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint64_t i = 0; i < n; ++i) {
+        const size_t g = std::lower_bound(ix->h_terms.begin(), ix->h_terms.end(), hashes[i]) - ix->h_terms.begin();
+        const bool found = g < ix->h_terms.size() && ix->h_terms[g] == hashes[i];
+        if (out_df) out_df[i] = found ? ix->h_df[g] : 0u;
+        if (out_idf) out_idf[i] = found ? idf[g] : std::nanf("");
+    }
+    return CDB_OK;
+}
+
+cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *ix, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes, uint32_t nq,
+                                         uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream) {
+    TF_REQUIRE(ix && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    return search_locked(ix, d_q_offsets, d_q_hashes, nq, k, d_ids, d_scores, d_counts, (cudaStream_t)stream);
+}
+
+cdb_status cdb_tfidf_search_batch(cdb_tfidf_index *ix, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
+                                  uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
+    TF_REQUIRE(ix && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    if (!nq) return CDB_OK;
+    cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
+    if (rc) return rc;
+    const uint64_t nqh = q_offsets[nq];
+    TF_REQUIRE(q_hashes || !nqh, "null query hashes");
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    const size_t kout = out_cols(k);
+    const size_t bytes = (nq + 1) * 8 + (size_t)nq * kout * 8 + (size_t)nq * 4 + nqh * 4;
+    uint8_t *buf = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
+    uint64_t *d_off = reinterpret_cast<uint64_t *>(buf);
+    uint32_t *d_ids = reinterpret_cast<uint32_t *>(d_off + nq + 1);
+    float *d_scores = reinterpret_cast<float *>(d_ids + (size_t)nq * kout);
+    uint32_t *d_counts = reinterpret_cast<uint32_t *>(d_scores + (size_t)nq * kout);
+    uint32_t *d_qh = d_counts + nq;
+    cudaError_t e = cudaMemcpyAsync(d_off, q_offsets, (nq + 1) * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && nqh) e = cudaMemcpyAsync(d_qh, q_hashes, nqh * 4, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) { set_error(std::string("cudaMemcpyAsync: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    if (!rc) rc = search_locked(ix, d_off, d_qh, nq, (uint32_t)k, d_ids, d_scores, d_counts, s);
+    if (!rc) {
+        e = cudaMemcpyAsync(out_ids, d_ids, (size_t)nq * kout * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, d_scores, (size_t)nq * kout * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out_counts, d_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) { set_error(std::string("tf-idf search: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    cudaFreeAsync(buf, s);
+    return rc;
+}
+
+}  // extern "C"

@@ -719,6 +719,76 @@ cdb_status cdb_itoe_load_sparse(const char *collection_dir, uint64_t first_entry
 cdb_status cdb_sparse_index_append_itoe(cdb_sparse_index *index, const char *collection_dir, uint32_t *out_internal_ids,
                                         uint64_t max_ids, uint64_t *out_appended);
 
+/* ------------------------------------------------ TF-IDF / BM25 index
+ * TFIDFIndex (src/indexes/tf_idf/mod.rs) over TFIDFIndexRoot (src/models/tf_idf_index.rs) and VersionedVec
+ * (src/models/versioned_vec.rs); the search is SparseAnnQueryBasic::search_bm25 (src/models/sparse_ann_query.rs:149-302).
+ * Text processing (process_text: tokenize, lowercase, stopwords, stemmer, xxhash32) stays with the caller, which passes
+ * what TFIDFIndexRoot::insert receives: per document the (term_hash, tf) pairs, tf = compute_bm25_term_frequency.
+ *
+ * Documents.  Rows are CSR: row r holds pairs [row_offsets[r], row_offsets[r+1]) and has id id_base + r.  tf is taken as
+ * given, 0, -0, negative, inf and NaN included.  A row repeating a hash is CDB_INVALID_PARAMS (process_text never makes
+ * one).  counted[r] = 0 marks a row for an id without text (internal ids are shared by a collection's indexes): it must be
+ * empty and never counts; counted = NULL counts every row.
+ * N (total_documents_count, mod.rs:85-137): +1 per counted row appended, -1 per counted row deleted.
+ * df of a term (VersionedVec::len, versioned_vec.rs:131-199): its entries, counted physically -- +1 per row appended with
+ * it; a delete in the row's insert version removes the entry (-1); a delete in a later version marks the entry and pushes
+ * a tombstone word, both of which count (+1).  So df can exceed N.
+ * idf (get_idf, sparse_ann_query.rs:298-302) = log1pf(((N - df) as f32 + 0.5) / (df as f32 + 0.5)) with u32 wrapping
+ * N - df and round-to-nearest u32 -> f32; computed on the host with the C library's log1pf (Rust's f32::ln_1p) and
+ * uploaded at the end of every append and delete, for every term.
+ * Versions.  append and delete_rows take the transaction's version; versions passed to either must not decrease (with it
+ * every list is in ascending id order, as push_sorted keeps it, versioned_vec.rs:207-226).
+ *
+ * Score (search_bm25).  A query is a list of term hashes (the query's own tf is not used).  Hashes the index never saw are
+ * skipped; a repeated hash counts once per occurrence.  A document's score is its first product tf * idf, then += of the
+ * later ones, f32 without FMA and not started from 0 (0 + -0 would turn a -0 score into +0).  The products are added in
+ * the caller's query-term order.  The reference adds them in its BinaryHeap's pop order, which is the same for documents
+ * that match at most 2 query terms (f32 addition commutes); with more terms the two can differ in the last bits, by at
+ * most gamma_{m-1} * (sum of the products) when every product is positive.  A term whose list has no live entry adds
+ * nothing; the reference can panic on it (unreachable! in PostingListHead::cmp once such a head meets another).
+ * Top-k (search_bm25's 512 buckets).  Document d competes in bucket d % 512 and replaces its holder only if
+ * score > bucket score (which starts at -inf): NaN and -inf never enter, equal scores (+0 and -0 too) stay with the smaller
+ * id.  The winners are sorted by f32::total_cmp descending (+0 above -0), ties to the smaller id (the reference's
+ * sort_unstable leaves ties open), and truncated to k; k = 0 is the reference's top_k None.  out_ids / out_scores have
+ * kout = (k == 0 || k > 512) ? 512 : k columns; unused slots hold CDB_INVALID_ID / 0, out_counts[q] = filled slots.
+ * Deleted rows are never results.
+ *
+ * Deviations.  Deleting a deleted row is a no-op (the reference decrements N again).  The reference packs an entry as
+ * id << 32 | tf bits and reads every word with bit 63 set as a tombstone, so it never returns an id >= 2^31; here every id
+ * below id_base + capacity_rows <= 2^32 - 1 is searched.
+ * Searches on one handle are re-entrant; append and delete take the handle exclusively and first wait for the searches
+ * already enqueued on the device.  An append that fails changes nothing.  Without a CUDA device every compute entry point
+ * returns CDB_CUDA_ERROR. */
+typedef struct cdb_tfidf_index cdb_tfidf_index; /* opaque */
+
+typedef struct {
+    int32_t device;
+    uint64_t capacity_rows;   /* id_base + capacity_rows <= 2^32 - 1 */
+    uint64_t capacity_pairs;  /* (term_hash, tf) pairs over all rows */
+    uint32_t id_base;
+} cdb_tfidf_index_desc;
+
+cdb_status cdb_tfidf_index_create(const cdb_tfidf_index_desc *desc, cdb_tfidf_index **out);
+cdb_status cdb_tfidf_index_destroy(cdb_tfidf_index *index);
+uint64_t cdb_tfidf_index_size(const cdb_tfidf_index *index);
+/* n rows inserted at `version`; row_offsets[n+1] (row_offsets[0] = 0), hashes / tfs [row_offsets[n]], counted [n] or NULL */
+cdb_status cdb_tfidf_index_append(cdb_tfidf_index *index, const uint64_t *row_offsets, const uint32_t *hashes, const float *tfs,
+                                  const uint8_t *counted, uint64_t n, uint32_t version);
+/* deletes rows[0..n) (local rows < cdb_tfidf_index_size) at `version` */
+cdb_status cdb_tfidf_index_delete_rows(cdb_tfidf_index *index, const uint32_t *rows, uint64_t n, uint32_t version);
+/* out[i] = 1 if row first+i is deleted (first + n <= capacity_rows); *out_total = deleted rows (either may be NULL) */
+cdb_status cdb_tfidf_index_deleted_rows(const cdb_tfidf_index *index, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total);
+/* df and the device's idf of hashes[0..n), and N; a hash the index never saw gets df 0 and idf NaN (any may be NULL) */
+cdb_status cdb_tfidf_index_term_stats(cdb_tfidf_index *index, const uint32_t *hashes, uint64_t n, uint32_t *out_df, float *out_idf,
+                                      uint32_t *out_documents_count);
+/* B queries as CSR of hashes (q_offsets[B+1]); out_ids / out_scores [B][kout], out_counts [B] */
+cdb_status cdb_tfidf_search_batch(cdb_tfidf_index *index, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t n_queries,
+                                  uint32_t k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts);
+/* same with every array in DEVICE memory on the index's device, asynchronous on `stream` (NULL = the legacy default stream) */
+cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *index, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes,
+                                         uint32_t n_queries, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                         void *stream);
+
 #ifdef __cplusplus
 }
 #endif
