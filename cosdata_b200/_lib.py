@@ -142,6 +142,22 @@ class TfIdfIndexDesc(C.Structure):
     ]
 
 
+class HybridSources(C.Structure):
+    _fields_ = [
+        ("dense", C.c_void_p),
+        ("dense_queries", C.c_void_p),
+        ("dense_params", SearchParams),
+        ("sparse", C.c_void_p),
+        ("sparse_offsets", C.c_void_p),
+        ("sparse_dims", C.c_void_p),
+        ("sparse_values", C.c_void_p),
+        ("sparse_params", SparseSearchParams),
+        ("tfidf", C.c_void_p),
+        ("tfidf_offsets", C.c_void_p),
+        ("tfidf_hashes", C.c_void_p),
+    ]
+
+
 # symbol -> (restype, argtypes); must list every function of include/cosdata_b200.h
 PROTOTYPES = {
     "cdb_abi_version": (C.c_int32, []),
@@ -249,6 +265,14 @@ PROTOTYPES = {
     "cdb_tfidf_search_batch": (C.c_int32, [C.c_void_p, c_vp, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p]),
     "cdb_tfidf_search_batch_device": (C.c_int32, [C.c_void_p, c_vp, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p,
                                                   C.c_void_p]),
+    "cdb_rrf_fuse": (C.c_int32, [C.c_int32, c_u32p, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_u32p, C.c_uint32, C.c_uint32,
+                                 C.c_uint32, C.c_float, C.c_uint32, c_u32p, c_f32p, c_u32p]),
+    "cdb_rrf_fuse_device": (C.c_int32, [C.c_int32, c_u32p, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_u32p, C.c_uint32,
+                                        C.c_uint32, C.c_uint32, C.c_float, C.c_uint32, c_u32p, c_f32p, c_u32p, C.c_void_p]),
+    "cdb_hybrid_search_batch": (C.c_int32, [C.POINTER(HybridSources), C.c_uint32, C.c_uint32, C.c_float, c_u32p, c_f32p, c_u32p,
+                                            c_u8p]),
+    "cdb_hybrid_search_batch_device": (C.c_int32, [C.POINTER(HybridSources), C.c_uint32, C.c_uint32, C.c_float, c_u32p, c_f32p,
+                                                   c_u32p, c_u8p, C.c_void_p]),
 }
 
 _lib = None

@@ -1071,3 +1071,75 @@ class TfIdfIndex:
         ids, scores, counts = self.batch_search([list(query)], top_k)
         c = int(counts[0])
         return list(zip(ids[0, :c].tolist(), scores[0, :c].tolist()))
+
+
+# ---------------------------------------------------------------- hybrid search (reciprocal-rank fusion)
+def rrf_fuse(first_ids, first_counts, second_ids, second_counts, fusion_constant_k=60.0, id_strides=(1, 1), device=0):
+    """batch_hybrid_search's fusion of two ranked id lists per query (cdb_rrf_fuse): ids u32[B, ld], counts u32[B] per list,
+    id_strides = the max_replica_per_node of each list (0 or 1: ids are keys)
+    -> ids u32[B, ld_first + ld_second], scores f32[B, ...], counts u32[B]: every distinct key, total_cmp descending"""
+    a = np.ascontiguousarray(first_ids, dtype=np.uint32)
+    b = np.ascontiguousarray(second_ids, dtype=np.uint32)
+    if a.ndim == 1:
+        a = a[None]
+    if b.ndim == 1:
+        b = b[None]
+    ca = np.ascontiguousarray(np.atleast_1d(first_counts), dtype=np.uint32)
+    cb = np.ascontiguousarray(np.atleast_1d(second_counts), dtype=np.uint32)
+    nq, ld_a, ld_b = a.shape[0], a.shape[1], b.shape[1]
+    if b.shape[0] != nq or ca.size != nq or cb.size != nq:
+        raise ValueError("both lists need the same number of queries")
+    ld = ld_a + ld_b
+    ids = np.zeros((max(nq, 1), max(ld, 1)), np.uint32)
+    scores = np.zeros((max(nq, 1), max(ld, 1)), np.float32)
+    counts = np.zeros(max(nq, 1), np.uint32)
+    _check(_lib.load().cdb_rrf_fuse(device, _ptr(a), _ptr(ca), ld_a, int(id_strides[0]), _ptr(b), _ptr(cb), ld_b, int(id_strides[1]),
+                                    nq, float(fusion_constant_k), ld, _ptr(ids), _ptr(scores), _ptr(counts)))
+    return ids[:nq, :ld], scores[:nq, :ld], counts[:nq]
+
+
+def hybrid_sources(dense=None, sparse=None, tfidf=None):
+    """the cdb_hybrid_sources of host queries -> (struct, arrays to keep alive, n_queries)
+    dense = (DenseIndex, queries f32[B, dim], DenseIndex.params keywords or None)
+    sparse = (SparseIndex, queries as for SparseIndex.batch_search, SparseSearchOptions or None)
+    tfidf = (TfIdfIndex, queries as for TfIdfIndex.batch_search[, None])"""
+    src, keep, nqs = _lib.HybridSources(), [], []
+    if dense is not None:
+        ix, q, opts = (tuple(dense) + (None,))[:3]
+        q = np.ascontiguousarray(q, dtype=np.float32)
+        if q.ndim == 1:
+            q = q[None]
+        src.dense, src.dense_queries, src.dense_params = ix._h, _ptr(q), ix.params(0, **(opts or {}))
+        keep.append(q)
+        nqs.append(q.shape[0])
+    if sparse is not None:
+        ix, q, opts = (tuple(sparse) + (None,))[:3]
+        o, d, v = _as_csr(q)
+        src.sparse, src.sparse_offsets, src.sparse_dims, src.sparse_values = ix.h, _ptr(o), _ptr(d), _ptr(v)
+        src.sparse_params = (opts or SparseSearchOptions(0)).params()
+        keep += [o, d, v]
+        nqs.append(len(o) - 1)
+    if tfidf is not None:
+        ix, q = tuple(tfidf)[:2]
+        o, h = _query_csr(q)
+        src.tfidf, src.tfidf_offsets, src.tfidf_hashes = ix.h, _ptr(o), _ptr(h)
+        keep += [o, h]
+        nqs.append(len(o) - 1)
+    if len(set(nqs)) > 1:
+        raise ValueError("every source needs the same number of queries")
+    return src, keep, (nqs[0] if nqs else 0)
+
+
+def hybrid_batch_search(top_k=10, fusion_constant_k=60.0, dense=None, sparse=None, tfidf=None):
+    """batch_hybrid_search over two of the three sources (cdb_hybrid_search_batch); see hybrid_sources for their form.
+    -> ids u32[B, 6 * top_k], scores f32[B, 6 * top_k], counts u32[B] (the whole fused union, not truncated to top_k, as in
+    the reference), dense err flags u8[B] (zeros without a dense source)"""
+    src, keep, nq = hybrid_sources(dense, sparse, tfidf)
+    w = 6 * int(top_k)
+    ids = np.zeros((max(nq, 1), max(w, 1)), np.uint32)
+    scores = np.zeros((max(nq, 1), max(w, 1)), np.float32)
+    counts = np.zeros(max(nq, 1), np.uint32)
+    err = np.zeros(max(nq, 1), np.uint8)
+    _check(_lib.load().cdb_hybrid_search_batch(C.byref(src), nq, int(top_k), float(fusion_constant_k), _ptr(ids), _ptr(scores),
+                                               _ptr(counts), _ptr(err)))
+    return ids[:nq, :w], scores[:nq, :w], counts[:nq], err[:nq]

@@ -25,6 +25,16 @@ void values_range_from_counts(const uint64_t *counts, uint64_t n_values, float c
 cdb_status sparse_index_room(cdb_sparse_index *ix, uint64_t *rows, uint64_t *rows_left, uint64_t *pairs_left);
 // drops the rows from `rows` on (their tombstones too): an append of several calls undone after a later call failed
 cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows);
+int sparse_index_device(const cdb_sparse_index *ix);
+
+// ---- tfidf.cu
+int tfidf_index_device(const cdb_tfidf_index *ix);
+
+// ---- api.cu
+int index_device(const cdb_index *ix);
+uint32_t index_dim(const cdb_index *ix);
+// graph metadata attached (results carry replica ids); read under the handle's shared lock
+bool index_has_graph_metadata(cdb_index *ix);
 
 // ---- pairs.cu
 cdb_status distance_pairs_device(int metric, int st, uint32_t dim, const uint8_t *d_x, const float *d_xm,

@@ -616,6 +616,8 @@ cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows) {
     CDB_CUDA_TRY(cudaDeviceSynchronize());
     return restore_rows(ix, rows, b, sg.s);
 }
+
+int sparse_index_device(const cdb_sparse_index *ix) { return ix->desc.device; }
 }  // namespace cdb
 
 extern "C" {

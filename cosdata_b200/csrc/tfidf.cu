@@ -443,6 +443,10 @@ cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint
 
 }  // namespace
 
+namespace cdb {
+int tfidf_index_device(const cdb_tfidf_index *ix) { return ix->desc.device; }
+}  // namespace cdb
+
 extern "C" {
 
 cdb_status cdb_tfidf_index_create(const cdb_tfidf_index_desc *desc, cdb_tfidf_index **out) {

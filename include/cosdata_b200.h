@@ -789,6 +789,89 @@ cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *index, const uint64_t 
                                          uint32_t n_queries, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
                                          void *stream);
 
+/* ------------------------------------------------ hybrid search (reciprocal-rank fusion)
+ * hybrid_search (src/api/vectordb/search/repo.rs:168-341) and batch_hybrid_search (repo.rs:343-555); request defaults
+ * top_k = 10, fusion_constant_k = 60.0 (src/api/vectordb/search/dtos.rs:6-12).
+ *
+ * Lists.  A request names two sources, DenseAndSparse, DenseAndTFIDF or SparseAndTFIDF (dtos.rs:73-90), and searches each
+ * with top_k Some(3 * top_k): the dense side is hnsw_index.search without a filter, TF-IDF returns at most 512 results (its
+ * buckets).  The first list is the one named first: dense before sparse, dense before TF-IDF, sparse before TF-IDF.
+ * Score.  The entry at 0-based position rank of a list contributes 1.0 / (rank as f32 + k + f32::EPSILON), f32, left to
+ * right, one rounding per operation ((rank + k) + eps and rank + (k + eps) round differently for some small negative k;
+ * never at k = 60).  The source's own score is not used.
+ * Key.  Entries are keyed by VectorId after remap_search_results (src/indexes/mod.rs:248-258), which is the internal id:
+ * a collection's indexes share them.  Dense results of a graph with metadata carry replica ids, which
+ * get_raw_emb_by_internal_id (src/models/collection.rs:358-384) maps to id - id % max_replica_per_node, so the replicas of
+ * one embedding are one key: id_stride = max_replica_per_node does the same here (0 or 1 = the id itself).
+ * Combining (FxHashMap final_scores).  First list: insert, so a key listed twice keeps its worse-ranked occurrence's
+ * score.  Second list: the batch form's and_modify(+=).or_insert(score) -- a key not in the first list starts from its
+ * first occurrence's score, every later occurrence adds.  Sums are f32 without FMA, in rank order.  The single form's
+ * or_insert(0.0).0 += score gives the same result except for a key only in the second list whose score is -0.0 (k = -inf),
+ * where 0.0 + -0.0 = +0.0; these entry points compute the batch form.
+ * Output.  Every distinct key, sorted by f32::total_cmp descending, ties to the smaller id (the reference's sort_unstable
+ * leaves them open).  The reference does NOT truncate to top_k (select_nth_unstable_by only partitions), so a query holds
+ * up to the whole union, 6 * top_k entries; a caller that wants top_k truncates.  Unused slots hold CDB_INVALID_ID / 0 and
+ * out_counts[q] = distinct keys.
+ * k.  Any f32: a negative k only logs a warning in the reference.  A zero denominator gives +inf, k = +inf gives +0 and
+ * k = -inf gives -0 scores, k near 3e38 gives subnormal scores (no flush to zero).  A NaN k makes every score NaN with
+ * k's payload and the quiet bit set (0xFFA00001 -> 0xFFE00001), as x86 SSE propagates it.  No other NaN or -inf arises.
+ * Threshold.  batch_hybrid_search searches the sparse side with early_terminate_threshold None (the config value) where
+ * hybrid_search passes the request's; here it is sparse_params.early_terminate_threshold, one value per call -- a single
+ * request is a batch of 1.  A batch that mixes kinds of request is split by kind pair by the caller (queries are
+ * independent, so the results do not change). */
+
+/* Generic fusion of two ranked id lists per query: ids [B][ld], counts [B] (entries below min(count, ld) are taken as
+ * given, CDB_INVALID_ID included), id_stride per list as above.  out_ids / out_scores [B][ld_out], out_counts [B].
+ * ld_first + ld_second > 2048 or ld_out < ld_first + ld_second: CDB_INVALID_PARAMS, checked before the device is touched.
+ * Use it for lists this library did not produce in one call: sharded dense results merged per query, or the replica-id
+ * results of cdb_search_batch_filtered (id_stride = max_replica_per_node). */
+cdb_status cdb_rrf_fuse(int32_t device, const uint32_t *first_ids, const uint32_t *first_counts, uint32_t ld_first,
+                        uint32_t first_id_stride, const uint32_t *second_ids, const uint32_t *second_counts, uint32_t ld_second,
+                        uint32_t second_id_stride, uint32_t n_queries, float fusion_constant_k, uint32_t ld_out, uint32_t *out_ids,
+                        float *out_scores, uint32_t *out_counts);
+/* same with every array in DEVICE memory on `device`, asynchronous on `stream` (NULL = the legacy default stream) */
+cdb_status cdb_rrf_fuse_device(int32_t device, const uint32_t *d_first_ids, const uint32_t *d_first_counts, uint32_t ld_first,
+                               uint32_t first_id_stride, const uint32_t *d_second_ids, const uint32_t *d_second_counts,
+                               uint32_t ld_second, uint32_t second_id_stride, uint32_t n_queries, float fusion_constant_k,
+                               uint32_t ld_out, uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts, void *stream);
+
+/* The two sources of a composed hybrid search: exactly two of the three handles are set (the third is NULL).  Queries are
+ * host arrays for cdb_hybrid_search_batch and device arrays for cdb_hybrid_search_batch_device.  The k of each params
+ * struct is ignored: every sub-search runs with k = 3 * top_k (TF-IDF: min(3 * top_k, 512) results). */
+typedef struct {
+    cdb_index *dense;
+    const float *dense_queries;               /* [B][dim] raw f32 */
+    cdb_search_params dense_params;           /* mode, ef_search, shortlist_size, ... of cdb_search_batch */
+    cdb_sparse_index *sparse;
+    const uint64_t *sparse_offsets;           /* CSR [B+1] */
+    const uint32_t *sparse_dims;
+    const float *sparse_values;
+    cdb_sparse_search_params sparse_params;
+    cdb_tfidf_index *tfidf;
+    const uint64_t *tfidf_offsets;            /* CSR [B+1] of term hashes */
+    const uint32_t *tfidf_hashes;
+} cdb_hybrid_sources;
+
+/* Composed hybrid search: both sub-searches through their public *_search_batch_device entry points, the second on a side
+ * stream forked from and joined back to the caller's stream (the device form's `stream`; NULL = the legacy default stream)
+ * so the two overlap, then the fusion on the caller's stream;
+ * intermediate lists live in stream-ordered scratch, and no stream, event or allocation outlives the call's work.
+ * out_ids / out_scores [B][6 * top_k], out_counts [B]; err_flags [B] (may be NULL) receives the dense search's flags and
+ * is written only when a dense source is given.
+ * Each sub-search takes its own handle's shared lock and sees that handle as of its own enqueue; there is no snapshot
+ * across the two handles (the reference takes none either).  Appends and deletes keep their contracts: they wait for the
+ * searches already enqueued on the device.
+ * CDB_INVALID_PARAMS: top_k > 341 (the dense and sparse searches take k <= 1024), a sparse source with rerank and
+ * 3 * top_k * reranking_factor > 5120, a source count other than two, null queries, handles on different devices.
+ * CDB_UNSUPPORTED: a dense handle with graph metadata (its HNSW searches go through the host-only cdb_search_batch_filtered;
+ * fuse those results with cdb_rrf_fuse and id_stride = max_replica_per_node).  Refusals of a sub-search's own parameter
+ * checks are returned as that search returns them.  top_k = 0: empty results (out_counts zeroed), no kernel launched. */
+cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k, float fusion_constant_k,
+                                   uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags);
+cdb_status cdb_hybrid_search_batch_device(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k,
+                                          float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                          uint8_t *d_err_flags, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
