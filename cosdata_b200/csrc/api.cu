@@ -245,11 +245,6 @@ static cdb_status lease_scratch(cdb_index *ix, Lease &l) {
     }
 }
 
-#define CDB_REQUIRE(cond, msg)                              \
-    do {                                                    \
-        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; } \
-    } while (0)
-
 extern "C" {
 
 int32_t cdb_abi_version(void) { return CDB_ABI_VERSION; }

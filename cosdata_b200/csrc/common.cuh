@@ -35,6 +35,26 @@ extern std::atomic<uint64_t> g_launch_count;
         }                                                                                      \
     } while (0)
 
+#define CDB_REQUIRE(cond, msg)                                                                 \
+    do {                                                                                       \
+        if (!(cond)) { ::cdb::set_error(msg); return CDB_INVALID_PARAMS; }                     \
+    } while (0)
+
+// a call's own stream: synchronized and destroyed on every way out
+struct StreamGuard {
+    cudaStream_t s = nullptr;
+    ~StreamGuard() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
+};
+
+// a CSR the caller passed (host): offsets start at 0 and never decrease
+inline cdb_status check_csr(const uint64_t *off, uint64_t n, const char *what) {
+    CDB_REQUIRE(off, "null offsets");
+    if (off[0] != 0) { set_error(std::string(what) + ": offsets[0] must be 0"); return CDB_INVALID_PARAMS; }
+    for (uint64_t i = 0; i < n; ++i)
+        if (off[i + 1] < off[i]) { set_error(std::string(what) + ": offsets decrease"); return CDB_INVALID_PARAMS; }
+    return CDB_OK;
+}
+
 // Opt a kernel in to the device's maximum dynamic shared memory ONCE (per device and kernel).  Setting the attribute to
 // the size of the launch at hand, as every launch site used to, races when searches run concurrently on one handle: a
 // thread lowers the limit between another thread's cudaFuncSetAttribute and its launch ("invalid argument").  The carve-out
@@ -95,6 +115,22 @@ __host__ __device__ inline uint32_t key64_id(uint64_t k) { return ~(uint32_t)(k 
 // operations such as 0/0; CUDA produces 0x7FFFFFFF.  total_cmp orders the two
 // at opposite ends, so results are canonicalised to the reference platform's.
 __device__ inline float canon_nan(float v) { return (v != v) ? __uint_as_float(0xFFC00000u) : v; }
+
+// ascending (DESC = false) or descending bitonic sort of s[0..n), n a power of two, by all threads of the block
+template <bool DESC>
+__device__ void bitonic_sort(uint64_t *s, uint32_t n) {
+    for (uint32_t size = 2; size <= n; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            for (uint32_t t = threadIdx.x; t < n / 2; t += blockDim.x) {
+                const uint32_t lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+                const bool dir = ((lo & size) == 0) == DESC;
+                const uint64_t x = s[lo], y = s[hi];
+                if ((x < y) == dir) { s[lo] = y; s[hi] = x; }
+            }
+            __syncthreads();
+        }
+    }
+}
 
 // ---------------------------------------------------------------- synthetic data
 __host__ __device__ inline float synth_value(uint64_t seed, uint64_t idx) {

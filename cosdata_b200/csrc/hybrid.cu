@@ -34,22 +34,6 @@ __device__ __forceinline__ float rrf_contribution(uint32_t rank, float k) {
 
 __device__ __forceinline__ uint32_t rrf_key(uint32_t id, uint32_t stride) { return stride <= 1 ? id : id - id % stride; }
 
-// ascending (DESC = false) or descending bitonic sort of s[0..n), n a power of two, by all threads of the block
-template <bool DESC>
-__device__ void bitonic_sort(uint64_t *s, uint32_t n) {
-    for (uint32_t size = 2; size <= n; size <<= 1) {
-        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-            for (uint32_t t = threadIdx.x; t < n / 2; t += blockDim.x) {
-                const uint32_t lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-                const bool dir = ((lo & size) == 0) == DESC;
-                const uint64_t x = s[lo], y = s[hi];
-                if ((x < y) == dir) { s[lo] = y; s[hi] = x; }
-            }
-            __syncthreads();
-        }
-    }
-}
-
 __global__ void __launch_bounds__(1024) rrf_fuse_kernel(RrfList a, RrfList b, float k, uint32_t n_sort, uint32_t ld_out,
                                                         uint32_t *__restrict__ out_ids, float *__restrict__ out_scores,
                                                         uint32_t *__restrict__ out_counts) {
@@ -108,18 +92,13 @@ __global__ void __launch_bounds__(1024) rrf_fuse_kernel(RrfList a, RrfList b, fl
     if (tid == 0) out_counts[q] = cnt;
 }
 
-#define HY_REQUIRE(cond, msg)                                              \
-    do {                                                                   \
-        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; }        \
-    } while (0)
-
 cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t ld_out, const void *ids_a, const void *cnt_a,
                            const void *ids_b, const void *cnt_b, const void *out_ids, const void *out_scores, const void *out_counts) {
-    HY_REQUIRE((uint64_t)ld_a + ld_b <= RRF_MAX, "ld_first + ld_second must be <= 2048");
-    HY_REQUIRE(ld_out >= ld_a + ld_b, "ld_out must be >= ld_first + ld_second");
-    HY_REQUIRE(!nq || (cnt_a && cnt_b && out_counts), "null counts");
-    HY_REQUIRE(!nq || ((ids_a || !ld_a) && (ids_b || !ld_b)), "null ids");
-    HY_REQUIRE(!nq || !ld_out || (out_ids && out_scores), "null output");
+    CDB_REQUIRE((uint64_t)ld_a + ld_b <= RRF_MAX, "ld_first + ld_second must be <= 2048");
+    CDB_REQUIRE(ld_out >= ld_a + ld_b, "ld_out must be >= ld_first + ld_second");
+    CDB_REQUIRE(!nq || (cnt_a && cnt_b && out_counts), "null counts");
+    CDB_REQUIRE(!nq || ((ids_a || !ld_a) && (ids_b || !ld_b)), "null ids");
+    CDB_REQUIRE(!nq || !ld_out || (out_ids && out_scores), "null output");
     return CDB_OK;
 }
 
@@ -134,11 +113,6 @@ cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k,
     return CDB_OK;
 }
 
-struct StreamGuard {
-    cudaStream_t s = nullptr;
-    ~StreamGuard() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
-};
-
 enum Source { SRC_DENSE = 0, SRC_SPARSE = 1, SRC_TFIDF = 2 };
 
 struct Plan {
@@ -147,36 +121,29 @@ struct Plan {
     int device;
 };
 
-cdb_status check_csr(const uint64_t *off, uint32_t n, const char *what) {
-    if (off[0] != 0) { set_error(std::string(what) + ": offsets[0] must be 0"); return CDB_INVALID_PARAMS; }
-    for (uint32_t i = 0; i < n; ++i)
-        if (off[i + 1] < off[i]) { set_error(std::string(what) + ": offsets decrease"); return CDB_INVALID_PARAMS; }
-    return CDB_OK;
-}
-
 // every refusal that needs no device: the handles are read only after the request itself is well-formed
 cdb_status make_plan(const cdb_hybrid_sources *h, uint32_t nq, uint32_t top_k, Plan *p) {
-    HY_REQUIRE(h, "null sources");
-    HY_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
+    CDB_REQUIRE(h, "null sources");
+    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
     const int n_src = (h->dense != nullptr) + (h->sparse != nullptr) + (h->tfidf != nullptr);
-    HY_REQUIRE(n_src == 2, "a hybrid search takes exactly two sources");
+    CDB_REQUIRE(n_src == 2, "a hybrid search takes exactly two sources");
     const uint32_t k3 = 3 * top_k;
     int i = 0;
     if (h->dense) { p->src[i] = SRC_DENSE; p->ld[i++] = k3; }
     if (h->sparse) { p->src[i] = SRC_SPARSE; p->ld[i++] = k3; }
     if (h->tfidf) { p->src[i] = SRC_TFIDF; p->ld[i++] = std::min(k3, TF_RESULTS); }
-    HY_REQUIRE(!h->dense || h->dense_queries || !nq, "null dense queries");
-    HY_REQUIRE(!h->sparse || h->sparse_offsets || !nq, "null sparse query offsets");
-    HY_REQUIRE(!h->tfidf || h->tfidf_offsets || !nq, "null tf-idf query offsets");
+    CDB_REQUIRE(!h->dense || h->dense_queries || !nq, "null dense queries");
+    CDB_REQUIRE(!h->sparse || h->sparse_offsets || !nq, "null sparse query offsets");
+    CDB_REQUIRE(!h->tfidf || h->tfidf_offsets || !nq, "null tf-idf query offsets");
     if (h->sparse && h->sparse_params.rerank)
-        HY_REQUIRE(h->sparse_params.reranking_factor >= 1 && (uint64_t)k3 * h->sparse_params.reranking_factor <= 5120,
+        CDB_REQUIRE(h->sparse_params.reranking_factor >= 1 && (uint64_t)k3 * h->sparse_params.reranking_factor <= 5120,
                    "3 * top_k * reranking_factor must be in 1..5120");
     // the handles' devices (immutable after create)
     int dev[2];
     for (int j = 0; j < 2; ++j)
         dev[j] = p->src[j] == SRC_DENSE ? index_device(h->dense)
                : p->src[j] == SRC_SPARSE ? sparse_index_device(h->sparse) : tfidf_index_device(h->tfidf);
-    HY_REQUIRE(dev[0] == dev[1], "the two handles live on different devices");
+    CDB_REQUIRE(dev[0] == dev[1], "the two handles live on different devices");
     p->device = dev[0];
     if (h->dense && index_has_graph_metadata(h->dense)) {
         set_error("a dense handle with graph metadata searches through cdb_search_batch_filtered: fuse with cdb_rrf_fuse");
@@ -318,7 +285,7 @@ cdb_status cdb_rrf_fuse(int32_t device, const uint32_t *first_ids, const uint32_
 
 cdb_status cdb_hybrid_search_batch_device(const cdb_hybrid_sources *sources, uint32_t nq, uint32_t top_k, float fusion_constant_k,
                                           uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err_flags, void *stream) {
-    HY_REQUIRE(!nq || !top_k || (d_ids && d_scores && d_counts), "null output");
+    CDB_REQUIRE(!nq || !top_k || (d_ids && d_scores && d_counts), "null output");
     Plan p;
     cdb_status rc = make_plan(sources, nq, top_k, &p);
     if (rc) return rc;
@@ -334,7 +301,7 @@ cdb_status cdb_hybrid_search_batch_device(const cdb_hybrid_sources *sources, uin
 
 cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t nq, uint32_t top_k, float fusion_constant_k,
                                    uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
-    HY_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
+    CDB_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
     Plan p;
     cdb_status rc = make_plan(sources, nq, top_k, &p);
     if (rc) return rc;
@@ -343,12 +310,12 @@ cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t n
     if (nq && h.sparse) {
         if ((rc = check_csr(h.sparse_offsets, nq, "sparse_offsets"))) return rc;
         sp_pairs = h.sparse_offsets[nq];
-        HY_REQUIRE((h.sparse_dims && h.sparse_values) || !sp_pairs, "null sparse query pairs");
+        CDB_REQUIRE((h.sparse_dims && h.sparse_values) || !sp_pairs, "null sparse query pairs");
     }
     if (nq && h.tfidf) {
         if ((rc = check_csr(h.tfidf_offsets, nq, "tfidf_offsets"))) return rc;
         tf_hashes = h.tfidf_offsets[nq];
-        HY_REQUIRE(h.tfidf_hashes || !tf_hashes, "null tf-idf query hashes");
+        CDB_REQUIRE(h.tfidf_hashes || !tf_hashes, "null tf-idf query hashes");
     }
     CDB_CUDA_TRY(cudaSetDevice(p.device));
     if (!nq) return CDB_OK;

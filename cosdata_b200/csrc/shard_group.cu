@@ -150,11 +150,6 @@ struct cdb_shard_group {
     std::mutex mu;
 };
 
-#define CDB_REQUIRE_G(cond, msg)                                   \
-    do {                                                           \
-        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; } \
-    } while (0)
-
 static cdb_status group_alloc_slots(cdb_shard_group *g, size_t n) {
     g->comm.assign(n, nullptr);
     g->shard.assign(n, nullptr);
@@ -172,7 +167,7 @@ static cdb_status group_alloc_slots(cdb_shard_group *g, size_t n) {
 extern "C" {
 
 cdb_status cdb_nccl_unique_id(uint8_t *out_id128) {
-    CDB_REQUIRE_G(out_id128, "null argument");
+    CDB_REQUIRE(out_id128, "null argument");
     NcclApi *n = nccl_api();
     if (!n) { set_error("libnccl.so.2 not found"); return CDB_NCCL_ERROR; }
     ncclUniqueId id;
@@ -183,7 +178,7 @@ cdb_status cdb_nccl_unique_id(uint8_t *out_id128) {
 }
 
 cdb_status cdb_shard_group_create(const int32_t *device_ordinals, uint32_t n_devices, cdb_shard_group **out) {
-    CDB_REQUIRE_G(device_ordinals && out && n_devices >= 1 && n_devices <= 64, "bad argument");
+    CDB_REQUIRE(device_ordinals && out && n_devices >= 1 && n_devices <= 64, "bad argument");
     std::unique_ptr<cdb_shard_group> g(new cdb_shard_group());
     g->world = n_devices;
     g->dev.assign(device_ordinals, device_ordinals + n_devices);
@@ -207,7 +202,7 @@ cdb_status cdb_shard_group_create(const int32_t *device_ordinals, uint32_t n_dev
 }
 
 cdb_status cdb_shard_group_create_rank(const uint8_t *id128, uint32_t world, uint32_t rank, int32_t device, cdb_shard_group **out) {
-    CDB_REQUIRE_G(out && world >= 1 && rank < world && (id128 || world == 1), "bad argument");
+    CDB_REQUIRE(out && world >= 1 && rank < world && (id128 || world == 1), "bad argument");
     std::unique_ptr<cdb_shard_group> g(new cdb_shard_group());
     g->world = world;
     g->rank0 = rank;
@@ -248,9 +243,9 @@ cdb_status cdb_shard_group_destroy(cdb_shard_group *g) {
 }
 
 cdb_status cdb_shard_group_attach(cdb_shard_group *g, uint32_t local_slot, cdb_index *shard) {
-    CDB_REQUIRE_G(g && shard && local_slot < g->dev.size(), "bad argument");
-    CDB_REQUIRE_G(index_device(shard) == g->dev[local_slot], "the shard lives on another device than the group slot");
-    CDB_REQUIRE_G(g->shard[0] == nullptr || local_slot == 0 || index_dim(shard) == index_dim(g->shard[0]), "shards differ in dimension");
+    CDB_REQUIRE(g && shard && local_slot < g->dev.size(), "bad argument");
+    CDB_REQUIRE(index_device(shard) == g->dev[local_slot], "the shard lives on another device than the group slot");
+    CDB_REQUIRE(g->shard[0] == nullptr || local_slot == 0 || index_dim(shard) == index_dim(g->shard[0]), "shards differ in dimension");
     g->shard[local_slot] = shard;
     return CDB_OK;
 }
@@ -265,7 +260,7 @@ static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_sea
     const size_t words = slot_words(nq, k);
     cdb_status rc;
     for (size_t i = 0; i < nl; ++i) {
-        CDB_REQUIRE_G(g->shard[i], "a group slot has no shard attached");
+        CDB_REQUIRE(g->shard[i], "a group slot has no shard attached");
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
         if ((rc = g->gather[i].ensure(g->world * words * 8)) || (rc = g->ids[i].ensure((size_t)nq * k * 4)) ||
             (rc = g->scores[i].ensure((size_t)nq * k * 4)) || (rc = g->counts[i].ensure((size_t)nq * 4)))
@@ -315,12 +310,12 @@ static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_sea
 
 cdb_status cdb_search_batch_sharded(cdb_shard_group *g, const float *queries, uint32_t nq, const cdb_search_params *p,
                                     uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
-    CDB_REQUIRE_G(g && p && (queries || !nq) && (out_ids || !nq) && (out_scores || !nq), "null argument");
-    CDB_REQUIRE_G(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    CDB_REQUIRE(g && p && (queries || !nq) && (out_ids || !nq) && (out_scores || !nq), "null argument");
+    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
     if (!nq) return CDB_OK;
     std::lock_guard<std::mutex> lock(g->mu);
     const size_t nl = g->dev.size();
-    CDB_REQUIRE_G(g->shard[0], "a group slot has no shard attached");
+    CDB_REQUIRE(g->shard[0], "a group slot has no shard attached");
     const uint32_t dim = index_dim(g->shard[0]);
     const size_t nk = (size_t)nq * p->k;
     cdb_status rc;
@@ -356,9 +351,9 @@ cdb_status cdb_search_batch_sharded(cdb_shard_group *g, const float *queries, ui
 cdb_status cdb_search_batch_sharded_device(cdb_shard_group *g, const float *d_queries, uint32_t nq, const cdb_search_params *p,
                                            uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts, uint8_t *d_err_flags,
                                            void *stream) {
-    CDB_REQUIRE_G(g && p && (d_queries || !nq) && (d_out_ids || !nq) && (d_out_scores || !nq), "null argument");
-    CDB_REQUIRE_G(g->dev.size() == 1, "the device form serves one-process-per-GPU groups (cdb_shard_group_create_rank)");
-    CDB_REQUIRE_G(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    CDB_REQUIRE(g && p && (d_queries || !nq) && (d_out_ids || !nq) && (d_out_scores || !nq), "null argument");
+    CDB_REQUIRE(g->dev.size() == 1, "the device form serves one-process-per-GPU groups (cdb_shard_group_create_rank)");
+    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
     if (!nq) return CDB_OK;
     std::lock_guard<std::mutex> lock(g->mu);
     std::vector<const float *> d_q(1, d_queries);

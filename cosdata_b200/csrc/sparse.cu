@@ -2,42 +2,31 @@
 // of posting lists (SparseAnnQueryBasic::sequential_search, src/models/sparse_ann_query.rs:68-147), the raw-value re-rank
 // (finalize_sparse_ann_results, inverted/mod.rs:331-381) and the values_upper_bound sampler (inverted/mod.rs:148-247).
 //
-// Layout (DESIGN.md section 8c).  Rows are kept as raw CSR on the device (dims u32, values f32, u64 row offsets).  Posting
-// lists are split into row tiles of 2^15 rows; a tile holds its distinct dims (ascending), one segment per dim and packed
-// u32 entries row_in_tile << 8 | key, sorted by key descending inside a segment.  An append rebuilds the last partial tile
-// and builds the new ones (CUB radix sort).  A search scores one (query, tile) per CTA into shared-memory u32 accumulators
-// plus a touched flag per row, selects the tile's top k*f touched rows exactly (radix select on (sim << 32) | ~id), merges
-// the tile lists, then sorts (and re-ranks) the survivors.
+// Layout (DESIGN.md section 8c).  The rows and posting tiles are a PostingTiles store (posting_tiles.cuh) keyed by dim, with
+// packed u32 entries row_in_tile << 8 | key, sorted by key descending inside a segment.  A search scores one (query, tile)
+// per CTA into shared-memory u32 accumulators plus a touched flag per row, selects the tile's top k*f touched rows exactly
+// (radix select on (sim << 32) | ~id), merges the tile lists, then sorts (and re-ranks) the survivors.
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <mutex>
 #include <shared_mutex>
 #include <vector>
 
 #include <cub/block/block_scan.cuh>
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
 
 #include "kernels.h"
+#include "posting_tiles.cuh"
 
 namespace cdb {
 namespace {
 
-constexpr uint32_t SP_TILE_SHIFT = 15;
-constexpr uint32_t SP_TILE = 1u << SP_TILE_SHIFT;
 constexpr int SP_THREADS = 512;
 constexpr uint32_t SP_QCHUNK = SP_THREADS;       // query pairs resolved per pass of the scoring kernel
 constexpr uint32_t SP_MAX_K = 1024;
 constexpr uint32_t SP_MAX_CAND = 5120;       // k * reranking_factor
 constexpr uint32_t SP_MERGE_KEYS = 25600;    // keys a merge CTA holds in shared memory (200 KB)
 constexpr uint32_t SP_MERGE_MAX_LISTS = 63;  // lists a merge CTA takes at once
-
-struct SpTile {
-    uint64_t entry_base;   // first entry of the tile in d_entries
-    uint64_t dim_base;     // first distinct dim in d_tdims; its segment starts are d_tseg[dim_base + tile ..]
-    uint32_t n_dims;
-    uint32_t pad;
-};
 
 // InvertedIndexNode::quantize (src/models/inverted_index.rs:168-172): an f32 divide then an f32 multiply (no FMA), clamp
 // keeps NaN, the saturating `as u8` sends NaN to 0
@@ -50,36 +39,20 @@ __device__ inline uint32_t sparse_quantize(float v, float ub, uint32_t maxq) {
     return q < maxq ? q : maxq;
 }
 
-// ---------------------------------------------------------------- build side
-__global__ void sp_tile_keys_kernel(const uint64_t *__restrict__ row_off, uint64_t r0, uint32_t nr, uint64_t p0,
-                                    const uint32_t *__restrict__ dims, const float *__restrict__ vals, float ub, uint32_t maxq,
-                                    uint64_t *__restrict__ sort_keys, uint32_t *__restrict__ sort_vals) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= nr) return;
-    const uint64_t b = row_off[r0 + warp], e = row_off[r0 + warp + 1];
-    for (uint64_t p = b + lane; p < e; p += 32) {
-        const uint32_t key = sparse_quantize(vals[p], ub, maxq);
-        sort_keys[p - p0] = ((uint64_t)dims[p] << 8) | (255u - key);
-        sort_vals[p - p0] = (warp << 8) | key;
+// posting entries row_in_tile << 8 | key, sorted on dim << 8 | 255 - key: key-descending inside a dim's segment, so the
+// keys >= etv of a low query value are a prefix of it.  A row may repeat a dim.
+struct SparseCodec {
+    using Entry = uint32_t;
+    static constexpr int END_BIT = 40, SEG_SHIFT = 8;
+    static constexpr const char *DUPLICATE_ERROR = nullptr;
+    float ub;
+    uint32_t maxq;
+    __device__ SortPair encode(uint32_t dim, float v, uint32_t row) const {
+        const uint32_t key = sparse_quantize(v, ub, maxq);
+        return {((uint64_t)dim << 8) | (255u - key), (row << 8) | key};
     }
-}
-
-__global__ void sp_seg_flags_kernel(const uint64_t *__restrict__ keys, uint32_t n, uint32_t *__restrict__ flags) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) flags[i] = (i == 0 || (keys[i] >> 8) != (keys[i - 1] >> 8)) ? 1u : 0u;
-}
-
-__global__ void sp_seg_scatter_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ flags,
-                                      const uint32_t *__restrict__ pos, uint32_t n, uint32_t *__restrict__ tdims,
-                                      uint32_t *__restrict__ tseg) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (flags[i]) {
-        tdims[pos[i] - 1] = (uint32_t)(keys[i] >> 8);
-        tseg[pos[i] - 1] = i;
-    }
-    if (i == n - 1) tseg[pos[i]] = n;
-}
+    __device__ Entry entry(uint64_t, uint32_t v) const { return v; }
+};
 
 // ---------------------------------------------------------------- search side
 // Exact threshold of the top `need` keys among the non-zero keys key_at(0..n) (unique; more than `need` of them):
@@ -128,7 +101,7 @@ __device__ uint64_t sp_select_threshold(uint32_t n, uint32_t need, KeyAt key_at,
 
 struct SpSearch {
     const uint32_t *entries, *tdims, *tseg, *deleted;
-    const SpTile *tiles;
+    const PostingTile *tiles;
     uint64_t n_rows;
     uint32_t id_base, maxq, etv, low;
     float ub;
@@ -142,13 +115,13 @@ struct SpSearch {
     uint32_t *out_cnt;      // [chunk][n_tiles]
 };
 
-constexpr size_t SP_SCORE_SMEM = (size_t)SP_TILE * 4 + SP_TILE + SP_QCHUNK * 8 + (SP_QCHUNK + 1) * 8 + SP_QCHUNK * 4 + 260 * 4;
+constexpr size_t SP_SCORE_SMEM = (size_t)TILE_ROWS * 4 + TILE_ROWS + SP_QCHUNK * 8 + (SP_QCHUNK + 1) * 8 + SP_QCHUNK * 4 + 260 * 4;
 
 __global__ void __launch_bounds__(SP_THREADS, 1) sp_score_tile_kernel(SpSearch a) {
     extern __shared__ __align__(16) uint8_t smem[];
     uint32_t *acc = reinterpret_cast<uint32_t *>(smem);
-    uint8_t *touched = smem + (size_t)SP_TILE * 4;
-    uint64_t *c_beg = reinterpret_cast<uint64_t *>(touched + SP_TILE);
+    uint8_t *touched = smem + (size_t)TILE_ROWS * 4;
+    uint64_t *c_beg = reinterpret_cast<uint64_t *>(touched + TILE_ROWS);
     uint64_t *c_pre = c_beg + SP_QCHUNK;
     uint32_t *c_qv = reinterpret_cast<uint32_t *>(c_pre + SP_QCHUNK + 1);
     uint32_t *hist = c_qv + SP_QCHUNK;   // 256 + state[4]
@@ -157,18 +130,18 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_score_tile_kernel(SpSearch a
     __shared__ uint32_t s_cnt;
 
     const uint32_t t = blockIdx.x, qi = blockIdx.y, q = a.q0 + qi, tid = threadIdx.x;
-    const SpTile tile = a.tiles[t];
-    const uint64_t row0 = (uint64_t)t << SP_TILE_SHIFT;
-    const uint32_t nr = (uint32_t)std::min<uint64_t>(SP_TILE, a.n_rows - row0);
+    const PostingTile tile = a.tiles[t];
+    const uint64_t row0 = (uint64_t)t << TILE_SHIFT;
+    const uint32_t nr = (uint32_t)std::min<uint64_t>(TILE_ROWS, a.n_rows - row0);
     uint4 *a4 = reinterpret_cast<uint4 *>(acc);
-    for (uint32_t i = tid; i < SP_TILE / 4; i += SP_THREADS) a4[i] = make_uint4(0, 0, 0, 0);
+    for (uint32_t i = tid; i < TILE_ROWS / 4; i += SP_THREADS) a4[i] = make_uint4(0, 0, 0, 0);
     uint4 *t4 = reinterpret_cast<uint4 *>(touched);
-    for (uint32_t i = tid; i < SP_TILE / 16; i += SP_THREADS) t4[i] = make_uint4(0, 0, 0, 0);
+    for (uint32_t i = tid; i < TILE_ROWS / 16; i += SP_THREADS) t4[i] = make_uint4(0, 0, 0, 0);
     if (tid == 0) s_cnt = 0;
     __syncthreads();   // an empty query reaches the touched scan below without passing another barrier
 
-    const uint32_t *tdims = a.tdims + tile.dim_base;
-    const uint32_t *tseg = a.tseg + tile.dim_base + t;
+    const uint32_t *tdims = a.tdims + tile.key_base;
+    const uint32_t *tseg = a.tseg + tile.key_base + t;
     const uint32_t *ent = a.entries + tile.entry_base;
     const uint64_t qb = a.q_off[q], qe = a.q_off[q + 1];
     for (uint64_t j0 = qb; j0 < qe; j0 += SP_QCHUNK) {
@@ -177,10 +150,9 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_score_tile_kernel(SpSearch a
         if (tid < nj) {
             const uint32_t d = a.q_dims[j0 + tid];
             const uint32_t qv = sparse_quantize(a.q_vals[j0 + tid], a.ub, a.maxq);
-            uint32_t lo = 0, hi = tile.n_dims;        // first tile dim >= d
-            while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (tdims[mid] < d) lo = mid + 1; else hi = mid; }
+            const uint32_t lo = lower_bound_u32(tdims, tile.n_keys, d);
             uint32_t s = 0, e = 0;
-            if (lo < tile.n_dims && tdims[lo] == d) {
+            if (lo < tile.n_keys && tdims[lo] == d) {
                 s = tseg[lo]; e = tseg[lo + 1];
                 if (!(qv > a.low)) {                  // keys etv..=max only: a prefix of the key-descending segment
                     uint32_t l2 = s, h2 = e;
@@ -322,18 +294,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_finalize_kernel(const uint64
         }
         __syncthreads();
     }
-    // bitonic sort, descending
-    for (uint32_t size = 2; size <= P; size <<= 1) {
-        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-            for (uint32_t i = tid; i < P / 2; i += SP_THREADS) {
-                const uint32_t lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                const bool desc = (lo & size) == 0;
-                const uint64_t x = keys[lo], y = keys[hi];
-                if ((x < y) == desc) { keys[lo] = y; keys[hi] = x; }
-            }
-            __syncthreads();
-        }
-    }
+    bitonic_sort<true>(keys, P);
     const uint32_t cnt = min(n, k);
     for (uint32_t i = tid; i < k; i += SP_THREADS) {
         uint32_t id = CDB_INVALID_ID;
@@ -380,129 +341,16 @@ using namespace cdb;
 struct cdb_sparse_index {
     cdb_sparse_index_desc desc;
     std::shared_mutex rw;
-    uint32_t maxq = 15;
-    uint64_t n_rows = 0, n_pairs = 0, n_deleted = 0;
-    std::vector<uint64_t> h_row_off{0};
-    std::vector<SpTile> h_tiles;
-    std::vector<uint32_t> h_deleted;
-    uint64_t *d_row_off = nullptr;
-    uint32_t *d_dims = nullptr, *d_entries = nullptr, *d_tdims = nullptr, *d_tseg = nullptr, *d_deleted = nullptr;
-    float *d_vals = nullptr;
-    SpTile *d_tiles = nullptr;
-    uint64_t max_tiles = 0;
-    int sms = 0;
-    ~cdb_sparse_index() {
-        for (void *p : {(void *)d_row_off, (void *)d_dims, (void *)d_entries, (void *)d_tdims, (void *)d_tseg, (void *)d_deleted,
-                        (void *)d_vals, (void *)d_tiles})
-            if (p) cudaFree(p);
-    }
+    PostingTiles<SparseCodec> st;   // keys: dims
 };
-
-#define SP_REQUIRE(cond, msg)                                              \
-    do {                                                                   \
-        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; }        \
-    } while (0)
 
 namespace {
 
-// CUB temp storage + sort buffers of one append, sized for its largest tile
-struct BuildBufs {
-    void *tmp = nullptr;
-    size_t tmp_bytes = 0;
-    uint64_t *keys_in = nullptr, *keys_out = nullptr;
-    uint32_t *vals_in = nullptr, *flags = nullptr, *pos = nullptr;
-    ~BuildBufs() {
-        for (void *p : {tmp, (void *)keys_in, (void *)keys_out, (void *)vals_in, (void *)flags, (void *)pos})
-            if (p) cudaFree(p);
-    }
-};
-
-// posting lists of tile t (rows [t*TILE, min(n_rows, (t+1)*TILE))) appended after the tiles below it
-cdb_status build_tile(cdb_sparse_index *ix, uint64_t t, BuildBufs &b, cudaStream_t s) {
-    const uint64_t r0 = t << SP_TILE_SHIFT, r1 = std::min<uint64_t>(ix->n_rows, r0 + SP_TILE);
-    const uint64_t p0 = ix->h_row_off[r0], p1 = ix->h_row_off[r1];
-    const uint32_t np = (uint32_t)(p1 - p0);
-    SpTile tile;
-    tile.entry_base = p0;   // a tile's entries are its rows' pairs, re-ordered
-    tile.dim_base = t ? ix->h_tiles[t - 1].dim_base + ix->h_tiles[t - 1].n_dims : 0;
-    tile.n_dims = 0;
-    tile.pad = 0;
-    uint32_t *tseg = ix->d_tseg + tile.dim_base + t;
-    if (np == 0) {
-        CDB_CUDA_TRY(cudaMemsetAsync(tseg, 0, 4, s));
-    } else {
-        const uint32_t nr = (uint32_t)(r1 - r0);
-        sp_tile_keys_kernel<<<(nr * 32 + 255) / 256, 256, 0, s>>>(ix->d_row_off, r0, nr, p0, ix->d_dims, ix->d_vals,
-                                                                   ix->desc.values_upper_bound, ix->maxq, b.keys_in, b.vals_in);
-        CDB_LAUNCH_CHECK();
-        size_t tb = b.tmp_bytes;
-        CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tb, b.keys_in, b.keys_out, b.vals_in, ix->d_entries + tile.entry_base,
-                                                     (int)np, 0, 40, s));
-        sp_seg_flags_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, np, b.flags);
-        CDB_LAUNCH_CHECK();
-        tb = b.tmp_bytes;
-        CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(b.tmp, tb, b.flags, b.pos, (int)np, s));
-        sp_seg_scatter_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, b.flags, b.pos, np, ix->d_tdims + tile.dim_base, tseg);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemcpyAsync(&tile.n_dims, b.pos + np - 1, 4, cudaMemcpyDeviceToHost, s));
-        CDB_CUDA_TRY(cudaStreamSynchronize(s));
-    }
-    ix->h_tiles.push_back(tile);
-    return CDB_OK;
-}
-
-cdb_status alloc_build_bufs(BuildBufs &b, uint64_t max_np, cudaStream_t s) {
-    if (!max_np) return CDB_OK;
-    CDB_CUDA_TRY(cudaMalloc(&b.keys_in, max_np * 8));
-    CDB_CUDA_TRY(cudaMalloc(&b.keys_out, max_np * 8));
-    CDB_CUDA_TRY(cudaMalloc(&b.vals_in, max_np * 4));
-    CDB_CUDA_TRY(cudaMalloc(&b.flags, max_np * 4));
-    CDB_CUDA_TRY(cudaMalloc(&b.pos, max_np * 4));
-    size_t t_sort = 0, t_scan = 0;
-    CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, b.keys_in, b.keys_out, b.vals_in, b.vals_in, (int)max_np, 0, 40, s));
-    CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, t_scan, b.flags, b.pos, (int)max_np, s));
-    b.tmp_bytes = std::max(t_sort, t_scan);
-    CDB_CUDA_TRY(cudaMalloc(&b.tmp, b.tmp_bytes));
-    return CDB_OK;
-}
-
-// tiles [t0, t1) of the current rows, host and device tables
-cdb_status build_tiles(cdb_sparse_index *ix, uint64_t t0, uint64_t t1, BuildBufs &b, cudaStream_t s) {
-    ix->h_tiles.resize(t0);
-    cdb_status rc;
-    for (uint64_t t = t0; t < t1; ++t)
-        if ((rc = build_tile(ix, t, b, s))) return rc;
-    if (t1 > t0)
-        CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_tiles + t0, ix->h_tiles.data() + t0, (t1 - t0) * sizeof(SpTile), cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaStreamSynchronize(s));
-    return CDB_OK;
-}
-
-// back to the first `rows` rows (rows <= n_rows): their pairs are still in place, the tile holding row `rows` is rebuilt and
-// tombstones of the dropped rows are cleared.  b must fit that tile.  Device work is ordered by the caller.
-cdb_status restore_rows(cdb_sparse_index *ix, uint64_t rows, BuildBufs &b, cudaStream_t s) {
-    ix->h_row_off.resize(rows + 1);
-    ix->n_rows = rows;
-    ix->n_pairs = ix->h_row_off[rows];
-    for (uint64_t w = rows >> 5; w < ix->h_deleted.size(); ++w) {
-        const uint32_t keep = w == (rows >> 5) ? (uint32_t)((1ull << (rows & 31)) - 1) : 0u;
-        ix->n_deleted -= __builtin_popcount(ix->h_deleted[w] & ~keep);
-        ix->h_deleted[w] &= keep;
-    }
-    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_deleted, ix->h_deleted.data(), ix->h_deleted.size() * 4, cudaMemcpyHostToDevice, s));
-    return build_tiles(ix, rows >> SP_TILE_SHIFT, (rows + SP_TILE - 1) >> SP_TILE_SHIFT, b, s);
-}
-
-struct StreamGuard {
-    cudaStream_t s = nullptr;
-    ~StreamGuard() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
-};
-
 cdb_status check_search_params(const cdb_sparse_search_params *p, uint32_t *m) {
-    SP_REQUIRE(p, "null params");
-    SP_REQUIRE(p->k >= 1 && p->k <= SP_MAX_K, "k must be in 1..1024");
+    CDB_REQUIRE(p, "null params");
+    CDB_REQUIRE(p->k >= 1 && p->k <= SP_MAX_K, "k must be in 1..1024");
     const uint64_t f = p->rerank ? p->reranking_factor : 1;
-    SP_REQUIRE(f >= 1 && (uint64_t)p->k * f <= SP_MAX_CAND, "k * reranking_factor must be in 1..5120");
+    CDB_REQUIRE(f >= 1 && (uint64_t)p->k * f <= SP_MAX_CAND, "k * reranking_factor must be in 1..5120");
     *m = (uint32_t)(p->k * f);
     return CDB_OK;
 }
@@ -513,19 +361,14 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
                          cudaStream_t s) {
     if (!nq) return CDB_OK;
     const uint32_t k = p->k;
-    const uint32_t n_tiles = (uint32_t)ix->h_tiles.size();
+    const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
     const uint32_t bits = ix->desc.quantization_bits;
     // sequential_search, sparse_ann_query.rs:80-83
     const float thr = p->early_terminate_threshold;
     const float prod = (float)(1u << bits) * thr;
     const float etv_f = std::isnan(prod) ? 255.0f : std::min(prod, 255.0f);
     const uint32_t etv = sat_u32(etv_f, 255), low = sat_u32(thr * (float)(1u << bits), 0xFFFFFFFFu);
-    if (n_tiles == 0) {
-        CDB_CUDA_TRY(cudaMemsetAsync(d_ids, 0xFF, (size_t)nq * k * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d_scores, 0, (size_t)nq * k * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
-        return CDB_OK;
-    }
+    if (n_tiles == 0) return fill_empty_results(nq, k, d_ids, d_scores, d_counts, s);
     const uint32_t g = std::min<uint32_t>(SP_MERGE_MAX_LISTS, std::max<uint32_t>(2, SP_MERGE_KEYS / m));
     const uint32_t n_lvl1 = (n_tiles + g - 1) / g;
     uint32_t sort_cap = 1;
@@ -550,10 +393,11 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
     }
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
+        const PostingTiles<SparseCodec> &st = ix->st;
         SpSearch a;
-        a.entries = ix->d_entries; a.tdims = ix->d_tdims; a.tseg = ix->d_tseg; a.deleted = ix->n_deleted ? ix->d_deleted : nullptr;
-        a.tiles = ix->d_tiles; a.n_rows = ix->n_rows; a.id_base = ix->desc.id_base; a.maxq = ix->maxq; a.etv = etv; a.low = low;
-        a.ub = ix->desc.values_upper_bound; a.q_off = d_qoff; a.q_dims = d_qdims; a.q_vals = d_qvals; a.q0 = q0; a.m = m;
+        a.entries = st.entries(); a.tdims = st.d_tkeys; a.tseg = st.d_tseg; a.deleted = st.deleted();
+        a.tiles = st.d_tiles; a.n_rows = st.n_rows; a.id_base = ix->desc.id_base; a.maxq = st.codec.maxq; a.etv = etv; a.low = low;
+        a.ub = st.codec.ub; a.q_off = d_qoff; a.q_dims = d_qdims; a.q_vals = d_qvals; a.q0 = q0; a.m = m;
         a.n_tiles = n_tiles; a.out_keys = ka; a.out_cnt = ca;
         sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(a);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
@@ -571,8 +415,8 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
             n_lists = n_out;
         }
         if (rc) break;
-        sp_finalize_kernel<<<c, SP_THREADS, (size_t)sort_cap * 8, s>>>(cur, ccur, m, k, p->rerank ? 1 : 0, q0, d_qoff, d_qdims, d_qvals, ix->d_row_off,
-                                                    ix->d_dims, ix->d_vals, ix->desc.id_base, d_ids + (size_t)q0 * k,
+        sp_finalize_kernel<<<c, SP_THREADS, (size_t)sort_cap * 8, s>>>(cur, ccur, m, k, p->rerank ? 1 : 0, q0, d_qoff, d_qdims, d_qvals, ix->st.d_row_off,
+                                                    ix->st.d_keys, ix->st.d_vals, ix->desc.id_base, d_ids + (size_t)q0 * k,
                                                     d_scores + (size_t)q0 * k, d_counts + q0);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
@@ -582,39 +426,31 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
     return rc;
 }
 
-// the query CSR the caller passed (host): offsets start at 0 and never decrease
-cdb_status check_csr(const uint64_t *off, uint64_t n, const char *what) {
-    SP_REQUIRE(off, "null offsets");
-    if (off[0] != 0) { set_error(std::string(what) + ": offsets[0] must be 0"); return CDB_INVALID_PARAMS; }
-    for (uint64_t i = 0; i < n; ++i)
-        if (off[i + 1] < off[i]) { set_error(std::string(what) + ": offsets decrease"); return CDB_INVALID_PARAMS; }
-    return CDB_OK;
-}
-
 }  // namespace
 
 namespace cdb {
 cdb_status sparse_index_room(cdb_sparse_index *ix, uint64_t *rows, uint64_t *rows_left, uint64_t *pairs_left) {
     std::shared_lock<std::shared_mutex> lock(ix->rw);
-    *rows = ix->n_rows;
-    *rows_left = ix->desc.capacity_rows - ix->n_rows;
-    *pairs_left = ix->desc.capacity_pairs - ix->n_pairs;
+    *rows = ix->st.n_rows;
+    *rows_left = ix->desc.capacity_rows - ix->st.n_rows;
+    *pairs_left = ix->desc.capacity_pairs - ix->st.n_pairs;
     return CDB_OK;
 }
 
 cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows) {
     std::unique_lock<std::shared_mutex> lock(ix->rw);
-    SP_REQUIRE(rows <= ix->n_rows, "truncate beyond the index");
-    if (rows == ix->n_rows) return CDB_OK;
+    PostingTiles<SparseCodec> &st = ix->st;
+    CDB_REQUIRE(rows <= st.n_rows, "truncate beyond the index");
+    if (rows == st.n_rows) return CDB_OK;
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    const uint64_t r0 = rows & ~(uint64_t)(SP_TILE - 1);
+    const uint64_t r0 = rows & ~(uint64_t)(TILE_ROWS - 1);
     StreamGuard sg;
     CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
     BuildBufs b;
-    cdb_status rc = alloc_build_bufs(b, ix->h_row_off[rows] - ix->h_row_off[r0], sg.s);
+    cdb_status rc = b.alloc(st.h_row_off[rows] - st.h_row_off[r0], SparseCodec::END_BIT, sg.s);
     if (rc) return rc;
     CDB_CUDA_TRY(cudaDeviceSynchronize());
-    return restore_rows(ix, rows, b, sg.s);
+    return st.restore_rows(rows, b, sg.s);
 }
 
 int sparse_index_device(const cdb_sparse_index *ix) { return ix->desc.device; }
@@ -623,31 +459,14 @@ int sparse_index_device(const cdb_sparse_index *ix) { return ix->desc.device; }
 extern "C" {
 
 cdb_status cdb_sparse_index_create(const cdb_sparse_index_desc *desc, cdb_sparse_index **out) {
-    SP_REQUIRE(desc && out, "null argument");
-    SP_REQUIRE(desc->quantization_bits >= 4 && desc->quantization_bits <= 8, "quantization_bits must be in 4..8");
-    SP_REQUIRE(desc->capacity_rows >= 1 && (uint64_t)desc->id_base + desc->capacity_rows <= 0xFFFFFFFFull,
-               "capacity_rows must be >= 1 and id_base + capacity_rows <= 2^32 - 1");
-    SP_REQUIRE(desc->capacity_pairs < (1ull << 40), "capacity_pairs too large");
+    CDB_REQUIRE(desc && out, "null argument");
+    CDB_REQUIRE(desc->quantization_bits >= 4 && desc->quantization_bits <= 8, "quantization_bits must be in 4..8");
     *out = nullptr;
-    CDB_CUDA_TRY(cudaSetDevice(desc->device));
     std::unique_ptr<cdb_sparse_index> ix(new cdb_sparse_index());
     ix->desc = *desc;
-    ix->maxq = (1u << desc->quantization_bits) - 1;
-    ix->max_tiles = (desc->capacity_rows + SP_TILE - 1) / SP_TILE;
-    const size_t pairs = std::max<uint64_t>(1, desc->capacity_pairs);
-    const size_t words = (desc->capacity_rows + 31) / 32;
-    CDB_CUDA_TRY(cudaDeviceGetAttribute(&ix->sms, cudaDevAttrMultiProcessorCount, desc->device));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_row_off, (desc->capacity_rows + 1) * 8));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_dims, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_vals, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_entries, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_tdims, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_tseg, (pairs + ix->max_tiles) * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_deleted, words * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_tiles, ix->max_tiles * sizeof(SpTile)));
-    CDB_CUDA_TRY(cudaMemset(ix->d_row_off, 0, 8));
-    CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
-    ix->h_deleted.assign(words, 0u);
+    ix->st.codec = SparseCodec{desc->values_upper_bound, (1u << desc->quantization_bits) - 1};
+    const cdb_status rc = ix->st.init(desc->device, desc->id_base, desc->capacity_rows, desc->capacity_pairs);
+    if (rc) return rc;
     *out = ix.release();
     return CDB_OK;
 }
@@ -660,91 +479,38 @@ cdb_status cdb_sparse_index_destroy(cdb_sparse_index *ix) {
     return CDB_OK;
 }
 
-uint64_t cdb_sparse_index_size(const cdb_sparse_index *ix) { return ix ? ix->n_rows : 0; }
+uint64_t cdb_sparse_index_size(const cdb_sparse_index *ix) { return ix ? ix->st.n_rows : 0; }
 
 cdb_status cdb_sparse_index_append(cdb_sparse_index *ix, const uint64_t *row_offsets, const uint32_t *dims, const float *values,
                                    uint64_t n) {
-    SP_REQUIRE(ix, "null index");
+    CDB_REQUIRE(ix, "null index");
     if (!n) return CDB_OK;
     cdb_status rc = check_csr(row_offsets, n, "row_offsets");
     if (rc) return rc;
     const uint64_t np = row_offsets[n];
-    SP_REQUIRE((dims && values) || !np, "null pairs");
+    CDB_REQUIRE((dims && values) || !np, "null pairs");
     std::unique_lock<std::shared_mutex> lock(ix->rw);
-    SP_REQUIRE(ix->n_rows + n <= ix->desc.capacity_rows, "append exceeds capacity_rows");
-    SP_REQUIRE(ix->n_pairs + np <= ix->desc.capacity_pairs, "append exceeds capacity_pairs");
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    // every check and allocation precedes the first change
-    const uint64_t r_old = ix->n_rows, p_old = ix->n_pairs, r_new = r_old + n;
-    std::vector<uint64_t> off(n);
-    for (uint64_t i = 0; i < n; ++i) off[i] = p_old + row_offsets[i + 1];
-    auto row_off = [&](uint64_t r) { return r <= r_old ? ix->h_row_off[r] : off[r - r_old - 1]; };
-    const uint64_t t0 = r_old >> SP_TILE_SHIFT, t1 = (r_new + SP_TILE - 1) >> SP_TILE_SHIFT;
-    uint64_t max_np = 0;
-    for (uint64_t t = t0; t < t1; ++t)
-        max_np = std::max(max_np, row_off(std::min<uint64_t>(r_new, (t + 1) << SP_TILE_SHIFT)) - row_off(t << SP_TILE_SHIFT));
-    SP_REQUIRE(max_np < (1ull << 31), "a row tile holds 2^31 pairs or more");
-    StreamGuard sg;
-    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-    cudaStream_t s = sg.s;
-    BuildBufs b;
-    if ((rc = alloc_build_bufs(b, max_np, s))) return rc;
-    // searches already enqueued on other streams (cdb_sparse_search_batch_device) read the tile this call rebuilds
-    CDB_CUDA_TRY(cudaDeviceSynchronize());
-    cudaError_t e = cudaSuccess;
-    if (np) {
-        e = cudaMemcpyAsync(ix->d_dims + p_old, dims, np * 4, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_vals + p_old, values, np * 4, cudaMemcpyHostToDevice, s);
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_row_off + r_old + 1, off.data(), n * 8, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { set_error(std::string("sparse append: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
-    ix->h_row_off.insert(ix->h_row_off.end(), off.begin(), off.end());
-    ix->n_rows = r_new;
-    ix->n_pairs += np;
-    // rebuild the last partial tile, build the new ones; on failure the index goes back to its r_old rows
-    if ((rc = build_tiles(ix, t0, t1, b, s))) {
-        const std::string msg = cdb_last_error_string();
-        restore_rows(ix, r_old, b, s);
-        set_error(msg);
-    }
-    return rc;
+    Append a;
+    if ((rc = ix->st.prepare_append(row_offsets, dims, values, n, 0, "sparse append", a))) return rc;
+    return ix->st.commit_append(a, [] { return CDB_OK; });
 }
 
 cdb_status cdb_sparse_index_delete_rows(cdb_sparse_index *ix, const uint32_t *rows, uint64_t n) {
-    SP_REQUIRE(ix && (rows || !n), "null argument");
+    CDB_REQUIRE(ix && (rows || !n), "null argument");
     std::unique_lock<std::shared_mutex> lock(ix->rw);
-    for (uint64_t i = 0; i < n; ++i) SP_REQUIRE(rows[i] < ix->n_rows, "row out of range");
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    if (!n) return CDB_OK;
-    std::vector<uint32_t> w = ix->h_deleted;
-    uint64_t added = 0;
-    for (uint64_t i = 0; i < n; ++i) {
-        uint32_t &x = w[rows[i] >> 5];
-        const uint32_t bit = 1u << (rows[i] & 31);
-        if (!(x & bit)) { x |= bit; ++added; }
-    }
-    // searches enqueued before this call finish first (they read the bitmap)
-    CDB_CUDA_TRY(cudaDeviceSynchronize());
-    CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
-    ix->h_deleted.swap(w);
-    ix->n_deleted += added;
-    return CDB_OK;
+    return ix->st.mark_deleted(rows, n, [](const std::vector<uint32_t> &) { return CDB_OK; });
 }
 
 cdb_status cdb_sparse_index_deleted_rows(const cdb_sparse_index *ix, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total) {
-    SP_REQUIRE(ix && (out || !n), "null argument");
-    SP_REQUIRE(first + n <= ix->desc.capacity_rows, "first + n exceeds capacity_rows");
+    CDB_REQUIRE(ix && (out || !n), "null argument");
     std::shared_lock<std::shared_mutex> lock(const_cast<cdb_sparse_index *>(ix)->rw);
-    for (uint64_t i = 0; i < n; ++i) out[i] = (ix->h_deleted[(first + i) >> 5] >> ((first + i) & 31)) & 1u;
-    if (out_total) *out_total = ix->n_deleted;
-    return CDB_OK;
+    return ix->st.deleted_rows(first, n, out, out_total);
 }
 
 cdb_status cdb_sparse_search_batch_device(cdb_sparse_index *ix, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
                                           const float *d_q_values, uint32_t nq, const cdb_sparse_search_params *p,
                                           uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream) {
-    SP_REQUIRE(ix && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
+    CDB_REQUIRE(ix && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
     uint32_t m = 0;
     cdb_status rc = check_search_params(p, &m);
     if (rc) return rc;
@@ -756,14 +522,14 @@ cdb_status cdb_sparse_search_batch_device(cdb_sparse_index *ix, const uint64_t *
 cdb_status cdb_sparse_search_batch(cdb_sparse_index *ix, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
                                    uint32_t nq, const cdb_sparse_search_params *p, uint32_t *out_ids, float *out_scores,
                                    uint32_t *out_counts) {
-    SP_REQUIRE(ix && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    CDB_REQUIRE(ix && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
     uint32_t m = 0;
     cdb_status rc = check_search_params(p, &m);
     if (rc) return rc;
     if (!nq) return CDB_OK;
     if ((rc = check_csr(q_offsets, nq, "q_offsets"))) return rc;
     const uint64_t nqp = q_offsets[nq];
-    SP_REQUIRE((q_dims && q_values) || !nqp, "null query pairs");
+    CDB_REQUIRE((q_dims && q_values) || !nqp, "null query pairs");
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     StreamGuard sg;
@@ -797,7 +563,7 @@ cdb_status cdb_sparse_search_batch(cdb_sparse_index *ix, const uint64_t *q_offse
 
 cdb_status cdb_sparse_sample_upper_bound(int32_t device, const float *values, uint64_t n, float clamp_margin_percent,
                                          const uint64_t *prior_counts, uint64_t prior_values, uint64_t *out_counts, float *out_ub) {
-    SP_REQUIRE((values || !n) && (out_counts || out_ub), "bad arguments");
+    CDB_REQUIRE((values || !n) && (out_counts || out_ub), "bad arguments");
     CDB_CUDA_TRY(cudaSetDevice(device));
     int sms = 0;
     CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));

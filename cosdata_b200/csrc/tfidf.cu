@@ -3,13 +3,12 @@
 // src/models/versioned_vec.rs) and SparseAnnQueryBasic::search_bm25 (src/models/sparse_ann_query.rs:149-233) with get_idf
 // (sparse_ann_query.rs:298-302).  The contract is the header comment of cdb_tfidf_index_create.
 //
-// Layout (DESIGN.md section 8d).  Rows are kept as raw CSR on the device (hashes u32, tf f32, u64 row offsets).  Posting
-// lists are split into row tiles of 2^15 rows; a tile holds its distinct hashes (ascending), one segment per hash and
-// entries (row_in_tile, tf bits), ascending by row inside a segment.  The host keeps the sorted table of every hash the
-// index has seen with its df (VersionedVec::len) and uploads the table and its idf (log1pf on the host) after every append
-// and delete.  An append rebuilds the last partial tile and builds the new ones (CUB radix sort).  A search scores one
-// (query, tile) per CTA into shared-memory f32 accumulators plus a touched flag per row, query terms strictly in the
-// caller's order, reduces the tile to its 512 bucket winners, then merges the tiles per bucket and sorts the winners.
+// Layout (DESIGN.md section 8d).  The rows and posting tiles are a PostingTiles store (posting_tiles.cuh) keyed by term
+// hash, with entries (row_in_tile, tf bits), ascending by row inside a segment.  The host keeps the sorted table of every
+// hash the index has seen with its df (VersionedVec::len) and uploads the table and its idf (log1pf on the host) after
+// every append and delete.  A search scores one (query, tile) per CTA into shared-memory f32 accumulators plus a touched
+// flag per row, query terms strictly in the caller's order, reduces the tile to its 512 bucket winners, then merges the
+// tiles per bucket and sorts the winners.
 #include <algorithm>
 #include <cmath>
 #include <mutex>
@@ -18,63 +17,29 @@
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
-#include <cub/device/device_scan.cuh>
 
 #include "kernels.h"
+#include "posting_tiles.cuh"
 
 namespace cdb {
 namespace {
 
-constexpr uint32_t TF_TILE_SHIFT = 15;
-constexpr uint32_t TF_TILE = 1u << TF_TILE_SHIFT;
 constexpr int TF_THREADS = 512;
 constexpr uint32_t TF_BUCKETS = 512;       // search_bm25's BUCKETS
 constexpr uint32_t TF_QCHUNK = TF_THREADS; // query terms resolved per pass of the scoring kernel
 static_assert(TF_THREADS == (int)TF_BUCKETS, "one thread per bucket in the tile reduction and the final sort");
 
-struct TfTile {
-    uint64_t entry_base;   // first entry of the tile in d_entries
-    uint64_t hash_base;    // first distinct hash in d_thash; its segment starts are d_tseg[hash_base + tile ..]
-    uint32_t n_hashes;
-    uint32_t pad;
+// posting entries (row_in_tile, tf bits), sorted on hash << 15 | row: ascending rows inside a hash's segment.  Equal sort
+// keys are a row that repeats a hash.
+struct TfCodec {
+    using Entry = uint2;
+    static constexpr int END_BIT = 32 + TILE_SHIFT, SEG_SHIFT = TILE_SHIFT;
+    static constexpr const char *DUPLICATE_ERROR = "a row repeats a term hash";
+    __device__ SortPair encode(uint32_t hash, float tf, uint32_t row) const {
+        return {((uint64_t)hash << TILE_SHIFT) | row, __float_as_uint(tf)};
+    }
+    __device__ Entry entry(uint64_t k, uint32_t v) const { return make_uint2((uint32_t)(k & (TILE_ROWS - 1)), v); }
 };
-
-// ---------------------------------------------------------------- build side
-// key = hash << 15 | row_in_tile (47 bits), value = tf bits
-__global__ void tf_tile_keys_kernel(const uint64_t *__restrict__ row_off, uint64_t r0, uint32_t nr, uint64_t p0,
-                                    const uint32_t *__restrict__ hashes, const float *__restrict__ tfs,
-                                    uint64_t *__restrict__ sort_keys, uint32_t *__restrict__ sort_vals) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= nr) return;
-    const uint64_t b = row_off[r0 + warp], e = row_off[r0 + warp + 1];
-    for (uint64_t p = b + lane; p < e; p += 32) {
-        sort_keys[p - p0] = ((uint64_t)hashes[p] << TF_TILE_SHIFT) | warp;
-        sort_vals[p - p0] = __float_as_uint(tfs[p]);
-    }
-}
-
-// entries from the sorted keys, segment flags, and a duplicate (hash, row) flag
-__global__ void tf_entries_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ vals, uint32_t n,
-                                  uint2 *__restrict__ entries, uint32_t *__restrict__ flags, uint32_t *__restrict__ dup) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint64_t k = keys[i];
-    entries[i] = make_uint2((uint32_t)(k & (TF_TILE - 1)), vals[i]);
-    flags[i] = (i == 0 || (k >> TF_TILE_SHIFT) != (keys[i - 1] >> TF_TILE_SHIFT)) ? 1u : 0u;
-    if (i > 0 && k == keys[i - 1]) *dup = 1u;
-}
-
-__global__ void tf_seg_scatter_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ flags,
-                                      const uint32_t *__restrict__ pos, uint32_t n, uint32_t *__restrict__ thash,
-                                      uint32_t *__restrict__ tseg) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (flags[i]) {
-        thash[pos[i] - 1] = (uint32_t)(keys[i] >> TF_TILE_SHIFT);
-        tseg[pos[i] - 1] = i;
-    }
-    if (i == n - 1) tseg[pos[i]] = n;
-}
 
 // the hashes of rows[0..n) packed at out[off[i] ..] (one warp per row)
 __global__ void tf_gather_rows_kernel(const uint64_t *__restrict__ row_off, const uint32_t *__restrict__ hashes,
@@ -90,7 +55,7 @@ __global__ void tf_gather_rows_kernel(const uint64_t *__restrict__ row_off, cons
 struct TfSearch {
     const uint2 *entries;
     const uint32_t *thash, *tseg, *deleted;
-    const TfTile *tiles;
+    const PostingTile *tiles;
     const uint32_t *terms;   // every hash the index has seen, ascending
     const float *idf;        // idf of terms[i]
     uint32_t n_terms;
@@ -103,32 +68,26 @@ struct TfSearch {
     uint2 *out;              // [chunk][n_tiles][512] bucket winners (id, score bits); id CDB_INVALID_ID = empty
 };
 
-constexpr size_t TF_SCORE_SMEM = (size_t)TF_TILE * 4 + TF_TILE + (size_t)TF_QCHUNK * 12;
-
-__device__ inline uint32_t lower_bound_u32(const uint32_t *a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
+constexpr size_t TF_SCORE_SMEM = (size_t)TILE_ROWS * 4 + TILE_ROWS + (size_t)TF_QCHUNK * 12;
 
 __global__ void __launch_bounds__(TF_THREADS, 1) tf_score_tile_kernel(TfSearch a) {
     extern __shared__ __align__(16) uint8_t smem[];
     float *acc = reinterpret_cast<float *>(smem);
-    uint8_t *touched = smem + (size_t)TF_TILE * 4;
-    uint32_t *c_beg = reinterpret_cast<uint32_t *>(touched + TF_TILE);   // segment of each resolved term (tile-relative)
+    uint8_t *touched = smem + (size_t)TILE_ROWS * 4;
+    uint32_t *c_beg = reinterpret_cast<uint32_t *>(touched + TILE_ROWS);   // segment of each resolved term (tile-relative)
     uint32_t *c_len = c_beg + TF_QCHUNK;
     float *c_idf = reinterpret_cast<float *>(c_len + TF_QCHUNK);
 
     const uint32_t t = blockIdx.x, qi = blockIdx.y, q = a.q0 + qi, tid = threadIdx.x;
-    const TfTile tile = a.tiles[t];
-    const uint64_t row0 = (uint64_t)t << TF_TILE_SHIFT;
-    const uint32_t nr = (uint32_t)std::min<uint64_t>(TF_TILE, a.n_rows - row0);
+    const PostingTile tile = a.tiles[t];
+    const uint64_t row0 = (uint64_t)t << TILE_SHIFT;
+    const uint32_t nr = (uint32_t)std::min<uint64_t>(TILE_ROWS, a.n_rows - row0);
     uint4 *t4 = reinterpret_cast<uint4 *>(touched);
-    for (uint32_t i = tid; i < TF_TILE / 16; i += TF_THREADS) t4[i] = make_uint4(0, 0, 0, 0);
+    for (uint32_t i = tid; i < TILE_ROWS / 16; i += TF_THREADS) t4[i] = make_uint4(0, 0, 0, 0);
     __syncthreads();
 
-    const uint32_t *thash = a.thash + tile.hash_base;
-    const uint32_t *tseg = a.tseg + tile.hash_base + t;
+    const uint32_t *thash = a.thash + tile.key_base;
+    const uint32_t *tseg = a.tseg + tile.key_base + t;
     const uint2 *ent = a.entries + tile.entry_base;
     const uint64_t qb = a.q_off[q], qe = a.q_off[q + 1];
     for (uint64_t j0 = qb; j0 < qe; j0 += TF_QCHUNK) {
@@ -141,8 +100,8 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_score_tile_kernel(TfSearch a
             float idf = 0.0f;
             if (g < a.n_terms && a.terms[g] == h) {
                 idf = a.idf[g];
-                const uint32_t l = lower_bound_u32(thash, tile.n_hashes, h);
-                if (l < tile.n_hashes && thash[l] == h) { s = tseg[l]; e = tseg[l + 1]; }
+                const uint32_t l = lower_bound_u32(thash, tile.n_keys, h);
+                if (l < tile.n_keys && thash[l] == h) { s = tseg[l]; e = tseg[l + 1]; }
             }
             c_beg[tid] = s;
             c_len[tid] = e - s;
@@ -204,17 +163,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_finalize_kernel(const uint2 
                                       : ((uint64_t)order_key(CDB_METRIC_DOT_PRODUCT, __float_as_uint(best)) << 32) | (uint64_t)(~bid);
     if (bid != CDB_INVALID_ID) atomicAdd(&s_cnt, 1u);
     __syncthreads();
-    for (uint32_t size = 2; size <= TF_BUCKETS; size <<= 1) {
-        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-            if (tid < TF_BUCKETS / 2) {
-                const uint32_t lo = 2 * tid - (tid & (stride - 1)), hi = lo + stride;
-                const bool desc = (lo & size) == 0;
-                const uint64_t x = keys[lo], y = keys[hi];
-                if ((x < y) == desc) { keys[lo] = y; keys[hi] = x; }
-            }
-            __syncthreads();
-        }
-    }
+    bitonic_sort<true>(keys, TF_BUCKETS);
     const uint32_t cnt = min(s_cnt, kout);
     if (tid < kout) {
         uint32_t id = CDB_INVALID_ID;
@@ -238,33 +187,21 @@ using namespace cdb;
 struct cdb_tfidf_index {
     cdb_tfidf_index_desc desc;
     std::shared_mutex rw;
-    uint64_t n_rows = 0, n_pairs = 0, n_deleted = 0;
+    PostingTiles<TfCodec> st;        // keys: term hashes
     uint32_t documents = 0;          // total_documents_count
     uint32_t version = 0;            // the latest version passed to append / delete_rows
-    std::vector<uint64_t> h_row_off{0};
     std::vector<uint8_t> h_counted;
     std::vector<uint32_t> h_version; // insert version per row
-    std::vector<uint32_t> h_deleted;
     std::vector<uint32_t> h_terms;   // every hash seen, ascending
     std::vector<uint32_t> h_df;      // VersionedVec::len of each
-    std::vector<TfTile> h_tiles;
-    uint64_t *d_row_off = nullptr;
-    uint32_t *d_hashes = nullptr, *d_thash = nullptr, *d_tseg = nullptr, *d_deleted = nullptr, *d_terms = nullptr;
-    float *d_tfs = nullptr, *d_idf = nullptr;
-    uint2 *d_entries = nullptr;
-    TfTile *d_tiles = nullptr;
-    uint64_t max_tiles = 0, terms_cap = 0;
+    uint32_t *d_terms = nullptr;
+    float *d_idf = nullptr;
+    uint64_t terms_cap = 0;
     ~cdb_tfidf_index() {
-        for (void *p : {(void *)d_row_off, (void *)d_hashes, (void *)d_thash, (void *)d_tseg, (void *)d_deleted, (void *)d_terms,
-                        (void *)d_tfs, (void *)d_idf, (void *)d_entries, (void *)d_tiles})
-            if (p) cudaFree(p);
+        if (d_terms) cudaFree(d_terms);
+        if (d_idf) cudaFree(d_idf);
     }
 };
-
-#define TF_REQUIRE(cond, msg)                                              \
-    do {                                                                   \
-        if (!(cond)) { set_error(msg); return CDB_INVALID_PARAMS; }        \
-    } while (0)
 
 namespace {
 
@@ -274,91 +211,6 @@ float tf_idf(uint32_t n_docs, uint32_t df) {
     const float num = (float)(uint32_t)(n_docs - df) + 0.5f;
     const float den = (float)df + 0.5f;
     return log1pf(num / den);
-}
-
-struct BuildBufs {
-    void *tmp = nullptr;
-    size_t tmp_bytes = 0;
-    uint64_t *keys_in = nullptr, *keys_out = nullptr;
-    uint32_t *vals_in = nullptr, *vals_out = nullptr, *flags = nullptr, *pos = nullptr, *dup = nullptr;
-    ~BuildBufs() {
-        for (void *p : {tmp, (void *)keys_in, (void *)keys_out, (void *)vals_in, (void *)vals_out, (void *)flags, (void *)pos, (void *)dup})
-            if (p) cudaFree(p);
-    }
-};
-
-cdb_status alloc_build_bufs(BuildBufs &b, uint64_t max_np, cudaStream_t s) {
-    CDB_CUDA_TRY(cudaMalloc(&b.dup, 4));
-    if (!max_np) return CDB_OK;
-    CDB_CUDA_TRY(cudaMalloc(&b.keys_in, max_np * 8));
-    CDB_CUDA_TRY(cudaMalloc(&b.keys_out, max_np * 8));
-    CDB_CUDA_TRY(cudaMalloc(&b.vals_in, max_np * 4));
-    CDB_CUDA_TRY(cudaMalloc(&b.vals_out, max_np * 4));
-    CDB_CUDA_TRY(cudaMalloc(&b.flags, max_np * 4));
-    CDB_CUDA_TRY(cudaMalloc(&b.pos, max_np * 4));
-    size_t t_sort = 0, t_scan = 0;
-    CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, b.keys_in, b.keys_out, b.vals_in, b.vals_out, (int)max_np, 0,
-                                                 32 + TF_TILE_SHIFT, s));
-    CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, t_scan, b.flags, b.pos, (int)max_np, s));
-    b.tmp_bytes = std::max(t_sort, t_scan);
-    CDB_CUDA_TRY(cudaMalloc(&b.tmp, b.tmp_bytes));
-    return CDB_OK;
-}
-
-// posting lists of tile t appended after the tiles below it; CDB_INVALID_PARAMS if a row of it repeats a hash
-cdb_status build_tile(cdb_tfidf_index *ix, uint64_t t, BuildBufs &b, cudaStream_t s) {
-    const uint64_t r0 = t << TF_TILE_SHIFT, r1 = std::min<uint64_t>(ix->n_rows, r0 + TF_TILE);
-    const uint64_t p0 = ix->h_row_off[r0], p1 = ix->h_row_off[r1];
-    const uint32_t np = (uint32_t)(p1 - p0);
-    TfTile tile;
-    tile.entry_base = p0;
-    tile.hash_base = t ? ix->h_tiles[t - 1].hash_base + ix->h_tiles[t - 1].n_hashes : 0;
-    tile.n_hashes = 0;
-    tile.pad = 0;
-    uint32_t *tseg = ix->d_tseg + tile.hash_base + t;
-    if (np == 0) {
-        CDB_CUDA_TRY(cudaMemsetAsync(tseg, 0, 4, s));
-    } else {
-        const uint32_t nr = (uint32_t)(r1 - r0);
-        tf_tile_keys_kernel<<<(nr * 32 + 255) / 256, 256, 0, s>>>(ix->d_row_off, r0, nr, p0, ix->d_hashes, ix->d_tfs, b.keys_in, b.vals_in);
-        CDB_LAUNCH_CHECK();
-        size_t tb = b.tmp_bytes;
-        CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(b.tmp, tb, b.keys_in, b.keys_out, b.vals_in, b.vals_out, (int)np, 0,
-                                                     32 + TF_TILE_SHIFT, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(b.dup, 0, 4, s));
-        tf_entries_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, b.vals_out, np, ix->d_entries + p0, b.flags, b.dup);
-        CDB_LAUNCH_CHECK();
-        tb = b.tmp_bytes;
-        CDB_CUDA_TRY(cub::DeviceScan::InclusiveSum(b.tmp, tb, b.flags, b.pos, (int)np, s));
-        tf_seg_scatter_kernel<<<(np + 255) / 256, 256, 0, s>>>(b.keys_out, b.flags, b.pos, np, ix->d_thash + tile.hash_base, tseg);
-        CDB_LAUNCH_CHECK();
-        uint32_t dup = 0;
-        CDB_CUDA_TRY(cudaMemcpyAsync(&tile.n_hashes, b.pos + np - 1, 4, cudaMemcpyDeviceToHost, s));
-        CDB_CUDA_TRY(cudaMemcpyAsync(&dup, b.dup, 4, cudaMemcpyDeviceToHost, s));
-        CDB_CUDA_TRY(cudaStreamSynchronize(s));
-        if (dup) { set_error("a row repeats a term hash"); return CDB_INVALID_PARAMS; }
-    }
-    ix->h_tiles.push_back(tile);
-    return CDB_OK;
-}
-
-cdb_status build_tiles(cdb_tfidf_index *ix, uint64_t t0, uint64_t t1, BuildBufs &b, cudaStream_t s) {
-    ix->h_tiles.resize(t0);
-    cdb_status rc;
-    for (uint64_t t = t0; t < t1; ++t)
-        if ((rc = build_tile(ix, t, b, s))) return rc;
-    if (t1 > t0)
-        CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_tiles + t0, ix->h_tiles.data() + t0, (t1 - t0) * sizeof(TfTile), cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaStreamSynchronize(s));
-    return CDB_OK;
-}
-
-// back to the first `rows` rows (their pairs are still in place; nothing was deleted among the dropped ones)
-cdb_status restore_rows(cdb_tfidf_index *ix, uint64_t rows, BuildBufs &b, cudaStream_t s) {
-    ix->h_row_off.resize(rows + 1);
-    ix->n_rows = rows;
-    ix->n_pairs = ix->h_row_off[rows];
-    return build_tiles(ix, rows >> TF_TILE_SHIFT, (rows + TF_TILE - 1) >> TF_TILE_SHIFT, b, s);
 }
 
 // the term table and its idf under `n_docs` to the device (the device is idle: the caller holds the handle exclusively
@@ -389,32 +241,14 @@ cdb_status upload_terms(cdb_tfidf_index *ix, const std::vector<uint32_t> &terms,
     return CDB_OK;
 }
 
-struct StreamGuard {
-    cudaStream_t s = nullptr;
-    ~StreamGuard() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
-};
-
-cdb_status check_csr(const uint64_t *off, uint64_t n, const char *what) {
-    TF_REQUIRE(off, "null offsets");
-    if (off[0] != 0) { set_error(std::string(what) + ": offsets[0] must be 0"); return CDB_INVALID_PARAMS; }
-    for (uint64_t i = 0; i < n; ++i)
-        if (off[i + 1] < off[i]) { set_error(std::string(what) + ": offsets decrease"); return CDB_INVALID_PARAMS; }
-    return CDB_OK;
-}
-
 uint32_t out_cols(uint32_t k) { return (k == 0 || k > TF_BUCKETS) ? TF_BUCKETS : k; }
 
 cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint32_t nq, uint32_t k,
                          uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t s) {
     if (!nq) return CDB_OK;
     const uint32_t kout = out_cols(k);
-    const uint32_t n_tiles = (uint32_t)ix->h_tiles.size();
-    if (n_tiles == 0) {
-        CDB_CUDA_TRY(cudaMemsetAsync(d_ids, 0xFF, (size_t)nq * kout * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d_scores, 0, (size_t)nq * kout * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
-        return CDB_OK;
-    }
+    const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
+    if (n_tiles == 0) return fill_empty_results(nq, kout, d_ids, d_scores, d_counts, s);
     const size_t per_q = (size_t)n_tiles * TF_BUCKETS * sizeof(uint2);
     const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, (512ull << 20) / per_q}));
     uint2 *win = nullptr;
@@ -425,9 +259,9 @@ cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
         TfSearch a;
-        a.entries = ix->d_entries; a.thash = ix->d_thash; a.tseg = ix->d_tseg; a.deleted = ix->n_deleted ? ix->d_deleted : nullptr;
-        a.tiles = ix->d_tiles; a.terms = ix->d_terms; a.idf = ix->d_idf; a.n_terms = (uint32_t)ix->h_terms.size();
-        a.n_rows = ix->n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q0 = q0; a.n_tiles = n_tiles;
+        a.entries = ix->st.entries(); a.thash = ix->st.d_tkeys; a.tseg = ix->st.d_tseg; a.deleted = ix->st.deleted();
+        a.tiles = ix->st.d_tiles; a.terms = ix->d_terms; a.idf = ix->d_idf; a.n_terms = (uint32_t)ix->h_terms.size();
+        a.n_rows = ix->st.n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q0 = q0; a.n_tiles = n_tiles;
         a.out = win;
         tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(a);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
@@ -450,28 +284,12 @@ int tfidf_index_device(const cdb_tfidf_index *ix) { return ix->desc.device; }
 extern "C" {
 
 cdb_status cdb_tfidf_index_create(const cdb_tfidf_index_desc *desc, cdb_tfidf_index **out) {
-    TF_REQUIRE(desc && out, "null argument");
-    TF_REQUIRE(desc->capacity_rows >= 1 && (uint64_t)desc->id_base + desc->capacity_rows <= 0xFFFFFFFFull,
-               "capacity_rows must be >= 1 and id_base + capacity_rows <= 2^32 - 1");
-    TF_REQUIRE(desc->capacity_pairs < (1ull << 40), "capacity_pairs too large");
+    CDB_REQUIRE(desc && out, "null argument");
     *out = nullptr;
-    CDB_CUDA_TRY(cudaSetDevice(desc->device));
     std::unique_ptr<cdb_tfidf_index> ix(new cdb_tfidf_index());
     ix->desc = *desc;
-    ix->max_tiles = (desc->capacity_rows + TF_TILE - 1) / TF_TILE;
-    const size_t pairs = std::max<uint64_t>(1, desc->capacity_pairs);
-    const size_t words = (desc->capacity_rows + 31) / 32;
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_row_off, (desc->capacity_rows + 1) * 8));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_hashes, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_tfs, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_entries, pairs * 8));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_thash, pairs * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_tseg, (pairs + ix->max_tiles) * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_deleted, words * 4));
-    CDB_CUDA_TRY(cudaMalloc(&ix->d_tiles, ix->max_tiles * sizeof(TfTile)));
-    CDB_CUDA_TRY(cudaMemset(ix->d_row_off, 0, 8));
-    CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
-    ix->h_deleted.assign(words, 0u);
+    const cdb_status rc = ix->st.init(desc->device, desc->id_base, desc->capacity_rows, desc->capacity_pairs);
+    if (rc) return rc;
     *out = ix.release();
     return CDB_OK;
 }
@@ -484,61 +302,43 @@ cdb_status cdb_tfidf_index_destroy(cdb_tfidf_index *ix) {
     return CDB_OK;
 }
 
-uint64_t cdb_tfidf_index_size(const cdb_tfidf_index *ix) { return ix ? ix->n_rows : 0; }
+uint64_t cdb_tfidf_index_size(const cdb_tfidf_index *ix) { return ix ? ix->st.n_rows : 0; }
 
 cdb_status cdb_tfidf_index_append(cdb_tfidf_index *ix, const uint64_t *row_offsets, const uint32_t *hashes, const float *tfs,
                                   const uint8_t *counted, uint64_t n, uint32_t version) {
-    TF_REQUIRE(ix, "null index");
+    CDB_REQUIRE(ix, "null index");
     if (!n) return CDB_OK;
     cdb_status rc = check_csr(row_offsets, n, "row_offsets");
     if (rc) return rc;
     const uint64_t np = row_offsets[n];
-    TF_REQUIRE((hashes && tfs) || !np, "null pairs");
+    CDB_REQUIRE((hashes && tfs) || !np, "null pairs");
+    CDB_REQUIRE(np < (1ull << 31), "a row tile or an append holds 2^31 pairs or more");   // the df count below takes an int
     uint32_t n_counted = 0;
     for (uint64_t i = 0; i < n; ++i) {
         if (!counted || counted[i]) ++n_counted;
-        else TF_REQUIRE(row_offsets[i + 1] == row_offsets[i], "an uncounted row must be empty");
+        else CDB_REQUIRE(row_offsets[i + 1] == row_offsets[i], "an uncounted row must be empty");
     }
     std::unique_lock<std::shared_mutex> lock(ix->rw);
-    TF_REQUIRE(ix->n_rows + n <= ix->desc.capacity_rows, "append exceeds capacity_rows");
-    TF_REQUIRE(ix->n_pairs + np <= ix->desc.capacity_pairs, "append exceeds capacity_pairs");
-    TF_REQUIRE(version >= ix->version, "version is older than the index's latest");
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    // every check and allocation precedes the first change
-    const uint64_t r_old = ix->n_rows, p_old = ix->n_pairs, r_new = r_old + n;
-    std::vector<uint64_t> off(n);
-    for (uint64_t i = 0; i < n; ++i) off[i] = p_old + row_offsets[i + 1];
-    auto row_off = [&](uint64_t r) { return r <= r_old ? ix->h_row_off[r] : off[r - r_old - 1]; };
-    const uint64_t t0 = r_old >> TF_TILE_SHIFT, t1 = (r_new + TF_TILE - 1) >> TF_TILE_SHIFT;
-    uint64_t max_np = 0;
-    for (uint64_t t = t0; t < t1; ++t)
-        max_np = std::max(max_np, row_off(std::min<uint64_t>(r_new, (t + 1) << TF_TILE_SHIFT)) - row_off(t << TF_TILE_SHIFT));
-    TF_REQUIRE(max_np < (1ull << 31) && np < (1ull << 31), "a row tile or an append holds 2^31 pairs or more");
-    StreamGuard sg;
-    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-    cudaStream_t s = sg.s;
-    BuildBufs b;
-    if ((rc = alloc_build_bufs(b, std::max(max_np, np), s))) return rc;
-    // searches already enqueued on other streams (cdb_tfidf_search_batch_device) read the tile and the idf this call rewrites
-    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    CDB_REQUIRE(version >= ix->version, "version is older than the index's latest");
+    // the scratch also holds the df count of the whole append; the drain covers searches reading the idf as well
+    Append a;
+    if ((rc = ix->st.prepare_append(row_offsets, hashes, tfs, n, np, "tf-idf append", a))) return rc;
+    const cudaStream_t s = a.sg.s;
+    BuildBufs &b = a.b;
+    const uint32_t *d_hashes = ix->st.d_keys + a.p_old;
     cudaError_t e = cudaSuccess;
-    if (np) {
-        e = cudaMemcpyAsync(ix->d_hashes + p_old, hashes, np * 4, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_tfs + p_old, tfs, np * 4, cudaMemcpyHostToDevice, s);
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_row_off + r_old + 1, off.data(), n * 8, cudaMemcpyHostToDevice, s);
     // df increments: the distinct hashes of the appended pairs and how many rows hold each (rows never repeat a hash)
     std::vector<uint32_t> uniq, cnt;
-    if (e == cudaSuccess && np) {
+    if (np) {
         uint32_t *runs = b.pos;   // scratch: sorted hashes -> b.vals_out, unique -> b.flags, counts -> b.vals_in, runs -> pos
         size_t t_sort = 0, t_rle = 0;
-        e = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, ix->d_hashes + p_old, b.vals_out, (int)np, 0, 32, s);
+        e = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d_hashes, b.vals_out, (int)np, 0, 32, s);
         if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
         const size_t need = std::max(t_sort, t_rle);
         void *tmp = b.tmp;
         if (e == cudaSuccess && need > b.tmp_bytes) e = cudaMallocAsync(&tmp, need, s);
         size_t tb = need;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp, tb, ix->d_hashes + p_old, b.vals_out, (int)np, 0, 32, s);
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp, tb, d_hashes, b.vals_out, (int)np, 0, 32, s);
         tb = need;
         if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(tmp, tb, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
         uint32_t n_runs = 0;
@@ -565,112 +365,93 @@ cdb_status cdb_tfidf_index_append(cdb_tfidf_index *ix, const uint64_t *row_offse
         else { terms.push_back(ix->h_terms[i]); df.push_back(ix->h_df[i] + cnt[j]); ++i; ++j; }
     }
     const bool new_terms = terms.size() != ix->h_terms.size();
-    ix->h_row_off.insert(ix->h_row_off.end(), off.begin(), off.end());
-    ix->n_rows = r_new;
-    ix->n_pairs += np;
-    // rebuild the last partial tile, build the new ones, then the idf of every term under the new N; on failure the index
-    // goes back to its r_old rows
+    // the tiles, then the idf of every term under the new N; if the upload fails the previous table goes back as well
     const uint32_t docs = ix->documents + n_counted;
-    if (!(rc = build_tiles(ix, t0, t1, b, s))) rc = upload_terms(ix, terms, df, docs, new_terms, s);
-    if (rc) {
-        const std::string msg = cdb_last_error_string();
-        restore_rows(ix, r_old, b, s);
-        upload_terms(ix, ix->h_terms, ix->h_df, ix->documents, true, s);
-        set_error(msg);
-        return rc;
-    }
+    rc = ix->st.commit_append(a, [&]() -> cdb_status {
+        const cdb_status r = upload_terms(ix, terms, df, docs, new_terms, s);
+        if (r) {
+            const std::string msg = cdb_last_error_string();
+            upload_terms(ix, ix->h_terms, ix->h_df, ix->documents, true, s);
+            set_error(msg);
+        }
+        return r;
+    });
+    if (rc) return rc;
     ix->h_terms.swap(terms);
     ix->h_df.swap(df);
     ix->documents = docs;
     ix->version = version;
     for (uint64_t r = 0; r < n; ++r) ix->h_counted.push_back(!counted || counted[r] ? 1 : 0);
-    ix->h_version.resize(r_new, version);
+    ix->h_version.resize(a.r_new, version);
     return CDB_OK;
 }
 
 cdb_status cdb_tfidf_index_delete_rows(cdb_tfidf_index *ix, const uint32_t *rows, uint64_t n, uint32_t version) {
-    TF_REQUIRE(ix && (rows || !n), "null argument");
+    CDB_REQUIRE(ix && (rows || !n), "null argument");
     std::unique_lock<std::shared_mutex> lock(ix->rw);
-    for (uint64_t i = 0; i < n; ++i) TF_REQUIRE(rows[i] < ix->n_rows, "row out of range");
-    TF_REQUIRE(version >= ix->version, "version is older than the index's latest");
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    if (!n) return CDB_OK;
-    std::vector<uint32_t> w = ix->h_deleted;
-    std::vector<uint32_t> fresh;      // rows this call deletes (already deleted rows are left alone)
-    for (uint64_t i = 0; i < n; ++i) {
-        uint32_t &x = w[rows[i] >> 5];
-        const uint32_t bit = 1u << (rows[i] & 31);
-        if (!(x & bit)) { x |= bit; fresh.push_back(rows[i]); }
-    }
-    // VersionedVec::delete of each of their terms: a delete in the insert's version removes the entry (df - 1), a later one
-    // marks it and pushes a tombstone word (df + 1)
-    std::vector<uint64_t> goff(fresh.size() + 1, 0);
-    for (size_t i = 0; i < fresh.size(); ++i) goff[i + 1] = goff[i] + ix->h_row_off[fresh[i] + 1] - ix->h_row_off[fresh[i]];
-    const uint64_t ng = goff.back();
-    std::vector<uint32_t> gh(ng);
-    StreamGuard sg;
-    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-    cudaStream_t s = sg.s;
-    if (ng) {
-        uint8_t *buf = nullptr;
-        const size_t bytes = fresh.size() * 4 + goff.size() * 8 + ng * 4;
-        CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
-        uint64_t *d_off = reinterpret_cast<uint64_t *>(buf);
-        uint32_t *d_rows = reinterpret_cast<uint32_t *>(d_off + goff.size());
-        uint32_t *d_out = d_rows + fresh.size();
-        cudaError_t e = cudaMemcpyAsync(d_off, goff.data(), goff.size() * 8, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_rows, fresh.data(), fresh.size() * 4, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess) {
-            tf_gather_rows_kernel<<<(uint32_t)((fresh.size() * 32 + 255) / 256), 256, 0, s>>>(ix->d_row_off, ix->d_hashes, d_rows, d_off,
-                                                                                          (uint32_t)fresh.size(), d_out);
-            g_launch_count.fetch_add(1, std::memory_order_relaxed);
-            e = cudaGetLastError();
+    CDB_REQUIRE(version >= ix->version, "version is older than the index's latest");
+    // fresh: the rows this call deletes (already deleted rows are left alone)
+    return ix->st.mark_deleted(rows, n, [&](const std::vector<uint32_t> &fresh) -> cdb_status {
+        // VersionedVec::delete of each of their terms: a delete in the insert's version removes the entry (df - 1), a later
+        // one marks it and pushes a tombstone word (df + 1)
+        std::vector<uint64_t> goff(fresh.size() + 1, 0);
+        for (size_t i = 0; i < fresh.size(); ++i) goff[i + 1] = goff[i] + ix->st.h_row_off[fresh[i] + 1] - ix->st.h_row_off[fresh[i]];
+        const uint64_t ng = goff.back();
+        std::vector<uint32_t> gh(ng);
+        StreamGuard sg;
+        CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+        cudaStream_t s = sg.s;
+        if (ng) {
+            uint8_t *buf = nullptr;
+            const size_t bytes = fresh.size() * 4 + goff.size() * 8 + ng * 4;
+            CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
+            uint64_t *d_off = reinterpret_cast<uint64_t *>(buf);
+            uint32_t *d_rows = reinterpret_cast<uint32_t *>(d_off + goff.size());
+            uint32_t *d_out = d_rows + fresh.size();
+            cudaError_t e = cudaMemcpyAsync(d_off, goff.data(), goff.size() * 8, cudaMemcpyHostToDevice, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(d_rows, fresh.data(), fresh.size() * 4, cudaMemcpyHostToDevice, s);
+            if (e == cudaSuccess) {
+                tf_gather_rows_kernel<<<(uint32_t)((fresh.size() * 32 + 255) / 256), 256, 0, s>>>(ix->st.d_row_off, ix->st.d_keys, d_rows,
+                                                                                              d_off, (uint32_t)fresh.size(), d_out);
+                g_launch_count.fetch_add(1, std::memory_order_relaxed);
+                e = cudaGetLastError();
+            }
+            if (e == cudaSuccess) e = cudaMemcpyAsync(gh.data(), d_out, ng * 4, cudaMemcpyDeviceToHost, s);
+            cudaFreeAsync(buf, s);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+            if (e != cudaSuccess) { set_error(std::string("tf-idf delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(gh.data(), d_out, ng * 4, cudaMemcpyDeviceToHost, s);
-        cudaFreeAsync(buf, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) { set_error(std::string("tf-idf delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
-    }
-    std::vector<uint32_t> df = ix->h_df;
-    uint32_t docs = ix->documents;
-    for (size_t i = 0; i < fresh.size(); ++i) {
-        const uint32_t r = fresh[i];
-        if (!ix->h_counted[r]) continue;     // delete_embedding returns early for an embedding without text
-        --docs;
-        const uint32_t delta = ix->h_version[r] == version ? 0xFFFFFFFFu : 1u;
-        for (uint64_t p = goff[i]; p < goff[i + 1]; ++p) {
-            const size_t g = std::lower_bound(ix->h_terms.begin(), ix->h_terms.end(), gh[p]) - ix->h_terms.begin();
-            df[g] += delta;
+        std::vector<uint32_t> df = ix->h_df;
+        uint32_t docs = ix->documents;
+        for (size_t i = 0; i < fresh.size(); ++i) {
+            const uint32_t r = fresh[i];
+            if (!ix->h_counted[r]) continue;     // delete_embedding returns early for an embedding without text
+            --docs;
+            const uint32_t delta = ix->h_version[r] == version ? 0xFFFFFFFFu : 1u;
+            for (uint64_t p = goff[i]; p < goff[i + 1]; ++p) {
+                const size_t g = std::lower_bound(ix->h_terms.begin(), ix->h_terms.end(), gh[p]) - ix->h_terms.begin();
+                df[g] += delta;
+            }
         }
-    }
-    // searches enqueued before this call finish first (they read the bitmap and the idf)
-    CDB_CUDA_TRY(cudaDeviceSynchronize());
-    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_deleted, w.data(), w.size() * 4, cudaMemcpyHostToDevice, s));
-    cdb_status rc = upload_terms(ix, ix->h_terms, df, docs, false, s);
-    if (rc) {
-        cudaMemcpyAsync(ix->d_deleted, ix->h_deleted.data(), w.size() * 4, cudaMemcpyHostToDevice, s);
-        return rc;
-    }
-    ix->h_deleted.swap(w);
-    ix->n_deleted += fresh.size();
-    ix->h_df.swap(df);
-    ix->documents = docs;
-    ix->version = version;
-    return CDB_OK;
+        // queued searches have drained (they read the idf)
+        const cdb_status rc = upload_terms(ix, ix->h_terms, df, docs, false, s);
+        if (rc) return rc;
+        ix->h_df.swap(df);
+        ix->documents = docs;
+        ix->version = version;
+        return CDB_OK;
+    });
 }
 
 cdb_status cdb_tfidf_index_deleted_rows(const cdb_tfidf_index *ix, uint64_t first, uint64_t n, uint8_t *out, uint64_t *out_total) {
-    TF_REQUIRE(ix && (out || !n), "null argument");
-    TF_REQUIRE(first + n <= ix->desc.capacity_rows, "first + n exceeds capacity_rows");
+    CDB_REQUIRE(ix && (out || !n), "null argument");
     std::shared_lock<std::shared_mutex> lock(const_cast<cdb_tfidf_index *>(ix)->rw);
-    for (uint64_t i = 0; i < n; ++i) out[i] = (ix->h_deleted[(first + i) >> 5] >> ((first + i) & 31)) & 1u;
-    if (out_total) *out_total = ix->n_deleted;
-    return CDB_OK;
+    return ix->st.deleted_rows(first, n, out, out_total);
 }
 
 cdb_status cdb_tfidf_index_term_stats(cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *out_df, float *out_idf,
                                       uint32_t *out_documents_count) {
-    TF_REQUIRE(ix && (hashes || !n), "null argument");
+    CDB_REQUIRE(ix && (hashes || !n), "null argument");
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     if (out_documents_count) *out_documents_count = ix->documents;
     if (!n) return CDB_OK;
@@ -689,7 +470,7 @@ cdb_status cdb_tfidf_index_term_stats(cdb_tfidf_index *ix, const uint32_t *hashe
 
 cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *ix, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes, uint32_t nq,
                                          uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream) {
-    TF_REQUIRE(ix && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
+    CDB_REQUIRE(ix && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     return search_locked(ix, d_q_offsets, d_q_hashes, nq, k, d_ids, d_scores, d_counts, (cudaStream_t)stream);
@@ -697,12 +478,12 @@ cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *ix, const uint64_t *d_
 
 cdb_status cdb_tfidf_search_batch(cdb_tfidf_index *ix, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
                                   uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
-    TF_REQUIRE(ix && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    CDB_REQUIRE(ix && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
     if (!nq) return CDB_OK;
     cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
     if (rc) return rc;
     const uint64_t nqh = q_offsets[nq];
-    TF_REQUIRE(q_hashes || !nqh, "null query hashes");
+    CDB_REQUIRE(q_hashes || !nqh, "null query hashes");
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     StreamGuard sg;

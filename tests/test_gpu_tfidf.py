@@ -214,6 +214,33 @@ def test_invalid_calls_change_nothing():
     ix.close()
 
 
+def test_failed_append_across_tiles_changes_nothing():
+    """an append that rebuilds the last partial tile, builds a new one and then fails on a row of that new tile (a repeated
+    hash) leaves rows, tiles, N, df and idf as they were, and a valid append continues from there"""
+    corpus = multi_tile(12, 60_000)
+    first, rest = slice_csr(corpus, 0, 20_000), slice_csr(corpus, 20_000, 60_000)
+    bad = concat_csr([rest, cdb.sparse_csr([[(7, 1.0), (9, 0.5), (7, 2.0)]])])   # row 60000: in tile 1, not tile 0
+    ix, orc = both(capacity_rows=70_000, capacity_pairs=len(bad[1]) + len(first[1]))
+    ix.append(first, 1)
+    orc.append(first, 1)
+    qs = zipf_queries(13, 256, vocab=5000)
+    hashes = np.concatenate([np.unique(corpus[1])[:1000], np.array([7, 9], np.uint32)])
+    with pytest.raises(cdb.CosdataError) as e:
+        ix.append(bad, 1)
+    assert e.value.status == cdb.Status.INVALID_PARAMS
+    assert len(ix) == 20_000
+    check_stats(ix, orc, hashes)
+    for k in (10, 0):
+        check(ix.batch_search(qs, k), orc.search(query_csr(qs), k))
+    ix.append(rest, 2)
+    orc.append(rest, 2)
+    assert len(ix) == 60_000
+    check_stats(ix, orc, hashes)
+    for k in (10, 0):
+        check(ix.batch_search(qs, k), orc.search(query_csr(qs), k))
+    ix.close()
+
+
 def test_one_million_documents_batch_1024():
     import torch
     free, _ = torch.cuda.mem_get_info(0)
