@@ -249,6 +249,11 @@ PROTOTYPES = {
                                             c_u32p, c_f32p, c_u32p]),
     "cdb_sparse_search_batch_device": (C.c_int32, [C.c_void_p, c_vp, c_u32p, c_f32p, C.c_uint32, C.POINTER(SparseSearchParams),
                                                    c_u32p, c_f32p, c_u32p, C.c_void_p]),
+    "cdb_sparse_search_batch_all": (C.c_int32, [C.c_void_p, c_vp, c_u32p, c_f32p, C.c_uint32, C.POINTER(SparseSearchParams),
+                                                C.POINTER(C.c_void_p)]),
+    "cdb_sparse_results_offsets": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint32), c_vp]),
+    "cdb_sparse_results_read": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint32, c_u32p, c_f32p]),
+    "cdb_sparse_results_destroy": (C.c_int32, [C.c_void_p]),
     "cdb_sparse_sample_upper_bound": (C.c_int32, [C.c_int32, c_f32p, C.c_uint64, C.c_float, c_vp, C.c_uint64, c_vp,
                                                   C.POINTER(C.c_float)]),
     "cdb_itoe_scan_sparse": (C.c_int32, [C.c_char_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),

@@ -823,7 +823,8 @@ def _as_csr(x):
 
 
 class SparseSearchOptions:
-    """SparseSearchOptions (inverted/mod.rs:29-32) plus the config values search_internal reads: top_k (required here),
+    """SparseSearchOptions (inverted/mod.rs:29-32) plus the config values search_internal reads: top_k (None = every
+    candidate, SparseIndex.batch_search_all; batch_search needs a number),
     early_terminate_threshold (None = config.search.early_terminate_threshold, 0.0), rerank_sparse_with_raw_values and
     sparse_raw_values_reranking_factor (config.toml:5-6)"""
 
@@ -893,9 +894,31 @@ class SparseIndex:
         return ids[:, :k], scores[:, :k], counts[:nq]
 
     def search(self, query, options):
+        if options.top_k is None:
+            _, ids, scores = self.batch_search_all([list(query)], options)
+            return list(zip(ids.tolist(), scores.tolist()))
         ids, scores, counts = self.batch_search([list(query)], options)
         c = int(counts[0])
         return list(zip(ids[0, :c].tolist(), scores[0, :c].tolist()))
+
+    def search_all_results(self, queries, options):
+        """top_k None (options.top_k = None): every candidate of every query -> a SparseResults handle"""
+        o, d, v = _as_csr(queries)
+        p = options.params()
+        h = C.c_void_p()
+        _check(_lib.load().cdb_sparse_search_batch_all(self.h, _ptr(o), _ptr(d), _ptr(v), len(o) - 1, C.byref(p), C.byref(h)))
+        return SparseResults(h)
+
+    def batch_search_all(self, queries, options):
+        """top_k None: every candidate of every query, best first -> (offsets u64[B+1], ids u32[total], scores f32[total]);
+        query q's results are ids[offsets[q]:offsets[q+1]]"""
+        r = self.search_all_results(queries, options)
+        try:
+            off = r.offsets()
+            ids, scores = r.read(0, len(off) - 1)
+        finally:
+            r.close()
+        return off, ids, scores
 
     def sample_embedding(self, pairs, device=None):
         """accumulates the sampling counters over the pair values (sample_embedding)"""
@@ -917,6 +940,38 @@ class SparseIndex:
         got = C.c_uint64(0)
         _check(_lib.load().cdb_sparse_index_append_itoe(self.h, os.fsencode(collection_dir), _ptr(ids), n, C.byref(got)))
         return ids[: got.value]
+
+
+class SparseResults:
+    """The results of a top_k None sparse search (cdb_sparse_results), held by the library in host memory"""
+
+    def __init__(self, h):
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            _lib.load().cdb_sparse_results_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def offsets(self):
+        """-> u64[n_queries + 1]"""
+        L = _lib.load()
+        n = C.c_uint32(0)
+        _check(L.cdb_sparse_results_offsets(self.h, C.byref(n), None))
+        off = np.zeros(n.value + 1, np.uint64)
+        _check(L.cdb_sparse_results_offsets(self.h, C.byref(n), _ptr(off)))
+        return off
+
+    def read(self, first, n):
+        """entries of queries [first, first + n) -> (ids u32, scores f32)"""
+        off = self.offsets()
+        m = int(off[first + n] - off[first]) if first + n < len(off) else 0
+        ids = np.zeros(max(m, 1), np.uint32)
+        scores = np.zeros(max(m, 1), np.float32)
+        _check(_lib.load().cdb_sparse_results_read(self.h, first, n, _ptr(ids), _ptr(scores)))
+        return ids[:m], scores[:m]
 
 
 def sparse_sample_upper_bound(values, clamp_margin_percent=1.0, prior_counts=None, prior_values=0, device=0):

@@ -10,10 +10,13 @@
 #include <cmath>
 #include <memory>
 #include <mutex>
+#include <new>
 #include <shared_mutex>
 #include <vector>
 
 #include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include "kernels.h"
 #include "posting_tiles.cuh"
@@ -242,6 +245,52 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_merge_kernel(const uint64_t 
     if (tid == 0) out_cnt[(size_t)qi * n_out + grp] = s_cnt;
 }
 
+// finalize_sparse_ann_results' dot product of one candidate row (pairs [rb, re)) with the query pairs [qb, qe), by one
+// whole warp: the query pairs of a 32-wide chunk meet the row's pairs through shuffles (a row's later pair of a dim
+// overwrites an earlier one, dims the row lacks are skipped), then dp = 0f32; dp += row_v * q_v sequentially in the
+// caller's order.  Every lane returns dp.  Both re-ranks (sp_finalize_kernel, sp_rerank_all_kernel) call this.
+__device__ __forceinline__ float sp_rerank_dot(uint64_t qb, uint64_t qe, const uint32_t *__restrict__ q_dims,
+                                               const float *__restrict__ q_vals, uint64_t rb, uint64_t re,
+                                               const uint32_t *__restrict__ dims, const float *__restrict__ vals) {
+    const uint32_t lane = threadIdx.x & 31;
+    float dp = 0.0f;
+    for (uint64_t j0 = qb; j0 < qe; j0 += 32) {
+        const uint32_t nj = (uint32_t)std::min<uint64_t>(32, qe - j0);
+        uint32_t qd = 0xFFFFFFFFu;
+        float qv = 0.0f, val = 0.0f;
+        bool found = false;
+        if (lane < nj) { qd = q_dims[j0 + lane]; qv = q_vals[j0 + lane]; }
+        for (uint64_t p0 = rb; p0 < re; p0 += 32) {
+            const uint32_t np = (uint32_t)std::min<uint64_t>(32, re - p0);
+            uint32_t rd = 0;
+            float rv = 0.0f;
+            if (lane < np) { rd = dims[p0 + lane]; rv = vals[p0 + lane]; }
+            for (uint32_t l = 0; l < np; ++l) {
+                const uint32_t d = __shfl_sync(0xFFFFFFFFu, rd, l);
+                const float v = __shfl_sync(0xFFFFFFFFu, rv, l);
+                if (lane < nj && d == qd) { val = v; found = true; }
+            }
+        }
+        for (uint32_t l = 0; l < nj; ++l) {
+            const bool f = __shfl_sync(0xFFFFFFFFu, found, l);
+            const float x = __shfl_sync(0xFFFFFFFFu, val, l), y = __shfl_sync(0xFFFFFFFFu, qv, l);
+            if (f) dp = __fadd_rn(dp, __fmul_rn(x, y));
+        }
+    }
+    return dp;
+}
+
+// the re-ranked selection key: total_cmp order of the canonicalised dp, then the smaller id
+__device__ __forceinline__ uint64_t sp_rerank_key(float dp, uint32_t id) {
+    return ((uint64_t)order_key(CDB_METRIC_DOT_PRODUCT, __float_as_uint(canon_nan(dp))) << 32) | (uint64_t)(~id);
+}
+
+// a selection key's score: the re-ranked f32, else the u32 similarity as f32
+__device__ __forceinline__ float sp_key_score(uint64_t key, int rerank) {
+    const uint32_t hi = (uint32_t)(key >> 32);
+    return rerank ? __uint_as_float(key_to_bits(CDB_METRIC_DOT_PRODUCT, hi)) : __uint2float_rn(hi);
+}
+
 // one list of <= m candidates per query -> the best k, best first.  rerank: finalize_sparse_ann_results -- for every
 // candidate dp = 0f32, dp += doc_val * q_val over the query pairs in the caller's order (a row's last pair of a dim wins),
 // then total_cmp order (NaN canonicalised), ties to the smaller id.  Otherwise the score is the u32 similarity as f32.
@@ -265,32 +314,8 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_finalize_kernel(const uint64
         const uint64_t qb = q_off[q], qe = q_off[q + 1];
         for (uint32_t c = warp; c < n; c += SP_THREADS / 32) {
             const uint32_t id = ~(uint32_t)keys[c];
-            const uint64_t rb = row_off[id - id_base], re = row_off[id - id_base + 1];
-            float dp = 0.0f;
-            for (uint64_t j0 = qb; j0 < qe; j0 += 32) {
-                const uint32_t nj = (uint32_t)std::min<uint64_t>(32, qe - j0);
-                uint32_t qd = 0xFFFFFFFFu;
-                float qv = 0.0f, val = 0.0f;
-                bool found = false;
-                if (lane < nj) { qd = q_dims[j0 + lane]; qv = q_vals[j0 + lane]; }
-                for (uint64_t p0 = rb; p0 < re; p0 += 32) {
-                    const uint32_t np = (uint32_t)std::min<uint64_t>(32, re - p0);
-                    uint32_t rd = 0;
-                    float rv = 0.0f;
-                    if (lane < np) { rd = dims[p0 + lane]; rv = vals[p0 + lane]; }
-                    for (uint32_t l = 0; l < np; ++l) {
-                        const uint32_t d = __shfl_sync(0xFFFFFFFFu, rd, l);
-                        const float v = __shfl_sync(0xFFFFFFFFu, rv, l);
-                        if (lane < nj && d == qd) { val = v; found = true; }
-                    }
-                }
-                for (uint32_t l = 0; l < nj; ++l) {
-                    const bool f = __shfl_sync(0xFFFFFFFFu, found, l);
-                    const float x = __shfl_sync(0xFFFFFFFFu, val, l), y = __shfl_sync(0xFFFFFFFFu, qv, l);
-                    if (f) dp = __fadd_rn(dp, __fmul_rn(x, y));
-                }
-            }
-            if (lane == 0) keys[c] = ((uint64_t)order_key(CDB_METRIC_DOT_PRODUCT, __float_as_uint(canon_nan(dp))) << 32) | (uint64_t)(~id);
+            const float dp = sp_rerank_dot(qb, qe, q_dims, q_vals, row_off[id - id_base], row_off[id - id_base + 1], dims, vals);
+            if (lane == 0) keys[c] = sp_rerank_key(dp, id);
         }
         __syncthreads();
     }
@@ -302,13 +327,58 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_finalize_kernel(const uint64
         if (i < cnt) {
             const uint64_t key = keys[i];
             id = ~(uint32_t)key;
-            const uint32_t hi = (uint32_t)(key >> 32);
-            s = rerank ? __uint_as_float(key_to_bits(CDB_METRIC_DOT_PRODUCT, hi)) : __uint2float_rn(hi);
+            s = sp_key_score(key, rerank);
         }
         out_ids[(size_t)qi * k + i] = id;
         out_scores[(size_t)qi * k + i] = s;
     }
     if (tid == 0) out_counts[qi] = cnt;
+}
+
+// ---------------------------------------------------------------- top_k None: every candidate
+// The scoring kernel runs with m = TILE_ROWS, so it never selects and writes every touched live row of (query qi, tile t)
+// into slot [qi][t].  pos = exclusive scan of the [chunk][n_tiles] counts, so query qi's candidates become the contiguous
+// segment [pos[qi * n_tiles], pos[(qi + 1) * n_tiles]).  One CTA per (tile, query) copies its slot there, tags each key with
+// its query, and the (0, qi) CTA writes the segment offset seg[qi] (the last query's also seg[chunk]).
+__global__ void __launch_bounds__(256) sp_all_gather_kernel(const uint64_t *__restrict__ slots, const uint32_t *__restrict__ cnt,
+                                                            const uint32_t *__restrict__ pos, uint32_t n_tiles, uint64_t *__restrict__ keys,
+                                                            uint32_t *__restrict__ qis, uint32_t *__restrict__ seg) {
+    const uint32_t t = blockIdx.x, qi = blockIdx.y, slot = qi * n_tiles + t;
+    const uint32_t n = cnt[slot], base = pos[slot];
+    const uint64_t *src = slots + (size_t)slot * TILE_ROWS;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+        keys[base + i] = src[i];
+        qis[base + i] = qi;
+    }
+    if (t == 0 && threadIdx.x == 0) {
+        seg[qi] = pos[slot];
+        if (qi == gridDim.y - 1) seg[qi + 1] = pos[(qi + 1) * n_tiles];
+    }
+}
+
+// rerank = 1 over the flat candidate array: one warp per candidate, the query from its tag, the same dot product as
+// sp_finalize_kernel, rekeyed in place
+__global__ void __launch_bounds__(256) sp_rerank_all_kernel(uint64_t *__restrict__ keys, const uint32_t *__restrict__ qis, uint32_t n,
+                                                            uint32_t q0, const uint64_t *__restrict__ q_off, const uint32_t *__restrict__ q_dims,
+                                                            const float *__restrict__ q_vals, const uint64_t *__restrict__ row_off,
+                                                            const uint32_t *__restrict__ dims, const float *__restrict__ vals, uint32_t id_base) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    for (uint64_t c = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < n; c += warps) {
+        const uint32_t id = ~(uint32_t)keys[c], q = q0 + qis[c];
+        const float dp = sp_rerank_dot(q_off[q], q_off[q + 1], q_dims, q_vals, row_off[id - id_base], row_off[id - id_base + 1], dims, vals);
+        if (lane == 0) keys[c] = sp_rerank_key(dp, id);
+    }
+}
+
+// keys -> ids and scores, as sp_finalize_kernel writes them
+__global__ void __launch_bounds__(256) sp_all_decode_kernel(const uint64_t *__restrict__ keys, uint32_t n, int rerank, uint32_t *__restrict__ ids,
+                                                            float *__restrict__ scores) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint64_t key = keys[i];
+        ids[i] = ~(uint32_t)key;
+        scores[i] = sp_key_score(key, rerank);
+    }
 }
 
 // sample_embedding: values > 1.0 ... > 9.0 (inverted/mod.rs:148-192)
@@ -344,6 +414,13 @@ struct cdb_sparse_index {
     PostingTiles<SparseCodec> st;   // keys: dims
 };
 
+// the results of a top_k None search, in host memory: query q's entries are [off[q], off[q+1])
+struct cdb_sparse_results {
+    std::vector<uint64_t> off{0};
+    std::vector<uint32_t> ids;
+    std::vector<float> scores;
+};
+
 namespace {
 
 cdb_status check_search_params(const cdb_sparse_search_params *p, uint32_t *m) {
@@ -355,6 +432,27 @@ cdb_status check_search_params(const cdb_sparse_search_params *p, uint32_t *m) {
     return CDB_OK;
 }
 
+// sequential_search, sparse_ann_query.rs:80-83: etv = ((2^bits * thr).min(255.0)) as u8, low = (thr * 2^bits) as u32
+void sp_thresholds(float thr, uint32_t bits, uint32_t *etv, uint32_t *low) {
+    const float prod = (float)(1u << bits) * thr;
+    const float etv_f = std::isnan(prod) ? 255.0f : std::min(prod, 255.0f);
+    *etv = sat_u32(etv_f, 255);
+    *low = sat_u32(thr * (float)(1u << bits), 0xFFFFFFFFu);
+}
+
+// the scoring kernel's arguments for queries [q0, q0 + chunk) keeping m candidates per (query, tile)
+SpSearch score_args(const cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals,
+                    const cdb_sparse_search_params *p, uint32_t q0, uint32_t m, uint64_t *out_keys, uint32_t *out_cnt) {
+    const PostingTiles<SparseCodec> &st = ix->st;
+    SpSearch a;
+    a.entries = st.entries(); a.tdims = st.d_tkeys; a.tseg = st.d_tseg; a.deleted = st.deleted();
+    a.tiles = st.d_tiles; a.n_rows = st.n_rows; a.id_base = ix->desc.id_base; a.maxq = st.codec.maxq;
+    sp_thresholds(p->early_terminate_threshold, ix->desc.quantization_bits, &a.etv, &a.low);
+    a.ub = st.codec.ub; a.q_off = d_qoff; a.q_dims = d_qdims; a.q_vals = d_qvals; a.q0 = q0; a.m = m;
+    a.n_tiles = (uint32_t)st.h_tiles.size(); a.out_keys = out_keys; a.out_cnt = out_cnt;
+    return a;
+}
+
 // the search on device buffers, under the reader lock
 cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
                          const cdb_sparse_search_params *p, uint32_t m, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
@@ -362,12 +460,6 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
     if (!nq) return CDB_OK;
     const uint32_t k = p->k;
     const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
-    const uint32_t bits = ix->desc.quantization_bits;
-    // sequential_search, sparse_ann_query.rs:80-83
-    const float thr = p->early_terminate_threshold;
-    const float prod = (float)(1u << bits) * thr;
-    const float etv_f = std::isnan(prod) ? 255.0f : std::min(prod, 255.0f);
-    const uint32_t etv = sat_u32(etv_f, 255), low = sat_u32(thr * (float)(1u << bits), 0xFFFFFFFFu);
     if (n_tiles == 0) return fill_empty_results(nq, k, d_ids, d_scores, d_counts, s);
     const uint32_t g = std::min<uint32_t>(SP_MERGE_MAX_LISTS, std::max<uint32_t>(2, SP_MERGE_KEYS / m));
     const uint32_t n_lvl1 = (n_tiles + g - 1) / g;
@@ -393,12 +485,7 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
     }
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
-        const PostingTiles<SparseCodec> &st = ix->st;
-        SpSearch a;
-        a.entries = st.entries(); a.tdims = st.d_tkeys; a.tseg = st.d_tseg; a.deleted = st.deleted();
-        a.tiles = st.d_tiles; a.n_rows = st.n_rows; a.id_base = ix->desc.id_base; a.maxq = st.codec.maxq; a.etv = etv; a.low = low;
-        a.ub = st.codec.ub; a.q_off = d_qoff; a.q_dims = d_qdims; a.q_vals = d_qvals; a.q0 = q0; a.m = m;
-        a.n_tiles = n_tiles; a.out_keys = ka; a.out_cnt = ca;
+        const SpSearch a = score_args(ix, d_qoff, d_qdims, d_qvals, p, q0, m, ka, ca);
         sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(a);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
@@ -422,6 +509,110 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
     }
     for (void *ptr : {(void *)ka, (void *)kb, (void *)ca, (void *)cb})
+        if (ptr) cudaFreeAsync(ptr, s);
+    return rc;
+}
+
+constexpr size_t SP_ALL_BUDGET = 512ull << 20;   // device scratch of one chunk of a top_k None search
+
+// Sorts each query's segment of keys descending: a stable radix sort of all keys descending carrying their query tags,
+// then a stable sort on the tags (qbits wide; none for a single query) carrying the keys.  Keys are unique per query.
+cudaError_t sp_sort_segments(void *tmp, size_t tmp_bytes, cub::DoubleBuffer<uint64_t> &keys, cub::DoubleBuffer<uint32_t> &qis, uint32_t n,
+                             int qbits, cudaStream_t s) {
+    size_t tb = tmp_bytes;
+    cudaError_t e = cub::DeviceRadixSort::SortPairsDescending(tmp, tb, keys, qis, (int)n, 0, 64, s);
+    if (e == cudaSuccess && qbits) {
+        tb = tmp_bytes;
+        e = cub::DeviceRadixSort::SortPairs(tmp, tb, qis, keys, (int)n, 0, qbits, s);
+    }
+    return e;
+}
+
+// The top_k None search on device queries, under the reader lock: every candidate of every query, sorted (and re-ranked),
+// appended to r in host memory.  Per chunk of queries: score into per-(query, tile) slots, scan the slot counts, gather
+// each query's keys into one segment, sort the segments, re-rank and sort again, decode, copy out.
+cdb_status search_all_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
+                             const cdb_sparse_search_params *p, cdb_sparse_results *r, cudaStream_t s) {
+    const PostingTiles<SparseCodec> &st = ix->st;
+    const uint32_t n_tiles = (uint32_t)st.h_tiles.size();
+    const uint64_t n_live = st.n_rows - st.n_deleted;   // a query's candidates, at most
+    r->off.assign((size_t)nq + 1, 0);
+    if (!nq || !n_tiles || !n_live) return CDB_OK;
+    CDB_REQUIRE(n_live < (1ull << 31), "top_k None: an index with 2^31 live rows or more");
+    const size_t per_q = (size_t)n_tiles * TILE_ROWS * 8 + (size_t)n_tiles * 8 + n_live * 24;
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, SP_ALL_BUDGET / per_q}));
+    const uint64_t cap = (uint64_t)chunk * n_live;      // candidates of a chunk, at most (< 2^31: budget or one query)
+    const uint32_t n_slots = chunk * n_tiles;
+    auto qbits_of = [](uint32_t c) { return c > 1 ? 32 - __builtin_clz(c - 1) : 0; };
+    uint64_t *slots = nullptr, *ka = nullptr, *kb = nullptr;
+    uint32_t *cnt = nullptr, *pos = nullptr, *qa = nullptr, *qb = nullptr, *seg = nullptr;
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    auto setup = [&]() -> cdb_status {
+        size_t t_scan = 0, t_sort1 = 0, t_sort2 = 0;
+        cub::DoubleBuffer<uint64_t> kd(nullptr, nullptr);
+        cub::DoubleBuffer<uint32_t> qd(nullptr, nullptr);
+        CDB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, cnt, pos, (int)n_slots + 1, s));
+        CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, t_sort1, kd, qd, (int)cap, 0, 64, s));
+        if (chunk > 1) CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort2, qd, kd, (int)cap, 0, qbits_of(chunk), s));
+        tmp_bytes = std::max({t_scan, t_sort1, t_sort2});
+        CDB_CUDA_TRY(cudaMallocAsync(&slots, (size_t)n_slots * TILE_ROWS * 8, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&cnt, ((size_t)n_slots + 1) * 4, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&pos, ((size_t)n_slots + 1) * 4, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&seg, ((size_t)chunk + 1) * 4, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&ka, cap * 8, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&kb, cap * 8, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&qa, cap * 4, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&qb, cap * 4, s));
+        CDB_CUDA_TRY(cudaMallocAsync(&tmp, std::max<size_t>(tmp_bytes, 1), s));
+        CDB_CUDA_TRY(allow_max_dynamic_smem((const void *)sp_score_tile_kernel));
+        return CDB_OK;
+    };
+    std::vector<uint32_t> h_seg((size_t)chunk + 1);
+    auto run_chunk = [&](uint32_t q0, uint32_t c) -> cdb_status {
+        const SpSearch a = score_args(ix, d_qoff, d_qdims, d_qvals, p, q0, TILE_ROWS, slots, cnt);
+        sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(a);
+        CDB_LAUNCH_CHECK();
+        CDB_CUDA_TRY(cudaMemsetAsync(cnt + (size_t)c * n_tiles, 0, 4, s));
+        size_t tb = tmp_bytes;
+        CDB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, pos, (int)(c * n_tiles) + 1, s));
+        sp_all_gather_kernel<<<dim3(n_tiles, c), 256, 0, s>>>(slots, cnt, pos, n_tiles, ka, qa, seg);
+        CDB_LAUNCH_CHECK();
+        CDB_CUDA_TRY(cudaMemcpyAsync(h_seg.data(), seg, ((size_t)c + 1) * 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaStreamSynchronize(s));
+        const uint32_t total = h_seg[c];
+        const uint64_t base = r->ids.size();
+        for (uint32_t i = 0; i < c; ++i) r->off[(size_t)q0 + i + 1] = base + h_seg[i + 1];
+        if (!total) return CDB_OK;
+        cub::DoubleBuffer<uint64_t> kd(ka, kb);
+        cub::DoubleBuffer<uint32_t> qd(qa, qb);
+        CDB_CUDA_TRY(sp_sort_segments(tmp, tmp_bytes, kd, qd, total, qbits_of(c), s));
+        if (p->rerank) {
+            const uint32_t blocks = (uint32_t)std::min<uint64_t>(((uint64_t)total + 7) / 8, 1u << 20);
+            sp_rerank_all_kernel<<<blocks, 256, 0, s>>>(kd.Current(), qd.Current(), total, q0, d_qoff, d_qdims, d_qvals, st.d_row_off,
+                                                        st.d_keys, st.d_vals, ix->desc.id_base);
+            CDB_LAUNCH_CHECK();
+            CDB_CUDA_TRY(sp_sort_segments(tmp, tmp_bytes, kd, qd, total, qbits_of(c), s));
+        }
+        uint32_t *ids = reinterpret_cast<uint32_t *>(kd.Alternate());   // the free half holds ids, then scores
+        float *scores = reinterpret_cast<float *>(ids + total);
+        sp_all_decode_kernel<<<std::min<uint32_t>((total + 255) / 256, 1u << 16), 256, 0, s>>>(kd.Current(), total, p->rerank ? 1 : 0, ids, scores);
+        CDB_LAUNCH_CHECK();
+        r->ids.resize(base + total);
+        r->scores.resize(base + total);
+        CDB_CUDA_TRY(cudaMemcpyAsync(r->ids.data() + base, ids, (size_t)total * 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaMemcpyAsync(r->scores.data() + base, scores, (size_t)total * 4, cudaMemcpyDeviceToHost, s));
+        CDB_CUDA_TRY(cudaStreamSynchronize(s));
+        return CDB_OK;
+    };
+    cdb_status rc = setup();
+    try {
+        for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) rc = run_chunk(q0, std::min(chunk, nq - q0));
+    } catch (const std::bad_alloc &) {
+        set_error("top_k None: host allocation of the results failed");
+        rc = CDB_CUDA_ERROR;
+    }
+    for (void *ptr : {(void *)slots, (void *)cnt, (void *)pos, (void *)seg, (void *)ka, (void *)kb, (void *)qa, (void *)qb, tmp})
         if (ptr) cudaFreeAsync(ptr, s);
     return rc;
 }
@@ -559,6 +750,71 @@ cdb_status cdb_sparse_search_batch(cdb_sparse_index *ix, const uint64_t *q_offse
     }
     cudaFreeAsync(buf, s);
     return rc;
+}
+
+cdb_status cdb_sparse_search_batch_all(cdb_sparse_index *ix, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
+                                       uint32_t nq, const cdb_sparse_search_params *p, cdb_sparse_results **out) {
+    CDB_REQUIRE(ix && p && out, "null argument");
+    *out = nullptr;
+    CDB_REQUIRE(p->k == 0, "cdb_sparse_search_batch_all takes k = 0 (top_k None)");
+    uint64_t nqp = 0;
+    if (nq) {
+        const cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
+        if (rc) return rc;
+        nqp = q_offsets[nq];
+        CDB_REQUIRE((q_dims && q_values) || !nqp, "null query pairs");
+    }
+    std::unique_ptr<cdb_sparse_results> r(new (std::nothrow) cdb_sparse_results());
+    CDB_REQUIRE(r, "out of host memory");
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    if (!nq || ix->st.h_tiles.empty()) {   // no query or no row: every query has no candidate, nothing runs on the device
+        r->off.assign((size_t)nq + 1, 0);
+        *out = r.release();
+        return CDB_OK;
+    }
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    cudaStream_t s = sg.s;
+    const size_t bytes = ((size_t)nq + 1) * 8 + nqp * 8;
+    uint8_t *buf = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
+    uint64_t *d_off = reinterpret_cast<uint64_t *>(buf);
+    uint32_t *d_qd = reinterpret_cast<uint32_t *>(d_off + nq + 1);
+    float *d_qv = reinterpret_cast<float *>(d_qd + nqp);
+    cdb_status rc = CDB_OK;
+    cudaError_t e = cudaMemcpyAsync(d_off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && nqp) e = cudaMemcpyAsync(d_qd, q_dims, nqp * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && nqp) e = cudaMemcpyAsync(d_qv, q_values, nqp * 4, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) { set_error(std::string("cudaMemcpyAsync: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    if (!rc) rc = search_all_locked(ix, d_off, d_qd, d_qv, nq, p, r.get(), s);
+    cudaFreeAsync(buf, s);
+    if (rc) return rc;
+    *out = r.release();
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_results_offsets(const cdb_sparse_results *r, uint32_t *out_n_queries, uint64_t *out_offsets) {
+    CDB_REQUIRE(r && out_n_queries, "null argument");
+    *out_n_queries = (uint32_t)(r->off.size() - 1);
+    if (out_offsets) std::copy(r->off.begin(), r->off.end(), out_offsets);
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_results_read(const cdb_sparse_results *r, uint32_t first, uint32_t n, uint32_t *out_ids, float *out_scores) {
+    CDB_REQUIRE(r, "null results");
+    CDB_REQUIRE((uint64_t)first + n <= r->off.size() - 1, "read range past the results' queries");
+    const uint64_t b = r->off[first], e = r->off[(size_t)first + n];
+    if (b == e) return CDB_OK;
+    CDB_REQUIRE(out_ids && out_scores, "null output");
+    std::copy(r->ids.begin() + b, r->ids.begin() + e, out_ids);
+    std::copy(r->scores.begin() + b, r->scores.begin() + e, out_scores);
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_results_destroy(cdb_sparse_results *r) {
+    delete r;
+    return CDB_OK;
 }
 
 cdb_status cdb_sparse_sample_upper_bound(int32_t device, const float *values, uint64_t n, float clamp_margin_percent,

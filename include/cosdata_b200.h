@@ -660,7 +660,7 @@ cdb_status cdb_index_last_candidate_counts(const cdb_index *index, uint32_t n, u
  *               query pairs in the caller's order (a row's last pair of a dim wins, dims the row lacks are skipped), sorted
  *               by total_cmp (NaN canonicalised to the sign-set quiet NaN), ties to the smaller id, truncated to k.
  * out_counts[q] = min(k, candidates); unused slots hold CDB_INVALID_ID / 0.  k must be 1..1024 and k * f <= 5120
- * (CDB_INVALID_PARAMS otherwise, nothing truncated).  Searches on one handle are re-entrant; append and delete take the
+ * (CDB_INVALID_PARAMS otherwise, nothing truncated); top_k None (k = 0) is cdb_sparse_search_batch_all.  Searches on one handle are re-entrant; append and delete take the
  * handle exclusively and first wait for the searches already enqueued on the device.  An append that fails changes nothing.  Deleted rows (a tombstone per row, as mark_embedding_as_deleted with the inserted pairs leaves it)
  * are never candidates; rows are not reused.  Without a CUDA device every compute entry point returns CDB_CUDA_ERROR. */
 typedef struct cdb_sparse_index cdb_sparse_index; /* opaque */
@@ -675,7 +675,8 @@ typedef struct {
 } cdb_sparse_index_desc;
 
 typedef struct {
-    uint32_t k;                        /* top_k (Some); the reference's None is not supported */
+    uint32_t k;                        /* top_k: 1..1024 for cdb_sparse_search_batch{,_device}; 0 = None, which only
+                                          cdb_sparse_search_batch_all takes (reranking_factor is then ignored) */
     float early_terminate_threshold;   /* the request's value, else config.search.early_terminate_threshold (0.0) */
     int32_t rerank;                    /* config.rerank_sparse_with_raw_values (default 0) */
     uint32_t reranking_factor;         /* config.sparse_raw_values_reranking_factor (default 5), used when rerank */
@@ -699,6 +700,34 @@ cdb_status cdb_sparse_search_batch(cdb_sparse_index *index, const uint64_t *q_of
 cdb_status cdb_sparse_search_batch_device(cdb_sparse_index *index, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
                                           const float *d_q_values, uint32_t n_queries, const cdb_sparse_search_params *params,
                                           uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream);
+/* top_k None (SparseSearchRequestDto.top_k omitted): sequential_search keeps every candidate and finalize_sparse_ann_results
+ * re-ranks and sorts all of them without truncating (sparse_ann_query.rs:136-145, inverted/mod.rs:331-381).  params->k must
+ * be 0 (else CDB_INVALID_PARAMS); reranking_factor is ignored; the threshold and rerank keep their meaning above.
+ *   candidates: exactly the rows the top-k search considers -- live rows touched by any visited list, rows reached only
+ *               through zero products included, deleted and empty rows never; the similarity is the same wrapping u32.
+ *   rerank = 0: every candidate with score = similarity as f32, ordered by (similarity desc, id asc).  The reference returns
+ *               HashMap order here, which is unspecified; this is the order the top-k search uses.
+ *   rerank = 1: every candidate re-ranked as in the top-k search (sequential dp in the caller's order, a row's last pair of a
+ *               dim wins, total_cmp with NaN canonicalised, ties to the smaller id), not truncated.
+ * The number of results is known only after scoring, so they come back in a handle the library owns, in host memory:
+ * *out receives it (NULL on failure), cdb_sparse_results_offsets gives the number of queries and offsets[n_queries+1]
+ * (query q's results are entries [offsets[q], offsets[q+1])), cdb_sparse_results_read copies the entries of queries
+ * [first_query, first_query + n_queries) -- offsets[first+n] - offsets[first] of them -- best first, and
+ * cdb_sparse_results_destroy frees it (NULL is a no-op).  The handle does not reference the index: appends, deletes and
+ * destroying the index afterwards leave it unchanged; reads of one handle are re-entrant.  n_queries = 0 or an index
+ * without rows gives a handle of n_queries empty queries without running anything on the device.  Null arguments,
+ * malformed query CSR and a read range past the handle's queries are CDB_INVALID_PARAMS, refused before the device is
+ * touched.  There is no device-memory form: a caller could not size its result buffers before the call.  Device scratch
+ * is bounded by searching the queries in chunks (512 MB of scratch; a chunk holds at least one query); failing
+ * allocations are CDB_CUDA_ERROR and leave nothing allocated.  The index's live rows must be fewer than 2^31. */
+typedef struct cdb_sparse_results cdb_sparse_results; /* opaque, host memory */
+cdb_status cdb_sparse_search_batch_all(cdb_sparse_index *index, const uint64_t *q_offsets, const uint32_t *q_dims,
+                                       const float *q_values, uint32_t n_queries, const cdb_sparse_search_params *params,
+                                       cdb_sparse_results **out);
+cdb_status cdb_sparse_results_offsets(const cdb_sparse_results *results, uint32_t *out_n_queries, uint64_t *out_offsets);
+cdb_status cdb_sparse_results_read(const cdb_sparse_results *results, uint32_t first_query, uint32_t n_queries, uint32_t *out_ids,
+                                   float *out_scores);
+cdb_status cdb_sparse_results_destroy(cdb_sparse_results *results);
 /* InvertedIndex::sample_embedding + finalize_sampling (inverted/mod.rs:148-247) over n pair values:
  *   out_counts[t-1] = #values > t for t = 1..9 (prior_counts, may be NULL, added first; prior_values = values they cover)
  *   out_ub = first t with (count as f32 / values as f32) * 100.0 <= clamp_margin_percent, else 10.0 (also with no values) */
