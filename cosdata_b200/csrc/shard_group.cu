@@ -15,9 +15,11 @@
 #include <dlfcn.h>
 #include <nccl.h>
 
+#include <algorithm>
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <shared_mutex>
 #include <string>
 #include <vector>
 
@@ -30,6 +32,36 @@ cdb_status index_search_device_keys(cdb_index *ix, const float *d_queries, uint3
 int index_device(const cdb_index *ix);
 uint32_t index_dim(const cdb_index *ix);
 int index_result_metric(const cdb_index *ix, int mode);
+
+// sparse.cu: a shard group's two-phase sparse search
+std::shared_mutex &sparse_index_mutex(cdb_sparse_index *ix);
+int sparse_index_device(const cdb_sparse_index *ix);
+uint32_t sparse_index_bits(const cdb_sparse_index *ix);
+float sparse_index_upper_bound(const cdb_sparse_index *ix);
+uint32_t sparse_index_id_base(const cdb_sparse_index *ix);
+uint64_t sparse_index_capacity(const cdb_sparse_index *ix);
+cdb_status sparse_check_params(const cdb_sparse_search_params *p, uint32_t *m);
+cdb_status sparse_shard_select(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
+                               const cdb_sparse_search_params *p, uint32_t m, uint64_t *keys, uint32_t *cnt, cudaStream_t s);
+cdb_status sparse_group_select(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t m, uint64_t *keys,
+                               uint32_t *cnt, cudaStream_t s);
+cdb_status sparse_shard_rerank(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
+                               uint32_t m, const uint64_t *keys, const uint32_t *cnt, uint64_t *out, cudaStream_t s);
+cdb_status sparse_group_finalize(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t m, uint32_t k, int rerank,
+                                 uint64_t *keys, const uint32_t *cnt, uint32_t *ids, float *scores, uint32_t *counts, cudaStream_t s);
+
+// tfidf.cu: a shard group's TF-IDF search under the group's idf
+std::shared_mutex &tfidf_index_mutex(cdb_tfidf_index *ix);
+int tfidf_index_device(const cdb_tfidf_index *ix);
+uint32_t tfidf_index_id_base(const cdb_tfidf_index *ix);
+uint64_t tfidf_index_capacity(const cdb_tfidf_index *ix);
+uint32_t tfidf_out_cols(uint32_t k);
+float tfidf_idf(uint32_t n_docs, uint32_t df);
+uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *df);
+cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, const float *d_qidf, uint32_t nq,
+                               uint2 *out, cudaStream_t s);
+cdb_status tfidf_group_finalize(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t k, uint32_t *ids, float *scores,
+                                uint32_t *counts, cudaStream_t s);
 
 namespace {
 struct NcclApi {
@@ -144,18 +176,22 @@ struct cdb_shard_group {
     std::vector<int> dev;                 // per local slot
     std::vector<ncclComm_t> comm;
     std::vector<cdb_index *> shard;
+    std::vector<cdb_sparse_index *> sparse;   // a slot may hold a dense, a sparse and a TF-IDF shard at once
+    std::vector<cdb_tfidf_index *> tfidf;
     std::vector<cudaStream_t> stream;
     std::vector<cudaEvent_t> ev;
-    std::vector<Buf> gather, q, ids, scores, counts, err;
+    std::vector<Buf> gather, q, ids, scores, counts, err, sel;
     std::mutex mu;
 };
 
 static cdb_status group_alloc_slots(cdb_shard_group *g, size_t n) {
     g->comm.assign(n, nullptr);
     g->shard.assign(n, nullptr);
+    g->sparse.assign(n, nullptr);
+    g->tfidf.assign(n, nullptr);
     g->stream.assign(n, nullptr);
     g->ev.assign(n, nullptr);
-    g->gather.resize(n); g->q.resize(n); g->ids.resize(n); g->scores.resize(n); g->counts.resize(n); g->err.resize(n);
+    g->gather.resize(n); g->q.resize(n); g->ids.resize(n); g->scores.resize(n); g->counts.resize(n); g->err.resize(n); g->sel.resize(n);
     for (size_t i = 0; i < n; ++i) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
         CDB_CUDA_TRY(cudaStreamCreateWithFlags(&g->stream[i], cudaStreamNonBlocking));
@@ -233,7 +269,7 @@ cdb_status cdb_shard_group_destroy(cdb_shard_group *g) {
         cudaSetDevice(g->dev[i]);
         if (i < g->stream.size() && g->stream[i]) cudaStreamSynchronize(g->stream[i]);
         if (i < g->comm.size() && g->comm[i] && n) n->CommDestroy(g->comm[i]);
-        for (auto *v : {&g->gather, &g->q, &g->ids, &g->scores, &g->counts, &g->err})
+        for (auto *v : {&g->gather, &g->q, &g->ids, &g->scores, &g->counts, &g->err, &g->sel})
             if (i < v->size()) (*v)[i].release();
         if (i < g->ev.size() && g->ev[i]) cudaEventDestroy(g->ev[i]);
         if (i < g->stream.size() && g->stream[i]) cudaStreamDestroy(g->stream[i]);
@@ -250,28 +286,52 @@ cdb_status cdb_shard_group_attach(cdb_shard_group *g, uint32_t local_slot, cdb_i
     return CDB_OK;
 }
 
+// [base, base + capacity) of two shards of one local group must not meet: a candidate belongs to exactly one shard
+static bool id_ranges_meet(uint32_t b0, uint64_t c0, uint32_t b1, uint64_t c1) { return b0 < b1 + c1 && b1 < b0 + c0; }
+
+cdb_status cdb_shard_group_attach_sparse(cdb_shard_group *g, uint32_t local_slot, cdb_sparse_index *shard) {
+    CDB_REQUIRE(g && shard && local_slot < g->dev.size(), "bad argument");
+    CDB_REQUIRE(sparse_index_device(shard) == g->dev[local_slot], "the shard lives on another device than the group slot");
+    const float ub = sparse_index_upper_bound(shard);
+    for (size_t j = 0; j < g->dev.size(); ++j) {
+        const cdb_sparse_index *o = g->sparse[j];
+        if (!o || j == local_slot) continue;
+        const float oub = sparse_index_upper_bound(o);
+        CDB_REQUIRE(sparse_index_bits(o) == sparse_index_bits(shard) && memcmp(&oub, &ub, 4) == 0,
+                    "sparse shards differ in quantization_bits or values_upper_bound");
+        CDB_REQUIRE(!id_ranges_meet(sparse_index_id_base(o), sparse_index_capacity(o), sparse_index_id_base(shard), sparse_index_capacity(shard)),
+                    "sparse shards' id ranges overlap");
+    }
+    g->sparse[local_slot] = shard;
+    return CDB_OK;
+}
+
+cdb_status cdb_shard_group_attach_tfidf(cdb_shard_group *g, uint32_t local_slot, cdb_tfidf_index *shard) {
+    CDB_REQUIRE(g && shard && local_slot < g->dev.size(), "bad argument");
+    CDB_REQUIRE(tfidf_index_device(shard) == g->dev[local_slot], "the shard lives on another device than the group slot");
+    for (size_t j = 0; j < g->dev.size(); ++j) {
+        const cdb_tfidf_index *o = g->tfidf[j];
+        if (!o || j == local_slot) continue;
+        CDB_REQUIRE(!id_ranges_meet(tfidf_index_id_base(o), tfidf_index_capacity(o), tfidf_index_id_base(shard), tfidf_index_capacity(shard)),
+                    "tf-idf shards' id ranges overlap");
+    }
+    g->tfidf[local_slot] = shard;
+    return CDB_OK;
+}
+
 uint32_t cdb_shard_group_world(const cdb_shard_group *g) { return g ? g->world : 0; }
 
-// local slot i: search its shard into its slot of its gather buffer, then the collective, then (slot 0 / this rank) the merge
-static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_search_params *p, const std::vector<const float *> &d_q,
-                                  uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
+// the stream local slot i works on: the caller's stream in a per-rank group's device form, else the slot's own
+static cudaStream_t slot_stream(const cdb_shard_group *g, size_t i, cudaStream_t out_stream) {
+    return (g->dev.size() == 1 && out_stream) ? out_stream : g->stream[i];
+}
+
+static uint64_t *gather_buf(const cdb_shard_group *g, size_t i) { return reinterpret_cast<uint64_t *>(g->gather[i].p); }
+
+// Rank r's `words` u64 words at gather_buf(slot) + r * words reach every local slot's gather buffer (NCCL all-gather), or,
+// in a loopback group, slot 0's buffer only (device copies ordered by events).  Nothing to do in a group of one rank.
+static cdb_status group_allgather(cdb_shard_group *g, size_t words, cudaStream_t out_stream) {
     const size_t nl = g->dev.size();
-    const uint32_t k = p->k;
-    const size_t words = slot_words(nq, k);
-    cdb_status rc;
-    for (size_t i = 0; i < nl; ++i) {
-        CDB_REQUIRE(g->shard[i], "a group slot has no shard attached");
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->gather[i].ensure(g->world * words * 8)) || (rc = g->ids[i].ensure((size_t)nq * k * 4)) ||
-            (rc = g->scores[i].ensure((size_t)nq * k * 4)) || (rc = g->counts[i].ensure((size_t)nq * 4)))
-            return rc;
-        uint64_t *slot = reinterpret_cast<uint64_t *>(g->gather[i].p) + (size_t)(g->rank0 + i) * words;
-        cudaStream_t s = (nl == 1 && out_stream) ? out_stream : g->stream[i];
-        if ((rc = index_search_device_keys(g->shard[i], d_q[i], nq, p, reinterpret_cast<uint32_t *>(g->ids[i].p),
-                                           reinterpret_cast<float *>(g->scores[i].p), reinterpret_cast<uint32_t *>(g->counts[i].p),
-                                           reinterpret_cast<uint8_t *>(slot + (size_t)nq * k), slot, s)))
-            return rc;
-    }
     if (g->world > 1) {
         if (g->loopback) {
             // test mode (a device listed twice): every slot copies its part into slot 0's buffer, ordered by events
@@ -296,6 +356,30 @@ static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_sea
             CDB_NCCL_TRY(n, n->GroupEnd());
         }
     }
+    return CDB_OK;
+}
+
+// local slot i: search its shard into its slot of its gather buffer, then the collective, then (slot 0 / this rank) the merge
+static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_search_params *p, const std::vector<const float *> &d_q,
+                                  uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
+    const size_t nl = g->dev.size();
+    const uint32_t k = p->k;
+    const size_t words = slot_words(nq, k);
+    cdb_status rc;
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_REQUIRE(g->shard[i], "a group slot has no shard attached");
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->gather[i].ensure(g->world * words * 8)) || (rc = g->ids[i].ensure((size_t)nq * k * 4)) ||
+            (rc = g->scores[i].ensure((size_t)nq * k * 4)) || (rc = g->counts[i].ensure((size_t)nq * 4)))
+            return rc;
+        uint64_t *slot = reinterpret_cast<uint64_t *>(g->gather[i].p) + (size_t)(g->rank0 + i) * words;
+        cudaStream_t s = (nl == 1 && out_stream) ? out_stream : g->stream[i];
+        if ((rc = index_search_device_keys(g->shard[i], d_q[i], nq, p, reinterpret_cast<uint32_t *>(g->ids[i].p),
+                                           reinterpret_cast<float *>(g->scores[i].p), reinterpret_cast<uint32_t *>(g->counts[i].p),
+                                           reinterpret_cast<uint8_t *>(slot + (size_t)nq * k), slot, s)))
+            return rc;
+    }
+    if ((rc = group_allgather(g, words, out_stream))) return rc;
     // merge on local slot 0
     CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
     cudaStream_t s0 = (nl == 1 && out_stream) ? out_stream : g->stream[0];
@@ -358,6 +442,251 @@ cdb_status cdb_search_batch_sharded_device(cdb_shard_group *g, const float *d_qu
     std::lock_guard<std::mutex> lock(g->mu);
     std::vector<const float *> d_q(1, d_queries);
     return sharded_enqueue(g, nq, p, d_q, d_out_ids, d_out_scores, d_out_counts, d_err_flags, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------- sparse and TF-IDF shards
+constexpr size_t GROUP_GATHER_BUDGET = 256ull << 20;   // bytes of one chunk's gather buffer; queries are searched in chunks
+
+// queries per chunk when a query takes `per_q` bytes of every rank's gather slot
+static uint32_t group_chunk(const cdb_shard_group *g, uint32_t nq, size_t per_q) {
+    return (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, GROUP_GATHER_BUDGET / (g->world * per_q)}));
+}
+
+// loopback: a chunk's slots write their gather buffers only after slot 0 copied the previous chunk's out of them
+static cdb_status loopback_fence(cdb_shard_group *g) {
+    if (!g->loopback) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    CDB_CUDA_TRY(cudaEventRecord(g->ev[0], g->stream[0]));
+    for (size_t i = 1; i < g->dev.size(); ++i) CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[i], g->ev[0], 0));
+    return CDB_OK;
+}
+
+struct SparseQueries {
+    const uint64_t *off;
+    const uint32_t *dims;
+    const float *vals;
+};
+
+// Per chunk of queries: phase 1 writes every shard's top m (keys, then counts) into its rank's slot; all-gather #1; the
+// group's top m per query (on every local slot, on slot 0 only in loopback).  Without re-rank (m = k) slot 0 sorts those.
+// With re-rank, every shard re-ranks the candidates it owns into its rank's slot (0 elsewhere), all-gather #2, and slot 0
+// ORs the ranks' lists and sorts them.  The caller holds every local shard's reader lock.
+static cdb_status sparse_sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_sparse_search_params *p, uint32_t m,
+                                         const std::vector<SparseQueries> &dq, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                         cudaStream_t out_stream) {
+    const size_t nl = g->dev.size(), n_sel = g->loopback ? 1 : nl;
+    const uint32_t k = p->k, chunk = group_chunk(g, nq, (size_t)m * 8 + 4);
+    const size_t cap_words = (size_t)chunk * m + (chunk + 1) / 2;
+    cdb_status rc;
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->gather[i].ensure(g->world * cap_words * 8)) || (i < n_sel && (rc = g->sel[i].ensure((size_t)chunk * m * 8 + chunk * 4))))
+            return rc;
+    }
+    const cudaStream_t s0 = slot_stream(g, 0, out_stream);
+    for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        const size_t words = (size_t)c * m + (c + 1) / 2;
+        if (q0 && (rc = loopback_fence(g))) return rc;
+        for (size_t i = 0; i < nl; ++i) {
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+            uint64_t *slot = gather_buf(g, i) + (g->rank0 + i) * words;
+            if ((rc = sparse_shard_select(g->sparse[i], dq[i].off + q0, dq[i].dims, dq[i].vals, c, p, m, slot,
+                                          reinterpret_cast<uint32_t *>(slot + (size_t)c * m), slot_stream(g, i, out_stream))))
+                return rc;
+        }
+        if ((rc = group_allgather(g, words, out_stream))) return rc;
+        auto sel_keys = [&](size_t i) { return reinterpret_cast<uint64_t *>(g->sel[i].p); };
+        auto sel_cnt = [&](size_t i) { return reinterpret_cast<uint32_t *>(sel_keys(i) + (size_t)c * m); };
+        for (size_t i = 0; i < n_sel; ++i) {
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+            if ((rc = sparse_group_select(gather_buf(g, i), words, g->world, c, m, sel_keys(i), sel_cnt(i), slot_stream(g, i, out_stream))))
+                return rc;
+        }
+        if (p->rerank) {
+            // loopback: every shard re-ranks on slot 0's stream from slot 0's list straight into slot 0's gather buffer
+            for (size_t i = 0; i < nl; ++i) {
+                const size_t j = g->loopback ? 0 : i;
+                CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+                if ((rc = sparse_shard_rerank(g->sparse[i], dq[i].off + q0, dq[i].dims, dq[i].vals, c, m, sel_keys(j), sel_cnt(j),
+                                              gather_buf(g, j) + (g->rank0 + i) * words, slot_stream(g, j, out_stream))))
+                    return rc;
+            }
+            if (!g->loopback && (rc = group_allgather(g, words, out_stream))) return rc;
+        }
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        if ((rc = sparse_group_finalize(gather_buf(g, 0), words, g->world, c, m, k, p->rerank ? 1 : 0, sel_keys(0), sel_cnt(0),
+                                        d_ids + (size_t)q0 * k, d_scores + (size_t)q0 * k, d_counts + q0, s0)))
+            return rc;
+    }
+    return CDB_OK;
+}
+
+// every local slot needs a sparse shard (both forms refuse before any device work: parameters, arguments, slots)
+static cdb_status sparse_sharded_slots(const cdb_shard_group *g) {
+    for (size_t i = 0; i < g->dev.size(); ++i) CDB_REQUIRE(g->sparse[i], "a group slot has no sparse shard attached");
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
+                                           uint32_t nq, const cdb_sparse_search_params *p, uint32_t *out_ids, float *out_scores,
+                                           uint32_t *out_counts) {
+    uint32_t m = 0;
+    cdb_status rc = sparse_check_params(p, &m);
+    if (rc) return rc;
+    CDB_REQUIRE(g && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    if ((rc = sparse_sharded_slots(g))) return rc;
+    if (!nq) return CDB_OK;
+    if ((rc = check_csr(q_offsets, nq, "q_offsets"))) return rc;
+    const uint64_t nqp = q_offsets[nq];
+    CDB_REQUIRE((q_dims && q_values) || !nqp, "null query pairs");
+    std::lock_guard<std::mutex> lock(g->mu);
+    const size_t nl = g->dev.size();
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    for (size_t i = 0; i < nl; ++i) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
+    std::vector<SparseQueries> dq(nl);
+    for (size_t i = 0; i < nl; ++i) {   // the same host batch goes to every local device
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqp * 8))) return rc;
+        uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
+        uint32_t *dims = reinterpret_cast<uint32_t *>(off + nq + 1);
+        float *vals = reinterpret_cast<float *>(dims + nqp);
+        CDB_CUDA_TRY(cudaMemcpyAsync(off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
+        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(dims, q_dims, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(vals, q_values, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        dq[i] = {off, dims, vals};
+    }
+    if (g->loopback) {   // slot 0's stream reads every slot's queries in phase 2
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        for (size_t i = 1; i < nl; ++i) {
+            CDB_CUDA_TRY(cudaEventRecord(g->ev[i], g->stream[i]));
+            CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[0], g->ev[i], 0));
+        }
+    }
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    const size_t nk = (size_t)nq * p->k;
+    if ((rc = g->ids[0].ensure(nk * 4)) || (rc = g->scores[0].ensure(nk * 4)) || (rc = g->counts[0].ensure((size_t)nq * 4))) return rc;
+    uint32_t *f_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
+    float *f_scores = reinterpret_cast<float *>(g->scores[0].p);
+    uint32_t *f_counts = reinterpret_cast<uint32_t *>(g->counts[0].p);
+    rc = sparse_sharded_enqueue(g, nq, p, m, dq, f_ids, f_scores, f_counts, nullptr);
+    if (!rc) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+    }
+    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collectives included) before the locks and host buffers go
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
+    }
+    return rc;
+}
+
+cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *g, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
+                                                  const float *d_q_values, uint32_t nq, const cdb_sparse_search_params *p, uint32_t *d_ids,
+                                                  float *d_scores, uint32_t *d_counts, void *stream) {
+    uint32_t m = 0;
+    cdb_status rc = sparse_check_params(p, &m);
+    if (rc) return rc;
+    CDB_REQUIRE(g && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
+    CDB_REQUIRE(g->dev.size() == 1, "the device form serves one-process-per-GPU groups (cdb_shard_group_create_rank)");
+    if ((rc = sparse_sharded_slots(g))) return rc;
+    if (!nq) return CDB_OK;
+    std::lock_guard<std::mutex> lock(g->mu);
+    std::shared_lock<std::shared_mutex> shard_lock(sparse_index_mutex(g->sparse[0]));
+    std::vector<SparseQueries> dq(1, SparseQueries{d_q_offsets, d_q_dims, d_q_values});
+    return sparse_sharded_enqueue(g, nq, p, m, dq, d_ids, d_scores, d_counts, (cudaStream_t)stream);
+}
+
+// Host form only.  The group's N and df of every query term: summed over the local shards' tables, then (per-rank
+// groups) over the ranks by one all-gather of [N, df...] per rank.  idf = tf_idf(N, df) on the host, one per query term;
+// each shard scores its tiles with it and writes all 512 bucket winners per query into its rank's slot; one all-gather;
+// slot 0 takes the best of the ranks per bucket and sorts.  The local shards' reader locks are held from the df look-up
+// until the scoring has run.
+cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
+                                          uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
+    CDB_REQUIRE(g && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    const size_t nl = g->dev.size();
+    for (size_t i = 0; i < nl; ++i) CDB_REQUIRE(g->tfidf[i], "a group slot has no tf-idf shard attached");
+    if (!nq) return CDB_OK;
+    cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
+    if (rc) return rc;
+    const uint64_t nqh = q_offsets[nq];
+    CDB_REQUIRE(q_hashes || !nqh, "null query hashes");
+    CDB_REQUIRE(nqh < (1ull << 31), "a batch of 2^31 query terms or more");
+    std::lock_guard<std::mutex> lock(g->mu);
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    for (size_t i = 0; i < nl; ++i) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
+    // [N, df of every query term], summed over the local shards (u32, wrapping), then over the ranks
+    std::vector<uint32_t> stats(1 + nqh, 0);
+    for (size_t i = 0; i < nl; ++i) stats[0] += tfidf_add_df(g->tfidf[i], q_hashes, nqh, stats.data() + 1);
+    if (nl < g->world) {
+        const size_t words = (stats.size() + 1) / 2;
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        if ((rc = g->gather[0].ensure(g->world * words * 8))) return rc;
+        std::vector<uint32_t> all(g->world * words * 2);
+        CDB_CUDA_TRY(cudaMemcpyAsync(gather_buf(g, 0) + (size_t)g->rank0 * words, stats.data(), stats.size() * 4, cudaMemcpyHostToDevice,
+                                     g->stream[0]));
+        if ((rc = group_allgather(g, words, nullptr))) return rc;
+        CDB_CUDA_TRY(cudaMemcpyAsync(all.data(), gather_buf(g, 0), all.size() * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[0]));
+        std::fill(stats.begin(), stats.end(), 0u);
+        for (uint32_t r = 0; r < g->world; ++r)
+            for (size_t j = 0; j < stats.size(); ++j) stats[j] += all[r * words * 2 + j];
+    }
+    std::vector<float> idf(nqh);
+    for (uint64_t j = 0; j < nqh; ++j) idf[j] = tfidf_idf(stats[0], stats[1 + j]);
+    for (size_t i = 0; i < nl; ++i) {   // queries and their idf to every local device
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqh * 8))) return rc;
+        uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
+        uint32_t *hashes = reinterpret_cast<uint32_t *>(off + nq + 1);
+        float *d_idf = reinterpret_cast<float *>(hashes + nqh);
+        CDB_CUDA_TRY(cudaMemcpyAsync(off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
+        if (nqh) CDB_CUDA_TRY(cudaMemcpyAsync(hashes, q_hashes, nqh * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        if (nqh) CDB_CUDA_TRY(cudaMemcpyAsync(d_idf, idf.data(), nqh * 4, cudaMemcpyHostToDevice, g->stream[i]));
+    }
+    const uint32_t kout = tfidf_out_cols(k), chunk = group_chunk(g, nq, 512 * 8);
+    const size_t nk = (size_t)nq * kout;
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->gather[i].ensure(g->world * (size_t)chunk * 512 * 8))) return rc;
+    }
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    if ((rc = g->ids[0].ensure(nk * 4)) || (rc = g->scores[0].ensure(nk * 4)) || (rc = g->counts[0].ensure((size_t)nq * 4))) return rc;
+    uint32_t *f_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
+    float *f_scores = reinterpret_cast<float *>(g->scores[0].p);
+    uint32_t *f_counts = reinterpret_cast<uint32_t *>(g->counts[0].p);
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        const size_t words = (size_t)c * 512;
+        if (q0 && (rc = loopback_fence(g))) break;
+        for (size_t i = 0; i < nl && !rc; ++i) {
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+            uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
+            uint32_t *hashes = reinterpret_cast<uint32_t *>(off + nq + 1);
+            rc = tfidf_shard_winners(g->tfidf[i], off + q0, hashes, reinterpret_cast<const float *>(hashes + nqh), c,
+                                     reinterpret_cast<uint2 *>(gather_buf(g, i) + (g->rank0 + i) * words), g->stream[i]);
+        }
+        if (!rc) rc = group_allgather(g, words, nullptr);
+        if (!rc) {
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+            rc = tfidf_group_finalize(gather_buf(g, 0), words, g->world, c, k, f_ids + (size_t)q0 * kout, f_scores + (size_t)q0 * kout,
+                                      f_counts + q0, g->stream[0]);
+        }
+    }
+    if (!rc) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, g->stream[0]));
+    }
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
+    }
+    return rc;
 }
 
 }  // extern "C"

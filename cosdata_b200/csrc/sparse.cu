@@ -212,10 +212,21 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_score_tile_kernel(SpSearch a
     if (tid == 0) a.out_cnt[(size_t)qi * a.n_tiles + t] = s_cnt;
 }
 
-// lists [q][n_in][m] -> [q][ceil(n_in / g)][m]: the top m of every group of g lists
-__global__ void __launch_bounds__(SP_THREADS, 1) sp_merge_kernel(const uint64_t *__restrict__ in_keys, const uint32_t *__restrict__ in_cnt,
-                                                                  uint32_t n_in, uint32_t g, uint32_t m, uint64_t *__restrict__ out_keys,
-                                                                  uint32_t *__restrict__ out_cnt) {
+// where the input lists of a merge live: list l of query qi is keys[qi * kq + l * kl ..] with cnt[qi * cq + l * cl] keys.
+// The tree's own levels are [q][n_in][m] (kq = n_in * m, kl = m, cq = n_in, cl = 1); a shard group's gather buffer is
+// rank-major, one list per rank (lists_rank_major).
+struct SpLists {
+    const uint64_t *keys;
+    const uint32_t *cnt;
+    size_t kq, kl, cq, cl;
+};
+inline SpLists lists_of_level(const uint64_t *keys, const uint32_t *cnt, uint32_t n_in, uint32_t m) {
+    return {keys, cnt, (size_t)n_in * m, m, n_in, 1};
+}
+
+// lists -> [q][ceil(n_in / g)][m]: the top m of every group of g lists
+__global__ void __launch_bounds__(SP_THREADS, 1) sp_merge_kernel(SpLists in, uint32_t n_in, uint32_t g, uint32_t m,
+                                                                  uint64_t *__restrict__ out_keys, uint32_t *__restrict__ out_cnt) {
     extern __shared__ __align__(16) uint8_t smem[];
     uint64_t *keys = reinterpret_cast<uint64_t *>(smem);
     __shared__ uint32_t hist[260], s_off[SP_MERGE_MAX_LISTS + 1], s_cnt;
@@ -223,13 +234,13 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_merge_kernel(const uint64_t 
     const uint32_t l0 = grp * g, nl = min(g, n_in - l0);
     if (tid == 0) {
         uint32_t o = 0;
-        for (uint32_t l = 0; l < nl; ++l) { s_off[l] = o; o += in_cnt[(size_t)qi * n_in + l0 + l]; }
+        for (uint32_t l = 0; l < nl; ++l) { s_off[l] = o; o += in.cnt[qi * in.cq + (l0 + l) * in.cl]; }
         s_off[nl] = o;
         s_cnt = 0;
     }
     __syncthreads();
     for (uint32_t l = 0; l < nl; ++l) {
-        const uint64_t *src = in_keys + ((size_t)qi * n_in + l0 + l) * m;
+        const uint64_t *src = in.keys + qi * in.kq + (l0 + l) * in.kl;
         for (uint32_t i = tid; i < s_off[l + 1] - s_off[l]; i += SP_THREADS) keys[s_off[l] + i] = src[i];
     }
     __syncthreads();
@@ -294,6 +305,7 @@ __device__ __forceinline__ float sp_key_score(uint64_t key, int rerank) {
 // one list of <= m candidates per query -> the best k, best first.  rerank: finalize_sparse_ann_results -- for every
 // candidate dp = 0f32, dp += doc_val * q_val over the query pairs in the caller's order (a row's last pair of a dim wins),
 // then total_cmp order (NaN canonicalised), ties to the smaller id.  Otherwise the score is the u32 similarity as f32.
+// rerank = 2: the keys are already re-ranked (a shard group's combined list); sort and decode only.
 __global__ void __launch_bounds__(SP_THREADS, 1) sp_finalize_kernel(const uint64_t *__restrict__ in_keys, const uint32_t *__restrict__ in_cnt,
                                                                      uint32_t m, uint32_t k, int rerank, uint32_t q0,
                                                                      const uint64_t *__restrict__ q_off, const uint32_t *__restrict__ q_dims,
@@ -310,7 +322,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sp_finalize_kernel(const uint64
     while (P < n) P <<= 1;
     for (uint32_t i = tid; i < P; i += SP_THREADS) keys[i] = i < n ? src[i] : 0ull;
     __syncthreads();
-    if (rerank) {
+    if (rerank == 1) {
         const uint64_t qb = q_off[q], qe = q_off[q + 1];
         for (uint32_t c = warp; c < n; c += SP_THREADS / 32) {
             const uint32_t id = ~(uint32_t)keys[c];
@@ -368,6 +380,37 @@ __global__ void __launch_bounds__(256) sp_rerank_all_kernel(uint64_t *__restrict
         const uint32_t id = ~(uint32_t)keys[c], q = q0 + qis[c];
         const float dp = sp_rerank_dot(q_off[q], q_off[q + 1], q_dims, q_vals, row_off[id - id_base], row_off[id - id_base + 1], dims, vals);
         if (lane == 0) keys[c] = sp_rerank_key(dp, id);
+    }
+}
+
+// a shard group's phase 2: keys [nq][m] are the group's top m candidates per query (cnt[q] of them).  One warp per
+// position: a candidate this shard owns (id_base <= id < id_base + n_rows) gets its re-ranked key from the same dot product
+// as sp_finalize_kernel, every other position 0, so OR-ing the ranks' lists gives each candidate its key exactly once.
+__global__ void __launch_bounds__(256) sp_rerank_owned_kernel(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ cnt, uint32_t nq,
+                                                              uint32_t m, const uint64_t *__restrict__ q_off, const uint32_t *__restrict__ q_dims,
+                                                              const float *__restrict__ q_vals, const uint64_t *__restrict__ row_off,
+                                                              const uint32_t *__restrict__ dims, const float *__restrict__ vals, uint32_t id_base,
+                                                              uint64_t n_rows, uint64_t *__restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5, n = (uint64_t)nq * m;
+    for (uint64_t c = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < n; c += warps) {
+        const uint32_t q = (uint32_t)(c / m), j = (uint32_t)(c - (uint64_t)q * m);
+        uint64_t key = 0;
+        if (j < cnt[q]) {
+            const uint32_t id = ~(uint32_t)keys[c], r = id - id_base;
+            if (r < n_rows) key = sp_rerank_key(sp_rerank_dot(q_off[q], q_off[q + 1], q_dims, q_vals, row_off[r], row_off[r + 1], dims, vals), id);
+        }
+        if (lane == 0) out[c] = key;
+    }
+}
+
+// out[i] = OR over the ranks of gathered[r * words + i]: the re-ranked lists of a shard group, one non-zero rank per position
+__global__ void __launch_bounds__(256) sp_or_ranks_kernel(const uint64_t *__restrict__ gathered, size_t words, uint32_t world, uint64_t n,
+                                                          uint64_t *__restrict__ out) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint64_t v = 0;
+        for (uint32_t r = 0; r < world; ++r) v |= gathered[r * words + i];
+        out[i] = v;
     }
 }
 
@@ -494,7 +537,8 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
         while (n_lists > 1) {
             const uint32_t n_out = (n_lists + g - 1) / g;
             const uint32_t held = std::min<uint32_t>(g, n_lists) * m;
-            sp_merge_kernel<<<dim3(n_out, c), SP_THREADS, (size_t)held * 8, s>>>(cur, ccur, n_lists, g, m, nxt, cnxt);
+            sp_merge_kernel<<<dim3(n_out, c), SP_THREADS, (size_t)held * 8, s>>>(lists_of_level(cur, ccur, n_lists, m), n_lists, g, m,
+                                                                                  nxt, cnxt);
             g_launch_count.fetch_add(1, std::memory_order_relaxed);
             if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
             std::swap(cur, nxt);
@@ -510,6 +554,38 @@ cdb_status search_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uin
     }
     for (void *ptr : {(void *)ka, (void *)kb, (void *)ca, (void *)cb})
         if (ptr) cudaFreeAsync(ptr, s);
+    return rc;
+}
+
+// The top m keys of n_lists lists per query, for c queries, into dest_keys [c][m] / dest_cnt [c], unsorted: the merge tree
+// of search_locked, whose last level writes the destination.  At least one level runs, so a single list is copied.
+cdb_status merge_lists(SpLists in, uint32_t n_lists, uint32_t c, uint32_t m, uint64_t *dest_keys, uint32_t *dest_cnt, cudaStream_t s) {
+    const uint32_t g = std::min<uint32_t>(SP_MERGE_MAX_LISTS, std::max<uint32_t>(2, SP_MERGE_KEYS / m));
+    const uint32_t n1 = (n_lists + g - 1) / g;
+    uint64_t *bk[2] = {nullptr, nullptr};
+    uint32_t *bc[2] = {nullptr, nullptr};
+    cdb_status rc = CDB_OK;
+    cudaError_t e = allow_max_dynamic_smem((const void *)sp_merge_kernel);
+    for (int i = 0; i < 2 && n1 > 1 && e == cudaSuccess; ++i) {
+        e = cudaMallocAsync(&bk[i], (size_t)c * n1 * m * 8, s);
+        if (e == cudaSuccess) e = cudaMallocAsync(&bc[i], (size_t)c * n1 * 4, s);
+    }
+    if (e != cudaSuccess) { set_error(std::string("sparse merge: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    for (uint32_t n = n_lists, w = 0; !rc; w ^= 1) {
+        const uint32_t n_out = (n + g - 1) / g;
+        uint64_t *ok = n_out == 1 ? dest_keys : bk[w];
+        uint32_t *oc = n_out == 1 ? dest_cnt : bc[w];
+        sp_merge_kernel<<<dim3(n_out, c), SP_THREADS, (size_t)std::min(g, n) * m * 8, s>>>(in, n, g, m, ok, oc);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+        in = lists_of_level(ok, oc, n_out, m);
+        n = n_out;
+        if (n == 1) break;
+    }
+    for (int i = 0; i < 2; ++i) {
+        if (bk[i]) cudaFreeAsync(bk[i], s);
+        if (bc[i]) cudaFreeAsync(bc[i], s);
+    }
     return rc;
 }
 
@@ -645,6 +721,82 @@ cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows) {
 }
 
 int sparse_index_device(const cdb_sparse_index *ix) { return ix->desc.device; }
+
+// ---------------------------------------------------------------- a shard group's sparse search (shard_group.cu)
+// Every function below runs on the caller's current device and stream; the ones taking an index expect its reader lock held.
+std::shared_mutex &sparse_index_mutex(cdb_sparse_index *ix) { return ix->rw; }
+uint32_t sparse_index_bits(const cdb_sparse_index *ix) { return ix->desc.quantization_bits; }
+float sparse_index_upper_bound(const cdb_sparse_index *ix) { return ix->desc.values_upper_bound; }
+uint32_t sparse_index_id_base(const cdb_sparse_index *ix) { return ix->desc.id_base; }
+uint64_t sparse_index_capacity(const cdb_sparse_index *ix) { return ix->desc.capacity_rows; }
+cdb_status sparse_check_params(const cdb_sparse_search_params *p, uint32_t *m) { return check_search_params(p, m); }
+
+// phase 1 on one shard: its top m candidates per query (the list sp_finalize_kernel would take), unsorted, into
+// keys [nq][m] / cnt [nq]
+cdb_status sparse_shard_select(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
+                               const cdb_sparse_search_params *p, uint32_t m, uint64_t *keys, uint32_t *cnt, cudaStream_t s) {
+    const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
+    if (!nq) return CDB_OK;
+    if (!n_tiles) { CDB_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)nq * 4, s)); return CDB_OK; }
+    const size_t per_q = (size_t)n_tiles * m * 12;
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, (512ull << 20) / per_q}));
+    uint64_t *ka = nullptr;
+    uint32_t *ca = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&ka, (size_t)chunk * n_tiles * m * 8, s));
+    cudaError_t e = cudaMallocAsync(&ca, (size_t)chunk * n_tiles * 4, s);
+    if (e == cudaSuccess) e = allow_max_dynamic_smem((const void *)sp_score_tile_kernel);
+    cdb_status rc = CDB_OK;
+    if (e != cudaSuccess) { set_error(std::string("sparse shard search: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qdims, d_qvals, p, q0, m, ka, ca));
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
+        rc = merge_lists(lists_of_level(ka, ca, n_tiles, m), n_tiles, c, m, keys + (size_t)q0 * m, cnt + q0, s);
+    }
+    if (ka) cudaFreeAsync(ka, s);
+    if (ca) cudaFreeAsync(ca, s);
+    return rc;
+}
+
+// the group's top m per query from the all-gathered phase-1 lists: rank r's slot is gathered[r * words ..], keys [nq][m]
+// then the u32 counts [nq]
+cdb_status sparse_group_select(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t m, uint64_t *keys,
+                               uint32_t *cnt, cudaStream_t s) {
+    const SpLists in{gathered, reinterpret_cast<const uint32_t *>(gathered + (size_t)nq * m), m, words, 1, 2 * words};
+    return merge_lists(in, world, nq, m, keys, cnt, s);
+}
+
+// phase 2 on one shard: out [nq][m] = the re-ranked key of every candidate of keys / cnt this shard owns, 0 elsewhere
+cdb_status sparse_shard_rerank(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
+                               uint32_t m, const uint64_t *keys, const uint32_t *cnt, uint64_t *out, cudaStream_t s) {
+    const uint64_t n = (uint64_t)nq * m;
+    if (!n) return CDB_OK;
+    const uint32_t blocks = (uint32_t)std::min<uint64_t>((n + 7) / 8, 1u << 20);
+    sp_rerank_owned_kernel<<<blocks, 256, 0, s>>>(keys, cnt, nq, m, d_qoff, d_qdims, d_qvals, ix->st.d_row_off, ix->st.d_keys, ix->st.d_vals,
+                                                  ix->desc.id_base, ix->st.n_rows, out);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
+// the group's results: rerank = 0 sorts the top-k keys / cnt and scores them by similarity; rerank = 1 first ORs the
+// ranks' phase-2 lists (gathered, rank r at r * words) into keys, then sorts the re-ranked keys.  Best k per query.
+cdb_status sparse_group_finalize(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t m, uint32_t k, int rerank,
+                                 uint64_t *keys, const uint32_t *cnt, uint32_t *ids, float *scores, uint32_t *counts, cudaStream_t s) {
+    if (!nq) return CDB_OK;
+    if (rerank) {
+        const uint64_t n = (uint64_t)nq * m;
+        sp_or_ranks_kernel<<<(uint32_t)std::min<uint64_t>((n + 255) / 256, 1u << 16), 256, 0, s>>>(gathered, words, world, n, keys);
+        CDB_LAUNCH_CHECK();
+    }
+    uint32_t sort_cap = 1;
+    while (sort_cap < m) sort_cap <<= 1;
+    CDB_CUDA_TRY(allow_max_dynamic_smem((const void *)sp_finalize_kernel));
+    sp_finalize_kernel<<<nq, SP_THREADS, (size_t)sort_cap * 8, s>>>(keys, cnt, m, k, rerank ? 2 : 0, 0, nullptr, nullptr, nullptr, nullptr,
+                                                                     nullptr, nullptr, 0, ids, scores, counts);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
 }  // namespace cdb
 
 extern "C" {

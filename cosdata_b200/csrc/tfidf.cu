@@ -58,6 +58,7 @@ struct TfSearch {
     const PostingTile *tiles;
     const uint32_t *terms;   // every hash the index has seen, ascending
     const float *idf;        // idf of terms[i]
+    const float *q_idf;      // NULL, or the idf of every query term (a shard group's global idf), used for terms this index holds
     uint32_t n_terms;
     uint64_t n_rows;
     uint32_t id_base;
@@ -99,7 +100,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_score_tile_kernel(TfSearch a
             uint32_t s = 0, e = 0;
             float idf = 0.0f;
             if (g < a.n_terms && a.terms[g] == h) {
-                idf = a.idf[g];
+                idf = a.q_idf ? a.q_idf[j0 + tid] : a.idf[g];
                 const uint32_t l = lower_bound_u32(thash, tile.n_keys, h);
                 if (l < tile.n_keys && thash[l] == h) { s = tseg[l]; e = tseg[l + 1]; }
             }
@@ -140,23 +141,33 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_score_tile_kernel(TfSearch a
     a.out[((size_t)qi * a.n_tiles + t) * TF_BUCKETS + tid] = make_uint2(bid, __float_as_uint(best));
 }
 
-// per query: the tiles' winners of each bucket merged in ascending tile order (ascending ids, so `>` keeps the reference's
-// winner), then the <= 512 winners sorted by total_cmp descending, ties to the smaller id, truncated to kout
-__global__ void __launch_bounds__(TF_THREADS, 1) tf_finalize_kernel(const uint2 *__restrict__ in, uint32_t n_tiles, uint32_t kout,
-                                                                     uint32_t *__restrict__ out_ids, float *__restrict__ out_scores,
-                                                                     uint32_t *__restrict__ out_counts) {
-    __shared__ uint64_t keys[TF_BUCKETS];
-    __shared__ uint32_t s_cnt;
-    const uint32_t qi = blockIdx.x, tid = threadIdx.x;
-    if (tid == 0) s_cnt = 0;
-    const uint2 *src = in + (size_t)qi * n_tiles * TF_BUCKETS + tid;
+// bucket threadIdx.x's winner over the tiles of one query (src = its [n_tiles][512] winners), merged in ascending tile
+// order: ascending ids, so `>` keeps the reference's winner.  (CDB_INVALID_ID, -inf) when the bucket is empty.
+__device__ __forceinline__ uint2 tf_bucket_winner(const uint2 *__restrict__ src, uint32_t n_tiles) {
     float best = -INFINITY;
     uint32_t bid = CDB_INVALID_ID;
     for (uint32_t t = 0; t < n_tiles; ++t) {
-        const uint2 w = src[(size_t)t * TF_BUCKETS];
+        const uint2 w = src[(size_t)t * TF_BUCKETS + threadIdx.x];
         const float s = __uint_as_float(w.y);
         if (w.x != CDB_INVALID_ID && s > best) { best = s; bid = w.x; }
     }
+    return make_uint2(bid, __float_as_uint(best));
+}
+
+// one shard's half of a shard group's search: every bucket's winner per query, [nq][512], neither sorted nor truncated
+__global__ void __launch_bounds__(TF_THREADS, 1) tf_winners_kernel(const uint2 *__restrict__ in, uint32_t n_tiles, uint2 *__restrict__ out) {
+    out[(size_t)blockIdx.x * TF_BUCKETS + threadIdx.x] = tf_bucket_winner(in + (size_t)blockIdx.x * n_tiles * TF_BUCKETS, n_tiles);
+}
+
+// the <= 512 bucket winners of one query (thread = bucket) sorted by total_cmp descending, ties to the smaller id, truncated
+// to kout and written out
+__device__ __forceinline__ void tf_sort_winners(uint2 win, uint32_t kout, uint32_t *__restrict__ out_ids, float *__restrict__ out_scores,
+                                                uint32_t *__restrict__ out_count) {
+    __shared__ uint64_t keys[TF_BUCKETS];
+    __shared__ uint32_t s_cnt;
+    const uint32_t tid = threadIdx.x, bid = win.x;
+    const float best = __uint_as_float(win.y);
+    if (tid == 0) s_cnt = 0;
     __syncthreads();
     // order_key of a non-NaN score is non-zero above -inf's; 0 marks an empty bucket
     keys[tid] = bid == CDB_INVALID_ID ? 0ull
@@ -173,10 +184,36 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_finalize_kernel(const uint2 
             id = ~(uint32_t)key;
             s = __uint_as_float(key_to_bits(CDB_METRIC_DOT_PRODUCT, (uint32_t)(key >> 32)));
         }
-        out_ids[(size_t)qi * kout + tid] = id;
-        out_scores[(size_t)qi * kout + tid] = s;
+        out_ids[tid] = id;
+        out_scores[tid] = s;
     }
-    if (tid == 0) out_counts[qi] = cnt;
+    if (tid == 0) *out_count = cnt;
+}
+
+// per query: the tiles' winners of each bucket, then sorted and truncated to kout
+__global__ void __launch_bounds__(TF_THREADS, 1) tf_finalize_kernel(const uint2 *__restrict__ in, uint32_t n_tiles, uint32_t kout,
+                                                                     uint32_t *__restrict__ out_ids, float *__restrict__ out_scores,
+                                                                     uint32_t *__restrict__ out_counts) {
+    const uint32_t qi = blockIdx.x;
+    tf_sort_winners(tf_bucket_winner(in + (size_t)qi * n_tiles * TF_BUCKETS, n_tiles), kout, out_ids + (size_t)qi * kout,
+                    out_scores + (size_t)qi * kout, out_counts + qi);
+}
+
+// a shard group's merge: per query and bucket the best of the ranks' winners (gathered, rank r's [nq][512] at r * words),
+// `score > best` with equal scores (+0 and -0 too) going to the smaller id, since rank order need not follow id order;
+// then sorted and truncated as tf_finalize_kernel does
+__global__ void __launch_bounds__(TF_THREADS, 1) tf_group_finalize_kernel(const uint2 *__restrict__ gathered, size_t words, uint32_t world,
+                                                                           uint32_t kout, uint32_t *__restrict__ out_ids,
+                                                                           float *__restrict__ out_scores, uint32_t *__restrict__ out_counts) {
+    const uint32_t qi = blockIdx.x;
+    float best = -INFINITY;
+    uint32_t bid = CDB_INVALID_ID;
+    for (uint32_t r = 0; r < world; ++r) {
+        const uint2 w = gathered[r * words + (size_t)qi * TF_BUCKETS + threadIdx.x];
+        const float s = __uint_as_float(w.y);
+        if (w.x != CDB_INVALID_ID && (s > best || (s == best && w.x < bid))) { best = s; bid = w.x; }
+    }
+    tf_sort_winners(make_uint2(bid, __float_as_uint(best)), kout, out_ids + (size_t)qi * kout, out_scores + (size_t)qi * kout, out_counts + qi);
 }
 
 }  // namespace
@@ -243,14 +280,30 @@ cdb_status upload_terms(cdb_tfidf_index *ix, const std::vector<uint32_t> &terms,
 
 uint32_t out_cols(uint32_t k) { return (k == 0 || k > TF_BUCKETS) ? TF_BUCKETS : k; }
 
+// the scoring kernel's arguments for queries [q0, q0 + chunk); q_idf as TfSearch::q_idf
+TfSearch score_args(const cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, const float *q_idf, uint32_t q0, uint2 *win) {
+    TfSearch a;
+    a.entries = ix->st.entries(); a.thash = ix->st.d_tkeys; a.tseg = ix->st.d_tseg; a.deleted = ix->st.deleted();
+    a.tiles = ix->st.d_tiles; a.terms = ix->d_terms; a.idf = ix->d_idf; a.q_idf = q_idf; a.n_terms = (uint32_t)ix->h_terms.size();
+    a.n_rows = ix->st.n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q0 = q0;
+    a.n_tiles = (uint32_t)ix->st.h_tiles.size(); a.out = win;
+    return a;
+}
+
+// queries per chunk and the tile winners' scratch of one chunk
+uint32_t score_chunk(uint32_t nq, uint32_t n_tiles, size_t *per_q) {
+    *per_q = (size_t)n_tiles * TF_BUCKETS * sizeof(uint2);
+    return (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, (512ull << 20) / *per_q}));
+}
+
 cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint32_t nq, uint32_t k,
                          uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t s) {
     if (!nq) return CDB_OK;
     const uint32_t kout = out_cols(k);
     const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
     if (n_tiles == 0) return fill_empty_results(nq, kout, d_ids, d_scores, d_counts, s);
-    const size_t per_q = (size_t)n_tiles * TF_BUCKETS * sizeof(uint2);
-    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, (512ull << 20) / per_q}));
+    size_t per_q = 0;
+    const uint32_t chunk = score_chunk(nq, n_tiles, &per_q);
     uint2 *win = nullptr;
     CDB_CUDA_TRY(cudaMallocAsync(&win, (size_t)chunk * per_q, s));
     cdb_status rc = CDB_OK;
@@ -258,12 +311,7 @@ cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint
     if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
-        TfSearch a;
-        a.entries = ix->st.entries(); a.thash = ix->st.d_tkeys; a.tseg = ix->st.d_tseg; a.deleted = ix->st.deleted();
-        a.tiles = ix->st.d_tiles; a.terms = ix->d_terms; a.idf = ix->d_idf; a.n_terms = (uint32_t)ix->h_terms.size();
-        a.n_rows = ix->st.n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q0 = q0; a.n_tiles = n_tiles;
-        a.out = win;
-        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(a);
+        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qhash, nullptr, q0, win));
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
         tf_finalize_kernel<<<c, TF_THREADS, 0, s>>>(win, n_tiles, kout, d_ids + (size_t)q0 * kout, d_scores + (size_t)q0 * kout,
@@ -279,6 +327,61 @@ cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint
 
 namespace cdb {
 int tfidf_index_device(const cdb_tfidf_index *ix) { return ix->desc.device; }
+
+// ---------------------------------------------------------------- a shard group's TF-IDF search (shard_group.cu)
+// Every function below runs on the caller's current device and stream; the ones taking an index expect its reader lock held.
+std::shared_mutex &tfidf_index_mutex(cdb_tfidf_index *ix) { return ix->rw; }
+uint32_t tfidf_index_id_base(const cdb_tfidf_index *ix) { return ix->desc.id_base; }
+uint64_t tfidf_index_capacity(const cdb_tfidf_index *ix) { return ix->desc.capacity_rows; }
+uint32_t tfidf_out_cols(uint32_t k) { return out_cols(k); }
+float tfidf_idf(uint32_t n_docs, uint32_t df) { return tf_idf(n_docs, df); }
+
+// df[i] += this index's df of hashes[i] (u32, wrapping; 0 for a hash it never saw); returns its N
+uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *df) {
+    for (uint64_t i = 0; i < n; ++i) {
+        const size_t g = std::lower_bound(ix->h_terms.begin(), ix->h_terms.end(), hashes[i]) - ix->h_terms.begin();
+        if (g < ix->h_terms.size() && ix->h_terms[g] == hashes[i]) df[i] += ix->h_df[g];
+    }
+    return ix->documents;
+}
+
+// one shard's half: every bucket winner of every query under the group's idf (d_qidf, one per query term) into out [nq][512]
+cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, const float *d_qidf, uint32_t nq,
+                               uint2 *out, cudaStream_t s) {
+    if (!nq) return CDB_OK;
+    const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
+    if (n_tiles == 0) {   // every bucket empty: id CDB_INVALID_ID
+        CDB_CUDA_TRY(cudaMemsetAsync(out, 0xFF, (size_t)nq * TF_BUCKETS * sizeof(uint2), s));
+        return CDB_OK;
+    }
+    size_t per_q = 0;
+    const uint32_t chunk = score_chunk(nq, n_tiles, &per_q);
+    uint2 *win = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&win, (size_t)chunk * per_q, s));
+    cdb_status rc = CDB_OK;
+    cudaError_t e = allow_max_dynamic_smem((const void *)tf_score_tile_kernel);
+    if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qhash, d_qidf, q0, win));
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
+        tf_winners_kernel<<<c, TF_THREADS, 0, s>>>(win, n_tiles, out + (size_t)q0 * TF_BUCKETS);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    cudaFreeAsync(win, s);
+    return rc;
+}
+
+// the group's results from the all-gathered winners (rank r's [nq][512] at gathered + r * words)
+cdb_status tfidf_group_finalize(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t k, uint32_t *ids, float *scores,
+                                uint32_t *counts, cudaStream_t s) {
+    if (!nq) return CDB_OK;
+    tf_group_finalize_kernel<<<nq, TF_THREADS, 0, s>>>(reinterpret_cast<const uint2 *>(gathered), words, world, out_cols(k), ids, scores, counts);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
 }  // namespace cdb
 
 extern "C" {

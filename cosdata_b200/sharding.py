@@ -71,6 +71,70 @@ def gather_and_merge(local_ids, local_scores, world, all_gather_fn, k=None, metr
     return merge_packed(all_gather_fn(keys), k, metric)[:2]
 
 
+# ----------------------------------------------------------------------------- sparse and TF-IDF shards (host mirrors)
+def sparse_keys(ids, sims):
+    """[.., m] global ids (INVALID_ID = empty) + u32 similarities -> u64 selection keys sim << 32 | ~id (0 = empty)"""
+    ids = np.asarray(ids, dtype=np.uint32)
+    keys = (np.asarray(sims, dtype=np.uint64) << np.uint64(32)) | (~ids).astype(np.uint64)
+    return np.where(ids == INVALID_ID, np.uint64(0), keys).astype(np.uint64)
+
+
+def _key_ids(keys):
+    return (~(keys & np.uint64(0xFFFFFFFF)).astype(np.uint32)).astype(np.uint32)
+
+
+def merge_sparse(gathered, k, rerank_fn=None):
+    """cdb_sparse_search_batch_sharded's merge.  gathered: [world, B, m] u64 keys, every rank's top m (all-gather #1).
+    The group's top m per query are the best m of the world * m keys.  Without rerank_fn (m = k) they are the results,
+    scored by similarity as f32.  With rerank_fn(q, ids) -> f32 dot products of those global ids for query q (each rank
+    re-ranks the ids it owns; here one function stands for all of them), the m candidates are rekeyed by the total_cmp
+    order of the dp (NaN canonicalised) then the smaller id, and the best k kept.
+    -> (ids u32[B, k], scores f32[B, k], counts u32[B])"""
+    world, b, m = gathered.shape
+    allk = np.transpose(gathered, (1, 0, 2)).reshape(b, world * m)
+    top = np.take_along_axis(allk, np.argsort(allk, axis=1)[:, ::-1][:, :m], axis=1)
+    ids = np.full((b, k), INVALID_ID, np.uint32)
+    scores = np.zeros((b, k), np.float32)
+    counts = np.zeros(b, np.uint32)
+    for q in range(b):
+        cand = top[q][top[q] != 0]
+        if rerank_fn is None:
+            best = cand[:k]
+            ids[q, :len(best)] = _key_ids(best)
+            scores[q, :len(best)] = (best >> np.uint64(32)).astype(np.float64).astype(np.float32)
+        else:
+            cid = _key_ids(cand)
+            dp = np.asarray(rerank_fn(q, cid), dtype=np.float32).reshape(-1)
+            dbits = np.where(np.isnan(dp), np.uint32(0xFFC00000), dp.view(np.uint32)).astype(np.uint32)
+            rk = (order_key_np(0, dbits).astype(np.uint64) << np.uint64(32)) | (~cid).astype(np.uint64)
+            best = np.sort(rk)[::-1][:k]
+            ids[q, :len(best)], scores[q, :len(best)] = unpack_keys(best)
+        counts[q] = len(best)
+    return ids, scores, counts
+
+
+def merge_buckets(g_ids, g_scores, k=0):
+    """cdb_tfidf_search_batch_sharded's merge.  g_ids / g_scores: [world, B, 512] every rank's bucket winners
+    (INVALID_ID = empty bucket; all-gathered).  Per bucket the best of the ranks by `score > best`, equal scores (+0 and -0
+    too) going to the smaller id; the winners sorted by total_cmp descending, ties to the smaller id, truncated to
+    kout = 512 for k = 0 or k > 512, else k.  -> (ids u32[B, kout], scores f32[B, kout], counts u32[B])"""
+    g_ids = np.asarray(g_ids, dtype=np.uint32)
+    g_scores = np.asarray(g_scores, dtype=np.float32)
+    world, b, nb = g_ids.shape
+    kout = nb if k == 0 or k > nb else k
+    best = np.full((b, nb), -np.inf, np.float32)
+    bid = np.full((b, nb), INVALID_ID, np.uint32)
+    for r in range(world):
+        i, s = g_ids[r], g_scores[r]
+        take = (i != INVALID_ID) & ((s > best) | ((s == best) & (i < bid)))
+        best = np.where(take, s, best)
+        bid = np.where(take, i, bid)
+    keys = pack_keys(bid, best)
+    top = np.take_along_axis(keys, np.argsort(keys, axis=1)[:, ::-1][:, :kout], axis=1)
+    ids, scores = unpack_keys(top)
+    return ids, scores, (top != 0).sum(axis=1).astype(np.uint32)
+
+
 # ----------------------------------------------------------------------------- C ABI wrapper
 class ShardGroup:
     """cdb_shard_group: the NCCL communicator + gather buffers owned by the library."""
@@ -78,6 +142,7 @@ class ShardGroup:
     def __init__(self, handle, lib):
         self._h, self._lib = handle, lib
         self._shards = []
+        self._text_shards = []              # sparse and TF-IDF shards, kept alive as long as the group
 
     @staticmethod
     def unique_id():
@@ -140,11 +205,56 @@ class ShardGroup:
                                                          C.c_void_p(d_err) if d_err else None,
                                                          C.c_void_p(stream_ptr) if stream_ptr else None))
 
+    def attach_sparse(self, local_slot, index):
+        """a SparseIndex shard (id_base = its first global id) into local slot `local_slot`, next to any dense shard"""
+        from .api import _check
+        _check(self._lib.cdb_shard_group_attach_sparse(self._h, local_slot, index.h))
+        self._text_shards.append(index)
+
+    def attach_tfidf(self, local_slot, index):
+        """a TfIdfIndex shard (id_base = its first global id) into local slot `local_slot`"""
+        from .api import _check
+        _check(self._lib.cdb_shard_group_attach_tfidf(self._h, local_slot, index.h))
+        self._text_shards.append(index)
+
+    def search_sparse(self, queries, options):
+        """SparseIndex.batch_search over the whole group -> ids u32[B, k], scores f32[B, k], counts u32[B]"""
+        from .api import _as_csr, _check, _ptr
+        o, d, v = _as_csr(queries)
+        nq, k = len(o) - 1, int(options.top_k or 0)
+        ids = np.zeros((nq, max(k, 1)), np.uint32)
+        scores = np.zeros((nq, max(k, 1)), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        p = options.params()
+        _check(self._lib.cdb_sparse_search_batch_sharded(self._h, _ptr(o), _ptr(d), _ptr(v), nq, C.byref(p), _ptr(ids), _ptr(scores),
+                                                         _ptr(counts)))
+        return ids[:, :k], scores[:, :k], counts[:nq]
+
+    def search_sparse_device(self, d_offsets, d_dims, d_values, nq, options, d_ids, d_scores, d_counts, stream_ptr=None):
+        """per-rank groups: the sparse search on device pointers (ints), asynchronous on the stream"""
+        from .api import _check
+        p = options.params()
+        _check(self._lib.cdb_sparse_search_batch_sharded_device(self._h, d_offsets, d_dims, d_values, nq, C.byref(p), d_ids, d_scores,
+                                                                d_counts, C.c_void_p(stream_ptr) if stream_ptr else None))
+
+    def search_tfidf(self, queries, top_k=None):
+        """TfIdfIndex.batch_search over the whole group (global N and df) -> ids u32[B, kout], scores f32[B, kout], counts u32[B]"""
+        from .api import _check, _ptr, _query_csr
+        o, h = _query_csr(queries)
+        nq, k = len(o) - 1, int(top_k or 0)
+        kout = 512 if k == 0 or k > 512 else k
+        ids = np.zeros((max(nq, 1), kout), np.uint32)
+        scores = np.zeros((max(nq, 1), kout), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        _check(self._lib.cdb_tfidf_search_batch_sharded(self._h, _ptr(o), _ptr(h), nq, k, _ptr(ids), _ptr(scores), _ptr(counts)))
+        return ids[:nq], scores[:nq], counts[:nq]
+
     def close(self):
         if self._h:
             self._lib.cdb_shard_group_destroy(self._h)
             self._h = None
         self._shards = []
+        self._text_shards = []
 
     def __del__(self):
         try:

@@ -818,6 +818,47 @@ cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *index, const uint64_t 
                                          uint32_t n_queries, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
                                          void *stream);
 
+/* ------------------------------------------------ multi-GPU: row-sharded sparse and TF-IDF search
+ * The sparse and TF-IDF indexes of a collection split over the slots of a cdb_shard_group, next to (or without) its dense
+ * shards: a slot holds at most one dense, one sparse and one TF-IDF shard, and one group and one communicator serve all
+ * three.  Each shard is an ordinary index whose id_base is the global id of its local row 0; appends and deletes go to the
+ * owning shard (TF-IDF with the same versions the whole index would see).
+ * Contract: ids, counts and score bits equal what cdb_sparse_search_batch / cdb_tfidf_search_batch return for ONE index
+ * holding every shard's rows at their global ids, with the same appends, deletes and versions.
+ *   attach      CDB_INVALID_PARAMS for a shard on another device than its slot and, in a local group
+ *               (cdb_shard_group_create), for sparse shards whose quantization_bits or values_upper_bound bits differ from
+ *               another slot's, and for shards of one kind whose [id_base, id_base + capacity_rows) ranges overlap.  In a
+ *               per-rank group (cdb_shard_group_create_rank) the caller guarantees both across the ranks, as it does id
+ *               ranges for dense shards.
+ *   search      CDB_INVALID_PARAMS, before any device work, for null arguments, malformed query CSR, a local slot without a
+ *               shard of that kind, and the single-index limits: sparse k in 1..1024 and k * f <= 5120; TF-IDF k keeps its
+ *               meaning (0 = top_k None, above 512 gives 512 columns).  In a per-rank group every rank calls the search with
+ *               the same batch and receives the same result.
+ *   sparse      every shard keeps its top m = k * f candidates (f = reranking_factor with rerank, else 1) and one all-gather
+ *               brings them to every rank, which selects the group's top m: the single index's candidates, since keys are
+ *               unique and each shard's top m holds every one of its rows in the group's top m.  Without rerank these are
+ *               the results.  With rerank each rank re-ranks only the candidates it owns, a second all-gather combines them,
+ *               and the top k of the m re-ranked keys are kept.  (Re-ranking each shard's own top m and merging would not be
+ *               the same: a row outside the group's top m can re-rank into the top k.)  Queries are searched in chunks that
+ *               keep the gather buffer within 256 MB; each local shard holds its reader lock through both phases.
+ *               The device form (per-rank groups only) takes device arrays and is asynchronous on `stream`.
+ *   TF-IDF      idf depends on the whole corpus: N = sum of the shards' N, df = sum of their df (u32, wrapping), gathered on
+ *               the host (per-rank groups: one all-gather of 1 + query terms u32 per rank) and idf computed on the host
+ *               with the function a single index uses.  Each shard scores under that idf and hands in all 512 bucket
+ *               winners per query; per bucket the best of the ranks wins with `>`, equal scores (+0 and -0 too) going to
+ *               the smaller id, then they are sorted and truncated as in cdb_tfidf_search_batch.  Each local shard holds its
+ *               reader lock from the df look-up through the scoring.  Host form only: the idf needs the host mid-call. */
+cdb_status cdb_shard_group_attach_sparse(cdb_shard_group *group, uint32_t local_slot, cdb_sparse_index *shard);
+cdb_status cdb_shard_group_attach_tfidf(cdb_shard_group *group, uint32_t local_slot, cdb_tfidf_index *shard);
+cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_dims,
+                                           const float *q_values, uint32_t n_queries, const cdb_sparse_search_params *params,
+                                           uint32_t *out_ids, float *out_scores, uint32_t *out_counts);
+cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *group, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
+                                                  const float *d_q_values, uint32_t n_queries, const cdb_sparse_search_params *params,
+                                                  uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream);
+cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t n_queries,
+                                          uint32_t k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts);
+
 /* ------------------------------------------------ hybrid search (reciprocal-rank fusion)
  * hybrid_search (src/api/vectordb/search/repo.rs:168-341) and batch_hybrid_search (repo.rs:343-555); request defaults
  * top_k = 10, fusion_constant_k = 60.0 (src/api/vectordb/search/dtos.rs:6-12).
