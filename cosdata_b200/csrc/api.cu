@@ -5,6 +5,7 @@
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <shared_mutex>
@@ -1296,6 +1297,49 @@ cdb_status cdb_index_last_kernel_ms(const cdb_index *ix, float *scan_ms, float *
     return CDB_OK;
 }
 
+// searches already enqueued on their callers' streams finish on the old graph (and the old deletion marks) before they change
+static cdb_status wait_searches(cdb_index *ix) {
+    {
+        std::lock_guard<std::mutex> g(ix->pool_mu);
+        for (auto &u : ix->pool)
+            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
+    }
+    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    return CDB_OK;
+}
+
+// drops the graph, its builder state and its metadata.  `started` names a write that failed after it had begun changing the
+// graph: a half-changed graph is not the reference's graph, so the index has none until a build / upload, and the error says so
+static void drop_graph(cdb_index *ix, const char *started = nullptr) {
+    const std::string why = started ? cdb_last_error_string() : "";
+    const bool had_md = ix->has_md;
+    hnsw_state_free(ix->bstate);
+    ix->bstate = nullptr;
+    for (void *g : ix->graph_allocs) cudaFree(g);
+    ix->graph_allocs.clear();
+    for (void *g : ix->md_allocs) cudaFree(g);
+    ix->md_allocs.clear();
+    ix->has_md = false;
+    ix->has_graph = false;
+    if (started)
+        set_error(why + " (the " + started + " had started: the graph " + (had_md ? "and its metadata were" : "was") + " dropped)");
+}
+
+// the build parameters of a graph writer; the graph's shape (neighbour counts, levels) only for one that makes a new graph
+static cdb_status check_build_params(const cdb_build_params *bp, bool new_graph) {
+    CDB_REQUIRE(!new_graph || (bp->neighbors_count >= 1 && bp->neighbors_count <= 64 && bp->level0_neighbors_count >= 1 &&
+                               bp->level0_neighbors_count <= 64), "neighbour counts must be in 1..64");
+    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64 &&
+                    (!new_graph || bp->num_levels <= 15), "bad build parameters");
+    return CDB_OK;
+}
+
+// graph writers refuse a metric / storage arm that is an Err in the reference
+static cdb_status check_graph_arm(const cdb_index *ix) {
+    const cdb_status rc = arm_status(ix->desc.metric, ix->desc.storage_type);
+    if (rc != CDB_OK) set_error("metric/storage arm is an Err in the reference");
+    return rc;
+}
 
 cdb_status cdb_index_set_graph(cdb_index *ix, const cdb_graph_desc *gd) {
     CDB_REQUIRE(ix && gd && gd->level_counts && gd->node_row && gd->adjacency && gd->child, "null argument");
@@ -1320,14 +1364,7 @@ cdb_status cdb_index_set_graph(cdb_index *ix, const cdb_graph_desc *gd) {
                         "an adjacency entry names a deleted row");
     }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    hnsw_state_free(ix->bstate);
-    ix->bstate = nullptr;
-    for (void *g : ix->graph_allocs) cudaFree(g);
-    ix->graph_allocs.clear();
-    for (void *g : ix->md_allocs) cudaFree(g);
-    ix->md_allocs.clear();
-    ix->has_md = false;
-    ix->has_graph = false;
+    drop_graph(ix);
     const uint32_t L1 = gd->num_levels + 1;
     std::vector<const uint32_t *> nr(L1), ad(L1), ch(L1);
     auto upload = [&](const uint32_t *src, size_t n, const uint32_t **dst) -> cdb_status {
@@ -1445,14 +1482,10 @@ cdb_status cdb_index_set_graph_slot_scores(cdb_index *ix, const float *const *sc
     const uint32_t L1 = ix->graph.num_levels + 1;
     for (uint32_t L = 0; L < L1; ++L) CDB_REQUIRE(scores[L] && (!tags || tags[L]), "null level array");
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    {   // searches already enqueued on their callers' streams finish before the graph's state changes
-        std::lock_guard<std::mutex> g(ix->pool_mu);
-        for (auto &u : ix->pool)
-            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
-    }
-    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    cdb_status rc = wait_searches(ix);
+    if (rc) return rc;
     HnswBuildState *st = nullptr;
-    cdb_status rc = hnsw_attach_replica_state_device(ix->desc.metric, graph_host(ix), scores, tags, ix->md_pseudo_entry, ix->md_rows,
+    rc = hnsw_attach_replica_state_device(ix->desc.metric, graph_host(ix), scores, tags, ix->md_pseudo_entry, ix->md_rows,
                                                      ix->md_dims, ix->md_bits, ix->md_mags, &st, ix->stream);
     if (rc) return rc;
     hnsw_state_release(ix->bstate, &ix->graph_allocs);   // a plain slot state derived before the metadata was uploaded
@@ -1467,33 +1500,19 @@ cdb_status cdb_index_set_graph_slot_scores(cdb_index *ix, const float *const *sc
 
 cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
     CDB_REQUIRE(ix && bp, "null argument");
-    CDB_REQUIRE(bp->neighbors_count >= 1 && bp->neighbors_count <= 64 && bp->level0_neighbors_count >= 1 &&
-                    bp->level0_neighbors_count <= 64, "neighbour counts must be in 1..64");
-    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64 &&
-                    bp->num_levels <= 15, "bad build parameters");
+    cdb_status rc;
+    if ((rc = check_build_params(bp, true))) return rc;
     std::unique_lock<std::shared_mutex> lock(ix->rw);
     CDB_REQUIRE(ix->size >= 1 && ix->size + 1 <= ix->desc.capacity, "build needs >= 1 row and capacity for the root row");
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    cdb_status rc;
-    if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
-        set_error("metric/storage arm is an Err in the reference");
-        return rc;
-    }
-    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
+    if ((rc = check_graph_arm(ix)) || (rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
     const uint32_t n = (uint32_t)ix->size;
     // root vector: uniform in [range_lo, range_hi) (vector_store.rs:57-64)
     std::vector<float> root(ix->desc.dim);
     for (uint32_t c = 0; c < ix->desc.dim; ++c)
         root[c] = ix->desc.range_lo + (synth_value(bp->seed ^ 0x526F6F74ull, c) + 1.0f) * 0.5f * (ix->desc.range_hi - ix->desc.range_lo);
     if ((rc = append_f32_locked(ix, root.data(), 1))) return rc;
-    for (void *g : ix->md_allocs) cudaFree(g);
-    ix->md_allocs.clear();
-    ix->has_md = false;
-    hnsw_state_free(ix->bstate);
-    ix->bstate = nullptr;
-    for (void *g : ix->graph_allocs) cudaFree(g);
-    ix->graph_allocs.clear();
-    ix->has_graph = false;
+    drop_graph(ix);
     HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, n};
     rc = hnsw_build_device(sc, n, bp->num_levels, bp->neighbors_count, bp->level0_neighbors_count, bp->ef_construction,
                            bp->shortlist_size, bp->max_batch, bp->seed, graph_host(ix), &ix->bstate, ix->stream, ix->del_dev(),
@@ -1505,10 +1524,8 @@ cdb_status cdb_index_build_graph(cdb_index *ix, const cdb_build_params *bp) {
 
 cdb_status cdb_index_build_graph_replicas(cdb_index *ix, const cdb_build_params *bp, const cdb_replica_build *rb, uint8_t *out_failed) {
     CDB_REQUIRE(ix && bp && rb, "null argument");
-    CDB_REQUIRE(bp->neighbors_count >= 1 && bp->neighbors_count <= 64 && bp->level0_neighbors_count >= 1 &&
-                    bp->level0_neighbors_count <= 64, "neighbour counts must be in 1..64");
-    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64 &&
-                    bp->num_levels <= 15, "bad build parameters");
+    cdb_status rc;
+    if ((rc = check_build_params(bp, true))) return rc;
     CDB_REQUIRE(rb->md_dims >= 1 && rb->md_dims <= 4096, "md_dims must be in 1..4096");
     CDB_REQUIRE((rb->row && rb->node_id && rb->base_id && rb->md_row && rb->max_level) || !rb->n_nodes, "null replica list");
     CDB_REQUIRE((rb->md_bits && rb->md_mags) || !rb->n_md, "null metadata table");
@@ -1523,43 +1540,35 @@ cdb_status cdb_index_build_graph_replicas(cdb_index *ix, const cdb_build_params 
         CDB_REQUIRE(rb->row[t] == CDB_INVALID_ID || !ix->is_deleted(rb->row[t]), "replica row is deleted");
     }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    cdb_status rc;
-    if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
-        set_error("metric/storage arm is an Err in the reference");
-        return rc;
-    }
-    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
+    if ((rc = check_graph_arm(ix)) || (rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
     // main root: uniform in [range_lo, range_hi) (vector_store.rs:57-64); pseudo root: pseudo_node_vector = zeros (metadata/mod.rs:214-216)
     std::vector<float> roots(2 * (size_t)ix->desc.dim, 0.0f);
     for (uint32_t c = 0; c < ix->desc.dim; ++c)
         roots[c] = ix->desc.range_lo + (synth_value(bp->seed ^ 0x526F6F74ull, c) + 1.0f) * 0.5f * (ix->desc.range_hi - ix->desc.range_lo);
     if ((rc = append_f32_locked(ix, roots.data(), 2))) return rc;
-    for (void *g : ix->md_allocs) cudaFree(g);
-    ix->md_allocs.clear();
-    ix->has_md = false;
-    hnsw_state_free(ix->bstate);
-    ix->bstate = nullptr;
-    for (void *g : ix->graph_allocs) cudaFree(g);
-    ix->graph_allocs.clear();
-    ix->has_graph = false;
+    drop_graph(ix);
+    // the node_id / node_md tables the search reads; the builder fills them as it publishes the levels (arrays in graph_allocs)
+    void *tbl[2];
+    for (void *&p : tbl) {
+        CDB_CUDA_TRY(cudaMalloc(&p, ((size_t)bp->num_levels + 1) * sizeof(void *)));
+        ix->graph_allocs.push_back(p);
+    }
+    ix->md_node_id = reinterpret_cast<const uint32_t *const *>(tbl[0]);
+    ix->md_node_md = reinterpret_cast<const uint32_t *const *>(tbl[1]);
+    GraphHost gh{&ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr, &ix->g_ad, &ix->g_ch, &ix->g_id, &ix->g_md, ix->md_node_id,
+                 ix->md_node_md};
     std::vector<uint32_t> rows(rb->row, rb->row + rb->n_nodes);
     for (auto &r : rows) if (r == CDB_INVALID_ID) r = n + 1;   // pseudo replicas reuse the pseudo root's prop_value (vector_store.rs:661)
     ReplicaHost rh{rb->n_nodes, rows.data(), rb->node_id, rb->base_id, rb->md_row, rb->max_level, rb->md_dims, rb->n_md,
                    rb->md_bits, rb->md_mags, n, rb->main_root_md, n + 1, rb->pseudo_root_md};
     HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, n};
-    ReplicaGraphDev mdv{};
-    std::vector<uint8_t> failed;
     rc = hnsw_build_replicas_device(sc, rh, bp->num_levels, bp->neighbors_count, bp->level0_neighbors_count, bp->ef_construction,
-                                    bp->shortlist_size, bp->max_batch, &ix->graph, &ix->graph_allocs, &ix->g_cnt, &ix->g_nr,
-                                    &ix->g_ad, &ix->g_ch, &mdv, &failed, &ix->bstate, ix->stream);
+                                    bp->shortlist_size, bp->max_batch, gh, out_failed, &ix->md_bits, &ix->md_mags, &ix->bstate, ix->stream);
     if (rc) return rc;
+    ix->md_dims = rb->md_dims;
+    ix->md_pseudo_entry = 1;
     ix->has_graph = true;
-    ix->md_node_id = mdv.node_id; ix->md_node_md = mdv.node_md;
-    ix->g_id = mdv.h_node_id; ix->g_md = mdv.h_node_md;
-    ix->md_bits = mdv.md_bits; ix->md_mags = mdv.md_mags;
-    ix->md_dims = mdv.md_dims; ix->md_pseudo_entry = mdv.pseudo_entry;
-    ix->has_md = true;   // the arrays live in graph_allocs
-    if (out_failed) std::copy(failed.begin(), failed.end(), out_failed);
+    ix->has_md = true;
     return CDB_OK;
 }
 
@@ -1597,11 +1606,33 @@ static cdb_status ensure_build_state(cdb_index *ix) {
     return hnsw_slot_state_device(sc, graph_host(ix), &ix->bstate, ix->stream);
 }
 
+// runs `write` on the graph once the searches enqueued before it have finished and the builder's state exists; a write that
+// failed after it had begun changing the graph (*changed) drops it, `what` names the write in the error
+using GraphWrite = std::function<cdb_status(const HnScoreCtx &, bool *changed)>;
+static cdb_status write_graph(cdb_index *ix, const char *what, const GraphWrite &write) {
+    cdb_status rc;
+    if ((rc = wait_searches(ix)) || (rc = ensure_build_state(ix))) return rc;
+    HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
+    bool changed = false;
+    if ((rc = write(sc, &changed)) && changed) drop_graph(ix, what);
+    return rc;
+}
+
+// the tail both inserts share once their refusals passed: `insert` of n entries into the graph
+static cdb_status insert_into_graph(cdb_index *ix, const cdb_build_params *bp, uint64_t n, uint64_t *out_inserted, const GraphWrite &insert) {
+    if (!n) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    cdb_status rc;
+    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction)) || (rc = write_graph(ix, "insert", insert))) return rc;
+    if (out_inserted) *out_inserted = n;
+    return CDB_OK;
+}
+
 cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, const uint8_t *max_level, uint8_t *out_failed,
                                   uint64_t *out_inserted) {
     CDB_REQUIRE(ix && bp, "null argument");
-    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64,
-                "bad build parameters");
+    cdb_status rc;
+    if ((rc = check_build_params(bp, false))) return rc;
     if (out_inserted) *out_inserted = 0;
     std::unique_lock<std::shared_mutex> lock(ix->rw);
     CDB_REQUIRE(ix->has_graph, "no graph: cdb_index_build_graph or cdb_index_set_graph first");
@@ -1610,47 +1641,20 @@ cdb_status cdb_index_insert_graph(cdb_index *ix, const cdb_build_params *bp, con
                     bp->level0_neighbors_count == ix->graph.nbrs0,
                 "params num_levels / neighbors_count / level0_neighbors_count differ from the graph's");
     CDB_REQUIRE((ix->graph.identity_mask & 1u) && ix->g_cnt[0] <= ix->size, "level 0 of the graph must list rows 0..level_counts[0]-1");
-    cdb_status rc;
-    if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
-        set_error("metric/storage arm is an Err in the reference");
-        return rc;
-    }
+    if ((rc = check_graph_arm(ix))) return rc;
     const uint64_t n_new = ix->size - ix->g_cnt[0];
-    if (!n_new) return CDB_OK;
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
-    {   // searches already enqueued on their callers' streams finish on the old graph before it changes
-        std::lock_guard<std::mutex> g(ix->pool_mu);
-        for (auto &u : ix->pool)
-            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
-    }
-    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
-    if ((rc = ensure_build_state(ix))) return rc;
-    HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
-    bool changed = false;
-    if ((rc = hnsw_insert_device(sc, graph_host(ix), ix->bstate, (uint32_t)n_new, max_level, bp->seed, bp->ef_construction,
-                                 bp->shortlist_size, bp->max_batch, ix->desc.capacity, out_failed, &changed, ix->stream, ix->del_dev(),
-                                 ix->del_host()))) {
-        if (changed) {   // a half-inserted graph is not the reference's graph: the index has none until a build / upload
-            const std::string why = cdb_last_error_string();
-            hnsw_state_free(ix->bstate);
-            ix->bstate = nullptr;
-            for (void *g : ix->graph_allocs) cudaFree(g);
-            ix->graph_allocs.clear();
-            ix->has_graph = false;
-            set_error(why + " (the insert had started: the graph was dropped)");
-        }
-        return rc;
-    }
-    if (out_inserted) *out_inserted = n_new;
-    return CDB_OK;
+    return insert_into_graph(ix, bp, n_new, out_inserted, [&](const HnScoreCtx &sc, bool *changed) {
+        return hnsw_insert_device(sc, graph_host(ix), ix->bstate, (uint32_t)n_new, max_level, bp->seed, bp->ef_construction,
+                                  bp->shortlist_size, bp->max_batch, ix->desc.capacity, out_failed, changed, ix->stream, ix->del_dev(),
+                                  ix->del_host());
+    });
 }
 
 cdb_status cdb_index_insert_graph_replicas(cdb_index *ix, const cdb_build_params *bp, const cdb_replica_insert *ri, uint8_t *out_failed,
                                            uint64_t *out_inserted) {
     CDB_REQUIRE(ix && bp && ri, "null argument");
-    CDB_REQUIRE(bp->ef_construction >= 1 && bp->ef_construction <= 4096 && bp->shortlist_size >= 1 && bp->shortlist_size <= 64,
-                "bad build parameters");
+    cdb_status rc;
+    if ((rc = check_build_params(bp, false))) return rc;
     if (out_inserted) *out_inserted = 0;
     std::unique_lock<std::shared_mutex> lock(ix->rw);
     CDB_REQUIRE(ix->has_graph && ix->has_md,
@@ -1685,44 +1689,15 @@ cdb_status cdb_index_insert_graph_replicas(cdb_index *ix, const cdb_build_params
         CDB_REQUIRE(r == CDB_INVALID_ID || !ix->is_deleted(r), "replica row is deleted");
         CDB_REQUIRE(ri->md_row[t] == CDB_INVALID_ID || ri->md_row[t] < n_md_all, "replica md_row out of range");
     }
-    cdb_status rc;
-    if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
-        set_error("metric/storage arm is an Err in the reference");
-        return rc;
-    }
-    if (!ri->n_nodes) return CDB_OK;
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    if ((rc = hnsw_build_smem_check(ix->row_pitch, bp->ef_construction))) return rc;
-    {   // searches already enqueued on their callers' streams finish on the old graph before it changes
-        std::lock_guard<std::mutex> g(ix->pool_mu);
-        for (auto &u : ix->pool)
-            if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
-    }
-    CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    if ((rc = check_graph_arm(ix))) return rc;
     std::vector<uint32_t> rows(ri->row, ri->row + ri->n_nodes);
     for (auto &r : rows) if (r == CDB_INVALID_ID) r = pseudo_row;   // pseudo replicas reuse the pseudo root's prop_value (vector_store.rs:661)
     ReplicaHost rh{ri->n_nodes, rows.data(), ri->node_id, ri->base_id, ri->md_row, ri->max_level, ri->md_dims, ri->n_md_new,
                    ri->md_bits_new, ri->md_mags_new, ix->graph.root_row, CDB_INVALID_ID, pseudo_row, CDB_INVALID_ID};
-    HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
-    bool changed = false;
-    if ((rc = hnsw_insert_replicas_device(sc, graph_host(ix), ix->bstate, rh, bp->ef_construction, bp->shortlist_size, bp->max_batch,
-                                          out_failed, &ix->md_bits, &ix->md_mags, &changed, ix->stream))) {
-        if (changed) {   // a half-inserted graph is not the reference's graph: the index has none until a build / upload
-            const std::string why = cdb_last_error_string();
-            hnsw_state_free(ix->bstate);
-            ix->bstate = nullptr;
-            for (void *g : ix->graph_allocs) cudaFree(g);
-            ix->graph_allocs.clear();
-            for (void *g : ix->md_allocs) cudaFree(g);
-            ix->md_allocs.clear();
-            ix->has_md = false;
-            ix->has_graph = false;
-            set_error(why + " (the insert had started: the graph and its metadata were dropped)");
-        }
-        return rc;
-    }
-    if (out_inserted) *out_inserted = ri->n_nodes;
-    return CDB_OK;
+    return insert_into_graph(ix, bp, ri->n_nodes, out_inserted, [&](const HnScoreCtx &sc, bool *changed) {
+        return hnsw_insert_replicas_device(sc, graph_host(ix), ix->bstate, rh, bp->ef_construction, bp->shortlist_size, bp->max_batch,
+                                           out_failed, &ix->md_bits, &ix->md_mags, changed, ix->stream);
+    });
 }
 
 // the prefilter shadows of newly deleted rows (marks already on the device): fp16 rows := 0, and the s8 tiles holding them
@@ -1749,17 +1724,10 @@ static cdb_status drop_from_shadows(cdb_index *ix, const std::vector<uint32_t> &
     return CDB_OK;
 }
 
-cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
-                                 uint8_t *out_status, uint64_t *out_deleted) {
-    CDB_REQUIRE(ix && (rows || !n), "null argument");
-    CDB_REQUIRE(shortlist_size >= 1 && shortlist_size <= 64, "shortlist_size must be in 1..64");
-    if (out_deleted) *out_deleted = 0;
-    std::unique_lock<std::shared_mutex> lock(ix->rw);
-    for (uint64_t i = 0; i < n; ++i) {
-        CDB_REQUIRE(rows[i] < ix->size, "row out of range");
-        CDB_REQUIRE(!ix->has_graph || rows[i] != ix->graph.root_row, "the graph's root row cannot be deleted");
-    }
-    if (ix->has_graph && ix->has_md) { set_error("delete from a graph with metadata is not supported"); return CDB_UNSUPPORTED; }
+// the body both deletes share once their refusals passed: the graph (if any) repaired around the distinct rows not deleted
+// yet, then their deletion marks
+static cdb_status delete_rows_locked(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
+                                     uint8_t *out_status, uint64_t *out_deleted) {
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     // status 1 for rows deleted before or earlier in the list
     std::vector<uint8_t> status(n, 1);
@@ -1769,7 +1737,7 @@ cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n
         if (!ix->is_deleted(rows[i]) && seen.insert(rows[i]).second) { status[i] = 0; fresh.push_back(rows[i]); }
     cdb_status rc;
     if (!fresh.empty()) {
-        if (ix->has_graph && (rc = hnsw_build_smem_check(ix->row_pitch, HNSW_DELETE_EF))) return rc;
+        if (ix->has_graph && ((rc = check_graph_arm(ix)) || (rc = hnsw_build_smem_check(ix->row_pitch, HNSW_DELETE_EF)))) return rc;
         const size_t words = ix->desc.capacity / 32 + 1;
         if (!ix->d_deleted) {   // allocated before anything changes; kernels see it only once a row is deleted
             void *p = nullptr;
@@ -1778,35 +1746,13 @@ cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n
             ix->h_deleted.assign(words, 0u);
             CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
         }
-        {   // searches already enqueued on their callers' streams finish on the old graph and the old marks
-            std::lock_guard<std::mutex> g(ix->pool_mu);
-            for (auto &u : ix->pool)
-                if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
-        }
-        CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
         std::vector<uint8_t> fst(fresh.size(), 0);
-        if (ix->has_graph) {
-            if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
-                set_error("metric/storage arm is an Err in the reference");
-                return rc;
-            }
-            if ((rc = ensure_build_state(ix))) return rc;
-            HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
-            bool changed = false;
-            if ((rc = hnsw_delete_device(sc, graph_host(ix), ix->bstate, fresh.data(), (uint32_t)fresh.size(), shortlist_size, max_batch,
-                                         fst.data(), &changed, ix->stream))) {
-                if (changed) {   // a half-repaired graph links deleted rows: the index has none until a build / upload
-                    const std::string why = cdb_last_error_string();
-                    hnsw_state_free(ix->bstate);
-                    ix->bstate = nullptr;
-                    for (void *g : ix->graph_allocs) cudaFree(g);
-                    ix->graph_allocs.clear();
-                    ix->has_graph = false;
-                    set_error(why + " (the delete had started: the graph was dropped)");
-                }
-                return rc;
-            }
-        }
+        rc = !ix->has_graph ? wait_searches(ix) : write_graph(ix, "delete", [&](const HnScoreCtx &sc, bool *changed) {
+            return (ix->has_md ? hnsw_delete_replicas_device : hnsw_delete_device)(sc, graph_host(ix), ix->bstate, fresh.data(),
+                                                                                  (uint32_t)fresh.size(), shortlist_size, max_batch,
+                                                                                  fst.data(), changed, ix->stream);
+        });
+        if (rc) return rc;
         // the marks, once the repair succeeded
         uint32_t lo = 0xFFFFFFFFu, hi = 0;
         for (uint32_t r : fresh) {
@@ -1826,6 +1772,20 @@ cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n
     return CDB_OK;
 }
 
+cdb_status cdb_index_delete_rows(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
+                                 uint8_t *out_status, uint64_t *out_deleted) {
+    CDB_REQUIRE(ix && (rows || !n), "null argument");
+    CDB_REQUIRE(shortlist_size >= 1 && shortlist_size <= 64, "shortlist_size must be in 1..64");
+    if (out_deleted) *out_deleted = 0;
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    for (uint64_t i = 0; i < n; ++i) {
+        CDB_REQUIRE(rows[i] < ix->size, "row out of range");
+        CDB_REQUIRE(!ix->has_graph || rows[i] != ix->graph.root_row, "the graph's root row cannot be deleted");
+    }
+    if (ix->has_graph && ix->has_md) { set_error("delete from a graph with metadata is not supported"); return CDB_UNSUPPORTED; }
+    return delete_rows_locked(ix, rows, n, shortlist_size, max_batch, out_status, out_deleted);
+}
+
 cdb_status cdb_index_delete_rows_replicas(cdb_index *ix, const uint32_t *rows, uint64_t n, uint32_t shortlist_size, uint32_t max_batch,
                                           uint8_t *out_status, uint64_t *out_deleted) {
     CDB_REQUIRE(ix && (rows || !n), "null argument");
@@ -1843,70 +1803,7 @@ cdb_status cdb_index_delete_rows_replicas(cdb_index *ix, const uint32_t *rows, u
         CDB_REQUIRE(rows[i] < ix->size, "row out of range");
         CDB_REQUIRE(rows[i] != ix->graph.root_row && rows[i] != pseudo_row, "the graph's root rows cannot be deleted");
     }
-    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    // status 1 for rows deleted before or earlier in the list
-    std::vector<uint8_t> status(n, 1);
-    std::vector<uint32_t> fresh;
-    std::unordered_set<uint32_t> seen;
-    for (uint64_t i = 0; i < n; ++i)
-        if (!ix->is_deleted(rows[i]) && seen.insert(rows[i]).second) { status[i] = 0; fresh.push_back(rows[i]); }
-    cdb_status rc;
-    if (!fresh.empty()) {
-        if ((rc = arm_status(ix->desc.metric, ix->desc.storage_type)) != CDB_OK) {
-            set_error("metric/storage arm is an Err in the reference");
-            return rc;
-        }
-        if ((rc = hnsw_build_smem_check(ix->row_pitch, HNSW_DELETE_EF))) return rc;
-        const size_t words = ix->desc.capacity / 32 + 1;
-        if (!ix->d_deleted) {   // allocated before anything changes; kernels see it only once a row is deleted
-            void *p = nullptr;
-            CDB_CUDA_TRY(cudaMalloc(&p, words * 4));
-            ix->d_deleted = (uint32_t *)p;
-            ix->h_deleted.assign(words, 0u);
-            CDB_CUDA_TRY(cudaMemset(ix->d_deleted, 0, words * 4));
-        }
-        {   // searches already enqueued on their callers' streams finish on the old graph and the old marks
-            std::lock_guard<std::mutex> g(ix->pool_mu);
-            for (auto &u : ix->pool)
-                if (u->ev_valid) CDB_CUDA_TRY(cudaStreamWaitEvent(ix->stream, u->ev[2], 0));
-        }
-        CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
-        std::vector<uint8_t> fst(fresh.size(), 0);
-        HnScoreCtx sc{ix->d_codes, ix->row_pitch, ix->d_mags, ix->desc.dim, ix->desc.storage_type, ix->desc.metric, ix->graph.root_row};
-        bool changed = false;
-        if ((rc = hnsw_delete_replicas_device(sc, graph_host(ix), ix->bstate, fresh.data(), (uint32_t)fresh.size(), shortlist_size,
-                                              max_batch, fst.data(), &changed, ix->stream))) {
-            if (changed) {   // a half-repaired graph links deleted rows: the index has no graph until a build / upload
-                const std::string why = cdb_last_error_string();
-                hnsw_state_free(ix->bstate);
-                ix->bstate = nullptr;
-                for (void *g : ix->graph_allocs) cudaFree(g);
-                ix->graph_allocs.clear();
-                for (void *g : ix->md_allocs) cudaFree(g);
-                ix->md_allocs.clear();
-                ix->has_md = false;
-                ix->has_graph = false;
-                set_error(why + " (the delete had started: the graph and its metadata were dropped)");
-            }
-            return rc;
-        }
-        // the marks, once the repair succeeded
-        uint32_t lo = 0xFFFFFFFFu, hi = 0;
-        for (uint32_t r : fresh) {
-            ix->h_deleted[r >> 5] |= 1u << (r & 31);
-            lo = std::min(lo, r >> 5);
-            hi = std::max(hi, r >> 5);
-        }
-        CDB_CUDA_TRY(cudaMemcpy(ix->d_deleted + lo, ix->h_deleted.data() + lo, (size_t)(hi - lo + 1) * 4, cudaMemcpyHostToDevice));
-        ix->n_deleted += fresh.size();
-        if ((rc = drop_from_shadows(ix, fresh))) return rc;
-        size_t j = 0;
-        for (uint64_t i = 0; i < n; ++i)
-            if (status[i] == 0) status[i] = fst[j++];
-        if (out_deleted) *out_deleted = fresh.size();
-    }
-    if (out_status) std::copy(status.begin(), status.end(), out_status);
-    return CDB_OK;
+    return delete_rows_locked(ix, rows, n, shortlist_size, max_batch, out_status, out_deleted);
 }
 
 cdb_status cdb_index_read_replica_slot_scores(cdb_index *ix, uint32_t level, float *out_scores) {

@@ -539,33 +539,89 @@ cdb_status hnsw_build_smem_check(uint32_t row_pitch, uint32_t ef) {
     return CDB_OK;
 }
 
-// index_embeddings for rows [first, first+count) (levels[i] = max insert level of row first+i), the one batch loop of both
-// the build and the insert.  Nodes for every level the rows reach are appended up front (level 0: node = row; levels >= 1:
-// ascending rows after the existing nodes, child pointing into the appended part of the level below), so node_row / child
-// are static while the adjacency evolves.  Batches hold max(1, min(max_batch, linked / 8)) rows, linked = data rows already
-// in the graph: a fresh build starts almost sequentially, a small transaction into a large graph runs as one batch.
-// Every allocation happens before the graph changes; *changed tells the caller whether an error left it half-inserted.
-static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState &st, uint32_t first, uint32_t count,
-                              const std::vector<uint8_t> &levels_in, uint32_t linked, uint32_t ef_construction, uint32_t shortlist,
-                              uint32_t max_batch, uint64_t rows_cap, uint8_t *out_failed, bool *changed, cudaStream_t s,
-                              const uint32_t *d_deleted, const uint32_t *h_deleted) {
-    const uint32_t L1 = st.g.num_levels + 1;
-    cdb_status rc;
-    std::vector<std::vector<uint32_t>> rows(L1), child(L1);
-    std::vector<uint8_t> levels = levels_in;
+// What an insert appends (planned before anything changes, so node_row / child are static while the adjacency evolves):
+// per level the nodes' vector rows and, on levels >= 1, their children one level down; on replica graphs the nodes'
+// columns; and the top level of each entry.
+struct InsertPlan {
+    std::vector<std::vector<uint32_t>> rows, child;
+    ReplicaCols cols;
+    std::vector<uint8_t> levels;
+};
+
+// rows [first, first + levels.size()) of a plain graph (levels[i] = max insert level of row first+i): level 0 holds node = row,
+// levels >= 1 take ascending rows after the existing nodes, with child pointing into the appended part of the level below
+static InsertPlan plan_rows(const HnswBuildState &st, uint32_t first, std::vector<uint8_t> levels, const uint32_t *h_deleted) {
+    const uint32_t L1 = st.g.num_levels + 1, count = (uint32_t)levels.size();
+    InsertPlan p;
+    p.rows.resize(L1); p.child.resize(L1);
     for (uint32_t i = 0; h_deleted && i < count; ++i)   // a deleted row gets no upper-level nodes (and is not linked)
         if ((h_deleted[(first + i) >> 5] >> ((first + i) & 31)) & 1u) levels[i] = 0;
-    for (uint32_t r = std::max(first, st.g.lv[0].cnt); r < first + count; ++r) rows[0].push_back(r);
+    for (uint32_t r = std::max(first, st.g.lv[0].cnt); r < first + count; ++r) p.rows[0].push_back(r);
     for (uint32_t i = 0; i < count; ++i)
-        for (uint32_t L = 1; L <= levels[i]; ++L) rows[L].push_back(first + i);
+        for (uint32_t L = 1; L <= levels[i]; ++L) p.rows[L].push_back(first + i);
     for (uint32_t L = 1; L < L1; ++L) {
         uint32_t j = 0;   // position in the rows appended one level down (both lists ascend)
-        for (uint32_t r : rows[L]) {
-            if (L == 1) { child[L].push_back(r); continue; }
-            while (rows[L - 1][j] != r) ++j;
-            child[L].push_back(st.g.lv[L - 1].cnt + j);
+        for (uint32_t r : p.rows[L]) {
+            if (L == 1) { p.child[L].push_back(r); continue; }
+            while (p.rows[L - 1][j] != r) ++j;
+            p.child[L].push_back(st.g.lv[L - 1].cnt + j);
         }
     }
+    p.levels = std::move(levels);
+    return p;
+}
+
+// the entries of `rh` on a replica graph: list positions continue from st.n_list, new nodes follow the existing ones on every
+// level they reach in list order, children at their position among the nodes appended one level down
+static InsertPlan plan_replicas(const HnswBuildState &st, const ReplicaHost &rh) {
+    const uint32_t L1 = st.g.num_levels + 1, n = rh.n_nodes;
+    InsertPlan p;
+    p.rows.resize(L1); p.child.resize(L1);
+    p.cols.id.resize(L1); p.cols.md.resize(L1); p.cols.ins.resize(L1);
+    p.levels.resize(n);
+    std::vector<std::vector<uint32_t>> members(L1);   // new list indices present on each level
+    for (uint32_t t = 0; t < n; ++t) {
+        p.levels[t] = (uint8_t)std::min<uint32_t>(rh.max_level[t], st.g.num_levels);
+        for (uint32_t L = 0; L <= p.levels[t]; ++L) {
+            members[L].push_back(t);
+            p.rows[L].push_back(rh.row[t]);
+            p.cols.id[L].push_back(rh.node_id[t]);
+            p.cols.md[L].push_back(rh.md_row[t]);
+            p.cols.ins[L].push_back(st.n_list + t);
+        }
+    }
+    for (uint32_t L = 1; L < L1; ++L) {
+        uint32_t j = 0;   // position among the nodes appended one level down (both lists ascend)
+        for (uint32_t t : members[L]) {
+            while (members[L - 1][j] != t) ++j;
+            p.child[L].push_back(st.g.lv[L - 1].cnt + j);
+        }
+    }
+    return p;
+}
+
+// the Metadata table and the edge rules' keys of a replica graph (rows and ids are the caller's)
+static ReplicaDev replica_table(const int32_t *md_bits, const float *md_mags, uint32_t M) {
+    ReplicaDev rl{};
+    rl.md_bits = md_bits;
+    rl.md_mags = md_mags;
+    rl.M = M;
+    rl.key_one = order_key(CDB_METRIC_COSINE, 0x3F800000u);
+    rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
+    return rl;
+}
+
+// index_embeddings for the planned entries [first, first + count) (rows, or on replica graphs list positions with `rl` indexed
+// by them), the one batch loop of the build, the insert and their replica forms.  The planned nodes are appended up front.
+// Batches hold max(1, min(max_batch, (linked + done) / 8)) entries, linked = entries already in the graph: a fresh build starts
+// almost sequentially, a small transaction into a large graph runs as one batch.  Every allocation happens before the graph
+// changes; *changed tells the caller whether an error left it half-inserted.
+static cdb_status insert_planned(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState &st, const InsertPlan &p, uint32_t first,
+                                 uint32_t linked, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t rows_cap,
+                                 uint8_t *out_failed, bool *changed, cudaStream_t s, const uint32_t *d_deleted, const ReplicaDev *rl,
+                                 const char *what) {
+    const uint32_t L1 = st.g.num_levels + 1, count = (uint32_t)p.levels.size();
+    cdb_status rc;
     if (max_batch == 0) max_batch = 4096;
     max_batch = std::max<uint32_t>(1, std::min(max_batch, count));
     DevAllocs tmp;
@@ -577,10 +633,10 @@ static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
         return rc;
     const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
     CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
-    if ((rc = append_levels(st, gh, rows, child, rows_cap, changed, s))) return rc;
+    if ((rc = append_levels(st, gh, p.rows, p.child, rows_cap, changed, s, rl ? &p.cols : nullptr))) return rc;
     if (!count) return CDB_OK;
     // ---- batches
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_levels, levels.data(), count, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_levels, p.levels.data(), count, cudaMemcpyHostToDevice, s));
     BuildArgs a{};
     a.g = st.g;
     a.sc = sc;
@@ -592,6 +648,8 @@ static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
     a.zcap = 64;
     a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
     a.deleted = d_deleted;
+    a.replicas = rl != nullptr;
+    if (rl) a.rl = *rl;
     for (uint32_t done = 0; done < count;) {
         uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, (uint32_t)(((uint64_t)linked + done) / 8)));
         batch = std::min<uint32_t>(batch, count - done);
@@ -607,21 +665,22 @@ static cdb_status insert_rows(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
     cudaError_t e = cudaStreamSynchronize(s);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e == cudaSuccess && out_failed) e = cudaMemcpy(out_failed, failed, count, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_error(std::string("hnsw build: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    if (e != cudaSuccess) { set_error(std::string(what) + ": " + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
     return CDB_OK;
 }
 
-cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root is row n */, uint32_t num_levels, uint32_t nbrs,
-                             uint32_t nbrs0, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed,
-                             const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s, const uint32_t *d_deleted,
-                             const uint32_t *h_deleted) {
+// a fresh builder state for a graph of num_levels + 1 empty levels, and the search layout's pointer tables; the roots are
+// appended next
+static cdb_status new_graph(int metric, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0, uint32_t root_row, uint32_t entry,
+                            uint32_t identity_mask, const GraphHost &gh, std::unique_ptr<HnswBuildState> &st) {
     if (num_levels + 1 > BUILD_MAX_LEVELS) { set_error("build: too many levels"); return CDB_INVALID_PARAMS; }
     const uint32_t L1 = num_levels + 1;
-    std::unique_ptr<HnswBuildState> st(new HnswBuildState());
+    st.reset(new HnswBuildState());
     st->g.num_levels = num_levels;
-    st->g.root_row = n;
-    st->g.entry = num_levels == 0 ? n : 0;
-    metric_key_range(sc.metric, &st->g.min_key, &st->g.max_key);
+    st->g.root_row = root_row;
+    st->g.entry = entry;
+    metric_key_range(metric, &st->g.min_key, &st->g.max_key);
+    for (uint32_t L = 0; L < L1; ++L) st->g.lv[L].nb = L == 0 ? nbrs0 : nbrs;
     const uint32_t *tbl[3];
     for (int t = 0; t < 3; ++t) {
         void *p = nullptr;
@@ -632,28 +691,36 @@ cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root
     gh.dev->num_levels = num_levels;
     gh.dev->nbrs = nbrs;
     gh.dev->nbrs0 = nbrs0;
-    gh.dev->entry = st->g.entry;
-    gh.dev->root_row = n;
-    gh.dev->identity_mask = 1u;   // level 0: node i is row i (lv_local), the search skips the node_row lookup there
+    gh.dev->entry = entry;
+    gh.dev->root_row = root_row;
+    gh.dev->identity_mask = identity_mask;
     gh.dev->node_row = reinterpret_cast<const uint32_t *const *>(tbl[0]);
     gh.dev->adj = reinterpret_cast<const uint32_t *const *>(tbl[1]);
     gh.dev->child = reinterpret_cast<const uint32_t *const *>(tbl[2]);
+    return CDB_OK;
+}
+
+cdb_status hnsw_build_device(const HnScoreCtx &sc, uint32_t n /* data rows; root is row n */, uint32_t num_levels, uint32_t nbrs,
+                             uint32_t nbrs0, uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint64_t seed,
+                             const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s, const uint32_t *d_deleted,
+                             const uint32_t *h_deleted) {
+    // level 0: node i is row i (lv_local), the search skips the node_row lookup there
+    std::unique_ptr<HnswBuildState> st;
+    cdb_status rc = new_graph(sc.metric, num_levels, nbrs, nbrs0, n, num_levels == 0 ? n : 0, 1u, gh, st);
+    if (rc) return rc;
     // ---- the root on every level (vector_store.rs:44-140); level 0 holds a node for every row, linked once inserted
-    cdb_status rc;
+    const uint32_t L1 = num_levels + 1;
     bool changed = false;
     std::vector<std::vector<uint32_t>> rows(L1), child(L1);
     for (uint32_t i = 0; i <= n; ++i) rows[0].push_back(i);
-    for (uint32_t L = 0; L < L1; ++L) {
-        st->g.lv[L].nb = L == 0 ? nbrs0 : nbrs;
-        if (L) { rows[L] = {n}; child[L] = {L == 1 ? n : 0u}; }
-    }
+    for (uint32_t L = 1; L < L1; ++L) { rows[L] = {n}; child[L] = {L == 1 ? n : 0u}; }
     if ((rc = append_levels(*st, gh, rows, child, n + 1, &changed, s))) return rc;
     // ---- then every data row through the insert path
     std::vector<uint8_t> levels(n);
     for (uint32_t r = 0; r < n; ++r) levels[r] = draw_level(seed, r, num_levels);
-    if ((rc = insert_rows(sc, gh, *st, 0, n, levels, 0, ef_construction, shortlist, max_batch, n + 1, nullptr, &changed, s,
-                          d_deleted, h_deleted)))
-        return rc;
+    rc = insert_planned(sc, gh, *st, plan_rows(*st, 0, std::move(levels), h_deleted), 0, 0, ef_construction, shortlist, max_batch, n + 1,
+                        nullptr, &changed, s, d_deleted, nullptr, "hnsw build");
+    if (rc) return rc;
     *out_state = st.release();
     return CDB_OK;
 }
@@ -665,8 +732,8 @@ cdb_status hnsw_insert_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
     std::vector<uint8_t> levels(n_new);
     for (uint32_t i = 0; i < n_new; ++i)
         levels[i] = max_level ? (uint8_t)std::min<uint32_t>(max_level[i], num_levels) : draw_level(seed, first + i, num_levels);
-    return insert_rows(sc, gh, *st, first, n_new, levels, first - 1, ef_construction, shortlist, max_batch, rows_cap, out_failed, changed, s,
-                       d_deleted, h_deleted);
+    return insert_planned(sc, gh, *st, plan_rows(*st, first, std::move(levels), h_deleted), first, first - 1, ef_construction, shortlist,
+                          max_batch, rows_cap, out_failed, changed, s, d_deleted, nullptr, "hnsw build");
 }
 
 cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState **out_state, cudaStream_t s) {
@@ -725,18 +792,19 @@ cdb_status hnsw_slot_state_device(const HnScoreCtx &sc, const GraphHost &gh, Hns
 struct DelArgs {
     BuildGraph g;
     HnScoreCtx sc;
-    const uint32_t *loc;    // [n][num_levels+1] level-local index of each deleted row (HN_EMPTY: not on that level)
+    // the batch positions are items: the deleted rows on a plain graph, every node of a deleted row on a replica graph; the
+    // batch's rows own items [row_items[j], row_items[j+1]) for j from rfirst
+    const uint32_t *loc;    // [items][num_levels+1] level-local index of each item (HN_EMPTY: not on that level)
     uint32_t first, count, zcap;
     const uint32_t *z_nodes, *z_n;
-    uint8_t *status;        // [n] 2 where a rescoring Err stopped a relink
+    uint8_t *status;        // [items] 2 where a rescoring Err stopped a relink
     uint32_t *dead[BUILD_MAX_LEVELS];      // [cnt/32+1] nodes deleted by this call
     uint32_t *dead_of[BUILD_MAX_LEVELS];   // [cnt] batch position of a deleted node
     uint32_t *touched[BUILD_MAX_LEVELS];   // [cnt/32+1] nodes the sweep cleared a slot of
     uint2 *list[BUILD_MAX_LEVELS];         // [cnt] (node, batch position) of each touched node
     uint32_t *list_n;                      // [num_levels+1]
-    // replica graphs (hnsw_delete_replicas_device): the batch positions are replica-list items (every node of a deleted row),
-    // the batch's rows own items [row_items[j], row_items[j+1]) for j from rfirst, relinks rescore with the replica arms
-    // and apply the edge rules, and a touched node takes the candidates of the smallest batch position it named (tmin)
+    // replica graphs (hnsw_delete_replicas_device): relinks rescore with the replica arms and apply the edge rules, and a
+    // touched node takes the candidates of the smallest batch position it named (tmin)
     bool replicas;
     ReplicaDev rl;                         // the Metadata table and the edge rules' keys
     const uint32_t *row_items;
@@ -899,21 +967,10 @@ __device__ void del_repair_node(const DelArgs &a, uint32_t level, uint32_t b, ui
     __syncwarp();
 }
 
-// phase B: one warp (one block) per (delete, level)
+// phase B: one warp (one block) per (deleted row, level) repairs the row's items on that level in order -- on a replica graph
+// two replicas of a row can share neighbours, so one after the other keeps the result deterministic; on a plain graph a row
+// is one item
 __global__ void __launch_bounds__(32) hnsw_delete_repair_kernel(DelArgs a) {
-    extern __shared__ __align__(128) uint8_t row[];
-    __shared__ DelSmem sm;
-    const uint32_t L1 = a.g.num_levels + 1, b = blockIdx.x / L1, level = blockIdx.x % L1;
-    const uint32_t D = a.loc[(size_t)(a.first + b) * L1 + level];
-    if (D == HN_EMPTY) return;
-    del_smem_init(sm);
-    uint32_t parity = 0;
-    del_repair_node(a, level, b, D, row, sm, parity);
-}
-
-// phase B on a replica graph: one warp (one block) per (deleted row, level) repairs the row's nodes on that level in list
-// order -- two replicas of a row can share neighbours, so one after the other keeps the result deterministic
-__global__ void __launch_bounds__(32) hnsw_delete_repair_replicas_kernel(DelArgs a) {
     extern __shared__ __align__(128) uint8_t row[];
     __shared__ DelSmem sm;
     const uint32_t L1 = a.g.num_levels + 1, j = a.rfirst + blockIdx.x / L1, level = blockIdx.x % L1;
@@ -1003,18 +1060,138 @@ __global__ void __launch_bounds__(32) hnsw_delete_relink_kernel(DelArgs a, uint3
     }
 }
 
+// The nodes a delete repairs, as items grouped by row: each item's level-local index per level, what phase A traverses, and
+// the index in the call of the row each item belongs to.  Plain graphs: one item per row with a level-0 node, traversed as
+// that row.  Replica graphs: every node of a deleted row, traversed as the per-item columns.
+struct DelItems {
+    std::vector<uint32_t> loc;         // [items][num_levels+1]
+    std::vector<uint32_t> row_items;   // [rows + 1] the items of the j-th row with items are [row_items[j], row_items[j+1])
+    std::vector<uint32_t> rowlist;     // [items] plain: the item's row; replica: 0..items-1, indexing `cols`
+    std::vector<uint32_t> cols;        // replica graphs: [3][items] vector row, node_id, Metadata row
+    std::vector<uint32_t> out;         // [items] index in the call of the item's row
+};
+
+// delete_embedding for the items (none empty), the one batch loop of both deletes: per batch of max_batch rows the mark, phase
+// A over the batch's items, the repair of each (row, level), then per level the sweep and the relink.  out_status[out[k]] = 2
+// where an Err hit item k.  Every allocation happens before the graph changes; *changed as for the insert.
+static cdb_status delete_items(const HnScoreCtx &sc, HnswBuildState *st, const DelItems &it, uint32_t shortlist, uint32_t max_batch,
+                               uint8_t *out_status, bool *changed, cudaStream_t s, int sms, const char *what) {
+    const uint32_t L1 = st->g.num_levels + 1, ni = (uint32_t)it.rowlist.size(), ng = (uint32_t)it.row_items.size() - 1;
+    const bool replicas = st->replicas;
+    constexpr uint32_t DEL_EF = HNSW_DELETE_EF, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
+    if (max_batch == 0) max_batch = 4096;
+    max_batch = std::max<uint32_t>(1, std::min(max_batch, ng));
+    uint32_t max_items = 0;
+    for (uint32_t j = 0; j < ng; j += max_batch)
+        max_items = std::max(max_items, it.row_items[std::min(ng, j + max_batch)] - it.row_items[j]);
+    // ---- every allocation before the graph changes
+    cdb_status rc;
+    DevAllocs tmp;
+    DelArgs d{};
+    uint32_t *d_rowlist = nullptr, *d_cols = nullptr, *d_loc = nullptr, *d_ri = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
+    uint8_t *failed = nullptr;
+    if ((rc = tmp.get((void **)&d_rowlist, (size_t)ni * 4)) || (replicas && (rc = tmp.get((void **)&d_cols, it.cols.size() * 4))) ||
+        (rc = tmp.get((void **)&d_loc, it.loc.size() * 4)) || (rc = tmp.get((void **)&d_ri, it.row_items.size() * 4)) ||
+        (rc = tmp.get((void **)&z_nodes, (size_t)max_items * L1 * DEL_KEEP * 4)) ||
+        (rc = tmp.get((void **)&z_keys, (size_t)max_items * L1 * DEL_KEEP * 4)) || (rc = tmp.get((void **)&z_n, (size_t)max_items * L1 * 4)) ||
+        (rc = tmp.get((void **)&failed, ni)) || (rc = tmp.get((void **)&d.status, ni)) || (rc = tmp.get((void **)&d.list_n, L1 * 4)))
+        return rc;
+    for (uint32_t L = 0; L < L1; ++L) {
+        const uint32_t cnt = st->g.lv[L].cnt, words = cnt / 32 + 1;
+        if ((rc = tmp.get((void **)&d.dead[L], (size_t)words * 4)) || (rc = tmp.get((void **)&d.touched[L], (size_t)words * 4)) ||
+            (rc = tmp.get((void **)&d.dead_of[L], (size_t)cnt * 4)) || (rc = tmp.get((void **)&d.list[L], (size_t)cnt * 8)) ||
+            (replicas && (rc = tmp.get((void **)&d.tmin[L], (size_t)cnt * 4))))
+            return rc;
+        CDB_CUDA_TRY(cudaMemsetAsync(d.dead[L], 0, (size_t)words * 4, s));
+        CDB_CUDA_TRY(cudaMemsetAsync(d.touched[L], 0, (size_t)words * 4, s));
+        if (replicas) CDB_CUDA_TRY(cudaMemsetAsync(d.tmin[L], 0xFF, (size_t)cnt * 4, s));
+    }
+    const size_t smem = hn_smem_bytes(sc.row_pitch, DEL_EF);
+    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    CDB_ALLOW_SMEM(hnsw_delete_repair_kernel, sc.row_pitch);
+    CDB_ALLOW_SMEM(hnsw_delete_relink_kernel, sc.row_pitch);
+    CDB_CUDA_TRY(cudaMemsetAsync(d.status, 0, ni, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_rowlist, it.rowlist.data(), (size_t)ni * 4, cudaMemcpyHostToDevice, s));
+    if (replicas) CDB_CUDA_TRY(cudaMemcpyAsync(d_cols, it.cols.data(), it.cols.size() * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_loc, it.loc.data(), it.loc.size() * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(d_ri, it.row_items.data(), it.row_items.size() * 4, cudaMemcpyHostToDevice, s));
+    // ---- batches of rows
+    *changed = true;
+    BuildArgs a{};
+    a.g = st->g;
+    a.sc = sc;
+    a.sc.root_row = st->g.root_row;
+    a.ef = DEL_EF;
+    a.shortlist = shortlist;
+    a.zcap = DEL_KEEP;
+    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
+    a.rowlist = d_rowlist;
+    a.replicas = replicas;
+    if (replicas) {
+        // the traversal of an item carries Some(its node_id) as the query id; that id only decides the Pseudo kind
+        // (types.rs:232), which a data row's replicas never have (the pseudo root's row cannot be deleted)
+        a.rl = replica_table(st->md_bits, st->md_mags, st->md_dims);
+        a.rl.row = d_cols;
+        a.rl.id = d_cols + ni;
+        a.rl.base_id = d_cols + ni;
+        a.rl.md = d_cols + 2 * (size_t)ni;
+    }
+    d.g = st->g;
+    d.sc = a.sc;
+    d.loc = d_loc;
+    d.zcap = DEL_KEEP;
+    d.z_nodes = z_nodes; d.z_n = z_n;
+    d.replicas = replicas;
+    d.rl = a.rl;
+    d.row_items = d_ri;
+    const bool ordered = max_batch == 1;
+    for (uint32_t rdone = 0; rdone < ng;) {
+        const uint32_t rb = std::min(max_batch, ng - rdone), first = it.row_items[rdone], count = it.row_items[rdone + rb] - first;
+        a.first = d.first = first;
+        a.count = d.count = count;
+        a.failed = failed + first;
+        d.rfirst = rdone;
+        hnsw_delete_mark_kernel<<<(count * L1 + 127) / 128, 128, 0, s>>>(d);
+        hnsw_build_search_kernel<<<count, HN_THREADS, smem, s>>>(a);
+        hnsw_delete_repair_kernel<<<rb * L1, 32, sc.row_pitch, s>>>(d);
+        g_launch_count.fetch_add(3, std::memory_order_relaxed);
+        for (uint32_t L = 0; L < L1; ++L) {
+            const uint64_t vecs = (uint64_t)a.g.lv[L].cnt * a.g.lv[L].nb / 4 + 1;
+            const uint32_t grid = (uint32_t)std::min<uint64_t>((vecs + 255) / 256, (uint64_t)sms * 8);
+            hnsw_delete_sweep_kernel<<<grid, 256, 0, s>>>(d, L);
+            hnsw_delete_relink_kernel<<<ordered ? 1 : 1024, 32, sc.row_pitch, s>>>(d, L, ordered);
+            g_launch_count.fetch_add(2, std::memory_order_relaxed);
+        }
+        rdone += rb;
+    }
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    std::vector<uint8_t> hf(ni), hs(ni);
+    if (e == cudaSuccess) e = cudaMemcpy(hf.data(), failed, ni, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(hs.data(), d.status, ni, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { set_error(std::string(what) + ": " + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    for (uint32_t k = 0; k < ni; ++k)
+        if (hf[k] || hs[k]) out_status[it.out[k]] = 2;
+    return CDB_OK;
+}
+
+static cdb_status sm_count(int *sms) {
+    int dev = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+    return CDB_OK;
+}
+
 cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
                               uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s) {
-    const GraphDev &gd = *gh.dev;
     const uint32_t L1 = st->g.num_levels + 1;
-    constexpr uint32_t DEL_EF = HNSW_DELETE_EF, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
     // level-local index of every row on every level (level 0 is the row when the level lists rows in order)
     std::vector<uint32_t> loc((size_t)n * L1, HN_EMPTY);
     std::unordered_map<uint32_t, uint32_t> pos;
     for (uint32_t i = 0; i < n; ++i) pos.emplace(rows[i], i);
     for (uint32_t L = 0; L < L1; ++L) {
         const uint32_t cnt = (*gh.cnt)[L];
-        if (L == 0 && (gd.identity_mask & 1u)) {
+        if (L == 0 && (gh.dev->identity_mask & 1u)) {
             for (uint32_t i = 0; i < n; ++i) if (rows[i] < cnt) loc[(size_t)i * L1] = rows[i];
             continue;
         }
@@ -1026,377 +1203,111 @@ cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
         }
     }
     // only rows with a level-0 node take part in the repair (a row appended after the graph was built is not in it)
-    std::vector<uint32_t> grows, gidx, gloc;
+    DelItems it;
     for (uint32_t i = 0; i < n; ++i) {
         out_status[i] = 0;
         if (loc[(size_t)i * L1] == HN_EMPTY) continue;
-        gidx.push_back(i);
-        grows.push_back(rows[i]);
-        gloc.insert(gloc.end(), loc.begin() + (size_t)i * L1, loc.begin() + (size_t)(i + 1) * L1);
+        it.row_items.push_back((uint32_t)it.out.size());
+        it.out.push_back(i);
+        it.rowlist.push_back(rows[i]);
+        it.loc.insert(it.loc.end(), loc.begin() + (size_t)i * L1, loc.begin() + (size_t)(i + 1) * L1);
     }
-    const uint32_t ng = (uint32_t)grows.size();
-    if (!ng) return CDB_OK;
-    if (max_batch == 0) max_batch = 4096;
-    max_batch = std::max<uint32_t>(1, std::min(max_batch, ng));
-    // ---- every allocation before the graph changes
-    cdb_status rc;
-    DevAllocs tmp;
-    DelArgs d{};
-    uint32_t *d_rows = nullptr, *d_loc = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
-    uint8_t *failed = nullptr;
-    if ((rc = tmp.get((void **)&d_rows, (size_t)ng * 4)) || (rc = tmp.get((void **)&d_loc, (size_t)ng * L1 * 4)) ||
-        (rc = tmp.get((void **)&z_nodes, (size_t)max_batch * L1 * DEL_KEEP * 4)) ||
-        (rc = tmp.get((void **)&z_keys, (size_t)max_batch * L1 * DEL_KEEP * 4)) || (rc = tmp.get((void **)&z_n, (size_t)max_batch * L1 * 4)) ||
-        (rc = tmp.get((void **)&failed, ng)) || (rc = tmp.get((void **)&d.status, ng)) || (rc = tmp.get((void **)&d.list_n, L1 * 4)))
-        return rc;
-    for (uint32_t L = 0; L < L1; ++L) {
-        const uint32_t cnt = (*gh.cnt)[L], words = cnt / 32 + 1;
-        if ((rc = tmp.get((void **)&d.dead[L], (size_t)words * 4)) || (rc = tmp.get((void **)&d.touched[L], (size_t)words * 4)) ||
-            (rc = tmp.get((void **)&d.dead_of[L], (size_t)cnt * 4)) || (rc = tmp.get((void **)&d.list[L], (size_t)cnt * 8)))
-            return rc;
-        CDB_CUDA_TRY(cudaMemsetAsync(d.dead[L], 0, (size_t)words * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d.touched[L], 0, (size_t)words * 4, s));
-    }
-    const size_t smem = hn_smem_bytes(sc.row_pitch, DEL_EF);
-    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
-    CDB_ALLOW_SMEM(hnsw_delete_repair_kernel, sc.row_pitch);
-    CDB_ALLOW_SMEM(hnsw_delete_relink_kernel, sc.row_pitch);
-    CDB_CUDA_TRY(cudaMemsetAsync(d.status, 0, ng, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_rows, grows.data(), (size_t)ng * 4, cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_loc, gloc.data(), (size_t)ng * L1 * 4, cudaMemcpyHostToDevice, s));
-    // ---- batches
-    *changed = true;
-    BuildArgs a{};
-    a.g = st->g;
-    a.sc = sc;
-    a.sc.root_row = st->g.root_row;
-    a.ef = DEL_EF;
-    a.shortlist = shortlist;
-    a.zcap = DEL_KEEP;
-    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
-    a.rowlist = d_rows;
-    d.g = st->g;
-    d.sc = a.sc;
-    d.loc = d_loc;
-    d.zcap = DEL_KEEP;
-    d.z_nodes = z_nodes; d.z_n = z_n;
-    int dev = 0, sms = 0;
-    CDB_CUDA_TRY(cudaGetDevice(&dev));
-    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const bool ordered = max_batch == 1;
-    for (uint32_t done = 0; done < ng;) {
-        const uint32_t batch = std::min(max_batch, ng - done);
-        a.first = d.first = done;
-        a.count = d.count = batch;
-        a.failed = failed + done;
-        hnsw_delete_mark_kernel<<<(batch * L1 + 127) / 128, 128, 0, s>>>(d);
-        hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
-        hnsw_delete_repair_kernel<<<batch * L1, 32, sc.row_pitch, s>>>(d);
-        g_launch_count.fetch_add(3, std::memory_order_relaxed);
-        for (uint32_t L = 0; L < L1; ++L) {
-            const uint64_t vecs = (uint64_t)(*gh.cnt)[L] * a.g.lv[L].nb / 4 + 1;
-            const uint32_t grid = (uint32_t)std::min<uint64_t>((vecs + 255) / 256, (uint64_t)sms * 8);
-            hnsw_delete_sweep_kernel<<<grid, 256, 0, s>>>(d, L);
-            hnsw_delete_relink_kernel<<<ordered ? 1 : 1024, 32, sc.row_pitch, s>>>(d, L, ordered);
-            g_launch_count.fetch_add(2, std::memory_order_relaxed);
-        }
-        done += batch;
-    }
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    std::vector<uint8_t> hf(ng), hs(ng);
-    if (e == cudaSuccess) e = cudaMemcpy(hf.data(), failed, ng, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(hs.data(), d.status, ng, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_error(std::string("hnsw delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
-    for (uint32_t j = 0; j < ng; ++j) out_status[gidx[j]] = (hf[j] || hs[j]) ? 2 : 0;
-    return CDB_OK;
+    if (it.out.empty()) return CDB_OK;
+    it.row_items.push_back((uint32_t)it.out.size());
+    int sms = 0;
+    cdb_status rc = sm_count(&sms);
+    return rc ? rc : delete_items(sc, st, it, shortlist, max_batch, out_status, changed, s, sms, "hnsw delete");
 }
 
 // ------------------------------------------------------------------ replica lists (collections with a metadata schema)
-// index_embeddings over the flattened IndexableEmbeddings (vector_store.rs:714-780): host arrays, one entry per node to create.
-// Level layout: [0] main root, [1] pseudo root (both on every level, create_root_node / create_pseudo_root_node), then the
-// created nodes in list order.  The same two kernels as above do the work; level draws come from the caller.
-cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &rh, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
-                                      uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, GraphDev *out_graph,
-                                      std::vector<void *> *out_allocs, std::vector<uint32_t> *out_counts,
-                                      std::vector<const uint32_t *> *out_nr, std::vector<const uint32_t *> *out_ad,
-                                      std::vector<const uint32_t *> *out_ch, ReplicaGraphDev *out_md, std::vector<uint8_t> *out_failed,
-                                      HnswBuildState **out_state, cudaStream_t s) {
-    if (num_levels + 1 > BUILD_MAX_LEVELS) { set_error("build: too many levels"); return CDB_INVALID_PARAMS; }
-    const uint32_t L1 = num_levels + 1, n = rh.n_nodes;
-    std::vector<uint8_t> levels(n);
-    std::vector<std::vector<uint32_t>> members(L1);   // list positions present on each level
-    for (uint32_t t = 0; t < n; ++t) {
-        levels[t] = (uint8_t)std::min<uint32_t>(rh.max_level[t], num_levels);
-        for (uint32_t L = 0; L <= levels[t]; ++L) members[L].push_back(t);
-    }
-    BuildGraph bg{};
-    bg.num_levels = num_levels;
-    bg.root_row = rh.main_root_row;
-    bg.entry = 0;
-    bg.pseudo_entry = 1;
-    metric_key_range(sc.metric, &bg.min_key, &bg.max_key);
-    auto dalloc = [&](void **p, size_t bytes) -> cdb_status {
-        CDB_CUDA_TRY(cudaMalloc(p, bytes ? bytes : 4));
-        out_allocs->push_back(*p);
-        return CDB_OK;
-    };
-    auto upload = [&](const void *src, size_t bytes, void **dst) -> cdb_status {
-        cdb_status rc = dalloc(dst, bytes);
-        if (rc) return rc;
-        if (bytes) CDB_CUDA_TRY(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
-        return CDB_OK;
-    };
-    cdb_status rc;
-    ReplicaDev rl{};
-    void *p = nullptr;
-    if ((rc = upload(rh.row, (size_t)n * 4, &p))) return rc;
-    rl.row = (const uint32_t *)p;
-    if ((rc = upload(rh.node_id, (size_t)n * 4, &p))) return rc;
-    rl.id = (const uint32_t *)p;
-    if ((rc = upload(rh.base_id, (size_t)n * 4, &p))) return rc;
-    rl.base_id = (const uint32_t *)p;
-    if ((rc = upload(rh.md_row, (size_t)n * 4, &p))) return rc;
-    rl.md = (const uint32_t *)p;
-    if ((rc = upload(rh.md_bits, (size_t)rh.n_md * rh.md_dims * 4, &p))) return rc;
-    rl.md_bits = (const int32_t *)p;
-    if ((rc = upload(rh.md_mags, (size_t)rh.n_md * 4, &p))) return rc;
-    rl.md_mags = (const float *)p;
-    rl.M = rh.md_dims;
-    rl.key_one = order_key(CDB_METRIC_COSINE, 0x3F800000u);
-    rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
-    std::vector<const uint32_t *> t_nr(L1), t_ad(L1), t_ch(L1), t_id(L1), t_md(L1);
-    for (uint32_t L = 0; L < L1; ++L) {
-        BuildLevel &l = bg.lv[L];
-        const std::vector<uint32_t> &mem = members[L];
-        l.nb = L == 0 ? nbrs0 : nbrs;
-        l.cnt = 2 + (uint32_t)mem.size();
-        l.app = 2;
-        std::vector<uint32_t> nr(l.cnt), ch(l.cnt, HN_EMPTY), ni(l.cnt), nm(l.cnt), ins(l.cnt, HN_EMPTY);
-        nr[0] = rh.main_root_row; ni[0] = 0xFFFFFFFFu; nm[0] = rh.main_root_md;
-        nr[1] = rh.pseudo_root_row; ni[1] = MD_PSEUDO_ID_LO; nm[1] = rh.pseudo_root_md;
-        if (L > 0) { ch[0] = 0; ch[1] = 1; }
-        uint32_t j = 0;   // position in the level below (both lists ascend)
-        for (uint32_t i = 0; i < mem.size(); ++i) {
-            const uint32_t t = mem[i];
-            nr[2 + i] = rh.row[t]; ni[2 + i] = rh.node_id[t]; nm[2 + i] = rh.md_row[t]; ins[2 + i] = t;
-            if (L > 0) { while (members[L - 1][j] != t) ++j; ch[2 + i] = 2 + j; }
-        }
-        void *d_nr, *d_ch, *d_ni, *d_nm, *d_ins;
-        if ((rc = upload(nr.data(), (size_t)l.cnt * 4, &d_nr)) || (rc = upload(ch.data(), (size_t)l.cnt * 4, &d_ch)) ||
-            (rc = upload(ni.data(), (size_t)l.cnt * 4, &d_ni)) || (rc = upload(nm.data(), (size_t)l.cnt * 4, &d_nm)) ||
-            (rc = upload(ins.data(), (size_t)l.cnt * 4, &d_ins)))
-            return rc;
-        l.node_row = (uint32_t *)d_nr; l.child = (uint32_t *)d_ch;
-        l.node_id = (const uint32_t *)d_ni; l.node_md = (const uint32_t *)d_nm; l.node_ins = (const uint32_t *)d_ins;
-        if ((rc = dalloc((void **)&l.adj, (size_t)l.cnt * l.nb * 4)) || (rc = dalloc((void **)&l.simkey, (size_t)l.cnt * l.nb * 4)) ||
-            (rc = dalloc((void **)&l.lowest_idx, (size_t)l.cnt * 4)) || (rc = dalloc((void **)&l.lowest_key, (size_t)l.cnt * 4)) ||
-            (rc = dalloc((void **)&l.lock, (size_t)l.cnt * 4)))
-            return rc;
-        const uint64_t slots = (uint64_t)l.cnt * l.nb;
-        fill_u32_kernel<<<(uint32_t)((slots + 255) / 256), 256, 0, s>>>(l.adj, HN_EMPTY, slots);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemsetAsync(l.simkey, 0, slots * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(l.lowest_idx, 0, (size_t)l.cnt * 4, s));
-        fill_u32_kernel<<<(l.cnt + 255) / 256, 256, 0, s>>>(l.lowest_key, bg.min_key, l.cnt);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemsetAsync(l.lock, 0, (size_t)l.cnt * 4, s));
-        t_nr[L] = l.node_row; t_ad[L] = l.adj; t_ch[L] = l.child; t_id[L] = l.node_id; t_md[L] = l.node_md;
-    }
-    uint8_t *d_levels = nullptr;
-    if ((rc = upload(levels.data(), n, (void **)&d_levels))) return rc;
-    if (max_batch == 0) max_batch = 4096;
-    max_batch = std::min<uint32_t>(max_batch, std::max<uint32_t>(n, 1));
-    uint32_t *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
-    uint8_t *failed = nullptr;
-    CDB_CUDA_TRY(cudaMalloc(&z_nodes, (size_t)max_batch * L1 * 64 * 4));
-    CDB_CUDA_TRY(cudaMalloc(&z_keys, (size_t)max_batch * L1 * 64 * 4));
-    CDB_CUDA_TRY(cudaMalloc(&z_n, (size_t)max_batch * L1 * 4));
-    CDB_CUDA_TRY(cudaMalloc(&failed, (size_t)std::max<uint32_t>(n, 1)));
-    const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
-    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
-    BuildArgs a{};
-    a.g = bg;
-    a.sc = sc;
-    a.sc.root_row = rh.main_root_row;
-    a.levels = d_levels;
-    a.ef = ef_construction;
-    a.shortlist = shortlist;
-    a.zcap = 64;
-    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
-    a.replicas = true;
-    a.rl = rl;
-    for (uint32_t done = 0; done < n;) {
-        uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, done / 8));
-        batch = std::min<uint32_t>(batch, n - done);
-        a.first = done;
-        a.count = batch;
-        a.failed = failed + done;   // per list position, read back below
-        hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        hnsw_build_link_kernel<<<(batch * 32 + 127) / 128, 128, 0, s>>>(a);
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        done += batch;
-    }
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && out_failed) {
-        out_failed->assign(n, 0);
-        if (n) e = cudaMemcpy(out_failed->data(), failed, n, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(z_nodes); cudaFree(z_keys); cudaFree(z_n); cudaFree(failed);
-    if (e != cudaSuccess) { set_error(std::string("hnsw replica build: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
-    const std::vector<const uint32_t *> *src[5] = {&t_nr, &t_ad, &t_ch, &t_id, &t_md};
-    const uint32_t *tbl[5];
-    for (int t = 0; t < 5; ++t) {
-        void *q = nullptr;
-        if ((rc = upload(src[t]->data(), L1 * sizeof(void *), &q))) return rc;
-        tbl[t] = (const uint32_t *)q;
-    }
-    out_counts->clear();
-    for (uint32_t L = 0; L < L1; ++L) out_counts->push_back(bg.lv[L].cnt);
-    *out_nr = t_nr; *out_ad = t_ad; *out_ch = t_ch;
-    out_graph->num_levels = num_levels;
-    out_graph->nbrs = nbrs;
-    out_graph->nbrs0 = nbrs0;
-    out_graph->entry = 0;
-    out_graph->root_row = rh.main_root_row;
-    out_graph->identity_mask = 0u;
-    out_graph->node_row = reinterpret_cast<const uint32_t *const *>(tbl[0]);
-    out_graph->adj = reinterpret_cast<const uint32_t *const *>(tbl[1]);
-    out_graph->child = reinterpret_cast<const uint32_t *const *>(tbl[2]);
-    out_md->node_id = reinterpret_cast<const uint32_t *const *>(tbl[3]);
-    out_md->node_md = reinterpret_cast<const uint32_t *const *>(tbl[4]);
-    out_md->h_node_id = t_id;
-    out_md->h_node_md = t_md;
-    out_md->md_bits = rl.md_bits;
-    out_md->md_mags = rl.md_mags;
-    out_md->md_dims = rh.md_dims;
-    out_md->pseudo_entry = 1;
-    // the builder's state stays with the graph, so hnsw_insert_replicas_device can continue where this build stopped
-    std::unique_ptr<HnswBuildState> st(new HnswBuildState());
-    st->g = bg;
-    for (uint32_t L = 0; L < L1; ++L) st->cap[L] = bg.lv[L].cnt;
-    st->replicas = true;
-    st->n_list = n;
-    st->pseudo_root_row = rh.pseudo_root_row;
-    st->n_md = rh.n_md;
-    st->md_dims = rh.md_dims;
-    st->md_bits = rl.md_bits;
-    st->md_mags = rl.md_mags;
-    *out_state = st.release();
-    return CDB_OK;
-}
-
-// index_embeddings over more IndexableEmbeddings of a collection with a metadata schema, into the graph a replica build made
-// (and earlier calls grew).  New nodes are appended to every level they reach, behind the existing ones in list order, with
-// node_ins continuing the list positions, so build_local's binary search and both kernels run unchanged; ReplicaDev is
-// offset so that it is indexed by those global positions.  Batches hold max(1, min(max_batch, nodes already linked / 8)).
-// Every allocation (the list, the batch buffers, the grown Metadata table, the grown level arrays) happens before the graph
-// changes; the table replaces the old one only once the insert has succeeded.
-cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const ReplicaHost &rh,
-                                       uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed,
-                                       const int32_t **md_bits, const float **md_mags, bool *changed, cudaStream_t s) {
-    const uint32_t L1 = st->g.num_levels + 1, n = rh.n_nodes, first = st->n_list, M = st->md_dims;
-    std::vector<uint8_t> levels(n);
-    std::vector<std::vector<uint32_t>> rows(L1), child(L1);
-    ReplicaCols cols;
-    cols.id.resize(L1); cols.md.resize(L1); cols.ins.resize(L1);
-    std::vector<std::vector<uint32_t>> members(L1);   // new list indices present on each level
-    for (uint32_t t = 0; t < n; ++t) {
-        levels[t] = (uint8_t)std::min<uint32_t>(rh.max_level[t], st->g.num_levels);
-        for (uint32_t L = 0; L <= levels[t]; ++L) {
-            members[L].push_back(t);
-            rows[L].push_back(rh.row[t]);
-            cols.id[L].push_back(rh.node_id[t]);
-            cols.md[L].push_back(rh.md_row[t]);
-            cols.ins[L].push_back(first + t);
-        }
-    }
-    for (uint32_t L = 1; L < L1; ++L) {
-        uint32_t j = 0;   // position among the nodes appended one level down (both lists ascend)
-        for (uint32_t t : members[L]) {
-            while (members[L - 1][j] != t) ++j;
-            child[L].push_back(st->g.lv[L - 1].cnt + j);
-        }
-    }
-    if (max_batch == 0) max_batch = 4096;
-    max_batch = std::max<uint32_t>(1, std::min(max_batch, n));
-    // ---- every allocation before the graph changes
+// index_embeddings over the flattened IndexableEmbeddings (vector_store.rs:714-780): host arrays, one entry per node to create,
+// into the replica graph of `st` behind the nodes earlier calls created.  Level layout: [0] main root, [1] pseudo root (both
+// on every level, create_root_node / create_pseudo_root_node), then the created nodes in list order, with node_ins continuing
+// the list positions, so build_local's binary search and both kernels run unchanged; ReplicaDev is offset so that it is indexed
+// by those global positions.  Level draws come from the caller.  Every allocation (the list, the batch buffers, the grown
+// Metadata table, the grown level arrays) happens before the graph changes; the table replaces the old one only once the
+// insert has succeeded.
+static cdb_status insert_replica_list(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState &st, const ReplicaHost &rh,
+                                      uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed, bool *changed,
+                                      cudaStream_t s, const char *what) {
+    const uint32_t n = rh.n_nodes, first = st.n_list, M = st.md_dims;
+    const InsertPlan p = plan_replicas(st, rh);
     cdb_status rc;
     DevAllocs tmp, table;
-    uint32_t *d_list = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
-    uint8_t *d_levels = nullptr, *failed = nullptr;
-    if ((rc = tmp.get((void **)&d_list, (size_t)n * 4 * 4)) || (rc = tmp.get((void **)&d_levels, n)) || (rc = tmp.get((void **)&failed, n)) ||
-        (rc = tmp.get((void **)&z_nodes, (size_t)max_batch * L1 * 64 * 4)) || (rc = tmp.get((void **)&z_keys, (size_t)max_batch * L1 * 64 * 4)) ||
-        (rc = tmp.get((void **)&z_n, (size_t)max_batch * L1 * 4)))
-        return rc;
-    const uint32_t n_md = st->n_md + rh.n_md;
+    uint32_t *d_list = nullptr;
+    if ((rc = tmp.get((void **)&d_list, (size_t)n * 4 * 4))) return rc;
+    const uint32_t n_md = st.n_md + rh.n_md;
     int32_t *new_bits = nullptr;
     float *new_mags = nullptr;
     if (rh.n_md) {   // the grown table: the old rows, then the new ones
         if ((rc = table.get((void **)&new_bits, (size_t)n_md * M * 4)) || (rc = table.get((void **)&new_mags, (size_t)n_md * 4))) return rc;
-        CDB_CUDA_TRY(cudaMemcpyAsync(new_bits, st->md_bits, (size_t)st->n_md * M * 4, cudaMemcpyDeviceToDevice, s));
-        CDB_CUDA_TRY(cudaMemcpyAsync(new_bits + (size_t)st->n_md * M, rh.md_bits, (size_t)rh.n_md * M * 4, cudaMemcpyHostToDevice, s));
-        CDB_CUDA_TRY(cudaMemcpyAsync(new_mags, st->md_mags, (size_t)st->n_md * 4, cudaMemcpyDeviceToDevice, s));
-        CDB_CUDA_TRY(cudaMemcpyAsync(new_mags + st->n_md, rh.md_mags, (size_t)rh.n_md * 4, cudaMemcpyHostToDevice, s));
+        if (st.n_md) {
+            CDB_CUDA_TRY(cudaMemcpyAsync(new_bits, st.md_bits, (size_t)st.n_md * M * 4, cudaMemcpyDeviceToDevice, s));
+            CDB_CUDA_TRY(cudaMemcpyAsync(new_mags, st.md_mags, (size_t)st.n_md * 4, cudaMemcpyDeviceToDevice, s));
+        }
+        CDB_CUDA_TRY(cudaMemcpyAsync(new_bits + (size_t)st.n_md * M, rh.md_bits, (size_t)rh.n_md * M * 4, cudaMemcpyHostToDevice, s));
+        CDB_CUDA_TRY(cudaMemcpyAsync(new_mags + st.n_md, rh.md_mags, (size_t)rh.n_md * 4, cudaMemcpyHostToDevice, s));
     }
     const uint32_t *src[4] = {rh.row, rh.node_id, rh.base_id, rh.md_row};
     for (int c = 0; c < 4; ++c) CDB_CUDA_TRY(cudaMemcpyAsync(d_list + (size_t)c * n, src[c], (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_levels, levels.data(), n, cudaMemcpyHostToDevice, s));
-    const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
-    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
-    if ((rc = append_levels(*st, gh, rows, child, ~0ull, changed, s, &cols))) return rc;
-    // ---- batches
-    BuildArgs a{};
-    a.g = st->g;
-    a.sc = sc;
-    a.sc.root_row = st->g.root_row;
-    a.levels = d_levels;
-    a.lv_first = first;
-    a.ef = ef_construction;
-    a.shortlist = shortlist;
-    a.zcap = 64;
-    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
-    a.replicas = true;
-    a.rl.row = d_list - first;   // indexed by global list position: entry t of this call is position first + t
-    a.rl.id = d_list + n - first;
-    a.rl.base_id = d_list + 2 * (size_t)n - first;
-    a.rl.md = d_list + 3 * (size_t)n - first;
-    a.rl.md_bits = rh.n_md ? new_bits : st->md_bits;
-    a.rl.md_mags = rh.n_md ? new_mags : st->md_mags;
-    a.rl.M = M;
-    a.rl.key_one = order_key(CDB_METRIC_COSINE, 0x3F800000u);
-    a.rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
-    for (uint32_t done = 0; done < n;) {
-        uint32_t batch = std::max<uint32_t>(1, std::min<uint32_t>(max_batch, (uint32_t)(((uint64_t)first + done) / 8)));
-        batch = std::min<uint32_t>(batch, n - done);
-        a.first = first + done;
-        a.count = batch;
-        a.failed = failed + done;
-        hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        hnsw_build_link_kernel<<<(batch * 32 + 127) / 128, 128, 0, s>>>(a);
-        g_launch_count.fetch_add(1, std::memory_order_relaxed);
-        done += batch;
-    }
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    if (e == cudaSuccess && out_failed) e = cudaMemcpy(out_failed, failed, n, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_error(std::string("hnsw replica insert: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+    ReplicaDev rl = replica_table(rh.n_md ? new_bits : st.md_bits, rh.n_md ? new_mags : st.md_mags, M);
+    rl.row = d_list - first;   // indexed by global list position: entry t of this call is position first + t
+    rl.id = d_list + n - first;
+    rl.base_id = d_list + 2 * (size_t)n - first;
+    rl.md = d_list + 3 * (size_t)n - first;
+    if ((rc = insert_planned(sc, gh, st, p, first, first, ef_construction, shortlist, max_batch, ~0ull, out_failed, changed, s, nullptr,
+                             &rl, what)))
+        return rc;
     // ---- the grown table replaces the old one
     if (rh.n_md) {
-        for (const void *old : {(const void *)st->md_bits, (const void *)st->md_mags}) {
+        for (const void *old : {(const void *)st.md_bits, (const void *)st.md_mags}) {
             auto it = std::find(gh.allocs->begin(), gh.allocs->end(), old);
             if (it != gh.allocs->end()) { gh.allocs->erase(it); cudaFree(const_cast<void *>(old)); }
         }
         gh.allocs->insert(gh.allocs->end(), table.p.begin(), table.p.end());
         table.release();
-        st->md_bits = new_bits;
-        st->md_mags = new_mags;
-        st->n_md = n_md;
+        st.md_bits = new_bits;
+        st.md_mags = new_mags;
+        st.n_md = n_md;
     }
-    st->n_list += n;
+    st.n_list += n;
+    return CDB_OK;
+}
+
+// as hnsw_build_device: the two roots on every level, then the whole list through the insert path, which installs the
+// Metadata table
+cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &rh, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
+                                      uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, const GraphHost &gh,
+                                      uint8_t *out_failed, const int32_t **md_bits, const float **md_mags, HnswBuildState **out_state,
+                                      cudaStream_t s) {
+    std::unique_ptr<HnswBuildState> st;
+    cdb_status rc = new_graph(sc.metric, num_levels, nbrs, nbrs0, rh.main_root_row, 0, 0u, gh, st);
+    if (rc) return rc;
+    st->replicas = true;
+    st->g.pseudo_entry = 1;
+    st->pseudo_root_row = rh.pseudo_root_row;
+    st->md_dims = rh.md_dims;
+    const uint32_t L1 = num_levels + 1;
+    bool changed = false;
+    const std::vector<std::vector<uint32_t>> rows(L1, {rh.main_root_row, rh.pseudo_root_row}), child(L1, {0u, 1u});
+    ReplicaCols cols;
+    cols.id.assign(L1, {0xFFFFFFFFu, MD_PSEUDO_ID_LO});
+    cols.md.assign(L1, {rh.main_root_md, rh.pseudo_root_md});
+    cols.ins.assign(L1, {HN_EMPTY, HN_EMPTY});
+    if ((rc = append_levels(*st, gh, rows, child, ~0ull, &changed, s, &cols)) ||
+        (rc = insert_replica_list(sc, gh, *st, rh, ef_construction, shortlist, max_batch, out_failed, &changed, s, "hnsw replica build")))
+        return rc;
+    *md_bits = st->md_bits;
+    *md_mags = st->md_mags;
+    *out_state = st.release();
+    return CDB_OK;
+}
+
+cdb_status hnsw_insert_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const ReplicaHost &rh,
+                                       uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, uint8_t *out_failed,
+                                       const int32_t **md_bits, const float **md_mags, bool *changed, cudaStream_t s) {
+    cdb_status rc = insert_replica_list(sc, gh, *st, rh, ef_construction, shortlist, max_batch, out_failed, changed, s, "hnsw replica insert");
+    if (rc) return rc;
     *md_bits = st->md_bits;
     *md_mags = st->md_mags;
     return CDB_OK;
@@ -1429,13 +1340,11 @@ __global__ void hnsw_delete_find_kernel(BuildLevel l, uint32_t level, const uint
 cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
                                        uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s) {
     const uint32_t L1 = st->g.num_levels + 1;
-    constexpr uint32_t DEL_EF = HNSW_DELETE_EF, DEL_KEEP = 100;   // the reference's literal ef and final_len (vector_store.rs:1194, 1247)
     for (uint32_t i = 0; i < n; ++i) out_status[i] = 0;
     if (!n) return CDB_OK;
     cdb_status rc;
-    int dev = 0, sms = 0;
-    CDB_CUDA_TRY(cudaGetDevice(&dev));
-    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int sms = 0;
+    if ((rc = sm_count(&sms))) return rc;
     // ---- the rows' nodes, found on the device (a replica graph has no level that lists rows in order)
     const uint32_t n_rows = *std::max_element(rows, rows + n) + 1;
     DevAllocs look;
@@ -1475,113 +1384,23 @@ cdb_status hnsw_delete_replicas_device(const HnScoreCtx &sc, const GraphHost &gh
         return px != py ? px < py : x.ins < y.ins;
     });
     const uint32_t ni = (uint32_t)items.size();
+    if (!ni) return CDB_OK;
     std::unordered_map<uint32_t, uint32_t> item_of;   // list position -> item
-    std::vector<uint32_t> loc((size_t)ni * L1, HN_EMPTY), cols((size_t)ni * 3), iota(ni), item_pos(ni), row_items;
+    DelItems it;
+    it.loc.assign((size_t)ni * L1, HN_EMPTY);
+    it.cols.resize((size_t)ni * 3);
+    it.rowlist.resize(ni);
+    it.out.resize(ni);
     for (uint32_t k = 0; k < ni; ++k) {
         item_of.emplace(items[k].ins, k);
-        cols[k] = items[k].row; cols[ni + k] = items[k].id; cols[2 * (size_t)ni + k] = items[k].md;
-        iota[k] = k;
-        item_pos[k] = pos[items[k].row];
-        if (!k || item_pos[k] != item_pos[k - 1]) row_items.push_back(k);
+        it.cols[k] = items[k].row; it.cols[ni + k] = items[k].id; it.cols[2 * (size_t)ni + k] = items[k].md;
+        it.rowlist[k] = k;
+        it.out[k] = pos[items[k].row];
+        if (!k || it.out[k] != it.out[k - 1]) it.row_items.push_back(k);
     }
-    for (const DelHit &h : hits) loc[(size_t)item_of.at(h.ins) * L1 + h.level] = h.node;
-    const uint32_t ng = (uint32_t)row_items.size();   // rows with nodes; the others are only marked
-    row_items.push_back(ni);
-    if (max_batch == 0) max_batch = 4096;
-    max_batch = std::max<uint32_t>(1, std::min(max_batch, ng));
-    uint32_t max_items = 0;
-    for (uint32_t j = 0; j < ng; j += max_batch)
-        max_items = std::max(max_items, row_items[std::min(ng, j + max_batch)] - row_items[j]);
-    // ---- every allocation before the graph changes
-    DevAllocs tmp;
-    DelArgs d{};
-    uint32_t *d_cols = nullptr, *d_iota = nullptr, *d_loc = nullptr, *d_ri = nullptr, *z_nodes = nullptr, *z_keys = nullptr, *z_n = nullptr;
-    uint8_t *failed = nullptr;
-    if ((rc = tmp.get((void **)&d_cols, cols.size() * 4)) || (rc = tmp.get((void **)&d_iota, (size_t)ni * 4)) ||
-        (rc = tmp.get((void **)&d_loc, loc.size() * 4)) || (rc = tmp.get((void **)&d_ri, row_items.size() * 4)) ||
-        (rc = tmp.get((void **)&z_nodes, (size_t)max_items * L1 * DEL_KEEP * 4)) ||
-        (rc = tmp.get((void **)&z_keys, (size_t)max_items * L1 * DEL_KEEP * 4)) || (rc = tmp.get((void **)&z_n, (size_t)max_items * L1 * 4)) ||
-        (rc = tmp.get((void **)&failed, ni)) || (rc = tmp.get((void **)&d.status, ni)) || (rc = tmp.get((void **)&d.list_n, L1 * 4)))
-        return rc;
-    for (uint32_t L = 0; L < L1; ++L) {
-        const uint32_t cnt = st->g.lv[L].cnt, words = cnt / 32 + 1;
-        if ((rc = tmp.get((void **)&d.dead[L], (size_t)words * 4)) || (rc = tmp.get((void **)&d.touched[L], (size_t)words * 4)) ||
-            (rc = tmp.get((void **)&d.dead_of[L], (size_t)cnt * 4)) || (rc = tmp.get((void **)&d.list[L], (size_t)cnt * 8)) ||
-            (rc = tmp.get((void **)&d.tmin[L], (size_t)cnt * 4)))
-            return rc;
-        CDB_CUDA_TRY(cudaMemsetAsync(d.dead[L], 0, (size_t)words * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d.touched[L], 0, (size_t)words * 4, s));
-        CDB_CUDA_TRY(cudaMemsetAsync(d.tmin[L], 0xFF, (size_t)cnt * 4, s));
-    }
-    const size_t smem = hn_smem_bytes(sc.row_pitch, DEL_EF);
-    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
-    CDB_ALLOW_SMEM(hnsw_delete_repair_replicas_kernel, sc.row_pitch);
-    CDB_ALLOW_SMEM(hnsw_delete_relink_kernel, sc.row_pitch);
-    CDB_CUDA_TRY(cudaMemsetAsync(d.status, 0, ni, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_cols, cols.data(), cols.size() * 4, cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_iota, iota.data(), (size_t)ni * 4, cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_loc, loc.data(), loc.size() * 4, cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(d_ri, row_items.data(), row_items.size() * 4, cudaMemcpyHostToDevice, s));
-    // ---- batches of rows
-    *changed = true;
-    BuildArgs a{};
-    a.g = st->g;
-    a.sc = sc;
-    a.sc.root_row = st->g.root_row;
-    a.ef = DEL_EF;
-    a.shortlist = shortlist;
-    a.zcap = DEL_KEEP;
-    a.z_nodes = z_nodes; a.z_keys = z_keys; a.z_n = z_n;
-    a.rowlist = d_iota;
-    a.replicas = true;
-    // the traversal of an item carries Some(its node_id) as the query id; that id only decides the Pseudo kind (types.rs:232),
-    // which a data row's replicas never have (the pseudo root's row cannot be deleted)
-    a.rl.row = d_cols;
-    a.rl.id = d_cols + ni;
-    a.rl.base_id = d_cols + ni;
-    a.rl.md = d_cols + 2 * (size_t)ni;
-    a.rl.md_bits = st->md_bits;
-    a.rl.md_mags = st->md_mags;
-    a.rl.M = st->md_dims;
-    a.rl.key_one = order_key(CDB_METRIC_COSINE, 0x3F800000u);
-    a.rl.key_minus_one = order_key(CDB_METRIC_COSINE, 0xBF800000u);
-    d.g = st->g;
-    d.sc = a.sc;
-    d.loc = d_loc;
-    d.zcap = DEL_KEEP;
-    d.z_nodes = z_nodes; d.z_n = z_n;
-    d.replicas = true;
-    d.rl = a.rl;
-    d.row_items = d_ri;
-    const bool ordered = max_batch == 1;
-    for (uint32_t rdone = 0; rdone < ng;) {
-        const uint32_t rb = std::min(max_batch, ng - rdone), first = row_items[rdone], count = row_items[rdone + rb] - first;
-        a.first = d.first = first;
-        a.count = d.count = count;
-        a.failed = failed + first;
-        d.rfirst = rdone;
-        hnsw_delete_mark_kernel<<<(count * L1 + 127) / 128, 128, 0, s>>>(d);
-        hnsw_build_search_kernel<<<count, HN_THREADS, smem, s>>>(a);
-        hnsw_delete_repair_replicas_kernel<<<rb * L1, 32, sc.row_pitch, s>>>(d);
-        g_launch_count.fetch_add(3, std::memory_order_relaxed);
-        for (uint32_t L = 0; L < L1; ++L) {
-            const uint64_t vecs = (uint64_t)a.g.lv[L].cnt * a.g.lv[L].nb / 4 + 1;
-            const uint32_t grid = (uint32_t)std::min<uint64_t>((vecs + 255) / 256, (uint64_t)sms * 8);
-            hnsw_delete_sweep_kernel<<<grid, 256, 0, s>>>(d, L);
-            hnsw_delete_relink_kernel<<<ordered ? 1 : 1024, 32, sc.row_pitch, s>>>(d, L, ordered);
-            g_launch_count.fetch_add(2, std::memory_order_relaxed);
-        }
-        rdone += rb;
-    }
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e == cudaSuccess) e = cudaGetLastError();
-    std::vector<uint8_t> hf(ni), hs(ni);
-    if (e == cudaSuccess) e = cudaMemcpy(hf.data(), failed, ni, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(hs.data(), d.status, ni, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_error(std::string("hnsw replica delete: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
-    for (uint32_t k = 0; k < ni; ++k)
-        if (hf[k] || hs[k]) out_status[item_pos[k]] = 2;
-    return CDB_OK;
+    for (const DelHit &h : hits) it.loc[(size_t)item_of.at(h.ins) * L1 + h.level] = h.node;
+    it.row_items.push_back(ni);
+    return delete_items(sc, st, it, shortlist, max_batch, out_status, changed, s, sms, "hnsw replica delete");
 }
 
 // ------------------------------------------------------------------ builder state of a loaded replica graph

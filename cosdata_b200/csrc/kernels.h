@@ -210,7 +210,8 @@ cdb_status hnsw_insert_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
 // deleted-row bitmaps (d_deleted device, h_deleted host, bit r = row r; null = none): build and insert skip those rows
 // (no upper-level nodes, not linked, out_failed 2)
 // cdb_index_delete_rows: delete_embedding for the distinct rows rows[0..n) with the deviations D1-D4 (DESIGN.md section 4);
-// out_status[i] = 0, or 2 where an Err stopped relinks.  *changed as for the insert.
+// out_status[i] = 0, or 2 where an Err stopped relinks.  *changed as for the insert.  The rows' nodes are looked up on the
+// host; the repair is the batch loop hnsw_delete_replicas_device runs too.
 cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBuildState *st, const uint32_t *rows, uint32_t n,
                               uint32_t shortlist, uint32_t max_batch, uint8_t *out_status, bool *changed, cudaStream_t s);
 // similarity keys of every slot of `level` ([cnt*nb], device)
@@ -231,20 +232,15 @@ struct ReplicaHost {
     const float *md_mags;
     uint32_t main_root_row, main_root_md, pseudo_root_row, pseudo_root_md;
 };
-struct ReplicaGraphDev {
-    const uint32_t *const *node_id, *const *node_md;   // device tables of device arrays
-    std::vector<const uint32_t *> h_node_id, h_node_md;   // the same per-level device pointers on the host
-    const int32_t *md_bits;
-    const float *md_mags;
-    uint32_t md_dims, pseudo_entry;
-};
-// out_state: the builder's state of the replica graph, which hnsw_insert_replicas_device continues from
+// cdb_index_build_graph_replicas: the main root (row main_root_row) and the pseudo root on every level, then the nodes of `rh`
+// inserted as hnsw_insert_replicas_device inserts them.  gh carries the node_id / node_md tables (id_tbl / md_tbl, allocated by
+// the caller); the node_row / adj / child tables are allocated here.  out_failed[n_nodes] may be NULL.  On success
+// *md_bits / *md_mags point at the Metadata table and out_state is the builder's state of the replica graph, which
+// hnsw_insert_replicas_device continues from.
 cdb_status hnsw_build_replicas_device(const HnScoreCtx &sc, const ReplicaHost &rh, uint32_t num_levels, uint32_t nbrs, uint32_t nbrs0,
-                                      uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, GraphDev *out_graph,
-                                      std::vector<void *> *out_allocs, std::vector<uint32_t> *out_counts,
-                                      std::vector<const uint32_t *> *out_nr, std::vector<const uint32_t *> *out_ad,
-                                      std::vector<const uint32_t *> *out_ch, ReplicaGraphDev *out_md, std::vector<uint8_t> *out_failed,
-                                      HnswBuildState **out_state, cudaStream_t s);
+                                      uint32_t ef_construction, uint32_t shortlist, uint32_t max_batch, const GraphHost &gh,
+                                      uint8_t *out_failed, const int32_t **md_bits, const float **md_mags, HnswBuildState **out_state,
+                                      cudaStream_t s);
 // true (and the pseudo root's row, the Metadata table's row count) when `st` is the state of a replica build
 bool hnsw_state_replica_info(const HnswBuildState *st, uint32_t *pseudo_root_row, uint32_t *n_md);
 // cdb_index_insert_graph_replicas: the nodes of `rh` (n_nodes entries; row already mapped to the pseudo root's row where the
