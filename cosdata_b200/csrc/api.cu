@@ -978,7 +978,8 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
         if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->q_codes.as<float>(),
                                     pitch / 4, sc->q_mags.as<float>(), nq, sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(),
-                                    cap, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr, sc->cur_keys, ix->del_dev())))
+                                    cap, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr, sc->cur_keys, ix->del_dev(),
+                                    /*dedup=*/true)))
             return rc;
         if ((rc = select_fallback_device(sc->cand_cnt.as<uint32_t>(), cap, sc->q_mags.as<float>(), nq, sc->qsel.as<uint32_t>(), flags, s)))
             return rc;
@@ -1237,6 +1238,11 @@ cdb_status cdb_rerank_f32(cdb_index *ix, const float *query, const uint32_t *can
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_REQUIRE(ix->d_raw, "re-rank needs raw f32 rows (F32 storage or keep_raw_f32)");
     CDB_REQUIRE(ix->raw_missing == 0, "rows appended as codes still lack their raw f32 rows (cdb_index_set_raw_f32 / cdb_index_fill_raw_from_itoe)");
+    for (uint32_t i = 0; i < n; ++i)
+        if (cand_ids[i] < ix->desc.id_base || cand_ids[i] - ix->desc.id_base >= ix->size) {
+            set_error("rerank: candidate id " + std::to_string(cand_ids[i]) + " is not a row of the index");
+            return CDB_INVALID_PARAMS;
+        }
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     const cdb_index_desc &d = ix->desc;
     Lease l;
@@ -1259,7 +1265,8 @@ cdb_status cdb_rerank_f32(cdb_index *ix, const float *query, const uint32_t *can
         return rc;
     if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->q_codes.as<float>(), qpitch,
                                 sc->q_mags.as<float>(), 1, sc->misc.as<uint32_t>(), nullptr, n, k, d.id_base, sc->io_ids.as<uint32_t>(),
-                                sc->io_scores.as<float>(), sc->io_counts.as<uint32_t>(), s)))
+                                sc->io_scores.as<float>(), sc->io_counts.as<uint32_t>(), s, nullptr, nullptr, nullptr,
+                                /*dedup=*/false)))
         return rc;
     CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, sc->io_ids.p, (size_t)k * 4, cudaMemcpyDeviceToHost, s));
     CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, sc->io_scores.p, (size_t)k * 4, cudaMemcpyDeviceToHost, s));

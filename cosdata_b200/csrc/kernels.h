@@ -64,7 +64,8 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
                              uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s,
                              const uint32_t *d_labels = nullptr,    // labels: ids reported instead of the candidate ids (replica ids)
                              uint64_t *d_out_keys = nullptr,        // [nq][k] packed selection keys as well (shard merge)
-                             const uint32_t *d_deleted = nullptr);  // deleted-row bitmap: such candidates are dropped
+                             const uint32_t *d_deleted = nullptr,   // deleted-row bitmap: such candidates are dropped
+                             bool dedup = true);                    // report a repeated candidate once (<= 64 repeats)
 // largest dimension rerank_f32_device accepts for any candidate count (its query and key buffer share 200 KB of smem)
 uint32_t rerank_f32_max_dim();
 

@@ -85,8 +85,10 @@ cdb_status score_ids_device(int metric, int st, uint32_t dim, const uint8_t *d_q
 // no zero check (vector_store.rs:427-429); sort by total_cmp desc, truncate k.
 // The candidate list is consumed in chunks through a fixed 2048-key buffer (best keys of the earlier chunks stay at
 // the front), so shared memory does not grow with the list and long prefilter lists cost time, not occupancy.
-// A candidate id may appear twice (degenerate rows are pre-seeded on prefilter lists and may be emitted again):
-// equal keys are adjacent after the sort and are reported once.
+// With `dedup`, a candidate id may appear twice (degenerate rows are pre-seeded on prefilter lists and may be emitted
+// again): equal keys are adjacent after the sort and are reported once -- at most RERANK_DUP of them, which bounds the
+// copies a prefilter list can hold.  Without it every candidate is reported, copies included, as finalize_ann_results
+// reports them.
 constexpr int RERANK_THREADS = 256;
 constexpr uint32_t RERANK_BUF = 2048;
 constexpr uint32_t RERANK_DUP = 64;    // duplicates tolerated inside the kept window
@@ -115,7 +117,7 @@ __global__ void __launch_bounds__(RERANK_THREADS) rerank_f32_kernel(
     uint32_t dim, const float *__restrict__ q, uint32_t q_pitch_elems, const float *__restrict__ qmags,
     const uint32_t *__restrict__ cand, const uint32_t *__restrict__ cand_counts, uint32_t cand_stride, uint32_t k, uint32_t id_base,
     uint32_t *__restrict__ out_ids, float *__restrict__ out_scores, uint32_t *__restrict__ out_counts,
-    const uint32_t *__restrict__ labels, uint64_t *__restrict__ out_keys, const uint32_t *__restrict__ deleted) {
+    const uint32_t *__restrict__ labels, uint64_t *__restrict__ out_keys, const uint32_t *__restrict__ deleted, bool dedup) {
     extern __shared__ __align__(16) uint8_t smem[];
     float *qs = reinterpret_cast<float *>(smem);
     uint64_t *keys = reinterpret_cast<uint64_t *>(qs + round_up(dim, 4));
@@ -164,7 +166,7 @@ __global__ void __launch_bounds__(RERANK_THREADS) rerank_f32_kernel(
     } while (pos < ncand);
     // equal keys (same score, same id) are duplicates of one candidate: report the first of each run
     const uint32_t lim = min(n, window);
-    for (uint32_t i = 1 + threadIdx.x; i < lim; i += blockDim.x)
+    for (uint32_t i = 1 + threadIdx.x; dedup && i < lim; i += blockDim.x)
         if (keys[i] != 0ull && keys[i] == keys[i - 1]) {
             const uint32_t p = atomicAdd(&ndup, 1u);
             if (p < RERANK_DUP) duppos[p] = i;
@@ -195,7 +197,7 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
                              uint32_t dim, const float *d_q, uint32_t q_pitch_elems, const float *d_qmags, uint32_t nq,
                              const uint32_t *d_cand, const uint32_t *d_cand_counts, uint32_t ncand, uint32_t k, uint32_t id_base,
                              uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s,
-                             const uint32_t *d_labels, uint64_t *d_out_keys, const uint32_t *d_deleted) {
+                             const uint32_t *d_labels, uint64_t *d_out_keys, const uint32_t *d_deleted, bool dedup) {
     if (!nq) return CDB_OK;
     if (k == 0 || k > 1024) { set_error("rerank: k must be in 1..1024"); return CDB_INVALID_PARAMS; }
     uint32_t pcap = 64;
@@ -206,7 +208,7 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
     CDB_ALLOW_SMEM(rerank_f32_kernel, smem);
     rerank_f32_kernel<<<nq, RERANK_THREADS, smem, s>>>(d_raw, pitch_elems, d_raw_mags, n_rows, dim, d_q, q_pitch_elems,
                                                         d_qmags, d_cand, d_cand_counts, ncand, k, id_base, d_out_ids, d_out_scores, d_out_counts, d_labels, d_out_keys,
-                                                        d_deleted);
+                                                        d_deleted, dedup);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }

@@ -25,6 +25,13 @@ __device__ inline uint32_t quant_u8(float x, float lo, float hi) {
     float t = __fmul_rn(__fdiv_rn(__fsub_rn(c, lo), __fsub_rn(hi, lo)), 255.0f);
     return rust_as_u8(t);
 }
+// half::f16::from_f32 (scalar.rs:40): round to nearest even; a NaN keeps its sign and top payload bits with the quiet bit
+// set, where __float2half_rn would return the canonical 0x7FFF
+__device__ inline uint16_t f32_to_f16_bits(float x) {
+    const uint32_t u = __float_as_uint(x);
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)(((u >> 16) & 0x8000u) | 0x7E00u | ((u & 0x7FFFFFu) >> 13));
+    return __half_as_ushort(__float2half_rn(x));
+}
 // low `r` bits of floor((x+1)/step) (to_float_flag)
 __device__ inline uint32_t quant_sub(float x, int r) {
     float step = __fdiv_rn(2.0f, (float)(1u << r));
@@ -81,8 +88,8 @@ __global__ void quantize_codes_kernel(Src src, uint64_t n, uint32_t dim, int st,
         break;
     }
     case CDB_ST_F16: {
-        __half *h = reinterpret_cast<__half *>(out) + c0;
-        for (uint32_t e = 0; e < cnt; ++e) h[e] = __float2half_rn(v[e]);
+        uint16_t *h = reinterpret_cast<uint16_t *>(out) + c0;
+        for (uint32_t e = 0; e < cnt; ++e) h[e] = f32_to_f16_bits(v[e]);
         break;
     }
     case CDB_ST_BF16: {

@@ -327,15 +327,24 @@ static cdb_status launch_scan(const ScanArgs &a, uint32_t sel_grid, cudaStream_t
     }
     size_t smem = scan_smem(QB, a.row_pitch, a.k);
     const bool f32path = (a.st == CDB_ST_F32 && a.metric == CDB_METRIC_COSINE);
-    if (f32path) {
-        auto kern = scan_f32_kernel<QB, 2>;
-        CDB_ALLOW_SMEM(kern, smem);
-        kern<<<grid, SCAN_THREADS, smem, s>>>(a);
-    } else {
-        auto kern = scan_generic_kernel<QB>;
-        CDB_ALLOW_SMEM(kern, smem);
-        kern<<<grid, SCAN_THREADS, smem, s>>>(a);
+    const void *kern = f32path ? reinterpret_cast<const void *>(scan_f32_kernel<QB, 2>)
+                               : reinterpret_cast<const void *>(scan_generic_kernel<QB>);
+    // the query rows and the candidate buffers live in shared memory: past the device's per-block limit no plan exists
+    // (the launch would fail), so the search is refused
+    int dev = 0, optin = 0;
+    CDB_CUDA_TRY(cudaGetDevice(&dev));
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa;
+    CDB_CUDA_TRY(cudaFuncGetAttributes(&fa, kern));
+    if (smem + fa.sharedSizeBytes > (size_t)optin) {
+        set_error("exact scan: dimension " + std::to_string(a.dim) + " with k " + std::to_string(a.k) + " needs " +
+                  std::to_string(smem + fa.sharedSizeBytes) + " bytes of shared memory per block, the device allows " +
+                  std::to_string(optin));
+        return CDB_INVALID_PARAMS;
     }
+    CDB_ALLOW_SMEM(kern, smem);
+    if (f32path) scan_f32_kernel<QB, 2><<<grid, SCAN_THREADS, smem, s>>>(a);
+    else scan_generic_kernel<QB><<<grid, SCAN_THREADS, smem, s>>>(a);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }

@@ -147,12 +147,17 @@ __device__ inline float euclid_bf16_seq(const uint16_t *a, const uint16_t *b, ui
 }
 
 // ------------------------------------------------------------------ u8
+// dot_product_u8 (x86_64.rs:22-66) widens each 32-byte chunk with unpacklo / unpackhi: bytes {0-7, 16-23} feed one set of
+// i32 lanes, bytes {8-15, 24-31} the other.  Each set is folded to a u32 that wraps (accumulate_u32), and only the byte
+// tail past the last full chunk is added in u64.  In a 16-byte word the .x/.y words belong to the first set and .z/.w to
+// the second, so two u32 dp4a accumulators that wrap naturally give the reference's sum: it differs from the exact one
+// once either half passes 2^32 (saturated codes from D = 132,128).
 __device__ inline uint64_t dot_u8_int(const uint8_t *__restrict__ a, const uint8_t *__restrict__ b, uint32_t n) {
-    uint64_t total = 0;
-    uint32_t acc = 0;
+    uint32_t lo = 0, hi = 0;
+    const uint32_t n32 = n & ~31u;
     uint32_t i = 0;
     if ((((uintptr_t)a | (uintptr_t)b) & 15) == 0) {
-        for (; i + 64 <= n; i += 64) {  // 16 dp4a per block: flush well before u32 could overflow (16384 dp4a)
+        for (; i + 64 <= n32; i += 64) {
             uint4 vb[4], va[4];
 #pragma unroll
             for (int t = 0; t < 4; ++t) vb[t] = *reinterpret_cast<const uint4 *>(b + i + 16 * t);
@@ -160,22 +165,22 @@ __device__ inline uint64_t dot_u8_int(const uint8_t *__restrict__ a, const uint8
             for (int t = 0; t < 4; ++t) va[t] = *reinterpret_cast<const uint4 *>(a + i + 16 * t);
 #pragma unroll
             for (int t = 0; t < 4; ++t) {
-                acc = __dp4a(va[t].x, vb[t].x, acc);
-                acc = __dp4a(va[t].y, vb[t].y, acc);
-                acc = __dp4a(va[t].z, vb[t].z, acc);
-                acc = __dp4a(va[t].w, vb[t].w, acc);
+                lo = __dp4a(va[t].x, vb[t].x, lo);
+                lo = __dp4a(va[t].y, vb[t].y, lo);
+                hi = __dp4a(va[t].z, vb[t].z, hi);
+                hi = __dp4a(va[t].w, vb[t].w, hi);
             }
-            if ((i & 0xFFC0) == 0xFFC0) { total += acc; acc = 0; }
         }
     }
     // rows are 16B-pitched so 4-byte reads are aligned
-    for (; i + 4 <= n; i += 4) {
-        uint32_t x = *reinterpret_cast<const uint32_t *>(a + i), y = *reinterpret_cast<const uint32_t *>(b + i);
-        acc = __dp4a(x, y, acc);
-        if ((i & 0xFFFC) == 0xFFFC) { total += acc; acc = 0; }  // flush before u32 could overflow
+    for (; i < n32; i += 4) {
+        const uint32_t x = *reinterpret_cast<const uint32_t *>(a + i), y = *reinterpret_cast<const uint32_t *>(b + i);
+        if ((i & 15) < 8) lo = __dp4a(x, y, lo);
+        else hi = __dp4a(x, y, hi);
     }
-    for (; i < n; ++i) acc += (uint32_t)a[i] * (uint32_t)b[i];
-    return total + acc;
+    uint64_t tail = 0;
+    for (; i < n; ++i) tail += (uint32_t)a[i] * (uint32_t)b[i];
+    return (uint64_t)lo + hi + tail;
 }
 
 // ------------------------------------------------------------------ sub-byte

@@ -566,7 +566,10 @@ cdb_status cdb_score_ids(cdb_index *index, const float *query, const uint32_t *i
 
 /* ------------------------------------------- S3 finalize_ann_results re-rank
  * exact f32 cosine of `query` against raw rows cand_ids[0..n), sorted best
- * first, truncated to k.  Needs keep_raw_f32 (or F32 storage). */
+ * first, truncated to k.  Needs keep_raw_f32 (or F32 storage).  A candidate listed
+ * more than once is reported once per listing, as finalize_ann_results reports it.
+ * An id outside [id_base, id_base + size) is refused with CDB_INVALID_PARAMS before
+ * any device work. */
 cdb_status cdb_rerank_f32(cdb_index *index, const float *query, const uint32_t *cand_ids, uint32_t n,
                           uint32_t k, uint32_t *out_ids, float *out_scores, uint32_t *out_count);
 
