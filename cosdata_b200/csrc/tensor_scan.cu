@@ -19,6 +19,8 @@
 //   warps 8..11  producer warpgroup (setmaxnreg: 40 registers), one thread issues the TMA loads:
 //                cp.async.bulk.tensor.2d, SWIZZLE_128B, 4-stage mbarrier ring
 // Tile: 128 queries (A, K-major) x 256 corpus rows (B, K-major), K block = 64 halfs (128 B).
+// The s8 form at k <= 12 and D <= 1024 runs tensor_scan_s8_kernel instead: query tile resident, the two consumer
+// warpgroups on the two 128-row halves of each corpus tile, taking turns at the tensor pipe.
 #include <atomic>
 #include <climits>
 #include <cmath>
@@ -52,6 +54,7 @@ enum : int {
     TS_PROF_CONSUMER,    // consumers: whole tile loop
     TS_PROF_PRODUCER,    // producer: whole issue loop
     TS_PROF_CTAS,        // CTAs
+    TS_PROF_MATH_WAIT,   // s8 form: consumers waiting for their turn at the tensor pipe (the other warpgroup's K loop)
     TS_PROF_SLOTS
 };
 
@@ -86,6 +89,7 @@ struct TensorScanArgs {
     const float2 *q_se;     // [n_queries] {s_q, e_q}
     float dn1;              // 1 + delta_n, rounded up: bound on |x_hat| and |q_hat|
     float dref;             // delta_ref(D), rounded up: the reference's f32 cosine against the exact q_hat . x_hat
+    uint32_t stages;        // tensor_scan_s8_kernel: depth of its corpus ring (16 KB stages)
 };
 
 // Candidate staging in shared memory: 40 bytes per (consumer thread, query row): slot 0 = count, then 9 row ids (f16 form)
@@ -98,11 +102,12 @@ constexpr int TS_GROUPS = 64;       // at most 64 class maxima per query; the fi
 // bit r of a row bitmap (null: no bit is set)
 __device__ __forceinline__ bool bit_is_set(const uint32_t *bits, uint64_t r) { return bits && ((bits[r >> 5] >> (r & 31)) & 1u); }
 
-// rare path: one approximate score passed the threshold -> stage the row id, flush TS_LSTAGE at a time
+// rare path: one approximate score passed the threshold -> stage the row id, flush CAP at a time
+template <uint32_t CAP = TS_LSTAGE>
 __device__ __noinline__ void epi_emit(const TensorScanArgs &a, uint32_t qi, uint32_t *stage, uint32_t id) {
     uint32_t c = stage[0];
     stage[1 + c] = id;
-    if (++c == TS_LSTAGE) {
+    if (++c == CAP) {
         const uint32_t pos = atomicAdd(a.cand_cnt + qi, c);
         for (uint32_t i = 0; i < c; ++i)
             if (pos + i < a.cand_cap) a.cand[(size_t)qi * a.cand_cap + pos + i] = stage[1 + i];
@@ -571,6 +576,309 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     }
 }
 
+// ------------------------------------------------------------------ s8 form: ping-pong consumers, query tile resident
+// tensor_scan_s8_kernel runs the KIND 2 filter of tensor_scan_kernel with the tile's work split differently, so that one
+// warpgroup's epilogue and bound refresh run while the other warpgroup's MMAs keep the tensor pipe busy:
+//   * the CTA's 128 x D query tile is loaded once and stays in shared memory (the ring carries corpus rows only);
+//   * warpgroup w takes rows [128w, 128w + 128) of every 256-row corpus tile: all 128 queries x 128 rows as two
+//     m64n128k32 wgmma chains (queries 0-63 and 64-127), 128 s32 accumulators per thread as before;
+//   * an ordered pair of named barriers hands the tensor pipe from one warpgroup's K loop to the other's
+//     (0, 1, 0, 1, ...); each warpgroup takes exactly one turn per corpus tile of the CTA, a half past the corpus end
+//     included (its stages arrive without data and its values are masked), so the turns always pair up;
+//   * the ring is one sequence of 16 KB stages (128 rows x 128 B): tile t's lower half's k-blocks, then its upper half's.
+//     Turns consume it in that order, so the producer only ever waits for a stage an earlier turn releases.
+// Shared memory (227 KB per block): query tile kblocks x 16 KB (96 KB at D = 768) + ring stages x 16 KB (6: one whole
+// half-tile at D = 768) + candidate staging 256 threads x 4 queries x 32 B (a count and 7 ids: 32 KB) + barriers.
+// Register layout of the epilogue: a thread holds 4 query rows, 16 wl + lane/4 + {0, 8} + {0, 64}, and of each the 32
+// columns 8j + 2(lane%4) + {0,1} of its warpgroup's half.  The half's offset (128) is a multiple of NG, so a column's class
+// (column mod NG) is the same as in tensor_scan_kernel and each thread owns NG/4 classes of each of its queries.
+constexpr uint32_t TS8_HALF = 128;                       // corpus rows per warpgroup turn
+constexpr uint32_t TS8_KB_BYTES = 128 * 128;             // one k-block of the query tile or of a half-tile
+constexpr uint32_t TS8_MAX_STAGES = 6;
+constexpr uint32_t TS8_MIN_STAGES = 4;                   // fewer: the streamed kernel (tensor_scan_kernel) runs instead
+constexpr uint32_t TS8_SLOT_BYTES = 32;
+constexpr uint32_t TS8_LSTAGE = TS8_SLOT_BYTES / 4 - 1;  // ids staged per (thread, query)
+constexpr int TS8_BAR_TURN = 2;                          // named barriers 2 and 3: "warpgroup 0 / 1 may issue its K loop"
+constexpr size_t TS8_SMEM_FIXED = 1024 + (size_t)TS_CONSUMERS * 4 * TS8_SLOT_BYTES + (2 * TS8_MAX_STAGES + 1) * 8;
+
+template <int NG, bool HAS_DEG, bool PROF>
+__global__ void __launch_bounds__(TS_THREADS, 1)
+tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x, TensorScanArgs a) {
+    constexpr int NL = NG / 4;   // classes a thread owns per query
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t *qtile = smem;                                          // [kblocks] x 16 KB
+    uint8_t *ring = qtile + (size_t)a.kblocks * TS8_KB_BYTES;       // [stages] x 16 KB
+    uint8_t *lstage = ring + (size_t)a.stages * TS8_KB_BYTES;       // [256][4] x 32 B
+    uint64_t *full_bar = reinterpret_cast<uint64_t *>(lstage + TS_CONSUMERS * 4 * TS8_SLOT_BYTES);
+    uint64_t *empty_bar = full_bar + TS8_MAX_STAGES, *q_bar = empty_bar + TS8_MAX_STAGES;
+
+    const int lane = threadIdx.x & 31;
+    const uint32_t mt = blockIdx.x % a.mtiles, g = blockIdx.x / a.mtiles, G = gridDim.x / a.mtiles;
+    const uint32_t T = g < a.ntiles ? (a.ntiles - g + G - 1) / G : 0;   // corpus tiles g, g+G, ... of this CTA
+
+    if (threadIdx.x == TS_CONSUMERS) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
+        for (uint32_t s = 0; s < a.stages; ++s) { mbar_init(smem_u32(&full_bar[s]), 1); mbar_init(smem_u32(&empty_bar[s]), 4); }
+        mbar_init(smem_u32(q_bar), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= TS_CONSUMERS) {
+        // ===================== TMA producer =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (threadIdx.x == TS_CONSUMERS && T > 0) {
+            unsigned long long p_empty = 0, p_drift = 0, p_t0 = PROF ? clock64() : 0;
+            mbar_expect_tx(smem_u32(q_bar), a.kblocks * TS8_KB_BYTES);
+            for (uint32_t kb = 0; kb < a.kblocks; ++kb)
+                tma_load_2d(smem_u32(qtile + (size_t)kb * TS8_KB_BYTES), &map_q, smem_u32(q_bar), (int)(kb * 128), (int)(mt * TS_BLOCK_M));
+            uint32_t s = 0, phase = 0;
+            for (uint32_t t = 0; t < T; ++t) {
+                const uint32_t nt = g + t * G;
+                if (a.mtiles > 1 && t >= a.window) {
+                    const unsigned long long c0 = PROF ? clock64() : 0;
+                    // bounded drift: every CTA of the group must have consumed tile t - window (as in tensor_scan_kernel)
+                    const uint32_t need = (t - a.window + 1) * a.mtiles;
+                    for (int spin = 0; spin < 20000 && *reinterpret_cast<volatile uint32_t *>(a.progress + g) < need; ++spin) __nanosleep(64);
+                    if (PROF) p_drift += clock64() - c0;
+                }
+                for (uint32_t h = 0; h < 2; ++h) {
+                    const uint64_t hrow0 = (uint64_t)nt * TS_BLOCK_N + h * TS8_HALF;
+                    for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
+                        const unsigned long long c0 = PROF ? clock64() : 0;
+                        mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+                        if (PROF) p_empty += clock64() - c0;
+                        const uint32_t fb = smem_u32(&full_bar[s]);
+                        if (hrow0 < a.n_rows) {
+                            mbar_expect_tx(fb, TS8_KB_BYTES);
+                            tma_load_2d(smem_u32(ring + (size_t)s * TS8_KB_BYTES), &map_x, fb, (int)(kb * 128), (int)hrow0);
+                        } else {
+                            mbar_arrive(fb);   // the upper half of a last tile that ends within its lower half: no rows
+                        }
+                        if (++s == a.stages) { s = 0; phase ^= 1; }
+                    }
+                }
+            }
+            if (PROF) {
+                atomicAdd(a.prof + TS_PROF_EMPTY_WAIT, p_empty);
+                atomicAdd(a.prof + TS_PROF_DRIFT, p_drift);
+                atomicAdd(a.prof + TS_PROF_PRODUCER, clock64() - p_t0);
+                atomicAdd(a.prof + TS_PROF_CTAS, 1ull);
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers: MMA + threshold filter =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const uint32_t ct = threadIdx.x, wg = ct >> 7, wl = (ct >> 5) & 3, qd = (uint32_t)lane & 3;
+    float bound[4], gm[4][NL];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const uint32_t ql = 64 * (i >> 1) + 16 * wl + ((uint32_t)lane >> 2) + 8 * (i & 1), qi = mt * TS_BLOCK_M + ql;
+        const bool qvalid = qi < a.n_queries;
+        reinterpret_cast<uint32_t *>(lstage + (size_t)(ct * 4 + i) * TS8_SLOT_BYTES)[0] = 0;
+#pragma unroll
+        for (int l = 0; l < NL; ++l) gm[i][l] = -INFINITY;
+        // what earlier launches (the seeding pass) and other CTAs already know
+        bound[i] = qvalid ? class_bound<NG>(a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql, a.k) : -INFINITY;
+    }
+    if (T == 0) return;
+    if (wg == 1) named_bar_arrive<TS8_BAR_TURN, 256>();   // warpgroup 0 takes the first turn
+    mbar_wait(smem_u32(q_bar), 0);
+    const uint32_t q0 = smem_u32(qtile), r0 = smem_u32(ring);
+    unsigned long long p_turn = 0, p_full = 0, p_mma = 0, p_epi = 0, p_ref = 0, p_c = PROF ? clock64() : 0;
+    for (uint32_t t = 0; t < T; ++t) {
+        const uint32_t nt = g + t * G;
+        const uint64_t row0 = (uint64_t)nt * TS_BLOCK_N + wg * TS8_HALF;   // this warpgroup's half
+        const float2 se = __ldg(a.tile_se + nt);                           // {s_T, E_T} of the 256-row tile, both halves
+        // ring position of this turn's first k-block: turn 2t + wg of the sequence
+        const uint32_t p0 = (2 * t + wg) * a.kblocks;
+        uint32_t s = p0 % a.stages, phase = (p0 / a.stages) & 1u;
+        unsigned long long c_turn = PROF ? clock64() : 0, c_full = 0;
+        if (wg == 0) named_bar_sync<TS8_BAR_TURN, 256>();
+        else named_bar_sync<TS8_BAR_TURN + 1, 256>();
+        const unsigned long long c_main = PROF ? clock64() : 0;
+        // zeroing ends the accumulators' live range for ptxas (see tensor_scan_kernel)
+        uint32_t acc[128];
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0;
+        uint32_t prev = 0;
+        for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
+            const unsigned long long c0 = PROF ? clock64() : 0;
+            mbar_wait(smem_u32(&full_bar[s]), phase);
+            if (PROF) c_full += clock64() - c0;
+            const uint32_t qa = q0 + kb * TS8_KB_BYTES;
+            const uint64_t adesc0 = make_smem_desc(qa), adesc1 = make_smem_desc(qa + TS8_KB_BYTES / 2);
+            const uint64_t bdesc = make_smem_desc(r0 + s * TS8_KB_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {   // +32 bytes along K = +2 in the encoded start address
+                wgmma_s8_n128(acc, adesc0 + 2 * kk, bdesc + 2 * kk);
+                wgmma_s8_n128(acc + 64, adesc1 + 2 * kk, bdesc + 2 * kk);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();   // the previous k-block's MMAs have retired
+            if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+            prev = s;
+            if (++s == a.stages) { s = 0; phase ^= 1; }
+        }
+        // every MMA of the turn is issued: the other warpgroup may start its K loop while these drain.  Warpgroup 1's
+        // last turn hands over nothing (warpgroup 0 has no turn left), so both barriers see as many arrivals as waits.
+        if (wg == 0) named_bar_arrive<TS8_BAR_TURN + 1, 256>();
+        else if (t + 1 < T) named_bar_arrive<TS8_BAR_TURN, 256>();
+        wgmma_wait<0>();
+        if (a.kblocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+        if (ct == 128 && a.mtiles > 1) atomicAdd(a.progress + g, 1u);   // the tile's upper half is in: all of its loads landed
+        unsigned long long c_epi = 0;
+        if (PROF) {
+            c_epi = clock64();
+            p_turn += c_main - c_turn;
+            p_full += c_full;
+            p_mma += c_epi - c_main - c_full;
+        }
+
+        // ---- epilogue (the filter of tensor_scan_kernel, KIND 2).  The per-query addresses below are derived from `me`,
+        //      which the empty asm makes opaque per tile: otherwise they are hoisted out of the tile loop and held in
+        //      registers (or spilled) across the K loop, where the accumulators need every register.
+        uint32_t me = ct;
+        asm volatile("" : "+r"(me));
+        const uint32_t qrow = 16 * ((me >> 5) & 3) + ((me & 31) >> 2);   // + 8 (i & 1) + 64 (i >> 1)
+        const bool full_half = row0 + TS8_HALF <= a.n_rows;   // only the corpus' last tile can be partial
+        const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;
+        // the four queries' thresholds first, as four independent chains: a warp runs this epilogue alone on its SM
+        // sub-partition (the other warpgroup is in its K loop), so a load -> divide chain per query would be exposed
+        // four times over.  {s_q, e_q} come from L1 rather than from 8 registers held across the K loop (a padding
+        // row's values are never used).
+        float slo[4], shi[4], eps[4];
+        int thrI[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t qi = mt * TS_BLOCK_M + qrow + 64 * (i >> 1) + 8 * (i & 1);
+            const float2 qse = __ldg(a.q_se + min(qi, a.n_queries - 1));
+            // s_T*s_q rounded down and up, eps(q,T) rounded up, thrI <= (A - eps) / (s_T*s_q)
+            slo[i] = __fmul_rd(se.x, qse.x);
+            shi[i] = __fmul_ru(se.x, qse.x);
+            eps[i] = __fmaf_ru(__fadd_ru(a.dn1, qse.y), se.y, __fmaf_ru(qse.y, a.dn1, a.dref));
+            const float num = __fsub_rd(bound[i], eps[i]);
+            thrI[i] = __float2int_rd(__fdiv_rd(num, num >= 0.0f ? shi[i] : slo[i]));
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1), qi = mt * TS_BLOCK_M + ql;
+            const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);   // value (j, b) at v_i[4j + b]
+            int cm[NL];
+#pragma unroll
+            for (int l = 0; l < NL; ++l) cm[l] = INT_MIN;
+            bool hit;
+            if (full_half) {
+                int zmax = INT_MIN;   // HAS_DEG: 0 if some accumulator of the half is exactly zero
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                    for (int b = 0; b < 2; ++b) {
+                        int v = (int)v_i[4 * j + b];
+                        if (HAS_DEG) {
+                            zmax = v == 0 ? 0 : zmax;
+                            v = v == 0 ? INT_MIN : v;
+                        }
+                        const int l = (j & (NG / 8 - 1)) * 2 + b;
+                        cm[l] = max(cm[l], v);
+                    }
+                }
+                int cmax = zmax;
+#pragma unroll
+                for (int l = 0; l < NL; ++l) cmax = max(cmax, cm[l]);
+                hit = cmax >= thrI[i];
+            } else {
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                    for (int b = 0; b < 2; ++b) {
+                        const uint32_t col = 8 * j + 2 * (me & 3) + b;
+                        const int v = (int)v_i[4 * j + b];
+                        const int l = (j & (NG / 8 - 1)) * 2 + b;
+                        if ((uint64_t)col < left && !(HAS_DEG && v == 0)) cm[l] = max(cm[l], v);
+                    }
+                }
+                hit = true;
+            }
+            // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class
+#pragma unroll
+            for (int l = 0; l < NL; ++l)
+                if (cm[l] != INT_MIN)
+                    gm[i][l] = fmaxf(gm[i][l], __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo[i] : shi[i]), eps[i]));
+            if (qi < a.n_queries && a.emit && hit) {
+                uint32_t *stage = reinterpret_cast<uint32_t *>(lstage + (size_t)(me * 4 + i) * TS8_SLOT_BYTES);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                    for (int b = 0; b < 2; ++b) {
+                        const uint32_t col = 8 * j + 2 * (me & 3) + b;
+                        if ((uint64_t)col < left && (int)v_i[4 * j + b] >= thrI[i])
+                            epi_emit<TS8_LSTAGE>(a, qi, stage, a.id_base + (uint32_t)(row0 + col));
+                    }
+                }
+            }
+        }
+        unsigned long long c_ref = 0;
+        if (PROF) {
+            c_ref = clock64();
+            p_epi += c_ref - c_epi;
+        }
+        // refresh the shared bound at tensor_scan_kernel's cadence (per tile of the CTA)
+        if (t < 8 || (t & a.refresh_mask) == a.refresh_mask || !a.emit) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
+                if (mt * TS_BLOCK_M + ql >= a.n_queries) continue;
+                int *ggm_q = a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql;
+#pragma unroll
+                for (int l = 0; l < NL; ++l) {
+                    int *p = ggm_q + (size_t)(8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M;
+                    const int mine = f2ord(gm[i][l]);
+                    if (mine > *reinterpret_cast<volatile int *>(p)) atomicMax(p, mine);
+                }
+            }
+            __syncwarp();
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
+                if (mt * TS_BLOCK_M + ql >= a.n_queries) continue;
+                bound[i] = fmaxf(bound[i], class_bound<NG>(a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql, a.k));
+            }
+        }
+        if (PROF) p_ref += clock64() - c_ref;
+    }
+    if (PROF && (ct & 127) == 0) {
+        atomicAdd(a.prof + TS_PROF_MATH_WAIT, p_turn);
+        atomicAdd(a.prof + TS_PROF_FULL_WAIT, p_full);
+        atomicAdd(a.prof + TS_PROF_MMA, p_mma);
+        atomicAdd(a.prof + TS_PROF_EPILOGUE, p_epi);
+        atomicAdd(a.prof + TS_PROF_REFRESH, p_ref);
+        atomicAdd(a.prof + TS_PROF_TILES, (unsigned long long)T);
+        atomicAdd(a.prof + TS_PROF_CONSUMER, clock64() - p_c);
+    }
+    // final publish + flush of the staged candidates
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const uint32_t ql = 64 * (i >> 1) + 16 * wl + ((uint32_t)lane >> 2) + 8 * (i & 1), qi = mt * TS_BLOCK_M + ql;
+        if (qi >= a.n_queries) continue;
+#pragma unroll
+        for (int l = 0; l < NL; ++l)
+            atomicMax(a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql + (size_t)(8 * (l >> 1) + 2 * qd + (l & 1)) * TS_BLOCK_M, f2ord(gm[i][l]));
+        const uint32_t *stage = reinterpret_cast<const uint32_t *>(lstage + (size_t)(ct * 4 + i) * TS8_SLOT_BYTES);
+        const uint32_t c = stage[0];
+        if (a.emit && c) {
+            const uint32_t pos = atomicAdd(a.cand_cnt + qi, c);
+            for (uint32_t x = 0; x < c; ++x)
+                if (pos + x < a.cand_cap) a.cand[(size_t)qi * a.cand_cap + pos + x] = stage[1 + x];
+        }
+    }
+}
+
 // ------------------------------------------------------------------ fp16 normalised copies
 // x_hat = x / |x| (IEEE), rounded to fp16.  Rows whose norm is outside [1e-15, 1e15] (zero, underflowed, overflowed,
 // inf/NaN) are DEGENERATE: the error bound of the prefilter does not cover them, their shadow row is all zero.
@@ -934,6 +1242,22 @@ static unsigned long long *g_scan_prof = nullptr;   // [TS_PROF_SLOTS] on the de
 template <int NG, bool HAS_DEG, int KIND>
 static cdb_status launch_tensor_scan_gd(const CUtensorMap &mq, const CUtensorMap &mx, const TensorScanArgs &a, uint32_t grid,
                                         cudaStream_t s) {
+    // s8 form: tensor_scan_s8_kernel for k <= 12.  At NG = 32 / 64 its 4 x NG/4 class maxima do not fit next to the 128
+    // accumulators in the consumers' 232 registers (ptxas spills 24 / 536 bytes), so larger k keep the streamed kernel.
+    if constexpr (KIND == 2 && NG == 16) {
+        if (a.stages) {
+            auto kern = tensor_scan_s8_kernel<NG, HAS_DEG, false>;
+            if (a.prof) {
+                if constexpr (NG == 16 && !HAS_DEG) kern = tensor_scan_s8_kernel<NG, HAS_DEG, true>;
+                else { set_error("tensor scan profile: only for k <= 12 on shards without degenerate or deleted rows"); return CDB_INVALID_PARAMS; }
+            }
+            const size_t smem = TS8_SMEM_FIXED + (size_t)(a.kblocks + a.stages) * TS8_KB_BYTES;
+            CDB_ALLOW_SMEM(kern, smem);
+            kern<<<grid, TS_THREADS, smem, s>>>(mq, mx, a);
+            CDB_LAUNCH_CHECK();
+            return CDB_OK;
+        }
+    }
     auto kern = tensor_scan_kernel<TS_STAGES, NG, HAS_DEG, KIND, false>;
     if (a.prof) {   // the instrumented instantiation exists for the headline's k <= 12 without degenerate rows
         if constexpr (NG == 16 && !HAS_DEG) kern = tensor_scan_kernel<TS_STAGES, NG, HAS_DEG, KIND, true>;
@@ -1080,10 +1404,16 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
     a.dref = f32_up((2.0 * dim + 16.0) * 0x1p-24);
     a.rel = 1.0f;
     if (!tensor_scan_stages(k)) { set_error("s8 tensor scan: k too large (class-maximum bound needs k <= 64)"); return CDB_INVALID_PARAMS; }
+    // tensor_scan_s8_kernel for k <= 12 (NG = 16, see launch_tensor_scan_gd) while the resident query tile leaves room for
+    // TS8_MIN_STAGES corpus stages (D <= 1024), else the streamed tensor_scan_kernel.  The two take differently shaped
+    // corpus boxes (128 / 256 rows), so a.stages != 0 must mean exactly "the s8 kernel runs".
+    const size_t room = 227 * 1024 - TS8_SMEM_FIXED;
+    const uint32_t fit = (uint32_t)(room / TS8_KB_BYTES) > a.kblocks ? (uint32_t)(room / TS8_KB_BYTES) - a.kblocks : 0;
+    a.stages = k <= 12 && fit >= TS8_MIN_STAGES ? std::min(fit, TS8_MAX_STAGES) : 0;
     CUtensorMap mq, mx;
     cdb_status rc;
     if ((rc = make_tensor_map_2d(&mq, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_qs8, (uint64_t)a.mtiles * TS_BLOCK_M, dim, pitch8, TS_BLOCK_M))) return rc;
-    if ((rc = make_tensor_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_xs8, n_rows, dim, pitch8, TS_BLOCK_N))) return rc;
+    if ((rc = make_tensor_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_xs8, n_rows, dim, pitch8, a.stages ? TS8_HALF : TS_BLOCK_N))) return rc;
     return run_tensor_scan<2>(mq, mx, a, n_rows, d_progress, sm_count, s);
 }
 
