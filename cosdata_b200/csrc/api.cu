@@ -163,7 +163,8 @@ struct cdb_index {
     uint32_t xh_pitch = 0;         // halfs per shadow row
     void *d_xs8 = nullptr;         // s8 shadow for the s8 form of the prefilter (tensor_scan.cu KIND 2, DESIGN.md section 5c)
     uint32_t xs8_pitch = 0;        // bytes per s8 shadow row
-    float2 *d_s8se = nullptr;      // [corpus tiles] {s_T, E_T}, then one float: E_max
+    float2 *d_s8se = nullptr;      // [corpus tiles] {s_T, E_T}, then one float: E_max, then d_s8rcp
+    float2 *d_s8rcp = nullptr;     // [corpus tiles] {1/s_T rounded down, rounded up} (inside the d_s8se allocation)
     uint32_t s8_tiles = 0;         // corpus tiles of the capacity
     float s8_emax = 0.0f;          // max E_T of the stored rows (host copy, read by the gate)
     uint64_t n_allzero_rows = 0;   // degenerate rows (tensor_scan.cu): all-zero rows score NaN against every query = last
@@ -482,8 +483,9 @@ cdb_status cdb_index_create(const cdb_index_desc *d, cdb_index **out) {
         ix->s8_tiles = (uint32_t)((d->capacity + 255) / 256);
         if ((e = cudaMalloc(&ix->d_xs8, (size_t)d->capacity * ix->xs8_pitch)) != cudaSuccess) return fail(e, "cudaMalloc(s8 shadow)");
         if ((e = cudaMemsetAsync(ix->d_xs8, 0, (size_t)d->capacity * ix->xs8_pitch, ix->stream)) != cudaSuccess) return fail(e, "memset");
-        if ((e = cudaMalloc(&ix->d_s8se, ((size_t)ix->s8_tiles + 1) * 8)) != cudaSuccess) return fail(e, "cudaMalloc(s8 scales)");
-        if ((e = cudaMemsetAsync(ix->d_s8se, 0, ((size_t)ix->s8_tiles + 1) * 8, ix->stream)) != cudaSuccess) return fail(e, "memset");
+        if ((e = cudaMalloc(&ix->d_s8se, (2 * (size_t)ix->s8_tiles + 1) * 8)) != cudaSuccess) return fail(e, "cudaMalloc(s8 scales)");
+        if ((e = cudaMemsetAsync(ix->d_s8se, 0, (2 * (size_t)ix->s8_tiles + 1) * 8, ix->stream)) != cudaSuccess) return fail(e, "memset");
+        ix->d_s8rcp = ix->d_s8se + ix->s8_tiles + 1;
     }
     if (d->tensor_prefilter && d->storage_type >= CDB_ST_SUB1 && d->storage_type <= CDB_ST_SUB3) {
         ix->digit_pitch = round_up(d->dim, 16);
@@ -557,7 +559,7 @@ static cdb_status index_after_append(cdb_index *ix, uint64_t first, uint64_t n) 
         // s8 shadow: every tile the range touches, the open tile's earlier rows included (its scale can change; deleted rows
         // among them keep zero codes)
         if ((rc = quantize_s8_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, first, n, first + n, ix->desc.dim, ix->d_xs8,
-                                     ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->del_dev(), ix->stream)))
+                                     ix->xs8_pitch, ix->d_s8se, ix->d_s8rcp, &ix->d_s8se[ix->s8_tiles].x, ix->del_dev(), ix->stream)))
             return rc;
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 4, ix->deg.p, 8, cudaMemcpyDeviceToHost, ix->stream));
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
@@ -665,7 +667,7 @@ cdb_status cdb_index_set_raw_f32(cdb_index *ix, uint64_t first_row, const float 
     }
     if (ix->d_xs8) {
         cdb_status rc = quantize_s8_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, first_row, n, ix->size, dim, ix->d_xs8,
-                                           ix->xs8_pitch, ix->d_s8se, &ix->d_s8se[ix->s8_tiles].x, ix->del_dev(), ix->stream);
+                                           ix->xs8_pitch, ix->d_s8se, ix->d_s8rcp, &ix->d_s8se[ix->s8_tiles].x, ix->del_dev(), ix->stream);
         if (rc) return rc;
         CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
         CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));
@@ -956,16 +958,17 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         uint32_t *flags = sc->flags.as<uint32_t>();  // [0] queries of the last search that needed the exact scan, [3] searches with a fallback
         const bool has_deg = ix->n_allzero_rows + ix->n_odd_rows + ix->n_deleted > 0;
         const bool s8 = use_s8_form(ix, nq);
-        if (s8 && (rc = sc->qse.ensure((size_t)nq * 8))) return rc;
+        if (s8 && (rc = sc->qse.ensure((size_t)nq * 16))) return rc;   // {s_q, e_q}, then {1/s_q rounded down, up}
         if ((rc = prep_queries_device(d_queries, nq, d.dim, sc->q_codes.as<float>(), pitch / 4, sc->q_mags.as<float>(), sc->qh.p,
                                       s8 ? ix->xs8_pitch : ix->xh_pitch, sc->gthr.as<int>(), ix->deg.as<uint32_t>(), has_deg, d.id_base,
                                       sc->cand.as<uint32_t>(), cap, sc->cand_cnt.as<uint32_t>(), sc->err32.as<uint32_t>(), d_err,
-                                      sc->progress.as<uint32_t>(), s8 ? sc->qse.as<float2>() : nullptr, s)))
+                                      sc->progress.as<uint32_t>(), s8 ? sc->qse.as<float2>() : nullptr,
+                                      s8 ? sc->qse.as<float2>() + nq : nullptr, s)))
             return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring0[slot], s));
         if (s8) {
-            if ((rc = tensor_scan_s8_device(ix->d_xs8, sc->qh.p, ix->xs8_pitch, ix->size, nq, d.dim, p->k, ix->d_s8se,
-                                            sc->qse.as<float2>(), d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(),
+            if ((rc = tensor_scan_s8_device(ix->d_xs8, sc->qh.p, ix->xs8_pitch, ix->size, nq, d.dim, p->k, ix->d_s8se, ix->d_s8rcp,
+                                            sc->qse.as<float2>(), sc->qse.as<float2>() + nq, d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(),
                                             sc->cand_cnt.as<uint32_t>(), cap, sc->progress.as<uint32_t>(), has_deg, ix->sm_count, s)))
                 return rc;
             ix->stat_s8_searches++;
@@ -1723,7 +1726,7 @@ static cdb_status drop_from_shadows(cdb_index *ix, const std::vector<uint32_t> &
     const uint32_t *d_list = ix->stage.as<uint32_t>();
     if ((rc = shadow_drop_rows_device(d_list, (uint32_t)n_rows, d_list + n_rows, (uint32_t)n_tiles, ix->d_xh, ix->xh_pitch, ix->d_raw,
                                       ix->raw_pitch_elems, ix->d_raw_mags, ix->size, ix->desc.dim, ix->d_xs8, ix->xs8_pitch, ix->d_s8se,
-                                      ix->d_xs8 ? &ix->d_s8se[ix->s8_tiles].x : nullptr, ix->d_deleted, ix->stream)))
+                                      ix->d_s8rcp, ix->d_xs8 ? &ix->d_s8se[ix->s8_tiles].x : nullptr, ix->d_deleted, ix->stream)))
         return rc;
     if (ix->d_xs8) CDB_CUDA_TRY(cudaMemcpyAsync(ix->h_flags + 6, &ix->d_s8se[ix->s8_tiles].x, 4, cudaMemcpyDeviceToHost, ix->stream));
     CDB_CUDA_TRY(cudaStreamSynchronize(ix->stream));

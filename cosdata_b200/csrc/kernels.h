@@ -276,8 +276,8 @@ cdb_status normalize_f16_device(const float *d_raw, uint32_t pitch_elems, const 
 // set in d_deleted (d_xs8 may be null: no s8 shadow), then *d_emax refreshed
 cdb_status shadow_drop_rows_device(const uint32_t *d_rows, uint32_t n_rows, const uint32_t *d_tiles, uint32_t n_tiles, void *d_xh,
                                    uint32_t xh_pitch_halfs, const float *d_raw, uint32_t pitch_elems, const float *d_mags,
-                                   uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
-                                   const uint32_t *d_deleted, cudaStream_t s);
+                                   uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float2 *d_tile_rcp,
+                                   float *d_emax, const uint32_t *d_deleted, cudaStream_t s);
 cdb_status classify_rows_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t n, uint32_t dim,
                                 uint32_t first_row, uint32_t *d_deg, cudaStream_t s);
 size_t tensor_scan_smem_bytes(uint32_t k);
@@ -289,14 +289,15 @@ cdb_status tensor_scan_device(const void *d_xh, const void *d_qh, uint32_t pitch
 cdb_status prep_queries_device(const float *d_q, uint32_t nq, uint32_t dim, float *d_q_raw, uint32_t raw_pitch_elems, float *d_q_mags,
                                void *d_qh, uint32_t qh_pitch_halfs, int *d_ggm, const uint32_t *d_deg, bool has_deg, uint32_t id_base,
                                uint32_t *d_cand, uint32_t cand_cap, uint32_t *d_cand_cnt, uint32_t *d_err32, uint8_t *d_err8,
-                               uint32_t *d_progress, float2 *d_q_se, cudaStream_t s);
+                               uint32_t *d_progress, float2 *d_q_se, float2 *d_q_rcp, cudaStream_t s);
 // s8 form of the prefilter (DESIGN.md section 5c): shadow of the tiles touching rows [first, first + n) of rows < row_end,
 // then *d_emax = max E_T over all tiles below row_end; rows set in d_deleted (may be null) are treated as degenerate
 cdb_status quantize_s8_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
-                              uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
-                              const uint32_t *d_deleted, cudaStream_t s);
+                              uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float2 *d_tile_rcp,
+                              float *d_emax, const uint32_t *d_deleted, cudaStream_t s);
 cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t pitch8, uint64_t n_rows, uint32_t nq, uint32_t dim,
-                                 uint32_t k, const float2 *d_tile_se, const float2 *d_q_se, uint32_t id_base, int *d_ggm,
+                                 uint32_t k, const float2 *d_tile_se, const float2 *d_tile_rcp, const float2 *d_q_se,
+                                 const float2 *d_q_rcp, uint32_t id_base, int *d_ggm,
                                  uint32_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_progress, bool has_deg,
                                  int sm_count, cudaStream_t s);
 cdb_status tensor_scan_i8_device(const uint8_t *d_x, const uint8_t *d_q, uint32_t pitch, uint64_t n_rows, uint32_t nq, uint32_t dim,

@@ -55,6 +55,10 @@ enum : int {
     TS_PROF_PRODUCER,    // producer: whole issue loop
     TS_PROF_CTAS,        // CTAs
     TS_PROF_MATH_WAIT,   // s8 form: consumers waiting for their turn at the tensor pipe (the other warpgroup's K loop)
+    TS_PROF_EPI_THR,     // s8 form, parts of TS_PROF_EPILOGUE: the four queries' thresholds
+    TS_PROF_EPI_FOLD,    //   class maxima, their fold into gm and the shared class maxima, the hit test
+    TS_PROF_EPI_EMIT,    //   the emission loops (only on a hit)
+    TS_PROF_BOUND_ROUNDS,   // s8 form: rounds of the bound warp (TS_PROF_REFRESH then sums the bound warp's clocks in them)
     TS_PROF_SLOTS
 };
 
@@ -73,7 +77,8 @@ struct TensorScanArgs {
     uint32_t cand_cap;
     uint32_t *progress;  // [groups] tiles completed by the CTAs of a group (bounded-drift window), zeroed per launch
     uint32_t window;     // a CTA may run at most `window` tiles ahead of the slowest CTA of its group
-    uint32_t refresh_mask;  // the shared bound is refreshed when (tile & mask) == mask (and for the first tiles)
+    uint32_t refresh_mask;  // tensor_scan_kernel: the shared bound is refreshed when (tile & mask) == mask (and for the
+                            // first tiles); tensor_scan_s8_kernel refreshes it in its bound warp instead
     uint32_t has_deg;       // the corpus holds degenerate rows: kernel variant that keeps zero accumulators out of the bound
     unsigned long long *prof;   // [TS_PROF_SLOTS] clock64 sums of the instrumented instantiation, null otherwise
     // ---- integer form (KIND 1: exact scoring of u8 codes / sub-byte digits on wgmma .s32.u8.u8, tensor_scan_u8.cu)
@@ -87,6 +92,8 @@ struct TensorScanArgs {
     // ---- s8 form (KIND 2: the prefilter on wgmma .s32.s8.s8 against the s8 shadow, DESIGN.md section 5c)
     const float2 *tile_se;  // [ntiles] {s_T, E_T} of each corpus tile
     const float2 *q_se;     // [n_queries] {s_q, e_q}
+    const float2 *tile_rcp; // [ntiles] {1/s_T rounded down, rounded up} (tensor_scan_s8_kernel)
+    const float2 *q_rcp;    // [n_queries] {1/s_q rounded down, rounded up} (tensor_scan_s8_kernel)
     float dn1;              // 1 + delta_n, rounded up: bound on |x_hat| and |q_hat|
     float dref;             // delta_ref(D), rounded up: the reference's f32 cosine against the exact q_hat . x_hat
     uint32_t stages;        // tensor_scan_s8_kernel: depth of its corpus ring (16 KB stages)
@@ -103,14 +110,15 @@ constexpr int TS_GROUPS = 64;       // at most 64 class maxima per query; the fi
 __device__ __forceinline__ bool bit_is_set(const uint32_t *bits, uint64_t r) { return bits && ((bits[r >> 5] >> (r & 31)) & 1u); }
 
 // rare path: one approximate score passed the threshold -> stage the row id, flush CAP at a time
+// (the few fields it needs by value: a reference to the kernel's arguments would copy them to the stack)
 template <uint32_t CAP = TS_LSTAGE>
-__device__ __noinline__ void epi_emit(const TensorScanArgs &a, uint32_t qi, uint32_t *stage, uint32_t id) {
+__device__ __noinline__ void epi_emit(uint32_t *cand, uint32_t *cand_cnt, uint32_t cand_cap, uint32_t qi, uint32_t *stage, uint32_t id) {
     uint32_t c = stage[0];
     stage[1 + c] = id;
     if (++c == CAP) {
-        const uint32_t pos = atomicAdd(a.cand_cnt + qi, c);
+        const uint32_t pos = atomicAdd(cand_cnt + qi, c);
         for (uint32_t i = 0; i < c; ++i)
-            if (pos + i < a.cand_cap) a.cand[(size_t)qi * a.cand_cap + pos + i] = stage[1 + i];
+            if (pos + i < cand_cap) cand[(size_t)qi * cand_cap + pos + i] = stage[1 + i];
         c = 0;
     }
     stage[0] = c;
@@ -458,7 +466,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                             for (int b = 0; b < 2; ++b) {
                                 const uint32_t col = 8 * j + 2 * qd + b;
                                 if ((uint64_t)col < left && (int)acc[4 * j + 2 * i + b] >= thrI)
-                                    epi_emit(a, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
+                                    epi_emit(a.cand, a.cand_cnt, a.cand_cap, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
                             }
                         }
                     }
@@ -513,7 +521,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                             const float v = acc_value<KIND>(acc[4 * j + 2 * i + b], cosine, cosine ? rs[col] : 0.0f);
                             if ((uint64_t)col < left && !((dead >> (2 * j + b)) & 1u) && v >= thr[i]) {
                                 if (KIND == 1) epi_emit_key(a, qi[i], kstage[i], (int)acc_bits(acc[4 * j + 2 * i + b]), row0 + col, qmag[i]);
-                                else epi_emit(a, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
+                                else epi_emit(a.cand, a.cand_cnt, a.cand_cap, qi[i], stage[i], a.id_base + (uint32_t)(row0 + col));
                             }
                         }
                     }
@@ -578,7 +586,7 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 
 // ------------------------------------------------------------------ s8 form: ping-pong consumers, query tile resident
 // tensor_scan_s8_kernel runs the KIND 2 filter of tensor_scan_kernel with the tile's work split differently, so that one
-// warpgroup's epilogue and bound refresh run while the other warpgroup's MMAs keep the tensor pipe busy:
+// warpgroup's epilogue runs while the other warpgroup's MMAs keep the tensor pipe busy:
 //   * the CTA's 128 x D query tile is loaded once and stays in shared memory (the ring carries corpus rows only);
 //   * warpgroup w takes rows [128w, 128w + 128) of every 256-row corpus tile: all 128 queries x 128 rows as two
 //     m64n128k32 wgmma chains (queries 0-63 and 64-127), 128 s32 accumulators per thread as before;
@@ -586,9 +594,18 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 //     (0, 1, 0, 1, ...); each warpgroup takes exactly one turn per corpus tile of the CTA, a half past the corpus end
 //     included (its stages arrive without data and its values are masked), so the turns always pair up;
 //   * the ring is one sequence of 16 KB stages (128 rows x 128 B): tile t's lower half's k-blocks, then its upper half's.
-//     Turns consume it in that order, so the producer only ever waits for a stage an earlier turn releases.
+//     Turns consume it in that order, so the producer only ever waits for a stage an earlier turn releases;
+//   * the bound refresh runs in a warp of its own, the bound warp (warp 1 of the producer warpgroup): the consumers raise
+//     the CTA's class maxima in shared memory (`cls`, shared atomicMax, only when a value grew) and read the queries'
+//     bounds from `sbound`; they never touch the global class maxima during the scan.  A bound-warp round pushes the
+//     CTA's class maxima that exceed the global ones to `ggm` (RED), takes the k-th largest of each query's NG class
+//     maxima (the larger of the global and the CTA's value) by rank counting, and raises `sbound`.  It runs once per
+//     completed warpgroup epilogue (back to back when it falls behind).  It only moves and selects values the consumers
+//     computed as rigorous lower bounds, and `sbound` only rises, so a stale bound costs candidates, never correctness.
 // Shared memory (227 KB per block): query tile kblocks x 16 KB (96 KB at D = 768) + ring stages x 16 KB (6: one whole
-// half-tile at D = 768) + candidate staging 256 threads x 4 queries x 32 B (a count and 7 ids: 32 KB) + barriers.
+// half-tile at D = 768) + candidate staging 256 threads x 4 queries x 16 B (a count and 3 ids: 16 KB) + class maxima
+// NG x 128 ints (8 KB) + per query the bound, {s_q, 1/s_q down, 1/s_q up, 1 + delta_n + e_q} and e_q (1 + delta_n) +
+// delta_ref (3 KB) + control words + barriers.
 // Register layout of the epilogue: a thread holds 4 query rows, 16 wl + lane/4 + {0, 8} + {0, 64}, and of each the 32
 // columns 8j + 2(lane%4) + {0,1} of its warpgroup's half.  The half's offset (128) is a multiple of NG, so a column's class
 // (column mod NG) is the same as in tensor_scan_kernel and each thread owns NG/4 classes of each of its queries.
@@ -596,21 +613,63 @@ constexpr uint32_t TS8_HALF = 128;                       // corpus rows per warp
 constexpr uint32_t TS8_KB_BYTES = 128 * 128;             // one k-block of the query tile or of a half-tile
 constexpr uint32_t TS8_MAX_STAGES = 6;
 constexpr uint32_t TS8_MIN_STAGES = 4;                   // fewer: the streamed kernel (tensor_scan_kernel) runs instead
-constexpr uint32_t TS8_SLOT_BYTES = 32;
+constexpr uint32_t TS8_SLOT_BYTES = 16;
 constexpr uint32_t TS8_LSTAGE = TS8_SLOT_BYTES / 4 - 1;  // ids staged per (thread, query)
+constexpr int TS8_NG = 16;                               // the kernel runs k <= 12 (NG = 16) only
 constexpr int TS8_BAR_TURN = 2;                          // named barriers 2 and 3: "warpgroup 0 / 1 may issue its K loop"
-constexpr size_t TS8_SMEM_FIXED = 1024 + (size_t)TS_CONSUMERS * 4 * TS8_SLOT_BYTES + (2 * TS8_MAX_STAGES + 1) * 8;
+constexpr uint32_t TS8_BOUND_WARP = TS_CONSUMERS / 32 + 1;
+constexpr size_t TS8_SMEM_FIXED = 1024 + (size_t)TS_CONSUMERS * 4 * TS8_SLOT_BYTES + (size_t)TS8_NG * TS_BLOCK_M * 4 +
+                                  (size_t)TS_BLOCK_M * (4 + 16 + 4) + 16 + (2 * TS8_MAX_STAGES + 1) * 8;
+
+// One bound-warp round over the CTA's query tile (lane: queries lane + 32j).  push: raise the global class maxima from the
+// CTA's first.
+template <int NG>
+__device__ __forceinline__ void s8_bound_round(const TensorScanArgs &a, uint32_t mt, const int *cls, float *sbound, int lane, bool push) {
+#pragma unroll 1
+    for (int j = 0; j < TS_BLOCK_M / 32; ++j) {
+        const uint32_t ql = lane + 32 * j;
+        if (mt * TS_BLOCK_M + ql >= a.n_queries) break;
+        int *gq = a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql;
+        int v[NG];
+#pragma unroll
+        for (int c = 0; c < NG; ++c) v[c] = *reinterpret_cast<const volatile int *>(gq + c * TS_BLOCK_M);
+        if (push) {
+#pragma unroll
+            for (int c = 0; c < NG; ++c) {
+                const int m = *reinterpret_cast<const volatile int *>(cls + c * TS_BLOCK_M + ql);
+                if (m > v[c]) { atomicMax(gq + c * TS_BLOCK_M, m); v[c] = m; }
+            }
+        }
+        // the k-th largest: the largest value that at least k of the NG values reach (ordered ints order like the floats)
+        int b = INT_MIN;
+#pragma unroll
+        for (int i = 0; i < NG; ++i) {
+            uint32_t n = 0;
+#pragma unroll
+            for (int c = 0; c < NG; ++c) n += v[c] >= v[i];
+            b = n >= a.k ? max(b, v[i]) : b;
+        }
+        volatile float *sb = sbound + ql;
+        if (ord2f(b) > *sb) *sb = ord2f(b);
+    }
+}
 
 template <int NG, bool HAS_DEG, bool PROF>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_x, TensorScanArgs a) {
+    static_assert(NG <= TS8_NG, "the shared class maxima hold TS8_NG classes");
     constexpr int NL = NG / 4;   // classes a thread owns per query
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t *qtile = smem;                                          // [kblocks] x 16 KB
     uint8_t *ring = qtile + (size_t)a.kblocks * TS8_KB_BYTES;       // [stages] x 16 KB
-    uint8_t *lstage = ring + (size_t)a.stages * TS8_KB_BYTES;       // [256][4] x 32 B
-    uint64_t *full_bar = reinterpret_cast<uint64_t *>(lstage + TS_CONSUMERS * 4 * TS8_SLOT_BYTES);
+    uint8_t *lstage = ring + (size_t)a.stages * TS8_KB_BYTES;       // [256][4] x 16 B
+    int *cls = reinterpret_cast<int *>(lstage + TS_CONSUMERS * 4 * TS8_SLOT_BYTES);   // [NG][128] CTA class maxima (ordered)
+    float *sbound = reinterpret_cast<float *>(cls + TS8_NG * TS_BLOCK_M);             // [128] bound A of each query
+    float4 *qpar = reinterpret_cast<float4 *>(sbound + TS_BLOCK_M);                   // [128] {s_q, 1/s_q down, up, eps_a}
+    float *qeps = reinterpret_cast<float *>(qpar + TS_BLOCK_M);                       // [128] eps_b
+    uint32_t *ctl = reinterpret_cast<uint32_t *>(qeps + TS_BLOCK_M);                  // [0] epilogues, [1] warpgroups done
+    uint64_t *full_bar = reinterpret_cast<uint64_t *>(ctl + 4);
     uint64_t *empty_bar = full_bar + TS8_MAX_STAGES, *q_bar = empty_bar + TS8_MAX_STAGES;
 
     const int lane = threadIdx.x & 31;
@@ -623,11 +682,26 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         for (uint32_t s = 0; s < a.stages; ++s) { mbar_init(smem_u32(&full_bar[s]), 1); mbar_init(smem_u32(&empty_bar[s]), 4); }
         mbar_init(smem_u32(q_bar), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        ctl[0] = ctl[1] = 0;
     }
+    for (uint32_t i = threadIdx.x; i < (uint32_t)NG * TS_BLOCK_M; i += TS_THREADS) cls[i] = (int)0x807FFFFF;   // f2ord(-inf)
+    if (threadIdx.x < TS_BLOCK_M) {
+        // per query: s_q and its reciprocals, and eps(q,T) = eps_a * E_T + eps_b rounded up (a padding row's values are
+        // never used)
+        const uint32_t qi = mt * TS_BLOCK_M + threadIdx.x;
+        const float2 se = qi < a.n_queries ? a.q_se[qi] : make_float2(0.0f, 0.0f);
+        const float2 rc = qi < a.n_queries ? a.q_rcp[qi] : make_float2(0.0f, 0.0f);
+        qpar[threadIdx.x] = make_float4(se.x, rc.x, rc.y, __fadd_ru(a.dn1, se.y));
+        qeps[threadIdx.x] = __fmaf_ru(se.y, a.dn1, a.dref);
+        sbound[threadIdx.x] = -INFINITY;
+    }
+    __syncthreads();
+    // what earlier launches (the seeding pass) and other CTAs already know, before the first epilogue reads it
+    if (threadIdx.x / 32 == TS8_BOUND_WARP && T > 0) s8_bound_round<NG>(a, mt, cls, sbound, lane, false);
     __syncthreads();
 
     if (threadIdx.x >= TS_CONSUMERS) {
-        // ===================== TMA producer =====================
+        // ===================== TMA producer and bound warp =====================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
         if (threadIdx.x == TS_CONSUMERS && T > 0) {
             unsigned long long p_empty = 0, p_drift = 0, p_t0 = PROF ? clock64() : 0;
@@ -667,6 +741,29 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                 atomicAdd(a.prof + TS_PROF_PRODUCER, clock64() - p_t0);
                 atomicAdd(a.prof + TS_PROF_CTAS, 1ull);
             }
+        } else if (threadIdx.x / 32 == TS8_BOUND_WARP && T > 0) {
+            // one round per completed warpgroup epilogue, until the consumers have published their final class maxima
+            unsigned long long p_ref = 0, n_rounds = 0;
+            uint32_t seen = 0;
+            for (;;) {
+                uint32_t done, ep;
+                for (;;) {
+                    ep = __shfl_sync(0xffffffffu, *reinterpret_cast<volatile uint32_t *>(ctl), 0);
+                    done = __shfl_sync(0xffffffffu, *reinterpret_cast<volatile uint32_t *>(ctl + 1), 0);
+                    if (ep != seen || done == 2) break;
+                    __nanosleep(128);
+                }
+                if (done == 2) break;
+                seen = ep;
+                const unsigned long long c0 = PROF ? clock64() : 0;
+                s8_bound_round<NG>(a, mt, cls, sbound, lane, true);
+                __syncwarp();
+                if (PROF) { p_ref += clock64() - c0; ++n_rounds; }
+            }
+            if (PROF && lane == 0) {
+                atomicAdd(a.prof + TS_PROF_REFRESH, p_ref);
+                atomicAdd(a.prof + TS_PROF_BOUND_ROUNDS, n_rounds);
+            }
         }
         return;
     }
@@ -674,26 +771,23 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     // ===================== consumers: MMA + threshold filter =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const uint32_t ct = threadIdx.x, wg = ct >> 7, wl = (ct >> 5) & 3, qd = (uint32_t)lane & 3;
-    float bound[4], gm[4][NL];
+    float gm[4][NL];   // this thread's share of the CTA's class maxima (the shared `cls` is raised whenever one grows)
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-        const uint32_t ql = 64 * (i >> 1) + 16 * wl + ((uint32_t)lane >> 2) + 8 * (i & 1), qi = mt * TS_BLOCK_M + ql;
-        const bool qvalid = qi < a.n_queries;
         reinterpret_cast<uint32_t *>(lstage + (size_t)(ct * 4 + i) * TS8_SLOT_BYTES)[0] = 0;
 #pragma unroll
         for (int l = 0; l < NL; ++l) gm[i][l] = -INFINITY;
-        // what earlier launches (the seeding pass) and other CTAs already know
-        bound[i] = qvalid ? class_bound<NG>(a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql, a.k) : -INFINITY;
     }
     if (T == 0) return;
     if (wg == 1) named_bar_arrive<TS8_BAR_TURN, 256>();   // warpgroup 0 takes the first turn
     mbar_wait(smem_u32(q_bar), 0);
     const uint32_t q0 = smem_u32(qtile), r0 = smem_u32(ring);
-    unsigned long long p_turn = 0, p_full = 0, p_mma = 0, p_epi = 0, p_ref = 0, p_c = PROF ? clock64() : 0;
+    unsigned long long p_turn = 0, p_full = 0, p_mma = 0, p_thr = 0, p_fold = 0, p_emit = 0, p_c = PROF ? clock64() : 0;
     for (uint32_t t = 0; t < T; ++t) {
         const uint32_t nt = g + t * G;
         const uint64_t row0 = (uint64_t)nt * TS_BLOCK_N + wg * TS8_HALF;   // this warpgroup's half
-        const float2 se = __ldg(a.tile_se + nt);                           // {s_T, E_T} of the 256-row tile, both halves
+        // {s_T, E_T} and {1/s_T down, up} of the 256-row tile (both halves), loaded before the MMAs
+        const float2 se = __ldg(a.tile_se + nt), rt = __ldg(a.tile_rcp + nt);
         // ring position of this turn's first k-block: turn 2t + wg of the sequence
         const uint32_t p0 = (2 * t + wg) * a.kblocks;
         uint32_t s = p0 % a.stages, phase = (p0 / a.stages) & 1u;
@@ -749,30 +843,36 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         const bool full_half = row0 + TS8_HALF <= a.n_rows;   // only the corpus' last tile can be partial
         const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;
         // the four queries' thresholds first, as four independent chains: a warp runs this epilogue alone on its SM
-        // sub-partition (the other warpgroup is in its K loop), so a load -> divide chain per query would be exposed
-        // four times over.  {s_q, e_q} come from L1 rather than from 8 registers held across the K loop (a padding
-        // row's values are never used).
+        // sub-partition (the other warpgroup is in its K loop).  s_T*s_q rounded down and up, eps(q,T) rounded up, and
+        // thrI <= (A - eps) / (s_T*s_q) through the reciprocals rounded the safe way for the numerator's sign:
+        // fl_down(fl_down(num * 1/s_T) * 1/s_q), down for num >= 0, up otherwise (s_T or s_q = 0: as the division did)
         float slo[4], shi[4], eps[4];
         int thrI[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const uint32_t qi = mt * TS_BLOCK_M + qrow + 64 * (i >> 1) + 8 * (i & 1);
-            const float2 qse = __ldg(a.q_se + min(qi, a.n_queries - 1));
-            // s_T*s_q rounded down and up, eps(q,T) rounded up, thrI <= (A - eps) / (s_T*s_q)
-            slo[i] = __fmul_rd(se.x, qse.x);
-            shi[i] = __fmul_ru(se.x, qse.x);
-            eps[i] = __fmaf_ru(__fadd_ru(a.dn1, qse.y), se.y, __fmaf_ru(qse.y, a.dn1, a.dref));
-            const float num = __fsub_rd(bound[i], eps[i]);
-            thrI[i] = __float2int_rd(__fdiv_rd(num, num >= 0.0f ? shi[i] : slo[i]));
+            const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
+            const float4 qp = qpar[ql];
+            slo[i] = __fmul_rd(se.x, qp.x);
+            shi[i] = __fmul_ru(se.x, qp.x);
+            eps[i] = __fmaf_ru(qp.w, se.y, qeps[ql]);
+            const float num = __fsub_rd(*reinterpret_cast<const volatile float *>(sbound + ql), eps[i]);
+            const bool pos = num >= 0.0f;
+            thrI[i] = __float2int_rd(__fmul_rd(__fmul_rd(num, pos ? rt.x : rt.y), pos ? qp.y : qp.z));
         }
+        unsigned long long c_fold = 0;
+        if (PROF) {
+            c_fold = clock64();
+            p_thr += c_fold - c_epi;
+        }
+        // class maxima, their fold and the hit test of all four queries, then one warp-uniform branch to the emission
+        bool hit[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1), qi = mt * TS_BLOCK_M + ql;
+            const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
             const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);   // value (j, b) at v_i[4j + b]
             int cm[NL];
 #pragma unroll
             for (int l = 0; l < NL; ++l) cm[l] = INT_MIN;
-            bool hit;
             if (full_half) {
                 int zmax = INT_MIN;   // HAS_DEG: 0 if some accumulator of the half is exactly zero
 #pragma unroll
@@ -791,7 +891,7 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                 int cmax = zmax;
 #pragma unroll
                 for (int l = 0; l < NL; ++l) cmax = max(cmax, cm[l]);
-                hit = cmax >= thrI[i];
+                hit[i] = cmax >= thrI[i];
             } else {
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -803,14 +903,30 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                         if ((uint64_t)col < left && !(HAS_DEG && v == 0)) cm[l] = max(cm[l], v);
                     }
                 }
-                hit = true;
+                hit[i] = true;
             }
+            hit[i] = hit[i] && mt * TS_BLOCK_M + ql < a.n_queries;
             // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class
 #pragma unroll
-            for (int l = 0; l < NL; ++l)
-                if (cm[l] != INT_MIN)
-                    gm[i][l] = fmaxf(gm[i][l], __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo[i] : shi[i]), eps[i]));
-            if (qi < a.n_queries && a.emit && hit) {
+            for (int l = 0; l < NL; ++l) {
+                const float lb = __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo[i] : shi[i]), eps[i]);
+                if (cm[l] != INT_MIN && lb > gm[i][l]) {
+                    gm[i][l] = lb;
+                    atomicMax(cls + (8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M + ql, f2ord(lb));
+                }
+            }
+        }
+        unsigned long long c_emit = 0;
+        if (PROF) {
+            c_emit = clock64();
+            p_fold += c_emit - c_fold;
+        }
+        if (a.emit && __any_sync(0xffffffffu, hit[0] || hit[1] || hit[2] || hit[3])) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                if (!hit[i]) continue;
+                const uint32_t qi = mt * TS_BLOCK_M + qrow + 64 * (i >> 1) + 8 * (i & 1);
+                const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);
                 uint32_t *stage = reinterpret_cast<uint32_t *>(lstage + (size_t)(me * 4 + i) * TS8_SLOT_BYTES);
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -818,46 +934,22 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                     for (int b = 0; b < 2; ++b) {
                         const uint32_t col = 8 * j + 2 * (me & 3) + b;
                         if ((uint64_t)col < left && (int)v_i[4 * j + b] >= thrI[i])
-                            epi_emit<TS8_LSTAGE>(a, qi, stage, a.id_base + (uint32_t)(row0 + col));
+                            epi_emit<TS8_LSTAGE>(a.cand, a.cand_cnt, a.cand_cap, qi, stage, a.id_base + (uint32_t)(row0 + col));
                     }
                 }
             }
         }
-        unsigned long long c_ref = 0;
-        if (PROF) {
-            c_ref = clock64();
-            p_epi += c_ref - c_epi;
-        }
-        // refresh the shared bound at tensor_scan_kernel's cadence (per tile of the CTA)
-        if (t < 8 || (t & a.refresh_mask) == a.refresh_mask || !a.emit) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
-                if (mt * TS_BLOCK_M + ql >= a.n_queries) continue;
-                int *ggm_q = a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql;
-#pragma unroll
-                for (int l = 0; l < NL; ++l) {
-                    int *p = ggm_q + (size_t)(8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M;
-                    const int mine = f2ord(gm[i][l]);
-                    if (mine > *reinterpret_cast<volatile int *>(p)) atomicMax(p, mine);
-                }
-            }
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
-                if (mt * TS_BLOCK_M + ql >= a.n_queries) continue;
-                bound[i] = fmaxf(bound[i], class_bound<NG>(a.ggm + (size_t)mt * NG * TS_BLOCK_M + ql, a.k));
-            }
-        }
-        if (PROF) p_ref += clock64() - c_ref;
+        if ((me & 127) == 0) atomicAdd(ctl, 1u);   // wakes the bound warp
+        if (PROF) p_emit += clock64() - c_emit;
     }
     if (PROF && (ct & 127) == 0) {
         atomicAdd(a.prof + TS_PROF_MATH_WAIT, p_turn);
         atomicAdd(a.prof + TS_PROF_FULL_WAIT, p_full);
         atomicAdd(a.prof + TS_PROF_MMA, p_mma);
-        atomicAdd(a.prof + TS_PROF_EPILOGUE, p_epi);
-        atomicAdd(a.prof + TS_PROF_REFRESH, p_ref);
+        atomicAdd(a.prof + TS_PROF_EPILOGUE, p_thr + p_fold + p_emit);
+        atomicAdd(a.prof + TS_PROF_EPI_THR, p_thr);
+        atomicAdd(a.prof + TS_PROF_EPI_FOLD, p_fold);
+        atomicAdd(a.prof + TS_PROF_EPI_EMIT, p_emit);
         atomicAdd(a.prof + TS_PROF_TILES, (unsigned long long)T);
         atomicAdd(a.prof + TS_PROF_CONSUMER, clock64() - p_c);
     }
@@ -877,6 +969,7 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                 if (pos + x < a.cand_cap) a.cand[(size_t)qi * a.cand_cap + pos + x] = stage[1 + x];
         }
     }
+    if ((ct & 127) == 0) atomicAdd(ctl + 1, 1u);   // the bound warp stops once both warpgroups have published
 }
 
 // ------------------------------------------------------------------ fp16 normalised copies
@@ -935,11 +1028,12 @@ __device__ __forceinline__ float residual_norm_up(double e2) {
 // x_hat = x / |x| exactly as normalize_f16_kernel computes it, s_T = max |x_hat_i| / 127 over the tile's proper rows,
 // codes rint(x_hat / s_T), E_T >= max over proper rows of |x_hat - s_T * codes| (f64, rounded up).  Degenerate and
 // deleted rows get zero codes and no say in s_T or E_T.  tiles (may be null): the CTA's tile is tiles[blockIdx.x].
+// tile_rcp[t] = {1/s_T rounded down, 1/s_T rounded up}: the s8 scan's threshold multiplies by them instead of dividing.
 __global__ void __launch_bounds__(256) quantize_s8_tiles_kernel(const float *__restrict__ raw, uint32_t pitch_elems,
                                                                 const float *__restrict__ mags, uint32_t tile0, uint64_t row_end,
                                                                 uint32_t dim, int8_t *__restrict__ xs8, uint32_t pitch8,
-                                                                float2 *__restrict__ tile_se, const uint32_t *__restrict__ tiles,
-                                                                const uint32_t *__restrict__ deleted) {
+                                                                float2 *__restrict__ tile_se, float2 *__restrict__ tile_rcp,
+                                                                const uint32_t *__restrict__ tiles, const uint32_t *__restrict__ deleted) {
     __shared__ float s_max[8];
     __shared__ double s_e2[8];
     const uint32_t t = tiles ? tiles[blockIdx.x] : tile0 + blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -975,6 +1069,7 @@ __global__ void __launch_bounds__(256) quantize_s8_tiles_kernel(const float *__r
     if (threadIdx.x == 0) {
         for (int w = 1; w < 8; ++w) e2 = fmax(e2, s_e2[w]);
         tile_se[t] = make_float2(st, residual_norm_up(e2));
+        tile_rcp[t] = make_float2(__frcp_rd(st), __frcp_ru(st));   // s_T = 0: +inf, see tensor_scan_s8_kernel's threshold
     }
 }
 
@@ -993,12 +1088,13 @@ __global__ void __launch_bounds__(1024) s8_emax_kernel(const float2 *__restrict_
 }
 
 cdb_status quantize_s8_device(const float *d_raw, uint32_t pitch_elems, const float *d_mags, uint64_t first, uint64_t n,
-                              uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
-                              const uint32_t *d_deleted, cudaStream_t s) {
+                              uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float2 *d_tile_rcp,
+                              float *d_emax, const uint32_t *d_deleted, cudaStream_t s) {
     if (!n) return CDB_OK;
     const uint32_t t0 = (uint32_t)(first / TS_BLOCK_N), t1 = (uint32_t)((first + n + TS_BLOCK_N - 1) / TS_BLOCK_N);
     quantize_s8_tiles_kernel<<<t1 - t0, 256, 0, s>>>(d_raw, pitch_elems, d_mags, t0, row_end, dim,
-                                                     reinterpret_cast<int8_t *>(d_xs8), pitch8, d_tile_se, nullptr, d_deleted);
+                                                     reinterpret_cast<int8_t *>(d_xs8), pitch8, d_tile_se, d_tile_rcp, nullptr,
+                                                     d_deleted);
     CDB_LAUNCH_CHECK();
     s8_emax_kernel<<<1, 1024, 0, s>>>(d_tile_se, (uint32_t)((row_end + TS_BLOCK_N - 1) / TS_BLOCK_N), d_emax);
     CDB_LAUNCH_CHECK();
@@ -1013,15 +1109,15 @@ __global__ void zero_rows_kernel(const uint32_t *__restrict__ rows, uint8_t *bas
 
 cdb_status shadow_drop_rows_device(const uint32_t *d_rows, uint32_t n_rows, const uint32_t *d_tiles, uint32_t n_tiles, void *d_xh,
                                    uint32_t xh_pitch_halfs, const float *d_raw, uint32_t pitch_elems, const float *d_mags,
-                                   uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float *d_emax,
-                                   const uint32_t *d_deleted, cudaStream_t s) {
+                                   uint64_t row_end, uint32_t dim, void *d_xs8, uint32_t pitch8, float2 *d_tile_se, float2 *d_tile_rcp,
+                                   float *d_emax, const uint32_t *d_deleted, cudaStream_t s) {
     if (n_rows) {
         zero_rows_kernel<<<n_rows, 128, 0, s>>>(d_rows, reinterpret_cast<uint8_t *>(d_xh), xh_pitch_halfs * 2);
         CDB_LAUNCH_CHECK();
     }
     if (d_xs8 && n_tiles) {
         quantize_s8_tiles_kernel<<<n_tiles, 256, 0, s>>>(d_raw, pitch_elems, d_mags, 0, row_end, dim, reinterpret_cast<int8_t *>(d_xs8),
-                                                         pitch8, d_tile_se, d_tiles, d_deleted);
+                                                         pitch8, d_tile_se, d_tile_rcp, d_tiles, d_deleted);
         CDB_LAUNCH_CHECK();
         s8_emax_kernel<<<1, 1024, 0, s>>>(d_tile_se, (uint32_t)((row_end + TS_BLOCK_N - 1) / TS_BLOCK_N), d_emax);
         CDB_LAUNCH_CHECK();
@@ -1058,7 +1154,7 @@ cdb_status classify_rows_device(const float *d_raw, uint32_t pitch_elems, const 
 //   q_mags  |q| = sqrt of the SEQUENTIAL fold of x*x (vector_store.rs:412), one thread, squares staged in shared memory
 //   qh      fp16 copy of q / |q| (zero row for a degenerate norm and for the padding rows up to mtiles*128), or with q_se
 //           (s8 form, KIND 2) s8 codes rint(q_hat / s_q) with s_q = max |q_hat_i| / 127 (qh_pitch then counts bytes) and
-//           q_se = {s_q, e_q >= |q_hat - s_q * codes|}
+//           q_se = {s_q, e_q >= |q_hat - s_q * codes|}, q_rcp = {1/s_q rounded down, rounded up}
 //   ggm     class maxima of the query := -inf;  cand_cnt := number of pre-seeded odd rows (+ their ids);  err := 0
 //   progress counters of the seeding and of the main pass := 0
 // One CTA of 128 threads per query slot (mtiles*128 slots).
@@ -1068,7 +1164,7 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const float *__restri
                                                            uint32_t has_deg, uint32_t id_base, uint32_t *__restrict__ cand,
                                                            uint32_t cand_cap, uint32_t *__restrict__ cand_cnt, uint32_t *__restrict__ err32,
                                                            uint8_t *__restrict__ err8, uint32_t *__restrict__ progress,
-                                                           float2 *__restrict__ q_se) {
+                                                           float2 *__restrict__ q_se, float2 *__restrict__ q_rcp) {
     extern __shared__ float sq[];     // [dim] squares, then (s8 form) q_hat
     __shared__ float s_mag;
     __shared__ float s_max[4];
@@ -1141,20 +1237,23 @@ __global__ void __launch_bounds__(128) prep_queries_kernel(const float *__restri
     e2 = warp_sum_d(e2);
     if (lane == 0) s_e2[warp] = e2;
     __syncthreads();
-    if (tid == 0) q_se[slot] = make_float2(sc, residual_norm_up((s_e2[0] + s_e2[1]) + (s_e2[2] + s_e2[3])));
+    if (tid == 0) {
+        q_se[slot] = make_float2(sc, residual_norm_up((s_e2[0] + s_e2[1]) + (s_e2[2] + s_e2[3])));
+        q_rcp[slot] = make_float2(__frcp_rd(sc), __frcp_ru(sc));
+    }
 }
 
 cdb_status prep_queries_device(const float *d_q, uint32_t nq, uint32_t dim, float *d_q_raw, uint32_t raw_pitch_elems, float *d_q_mags,
                                void *d_qh, uint32_t qh_pitch_halfs, int *d_ggm, const uint32_t *d_deg, bool has_deg, uint32_t id_base,
                                uint32_t *d_cand, uint32_t cand_cap, uint32_t *d_cand_cnt, uint32_t *d_err32, uint8_t *d_err8,
-                               uint32_t *d_progress, float2 *d_q_se, cudaStream_t s) {
+                               uint32_t *d_progress, float2 *d_q_se, float2 *d_q_rcp, cudaStream_t s) {
     const uint32_t mtiles = (nq + TS_BLOCK_M - 1) / TS_BLOCK_M;
     // dim*4 bytes of squares: above 12287 dims that exceeds the 48 KB a launch gets without the opt-in
     CDB_ALLOW_SMEM(prep_queries_kernel, (size_t)dim * 4);
     prep_queries_kernel<<<mtiles * TS_BLOCK_M, 128, (size_t)dim * 4, s>>>(d_q, nq, dim, d_q_raw, raw_pitch_elems, d_q_mags,
                                                                           reinterpret_cast<__half *>(d_qh), qh_pitch_halfs, d_ggm, d_deg,
                                                                           has_deg ? 1u : 0u, id_base, d_cand, cand_cap, d_cand_cnt, d_err32,
-                                                                          d_err8, d_progress, d_q_se);
+                                                                          d_err8, d_progress, d_q_se, d_q_rcp);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }
@@ -1372,10 +1471,11 @@ static float f32_up(double x) {
 }
 
 // s8 form (KIND 2, DESIGN.md section 5c): d_xs8 s8 shadow [n_rows][pitch8], d_qs8 query codes padded with zero rows to a
-// multiple of 128, d_tile_se / d_q_se their {scale, residual bound}.  Same candidates / class maxima contract as
+// multiple of 128, d_tile_se / d_q_se their {scale, residual bound}, d_tile_rcp / d_q_rcp the scales' reciprocals.  Same candidates / class maxima contract as
 // tensor_scan_device; prep_queries_device (s8 mode) has reset them.
 cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t pitch8, uint64_t n_rows, uint32_t nq, uint32_t dim,
-                                 uint32_t k, const float2 *d_tile_se, const float2 *d_q_se, uint32_t id_base, int *d_ggm,
+                                 uint32_t k, const float2 *d_tile_se, const float2 *d_tile_rcp, const float2 *d_q_se,
+                                 const float2 *d_q_rcp, uint32_t id_base, int *d_ggm,
                                  uint32_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_progress, bool has_deg,
                                  int sm_count, cudaStream_t s) {
     TensorScanArgs a{};
@@ -1396,7 +1496,9 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
     a.cand_cnt = d_cand_cnt;
     a.cand_cap = cand_cap;
     a.tile_se = d_tile_se;
+    a.tile_rcp = d_tile_rcp;
     a.q_se = d_q_se;
+    a.q_rcp = d_q_rcp;
     // u = 2^-24.  |x_hat|, |q_hat| <= 1 + (D/2 + 2) u + O(D^2 u^2) (sequential f32 norm, one division per entry);
     // |cos_ref - q_hat . x_hat| <= (D + 4) u + O(D^2 u^2) (FMA dot product, norm product, division).  Both are taken
     // twice over, which covers the second-order terms for every D <= rerank_f32_max_dim().
