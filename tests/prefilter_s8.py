@@ -73,9 +73,12 @@ def quantize_set(xh, ok):
     return c, s, _up(e * (1 + 2.0 ** -30))
 
 
-def quantize_corpus(x):
-    """-> (codes [n, D], s_T [tiles], E_T [tiles]) with tiles of 256 rows aligned to row 0"""
+def quantize_corpus(x, deleted=None):
+    """-> (codes [n, D], s_T [tiles], E_T [tiles]) with tiles of 256 rows aligned to row 0.  deleted (bool [n], may be
+    None): those rows get zero codes and no say in s_T / E_T, as in quantize_s8_tiles_kernel"""
     xh, ok = normalized(x)
+    if deleted is not None:
+        ok = ok & ~np.asarray(deleted, bool)
     codes = np.zeros(xh.shape, np.int64)
     nt = (len(x) + TILE - 1) // TILE
     s, e = np.zeros(nt, F32), np.zeros(nt)
@@ -91,17 +94,53 @@ def quantize_queries(q):
     return np.concatenate([o[0] for o in out]), np.array([o[1] for o in out], F32), np.array([o[2] for o in out])
 
 
-def scores_and_eps(queries, rows):
-    """a[q, r] = s_T s_q (c_q . c_x) (f64) and eps[q, r] = eps(q, T(r))"""
+def filter_terms(queries, rows, deleted=None, corpus=None):
+    """-> (dp, s, eps), each [nq, n] f64: the exact s32 dot product c_q . c_x of the codes, s = s_T s_q and eps(q, T(r)).
+    The float64 product of the integer codes is exact: |dp| <= 127^2 D < 2^53.  corpus: quantize_corpus(rows, deleted)
+    if the caller has it already."""
     dim = rows.shape[1]
-    cx, sx, ex = quantize_corpus(rows)
+    cx, sx, ex = corpus if corpus is not None else quantize_corpus(rows, deleted)
     cq, sq, eq = quantize_queries(queries)
     tile = np.arange(len(rows)) // TILE
-    dp = cq @ cx.T
-    a = dp * (sq.astype(np.float64)[:, None] * sx.astype(np.float64)[tile][None, :])
+    dp = cq.astype(np.float64) @ cx.astype(np.float64).T
+    s = sq.astype(np.float64)[:, None] * sx.astype(np.float64)[tile][None, :]
     dn, dref = deltas(dim)
     e = (1 + dn + eq[:, None]) * ex[tile][None, :] + eq[:, None] * (1 + dn) + dref
-    return a, e
+    return dp, s, e
+
+
+def scores_and_eps(queries, rows, deleted=None):
+    """a[q, r] = s_T s_q (c_q . c_x) (f64) and eps[q, r] = eps(q, T(r))"""
+    dp, s, e = filter_terms(queries, rows, deleted)
+    return dp * s, e
+
+
+def class_maxima(lb, ng, use=None):
+    """-> (maxima [nq, ng], argmax rows [nq, ng]) of lb [nq, n] over the classes row mod ng; rows where use [nq, n] (or
+    [n]) is False have no say, an empty class is -inf"""
+    nq, n = lb.shape
+    v = np.where(use, lb, -np.inf) if use is not None else lb
+    v = np.concatenate([v, np.full((nq, (-n) % ng), -np.inf)], axis=1).reshape(nq, -1, ng)
+    j = v.argmax(axis=1)
+    return np.take_along_axis(v, j[:, None, :], axis=1)[:, 0, :], j * ng + np.arange(ng)[None, :]
+
+
+def kth_largest(cm, k):
+    """A = the k-th largest of each query's class maxima"""
+    return np.sort(cm, axis=1)[:, cm.shape[1] - k]
+
+
+def filter_bounds(dp, s, e, k, has_deg, seed_rows):
+    """-> (A*, A_seed) per query: the k-th largest class maximum of the lower bounds a - eps over all rows, and over the
+    seeding pass's row prefix [0, seed_rows).  has_deg: rows with dp == 0 have no say (the HAS_DEG rule: a deleted or
+    degenerate row has a zero code row, and the kernel cannot tell it from a proper row that scores exactly 0)."""
+    ng = pa.ng_for_k(k)
+    lb = dp * s - e
+    use = dp != 0 if has_deg else np.ones(dp.shape, bool)
+    a_all = kth_largest(class_maxima(lb, ng, use)[0], k)
+    m = min(seed_rows, dp.shape[1])
+    a_seed = kth_largest(class_maxima(lb[:, :m], ng, use[:, :m])[0], k)
+    return a_all, a_seed
 
 
 def filter_keeps(a_row, e_row, k, scale=1.0):
