@@ -216,6 +216,8 @@ PROTOTYPES = {
     "cdb_index_hnsw_counters": (C.c_int32, [C.c_void_p, C.c_void_p]),
     "cdb_search_batch": (C.c_int32, [C.c_void_p, c_f32p, C.c_uint32, C.POINTER(SearchParams), c_u32p, c_f32p, c_u32p, c_u8p]),
     "cdb_search_batch_device": (C.c_int32, [C.c_void_p, c_f32p, C.c_uint32, C.POINTER(SearchParams), c_u32p, c_f32p, c_u32p, c_u8p, C.c_void_p]),
+    "cdb_search_batch_filtered_device": (C.c_int32, [C.c_void_p, c_f32p, C.c_uint32, C.POINTER(SearchParams), c_u32p, c_vp, C.c_uint32,
+                                                     c_u8p, c_u32p, c_f32p, c_u32p, c_u8p, C.c_void_p]),
     "cdb_score_ids": (C.c_int32, [C.c_void_p, c_f32p, c_u32p, C.c_uint32, c_f32p, c_i32p]),
     "cdb_rerank_f32": (C.c_int32, [C.c_void_p, c_f32p, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p]),
     "cdb_nccl_unique_id": (C.c_int32, [C.c_void_p]),

@@ -564,6 +564,18 @@ class DenseIndex:
         _check(self._lib.cdb_index_set_graph_slot_scores(self._h, C.cast(t_sc, C.c_void_p),
                                                          None if t_tg is None else C.cast(t_tg, C.c_void_p)))
 
+    def pack_filters(self, filters):
+        """filters[q]: None (no filter) or a list of int8[md_dims] (QueryFilterDimensions) -> the CSR form of the C API:
+        (offsets u32[B+1], dims i8[rows, md_dims], has_filter u8[B])"""
+        offs, rows, has = [0], [], []
+        for f in filters:
+            has.append(0 if f is None else 1)
+            for dims in (f or []):
+                rows.append(np.asarray(dims, dtype=np.int8).reshape(self.md_dims))
+            offs.append(len(rows))
+        dims = np.ascontiguousarray(np.stack(rows)) if rows else np.zeros((0, self.md_dims), dtype=np.int8)
+        return np.array(offs, dtype=np.uint32), dims, np.array(has, dtype=np.uint8)
+
     def batch_search_filtered(self, queries, filters, k, **kw):
         """search_internal with per-query metadata filters: filters[q] is None or a list of int8[md_dims] (QueryFilterDimensions)
         -> (replica ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B])"""
@@ -571,15 +583,9 @@ class DenseIndex:
         if q.ndim == 1:
             q = q[None]
         b = q.shape[0]
-        offs, rows, has = [0], [], []
-        for f in filters:
-            has.append(0 if f is None else 1)
-            for dims in (f or []):
-                rows.append(np.asarray(dims, dtype=np.int8).reshape(self.md_dims))
-            offs.append(len(rows))
-        offs = np.array(offs, dtype=np.uint32)
-        has = np.array(has, dtype=np.uint8)
-        dims = np.ascontiguousarray(np.stack(rows)) if rows else np.zeros((1, self.md_dims), dtype=np.int8)
+        offs, dims, has = self.pack_filters(filters)
+        if dims.shape[0] == 0:
+            dims = np.zeros((1, self.md_dims), dtype=np.int8)
         ids = np.zeros((b, k), dtype=np.uint32)
         scores = np.zeros((b, k), dtype=np.float32)
         counts = np.zeros(b, dtype=np.uint32)
@@ -588,6 +594,16 @@ class DenseIndex:
         _check(self._lib.cdb_search_batch_filtered(self._h, _ptr(q), b, C.byref(p), _ptr(offs), _ptr(dims), _ptr(has), _ptr(ids),
                                                    _ptr(scores), _ptr(counts), _ptr(err)))
         return ids, scores, counts, err
+
+    def batch_search_filtered_device(self, d_queries_ptr, b, k, d_offsets_ptr, d_dims_ptr, n_filter_rows, d_has_ptr, d_ids_ptr,
+                                     d_scores_ptr, d_counts_ptr=None, d_err_ptr=None, stream_ptr=None, **kw):
+        """batch_search_filtered on device buffers (cdb_search_batch_filtered_device): every pointer is a device address (int),
+        the filters in the CSR form of pack_filters (d_has_ptr None = no query has a filter); asynchronous on stream_ptr.
+        A query whose offsets are out of order or past n_filter_rows gets err flag 8 (BAD_FILTER) and count 0."""
+        p = self.params(k, SearchMode.HNSW, **kw)
+        _check(self._lib.cdb_search_batch_filtered_device(self._h, d_queries_ptr, b, C.byref(p), d_offsets_ptr, d_dims_ptr,
+                                                          n_filter_rows, d_has_ptr, d_ids_ptr, d_scores_ptr, d_counts_ptr, d_err_ptr,
+                                                          stream_ptr))
 
     def hnsw_counters(self):
         out = np.zeros(2, dtype=np.uint64)

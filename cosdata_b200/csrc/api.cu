@@ -778,7 +778,8 @@ static cdb_status exact_scan_locked(cdb_index *ix, Scratch *sc, bool raw, int st
 // remove_duplicates_and_filter and the exact f32 re-rank of finalize_ann_results.
 static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
                                      uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s,
-                                     const uint32_t *d_foff = nullptr, const int8_t *d_fdims = nullptr, const uint8_t *d_fhas = nullptr) {
+                                     const uint32_t *d_foff = nullptr, const int8_t *d_fdims = nullptr, uint32_t n_frows = 0,
+                                     const uint8_t *d_fhas = nullptr) {
     const cdb_index_desc &d = ix->desc;
     CDB_REQUIRE(ix->has_graph, "CDB_MODE_HNSW needs cdb_index_set_graph");
     CDB_REQUIRE(ix->has_md || !d_fhas, "metadata filters need cdb_index_set_graph_metadata");
@@ -833,12 +834,14 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
     a.out_n = sc->hn_n.as<uint32_t>();
     a.err32 = sc->err32.as<uint32_t>();
     a.counters = ix->hn_counters.as<unsigned long long>();
+    a.flags = g_hnsw_flags.load();
     const int slot = (int)(ix->n_search.fetch_add(1) % cdb_index::EV_RING);
     CDB_CUDA_TRY(cudaEventRecord(sc->ev[0], s));
     CDB_CUDA_TRY(cudaEventRecord(ix->ring0[slot], s));
     if (ix->has_md) {
-        // graph with replica nodes: metadata-aware traversal (hnsw_md.cu); results carry replica ids, the re-rank scores
-        // the base vector of each replica (collection.rs:368-384)
+        // graph with replica nodes: metadata-aware traversal (one warp per query, hnsw_warp.cu; CDB_HNSW_F_CTA selects the
+        // CTA-per-query kernel of hnsw_md.cu); results carry replica ids, the re-rank scores the base vector of each replica
+        // (collection.rs:368-384)
         HnswMdArgs ma{};
         ma.a = a;
         ma.node_id = ix->md_node_id;
@@ -849,6 +852,7 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
         ma.pseudo_entry = ix->md_pseudo_entry;
         ma.filter_offsets = d_foff;
         ma.filter_dims = d_fdims;
+        ma.n_filter_rows = n_frows;
         ma.has_filter = d_fhas;
         ma.out_ids = sc->hn_ids.as<uint32_t>();
         if ((rc = hnsw_search_md_device(ma, s))) return rc;
@@ -863,7 +867,6 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
             return rc;
     } else {
         // one warp per query (hnsw_warp.cu); CDB_HNSW_F_CTA selects the round-1 CTA-per-query kernel for A/B measurements
-        a.flags = g_hnsw_flags.load();
         a.prof = ix->hn_prof_on ? ix->hn_prof.as<unsigned long long>() : nullptr;
         if ((rc = (a.flags & CDB_HNSW_F_CTA) ? hnsw_search_device(a, s) : hnsw_search_warp_device(a, s))) return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
@@ -1139,6 +1142,27 @@ cdb_status cdb_search_batch(cdb_index *ix, const float *queries, uint32_t nq, co
     return CDB_OK;
 }
 
+}  // extern "C"
+
+// search_internal with metadata filters on device buffers, in chunks of <= 2048 queries (the host and device entry points)
+static cdb_status filtered_device_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
+                                         const uint32_t *d_off, const int8_t *d_dims, uint32_t n_rows, const uint8_t *d_has,
+                                         uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s) {
+    if (sc->ev_valid && sc->last_stream != s) CDB_CUDA_TRY(cudaStreamWaitEvent(s, sc->ev[2], 0));
+    sc->last_stream = s;
+    const uint32_t CH = 2048;
+    for (uint32_t q0 = 0; q0 < nq; q0 += CH) {
+        const uint32_t m = std::min(CH, nq - q0);
+        const cdb_status rc = hnsw_search_locked(ix, sc, d_queries + (size_t)q0 * ix->desc.dim, m, p, d_ids + (size_t)q0 * p->k,
+                                                 d_scores + (size_t)q0 * p->k, d_counts + q0, d_err ? d_err + q0 : nullptr, s,
+                                                 d_off ? d_off + q0 : nullptr, d_dims, n_rows, d_has ? d_has + q0 : nullptr);
+        if (rc) return rc;
+    }
+    return CDB_OK;
+}
+
+extern "C" {
+
 cdb_status cdb_search_batch_filtered(cdb_index *ix, const float *queries, uint32_t nq, const cdb_search_params *p,
                                      const uint32_t *filter_offsets, const int8_t *filter_dims, const uint8_t *has_filter,
                                      uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
@@ -1162,8 +1186,8 @@ cdb_status cdb_search_batch_filtered(cdb_index *ix, const float *queries, uint32
     const uint32_t *d_off = nullptr;
     const int8_t *d_dims = nullptr;
     const uint8_t *d_has = nullptr;
+    uint32_t total = 0;
     if (has_filter) {
-        uint32_t total = 0;
         for (uint32_t q = 0; q < nq; ++q) {
             CDB_REQUIRE(filter_offsets[q] <= filter_offsets[q + 1], "filter_offsets must be non-decreasing");
             CDB_REQUIRE(!has_filter[q] || filter_offsets[q + 1] - filter_offsets[q] <= 4096, "too many filters for one query");
@@ -1179,22 +1203,44 @@ cdb_status cdb_search_batch_filtered(cdb_index *ix, const float *queries, uint32
         d_off = sc->flt_off.as<uint32_t>(); d_dims = sc->flt_dims.as<int8_t>(); d_has = sc->flt_has.as<uint8_t>();
     }
     CDB_CUDA_TRY(cudaMemcpyAsync(sc->io_q.p, queries, (size_t)nq * ix->desc.dim * 4, cudaMemcpyHostToDevice, s));
-    if (sc->ev_valid && sc->last_stream != s) CDB_CUDA_TRY(cudaStreamWaitEvent(s, sc->ev[2], 0));
-    sc->last_stream = s;
-    const uint32_t CH = 2048;
-    for (uint32_t q0 = 0; q0 < nq; q0 += CH) {
-        const uint32_t m = std::min(CH, nq - q0);
-        rc = hnsw_search_locked(ix, sc, sc->io_q.as<float>() + (size_t)q0 * ix->desc.dim, m, p, sc->io_ids.as<uint32_t>() + (size_t)q0 * p->k,
-                                sc->io_scores.as<float>() + (size_t)q0 * p->k, sc->io_counts.as<uint32_t>() + q0,
-                                sc->io_err.as<uint8_t>() + q0, s, d_off ? d_off + q0 : nullptr, d_dims, d_has ? d_has + q0 : nullptr);
-        if (rc) return rc;
-    }
+    if ((rc = filtered_device_locked(ix, sc, sc->io_q.as<float>(), nq, p, d_off, d_dims, total, d_has, sc->io_ids.as<uint32_t>(),
+                                     sc->io_scores.as<float>(), sc->io_counts.as<uint32_t>(), sc->io_err.as<uint8_t>(), s)))
+        return rc;
     CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, sc->io_ids.p, nk * 4, cudaMemcpyDeviceToHost, s));
     CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, sc->io_scores.p, nk * 4, cudaMemcpyDeviceToHost, s));
     if (out_counts) CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, sc->io_counts.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, s));
     if (err_flags) CDB_CUDA_TRY(cudaMemcpyAsync(err_flags, sc->io_err.p, nq, cudaMemcpyDeviceToHost, s));
     CDB_CUDA_TRY(cudaStreamSynchronize(s));
     return CDB_OK;
+}
+
+// the argument checks need no device: they come first so that a refusal never depends on the handle's state
+cdb_status cdb_search_batch_filtered_device(cdb_index *ix, const float *d_queries, uint32_t nq, const cdb_search_params *p,
+                                            const uint32_t *d_filter_offsets, const int8_t *d_filter_dims, uint32_t n_filter_rows,
+                                            const uint8_t *d_has_filter, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                            uint8_t *d_err, void *stream) {
+    CDB_REQUIRE(p, "null params");
+    CDB_REQUIRE(p->mode == CDB_MODE_HNSW, "metadata filters apply to CDB_MODE_HNSW");
+    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    CDB_REQUIRE(!d_has_filter || d_filter_offsets, "has_filter needs filter_offsets");
+    CDB_REQUIRE(d_filter_dims || !n_filter_rows, "n_filter_rows > 0 needs filter_dims");
+    CDB_REQUIRE(ix && (d_queries || !nq) && (d_ids || !nq) && (d_scores || !nq), "null argument");
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    CDB_REQUIRE(ix->has_md || !d_has_filter, "metadata filters need cdb_index_set_graph_metadata");
+    if (!nq) return CDB_OK;
+    Lease l;
+    cdb_status rc = lease_scratch(ix, l);
+    if (rc) return rc;
+    Scratch *sc = l.sc;
+    cudaStream_t s = stream ? (cudaStream_t)stream : sc->stream;
+    if (!d_counts) {
+        if ((rc = sc->io_counts.ensure((size_t)nq * 4))) return rc;
+        d_counts = sc->io_counts.as<uint32_t>();
+    }
+    // asynchronous like cdb_search_batch_device: the set's next user orders itself behind this search
+    return filtered_device_locked(ix, sc, d_queries, nq, p, d_filter_offsets, d_filter_dims, n_filter_rows, d_has_filter, d_ids,
+                                  d_scores, d_counts, d_err, s);
 }
 
 // ------------------------------------------------------------------ S2 / S3

@@ -4,7 +4,9 @@
 //   CosineSimilarity::calculate arms      src/distance/cosine.rs:34-102 (metadata.cuh)
 //   remove_duplicates_and_filter          src/models/common.rs:381-412 (dedup by replica id, pseudo nodes dropped)
 //   get_raw_emb_by_internal_id            src/models/collection.rs:368-384 (replica id -> base vector; here node_row)
-// One CTA per query like hnsw.cu; the traversal itself is the shared hn_traverse_level with a metadata context.
+// One CTA per query like hnsw.cu; the traversal itself is the shared hn_traverse_level with a metadata context.  Searches run
+// the warp-per-query form of the same steps (hnsw_warp.cu); this kernel answers CDB_HNSW_F_CTA and shapes whose warp carve
+// does not fit.
 // Per level and filter the <= 100 results are merged into the level's candidate list z (<= 100 best of all filters,
 // vector_store.rs:306-312), entries scoring exactly -1.0 dropped (:294-303); the fixed set is shared by the filters of a level.
 #include "hnsw_traverse.cuh"
@@ -13,13 +15,6 @@ namespace cdb {
 
 constexpr uint32_t HNM_FINAL = 100;   // vector_store.rs:311, 1194
 constexpr uint32_t HNM_Z = 256;       // z (<= 100) + one traversal (<= 100), padded for the bitonic sort
-
-__device__ __forceinline__ bool hnm_is_pseudo(const HnswMdArgs &a, int level, uint32_t node) {
-    const uint32_t mrow = a.node_md[level][node];
-    if (mrow == HN_EMPTY || a.md_mags[mrow] == 0.0f) return false;
-    const uint32_t id = a.node_id[level][node];
-    return id >= MD_PSEUDO_ID_LO && id <= MD_PSEUDO_ID_HI;
-}
 
 __global__ void __launch_bounds__(HN_THREADS) hnsw_search_md_kernel(HnswMdArgs a) {
     extern __shared__ __align__(16) uint8_t smem[];
@@ -32,12 +27,16 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_search_md_kernel(HnswMdArgs a
     __shared__ float s_fmag;
     const uint32_t qi = blockIdx.x;
     const int tid = threadIdx.x;
+    const bool hasf = a.has_filter && a.has_filter[qi];
+    uint32_t f0 = 0, f1 = 0;
+    if (hasf && !hnm_filter_rows(a, qi, &f0, &f1)) {   // (uniform over the CTA: no barrier is skipped by part of it)
+        if (tid == 0) { a.a.out_n[qi] = 0; atomicOr(a.a.err32 + qi, (uint32_t)CDB_ERRFLAG_BAD_FILTER); }
+        return;
+    }
     for (uint32_t i = tid; i < a.a.row_pitch / 4; i += HN_THREADS)
         reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(a.a.q + (size_t)qi * a.a.row_pitch)[i];
     const float qmag = a.a.qmags[qi];
     const HnScoreCtx sc{a.a.rows, a.a.row_pitch, a.a.mags, a.a.dim, a.a.st, a.a.metric, a.a.g.root_row};
-    const bool hasf = a.has_filter && a.has_filter[qi];
-    const uint32_t f0 = hasf ? a.filter_offsets[qi] : 0u, f1 = hasf ? a.filter_offsets[qi + 1] : 0u;
     if (tid == 0) { sh.err = 0; s_entry = hasf ? a.pseudo_entry : a.a.g.entry; }
     uint32_t out_total = 0;
     unsigned long long evals = 0, pops = 0;
@@ -199,6 +198,9 @@ cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s) {
     if (a.a.ef == 0 || a.a.ef > 4096) { set_error("hnsw: ef_search must be in 1..4096"); return CDB_INVALID_PARAMS; }
     const size_t smem = round_up((uint32_t)hn_smem_bytes(a.a.row_pitch, a.a.ef), 16) + (size_t)HNM_Z * 12 + (size_t)a.M * 4 + 16;
     if (smem > 200 * 1024) { set_error("hnsw: ef_search / metadata dims too large for shared memory"); return CDB_INVALID_PARAMS; }
+    // the shapes accepted are this kernel's; the warp form takes every one of them whose own carve fits
+    if (!(a.a.flags & CDB_HNSW_F_CTA) && hnsw_warp_md_smem(a.a.row_pitch, a.a.dim, a.a.ef, a.a.st, a.a.metric, a.M) <= 200 * 1024)
+        return hnsw_search_warp_md_device(a, s);
     CDB_ALLOW_SMEM(hnsw_search_md_kernel, smem);
     hnsw_search_md_kernel<<<a.a.nq, HN_THREADS, smem, s>>>(a);
     CDB_LAUNCH_CHECK();

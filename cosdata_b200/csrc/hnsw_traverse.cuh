@@ -126,6 +126,24 @@ __device__ inline HnSmem hn_carve(uint8_t *smem, uint32_t row_pitch, uint32_t ef
 }
 __device__ __forceinline__ uint32_t hn_id(uint32_t root_row, uint32_t row) { return row == root_row ? HN_ROOT_ID : row; }
 
+// metadata search (hnsw_md.cu, hnsw_warp.cu): a pseudo node's results carry no vector row
+__device__ __forceinline__ bool hnm_is_pseudo(const HnswMdArgs &a, int level, uint32_t node) {
+    const uint32_t mrow = a.node_md[level][node];
+    if (mrow == HN_EMPTY || a.md_mags[mrow] == 0.0f) return false;
+    const uint32_t id = a.node_id[level][node];
+    return id >= MD_PSEUDO_ID_LO && id <= MD_PSEUDO_ID_HI;
+}
+// rows [*f0, *f1) of filter_dims for filtered query qi.  The offsets may come from device memory the host never read, so a
+// range that is not off[q] <= off[q+1] <= n_filter_rows with at most HN_MAX_FILTERS rows fails the query (false, empty range).
+constexpr uint32_t HN_MAX_FILTERS = 4096;
+__device__ __forceinline__ bool hnm_filter_rows(const HnswMdArgs &a, uint32_t qi, uint32_t *f0, uint32_t *f1) {
+    const uint32_t lo = a.filter_offsets[qi], hi = a.filter_offsets[qi + 1];
+    const bool ok = lo <= hi && hi <= a.n_filter_rows && hi - lo <= HN_MAX_FILTERS;
+    *f0 = ok ? lo : 0u;
+    *f1 = ok ? hi : 0u;
+    return ok;
+}
+
 // bitonic sort (descending) of n keys with a payload, padded to P (power of two) with zeros
 __device__ inline void hn_sort_desc(uint64_t *keys, uint32_t *vals, uint32_t n, uint32_t P) {
     for (uint32_t i = n + threadIdx.x; i < P; i += blockDim.x) { keys[i] = 0ull; vals[i] = 0; }

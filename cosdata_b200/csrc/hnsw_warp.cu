@@ -1,4 +1,4 @@
-// hnsw_warp.cu -- batched HNSW search, ONE WARP PER QUERY (S1, CDB_MODE_HNSW on graphs without metadata):
+// hnsw_warp.cu -- batched HNSW search, ONE WARP PER QUERY (S1, CDB_MODE_HNSW; graphs with metadata: the md form at the end):
 //   ann_search              src/vector_store.rs:256-402
 //   traverse_find_nearest   src/vector_store.rs:1112-1204
 //   PerformantFixedSet      src/models/fixedset.rs:2-29
@@ -39,13 +39,18 @@ constexpr uint32_t HW_WORK = HN_MAX_TAKE + 32;  // speculative form: rows to sco
 // speculative form: [9] cache look-ups + choice of speculative rows, [10] chain phases, [11] speculative evaluations
 constexpr int HW_PROF_SLOTS = 12;
 
+constexpr uint32_t HW_MD_Z = 256;   // metadata form: a level's merged list z (<= 100) + one traversal's results (<= 100)
+
 struct HwCarve {
     uint32_t EFP, stage_pitch, stage_rows;
     uint32_t off_q32, off_qkeys, off_rkeys, off_nkeys, off_fs, off_qnodes, off_rnodes, off_nnodes, off_nrow, off_bar, off_stage, total;
     uint32_t off_cache, off_work, off_sadj;   // speculative form only
+    uint32_t off_zkeys, off_znodes, off_qvars, off_qbits; // metadata form only: z list, {f0, f1, results so far}, the filter's dims as i32 [M]
 };
 
-__host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, uint32_t ef, bool f16fast, bool spec = false) {
+// md: metadata form with M metadata dims (never speculative)
+__host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, uint32_t ef, bool f16fast, bool spec = false,
+                                            bool md = false, uint32_t M = 0) {
     HwCarve c;
     c.EFP = hn_efp(ef);
     c.stage_pitch = round_up(row_pitch, 16) + 16;   // + 16 bytes: the lanes' rows start on different banks
@@ -68,6 +73,14 @@ __host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, ui
         c.off_cache = o;      o += HW_CACHE * 8;
         c.off_work = o;       o += 3 * HW_WORK * 4;
         c.off_sadj = o;       o += HW_NSRC * HN_MAX_TAKE * 4;
+    }
+    c.off_zkeys = c.off_znodes = c.off_qvars = c.off_qbits = 0;
+    if (md) {
+        o = round_up(o, 8);
+        c.off_zkeys = o;      o += HW_MD_Z * 8;
+        c.off_znodes = o;     o += HW_MD_Z * 4;
+        c.off_qvars = o;      o += 4 * 4;
+        c.off_qbits = o;      o += M * 4;
     }
     c.off_stage = round_up(o, 16);
     c.total = c.off_stage + c.stage_rows * c.stage_pitch;
@@ -174,22 +187,30 @@ struct HwState {
 // Score the compacted neighbours nnodes/nrow[first .. first+n) into nkeys (slot order kept).  Rows are staged through
 // shared memory (one TMA bulk copy per row, all in flight together: one memory round trip per group), then one lane per
 // row runs the reference chain.  Returns the (position << 8 | flag) of the first failing evaluation, 0xFFFFFFFF if none.
-template <int FAST, bool PROF>
+// MD (metadata form): keys carry replica ids, and the metadata arm of each pair (md_arm) is applied first; a lane whose arm
+// is a constant skips the chain.
+template <int FAST, bool PROF, bool MD>
 __device__ __forceinline__ uint32_t hw_score_group(const HnScoreCtx &sc, const HwSmem &m, float qmag, uint32_t pp, uint32_t first,
-                                                   uint32_t n, int lane, HwState &st) {
+                                                   uint32_t n, int lane, HwState &st, const HnMdCtx *md) {
     uint32_t err_first = 0xFFFFFFFFu;
     for (uint32_t g0 = 0; g0 < n; g0 += m.stage_rows) {
         const uint32_t gn = min(m.stage_rows, n - g0);
         long long ts = 0, ti = 0, tw = 0;
         if (PROF) ts = clock64();
-        uint32_t row = 0;
-        float rmag = 0.0f;
+        uint32_t row = 0, nid = 0, mrow = HN_EMPTY;
+        float rmag = 0.0f, ymag = 0.0f;
         // (a copy may complete before the expect_tx is posted: the phase cannot end before lane 0's arrive)
         if (lane == 0) hw_mbar_expect(m.bar, gn * sc.row_pitch);
         if ((uint32_t)lane < gn) {
             row = m.nrow[first + g0 + lane];
             hw_bulk_g2s(hw_smem_u32(m.stage + (size_t)lane * m.stage_pitch), sc.rows + (size_t)row * sc.row_pitch, sc.row_pitch, m.bar);
             rmag = sc.mags[row];   // in flight together with the rows
+            if (MD) {
+                const uint32_t node = m.nnodes[first + g0 + lane];
+                nid = md->node_id[node];
+                mrow = md->node_md[node];
+                if (mrow != HN_EMPTY) ymag = md->md_mags[mrow];
+            }
         }
         if (PROF) ti = clock64();
         hw_mbar_wait(m.bar, st.bar_phase);
@@ -200,7 +221,14 @@ __device__ __forceinline__ uint32_t hw_score_group(const HnScoreCtx &sc, const H
             const uint32_t pos = first + g0 + lane;
             const uint8_t *code = m.stage + (size_t)lane * m.stage_pitch;
             float d = 0.0f;
-            if (FAST) {
+            int arm = MD_ARM_VECTOR;
+            if (MD) {
+                const MdSide x{m.qs, qmag, pp, md->q_has_id, md->q_id, md->q_bits, md->q_mag};
+                const MdSide y{code, rmag, pp, true, nid, mrow == HN_EMPTY ? nullptr : md->md_bits + (size_t)mrow * md->M, ymag};
+                arm = md_arm(sc.metric, md->M, x, y, &d);
+                if (arm != MD_ARM_VECTOR) rc = arm;
+            }
+            if (arm == MD_ARM_VECTOR && FAST) {
                 const float dot = hw_dot16<FAST>(m.qs, code, sc.dim);
                 if (sc.metric == CDB_METRIC_COSINE) {
                     const float denom = __fmul_rn(qmag, rmag);
@@ -209,10 +237,10 @@ __device__ __forceinline__ uint32_t hw_score_group(const HnScoreCtx &sc, const H
                 } else {
                     d = dot;
                 }
-            } else {
+            } else if (arm == MD_ARM_VECTOR) {
                 rc = pair_distance(sc.metric, sc.st, sc.dim, m.qs, qmag, pp, code, rmag, pp, &d);
             }
-            m.nkeys[pos] = make_key64(order_key(sc.metric, __float_as_uint(d)), hn_id(sc.root_row, row));
+            m.nkeys[pos] = make_key64(order_key(sc.metric, __float_as_uint(d)), MD ? nid : hn_id(sc.root_row, row));
         }
         const uint32_t bad = __ballot_sync(0xFFFFFFFFu, rc != CDB_OK);
         if (bad && err_first == 0xFFFFFFFFu) {   // the reference stops at the first Err (slot order)
@@ -287,33 +315,37 @@ __device__ __forceinline__ uint32_t hw_score_work(const HnScoreCtx &sc, const Hw
 
 // One level (traverse_find_nearest).  All 32 lanes call it with warp-uniform arguments.  On return (st.err == 0)
 // rkeys/rnodes[0..st.rlen) hold every popped entry sorted best first.
-template <int FAST, bool PROF>
+// MD (metadata form, md != null): the fixed set and the keys use the replica ids md->node_id, pairs are scored through the
+// metadata arms, md->keep_fs keeps the fixed set of the previous traversal of the level; always the sorted-queue,
+// non-speculative form (SPEC / POOL are ignored).
+template <int FAST, bool PROF, bool MD>
 __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null: identity */, const uint32_t *__restrict__ adj,
                                   uint32_t nb, uint32_t take, const HnScoreCtx &sc, const HwSmem &m, float qmag, uint32_t self_id,
-                                  uint32_t ef, uint32_t entry, HwState &st, int lane, uint32_t flags) {
+                                  uint32_t ef, uint32_t entry, HwState &st, int lane, uint32_t flags, const HnMdCtx *md = nullptr) {
     const uint32_t pp = plane_pitch(sc.dim);
     const bool f_preload = (flags & CDB_HNSW_F_PRELOAD) != 0, f_atomfs = (flags & CDB_HNSW_F_ATOMFS) != 0;
-    const bool f_pool = (flags & CDB_HNSW_F_POOL) != 0;
-    const bool f_spec = (flags & CDB_HNSW_F_SPEC) != 0 && !f_pool;
+    const bool f_pool = !MD && (flags & CDB_HNSW_F_POOL) != 0;
+    const bool f_spec = !MD && (flags & CDB_HNSW_F_SPEC) != 0 && !f_pool;
     const uint32_t EFP = m.EFP;
     const uint32_t CAPQ = 2 * EFP;      // pool form: both queue buffers are one unsorted pool
     const uint32_t bmask = nb - 1u;
     const uint32_t lt = (1u << lane) - 1u;
     long long t0 = 0;
     if (PROF) t0 = clock64();
+    if (!MD || !md->keep_fs)
 #pragma unroll
-    for (int i = 0; i < 4; ++i) m.fs[lane + 32 * i] = 0u;
+        for (int i = 0; i < 4; ++i) m.fs[lane + 32 * i] = 0u;
     if (f_spec)   // node indices are level-local: the score cache starts empty on every level
         for (uint32_t i = lane; i < HW_CACHE; i += 32) m.cache[i] = ~0ull;
     uint32_t sd0 = HN_EMPTY, sd1 = HN_EMPTY, sd2 = HN_EMPTY, sd3 = HN_EMPTY;   // queue entries whose neighbours are all cached
     if (lane == 0) { m.nnodes[0] = entry; m.nrow[0] = node_row ? node_row[entry] : entry; }
     __syncwarp();
     {
-        const uint32_t e = hw_score_group<FAST, PROF>(sc, m, qmag, pp, 0, 1, lane, st);
+        const uint32_t e = hw_score_group<FAST, PROF, MD>(sc, m, qmag, pp, 0, 1, lane, st, md);
         st.evals += 1;
         if (e != 0xFFFFFFFFu) { st.err = e & 0xFFu; return; }
         if (lane == 0) {
-            const uint32_t eid = hn_id(sc.root_row, m.nrow[0]);
+            const uint32_t eid = MD ? md->node_id[entry] : hn_id(sc.root_row, m.nrow[0]);
             const uint32_t b0 = (((self_id >> 6) & bmask) << 6) | (self_id & 0x3f), b1 = (((eid >> 6) & bmask) << 6) | (eid & 0x3f);
             m.fs[b0 >> 5] |= 1u << (b0 & 31);
             m.fs[b1 >> 5] |= 1u << (b1 & 31);
@@ -366,7 +398,7 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
             bk[h] = 0x80000000u | ((uint32_t)lane + 32u * h);   // unique per slot: never matches another slot
             if (nbl[h] != HN_EMPTY) {
                 row[h] = node_row ? __ldg(node_row + nbl[h]) : nbl[h];
-                const uint32_t id = hn_id(sc.root_row, row[h]);
+                const uint32_t id = MD ? __ldg(md->node_id + nbl[h]) : hn_id(sc.root_row, row[h]);
                 bk[h] = (((id >> 6) & bmask) << 6) | (id & 0x3f);
             }
         }
@@ -529,7 +561,7 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
             if (PROF) { const long long tq = clock64(); st.prof[9] += tq - t3; st.prof[11] += nt - nm; t3 = tq; }
             if (nt) e = hw_score_work<FAST, PROF>(sc, m, qmag, pp, nm, nt, lane, st);
         } else {
-            e = hw_score_group<FAST, PROF>(sc, m, qmag, pp, 0, nc, lane, st);
+            e = hw_score_group<FAST, PROF, MD>(sc, m, qmag, pp, 0, nc, lane, st, md);
         }
         st.evals += nc;
         if (e != 0xFFFFFFFFu) { st.err = e & 0xFFu; st.rlen = rlen; return; }
@@ -718,11 +750,7 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
     if (PROF) { const long long t7 = clock64(); st.prof[6] += t7 - t6; st.prof[7] += t7 - t0; }
 }
 
-template <int FAST, bool PROF>
-__global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarve cv) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    const int lane = threadIdx.x;
-    const uint32_t qi = blockIdx.x;
+__device__ __forceinline__ HwSmem hw_smem(uint8_t *smem, const HwCarve &cv) {
     HwSmem m;
     m.qs = smem;
     m.q32 = reinterpret_cast<float *>(smem + cv.off_q32);
@@ -742,6 +770,15 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarv
     m.wdst = m.wrow + HW_WORK;
     m.sadj = reinterpret_cast<uint32_t *>(smem + cv.off_sadj);
     m.EFP = cv.EFP; m.stage_pitch = cv.stage_pitch; m.stage_rows = cv.stage_rows;
+    return m;
+}
+
+template <int FAST, bool PROF>
+__global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarve cv) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int lane = threadIdx.x;
+    const uint32_t qi = blockIdx.x;
+    const HwSmem m = hw_smem(smem, cv);
 
     for (uint32_t i = lane; i < a.row_pitch / 4; i += 32)
         reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(a.q + (size_t)qi * a.row_pitch)[i];
@@ -762,7 +799,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarv
         const uint32_t nb = level == 0 ? a.g.nbrs0 : a.g.nbrs;
         const uint32_t take = min(min(a.shortlist, nb), HN_MAX_TAKE);
         const uint32_t *node_row = ((a.g.identity_mask >> level) & 1u) ? nullptr : a.g.node_row[level];
-        hw_traverse_level<FAST, PROF>(node_row, a.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, a.ef, entry, st, lane, a.flags);
+        hw_traverse_level<FAST, PROF, false>(node_row, a.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, a.ef, entry, st, lane, a.flags);
         if (st.err) break;
         const uint32_t keep = min(st.rlen, HW_FINAL_LEN);
         for (uint32_t i = lane; i < keep; i += 32) {
@@ -816,6 +853,155 @@ cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s) {
     if (fast == 1) return prof ? launch_warp<1, true>(a, cv, s) : launch_warp<1, false>(a, cv, s);
     if (fast == 2) return prof ? launch_warp<2, true>(a, cv, s) : launch_warp<2, false>(a, cv, s);
     return prof ? launch_warp<0, true>(a, cv, s) : launch_warp<0, false>(a, cv, s);
+}
+
+// ---- metadata form (graphs with replica nodes): the steps of hnsw_search_md_kernel (hnsw_md.cu) on one warp per query.
+// Per level, one traversal per filter row, all of them on the level's fixed set; their <= 100 results minus the strong
+// mismatches (cosine -1.0, vector_store.rs:294-303) are merged into the level's best-100 list z.  A level that ends empty
+// scores its entry against every filter and keeps the strongest (vector_store.rs:329-380).  out_rows is CDB_INVALID_ID for
+// pseudo nodes, out_ids the replica ids (hnsw_dedup_md_kernel and the re-rank take them unchanged).
+template <int FAST>
+__global__ void __launch_bounds__(32) hnsw_search_warp_md_kernel(HnswMdArgs a, HwCarve cv) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int lane = threadIdx.x;
+    const uint32_t qi = blockIdx.x;
+    const HwSmem m = hw_smem(smem, cv);
+    uint64_t *zkeys = reinterpret_cast<uint64_t *>(smem + cv.off_zkeys);
+    uint32_t *znodes = reinterpret_cast<uint32_t *>(smem + cv.off_znodes);
+    int32_t *qbits = reinterpret_cast<int32_t *>(smem + cv.off_qbits);
+    // the filter rows [f0, f1) and the result count are touched once per level: they live in shared memory (volatile: re-read
+    // there) instead of registers that ptxas would spill around the chains' division calls
+    volatile uint32_t *qv = reinterpret_cast<uint32_t *>(smem + cv.off_qvars);
+    const HnswArgs &g = a.a;
+    const uint32_t lt = (1u << lane) - 1u;
+
+    for (uint32_t i = lane; i < g.row_pitch / 4; i += 32)
+        reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(g.q + (size_t)qi * g.row_pitch)[i];
+    const float qmag = g.qmags[qi];
+    const HnScoreCtx sc{g.rows, g.row_pitch, g.mags, g.dim, g.st, g.metric, g.g.root_row};
+    const uint32_t pp = plane_pitch(g.dim);
+    if (lane == 0) hw_mbar_init(m.bar, 1);
+    HwState st;
+    st.err = 0; st.rlen = 0; st.evals = 0; st.pops = 0; st.bar_phase = 0;
+    const bool hasf = a.has_filter && a.has_filter[qi];
+    {
+        uint32_t f0 = 0, f1 = 0;
+        if (hasf && !hnm_filter_rows(a, qi, &f0, &f1)) st.err = CDB_ERRFLAG_BAD_FILTER;
+        if (lane == 0) { qv[0] = f0; qv[1] = f1; qv[2] = 0; }
+    }
+    uint32_t entry = hasf ? a.pseudo_entry : g.g.entry;
+    __syncwarp();
+
+    // Metadata::from(&QueryFilterDimensions) (types.rs:127-146): mbits = dims as i32, mag = sqrt(sequential sum of squares);
+    // every lane folds the same values in the same order
+    auto load_filter = [&](uint32_t f) {
+        __syncwarp();
+        for (uint32_t i = lane; i < a.M; i += 32) qbits[i] = (int32_t)a.filter_dims[(size_t)f * a.M + i];
+        __syncwarp();
+        float t = 0.0f;
+        for (uint32_t i = 0; i < a.M; ++i) { const float x = (float)qbits[i]; t = __fadd_rn(t, __fmul_rn(x, x)); }
+        return __fsqrt_rn(t);
+    };
+    const uint32_t minus1 = order_key(CDB_METRIC_COSINE, __float_as_uint(-1.0f));
+
+    for (int level = (int)g.g.num_levels; level >= 0 && !st.err; --level) {
+        const uint32_t nb = level == 0 ? g.g.nbrs0 : g.g.nbrs;
+        const uint32_t take = min(min(g.shortlist, nb), HN_MAX_TAKE);
+        const uint32_t *node_row = g.g.node_row[level];
+        HnMdCtx md{a.node_id[level], a.node_md[level], a.md_bits, a.md_mags, a.M, nullptr, 0.0f, false, false, 0u};
+        uint32_t zn = 0;
+        if (hasf) {
+            for (uint32_t f = qv[0]; f < qv[1]; ++f) {
+                md.q_mag = load_filter(f); md.q_bits = qbits; md.keep_fs = f > qv[0];
+                hw_traverse_level<FAST, false, true>(node_row, g.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, g.ef, entry, st,
+                                                     lane, g.flags, &md);
+                if (st.err) break;
+                const uint32_t keep = min(st.rlen, HW_FINAL_LEN);
+                for (uint32_t i0 = 0; i0 < keep; i0 += 32) {   // append in rank order; z is sorted below
+                    const uint32_t i = i0 + (uint32_t)lane;
+                    const uint64_t key = i < keep ? m.rkeys[i] : 0ull;
+                    const bool app = i < keep && !(g.metric == CDB_METRIC_COSINE && (uint32_t)(key >> 32) == minus1);
+                    const uint32_t b = __ballot_sync(0xFFFFFFFFu, app);
+                    if (app) { const uint32_t pos = zn + (uint32_t)__popc(b & lt); zkeys[pos] = key; znodes[pos] = m.rnodes[i]; }
+                    zn += (uint32_t)__popc(b);
+                }
+                __syncwarp();
+                uint32_t P = 1;
+                while (P < zn) P <<= 1;
+                hw_sort_desc(zkeys, znodes, zn, P, lane);
+                zn = min(zn, HW_FINAL_LEN);
+            }
+        } else {
+            hw_traverse_level<FAST, false, true>(node_row, g.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, g.ef, entry, st, lane,
+                                                 g.flags, &md);
+            if (!st.err) {
+                zn = min(st.rlen, HW_FINAL_LEN);
+                for (uint32_t i = lane; i < zn; i += 32) { zkeys[i] = m.rkeys[i]; znodes[i] = m.rnodes[i]; }
+            }
+        }
+        if (st.err) break;
+        if (zn == 0) {
+            // the level's entry node itself, scored against every filter (not counted as an evaluation), strongest match kept
+            uint64_t best = 0ull;
+            bool have = false;
+            for (uint32_t f = qv[0]; f < (hasf ? qv[1] : qv[0] + 1); ++f) {
+                if (hasf) { md.q_mag = load_filter(f); md.q_bits = qbits; }
+                if (lane == 0) { m.nnodes[0] = entry; m.nrow[0] = node_row[entry]; }
+                __syncwarp();
+                const uint32_t e = hw_score_group<FAST, false, true>(sc, m, qmag, pp, 0, 1, lane, st, &md);
+                if (e != 0xFFFFFFFFu) { st.err = e & 0xFFu; break; }
+                const uint64_t key = m.nkeys[0];   // same id every time: the score decides, the first maximum is kept
+                if (!have || key > best) { best = key; have = true; }
+            }
+            if (st.err) break;
+            if (!have) { st.err = CDB_ERRFLAG_UNREACHABLE; break; }   // Some(empty filter list): max().unwrap() panics
+            __syncwarp();
+            if (lane == 0) { zkeys[0] = best; znodes[0] = entry; }
+            zn = 1;
+            __syncwarp();
+        }
+        const uint32_t out_total = qv[2];
+        for (uint32_t i = lane; i < zn; i += 32) {
+            const uint32_t slot = out_total + i, node = znodes[i];
+            if (slot < g.out_cap) {
+                const size_t o = (size_t)qi * g.out_cap + slot;
+                a.out_ids[o] = md.node_id[node];
+                g.out_rows[o] = hnm_is_pseudo(a, level, node) ? CDB_INVALID_ID : node_row[node];
+                g.out_scores[o] = __uint_as_float(key_to_bits(g.metric, (uint32_t)(zkeys[i] >> 32)));
+            }
+        }
+        __syncwarp();
+        if (lane == 0) qv[2] = out_total + zn;
+        if (level > 0) entry = g.g.child[level][znodes[0]];
+        __syncwarp();
+    }
+    if (lane == 0) {
+        g.out_n[qi] = st.err ? 0u : min(qv[2], g.out_cap);
+        if (st.err) atomicOr(g.err32 + qi, st.err);
+        if (g.counters) { atomicAdd(g.counters, st.evals); atomicAdd(g.counters + 1, st.pops); }
+    }
+}
+
+size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t dim, uint32_t ef, int st, int metric, uint32_t M) {
+    return hw_carve(row_pitch, dim, ef, hw_fast_kind(st, metric) != 0, false, true, M).total;
+}
+
+template <int FAST>
+static cdb_status launch_warp_md(const HnswMdArgs &a, const HwCarve &cv, cudaStream_t s) {
+    auto kern = hnsw_search_warp_md_kernel<FAST>;
+    CDB_ALLOW_SMEM(kern, cv.total);
+    kern<<<a.a.nq, 32, cv.total, s>>>(a, cv);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
+// the caller (hnsw_search_md_device) has checked the shape against both carves
+cdb_status hnsw_search_warp_md_device(const HnswMdArgs &a, cudaStream_t s) {
+    const int fast = hw_fast_kind(a.a.st, a.a.metric);
+    const HwCarve cv = hw_carve(a.a.row_pitch, a.a.dim, a.a.ef, fast != 0, false, true, a.M);
+    if (fast == 1) return launch_warp_md<1>(a, cv, s);
+    if (fast == 2) return launch_warp_md<2>(a, cv, s);
+    return launch_warp_md<0>(a, cv, s);
 }
 
 }  // namespace cdb

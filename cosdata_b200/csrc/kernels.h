@@ -141,7 +141,9 @@ struct HnswArgs {
     unsigned long long *prof;         // null, or clock64 sums (hnsw_warp.cu)
     uint32_t flags;                   // CDB_HNSW_F_* variant switches of the warp kernel
 };
-// variant switches of hnsw_search_warp_kernel (cdb_debug_set_hnsw_flags; the default is the best measured combination)
+// variant switches of hnsw_search_warp_kernel (cdb_debug_set_hnsw_flags; the default is the best measured combination).
+// The metadata form (hnsw_search_warp_md_kernel) takes PRELOAD / ATOMFS and CTA (-> hnsw_search_md_kernel); it always runs
+// the sorted-queue, non-speculative form, whatever SPEC / POOL say.
 constexpr uint32_t CDB_HNSW_F_PRELOAD = 2;   // load the next head's adjacency slots while the queue merge runs
 constexpr uint32_t CDB_HNSW_F_ATOMFS = 4;    // fixed-set walk through atomicOr return values (slot-order loop only on aliasing)
 constexpr uint32_t CDB_HNSW_F_CTA = 8;       // round-1 kernel: one CTA per query
@@ -165,11 +167,15 @@ struct HnswMdArgs {
     uint32_t M;
     uint32_t pseudo_entry;
     const uint32_t *filter_offsets;   // [nq+1] rows of filter_dims per query
-    const int8_t *filter_dims;        // [total][M]
+    const int8_t *filter_dims;        // [n_filter_rows][M]
+    uint32_t n_filter_rows;
     const uint8_t *has_filter;        // [nq] (nullptr = no query has a filter)
     uint32_t *out_ids;                // [nq][out_cap] replica ids
 };
+// the warp-per-query form (hnsw_warp.cu) unless a.a.flags has CDB_HNSW_F_CTA or its shared memory does not fit
 cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s);
+size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t dim, uint32_t ef, int st, int metric, uint32_t M);
+cdb_status hnsw_search_warp_md_device(const HnswMdArgs &a, cudaStream_t s);
 cdb_status hnsw_dedup_md_device(const uint32_t *d_ids, const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n,
                                 uint32_t in_cap, int metric, uint32_t id_base, uint32_t k5, uint32_t nq, uint32_t *d_cand,
                                 uint32_t *d_labels, uint32_t *d_cand_cnt, cudaStream_t s);

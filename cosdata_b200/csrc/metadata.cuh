@@ -48,11 +48,14 @@ __device__ inline int md_mdims_cosine(const MdSide &x, const MdSide &y, uint32_t
     return CDB_OK;
 }
 
-// DistanceMetric::calculate(x, y) with metadata: x = query side (fvec_data), y = node side
-__device__ inline int md_pair_distance(int metric, int st, uint32_t dim, uint32_t M, const MdSide &x, const MdSide &y, float *out) {
-    if (metric != CDB_METRIC_COSINE) return pair_distance(metric, st, dim, x.code, x.mag, x.pp, y.code, y.mag, y.pp, out);
+// The arm of DistanceMetric::calculate(x, y) with metadata (x = query side / fvec_data, y = node side): MD_ARM_VECTOR when
+// the result is the vector metric of the pair, else the arm's status (and *out).  Only the vector arms read the codes, so a
+// caller with its own vector chain (hnsw_warp.cu) skips it for the constant arms.
+constexpr int MD_ARM_VECTOR = -1;
+__device__ inline int md_arm(int metric, uint32_t M, const MdSide &x, const MdSide &y, float *out) {
+    if (metric != CDB_METRIC_COSINE) return MD_ARM_VECTOR;
     const int xk = md_kind(x), yk = md_kind(y);
-    if (yk == MD_KIND_BASE && xk == MD_KIND_BASE) return pair_distance(metric, st, dim, x.code, x.mag, x.pp, y.code, y.mag, y.pp, out);
+    if (yk == MD_KIND_BASE && xk == MD_KIND_BASE) return MD_ARM_VECTOR;
     if (yk == MD_KIND_PSEUDO && xk == MD_KIND_PSEUDO) return md_mdims_cosine(x, y, M, out);
     if (yk == MD_KIND_PSEUDO && xk == MD_KIND_METADATA) {   // a metadata node strongly (mis)matches a pseudo node
         bool same = true;
@@ -64,12 +67,17 @@ __device__ inline int md_pair_distance(int metric, int st, uint32_t dim, uint32_
         float mc;
         const int rc = md_mdims_cosine(x, y, M, &mc);
         if (rc != CDB_OK) return rc;
-        if (mc > 0.99f) return pair_distance(metric, st, dim, x.code, x.mag, x.pp, y.code, y.mag, y.pp, out);
+        if (mc > 0.99f) return MD_ARM_VECTOR;
         *out = -1.0f;
         return CDB_OK;
     }
     if (yk == MD_KIND_BASE && xk == MD_KIND_METADATA) { *out = 0.0f; return CDB_OK; }
     return CDB_UNREACHABLE_ARM;   // (Pseudo,Base) (Base,Pseudo) (Metadata,Pseudo) (Metadata,Base): unreachable!() in the reference
+}
+
+__device__ inline int md_pair_distance(int metric, int st, uint32_t dim, uint32_t M, const MdSide &x, const MdSide &y, float *out) {
+    const int rc = md_arm(metric, M, x, y, out);
+    return rc == MD_ARM_VECTOR ? pair_distance(metric, st, dim, x.code, x.mag, x.pp, y.code, y.mag, y.pp, out) : rc;
 }
 
 __device__ __forceinline__ uint32_t md_err_flag(int rc) {

@@ -90,7 +90,9 @@ enum {
     CDB_ERRFLAG_CALCULATION = 1, /* some scored pair had a zero denominator (cosine.rs:230-231);
                                     the reference `?`-propagates this and fails the query */
     CDB_ERRFLAG_OTHER = 2,       /* another Err of DistanceFunction::calculate */
-    CDB_ERRFLAG_UNREACHABLE = 4  /* a replica-kind pair the reference marks unreachable!() was scored (the reference panics) */
+    CDB_ERRFLAG_UNREACHABLE = 4, /* a replica-kind pair the reference marks unreachable!() was scored (the reference panics) */
+    CDB_ERRFLAG_BAD_FILTER = 8   /* cdb_search_batch_filtered_device: the query's filter offsets are out of order, past
+                                    n_filter_rows or span more than 4096 rows; the query returns no results */
 };
 
 #define CDB_INVALID_ID 0xFFFFFFFFu
@@ -550,6 +552,19 @@ cdb_status cdb_search_batch(cdb_index *index, const float *queries, uint32_t n_q
 cdb_status cdb_search_batch_filtered(cdb_index *index, const float *queries, uint32_t n_queries, const cdb_search_params *params,
                                      const uint32_t *filter_offsets, const int8_t *filter_dims, const uint8_t *has_filter,
                                      uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags);
+/* same, every pointer is DEVICE memory on the index's device; asynchronous on `stream` (NULL: the handle's own stream) and
+ * re-entrant through the scratch pool like cdb_search_batch_device.  d_filter_dims holds n_filter_rows rows of md_dims i8
+ * values; d_filter_offsets [n_queries + 1] index those rows.  d_out_counts and d_err_flags may be NULL.
+ * Refused with CDB_INVALID_PARAMS before any device work: a null handle, params, queries or outputs (n_queries > 0), a mode
+ * other than CDB_MODE_HNSW, k outside 1..1024, d_has_filter without d_filter_offsets, n_filter_rows > 0 without
+ * d_filter_dims, and d_has_filter on a graph without metadata (d_has_filter == NULL there runs the plain HNSW search).
+ * The host cannot read the offsets: a filtered query whose range is not off[q] <= off[q+1] <= n_filter_rows with at most
+ * 4096 rows gets CDB_ERRFLAG_BAD_FILTER and count 0, and no row outside [0, n_filter_rows) is read. */
+cdb_status cdb_search_batch_filtered_device(cdb_index *index, const float *d_queries, uint32_t n_queries,
+                                            const cdb_search_params *params, const uint32_t *d_filter_offsets,
+                                            const int8_t *d_filter_dims, uint32_t n_filter_rows, const uint8_t *d_has_filter,
+                                            uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts,
+                                            uint8_t *d_err_flags, void *stream);
 /* same, every pointer is DEVICE memory on the index's device; asynchronous on `stream`.  Each search leases one of the
  * handle's scratch sets (a small pool, grown on demand): searches on different streams run concurrently, a scratch set is
  * handed to its next user only behind the event that ends its previous search. */
@@ -622,8 +637,10 @@ cdb_status cdb_index_hnsw_profile(cdb_index *index, int32_t enable, uint64_t *ou
  * iters = 0 -> default length (~10 ms). */
 cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters, double *out_tops, float *out_ms);
 /* measurement switch: kernel variant of CDB_MODE_HNSW searches (results are identical for every value).  Bits: 1 cooperative
- * f16 conversion, 2 next-head adjacency preload, 4 fixed-set walk through atomics, 8 round-1 CTA-per-query kernel;
- * 0xFFFFFFFF restores the default.  Process-wide. */
+ * f16 conversion, 2 next-head adjacency preload, 4 fixed-set walk through atomics, 8 round-1 CTA-per-query kernel (on graphs
+ * with metadata: the CTA-per-query metadata kernel), 16 unsorted candidate pool, 32 speculative scoring; 0xFFFFFFFF restores
+ * the default.  On graphs with metadata 2 and 4 apply as on plain graphs, while 16 and 32 are ignored: the metadata search
+ * always runs the sorted-queue, non-speculative form.  Process-wide. */
 cdb_status cdb_debug_set_hnsw_flags(uint32_t flags);
 
 /* ----------------------------------------------------- instrumentation
@@ -936,7 +953,7 @@ typedef struct {
  * searches already enqueued on the device.
  * CDB_INVALID_PARAMS: top_k > 341 (the dense and sparse searches take k <= 1024), a sparse source with rerank and
  * 3 * top_k * reranking_factor > 5120, a source count other than two, null queries, handles on different devices.
- * CDB_UNSUPPORTED: a dense handle with graph metadata (its HNSW searches go through the host-only cdb_search_batch_filtered;
+ * CDB_UNSUPPORTED: a dense handle with graph metadata (its HNSW searches go through cdb_search_batch_filtered[_device];
  * fuse those results with cdb_rrf_fuse and id_stride = max_replica_per_node).  Refusals of a sub-search's own parameter
  * checks are returned as that search returns them.  top_k = 0: empty results (out_counts zeroed), no kernel launched. */
 cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k, float fusion_constant_k,
