@@ -143,8 +143,9 @@ __device__ __forceinline__ void wgmma_s8(uint32_t (&d)[128], uint64_t adesc, uin
         : "l"(adesc), "l"(bdesc), "r"(1)
         : "memory");
 }
-// D[64 x 128] += A[64 x K] * B[128 x K]^T on s8 codes: the layout of wgmma_s8 with j < 16 (d[4j + ...], columns 8j + ...)
-__device__ __forceinline__ void wgmma_s8_n128(uint32_t *d, uint64_t adesc, uint64_t bdesc) {
+// D[64 x 128] (+)= A[64 x K] * B[128 x K]^T on s8 codes: the layout of wgmma_s8 with j < 16 (d[4j + ...], columns 8j + ...);
+// accumulate = 0 overwrites d instead of adding to it
+__device__ __forceinline__ void wgmma_s8_n128(uint32_t *d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
@@ -160,7 +161,7 @@ __device__ __forceinline__ void wgmma_s8_n128(uint32_t *d, uint64_t adesc, uint6
           "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
           "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
           "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
-        : "l"(adesc), "l"(bdesc), "r"(1)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
 

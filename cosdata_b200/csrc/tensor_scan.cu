@@ -772,11 +772,13 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const uint32_t ct = threadIdx.x, wg = ct >> 7, wl = (ct >> 5) & 3, qd = (uint32_t)lane & 3;
     float gm[4][NL];   // this thread's share of the CTA's class maxima (the shared `cls` is raised whenever one grows)
+    float gmin[4];     // min_l gm[i][l]: a tile whose largest lower bound does not exceed it raises none of them
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         reinterpret_cast<uint32_t *>(lstage + (size_t)(ct * 4 + i) * TS8_SLOT_BYTES)[0] = 0;
 #pragma unroll
         for (int l = 0; l < NL; ++l) gm[i][l] = -INFINITY;
+        gmin[i] = -INFINITY;
     }
     if (T == 0) return;
     if (wg == 1) named_bar_arrive<TS8_BAR_TURN, 256>();   // warpgroup 0 takes the first turn
@@ -795,10 +797,8 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         if (wg == 0) named_bar_sync<TS8_BAR_TURN, 256>();
         else named_bar_sync<TS8_BAR_TURN + 1, 256>();
         const unsigned long long c_main = PROF ? clock64() : 0;
-        // zeroing ends the accumulators' live range for ptxas (see tensor_scan_kernel)
+        // the turn's first k-block overwrites the accumulators (scale-d 0) instead of 128 zeroing moves per turn
         uint32_t acc[128];
-#pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0;
         uint32_t prev = 0;
         for (uint32_t kb = 0; kb < a.kblocks; ++kb) {
             const unsigned long long c0 = PROF ? clock64() : 0;
@@ -810,8 +810,8 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
             wgmma_fence();
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {   // +32 bytes along K = +2 in the encoded start address
-                wgmma_s8_n128(acc, adesc0 + 2 * kk, bdesc + 2 * kk);
-                wgmma_s8_n128(acc + 64, adesc1 + 2 * kk, bdesc + 2 * kk);
+                wgmma_s8_n128(acc, adesc0 + 2 * kk, bdesc + 2 * kk, kb | kk);
+                wgmma_s8_n128(acc + 64, adesc1 + 2 * kk, bdesc + 2 * kk, kb | kk);
             }
             wgmma_commit();
             wgmma_wait<1>();   // the previous k-block's MMAs have retired
@@ -906,14 +906,26 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                 hit[i] = true;
             }
             hit[i] = hit[i] && mt * TS_BLOCK_M + ql < a.n_queries;
-            // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class
+            // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class.
+            // The lower bound fl_down(fl_down(cm * s) - eps) (s = slo for cm >= 0, shi >= slo >= 0 otherwise) does not
+            // decrease with cm, so no class can grow unless the largest class maximum's bound exceeds gmin: one bound per
+            // query and tile instead of NL, and the per-class fold only on the rare tiles that can raise one.
+            int cmx = cm[0];
 #pragma unroll
-            for (int l = 0; l < NL; ++l) {
-                const float lb = __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo[i] : shi[i]), eps[i]);
-                if (cm[l] != INT_MIN && lb > gm[i][l]) {
-                    gm[i][l] = lb;
-                    atomicMax(cls + (8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M + ql, f2ord(lb));
+            for (int l = 1; l < NL; ++l) cmx = max(cmx, cm[l]);
+            const float lbx = __fsub_rd(__fmul_rd(__int2float_rd(cmx), cmx >= 0 ? slo[i] : shi[i]), eps[i]);
+            if (cmx != INT_MIN && lbx > gmin[i]) {
+                float mn = INFINITY;
+#pragma unroll
+                for (int l = 0; l < NL; ++l) {
+                    const float lb = __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo[i] : shi[i]), eps[i]);
+                    if (cm[l] != INT_MIN && lb > gm[i][l]) {
+                        gm[i][l] = lb;
+                        atomicMax(cls + (8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M + ql, f2ord(lb));
+                    }
+                    mn = fminf(mn, gm[i][l]);
                 }
+                gmin[i] = mn;
             }
         }
         unsigned long long c_emit = 0;
