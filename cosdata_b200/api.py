@@ -92,7 +92,8 @@ def device_count():
 
 
 def debug_set_hnsw_flags(flags=0xFFFFFFFF):
-    """kernel-variant switch of CDB_MODE_HNSW searches (measurement only; results are identical); default restores"""
+    """kernel-variant switch of CDB_MODE_HNSW searches (measurement only; results are identical): 8 = the CTA-per-query
+    kernel on graphs with metadata, 16 = the unsorted candidate pool on plain graphs, other bits ignored; default restores"""
     _check(_lib.load().cdb_debug_set_hnsw_flags(flags & 0xFFFFFFFF))
 
 
@@ -498,8 +499,7 @@ class DenseIndex:
         _check(self._lib.cdb_index_hnsw_profile(self._h, 1 if enable else 0, _ptr(out)))
         if out is None:
             return None
-        names = ["adjacency", "fixed_set", "stage_issue", "stage_wait", "chains", "merge", "level_sort", "levels_total", "pops",
-                 "speculation", "chain_phases", "speculative_evals"]
+        names = ["adjacency", "fixed_set", "stage_issue", "stage_wait", "chains", "merge", "level_sort", "levels_total", "pops"]
         return {n: int(v) for n, v in zip(names, out)}
 
     def stats(self):

@@ -20,7 +20,7 @@ namespace cdb {
 static thread_local std::string t_last_error;
 void set_error(const std::string &msg) { t_last_error = msg; }
 std::atomic<uint64_t> g_launch_count{0};
-std::atomic<uint32_t> g_hnsw_flags{CDB_HNSW_F_DEFAULT};
+std::atomic<uint32_t> g_hnsw_flags{0};
 
 cudaError_t allow_max_dynamic_smem(const void *kernel) {
     static std::mutex mu;
@@ -866,9 +866,9 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
                                     sc->hn_labels.as<uint32_t>(), sc->cur_keys)))
             return rc;
     } else {
-        // one warp per query (hnsw_warp.cu); CDB_HNSW_F_CTA selects the round-1 CTA-per-query kernel for A/B measurements
+        // one warp per query (hnsw_warp.cu)
         a.prof = ix->hn_prof_on ? ix->hn_prof.as<unsigned long long>() : nullptr;
-        if ((rc = (a.flags & CDB_HNSW_F_CTA) ? hnsw_search_device(a, s) : hnsw_search_warp_device(a, s))) return rc;
+        if ((rc = hnsw_search_warp_device(a, s))) return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
         if ((rc = hnsw_dedup_device(a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, ix->graph.root_row, d.id_base, k5, nq,
                                     sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), s)))
@@ -1921,7 +1921,7 @@ cdb_status cdb_index_hnsw_counters(const cdb_index *ix, uint64_t *out2) {
 }
 
 cdb_status cdb_debug_set_hnsw_flags(uint32_t flags) {
-    g_hnsw_flags.store(flags == 0xFFFFFFFFu ? CDB_HNSW_F_DEFAULT : flags);
+    g_hnsw_flags.store(flags == 0xFFFFFFFFu ? 0u : flags);
     return CDB_OK;
 }
 

@@ -1,72 +1,8 @@
-// hnsw.cu -- batched HNSW search on a flat graph (S1, CDB_MODE_HNSW):
-//   ann_search              src/vector_store.rs:256-402
-//   traverse_find_nearest   src/vector_store.rs:1112-1204
-//   PerformantFixedSet      src/models/fixedset.rs:2-29
+// hnsw.cu -- the step between the HNSW traversal (hnsw_warp.cu) and the exact re-rank (S1, CDB_MODE_HNSW):
 //   remove_duplicates_and_filter  src/models/common.rs:381-412
-// One CTA per query (the data-parallel axis of IndexOps::batch_search); all queries of a batch
-// are resident at once.  Per pop the CTA
-//   1. walks the popped node's first `shortlist_size` slots IN ORDER through the lossy fixed set
-//      (one thread: the membership test + insert is order dependent, aliasing ids included),
-//   2. scores the surviving neighbours in parallel, one thread per neighbour, with the reference's
-//      exact per-pair arithmetic (pair_distance), gathering the rows straight from HBM,
-//   3. merges them into the candidate queue.
-// The reference's BinaryHeap is unbounded but performs exactly `ef` pops, so an entry ranked
-// below the number of pops still to come can never be popped: the queue is a sorted array of at
-// most `ef` entries and the pop order is identical to the heap's.  Keys are
-// (order_key(score) << 32 | ~id): "better score first, then smaller id" -- the oracle's tie rule.
 #include "hnsw_traverse.cuh"
 
 namespace cdb {
-
-constexpr uint32_t HN_FINAL_LEN = 100;  // vector_store.rs:1194
-
-__global__ void __launch_bounds__(HN_THREADS) hnsw_search_kernel(HnswArgs a) {
-    extern __shared__ __align__(16) uint8_t smem[];
-    const HnSmem m = hn_carve(smem, a.row_pitch, a.ef);
-    __shared__ HnShared sh;
-    const uint32_t qi = blockIdx.x;
-    const int tid = threadIdx.x;
-    for (uint32_t i = tid; i < a.row_pitch / 4; i += HN_THREADS)
-        reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(a.q + (size_t)qi * a.row_pitch)[i];
-    const float qmag = a.qmags[qi];
-    const HnScoreCtx sc{a.rows, a.row_pitch, a.mags, a.dim, a.st, a.metric, a.g.root_row};
-    if (tid == 0) { sh.err = 0; sh.entry = a.g.entry; }
-    uint32_t out_total = 0;
-    unsigned long long evals = 0, pops = 0;
-    long long prof[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    __syncthreads();
-
-    // ann_search (vector_store.rs:256-402): fresh fixed set and ef budget per level, results of all levels
-    // concatenated, child of the best result is the entry of the next level
-    for (int level = (int)a.g.num_levels; level >= 0; --level) {
-        const uint32_t nb = level == 0 ? a.g.nbrs0 : a.g.nbrs;
-        const uint32_t take = min(min(a.shortlist, nb), HN_MAX_TAKE);
-        const uint32_t *node_row = a.g.node_row[level];
-        hn_traverse_level(node_row, a.g.adj[level], nb, take, sc, m, sh, qmag, HN_QUERY_ID, a.ef, evals, pops, nullptr,
-                          a.prof ? prof : nullptr);
-        if (sh.err) break;
-        const uint32_t keep = min(sh.rlen, HN_FINAL_LEN);
-        for (uint32_t i = tid; i < keep; i += HN_THREADS) {
-            const uint32_t slot = out_total + i;
-            if (slot < a.out_cap) {
-                a.out_rows[(size_t)qi * a.out_cap + slot] = node_row[m.rnodes[i]];
-                a.out_scores[(size_t)qi * a.out_cap + slot] = __uint_as_float(key_to_bits(a.metric, (uint32_t)(m.rkeys[i] >> 32)));
-            }
-        }
-        out_total += keep;
-        if (tid == 0 && level > 0) sh.entry = a.g.child[level][m.rnodes[0]];
-        __syncthreads();
-    }
-    if (tid == 0) {
-        a.out_n[qi] = sh.err ? 0u : min(out_total, a.out_cap);
-        if (sh.err) atomicOr(a.err32 + qi, sh.err);
-        if (a.counters) { atomicAdd(a.counters, evals); atomicAdd(a.counters + 1, pops); }
-        if (a.prof) {
-            prof[8] = (long long)pops;
-            for (int i = 0; i < 9; ++i) atomicAdd(a.prof + i, (unsigned long long)prof[i]);
-        }
-    }
-}
 
 // remove_duplicates_and_filter: dedup by id keeping the first occurrence, drop the root, sort
 // best-first, truncate to 5*k.  One CTA per query; writes global candidate ids for the re-rank.
@@ -114,19 +50,6 @@ __global__ void __launch_bounds__(256) hnsw_dedup_kernel(const uint32_t *__restr
     const uint32_t m = min((uint32_t)kept, k5);
     for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) cand[(size_t)q * k5 + i] = id_base + vals[i];
     if (threadIdx.x == 0) cand_cnt[q] = m;
-}
-
-size_t hnsw_search_smem(uint32_t row_pitch, uint32_t ef) { return hn_smem_bytes(row_pitch, ef); }
-
-cdb_status hnsw_search_device(const HnswArgs &a, cudaStream_t s) {
-    if (!a.nq) return CDB_OK;
-    if (a.ef == 0 || a.ef > 4096) { set_error("hnsw: ef_search must be in 1..4096"); return CDB_INVALID_PARAMS; }
-    const size_t smem = hnsw_search_smem(a.row_pitch, a.ef);
-    if (smem > 200 * 1024) { set_error("hnsw: ef_search too large for shared memory"); return CDB_INVALID_PARAMS; }
-    CDB_ALLOW_SMEM(hnsw_search_kernel, smem);
-    hnsw_search_kernel<<<a.nq, HN_THREADS, smem, s>>>(a);
-    CDB_LAUNCH_CHECK();
-    return CDB_OK;
 }
 
 cdb_status hnsw_dedup_device(const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n, uint32_t in_cap, int metric,

@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs
         const uint32_t take = min(min(a.shortlist, l.nb), HN_MAX_TAKE);
         if (a.replicas) { md.node_id = l.node_id; md.node_md = l.node_md; }
         hn_traverse_level(l.node_row, l.adj, l.nb, take, a.sc, m, sh, qmag, self_id, a.ef, evals, pops, a.replicas ? &md : nullptr,
-                          nullptr, !del);
+                          !del);
         if (sh.err) {
             if (del && tid == 0)   // D3: no relinks on this level or below
                 for (int lv = level; lv >= 0; --lv) a.z_n[(size_t)b * L1 + lv] = HN_EMPTY;

@@ -4,7 +4,7 @@
 //   CosineSimilarity::calculate arms      src/distance/cosine.rs:34-102 (metadata.cuh)
 //   remove_duplicates_and_filter          src/models/common.rs:381-412 (dedup by replica id, pseudo nodes dropped)
 //   get_raw_emb_by_internal_id            src/models/collection.rs:368-384 (replica id -> base vector; here node_row)
-// One CTA per query like hnsw.cu; the traversal itself is the shared hn_traverse_level with a metadata context.  Searches run
+// One CTA per query; the traversal itself is the shared hn_traverse_level with a metadata context.  Searches run
 // the warp-per-query form of the same steps (hnsw_warp.cu); this kernel answers CDB_HNSW_F_CTA and shapes whose warp carve
 // does not fit.
 // Per level and filter the <= 100 results are merged into the level's candidate list z (<= 100 best of all filters,
@@ -199,7 +199,7 @@ cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s) {
     const size_t smem = round_up((uint32_t)hn_smem_bytes(a.a.row_pitch, a.a.ef), 16) + (size_t)HNM_Z * 12 + (size_t)a.M * 4 + 16;
     if (smem > 200 * 1024) { set_error("hnsw: ef_search / metadata dims too large for shared memory"); return CDB_INVALID_PARAMS; }
     // the shapes accepted are this kernel's; the warp form takes every one of them whose own carve fits
-    if (!(a.a.flags & CDB_HNSW_F_CTA) && hnsw_warp_md_smem(a.a.row_pitch, a.a.dim, a.a.ef, a.a.st, a.a.metric, a.M) <= 200 * 1024)
+    if (!(a.a.flags & CDB_HNSW_F_CTA) && hnsw_warp_md_smem(a.a.row_pitch, a.a.ef, a.M) <= 200 * 1024)
         return hnsw_search_warp_md_device(a, s);
     CDB_ALLOW_SMEM(hnsw_search_md_kernel, smem);
     hnsw_search_md_kernel<<<a.a.nq, HN_THREADS, smem, s>>>(a);

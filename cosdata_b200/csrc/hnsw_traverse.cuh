@@ -1,5 +1,5 @@
-// hnsw_traverse.cuh -- traverse_find_nearest (src/vector_store.rs:1112-1204) for one CTA, shared by the search
-// kernel (hnsw.cu) and the index builder (hnsw_build.cu).
+// hnsw_traverse.cuh -- traverse_find_nearest (src/vector_store.rs:1112-1204) for one CTA, shared by the metadata search
+// kernel (hnsw_md.cu) and the index builder (hnsw_build.cu).
 //
 // The reference's BinaryHeap is unbounded but performs exactly `ef` pops, so an entry ranked below the number of
 // pops still to come can never be popped: the queue is a sorted array of at most `ef` entries in shared memory and
@@ -86,7 +86,7 @@ __device__ __forceinline__ void hn_cp_async16(void *smem_dst, const void *gsrc) 
 __device__ __forceinline__ void hn_cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ uint32_t hw_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // TMA bulk copy (UBLKCP): `bytes` contiguous bytes global -> shared, completion counted on the mbarrier.  One instruction
-// per row, issued by one lane: no per-lane address arithmetic, no LSU slots (the round-1 kernel issued 96 cp.async per row).
+// per row, issued by one lane: no per-lane address arithmetic, no LSU slots (the CTA traversal issues 96 cp.async per f16 x 768 row).
 __device__ __forceinline__ void hw_bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
@@ -188,12 +188,9 @@ __device__ __forceinline__ int hn_score_node(const uint32_t *__restrict__ node_r
 __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, const uint32_t *__restrict__ adj, uint32_t nb,
                                          uint32_t take, const HnScoreCtx &sc, const HnSmem &m, HnShared &sh, float qmag,
                                          uint32_t self_id, uint32_t ef, unsigned long long &evals, unsigned long long &pops,
-                                         const HnMdCtx *md = nullptr, long long *prof = nullptr, bool seed_self = true) {
-    // prof (thread 0 only, may be null): clock64 sums with the slot meaning of hnsw_warp.cu's HW_PROF_SLOTS
+                                         const HnMdCtx *md = nullptr, bool seed_self = true) {
     // seed_self = false: nothing is pre-inserted into the fixed set (delete_embedding, vector_store.rs:1231-1235)
     const int tid = threadIdx.x;
-    long long pt0 = 0, pt1 = 0, pt2 = 0, pt3 = 0, pts = 0, ptg = 0, ptw = 0;
-    if (prof && tid == 0) pt0 = clock64();
     const uint32_t pp = plane_pitch(sc.dim);
     const uint32_t EFP = m.EFP;
     const bool keep_fs = md && md->keep_fs;
@@ -221,7 +218,6 @@ __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, 
         if (qlen == 0 || visited >= ef) break;
         uint64_t *Q = m.qkeys + cur * EFP;
         uint32_t *QN = m.qnodes + cur * EFP;
-        if (prof && tid == 0) pt1 = clock64();
         // ---- pop (one thread), then the walk through the lossy fixed set for all slots at once.
         // The reference tests and inserts slot by slot: a slot is scored iff its bit is not yet set AND no
         // earlier non-empty slot of this pop maps to the same bit (that one either set it or found it set).
@@ -242,7 +238,6 @@ __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, 
             sh.bitkey[tid] = my_bitkey;
         }
         __syncthreads();
-        if (prof && tid == 0) { pt2 = clock64(); prof[0] += pt2 - pt1; }
         bool accept = false;
         if (my_bitkey != 0xFFFFFFFFu) {
             accept = ((m.fs[my_bitkey >> 6] >> (my_bitkey & 0x3f)) & 1ull) == 0;
@@ -262,21 +257,17 @@ __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, 
         // ---- score the new neighbours, one thread each, reference arithmetic, rows staged through shared memory
         if ((uint32_t)tid < nc) sh.nrow[tid] = node_row[m.nnodes[tid]];
         __syncthreads();
-        if (prof && tid == 0) { pt3 = clock64(); prof[1] += pt3 - pt2; }
         {
             const uint32_t cpr = sc.row_pitch >> 4;   // 16-byte chunks per stored row
             for (uint32_t g0 = 0; g0 < nc; g0 += m.stage_rows) {
                 const uint32_t gn = min(m.stage_rows, nc - g0);
-                if (prof && tid == 0) ptg = clock64();
                 for (uint32_t c = tid; c < gn * cpr; c += HN_THREADS) {
                     const uint32_t r = c / cpr, o = c - r * cpr;
                     hn_cp_async16(m.stage + (size_t)r * m.stage_pitch + (size_t)o * 16,
                                   sc.rows + (size_t)sh.nrow[g0 + r] * sc.row_pitch + (size_t)o * 16);
                 }
-                if (prof && tid == 0) pts = clock64();
                 hn_cp_async_wait_all();
                 __syncthreads();
-                if (prof && tid == 0) { ptw = clock64(); prof[2] += pts - ptg; prof[3] += ptw - pts; }
                 if ((uint32_t)tid < gn) {
                     const uint32_t pos = g0 + tid;
                     float d = 0.f;
@@ -286,11 +277,9 @@ __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, 
                     m.nkeys[pos] = make_key64(order_key(sc.metric, __float_as_uint(d)), nid);
                 }
                 __syncthreads();   // the stage is reused by the next group
-                if (prof && tid == 0) prof[4] += clock64() - ptw;
             }
         }
         if (tid == 0) evals += nc;
-        if (prof && tid == 0) pt2 = clock64();
         if (sh.err_first != 0xFFFFFFFFu) {
             if (tid == 0) sh.err = sh.err_first & 0xFFu;
             __syncthreads();
@@ -331,15 +320,12 @@ __device__ inline void hn_traverse_level(const uint32_t *__restrict__ node_row, 
             if (tid == 0) { sh.qlen = min(oldn + nc, cap); sh.cur = cur ^ 1; sh.visited = visited + 1; }
         }
         __syncthreads();
-        if (prof && tid == 0) prof[5] += clock64() - pt2;
     }
     __syncthreads();
-    if (prof && tid == 0) pt1 = clock64();
     const uint32_t rlen = sh.rlen;
     uint32_t P = 1;
     while (P < rlen) P <<= 1;
     hn_sort_desc(m.rkeys, m.rnodes, rlen, P);
-    if (prof && tid == 0) { const long long t = clock64(); prof[6] += t - pt1; prof[7] += t - pt0; }
 }
 
 }  // namespace cdb

@@ -29,35 +29,27 @@ namespace cdb {
 constexpr uint32_t HW_FINAL_LEN = 100;          // vector_store.rs:1194
 // staged neighbour rows per group, sized so that 7 warps (queries) per SM still fit in shared memory at D = 768:
 constexpr uint32_t HW_STAGE_BYTES = 18700;      // 12 rows of f16 x 768, 6 of f32 x 768
-constexpr uint32_t HW_STAGE_BYTES_SPEC = 20200; // speculative form (score cache + work list added): 13 rows of f16 x 768
-constexpr uint32_t HW_CACHE = 256;              // speculative form: direct-mapped (node -> score key) cache entries per query
-constexpr int HW_NSRC = 3;                      // speculative form: upcoming heads examined per chain phase
-constexpr uint32_t HW_WORK = HN_MAX_TAKE + 32;  // speculative form: rows to score in one pop (misses of the head + fill)
 // clock64 sums per query (lane 0): [0] pop + adjacency (+ node_row) loads, [1] fixed-set walk + compaction + prefetches,
 // [2] issue of the row copies, [3] wait for the rows, [4] distance chains, [5] queue merge, [6] end-of-level result sort,
 // [7] whole levels, [8] pops
-// speculative form: [9] cache look-ups + choice of speculative rows, [10] chain phases, [11] speculative evaluations
-constexpr int HW_PROF_SLOTS = 12;
+constexpr int HW_PROF_SLOTS = 9;
 
 constexpr uint32_t HW_MD_Z = 256;   // metadata form: a level's merged list z (<= 100) + one traversal's results (<= 100)
 
 struct HwCarve {
     uint32_t EFP, stage_pitch, stage_rows;
-    uint32_t off_q32, off_qkeys, off_rkeys, off_nkeys, off_fs, off_qnodes, off_rnodes, off_nnodes, off_nrow, off_bar, off_stage, total;
-    uint32_t off_cache, off_work, off_sadj;   // speculative form only
+    uint32_t off_qkeys, off_rkeys, off_nkeys, off_fs, off_qnodes, off_rnodes, off_nnodes, off_nrow, off_bar, off_stage, total;
     uint32_t off_zkeys, off_znodes, off_qvars, off_qbits; // metadata form only: z list, {f0, f1, results so far}, the filter's dims as i32 [M]
 };
 
-// md: metadata form with M metadata dims (never speculative)
-__host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, uint32_t ef, bool f16fast, bool spec = false,
-                                            bool md = false, uint32_t M = 0) {
+// md: metadata form with M metadata dims
+__host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t ef, bool md = false, uint32_t M = 0) {
     HwCarve c;
     c.EFP = hn_efp(ef);
     c.stage_pitch = round_up(row_pitch, 16) + 16;   // + 16 bytes: the lanes' rows start on different banks
-    uint32_t r = (spec ? HW_STAGE_BYTES_SPEC : HW_STAGE_BYTES) / c.stage_pitch;
+    uint32_t r = HW_STAGE_BYTES / c.stage_pitch;
     c.stage_rows = r > 32 ? 32 : (r ? r : 1u);      // one lane scores one staged row
-    uint32_t o = round_up(row_pitch, 16);
-    c.off_q32 = o;            // (no f32 copy of the query: the chain widens the f16 / bf16 code directly)
+    uint32_t o = round_up(row_pitch, 16);           // the query's code (the chains widen it directly: no f32 copy)
     c.off_qkeys = o;          o += 2 * c.EFP * 8;
     c.off_rkeys = o;          o += c.EFP * 8;
     c.off_nkeys = o;          o += HN_MAX_TAKE * 8;
@@ -67,13 +59,6 @@ __host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, ui
     c.off_rnodes = o;         o += c.EFP * 4;
     c.off_nnodes = o;         o += HN_MAX_TAKE * 4;
     c.off_nrow = o;           o += HN_MAX_TAKE * 4;
-    c.off_cache = c.off_work = c.off_sadj = 0;
-    if (spec) {
-        o = round_up(o, 8);
-        c.off_cache = o;      o += HW_CACHE * 8;
-        c.off_work = o;       o += 3 * HW_WORK * 4;
-        c.off_sadj = o;       o += HW_NSRC * HN_MAX_TAKE * 4;
-    }
     c.off_zkeys = c.off_znodes = c.off_qvars = c.off_qbits = 0;
     if (md) {
         o = round_up(o, 8);
@@ -89,13 +74,9 @@ __host__ __device__ inline HwCarve hw_carve(uint32_t row_pitch, uint32_t dim, ui
 
 struct HwSmem {
     uint8_t *qs;
-    float *q32;
     uint64_t *qkeys, *rkeys, *nkeys;
     uint32_t *fs;            // PerformantFixedSet as 128 x 32-bit words: bucket b = words 2b, 2b+1 (native 32-bit shared atomics)
     uint32_t *qnodes, *rnodes, *nnodes, *nrow;
-    uint64_t *cache;         // speculative form: (node << 32 | score order key), tag 0xFFFFFFFF = empty
-    uint32_t *wnode, *wrow, *wdst;
-    uint32_t *sadj;          // speculative form: adjacency slots of the next heads, [HW_NSRC][64], filled by cp.async
     uint8_t *stage;
     uint32_t bar;            // shared-space address of the warp's mbarrier (row copies complete on it)
     uint32_t EFP, stage_pitch, stage_rows;
@@ -254,78 +235,17 @@ __device__ __forceinline__ uint32_t hw_score_group(const HnScoreCtx &sc, const H
     return err_first;
 }
 
-__device__ __forceinline__ uint32_t hw_cache_slot(uint32_t node) { return (node * 0x9E3779B1u) >> 24; }   // HW_CACHE = 256
-
-// Speculative form: score the work list wnode/wrow[0 .. nt).  Entries [0, nm) are the head's neighbours whose score is not
-// cached (slot order kept; the key goes to nkeys[wdst]); entries [nm, nt) are neighbours of upcoming heads that fill the
-// otherwise idle lanes of the chain phase -- their score keys go to the cache (an evaluation that fails is simply not cached:
-// the error belongs to the pop that commits it).  Same staging and the same chains as hw_score_group.
-template <int FAST, bool PROF>
-__device__ __forceinline__ uint32_t hw_score_work(const HnScoreCtx &sc, const HwSmem &m, float qmag, uint32_t pp, uint32_t nm,
-                                                  uint32_t nt, int lane, HwState &st) {
-    uint32_t err_first = 0xFFFFFFFFu;
-    for (uint32_t g0 = 0; g0 < nt; g0 += m.stage_rows) {
-        const uint32_t gn = min(m.stage_rows, nt - g0);
-        long long ts = 0, ti = 0, tw = 0;
-        if (PROF) ts = clock64();
-        uint32_t row = 0;
-        float rmag = 0.0f;
-        if (lane == 0) hw_mbar_expect(m.bar, gn * sc.row_pitch);
-        if ((uint32_t)lane < gn) {
-            row = m.wrow[g0 + lane];
-            hw_bulk_g2s(hw_smem_u32(m.stage + (size_t)lane * m.stage_pitch), sc.rows + (size_t)row * sc.row_pitch, sc.row_pitch, m.bar);
-            rmag = sc.mags[row];
-        }
-        if (PROF) ti = clock64();
-        hw_mbar_wait(m.bar, st.bar_phase);
-        st.bar_phase ^= 1u;
-        if (PROF) tw = clock64();
-        int rc = CDB_OK;
-        const uint32_t idx = g0 + (uint32_t)lane;
-        if ((uint32_t)lane < gn) {
-            const uint8_t *code = m.stage + (size_t)lane * m.stage_pitch;
-            float d = 0.0f;
-            if (FAST) {
-                const float dot = hw_dot16<FAST>(m.qs, code, sc.dim);
-                if (sc.metric == CDB_METRIC_COSINE) {
-                    const float denom = __fmul_rn(qmag, rmag);
-                    if (denom == 0.0f) rc = CDB_CALCULATION_ERROR;   // cosine.rs:230-231
-                    else d = canon_nan(__fdiv_rn(dot, denom));
-                } else {
-                    d = dot;
-                }
-            } else {
-                rc = pair_distance(sc.metric, sc.st, sc.dim, m.qs, qmag, pp, code, rmag, pp, &d);
-            }
-            const uint32_t okey = order_key(sc.metric, __float_as_uint(d));
-            if (idx < nm) m.nkeys[m.wdst[idx]] = make_key64(okey, hn_id(sc.root_row, row));
-            else if (rc == CDB_OK) { const uint32_t nd = m.wnode[idx]; m.cache[hw_cache_slot(nd)] = ((uint64_t)nd << 32) | okey; }
-        }
-        const uint32_t bad = __ballot_sync(0xFFFFFFFFu, rc != CDB_OK && idx < nm);
-        if (bad && err_first == 0xFFFFFFFFu) {   // the reference stops at the first Err (slot order)
-            const int src_lane = __ffs(bad) - 1;
-            const int flag = __shfl_sync(0xFFFFFFFFu, (int)md_err_flag(rc), src_lane);
-            err_first = ((g0 + (uint32_t)src_lane) << 8) | (uint32_t)flag;
-        }
-        __syncwarp();
-        if (PROF) { const long long te = clock64(); st.prof[2] += ti - ts; st.prof[3] += tw - ti; st.prof[4] += te - tw; st.prof[10] += 1; }
-    }
-    return err_first;
-}
-
 // One level (traverse_find_nearest).  All 32 lanes call it with warp-uniform arguments.  On return (st.err == 0)
 // rkeys/rnodes[0..st.rlen) hold every popped entry sorted best first.
+// pool_form: the candidates are an unsorted pool instead of the sorted queue (CDB_HNSW_F_POOL; ignored by the metadata form).
 // MD (metadata form, md != null): the fixed set and the keys use the replica ids md->node_id, pairs are scored through the
-// metadata arms, md->keep_fs keeps the fixed set of the previous traversal of the level; always the sorted-queue,
-// non-speculative form (SPEC / POOL are ignored).
+// metadata arms, md->keep_fs keeps the fixed set of the previous traversal of the level.
 template <int FAST, bool PROF, bool MD>
 __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null: identity */, const uint32_t *__restrict__ adj,
                                   uint32_t nb, uint32_t take, const HnScoreCtx &sc, const HwSmem &m, float qmag, uint32_t self_id,
-                                  uint32_t ef, uint32_t entry, HwState &st, int lane, uint32_t flags, const HnMdCtx *md = nullptr) {
+                                  uint32_t ef, uint32_t entry, HwState &st, int lane, bool pool_form, const HnMdCtx *md = nullptr) {
+    const bool pool = !MD && pool_form;
     const uint32_t pp = plane_pitch(sc.dim);
-    const bool f_preload = (flags & CDB_HNSW_F_PRELOAD) != 0, f_atomfs = (flags & CDB_HNSW_F_ATOMFS) != 0;
-    const bool f_pool = !MD && (flags & CDB_HNSW_F_POOL) != 0;
-    const bool f_spec = !MD && (flags & CDB_HNSW_F_SPEC) != 0 && !f_pool;
     const uint32_t EFP = m.EFP;
     const uint32_t CAPQ = 2 * EFP;      // pool form: both queue buffers are one unsorted pool
     const uint32_t bmask = nb - 1u;
@@ -335,9 +255,6 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
     if (!MD || !md->keep_fs)
 #pragma unroll
         for (int i = 0; i < 4; ++i) m.fs[lane + 32 * i] = 0u;
-    if (f_spec)   // node indices are level-local: the score cache starts empty on every level
-        for (uint32_t i = lane; i < HW_CACHE; i += 32) m.cache[i] = ~0ull;
-    uint32_t sd0 = HN_EMPTY, sd1 = HN_EMPTY, sd2 = HN_EMPTY, sd3 = HN_EMPTY;   // queue entries whose neighbours are all cached
     if (lane == 0) { m.nnodes[0] = entry; m.nrow[0] = node_row ? node_row[entry] : entry; }
     __syncwarp();
     {
@@ -357,22 +274,22 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
     uint32_t qlen = 1, cur = 0, visited = 0, rlen = 0;
     // adjacency slots of the head, loaded one pop ahead (while the previous pop's queue merge runs)
     uint32_t pre_node = HN_EMPTY, pre_nbl[2] = {HN_EMPTY, HN_EMPTY};
-    // POOL form (CDB_HNSW_F_POOL): the candidates are an UNSORTED pool in shared memory and the head is found by an
-    // arg-max (8 slots per lane, two 32-bit REDUX) instead of keeping a sorted queue that every pop has to merge into.
-    // The pop order is the same: the head is the best entry present, and an entry is only ever dropped when at least
-    // (pops still to come) better entries exist, so it could never have been popped.
-    uint64_t hkey = f_pool ? m.qkeys[0] : 0ull;
+    // POOL form: the candidates are an UNSORTED pool in shared memory and the head is found by an arg-max (8 slots per lane,
+    // two 32-bit REDUX) instead of keeping a sorted queue that every pop has to merge into.  The pop order is the same: the
+    // head is the best entry present, and an entry is only ever dropped when at least (pops still to come) better entries
+    // exist, so it could never have been popped.
+    uint64_t hkey = pool ? m.qkeys[0] : 0ull;
     uint32_t hnode = entry;
     bool have_head = true;
-    if (f_pool) qlen = 0;
-    while ((f_pool ? have_head : qlen > 0) && visited < ef) {
+    if (pool) qlen = 0;
+    while ((pool ? have_head : qlen > 0) && visited < ef) {
         uint64_t *Q = m.qkeys + cur * EFP;
         uint32_t *QN = m.qnodes + cur * EFP;
         long long t1 = 0, t2 = 0, t3 = 0, t4 = 0;
         if (PROF) t1 = clock64();
         // ---- pop
-        const uint32_t bn = f_pool ? hnode : QN[0];
-        if (lane == 0) { m.rkeys[rlen] = f_pool ? hkey : Q[0]; m.rnodes[rlen] = bn; }
+        const uint32_t bn = pool ? hnode : QN[0];
+        if (lane == 0) { m.rkeys[rlen] = pool ? hkey : Q[0]; m.rnodes[rlen] = bn; }
         ++rlen;
         st.pops += 1;
         // ---- adjacency: slots lane and lane + 32; ids and fixed-set bit positions
@@ -386,12 +303,6 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
                 nbl[h] = slot < take ? __ldg(adj + (size_t)bn * nb + slot) : HN_EMPTY;
             }
         }
-        // SPECULATIVE form (CDB_HNSW_F_SPEC): a pop scores ~4 rows, so ~28 lanes idle through a 768-step dependent chain.  The
-        // next heads are already known (the sorted queue), a score is a pure function of (query, node), and the fixed set only
-        // grows: whatever a later pop will score is among the neighbours of that head whose bit is clear NOW.  So the free
-        // lanes of this pop's chain phase score those rows ahead of time into a small cache; the later pop walks its fixed
-        // set exactly as before (same order, same insertions, same evals count) and takes the keys from the cache, and a pop
-        // whose accepted neighbours are all cached has no chain phase at all.
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             row[h] = 0;
@@ -401,30 +312,6 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
                 const uint32_t id = MD ? __ldg(md->node_id + nbl[h]) : hn_id(sc.root_row, row[h]);
                 bk[h] = (((id >> 6) & bmask) << 6) | (id & 0x3f);
             }
-        }
-        uint32_t ssrc[HW_NSRC];
-#pragma unroll
-        for (int sidx = 0; sidx < HW_NSRC; ++sidx) ssrc[sidx] = HN_EMPTY;
-        if (f_spec) {
-            // the next queue entries whose neighbours are not all cached yet (lanes 1..6 look at one entry each).  Their adjacency
-            // slots are copied to shared memory with cp.async: no registers and no scoreboard are held across the fixed-set walk
-            // (register loads issued here made the walk's own shared-memory waits stall on the same scoreboards), and the data is
-            // there when the chain phase of this pop -- if it has one -- chooses its fill
-            const uint32_t mine = (lane >= 1 && (uint32_t)lane < qlen && lane <= 2 * HW_NSRC) ? QN[lane] : HN_EMPTY;
-            uint32_t pick = __ballot_sync(0xFFFFFFFFu, mine != HN_EMPTY && mine != sd0 && mine != sd1 && mine != sd2 && mine != sd3);
-#pragma unroll
-            for (int sidx = 0; sidx < HW_NSRC; ++sidx)
-                if (pick) { ssrc[sidx] = __shfl_sync(0xFFFFFFFFu, mine, __ffs(pick) - 1); pick &= pick - 1; }
-            asm volatile("cp.async.wait_all;" ::: "memory");   // copies of the previous pop (long finished)
-#pragma unroll
-            for (int sidx = 0; sidx < HW_NSRC; ++sidx)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const uint32_t slot = (uint32_t)lane + 32u * h;
-                    if (ssrc[sidx] != HN_EMPTY && slot < take)
-                        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(hw_smem_u32(m.sadj + sidx * HN_MAX_TAKE + slot)),
-                                     "l"(adj + (size_t)ssrc[sidx] * nb + slot) : "memory");
-                }
         }
         if (PROF) t2 = clock64();
         // ---- the walk through the lossy fixed set, slot order: a slot is scored iff its bit is not yet set AND no
@@ -442,15 +329,12 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
             const uint32_t cand0 = __ballot_sync(0xFFFFFFFFu, clear[0]);
             const uint32_t cand1 = two ? __ballot_sync(0xFFFFFFFFu, clear[1]) : 0u;
             accept[0] = clear[0]; accept[1] = clear[1];
-            bool resolve = true;   // apply the slot-order rule explicitly
-            if (f_atomfs) {
-                bool won0 = false, won1 = false;
-                if (clear[0]) { const uint32_t bit = 1u << (bk[0] & 31); won0 = (atomicOr(&m.fs[bk[0] >> 5], bit) & bit) == 0; }
-                if (clear[1]) { const uint32_t bit = 1u << (bk[1] & 31); won1 = (atomicOr(&m.fs[bk[1] >> 5], bit) & bit) == 0; }
-                const uint32_t w0 = __ballot_sync(0xFFFFFFFFu, won0);
-                const uint32_t w1 = two ? __ballot_sync(0xFFFFFFFFu, won1) : 0u;
-                resolve = __popc(w0) + __popc(w1) != __popc(cand0) + __popc(cand1);
-            }
+            bool won0 = false, won1 = false;
+            if (clear[0]) { const uint32_t bit = 1u << (bk[0] & 31); won0 = (atomicOr(&m.fs[bk[0] >> 5], bit) & bit) == 0; }
+            if (clear[1]) { const uint32_t bit = 1u << (bk[1] & 31); won1 = (atomicOr(&m.fs[bk[1] >> 5], bit) & bit) == 0; }
+            const uint32_t w0 = __ballot_sync(0xFFFFFFFFu, won0);
+            const uint32_t w1 = two ? __ballot_sync(0xFFFFFFFFu, won1) : 0u;
+            const bool resolve = __popc(w0) + __popc(w1) != __popc(cand0) + __popc(cand1);   // apply the slot-order rule explicitly
             if (resolve) {
                 for (uint32_t rest = cand0; rest; rest &= rest - 1) {   // ascending slot order
                     const int c = __ffs(rest) - 1;
@@ -462,11 +346,6 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
                     const int c = __ffs(rest) - 1;
                     const uint32_t cb = __shfl_sync(0xFFFFFFFFu, bk[1], c);
                     if (lane > c && cb == bk[1]) accept[1] = false;
-                }
-                if (!f_atomfs) {
-#pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        if (accept[h]) atomicOr(&m.fs[bk[h] >> 5], 1u << (bk[h] & 31));
                 }
             }
             // without a conflict the accepted slots are exactly the candidates: no further ballot needed
@@ -489,84 +368,11 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
         }
         if (PROF) t3 = clock64();
         // ---- score the new neighbours
-        uint32_t e = 0xFFFFFFFFu;
-        if (f_spec) {
-            // keys of accepted neighbours that were scored ahead of time; the others form the work list
-            bool miss[2];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const uint32_t pos = (uint32_t)lane + 32u * h;
-                miss[h] = false;
-                if (pos < nc) {
-                    const uint32_t nd = m.nnodes[pos];
-                    const uint64_t ce = m.cache[hw_cache_slot(nd)];
-                    if ((uint32_t)(ce >> 32) == nd) m.nkeys[pos] = make_key64((uint32_t)ce, hn_id(sc.root_row, m.nrow[pos]));
-                    else miss[h] = true;
-                }
-            }
-            const uint32_t mb0 = __ballot_sync(0xFFFFFFFFu, miss[0]);
-            const uint32_t mb1 = nc > 32 ? __ballot_sync(0xFFFFFFFFu, miss[1]) : 0u;
-            const uint32_t nm0 = (uint32_t)__popc(mb0), nm = nm0 + (uint32_t)__popc(mb1);
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-                if (miss[h]) {
-                    const uint32_t pos = (uint32_t)lane + 32u * h;
-                    const uint32_t w = (h ? nm0 : 0u) + (uint32_t)__popc((h ? mb1 : mb0) & lt);
-                    m.wnode[w] = m.nnodes[pos]; m.wrow[w] = m.nrow[pos]; m.wdst[w] = pos;
-                }
-            uint32_t nt = nm;
-            if (nm > 0 && nm < m.stage_rows) {
-                asm volatile("cp.async.wait_all;" ::: "memory");   // every lane reads back exactly the slots it copied
-                // one chain phase is due anyway: fill its free lanes with the uncached, not yet visited neighbours of the next heads
-#pragma unroll
-                for (int sidx = 0; sidx < HW_NSRC; ++sidx) {
-                    const uint32_t room = m.stage_rows - nt;
-                    if (ssrc[sidx] == HN_EMPTY || room == 0) continue;
-                    bool c[2];
-                    uint32_t r[2], snb[2];
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        c[h] = false; r[h] = 0;
-                        const uint32_t slot = (uint32_t)lane + 32u * h;
-                        const uint32_t nd = slot < take ? m.sadj[sidx * HN_MAX_TAKE + slot] : HN_EMPTY;
-                        snb[h] = nd;
-                        if (nd != HN_EMPTY) {
-                            r[h] = node_row ? __ldg(node_row + nd) : nd;
-                            const uint32_t id = hn_id(sc.root_row, r[h]);
-                            const uint32_t b = (((id >> 6) & bmask) << 6) | (id & 0x3f);
-                            if (((m.fs[b >> 5] >> (b & 31)) & 1u) == 0) c[h] = (uint32_t)(m.cache[hw_cache_slot(nd)] >> 32) != nd;
-                        }
-                    }
-                    const uint32_t c0 = __ballot_sync(0xFFFFFFFFu, c[0]);
-                    const uint32_t c1 = take > 32 ? __ballot_sync(0xFFFFFFFFu, c[1]) : 0u;
-                    const uint32_t n0 = (uint32_t)__popc(c0), tot = n0 + (uint32_t)__popc(c1);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        if (c[h]) {
-                            const uint32_t pch = (h ? n0 : 0u) + (uint32_t)__popc((h ? c1 : c0) & lt);
-                            if (pch < room) {
-                                m.wnode[nt + pch] = snb[h]; m.wrow[nt + pch] = r[h];
-                                // a row scored ahead of time is accepted later WITHOUT a chain phase and may be the very next
-                                // head: its adjacency slots must be on their way to L2 now, not when it is accepted
-                                const uint8_t *ap = reinterpret_cast<const uint8_t *>(adj + (size_t)snb[h] * nb);
-                                hw_prefetch_l2(ap);
-                                if (nb > 32) hw_prefetch_l2(ap + 128);
-                            }
-                        }
-                    if (tot <= room) { sd3 = sd2; sd2 = sd1; sd1 = sd0; sd0 = ssrc[sidx]; }   // nothing left to score for this entry
-                    nt += min(tot, room);
-                }
-            }
-            __syncwarp();   // work list visible
-            if (PROF) { const long long tq = clock64(); st.prof[9] += tq - t3; st.prof[11] += nt - nm; t3 = tq; }
-            if (nt) e = hw_score_work<FAST, PROF>(sc, m, qmag, pp, nm, nt, lane, st);
-        } else {
-            e = hw_score_group<FAST, PROF, MD>(sc, m, qmag, pp, 0, nc, lane, st, md);
-        }
+        const uint32_t e = hw_score_group<FAST, PROF, MD>(sc, m, qmag, pp, 0, nc, lane, st, md);
         st.evals += nc;
         if (e != 0xFFFFFFFFu) { st.err = e & 0xFFu; st.rlen = rlen; return; }
         if (PROF) t4 = clock64();
-        if (f_pool) {
+        if (pool) {
             uint64_t *P = m.qkeys;
             uint32_t *PN = m.qnodes;
             // ---- append the new entries, pick the next head, keep the pool bounded
@@ -590,13 +396,11 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
                 hkey = mx;
                 hnode = PN[idx];
                 have_head = true;
-                if (f_preload) {   // its adjacency slots travel while the pool is tidied up
-                    pre_node = hnode;
+                pre_node = hnode;   // its adjacency slots travel while the pool is tidied up
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const uint32_t slot = (uint32_t)lane + 32u * h;
-                        pre_nbl[h] = slot < take ? __ldg(adj + (size_t)hnode * nb + slot) : HN_EMPTY;
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    const uint32_t slot = (uint32_t)lane + 32u * h;
+                    pre_nbl[h] = slot < take ? __ldg(adj + (size_t)hnode * nb + slot) : HN_EMPTY;
                 }
                 __syncwarp();
                 if (lane == 0 && idx != qlen - 1) { P[idx] = P[qlen - 1]; PN[idx] = PN[qlen - 1]; }   // remove: last entry fills the hole
@@ -657,7 +461,7 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
             // the next head is the better of the runner-up and the best new entry: start loading its adjacency slots now,
             // the loads complete while the merge below runs
             pre_node = HN_EMPTY;
-            if (f_preload && cap > 0 && oldn + nc > 0) {
+            if (cap > 0 && oldn + nc > 0) {
                 uint64_t best = oldn ? Q[1] : 0ull;
                 uint32_t next = oldn ? QN[1] : HN_EMPTY;
                 if (nc) {
@@ -753,7 +557,6 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
 __device__ __forceinline__ HwSmem hw_smem(uint8_t *smem, const HwCarve &cv) {
     HwSmem m;
     m.qs = smem;
-    m.q32 = reinterpret_cast<float *>(smem + cv.off_q32);
     m.qkeys = reinterpret_cast<uint64_t *>(smem + cv.off_qkeys);
     m.rkeys = reinterpret_cast<uint64_t *>(smem + cv.off_rkeys);
     m.nkeys = reinterpret_cast<uint64_t *>(smem + cv.off_nkeys);
@@ -764,11 +567,6 @@ __device__ __forceinline__ HwSmem hw_smem(uint8_t *smem, const HwCarve &cv) {
     m.nnodes = reinterpret_cast<uint32_t *>(smem + cv.off_nnodes);
     m.nrow = reinterpret_cast<uint32_t *>(smem + cv.off_nrow);
     m.stage = smem + cv.off_stage;
-    m.cache = reinterpret_cast<uint64_t *>(smem + cv.off_cache);
-    m.wnode = reinterpret_cast<uint32_t *>(smem + cv.off_work);
-    m.wrow = m.wnode + HW_WORK;
-    m.wdst = m.wrow + HW_WORK;
-    m.sadj = reinterpret_cast<uint32_t *>(smem + cv.off_sadj);
     m.EFP = cv.EFP; m.stage_pitch = cv.stage_pitch; m.stage_rows = cv.stage_rows;
     return m;
 }
@@ -791,6 +589,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarv
 #pragma unroll
     for (int i = 0; i < HW_PROF_SLOTS; ++i) st.prof[i] = 0;
     uint32_t entry = a.g.entry, out_total = 0;
+    const bool pool = (a.flags & CDB_HNSW_F_POOL) != 0;
     __syncwarp();
 
     // ann_search (vector_store.rs:256-402): fresh fixed set and ef budget per level, results of all levels
@@ -799,7 +598,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarv
         const uint32_t nb = level == 0 ? a.g.nbrs0 : a.g.nbrs;
         const uint32_t take = min(min(a.shortlist, nb), HN_MAX_TAKE);
         const uint32_t *node_row = ((a.g.identity_mask >> level) & 1u) ? nullptr : a.g.node_row[level];
-        hw_traverse_level<FAST, PROF, false>(node_row, a.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, a.ef, entry, st, lane, a.flags);
+        hw_traverse_level<FAST, PROF, false>(node_row, a.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, a.ef, entry, st, lane, pool);
         if (st.err) break;
         const uint32_t keep = min(st.rlen, HW_FINAL_LEN);
         for (uint32_t i = lane; i < keep; i += 32) {
@@ -829,9 +628,6 @@ static int hw_fast_kind(int st, int metric) {   // 1: f16 chain, 2: bf16 chain, 
     if (metric != CDB_METRIC_COSINE && metric != CDB_METRIC_DOT_PRODUCT) return 0;
     return st == CDB_ST_F16 ? 1 : (st == CDB_ST_BF16 ? 2 : 0);
 }
-size_t hnsw_warp_smem(uint32_t row_pitch, uint32_t dim, uint32_t ef, int st, int metric) {
-    return hw_carve(row_pitch, dim, ef, hw_fast_kind(st, metric) != 0, true).total;
-}
 
 template <int FAST, bool PROF>
 static cdb_status launch_warp(const HnswArgs &a, const HwCarve &cv, cudaStream_t s) {
@@ -846,8 +642,7 @@ cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s) {
     if (!a.nq) return CDB_OK;
     if (a.ef == 0 || a.ef > 4096) { set_error("hnsw: ef_search must be in 1..4096"); return CDB_INVALID_PARAMS; }
     const int fast = hw_fast_kind(a.st, a.metric);
-    const bool spec = (a.flags & CDB_HNSW_F_SPEC) != 0 && (a.flags & CDB_HNSW_F_POOL) == 0;
-    const HwCarve cv = hw_carve(a.row_pitch, a.dim, a.ef, fast != 0, spec);
+    const HwCarve cv = hw_carve(a.row_pitch, a.ef);
     if (cv.total > 200 * 1024) { set_error("hnsw: ef_search / row size too large for shared memory"); return CDB_INVALID_PARAMS; }
     const bool prof = a.prof != nullptr;
     if (fast == 1) return prof ? launch_warp<1, true>(a, cv, s) : launch_warp<1, false>(a, cv, s);
@@ -860,8 +655,10 @@ cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s) {
 // mismatches (cosine -1.0, vector_store.rs:294-303) are merged into the level's best-100 list z.  A level that ends empty
 // scores its entry against every filter and keeps the strongest (vector_store.rs:329-380).  out_rows is CDB_INVALID_ID for
 // pseudo nodes, out_ids the replica ids (hnsw_dedup_md_kernel and the re-rank take them unchanged).
+// (32, 7): shared memory keeps 7 queries per SM at D = 768.  Stating that minimum lets ptxas hold the kernel's per-level state
+// in registers; without it ptxas spilled that state around the chains' division calls.
 template <int FAST>
-__global__ void __launch_bounds__(32) hnsw_search_warp_md_kernel(HnswMdArgs a, HwCarve cv) {
+__global__ void __launch_bounds__(32, 7) hnsw_search_warp_md_kernel(HnswMdArgs a, HwCarve cv) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int lane = threadIdx.x;
     const uint32_t qi = blockIdx.x;
@@ -914,7 +711,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_md_kernel(HnswMdArgs a, H
             for (uint32_t f = qv[0]; f < qv[1]; ++f) {
                 md.q_mag = load_filter(f); md.q_bits = qbits; md.keep_fs = f > qv[0];
                 hw_traverse_level<FAST, false, true>(node_row, g.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, g.ef, entry, st,
-                                                     lane, g.flags, &md);
+                                                     lane, false, &md);
                 if (st.err) break;
                 const uint32_t keep = min(st.rlen, HW_FINAL_LEN);
                 for (uint32_t i0 = 0; i0 < keep; i0 += 32) {   // append in rank order; z is sorted below
@@ -933,7 +730,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_md_kernel(HnswMdArgs a, H
             }
         } else {
             hw_traverse_level<FAST, false, true>(node_row, g.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, g.ef, entry, st, lane,
-                                                 g.flags, &md);
+                                                 false, &md);
             if (!st.err) {
                 zn = min(st.rlen, HW_FINAL_LEN);
                 for (uint32_t i = lane; i < zn; i += 32) { zkeys[i] = m.rkeys[i]; znodes[i] = m.rnodes[i]; }
@@ -982,9 +779,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_md_kernel(HnswMdArgs a, H
     }
 }
 
-size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t dim, uint32_t ef, int st, int metric, uint32_t M) {
-    return hw_carve(row_pitch, dim, ef, hw_fast_kind(st, metric) != 0, false, true, M).total;
-}
+size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t ef, uint32_t M) { return hw_carve(row_pitch, ef, true, M).total; }
 
 template <int FAST>
 static cdb_status launch_warp_md(const HnswMdArgs &a, const HwCarve &cv, cudaStream_t s) {
@@ -998,7 +793,7 @@ static cdb_status launch_warp_md(const HnswMdArgs &a, const HwCarve &cv, cudaStr
 // the caller (hnsw_search_md_device) has checked the shape against both carves
 cdb_status hnsw_search_warp_md_device(const HnswMdArgs &a, cudaStream_t s) {
     const int fast = hw_fast_kind(a.a.st, a.a.metric);
-    const HwCarve cv = hw_carve(a.a.row_pitch, a.a.dim, a.a.ef, fast != 0, false, true, a.M);
+    const HwCarve cv = hw_carve(a.a.row_pitch, a.a.ef, true, a.M);
     if (fast == 1) return launch_warp_md<1>(a, cv, s);
     if (fast == 2) return launch_warp_md<2>(a, cv, s);
     return launch_warp_md<0>(a, cv, s);

@@ -139,19 +139,11 @@ struct HnswArgs {
     uint32_t *err32;
     unsigned long long *counters;
     unsigned long long *prof;         // null, or clock64 sums (hnsw_warp.cu)
-    uint32_t flags;                   // CDB_HNSW_F_* variant switches of the warp kernel
+    uint32_t flags;                   // CDB_HNSW_F_* measurement switches (cdb_debug_set_hnsw_flags); other bits are ignored
 };
-// variant switches of hnsw_search_warp_kernel (cdb_debug_set_hnsw_flags; the default is the best measured combination).
-// The metadata form (hnsw_search_warp_md_kernel) takes PRELOAD / ATOMFS and CTA (-> hnsw_search_md_kernel); it always runs
-// the sorted-queue, non-speculative form, whatever SPEC / POOL say.
-constexpr uint32_t CDB_HNSW_F_PRELOAD = 2;   // load the next head's adjacency slots while the queue merge runs
-constexpr uint32_t CDB_HNSW_F_ATOMFS = 4;    // fixed-set walk through atomicOr return values (slot-order loop only on aliasing)
-constexpr uint32_t CDB_HNSW_F_CTA = 8;       // round-1 kernel: one CTA per query
-constexpr uint32_t CDB_HNSW_F_SPEC = 32;     // idle lanes of a chain phase score the next heads' neighbours ahead of time (hnsw_warp.cu)
-constexpr uint32_t CDB_HNSW_F_POOL = 16;     // candidates as an unsorted pool + arg-max pops instead of a sorted queue + merges
-constexpr uint32_t CDB_HNSW_F_DEFAULT = CDB_HNSW_F_PRELOAD | CDB_HNSW_F_ATOMFS;
+constexpr uint32_t CDB_HNSW_F_CTA = 8;       // graphs with metadata: the CTA-per-query kernel hnsw_search_md_kernel
+constexpr uint32_t CDB_HNSW_F_POOL = 16;     // plain graphs: candidates as an unsorted pool + arg-max pops instead of a sorted queue + merges
 extern std::atomic<uint32_t> g_hnsw_flags;
-cdb_status hnsw_search_device(const HnswArgs &a, cudaStream_t s);        // one CTA per query (round-1 kernel; A/B runs)
 cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s);   // one warp per query (hnsw_warp.cu)
 cdb_status hnsw_dedup_device(const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n, uint32_t in_cap, int metric,
                              uint32_t root_row, uint32_t id_base, uint32_t k5, uint32_t nq, uint32_t *d_cand, uint32_t *d_cand_cnt,
@@ -174,7 +166,7 @@ struct HnswMdArgs {
 };
 // the warp-per-query form (hnsw_warp.cu) unless a.a.flags has CDB_HNSW_F_CTA or its shared memory does not fit
 cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s);
-size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t dim, uint32_t ef, int st, int metric, uint32_t M);
+size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t ef, uint32_t M);
 cdb_status hnsw_search_warp_md_device(const HnswMdArgs &a, cudaStream_t s);
 cdb_status hnsw_dedup_md_device(const uint32_t *d_ids, const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n,
                                 uint32_t in_cap, int metric, uint32_t id_base, uint32_t k5, uint32_t nq, uint32_t *d_cand,

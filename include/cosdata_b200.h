@@ -624,9 +624,8 @@ cdb_status cdb_merge_topk_device(int32_t device, int32_t metric, const uint32_t 
                                  uint32_t *d_out_ids, float *d_out_scores, void *stream);
 
 /* per-phase clock64 sums of the HNSW search kernel (lane 0 of every query, summed over the queries of all searches since
- * profiling was enabled): out[0..12) = {pop + adjacency loads, fixed-set walk + compaction, issue of the row copies, wait for
- * the rows, distance chains, queue merge, end-of-level result sort, whole levels, pops, score-cache look-ups + choice of
- * speculative rows, chain phases, speculative evaluations} (the last three only with CDB_HNSW_F_SPEC); the remaining slots are 0.
+ * profiling was enabled): out[0..9) = {pop + adjacency loads, fixed-set walk + compaction, issue of the row copies, wait for
+ * the rows, distance chains, queue merge, end-of-level result sort, whole levels, pops}; the remaining slots are 0.
  * enable != 0 zeroes the sums and switches the instrumented kernel variant on; 0 switches it off.  out (may be NULL,
  * CDB_HNSW_PROF_SLOTS entries) receives the sums accumulated so far.  Synchronizes the device. */
 #define CDB_HNSW_PROF_SLOTS 16
@@ -636,11 +635,9 @@ cdb_status cdb_index_hnsw_profile(cdb_index *index, int32_t enable, uint64_t *ou
  * TOP/s resp. TFLOP/s: the measured roofline denominator of the integer tensor path (MEASURED_PEAKS.json only has bf16).
  * iters = 0 -> default length (~10 ms). */
 cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters, double *out_tops, float *out_ms);
-/* measurement switch: kernel variant of CDB_MODE_HNSW searches (results are identical for every value).  Bits: 1 cooperative
- * f16 conversion, 2 next-head adjacency preload, 4 fixed-set walk through atomics, 8 round-1 CTA-per-query kernel (on graphs
- * with metadata: the CTA-per-query metadata kernel), 16 unsorted candidate pool, 32 speculative scoring; 0xFFFFFFFF restores
- * the default.  On graphs with metadata 2 and 4 apply as on plain graphs, while 16 and 32 are ignored: the metadata search
- * always runs the sorted-queue, non-speculative form.  Process-wide. */
+/* measurement switch: kernel variant of CDB_MODE_HNSW searches (results are identical for every value).  Bits: 8 the
+ * CTA-per-query kernel on graphs with metadata, 16 an unsorted candidate pool with arg-max pops on plain graphs; every other
+ * bit is accepted and ignored.  0xFFFFFFFF restores the default.  Process-wide. */
 cdb_status cdb_debug_set_hnsw_flags(uint32_t flags);
 
 /* ----------------------------------------------------- instrumentation

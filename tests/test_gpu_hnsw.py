@@ -63,23 +63,32 @@ def test_hnsw_search_matches_oracle(st, metric, ef):
 @pytest.mark.parametrize("st,ef,nb0", [(ST.HalfPrecisionFP, 128, 32), (ST.HalfPrecisionFP, 300, 64), (ST.UnsignedByte, 40, 32),
                                        (ST.BFloat16, 64, 64)])
 def test_hnsw_kernel_variants_walk_the_same_path(flags, name, st, ef, nb0):
-    # every variant of the search kernel (cdb_debug_set_hnsw_flags) must pop the same nodes in the same order as the oracle
+    # the search kernel must pop the same nodes in the same order as the oracle (ef 300: the long-queue merge; nb0 64: the
+    # second slot per lane), and every value cdb_debug_set_hnsw_flags accepts must give the default's arrays and counters:
+    # bit 16 selects the unsorted candidate pool, the other bits of these values select nothing on a plain graph
     n, dim, k = 3000, 40, 10
     vecs = clustered(n, dim, 21)
     fg, ix = build_both(vecs, st, MK.Cosine, levels=4, nb=16, nb0=nb0, efc=48, seed=3)
     rng = np.random.default_rng(22)
     queries = (vecs[rng.integers(0, n, 70)] + 0.05 * rng.normal(size=(70, dim))).astype(np.float32)
     want = pyhnsw.search_batch(fg, vecs, queries, k, ef_search=ef)
-    try:
-        cdb.debug_set_hnsw_flags(flags)
-        ev0, pp0 = ix.hnsw_counters()
-        ids, scores, counts, err = ix.batch_search(queries, k, cdb.SearchMode.HNSW, ef_search=ef, shortlist_size=64)
-        ev1, pp1 = ix.hnsw_counters()
-    finally:
-        cdb.debug_set_hnsw_flags()
-    assert np.array_equal(ids, want[0]) and np.array_equal(bits(scores), bits(want[1])), name
+
+    def search(fl):
+        try:
+            cdb.debug_set_hnsw_flags(fl)
+            ev0, pp0 = ix.hnsw_counters()
+            ids, scores, counts, err = ix.batch_search(queries, k, cdb.SearchMode.HNSW, ef_search=ef, shortlist_size=64)
+            ev1, pp1 = ix.hnsw_counters()
+        finally:
+            cdb.debug_set_hnsw_flags()
+        return ids, bits(scores), counts, err, np.array([ev1 - ev0, pp1 - pp0])
+
+    ids, scores, counts, err, evpp = search(0xFFFFFFFF)
+    assert np.array_equal(ids, want[0]) and np.array_equal(scores, bits(want[1]))
     assert np.array_equal(counts, want[2]) and np.array_equal(err, want[3])
-    assert (ev1 - ev0, pp1 - pp0) == (want[4], want[5]), name
+    assert tuple(evpp) == (want[4], want[5])
+    for got, default in zip(search(flags), (ids, scores, counts, err, evpp)):
+        assert np.array_equal(got, default), name
     ix.close()
 
 
@@ -100,12 +109,12 @@ def test_hnsw_default_params_recall_and_shortlist():
     ix.close()
 
 
-@pytest.mark.parametrize("flags", [None, 38])
+@pytest.mark.parametrize("flags", [None, 38, 22])
 def test_hnsw_zero_norm_row_fails_the_query_like_the_reference(flags):
     # a row whose norm is 0 is a CalculationError the moment a traversal scores it (cosine.rs:230-231): exactly the queries that
     # reach it fail.  The graph is built over normal vectors (an insert that errors is not indexed at all), then the stored vector
-    # of one well-connected node is replaced by zeros.  flags 38 = speculative scoring: a zero-norm row scored ahead of time must
-    # fail only the queries whose own traversal commits it.
+    # of one well-connected node is replaced by zeros.  flags 38: a value that once selected speculative scoring, still accepted
+    # and now running the default form; flags 22 = the unsorted candidate pool.
     n, dim, k = 1500, 32, 5
     vecs = clustered(n, dim, 3)
     st, metric = ST.HalfPrecisionFP, MK.Cosine

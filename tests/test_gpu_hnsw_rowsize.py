@@ -2,7 +2,7 @@
 longer fit one staging group.
 
 Both traversal kernels score a pop's accepted neighbours in groups of staged rows: the CTA traversal (hn_traverse_level, used
-by the build, the insert, the delete's phase A, the filtered search and the CTA search) stages rows with cp.async through one
+by the build, the insert, the delete's phase A and the CTA form of the filtered search) stages rows with cp.async through one
 buffer reused across __syncthreads, the warp search (hnsw_warp.cu) with TMA bulk copies completing on an mbarrier, one phase
 per group.  At D <= 64 every pop fits one group; at D = 768 a group holds about a dozen rows, so with 64 level-0 neighbours a
 pop runs several groups and the first Err may sit in a later one.  D = 769 reaches the scalar tail of the f16 dot chain.
@@ -23,8 +23,7 @@ pytestmark = pytest.mark.gpu
 ST, MK = cdb.StorageType, cdb.DistanceMetricKind
 EMPTY = 0xFFFFFFFF
 LEVELS, NB, NB0, SHORTLIST = 4, 16, 64, 64
-FLAGS = [(None, "default"), (0, "plain"), (2, "preload"), (4, "atomic fixed set"), (22, "pool + arg-max pops"),
-         (32, "speculative, plain"), (38, "speculative scoring"), (8, "cta per query")]
+FLAGS = [(None, "default"), (22, "pool + arg-max pops")]
 
 
 # ----------------------------------------------------------------------------- staged rows per group, restated
@@ -48,8 +47,8 @@ def cta_stage_rows(pitch):   # hn_stage_rows: 18 KB, at most HN_MAX_TAKE = 64
     return min(64, max(1, 18 * 1024 // stage_pitch(pitch)))
 
 
-def warp_stage_rows(pitch, spec=False):   # hw_carve: 18700 B (20200 B speculative), at most one row per lane
-    return min(32, max(1, (20200 if spec else 18700) // stage_pitch(pitch)))
+def warp_stage_rows(pitch):   # hw_carve: 18700 B, at most one row per lane
+    return min(32, max(1, 18700 // stage_pitch(pitch)))
 
 
 def hn_smem_bytes(pitch, ef):   # hnsw_traverse.cuh: the traversal's dynamic shared memory
@@ -58,19 +57,19 @@ def hn_smem_bytes(pitch, ef):   # hnsw_traverse.cuh: the traversal's dynamic sha
     return round16(base) + cta_stage_rows(pitch) * stage_pitch(pitch)
 
 
-# (storage, metric, D) -> (CTA, warp, warp speculative) rows per group
+# (storage, metric, D) -> (CTA, warp) rows per group
 SHAPES = {
-    (ST.HalfPrecisionFP, MK.Cosine, 768): (11, 12, 13),
-    (ST.HalfPrecisionFP, MK.DotProduct, 768): (11, 12, 13),
-    (ST.BFloat16, MK.Cosine, 768): (11, 12, 13),
-    (ST.HalfPrecisionFP, MK.Cosine, 769): (11, 11, 12),
-    (ST.HalfPrecisionFP, MK.Cosine, 1000): (9, 9, 10),
-    (ST.FullPrecisionFP, MK.Cosine, 768): (5, 6, 6),
-    (ST.UnsignedByte, MK.Cosine, 768): (23, 23, 25),
-    (ST.SubByte3, MK.Cosine, 1000): (46, 32, 32),
-    (ST.SubByte2, MK.Cosine, 4096): (17, 17, 19),
-    (ST.SubByte2, MK.DotProduct, 4096): (17, 17, 19),
-    (ST.FullPrecisionFP, MK.Cosine, 4096): (1, 1, 1),
+    (ST.HalfPrecisionFP, MK.Cosine, 768): (11, 12),
+    (ST.HalfPrecisionFP, MK.DotProduct, 768): (11, 12),
+    (ST.BFloat16, MK.Cosine, 768): (11, 12),
+    (ST.HalfPrecisionFP, MK.Cosine, 769): (11, 11),
+    (ST.HalfPrecisionFP, MK.Cosine, 1000): (9, 9),
+    (ST.FullPrecisionFP, MK.Cosine, 768): (5, 6),
+    (ST.UnsignedByte, MK.Cosine, 768): (23, 23),
+    (ST.SubByte3, MK.Cosine, 1000): (46, 32),
+    (ST.SubByte2, MK.Cosine, 4096): (17, 17),
+    (ST.SubByte2, MK.DotProduct, 4096): (17, 17),
+    (ST.FullPrecisionFP, MK.Cosine, 4096): (1, 1),
 }
 
 
@@ -153,7 +152,7 @@ def nodes_over(adj0, rows):
 @pytest.mark.parametrize("st,metric,dim", list(SHAPES), ids=[f"{s.name}-{m.name}-{d}" for s, m, d in SHAPES])
 def test_search_variants_at_production_row_sizes(st, metric, dim):
     pitch = row_pitch(st, dim)
-    groups = (cta_stage_rows(pitch), warp_stage_rows(pitch), warp_stage_rows(pitch, spec=True))
+    groups = (cta_stage_rows(pitch), warp_stage_rows(pitch))
     assert groups == SHAPES[(st, metric, dim)]
     assert max(groups) < NB0                       # a pop can score more neighbours than one group holds
     vecs, root, fg = oracle_graph(st, metric, dim)
@@ -192,13 +191,13 @@ def test_zero_norm_hub_fails_the_queries_that_reach_it(st, dim):
     k, ef = 5, 8
     want = pyhnsw.search_batch(fz, stored, queries, k, ef_search=ef)
     assert 0 < (want[3] != 0).sum() < len(queries)                      # some traversals reach the zero row, others do not
-    for flags, name in [(None, "default"), (38, "speculative scoring"), (8, "cta per query")]:
+    for flags, name in FLAGS:
         ids, scores, counts, err, _, _ = gpu_search(ix, queries, k, ef, flags)
         assert np.array_equal(err, want[3]) and np.array_equal(counts, want[2]), name
         assert np.array_equal(ids, want[0]) and np.array_equal(bits(scores), bits(want[1])), name
     ok = np.flatnonzero(want[3] == 0)                                   # error-free traversals: node for node
     w_ok = pyhnsw.search_batch(fz, stored, queries[ok], k, ef_search=ef)
-    for flags, name in [(None, "default"), (38, "speculative scoring"), (8, "cta per query")]:
+    for flags, name in FLAGS:
         assert_search_equal(gpu_search(ix, queries[ok], k, ef, flags), w_ok, name)
     ix.close()
 
@@ -392,21 +391,14 @@ def test_build_insert_and_search_refuse_shapes_over_the_shared_memory_limit():
         assert np.array_equal(g1["node_row"][lv], g["node_row"][lv]) and np.array_equal(g1["adj"][lv], g["adj"][lv]), lv
         assert np.array_equal(g1["child"][lv], g["child"][lv]) and np.array_equal(bits(sc1[lv]), bits(sc[lv])), lv
     assert g1["entry"] == g["entry"] and len(ix) == n + 21
-    # search: ef_search 4096 is refused by both kernels, ef_search 64 equals the oracle on the built graph
+    # search: ef_search 4096 is refused, ef_search 64 equals the oracle on the built graph
     queries = near(vecs[:n], 16, 4)
-    for flags in (None, 8):
-        try:
-            if flags is not None:
-                cdb.debug_set_hnsw_flags(flags)
-            with pytest.raises(cdb.CosdataError) as e:
-                ix.batch_search(queries, 5, cdb.SearchMode.HNSW, ef_search=4096, shortlist_size=SHORTLIST)
-        finally:
-            cdb.debug_set_hnsw_flags()
-        assert e.value.status == cdb.Status.INVALID_PARAMS, flags
+    with pytest.raises(cdb.CosdataError) as e:
+        ix.batch_search(queries, 5, cdb.SearchMode.HNSW, ef_search=4096, shortlist_size=SHORTLIST)
+    assert e.value.status == cdb.Status.INVALID_PARAMS
     fg = pyhnsw.FlatGraph(int(metric), int(st), dim, codes, mags, n, LEVELS, NB, NB0, g["entry"], g["node_row"], g["adj"], g["child"])
     want = pyhnsw.search_batch(fg, vecs[:n], queries, 5, ef_search=64)
-    for flags, name in [(None, "default"), (8, "cta per query")]:
-        assert_search_equal(gpu_search(ix, queries, 5, 64, flags), want, name)
+    assert_search_equal(gpu_search(ix, queries, 5, 64, None), want, "default")
     ix.close()
 
 
