@@ -93,7 +93,7 @@ def device_count():
 
 def debug_set_hnsw_flags(flags=0xFFFFFFFF):
     """kernel-variant switch of CDB_MODE_HNSW searches (measurement only; results are identical): 8 = the CTA-per-query
-    kernel on graphs with metadata, 16 = the unsorted candidate pool on plain graphs, other bits ignored; default restores"""
+    kernel on graphs with metadata, other bits ignored; default restores"""
     _check(_lib.load().cdb_debug_set_hnsw_flags(flags & 0xFFFFFFFF))
 
 
@@ -499,7 +499,8 @@ class DenseIndex:
         _check(self._lib.cdb_index_hnsw_profile(self._h, 1 if enable else 0, _ptr(out)))
         if out is None:
             return None
-        names = ["adjacency", "fixed_set", "stage_issue", "stage_wait", "chains", "merge", "level_sort", "levels_total", "pops"]
+        names = ["adjacency", "fixed_set", "stage_issue", "stage_wait", "chains", "queue", "level_sort", "levels_total", "pops",
+                 "trims", "exact_selections"]
         return {n: int(v) for n, v in zip(names, out)}
 
     def stats(self):

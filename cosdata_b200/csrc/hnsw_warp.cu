@@ -9,7 +9,7 @@
 // at 9 block barriers per pop while one warp ran the chains (ncu: 63 % of warp samples parked at the barrier, 0.27 IPC on
 // the scoring warp).  Here the 32 lanes of one warp ARE the neighbour slots (two slots per lane cover the <= 64 slots a
 // pop examines), every hand-over is a __syncwarp / ballot / match, and the SM's four schedulers each see ~2 independent
-// queries whose chains interleave.  Queue, results, fixed set and the staged neighbour rows live in the warp's slice of
+// queries whose chains interleave.  Candidates, results, fixed set and the staged neighbour rows live in the warp's slice of
 // shared memory (~24 KB at ef = 128, f16 x 768), so 7-9 queries are resident per SM -- all 1024 queries of a batch at once.
 //
 // Parity.  Pop order, fixed-set walk (slot order, aliasing ids included), first-Err rule, the (score, id) key and the
@@ -30,9 +30,9 @@ constexpr uint32_t HW_FINAL_LEN = 100;          // vector_store.rs:1194
 // staged neighbour rows per group, sized so that 7 warps (queries) per SM still fit in shared memory at D = 768:
 constexpr uint32_t HW_STAGE_BYTES = 18700;      // 12 rows of f16 x 768, 6 of f32 x 768
 // clock64 sums per query (lane 0): [0] pop + adjacency (+ node_row) loads, [1] fixed-set walk + compaction + prefetches,
-// [2] issue of the row copies, [3] wait for the rows, [4] distance chains, [5] queue merge, [6] end-of-level result sort,
-// [7] whole levels, [8] pops
-constexpr int HW_PROF_SLOTS = 9;
+// [2] issue of the row copies, [3] wait for the rows, [4] distance chains, [5] pool update (append, head, trim),
+// [6] end-of-level result sort, [7] whole levels, [8] pops; counts: [9] pool trims, [10] of them by exact selection
+constexpr int HW_PROF_SLOTS = 11;
 
 constexpr uint32_t HW_MD_Z = 256;   // metadata form: a level's merged list z (<= 100) + one traversal's results (<= 100)
 
@@ -237,17 +237,14 @@ __device__ __forceinline__ uint32_t hw_score_group(const HnScoreCtx &sc, const H
 
 // One level (traverse_find_nearest).  All 32 lanes call it with warp-uniform arguments.  On return (st.err == 0)
 // rkeys/rnodes[0..st.rlen) hold every popped entry sorted best first.
-// pool_form: the candidates are an unsorted pool instead of the sorted queue (CDB_HNSW_F_POOL; ignored by the metadata form).
 // MD (metadata form, md != null): the fixed set and the keys use the replica ids md->node_id, pairs are scored through the
 // metadata arms, md->keep_fs keeps the fixed set of the previous traversal of the level.
 template <int FAST, bool PROF, bool MD>
 __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null: identity */, const uint32_t *__restrict__ adj,
                                   uint32_t nb, uint32_t take, const HnScoreCtx &sc, const HwSmem &m, float qmag, uint32_t self_id,
-                                  uint32_t ef, uint32_t entry, HwState &st, int lane, bool pool_form, const HnMdCtx *md = nullptr) {
-    const bool pool = !MD && pool_form;
+                                  uint32_t ef, uint32_t entry, HwState &st, int lane, const HnMdCtx *md = nullptr) {
     const uint32_t pp = plane_pitch(sc.dim);
-    const uint32_t EFP = m.EFP;
-    const uint32_t CAPQ = 2 * EFP;      // pool form: both queue buffers are one unsorted pool
+    const uint32_t CAPQ = 2 * m.EFP;    // entries the candidate pool qkeys / qnodes holds
     const uint32_t bmask = nb - 1u;
     const uint32_t lt = (1u << lane) - 1u;
     long long t0 = 0;
@@ -266,30 +263,25 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
             const uint32_t b0 = (((self_id >> 6) & bmask) << 6) | (self_id & 0x3f), b1 = (((eid >> 6) & bmask) << 6) | (eid & 0x3f);
             m.fs[b0 >> 5] |= 1u << (b0 & 31);
             m.fs[b1 >> 5] |= 1u << (b1 & 31);
-            m.qkeys[0] = m.nkeys[0];
-            m.qnodes[0] = entry;
         }
         __syncwarp();
     }
-    uint32_t qlen = 1, cur = 0, visited = 0, rlen = 0;
-    // adjacency slots of the head, loaded one pop ahead (while the previous pop's queue merge runs)
-    uint32_t pre_node = HN_EMPTY, pre_nbl[2] = {HN_EMPTY, HN_EMPTY};
-    // POOL form: the candidates are an UNSORTED pool in shared memory and the head is found by an arg-max (8 slots per lane,
-    // two 32-bit REDUX) instead of keeping a sorted queue that every pop has to merge into.  The pop order is the same: the
-    // head is the best entry present, and an entry is only ever dropped when at least (pops still to come) better entries
-    // exist, so it could never have been popped.
-    uint64_t hkey = pool ? m.qkeys[0] : 0ull;
+    // The candidates other than the head are an UNSORTED pool in shared memory (qkeys / qnodes [0..qlen)), and each pop finds
+    // the next head by an arg-max (8 slots per lane, two 32-bit REDUX).  The pop order is the reference heap's: the head is
+    // the best entry present, and an entry is only ever dropped when at least (pops still to come) better entries exist, so
+    // it could never have been popped.
+    uint32_t qlen = 0, visited = 0, rlen = 0;
+    uint64_t hkey = m.nkeys[0];
     uint32_t hnode = entry;
     bool have_head = true;
-    if (pool) qlen = 0;
-    while ((pool ? have_head : qlen > 0) && visited < ef) {
-        uint64_t *Q = m.qkeys + cur * EFP;
-        uint32_t *QN = m.qnodes + cur * EFP;
+    // adjacency slots of the head, loaded one pop ahead (while the previous pop tidies up the pool)
+    uint32_t pre_node = HN_EMPTY, pre_nbl[2] = {HN_EMPTY, HN_EMPTY};
+    while (have_head) {   // false once the ef pops are done (R = 0 below) or the pool is empty
         long long t1 = 0, t2 = 0, t3 = 0, t4 = 0;
         if (PROF) t1 = clock64();
         // ---- pop
-        const uint32_t bn = pool ? hnode : QN[0];
-        if (lane == 0) { m.rkeys[rlen] = pool ? hkey : Q[0]; m.rnodes[rlen] = bn; }
+        const uint32_t bn = hnode;
+        if (lane == 0) { m.rkeys[rlen] = hkey; m.rnodes[rlen] = bn; }
         ++rlen;
         st.pops += 1;
         // ---- adjacency: slots lane and lane + 32; ids and fixed-set bit positions
@@ -372,172 +364,82 @@ __device__ void hw_traverse_level(const uint32_t *__restrict__ node_row /* null:
         st.evals += nc;
         if (e != 0xFFFFFFFFu) { st.err = e & 0xFFu; st.rlen = rlen; return; }
         if (PROF) t4 = clock64();
-        if (pool) {
-            uint64_t *P = m.qkeys;
-            uint32_t *PN = m.qnodes;
-            // ---- append the new entries, pick the next head, keep the pool bounded
-            if ((uint32_t)lane < nc) { P[qlen + lane] = m.nkeys[lane]; PN[qlen + lane] = m.nnodes[lane]; }
-            if ((uint32_t)lane + 32u < nc) { P[qlen + lane + 32] = m.nkeys[lane + 32]; PN[qlen + lane + 32] = m.nnodes[lane + 32]; }
-            qlen += nc;
-            ++visited;
-            __syncwarp();
-            const uint32_t R = ef - visited;   // pops still to come
-            have_head = false;
-            pre_node = HN_EMPTY;
-            if (R > 0 && qlen > 0) {
-                uint64_t best = 0ull;
-                uint32_t bidx = 0;
-                for (uint32_t i = lane; i < qlen; i += 32) { const uint64_t k = P[i]; if (k > best) { best = k; bidx = i; } }
-                const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, (uint32_t)(best >> 32));
-                const uint32_t lo = __reduce_max_sync(0xFFFFFFFFu, (uint32_t)(best >> 32) == hi ? (uint32_t)best : 0u);
-                const uint64_t mx = ((uint64_t)hi << 32) | lo;
-                const uint32_t who = __ballot_sync(0xFFFFFFFFu, best == mx);
-                const uint32_t idx = __shfl_sync(0xFFFFFFFFu, bidx, __ffs(who) - 1);
-                hkey = mx;
-                hnode = PN[idx];
-                have_head = true;
-                pre_node = hnode;   // its adjacency slots travel while the pool is tidied up
+        // ---- append the new entries, pick the next head, keep the pool bounded
+        uint64_t *P = m.qkeys;
+        uint32_t *PN = m.qnodes;
+        if ((uint32_t)lane < nc) { P[qlen + lane] = m.nkeys[lane]; PN[qlen + lane] = m.nnodes[lane]; }
+        if ((uint32_t)lane + 32u < nc) { P[qlen + lane + 32] = m.nkeys[lane + 32]; PN[qlen + lane + 32] = m.nnodes[lane + 32]; }
+        qlen += nc;
+        ++visited;
+        __syncwarp();
+        const uint32_t R = ef - visited;   // pops still to come
+        have_head = false;
+        pre_node = HN_EMPTY;
+        if (R > 0 && qlen > 0) {
+            uint64_t best = 0ull;
+            uint32_t bidx = 0;
+            for (uint32_t i = lane; i < qlen; i += 32) { const uint64_t k = P[i]; if (k > best) { best = k; bidx = i; } }
+            const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, (uint32_t)(best >> 32));
+            const uint32_t lo = __reduce_max_sync(0xFFFFFFFFu, (uint32_t)(best >> 32) == hi ? (uint32_t)best : 0u);
+            const uint64_t mx = ((uint64_t)hi << 32) | lo;
+            const uint32_t who = __ballot_sync(0xFFFFFFFFu, best == mx);
+            const uint32_t idx = __shfl_sync(0xFFFFFFFFu, bidx, __ffs(who) - 1);
+            hkey = mx;
+            hnode = PN[idx];
+            have_head = true;
+            pre_node = hnode;   // its adjacency slots travel while the pool is tidied up
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const uint32_t slot = (uint32_t)lane + 32u * h;
-                    pre_nbl[h] = slot < take ? __ldg(adj + (size_t)hnode * nb + slot) : HN_EMPTY;
+            for (int h = 0; h < 2; ++h) {
+                const uint32_t slot = (uint32_t)lane + 32u * h;
+                pre_nbl[h] = slot < take ? __ldg(adj + (size_t)hnode * nb + slot) : HN_EMPTY;
+            }
+            __syncwarp();
+            if (lane == 0 && idx != qlen - 1) { P[idx] = P[qlen - 1]; PN[idx] = PN[qlen - 1]; }   // remove: last entry fills the hole
+            --qlen;
+            __syncwarp();
+            if (qlen + HN_MAX_TAKE > CAPQ) {
+                // the next pop's up to 64 new entries might not fit: drop entries that can never be popped.  T is raised
+                // to pivots that still have >= R better entries; anything <= T is droppable.
+                if (PROF) st.prof[9] += 1;
+                uint64_t T = 0ull;
+                uint32_t kept = qlen;
+                for (uint32_t it = 0; it < 12 && kept + HN_MAX_TAKE + 32 > CAPQ; ++it) {
+                    const uint64_t pivot = P[(visited * 7u + it * 61u) % qlen];
+                    if (pivot <= T) continue;
+                    uint32_t c = 0;
+                    for (uint32_t i = lane; i < qlen; i += 32) c += P[i] > pivot;
+                    c = __reduce_add_sync(0xFFFFFFFFu, c);
+                    if (c >= R) { T = pivot; kept = c; }
                 }
-                __syncwarp();
-                if (lane == 0 && idx != qlen - 1) { P[idx] = P[qlen - 1]; PN[idx] = PN[qlen - 1]; }   // remove: last entry fills the hole
-                --qlen;
-                __syncwarp();
-                if (qlen + HN_MAX_TAKE > CAPQ) {
-                    // the next pop's up to 64 new entries might not fit: drop entries that can never be popped.  T is raised
-                    // to pivots that still have >= R better entries; anything <= T is droppable.
-                    uint64_t T = 0ull;
-                    uint32_t kept = qlen;
-                    for (uint32_t it = 0; it < 12 && kept + HN_MAX_TAKE + 32 > CAPQ; ++it) {
-                        const uint64_t pivot = P[(visited * 7u + it * 61u) % qlen];
-                        if (pivot <= T) continue;
-                        uint32_t c = 0;
-                        for (uint32_t i = lane; i < qlen; i += 32) c += P[i] > pivot;
-                        c = __reduce_add_sync(0xFFFFFFFFu, c);
-                        if (c >= R) { T = pivot; kept = c; }
-                    }
-                    if (kept + HN_MAX_TAKE > CAPQ) {
-                        // unlucky pivots: exact selection of the R best (rank by counting), slow but always sufficient (R <= EFP)
-                        for (uint32_t i0 = 0; i0 < qlen; i0 += 32) {
-                            const uint32_t i = i0 + lane;
-                            const uint64_t k = i < qlen ? P[i] : 0ull;
-                            uint32_t rank = 0;
-                            for (uint32_t j = 0; j < qlen; ++j) rank += P[j] > k;
-                            const uint32_t cand = (i < qlen && rank == R - 1) ? 1u : 0u;   // the R-th best key
-                            const uint32_t b = __ballot_sync(0xFFFFFFFFu, cand);
-                            if (b) { const uint64_t kk = __shfl_sync(0xFFFFFFFFu, k, __ffs(b) - 1); T = kk - 1; }
-                        }
-                        if (qlen < R) T = 0ull;
-                    }
-                    // in-place stream compaction (destinations never overtake the rows still to be read)
-                    uint32_t dst = 0;
+                if (kept + HN_MAX_TAKE > CAPQ) {
+                    // unlucky pivots: exact selection of the R best (rank by counting), slow but always sufficient (R <= EFP)
+                    if (PROF) st.prof[10] += 1;
                     for (uint32_t i0 = 0; i0 < qlen; i0 += 32) {
                         const uint32_t i = i0 + lane;
                         const uint64_t k = i < qlen ? P[i] : 0ull;
-                        const uint32_t nd = i < qlen ? PN[i] : 0u;
-                        const bool keep = i < qlen && k > T;
-                        const uint32_t b = __ballot_sync(0xFFFFFFFFu, keep);
-                        __syncwarp();
-                        if (keep) { const uint32_t d = dst + (uint32_t)__popc(b & lt); P[d] = k; PN[d] = nd; }
-                        dst += (uint32_t)__popc(b);
-                        __syncwarp();
+                        uint32_t rank = 0;
+                        for (uint32_t j = 0; j < qlen; ++j) rank += P[j] > k;
+                        const uint32_t cand = (i < qlen && rank == R - 1) ? 1u : 0u;   // the R-th best key
+                        const uint32_t b = __ballot_sync(0xFFFFFFFFu, cand);
+                        if (b) { const uint64_t kk = __shfl_sync(0xFFFFFFFFu, k, __ffs(b) - 1); T = kk - 1; }
                     }
-                    qlen = dst;
+                    if (qlen < R) T = 0ull;
                 }
+                // in-place stream compaction (destinations never overtake the rows still to be read)
+                uint32_t dst = 0;
+                for (uint32_t i0 = 0; i0 < qlen; i0 += 32) {
+                    const uint32_t i = i0 + lane;
+                    const uint64_t k = i < qlen ? P[i] : 0ull;
+                    const uint32_t nd = i < qlen ? PN[i] : 0u;
+                    const bool keep = i < qlen && k > T;
+                    const uint32_t b = __ballot_sync(0xFFFFFFFFu, keep);
+                    __syncwarp();
+                    if (keep) { const uint32_t d = dst + (uint32_t)__popc(b & lt); P[d] = k; PN[d] = nd; }
+                    dst += (uint32_t)__popc(b);
+                    __syncwarp();
+                }
+                qlen = dst;
             }
-        } else
-        // ---- merge the old queue (minus the popped head) with the new entries, keep what can still be popped.
-        // Final position of an entry = number of entries of the union that are better; no sort of the new entries needed.
-        {
-            const uint32_t oldn = qlen - 1;
-            const uint32_t cap = min(ef - (visited + 1), EFP);
-            uint64_t *D = m.qkeys + (cur ^ 1) * EFP;
-            uint32_t *DN = m.qnodes + (cur ^ 1) * EFP;
-            const uint64_t mynk0 = (uint32_t)lane < nc ? m.nkeys[lane] : 0ull;
-            const uint64_t mynk1 = (uint32_t)lane + 32u < nc ? m.nkeys[lane + 32] : 0ull;
-            // the next head is the better of the runner-up and the best new entry: start loading its adjacency slots now,
-            // the loads complete while the merge below runs
-            pre_node = HN_EMPTY;
-            if (cap > 0 && oldn + nc > 0) {
-                uint64_t best = oldn ? Q[1] : 0ull;
-                uint32_t next = oldn ? QN[1] : HN_EMPTY;
-                if (nc) {
-                    // max of the (unique) 64-bit keys: two 32-bit warp reductions (REDUX) instead of a shuffle tree
-                    const uint64_t loc = mynk0 > mynk1 ? mynk0 : mynk1;
-                    const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, (uint32_t)(loc >> 32));
-                    const uint32_t lo = __reduce_max_sync(0xFFFFFFFFu, (uint32_t)(loc >> 32) == hi ? (uint32_t)loc : 0u);
-                    const uint64_t mx = ((uint64_t)hi << 32) | lo;
-                    if (mx > best) {
-                        const uint32_t who0 = __ballot_sync(0xFFFFFFFFu, mynk0 == mx), who1 = __ballot_sync(0xFFFFFFFFu, mynk1 == mx);
-                        next = m.nnodes[who0 ? (uint32_t)__ffs(who0) - 1u : 32u + (uint32_t)__ffs(who1) - 1u];
-                        best = mx;
-                    }
-                }
-                pre_node = next;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const uint32_t slot = (uint32_t)lane + 32u * h;
-                    pre_nbl[h] = slot < take ? __ldg(adj + (size_t)next * nb + slot) : HN_EMPTY;
-                }
-            }
-            uint32_t r0 = 0, r1 = 0;       // new entries better than my new entries
-            if (oldn <= 128) {
-                // every lane keeps 4 old entries in registers; one pass over the few new keys (broadcast reads) yields, for the
-                // old entries, how far they move down and, through ballots, how many old entries beat each new one
-                uint64_t ok[4];
-                uint32_t lo[4] = {0, 0, 0, 0};
-#pragma unroll
-                for (int t = 0; t < 4; ++t) ok[t] = (uint32_t)lane + 32u * t < oldn ? Q[1 + lane + 32 * t] : 0ull;   // 0 = no entry (never better)
-                uint32_t c0 = 0, c1 = 0;   // old entries better than my new entries (lane j & 31 keeps the count of new entry j)
-                for (uint32_t j = 0; j < nc; ++j) {
-                    const uint64_t nk = m.nkeys[j];
-                    uint32_t cnt = 0;
-#pragma unroll
-                    for (int t = 0; t < 4; ++t) {   // keys are unique and "no entry" is 0: ok[t] > nk  <=>  !(nk > ok[t])
-                        const bool gt = nk > ok[t];
-                        lo[t] += gt;
-                        cnt += 32u - (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, gt));
-                    }
-                    r0 += nk > mynk0;
-                    r1 += nk > mynk1;
-                    if (lane == (int)(j & 31)) { if (j < 32) c0 = cnt; else c1 = cnt; }
-                }
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                    const uint32_t i = (uint32_t)lane + 32u * t;
-                    const uint32_t pos = i + lo[t];
-                    if (i < oldn && pos < cap) { D[pos] = ok[t]; DN[pos] = QN[1 + i]; }
-                }
-                if ((uint32_t)lane < nc && r0 + c0 < cap) { D[r0 + c0] = mynk0; DN[r0 + c0] = m.nnodes[lane]; }
-                if ((uint32_t)lane + 32u < nc && r1 + c1 < cap) { D[r1 + c1] = mynk1; DN[r1 + c1] = m.nnodes[lane + 32]; }
-            } else {
-                // long queues (ef_search > 128): counting for the old entries, binary search in the sorted old queue for the new
-                for (uint32_t i = lane; i < oldn; i += 32) {
-                    const uint64_t k = Q[1 + i];
-                    uint32_t lo = 0;
-                    for (uint32_t j = 0; j < nc; ++j) lo += m.nkeys[j] > k;
-                    const uint32_t pos = i + lo;
-                    if (pos < cap) { D[pos] = k; DN[pos] = QN[1 + i]; }
-                }
-                for (uint32_t j = 0; j < nc; ++j) { const uint64_t nk = m.nkeys[j]; r0 += nk > mynk0; r1 += nk > mynk1; }
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const uint32_t p = (uint32_t)lane + 32u * h;
-                    if (p < nc) {
-                        const uint64_t k = h ? mynk1 : mynk0;
-                        uint32_t lo = 0, hi = oldn;  // number of old entries better than k
-                        while (lo < hi) { const uint32_t md = (lo + hi) >> 1; if (Q[1 + md] > k) lo = md + 1; else hi = md; }
-                        const uint32_t pos = (h ? r1 : r0) + lo;
-                        if (pos < cap) { D[pos] = k; DN[pos] = m.nnodes[p]; }
-                    }
-                }
-            }
-            qlen = min(oldn + nc, cap);
-            cur ^= 1;
-            ++visited;
         }
         __syncwarp();
         if (PROF) {
@@ -589,7 +491,6 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarv
 #pragma unroll
     for (int i = 0; i < HW_PROF_SLOTS; ++i) st.prof[i] = 0;
     uint32_t entry = a.g.entry, out_total = 0;
-    const bool pool = (a.flags & CDB_HNSW_F_POOL) != 0;
     __syncwarp();
 
     // ann_search (vector_store.rs:256-402): fresh fixed set and ef budget per level, results of all levels
@@ -598,7 +499,7 @@ __global__ void __launch_bounds__(32) hnsw_search_warp_kernel(HnswArgs a, HwCarv
         const uint32_t nb = level == 0 ? a.g.nbrs0 : a.g.nbrs;
         const uint32_t take = min(min(a.shortlist, nb), HN_MAX_TAKE);
         const uint32_t *node_row = ((a.g.identity_mask >> level) & 1u) ? nullptr : a.g.node_row[level];
-        hw_traverse_level<FAST, PROF, false>(node_row, a.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, a.ef, entry, st, lane, pool);
+        hw_traverse_level<FAST, PROF, false>(node_row, a.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, a.ef, entry, st, lane);
         if (st.err) break;
         const uint32_t keep = min(st.rlen, HW_FINAL_LEN);
         for (uint32_t i = lane; i < keep; i += 32) {
@@ -711,7 +612,7 @@ __global__ void __launch_bounds__(32, 7) hnsw_search_warp_md_kernel(HnswMdArgs a
             for (uint32_t f = qv[0]; f < qv[1]; ++f) {
                 md.q_mag = load_filter(f); md.q_bits = qbits; md.keep_fs = f > qv[0];
                 hw_traverse_level<FAST, false, true>(node_row, g.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, g.ef, entry, st,
-                                                     lane, false, &md);
+                                                     lane, &md);
                 if (st.err) break;
                 const uint32_t keep = min(st.rlen, HW_FINAL_LEN);
                 for (uint32_t i0 = 0; i0 < keep; i0 += 32) {   // append in rank order; z is sorted below
@@ -730,7 +631,7 @@ __global__ void __launch_bounds__(32, 7) hnsw_search_warp_md_kernel(HnswMdArgs a
             }
         } else {
             hw_traverse_level<FAST, false, true>(node_row, g.g.adj[level], nb, take, sc, m, qmag, HN_QUERY_ID, g.ef, entry, st, lane,
-                                                 false, &md);
+                                                 &md);
             if (!st.err) {
                 zn = min(st.rlen, HW_FINAL_LEN);
                 for (uint32_t i = lane; i < zn; i += 32) { zkeys[i] = m.rkeys[i]; znodes[i] = m.rnodes[i]; }

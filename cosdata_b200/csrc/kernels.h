@@ -142,7 +142,6 @@ struct HnswArgs {
     uint32_t flags;                   // CDB_HNSW_F_* measurement switches (cdb_debug_set_hnsw_flags); other bits are ignored
 };
 constexpr uint32_t CDB_HNSW_F_CTA = 8;       // graphs with metadata: the CTA-per-query kernel hnsw_search_md_kernel
-constexpr uint32_t CDB_HNSW_F_POOL = 16;     // plain graphs: candidates as an unsorted pool + arg-max pops instead of a sorted queue + merges
 extern std::atomic<uint32_t> g_hnsw_flags;
 cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s);   // one warp per query (hnsw_warp.cu)
 cdb_status hnsw_dedup_device(const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n, uint32_t in_cap, int metric,

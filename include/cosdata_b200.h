@@ -625,7 +625,8 @@ cdb_status cdb_merge_topk_device(int32_t device, int32_t metric, const uint32_t 
 
 /* per-phase clock64 sums of the HNSW search kernel (lane 0 of every query, summed over the queries of all searches since
  * profiling was enabled): out[0..9) = {pop + adjacency loads, fixed-set walk + compaction, issue of the row copies, wait for
- * the rows, distance chains, queue merge, end-of-level result sort, whole levels, pops}; the remaining slots are 0.
+ * the rows, distance chains, candidate-pool update (append, next head, trim), end-of-level result sort, whole levels, pops},
+ * then out[9] = pool trims and out[10] = trims that fell back to an exact selection (counts); the remaining slots are 0.
  * enable != 0 zeroes the sums and switches the instrumented kernel variant on; 0 switches it off.  out (may be NULL,
  * CDB_HNSW_PROF_SLOTS entries) receives the sums accumulated so far.  Synchronizes the device. */
 #define CDB_HNSW_PROF_SLOTS 16
@@ -635,9 +636,9 @@ cdb_status cdb_index_hnsw_profile(cdb_index *index, int32_t enable, uint64_t *ou
  * TOP/s resp. TFLOP/s: the measured roofline denominator of the integer tensor path (MEASURED_PEAKS.json only has bf16).
  * iters = 0 -> default length (~10 ms). */
 cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters, double *out_tops, float *out_ms);
-/* measurement switch: kernel variant of CDB_MODE_HNSW searches (results are identical for every value).  Bits: 8 the
- * CTA-per-query kernel on graphs with metadata, 16 an unsorted candidate pool with arg-max pops on plain graphs; every other
- * bit is accepted and ignored.  0xFFFFFFFF restores the default.  Process-wide. */
+/* measurement switch: kernel variant of CDB_MODE_HNSW searches (results are identical for every value).  Bit 8 selects the
+ * CTA-per-query kernel on graphs with metadata; every other bit is accepted and ignored.  0xFFFFFFFF restores the default.
+ * Process-wide. */
 cdb_status cdb_debug_set_hnsw_flags(uint32_t flags);
 
 /* ----------------------------------------------------- instrumentation

@@ -63,9 +63,9 @@ def test_hnsw_search_matches_oracle(st, metric, ef):
 @pytest.mark.parametrize("st,ef,nb0", [(ST.HalfPrecisionFP, 128, 32), (ST.HalfPrecisionFP, 300, 64), (ST.UnsignedByte, 40, 32),
                                        (ST.BFloat16, 64, 64)])
 def test_hnsw_kernel_variants_walk_the_same_path(flags, name, st, ef, nb0):
-    # the search kernel must pop the same nodes in the same order as the oracle (ef 300: the long-queue merge; nb0 64: the
-    # second slot per lane), and every value cdb_debug_set_hnsw_flags accepts must give the default's arrays and counters:
-    # bit 16 selects the unsorted candidate pool, the other bits of these values select nothing on a plain graph
+    # the search kernel must pop the same nodes in the same order as the oracle (ef 300: not a power of two, EFP 512; nb0 64:
+    # the second slot per lane), and every value cdb_debug_set_hnsw_flags accepts must give the default's arrays and counters:
+    # none of these values selects anything on a plain graph
     n, dim, k = 3000, 40, 10
     vecs = clustered(n, dim, 21)
     fg, ix = build_both(vecs, st, MK.Cosine, levels=4, nb=16, nb0=nb0, efc=48, seed=3)
@@ -92,6 +92,31 @@ def test_hnsw_kernel_variants_walk_the_same_path(flags, name, st, ef, nb0):
     ix.close()
 
 
+def test_hnsw_pool_trims_and_exact_selections_walk_the_same_path():
+    # ef = EFP = 128 and 64 level-0 slots over spread-out rows: the first pops bring up to 64 new candidates each, so the pool
+    # (2 * EFP entries) fills while R, the pops still to come, is close to ef.  Then the pool is trimmed, and some trims find
+    # no sampled pivot with between R and 2 * EFP - 64 better entries and fall back to the exact selection.  The pop order
+    # must stay the oracle's, in the plain kernel and in the instrumented one that counts both events.
+    n, dim, k, ef = 5000, 40, 10, 128
+    vecs = np.random.default_rng(21).uniform(-0.9, 0.9, size=(n, dim)).astype(np.float32)
+    fg, ix = build_both(vecs, ST.HalfPrecisionFP, MK.Cosine, levels=4, nb=16, nb0=64, efc=48, seed=3)
+    rng = np.random.default_rng(22)
+    queries = (vecs[rng.integers(0, n, 500)] + 0.05 * rng.normal(size=(500, dim))).astype(np.float32)
+    want = pyhnsw.search_batch(fg, vecs, queries, k, ef_search=ef)
+    for profile in (False, True):
+        if profile:
+            ix.hnsw_profile(enable=True, read=False)
+        ev0, pp0 = ix.hnsw_counters()
+        ids, scores, counts, err = ix.batch_search(queries, k, cdb.SearchMode.HNSW, ef_search=ef, shortlist_size=64)
+        ev1, pp1 = ix.hnsw_counters()
+        assert np.array_equal(ids, want[0]) and np.array_equal(bits(scores), bits(want[1]))
+        assert np.array_equal(counts, want[2]) and np.array_equal(err, want[3])
+        assert (ev1 - ev0, pp1 - pp0) == (want[4], want[5])
+    prof = ix.hnsw_profile(enable=False, read=True)
+    assert prof["trims"] > 0 and prof["exact_selections"] > 0, prof
+    ix.close()
+
+
 def test_hnsw_default_params_recall_and_shortlist():
     # reference defaults (config.toml:19-33): nbrs 32/64, ef_search 256, shortlist 64, 9 layers
     n, dim, k = 4000, 64, 10
@@ -113,8 +138,8 @@ def test_hnsw_default_params_recall_and_shortlist():
 def test_hnsw_zero_norm_row_fails_the_query_like_the_reference(flags):
     # a row whose norm is 0 is a CalculationError the moment a traversal scores it (cosine.rs:230-231): exactly the queries that
     # reach it fail.  The graph is built over normal vectors (an insert that errors is not indexed at all), then the stored vector
-    # of one well-connected node is replaced by zeros.  flags 38: a value that once selected speculative scoring, still accepted
-    # and now running the default form; flags 22 = the unsorted candidate pool.
+    # of one well-connected node is replaced by zeros.  flags 38 and 22: values that once selected speculative scoring and the
+    # unsorted candidate pool, still accepted and now running the default form.
     n, dim, k = 1500, 32, 5
     vecs = clustered(n, dim, 3)
     st, metric = ST.HalfPrecisionFP, MK.Cosine

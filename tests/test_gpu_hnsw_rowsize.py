@@ -23,7 +23,6 @@ pytestmark = pytest.mark.gpu
 ST, MK = cdb.StorageType, cdb.DistanceMetricKind
 EMPTY = 0xFFFFFFFF
 LEVELS, NB, NB0, SHORTLIST = 4, 16, 64, 64
-FLAGS = [(None, "default"), (22, "pool + arg-max pops")]
 
 
 # ----------------------------------------------------------------------------- staged rows per group, restated
@@ -112,15 +111,10 @@ def upload(stored, root, fg, st, metric):
     return ix
 
 
-def gpu_search(ix, queries, k, ef, flags):
-    try:
-        if flags is not None:
-            cdb.debug_set_hnsw_flags(flags)
-        ev0, pp0 = ix.hnsw_counters()
-        ids, scores, counts, err = ix.batch_search(queries, k, cdb.SearchMode.HNSW, ef_search=ef, shortlist_size=SHORTLIST)
-        ev1, pp1 = ix.hnsw_counters()
-    finally:
-        cdb.debug_set_hnsw_flags()
+def gpu_search(ix, queries, k, ef):
+    ev0, pp0 = ix.hnsw_counters()
+    ids, scores, counts, err = ix.batch_search(queries, k, cdb.SearchMode.HNSW, ef_search=ef, shortlist_size=SHORTLIST)
+    ev1, pp1 = ix.hnsw_counters()
     return ids, scores, counts, err, ev1 - ev0, pp1 - pp0
 
 
@@ -167,8 +161,7 @@ def test_search_variants_at_production_row_sizes(st, metric, dim):
     for ef in (64, 300):
         want = pyhnsw.search_batch(fg, vecs, queries, k, ef_search=ef)
         assert (want[3] == 0).all() and (want[2] == k).all()
-        for flags, name in FLAGS:
-            assert_search_equal(gpu_search(ix, queries, k, ef, flags), want, (name, ef))
+        assert_search_equal(gpu_search(ix, queries, k, ef), want, ef)
     ix.close()
 
 
@@ -191,14 +184,12 @@ def test_zero_norm_hub_fails_the_queries_that_reach_it(st, dim):
     k, ef = 5, 8
     want = pyhnsw.search_batch(fz, stored, queries, k, ef_search=ef)
     assert 0 < (want[3] != 0).sum() < len(queries)                      # some traversals reach the zero row, others do not
-    for flags, name in FLAGS:
-        ids, scores, counts, err, _, _ = gpu_search(ix, queries, k, ef, flags)
-        assert np.array_equal(err, want[3]) and np.array_equal(counts, want[2]), name
-        assert np.array_equal(ids, want[0]) and np.array_equal(bits(scores), bits(want[1])), name
+    ids, scores, counts, err, _, _ = gpu_search(ix, queries, k, ef)
+    assert np.array_equal(err, want[3]) and np.array_equal(counts, want[2])
+    assert np.array_equal(ids, want[0]) and np.array_equal(bits(scores), bits(want[1]))
     ok = np.flatnonzero(want[3] == 0)                                   # error-free traversals: node for node
     w_ok = pyhnsw.search_batch(fz, stored, queries[ok], k, ef_search=ef)
-    for flags, name in FLAGS:
-        assert_search_equal(gpu_search(ix, queries[ok], k, ef, flags), w_ok, name)
+    assert_search_equal(gpu_search(ix, queries[ok], k, ef), w_ok, "error-free queries")
     ix.close()
 
 
@@ -329,7 +320,7 @@ def test_batched_build_at_250k_f16_768_search_parity_and_recall():
     g = ix.read_graph()
     codes, mags = ix.read_codes(0, n + 1)
     fg = pyhnsw.FlatGraph(int(metric), int(st), dim, codes, mags, n, LEVELS, NB, NB0, g["entry"], g["node_row"], g["adj"], g["child"])
-    got = gpu_search(ix, queries, k, ef, None)
+    got = gpu_search(ix, queries, k, ef)
     want = pyhnsw.search_batch(fg, vecs, queries, k, ef_search=ef)
     assert_search_equal(got, want, "default flags")
     gt, _, _, _ = ix.batch_search(queries, k, cdb.SearchMode.BRUTE_RAW)   # the exact f32 scan
@@ -398,7 +389,7 @@ def test_build_insert_and_search_refuse_shapes_over_the_shared_memory_limit():
     assert e.value.status == cdb.Status.INVALID_PARAMS
     fg = pyhnsw.FlatGraph(int(metric), int(st), dim, codes, mags, n, LEVELS, NB, NB0, g["entry"], g["node_row"], g["adj"], g["child"])
     want = pyhnsw.search_batch(fg, vecs[:n], queries, 5, ef_search=64)
-    assert_search_equal(gpu_search(ix, queries, 5, 64, None), want, "default")
+    assert_search_equal(gpu_search(ix, queries, 5, 64), want, "default")
     ix.close()
 
 
