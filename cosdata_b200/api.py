@@ -92,8 +92,8 @@ def device_count():
 
 
 def debug_set_hnsw_flags(flags=0xFFFFFFFF):
-    """kernel-variant switch of CDB_MODE_HNSW searches (measurement only; results are identical): 8 = the CTA-per-query
-    kernel on graphs with metadata, other bits ignored; default restores"""
+    """former kernel-variant switch of CDB_MODE_HNSW searches: every value is accepted and selects nothing (HNSW search
+    has one kernel per graph kind)"""
     _check(_lib.load().cdb_debug_set_hnsw_flags(flags & 0xFFFFFFFF))
 
 

@@ -20,7 +20,6 @@ namespace cdb {
 static thread_local std::string t_last_error;
 void set_error(const std::string &msg) { t_last_error = msg; }
 std::atomic<uint64_t> g_launch_count{0};
-std::atomic<uint32_t> g_hnsw_flags{0};
 
 cudaError_t allow_max_dynamic_smem(const void *kernel) {
     static std::mutex mu;
@@ -834,14 +833,12 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
     a.out_n = sc->hn_n.as<uint32_t>();
     a.err32 = sc->err32.as<uint32_t>();
     a.counters = ix->hn_counters.as<unsigned long long>();
-    a.flags = g_hnsw_flags.load();
     const int slot = (int)(ix->n_search.fetch_add(1) % cdb_index::EV_RING);
     CDB_CUDA_TRY(cudaEventRecord(sc->ev[0], s));
     CDB_CUDA_TRY(cudaEventRecord(ix->ring0[slot], s));
     if (ix->has_md) {
-        // graph with replica nodes: metadata-aware traversal (one warp per query, hnsw_warp.cu; CDB_HNSW_F_CTA selects the
-        // CTA-per-query kernel of hnsw_md.cu); results carry replica ids, the re-rank scores the base vector of each replica
-        // (collection.rs:368-384)
+        // graph with replica nodes: metadata-aware traversal (one warp per query, hnsw_warp.cu); results carry replica ids,
+        // the re-rank scores the base vector of each replica (collection.rs:368-384)
         HnswMdArgs ma{};
         ma.a = a;
         ma.node_id = ix->md_node_id;
@@ -857,8 +854,8 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
         ma.out_ids = sc->hn_ids.as<uint32_t>();
         if ((rc = hnsw_search_md_device(ma, s))) return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
-        if ((rc = hnsw_dedup_md_device(ma.out_ids, a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, d.id_base, k5, nq,
-                                       sc->cand.as<uint32_t>(), sc->hn_labels.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), s)))
+        if ((rc = hnsw_dedup_device(ma.out_ids, a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, HN_ROOT_ID, d.id_base, k5, nq,
+                                    sc->cand.as<uint32_t>(), sc->hn_labels.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), s)))
             return rc;
         if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
                                     ix->raw_pitch_elems, sc->qraw_mags.as<float>(), nq, sc->cand.as<uint32_t>(),
@@ -870,8 +867,8 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
         a.prof = ix->hn_prof_on ? ix->hn_prof.as<unsigned long long>() : nullptr;
         if ((rc = hnsw_search_warp_device(a, s))) return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
-        if ((rc = hnsw_dedup_device(a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, ix->graph.root_row, d.id_base, k5, nq,
-                                    sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), s)))
+        if ((rc = hnsw_dedup_device(nullptr, a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, ix->graph.root_row, d.id_base, k5,
+                                    nq, sc->cand.as<uint32_t>(), nullptr, sc->cand_cnt.as<uint32_t>(), s)))
             return rc;
         if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
                                     ix->raw_pitch_elems, sc->qraw_mags.as<float>(), nq, sc->cand.as<uint32_t>(),
@@ -1920,10 +1917,7 @@ cdb_status cdb_index_hnsw_counters(const cdb_index *ix, uint64_t *out2) {
     return CDB_OK;
 }
 
-cdb_status cdb_debug_set_hnsw_flags(uint32_t flags) {
-    g_hnsw_flags.store(flags == 0xFFFFFFFFu ? 0u : flags);
-    return CDB_OK;
-}
+cdb_status cdb_debug_set_hnsw_flags(uint32_t) { return CDB_OK; }
 
 cdb_status cdb_index_hnsw_profile(cdb_index *ix, int32_t enable, uint64_t *out) {
     CDB_REQUIRE(ix, "null index");

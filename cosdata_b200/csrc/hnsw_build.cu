@@ -95,19 +95,23 @@ __device__ inline uint32_t build_local(const BuildLevel &l, uint32_t level, uint
     return lo;
 }
 
-__global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs a) {
+// Phase A: one warp per entry of the batch runs the searches' traversal (hw_traverse_level) from the top level down.
+// FAST = hw_fast_kind of the storage type and metric; MD = replica graph.  The traversal reads adj, node_row and node_id
+// through the read-only cache (__ldg): node_row / node_id are fixed for the whole call, and the adjacency is written only by
+// other launches on the same stream (phase B, the delete's repair and relink kernels), never while this kernel runs.
+template <int FAST, bool MD>
+__global__ void __launch_bounds__(32) hnsw_build_search_kernel(BuildArgs a, HwCarve cv) {
     extern __shared__ __align__(16) uint8_t smem[];
-    const HnSmem m = hn_carve(smem, a.sc.row_pitch, a.ef);
-    __shared__ HnShared sh;
+    const HwSmem m = hw_smem(smem, cv);
     const uint32_t b = blockIdx.x, r = a.rowlist ? a.rowlist[a.first + b] : a.first + b;
-    const int tid = threadIdx.x;
+    const int lane = threadIdx.x;
     const bool del = a.rowlist != nullptr;
-    if (!del && !a.replicas && a.deleted && bit_set(a.deleted, r)) {   // a deleted row is not inserted
-        if (tid == 0) a.failed[b] = 2;
+    if (!del && !MD && a.deleted && bit_set(a.deleted, r)) {   // a deleted row is not inserted
+        if (lane == 0) a.failed[b] = 2;
         return;
     }
-    const uint32_t vrow = a.replicas ? a.rl.row[r] : r;
-    for (uint32_t i = tid; i < a.sc.row_pitch / 4; i += HN_THREADS)
+    const uint32_t vrow = MD ? a.rl.row[r] : r;
+    for (uint32_t i = lane; i < a.sc.row_pitch / 4; i += 32)
         reinterpret_cast<uint32_t *>(m.qs)[i] = reinterpret_cast<const uint32_t *>(a.sc.rows + (size_t)vrow * a.sc.row_pitch)[i];
     const float qmag = a.sc.mags[vrow];
     const uint32_t max_level = del ? a.g.num_levels : a.levels[r - a.lv_first];
@@ -117,7 +121,7 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs
     HnMdCtx md{};
     uint32_t self_id = r;
     bool under_pseudo = false;
-    if (a.replicas) {
+    if (MD) {
         const uint32_t mrow = a.rl.md[r];
         md.md_bits = a.rl.md_bits; md.md_mags = a.rl.md_mags; md.M = a.rl.M;
         md.q_bits = mrow == HN_EMPTY ? nullptr : a.rl.md_bits + (size_t)mrow * a.rl.M;
@@ -126,33 +130,43 @@ __global__ void __launch_bounds__(HN_THREADS) hnsw_build_search_kernel(BuildArgs
         self_id = a.rl.id[r];
         under_pseudo = md.q_bits && md.q_mag != 0.0f;
     }
-    if (tid == 0) { sh.err = 0; sh.entry = under_pseudo ? a.g.pseudo_entry : a.g.entry; }
-    unsigned long long evals = 0, pops = 0;
-    __syncthreads();
+    if (lane == 0) hw_mbar_init(m.bar, 1);
+    HwState st;
+    st.err = 0; st.rlen = 0; st.evals = 0; st.pops = 0; st.bar_phase = 0;
+    uint32_t entry = under_pseudo ? a.g.pseudo_entry : a.g.entry;
+    __syncwarp();
     for (int level = (int)a.g.num_levels; level >= 0; --level) {
         const BuildLevel &l = a.g.lv[level];
         const uint32_t take = min(min(a.shortlist, l.nb), HN_MAX_TAKE);
-        if (a.replicas) { md.node_id = l.node_id; md.node_md = l.node_md; }
-        hn_traverse_level(l.node_row, l.adj, l.nb, take, a.sc, m, sh, qmag, self_id, a.ef, evals, pops, a.replicas ? &md : nullptr,
-                          !del);
-        if (sh.err) {
-            if (del && tid == 0)   // D3: no relinks on this level or below
+        if (MD) { md.node_id = l.node_id; md.node_md = l.node_md; }
+        hw_traverse_level<FAST, false, MD>(l.node_row, l.adj, l.nb, take, a.sc, m, qmag, self_id, !del, a.ef, entry, st, lane,
+                                           MD ? &md : nullptr);
+        if (st.err) {
+            if (del && lane == 0)   // D3: no relinks on this level or below
                 for (int lv = level; lv >= 0; --lv) a.z_n[(size_t)b * L1 + lv] = HN_EMPTY;
             break;
         }
-        const uint32_t keep = min(sh.rlen, a.zcap);  // final_len: 64 while indexing, 100 otherwise (vector_store.rs:1194)
+        const uint32_t keep = min(st.rlen, a.zcap);  // final_len: 64 while indexing, 100 otherwise (vector_store.rs:1194)
         if ((uint32_t)level <= max_level) {
             const size_t base = ((size_t)b * L1 + level) * a.zcap;
-            for (uint32_t i = tid; i < keep; i += HN_THREADS) {
+            for (uint32_t i = lane; i < keep; i += 32) {
                 a.z_nodes[base + i] = m.rnodes[i];
                 a.z_keys[base + i] = (uint32_t)(m.rkeys[i] >> 32);
             }
-            if (tid == 0) a.z_n[(size_t)b * L1 + level] = keep;
+            if (lane == 0) a.z_n[(size_t)b * L1 + level] = keep;
         }
-        if (tid == 0 && level > 0) sh.entry = l.child[m.rnodes[0]];
-        __syncthreads();
+        if (level > 0) entry = l.child[m.rnodes[0]];
+        __syncwarp();
     }
-    if (tid == 0) a.failed[b] = sh.err ? 1 : 0;  // the reference returns Err: the embedding is not indexed
+    if (lane == 0) a.failed[b] = st.err ? 1 : 0;  // the reference returns Err: the embedding is not indexed
+}
+using BuildSearchKernel = void (*)(BuildArgs, HwCarve);
+constexpr BuildSearchKernel BUILD_SEARCH[3][2] = {   // [hw_fast_kind][replica graph]
+    {hnsw_build_search_kernel<0, false>, hnsw_build_search_kernel<0, true>},
+    {hnsw_build_search_kernel<1, false>, hnsw_build_search_kernel<1, true>},
+    {hnsw_build_search_kernel<2, false>, hnsw_build_search_kernel<2, true>}};
+static BuildSearchKernel build_search_kernel(const HnScoreCtx &sc, bool replicas) {
+    return BUILD_SEARCH[hw_fast_kind(sc.st, sc.metric)][replicas ? 1 : 0];
 }
 
 __device__ inline void node_lock(int *lk) {
@@ -515,7 +529,7 @@ static cdb_status publish(const HnswBuildState &st, const GraphHost &gh) {
     CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->node_row, gh.nr->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
     CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->adj, gh.ad->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
     CDB_CUDA_TRY(cudaMemcpy((void *)gh.dev->child, gh.ch->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
-    if (gh.id) {   // replica graphs: the tables the filtered search (hnsw_md.cu) reads
+    if (gh.id) {   // replica graphs: the tables the filtered search (hnsw_warp.cu) reads
         gh.id->assign(L1, nullptr); gh.md->assign(L1, nullptr);
         for (uint32_t L = 0; L < L1; ++L) { (*gh.id)[L] = st.g.lv[L].node_id; (*gh.md)[L] = st.g.lv[L].node_md; }
         CDB_CUDA_TRY(cudaMemcpy((void *)gh.id_tbl, gh.id->data(), L1 * sizeof(void *), cudaMemcpyHostToDevice));
@@ -528,9 +542,7 @@ cdb_status hnsw_build_smem_check(uint32_t row_pitch, uint32_t ef) {
     int dev = 0, optin = 0;
     CDB_CUDA_TRY(cudaGetDevice(&dev));
     CDB_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    cudaFuncAttributes fa;
-    CDB_CUDA_TRY(cudaFuncGetAttributes(&fa, reinterpret_cast<const void *>(hnsw_build_search_kernel)));
-    const size_t need = hn_smem_bytes(row_pitch, ef) + fa.sharedSizeBytes;
+    const size_t need = hw_carve(row_pitch, ef).total;   // hnsw_build_search_kernel declares no static shared memory
     if (need > (size_t)optin) {
         set_error("hnsw build: ef " + std::to_string(ef) + " with " + std::to_string(row_pitch) + "-byte rows needs " +
                   std::to_string(need) + " bytes of shared memory per block, the device allows " + std::to_string(optin));
@@ -631,8 +643,9 @@ static cdb_status insert_planned(const HnScoreCtx &sc, const GraphHost &gh, Hnsw
         (rc = tmp.get((void **)&z_nodes, (size_t)max_batch * L1 * 64 * 4)) || (rc = tmp.get((void **)&z_keys, (size_t)max_batch * L1 * 64 * 4)) ||
         (rc = tmp.get((void **)&z_n, (size_t)max_batch * L1 * 4)))
         return rc;
-    const size_t smem = hn_smem_bytes(sc.row_pitch, ef_construction);
-    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    const HwCarve cv = hw_carve(sc.row_pitch, ef_construction);
+    const BuildSearchKernel search = build_search_kernel(sc, rl != nullptr);
+    CDB_ALLOW_SMEM(search, cv.total);
     if ((rc = append_levels(st, gh, p.rows, p.child, rows_cap, changed, s, rl ? &p.cols : nullptr))) return rc;
     if (!count) return CDB_OK;
     // ---- batches
@@ -656,7 +669,7 @@ static cdb_status insert_planned(const HnScoreCtx &sc, const GraphHost &gh, Hnsw
         a.first = first + done;
         a.count = batch;
         a.failed = failed + done;
-        hnsw_build_search_kernel<<<batch, HN_THREADS, smem, s>>>(a);
+        search<<<batch, 32, cv.total, s>>>(a, cv);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         hnsw_build_link_kernel<<<(batch * 32 + 127) / 128, 128, 0, s>>>(a);
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
@@ -1106,8 +1119,9 @@ static cdb_status delete_items(const HnScoreCtx &sc, HnswBuildState *st, const D
         CDB_CUDA_TRY(cudaMemsetAsync(d.touched[L], 0, (size_t)words * 4, s));
         if (replicas) CDB_CUDA_TRY(cudaMemsetAsync(d.tmin[L], 0xFF, (size_t)cnt * 4, s));
     }
-    const size_t smem = hn_smem_bytes(sc.row_pitch, DEL_EF);
-    CDB_ALLOW_SMEM(hnsw_build_search_kernel, smem);
+    const HwCarve cv = hw_carve(sc.row_pitch, DEL_EF);
+    const BuildSearchKernel search = build_search_kernel(sc, replicas);
+    CDB_ALLOW_SMEM(search, cv.total);
     CDB_ALLOW_SMEM(hnsw_delete_repair_kernel, sc.row_pitch);
     CDB_ALLOW_SMEM(hnsw_delete_relink_kernel, sc.row_pitch);
     CDB_CUDA_TRY(cudaMemsetAsync(d.status, 0, ni, s));
@@ -1152,7 +1166,7 @@ static cdb_status delete_items(const HnScoreCtx &sc, HnswBuildState *st, const D
         a.failed = failed + first;
         d.rfirst = rdone;
         hnsw_delete_mark_kernel<<<(count * L1 + 127) / 128, 128, 0, s>>>(d);
-        hnsw_build_search_kernel<<<count, HN_THREADS, smem, s>>>(a);
+        search<<<count, 32, cv.total, s>>>(a, cv);
         hnsw_delete_repair_kernel<<<rb * L1, 32, sc.row_pitch, s>>>(d);
         g_launch_count.fetch_add(3, std::memory_order_relaxed);
         for (uint32_t L = 0; L < L1; ++L) {

@@ -139,16 +139,16 @@ struct HnswArgs {
     uint32_t *err32;
     unsigned long long *counters;
     unsigned long long *prof;         // null, or clock64 sums (hnsw_warp.cu)
-    uint32_t flags;                   // CDB_HNSW_F_* measurement switches (cdb_debug_set_hnsw_flags); other bits are ignored
 };
-constexpr uint32_t CDB_HNSW_F_CTA = 8;       // graphs with metadata: the CTA-per-query kernel hnsw_search_md_kernel
-extern std::atomic<uint32_t> g_hnsw_flags;
-cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s);   // one warp per query (hnsw_warp.cu)
-cdb_status hnsw_dedup_device(const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n, uint32_t in_cap, int metric,
-                             uint32_t root_row, uint32_t id_base, uint32_t k5, uint32_t nq, uint32_t *d_cand, uint32_t *d_cand_cnt,
-                             cudaStream_t s);
+// remove_duplicates_and_filter: ids of the entries d_ids (replica ids) or, with d_ids == null, their rows; entries with
+// id == drop_id (the root) or row == CDB_INVALID_ID (pseudo nodes) are dropped; d_labels (may be null) receives the kept ids
+cdb_status hnsw_dedup_device(const uint32_t *d_ids, const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n, uint32_t in_cap,
+                             int metric, uint32_t drop_id, uint32_t id_base, uint32_t k5, uint32_t nq, uint32_t *d_cand,
+                             uint32_t *d_labels, uint32_t *d_cand_cnt, cudaStream_t s);
 
-// ---- hnsw_md.cu (metadata-filtered search on graphs with replica nodes)
+// ---- hnsw_warp.cu: HNSW search, one warp per query
+cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s);
+// metadata-filtered search on graphs with replica nodes
 struct HnswMdArgs {
     HnswArgs a;                       // out_rows = vector row of each result (CDB_INVALID_ID for pseudo nodes)
     const uint32_t *const *node_id;   // device table [num_levels+1] of device arrays
@@ -163,13 +163,8 @@ struct HnswMdArgs {
     const uint8_t *has_filter;        // [nq] (nullptr = no query has a filter)
     uint32_t *out_ids;                // [nq][out_cap] replica ids
 };
-// the warp-per-query form (hnsw_warp.cu) unless a.a.flags has CDB_HNSW_F_CTA or its shared memory does not fit
+// CDB_INVALID_PARAMS when ef_search is outside 1..4096 or the warp's shared memory (hw_carve) exceeds 200 KB
 cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s);
-size_t hnsw_warp_md_smem(uint32_t row_pitch, uint32_t ef, uint32_t M);
-cdb_status hnsw_search_warp_md_device(const HnswMdArgs &a, cudaStream_t s);
-cdb_status hnsw_dedup_md_device(const uint32_t *d_ids, const uint32_t *d_rows, const float *d_scores, const uint32_t *d_n,
-                                uint32_t in_cap, int metric, uint32_t id_base, uint32_t k5, uint32_t nq, uint32_t *d_cand,
-                                uint32_t *d_labels, uint32_t *d_cand_cnt, cudaStream_t s);
 
 // ---- hnsw_build.cu
 struct HnScoreCtx;
@@ -216,7 +211,7 @@ cdb_status hnsw_delete_device(const HnScoreCtx &sc, const GraphHost &gh, HnswBui
 const uint32_t *hnsw_state_slot_keys(const HnswBuildState *st, uint32_t level);
 constexpr uint32_t HNSW_DELETE_EF = 512;   // the ef of a delete's traversal (vector_store.rs:1247)
 // CDB_INVALID_PARAMS (with a message) when the graph writers' traversal kernel cannot run at this row pitch and ef: its
-// dynamic shared memory (hn_smem_bytes) plus its static shared memory exceed the current device's opt-in limit per block.
+// shared memory (hw_carve, all of it dynamic) exceeds the current device's opt-in limit per block.
 // The build, replica build, insert and delete entry points call it before they change anything.
 cdb_status hnsw_build_smem_check(uint32_t row_pitch, uint32_t ef);
 

@@ -636,9 +636,8 @@ cdb_status cdb_index_hnsw_profile(cdb_index *index, int32_t enable, uint64_t *ou
  * TOP/s resp. TFLOP/s: the measured roofline denominator of the integer tensor path (MEASURED_PEAKS.json only has bf16).
  * iters = 0 -> default length (~10 ms). */
 cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters, double *out_tops, float *out_ms);
-/* measurement switch: kernel variant of CDB_MODE_HNSW searches (results are identical for every value).  Bit 8 selects the
- * CTA-per-query kernel on graphs with metadata; every other bit is accepted and ignored.  0xFFFFFFFF restores the default.
- * Process-wide. */
+/* former measurement switch of CDB_MODE_HNSW kernel variants.  HNSW search now has one kernel per graph kind, so every value
+ * is accepted and selects nothing; the entry point stays for callers built against it. */
 cdb_status cdb_debug_set_hnsw_flags(uint32_t flags);
 
 /* ----------------------------------------------------- instrumentation

@@ -2,9 +2,10 @@
   * the warp kernel equals oracle/metadata_oracle.c bit for bit (ids, scores, counts, error flags, and the evaluation and pop
     counts of error-free queries) over storage types, metrics, ef, shortlists, filter shapes and D = 768 / 769;
   * the same on graphs built, grown, shrunk on the GPU and loaded from index files;
-  * CDB_HNSW_F_CTA (the CTA-per-query kernel) returns identical arrays and counters;
+  * with edge filters at D = 768 f16 and D = 40 u8, the filtered search and the plain entry point on the same graph (every
+    query unfiltered, deduplicated by replica id and re-ranked) equal the oracle;
   * cdb_search_batch_filtered_device equals the host form on caller streams, and flags bad filter ranges per query;
-  * the shared-memory limits refuse and accept the shapes they did before the warp form existed."""
+  * the shared-memory limit accepts ef 4096 at D = 768 f32 and refuses it at D = 8192."""
 import numpy as np
 import pytest
 import torch
@@ -17,7 +18,6 @@ from tests.test_gpu_hnsw_loaded_graph import cold_start
 
 pytestmark = pytest.mark.gpu
 ST, MK = cdb.StorageType, cdb.DistanceMetricKind
-CTA = 8
 BAD_FILTER = 8
 
 
@@ -125,25 +125,19 @@ def test_graphs_built_grown_shrunk_and_loaded(tmp_path):
 
 
 @pytest.mark.parametrize("st,metric,dim", [(ST.HalfPrecisionFP, MK.Cosine, 768), (ST.UnsignedByte, MK.DotProduct, 40)])
-def test_cta_kernel_returns_the_same(st, metric, dim):
+def test_edge_filters_and_the_plain_entry_point_match_oracle(st, metric, dim):
     vecs, mg = mdgraph.build(n=500, dim=dim, md_dims=7, levels=3, storage_type=int(st), metric=int(metric), seed=12)
     q, filters = with_edge_filters(*mdgraph.make_queries(vecs, mg, 64, seed=6), mg.md_dims)
     ix = md_index(vecs, mg, st, metric)
-    runs = []
-    try:
-        for flags in (0xFFFFFFFF, CTA):
-            cdb.debug_set_hnsw_flags(flags)
-            e0 = ix.hnsw_counters()
-            r = ix.batch_search_filtered(q, filters, 10, ef_search=64, shortlist_size=64)
-            e1 = ix.hnsw_counters()
-            u = ix.batch_search(q, 10, cdb.SearchMode.HNSW, ef_search=64, shortlist_size=64)
-            runs.append((r, u, (e1[0] - e0[0], e1[1] - e0[1])))
-    finally:
-        cdb.debug_set_hnsw_flags()
-    (r0, u0, c0), (r1, u1, c1) = runs
-    for x, y in list(zip(r0, r1)) + list(zip(u0, u1)):
-        assert np.array_equal(np.asarray(x).view(np.uint8), np.asarray(y).view(np.uint8))
-    assert c0 == c1
+    assert_oracle(ix, mg, vecs, q, filters, 10, 64)
+    # the plain entry point on the same graph: every query unfiltered, deduplicated by replica id (root and pseudo nodes
+    # dropped) and re-ranked on the base vectors
+    got = ix.batch_search(q, 10, cdb.SearchMode.HNSW, ef_search=64, shortlist_size=64)
+    want = pymeta.search_batch_md(mg, vecs, q, [None] * q.shape[0], 10, ef_search=64, shortlist_size=64)
+    assert np.array_equal(got[3], want[3]) and np.array_equal(got[2], want[2])
+    assert np.array_equal(got[0], want[0]) and np.array_equal(bits(got[1]), bits(want[1]))
+    assert (want[2] > 0).sum() > 32
+    ix.close()
 
 
 class DeviceBatch:
@@ -237,20 +231,14 @@ def test_bad_filter_ranges_fail_only_their_queries():
 
 
 def test_shared_memory_limits_are_unchanged():
-    # ef 4096 with f32 rows at D = 768 is accepted (both kernels, same results as the oracle) ...
+    # ef 4096 with f32 rows at D = 768 is accepted (same results as the oracle) ...
     st, metric = ST.FullPrecisionFP, MK.Cosine
     vecs, mg = mdgraph.build(n=300, dim=768, md_dims=6, levels=2, storage_type=int(st), metric=int(metric), seed=16)
     q, filters = mdgraph.make_queries(vecs, mg, 16, seed=1)
     ix = md_index(vecs, mg, st, metric)
-    want = assert_oracle(ix, mg, vecs, q, filters, 10, 4096)
-    try:
-        cdb.debug_set_hnsw_flags(CTA)
-        got = ix.batch_search_filtered(q, filters, 10, ef_search=4096)
-    finally:
-        cdb.debug_set_hnsw_flags()
-    assert np.array_equal(got[0], want[0]) and np.array_equal(bits(got[1]), bits(want[1]))
+    assert_oracle(ix, mg, vecs, q, filters, 10, 4096)
     ix.close()
-    # ... and at D = 8192 it is refused, as it was by the CTA kernel alone
+    # ... and at D = 8192 it is refused: the warp's shared memory would be 217,664 bytes, over the 200 KB the search allows
     vecs, mg = mdgraph.build(n=40, dim=8192, md_dims=6, levels=2, storage_type=int(st), metric=int(metric), seed=17)
     ix = md_index(vecs, mg, st, metric)
     with pytest.raises(cdb.CosdataError) as e:

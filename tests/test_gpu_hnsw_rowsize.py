@@ -1,11 +1,10 @@
-"""HNSW at production row sizes (D = 768 .. 12288): every traversal kernel against its oracle where a pop's neighbours no
-longer fit one staging group.
+"""HNSW at production row sizes (D = 768 .. 12288): the traversal against its oracles where a pop's neighbours no longer fit
+one staging group.
 
-Both traversal kernels score a pop's accepted neighbours in groups of staged rows: the CTA traversal (hn_traverse_level, used
-by the build, the insert, the delete's phase A and the CTA form of the filtered search) stages rows with cp.async through one
-buffer reused across __syncthreads, the warp search (hnsw_warp.cu) with TMA bulk copies completing on an mbarrier, one phase
-per group.  At D <= 64 every pop fits one group; at D = 768 a group holds about a dozen rows, so with 64 level-0 neighbours a
-pop runs several groups and the first Err may sit in a later one.  D = 769 reaches the scalar tail of the f16 dot chain.
+The traversal (hw_traverse_level, hnsw_traverse.cuh: the searches, the build, the insert and the delete's phase A) scores a
+pop's accepted neighbours in groups of staged rows, copied with TMA bulk copies that complete on the warp's mbarrier, one
+phase per group.  At D <= 64 every pop fits one group; at D = 768 a group holds about a dozen rows, so with 64 level-0
+neighbours a pop runs several groups and the first Err may sit in a later one.  D = 769 reaches the scalar tail of the f16 dot chain.
 Every comparison is exact: ids, score bits, counts, error flags, evaluation and pop counts, graphs array for array.
 The graph writers refuse an ef whose shared memory exceeds the device's limit before anything changes."""
 import ctypes as C
@@ -42,33 +41,30 @@ def stage_pitch(pitch):
     return round16(pitch) + 16
 
 
-def cta_stage_rows(pitch):   # hn_stage_rows: 18 KB, at most HN_MAX_TAKE = 64
-    return min(64, max(1, 18 * 1024 // stage_pitch(pitch)))
-
-
-def warp_stage_rows(pitch):   # hw_carve: 18700 B, at most one row per lane
+def stage_rows(pitch):   # hw_carve: 18700 B, at most one row per lane
     return min(32, max(1, 18700 // stage_pitch(pitch)))
 
 
-def hn_smem_bytes(pitch, ef):   # hnsw_traverse.cuh: the traversal's dynamic shared memory
+def carve_bytes(pitch, ef):   # hw_carve(pitch, ef).total: the traversal's dynamic shared memory (plain graphs, writers)
     efp = max(128, 1 << max(0, (ef - 1).bit_length()))
-    base = round16(pitch) + (3 * efp + 2 * 64 + 64) * 8 + (3 * efp + 2 * 64) * 4 + 64
-    return round16(base) + cta_stage_rows(pitch) * stage_pitch(pitch)
+    # query row, qkeys [2 EFP], rkeys [EFP], nkeys [64], mbarrier, fixed set [128 words], qnodes [2 EFP], rnodes [EFP], nnodes, nrow
+    base = round16(pitch) + (3 * efp + 64) * 8 + 8 + 128 * 4 + (3 * efp + 2 * 64) * 4
+    return round16(base) + stage_rows(pitch) * stage_pitch(pitch)
 
 
-# (storage, metric, D) -> (CTA, warp) rows per group
+# (storage, metric, D) -> rows per group
 SHAPES = {
-    (ST.HalfPrecisionFP, MK.Cosine, 768): (11, 12),
-    (ST.HalfPrecisionFP, MK.DotProduct, 768): (11, 12),
-    (ST.BFloat16, MK.Cosine, 768): (11, 12),
-    (ST.HalfPrecisionFP, MK.Cosine, 769): (11, 11),
-    (ST.HalfPrecisionFP, MK.Cosine, 1000): (9, 9),
-    (ST.FullPrecisionFP, MK.Cosine, 768): (5, 6),
-    (ST.UnsignedByte, MK.Cosine, 768): (23, 23),
-    (ST.SubByte3, MK.Cosine, 1000): (46, 32),
-    (ST.SubByte2, MK.Cosine, 4096): (17, 17),
-    (ST.SubByte2, MK.DotProduct, 4096): (17, 17),
-    (ST.FullPrecisionFP, MK.Cosine, 4096): (1, 1),
+    (ST.HalfPrecisionFP, MK.Cosine, 768): 12,
+    (ST.HalfPrecisionFP, MK.DotProduct, 768): 12,
+    (ST.BFloat16, MK.Cosine, 768): 12,
+    (ST.HalfPrecisionFP, MK.Cosine, 769): 11,
+    (ST.HalfPrecisionFP, MK.Cosine, 1000): 9,
+    (ST.FullPrecisionFP, MK.Cosine, 768): 6,
+    (ST.UnsignedByte, MK.Cosine, 768): 23,
+    (ST.SubByte3, MK.Cosine, 1000): 32,
+    (ST.SubByte2, MK.Cosine, 4096): 17,
+    (ST.SubByte2, MK.DotProduct, 4096): 17,
+    (ST.FullPrecisionFP, MK.Cosine, 4096): 1,
 }
 
 
@@ -146,15 +142,15 @@ def nodes_over(adj0, rows):
 @pytest.mark.parametrize("st,metric,dim", list(SHAPES), ids=[f"{s.name}-{m.name}-{d}" for s, m, d in SHAPES])
 def test_search_variants_at_production_row_sizes(st, metric, dim):
     pitch = row_pitch(st, dim)
-    groups = (cta_stage_rows(pitch), warp_stage_rows(pitch))
-    assert groups == SHAPES[(st, metric, dim)]
-    assert max(groups) < NB0                       # a pop can score more neighbours than one group holds
+    rows = stage_rows(pitch)
+    assert rows == SHAPES[(st, metric, dim)]
+    assert rows < NB0                              # a pop can score more neighbours than one group holds
     vecs, root, fg = oracle_graph(st, metric, dim)
     n = vecs.shape[0]
     ix = upload(vecs, root, fg, st, metric)
     codes, mags = ix.read_codes(0, n + 1)
     assert np.array_equal(codes, fg.codes) and np.array_equal(bits(mags), bits(fg.mags))
-    assert nodes_over(fg.adj[0], max(groups)) > n // 4
+    assert nodes_over(fg.adj[0], rows) > n // 4
     nq = 130 if (st, metric, dim) == (ST.HalfPrecisionFP, MK.Cosine, 768) else 64
     queries = near(vecs, nq, 2)
     k = 10
@@ -210,7 +206,7 @@ def test_sequential_build_equals_oracle_builder(st, metric, dim):
     o = pyinsert.Graph.init(int(metric), int(st), dim, codes, mags, n, LEVELS, NB, NB0)
     assert o.insert(0, n, ef_construction=efc, seed=seed).sum() == 0
     assert_graph_equal(g, o.export(), sc, int(metric))
-    assert nodes_over(g["adj"][0], cta_stage_rows(row_pitch(st, dim))) > n // 4
+    assert nodes_over(g["adj"][0], stage_rows(row_pitch(st, dim))) > n // 4
     o.close()
     ix.close()
 
@@ -351,7 +347,7 @@ def optin_limit():
 
 def test_build_insert_and_search_refuse_shapes_over_the_shared_memory_limit():
     st, metric, dim, n, seed = ST.FullPrecisionFP, MK.Cosine, 12288, 200, 3
-    assert hn_smem_bytes(row_pitch(st, dim), 4096) == 247888 > optin_limit()
+    assert carve_bytes(row_pitch(st, dim), 4096) == 247328 > optin_limit()
     vecs = clustered(n + 20, dim, 23)
     ix = cdb.DenseIndex(dim=dim, storage_type=st, metric=metric, capacity=n + 21, keep_raw_f32=True)
     ix.append(vecs[:n])
@@ -395,7 +391,7 @@ def test_build_insert_and_search_refuse_shapes_over_the_shared_memory_limit():
 
 def test_build_above_200kb_but_under_the_limit_still_builds():
     st, metric, dim, n, seed = ST.FullPrecisionFP, MK.Cosine, 8192, 200, 4
-    assert 200 * 1024 < hn_smem_bytes(row_pitch(st, dim), 4096) == 215120 < optin_limit()
+    assert 200 * 1024 < carve_bytes(row_pitch(st, dim), 4096) == 214560 < optin_limit()
     vecs = clustered(n, dim, 29)
     ix = cdb.DenseIndex(dim=dim, storage_type=st, metric=metric, capacity=n + 1, keep_raw_f32=True)
     ix.append(vecs)
@@ -425,7 +421,7 @@ def test_replica_build_and_delete_refuse_shapes_over_the_shared_memory_limit():
     ix.close()
     # a delete traverses at ef 512, which holds the row twice (query and stage): f32 x 28672 is over the limit
     big = 28672
-    assert hn_smem_bytes(row_pitch(ST.FullPrecisionFP, big), 512) > optin_limit()
+    assert carve_bytes(row_pitch(ST.FullPrecisionFP, big), 512) == 249376 > optin_limit()
     d = cdb.DenseIndex(dim=big, storage_type=ST.FullPrecisionFP, metric=MK.Cosine, capacity=4)
     d.append(clustered(3, big, 5))
     adj = np.array([1, EMPTY, 0, EMPTY, 0, 1], np.uint32)

@@ -1,14 +1,13 @@
-"""Filtered HNSW search on a replica graph (a collection with a metadata schema): the warp-per-query metadata kernel against
-the CTA-per-query one (CDB_HNSW_F_CTA), and the device entry point against the host one.
+"""Filtered HNSW search on a replica graph (a collection with a metadata schema): the device entry point and the host one.
 
 The graph: N embeddings (default 1M) of bench.py's clustered c3 rows, 768-dim f16 storage with raw f32 rows kept, cosine,
 the node population of tools/bench_insert_replicas.py (7 pseudo replicas; per embedding a base replica and, for two thirds
 of the embeddings, one or two metadata replicas over 7 patterns of 6 binary dimensions), built on the GPU with
 build_graph_replicas (9 levels, 32/64 neighbours, ef_construction 128).  Workloads: ef 128, k 10, batches of 1, 64 and 1024
-queries, each unfiltered, with one filter and with three filters per query.  Per workload the two kernels alternate call by
-call through the device form on one stream (ms per call from CUDA events, median after warm-up), the host form is timed
-with a host clock around its synchronising call, and the kernels' ids, counts and score bits are compared on every timed
-batch.  Prints a table, the parity line and one JSON line with the card name and power limit of the same run.
+queries, each unfiltered, with one filter and with three filters per query.  Per workload the device form runs on one stream
+(ms per call from CUDA events, median after warm-up), the host form is timed with a host clock around its synchronising
+call, and the ids, counts, score bits and error flags of every timed device batch are compared with the first one's and the
+host form's.  Prints a table, the parity line and one JSON line with the card name and power limit of the same run.
 
     python tools/bench_filtered.py [--rows 1000000] [--dim 768]
 """
@@ -26,9 +25,6 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from bench_insert_replicas import N_PATTERNS, card, population  # noqa: E402
-
-CTA = 8
-
 
 def main():
     ap = argparse.ArgumentParser()
@@ -71,7 +67,7 @@ def main():
     rec = {"card": card(), "embeddings": N, "graph_nodes": int(lst["row"].size + 2), "dim": D, "storage": "f16", "metric": "cosine",
            "ef_search": ef, "k": k, "build_s": build_s, "build_failed": int(failed.sum()), "workloads": []}
     parity_batches, parity_ok = 0, True
-    print(f"{'batch':>5} {'filters':>7} | {'warp ms':>9} {'CTA ms':>9} {'speed-up':>8} | {'device ms':>9} {'host ms':>9}")
+    print(f"{'batch':>5} {'filters':>7} | {'device ms':>9} {'host ms':>9}")
     for B in (1, 64, 1024):
         reps = {1: 40, 64: 15, 1024: 5}[B]
         for nf in (0, 1, 3):
@@ -92,8 +88,7 @@ def main():
                                                 None if d_has is None else d_has.data_ptr(), ids.data_ptr(), scores.data_ptr(),
                                                 counts.data_ptr(), err.data_ptr(), stream.cuda_stream, ef_search=ef, shortlist_size=64)
 
-            def timed_device(flags):
-                cdb.debug_set_hnsw_flags(flags)
+            def timed_device():
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record(stream)
                 device_call()
@@ -103,16 +98,13 @@ def main():
                        err.cpu().numpy().copy())
                 return e0.elapsed_time(e1), out
 
-            for flags in (0xFFFFFFFF, CTA):   # warm-up
-                timed_device(flags)
-            tw, tc = [], []
+            _, ra = timed_device()   # warm-up
+            tw = []
             for _ in range(reps):
-                a, ra = timed_device(0xFFFFFFFF)
-                b, rb = timed_device(CTA)
-                tw.append(a); tc.append(b)
+                a, rb = timed_device()
+                tw.append(a)
                 parity_batches += 1
                 parity_ok &= all(np.array_equal(x, y) for x, y in zip(ra, rb))
-            cdb.debug_set_hnsw_flags()
             qh = q.cpu().numpy()
             p = ix.params(k, cdb.SearchMode.HNSW, ef_search=ef, shortlist_size=64)
             hids, hsc = np.zeros((B, k), np.uint32), np.zeros((B, k), np.float32)
@@ -130,12 +122,13 @@ def main():
                 host_call()
                 th.append((time.perf_counter() - t0) * 1e3)
             parity_ok &= np.array_equal(hids, ra[0].view(np.uint32)) and np.array_equal(hsc.view(np.uint32), ra[1])
-            w, c, h = float(np.median(tw)), float(np.median(tc)), float(np.median(th))
-            print(f"{B:>5} {nf:>7} | {w:>9.3f} {c:>9.3f} {c / w:>7.2f}x | {w:>9.3f} {h:>9.3f}")
-            rec["workloads"].append({"batch": B, "filters_per_query": nf, "warp_ms": w, "cta_ms": c, "speedup": c / w,
-                                     "host_form_ms": h, "warp_qps": B / w * 1e3, "mean_count": float(counts.float().mean())})
-    print(f"parity: {'ok' if parity_ok else 'MISMATCH'} (ids, counts, score bits, error flags of the warp and CTA kernels on "
-          f"{parity_batches} timed batches; host form = device form)")
+            parity_ok &= np.array_equal(hcnt, ra[2].view(np.uint32)) and np.array_equal(herr, ra[3])
+            w, h = float(np.median(tw)), float(np.median(th))
+            print(f"{B:>5} {nf:>7} | {w:>9.3f} {h:>9.3f}")
+            rec["workloads"].append({"batch": B, "filters_per_query": nf, "warp_ms": w, "host_form_ms": h, "warp_qps": B / w * 1e3,
+                                     "mean_count": float(counts.float().mean())})
+    print(f"parity: {'ok' if parity_ok else 'MISMATCH'} (ids, counts, score bits, error flags of {parity_batches} timed device "
+          f"batches equal to the first one's; host form = device form)")
     rec["parity"] = bool(parity_ok)
     print(json.dumps(rec))
     ix.close()
