@@ -787,6 +787,8 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
     CDB_REQUIRE(p->shortlist_size >= 1 && p->shortlist_size <= 64, "shortlist_size must be in 1..64");
     CDB_REQUIRE(p->ef_search >= 1 && p->ef_search <= 4096, "ef_search must be in 1..4096");
     cdb_status rc;
+    // a shape whose warp does not fit shared memory is refused before the queries are quantized
+    if ((rc = hnsw_search_check(ix->row_pitch, p->ef_search, ix->has_md, ix->has_md ? ix->md_dims : 0u))) return rc;
     if ((rc = arm_status(d.metric, d.storage_type)) != CDB_OK) {
         set_error("metric/storage arm is an Err in the reference (StorageMismatch / unimplemented)");
         return rc;

@@ -68,12 +68,20 @@ static cdb_status launch_warp(const HnswArgs &a, const HwCarve &cv, cudaStream_t
     return CDB_OK;
 }
 
+cdb_status hnsw_search_check(uint32_t row_pitch, uint32_t ef, bool md, uint32_t M) {
+    if (ef == 0 || ef > 4096) { set_error("hnsw: ef_search must be in 1..4096"); return CDB_INVALID_PARAMS; }
+    if (hw_carve(row_pitch, ef, md, M).total > 200 * 1024) {
+        set_error(md ? "hnsw: ef_search / metadata dims too large for shared memory" : "hnsw: ef_search / row size too large for shared memory");
+        return CDB_INVALID_PARAMS;
+    }
+    return CDB_OK;
+}
+
 cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s) {
     if (!a.nq) return CDB_OK;
-    if (a.ef == 0 || a.ef > 4096) { set_error("hnsw: ef_search must be in 1..4096"); return CDB_INVALID_PARAMS; }
+    if (const cdb_status rc = hnsw_search_check(a.row_pitch, a.ef, false, 0)) return rc;
     const int fast = hw_fast_kind(a.st, a.metric);
     const HwCarve cv = hw_carve(a.row_pitch, a.ef);
-    if (cv.total > 200 * 1024) { set_error("hnsw: ef_search / row size too large for shared memory"); return CDB_INVALID_PARAMS; }
     const bool prof = a.prof != nullptr;
     if (fast == 1) return prof ? launch_warp<1, true>(a, cv, s) : launch_warp<1, false>(a, cv, s);
     if (fast == 2) return prof ? launch_warp<2, true>(a, cv, s) : launch_warp<2, false>(a, cv, s);
@@ -223,9 +231,8 @@ static cdb_status launch_warp_md(const HnswMdArgs &a, const HwCarve &cv, cudaStr
 
 cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s) {
     if (!a.a.nq) return CDB_OK;
-    if (a.a.ef == 0 || a.a.ef > 4096) { set_error("hnsw: ef_search must be in 1..4096"); return CDB_INVALID_PARAMS; }
+    if (const cdb_status rc = hnsw_search_check(a.a.row_pitch, a.a.ef, true, a.M)) return rc;
     const HwCarve cv = hw_carve(a.a.row_pitch, a.a.ef, true, a.M);
-    if (cv.total > 200 * 1024) { set_error("hnsw: ef_search / metadata dims too large for shared memory"); return CDB_INVALID_PARAMS; }
     const int fast = hw_fast_kind(a.a.st, a.a.metric);
     if (fast == 1) return launch_warp_md<1>(a, cv, s);
     if (fast == 2) return launch_warp_md<2>(a, cv, s);

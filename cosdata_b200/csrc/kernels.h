@@ -147,6 +147,9 @@ cdb_status hnsw_dedup_device(const uint32_t *d_ids, const uint32_t *d_rows, cons
                              uint32_t *d_labels, uint32_t *d_cand_cnt, cudaStream_t s);
 
 // ---- hnsw_warp.cu: HNSW search, one warp per query
+// CDB_INVALID_PARAMS when ef_search is outside 1..4096 or the warp's shared memory (hw_carve: rows of row_pitch bytes; md: the
+// metadata form with M dims) exceeds 200 KB.  Host only, so a search can refuse before it touches the device.
+cdb_status hnsw_search_check(uint32_t row_pitch, uint32_t ef, bool md, uint32_t M);
 cdb_status hnsw_search_warp_device(const HnswArgs &a, cudaStream_t s);
 // metadata-filtered search on graphs with replica nodes
 struct HnswMdArgs {
@@ -163,7 +166,7 @@ struct HnswMdArgs {
     const uint8_t *has_filter;        // [nq] (nullptr = no query has a filter)
     uint32_t *out_ids;                // [nq][out_cap] replica ids
 };
-// CDB_INVALID_PARAMS when ef_search is outside 1..4096 or the warp's shared memory (hw_carve) exceeds 200 KB
+// CDB_INVALID_PARAMS as hnsw_search_check
 cdb_status hnsw_search_md_device(const HnswMdArgs &a, cudaStream_t s);
 
 // ---- hnsw_build.cu

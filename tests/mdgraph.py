@@ -15,14 +15,38 @@ EMPTY = 0xFFFFFFFF
 PSEUDO_ROOT_ID = 0xFFFFFFFF - 257
 
 
-def build(n=300, dim=24, md_dims=6, levels=3, nb=8, nb0=16, replicas=4, n_pseudo=9, storage_type=4, metric=0, seed=1):
+def schema_patterns(md_dims, n_patterns, rng):
+    """dimension vectors of a schema-like collection: md_dims split into power-of-two fields (the set bits of md_dims, widest
+    first; the reference sizes each field by nearest_power_of_two(cardinality + 1), metadata/schema.rs), each field absent
+    (zeros) or holding a non-zero value id in binary (HIGH_WEIGHT = 1).  Rows are distinct and non-zero."""
+    widths = [1 << b for b in reversed(range(md_dims.bit_length())) if (md_dims >> b) & 1]
+    out, seen = [], set()
+    while len(out) < n_patterns:
+        row = []
+        for w in widths:
+            field = (rng.random(w) < 0.5).astype(np.int32) if rng.random() < 0.75 else np.zeros(w, np.int32)
+            row.append(field)
+        row = np.concatenate(row)
+        if row.any() and row.tobytes() not in seen:
+            seen.add(row.tobytes())
+            out.append(row)
+    return np.stack(out)
+
+
+def build(n=300, dim=24, md_dims=6, levels=3, nb=8, nb0=16, replicas=4, n_pseudo=9, storage_type=4, metric=0, seed=1,
+          patterns=None):
+    """patterns: None (random 0/1 rows) or a function (md_dims, n_patterns, rng) -> int32[n_patterns, md_dims], such as
+    schema_patterns"""
     rng = np.random.default_rng(seed)
     vecs = orc.synth_matrix(7000 + seed, n + 2, dim)                    # rows n = main root vector, n+1 = pseudo root vector
     codes, mags = orc.quantize_batch(storage_type, vecs)
-    # metadata table: row 0 = base dims (zeros), row 1 = pseudo root (ones), then random 0/1 patterns
+    # metadata table: row 0 = base dims (zeros), row 1 = pseudo root (ones), then the patterns
     n_patterns = 10
-    patterns = (rng.random((n_patterns, md_dims)) < 0.5).astype(np.int32)
-    patterns[patterns.sum(axis=1) == 0, 0] = 1
+    if patterns is None:
+        patterns = (rng.random((n_patterns, md_dims)) < 0.5).astype(np.int32)
+        patterns[patterns.sum(axis=1) == 0, 0] = 1
+    else:
+        patterns = np.asarray(patterns(md_dims, n_patterns, rng), np.int32)
     md_bits = np.concatenate([np.zeros((1, md_dims), np.int32), np.ones((1, md_dims), np.int32), patterns])
     md_mags = np.array([pymeta.metadata_mag(r) for r in md_bits], dtype=np.float32)
     # node population: (id, row, md row, component)
@@ -88,22 +112,26 @@ def make_queries(vecs, mg, nq, seed=2):
     return q, filters
 
 
-def replica_population(n=400, dim=24, md_dims=6, levels=4, n_patterns=7, seed=3, lo=-1.0, hi=1.0):
+def replica_population(n=400, dim=24, md_dims=6, levels=4, n_patterns=7, seed=3, lo=-1.0, hi=1.0, patterns=None):
     """The node list the reference would index for a collection with a metadata schema, in its insertion order
     (vector_store.rs:629-712): pseudo replicas first (created with the collection), then per embedding its base replica
     (base dimensions, mag 0 -> main root) and, for embeddings with metadata fields, one replica per field combination.
     Dimension vectors are 0/1 (HIGH_WEIGHT = 1 binary encodings, metadata/mod.rs:19); pseudo replicas carry the same patterns
-    the metadata replicas use, so perfect matches (cs == 1.0) exist.
+    the metadata replicas use, so perfect matches (cs == 1.0) exist.  patterns: None (the binary codes 1..n_patterns) or a
+    function like schema_patterns.
     -> dict(vecs f32[n, dim], md_bits, md_mags, row, node_id, base_id, md_row, max_level, main_root_md, pseudo_root_md)"""
     from cosdata_b200.api import level_probs, max_insert_level, pseudo_level_probs
     rng = np.random.default_rng(seed)
     centres = rng.normal(size=(16, dim)).astype(np.float32)
     v = (centres[rng.integers(0, 16, n)] + 0.35 * rng.normal(size=(n, dim))).astype(np.float32)
     vecs = (v / (np.abs(v).max() * 1.01) * max(abs(lo), abs(hi))).astype(np.float32)
-    patterns = np.zeros((n_patterns, md_dims), np.int32)
-    for p in range(n_patterns):                                         # distinct non-zero binary codes
-        code = p + 1
-        patterns[p] = [(code >> b) & 1 for b in range(md_dims)]
+    if patterns is None:
+        patterns = np.zeros((n_patterns, md_dims), np.int32)
+        for p in range(n_patterns):                                     # distinct non-zero binary codes
+            code = p + 1
+            patterns[p] = [(code >> b) & 1 for b in range(md_dims)]
+    else:
+        patterns = np.asarray(patterns(md_dims, n_patterns, np.random.default_rng(seed + 1)), np.int32)
     md_bits = np.concatenate([np.zeros((1, md_dims), np.int32), np.ones((1, md_dims), np.int32), patterns])
     md_mags = np.array([pymeta.metadata_mag(r) for r in md_bits], dtype=np.float32)
     md_mags[0] = 0.0
