@@ -1086,6 +1086,10 @@ cdb_status index_search_device_keys(cdb_index *ix, const float *d_queries, uint3
 }
 int index_device(const cdb_index *ix) { return ix->desc.device; }
 uint32_t index_dim(const cdb_index *ix) { return ix->desc.dim; }
+int index_metric(const cdb_index *ix) { return ix->desc.metric; }
+int index_storage_type(const cdb_index *ix) { return ix->desc.storage_type; }
+uint32_t index_id_base(const cdb_index *ix) { return ix->desc.id_base; }
+uint64_t index_capacity(const cdb_index *ix) { return ix->desc.capacity; }
 int index_result_metric(const cdb_index *ix, int mode) { return mode == CDB_MODE_BRUTE_CODES ? ix->desc.metric : CDB_METRIC_COSINE; }
 bool index_has_graph_metadata(cdb_index *ix) {
     std::shared_lock<std::shared_mutex> lock(ix->rw);

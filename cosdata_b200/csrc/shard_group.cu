@@ -31,6 +31,10 @@ cdb_status index_search_device_keys(cdb_index *ix, const float *d_queries, uint3
                                     float *d_scores, uint32_t *d_counts, uint8_t *d_err, uint64_t *d_keys, cudaStream_t s);
 int index_device(const cdb_index *ix);
 uint32_t index_dim(const cdb_index *ix);
+int index_metric(const cdb_index *ix);
+int index_storage_type(const cdb_index *ix);
+uint32_t index_id_base(const cdb_index *ix);
+uint64_t index_capacity(const cdb_index *ix);
 int index_result_metric(const cdb_index *ix, int mode);
 
 // sparse.cu: a shard group's two-phase sparse search
@@ -278,16 +282,26 @@ cdb_status cdb_shard_group_destroy(cdb_shard_group *g) {
     return CDB_OK;
 }
 
+// [base, base + capacity) of two shards of one local group must not meet: a candidate belongs to exactly one shard
+static bool id_ranges_meet(uint32_t b0, uint64_t c0, uint32_t b1, uint64_t c1) { return b0 < b1 + c1 && b1 < b0 + c0; }
+
+// Every local shard gets the same query batch (nq * dim floats) and the merge decodes all their keys with one metric, and
+// relies on every key being unique: a shard must agree with every other attached one, whatever the attach order.
 cdb_status cdb_shard_group_attach(cdb_shard_group *g, uint32_t local_slot, cdb_index *shard) {
     CDB_REQUIRE(g && shard && local_slot < g->dev.size(), "bad argument");
     CDB_REQUIRE(index_device(shard) == g->dev[local_slot], "the shard lives on another device than the group slot");
-    CDB_REQUIRE(g->shard[0] == nullptr || local_slot == 0 || index_dim(shard) == index_dim(g->shard[0]), "shards differ in dimension");
+    for (size_t j = 0; j < g->dev.size(); ++j) {
+        const cdb_index *o = g->shard[j];
+        if (!o || j == local_slot) continue;
+        CDB_REQUIRE(index_dim(o) == index_dim(shard), "shards differ in dimension");
+        CDB_REQUIRE(index_metric(o) == index_metric(shard), "shards differ in metric");
+        CDB_REQUIRE(index_storage_type(o) == index_storage_type(shard), "shards differ in storage_type");
+        CDB_REQUIRE(!id_ranges_meet(index_id_base(o), index_capacity(o), index_id_base(shard), index_capacity(shard)),
+                    "dense shards' id ranges overlap");
+    }
     g->shard[local_slot] = shard;
     return CDB_OK;
 }
-
-// [base, base + capacity) of two shards of one local group must not meet: a candidate belongs to exactly one shard
-static bool id_ranges_meet(uint32_t b0, uint64_t c0, uint32_t b1, uint64_t c1) { return b0 < b1 + c1 && b1 < b0 + c0; }
 
 cdb_status cdb_shard_group_attach_sparse(cdb_shard_group *g, uint32_t local_slot, cdb_sparse_index *shard) {
     CDB_REQUIRE(g && shard && local_slot < g->dev.size(), "bad argument");
@@ -359,6 +373,15 @@ static cdb_status group_allgather(cdb_shard_group *g, size_t words, cudaStream_t
     return CDB_OK;
 }
 
+// shared memory of merge_gathered_kernel: the world * k keys of one query
+constexpr size_t MERGE_SMEM_MAX = 200 * 1024;
+
+// both forms refuse a merge that cannot run before any copy or search is issued
+static cdb_status merge_check(const cdb_shard_group *g, uint32_t k) {
+    CDB_REQUIRE((size_t)g->world * k * 8 <= MERGE_SMEM_MAX, "sharded merge: world * k * 8 bytes exceed 200 KB");
+    return CDB_OK;
+}
+
 // local slot i: search its shard into its slot of its gather buffer, then the collective, then (slot 0 / this rank) the merge
 static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_search_params *p, const std::vector<const float *> &d_q,
                                   uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
@@ -384,7 +407,6 @@ static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_sea
     CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
     cudaStream_t s0 = (nl == 1 && out_stream) ? out_stream : g->stream[0];
     const size_t smem = (size_t)g->world * k * 8;
-    if (smem > 200 * 1024) { set_error("sharded merge: world * k too large"); return CDB_INVALID_PARAMS; }
     CDB_ALLOW_SMEM(merge_gathered_kernel, smem);
     merge_gathered_kernel<<<nq, 128, smem, s0>>>(reinterpret_cast<const uint64_t *>(g->gather[0].p), g->world, nq, k, words,
                                                   index_result_metric(g->shard[0], p->mode), d_ids, d_scores, d_counts, d_err);
@@ -397,12 +419,13 @@ cdb_status cdb_search_batch_sharded(cdb_shard_group *g, const float *queries, ui
     CDB_REQUIRE(g && p && (queries || !nq) && (out_ids || !nq) && (out_scores || !nq), "null argument");
     CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
     if (!nq) return CDB_OK;
+    cdb_status rc = merge_check(g, p->k);
+    if (rc) return rc;
     std::lock_guard<std::mutex> lock(g->mu);
     const size_t nl = g->dev.size();
     CDB_REQUIRE(g->shard[0], "a group slot has no shard attached");
     const uint32_t dim = index_dim(g->shard[0]);
     const size_t nk = (size_t)nq * p->k;
-    cdb_status rc;
     std::vector<const float *> d_q(nl);
     for (size_t i = 0; i < nl; ++i) {   // the same host batch goes to every local device
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
@@ -439,6 +462,8 @@ cdb_status cdb_search_batch_sharded_device(cdb_shard_group *g, const float *d_qu
     CDB_REQUIRE(g->dev.size() == 1, "the device form serves one-process-per-GPU groups (cdb_shard_group_create_rank)");
     CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
     if (!nq) return CDB_OK;
+    cdb_status rc = merge_check(g, p->k);
+    if (rc) return rc;
     std::lock_guard<std::mutex> lock(g->mu);
     std::vector<const float *> d_q(1, d_queries);
     return sharded_enqueue(g, nq, p, d_q, d_out_ids, d_out_scores, d_out_counts, d_err_flags, (cudaStream_t)stream);

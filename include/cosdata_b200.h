@@ -596,10 +596,15 @@ cdb_status cdb_rerank_f32(cdb_index *index, const float *query, const uint32_t *
  *   cdb_shard_group_create       one process drives n devices (ncclCommInitAll over device_ordinals[]); a device listed
  *                                twice selects a copy-based loopback gather (single-GPU tests of the same code path)
  *   cdb_nccl_unique_id + cdb_shard_group_create_rank   one process per GPU: rank 0 creates the id, every rank passes it in
- *   cdb_shard_group_attach       local slot i <- the shard living on that slot's device
+ *   cdb_shard_group_attach       local slot i <- the shard living on that slot's device.  CDB_INVALID_PARAMS, nothing
+ *                                attached, unless the shard has the dimension, metric and storage type of every shard
+ *                                already attached to another local slot and its [id_base, id_base + capacity) meets
+ *                                none of theirs (checked whatever the attach order)
  *   cdb_search_batch_sharded     host queries in, merged host results out (every local device gets the batch); in a
  *                                per-rank group every rank must call it with the same batch and receives the same result
  *   cdb_search_batch_sharded_device   per-rank groups only: device buffers, asynchronous on `stream`
+ * Both searches refuse world * k * 8 > 200 KB (the merge's shared memory) with CDB_INVALID_PARAMS before any copy or
+ * search is issued.
  * Results are those cdb_search_batch would return on the concatenated corpus (exact modes), resp. the merge of the
  * per-shard HNSW results (one independent graph per shard). */
 #define CDB_NCCL_UNIQUE_ID_BYTES 128
