@@ -8,6 +8,30 @@ namespace cdb {
 
 // ------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// Shared-memory accesses by shared address (smem_u32).  A kernel that aligns its dynamic shared memory through an integer
+// leaves the compiler unaware that pointers into it are shared: it emits generic loads and atomics for them.  The loads are
+// `asm volatile` so that they stay where the kernel places them (e.g. between a wgmma hand-off and its wait).
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ float lds_volatile_f32(uint32_t addr) {   // a value another warp may change concurrently
+    float v;
+    asm volatile("ld.volatile.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ float4 lds_f32x4(uint32_t addr) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void red_shared_add_u32(uint32_t addr, uint32_t v) {
+    asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void red_shared_max_s32(uint32_t addr, int v) {
+    asm volatile("red.shared.max.s32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));

@@ -55,10 +55,11 @@ enum : int {
     TS_PROF_PRODUCER,    // producer: whole issue loop
     TS_PROF_CTAS,        // CTAs
     TS_PROF_MATH_WAIT,   // s8 form: consumers waiting for their turn at the tensor pipe (the other warpgroup's K loop)
-    TS_PROF_EPI_THR,     // s8 form, parts of TS_PROF_EPILOGUE: the four queries' thresholds
-    TS_PROF_EPI_FOLD,    //   class maxima, their fold into gm and the shared class maxima, the hit test
+    TS_PROF_EPI_THR,     // s8 form, parts of TS_PROF_EPILOGUE: the four queries' thresholds (while the turn's MMAs drain)
+    TS_PROF_EPI_FOLD,    //   the per-class fold into gm and the shared class maxima (only where a class can grow)
     TS_PROF_EPI_EMIT,    //   the emission loops (only on a hit)
     TS_PROF_BOUND_ROUNDS,   // s8 form: rounds of the bound warp (TS_PROF_REFRESH then sums the bound warp's clocks in them)
+    TS_PROF_EPI_CMAX,    // s8 form, part of TS_PROF_EPILOGUE: class maxima, hit test and the test whether a class can grow
     TS_PROF_SLOTS
 };
 
@@ -600,8 +601,9 @@ tensor_scan_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 //     bounds from `sbound`; they never touch the global class maxima during the scan.  A bound-warp round pushes the
 //     CTA's class maxima that exceed the global ones to `ggm` (RED), takes the k-th largest of each query's NG class
 //     maxima (the larger of the global and the CTA's value) by rank counting, and raises `sbound`.  It runs once per
-//     completed warpgroup epilogue (back to back when it falls behind).  It only moves and selects values the consumers
-//     computed as rigorous lower bounds, and `sbound` only rises, so a stale bound costs candidates, never correctness.
+//     warpgroup epilogue (woken as the epilogue starts; back to back when it falls behind).  It only moves and selects
+//     values the consumers computed as rigorous lower bounds, and `sbound` only rises, so a stale bound costs
+//     candidates, never correctness.
 // Shared memory (227 KB per block): query tile kblocks x 16 KB (96 KB at D = 768) + ring stages x 16 KB (6: one whole
 // half-tile at D = 768) + candidate staging 256 threads x 4 queries x 16 B (a count and 3 ids: 16 KB) + class maxima
 // NG x 128 ints (8 KB) + per query the bound, {s_q, 1/s_q down, 1/s_q up, 1 + delta_n + e_q} and e_q (1 + delta_n) +
@@ -742,7 +744,7 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                 atomicAdd(a.prof + TS_PROF_CTAS, 1ull);
             }
         } else if (threadIdx.x / 32 == TS8_BOUND_WARP && T > 0) {
-            // one round per completed warpgroup epilogue, until the consumers have published their final class maxima
+            // one round per warpgroup epilogue, until the consumers have published their final class maxima
             unsigned long long p_ref = 0, n_rounds = 0;
             uint32_t seen = 0;
             for (;;) {
@@ -784,7 +786,7 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
     if (wg == 1) named_bar_arrive<TS8_BAR_TURN, 256>();   // warpgroup 0 takes the first turn
     mbar_wait(smem_u32(q_bar), 0);
     const uint32_t q0 = smem_u32(qtile), r0 = smem_u32(ring);
-    unsigned long long p_turn = 0, p_full = 0, p_mma = 0, p_thr = 0, p_fold = 0, p_emit = 0, p_c = PROF ? clock64() : 0;
+    unsigned long long p_turn = 0, p_full = 0, p_mma = 0, p_thr = 0, p_cmax = 0, p_fold = 0, p_emit = 0, p_c = PROF ? clock64() : 0;
     for (uint32_t t = 0; t < T; ++t) {
         const uint32_t nt = g + t * G;
         const uint64_t row0 = (uint64_t)nt * TS_BLOCK_N + wg * TS8_HALF;   // this warpgroup's half
@@ -823,27 +825,20 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
         // last turn hands over nothing (warpgroup 0 has no turn left), so both barriers see as many arrivals as waits.
         if (wg == 0) named_bar_arrive<TS8_BAR_TURN + 1, 256>();
         else if (t + 1 < T) named_bar_arrive<TS8_BAR_TURN, 256>();
-        wgmma_wait<0>();
-        if (a.kblocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
-        if (ct == 128 && a.mtiles > 1) atomicAdd(a.progress + g, 1u);   // the tile's upper half is in: all of its loads landed
-        unsigned long long c_epi = 0;
-        if (PROF) {
-            c_epi = clock64();
-            p_turn += c_main - c_turn;
-            p_full += c_full;
-            p_mma += c_epi - c_main - c_full;
-        }
+        const unsigned long long c_thr = PROF ? clock64() : 0;
 
-        // ---- epilogue (the filter of tensor_scan_kernel, KIND 2).  The per-query addresses below are derived from `me`,
-        //      which the empty asm makes opaque per tile: otherwise they are hoisted out of the tile loop and held in
-        //      registers (or spilled) across the K loop, where the accumulators need every register.
+        // ---- epilogue (the filter of tensor_scan_kernel, KIND 2).  Up to wgmma_wait<0> it needs no accumulator, so it
+        //      runs while the turn's last MMAs drain.  The per-query addresses below are derived from `me`, which the empty
+        //      asm makes opaque per tile: otherwise they are hoisted out of the tile loop and held in registers (or spilled)
+        //      across the K loop, where the accumulators need every register.
         uint32_t me = ct;
         asm volatile("" : "+r"(me));
+        // non-returning reductions that nothing below waits for.  progress: the tile's upper half is in (its K loop waited
+        // for every one of its loads).  ctl: wakes the bound warp, which runs its rounds back to back at this cadence anyway.
+        if (me == 128 && a.mtiles > 1) atomicAdd(a.progress + g, 1u);
+        if ((me & 127) == 0) red_shared_add_u32(smem_u32(ctl), 1u);
         const uint32_t qrow = 16 * ((me >> 5) & 3) + ((me & 31) >> 2);   // + 8 (i & 1) + 64 (i >> 1)
-        const bool full_half = row0 + TS8_HALF <= a.n_rows;   // only the corpus' last tile can be partial
-        const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;
-        // the four queries' thresholds first, as four independent chains: a warp runs this epilogue alone on its SM
-        // sub-partition (the other warpgroup is in its K loop).  s_T*s_q rounded down and up, eps(q,T) rounded up, and
+        // the four queries' thresholds, as four independent chains.  s_T*s_q rounded down and up, eps(q,T) rounded up, and
         // thrI <= (A - eps) / (s_T*s_q) through the reciprocals rounded the safe way for the numerator's sign:
         // fl_down(fl_down(num * 1/s_T) * 1/s_q), down for num >= 0, up otherwise (s_T or s_q = 0: as the division did)
         float slo[4], shi[4], eps[4];
@@ -851,29 +846,38 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
-            const float4 qp = qpar[ql];
+            const float4 qp = lds_f32x4(smem_u32(qpar + ql));
             slo[i] = __fmul_rd(se.x, qp.x);
             shi[i] = __fmul_ru(se.x, qp.x);
-            eps[i] = __fmaf_ru(qp.w, se.y, qeps[ql]);
-            const float num = __fsub_rd(*reinterpret_cast<const volatile float *>(sbound + ql), eps[i]);
+            eps[i] = __fmaf_ru(qp.w, se.y, lds_f32(smem_u32(qeps + ql)));
+            const float num = __fsub_rd(lds_volatile_f32(smem_u32(sbound + ql)), eps[i]);
             const bool pos = num >= 0.0f;
             thrI[i] = __float2int_rd(__fmul_rd(__fmul_rd(num, pos ? rt.x : rt.y), pos ? qp.y : qp.z));
         }
-        unsigned long long c_fold = 0;
+        const unsigned long long c_wait = PROF ? clock64() : 0;
+        wgmma_wait<0>();
+        if (a.kblocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+        unsigned long long c_epi = 0;
         if (PROF) {
-            c_fold = clock64();
-            p_thr += c_fold - c_epi;
+            c_epi = clock64();
+            p_turn += c_main - c_turn;
+            p_full += c_full;
+            p_mma += (c_thr - c_main - c_full) + (c_epi - c_wait);
+            p_thr += c_wait - c_thr;
         }
-        // class maxima, their fold and the hit test of all four queries, then one warp-uniform branch to the emission
+        // class maxima and hit test of all four queries, with no branch between the queries so that their chains interleave
+        const bool full_half = row0 + TS8_HALF <= a.n_rows;   // only the corpus' last tile can be partial
+        const uint64_t left = a.n_rows > row0 ? a.n_rows - row0 : 0;
+        int cm[4][NL];
         bool hit[4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
-            const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);   // value (j, b) at v_i[4j + b]
-            int cm[NL];
+        for (int i = 0; i < 4; ++i)
 #pragma unroll
-            for (int l = 0; l < NL; ++l) cm[l] = INT_MIN;
-            if (full_half) {
+            for (int l = 0; l < NL; ++l) cm[i][l] = INT_MIN;
+        if (full_half) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);   // value (j, b) at v_i[4j + b]
                 int zmax = INT_MIN;   // HAS_DEG: 0 if some accumulator of the half is exactly zero
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -885,14 +889,18 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                             v = v == 0 ? INT_MIN : v;
                         }
                         const int l = (j & (NG / 8 - 1)) * 2 + b;
-                        cm[l] = max(cm[l], v);
+                        cm[i][l] = max(cm[i][l], v);
                     }
                 }
                 int cmax = zmax;
 #pragma unroll
-                for (int l = 0; l < NL; ++l) cmax = max(cmax, cm[l]);
+                for (int l = 0; l < NL; ++l) cmax = max(cmax, cm[i][l]);
                 hit[i] = cmax >= thrI[i];
-            } else {
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
 #pragma unroll
@@ -900,28 +908,44 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
                         const uint32_t col = 8 * j + 2 * (me & 3) + b;
                         const int v = (int)v_i[4 * j + b];
                         const int l = (j & (NG / 8 - 1)) * 2 + b;
-                        if ((uint64_t)col < left && !(HAS_DEG && v == 0)) cm[l] = max(cm[l], v);
+                        if ((uint64_t)col < left && !(HAS_DEG && v == 0)) cm[i][l] = max(cm[i][l], v);
                     }
                 }
                 hit[i] = true;
             }
-            hit[i] = hit[i] && mt * TS_BLOCK_M + ql < a.n_queries;
-            // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class.
-            // The lower bound fl_down(fl_down(cm * s) - eps) (s = slo for cm >= 0, shi >= slo >= 0 otherwise) does not
-            // decrease with cm, so no class can grow unless the largest class maximum's bound exceeds gmin: one bound per
-            // query and tile instead of NL, and the per-class fold only on the rare tiles that can raise one.
-            int cmx = cm[0];
+        }
+        // |dp| < 2^31 (127^2 * D, D <= rerank_f32_max_dim()): INT_MIN only marks an empty class.
+        // The lower bound fl_down(fl_down(cm * s) - eps) (s = slo for cm >= 0, shi >= slo >= 0 otherwise) does not
+        // decrease with cm, so no class can grow unless the largest class maximum's bound exceeds gmin: one bound per
+        // query and tile instead of NL, and the per-class fold only on the rare tiles that can raise one.
+        bool grow[4];
 #pragma unroll
-            for (int l = 1; l < NL; ++l) cmx = max(cmx, cm[l]);
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
+            hit[i] = hit[i] && mt * TS_BLOCK_M + ql < a.n_queries;
+            int cmx = cm[i][0];
+#pragma unroll
+            for (int l = 1; l < NL; ++l) cmx = max(cmx, cm[i][l]);
             const float lbx = __fsub_rd(__fmul_rd(__int2float_rd(cmx), cmx >= 0 ? slo[i] : shi[i]), eps[i]);
-            if (cmx != INT_MIN && lbx > gmin[i]) {
+            grow[i] = cmx != INT_MIN && lbx > gmin[i];
+        }
+        unsigned long long c_fold = 0;
+        if (PROF) {
+            c_fold = clock64();
+            p_cmax += c_fold - c_epi;
+        }
+        if (__any_sync(0xffffffffu, grow[0] || grow[1] || grow[2] || grow[3])) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                if (!grow[i]) continue;
+                const uint32_t ql = qrow + 64 * (i >> 1) + 8 * (i & 1);
                 float mn = INFINITY;
 #pragma unroll
                 for (int l = 0; l < NL; ++l) {
-                    const float lb = __fsub_rd(__fmul_rd(__int2float_rd(cm[l]), cm[l] >= 0 ? slo[i] : shi[i]), eps[i]);
-                    if (cm[l] != INT_MIN && lb > gm[i][l]) {
+                    const float lb = __fsub_rd(__fmul_rd(__int2float_rd(cm[i][l]), cm[i][l] >= 0 ? slo[i] : shi[i]), eps[i]);
+                    if (cm[i][l] != INT_MIN && lb > gm[i][l]) {
                         gm[i][l] = lb;
-                        atomicMax(cls + (8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M + ql, f2ord(lb));
+                        red_shared_max_s32(smem_u32(cls + (8 * (l >> 1) + 2 * (me & 3) + (l & 1)) * TS_BLOCK_M + ql), f2ord(lb));
                     }
                     mn = fminf(mn, gm[i][l]);
                 }
@@ -934,32 +958,41 @@ tensor_scan_s8_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_co
             p_fold += c_emit - c_fold;
         }
         if (a.emit && __any_sync(0xffffffffu, hit[0] || hit[1] || hit[2] || hit[3])) {
+            const uint32_t lim = left < TS8_HALF ? (uint32_t)left : TS8_HALF;   // columns of the half that hold rows
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 if (!hit[i]) continue;
                 const uint32_t qi = mt * TS_BLOCK_M + qrow + 64 * (i >> 1) + 8 * (i & 1);
                 const uint32_t *v_i = acc + 64 * (i >> 1) + 2 * (i & 1);
                 uint32_t *stage = reinterpret_cast<uint32_t *>(lstage + (size_t)(me * 4 + i) * TS8_SLOT_BYTES);
+                // the passing values as a mask (bit 2j + b: column 8j + 2(me & 3) + b) without a branch per value, then
+                // one emission per set bit in column order: a warp with a hit delays its warpgroup's next turn
+                uint32_t pass = 0;
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
                         const uint32_t col = 8 * j + 2 * (me & 3) + b;
-                        if ((uint64_t)col < left && (int)v_i[4 * j + b] >= thrI[i])
-                            epi_emit<TS8_LSTAGE>(a.cand, a.cand_cnt, a.cand_cap, qi, stage, a.id_base + (uint32_t)(row0 + col));
+                        if (col < lim && (int)v_i[4 * j + b] >= thrI[i]) pass |= 1u << (2 * j + b);
                     }
+                }
+                while (pass) {
+                    const uint32_t x = __ffs(pass) - 1;
+                    pass &= pass - 1;
+                    epi_emit<TS8_LSTAGE>(a.cand, a.cand_cnt, a.cand_cap, qi, stage,
+                                         a.id_base + (uint32_t)(row0 + 8 * (x >> 1) + 2 * (me & 3) + (x & 1)));
                 }
             }
         }
-        if ((me & 127) == 0) atomicAdd(ctl, 1u);   // wakes the bound warp
         if (PROF) p_emit += clock64() - c_emit;
     }
     if (PROF && (ct & 127) == 0) {
         atomicAdd(a.prof + TS_PROF_MATH_WAIT, p_turn);
         atomicAdd(a.prof + TS_PROF_FULL_WAIT, p_full);
         atomicAdd(a.prof + TS_PROF_MMA, p_mma);
-        atomicAdd(a.prof + TS_PROF_EPILOGUE, p_thr + p_fold + p_emit);
+        atomicAdd(a.prof + TS_PROF_EPILOGUE, p_thr + p_cmax + p_fold + p_emit);
         atomicAdd(a.prof + TS_PROF_EPI_THR, p_thr);
+        atomicAdd(a.prof + TS_PROF_EPI_CMAX, p_cmax);
         atomicAdd(a.prof + TS_PROF_EPI_FOLD, p_fold);
         atomicAdd(a.prof + TS_PROF_EPI_EMIT, p_emit);
         atomicAdd(a.prof + TS_PROF_TILES, (unsigned long long)T);

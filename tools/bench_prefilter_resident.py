@@ -28,7 +28,7 @@ SEED_C4, SEED_C4_QUERY = 0xC05DA7A + 4, 0xC05DA7A + 104
 
 # the TS_PROF_* slots of cdb_debug_scan_profile (csrc/tensor_scan.cu)
 SLOTS = ["full_wait", "mma", "epilogue", "refresh", "empty_wait", "drift", "tiles", "consumer", "producer", "ctas", "math_wait",
-         "epi_thr", "epi_fold", "epi_emit", "bound_rounds"]
+         "epi_thr", "epi_fold", "epi_emit", "bound_rounds", "epi_cmax"]
 
 
 def gpu_query(fields):
@@ -51,10 +51,11 @@ def scan_profile(enable):
 def per_tile(p):
     """consumer phases per tile and warpgroup, producer phases per tile (the producer issues every tile once per CTA).
     math_wait: the s8 kernel's warpgroups waiting for their turn at the tensor pipe (0 for the other forms).
-    s8 kernel: epi_thr / epi_fold / epi_emit split the epilogue (threshold, class maxima and fold, emission), refresh is the
-    bound warp's clocks in its rounds, bound_rounds its rounds per corpus tile of a CTA"""
+    s8 kernel: epi_thr / epi_cmax / epi_fold / epi_emit split the epilogue (threshold, class maxima and hit test, per-class
+    fold, emission), refresh is the bound warp's clocks in its rounds, bound_rounds its rounds per corpus tile of a CTA"""
     t = max(p["tiles"], 1)
-    r = {k: p[k] / t for k in ("full_wait", "mma", "epilogue", "refresh", "consumer", "math_wait", "epi_thr", "epi_fold", "epi_emit")}
+    r = {k: p[k] / t for k in ("full_wait", "mma", "epilogue", "refresh", "consumer", "math_wait", "epi_thr", "epi_cmax", "epi_fold",
+                                "epi_emit")}
     r.update({k: 2 * p[k] / t for k in ("empty_wait", "drift", "producer", "bound_rounds")})
     return r
 
