@@ -117,6 +117,7 @@ using namespace cdb;
 struct Scratch {
     DevBuf q_codes, q_mags, partial, err32, io_ids, io_scores, io_counts, io_err, io_q, misc;
     DevBuf qh, gthr, cand, cand_cnt, flags, progress, qsel, qse;
+    DevBuf kept_cnt;                       // s8 form: candidates left per query after the final-bound refilter
     DevBuf hn_rows, hn_scores, hn_n, qraw, qraw_mags, hn_ids, hn_labels, flt_off, flt_dims, flt_has;
     cudaStream_t stream = nullptr;         // used by the host-buffer entry points
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
@@ -138,7 +139,7 @@ struct Scratch {
         if (stream) cudaStreamSynchronize(stream);
         for (DevBuf *b : {&q_codes, &q_mags, &partial, &err32, &io_ids, &io_scores, &io_counts, &io_err, &io_q, &misc, &qh, &gthr, &cand,
                           &cand_cnt, &flags, &progress, &qsel, &hn_rows, &hn_scores, &hn_n, &qraw, &qraw_mags, &hn_ids, &hn_labels,
-                          &flt_off, &flt_dims, &flt_has, &qse})
+                          &flt_off, &flt_dims, &flt_has, &qse, &kept_cnt})
             b->release();
         for (auto &e : ev) if (e) cudaEventDestroy(e);
         if (stream) cudaStreamDestroy(stream);
@@ -960,6 +961,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         uint32_t *flags = sc->flags.as<uint32_t>();  // [0] queries of the last search that needed the exact scan, [3] searches with a fallback
         const bool has_deg = ix->n_allzero_rows + ix->n_odd_rows + ix->n_deleted > 0;
         const bool s8 = use_s8_form(ix, nq);
+        const uint32_t *rerank_cnt = sc->cand_cnt.as<uint32_t>();   // (the fallback selection keeps reading cand_cnt)
         if (s8 && (rc = sc->qse.ensure((size_t)nq * 16))) return rc;   // {s_q, e_q}, then {1/s_q rounded down, up}
         if ((rc = prep_queries_device(d_queries, nq, d.dim, sc->q_codes.as<float>(), pitch / 4, sc->q_mags.as<float>(), sc->qh.p,
                                       s8 ? ix->xs8_pitch : ix->xh_pitch, sc->gthr.as<int>(), ix->deg.as<uint32_t>(), has_deg, d.id_base,
@@ -969,10 +971,14 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
             return rc;
         CDB_CUDA_TRY(cudaEventRecord(ix->ring0[slot], s));
         if (s8) {
-            if ((rc = tensor_scan_s8_device(ix->d_xs8, sc->qh.p, ix->xs8_pitch, ix->size, nq, d.dim, p->k, ix->d_s8se, ix->d_s8rcp,
+            bool refiltered = false;
+            if ((rc = sc->kept_cnt.ensure((size_t)nq * 4)) ||
+                (rc = tensor_scan_s8_device(ix->d_xs8, sc->qh.p, ix->xs8_pitch, ix->size, nq, d.dim, p->k, ix->d_s8se, ix->d_s8rcp,
                                             sc->qse.as<float2>(), sc->qse.as<float2>() + nq, d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(),
-                                            sc->cand_cnt.as<uint32_t>(), cap, sc->progress.as<uint32_t>(), has_deg, ix->sm_count, s)))
+                                            sc->cand_cnt.as<uint32_t>(), cap, sc->progress.as<uint32_t>(), has_deg, ix->sm_count, s,
+                                            sc->kept_cnt.as<uint32_t>(), &refiltered)))
                 return rc;
+            if (refiltered) rerank_cnt = sc->kept_cnt.as<uint32_t>();
             ix->stat_s8_searches++;
         } else if ((rc = tensor_scan_device(ix->d_xh, sc->qh.p, ix->xh_pitch, ix->size, nq, d.dim, p->k, 2.0f * prefilter_eps(d.dim),
                                             d.id_base, sc->gthr.as<int>(), sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), cap,
@@ -982,7 +988,7 @@ static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d
         }
         CDB_CUDA_TRY(cudaEventRecord(ix->ring1[slot], s));
         if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->q_codes.as<float>(),
-                                    pitch / 4, sc->q_mags.as<float>(), nq, sc->cand.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(),
+                                    pitch / 4, sc->q_mags.as<float>(), nq, sc->cand.as<uint32_t>(), rerank_cnt,
                                     cap, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr, sc->cur_keys, ix->del_dev(),
                                     /*dedup=*/true)))
             return rc;

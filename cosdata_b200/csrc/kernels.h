@@ -294,7 +294,10 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
                                  uint32_t k, const float2 *d_tile_se, const float2 *d_tile_rcp, const float2 *d_q_se,
                                  const float2 *d_q_rcp, uint32_t id_base, int *d_ggm,
                                  uint32_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_progress, bool has_deg,
-                                 int sm_count, cudaStream_t s);
+                                 int sm_count, cudaStream_t s, uint32_t *d_kept_cnt, bool *refiltered);
+// d_kept_cnt (may be null): after tensor_scan_s8_kernel on a shard without degenerate or deleted rows, the candidates are
+// tested again against the final bound (s8_refilter_kernel): the survivors are compacted to the front of each list and
+// d_kept_cnt[q] is their number (cap for an overflowed list), *refiltered = true; d_cand_cnt keeps the emitted counts.
 cdb_status tensor_scan_i8_device(const uint8_t *d_x, const uint8_t *d_q, uint32_t pitch, uint64_t n_rows, uint32_t nq, uint32_t dim,
                                  uint32_t k, int metric, const float *d_mags, const float *d_qmags, uint32_t id_base, int *d_ggm,
                                  uint64_t *d_cand64, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_err32,

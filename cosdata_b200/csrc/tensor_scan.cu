@@ -11,7 +11,8 @@
 //     Rows passing that test are appended to the query's candidate list; the class maxima are
 //     shared between CTAs through global atomicMax.
 // The candidates are then re-scored by rerank_f32_kernel with the reference's exact
-// arithmetic, so the final ids/scores are bit-identical to the exact scan.
+// arithmetic, so the final ids/scores are bit-identical to the exact scan (the s8 form first drops the candidates that
+// fail its filter against the final bound, s8_refilter_kernel).
 //
 // Kernel anatomy (one CTA per SM, 384 threads):
 //   warps 0..7   two consumer warpgroups: wgmma M64 x N256 x K16 on their half of the query tile, accumulators in
@@ -1509,6 +1510,88 @@ cdb_status tensor_scan_device(const void *d_xh, const void *d_qh, uint32_t pitch
     return run_tensor_scan<0>(mq, mx, a, n_rows, d_progress, sm_count, s);
 }
 
+// ------------------------------------------------------------------ s8 form: refilter against the final bound
+// tensor_scan_s8_kernel tests every value against the bound its CTA knew at the time, and that bound only rises during the
+// scan: rows of the early tiles pass against a bound far below the final one.  The test stays sound for any rigorous lower
+// bound of the k-th best exact score, so it is applied once more, after the scan, against the final one (the k-th largest
+// of the query's final class maxima): the value v = q_codes . x_codes (exact in s32, as the MMA computes it) and the
+// threshold thrI(q, T) with the epilogue's arithmetic, rounding for rounding.  The survivors (every row of the exact
+// top-k among them) are compacted to the front of the list and counted in out_cnt; the re-rank gathers their f32 rows
+// only: a candidate costs 768 bytes of s8 row here instead of 3 KB of f32 row there (D = 768).  Shards without degenerate
+// or deleted rows only (no pre-seeded rows, no zero shadow rows), and only the queries whose list did not overflow.
+constexpr int TS8_RF_THREADS = 256;
+
+__global__ void __launch_bounds__(TS8_RF_THREADS) s8_refilter_kernel(
+    const int8_t *__restrict__ xs8, const int8_t *__restrict__ qs8, uint32_t pitch8, uint32_t dim, uint32_t k,
+    const int *__restrict__ ggm, const float2 *__restrict__ tile_se, const float2 *__restrict__ tile_rcp,
+    const float2 *__restrict__ q_se, const float2 *__restrict__ q_rcp, float dn1, float dref, uint32_t id_base,
+    uint32_t *__restrict__ cand, const uint32_t *__restrict__ cand_cnt, uint32_t cap, uint32_t *__restrict__ out_cnt) {
+    __shared__ float s_bound;
+    __shared__ uint32_t s_kept;
+    const uint32_t qi = blockIdx.x;
+    const uint32_t cnt = cand_cnt[qi];
+    if (cnt > cap) {   // the exact scan re-does this query; its list is left as it is
+        if (threadIdx.x == 0) out_cnt[qi] = cap;
+        return;
+    }
+    if (threadIdx.x == 0) {
+        // the bound warp's selection (s8_bound_round) over the final class maxima
+        const int *gq = ggm + (size_t)(qi / TS_BLOCK_M) * TS8_NG * TS_BLOCK_M + qi % TS_BLOCK_M;
+        int v[TS8_NG];
+        for (int c = 0; c < TS8_NG; ++c) v[c] = gq[c * TS_BLOCK_M];
+        int b = INT_MIN;
+        for (int i = 0; i < TS8_NG; ++i) {
+            uint32_t n = 0;
+            for (int c = 0; c < TS8_NG; ++c) n += v[c] >= v[i];
+            b = n >= k ? max(b, v[i]) : b;
+        }
+        s_bound = ord2f(b);
+        s_kept = 0;
+    }
+    __syncthreads();
+    const float bound = s_bound;
+    const float2 qse = q_se[qi], qrc = q_rcp[qi];
+    const float qw = __fadd_ru(dn1, qse.y), qeps = __fmaf_ru(qse.y, dn1, dref);   // qpar.w and qeps of the scan
+    const int8_t *qrow = qs8 + (size_t)qi * pitch8;
+    // an 8-lane group per candidate, 16-byte loads (rows are 16-byte pitched): a round keeps 32 rows in flight per CTA
+    const uint32_t grp = threadIdx.x >> 3, j = threadIdx.x & 7, vecs = dim / 16;
+    for (uint32_t base = 0; base < cnt; base += TS8_RF_THREADS / 8) {
+        const uint32_t ci = base + grp;
+        const uint32_t id = ci < cnt ? cand[(size_t)qi * cap + ci] : CDB_INVALID_ID;
+        __syncthreads();   // every id of this round is read before any survivor is written back
+        const uint64_t row = id != CDB_INVALID_ID ? (uint64_t)(id - id_base) : 0;
+        const int8_t *xrow = xs8 + row * pitch8;
+        int dp = 0;
+        if (id != CDB_INVALID_ID) {
+            for (uint32_t v = j; v < vecs; v += 8) {
+                const int4 x4 = reinterpret_cast<const int4 *>(xrow)[v], q4 = reinterpret_cast<const int4 *>(qrow)[v];
+                dp = __dp4a(x4.x, q4.x, dp);
+                dp = __dp4a(x4.y, q4.y, dp);
+                dp = __dp4a(x4.z, q4.z, dp);
+                dp = __dp4a(x4.w, q4.w, dp);
+            }
+            if (j == 0)
+                for (uint32_t c = vecs * 16; c < dim; ++c) dp += (int)xrow[c] * (int)qrow[c];
+        }
+        // integer sums: exact in any order, the value the MMA accumulated
+        dp += __shfl_xor_sync(0xFFFFFFFFu, dp, 1);
+        dp += __shfl_xor_sync(0xFFFFFFFFu, dp, 2);
+        dp += __shfl_xor_sync(0xFFFFFFFFu, dp, 4);
+        if (j == 0 && id != CDB_INVALID_ID) {
+            const uint64_t nt = row / TS_BLOCK_N;
+            const float2 se = tile_se[nt], rt = tile_rcp[nt];
+            const float eps = __fmaf_ru(qw, se.y, qeps);
+            const float num = __fsub_rd(bound, eps);
+            const bool pos = num >= 0.0f;
+            const int thr = __float2int_rd(__fmul_rd(__fmul_rd(num, pos ? rt.x : rt.y), pos ? qrc.x : qrc.y));
+            if (dp >= thr) cand[(size_t)qi * cap + atomicAdd(&s_kept, 1u)] = id;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) out_cnt[qi] = s_kept;
+}
+
+
 // smallest float >= x
 static float f32_up(double x) {
     float f = (float)x;
@@ -1522,7 +1605,7 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
                                  uint32_t k, const float2 *d_tile_se, const float2 *d_tile_rcp, const float2 *d_q_se,
                                  const float2 *d_q_rcp, uint32_t id_base, int *d_ggm,
                                  uint32_t *d_cand, uint32_t *d_cand_cnt, uint32_t cand_cap, uint32_t *d_progress, bool has_deg,
-                                 int sm_count, cudaStream_t s) {
+                                 int sm_count, cudaStream_t s, uint32_t *d_kept_cnt, bool *refiltered) {
     TensorScanArgs a{};
     a.has_deg = has_deg ? 1u : 0u;
     a.window = 3;
@@ -1561,7 +1644,14 @@ cdb_status tensor_scan_s8_device(const void *d_xs8, const void *d_qs8, uint32_t 
     cdb_status rc;
     if ((rc = make_tensor_map_2d(&mq, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_qs8, (uint64_t)a.mtiles * TS_BLOCK_M, dim, pitch8, TS_BLOCK_M))) return rc;
     if ((rc = make_tensor_map_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, d_xs8, n_rows, dim, pitch8, a.stages ? TS8_HALF : TS_BLOCK_N))) return rc;
-    return run_tensor_scan<2>(mq, mx, a, n_rows, d_progress, sm_count, s);
+    if ((rc = run_tensor_scan<2>(mq, mx, a, n_rows, d_progress, sm_count, s))) return rc;
+    *refiltered = d_kept_cnt && a.stages && !has_deg;
+    if (!*refiltered) return CDB_OK;
+    s8_refilter_kernel<<<nq, TS8_RF_THREADS, 0, s>>>(static_cast<const int8_t *>(d_xs8), static_cast<const int8_t *>(d_qs8), pitch8,
+                                                     dim, k, d_ggm, d_tile_se, d_tile_rcp, d_q_se, d_q_rcp, a.dn1, a.dref, id_base,
+                                                     d_cand, d_cand_cnt, cand_cap, d_kept_cnt);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
 }
 
 // Integer form (tensor_scan_u8.cu): d_x u8 operand rows [n_rows][pitch] (u8 codes or unpacked digits), d_q the query operand
