@@ -228,6 +228,10 @@ PROTOTYPES = {
     "cdb_shard_group_world": (C.c_uint32, [C.c_void_p]),
     "cdb_search_batch_sharded": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cdb_search_batch_sharded_device": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cdb_search_batch_filtered_sharded": (C.c_int32, [C.c_void_p, c_f32p, C.c_uint32, C.POINTER(SearchParams), c_u32p, c_vp, c_u8p, c_u32p,
+                                                      c_f32p, c_u32p, c_u8p]),
+    "cdb_search_batch_filtered_sharded_device": (C.c_int32, [C.c_void_p, c_f32p, C.c_uint32, C.POINTER(SearchParams), c_u32p, c_vp,
+                                                             C.c_uint32, c_u8p, c_u32p, c_f32p, c_u32p, c_u8p, C.c_void_p]),
     "cdb_shard_group_attach_sparse": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "cdb_shard_group_attach_tfidf": (C.c_int32, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "cdb_sparse_search_batch_sharded": (C.c_int32, [C.c_void_p, c_vp, c_vp, c_vp, C.c_uint32, C.POINTER(SparseSearchParams), c_vp, c_vp, c_vp]),

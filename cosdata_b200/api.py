@@ -23,6 +23,7 @@ from ._lib import BuildParams, GraphDesc, GraphMetadata, IndexDesc, SearchParams
 
 INVALID_ID = 0xFFFFFFFF
 SEARCH_TENSOR_WITH_DELETED = 1      # cdb_search_params.flags bit CDB_SEARCH_TENSOR_WITH_DELETED
+SEARCH_ALL_CANDIDATES = 2           # cdb_search_params.flags bit CDB_SEARCH_ALL_CANDIDATES (top_k None; k = the row width)
 
 
 class Status(enum.IntEnum):
@@ -436,18 +437,36 @@ class DenseIndex:
         return int(self._lib.cdb_index_size(self._h))
 
     def params(self, k, mode=SearchMode.BRUTE_RAW, ef_search=256, shortlist_size=64, exact_only=False, prefilter_k=0,
-               tensor_with_deleted=False):
+               tensor_with_deleted=False, all_candidates=False):
         """tensor_with_deleted: brute-force searches may take the tensor-core paths while rows are deleted (the kernels skip
-        them; results are identical, CDB_SEARCH_TENSOR_WITH_DELETED)"""
-        flags = SEARCH_TENSOR_WITH_DELETED if tensor_with_deleted else 0
+        them; results are identical, CDB_SEARCH_TENSOR_WITH_DELETED).  all_candidates: top_k None, k is the row width
+        (CDB_SEARCH_ALL_CANDIDATES)"""
+        flags = (SEARCH_TENSOR_WITH_DELETED if tensor_with_deleted else 0) | (SEARCH_ALL_CANDIDATES if all_candidates else 0)
         return SearchParams(k, int(mode), ef_search, shortlist_size, 1 if exact_only else 0, prefilter_k, flags, 0)
 
+    def hnsw_out_cap(self):
+        """(num_levels + 1) * 100: the most candidates one HNSW search reports per query, the row width of a top_k None search"""
+        info = np.zeros(5, dtype=np.uint32)
+        counts = np.zeros(32, dtype=np.uint32)
+        _check(self._lib.cdb_index_graph_info(self._h, _ptr(info), _ptr(counts)))
+        return (int(info[0]) + 1) * 100
+
+    def _width(self, k, mode):
+        """k=None (top_k None): (row width, True), the width that of the graph (1 for a brute-force mode, which refuses it)"""
+        if k is not None:
+            return k, False
+        return (self.hnsw_out_cap() if int(mode) == SearchMode.HNSW else 1), True
+
     def batch_search(self, queries, k, mode=SearchMode.BRUTE_RAW, **kw):
-        """IndexOps::batch_search -> (ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B])"""
+        """IndexOps::batch_search -> (ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B]).
+        k=None (top_k None, HNSW only): every candidate, best first, in rows of hnsw_out_cap() columns"""
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
             q = q[None]
         b = q.shape[0]
+        k, all_candidates = self._width(k, mode)
+        if all_candidates:
+            kw["all_candidates"] = True
         ids = np.zeros((b, k), dtype=np.uint32)
         scores = np.zeros((b, k), dtype=np.float32)
         counts = np.zeros(b, dtype=np.uint32)
@@ -579,11 +598,14 @@ class DenseIndex:
 
     def batch_search_filtered(self, queries, filters, k, **kw):
         """search_internal with per-query metadata filters: filters[q] is None or a list of int8[md_dims] (QueryFilterDimensions)
-        -> (replica ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B])"""
+        -> (replica ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B]); k=None (top_k None): rows of hnsw_out_cap()"""
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
             q = q[None]
         b = q.shape[0]
+        k, all_candidates = self._width(k, SearchMode.HNSW)
+        if all_candidates:
+            kw["all_candidates"] = True
         offs, dims, has = self.pack_filters(filters)
         if dims.shape[0] == 0:
             dims = np.zeros((1, self.md_dims), dtype=np.int8)

@@ -774,8 +774,28 @@ static cdb_status exact_scan_locked(cdb_index *ix, Scratch *sc, bool raw, int st
     return CDB_OK;
 }
 
+// the most candidates the HNSW traversal reports per query: <= 100 per level (vector_store.rs:273-313)
+static uint32_t hnsw_out_cap(const cdb_index *ix) { return (ix->graph.num_levels + 1) * 100; }
+
+// the re-rank of every candidate holds the query and next_pow2(cap) keys in 200 KB of shared memory
+static cdb_status check_all_dim(const cdb_index *ix) {
+    CDB_REQUIRE(rerank_all_fits(ix->desc.dim, hnsw_out_cap(ix)),
+                "CDB_SEARCH_ALL_CANDIDATES: dimension too large for the re-rank of every candidate (4 * dim + 8 * next_pow2((num_levels + 1) * 100) > 200 KB)");
+    return CDB_OK;
+}
+
+// top_k None: the row width k must hold every candidate and the re-rank must take the dimension (caller holds the handle's
+// lock; nothing to check without the flag)
+static cdb_status check_all_width(const cdb_index *ix, const cdb_search_params *p) {
+    if (!(p->flags & CDB_SEARCH_ALL_CANDIDATES)) return CDB_OK;
+    CDB_REQUIRE(ix->has_graph, "CDB_MODE_HNSW needs cdb_index_set_graph");
+    CDB_REQUIRE(p->k >= hnsw_out_cap(ix), "CDB_SEARCH_ALL_CANDIDATES: k (the row width) must be >= (num_levels + 1) * 100");
+    return check_all_dim(ix);
+}
+
 // search_internal (hnsw/mod.rs:390-440): quantized ann_search on the uploaded graph, then
 // remove_duplicates_and_filter and the exact f32 re-rank of finalize_ann_results.
+// CDB_SEARCH_ALL_CANDIDATES (top_k None): the dedup keeps every candidate instead of 5 * k and all of them are re-ranked.
 static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
                                      uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s,
                                      const uint32_t *d_foff = nullptr, const int8_t *d_fdims = nullptr, uint32_t n_frows = 0,
@@ -794,8 +814,10 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
         set_error("metric/storage arm is an Err in the reference (StorageMismatch / unimplemented)");
         return rc;
     }
-    const uint32_t out_cap = (ix->graph.num_levels + 1) * 100;
-    const uint32_t k5 = 5 * p->k;
+    if ((rc = check_all_width(ix, p))) return rc;
+    const bool all = p->flags & CDB_SEARCH_ALL_CANDIDATES;
+    const uint32_t out_cap = hnsw_out_cap(ix);
+    const uint32_t k5 = all ? out_cap : 5 * p->k;   // candidate slots per query after the dedup
     const uint32_t rpitch = ix->raw_pitch_elems * 4;
     if ((rc = sc->q_codes.ensure((size_t)nq * ix->row_pitch)) || (rc = sc->q_mags.ensure((size_t)nq * 4)) ||
         (rc = sc->qraw.ensure((size_t)nq * rpitch)) || (rc = sc->qraw_mags.ensure((size_t)nq * 4)) ||
@@ -860,7 +882,13 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
         if ((rc = hnsw_dedup_device(ma.out_ids, a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, HN_ROOT_ID, d.id_base, k5, nq,
                                     sc->cand.as<uint32_t>(), sc->hn_labels.as<uint32_t>(), sc->cand_cnt.as<uint32_t>(), s)))
             return rc;
-        if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
+        if (all) {
+            if ((rc = rerank_all_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
+                                            ix->raw_pitch_elems, sc->qraw_mags.as<float>(), nq, sc->cand.as<uint32_t>(),
+                                            sc->cand_cnt.as<uint32_t>(), k5, p->k, d.id_base, d_ids, d_scores, d_counts, s,
+                                            sc->hn_labels.as<uint32_t>(), sc->cur_keys)))
+                return rc;
+        } else if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
                                     ix->raw_pitch_elems, sc->qraw_mags.as<float>(), nq, sc->cand.as<uint32_t>(),
                                     sc->cand_cnt.as<uint32_t>(), k5, p->k, d.id_base, d_ids, d_scores, d_counts, s,
                                     sc->hn_labels.as<uint32_t>(), sc->cur_keys)))
@@ -873,7 +901,13 @@ static cdb_status hnsw_search_locked(cdb_index *ix, Scratch *sc, const float *d_
         if ((rc = hnsw_dedup_device(nullptr, a.out_rows, a.out_scores, a.out_n, out_cap, d.metric, ix->graph.root_row, d.id_base, k5,
                                     nq, sc->cand.as<uint32_t>(), nullptr, sc->cand_cnt.as<uint32_t>(), s)))
             return rc;
-        if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
+        if (all) {
+            if ((rc = rerank_all_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
+                                            ix->raw_pitch_elems, sc->qraw_mags.as<float>(), nq, sc->cand.as<uint32_t>(),
+                                            sc->cand_cnt.as<uint32_t>(), k5, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr,
+                                            sc->cur_keys)))
+                return rc;
+        } else if ((rc = rerank_f32_device(ix->d_raw, ix->raw_pitch_elems, ix->d_raw_mags, ix->size, d.dim, sc->qraw.as<float>(),
                                     ix->raw_pitch_elems, sc->qraw_mags.as<float>(), nq, sc->cand.as<uint32_t>(),
                                     sc->cand_cnt.as<uint32_t>(), k5, p->k, d.id_base, d_ids, d_scores, d_counts, s, nullptr,
                                     sc->cur_keys)))
@@ -906,7 +940,7 @@ static bool use_s8_form(const cdb_index *ix, uint32_t nq) {
 static cdb_status search_chunk_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
                                       uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s) {
     const cdb_index_desc &d = ix->desc;
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
     if (nq == 0) return CDB_OK;
     cdb_status rc;
     if (p->mode == CDB_MODE_HNSW) return hnsw_search_locked(ix, sc, d_queries, nq, p, d_ids, d_scores, d_counts, d_err, s);
@@ -1074,21 +1108,45 @@ static cdb_status search_device_locked(cdb_index *ix, Scratch *sc, const float *
 }
 
 }  // extern "C"
+static cdb_status filtered_device_locked(cdb_index *ix, Scratch *sc, const float *d_queries, uint32_t nq, const cdb_search_params *p,
+                                         const uint32_t *d_off, const int8_t *d_dims, uint32_t n_rows, const uint8_t *d_has,
+                                         uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s);
 namespace cdb {
-// shard_group.cu: search one shard with device buffers on `s`; d_keys ([nq][k], may be null) receives the packed keys
+// shard_group.cu: search one shard with device buffers on `s`; d_keys ([nq][k], may be null) receives the packed keys.
+// With f (the filter CSR on the shard's device, its offsets and has-flags starting at this batch's first query) the shard
+// runs cdb_search_batch_filtered_device's search.
 cdb_status index_search_device_keys(cdb_index *ix, const float *d_queries, uint32_t nq, const cdb_search_params *p, uint32_t *d_ids,
-                                    float *d_scores, uint32_t *d_counts, uint8_t *d_err, uint64_t *d_keys, cudaStream_t s) {
+                                    float *d_scores, uint32_t *d_counts, uint8_t *d_err, uint64_t *d_keys, cudaStream_t s,
+                                    const ShardFilters *f) {
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
+    if (cdb_status kc = check_all_width(ix, p)) return kc;
+    if (f) CDB_REQUIRE(ix->has_md, "metadata filters need cdb_index_set_graph_metadata");
     Lease l;
     cdb_status rc = lease_scratch(ix, l);
     if (rc) return rc;
     Scratch *sc = l.sc;
     sc->keys_out = d_keys;
-    rc = search_device_locked(ix, sc, d_queries, nq, p, d_ids, d_scores, d_counts, d_err, s ? s : sc->stream);
+    if (f)
+        rc = filtered_device_locked(ix, sc, d_queries, nq, p, f->off, f->dims, f->n_rows, f->has, d_ids, d_scores, d_counts, d_err,
+                                    s ? s : sc->stream);
+    else
+        rc = search_device_locked(ix, sc, d_queries, nq, p, d_ids, d_scores, d_counts, d_err, s ? s : sc->stream);
     sc->keys_out = sc->cur_keys = nullptr;
     return rc;
+}
+// a shard group's top_k None check of one shard (before any copy): its candidates fit the rank's w columns, its re-rank fits
+cdb_status index_check_all_width(cdb_index *ix, uint32_t w) {
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->has_graph, "CDB_MODE_HNSW needs cdb_index_set_graph");
+    CDB_REQUIRE(hnsw_out_cap(ix) <= w, "CDB_SEARCH_ALL_CANDIDATES: every shard's (num_levels + 1) * 100 must be <= k / world");
+    return check_all_dim(ix);
+}
+// md_dims of the shard's graph metadata, 0 without metadata
+uint32_t index_md_dims(cdb_index *ix) {
+    std::shared_lock<std::shared_mutex> lock(ix->rw);
+    return ix->has_md ? ix->md_dims : 0;
 }
 int index_device(const cdb_index *ix) { return ix->desc.device; }
 uint32_t index_dim(const cdb_index *ix) { return ix->desc.dim; }
@@ -1109,6 +1167,10 @@ cdb_status cdb_search_batch_device(cdb_index *ix, const float *d_queries, uint32
     CDB_REQUIRE(ix && p && (d_queries || !nq) && (d_ids || !nq) && (d_scores || !nq), "null argument");
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    if (nq) {
+        if (cdb_status kc = check_search_k(p)) return kc;
+        if (cdb_status kc = check_all_width(ix, p)) return kc;
+    }
     Lease l;
     cdb_status rc = lease_scratch(ix, l);
     if (rc) return rc;
@@ -1129,7 +1191,8 @@ cdb_status cdb_search_batch(cdb_index *ix, const float *queries, uint32_t nq, co
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     if (!nq) return CDB_OK;
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
+    if (cdb_status kc = check_all_width(ix, p)) return kc;
     Lease l;
     cdb_status rc = lease_scratch(ix, l);
     if (rc) return rc;
@@ -1162,6 +1225,7 @@ static cdb_status filtered_device_locked(cdb_index *ix, Scratch *sc, const float
     const uint32_t CH = 2048;
     for (uint32_t q0 = 0; q0 < nq; q0 += CH) {
         const uint32_t m = std::min(CH, nq - q0);
+        sc->cur_keys = sc->keys_out ? sc->keys_out + (size_t)q0 * p->k : nullptr;
         const cdb_status rc = hnsw_search_locked(ix, sc, d_queries + (size_t)q0 * ix->desc.dim, m, p, d_ids + (size_t)q0 * p->k,
                                                  d_scores + (size_t)q0 * p->k, d_counts + q0, d_err ? d_err + q0 : nullptr, s,
                                                  d_off ? d_off + q0 : nullptr, d_dims, n_rows, d_has ? d_has + q0 : nullptr);
@@ -1181,8 +1245,9 @@ cdb_status cdb_search_batch_filtered(cdb_index *ix, const float *queries, uint32
     std::shared_lock<std::shared_mutex> lock(ix->rw);
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     if (!nq) return CDB_OK;
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
     CDB_REQUIRE(ix->has_md, "metadata filters need cdb_index_set_graph_metadata");
+    if (cdb_status kc = check_all_width(ix, p)) return kc;
     Lease l;
     cdb_status rc = lease_scratch(ix, l);
     if (rc) return rc;
@@ -1230,7 +1295,7 @@ cdb_status cdb_search_batch_filtered_device(cdb_index *ix, const float *d_querie
                                             uint8_t *d_err, void *stream) {
     CDB_REQUIRE(p, "null params");
     CDB_REQUIRE(p->mode == CDB_MODE_HNSW, "metadata filters apply to CDB_MODE_HNSW");
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
     CDB_REQUIRE(!d_has_filter || d_filter_offsets, "has_filter needs filter_offsets");
     CDB_REQUIRE(d_filter_dims || !n_filter_rows, "n_filter_rows > 0 needs filter_dims");
     CDB_REQUIRE(ix && (d_queries || !nq) && (d_ids || !nq) && (d_scores || !nq), "null argument");
@@ -1238,6 +1303,7 @@ cdb_status cdb_search_batch_filtered_device(cdb_index *ix, const float *d_querie
     CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
     CDB_REQUIRE(ix->has_md || !d_has_filter, "metadata filters need cdb_index_set_graph_metadata");
     if (!nq) return CDB_OK;
+    if (cdb_status kc = check_all_width(ix, p)) return kc;
     Lease l;
     cdb_status rc = lease_scratch(ix, l);
     if (rc) return rc;

@@ -127,6 +127,9 @@ cdb_status make_plan(const cdb_hybrid_sources *h, uint32_t nq, uint32_t top_k, P
     CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
     const int n_src = (h->dense != nullptr) + (h->sparse != nullptr) + (h->tfidf != nullptr);
     CDB_REQUIRE(n_src == 2, "a hybrid search takes exactly two sources");
+    // the reference's dense sub-search always has Some(3 * top_k): top_k None has no hybrid form
+    CDB_REQUIRE(!h->dense || !(h->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
+                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
     const uint32_t k3 = 3 * top_k;
     int i = 0;
     if (h->dense) { p->src[i] = SRC_DENSE; p->ld[i++] = k3; }

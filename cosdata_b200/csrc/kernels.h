@@ -7,6 +7,25 @@
 
 namespace cdb {
 
+// k of a dense search: 1..1024, or under CDB_SEARCH_ALL_CANDIDATES (top_k None, HNSW only) the output row width, which is
+// checked against the graph once the handle is locked
+inline cdb_status check_search_k(const cdb_search_params *p) {
+    if (p->flags & CDB_SEARCH_ALL_CANDIDATES) {
+        CDB_REQUIRE(p->mode == CDB_MODE_HNSW, "CDB_SEARCH_ALL_CANDIDATES (top_k None) applies to CDB_MODE_HNSW");
+        return CDB_OK;
+    }
+    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    return CDB_OK;
+}
+
+// metadata filters of a batch in device memory, the arguments of cdb_search_batch_filtered_device (a shard group's filtered search)
+struct ShardFilters {
+    const uint32_t *off;   // [n_queries + 1], may be null when has is
+    const int8_t *dims;    // [n_rows][md_dims]
+    uint32_t n_rows;
+    const uint8_t *has;    // [n_queries], null: no query has a filter
+};
+
 // ---- quantize.cu
 cdb_status quantize_rows_device(const float *d_vecs, uint64_t n, uint32_t dim, int st, float lo, float hi,
                                 uint8_t *d_codes, uint32_t row_pitch, float *d_mags, float *d_raw,
@@ -68,6 +87,17 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
                              bool dedup = true);                    // report a repeated candidate once (<= 64 repeats)
 // largest dimension rerank_f32_device accepts for any candidate count (its query and key buffer share 200 KB of smem)
 uint32_t rerank_f32_max_dim();
+// the same re-rank without truncation (top_k None): every one of the <= ncand candidates of a query is scored and sorted in
+// one CTA, ncand <= RERANK_ALL_MAX_CAND; row b of the outputs is `width` wide, the first d_out_counts[b] entries best first.
+// Query and keys share 200 KB of smem: dim <= (200 KB - 8 * next_pow2(ncand)) / 4, i.e. 43008 at 4096 slots.
+constexpr uint32_t RERANK_ALL_MAX_CAND = 4096;
+// whether rerank_all_f32_device takes this dimension and candidate count (checked before a top_k None search is enqueued)
+bool rerank_all_fits(uint32_t dim, uint32_t ncand);
+cdb_status rerank_all_f32_device(const float *d_raw, uint32_t pitch_elems, const float *d_raw_mags, uint64_t n_rows, uint32_t dim,
+                                 const float *d_q, uint32_t q_pitch_elems, const float *d_qmags, uint32_t nq, const uint32_t *d_cand,
+                                 const uint32_t *d_cand_counts, uint32_t ncand, uint32_t width, uint32_t id_base, uint32_t *d_out_ids,
+                                 float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s, const uint32_t *d_labels = nullptr,
+                                 uint64_t *d_out_keys = nullptr);
 
 // ---- scan.cu
 struct ScanArgs {

@@ -213,4 +213,82 @@ cdb_status rerank_f32_device(const float *d_raw, uint32_t pitch_elems, const flo
     return CDB_OK;
 }
 
+// finalize_ann_results with top_k None: every candidate of the query is scored and the whole list is sorted and returned
+// (vector_store.rs:404-445 without the truncation).  One CTA per query holds all of its keys at once, so the list is bounded
+// by the HNSW output, (num_levels + 1) * 100 <= 3200 candidates; the arithmetic, the key and the order are those of
+// rerank_f32_kernel.  The candidates' keys are unique (hnsw_dedup_kernel removed repeated ids), so nothing is deduplicated.
+// Row q of the outputs has `width` columns: the counts[q] sorted results, then CDB_INVALID_ID / 0 (keys 0).
+constexpr int RERANK_ALL_THREADS = 512;
+
+__global__ void __launch_bounds__(RERANK_ALL_THREADS) rerank_all_f32_kernel(
+    const float *__restrict__ raw, uint32_t pitch_elems, const float *__restrict__ raw_mags, uint64_t n_rows,
+    uint32_t dim, const float *__restrict__ q, uint32_t q_pitch_elems, const float *__restrict__ qmags,
+    const uint32_t *__restrict__ cand, const uint32_t *__restrict__ cand_counts, uint32_t cand_stride, uint32_t width,
+    uint32_t id_base, uint32_t *__restrict__ out_ids, float *__restrict__ out_scores, uint32_t *__restrict__ out_counts,
+    const uint32_t *__restrict__ labels, uint64_t *__restrict__ out_keys) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    float *qs = reinterpret_cast<float *>(smem);
+    uint64_t *keys = reinterpret_cast<uint64_t *>(qs + round_up(dim, 4));
+    __shared__ int nvalid;
+    const uint32_t b = blockIdx.x;
+    const uint32_t ncand = min(cand_counts[b], cand_stride);
+    for (uint32_t c = threadIdx.x; c < dim; c += blockDim.x) qs[c] = q[(size_t)b * q_pitch_elems + c];
+    if (threadIdx.x == 0) nvalid = 0;
+    __syncthreads();
+    const float mag_q = qmags[b];
+    const int j = threadIdx.x & 7, grp = threadIdx.x >> 3;
+    const uint32_t rounds = (ncand + RERANK_ALL_THREADS / 8 - 1) / (RERANK_ALL_THREADS / 8);
+    for (uint32_t r = 0; r < rounds; ++r) {
+        const uint32_t ci = r * (RERANK_ALL_THREADS / 8) + grp;
+        const uint32_t id = ci < ncand ? cand[(size_t)b * cand_stride + ci] : CDB_INVALID_ID;
+        const bool ok = id != CDB_INVALID_ID && id >= id_base && (uint64_t)(id - id_base) < n_rows;
+        const uint64_t rowi = ok ? (uint64_t)(id - id_base) : 0;
+        const float dp = dot_f32_avx_order_8t(qs, raw + rowi * pitch_elems, dim, j);   // all lanes take part in the shuffles
+        if (j == 0 && ci < ncand) {
+            uint64_t key = 0;
+            if (ok) {
+                const float cs = canon_nan(__fdiv_rn(dp, __fmul_rn(mag_q, raw_mags[rowi])));
+                key = make_key64(order_key(CDB_METRIC_COSINE, __float_as_uint(cs)), labels ? labels[(size_t)b * cand_stride + ci] : id);
+                atomicAdd(&nvalid, 1);
+            }
+            keys[ci] = key;
+        }
+    }
+    __syncthreads();
+    rerank_sort_desc(keys, ncand);   // zero (empty) keys sort last
+    const uint32_t nout = min((uint32_t)nvalid, width);
+    for (uint32_t i = threadIdx.x; i < width; i += blockDim.x) {
+        const uint64_t key = i < nout ? keys[i] : 0ull;
+        out_ids[(size_t)b * width + i] = key ? key64_id(key) : CDB_INVALID_ID;
+        out_scores[(size_t)b * width + i] = key ? __uint_as_float(key_to_bits(CDB_METRIC_COSINE, (uint32_t)(key >> 32))) : 0.0f;
+        if (out_keys) out_keys[(size_t)b * width + i] = key;
+    }
+    if (threadIdx.x == 0 && out_counts) out_counts[b] = nout;
+}
+
+bool rerank_all_fits(uint32_t dim, uint32_t ncand) {
+    uint32_t P = 1;
+    while (P < ncand) P <<= 1;
+    return ncand <= RERANK_ALL_MAX_CAND && (size_t)round_up(dim, 4) * 4 + (size_t)P * 8 <= 200 * 1024;
+}
+
+cdb_status rerank_all_f32_device(const float *d_raw, uint32_t pitch_elems, const float *d_raw_mags, uint64_t n_rows, uint32_t dim,
+                                 const float *d_q, uint32_t q_pitch_elems, const float *d_qmags, uint32_t nq, const uint32_t *d_cand,
+                                 const uint32_t *d_cand_counts, uint32_t ncand, uint32_t width, uint32_t id_base, uint32_t *d_out_ids,
+                                 float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s, const uint32_t *d_labels,
+                                 uint64_t *d_out_keys) {
+    if (!nq) return CDB_OK;
+    if (ncand == 0 || ncand > RERANK_ALL_MAX_CAND) { set_error("rerank: 1..4096 candidate slots per query"); return CDB_INVALID_PARAMS; }
+    if (!rerank_all_fits(dim, ncand)) { set_error("rerank: dimension too large"); return CDB_INVALID_PARAMS; }
+    uint32_t P = 1;
+    while (P < ncand) P <<= 1;
+    const size_t smem = (size_t)round_up(dim, 4) * 4 + (size_t)P * 8;
+    CDB_ALLOW_SMEM(rerank_all_f32_kernel, smem);
+    rerank_all_f32_kernel<<<nq, RERANK_ALL_THREADS, smem, s>>>(d_raw, pitch_elems, d_raw_mags, n_rows, dim, d_q, q_pitch_elems, d_qmags,
+                                                               d_cand, d_cand_counts, ncand, width, id_base, d_out_ids, d_out_scores,
+                                                               d_out_counts, d_labels, d_out_keys);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
 }  // namespace cdb

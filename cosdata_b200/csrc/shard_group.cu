@@ -28,7 +28,10 @@
 struct cdb_index;
 namespace cdb {
 cdb_status index_search_device_keys(cdb_index *ix, const float *d_queries, uint32_t nq, const cdb_search_params *p, uint32_t *d_ids,
-                                    float *d_scores, uint32_t *d_counts, uint8_t *d_err, uint64_t *d_keys, cudaStream_t s);
+                                    float *d_scores, uint32_t *d_counts, uint8_t *d_err, uint64_t *d_keys, cudaStream_t s,
+                                    const ShardFilters *f);
+cdb_status index_check_all_width(cdb_index *ix, uint32_t w);
+uint32_t index_md_dims(cdb_index *ix);
 int index_device(const cdb_index *ix);
 uint32_t index_dim(const cdb_index *ix);
 int index_metric(const cdb_index *ix);
@@ -167,6 +170,51 @@ __global__ void merge_gathered_kernel(const uint64_t *__restrict__ gathered, uin
             for (uint32_t r = 0; r < world; ++r) e |= reinterpret_cast<const uint8_t *>(gathered + (size_t)r * words + (size_t)nq * k)[q];
             err[q] = e;
         }
+    }
+}
+
+// top_k None: one CTA per query merges `world` runs of w keys (each sorted descending, zero padded) into one sorted row of
+// W = world * w columns.  An entry's position is its index in its run plus, for every other run, the number of that run's
+// keys greater than it (binary search over all w slots: a zero key is never greater), so neither the run length nor the
+// world size has a shared-memory bound.  The row is filled with CDB_INVALID_ID / 0 first: keys are unique (the shards' id
+// ranges, and their replica ids, are disjoint), so the counts[q] = the number of non-zero keys land on [0, counts[q]), and a
+// violated precondition leaves empty slots rather than stale ones.  Error bytes OR-ed over the ranks.
+__global__ void merge_runs_kernel(const uint64_t *__restrict__ gathered, uint32_t world, uint32_t nq, uint32_t w, size_t words,
+                                  int metric, uint32_t *__restrict__ ids, float *__restrict__ scores, uint32_t *__restrict__ counts,
+                                  uint8_t *__restrict__ err) {
+    __shared__ uint32_t total;
+    const uint32_t q = blockIdx.x, W = world * w;
+    auto run = [&](uint32_t r) { return gathered + (size_t)r * words + (size_t)q * w; };
+    if (threadIdx.x == 0) total = 0;
+    for (uint32_t o = threadIdx.x; o < W; o += blockDim.x) { ids[(size_t)q * W + o] = CDB_INVALID_ID; scores[(size_t)q * W + o] = 0.0f; }
+    __syncthreads();
+    uint32_t mine = 0;
+    for (uint32_t i = threadIdx.x; i < W; i += blockDim.x) {
+        const uint32_t r = i / w, j = i - r * w;
+        const uint64_t key = run(r)[j];
+        if (!key) continue;
+        ++mine;
+        uint32_t pos = j;
+        for (uint32_t o = 0; o < world; ++o) {
+            if (o == r) continue;
+            const uint64_t *R = run(o);
+            uint32_t lo = 0, hi = w;   // keys of run o greater than `key`
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (R[mid] > key) lo = mid + 1; else hi = mid;
+            }
+            pos += lo;
+        }
+        ids[(size_t)q * W + pos] = key64_id(key);
+        scores[(size_t)q * W + pos] = __uint_as_float(key_to_bits(metric, (uint32_t)(key >> 32)));
+    }
+    if (mine) atomicAdd(&total, mine);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint8_t e = 0;
+        for (uint32_t r = 0; r < world; ++r) e |= reinterpret_cast<const uint8_t *>(gathered + (size_t)r * words + (size_t)nq * w)[q];
+        if (counts) counts[q] = total;
+        if (err) err[q] = e;
     }
 }
 }  // namespace
@@ -376,54 +424,126 @@ static cdb_status group_allgather(cdb_shard_group *g, size_t words, cudaStream_t
 // shared memory of merge_gathered_kernel: the world * k keys of one query
 constexpr size_t MERGE_SMEM_MAX = 200 * 1024;
 
-// both forms refuse a merge that cannot run before any copy or search is issued
-static cdb_status merge_check(const cdb_shard_group *g, uint32_t k) {
-    CDB_REQUIRE((size_t)g->world * k * 8 <= MERGE_SMEM_MAX, "sharded merge: world * k * 8 bytes exceed 200 KB");
+// both forms refuse a merge that cannot run before any copy or search is issued; top_k None (merge_runs_kernel, no shared
+// memory bound) splits the row width W = k evenly over the ranks
+static cdb_status merge_check(const cdb_shard_group *g, const cdb_search_params *p) {
+    if (p->flags & CDB_SEARCH_ALL_CANDIDATES) {
+        CDB_REQUIRE(p->k % g->world == 0, "CDB_SEARCH_ALL_CANDIDATES: k (the row width) must be a multiple of the world size");
+        return CDB_OK;
+    }
+    CDB_REQUIRE((size_t)g->world * p->k * 8 <= MERGE_SMEM_MAX, "sharded merge: world * k * 8 bytes exceed 200 KB");
     return CDB_OK;
 }
 
-// local slot i: search its shard into its slot of its gather buffer, then the collective, then (slot 0 / this rank) the merge
-static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_search_params *p, const std::vector<const float *> &d_q,
-                                  uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
-    const size_t nl = g->dev.size();
-    const uint32_t k = p->k;
-    const size_t words = slot_words(nq, k);
-    cdb_status rc;
-    for (size_t i = 0; i < nl; ++i) {
+// checks that need the shards, under the group's lock and before any copy: every slot has a shard; top_k None: every local
+// shard's candidates fit its rank's k / world columns; filtered: every local shard has graph metadata of one md_dims
+// (metadata may be attached after cdb_shard_group_attach), returned in *md_dims
+static cdb_status shards_check(const cdb_shard_group *g, const cdb_search_params *p, bool filtered, uint32_t *md_dims) {
+    for (size_t i = 0; i < g->dev.size(); ++i) {
         CDB_REQUIRE(g->shard[i], "a group slot has no shard attached");
+        cdb_status rc;
+        if ((p->flags & CDB_SEARCH_ALL_CANDIDATES) && (rc = index_check_all_width(g->shard[i], p->k / g->world))) return rc;
+        if (filtered) {
+            const uint32_t d = index_md_dims(g->shard[i]);
+            CDB_REQUIRE(d, "metadata filters need cdb_index_set_graph_metadata on every shard");
+            CDB_REQUIRE(i == 0 || d == *md_dims, "shards differ in md_dims");
+            *md_dims = d;
+        }
+    }
+    return CDB_OK;
+}
+
+constexpr size_t GROUP_GATHER_BUDGET = 256ull << 20;   // bytes of one chunk's gather buffer; queries are searched in chunks
+
+// queries per chunk when a query takes `per_q` bytes of every rank's gather slot
+static uint32_t group_chunk(const cdb_shard_group *g, uint32_t nq, size_t per_q) {
+    return (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, GROUP_GATHER_BUDGET / (g->world * per_q)}));
+}
+
+// loopback: a chunk's slots write their gather buffers only after slot 0 copied the previous chunk's out of them
+static cdb_status loopback_fence(cdb_shard_group *g) {
+    if (!g->loopback) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    CDB_CUDA_TRY(cudaEventRecord(g->ev[0], g->stream[0]));
+    for (size_t i = 1; i < g->dev.size(); ++i) CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[i], g->ev[0], 0));
+    return CDB_OK;
+}
+
+// local slot i: search its shard into its slot of its gather buffer, then the collective, then (slot 0 / this rank) the merge.
+// flt (may be null): slot i's filter CSR on its device.  With k <= 1024 the whole batch is one chunk and merge_gathered_kernel
+// keeps the best k; under CDB_SEARCH_ALL_CANDIDATES each rank writes its sorted list into w = k / world columns, the batch is
+// searched in chunks whose gather buffer stays within GROUP_GATHER_BUDGET, and merge_runs_kernel concatenates the runs in
+// order.  Each shard's reader lock is held while its search is enqueued.
+static cdb_status sharded_enqueue(cdb_shard_group *g, uint32_t nq, const cdb_search_params *p, const std::vector<const float *> &d_q,
+                                  const std::vector<ShardFilters> *flt, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                  uint8_t *d_err, cudaStream_t out_stream) {
+    const size_t nl = g->dev.size();
+    const bool all = p->flags & CDB_SEARCH_ALL_CANDIDATES;
+    const uint32_t W = p->k, k = all ? W / g->world : W;   // output columns; columns of one rank's slot
+    const uint32_t chunk = all ? group_chunk(g, nq, (size_t)k * 8 + 1) : nq;
+    cdb_search_params sp = *p;
+    sp.k = k;
+    cdb_status rc;
+    for (size_t i = 0; i < nl; ++i) CDB_REQUIRE(g->shard[i], "a group slot has no shard attached");
+    const uint32_t dim = index_dim(g->shard[0]);
+    for (size_t i = 0; i < nl; ++i) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->gather[i].ensure(g->world * words * 8)) || (rc = g->ids[i].ensure((size_t)nq * k * 4)) ||
-            (rc = g->scores[i].ensure((size_t)nq * k * 4)) || (rc = g->counts[i].ensure((size_t)nq * 4)))
-            return rc;
-        uint64_t *slot = reinterpret_cast<uint64_t *>(g->gather[i].p) + (size_t)(g->rank0 + i) * words;
-        cudaStream_t s = (nl == 1 && out_stream) ? out_stream : g->stream[i];
-        if ((rc = index_search_device_keys(g->shard[i], d_q[i], nq, p, reinterpret_cast<uint32_t *>(g->ids[i].p),
-                                           reinterpret_cast<float *>(g->scores[i].p), reinterpret_cast<uint32_t *>(g->counts[i].p),
-                                           reinterpret_cast<uint8_t *>(slot + (size_t)nq * k), slot, s)))
+        if ((rc = g->gather[i].ensure(g->world * slot_words(chunk, k) * 8)) || (rc = g->ids[i].ensure((size_t)chunk * k * 4)) ||
+            (rc = g->scores[i].ensure((size_t)chunk * k * 4)) || (rc = g->counts[i].ensure((size_t)chunk * 4)))
             return rc;
     }
-    if ((rc = group_allgather(g, words, out_stream))) return rc;
-    // merge on local slot 0
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    cudaStream_t s0 = (nl == 1 && out_stream) ? out_stream : g->stream[0];
-    const size_t smem = (size_t)g->world * k * 8;
-    CDB_ALLOW_SMEM(merge_gathered_kernel, smem);
-    merge_gathered_kernel<<<nq, 128, smem, s0>>>(reinterpret_cast<const uint64_t *>(g->gather[0].p), g->world, nq, k, words,
-                                                  index_result_metric(g->shard[0], p->mode), d_ids, d_scores, d_counts, d_err);
-    CDB_LAUNCH_CHECK();
+    const int metric = index_result_metric(g->shard[0], p->mode);
+    for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        const size_t words = slot_words(c, k);
+        if (q0 && (rc = loopback_fence(g))) return rc;
+        for (size_t i = 0; i < nl; ++i) {
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+            uint64_t *slot = reinterpret_cast<uint64_t *>(g->gather[i].p) + (size_t)(g->rank0 + i) * words;
+            ShardFilters f{};
+            if (flt) {
+                const ShardFilters &a = (*flt)[i];
+                f = {a.off ? a.off + q0 : nullptr, a.dims, a.n_rows, a.has ? a.has + q0 : nullptr};
+            }
+            if ((rc = index_search_device_keys(g->shard[i], d_q[i] + (size_t)q0 * dim, c, &sp, reinterpret_cast<uint32_t *>(g->ids[i].p),
+                                               reinterpret_cast<float *>(g->scores[i].p), reinterpret_cast<uint32_t *>(g->counts[i].p),
+                                               reinterpret_cast<uint8_t *>(slot + (size_t)c * k), slot, slot_stream(g, i, out_stream),
+                                               flt ? &f : nullptr)))
+                return rc;
+        }
+        if ((rc = group_allgather(g, words, out_stream))) return rc;
+        // merge on local slot 0
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        const cudaStream_t s0 = slot_stream(g, 0, out_stream);
+        const uint64_t *gathered = reinterpret_cast<const uint64_t *>(g->gather[0].p);
+        uint32_t *o_ids = d_ids + (size_t)q0 * W;
+        float *o_scores = d_scores + (size_t)q0 * W;
+        uint32_t *o_counts = d_counts ? d_counts + q0 : nullptr;
+        uint8_t *o_err = d_err ? d_err + q0 : nullptr;
+        if (all) {
+            merge_runs_kernel<<<c, 256, 0, s0>>>(gathered, g->world, c, k, words, metric, o_ids, o_scores, o_counts, o_err);
+        } else {
+            const size_t smem = (size_t)g->world * k * 8;
+            CDB_ALLOW_SMEM(merge_gathered_kernel, smem);
+            merge_gathered_kernel<<<c, 128, smem, s0>>>(gathered, g->world, c, k, words, metric, o_ids, o_scores, o_counts, o_err);
+        }
+        CDB_LAUNCH_CHECK();
+    }
     return CDB_OK;
 }
 
 cdb_status cdb_search_batch_sharded(cdb_shard_group *g, const float *queries, uint32_t nq, const cdb_search_params *p,
                                     uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
     CDB_REQUIRE(g && p && (queries || !nq) && (out_ids || !nq) && (out_scores || !nq), "null argument");
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
     if (!nq) return CDB_OK;
-    cdb_status rc = merge_check(g, p->k);
+    cdb_status rc = merge_check(g, p);
     if (rc) return rc;
     std::lock_guard<std::mutex> lock(g->mu);
     const size_t nl = g->dev.size();
     CDB_REQUIRE(g->shard[0], "a group slot has no shard attached");
+    uint32_t md_dims = 0;
+    if ((p->flags & CDB_SEARCH_ALL_CANDIDATES) && (rc = shards_check(g, p, false, &md_dims))) return rc;
     const uint32_t dim = index_dim(g->shard[0]);
     const size_t nk = (size_t)nq * p->k;
     std::vector<const float *> d_q(nl);
@@ -441,7 +561,7 @@ cdb_status cdb_search_batch_sharded(cdb_shard_group *g, const float *queries, ui
     float *f_scores = reinterpret_cast<float *>(f_ids + nk);
     uint32_t *f_counts = reinterpret_cast<uint32_t *>(f_scores + nk);
     uint8_t *f_err = reinterpret_cast<uint8_t *>(f_counts + nq);
-    if ((rc = sharded_enqueue(g, nq, p, d_q, f_ids, f_scores, f_counts, f_err, nullptr))) return rc;
+    if ((rc = sharded_enqueue(g, nq, p, d_q, nullptr, f_ids, f_scores, f_counts, f_err, nullptr))) return rc;
     CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
     cudaStream_t s0 = g->stream[0];
     CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, s0));
@@ -460,31 +580,111 @@ cdb_status cdb_search_batch_sharded_device(cdb_shard_group *g, const float *d_qu
                                            void *stream) {
     CDB_REQUIRE(g && p && (d_queries || !nq) && (d_out_ids || !nq) && (d_out_scores || !nq), "null argument");
     CDB_REQUIRE(g->dev.size() == 1, "the device form serves one-process-per-GPU groups (cdb_shard_group_create_rank)");
-    CDB_REQUIRE(p->k >= 1 && p->k <= 1024, "k must be in 1..1024");
+    if (cdb_status kc = check_search_k(p)) return kc;
     if (!nq) return CDB_OK;
-    cdb_status rc = merge_check(g, p->k);
+    cdb_status rc = merge_check(g, p);
     if (rc) return rc;
     std::lock_guard<std::mutex> lock(g->mu);
+    uint32_t md_dims = 0;
+    if ((p->flags & CDB_SEARCH_ALL_CANDIDATES) && (rc = shards_check(g, p, false, &md_dims))) return rc;
     std::vector<const float *> d_q(1, d_queries);
-    return sharded_enqueue(g, nq, p, d_q, d_out_ids, d_out_scores, d_out_counts, d_err_flags, (cudaStream_t)stream);
+    return sharded_enqueue(g, nq, p, d_q, nullptr, d_out_ids, d_out_scores, d_out_counts, d_err_flags, (cudaStream_t)stream);
+}
+
+// the refusals of cdb_search_batch_filtered[_device] that need no handle, in their order
+static cdb_status filtered_params_check(const cdb_search_params *p, const void *offsets, const void *has) {
+    CDB_REQUIRE(p->mode == CDB_MODE_HNSW, "metadata filters apply to CDB_MODE_HNSW");
+    if (cdb_status kc = check_search_k(p)) return kc;
+    CDB_REQUIRE(!has || offsets, "has_filter needs filter_offsets");
+    return CDB_OK;
+}
+
+cdb_status cdb_search_batch_filtered_sharded(cdb_shard_group *g, const float *queries, uint32_t nq, const cdb_search_params *p,
+                                             const uint32_t *filter_offsets, const int8_t *filter_dims, const uint8_t *has_filter,
+                                             uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
+    CDB_REQUIRE(g && p && (queries || !nq) && (out_ids || !nq) && (out_scores || !nq), "null argument");
+    cdb_status rc = filtered_params_check(p, filter_offsets, has_filter);
+    if (rc) return rc;
+    if (!nq) return CDB_OK;
+    if ((rc = merge_check(g, p))) return rc;
+    uint32_t total = 0;
+    if (has_filter) {
+        for (uint32_t q = 0; q < nq; ++q) {
+            CDB_REQUIRE(filter_offsets[q] <= filter_offsets[q + 1], "filter_offsets must be non-decreasing");
+            CDB_REQUIRE(!has_filter[q] || filter_offsets[q + 1] - filter_offsets[q] <= 4096, "too many filters for one query");
+        }
+        total = filter_offsets[nq];
+        CDB_REQUIRE(filter_dims || !total, "null filter_dims");
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    const size_t nl = g->dev.size();
+    uint32_t md_dims = 0;
+    if ((rc = shards_check(g, p, true, &md_dims))) return rc;
+    const uint32_t dim = index_dim(g->shard[0]);
+    auto al16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t nk = (size_t)nq * p->k, qbytes = al16((size_t)nq * dim * 4), obytes = al16(((size_t)nq + 1) * 4);
+    std::vector<const float *> d_q(nl);
+    std::vector<ShardFilters> flt(nl, ShardFilters{nullptr, nullptr, 0, nullptr});
+    for (size_t i = 0; i < nl; ++i) {   // queries, then offsets, has-flags and filter rows, to every local device
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->q[i].ensure(qbytes + obytes + al16(nq) + (size_t)total * md_dims + 1))) return rc;
+        uint8_t *base = reinterpret_cast<uint8_t *>(g->q[i].p);
+        CDB_CUDA_TRY(cudaMemcpyAsync(base, queries, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        d_q[i] = reinterpret_cast<const float *>(base);
+        if (has_filter) {
+            uint32_t *off = reinterpret_cast<uint32_t *>(base + qbytes);
+            uint8_t *has = base + qbytes + obytes;
+            int8_t *dims = reinterpret_cast<int8_t *>(has + al16(nq));
+            CDB_CUDA_TRY(cudaMemcpyAsync(off, filter_offsets, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, g->stream[i]));
+            CDB_CUDA_TRY(cudaMemcpyAsync(has, has_filter, nq, cudaMemcpyHostToDevice, g->stream[i]));
+            if (total) CDB_CUDA_TRY(cudaMemcpyAsync(dims, filter_dims, (size_t)total * md_dims, cudaMemcpyHostToDevice, g->stream[i]));
+            flt[i] = {off, dims, total, has};
+        }
+    }
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    Buf &o_err = g->err[0];
+    if ((rc = o_err.ensure(nk * 8 + (size_t)nq * 8))) return rc;
+    uint32_t *f_ids = reinterpret_cast<uint32_t *>(o_err.p);
+    float *f_scores = reinterpret_cast<float *>(f_ids + nk);
+    uint32_t *f_counts = reinterpret_cast<uint32_t *>(f_scores + nk);
+    uint8_t *f_err = reinterpret_cast<uint8_t *>(f_counts + nq);
+    rc = sharded_enqueue(g, nq, p, d_q, &flt, f_ids, f_scores, f_counts, f_err, nullptr);
+    if (!rc) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        cudaStream_t s0 = g->stream[0];
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, s0));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, s0));
+        if (out_counts) CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s0));
+        if (err_flags) CDB_CUDA_TRY(cudaMemcpyAsync(err_flags, f_err, nq, cudaMemcpyDeviceToHost, s0));
+    }
+    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collectives included) before the host buffers are reused
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
+    }
+    return rc;
+}
+
+cdb_status cdb_search_batch_filtered_sharded_device(cdb_shard_group *g, const float *d_queries, uint32_t nq, const cdb_search_params *p,
+                                                    const uint32_t *d_filter_offsets, const int8_t *d_filter_dims, uint32_t n_filter_rows,
+                                                    const uint8_t *d_has_filter, uint32_t *d_out_ids, float *d_out_scores,
+                                                    uint32_t *d_out_counts, uint8_t *d_err_flags, void *stream) {
+    CDB_REQUIRE(p, "null params");
+    cdb_status rc = filtered_params_check(p, d_filter_offsets, d_has_filter);
+    if (rc) return rc;
+    CDB_REQUIRE(d_filter_dims || !n_filter_rows, "n_filter_rows > 0 needs filter_dims");
+    CDB_REQUIRE(g && (d_queries || !nq) && (d_out_ids || !nq) && (d_out_scores || !nq), "null argument");
+    CDB_REQUIRE(g->dev.size() == 1, "the device form serves one-process-per-GPU groups (cdb_shard_group_create_rank)");
+    if (!nq) return CDB_OK;
+    if ((rc = merge_check(g, p))) return rc;
+    std::lock_guard<std::mutex> lock(g->mu);
+    uint32_t md_dims = 0;
+    if ((rc = shards_check(g, p, true, &md_dims))) return rc;
+    std::vector<const float *> d_q(1, d_queries);
+    std::vector<ShardFilters> flt(1, ShardFilters{d_filter_offsets, d_filter_dims, n_filter_rows, d_has_filter});
+    return sharded_enqueue(g, nq, p, d_q, &flt, d_out_ids, d_out_scores, d_out_counts, d_err_flags, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------- sparse and TF-IDF shards
-constexpr size_t GROUP_GATHER_BUDGET = 256ull << 20;   // bytes of one chunk's gather buffer; queries are searched in chunks
-
-// queries per chunk when a query takes `per_q` bytes of every rank's gather slot
-static uint32_t group_chunk(const cdb_shard_group *g, uint32_t nq, size_t per_q) {
-    return (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, GROUP_GATHER_BUDGET / (g->world * per_q)}));
-}
-
-// loopback: a chunk's slots write their gather buffers only after slot 0 copied the previous chunk's out of them
-static cdb_status loopback_fence(cdb_shard_group *g) {
-    if (!g->loopback) return CDB_OK;
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    CDB_CUDA_TRY(cudaEventRecord(g->ev[0], g->stream[0]));
-    for (size_t i = 1; i < g->dev.size(); ++i) CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[i], g->ev[0], 0));
-    return CDB_OK;
-}
 
 struct SparseQueries {
     const uint64_t *off;

@@ -61,6 +61,26 @@ def merge_packed(gathered, k, metric=0):
     return ids, scores, (best != 0).sum(axis=1).astype(np.uint32)
 
 
+def merge_runs(gathered, metric=0):
+    """the top_k None merge of the sharded dense search.  gathered: [world, B, w] keys, every rank's whole sorted list
+    (descending, unique, zero padded) -> (ids u32[B, world*w], scores f32[B, world*w], counts u32[B]).  An entry's position
+    is its index in its run plus, for every other run, the number of that run's keys greater than it."""
+    gathered = np.asarray(gathered, dtype=np.uint64)
+    world, b, w = gathered.shape
+    out = np.zeros((b, world * w), np.uint64)
+    for q in range(b):
+        runs = [gathered[r, q][gathered[r, q] != 0] for r in range(world)]
+        asc = [np.sort(x) for x in runs]
+        for r, x in enumerate(runs):
+            pos = np.arange(len(x), dtype=np.int64)
+            for o in range(world):
+                if o != r:
+                    pos += len(asc[o]) - np.searchsorted(asc[o], x, side="right")
+            out[q, pos] = x
+    ids, scores = unpack_keys(out, metric)
+    return ids, scores, (out != 0).sum(axis=1).astype(np.uint32)
+
+
 def gather_and_merge(local_ids, local_scores, world, all_gather_fn, k=None, metric=0):
     """host logic of the sharded search: pack -> ONE all-gather of B*k u64 -> merge.
     all_gather_fn(x: u64[B,k]) -> u64[world,B,k] stacked over ranks."""
@@ -142,6 +162,7 @@ class ShardGroup:
     def __init__(self, handle, lib):
         self._h, self._lib = handle, lib
         self._shards = []
+        self._ranks_elsewhere = False        # a per-rank group of world > 1: the other ranks' shards are not visible here
         self._text_shards = []              # sparse and TF-IDF shards, kept alive as long as the group
 
     @staticmethod
@@ -172,7 +193,9 @@ class ShardGroup:
         buf = (C.c_uint8 * NCCL_UNIQUE_ID_BYTES).from_buffer_copy(unique_id) if unique_id is not None else None
         h = C.c_void_p()
         _check(lib.cdb_shard_group_create_rank(buf, world, rank, device, C.byref(h)))
-        return cls(h, lib)
+        g = cls(h, lib)
+        g._ranks_elsewhere = world > 1
+        return g
 
     @property
     def world(self):
@@ -183,11 +206,25 @@ class ShardGroup:
         _check(self._lib.cdb_shard_group_attach(self._h, local_slot, index._h))
         self._shards.append(index)          # keep the shard alive as long as the group
 
-    def search(self, queries, k, mode=0, **kw):
-        """host queries -> merged (ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B])"""
+    def all_width(self, width=None):
+        """row width W of a top_k None search over this group.  Every rank must pass the same W, a multiple of the world size
+        with W / world >= every shard's (num_levels + 1) * 100: ranks that disagree run all-gathers of different sizes, and a
+        rank that refuses leaves the others waiting in theirs.  A local group sees every shard, so W defaults to world * the
+        largest (num_levels + 1) * 100; a per-rank group of more than one rank must pass `width` (the same on every rank)."""
+        if width is not None:
+            return int(width)
+        if self._ranks_elsewhere:
+            raise ValueError("a per-rank group's top_k None search needs width= (the same W on every rank)")
+        return self.world * max(s.hnsw_out_cap() for s in self._shards)
+
+    def search(self, queries, k, mode=0, width=None, **kw):
+        """host queries -> merged (ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B]).
+        k=None (top_k None, HNSW): every shard's candidates, merged best first, in rows of all_width(width) columns"""
         from .api import _check, _ptr
         q = np.ascontiguousarray(queries, dtype=np.float32)
         b = q.shape[0]
+        if k is None:
+            k, kw["all_candidates"] = self.all_width(width), True
         ids = np.zeros((b, k), dtype=np.uint32)
         scores = np.zeros((b, k), dtype=np.float32)
         counts = np.zeros(b, dtype=np.uint32)
@@ -204,6 +241,38 @@ class ShardGroup:
                                                          C.c_void_p(d_scores), C.c_void_p(d_counts) if d_counts else None,
                                                          C.c_void_p(d_err) if d_err else None,
                                                          C.c_void_p(stream_ptr) if stream_ptr else None))
+
+    def search_filtered(self, queries, filters, k, width=None, **kw):
+        """DenseIndex.batch_search_filtered over the group (every shard a graph with metadata of one md_dims): filters[q] is
+        None or a list of int8[md_dims] -> (replica ids u32[B,k], scores f32[B,k], counts u32[B], err u8[B]); k=None: top_k None"""
+        from .api import SearchMode, _check, _ptr
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        if q.ndim == 1:
+            q = q[None]
+        b = q.shape[0]
+        offs, dims, has = self._shards[0].pack_filters(filters)
+        if dims.shape[0] == 0:
+            dims = np.zeros((1, self._shards[0].md_dims), dtype=np.int8)
+        if k is None:
+            k, kw["all_candidates"] = self.all_width(width), True
+        ids = np.zeros((b, k), dtype=np.uint32)
+        scores = np.zeros((b, k), dtype=np.float32)
+        counts = np.zeros(b, dtype=np.uint32)
+        err = np.zeros(b, dtype=np.uint8)
+        p = self._shards[0].params(k, SearchMode.HNSW, **kw)
+        _check(self._lib.cdb_search_batch_filtered_sharded(self._h, _ptr(q), b, C.byref(p), _ptr(offs), _ptr(dims), _ptr(has), _ptr(ids),
+                                                           _ptr(scores), _ptr(counts), _ptr(err)))
+        return ids, scores, counts, err
+
+    def search_filtered_device(self, d_queries, nq, k, d_offsets, d_dims, n_filter_rows, d_has, d_ids, d_scores, d_counts=None,
+                               d_err=None, stream_ptr=None, **kw):
+        """per-rank groups: search_filtered on device pointers (ints), the filters in the CSR form of DenseIndex.pack_filters
+        (d_has None: no query has a filter); asynchronous on the stream.  all_candidates=True: top_k None, k = the row width"""
+        from .api import SearchMode, _check
+        p = self._shards[0].params(k, SearchMode.HNSW, **kw)
+        _check(self._lib.cdb_search_batch_filtered_sharded_device(self._h, d_queries, nq, C.byref(p), d_offsets, d_dims, n_filter_rows,
+                                                                  d_has, d_ids, d_scores, d_counts, d_err,
+                                                                  C.c_void_p(stream_ptr) if stream_ptr else None))
 
     def attach_sparse(self, local_slot, index):
         """a SparseIndex shard (id_base = its first global id) into local slot `local_slot`, next to any dense shard"""

@@ -130,6 +130,21 @@ typedef struct {
  * its tiles' epilogue).  Results are bit-identical with and without the flag, as with exact_only, which still wins.
  * Without it a shard with deleted rows is answered by the exact scan.  HNSW mode ignores it. */
 #define CDB_SEARCH_TENSOR_WITH_DELETED 1u
+/* top_k None (a dense search request without top_k, finalize_ann_results at src/vector_store.rs:404-445 with k = None):
+ * every deduplicated candidate of the HNSW search is re-ranked by exact f32 cosine and the whole sorted list is returned.
+ * Under the flag k is only the output row width W: row q holds counts[q] results, best first, then CDB_INVALID_ID / 0.
+ *   single index (cdb_search_batch[_device], cdb_search_batch_filtered[_device]): W >= (num_levels + 1) * 100, the most
+ *     candidates the traversal can report (cdb_index_graph_info gives num_levels); checked once the handle's lock is held
+ *   shard groups (cdb_search_batch_sharded[_device], cdb_search_batch_filtered_sharded[_device]): W is a multiple of the
+ *     world size and every local shard's (num_levels + 1) * 100 <= W / world; counts[q] is the sum over the shards.  In a
+ *     per-rank group every rank must pass the same W: it sets the size of the all-gather, and a rank only checks its own
+ *     shard, so a rank that refuses leaves the others waiting in the collective.  Any world size.
+ * The re-rank holds the query and next_pow2((num_levels + 1) * 100) keys in 200 KB of shared memory:
+ * 4 * dim + 8 * next_pow2(cap) <= 200 KB (dim <= 43008 at cap 3200).
+ * Refused with CDB_INVALID_PARAMS before any device work: the flag with a CDB_MODE_BRUTE_* mode, in the dense params of
+ * cdb_hybrid_search_batch[_device], W below its bound, and a dimension above that one.  Without the flag k stays in
+ * 1..1024. */
+#define CDB_SEARCH_ALL_CANDIDATES 2u
 
 /* ---------------------------------------------------------------- misc */
 int32_t cdb_abi_version(void);
@@ -535,7 +550,7 @@ cdb_status cdb_index_hnsw_counters(const cdb_index *index, uint64_t *out2);
  * queries: B x dim raw f32 (search_internal quantizes them with the index's
  * storage type, hnsw/mod.rs:399-403).  out_ids/out_scores: B x k, best first;
  * unused slots get CDB_INVALID_ID / 0.  out_counts[q] = valid slots.
- * err_flags may be NULL.  k <= 1024.
+ * err_flags may be NULL.  k <= 1024 (CDB_SEARCH_ALL_CANDIDATES: every candidate, k = the row width).
  * Execution paths (same results, chosen by shape): BRUTE_RAW with an fp16 shadow, >= 4 queries, >= 16384 rows and
  * k <= 64 -> wgmma fp16 prefilter + exact re-rank; BRUTE_CODES over u8 / sub-byte codes with cosine or dot product,
  * >= 16384 rows and k <= 64 -> exact wgmma u8 scoring; everything else -> exact SIMT scan. */
@@ -604,7 +619,8 @@ cdb_status cdb_rerank_f32(cdb_index *index, const float *query, const uint32_t *
  *                                per-rank group every rank must call it with the same batch and receives the same result
  *   cdb_search_batch_sharded_device   per-rank groups only: device buffers, asynchronous on `stream`
  * Both searches refuse world * k * 8 > 200 KB (the merge's shared memory) with CDB_INVALID_PARAMS before any copy or
- * search is issued.
+ * search is issued.  Under CDB_SEARCH_ALL_CANDIDATES (HNSW) that bound does not apply: each rank's sorted list fills
+ * k / world columns and the lists are merged without truncation, the batch in chunks that keep the gather within 256 MB.
  * Results are those cdb_search_batch would return on the concatenated corpus (exact modes), resp. the merge of the
  * per-shard HNSW results (one independent graph per shard). */
 #define CDB_NCCL_UNIQUE_ID_BYTES 128
@@ -620,6 +636,22 @@ cdb_status cdb_search_batch_sharded(cdb_shard_group *group, const float *queries
 cdb_status cdb_search_batch_sharded_device(cdb_shard_group *group, const float *d_queries, uint32_t n_queries,
                                            const cdb_search_params *params, uint32_t *d_out_ids, float *d_out_scores,
                                            uint32_t *d_out_counts, uint8_t *d_err_flags, void *stream);
+/* cdb_search_batch_filtered over a shard group: every shard runs its own filtered HNSW search (from its own pseudo root for a
+ * filtered query) and the results are merged like cdb_search_batch_sharded's, error bytes OR-ed over the ranks.  The filter
+ * arguments are those of cdb_search_batch_filtered (host form: queries and filter CSR go to every local device) and of
+ * cdb_search_batch_filtered_device (device form: per-rank groups only, like cdb_search_batch_sharded_device; every rank
+ * passes the same batch and filters, and a bad filter range gives CDB_ERRFLAG_BAD_FILTER and count 0).  Every local shard
+ * must have graph metadata with the same md_dims, checked at search time (metadata may be attached after
+ * cdb_shard_group_attach): CDB_INVALID_PARAMS otherwise.  out_ids are replica ids. */
+cdb_status cdb_search_batch_filtered_sharded(cdb_shard_group *group, const float *queries, uint32_t n_queries,
+                                             const cdb_search_params *params, const uint32_t *filter_offsets, const int8_t *filter_dims,
+                                             const uint8_t *has_filter, uint32_t *out_ids, float *out_scores, uint32_t *out_counts,
+                                             uint8_t *err_flags);
+cdb_status cdb_search_batch_filtered_sharded_device(cdb_shard_group *group, const float *d_queries, uint32_t n_queries,
+                                                    const cdb_search_params *params, const uint32_t *d_filter_offsets,
+                                                    const int8_t *d_filter_dims, uint32_t n_filter_rows, const uint8_t *d_has_filter,
+                                                    uint32_t *d_out_ids, float *d_out_scores, uint32_t *d_out_counts,
+                                                    uint8_t *d_err_flags, void *stream);
 
 /* ------------------------------------------------ multi-GPU shard merge (5e)
  * d_ids/d_scores: [n_shards][n_queries][k] gathered per-shard results (device);

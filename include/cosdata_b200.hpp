@@ -130,15 +130,16 @@ class DenseIndex {
     void set_graph(const cdb_graph_desc &g) { check(cdb_index_set_graph(h_, &g)); }
 
     // IndexOps::batch_search
+    // all_candidates (top_k None, HNSW): every candidate, best first; k is the row width, >= (num_levels + 1) * 100
     SearchResults batch_search(const float *queries, uint32_t b, uint32_t k, SearchMode mode = SearchMode::BruteRaw,
-                               uint32_t ef_search = 256, uint32_t shortlist_size = 64) const {
+                               uint32_t ef_search = 256, uint32_t shortlist_size = 64, bool all_candidates = false) const {
         SearchResults r;
         r.k = k;
         r.ids.resize((size_t)b * k);
         r.scores.resize((size_t)b * k);
         r.counts.resize(b);
         r.err.resize(b);
-        cdb_search_params p{k, (int32_t)mode, ef_search, shortlist_size, 0, 0, 0, 0};
+        cdb_search_params p{k, (int32_t)mode, ef_search, shortlist_size, 0, 0, all_candidates ? CDB_SEARCH_ALL_CANDIDATES : 0u, 0};
         check(cdb_search_batch(h_, queries, b, &p, r.ids.data(), r.scores.data(), r.counts.data(), r.err.data()));
         return r;
     }
@@ -250,17 +251,34 @@ class ShardGroup {
     }
     void attach(uint32_t local_slot, DenseIndex &shard) { check(cdb_shard_group_attach(g_, local_slot, shard.handle())); }
     uint32_t world() const { return cdb_shard_group_world(g_); }
-    // IndexOps::batch_search over all shards: one all-gather of packed keys, merged with "better score, then smaller id"
+    // IndexOps::batch_search over all shards: one all-gather of packed keys, merged with "better score, then smaller id".
+    // all_candidates (top_k None, HNSW): k is the row width, world * w with w >= every shard's (num_levels + 1) * 100
     SearchResults batch_search(const float *queries, uint32_t b, uint32_t k, SearchMode mode = SearchMode::BruteRaw,
-                               uint32_t ef_search = 256, uint32_t shortlist_size = 64) const {
+                               uint32_t ef_search = 256, uint32_t shortlist_size = 64, bool all_candidates = false) const {
         SearchResults r;
         r.k = k;
         r.ids.resize((size_t)b * k);
         r.scores.resize((size_t)b * k);
         r.counts.resize(b);
         r.err.resize(b);
-        cdb_search_params p{k, (int32_t)mode, ef_search, shortlist_size, 0, 0, 0, 0};
+        cdb_search_params p{k, (int32_t)mode, ef_search, shortlist_size, 0, 0, all_candidates ? CDB_SEARCH_ALL_CANDIDATES : 0u, 0};
         check(cdb_search_batch_sharded(g_, queries, b, &p, r.ids.data(), r.scores.data(), r.counts.data(), r.err.data()));
+        return r;
+    }
+    // the same with metadata filters (every shard a graph with metadata of one md_dims): filter_offsets [b + 1] index the
+    // md_dims-wide i8 rows of filter_dims, has_filter[q] != 0 marks a filtered query (NULL: none); ids are replica ids
+    SearchResults batch_search_filtered(const float *queries, uint32_t b, uint32_t k, const uint32_t *filter_offsets,
+                                        const int8_t *filter_dims, const uint8_t *has_filter, uint32_t ef_search = 256,
+                                        uint32_t shortlist_size = 64, bool all_candidates = false) const {
+        SearchResults r;
+        r.k = k;
+        r.ids.resize((size_t)b * k);
+        r.scores.resize((size_t)b * k);
+        r.counts.resize(b);
+        r.err.resize(b);
+        cdb_search_params p{k, (int32_t)SearchMode::Hnsw, ef_search, shortlist_size, 0, 0, all_candidates ? CDB_SEARCH_ALL_CANDIDATES : 0u, 0};
+        check(cdb_search_batch_filtered_sharded(g_, queries, b, &p, filter_offsets, filter_dims, has_filter, r.ids.data(), r.scores.data(),
+                                                r.counts.data(), r.err.data()));
         return r;
     }
 
