@@ -158,6 +158,23 @@ class HybridSources(C.Structure):
     ]
 
 
+class HybridGroupSources(C.Structure):
+    _fields_ = [
+        ("use_dense", C.c_uint32),
+        ("use_sparse", C.c_uint32),
+        ("use_tfidf", C.c_uint32),
+        ("dense_queries", C.c_void_p),
+        ("dense_params", SearchParams),
+        ("dense_id_stride", C.c_uint32),
+        ("sparse_offsets", C.c_void_p),
+        ("sparse_dims", C.c_void_p),
+        ("sparse_values", C.c_void_p),
+        ("sparse_params", SparseSearchParams),
+        ("tfidf_offsets", C.c_void_p),
+        ("tfidf_hashes", C.c_void_p),
+    ]
+
+
 # symbol -> (restype, argtypes); must list every function of include/cosdata_b200.h
 PROTOTYPES = {
     "cdb_abi_version": (C.c_int32, []),
@@ -290,6 +307,10 @@ PROTOTYPES = {
                                             c_u8p]),
     "cdb_hybrid_search_batch_device": (C.c_int32, [C.POINTER(HybridSources), C.c_uint32, C.c_uint32, C.c_float, c_u32p, c_f32p,
                                                    c_u32p, c_u8p, C.c_void_p]),
+    "cdb_hybrid_search_batch_sharded": (C.c_int32, [C.c_void_p, C.POINTER(HybridGroupSources), C.c_uint32, C.c_uint32, C.c_float, c_vp,
+                                                    c_vp, c_vp, c_vp]),
+    "cdb_hybrid_search_batch_sharded_device": (C.c_int32, [C.c_void_p, C.POINTER(HybridGroupSources), C.c_uint32, C.c_uint32, C.c_float,
+                                                           c_vp, c_vp, c_vp, c_vp, C.c_void_p]),
 }
 
 _lib = None

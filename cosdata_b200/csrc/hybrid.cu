@@ -1,6 +1,7 @@
 // hybrid.cu -- hybrid search (hybrid_search / batch_hybrid_search, src/api/vectordb/search/repo.rs:168-555): reciprocal-rank
 // fusion of two ranked lists per query, and the composed search that runs two of the dense, sparse and TF-IDF searches and
 // fuses their results on the device.  The contract is the header comment of cdb_rrf_fuse (DESIGN.md section 8e).
+// check_fuse_args and fuse_launch also serve a shard group's hybrid search (shard_group.cu, DESIGN.md section 8h).
 //
 // rrf_fuse_kernel: one CTA per query.  Every live entry becomes (key << 32 | list << 31 | rank) in shared memory; a bitonic
 // sort groups each key's entries, first list before second, each in rank order; the head of every run folds it (first
@@ -18,14 +19,7 @@ namespace cdb {
 namespace {
 
 constexpr uint32_t RRF_MAX = 2048;      // entries of both lists of one query
-constexpr uint32_t HYB_MAX_TOP_K = 341; // 3 * top_k <= 1024, the dense and sparse searches' k limit
 constexpr uint32_t TF_RESULTS = 512;    // TF-IDF's bucket count: its searches return at most 512 results
-
-struct RrfList {
-    const uint32_t *ids;      // [B][ld]
-    const uint32_t *counts;   // [B]
-    uint32_t ld, stride;
-};
 
 // 1.0 / (rank as f32 + k + f32::EPSILON): one rounding per operation, left to right, no FMA, no approximate reciprocal
 __device__ __forceinline__ float rrf_contribution(uint32_t rank, float k) {
@@ -92,6 +86,8 @@ __global__ void __launch_bounds__(1024) rrf_fuse_kernel(RrfList a, RrfList b, fl
     if (tid == 0) out_counts[q] = cnt;
 }
 
+}  // namespace
+
 cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t ld_out, const void *ids_a, const void *cnt_a,
                            const void *ids_b, const void *cnt_b, const void *out_ids, const void *out_scores, const void *out_counts) {
     CDB_REQUIRE((uint64_t)ld_a + ld_b <= RRF_MAX, "ld_first + ld_second must be <= 2048");
@@ -112,6 +108,8 @@ cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k,
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }
+
+namespace {
 
 enum Source { SRC_DENSE = 0, SRC_SPARSE = 1, SRC_TFIDF = 2 };
 

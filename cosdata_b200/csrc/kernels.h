@@ -55,6 +55,18 @@ uint32_t index_dim(const cdb_index *ix);
 // graph metadata attached (results carry replica ids); read under the handle's shared lock
 bool index_has_graph_metadata(cdb_index *ix);
 
+// ---- hybrid.cu: the fusion of two ranked lists per query (cdb_rrf_fuse's kernel), shared with the shard group's hybrid search
+constexpr uint32_t HYB_MAX_TOP_K = 341;   // 3 * top_k <= 1024, the dense and sparse searches' k limit
+struct RrfList {
+    const uint32_t *ids;      // [B][ld]
+    const uint32_t *counts;   // [B]
+    uint32_t ld, stride;
+};
+cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t ld_out, const void *ids_a, const void *cnt_a,
+                           const void *ids_b, const void *cnt_b, const void *out_ids, const void *out_scores, const void *out_counts);
+cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k, uint32_t ld_out, uint32_t *d_ids, float *d_scores,
+                       uint32_t *d_counts, cudaStream_t s);
+
 // ---- pairs.cu
 cdb_status distance_pairs_device(int metric, int st, uint32_t dim, const uint8_t *d_x, const float *d_xm,
                                  const uint8_t *d_y, const float *d_ym, uint32_t row_pitch, uint64_t n,

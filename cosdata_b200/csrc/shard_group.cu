@@ -233,6 +233,7 @@ struct cdb_shard_group {
     std::vector<cudaStream_t> stream;
     std::vector<cudaEvent_t> ev;
     std::vector<Buf> gather, q, ids, scores, counts, err, sel;
+    std::vector<Buf> hq;                  // a hybrid search's dense and sparse queries (host form), kept apart from q
     std::mutex mu;
 };
 
@@ -244,6 +245,7 @@ static cdb_status group_alloc_slots(cdb_shard_group *g, size_t n) {
     g->stream.assign(n, nullptr);
     g->ev.assign(n, nullptr);
     g->gather.resize(n); g->q.resize(n); g->ids.resize(n); g->scores.resize(n); g->counts.resize(n); g->err.resize(n); g->sel.resize(n);
+    g->hq.resize(n);
     for (size_t i = 0; i < n; ++i) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
         CDB_CUDA_TRY(cudaStreamCreateWithFlags(&g->stream[i], cudaStreamNonBlocking));
@@ -321,7 +323,7 @@ cdb_status cdb_shard_group_destroy(cdb_shard_group *g) {
         cudaSetDevice(g->dev[i]);
         if (i < g->stream.size() && g->stream[i]) cudaStreamSynchronize(g->stream[i]);
         if (i < g->comm.size() && g->comm[i] && n) n->CommDestroy(g->comm[i]);
-        for (auto *v : {&g->gather, &g->q, &g->ids, &g->scores, &g->counts, &g->err, &g->sel})
+        for (auto *v : {&g->gather, &g->q, &g->ids, &g->scores, &g->counts, &g->err, &g->sel, &g->hq})
             if (i < v->size()) (*v)[i].release();
         if (i < g->ev.size() && g->ev[i]) cudaEventDestroy(g->ev[i]);
         if (i < g->stream.size() && g->stream[i]) cudaStreamDestroy(g->stream[i]);
@@ -824,25 +826,24 @@ cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *g, const uint
     return sparse_sharded_enqueue(g, nq, p, m, dq, d_ids, d_scores, d_counts, (cudaStream_t)stream);
 }
 
-// Host form only.  The group's N and df of every query term: summed over the local shards' tables, then (per-rank
-// groups) over the ranks by one all-gather of [N, df...] per rank.  idf = tf_idf(N, df) on the host, one per query term;
-// each shard scores its tiles with it and writes all 512 bucket winners per query into its rank's slot; one all-gather;
-// slot 0 takes the best of the ranks per bucket and sorts.  The local shards' reader locks are held from the df look-up
-// until the scoring has run.
-cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
-                                          uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
-    CDB_REQUIRE(g && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+// The group's N and df of every query term: summed over the local shards' tables, then (per-rank groups) over the ranks by
+// one all-gather of [N, df...] per rank.  idf = tf_idf(N, df) on the host, one per query term; each shard scores its tiles
+// with it and writes all 512 bucket winners per query into its rank's slot; one all-gather; slot 0 takes the best of the
+// ranks per bucket and sorts into ids / scores [nq][tfidf_out_cols(k)] and counts [nq] on slot 0.  The caller holds g->mu
+// and every local shard's reader lock until the scoring has run, and drains the streams.  q_offsets may be a window of a
+// larger CSR (q_offsets[0] != 0): q_hashes is that CSR's hash array.  Host only: a per-rank group waits for its df all-gather.
+static cdb_status tfidf_sharded_run(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
+                                    uint32_t *f_ids, float *f_scores, uint32_t *f_counts) {
     const size_t nl = g->dev.size();
-    for (size_t i = 0; i < nl; ++i) CDB_REQUIRE(g->tfidf[i], "a group slot has no tf-idf shard attached");
-    if (!nq) return CDB_OK;
-    cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
-    if (rc) return rc;
-    const uint64_t nqh = q_offsets[nq];
-    CDB_REQUIRE(q_hashes || !nqh, "null query hashes");
-    CDB_REQUIRE(nqh < (1ull << 31), "a batch of 2^31 query terms or more");
-    std::lock_guard<std::mutex> lock(g->mu);
-    std::vector<std::shared_lock<std::shared_mutex>> locks;
-    for (size_t i = 0; i < nl; ++i) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
+    const uint64_t h0 = q_offsets[0], nqh = q_offsets[nq] - h0;
+    q_hashes += h0;
+    std::vector<uint64_t> rebased;
+    if (h0) {
+        rebased.assign(q_offsets, q_offsets + nq + 1);
+        for (auto &o : rebased) o -= h0;
+        q_offsets = rebased.data();
+    }
+    cdb_status rc = CDB_OK;
     // [N, df of every query term], summed over the local shards (u32, wrapping), then over the ranks
     std::vector<uint32_t> stats(1 + nqh, 0);
     for (size_t i = 0; i < nl; ++i) stats[0] += tfidf_add_df(g->tfidf[i], q_hashes, nqh, stats.data() + 1);
@@ -873,16 +874,10 @@ cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_
         if (nqh) CDB_CUDA_TRY(cudaMemcpyAsync(d_idf, idf.data(), nqh * 4, cudaMemcpyHostToDevice, g->stream[i]));
     }
     const uint32_t kout = tfidf_out_cols(k), chunk = group_chunk(g, nq, 512 * 8);
-    const size_t nk = (size_t)nq * kout;
     for (size_t i = 0; i < nl; ++i) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
         if ((rc = g->gather[i].ensure(g->world * (size_t)chunk * 512 * 8))) return rc;
     }
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    if ((rc = g->ids[0].ensure(nk * 4)) || (rc = g->scores[0].ensure(nk * 4)) || (rc = g->counts[0].ensure((size_t)nq * 4))) return rc;
-    uint32_t *f_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
-    float *f_scores = reinterpret_cast<float *>(g->scores[0].p);
-    uint32_t *f_counts = reinterpret_cast<uint32_t *>(g->counts[0].p);
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
         const size_t words = (size_t)c * 512;
@@ -901,6 +896,32 @@ cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_
                                       f_counts + q0, g->stream[0]);
         }
     }
+    return rc;
+}
+
+// Host form only: the idf needs the host mid-call (tfidf_sharded_run).  The local shards' reader locks are held from the
+// df look-up until the scoring has run.
+cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
+                                          uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
+    CDB_REQUIRE(g && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
+    const size_t nl = g->dev.size();
+    for (size_t i = 0; i < nl; ++i) CDB_REQUIRE(g->tfidf[i], "a group slot has no tf-idf shard attached");
+    if (!nq) return CDB_OK;
+    cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
+    if (rc) return rc;
+    const uint64_t nqh = q_offsets[nq];
+    CDB_REQUIRE(q_hashes || !nqh, "null query hashes");
+    CDB_REQUIRE(nqh < (1ull << 31), "a batch of 2^31 query terms or more");
+    std::lock_guard<std::mutex> lock(g->mu);
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    for (size_t i = 0; i < nl; ++i) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
+    const size_t nk = (size_t)nq * tfidf_out_cols(k);
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    if ((rc = g->ids[0].ensure(nk * 4)) || (rc = g->scores[0].ensure(nk * 4)) || (rc = g->counts[0].ensure((size_t)nq * 4))) return rc;
+    uint32_t *f_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
+    float *f_scores = reinterpret_cast<float *>(g->scores[0].p);
+    uint32_t *f_counts = reinterpret_cast<uint32_t *>(g->counts[0].p);
+    rc = tfidf_sharded_run(g, q_offsets, q_hashes, nq, k, f_ids, f_scores, f_counts);
     if (!rc) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
         CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
@@ -912,6 +933,253 @@ cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_
         CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
     }
     return rc;
+}
+
+// ---------------------------------------------------------------- hybrid search over the group (DESIGN.md section 8h)
+
+enum HybSource { HYB_DENSE = 0, HYB_SPARSE = 1, HYB_TFIDF = 2 };
+
+struct HybPlan {
+    HybSource src[2];              // first list, second list
+    uint32_t ld[2];                // columns of each intermediate list
+    cdb_search_params dense;       // at k = 3 * top_k
+    cdb_sparse_search_params sparse;
+    uint32_t m = 0;                // the sparse search's candidates per query
+    bool md = false;               // the dense shards have graph metadata: the filtered path, no filter
+};
+
+// the refusals that need no group, in the order of cdb_hybrid_search_batch's (make_plan in hybrid.cu), then the sub-searches'
+// own parameter checks at k = 3 * top_k
+static cdb_status hyb_plan(const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k, HybPlan *p) {
+    CDB_REQUIRE(h, "null sources");
+    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
+    CDB_REQUIRE((h->use_dense != 0) + (h->use_sparse != 0) + (h->use_tfidf != 0) == 2, "a hybrid search takes exactly two sources");
+    CDB_REQUIRE(!h->use_dense || !(h->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
+                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
+    const uint32_t k3 = 3 * top_k;
+    int i = 0;
+    if (h->use_dense) { p->src[i] = HYB_DENSE; p->ld[i++] = k3; }
+    if (h->use_sparse) { p->src[i] = HYB_SPARSE; p->ld[i++] = k3; }
+    if (h->use_tfidf) { p->src[i] = HYB_TFIDF; p->ld[i++] = std::min(k3, 512u); }
+    CDB_REQUIRE(!h->use_dense || h->dense_queries || !nq, "null dense queries");
+    CDB_REQUIRE(!h->use_sparse || h->sparse_offsets || !nq, "null sparse query offsets");
+    CDB_REQUIRE(!h->use_tfidf || h->tfidf_offsets || !nq, "null tf-idf query offsets");
+    if (h->use_sparse && h->sparse_params.rerank)
+        CDB_REQUIRE(h->sparse_params.reranking_factor >= 1 && (uint64_t)k3 * h->sparse_params.reranking_factor <= 5120,
+                    "3 * top_k * reranking_factor must be in 1..5120");
+    p->dense = h->dense_params;
+    p->dense.k = k3;
+    p->sparse = h->sparse_params;
+    p->sparse.k = k3;
+    if (top_k && h->use_dense)
+        if (cdb_status rc = check_search_k(&p->dense)) return rc;
+    if (top_k && h->use_sparse)
+        if (cdb_status rc = sparse_check_params(&p->sparse, &p->m)) return rc;
+    return CDB_OK;
+}
+
+// the host form's query CSRs, before the group is locked
+static cdb_status hyb_check_csr(const cdb_hybrid_group_sources *h, uint32_t nq) {
+    cdb_status rc;
+    if (nq && h->use_sparse) {
+        if ((rc = check_csr(h->sparse_offsets, nq, "sparse_offsets"))) return rc;
+        CDB_REQUIRE((h->sparse_dims && h->sparse_values) || !h->sparse_offsets[nq], "null sparse query pairs");
+    }
+    if (nq && h->use_tfidf) {
+        if ((rc = check_csr(h->tfidf_offsets, nq, "tfidf_offsets"))) return rc;
+        CDB_REQUIRE(h->tfidf_hashes || !h->tfidf_offsets[nq], "null tf-idf query hashes");
+        CDB_REQUIRE(h->tfidf_offsets[nq] < (1ull << 31), "a batch of 2^31 query terms or more");
+    }
+    return CDB_OK;
+}
+
+// under g->mu, before any copy: every local slot has a shard of each named kind; the dense shards all have graph metadata
+// (of one md_dims; HNSW only) or none has; the dense merge fits
+static cdb_status hyb_group_check(const cdb_shard_group *g, const cdb_hybrid_group_sources *h, HybPlan *p) {
+    const size_t nl = g->dev.size();
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_REQUIRE(!h->use_dense || g->shard[i], "a group slot has no shard attached");
+        CDB_REQUIRE(!h->use_sparse || g->sparse[i], "a group slot has no sparse shard attached");
+        CDB_REQUIRE(!h->use_tfidf || g->tfidf[i], "a group slot has no tf-idf shard attached");
+    }
+    if (!h->use_dense) return CDB_OK;
+    size_t with_md = 0;
+    for (size_t i = 0; i < nl; ++i) with_md += index_md_dims(g->shard[i]) != 0;
+    CDB_REQUIRE(with_md == 0 || with_md == nl,
+                "hybrid search: some local dense shards have graph metadata and some do not (the dense side takes one path)");
+    p->md = with_md != 0;
+    CDB_REQUIRE(!p->md || p->dense.mode == CDB_MODE_HNSW, "dense shards with graph metadata search in CDB_MODE_HNSW");
+    uint32_t md_dims = 0;
+    cdb_status rc = shards_check(g, &p->dense, p->md, &md_dims);
+    if (rc) return rc;
+    return merge_check(g, &p->dense);
+}
+
+// Both sub-searches and the fusion, per chunk of queries, under g->mu and every named text shard's reader lock.  dq / sq:
+// each local slot's dense queries and sparse CSR on its device; the TF-IDF queries stay on the host (host form only).  The
+// sub-searches run one after the other in list order, each on the streams its public entry point uses, so every rank
+// issues the same collectives in the same order; each one's merged list lands in this call's scratch on slot 0, where the
+// fusion writes rows q0.. of the output.  Nothing here waits for the device except a per-rank group's TF-IDF df gather.
+static cdb_status hybrid_group_run(cdb_shard_group *g, const cdb_hybrid_group_sources *h, const HybPlan &p, uint32_t nq, uint32_t top_k,
+                                   float fusion_k, const std::vector<const float *> &dq, const std::vector<SparseQueries> &sq,
+                                   uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
+    const size_t nl = g->dev.size();
+    const uint32_t k3 = 3 * top_k, ld_out = 6 * top_k;
+    const size_t per_q = ((size_t)p.ld[0] + p.ld[1]) * 8 + 8;   // ids and scores of both lists, two counts
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nq, GROUP_GATHER_BUDGET / per_q));
+    const uint32_t dim = h->use_dense ? index_dim(g->shard[0]) : 0;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    const cudaStream_t s0 = slot_stream(g, 0, out_stream);
+    uint8_t *buf = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&buf, chunk * per_q, s0));
+    uint32_t *ids[2], *counts[2];
+    float *scores[2];
+    ids[0] = reinterpret_cast<uint32_t *>(buf);
+    ids[1] = ids[0] + (size_t)chunk * p.ld[0];
+    scores[0] = reinterpret_cast<float *>(ids[1] + (size_t)chunk * p.ld[1]);
+    scores[1] = scores[0] + (size_t)chunk * p.ld[0];
+    counts[0] = reinterpret_cast<uint32_t *>(scores[1] + (size_t)chunk * p.ld[1]);
+    counts[1] = counts[0] + chunk;
+    const std::vector<ShardFilters> no_filters(nl, ShardFilters{nullptr, nullptr, 0, nullptr});
+    cdb_status rc = CDB_OK;
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        for (int j = 0; j < 2 && !rc; ++j) {
+            // loopback: the slots write their gather buffers only after slot 0 copied the previous search's out of them
+            if ((q0 || j) && (rc = loopback_fence(g))) break;
+            if (p.src[j] == HYB_DENSE) {
+                std::vector<const float *> q(nl);
+                for (size_t i = 0; i < nl; ++i) q[i] = dq[i] + (size_t)q0 * dim;
+                rc = sharded_enqueue(g, c, &p.dense, q, p.md ? &no_filters : nullptr, ids[j], scores[j], counts[j],
+                                     d_err ? d_err + q0 : nullptr, out_stream);
+            } else if (p.src[j] == HYB_SPARSE) {
+                std::vector<SparseQueries> q(nl);
+                for (size_t i = 0; i < nl; ++i) q[i] = {sq[i].off + q0, sq[i].dims, sq[i].vals};
+                rc = sparse_sharded_enqueue(g, c, &p.sparse, p.m, q, ids[j], scores[j], counts[j], out_stream);
+            } else {
+                rc = tfidf_sharded_run(g, h->tfidf_offsets + q0, h->tfidf_hashes, c, k3, ids[j], scores[j], counts[j]);
+            }
+        }
+        if (rc) break;
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        const RrfList a{ids[0], counts[0], p.ld[0], p.src[0] == HYB_DENSE ? h->dense_id_stride : 1u}, b{ids[1], counts[1], p.ld[1], 1u};
+        uint32_t *o_ids = d_ids + (size_t)q0 * ld_out, *o_counts = d_counts + q0;
+        float *o_scores = d_scores + (size_t)q0 * ld_out;
+        if (!(rc = check_fuse_args(a.ld, b.ld, c, ld_out, a.ids, a.counts, b.ids, b.counts, o_ids, o_scores, o_counts)))
+            rc = fuse_launch(a, b, c, fusion_k, ld_out, o_ids, o_scores, o_counts, s0);
+    }
+    // freed behind everything enqueued on slot 0's stream, which every slot's last work joined (collective or loopback copy)
+    cudaSetDevice(g->dev[0]);
+    cudaFreeAsync(buf, s0);
+    return rc;
+}
+
+cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *g, const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k,
+                                           float fusion_constant_k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts,
+                                           uint8_t *err_flags) {
+    CDB_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
+    CDB_REQUIRE(g, "null group");
+    HybPlan p;
+    cdb_status rc = hyb_plan(h, nq, top_k, &p);
+    if (rc || (rc = hyb_check_csr(h, nq))) return rc;
+    std::lock_guard<std::mutex> lock(g->mu);
+    if ((rc = hyb_group_check(g, h, &p))) return rc;
+    if (!nq) return CDB_OK;
+    if (!top_k) {
+        memset(out_counts, 0, (size_t)nq * 4);
+        return CDB_OK;
+    }
+    const size_t nl = g->dev.size();
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    for (size_t i = 0; i < nl; ++i) {
+        if (h->use_sparse) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
+        if (h->use_tfidf) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
+    }
+    // the dense batch, then the sparse CSR, to every local device
+    const uint32_t dim = h->use_dense ? index_dim(g->shard[0]) : 0;
+    const uint64_t nqp = h->use_sparse ? h->sparse_offsets[nq] : 0;
+    const size_t dbytes = ((size_t)nq * dim * 4 + 15) & ~(size_t)15, sbytes = h->use_sparse ? ((size_t)nq + 1) * 8 + nqp * 8 : 0;
+    std::vector<const float *> dq(nl, nullptr);
+    std::vector<SparseQueries> sq(nl, SparseQueries{nullptr, nullptr, nullptr});
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->hq[i].ensure(dbytes + sbytes))) return rc;
+        uint8_t *base = reinterpret_cast<uint8_t *>(g->hq[i].p);
+        if (h->use_dense) {
+            CDB_CUDA_TRY(cudaMemcpyAsync(base, h->dense_queries, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, g->stream[i]));
+            dq[i] = reinterpret_cast<const float *>(base);
+        }
+        if (h->use_sparse) {
+            uint64_t *off = reinterpret_cast<uint64_t *>(base + dbytes);
+            uint32_t *dims = reinterpret_cast<uint32_t *>(off + nq + 1);
+            float *vals = reinterpret_cast<float *>(dims + nqp);
+            CDB_CUDA_TRY(cudaMemcpyAsync(off, h->sparse_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
+            if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(dims, h->sparse_dims, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
+            if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(vals, h->sparse_values, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
+            sq[i] = {off, dims, vals};
+        }
+    }
+    if (g->loopback) {   // slot 0's stream reads every slot's sparse queries in the re-rank
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        for (size_t i = 1; i < nl; ++i) {
+            CDB_CUDA_TRY(cudaEventRecord(g->ev[i], g->stream[i]));
+            CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[0], g->ev[i], 0));
+        }
+    }
+    // the fused rows and the error bytes on slot 0
+    const size_t no = (size_t)nq * 6 * top_k;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    Buf &o = g->err[0];
+    if ((rc = o.ensure(no * 8 + (size_t)nq * 8))) return rc;
+    uint32_t *f_ids = reinterpret_cast<uint32_t *>(o.p);
+    float *f_scores = reinterpret_cast<float *>(f_ids + no);
+    uint32_t *f_counts = reinterpret_cast<uint32_t *>(f_scores + no);
+    uint8_t *f_err = reinterpret_cast<uint8_t *>(f_counts + nq);
+    rc = hybrid_group_run(g, h, p, nq, top_k, fusion_constant_k, dq, sq, f_ids, f_scores, f_counts, h->use_dense ? f_err : nullptr, nullptr);
+    if (!rc) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        cudaStream_t s0 = g->stream[0];
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, no * 4, cudaMemcpyDeviceToHost, s0));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, no * 4, cudaMemcpyDeviceToHost, s0));
+        CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s0));
+        if (err_flags && h->use_dense) CDB_CUDA_TRY(cudaMemcpyAsync(err_flags, f_err, nq, cudaMemcpyDeviceToHost, s0));
+    }
+    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collectives included) before the locks and host buffers go
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
+    }
+    return rc;
+}
+
+cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *g, const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k,
+                                                  float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                                  uint8_t *d_err_flags, void *stream) {
+    CDB_REQUIRE(!nq || !top_k || (d_ids && d_scores && d_counts), "null output");
+    CDB_REQUIRE(!nq || d_counts, "null output");
+    CDB_REQUIRE(g, "null group");
+    HybPlan p;
+    cdb_status rc = hyb_plan(h, nq, top_k, &p);
+    if (rc) return rc;
+    if (h->use_tfidf) {
+        set_error("the sharded TF-IDF search needs the host mid-call (the group's idf): use cdb_hybrid_search_batch_sharded");
+        return CDB_UNSUPPORTED;
+    }
+    CDB_REQUIRE(g->dev.size() == 1, "the device form serves groups of one local slot (cdb_shard_group_create_rank, or one device)");
+    std::lock_guard<std::mutex> lock(g->mu);
+    if ((rc = hyb_group_check(g, h, &p))) return rc;
+    if (!nq) return CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    const cudaStream_t s = slot_stream(g, 0, (cudaStream_t)stream);
+    if (!top_k) {
+        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
+        return CDB_OK;
+    }
+    std::unique_ptr<std::shared_lock<std::shared_mutex>> shard_lock;
+    if (h->use_sparse) shard_lock.reset(new std::shared_lock<std::shared_mutex>(sparse_index_mutex(g->sparse[0])));
+    const std::vector<const float *> dq(1, h->dense_queries);
+    const std::vector<SparseQueries> sq(1, SparseQueries{h->sparse_offsets, h->sparse_dims, h->sparse_values});
+    return hybrid_group_run(g, h, p, nq, top_k, fusion_constant_k, dq, sq, d_ids, d_scores, d_counts,
+                            h->use_dense ? d_err_flags : nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"

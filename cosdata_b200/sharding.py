@@ -318,6 +318,69 @@ class ShardGroup:
         _check(self._lib.cdb_tfidf_search_batch_sharded(self._h, _ptr(o), _ptr(h), nq, k, _ptr(ids), _ptr(scores), _ptr(counts)))
         return ids[:nq], scores[:nq], counts[:nq]
 
+    def _hybrid_sources(self, dense, sparse, tfidf, dense_id_stride, host):
+        """cdb_hybrid_group_sources -> (struct, arrays to keep alive, n_queries or None).  Host form: dense = (queries f32[B, dim],
+        DenseIndex.params keywords or None), sparse = (queries as for SparseIndex.batch_search, SparseSearchOptions or None),
+        tfidf = queries as for TfIdfIndex.batch_search.  Device form: the queries are device pointers (ints): dense =
+        (d_queries, kw), sparse = ((d_offsets, d_dims, d_values), options), tfidf = (d_offsets, d_hashes)."""
+        from . import _lib
+        from .api import SparseSearchOptions, _as_csr, _ptr, _query_csr
+        src, keep, nqs = _lib.HybridGroupSources(), [], []
+        if dense is not None:
+            q, opts = (tuple(dense) + (None,))[:2]
+            if host:
+                q = np.ascontiguousarray(q, dtype=np.float32)
+                q = q[None] if q.ndim == 1 else q
+                keep.append(q)
+                nqs.append(q.shape[0])
+            src.use_dense, src.dense_queries = 1, _ptr(q) if host else q
+            src.dense_params = self._shards[0].params(0, **(opts or {}))
+            src.dense_id_stride = int(dense_id_stride)
+        if sparse is not None:
+            q, opts = (tuple(sparse) + (None,))[:2]
+            if host:
+                q = _as_csr(q)
+                keep += list(q)
+                nqs.append(len(q[0]) - 1)
+            src.use_sparse = 1
+            src.sparse_offsets, src.sparse_dims, src.sparse_values = [_ptr(a) for a in q] if host else q
+            src.sparse_params = (opts or SparseSearchOptions(0)).params()
+        if tfidf is not None:
+            q = _query_csr(tfidf) if host else tuple(tfidf)
+            if host:
+                keep += list(q)
+                nqs.append(len(q[0]) - 1)
+            src.use_tfidf = 1
+            src.tfidf_offsets, src.tfidf_hashes = [_ptr(a) for a in q] if host else q
+        if len(set(nqs)) > 1:
+            raise ValueError("every source needs the same number of queries")
+        return src, keep, (nqs[0] if nqs else 0)
+
+    def hybrid_search(self, top_k=10, fusion_constant_k=60.0, dense=None, sparse=None, tfidf=None, dense_id_stride=1):
+        """batch_hybrid_search over the group's shards of two kinds (cdb_hybrid_search_batch_sharded): dense = (queries,
+        DenseIndex.params keywords), sparse = (queries, SparseSearchOptions), tfidf = queries.  dense_id_stride =
+        max_replica_per_node for replica graphs.  -> ids u32[B, 6 * top_k], scores f32[B, 6 * top_k], counts u32[B] (the
+        whole fused union), dense err flags u8[B] (zeros without a dense source)"""
+        from .api import _check, _ptr
+        src, keep, nq = self._hybrid_sources(dense, sparse, tfidf, dense_id_stride, True)
+        w = 6 * int(top_k)
+        ids = np.zeros((max(nq, 1), max(w, 1)), np.uint32)
+        scores = np.zeros((max(nq, 1), max(w, 1)), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        err = np.zeros(max(nq, 1), np.uint8)
+        _check(self._lib.cdb_hybrid_search_batch_sharded(self._h, C.byref(src), nq, int(top_k), float(fusion_constant_k), _ptr(ids),
+                                                         _ptr(scores), _ptr(counts), _ptr(err)))
+        return ids[:nq, :w], scores[:nq, :w], counts[:nq], err[:nq]
+
+    def hybrid_search_device(self, nq, d_ids, d_scores, d_counts, d_err=None, stream_ptr=None, top_k=10, fusion_constant_k=60.0,
+                             dense=None, sparse=None, tfidf=None, dense_id_stride=1):
+        """groups of one local slot: hybrid_search on device pointers (ints), asynchronous on the stream; see _hybrid_sources
+        for the source forms.  A TF-IDF source is refused (CDB_UNSUPPORTED): the group's idf needs the host."""
+        from .api import _check
+        src, keep, _ = self._hybrid_sources(dense, sparse, tfidf, dense_id_stride, False)
+        _check(self._lib.cdb_hybrid_search_batch_sharded_device(self._h, C.byref(src), nq, int(top_k), float(fusion_constant_k), d_ids,
+                                                                d_scores, d_counts, d_err, C.c_void_p(stream_ptr) if stream_ptr else None))
+
     def close(self):
         if self._h:
             self._lib.cdb_shard_group_destroy(self._h)

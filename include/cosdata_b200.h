@@ -988,13 +988,59 @@ typedef struct {
  * CDB_INVALID_PARAMS: top_k > 341 (the dense and sparse searches take k <= 1024), a sparse source with rerank and
  * 3 * top_k * reranking_factor > 5120, a source count other than two, null queries, handles on different devices.
  * CDB_UNSUPPORTED: a dense handle with graph metadata (its HNSW searches go through cdb_search_batch_filtered[_device];
- * fuse those results with cdb_rrf_fuse and id_stride = max_replica_per_node).  Refusals of a sub-search's own parameter
+ * attach it to a one-slot shard group and use cdb_hybrid_search_batch_sharded, below).  Refusals of a sub-search's own parameter
  * checks are returned as that search returns them.  top_k = 0: empty results (out_counts zeroed), no kernel launched. */
 cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k, float fusion_constant_k,
                                    uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags);
 cdb_status cdb_hybrid_search_batch_device(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k,
                                           float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
                                           uint8_t *d_err_flags, void *stream);
+
+/* Hybrid search over a shard group (DESIGN.md section 8h): the group's dense, sparse and TF-IDF shards are already
+ * attached, so the sources name kinds, not handles; exactly two of use_dense, use_sparse, use_tfidf are 1.  The k of each
+ * params struct is ignored, as above.  dense_id_stride is the first list's id_stride when the dense side is first:
+ * max_replica_per_node for replica graphs, 0 or 1 when ids are keys; every other list has stride 1. */
+typedef struct {
+    uint32_t use_dense, use_sparse, use_tfidf;
+    const float *dense_queries;               /* [B][dim] raw f32 */
+    cdb_search_params dense_params;
+    uint32_t dense_id_stride;
+    const uint64_t *sparse_offsets;           /* CSR [B+1] */
+    const uint32_t *sparse_dims;
+    const float *sparse_values;
+    cdb_sparse_search_params sparse_params;
+    const uint64_t *tfidf_offsets;            /* CSR [B+1] of term hashes */
+    const uint32_t *tfidf_hashes;
+} cdb_hybrid_group_sources;
+
+/* The group's two sub-searches at k = 3 * top_k, as cdb_search_batch_sharded / cdb_search_batch_filtered_sharded,
+ * cdb_sparse_search_batch_sharded and cdb_tfidf_search_batch_sharded return them, fused on the device with the contract
+ * above (lists, scores, keys, output [B][6 * top_k], err_flags written only with a dense source and OR-ed over the ranks).
+ * Dense side: when every local dense shard has graph metadata, the filtered path with no filter on any query (the
+ * reference's hnsw_index.search(.., None) for a collection with a metadata schema; results carry replica ids, so pass
+ * dense_id_stride = max_replica_per_node); when none has, the path of cdb_search_batch_sharded in any mode.  A group of
+ * one local slot (cdb_shard_group_create with one device) is a real group, so a single index with graph metadata gets its
+ * hybrid search here, which cdb_hybrid_search_batch refuses.
+ * Both sub-searches run under one hold of the group's lock, one after the other in list order on the group's streams (the
+ * caller's stream in the device form), so every rank issues the same collectives in the same order; the first list lives
+ * in scratch of this call until the fusion on local slot 0 (this rank's device in a per-rank group), which every rank
+ * runs and so ends with the same rows.  Queries are fused in chunks that keep both intermediate lists within 256 MB.  The
+ * host form copies nothing back but the fused ids, scores, counts and error bytes.
+ * CDB_INVALID_PARAMS, before any copy or launch: a null group, sources or output; a source count other than two;
+ * top_k > 341; sparse rerank with 3 * top_k * reranking_factor > 5120 (and the sparse search's other parameter checks);
+ * CDB_SEARCH_ALL_CANDIDATES in dense_params; null queries of a named source; malformed query CSR (host form); a local
+ * slot without a shard of a named kind; local dense shards of which some have graph metadata and some do not, or a
+ * mode other than CDB_MODE_HNSW on metadata shards; world * 3 * top_k * 8 > 200 KB (the dense merge).  top_k = 0: counts
+ * zeroed, nothing launched.
+ * The device form serves groups of one local slot (per-rank groups and one-device local groups), takes device arrays and
+ * is asynchronous on `stream`.  It refuses a TF-IDF source with CDB_UNSUPPORTED: the group's idf sums every rank's df on
+ * the host before the scoring (cdb_tfidf_search_batch_sharded is host-only for the same reason). */
+cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *group, const cdb_hybrid_group_sources *sources, uint32_t n_queries,
+                                           uint32_t top_k, float fusion_constant_k, uint32_t *out_ids, float *out_scores,
+                                           uint32_t *out_counts, uint8_t *err_flags);
+cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *group, const cdb_hybrid_group_sources *sources,
+                                                  uint32_t n_queries, uint32_t top_k, float fusion_constant_k, uint32_t *d_ids,
+                                                  float *d_scores, uint32_t *d_counts, uint8_t *d_err_flags, void *stream);
 
 #ifdef __cplusplus
 }

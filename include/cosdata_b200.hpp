@@ -281,6 +281,20 @@ class ShardGroup {
                                                 r.counts.data(), r.err.data()));
         return r;
     }
+    // batch_hybrid_search over two kinds of the group's shards (host arrays in `sources`, exactly two use_* set): rows of
+    // 6 * top_k columns holding the whole fused union, err = the dense search's flags (zeros without a dense source)
+    SearchResults hybrid_search(const cdb_hybrid_group_sources &sources, uint32_t b, uint32_t top_k = 10,
+                                float fusion_constant_k = 60.0f) const {
+        SearchResults r;
+        r.k = 6 * top_k;
+        r.ids.resize((size_t)b * r.k);
+        r.scores.resize((size_t)b * r.k);
+        r.counts.resize(b);
+        r.err.resize(b);
+        check(cdb_hybrid_search_batch_sharded(g_, &sources, b, top_k, fusion_constant_k, r.ids.data(), r.scores.data(), r.counts.data(),
+                                              r.err.data()));
+        return r;
+    }
 
   private:
     cdb_shard_group *g_ = nullptr;
