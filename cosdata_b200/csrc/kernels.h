@@ -45,6 +45,27 @@ cdb_status sparse_index_room(cdb_sparse_index *ix, uint64_t *rows, uint64_t *row
 // drops the rows from `rows` on (their tombstones too): an append of several calls undone after a later call failed
 cdb_status sparse_index_truncate(cdb_sparse_index *ix, uint64_t rows);
 int sparse_index_device(const cdb_sparse_index *ix);
+// The device half of a top_k None search (a single index's, and each shard's of a shard group).  One chunk of queries is
+// scored, its candidates gathered per query, sorted descending and, with rerank, re-ranked and sorted again: query qi's
+// keys are keys[seg_h[qi], seg_h[qi + 1]), contiguous in device memory.  The caller holds the index's reader lock.
+struct SparseAllScratch {
+    uint64_t *slots = nullptr, *ka = nullptr, *kb = nullptr;
+    uint32_t *cnt = nullptr, *pos = nullptr, *seg = nullptr, *qa = nullptr, *qb = nullptr;
+    void *tmp = nullptr;
+    size_t tmp_bytes = 0;
+    uint32_t chunk = 0;
+    std::vector<uint32_t> seg_h;        // [chunk + 1], host
+    const uint64_t *keys = nullptr;     // the sorted keys of the last chunk (null without candidates)
+    uint64_t *spare = nullptr;          // a free buffer of as many keys
+};
+// tiles, and live rows (a query's candidates, at most)
+void sparse_index_all_bounds(const cdb_sparse_index *ix, uint64_t *n_tiles, uint64_t *n_live);
+// queries per chunk: the scratch of a chunk over at most n_tiles tiles and n_live live rows stays within 512 MB
+uint32_t sparse_all_chunk(uint32_t nq, uint64_t n_tiles, uint64_t n_live);
+cdb_status sparse_all_alloc(cdb_sparse_index *ix, uint32_t chunk, SparseAllScratch *sc, cudaStream_t s);
+cdb_status sparse_all_keys(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals,
+                           const cdb_sparse_search_params *p, uint32_t q0, uint32_t c, SparseAllScratch *sc, cudaStream_t s);
+void sparse_all_free(SparseAllScratch *sc, cudaStream_t s);
 
 // ---- tfidf.cu
 int tfidf_index_device(const cdb_tfidf_index *ix);
@@ -359,3 +380,10 @@ cdb_status tensor_u8_scan_device(const uint8_t *d_x, const uint8_t *d_q, uint32_
                                  cudaStream_t s, uint64_t *d_out_keys = nullptr);
 
 }  // namespace cdb
+
+// the results of a top_k None sparse search, in host memory: query q's entries are [off[q], off[q+1])
+struct cdb_sparse_results {
+    std::vector<uint64_t> off{0};
+    std::vector<uint32_t> ids;
+    std::vector<float> scores;
+};

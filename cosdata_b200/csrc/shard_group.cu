@@ -19,6 +19,7 @@
 #include <cstring>
 #include <memory>
 #include <mutex>
+#include <new>
 #include <shared_mutex>
 #include <string>
 #include <vector>
@@ -56,6 +57,8 @@ cdb_status sparse_shard_rerank(cdb_sparse_index *ix, const uint64_t *d_qoff, con
                                uint32_t m, const uint64_t *keys, const uint32_t *cnt, uint64_t *out, cudaStream_t s);
 cdb_status sparse_group_finalize(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t m, uint32_t k, int rerank,
                                  uint64_t *keys, const uint32_t *cnt, uint32_t *ids, float *scores, uint32_t *counts, cudaStream_t s);
+cdb_status sparse_group_merge_all(const uint64_t *gathered, size_t words, uint32_t world, const uint32_t *d_pre, uint32_t nb, uint32_t n,
+                                  int rerank, uint32_t *ids, float *scores, cudaStream_t s);
 
 // tfidf.cu: a shard group's TF-IDF search under the group's idf
 std::shared_mutex &tfidf_index_mutex(cdb_tfidf_index *ix);
@@ -755,6 +758,25 @@ static cdb_status sparse_sharded_slots(const cdb_shard_group *g) {
     return CDB_OK;
 }
 
+// the same host query batch to every local device, on each slot's stream
+static cdb_status sparse_upload_queries(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
+                                        uint32_t nq, std::vector<SparseQueries> *dq) {
+    const uint64_t nqp = q_offsets[nq];
+    cdb_status rc;
+    for (size_t i = 0; i < g->dev.size(); ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqp * 8))) return rc;
+        uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
+        uint32_t *dims = reinterpret_cast<uint32_t *>(off + nq + 1);
+        float *vals = reinterpret_cast<float *>(dims + nqp);
+        CDB_CUDA_TRY(cudaMemcpyAsync(off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
+        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(dims, q_dims, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(vals, q_values, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        (*dq)[i] = {off, dims, vals};
+    }
+    return CDB_OK;
+}
+
 cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
                                            uint32_t nq, const cdb_sparse_search_params *p, uint32_t *out_ids, float *out_scores,
                                            uint32_t *out_counts) {
@@ -772,17 +794,7 @@ cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *g, const uint64_t *q
     std::vector<std::shared_lock<std::shared_mutex>> locks;
     for (size_t i = 0; i < nl; ++i) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
     std::vector<SparseQueries> dq(nl);
-    for (size_t i = 0; i < nl; ++i) {   // the same host batch goes to every local device
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqp * 8))) return rc;
-        uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
-        uint32_t *dims = reinterpret_cast<uint32_t *>(off + nq + 1);
-        float *vals = reinterpret_cast<float *>(dims + nqp);
-        CDB_CUDA_TRY(cudaMemcpyAsync(off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
-        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(dims, q_dims, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(vals, q_values, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        dq[i] = {off, dims, vals};
-    }
+    if ((rc = sparse_upload_queries(g, q_offsets, q_dims, q_values, nq, &dq))) return rc;
     if (g->loopback) {   // slot 0's stream reads every slot's queries in phase 2
         CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
         for (size_t i = 1; i < nl; ++i) {
@@ -824,6 +836,189 @@ cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *g, const uint
     std::shared_lock<std::shared_mutex> shard_lock(sparse_index_mutex(g->sparse[0]));
     std::vector<SparseQueries> dq(1, SparseQueries{d_q_offsets, d_q_dims, d_q_values});
     return sparse_sharded_enqueue(g, nq, p, m, dq, d_ids, d_scores, d_counts, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------- top_k None over the sparse shards (DESIGN.md section 8f)
+
+// The key exchange of one scoring chunk of c queries, from the all-gathered counts cnt[r * c + qi] alone, so every rank
+// derives the same sub-batches: consecutive queries [b[s], b[s+1]) whose largest rank total `words` keeps world * words * 8
+// bytes within GROUP_GATHER_BUDGET (a sub-batch holds at least one query, which may exceed it).  Sub-batches without a key
+// are dropped: they need no exchange.
+struct KeyBatch {
+    uint32_t a, b;   // queries [a, b) of the chunk
+    size_t words;    // keys of the largest rank
+};
+static std::vector<KeyBatch> key_batches(const std::vector<uint32_t> &cnt, uint32_t world, uint32_t c) {
+    std::vector<KeyBatch> out;
+    std::vector<uint64_t> tot(world);
+    const uint64_t cap = GROUP_GATHER_BUDGET / (8ull * world);
+    for (uint32_t a = 0; a < c;) {
+        std::fill(tot.begin(), tot.end(), 0);
+        uint64_t words = 0;
+        uint32_t b = a;
+        for (; b < c; ++b) {
+            uint64_t w = 0;
+            for (uint32_t r = 0; r < world; ++r) w = std::max(w, tot[r] + cnt[(size_t)r * c + b]);
+            if (b > a && w > cap) break;
+            for (uint32_t r = 0; r < world; ++r) tot[r] += cnt[(size_t)r * c + b];
+            words = w;
+        }
+        if (words) out.push_back({a, b, (size_t)words});
+        a = b;
+    }
+    return out;
+}
+
+// Under g->mu and every local shard's reader lock.  Plan (per-rank groups: one all-gather of each rank's tiles and live
+// rows), then per scoring chunk: every local shard's device half into its own scratch; an all-gather of the per-query
+// counts; per key sub-batch, every rank's sorted keys into its slot, an all-gather, and the merge on local slot 0, copied
+// into r.  Every rank issues the same collectives: the chunk comes from group-wide maxima, the sub-batches from the
+// gathered counts.
+static cdb_status sparse_all_sharded_run(cdb_shard_group *g, const std::vector<SparseQueries> &dq, uint32_t nq,
+                                         const cdb_sparse_search_params *p, cdb_sparse_results *r, std::vector<SparseAllScratch> &sc) {
+    const size_t nl = g->dev.size();
+    const uint32_t world = g->world;
+    cdb_status rc;
+    // plan: [tiles, live rows] of every rank
+    std::vector<uint64_t> bounds(2 * (size_t)world, 0);
+    for (size_t i = 0; i < nl; ++i) sparse_index_all_bounds(g->sparse[i], &bounds[2 * (g->rank0 + i)], &bounds[2 * (g->rank0 + i) + 1]);
+    if (nl < world) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        if ((rc = g->gather[0].ensure((size_t)world * 16))) return rc;
+        CDB_CUDA_TRY(cudaMemcpyAsync(gather_buf(g, 0) + 2 * g->rank0, &bounds[2 * g->rank0], 16, cudaMemcpyHostToDevice, g->stream[0]));
+        if ((rc = group_allgather(g, 2, nullptr))) return rc;
+        CDB_CUDA_TRY(cudaMemcpyAsync(bounds.data(), gather_buf(g, 0), (size_t)world * 16, cudaMemcpyDeviceToHost, g->stream[0]));
+        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[0]));
+    }
+    uint64_t max_tiles = 0, max_live = 0, sum_live = 0;
+    for (uint32_t k = 0; k < world; ++k) {
+        max_tiles = std::max(max_tiles, bounds[2 * k]);
+        max_live = std::max(max_live, bounds[2 * k + 1]);
+        sum_live += bounds[2 * k + 1];
+    }
+    CDB_REQUIRE(sum_live < (1ull << 31), "top_k None: a shard group with 2^31 live rows or more");
+    if (!max_tiles || !max_live) return CDB_OK;   // no rank has a candidate: r holds nq empty queries
+    const uint32_t chunk = sparse_all_chunk(nq, max_tiles, max_live);
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = sparse_all_alloc(g->sparse[i], chunk, &sc[i], g->stream[i]))) return rc;
+    }
+    const cudaStream_t s0 = g->stream[0];
+    std::vector<uint32_t> cnt, pre;
+    for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        const size_t cw = ((size_t)c + 1) / 2;   // u64 words of c u32 counts
+        if (q0 && (rc = loopback_fence(g))) return rc;
+        for (size_t i = 0; i < nl; ++i) {
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+            if ((rc = sparse_all_keys(g->sparse[i], dq[i].off, dq[i].dims, dq[i].vals, p, q0, c, &sc[i], g->stream[i]))) return rc;
+            std::vector<uint32_t> &seg = sc[i].seg_h;
+            for (uint32_t qi = 0; qi < c; ++qi) seg[qi] = seg[qi + 1] - seg[qi];   // counts; seg[c] stays the total
+            if ((rc = g->gather[i].ensure((size_t)world * cw * 8))) return rc;
+            CDB_CUDA_TRY(cudaMemcpyAsync(gather_buf(g, i) + (g->rank0 + i) * cw, seg.data(), (size_t)c * 4, cudaMemcpyHostToDevice, g->stream[i]));
+        }
+        if ((rc = group_allgather(g, cw, nullptr))) return rc;
+        std::vector<uint32_t> all(world * cw * 2);
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        CDB_CUDA_TRY(cudaMemcpyAsync(all.data(), gather_buf(g, 0), all.size() * 4, cudaMemcpyDeviceToHost, s0));
+        CDB_CUDA_TRY(cudaStreamSynchronize(s0));
+        cnt.assign((size_t)world * c, 0);
+        for (uint32_t k = 0; k < world; ++k) std::copy(&all[k * cw * 2], &all[k * cw * 2] + c, &cnt[(size_t)k * c]);
+        for (uint32_t qi = 0; qi < c; ++qi) {
+            uint64_t t = 0;
+            for (uint32_t k = 0; k < world; ++k) t += cnt[(size_t)k * c + qi];
+            r->off[(size_t)q0 + qi + 1] = r->off[(size_t)q0 + qi] + t;
+        }
+        r->ids.resize(r->off[(size_t)q0 + c]);
+        r->scores.resize(r->off[(size_t)q0 + c]);
+        // every local shard's keys of query qi start at key_beg[i][qi] of its sorted run
+        std::vector<std::vector<uint32_t>> key_beg(nl, std::vector<uint32_t>((size_t)c + 1, 0));
+        for (size_t i = 0; i < nl; ++i)
+            for (uint32_t qi = 0; qi < c; ++qi) key_beg[i][qi + 1] = key_beg[i][qi] + sc[i].seg_h[qi];
+        for (const KeyBatch &kb : key_batches(cnt, world, c)) {
+            const uint32_t nb = kb.b - kb.a;
+            if ((rc = loopback_fence(g))) return rc;
+            for (size_t i = 0; i < nl; ++i) {
+                CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+                if ((rc = g->gather[i].ensure((size_t)world * kb.words * 8))) return rc;
+                const uint32_t b = key_beg[i][kb.a], e = key_beg[i][kb.b];
+                if (e > b)
+                    CDB_CUDA_TRY(cudaMemcpyAsync(gather_buf(g, i) + (g->rank0 + i) * kb.words, sc[i].keys + b, (size_t)(e - b) * 8,
+                                                 cudaMemcpyDeviceToDevice, g->stream[i]));
+            }
+            if ((rc = group_allgather(g, kb.words, nullptr))) return rc;
+            pre.assign((size_t)world * (nb + 1), 0);
+            uint64_t n = 0;
+            for (uint32_t k = 0; k < world; ++k) {
+                uint32_t *P = &pre[(size_t)k * (nb + 1)];
+                for (uint32_t j = 0; j < nb; ++j) P[j + 1] = P[j] + cnt[(size_t)k * c + kb.a + j];
+                n += P[nb];
+            }
+            CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+            if ((rc = g->sel[0].ensure(pre.size() * 4)) || (rc = g->ids[0].ensure(n * 4)) || (rc = g->scores[0].ensure(n * 4))) return rc;
+            uint32_t *d_pre = reinterpret_cast<uint32_t *>(g->sel[0].p);
+            uint32_t *d_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
+            float *d_scores = reinterpret_cast<float *>(g->scores[0].p);
+            CDB_CUDA_TRY(cudaMemcpyAsync(d_pre, pre.data(), pre.size() * 4, cudaMemcpyHostToDevice, s0));
+            if ((rc = sparse_group_merge_all(gather_buf(g, 0), kb.words, world, d_pre, nb, (uint32_t)n, p->rerank ? 1 : 0, d_ids, d_scores, s0)))
+                return rc;
+            const uint64_t base = r->off[(size_t)q0 + kb.a];
+            CDB_CUDA_TRY(cudaMemcpyAsync(r->ids.data() + base, d_ids, n * 4, cudaMemcpyDeviceToHost, s0));
+            CDB_CUDA_TRY(cudaMemcpyAsync(r->scores.data() + base, d_scores, n * 4, cudaMemcpyDeviceToHost, s0));
+            CDB_CUDA_TRY(cudaStreamSynchronize(s0));
+        }
+    }
+    return CDB_OK;
+}
+
+cdb_status cdb_sparse_search_batch_all_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
+                                               uint32_t nq, const cdb_sparse_search_params *p, cdb_sparse_results **out) {
+    CDB_REQUIRE(g && p && out, "null argument");
+    *out = nullptr;
+    CDB_REQUIRE(p->k == 0, "cdb_sparse_search_batch_all_sharded takes k = 0 (top_k None)");
+    if (nq) {
+        cdb_status rc = check_csr(q_offsets, nq, "q_offsets");
+        if (rc) return rc;
+        CDB_REQUIRE((q_dims && q_values) || !q_offsets[nq], "null query pairs");
+    }
+    if (cdb_status rc = sparse_sharded_slots(g)) return rc;
+    std::unique_ptr<cdb_sparse_results> r(new (std::nothrow) cdb_sparse_results());
+    CDB_REQUIRE(r, "out of host memory");
+    cdb_status rc = CDB_OK;
+    try {
+        r->off.assign((size_t)nq + 1, 0);
+    } catch (const std::bad_alloc &) {
+        set_error("top_k None: host allocation of the results failed");
+        return CDB_CUDA_ERROR;
+    }
+    if (!nq) {   // every rank passes the same n_queries: none runs a collective
+        *out = r.release();
+        return CDB_OK;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    const size_t nl = g->dev.size();
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    for (size_t i = 0; i < nl; ++i) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
+    std::vector<SparseQueries> dq(nl);
+    std::vector<SparseAllScratch> sc(nl);
+    rc = sparse_upload_queries(g, q_offsets, q_dims, q_values, nq, &dq);
+    if (!rc) {
+        try {
+            rc = sparse_all_sharded_run(g, dq, nq, p, r.get(), sc);
+        } catch (const std::bad_alloc &) {
+            set_error("top_k None: host allocation of the results failed");
+            rc = CDB_CUDA_ERROR;
+        }
+    }
+    for (size_t i = 0; i < nl; ++i) {   // scratch is freed behind its last use; every stream drains before the locks go
+        cudaSetDevice(g->dev[i]);
+        sparse_all_free(&sc[i], g->stream[i]);
+        const cudaError_t e = cudaStreamSynchronize(g->stream[i]);
+        if (e != cudaSuccess && !rc) { set_error(std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    if (rc) return rc;
+    *out = r.release();
+    return CDB_OK;
 }
 
 // The group's N and df of every query term: summed over the local shards' tables, then (per-rank groups) over the ranks by

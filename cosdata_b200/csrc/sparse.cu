@@ -424,6 +424,44 @@ __global__ void __launch_bounds__(256) sp_all_decode_kernel(const uint64_t *__re
     }
 }
 
+// top_k None over a shard group: the ranks' sorted runs of one key sub-batch of nb queries -> the merged entries, decoded.
+// gathered: rank r's keys at r * words, query j's run at pre[r * (nb + 1) + j] with pre[r * (nb + 1) + nb] - its start keys
+// (an exclusive scan of the rank's counts).  The n entries are numbered rank after rank; each thread takes one, finds its
+// rank and query, and writes it at its index in its run plus, for every rank, that rank's entries of the earlier queries
+// and, for every other rank, the number of that rank's keys of the query greater than it (binary search; keys are unique
+// across ranks).  One grid covers every entry of the sub-batch, however its queries' sizes are spread.
+__global__ void __launch_bounds__(256) sp_merge_runs_all_kernel(const uint64_t *__restrict__ gathered, size_t words, uint32_t world,
+                                                                const uint32_t *__restrict__ pre, uint32_t nb, uint32_t n, int rerank,
+                                                                uint32_t *__restrict__ ids, float *__restrict__ scores) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        uint32_t r = 0, l = i;
+        while (l >= pre[(size_t)r * (nb + 1) + nb]) { l -= pre[(size_t)r * (nb + 1) + nb]; ++r; }
+        const uint32_t *P = pre + (size_t)r * (nb + 1);
+        uint32_t lo = 0, hi = nb - 1;   // the query: the last j with P[j] <= l (P[nb] > l)
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if (P[mid] <= l) lo = mid; else hi = mid - 1;
+        }
+        const uint32_t j = lo;
+        const uint64_t key = gathered[(size_t)r * words + l];
+        uint32_t pos = l;
+        for (uint32_t o = 0; o < world; ++o) {
+            if (o == r) continue;
+            const uint32_t *O = pre + (size_t)o * (nb + 1);
+            const uint64_t *R = gathered + (size_t)o * words;
+            uint32_t b = O[j], e = O[j + 1];
+            pos += b;
+            while (b < e) {   // keys of rank o's run greater than `key`
+                const uint32_t mid = (b + e) >> 1;
+                if (R[mid] > key) b = mid + 1; else e = mid;
+            }
+            pos += b - O[j];
+        }
+        ids[pos] = ~(uint32_t)key;
+        scores[pos] = sp_key_score(key, rerank);
+    }
+}
+
 // sample_embedding: values > 1.0 ... > 9.0 (inverted/mod.rs:148-192)
 __global__ void sp_sample_kernel(const float *__restrict__ v, uint64_t n, unsigned long long *__restrict__ counts) {
     uint32_t c[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -455,13 +493,6 @@ struct cdb_sparse_index {
     cdb_sparse_index_desc desc;
     std::shared_mutex rw;
     PostingTiles<SparseCodec> st;   // keys: dims
-};
-
-// the results of a top_k None search, in host memory: query q's entries are [off[q], off[q+1])
-struct cdb_sparse_results {
-    std::vector<uint64_t> off{0};
-    std::vector<uint32_t> ids;
-    std::vector<float> scores;
 };
 
 namespace {
@@ -604,75 +635,29 @@ cudaError_t sp_sort_segments(void *tmp, size_t tmp_bytes, cub::DoubleBuffer<uint
     return e;
 }
 
+int qbits_of(uint32_t c) { return c > 1 ? 32 - __builtin_clz(c - 1) : 0; }
+
 // The top_k None search on device queries, under the reader lock: every candidate of every query, sorted (and re-ranked),
-// appended to r in host memory.  Per chunk of queries: score into per-(query, tile) slots, scan the slot counts, gather
-// each query's keys into one segment, sort the segments, re-rank and sort again, decode, copy out.
+// appended to r in host memory.  Per chunk: the device half (sparse_all_keys), decode, copy out.
 cdb_status search_all_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals, uint32_t nq,
                              const cdb_sparse_search_params *p, cdb_sparse_results *r, cudaStream_t s) {
     const PostingTiles<SparseCodec> &st = ix->st;
-    const uint32_t n_tiles = (uint32_t)st.h_tiles.size();
     const uint64_t n_live = st.n_rows - st.n_deleted;   // a query's candidates, at most
     r->off.assign((size_t)nq + 1, 0);
-    if (!nq || !n_tiles || !n_live) return CDB_OK;
+    if (!nq || st.h_tiles.empty() || !n_live) return CDB_OK;
     CDB_REQUIRE(n_live < (1ull << 31), "top_k None: an index with 2^31 live rows or more");
-    const size_t per_q = (size_t)n_tiles * TILE_ROWS * 8 + (size_t)n_tiles * 8 + n_live * 24;
-    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, SP_ALL_BUDGET / per_q}));
-    const uint64_t cap = (uint64_t)chunk * n_live;      // candidates of a chunk, at most (< 2^31: budget or one query)
-    const uint32_t n_slots = chunk * n_tiles;
-    auto qbits_of = [](uint32_t c) { return c > 1 ? 32 - __builtin_clz(c - 1) : 0; };
-    uint64_t *slots = nullptr, *ka = nullptr, *kb = nullptr;
-    uint32_t *cnt = nullptr, *pos = nullptr, *qa = nullptr, *qb = nullptr, *seg = nullptr;
-    void *tmp = nullptr;
-    size_t tmp_bytes = 0;
-    auto setup = [&]() -> cdb_status {
-        size_t t_scan = 0, t_sort1 = 0, t_sort2 = 0;
-        cub::DoubleBuffer<uint64_t> kd(nullptr, nullptr);
-        cub::DoubleBuffer<uint32_t> qd(nullptr, nullptr);
-        CDB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, cnt, pos, (int)n_slots + 1, s));
-        CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, t_sort1, kd, qd, (int)cap, 0, 64, s));
-        if (chunk > 1) CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort2, qd, kd, (int)cap, 0, qbits_of(chunk), s));
-        tmp_bytes = std::max({t_scan, t_sort1, t_sort2});
-        CDB_CUDA_TRY(cudaMallocAsync(&slots, (size_t)n_slots * TILE_ROWS * 8, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&cnt, ((size_t)n_slots + 1) * 4, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&pos, ((size_t)n_slots + 1) * 4, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&seg, ((size_t)chunk + 1) * 4, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&ka, cap * 8, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&kb, cap * 8, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&qa, cap * 4, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&qb, cap * 4, s));
-        CDB_CUDA_TRY(cudaMallocAsync(&tmp, std::max<size_t>(tmp_bytes, 1), s));
-        CDB_CUDA_TRY(allow_max_dynamic_smem((const void *)sp_score_tile_kernel));
-        return CDB_OK;
-    };
-    std::vector<uint32_t> h_seg((size_t)chunk + 1);
+    SparseAllScratch sc;
+    cdb_status rc = sparse_all_alloc(ix, sparse_all_chunk(nq, st.h_tiles.size(), n_live), &sc, s);
     auto run_chunk = [&](uint32_t q0, uint32_t c) -> cdb_status {
-        const SpSearch a = score_args(ix, d_qoff, d_qdims, d_qvals, p, q0, TILE_ROWS, slots, cnt);
-        sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(a);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemsetAsync(cnt + (size_t)c * n_tiles, 0, 4, s));
-        size_t tb = tmp_bytes;
-        CDB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, pos, (int)(c * n_tiles) + 1, s));
-        sp_all_gather_kernel<<<dim3(n_tiles, c), 256, 0, s>>>(slots, cnt, pos, n_tiles, ka, qa, seg);
-        CDB_LAUNCH_CHECK();
-        CDB_CUDA_TRY(cudaMemcpyAsync(h_seg.data(), seg, ((size_t)c + 1) * 4, cudaMemcpyDeviceToHost, s));
-        CDB_CUDA_TRY(cudaStreamSynchronize(s));
-        const uint32_t total = h_seg[c];
+        cdb_status rc = sparse_all_keys(ix, d_qoff, d_qdims, d_qvals, p, q0, c, &sc, s);
+        if (rc) return rc;
+        const uint32_t total = sc.seg_h[c];
         const uint64_t base = r->ids.size();
-        for (uint32_t i = 0; i < c; ++i) r->off[(size_t)q0 + i + 1] = base + h_seg[i + 1];
+        for (uint32_t i = 0; i < c; ++i) r->off[(size_t)q0 + i + 1] = base + sc.seg_h[i + 1];
         if (!total) return CDB_OK;
-        cub::DoubleBuffer<uint64_t> kd(ka, kb);
-        cub::DoubleBuffer<uint32_t> qd(qa, qb);
-        CDB_CUDA_TRY(sp_sort_segments(tmp, tmp_bytes, kd, qd, total, qbits_of(c), s));
-        if (p->rerank) {
-            const uint32_t blocks = (uint32_t)std::min<uint64_t>(((uint64_t)total + 7) / 8, 1u << 20);
-            sp_rerank_all_kernel<<<blocks, 256, 0, s>>>(kd.Current(), qd.Current(), total, q0, d_qoff, d_qdims, d_qvals, st.d_row_off,
-                                                        st.d_keys, st.d_vals, ix->desc.id_base);
-            CDB_LAUNCH_CHECK();
-            CDB_CUDA_TRY(sp_sort_segments(tmp, tmp_bytes, kd, qd, total, qbits_of(c), s));
-        }
-        uint32_t *ids = reinterpret_cast<uint32_t *>(kd.Alternate());   // the free half holds ids, then scores
+        uint32_t *ids = reinterpret_cast<uint32_t *>(sc.spare);   // the free half of the key buffers holds ids, then scores
         float *scores = reinterpret_cast<float *>(ids + total);
-        sp_all_decode_kernel<<<std::min<uint32_t>((total + 255) / 256, 1u << 16), 256, 0, s>>>(kd.Current(), total, p->rerank ? 1 : 0, ids, scores);
+        sp_all_decode_kernel<<<std::min<uint32_t>((total + 255) / 256, 1u << 16), 256, 0, s>>>(sc.keys, total, p->rerank ? 1 : 0, ids, scores);
         CDB_LAUNCH_CHECK();
         r->ids.resize(base + total);
         r->scores.resize(base + total);
@@ -681,15 +666,13 @@ cdb_status search_all_locked(cdb_sparse_index *ix, const uint64_t *d_qoff, const
         CDB_CUDA_TRY(cudaStreamSynchronize(s));
         return CDB_OK;
     };
-    cdb_status rc = setup();
     try {
-        for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) rc = run_chunk(q0, std::min(chunk, nq - q0));
+        for (uint32_t q0 = 0; q0 < nq && !rc; q0 += sc.chunk) rc = run_chunk(q0, std::min(sc.chunk, nq - q0));
     } catch (const std::bad_alloc &) {
         set_error("top_k None: host allocation of the results failed");
         rc = CDB_CUDA_ERROR;
     }
-    for (void *ptr : {(void *)slots, (void *)cnt, (void *)pos, (void *)seg, (void *)ka, (void *)kb, (void *)qa, (void *)qb, tmp})
-        if (ptr) cudaFreeAsync(ptr, s);
+    sparse_all_free(&sc, s);
     return rc;
 }
 
@@ -794,6 +777,102 @@ cdb_status sparse_group_finalize(const uint64_t *gathered, size_t words, uint32_
     CDB_CUDA_TRY(allow_max_dynamic_smem((const void *)sp_finalize_kernel));
     sp_finalize_kernel<<<nq, SP_THREADS, (size_t)sort_cap * 8, s>>>(keys, cnt, m, k, rerank ? 2 : 0, 0, nullptr, nullptr, nullptr, nullptr,
                                                                      nullptr, nullptr, 0, ids, scores, counts);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
+// ---------------------------------------------------------------- the device half of a top_k None search
+void sparse_index_all_bounds(const cdb_sparse_index *ix, uint64_t *n_tiles, uint64_t *n_live) {
+    *n_tiles = ix->st.h_tiles.size();
+    *n_live = ix->st.n_rows - ix->st.n_deleted;
+}
+
+uint32_t sparse_all_chunk(uint32_t nq, uint64_t n_tiles, uint64_t n_live) {
+    const size_t per_q = (size_t)n_tiles * TILE_ROWS * 8 + (size_t)n_tiles * 8 + n_live * 24;
+    return (uint32_t)std::max<size_t>(1, std::min<size_t>({(size_t)nq, 65535, SP_ALL_BUDGET / std::max<size_t>(per_q, 1)}));
+}
+
+// nothing is allocated for an index without tiles or live rows: sparse_all_keys gives it no candidates
+cdb_status sparse_all_alloc(cdb_sparse_index *ix, uint32_t chunk, SparseAllScratch *sc, cudaStream_t s) {
+    const PostingTiles<SparseCodec> &st = ix->st;
+    const uint32_t n_tiles = (uint32_t)st.h_tiles.size();
+    const uint64_t n_live = st.n_rows - st.n_deleted;
+    sc->chunk = chunk;
+    sc->seg_h.assign((size_t)chunk + 1, 0);
+    if (!n_tiles || !n_live) return CDB_OK;
+    const uint64_t cap = (uint64_t)chunk * n_live;      // candidates of a chunk, at most (< 2^31: budget or one query)
+    const uint32_t n_slots = chunk * n_tiles;
+    size_t t_scan = 0, t_sort1 = 0, t_sort2 = 0;
+    cub::DoubleBuffer<uint64_t> kd(nullptr, nullptr);
+    cub::DoubleBuffer<uint32_t> qd(nullptr, nullptr);
+    CDB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, sc->cnt, sc->pos, (int)n_slots + 1, s));
+    CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, t_sort1, kd, qd, (int)cap, 0, 64, s));
+    if (chunk > 1) CDB_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t_sort2, qd, kd, (int)cap, 0, qbits_of(chunk), s));
+    sc->tmp_bytes = std::max({t_scan, t_sort1, t_sort2});
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->slots, (size_t)n_slots * TILE_ROWS * 8, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->cnt, ((size_t)n_slots + 1) * 4, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->pos, ((size_t)n_slots + 1) * 4, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->seg, ((size_t)chunk + 1) * 4, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->ka, cap * 8, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->kb, cap * 8, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->qa, cap * 4, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->qb, cap * 4, s));
+    CDB_CUDA_TRY(cudaMallocAsync(&sc->tmp, std::max<size_t>(sc->tmp_bytes, 1), s));
+    CDB_CUDA_TRY(allow_max_dynamic_smem((const void *)sp_score_tile_kernel));
+    return CDB_OK;
+}
+
+void sparse_all_free(SparseAllScratch *sc, cudaStream_t s) {
+    for (void *ptr : {(void *)sc->slots, (void *)sc->cnt, (void *)sc->pos, (void *)sc->seg, (void *)sc->ka, (void *)sc->kb, (void *)sc->qa,
+                      (void *)sc->qb, sc->tmp})
+        if (ptr) cudaFreeAsync(ptr, s);
+    *sc = SparseAllScratch();
+}
+
+// Queries [q0, q0 + c), c <= sc->chunk: score into per-(query, tile) slots, scan the slot counts, gather each query's keys into
+// one segment, sort the segments, re-rank and sort again.  Waits for the stream once, to size the sort.
+cdb_status sparse_all_keys(cdb_sparse_index *ix, const uint64_t *d_qoff, const uint32_t *d_qdims, const float *d_qvals,
+                           const cdb_sparse_search_params *p, uint32_t q0, uint32_t c, SparseAllScratch *sc, cudaStream_t s) {
+    const PostingTiles<SparseCodec> &st = ix->st;
+    const uint32_t n_tiles = (uint32_t)st.h_tiles.size();
+    sc->keys = sc->spare = nullptr;
+    if (!sc->slots) {   // no tiles or no live rows
+        std::fill(sc->seg_h.begin(), sc->seg_h.begin() + c + 1, 0u);
+        return CDB_OK;
+    }
+    const SpSearch a = score_args(ix, d_qoff, d_qdims, d_qvals, p, q0, TILE_ROWS, sc->slots, sc->cnt);
+    sp_score_tile_kernel<<<dim3(n_tiles, c), SP_THREADS, SP_SCORE_SMEM, s>>>(a);
+    CDB_LAUNCH_CHECK();
+    CDB_CUDA_TRY(cudaMemsetAsync(sc->cnt + (size_t)c * n_tiles, 0, 4, s));
+    size_t tb = sc->tmp_bytes;
+    CDB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(sc->tmp, tb, sc->cnt, sc->pos, (int)(c * n_tiles) + 1, s));
+    sp_all_gather_kernel<<<dim3(n_tiles, c), 256, 0, s>>>(sc->slots, sc->cnt, sc->pos, n_tiles, sc->ka, sc->qa, sc->seg);
+    CDB_LAUNCH_CHECK();
+    CDB_CUDA_TRY(cudaMemcpyAsync(sc->seg_h.data(), sc->seg, ((size_t)c + 1) * 4, cudaMemcpyDeviceToHost, s));
+    CDB_CUDA_TRY(cudaStreamSynchronize(s));
+    const uint32_t total = sc->seg_h[c];
+    if (!total) return CDB_OK;
+    cub::DoubleBuffer<uint64_t> kd(sc->ka, sc->kb);
+    cub::DoubleBuffer<uint32_t> qd(sc->qa, sc->qb);
+    CDB_CUDA_TRY(sp_sort_segments(sc->tmp, sc->tmp_bytes, kd, qd, total, qbits_of(c), s));
+    if (p->rerank) {
+        const uint32_t blocks = (uint32_t)std::min<uint64_t>(((uint64_t)total + 7) / 8, 1u << 20);
+        sp_rerank_all_kernel<<<blocks, 256, 0, s>>>(kd.Current(), qd.Current(), total, q0, d_qoff, d_qdims, d_qvals, st.d_row_off,
+                                                    st.d_keys, st.d_vals, ix->desc.id_base);
+        CDB_LAUNCH_CHECK();
+        CDB_CUDA_TRY(sp_sort_segments(sc->tmp, sc->tmp_bytes, kd, qd, total, qbits_of(c), s));
+    }
+    sc->keys = kd.Current();
+    sc->spare = kd.Alternate();
+    return CDB_OK;
+}
+
+// a shard group's top_k None merge of one key sub-batch (sp_merge_runs_all_kernel); d_pre as the kernel takes it
+cdb_status sparse_group_merge_all(const uint64_t *gathered, size_t words, uint32_t world, const uint32_t *d_pre, uint32_t nb, uint32_t n,
+                                  int rerank, uint32_t *ids, float *scores, cudaStream_t s) {
+    if (!n) return CDB_OK;
+    sp_merge_runs_all_kernel<<<std::min<uint32_t>((n + 255) / 256, 1u << 16), 256, 0, s>>>(gathered, words, world, d_pre, nb, n, rerank,
+                                                                                             ids, scores);
     CDB_LAUNCH_CHECK();
     return CDB_OK;
 }

@@ -133,6 +133,52 @@ def merge_sparse(gathered, k, rerank_fn=None):
     return ids, scores, counts
 
 
+def merge_runs_var(keys, counts):
+    """the top_k None merge of the sharded sparse search.  keys[r]: rank r's sorted keys of a batch of queries, query after
+    query (descending within a query, unique across ranks); counts: u32[world, B], rank r's keys of each query.  ->
+    (offsets u64[B+1], merged keys u64[total]).  An entry's position is its query's output offset, plus its index in its
+    run, plus for every other rank the number of that rank's keys of the query greater than it."""
+    counts = np.asarray(counts, dtype=np.int64)
+    world, b = counts.shape
+    pre = np.zeros((world, b + 1), np.int64)
+    pre[:, 1:] = np.cumsum(counts, axis=1)
+    offsets = np.zeros(b + 1, np.uint64)
+    offsets[1:] = np.cumsum(counts.sum(axis=0))
+    out = np.zeros(int(offsets[-1]), np.uint64)
+    for q in range(b):
+        runs = [np.asarray(keys[r], dtype=np.uint64)[pre[r, q]:pre[r, q + 1]] for r in range(world)]
+        asc = [np.sort(x) for x in runs]
+        for r, x in enumerate(runs):
+            pos = int(offsets[q]) + np.arange(len(x), dtype=np.int64)
+            for o in range(world):
+                if o != r:
+                    pos += len(asc[o]) - np.searchsorted(asc[o], x, side="right")
+            out[pos] = x
+    return offsets, out
+
+
+def key_batches(counts, budget=256 << 20):
+    """the key exchange of one scoring chunk of a sharded top_k None sparse search, from the all-gathered counts
+    u32[world, c] alone: consecutive queries [a, b) whose largest rank total `words` keeps world * words * 8 bytes within
+    the budget (at least one query each), sub-batches without a key dropped -> [(a, b, words)]"""
+    counts = np.asarray(counts, dtype=np.int64)
+    world, c = counts.shape
+    cap = budget // (8 * world)
+    out, a = [], 0
+    while a < c:
+        tot, words, b = np.zeros(world, np.int64), 0, a
+        while b < c:
+            w = int((tot + counts[:, b]).max())
+            if b > a and w > cap:
+                break
+            tot += counts[:, b]
+            words, b = w, b + 1
+        if words:
+            out.append((a, b, words))
+        a = b
+    return out
+
+
 def merge_buckets(g_ids, g_scores, k=0):
     """cdb_tfidf_search_batch_sharded's merge.  g_ids / g_scores: [world, B, 512] every rank's bucket winners
     (INVALID_ID = empty bucket; all-gathered).  Per bucket the best of the ranks by `score > best`, equal scores (+0 and -0
@@ -298,6 +344,22 @@ class ShardGroup:
         _check(self._lib.cdb_sparse_search_batch_sharded(self._h, _ptr(o), _ptr(d), _ptr(v), nq, C.byref(p), _ptr(ids), _ptr(scores),
                                                          _ptr(counts)))
         return ids[:, :k], scores[:, :k], counts[:nq]
+
+    def search_sparse_all(self, queries, options):
+        """SparseIndex.batch_search_all over the whole group (top_k None: options.top_k None or 0) -> (offsets u64[B+1],
+        ids u32[total], scores f32[total]); query q's results are ids[offsets[q]:offsets[q+1]], best first"""
+        from .api import SparseResults, _as_csr, _check, _ptr
+        o, d, v = _as_csr(queries)
+        p = options.params()
+        h = C.c_void_p()
+        _check(self._lib.cdb_sparse_search_batch_all_sharded(self._h, _ptr(o), _ptr(d), _ptr(v), len(o) - 1, C.byref(p), C.byref(h)))
+        r = SparseResults(h)
+        try:
+            off = r.offsets()
+            ids, scores = r.read(0, len(off) - 1)
+        finally:
+            r.close()
+        return off, ids, scores
 
     def search_sparse_device(self, d_offsets, d_dims, d_values, nq, options, d_ids, d_scores, d_counts, stream_ptr=None):
         """per-rank groups: the sparse search on device pointers (ints), asynchronous on the stream"""

@@ -912,6 +912,25 @@ cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *group, const 
                                                   uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream);
 cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t n_queries,
                                           uint32_t k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts);
+/* Sparse top_k None over the group (params->k = 0): every candidate of every query, in a cdb_sparse_results handle read
+ * with cdb_sparse_results_offsets / _read / _destroy.  Contract: offsets, ids and score bits equal what
+ * cdb_sparse_search_batch_all returns for ONE index holding every shard's rows at their global ids, with the same appends
+ * and deletes, with and without rerank: a row's candidacy and its re-ranked score depend only on the query, the params and
+ * the row, and the result order is a total order on unique keys, so each shard scores, re-ranks and sorts its own
+ * candidates and the group merges the ranks' sorted runs.
+ *   refusals    CDB_INVALID_PARAMS before any device work, in cdb_sparse_search_batch_all's order: null group, params or
+ *               out; params->k != 0; malformed query CSR; null query pairs; then a local slot without a sparse shard.
+ *               A group whose shards hold 2^31 live rows or more in total is CDB_INVALID_PARAMS on every rank.
+ *   exchange    one all-gather of each rank's tiles and live rows (per-rank groups only), then per chunk of queries (the
+ *               same chunk on every rank, from the group's largest shard) one all-gather of the per-query candidate counts
+ *               and all-gathers of the sorted keys in sub-batches of queries whose gather buffer stays within 256 MB (a
+ *               sub-batch holds at least one query).  Local slot 0 merges and copies the results to the host.
+ *   n_queries = 0 gives a handle of 0 queries without a collective.  In a per-rank group every rank calls with the same
+ *   batch and receives the same handle contents.  Host form only: the result size is known only after scoring.  Each
+ *   local shard holds its reader lock until every stream has drained. */
+cdb_status cdb_sparse_search_batch_all_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_dims,
+                                               const float *q_values, uint32_t n_queries, const cdb_sparse_search_params *params,
+                                               cdb_sparse_results **out);
 
 /* ------------------------------------------------ hybrid search (reciprocal-rank fusion)
  * hybrid_search (src/api/vectordb/search/repo.rs:168-341) and batch_hybrid_search (repo.rs:343-555); request defaults
