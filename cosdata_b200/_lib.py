@@ -257,6 +257,8 @@ PROTOTYPES = {
     "cdb_sparse_search_batch_all_sharded": (C.c_int32, [C.c_void_p, c_vp, c_vp, c_vp, C.c_uint32, C.POINTER(SparseSearchParams),
                                                         C.POINTER(C.c_void_p)]),
     "cdb_tfidf_search_batch_sharded": (C.c_int32, [C.c_void_p, c_vp, c_vp, C.c_uint32, C.c_uint32, c_vp, c_vp, c_vp]),
+    "cdb_tfidf_search_batch_sharded_device": (C.c_int32, [C.c_void_p, c_vp, c_vp, C.c_uint32, C.c_uint64, C.c_uint32, c_vp, c_vp, c_vp,
+                                                          C.c_void_p]),
     "cdb_merge_topk_device": (C.c_int32, [C.c_int32, C.c_int32, c_u32p, c_f32p, C.c_uint32, C.c_uint32, C.c_uint32, c_u32p, c_f32p, C.c_void_p]),
     "cdb_kernel_launch_count": (C.c_uint64, []),
     "cdb_index_last_kernel_ms": (C.c_int32, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]),

@@ -24,6 +24,7 @@
 #include <string>
 #include <vector>
 
+#include "bm25_idf.h"
 #include "kernels.h"
 
 struct cdb_index;
@@ -66,9 +67,10 @@ int tfidf_index_device(const cdb_tfidf_index *ix);
 uint32_t tfidf_index_id_base(const cdb_tfidf_index *ix);
 uint64_t tfidf_index_capacity(const cdb_tfidf_index *ix);
 uint32_t tfidf_out_cols(uint32_t k);
-float tfidf_idf(uint32_t n_docs, uint32_t df);
 uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *df);
-cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, const float *d_qidf, uint32_t nq,
+cdb_status tfidf_shard_stats(const cdb_tfidf_index *ix, const uint32_t *d_qhash, uint64_t n_qh, uint32_t *out, cudaStream_t s);
+cdb_status tfidf_group_idf(const uint64_t *gathered, size_t words, uint32_t world, uint64_t n_qh, float *q_idf, cudaStream_t s);
+cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint64_t n_qh, const float *d_qidf, uint32_t nq,
                                uint2 *out, cudaStream_t s);
 cdb_status tfidf_group_finalize(const uint64_t *gathered, size_t words, uint32_t world, uint32_t nq, uint32_t k, uint32_t *ids, float *scores,
                                 uint32_t *counts, cudaStream_t s);
@@ -1026,7 +1028,8 @@ cdb_status cdb_sparse_search_batch_all_sharded(cdb_shard_group *g, const uint64_
 // with it and writes all 512 bucket winners per query into its rank's slot; one all-gather; slot 0 takes the best of the
 // ranks per bucket and sorts into ids / scores [nq][tfidf_out_cols(k)] and counts [nq] on slot 0.  The caller holds g->mu
 // and every local shard's reader lock until the scoring has run, and drains the streams.  q_offsets may be a window of a
-// larger CSR (q_offsets[0] != 0): q_hashes is that CSR's hash array.  Host only: a per-rank group waits for its df all-gather.
+// larger CSR (q_offsets[0] != 0): q_hashes is that CSR's hash array.  Host only: a per-rank group waits for its df all-gather
+// (tfidf_sharded_device_run is the device form's plan).
 static cdb_status tfidf_sharded_run(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
                                     uint32_t *f_ids, float *f_scores, uint32_t *f_counts) {
     const size_t nl = g->dev.size();
@@ -1057,7 +1060,7 @@ static cdb_status tfidf_sharded_run(cdb_shard_group *g, const uint64_t *q_offset
             for (size_t j = 0; j < stats.size(); ++j) stats[j] += all[r * words * 2 + j];
     }
     std::vector<float> idf(nqh);
-    for (uint64_t j = 0; j < nqh; ++j) idf[j] = tfidf_idf(stats[0], stats[1 + j]);
+    for (uint64_t j = 0; j < nqh; ++j) idf[j] = bm25_idf(stats[0], stats[1 + j]);
     for (size_t i = 0; i < nl; ++i) {   // queries and their idf to every local device
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
         if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqh * 8))) return rc;
@@ -1081,7 +1084,7 @@ static cdb_status tfidf_sharded_run(cdb_shard_group *g, const uint64_t *q_offset
             CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
             uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
             uint32_t *hashes = reinterpret_cast<uint32_t *>(off + nq + 1);
-            rc = tfidf_shard_winners(g->tfidf[i], off + q0, hashes, reinterpret_cast<const float *>(hashes + nqh), c,
+            rc = tfidf_shard_winners(g->tfidf[i], off + q0, hashes, nqh, reinterpret_cast<const float *>(hashes + nqh), c,
                                      reinterpret_cast<uint2 *>(gather_buf(g, i) + (g->rank0 + i) * words), g->stream[i]);
         }
         if (!rc) rc = group_allgather(g, words, nullptr);
@@ -1094,8 +1097,7 @@ static cdb_status tfidf_sharded_run(cdb_shard_group *g, const uint64_t *q_offset
     return rc;
 }
 
-// Host form only: the idf needs the host mid-call (tfidf_sharded_run).  The local shards' reader locks are held from the
-// df look-up until the scoring has run.
+// The local shards' reader locks are held from the df look-up until the scoring has run.
 cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
                                           uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
     CDB_REQUIRE(g && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
@@ -1128,6 +1130,76 @@ cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_
         CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
     }
     return rc;
+}
+
+// The device form's plan, all of it enqueued: every local slot writes its shard's [N, df of every query term] (u32) into its
+// rank's slot of the gather buffer; one all-gather; slot 0 sums N and each df over the ranks and writes the idf of every
+// query term into stream-ordered scratch; then, per group chunk, tfidf_sharded_run's scoring, all-gather and finalize into
+// the caller's arrays.  Every local slot sits on the caller's device, so each reads the caller's query arrays and slot 0's
+// idf.  The call's work follows what out_stream held, and out_stream's later work follows it.  The caller holds g->mu and
+// every local shard's reader lock through the enqueue.
+static cdb_status tfidf_sharded_device_run(cdb_shard_group *g, const uint64_t *d_qoff, const uint32_t *d_qhash, uint32_t nq, uint64_t nqh,
+                                           uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t out_stream) {
+    const size_t nl = g->dev.size();
+    const uint32_t kout = tfidf_out_cols(k), chunk = group_chunk(g, nq, 512 * 8);
+    const size_t stat_words = (nqh + 2) / 2;   // one rank's [N, df...] in u64 words
+    cdb_status rc = CDB_OK;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    for (size_t i = 0; i < nl; ++i)
+        if ((rc = g->gather[i].ensure(g->world * std::max(stat_words, (size_t)chunk * 512) * 8))) return rc;
+    const cudaStream_t s0 = slot_stream(g, 0, out_stream);
+    bool fenced = false;
+    for (size_t i = 0; i < nl; ++i) {
+        const cudaStream_t si = slot_stream(g, i, out_stream);
+        if (si == out_stream) continue;
+        if (!fenced) CDB_CUDA_TRY(cudaEventRecord(g->ev[0], out_stream));
+        fenced = true;
+        CDB_CUDA_TRY(cudaStreamWaitEvent(si, g->ev[0], 0));
+    }
+    float *q_idf = nullptr;
+    if (nqh) CDB_CUDA_TRY(cudaMallocAsync(&q_idf, nqh * 4, s0));
+    for (size_t i = 0; i < nl && !rc; ++i)
+        rc = tfidf_shard_stats(g->tfidf[i], d_qhash, nqh, reinterpret_cast<uint32_t *>(gather_buf(g, i) + (g->rank0 + i) * stat_words),
+                               slot_stream(g, i, out_stream));
+    if (!rc) rc = group_allgather(g, stat_words, out_stream);
+    if (!rc) rc = tfidf_group_idf(gather_buf(g, 0), stat_words, g->world, nqh, q_idf, s0);
+    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
+        const uint32_t c = std::min(chunk, nq - q0);
+        const size_t words = (size_t)c * 512;
+        // loopback: the slots read slot 0's idf, and overwrite their gather buffers, after slot 0's work so far
+        if ((rc = loopback_fence(g))) break;
+        for (size_t i = 0; i < nl && !rc; ++i)
+            rc = tfidf_shard_winners(g->tfidf[i], d_qoff + q0, d_qhash, nqh, q_idf, c,
+                                     reinterpret_cast<uint2 *>(gather_buf(g, i) + (g->rank0 + i) * words), slot_stream(g, i, out_stream));
+        if (!rc) rc = group_allgather(g, words, out_stream);
+        if (!rc)
+            rc = tfidf_group_finalize(gather_buf(g, 0), words, g->world, c, k, d_ids + (size_t)q0 * kout, d_scores + (size_t)q0 * kout,
+                                      d_counts + q0, s0);
+    }
+    // slot 0's stream has joined every slot's last work (collective or loopback copy)
+    if (q_idf) cudaFreeAsync(q_idf, s0);
+    if (s0 != out_stream) {
+        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], s0));
+        CDB_CUDA_TRY(cudaStreamWaitEvent(out_stream, g->ev[0], 0));
+    }
+    return rc;
+}
+
+cdb_status cdb_tfidf_search_batch_sharded_device(cdb_shard_group *g, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes, uint32_t nq,
+                                                 uint64_t n_query_hashes, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                                 void *stream) {
+    CDB_REQUIRE(g && (d_q_offsets || !nq) && (d_ids || !nq) && (d_scores || !nq) && (d_counts || !nq), "null argument");
+    CDB_REQUIRE(d_q_hashes || !nq || !n_query_hashes, "null query hashes");
+    CDB_REQUIRE(n_query_hashes < (1ull << 31), "a batch of 2^31 query terms or more");
+    const size_t nl = g->dev.size();
+    for (size_t i = 1; i < nl; ++i)
+        CDB_REQUIRE(g->dev[i] == g->dev[0], "the device form serves groups whose local slots share one device (per-rank, one-slot or loopback)");
+    for (size_t i = 0; i < nl; ++i) CDB_REQUIRE(g->tfidf[i], "a group slot has no tf-idf shard attached");
+    if (!nq) return CDB_OK;
+    std::lock_guard<std::mutex> lock(g->mu);
+    std::vector<std::shared_lock<std::shared_mutex>> locks;
+    for (size_t i = 0; i < nl; ++i) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
+    return tfidf_sharded_device_run(g, d_q_offsets, d_q_hashes, nq, n_query_hashes, k, d_ids, d_scores, d_counts, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------- hybrid search over the group (DESIGN.md section 8h)
@@ -1356,7 +1428,7 @@ cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *g, const cdb_
     cdb_status rc = hyb_plan(h, nq, top_k, &p);
     if (rc) return rc;
     if (h->use_tfidf) {
-        set_error("the sharded TF-IDF search needs the host mid-call (the group's idf): use cdb_hybrid_search_batch_sharded");
+        set_error("the hybrid device form has no TF-IDF sub-search (its plan sums the group's df on the host): use cdb_hybrid_search_batch_sharded");
         return CDB_UNSUPPORTED;
     }
     CDB_REQUIRE(g->dev.size() == 1, "the device form serves groups of one local slot (cdb_shard_group_create_rank, or one device)");

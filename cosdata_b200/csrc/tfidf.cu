@@ -5,10 +5,10 @@
 //
 // Layout (DESIGN.md section 8d).  The rows and posting tiles are a PostingTiles store (posting_tiles.cuh) keyed by term
 // hash, with entries (row_in_tile, tf bits), ascending by row inside a segment.  The host keeps the sorted table of every
-// hash the index has seen with its df (VersionedVec::len) and uploads the table and its idf (log1pf on the host) after
-// every append and delete.  A search scores one (query, tile) per CTA into shared-memory f32 accumulators plus a touched
-// flag per row, query terms strictly in the caller's order, reduces the tile to its 512 bucket winners, then merges the
-// tiles per bucket and sorts the winners.
+// hash the index has seen with its df (VersionedVec::len) and uploads the table and its df after every append and delete;
+// a kernel then computes the idf of every term on the device (bm25_idf.h).  A search scores one (query, tile) per CTA into
+// shared-memory f32 accumulators plus a touched flag per row, query terms strictly in the caller's order, reduces the tile
+// to its 512 bucket winners, then merges the tiles per bucket and sorts the winners.
 #include <algorithm>
 #include <cmath>
 #include <mutex>
@@ -18,6 +18,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 
+#include "bm25_idf.h"
 #include "kernels.h"
 #include "posting_tiles.cuh"
 
@@ -64,6 +65,7 @@ struct TfSearch {
     uint32_t id_base;
     const uint64_t *q_off;
     const uint32_t *q_hash;
+    uint64_t q_end;          // query terms the caller's arrays hold: no term at or past it is read, whatever q_off says
     uint32_t q0;             // first query of the chunk
     uint32_t n_tiles;
     uint2 *out;              // [chunk][n_tiles][512] bucket winners (id, score bits); id CDB_INVALID_ID = empty
@@ -90,7 +92,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_score_tile_kernel(TfSearch a
     const uint32_t *thash = a.thash + tile.key_base;
     const uint32_t *tseg = a.tseg + tile.key_base + t;
     const uint2 *ent = a.entries + tile.entry_base;
-    const uint64_t qb = a.q_off[q], qe = a.q_off[q + 1];
+    const uint64_t qe = min(a.q_off[q + 1], a.q_end), qb = min(a.q_off[q], qe);
     for (uint64_t j0 = qb; j0 < qe; j0 += TF_QCHUNK) {
         const uint32_t nj = (uint32_t)std::min<uint64_t>(TF_QCHUNK, qe - j0);
         if (tid < nj) {
@@ -152,6 +154,38 @@ __device__ __forceinline__ uint2 tf_bucket_winner(const uint2 *__restrict__ src,
         if (w.x != CDB_INVALID_ID && s > best) { best = s; bid = w.x; }
     }
     return make_uint2(bid, __float_as_uint(best));
+}
+
+// idf[i] = bm25_idf(n_docs, df[i]): the index's idf table after an append or a delete
+__global__ void tf_idf_table_kernel(const uint32_t *__restrict__ df, uint32_t n, uint32_t n_docs, float *__restrict__ idf) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) idf[i] = bm25_idf(n_docs, df[i]);
+}
+
+// one shard's statistics for a shard group's idf: out = [n_docs, df of hashes[0..n)] (u32; 0 for a hash the shard never saw)
+__global__ void tf_query_stats_kernel(const uint32_t *__restrict__ terms, const uint32_t *__restrict__ df, uint32_t n_terms,
+                                      uint32_t n_docs, const uint32_t *__restrict__ hashes, uint64_t n, uint32_t *__restrict__ out) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j == 0) out[0] = n_docs;
+    if (j >= n) return;
+    const uint32_t h = hashes[j];
+    const uint32_t g = lower_bound_u32(terms, n_terms, h);
+    out[1 + j] = g < n_terms && terms[g] == h ? df[g] : 0u;
+}
+
+// a shard group's idf of every query term: N and df summed over the ranks' statistics (rank r's at gathered + r * words,
+// u32, wrapping), then bm25_idf
+__global__ void tf_group_idf_kernel(const uint64_t *__restrict__ gathered, size_t words, uint32_t world, uint64_t n,
+                                    float *__restrict__ q_idf) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    uint32_t n_docs = 0, df = 0;
+    for (uint32_t r = 0; r < world; ++r) {
+        const uint32_t *st = reinterpret_cast<const uint32_t *>(gathered + r * words);
+        n_docs += st[0];
+        df += st[1 + j];
+    }
+    q_idf[j] = bm25_idf(n_docs, df);
 }
 
 // one shard's half of a shard group's search: every bucket's winner per query, [nq][512], neither sorted nor truncated
@@ -232,48 +266,50 @@ struct cdb_tfidf_index {
     std::vector<uint32_t> h_terms;   // every hash seen, ascending
     std::vector<uint32_t> h_df;      // VersionedVec::len of each
     uint32_t *d_terms = nullptr;
-    float *d_idf = nullptr;
+    uint32_t *d_df = nullptr;        // h_df on the device
+    float *d_idf = nullptr;          // bm25_idf(documents, d_df[i])
     uint64_t terms_cap = 0;
     ~cdb_tfidf_index() {
         if (d_terms) cudaFree(d_terms);
+        if (d_df) cudaFree(d_df);
         if (d_idf) cudaFree(d_idf);
     }
 };
 
 namespace {
 
-// get_idf (sparse_ann_query.rs:298-302): u32 wrapping N - df, round-to-nearest u32 -> f32, f32 add / divide, and Rust's
-// f32::ln_1p, which is the platform libm's log1pf
-float tf_idf(uint32_t n_docs, uint32_t df) {
-    const float num = (float)(uint32_t)(n_docs - df) + 0.5f;
-    const float den = (float)df + 0.5f;
-    return log1pf(num / den);
-}
-
-// the term table and its idf under `n_docs` to the device (the device is idle: the caller holds the handle exclusively
-// and has drained queued searches)
+// the term table and its df to the device, and the idf under `n_docs` computed there (the device is idle: the caller holds
+// the handle exclusively and has drained queued searches)
 cdb_status upload_terms(cdb_tfidf_index *ix, const std::vector<uint32_t> &terms, const std::vector<uint32_t> &df, uint32_t n_docs,
                         bool terms_changed, cudaStream_t s) {
     const size_t n = terms.size();
     if (n > ix->terms_cap) {
         const uint64_t cap = std::max<uint64_t>(n, 2 * ix->terms_cap);
-        uint32_t *t = nullptr;
+        uint32_t *t = nullptr, *d = nullptr;
         float *f = nullptr;
         CDB_CUDA_TRY(cudaMalloc(&t, cap * 4));
-        cudaError_t e = cudaMalloc(&f, cap * 4);
-        if (e != cudaSuccess) { cudaFree(t); set_error(std::string("cudaMalloc: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+        cudaError_t e = cudaMalloc(&d, cap * 4);
+        if (e == cudaSuccess) e = cudaMalloc(&f, cap * 4);
+        if (e != cudaSuccess) {
+            cudaFree(t);
+            if (d) cudaFree(d);
+            set_error(std::string("cudaMalloc: ") + cudaGetErrorString(e));
+            return CDB_CUDA_ERROR;
+        }
         if (ix->d_terms) cudaFree(ix->d_terms);
+        if (ix->d_df) cudaFree(ix->d_df);
         if (ix->d_idf) cudaFree(ix->d_idf);
         ix->d_terms = t;
+        ix->d_df = d;
         ix->d_idf = f;
         ix->terms_cap = cap;
         terms_changed = true;
     }
     if (!n) return CDB_OK;
-    std::vector<float> idf(n);
-    for (size_t i = 0; i < n; ++i) idf[i] = tf_idf(n_docs, df[i]);
     if (terms_changed) CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_terms, terms.data(), n * 4, cudaMemcpyHostToDevice, s));
-    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_idf, idf.data(), n * 4, cudaMemcpyHostToDevice, s));
+    CDB_CUDA_TRY(cudaMemcpyAsync(ix->d_df, df.data(), n * 4, cudaMemcpyHostToDevice, s));
+    tf_idf_table_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, s>>>(ix->d_df, (uint32_t)n, n_docs, ix->d_idf);
+    CDB_LAUNCH_CHECK();
     CDB_CUDA_TRY(cudaStreamSynchronize(s));
     return CDB_OK;
 }
@@ -281,11 +317,12 @@ cdb_status upload_terms(cdb_tfidf_index *ix, const std::vector<uint32_t> &terms,
 uint32_t out_cols(uint32_t k) { return (k == 0 || k > TF_BUCKETS) ? TF_BUCKETS : k; }
 
 // the scoring kernel's arguments for queries [q0, q0 + chunk); q_idf as TfSearch::q_idf
-TfSearch score_args(const cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, const float *q_idf, uint32_t q0, uint2 *win) {
+TfSearch score_args(const cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint64_t q_end, const float *q_idf, uint32_t q0,
+                    uint2 *win) {
     TfSearch a;
     a.entries = ix->st.entries(); a.thash = ix->st.d_tkeys; a.tseg = ix->st.d_tseg; a.deleted = ix->st.deleted();
     a.tiles = ix->st.d_tiles; a.terms = ix->d_terms; a.idf = ix->d_idf; a.q_idf = q_idf; a.n_terms = (uint32_t)ix->h_terms.size();
-    a.n_rows = ix->st.n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q0 = q0;
+    a.n_rows = ix->st.n_rows; a.id_base = ix->desc.id_base; a.q_off = d_qoff; a.q_hash = d_qhash; a.q_end = q_end; a.q0 = q0;
     a.n_tiles = (uint32_t)ix->st.h_tiles.size(); a.out = win;
     return a;
 }
@@ -311,7 +348,7 @@ cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint
     if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
-        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qhash, nullptr, q0, win));
+        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qhash, UINT64_MAX, nullptr, q0, win));
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
         tf_finalize_kernel<<<c, TF_THREADS, 0, s>>>(win, n_tiles, kout, d_ids + (size_t)q0 * kout, d_scores + (size_t)q0 * kout,
@@ -334,7 +371,6 @@ std::shared_mutex &tfidf_index_mutex(cdb_tfidf_index *ix) { return ix->rw; }
 uint32_t tfidf_index_id_base(const cdb_tfidf_index *ix) { return ix->desc.id_base; }
 uint64_t tfidf_index_capacity(const cdb_tfidf_index *ix) { return ix->desc.capacity_rows; }
 uint32_t tfidf_out_cols(uint32_t k) { return out_cols(k); }
-float tfidf_idf(uint32_t n_docs, uint32_t df) { return tf_idf(n_docs, df); }
 
 // df[i] += this index's df of hashes[i] (u32, wrapping; 0 for a hash it never saw); returns its N
 uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *df) {
@@ -345,9 +381,26 @@ uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_
     return ix->documents;
 }
 
-// one shard's half: every bucket winner of every query under the group's idf (d_qidf, one per query term) into out [nq][512]
-cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, const float *d_qidf, uint32_t nq,
-                               uint2 *out, cudaStream_t s) {
+// one shard's statistics for the group's idf, [N, df of d_qhash[0..n_qh)] as u32 at out (tf_query_stats_kernel)
+cdb_status tfidf_shard_stats(const cdb_tfidf_index *ix, const uint32_t *d_qhash, uint64_t n_qh, uint32_t *out, cudaStream_t s) {
+    tf_query_stats_kernel<<<(uint32_t)((n_qh + 256) / 256), 256, 0, s>>>(ix->d_terms, ix->d_df, (uint32_t)ix->h_terms.size(),
+                                                                      ix->documents, d_qhash, n_qh, out);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
+// the group's idf of every query term into q_idf[0..n_qh) from the all-gathered statistics (rank r's at gathered + r * words)
+cdb_status tfidf_group_idf(const uint64_t *gathered, size_t words, uint32_t world, uint64_t n_qh, float *q_idf, cudaStream_t s) {
+    if (!n_qh) return CDB_OK;
+    tf_group_idf_kernel<<<(uint32_t)((n_qh + 255) / 256), 256, 0, s>>>(gathered, words, world, n_qh, q_idf);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
+}
+
+// one shard's half: every bucket winner of every query under the group's idf (d_qidf, one per query term) into out [nq][512].
+// No term at or past n_qh is read.
+cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint64_t n_qh, const float *d_qidf,
+                               uint32_t nq, uint2 *out, cudaStream_t s) {
     if (!nq) return CDB_OK;
     const uint32_t n_tiles = (uint32_t)ix->st.h_tiles.size();
     if (n_tiles == 0) {   // every bucket empty: id CDB_INVALID_ID
@@ -363,7 +416,7 @@ cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, cons
     if (e != cudaSuccess) { set_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
-        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qhash, d_qidf, q0, win));
+        tf_score_tile_kernel<<<dim3(n_tiles, c), TF_THREADS, TF_SCORE_SMEM, s>>>(score_args(ix, d_qoff, d_qhash, n_qh, d_qidf, q0, win));
         g_launch_count.fetch_add(1, std::memory_order_relaxed);
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error(std::string("kernel launch: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; break; }
         tf_winners_kernel<<<c, TF_THREADS, 0, s>>>(win, n_tiles, out + (size_t)q0 * TF_BUCKETS);

@@ -380,6 +380,14 @@ class ShardGroup:
         _check(self._lib.cdb_tfidf_search_batch_sharded(self._h, _ptr(o), _ptr(h), nq, k, _ptr(ids), _ptr(scores), _ptr(counts)))
         return ids[:nq], scores[:nq], counts[:nq]
 
+    def search_tfidf_device(self, d_offsets, d_hashes, nq, n_hashes, top_k, d_ids, d_scores, d_counts, stream_ptr=None):
+        """search_tfidf on device pointers (ints), asynchronous on the stream: d_offsets u64[nq + 1] with d_offsets[0] = 0 and
+        d_offsets[nq] = n_hashes, d_hashes u32[n_hashes], d_ids / d_scores [nq, kout], d_counts u32[nq].  Groups whose local
+        slots share the arrays' device: per-rank, one-slot and loopback groups."""
+        from .api import _check
+        _check(self._lib.cdb_tfidf_search_batch_sharded_device(self._h, d_offsets, d_hashes, nq, n_hashes, int(top_k or 0), d_ids,
+                                                               d_scores, d_counts, C.c_void_p(stream_ptr) if stream_ptr else None))
+
     def _hybrid_sources(self, dense, sparse, tfidf, dense_id_stride, host):
         """cdb_hybrid_group_sources -> (struct, arrays to keep alive, n_queries or None).  Host form: dense = (queries f32[B, dim],
         DenseIndex.params keywords or None), sparse = (queries as for SparseIndex.batch_search, SparseSearchOptions or None),
@@ -437,7 +445,7 @@ class ShardGroup:
     def hybrid_search_device(self, nq, d_ids, d_scores, d_counts, d_err=None, stream_ptr=None, top_k=10, fusion_constant_k=60.0,
                              dense=None, sparse=None, tfidf=None, dense_id_stride=1):
         """groups of one local slot: hybrid_search on device pointers (ints), asynchronous on the stream; see _hybrid_sources
-        for the source forms.  A TF-IDF source is refused (CDB_UNSUPPORTED): the group's idf needs the host."""
+        for the source forms.  A TF-IDF source is refused (CDB_UNSUPPORTED): its TF-IDF sub-search is the host form's."""
         from .api import _check
         src, keep, _ = self._hybrid_sources(dense, sparse, tfidf, dense_id_stride, False)
         _check(self._lib.cdb_hybrid_search_batch_sharded_device(self._h, C.byref(src), nq, int(top_k), float(fusion_constant_k), d_ids,

@@ -817,8 +817,9 @@ cdb_status cdb_sparse_index_append_itoe(cdb_sparse_index *index, const char *col
  * it; a delete in the row's insert version removes the entry (-1); a delete in a later version marks the entry and pushes
  * a tombstone word, both of which count (+1).  So df can exceed N.
  * idf (get_idf, sparse_ann_query.rs:298-302) = log1pf(((N - df) as f32 + 0.5) / (df as f32 + 0.5)) with u32 wrapping
- * N - df and round-to-nearest u32 -> f32; computed on the host with the C library's log1pf (Rust's f32::ln_1p) and
- * uploaded at the end of every append and delete, for every term.
+ * N - df and round-to-nearest u32 -> f32, and Rust's f32::ln_1p, the C library's log1pf.  At the end of every append and
+ * delete the df of every term is uploaded and the idf computed on the device by the fdlibm log1pf (csrc/bm25_idf.h),
+ * which gives glibc's log1pf bits on every non-negative finite float.
  * Versions.  append and delete_rows take the transaction's version; versions passed to either must not decrease (with it
  * every list is in ascending id order, as push_sorted keeps it, versioned_vec.rs:207-226).
  *
@@ -896,12 +897,13 @@ cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *index, const uint64_t 
  *               the same: a row outside the group's top m can re-rank into the top k.)  Queries are searched in chunks that
  *               keep the gather buffer within 256 MB; each local shard holds its reader lock through both phases.
  *               The device form (per-rank groups only) takes device arrays and is asynchronous on `stream`.
- *   TF-IDF      idf depends on the whole corpus: N = sum of the shards' N, df = sum of their df (u32, wrapping), gathered on
- *               the host (per-rank groups: one all-gather of 1 + query terms u32 per rank) and idf computed on the host
- *               with the function a single index uses.  Each shard scores under that idf and hands in all 512 bucket
- *               winners per query; per bucket the best of the ranks wins with `>`, equal scores (+0 and -0 too) going to
- *               the smaller id, then they are sorted and truncated as in cdb_tfidf_search_batch.  Each local shard holds its
- *               reader lock from the df look-up through the scoring.  Host form only: the idf needs the host mid-call. */
+ *   TF-IDF      idf depends on the whole corpus: N = sum of the shards' N, df = sum of their df (u32, wrapping), and idf
+ *               computed with the function a single index uses (csrc/bm25_idf.h).  The host form sums them on the host
+ *               (per-rank groups: one all-gather of 1 + query terms u32 per rank, waited for); the device form sums them on
+ *               the device.  Each shard scores under that idf and hands in all 512 bucket winners per query; per bucket the
+ *               best of the ranks wins with `>`, equal scores (+0 and -0 too) going to the smaller id, then they are sorted
+ *               and truncated as in cdb_tfidf_search_batch.  Each local shard holds its reader lock from the df look-up
+ *               through the scoring. */
 cdb_status cdb_shard_group_attach_sparse(cdb_shard_group *group, uint32_t local_slot, cdb_sparse_index *shard);
 cdb_status cdb_shard_group_attach_tfidf(cdb_shard_group *group, uint32_t local_slot, cdb_tfidf_index *shard);
 cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_dims,
@@ -912,6 +914,19 @@ cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *group, const 
                                                   uint32_t *d_ids, float *d_scores, uint32_t *d_counts, void *stream);
 cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t n_queries,
                                           uint32_t k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts);
+/* The TF-IDF search with every array in DEVICE memory, asynchronous on `stream` (NULL = the legacy default stream): no host
+ * synchronisation and no device-to-host copy.  Ids, counts and score bits equal cdb_tfidf_search_batch_sharded's on the same
+ * group and batch.  n_query_hashes must equal d_q_offsets[n_queries] (d_q_offsets[0] = 0): the host sizes the df exchange by
+ * it.  The device CSR is not validated, but no kernel reads d_q_hashes at or past n_query_hashes.  Each local slot writes its
+ * shard's [N, df of every query term] into its rank's slot of the gather buffer, one all-gather brings them to every rank,
+ * and a kernel sums them and computes the idf of every query term; the scoring, all-gather and merge follow as in the host
+ * form.  Served groups: those whose local slots all sit on one device, the one holding the caller's arrays -- per-rank
+ * groups, one-slot local groups and loopback groups (a device listed more than once).
+ * CDB_INVALID_PARAMS, before any device work: null arguments (with n_queries > 0), n_query_hashes >= 2^31, a local group
+ * spanning devices, a local slot without a TF-IDF shard.  n_queries = 0 returns with nothing launched. */
+cdb_status cdb_tfidf_search_batch_sharded_device(cdb_shard_group *group, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes,
+                                                 uint32_t n_queries, uint64_t n_query_hashes, uint32_t k, uint32_t *d_ids,
+                                                 float *d_scores, uint32_t *d_counts, void *stream);
 /* Sparse top_k None over the group (params->k = 0): every candidate of every query, in a cdb_sparse_results handle read
  * with cdb_sparse_results_offsets / _read / _destroy.  Contract: offsets, ids and score bits equal what
  * cdb_sparse_search_batch_all returns for ONE index holding every shard's rows at their global ids, with the same appends
@@ -1052,8 +1067,8 @@ typedef struct {
  * mode other than CDB_MODE_HNSW on metadata shards; world * 3 * top_k * 8 > 200 KB (the dense merge).  top_k = 0: counts
  * zeroed, nothing launched.
  * The device form serves groups of one local slot (per-rank groups and one-device local groups), takes device arrays and
- * is asynchronous on `stream`.  It refuses a TF-IDF source with CDB_UNSUPPORTED: the group's idf sums every rank's df on
- * the host before the scoring (cdb_tfidf_search_batch_sharded is host-only for the same reason). */
+ * is asynchronous on `stream`.  It refuses a TF-IDF source with CDB_UNSUPPORTED: its TF-IDF sub-search is the host form's,
+ * which sums every rank's df on the host before the scoring (cdb_tfidf_search_batch_sharded_device is not wired in yet). */
 cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *group, const cdb_hybrid_group_sources *sources, uint32_t n_queries,
                                            uint32_t top_k, float fusion_constant_k, uint32_t *out_ids, float *out_scores,
                                            uint32_t *out_counts, uint8_t *err_flags);

@@ -1,7 +1,9 @@
 """Sharded sparse and TF-IDF search against one index over the same corpus: host-form call time (queries in, results out,
 median of --steps calls after one warm-up) at batch 1 / 64 / 1024, sparse with and without the raw-value re-rank (top 10,
 factor 5) and TF-IDF (top 10), plus a parity check of every batch (ids, counts and score bits of the group against the
-single index).  Corpora: the 1M-row corpora of tools/bench_sparse.py and tools/bench_tfidf.py, split into --shards
+single index).  TF-IDF also times the device form (cdb_tfidf_search_batch_sharded_device: queries and results in device
+memory, the group's idf summed on the device) by CUDA events over --steps calls on one stream, next to the host form, on
+the --shards group and on a one-slot group holding the whole index, and checks its results against the host form's.  Corpora: the 1M-row corpora of tools/bench_sparse.py and tools/bench_tfidf.py, split into --shards
 contiguous id ranges.  With one GPU the shards share it and the gathers are device copies (loopback), so the numbers are
 the protocol's overhead on one card, not scaling; with as many GPUs as shards each shard has its own card and NCCL.
 Prints the card and its power limit, then one JSON line per workload.
@@ -23,7 +25,7 @@ sys.path.insert(0, ROOT)
 import cosdata_b200 as cdb  # noqa: E402
 from cosdata_b200.sharding import ShardGroup, shard_range  # noqa: E402
 from tests.sparse_data import concat_csr, slice_csr, zipf_csr  # noqa: E402
-from tests.tfidf_data import zipf_docs, zipf_queries  # noqa: E402
+from tests.tfidf_data import query_csr, zipf_docs, zipf_queries  # noqa: E402
 
 CHUNK = 500_000
 VOCAB_TFIDF = 1_000_000
@@ -49,12 +51,40 @@ def same(a, b):
             and np.array_equal(np.ascontiguousarray(a[1]).view(np.uint32), np.ascontiguousarray(b[1]).view(np.uint32)))
 
 
+def device_form(g, qs, k, steps):
+    """(ms per call by CUDA events, results) of the group's device-form TF-IDF search on one torch stream"""
+    import torch
+    dev = torch.device("cuda", 0)
+    o, h = query_csr(qs)
+    d_o = torch.from_numpy(o.astype(np.int64)).to(dev)
+    d_h = torch.from_numpy(h.view(np.int32)).to(dev)
+    nq = len(qs)
+    ids = torch.zeros((nq, k), dtype=torch.int32, device=dev)
+    sc = torch.zeros((nq, k), dtype=torch.float32, device=dev)
+    ct = torch.zeros(nq, dtype=torch.int32, device=dev)
+    s = torch.cuda.current_stream(dev)
+
+    def call():
+        g.search_tfidf_device(d_o.data_ptr(), d_h.data_ptr(), nq, int(h.size), k, ids.data_ptr(), sc.data_ptr(), ct.data_ptr(),
+                              s.cuda_stream)
+    call()
+    s.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(s)
+    for _ in range(steps):
+        call()
+    e1.record(s)
+    e1.synchronize()
+    return e0.elapsed_time(e1) / steps, (ids.cpu().numpy().view(np.uint32), sc.cpu().numpy(), ct.cpu().numpy().view(np.uint32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=1_000_000)
     ap.add_argument("--shards", type=int, default=2)
     ap.add_argument("--steps", type=int, default=10)
     a = ap.parse_args()
+    import torch  # noqa: F401  before the library can load a system libnccl.so.2 that torch's CUDA library cannot share
     assert cdb.device_count() > 0, "needs a CUDA device"
     n, w = a.rows, a.shards
     devs = list(range(w)) if cdb.device_count() >= w else [0] * w
@@ -105,6 +135,8 @@ def main():
         ix.append(piece, 1)
         g.attach_tfidf(r, ix)
         parts.append(ix)
+    one = ShardGroup.local([0])
+    one.attach_tfidf(0, whole)
     for b in (1, 64, 1024):
         q = tq[:b]
         single = timed(lambda: whole.batch_search(q, 10), a.steps)
@@ -113,6 +145,13 @@ def main():
                    sharded_ms=round(sharded, 3), sharded_over_single=round(sharded / single, 3),
                    parity=bool(same(g.search_tfidf(q, 10), whole.batch_search(q, 10))))
         print(json.dumps(res), flush=True)
+        for label, grp in ((f"{w}_slots_{mode}", g), ("1_slot", one)):
+            host = timed(lambda: grp.search_tfidf(q, 10), a.steps)
+            dev_ms, got = device_form(grp, q, 10, a.steps)
+            res = dict(workload="tfidf_device_form", group=label, rows=n, batch=b, top_k=10, card=name, host_form_ms=round(host, 3),
+                       device_form_event_ms=round(dev_ms, 3), parity_with_host_form=bool(same(got, grp.search_tfidf(q, 10))))
+            print(json.dumps(res), flush=True)
+    one.close()
     g.close()
     for x in parts + [whole]:
         x.close()
