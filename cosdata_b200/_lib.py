@@ -265,6 +265,7 @@ PROTOTYPES = {
     "cdb_index_hnsw_profile": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
     "cdb_debug_set_hnsw_flags": (C.c_int32, [C.c_uint32]),
     "cdb_debug_tensor_peak": (C.c_int32, [C.c_int32, C.c_int32, C.c_uint32, C.POINTER(C.c_double), C.POINTER(C.c_float)]),
+    "cdb_debug_bm25": (C.c_int32, [C.c_int32, c_f32p, C.c_uint64, c_f32p, c_u32p, c_u32p, C.c_uint64, c_f32p, C.c_void_p]),
     "cdb_index_set_raw_f32": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]),
     "cdb_index_raw_missing": (C.c_uint64, [C.c_void_p]),
     "cdb_index_fill_raw_from_itoe": (C.c_int32, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),

@@ -1099,6 +1099,24 @@ def _query_csr(queries):
     return off, np.array([h for q in queries for h in q], np.uint32)
 
 
+def debug_bm25_host(x=(), n_docs=(), df=()):
+    """the library's host copy of csrc/bm25_idf.h, the one a shard group's host form runs
+    -> (bm25_log1pf(x) f32[n], bm25_idf(n_docs, df) f32[m])"""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    n_docs, df = np.ascontiguousarray(n_docs, dtype=np.uint32), np.ascontiguousarray(df, dtype=np.uint32)
+    if n_docs.shape != df.shape:
+        raise ValueError("n_docs and df differ in length")
+    out_log1p, out_idf = np.empty_like(x), np.empty(df.shape, np.float32)
+    _check(_lib.load().cdb_debug_bm25(0, _ptr(x), x.size, _ptr(out_log1p), _ptr(n_docs), _ptr(df), df.size, _ptr(out_idf), None))
+    return out_log1p, out_idf
+
+
+def debug_bm25_device(d_x, n, d_out_log1p, d_n_docs, d_df, n_pairs, d_out_idf, stream_ptr=None):
+    """the library's device copy of csrc/bm25_idf.h, the one the idf kernels inline, on device pointers (ints) of the current
+    device: bm25_log1pf(d_x[:n]) -> d_out_log1p, bm25_idf(d_n_docs, d_df)[:n_pairs] -> d_out_idf; asynchronous on the stream"""
+    _check(_lib.load().cdb_debug_bm25(1, d_x, n, d_out_log1p, d_n_docs, d_df, n_pairs, d_out_idf, stream_ptr))
+
+
 class TfIdfIndex:
     """TFIDFIndex's IndexOps surface on one GPU (cdb_tfidf_index) from (term_hash, tf) pairs.  Row r has id id_base + r."""
 

@@ -7,7 +7,8 @@
 // copy of it (x < 0x3ed413d7 unsplit, mantissa split at 0x3504f7, 2^-29 and 2^-54 for tiny x): on every
 // non-negative finite float, a range that holds every argument the idf formula produces, it returns the C library's
 // log1pf bit for bit.  tests/test_bm25_idf.py sweeps all 2^31 - 2^23 such floats against the host's log1pf and fails on
-// the first difference.
+// the first difference; tests/test_gpu_bm25_idf.py sweeps them through the library's compiled device copy and checks
+// bm25_idf through its device and host copies (cdb_debug_bm25).
 //
 // Bit identity needs every float operation rounded on its own.  On the device each one is an explicit __f*_rn intrinsic,
 // which nvcc never contracts into an FFMA.  On the host the operations are plain: the library's host flags (-O2, no

@@ -188,6 +188,15 @@ __global__ void tf_group_idf_kernel(const uint64_t *__restrict__ gathered, size_
     q_idf[j] = bm25_idf(n_docs, df);
 }
 
+// cdb_debug_bm25's device form: the bm25_log1pf and bm25_idf the two kernels above inline, over arrays (grid-stride)
+__global__ void tf_debug_bm25_kernel(const float *__restrict__ x, uint64_t n, float *__restrict__ out_log1p,
+                                     const uint32_t *__restrict__ n_docs, const uint32_t *__restrict__ df, uint64_t n_pairs,
+                                     float *__restrict__ out_idf) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out_log1p[i] = bm25_log1pf(x[i]);
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_pairs; j += stride) out_idf[j] = bm25_idf(n_docs[j], df[j]);
+}
+
 // one shard's half of a shard group's search: every bucket's winner per query, [nq][512], neither sorted nor truncated
 __global__ void __launch_bounds__(TF_THREADS, 1) tf_winners_kernel(const uint2 *__restrict__ in, uint32_t n_tiles, uint2 *__restrict__ out) {
     out[(size_t)blockIdx.x * TF_BUCKETS + threadIdx.x] = tf_bucket_winner(in + (size_t)blockIdx.x * n_tiles * TF_BUCKETS, n_tiles);
@@ -667,6 +676,24 @@ cdb_status cdb_tfidf_search_batch(cdb_tfidf_index *ix, const uint64_t *q_offsets
     }
     cudaFreeAsync(buf, s);
     return rc;
+}
+
+// the library's two copies of the idf arithmetic (bm25_idf.h): the device one as the idf kernels run it, the host one as
+// tfidf_sharded_run (shard_group.cu, same flags) runs it
+cdb_status cdb_debug_bm25(int32_t on_device, const float *x, uint64_t n, float *out_log1p, const uint32_t *n_docs, const uint32_t *df,
+                          uint64_t n_pairs, float *out_idf, void *stream) {
+    CDB_REQUIRE((x && out_log1p) || !n, "null argument");
+    CDB_REQUIRE((n_docs && df && out_idf) || !n_pairs, "null argument");
+    if (!on_device) {
+        for (uint64_t i = 0; i < n; ++i) out_log1p[i] = bm25_log1pf(x[i]);
+        for (uint64_t j = 0; j < n_pairs; ++j) out_idf[j] = bm25_idf(n_docs[j], df[j]);
+        return CDB_OK;
+    }
+    if (!n && !n_pairs) return CDB_OK;
+    const uint64_t blocks = std::min<uint64_t>((std::max(n, n_pairs) + 255) / 256, 4096);
+    tf_debug_bm25_kernel<<<(uint32_t)blocks, 256, 0, (cudaStream_t)stream>>>(x, n, out_log1p, n_docs, df, n_pairs, out_idf);
+    CDB_LAUNCH_CHECK();
+    return CDB_OK;
 }
 
 }  // extern "C"

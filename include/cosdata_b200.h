@@ -673,6 +673,13 @@ cdb_status cdb_index_hnsw_profile(cdb_index *index, int32_t enable, uint64_t *ou
  * TOP/s resp. TFLOP/s: the measured roofline denominator of the integer tensor path (MEASURED_PEAKS.json only has bf16).
  * iters = 0 -> default length (~10 ms). */
 cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters, double *out_tops, float *out_ms);
+/* the BM25 idf arithmetic (csrc/bm25_idf.h) as the library runs it, so that a binding can check its bits against the
+ * platform's log1pf (f32::ln_1p): bm25_log1pf(x[i]) -> out_log1p[i] for i < n, and
+ * bm25_idf(n_docs[j], df[j]) -> out_idf[j] for j < n_pairs.  on_device != 0: the device copy the idf kernels inline, every
+ * pointer a device pointer on the current device, enqueued on `stream` (NULL = the legacy default stream), asynchronous.
+ * on_device == 0: the host copy a shard group's host form runs, host pointers, synchronous (stream unused). */
+cdb_status cdb_debug_bm25(int32_t on_device, const float *x, uint64_t n, float *out_log1p, const uint32_t *n_docs,
+                          const uint32_t *df, uint64_t n_pairs, float *out_idf, void *stream);
 /* former measurement switch of CDB_MODE_HNSW kernel variants.  HNSW search now has one kernel per graph kind, so every value
  * is accepted and selects nothing; the entry point stays for callers built against it. */
 cdb_status cdb_debug_set_hnsw_flags(uint32_t flags);

@@ -6,73 +6,24 @@ log1pf.  That is only right while the two agree bit for bit, so this sweeps ever
 argument is always one) and compares bm25_idf with the log1pf formula on edge and sampled (N, df) pairs.  It is meant to
 fail loudly on a machine whose C library's log1pf differs: there the device idf no longer matches the reference.
 
-The driver is built with g++ under the library's host flags (-O2, no -march) plus -ffp-contract=off and OpenMP."""
-import os
-import shutil
-import subprocess
-
+The driver (tests/bm25_driver.py) is built with g++ under the library's host flags (-O2, no -march) plus -ffp-contract=off
+and OpenMP.  tests/test_gpu_bm25_idf.py checks the library's own device and host copies of the header against the same
+C library."""
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "cosdata_b200", "csrc")
-GXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-
-DRIVER = r"""
-#include <cmath>
-#include <cstdio>
-#include <cstring>
-#include "bm25_idf.h"
-
-static uint32_t fbits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
-
-// get_idf as the reference writes it, with the C library's log1pf
-static float libc_idf(uint32_t n_docs, uint32_t df) {
-    const float num = (float)(uint32_t)(n_docs - df) + 0.5f;
-    const float den = (float)df + 0.5f;
-    return log1pf(num / den);
-}
-
-int main(int argc, char **argv) {
-    if (argc > 1 && !strcmp(argv[1], "sweep")) {
-        // every non-negative finite float: bits 0 .. 0x7f7fffff
-        unsigned long long bad = 0;
-        uint32_t first = 0xffffffffu;
-        #pragma omp parallel for schedule(static, 1 << 20) reduction(+ : bad)
-        for (long long i = 0; i < 0x7f800000LL; ++i) {
-            const uint32_t u = (uint32_t)i;
-            float x;
-            memcpy(&x, &u, 4);
-            if (fbits(bm25_log1pf(x)) != fbits(log1pf(x))) {
-                ++bad;
-                #pragma omp critical
-                if (u < first) first = u;
-            }
-        }
-        printf("%llu %u\n", bad, first);
-        return 0;
-    }
-    // pairs: "N df" per line on stdin -> "bm25_idf_bits libc_bits" per line
-    unsigned n, d;
-    while (scanf("%u %u", &n, &d) == 2) printf("%u %u\n", fbits(bm25_idf(n, d)), fbits(libc_idf(n, d)));
-    return 0;
-}
-"""
+from tests import bm25_driver
 
 
 @pytest.fixture(scope="module")
-def driver(tmp_path_factory):
-    if not GXX:
+def driver():
+    if not bm25_driver.GXX:
         pytest.fail("g++ is needed to check bm25_idf.h against the C library's log1pf")
-    d = tmp_path_factory.mktemp("bm25")
-    src, exe = d / "driver.cpp", d / "driver"
-    src.write_text(DRIVER)
-    subprocess.run([GXX, "-O2", "-ffp-contract=off", "-fopenmp", "-I", CSRC, str(src), "-o", str(exe), "-lm"], check=True)
-    return str(exe)
+    return bm25_driver.build()
 
 
 def test_bm25_log1pf_equals_the_c_librarys_log1pf_on_every_non_negative_float(driver):
-    out = subprocess.run([driver, "sweep"], check=True, capture_output=True, text=True).stdout.split()
+    out = bm25_driver.run(driver, "sweep").split()
     bad, first = int(out[0]), int(out[1])
     assert bad == 0, (f"bm25_log1pf differs from this C library's log1pf on {bad} inputs, the first at bits {first:#010x}: "
                       "the device idf would not match the reference's f32::ln_1p here")
@@ -94,9 +45,7 @@ def idf_pairs():
 
 def test_bm25_idf_on_edge_and_sampled_pairs(driver):
     pairs = idf_pairs()
-    inp = "".join(f"{a} {b}\n" for a, b in pairs)
-    out = np.array(subprocess.run([driver], input=inp, check=True, capture_output=True, text=True).stdout.split(), np.uint64)
-    got, want = out[0::2], out[1::2]
+    got, want = bm25_driver.pairs(driver, *zip(*pairs))
     assert got.size == len(pairs)
     bad = np.nonzero(got != want)[0]
     assert bad.size == 0, f"bm25_idf differs on {bad.size} pairs, the first (N, df) = {pairs[bad[0]]}"
