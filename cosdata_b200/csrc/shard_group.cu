@@ -24,7 +24,6 @@
 #include <string>
 #include <vector>
 
-#include "bm25_idf.h"
 #include "kernels.h"
 
 struct cdb_index;
@@ -67,7 +66,6 @@ int tfidf_index_device(const cdb_tfidf_index *ix);
 uint32_t tfidf_index_id_base(const cdb_tfidf_index *ix);
 uint64_t tfidf_index_capacity(const cdb_tfidf_index *ix);
 uint32_t tfidf_out_cols(uint32_t k);
-uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *df);
 cdb_status tfidf_shard_stats(const cdb_tfidf_index *ix, const uint32_t *d_qhash, uint64_t n_qh, uint32_t *out, cudaStream_t s);
 cdb_status tfidf_group_idf(const uint64_t *gathered, size_t words, uint32_t world, uint64_t n_qh, float *q_idf, cudaStream_t s);
 cdb_status tfidf_shard_winners(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint32_t *d_qhash, uint64_t n_qh, const float *d_qidf, uint32_t nq,
@@ -237,8 +235,7 @@ struct cdb_shard_group {
     std::vector<cdb_tfidf_index *> tfidf;
     std::vector<cudaStream_t> stream;
     std::vector<cudaEvent_t> ev;
-    std::vector<Buf> gather, q, ids, scores, counts, err, sel;
-    std::vector<Buf> hq;                  // a hybrid search's dense and sparse queries (host form), kept apart from q
+    std::vector<Buf> gather, q, ids, scores, counts, rows, sel;   // rows: a host form's final rows (slot 0)
     std::mutex mu;
 };
 
@@ -249,14 +246,103 @@ static cdb_status group_alloc_slots(cdb_shard_group *g, size_t n) {
     g->tfidf.assign(n, nullptr);
     g->stream.assign(n, nullptr);
     g->ev.assign(n, nullptr);
-    g->gather.resize(n); g->q.resize(n); g->ids.resize(n); g->scores.resize(n); g->counts.resize(n); g->err.resize(n); g->sel.resize(n);
-    g->hq.resize(n);
+    g->gather.resize(n); g->q.resize(n); g->ids.resize(n); g->scores.resize(n); g->counts.resize(n); g->rows.resize(n); g->sel.resize(n);
     for (size_t i = 0; i < n; ++i) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
         CDB_CUDA_TRY(cudaStreamCreateWithFlags(&g->stream[i], cudaStreamNonBlocking));
         CDB_CUDA_TRY(cudaEventCreateWithFlags(&g->ev[i], cudaEventDisableTiming));
     }
     return CDB_OK;
+}
+
+// ---------------------------------------------------------------- the host forms' staging: queries in, final rows out
+
+struct HostArray {
+    const void *h;
+    size_t bytes;   // 0: not copied
+};
+
+// where a host form's query arrays landed: array j on local slot i at base[i] + off[j]
+struct Staged {
+    std::vector<uint8_t *> base;
+    std::vector<size_t> off;
+    template <class T> const T *at(size_t i, size_t j) const { return reinterpret_cast<const T *>(base[i] + off[j]); }
+};
+
+// The host arrays a into every local slot's q buffer, each 16-byte aligned behind the one before, on the slot's stream.
+// Loopback: slot 0's stream then joins every slot's, since it may read any slot's queries (the sparse re-rank).
+static cdb_status stage_queries(cdb_shard_group *g, const std::vector<HostArray> &a, Staged *st) {
+    size_t bytes = 0;
+    for (const HostArray &x : a) {
+        st->off.push_back(bytes);
+        bytes += (x.bytes + 15) & ~(size_t)15;
+    }
+    cdb_status rc;
+    for (size_t i = 0; i < g->dev.size(); ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = g->q[i].ensure(bytes))) return rc;
+        st->base.push_back(reinterpret_cast<uint8_t *>(g->q[i].p));
+        for (size_t j = 0; j < a.size(); ++j)
+            if (a[j].bytes)
+                CDB_CUDA_TRY(cudaMemcpyAsync(st->base[i] + st->off[j], a[j].h, a[j].bytes, cudaMemcpyHostToDevice, g->stream[i]));
+    }
+    if (g->loopback) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        for (size_t i = 1; i < g->dev.size(); ++i) {
+            CDB_CUDA_TRY(cudaEventRecord(g->ev[i], g->stream[i]));
+            CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[0], g->ev[i], 0));
+        }
+    }
+    return CDB_OK;
+}
+
+// A host form's final rows on slot 0, carved from g->rows[0] (the shards' own buffers hold their local results): ids and
+// scores [nq][w], counts [nq], error bytes [nq]; and the caller's arrays they go to (null counts / err: not copied).
+struct HostRows {
+    size_t nq = 0, nk = 0;
+    uint32_t *ids = nullptr, *counts = nullptr;
+    float *scores = nullptr;
+    uint8_t *err = nullptr;
+    uint32_t *h_ids = nullptr, *h_counts = nullptr;
+    float *h_scores = nullptr;
+    uint8_t *h_err = nullptr;
+};
+
+static cdb_status host_rows(cdb_shard_group *g, uint32_t nq, uint32_t w, uint32_t *h_ids, float *h_scores, uint32_t *h_counts,
+                            uint8_t *h_err, HostRows *r) {
+    const size_t nk = (size_t)nq * w;
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    if (cdb_status rc = g->rows[0].ensure(nk * 8 + (size_t)nq * 8)) return rc;
+    r->nq = nq;
+    r->nk = nk;
+    r->ids = reinterpret_cast<uint32_t *>(g->rows[0].p);
+    r->scores = reinterpret_cast<float *>(r->ids + nk);
+    r->counts = reinterpret_cast<uint32_t *>(r->scores + nk);
+    r->err = reinterpret_cast<uint8_t *>(r->counts + nq);
+    r->h_ids = h_ids; r->h_scores = h_scores; r->h_counts = h_counts; r->h_err = h_err;
+    return CDB_OK;
+}
+
+static cdb_status copy_rows(cdb_shard_group *g, const HostRows &r) {
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    const cudaStream_t s0 = g->stream[0];
+    CDB_CUDA_TRY(cudaMemcpyAsync(r.h_ids, r.ids, r.nk * 4, cudaMemcpyDeviceToHost, s0));
+    CDB_CUDA_TRY(cudaMemcpyAsync(r.h_scores, r.scores, r.nk * 4, cudaMemcpyDeviceToHost, s0));
+    if (r.h_counts) CDB_CUDA_TRY(cudaMemcpyAsync(r.h_counts, r.counts, r.nq * 4, cudaMemcpyDeviceToHost, s0));
+    if (r.h_err) CDB_CUDA_TRY(cudaMemcpyAsync(r.h_err, r.err, r.nq, cudaMemcpyDeviceToHost, s0));
+    return CDB_OK;
+}
+
+// The end of every host form, whatever rc says: the final rows r (if any) are copied back when the search was enqueued,
+// then every local stream drains, collectives included, before the caller's locks and host buffers go.  The first error.
+static cdb_status host_finish(cdb_shard_group *g, cdb_status rc, const HostRows *r) {
+    if (!rc && r) rc = copy_rows(g, *r);
+    for (size_t i = 0; i < g->dev.size(); ++i) {
+        cudaSetDevice(g->dev[i]);
+        const cudaError_t e = cudaStreamSynchronize(g->stream[i]);
+        if (e != cudaSuccess && !rc) { set_error(std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
+    }
+    return rc;
 }
 
 extern "C" {
@@ -328,7 +414,7 @@ cdb_status cdb_shard_group_destroy(cdb_shard_group *g) {
         cudaSetDevice(g->dev[i]);
         if (i < g->stream.size() && g->stream[i]) cudaStreamSynchronize(g->stream[i]);
         if (i < g->comm.size() && g->comm[i] && n) n->CommDestroy(g->comm[i]);
-        for (auto *v : {&g->gather, &g->q, &g->ids, &g->scores, &g->counts, &g->err, &g->sel, &g->hq})
+        for (auto *v : {&g->gather, &g->q, &g->ids, &g->scores, &g->counts, &g->rows, &g->sel})
             if (i < v->size()) (*v)[i].release();
         if (i < g->ev.size() && g->ev[i]) cudaEventDestroy(g->ev[i]);
         if (i < g->stream.size() && g->stream[i]) cudaStreamDestroy(g->stream[i]);
@@ -547,39 +633,18 @@ cdb_status cdb_search_batch_sharded(cdb_shard_group *g, const float *queries, ui
     cdb_status rc = merge_check(g, p);
     if (rc) return rc;
     std::lock_guard<std::mutex> lock(g->mu);
-    const size_t nl = g->dev.size();
     CDB_REQUIRE(g->shard[0], "a group slot has no shard attached");
     uint32_t md_dims = 0;
     if ((p->flags & CDB_SEARCH_ALL_CANDIDATES) && (rc = shards_check(g, p, false, &md_dims))) return rc;
-    const uint32_t dim = index_dim(g->shard[0]);
-    const size_t nk = (size_t)nq * p->k;
-    std::vector<const float *> d_q(nl);
-    for (size_t i = 0; i < nl; ++i) {   // the same host batch goes to every local device
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->q[i].ensure((size_t)nq * dim * 4))) return rc;
-        CDB_CUDA_TRY(cudaMemcpyAsync(g->q[i].p, queries, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        d_q[i] = reinterpret_cast<const float *>(g->q[i].p);
+    Staged st;
+    HostRows r;
+    if (!(rc = stage_queries(g, {{queries, (size_t)nq * index_dim(g->shard[0]) * 4}}, &st)) &&
+        !(rc = host_rows(g, nq, p->k, out_ids, out_scores, out_counts, err_flags, &r))) {
+        std::vector<const float *> d_q(g->dev.size());
+        for (size_t i = 0; i < d_q.size(); ++i) d_q[i] = st.at<float>(i, 0);
+        rc = sharded_enqueue(g, nq, p, d_q, nullptr, r.ids, r.scores, r.counts, r.err, nullptr);
     }
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    // final results land in slot 0's ids/scores buffers AFTER the local search wrote them: separate output buffers
-    Buf &o_err = g->err[0];
-    if ((rc = o_err.ensure(nk * 8 + (size_t)nq * 8))) return rc;
-    uint32_t *f_ids = reinterpret_cast<uint32_t *>(o_err.p);
-    float *f_scores = reinterpret_cast<float *>(f_ids + nk);
-    uint32_t *f_counts = reinterpret_cast<uint32_t *>(f_scores + nk);
-    uint8_t *f_err = reinterpret_cast<uint8_t *>(f_counts + nq);
-    if ((rc = sharded_enqueue(g, nq, p, d_q, nullptr, f_ids, f_scores, f_counts, f_err, nullptr))) return rc;
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    cudaStream_t s0 = g->stream[0];
-    CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, s0));
-    CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, s0));
-    if (out_counts) CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s0));
-    if (err_flags) CDB_CUDA_TRY(cudaMemcpyAsync(err_flags, f_err, nq, cudaMemcpyDeviceToHost, s0));
-    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collective included) before the host buffers are reused
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
-    }
-    return CDB_OK;
+    return host_finish(g, rc, &r);
 }
 
 cdb_status cdb_search_batch_sharded_device(cdb_shard_group *g, const float *d_queries, uint32_t nq, const cdb_search_params *p,
@@ -624,51 +689,23 @@ cdb_status cdb_search_batch_filtered_sharded(cdb_shard_group *g, const float *qu
         CDB_REQUIRE(filter_dims || !total, "null filter_dims");
     }
     std::lock_guard<std::mutex> lock(g->mu);
-    const size_t nl = g->dev.size();
     uint32_t md_dims = 0;
     if ((rc = shards_check(g, p, true, &md_dims))) return rc;
-    const uint32_t dim = index_dim(g->shard[0]);
-    auto al16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t nk = (size_t)nq * p->k, qbytes = al16((size_t)nq * dim * 4), obytes = al16(((size_t)nq + 1) * 4);
-    std::vector<const float *> d_q(nl);
-    std::vector<ShardFilters> flt(nl, ShardFilters{nullptr, nullptr, 0, nullptr});
-    for (size_t i = 0; i < nl; ++i) {   // queries, then offsets, has-flags and filter rows, to every local device
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->q[i].ensure(qbytes + obytes + al16(nq) + (size_t)total * md_dims + 1))) return rc;
-        uint8_t *base = reinterpret_cast<uint8_t *>(g->q[i].p);
-        CDB_CUDA_TRY(cudaMemcpyAsync(base, queries, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        d_q[i] = reinterpret_cast<const float *>(base);
-        if (has_filter) {
-            uint32_t *off = reinterpret_cast<uint32_t *>(base + qbytes);
-            uint8_t *has = base + qbytes + obytes;
-            int8_t *dims = reinterpret_cast<int8_t *>(has + al16(nq));
-            CDB_CUDA_TRY(cudaMemcpyAsync(off, filter_offsets, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, g->stream[i]));
-            CDB_CUDA_TRY(cudaMemcpyAsync(has, has_filter, nq, cudaMemcpyHostToDevice, g->stream[i]));
-            if (total) CDB_CUDA_TRY(cudaMemcpyAsync(dims, filter_dims, (size_t)total * md_dims, cudaMemcpyHostToDevice, g->stream[i]));
-            flt[i] = {off, dims, total, has};
+    const size_t f = has_filter ? 1 : 0;   // the filter arrays are staged only with has_filter
+    Staged st;
+    HostRows r;
+    if (!(rc = stage_queries(g, {{queries, (size_t)nq * index_dim(g->shard[0]) * 4}, {filter_offsets, f * ((size_t)nq + 1) * 4},
+                                 {has_filter, f * nq}, {filter_dims, (size_t)total * md_dims}}, &st)) &&
+        !(rc = host_rows(g, nq, p->k, out_ids, out_scores, out_counts, err_flags, &r))) {
+        std::vector<const float *> d_q(g->dev.size());
+        std::vector<ShardFilters> flt(g->dev.size(), ShardFilters{nullptr, nullptr, 0, nullptr});
+        for (size_t i = 0; i < d_q.size(); ++i) {
+            d_q[i] = st.at<float>(i, 0);
+            if (has_filter) flt[i] = {st.at<uint32_t>(i, 1), st.at<int8_t>(i, 3), total, st.at<uint8_t>(i, 2)};
         }
+        rc = sharded_enqueue(g, nq, p, d_q, &flt, r.ids, r.scores, r.counts, r.err, nullptr);
     }
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    Buf &o_err = g->err[0];
-    if ((rc = o_err.ensure(nk * 8 + (size_t)nq * 8))) return rc;
-    uint32_t *f_ids = reinterpret_cast<uint32_t *>(o_err.p);
-    float *f_scores = reinterpret_cast<float *>(f_ids + nk);
-    uint32_t *f_counts = reinterpret_cast<uint32_t *>(f_scores + nk);
-    uint8_t *f_err = reinterpret_cast<uint8_t *>(f_counts + nq);
-    rc = sharded_enqueue(g, nq, p, d_q, &flt, f_ids, f_scores, f_counts, f_err, nullptr);
-    if (!rc) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        cudaStream_t s0 = g->stream[0];
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, s0));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, s0));
-        if (out_counts) CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s0));
-        if (err_flags) CDB_CUDA_TRY(cudaMemcpyAsync(err_flags, f_err, nq, cudaMemcpyDeviceToHost, s0));
-    }
-    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collectives included) before the host buffers are reused
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
-    }
-    return rc;
+    return host_finish(g, rc, &r);
 }
 
 cdb_status cdb_search_batch_filtered_sharded_device(cdb_shard_group *g, const float *d_queries, uint32_t nq, const cdb_search_params *p,
@@ -760,23 +797,11 @@ static cdb_status sparse_sharded_slots(const cdb_shard_group *g) {
     return CDB_OK;
 }
 
-// the same host query batch to every local device, on each slot's stream
-static cdb_status sparse_upload_queries(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
-                                        uint32_t nq, std::vector<SparseQueries> *dq) {
-    const uint64_t nqp = q_offsets[nq];
-    cdb_status rc;
-    for (size_t i = 0; i < g->dev.size(); ++i) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqp * 8))) return rc;
-        uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
-        uint32_t *dims = reinterpret_cast<uint32_t *>(off + nq + 1);
-        float *vals = reinterpret_cast<float *>(dims + nqp);
-        CDB_CUDA_TRY(cudaMemcpyAsync(off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
-        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(dims, q_dims, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(vals, q_values, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        (*dq)[i] = {off, dims, vals};
-    }
-    return CDB_OK;
+// a sparse query CSR staged as arrays j, j + 1, j + 2 (offsets, dims, values), on every local slot
+static std::vector<SparseQueries> staged_sparse(const Staged &st, size_t j) {
+    std::vector<SparseQueries> q(st.base.size());
+    for (size_t i = 0; i < q.size(); ++i) q[i] = {st.at<uint64_t>(i, j), st.at<uint32_t>(i, j + 1), st.at<float>(i, j + 2)};
+    return q;
 }
 
 cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_dims, const float *q_values,
@@ -795,33 +820,12 @@ cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *g, const uint64_t *q
     const size_t nl = g->dev.size();
     std::vector<std::shared_lock<std::shared_mutex>> locks;
     for (size_t i = 0; i < nl; ++i) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
-    std::vector<SparseQueries> dq(nl);
-    if ((rc = sparse_upload_queries(g, q_offsets, q_dims, q_values, nq, &dq))) return rc;
-    if (g->loopback) {   // slot 0's stream reads every slot's queries in phase 2
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        for (size_t i = 1; i < nl; ++i) {
-            CDB_CUDA_TRY(cudaEventRecord(g->ev[i], g->stream[i]));
-            CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[0], g->ev[i], 0));
-        }
-    }
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    const size_t nk = (size_t)nq * p->k;
-    if ((rc = g->ids[0].ensure(nk * 4)) || (rc = g->scores[0].ensure(nk * 4)) || (rc = g->counts[0].ensure((size_t)nq * 4))) return rc;
-    uint32_t *f_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
-    float *f_scores = reinterpret_cast<float *>(g->scores[0].p);
-    uint32_t *f_counts = reinterpret_cast<uint32_t *>(g->counts[0].p);
-    rc = sparse_sharded_enqueue(g, nq, p, m, dq, f_ids, f_scores, f_counts, nullptr);
-    if (!rc) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-    }
-    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collectives included) before the locks and host buffers go
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
-    }
-    return rc;
+    Staged st;
+    HostRows r;
+    if (!(rc = stage_queries(g, {{q_offsets, ((size_t)nq + 1) * 8}, {q_dims, nqp * 4}, {q_values, nqp * 4}}, &st)) &&
+        !(rc = host_rows(g, nq, p->k, out_ids, out_scores, out_counts, nullptr, &r)))
+        rc = sparse_sharded_enqueue(g, nq, p, m, staged_sparse(st, 0), r.ids, r.scores, r.counts, nullptr);
+    return host_finish(g, rc, &r);
 }
 
 cdb_status cdb_sparse_search_batch_sharded_device(cdb_shard_group *g, const uint64_t *d_q_offsets, const uint32_t *d_q_dims,
@@ -1001,103 +1005,120 @@ cdb_status cdb_sparse_search_batch_all_sharded(cdb_shard_group *g, const uint64_
     const size_t nl = g->dev.size();
     std::vector<std::shared_lock<std::shared_mutex>> locks;
     for (size_t i = 0; i < nl; ++i) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
-    std::vector<SparseQueries> dq(nl);
+    const uint64_t nqp = q_offsets[nq];
     std::vector<SparseAllScratch> sc(nl);
-    rc = sparse_upload_queries(g, q_offsets, q_dims, q_values, nq, &dq);
+    Staged st;
+    rc = stage_queries(g, {{q_offsets, ((size_t)nq + 1) * 8}, {q_dims, nqp * 4}, {q_values, nqp * 4}}, &st);
     if (!rc) {
         try {
-            rc = sparse_all_sharded_run(g, dq, nq, p, r.get(), sc);
+            rc = sparse_all_sharded_run(g, staged_sparse(st, 0), nq, p, r.get(), sc);
         } catch (const std::bad_alloc &) {
             set_error("top_k None: host allocation of the results failed");
             rc = CDB_CUDA_ERROR;
         }
     }
-    for (size_t i = 0; i < nl; ++i) {   // scratch is freed behind its last use; every stream drains before the locks go
+    for (size_t i = 0; i < nl; ++i) {   // scratch is freed behind its last use
         cudaSetDevice(g->dev[i]);
         sparse_all_free(&sc[i], g->stream[i]);
-        const cudaError_t e = cudaStreamSynchronize(g->stream[i]);
-        if (e != cudaSuccess && !rc) { set_error(std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
     }
-    if (rc) return rc;
+    if ((rc = host_finish(g, rc, nullptr))) return rc;
     *out = r.release();
     return CDB_OK;
 }
 
-// The group's N and df of every query term: summed over the local shards' tables, then (per-rank groups) over the ranks by
-// one all-gather of [N, df...] per rank.  idf = tf_idf(N, df) on the host, one per query term; each shard scores its tiles
-// with it and writes all 512 bucket winners per query into its rank's slot; one all-gather; slot 0 takes the best of the
-// ranks per bucket and sorts into ids / scores [nq][tfidf_out_cols(k)] and counts [nq] on slot 0.  The caller holds g->mu
-// and every local shard's reader lock until the scoring has run, and drains the streams.  q_offsets may be a window of a
-// larger CSR (q_offsets[0] != 0): q_hashes is that CSR's hash array.  Host only: a per-rank group waits for its df all-gather
-// (tfidf_sharded_device_run is the device form's plan).
-static cdb_status tfidf_sharded_run(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
-                                    uint32_t *f_ids, float *f_scores, uint32_t *f_counts) {
-    const size_t nl = g->dev.size();
-    const uint64_t h0 = q_offsets[0], nqh = q_offsets[nq] - h0;
-    q_hashes += h0;
-    std::vector<uint64_t> rebased;
-    if (h0) {
-        rebased.assign(q_offsets, q_offsets + nq + 1);
-        for (auto &o : rebased) o -= h0;
-        q_offsets = rebased.data();
-    }
-    cdb_status rc = CDB_OK;
-    // [N, df of every query term], summed over the local shards (u32, wrapping), then over the ranks
-    std::vector<uint32_t> stats(1 + nqh, 0);
-    for (size_t i = 0; i < nl; ++i) stats[0] += tfidf_add_df(g->tfidf[i], q_hashes, nqh, stats.data() + 1);
-    if (nl < g->world) {
-        const size_t words = (stats.size() + 1) / 2;
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        if ((rc = g->gather[0].ensure(g->world * words * 8))) return rc;
-        std::vector<uint32_t> all(g->world * words * 2);
-        CDB_CUDA_TRY(cudaMemcpyAsync(gather_buf(g, 0) + (size_t)g->rank0 * words, stats.data(), stats.size() * 4, cudaMemcpyHostToDevice,
-                                     g->stream[0]));
-        if ((rc = group_allgather(g, words, nullptr))) return rc;
-        CDB_CUDA_TRY(cudaMemcpyAsync(all.data(), gather_buf(g, 0), all.size() * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[0]));
-        std::fill(stats.begin(), stats.end(), 0u);
-        for (uint32_t r = 0; r < g->world; ++r)
-            for (size_t j = 0; j < stats.size(); ++j) stats[j] += all[r * words * 2 + j];
-    }
-    std::vector<float> idf(nqh);
-    for (uint64_t j = 0; j < nqh; ++j) idf[j] = bm25_idf(stats[0], stats[1 + j]);
-    for (size_t i = 0; i < nl; ++i) {   // queries and their idf to every local device
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->q[i].ensure(((size_t)nq + 1) * 8 + nqh * 8))) return rc;
-        uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
-        uint32_t *hashes = reinterpret_cast<uint32_t *>(off + nq + 1);
-        float *d_idf = reinterpret_cast<float *>(hashes + nqh);
-        CDB_CUDA_TRY(cudaMemcpyAsync(off, q_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
-        if (nqh) CDB_CUDA_TRY(cudaMemcpyAsync(hashes, q_hashes, nqh * 4, cudaMemcpyHostToDevice, g->stream[i]));
-        if (nqh) CDB_CUDA_TRY(cudaMemcpyAsync(d_idf, idf.data(), nqh * 4, cudaMemcpyHostToDevice, g->stream[i]));
-    }
-    const uint32_t kout = tfidf_out_cols(k), chunk = group_chunk(g, nq, 512 * 8);
+// ---------------------------------------------------------------- TF-IDF shards (DESIGN.md section 8f)
+
+// one local slot's query CSR on its device: offsets index the batch's whole hash array
+struct TfQueries {
+    const uint64_t *off;
+    const uint32_t *hashes;
+};
+
+// a TF-IDF query CSR staged as arrays j, j + 1 (offsets, hashes), on every local slot
+static std::vector<TfQueries> staged_tfidf(const Staged &st, size_t j) {
+    std::vector<TfQueries> q(st.base.size());
+    for (size_t i = 0; i < q.size(); ++i) q[i] = {st.at<uint64_t>(i, j), st.at<uint32_t>(i, j + 1)};
+    return q;
+}
+
+// The TF-IDF plan's first step, once per batch: the group's idf of its nqh query terms.  Every local slot writes its
+// shard's [N, df of every query term] (u32) into its rank's slot of its gather buffer; one all-gather; then N and each df
+// are summed over the ranks (u32, wrapping) and bm25_idf of every term lands in scratch allocated on the slot's stream:
+// every local slot's from its own gather buffer into (*idf)[i], or, in loopback, where only slot 0's buffer is complete,
+// slot 0's into (*idf)[0], which every slot reads behind the fence at the end.  The gather buffers are sized for the
+// scoring of nq queries as well.  tfidf_idf_free releases the scratch behind its last reader.
+static cdb_status tfidf_idf_enqueue(cdb_shard_group *g, const std::vector<TfQueries> &tq, uint32_t nq, uint64_t nqh,
+                                    std::vector<float *> *idf, cudaStream_t out_stream) {
+    const size_t nl = g->dev.size(), words = (nqh + 2) / 2;   // one rank's [N, df...] in u64 words
+    const size_t score_words = (size_t)group_chunk(g, nq, 512 * 8) * 512;
+    cdb_status rc;
+    idf->assign(g->loopback ? 1 : nl, nullptr);
     for (size_t i = 0; i < nl; ++i) {
         CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->gather[i].ensure(g->world * (size_t)chunk * 512 * 8))) return rc;
+        if ((rc = g->gather[i].ensure(g->world * std::max(words, score_words) * 8))) return rc;
     }
-    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
-        const uint32_t c = std::min(chunk, nq - q0);
-        const size_t words = (size_t)c * 512;
-        if (q0 && (rc = loopback_fence(g))) break;
-        for (size_t i = 0; i < nl && !rc; ++i) {
+    for (size_t i = 0; i < nl; ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        const cudaStream_t s = slot_stream(g, i, out_stream);
+        if (i < idf->size() && nqh) CDB_CUDA_TRY(cudaMallocAsync(&(*idf)[i], nqh * 4, s));
+        if ((rc = tfidf_shard_stats(g->tfidf[i], tq[i].hashes, nqh, reinterpret_cast<uint32_t *>(gather_buf(g, i) + (g->rank0 + i) * words), s)))
+            return rc;
+    }
+    if ((rc = group_allgather(g, words, out_stream))) return rc;
+    for (size_t i = 0; i < idf->size(); ++i) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
+        if ((rc = tfidf_group_idf(gather_buf(g, i), words, g->world, nqh, (*idf)[i], slot_stream(g, i, out_stream)))) return rc;
+    }
+    return loopback_fence(g);
+}
+
+// on the stream that allocated it: every reader's last work is on it, or (loopback) joined it in the last all-gather
+static void tfidf_idf_free(cdb_shard_group *g, const std::vector<float *> &idf, cudaStream_t out_stream) {
+    for (size_t i = 0; i < idf.size(); ++i)
+        if (idf[i]) {
+            cudaSetDevice(g->dev[i]);
+            cudaFreeAsync(idf[i], slot_stream(g, i, out_stream));
+        }
+}
+
+// The TF-IDF plan's second step, for queries [q0, q0 + c) of the batch under its idf, per group chunk: every local shard
+// writes all 512 bucket winners per query into its rank's slot; one all-gather; slot 0 takes the best of the ranks per
+// bucket and sorts them into ids / scores [c][tfidf_out_cols(k)] and counts [c] on slot 0.
+static cdb_status tfidf_sharded_enqueue(cdb_shard_group *g, const std::vector<TfQueries> &tq, uint64_t nqh, const std::vector<float *> &idf,
+                                        uint32_t q0, uint32_t c, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                        cudaStream_t out_stream) {
+    const uint32_t kout = tfidf_out_cols(k), chunk = group_chunk(g, c, 512 * 8);
+    cdb_status rc;
+    for (uint32_t a = 0; a < c; a += chunk) {
+        const uint32_t n = std::min(chunk, c - a);
+        const size_t words = (size_t)n * 512;
+        if (a && (rc = loopback_fence(g))) return rc;
+        for (size_t i = 0; i < g->dev.size(); ++i) {
             CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-            uint64_t *off = reinterpret_cast<uint64_t *>(g->q[i].p);
-            uint32_t *hashes = reinterpret_cast<uint32_t *>(off + nq + 1);
-            rc = tfidf_shard_winners(g->tfidf[i], off + q0, hashes, nqh, reinterpret_cast<const float *>(hashes + nqh), c,
-                                     reinterpret_cast<uint2 *>(gather_buf(g, i) + (g->rank0 + i) * words), g->stream[i]);
+            if ((rc = tfidf_shard_winners(g->tfidf[i], tq[i].off + q0 + a, tq[i].hashes, nqh, idf[g->loopback ? 0 : i], n,
+                                          reinterpret_cast<uint2 *>(gather_buf(g, i) + (g->rank0 + i) * words), slot_stream(g, i, out_stream))))
+                return rc;
         }
-        if (!rc) rc = group_allgather(g, words, nullptr);
-        if (!rc) {
-            CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-            rc = tfidf_group_finalize(gather_buf(g, 0), words, g->world, c, k, f_ids + (size_t)q0 * kout, f_scores + (size_t)q0 * kout,
-                                      f_counts + q0, g->stream[0]);
-        }
+        if ((rc = group_allgather(g, words, out_stream))) return rc;
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        if ((rc = tfidf_group_finalize(gather_buf(g, 0), words, g->world, n, k, d_ids + (size_t)a * kout, d_scores + (size_t)a * kout,
+                                       d_counts + a, slot_stream(g, 0, out_stream))))
+            return rc;
     }
+    return CDB_OK;
+}
+
+// Both steps over a whole batch, on the group's streams (or out_stream, see slot_stream).  The caller holds g->mu and every
+// local shard's reader lock through the enqueue.
+static cdb_status tfidf_sharded_search(cdb_shard_group *g, const std::vector<TfQueries> &tq, uint32_t nq, uint64_t nqh, uint32_t k,
+                                       uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t out_stream) {
+    std::vector<float *> idf;
+    cdb_status rc = tfidf_idf_enqueue(g, tq, nq, nqh, &idf, out_stream);
+    if (!rc) rc = tfidf_sharded_enqueue(g, tq, nqh, idf, 0, nq, k, d_ids, d_scores, d_counts, out_stream);
+    tfidf_idf_free(g, idf, out_stream);
     return rc;
 }
 
-// The local shards' reader locks are held from the df look-up until the scoring has run.
 cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_offsets, const uint32_t *q_hashes, uint32_t nq, uint32_t k,
                                           uint32_t *out_ids, float *out_scores, uint32_t *out_counts) {
     CDB_REQUIRE(g && (out_ids || !nq) && (out_scores || !nq) && (out_counts || !nq), "null argument");
@@ -1112,77 +1133,12 @@ cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *g, const uint64_t *q_
     std::lock_guard<std::mutex> lock(g->mu);
     std::vector<std::shared_lock<std::shared_mutex>> locks;
     for (size_t i = 0; i < nl; ++i) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
-    const size_t nk = (size_t)nq * tfidf_out_cols(k);
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    if ((rc = g->ids[0].ensure(nk * 4)) || (rc = g->scores[0].ensure(nk * 4)) || (rc = g->counts[0].ensure((size_t)nq * 4))) return rc;
-    uint32_t *f_ids = reinterpret_cast<uint32_t *>(g->ids[0].p);
-    float *f_scores = reinterpret_cast<float *>(g->scores[0].p);
-    uint32_t *f_counts = reinterpret_cast<uint32_t *>(g->counts[0].p);
-    rc = tfidf_sharded_run(g, q_offsets, q_hashes, nq, k, f_ids, f_scores, f_counts);
-    if (!rc) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, nk * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, g->stream[0]));
-    }
-    for (size_t i = 0; i < nl; ++i) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
-    }
-    return rc;
-}
-
-// The device form's plan, all of it enqueued: every local slot writes its shard's [N, df of every query term] (u32) into its
-// rank's slot of the gather buffer; one all-gather; slot 0 sums N and each df over the ranks and writes the idf of every
-// query term into stream-ordered scratch; then, per group chunk, tfidf_sharded_run's scoring, all-gather and finalize into
-// the caller's arrays.  Every local slot sits on the caller's device, so each reads the caller's query arrays and slot 0's
-// idf.  The call's work follows what out_stream held, and out_stream's later work follows it.  The caller holds g->mu and
-// every local shard's reader lock through the enqueue.
-static cdb_status tfidf_sharded_device_run(cdb_shard_group *g, const uint64_t *d_qoff, const uint32_t *d_qhash, uint32_t nq, uint64_t nqh,
-                                           uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t out_stream) {
-    const size_t nl = g->dev.size();
-    const uint32_t kout = tfidf_out_cols(k), chunk = group_chunk(g, nq, 512 * 8);
-    const size_t stat_words = (nqh + 2) / 2;   // one rank's [N, df...] in u64 words
-    cdb_status rc = CDB_OK;
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    for (size_t i = 0; i < nl; ++i)
-        if ((rc = g->gather[i].ensure(g->world * std::max(stat_words, (size_t)chunk * 512) * 8))) return rc;
-    const cudaStream_t s0 = slot_stream(g, 0, out_stream);
-    bool fenced = false;
-    for (size_t i = 0; i < nl; ++i) {
-        const cudaStream_t si = slot_stream(g, i, out_stream);
-        if (si == out_stream) continue;
-        if (!fenced) CDB_CUDA_TRY(cudaEventRecord(g->ev[0], out_stream));
-        fenced = true;
-        CDB_CUDA_TRY(cudaStreamWaitEvent(si, g->ev[0], 0));
-    }
-    float *q_idf = nullptr;
-    if (nqh) CDB_CUDA_TRY(cudaMallocAsync(&q_idf, nqh * 4, s0));
-    for (size_t i = 0; i < nl && !rc; ++i)
-        rc = tfidf_shard_stats(g->tfidf[i], d_qhash, nqh, reinterpret_cast<uint32_t *>(gather_buf(g, i) + (g->rank0 + i) * stat_words),
-                               slot_stream(g, i, out_stream));
-    if (!rc) rc = group_allgather(g, stat_words, out_stream);
-    if (!rc) rc = tfidf_group_idf(gather_buf(g, 0), stat_words, g->world, nqh, q_idf, s0);
-    for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
-        const uint32_t c = std::min(chunk, nq - q0);
-        const size_t words = (size_t)c * 512;
-        // loopback: the slots read slot 0's idf, and overwrite their gather buffers, after slot 0's work so far
-        if ((rc = loopback_fence(g))) break;
-        for (size_t i = 0; i < nl && !rc; ++i)
-            rc = tfidf_shard_winners(g->tfidf[i], d_qoff + q0, d_qhash, nqh, q_idf, c,
-                                     reinterpret_cast<uint2 *>(gather_buf(g, i) + (g->rank0 + i) * words), slot_stream(g, i, out_stream));
-        if (!rc) rc = group_allgather(g, words, out_stream);
-        if (!rc)
-            rc = tfidf_group_finalize(gather_buf(g, 0), words, g->world, c, k, d_ids + (size_t)q0 * kout, d_scores + (size_t)q0 * kout,
-                                      d_counts + q0, s0);
-    }
-    // slot 0's stream has joined every slot's last work (collective or loopback copy)
-    if (q_idf) cudaFreeAsync(q_idf, s0);
-    if (s0 != out_stream) {
-        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], s0));
-        CDB_CUDA_TRY(cudaStreamWaitEvent(out_stream, g->ev[0], 0));
-    }
-    return rc;
+    Staged st;
+    HostRows r;
+    if (!(rc = stage_queries(g, {{q_offsets, ((size_t)nq + 1) * 8}, {q_hashes, nqh * 4}}, &st)) &&
+        !(rc = host_rows(g, nq, tfidf_out_cols(k), out_ids, out_scores, out_counts, nullptr, &r)))
+        rc = tfidf_sharded_search(g, staged_tfidf(st, 0), nq, nqh, k, r.ids, r.scores, r.counts, nullptr);
+    return host_finish(g, rc, &r);
 }
 
 cdb_status cdb_tfidf_search_batch_sharded_device(cdb_shard_group *g, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes, uint32_t nq,
@@ -1199,7 +1155,26 @@ cdb_status cdb_tfidf_search_batch_sharded_device(cdb_shard_group *g, const uint6
     std::lock_guard<std::mutex> lock(g->mu);
     std::vector<std::shared_lock<std::shared_mutex>> locks;
     for (size_t i = 0; i < nl; ++i) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
-    return tfidf_sharded_device_run(g, d_q_offsets, d_q_hashes, nq, n_query_hashes, k, d_ids, d_scores, d_counts, (cudaStream_t)stream);
+    // every slot's work follows what the caller's stream held, and the caller's later work follows slot 0's, which joined
+    // every slot's last work (collective or loopback copy)
+    const cudaStream_t out = (cudaStream_t)stream, s0 = slot_stream(g, 0, out);
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    bool fenced = false;
+    for (size_t i = 0; i < nl; ++i) {
+        const cudaStream_t si = slot_stream(g, i, out);
+        if (si == out) continue;
+        if (!fenced) CDB_CUDA_TRY(cudaEventRecord(g->ev[0], out));
+        fenced = true;
+        CDB_CUDA_TRY(cudaStreamWaitEvent(si, g->ev[0], 0));
+    }
+    const cdb_status rc = tfidf_sharded_search(g, std::vector<TfQueries>(nl, TfQueries{d_q_offsets, d_q_hashes}), nq, n_query_hashes, k, d_ids,
+                                               d_scores, d_counts, out);
+    if (s0 != out) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], s0));
+        CDB_CUDA_TRY(cudaStreamWaitEvent(out, g->ev[0], 0));
+    }
+    return rc;
 }
 
 // ---------------------------------------------------------------- hybrid search over the group (DESIGN.md section 8h)
@@ -1282,14 +1257,16 @@ static cdb_status hyb_group_check(const cdb_shard_group *g, const cdb_hybrid_gro
     return merge_check(g, &p->dense);
 }
 
-// Both sub-searches and the fusion, per chunk of queries, under g->mu and every named text shard's reader lock.  dq / sq:
-// each local slot's dense queries and sparse CSR on its device; the TF-IDF queries stay on the host (host form only).  The
-// sub-searches run one after the other in list order, each on the streams its public entry point uses, so every rank
-// issues the same collectives in the same order; each one's merged list lands in this call's scratch on slot 0, where the
-// fusion writes rows q0.. of the output.  Nothing here waits for the device except a per-rank group's TF-IDF df gather.
+// Both sub-searches and the fusion, per chunk of queries, under g->mu and every named text shard's reader lock.  dq / sq /
+// tq: each local slot's dense queries, sparse CSR and TF-IDF CSR on its device (nqh: the TF-IDF batch's term count).  A
+// TF-IDF source's idf step runs once, over the whole batch, before the chunks.  The sub-searches run one after the other
+// in list order, each on the streams its public entry point uses, so every rank issues the same collectives in the same
+// order; each one's merged list lands in this call's scratch on slot 0, where the fusion writes rows q0.. of the output.
+// Nothing here waits for the device.
 static cdb_status hybrid_group_run(cdb_shard_group *g, const cdb_hybrid_group_sources *h, const HybPlan &p, uint32_t nq, uint32_t top_k,
                                    float fusion_k, const std::vector<const float *> &dq, const std::vector<SparseQueries> &sq,
-                                   uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
+                                   const std::vector<TfQueries> &tq, uint64_t nqh, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                   uint8_t *d_err, cudaStream_t out_stream) {
     const size_t nl = g->dev.size();
     const uint32_t k3 = 3 * top_k, ld_out = 6 * top_k;
     const size_t per_q = ((size_t)p.ld[0] + p.ld[1]) * 8 + 8;   // ids and scores of both lists, two counts
@@ -1308,7 +1285,8 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const cdb_hybrid_group_so
     counts[0] = reinterpret_cast<uint32_t *>(scores[1] + (size_t)chunk * p.ld[1]);
     counts[1] = counts[0] + chunk;
     const std::vector<ShardFilters> no_filters(nl, ShardFilters{nullptr, nullptr, 0, nullptr});
-    cdb_status rc = CDB_OK;
+    std::vector<float *> idf;
+    cdb_status rc = h->use_tfidf ? tfidf_idf_enqueue(g, tq, nq, nqh, &idf, out_stream) : CDB_OK;
     for (uint32_t q0 = 0; q0 < nq && !rc; q0 += chunk) {
         const uint32_t c = std::min(chunk, nq - q0);
         for (int j = 0; j < 2 && !rc; ++j) {
@@ -1324,7 +1302,7 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const cdb_hybrid_group_so
                 for (size_t i = 0; i < nl; ++i) q[i] = {sq[i].off + q0, sq[i].dims, sq[i].vals};
                 rc = sparse_sharded_enqueue(g, c, &p.sparse, p.m, q, ids[j], scores[j], counts[j], out_stream);
             } else {
-                rc = tfidf_sharded_run(g, h->tfidf_offsets + q0, h->tfidf_hashes, c, k3, ids[j], scores[j], counts[j]);
+                rc = tfidf_sharded_enqueue(g, tq, nqh, idf, q0, c, k3, ids[j], scores[j], counts[j], out_stream);
             }
         }
         if (rc) break;
@@ -1336,6 +1314,7 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const cdb_hybrid_group_so
             rc = fuse_launch(a, b, c, fusion_k, ld_out, o_ids, o_scores, o_counts, s0);
     }
     // freed behind everything enqueued on slot 0's stream, which every slot's last work joined (collective or loopback copy)
+    tfidf_idf_free(g, idf, out_stream);
     cudaSetDevice(g->dev[0]);
     cudaFreeAsync(buf, s0);
     return rc;
@@ -1362,60 +1341,22 @@ cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *g, const cdb_hybrid_
         if (h->use_sparse) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
         if (h->use_tfidf) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
     }
-    // the dense batch, then the sparse CSR, to every local device
+    // the dense batch, the sparse CSR and the TF-IDF CSR of the named sources to every local device
     const uint32_t dim = h->use_dense ? index_dim(g->shard[0]) : 0;
-    const uint64_t nqp = h->use_sparse ? h->sparse_offsets[nq] : 0;
-    const size_t dbytes = ((size_t)nq * dim * 4 + 15) & ~(size_t)15, sbytes = h->use_sparse ? ((size_t)nq + 1) * 8 + nqp * 8 : 0;
-    std::vector<const float *> dq(nl, nullptr);
-    std::vector<SparseQueries> sq(nl, SparseQueries{nullptr, nullptr, nullptr});
-    for (size_t i = 0; i < nl; ++i) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        if ((rc = g->hq[i].ensure(dbytes + sbytes))) return rc;
-        uint8_t *base = reinterpret_cast<uint8_t *>(g->hq[i].p);
-        if (h->use_dense) {
-            CDB_CUDA_TRY(cudaMemcpyAsync(base, h->dense_queries, (size_t)nq * dim * 4, cudaMemcpyHostToDevice, g->stream[i]));
-            dq[i] = reinterpret_cast<const float *>(base);
-        }
-        if (h->use_sparse) {
-            uint64_t *off = reinterpret_cast<uint64_t *>(base + dbytes);
-            uint32_t *dims = reinterpret_cast<uint32_t *>(off + nq + 1);
-            float *vals = reinterpret_cast<float *>(dims + nqp);
-            CDB_CUDA_TRY(cudaMemcpyAsync(off, h->sparse_offsets, ((size_t)nq + 1) * 8, cudaMemcpyHostToDevice, g->stream[i]));
-            if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(dims, h->sparse_dims, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
-            if (nqp) CDB_CUDA_TRY(cudaMemcpyAsync(vals, h->sparse_values, nqp * 4, cudaMemcpyHostToDevice, g->stream[i]));
-            sq[i] = {off, dims, vals};
-        }
+    const uint64_t nqp = h->use_sparse ? h->sparse_offsets[nq] : 0, nqh = h->use_tfidf ? h->tfidf_offsets[nq] : 0;
+    const size_t off_bytes = ((size_t)nq + 1) * 8;
+    Staged st;
+    HostRows r;
+    if (!(rc = stage_queries(g, {{h->dense_queries, (size_t)nq * dim * 4}, {h->sparse_offsets, h->use_sparse ? off_bytes : 0},
+                                 {h->sparse_dims, nqp * 4}, {h->sparse_values, nqp * 4}, {h->tfidf_offsets, h->use_tfidf ? off_bytes : 0},
+                                 {h->tfidf_hashes, nqh * 4}}, &st)) &&
+        !(rc = host_rows(g, nq, 6 * top_k, out_ids, out_scores, out_counts, h->use_dense ? err_flags : nullptr, &r))) {
+        std::vector<const float *> dq(nl);
+        for (size_t i = 0; i < nl; ++i) dq[i] = st.at<float>(i, 0);
+        rc = hybrid_group_run(g, h, p, nq, top_k, fusion_constant_k, dq, staged_sparse(st, 1), staged_tfidf(st, 4), nqh, r.ids, r.scores,
+                              r.counts, h->use_dense ? r.err : nullptr, nullptr);
     }
-    if (g->loopback) {   // slot 0's stream reads every slot's sparse queries in the re-rank
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        for (size_t i = 1; i < nl; ++i) {
-            CDB_CUDA_TRY(cudaEventRecord(g->ev[i], g->stream[i]));
-            CDB_CUDA_TRY(cudaStreamWaitEvent(g->stream[0], g->ev[i], 0));
-        }
-    }
-    // the fused rows and the error bytes on slot 0
-    const size_t no = (size_t)nq * 6 * top_k;
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    Buf &o = g->err[0];
-    if ((rc = o.ensure(no * 8 + (size_t)nq * 8))) return rc;
-    uint32_t *f_ids = reinterpret_cast<uint32_t *>(o.p);
-    float *f_scores = reinterpret_cast<float *>(f_ids + no);
-    uint32_t *f_counts = reinterpret_cast<uint32_t *>(f_scores + no);
-    uint8_t *f_err = reinterpret_cast<uint8_t *>(f_counts + nq);
-    rc = hybrid_group_run(g, h, p, nq, top_k, fusion_constant_k, dq, sq, f_ids, f_scores, f_counts, h->use_dense ? f_err : nullptr, nullptr);
-    if (!rc) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        cudaStream_t s0 = g->stream[0];
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_ids, f_ids, no * 4, cudaMemcpyDeviceToHost, s0));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_scores, f_scores, no * 4, cudaMemcpyDeviceToHost, s0));
-        CDB_CUDA_TRY(cudaMemcpyAsync(out_counts, f_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s0));
-        if (err_flags && h->use_dense) CDB_CUDA_TRY(cudaMemcpyAsync(err_flags, f_err, nq, cudaMemcpyDeviceToHost, s0));
-    }
-    for (size_t i = 0; i < nl; ++i) {   // every local stream drains (collectives included) before the locks and host buffers go
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[i]));
-        CDB_CUDA_TRY(cudaStreamSynchronize(g->stream[i]));
-    }
-    return rc;
+    return host_finish(g, rc, &r);
 }
 
 cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *g, const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k,
@@ -1428,7 +1369,8 @@ cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *g, const cdb_
     cdb_status rc = hyb_plan(h, nq, top_k, &p);
     if (rc) return rc;
     if (h->use_tfidf) {
-        set_error("the hybrid device form has no TF-IDF sub-search (its plan sums the group's df on the host): use cdb_hybrid_search_batch_sharded");
+        set_error("the hybrid device form has no TF-IDF sub-search (the host sizes its idf exchange by the batch's term count, "
+                  "which cdb_hybrid_group_sources does not carry): use cdb_hybrid_search_batch_sharded");
         return CDB_UNSUPPORTED;
     }
     CDB_REQUIRE(g->dev.size() == 1, "the device form serves groups of one local slot (cdb_shard_group_create_rank, or one device)");
@@ -1445,7 +1387,7 @@ cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *g, const cdb_
     if (h->use_sparse) shard_lock.reset(new std::shared_lock<std::shared_mutex>(sparse_index_mutex(g->sparse[0])));
     const std::vector<const float *> dq(1, h->dense_queries);
     const std::vector<SparseQueries> sq(1, SparseQueries{h->sparse_offsets, h->sparse_dims, h->sparse_values});
-    return hybrid_group_run(g, h, p, nq, top_k, fusion_constant_k, dq, sq, d_ids, d_scores, d_counts,
+    return hybrid_group_run(g, h, p, nq, top_k, fusion_constant_k, dq, sq, {}, 0, d_ids, d_scores, d_counts,
                             h->use_dense ? d_err_flags : nullptr, (cudaStream_t)stream);
 }
 

@@ -381,15 +381,6 @@ uint32_t tfidf_index_id_base(const cdb_tfidf_index *ix) { return ix->desc.id_bas
 uint64_t tfidf_index_capacity(const cdb_tfidf_index *ix) { return ix->desc.capacity_rows; }
 uint32_t tfidf_out_cols(uint32_t k) { return out_cols(k); }
 
-// df[i] += this index's df of hashes[i] (u32, wrapping; 0 for a hash it never saw); returns its N
-uint32_t tfidf_add_df(const cdb_tfidf_index *ix, const uint32_t *hashes, uint64_t n, uint32_t *df) {
-    for (uint64_t i = 0; i < n; ++i) {
-        const size_t g = std::lower_bound(ix->h_terms.begin(), ix->h_terms.end(), hashes[i]) - ix->h_terms.begin();
-        if (g < ix->h_terms.size() && ix->h_terms[g] == hashes[i]) df[i] += ix->h_df[g];
-    }
-    return ix->documents;
-}
-
 // one shard's statistics for the group's idf, [N, df of d_qhash[0..n_qh)] as u32 at out (tf_query_stats_kernel)
 cdb_status tfidf_shard_stats(const cdb_tfidf_index *ix, const uint32_t *d_qhash, uint64_t n_qh, uint32_t *out, cudaStream_t s) {
     tf_query_stats_kernel<<<(uint32_t)((n_qh + 256) / 256), 256, 0, s>>>(ix->d_terms, ix->d_df, (uint32_t)ix->h_terms.size(),
@@ -678,8 +669,8 @@ cdb_status cdb_tfidf_search_batch(cdb_tfidf_index *ix, const uint64_t *q_offsets
     return rc;
 }
 
-// the library's two copies of the idf arithmetic (bm25_idf.h): the device one as the idf kernels run it, the host one as
-// tfidf_sharded_run (shard_group.cu, same flags) runs it
+// the library's two copies of the idf arithmetic (bm25_idf.h): the device one as the idf kernels run it, and the same source
+// compiled for the host, which no search runs
 cdb_status cdb_debug_bm25(int32_t on_device, const float *x, uint64_t n, float *out_log1p, const uint32_t *n_docs, const uint32_t *df,
                           uint64_t n_pairs, float *out_idf, void *stream) {
     CDB_REQUIRE((x && out_log1p) || !n, "null argument");

@@ -445,7 +445,8 @@ class ShardGroup:
     def hybrid_search_device(self, nq, d_ids, d_scores, d_counts, d_err=None, stream_ptr=None, top_k=10, fusion_constant_k=60.0,
                              dense=None, sparse=None, tfidf=None, dense_id_stride=1):
         """groups of one local slot: hybrid_search on device pointers (ints), asynchronous on the stream; see _hybrid_sources
-        for the source forms.  A TF-IDF source is refused (CDB_UNSUPPORTED): its TF-IDF sub-search is the host form's."""
+        for the source forms.  A TF-IDF source is refused (CDB_UNSUPPORTED): the host sizes the TF-IDF idf exchange by the
+        batch's term count, which cdb_hybrid_group_sources does not carry."""
         from .api import _check
         src, keep, _ = self._hybrid_sources(dense, sparse, tfidf, dense_id_stride, False)
         _check(self._lib.cdb_hybrid_search_batch_sharded_device(self._h, C.byref(src), nq, int(top_k), float(fusion_constant_k), d_ids,

@@ -677,7 +677,7 @@ cdb_status cdb_debug_tensor_peak(int32_t device, int32_t kind_i8, uint32_t iters
  * platform's log1pf (f32::ln_1p): bm25_log1pf(x[i]) -> out_log1p[i] for i < n, and
  * bm25_idf(n_docs[j], df[j]) -> out_idf[j] for j < n_pairs.  on_device != 0: the device copy the idf kernels inline, every
  * pointer a device pointer on the current device, enqueued on `stream` (NULL = the legacy default stream), asynchronous.
- * on_device == 0: the host copy a shard group's host form runs, host pointers, synchronous (stream unused). */
+ * on_device == 0: the same source compiled for the host (no search runs it), host pointers, synchronous (stream unused). */
 cdb_status cdb_debug_bm25(int32_t on_device, const float *x, uint64_t n, float *out_log1p, const uint32_t *n_docs,
                           const uint32_t *df, uint64_t n_pairs, float *out_idf, void *stream);
 /* former measurement switch of CDB_MODE_HNSW kernel variants.  HNSW search now has one kernel per graph kind, so every value
@@ -905,12 +905,13 @@ cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *index, const uint64_t 
  *               keep the gather buffer within 256 MB; each local shard holds its reader lock through both phases.
  *               The device form (per-rank groups only) takes device arrays and is asynchronous on `stream`.
  *   TF-IDF      idf depends on the whole corpus: N = sum of the shards' N, df = sum of their df (u32, wrapping), and idf
- *               computed with the function a single index uses (csrc/bm25_idf.h).  The host form sums them on the host
- *               (per-rank groups: one all-gather of 1 + query terms u32 per rank, waited for); the device form sums them on
- *               the device.  Each shard scores under that idf and hands in all 512 bucket winners per query; per bucket the
- *               best of the ranks wins with `>`, equal scores (+0 and -0 too) going to the smaller id, then they are sorted
- *               and truncated as in cdb_tfidf_search_batch.  Each local shard holds its reader lock from the df look-up
- *               through the scoring. */
+ *               computed with the function a single index uses (csrc/bm25_idf.h).  Both forms run one plan on the device:
+ *               each local slot writes its shard's [N, df of every query term], one all-gather of 1 + query terms u32 per
+ *               rank brings them to every rank, and a kernel sums them and computes the idf of every query term; the host
+ *               never waits in between.  Each shard scores under that idf and hands in all 512 bucket winners per query;
+ *               per bucket the best of the ranks wins with `>`, equal scores (+0 and -0 too) going to the smaller id, then
+ *               they are sorted and truncated as in cdb_tfidf_search_batch.  Each local shard holds its reader lock from
+ *               the df look-up through the scoring. */
 cdb_status cdb_shard_group_attach_sparse(cdb_shard_group *group, uint32_t local_slot, cdb_sparse_index *shard);
 cdb_status cdb_shard_group_attach_tfidf(cdb_shard_group *group, uint32_t local_slot, cdb_tfidf_index *shard);
 cdb_status cdb_sparse_search_batch_sharded(cdb_shard_group *group, const uint64_t *q_offsets, const uint32_t *q_dims,
@@ -923,12 +924,10 @@ cdb_status cdb_tfidf_search_batch_sharded(cdb_shard_group *group, const uint64_t
                                           uint32_t k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts);
 /* The TF-IDF search with every array in DEVICE memory, asynchronous on `stream` (NULL = the legacy default stream): no host
  * synchronisation and no device-to-host copy.  Ids, counts and score bits equal cdb_tfidf_search_batch_sharded's on the same
- * group and batch.  n_query_hashes must equal d_q_offsets[n_queries] (d_q_offsets[0] = 0): the host sizes the df exchange by
- * it.  The device CSR is not validated, but no kernel reads d_q_hashes at or past n_query_hashes.  Each local slot writes its
- * shard's [N, df of every query term] into its rank's slot of the gather buffer, one all-gather brings them to every rank,
- * and a kernel sums them and computes the idf of every query term; the scoring, all-gather and merge follow as in the host
- * form.  Served groups: those whose local slots all sit on one device, the one holding the caller's arrays -- per-rank
- * groups, one-slot local groups and loopback groups (a device listed more than once).
+ * group and batch: it runs the host form's plan, on the caller's stream.  n_query_hashes must equal d_q_offsets[n_queries]
+ * (d_q_offsets[0] = 0): the host sizes the df exchange by it.  The device CSR is not validated, but no kernel reads
+ * d_q_hashes at or past n_query_hashes.  Served groups: those whose local slots all sit on one device, the one holding the
+ * caller's arrays -- per-rank groups, one-slot local groups and loopback groups (a device listed more than once).
  * CDB_INVALID_PARAMS, before any device work: null arguments (with n_queries > 0), n_query_hashes >= 2^31, a local group
  * spanning devices, a local slot without a TF-IDF shard.  n_queries = 0 returns with nothing launched. */
 cdb_status cdb_tfidf_search_batch_sharded_device(cdb_shard_group *group, const uint64_t *d_q_offsets, const uint32_t *d_q_hashes,
@@ -1074,8 +1073,8 @@ typedef struct {
  * mode other than CDB_MODE_HNSW on metadata shards; world * 3 * top_k * 8 > 200 KB (the dense merge).  top_k = 0: counts
  * zeroed, nothing launched.
  * The device form serves groups of one local slot (per-rank groups and one-device local groups), takes device arrays and
- * is asynchronous on `stream`.  It refuses a TF-IDF source with CDB_UNSUPPORTED: its TF-IDF sub-search is the host form's,
- * which sums every rank's df on the host before the scoring (cdb_tfidf_search_batch_sharded_device is not wired in yet). */
+ * is asynchronous on `stream`.  It refuses a TF-IDF source with CDB_UNSUPPORTED: the host sizes the TF-IDF idf exchange by
+ * the batch's term count, and cdb_hybrid_group_sources carries none. */
 cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *group, const cdb_hybrid_group_sources *sources, uint32_t n_queries,
                                            uint32_t top_k, float fusion_constant_k, uint32_t *out_ids, float *out_scores,
                                            uint32_t *out_counts, uint8_t *err_flags);

@@ -2,7 +2,7 @@
 and at production document counts.
 
 Every TF-IDF score goes through bm25_idf, in two compiled copies: the device one the idf kernels inline (a single index's
-table, a shard group's device form) and the host one a shard group's host form runs.  tests/test_bm25_idf.py checks the
+table, a shard group's idf in both forms) and the same source compiled for the host.  tests/test_bm25_idf.py checks the
 header's arithmetic through a separate g++ build; here cdb_debug_bm25 runs the library's own copies:
 
   - the device bm25_log1pf on every non-negative finite float (2^31 - 2^23 of them), compared as checksums of blocks of
@@ -118,7 +118,7 @@ def production_pairs(rng):
 
 def group_pairs(rng, groups=5000):
     """(N, df) as a shard group of 2..8 ranks forms them: each rank's N and df summed in u32, wrapping
-    (tf_group_idf_kernel's and tfidf_sharded_run's arithmetic).  Ranks hold up to 2^31 documents, so many sums wrap."""
+    (tf_group_idf_kernel's arithmetic).  Ranks hold up to 2^31 documents, so many sums wrap."""
     world = rng.integers(2, 9, groups)
     live = np.arange(8)[None, :] < world[:, None]
     n_r = np.where(live, rng.integers(0, 1 << 31, (groups, 8)), 0).astype(np.uint64)
@@ -236,7 +236,7 @@ def test_an_index_past_2_24_documents_end_to_end(driver):
     orc.close()
     print(f"oracle: the whole corpus replayed and searched in {time.perf_counter() - t1:.2f} s")
 
-    # the same corpus over a two-slot loopback group: its host form sums N and df on the host and runs the host bm25_idf
+    # the same corpus over a two-slot loopback group, in both forms
     g = ShardGroup.local([0, 0])
     parts = []
     for r, (a, b) in enumerate(((0, SPLIT), (SPLIT, rows))):

@@ -4,7 +4,7 @@ ids, counts and score bits:
     the group's own sub-searches at k = 3 * top_k (HNSW and BRUTE_RAW dense, sparse with and without re-rank and with a
     threshold), before and after deletes in every kind of shard;
   * whole corpus: where every sub-search is exact across shards (BRUTE_RAW on the tensor-core path, sparse, TF-IDF), equal
-    to cdb_hybrid_search_batch over single indexes holding the whole corpus;
+    to cdb_hybrid_search_batch over single indexes holding the whole corpus, also over two fusion chunks with a TF-IDF source;
   * replica graphs: a one-slot group over a replica-graph index (the hybrid search cdb_hybrid_search_batch refuses), a
     two-shard replica group, and the refusal of a group that mixes replica and plain graphs;
   * the device form on a side stream equals the host form, on a per-rank group and a one-device local group; a TF-IDF
@@ -197,6 +197,24 @@ def test_group_hybrid_equals_whole_corpus_hybrid(world, pair):
         want = cdb.hybrid_batch_search(top_k, 60.0, **{p: whole[p] for p in pair})
         check(got, want)
         assert np.array_equal(got[3], want[3])
+
+
+def test_tfidf_source_over_two_fusion_chunks(world):
+    """sparse + TF-IDF at top_k 341: a fusion chunk holds 256 MB / ((1023 + 512) * 8 + 8) bytes of lists, 21845 queries, so
+    a batch of five more takes two.  The group's idf is computed once for the whole batch and each chunk scores its window
+    of the TF-IDF query CSR.  Every query against the whole-corpus hybrid; the fusion of the group's own searches on a sample
+    that holds both sides of the chunk boundary."""
+    top_k = 341
+    chunk = (256 << 20) // ((3 * top_k + min(3 * top_k, 512)) * 8 + 8)
+    b = chunk + 5
+    sq, tq = zipf_csr(45, b, vocab=VOCAB, mean_pairs=10), zipf_queries(46, b, vocab=VOCAB)
+    sp_opts = SPARSE_OPTS[2]
+    kw, lists = group_sources(world.gh, ("sparse", "tfidf"), None, sq, tq, None, sp_opts)
+    got = world.gh.hybrid_search(top_k, 60.0, **kw)
+    check(got, cdb.hybrid_batch_search(top_k, 60.0, sparse=(world.w_sp, sq, sp_opts), tfidf=(world.w_tf, tq)))
+    (a, _, ca), (b_ids, _, cb) = lists(top_k)
+    rows = np.unique(np.concatenate([np.arange(8), np.arange(chunk - 8, b), np.random.default_rng(3).choice(b, 48)]))
+    check(tuple(x[rows] for x in got[:3]), ph.fuse_batch(a[rows], ca[rows], b_ids[rows], cb[rows], 60.0, ld_out=6 * top_k))
 
 
 def test_error_bytes_only_with_a_dense_source_and_top_k_zero(world):

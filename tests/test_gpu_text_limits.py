@@ -21,7 +21,7 @@ from tests import pysparse as ps
 from tests import pytfidf as pt
 from tests import text_plan as tp
 from tests.sparse_data import concat_csr, quirky_rows, slice_csr
-from tests.test_gpu_sharded_text import Routed
+from tests.test_gpu_sharded_text import Routed, devices
 from tests.tfidf_data import query_csr, random_queries, random_rows
 
 pytestmark = pytest.mark.gpu
@@ -424,14 +424,15 @@ def test_long_tfidf_queries(k):
     orc.close()
 
 
-def test_long_tfidf_queries_in_a_group_of_three():
-    """the shards score with the group's idf of every query term, q_idf[j0 + tid], in every 512-term pass"""
+def test_long_tfidf_queries_in_a_group_of_three_with_the_idf_step():
+    """the shards score with the group's idf of every query term, q_idf[j0 + tid], in every 512-term pass; the host form
+    launches the group's idf step (a statistics kernel per slot, the idf kernel) before the scoring"""
     rows, counted, qs = long_tfidf()
     grp = Routed([0, 1000, 2000, 3000])
     grp.append(rows, counted, 2)
     for k in (10, 0):
         got, n = launches(lambda: grp.g.search_tfidf(query_csr(qs), k))
-        assert n == tp.tfidf_group_launches(len(qs), [1, 1, 1])
+        assert n == tp.tfidf_group_search_launches(len(qs), [1, 1, 1], sum(map(len, qs)), len(set(devices(3))) < 3)
         check(got, grp.whole.batch_search(query_csr(qs), k))
         check(got, grp.orc.search(query_csr(qs), k))
     grp.close()
@@ -473,9 +474,10 @@ def test_wide_sparse_groups(short_ix, world):
     close_group(g, parts)
 
 
-def test_tfidf_group_of_eight_bucket_ties_across_ranks():
+def test_tfidf_group_of_eight_bucket_ties_across_ranks_with_the_idf_step():
     """shard r (ids 600r..) sits in slot 7 - r, so later ranks hold smaller ids.  Every id = 5 (mod 512) holds the same row:
-    one tie per bucket across ranks, won by id 5 on the last rank; ids = 7 (mod 512) tie at +0 and -0."""
+    one tie per bucket across ranks, won by id 5 on the last rank; ids = 7 (mod 512) tie at +0 and -0.  The launch count
+    includes the group's idf step."""
     rng = np.random.default_rng(12)
     vocab = rng.choice(1 << 30, 40, replace=False).astype(np.uint32)
     h1, h2 = (1 << 30) + 1, (1 << 30) + 2
@@ -492,7 +494,7 @@ def test_tfidf_group_of_eight_bucket_ties_across_ranks():
     qs = [[h1], [h2], [h1, h2], [h2, int(vocab[0])]] + random_queries(np.random.default_rng(13), np.concatenate([vocab, [h1, h2]]), 60)
     for k in (0, 1, 10, 600):
         got, n = launches(lambda: grp.g.search_tfidf(query_csr(qs), k))
-        assert n == tp.tfidf_group_launches(len(qs), [1] * 8)
+        assert n == tp.tfidf_group_search_launches(len(qs), [1] * 8, sum(map(len, qs)), len(set(devices(8))) < 8)
         check(got, grp.whole.batch_search(query_csr(qs), k))
         check(got, grp.orc.search(query_csr(qs), k))
     ids = grp.g.search_tfidf([[h1]], 10)[0][0]

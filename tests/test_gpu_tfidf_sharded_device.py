@@ -2,7 +2,8 @@
 group's idf computed on the device, and the single index's idf refresh on the device (bm25_idf.h).
 
 The device form must return the host form's ids, counts and score bits, and so one index's over every shard's rows, on a
-per-rank group of world 1, a one-slot local group and loopback groups of 2 and 3 slots on device 0.  The shards see
+per-rank group of world 1, a one-slot local group and loopback groups of 2 and 3 slots on device 0; both forms run one
+plan, so both launch the same kernels.  The shards see
 appends in several versions, deletes in the insert's version and later ones (df > N), an empty shard, hashes some or all
 shards never saw, repeated hashes, a query of more than 512 terms, every k class and a batch of two group chunks.  The
 launch plan, the asynchrony on the caller's stream and the refusals that need the group are pinned here too."""
@@ -21,12 +22,8 @@ KS = (0, 1, 10, 512, 600)
 
 
 def device_launches(nq, shard_rows, n_hashes):
-    """kernel launches of one device-form call: a statistics kernel per local slot, the idf kernel (when the batch has a
-    term), then the host form's per-chunk scoring, winner and finalize kernels; nothing for an empty batch"""
-    if nq == 0:
-        return 0
-    tiles = [tp.n_tiles(r) for r in shard_rows]
-    return len(tiles) + (1 if n_hashes else 0) + tp.tfidf_group_launches(nq, tiles)
+    """kernel launches of one call, host or device form, on the one-slot and loopback groups here"""
+    return tp.tfidf_group_search_launches(nq, [tp.n_tiles(r) for r in shard_rows], n_hashes, loopback=True)
 
 
 def kout(k):
@@ -165,7 +162,10 @@ def test_device_form_equals_host_form_and_whole_index(kind, bounds):
                 before = cdb.kernel_launch_count()
                 got = device_search(lay.g, qs, k)
                 assert cdb.kernel_launch_count() - before == device_launches(len(qs), lay.shard_rows(), h.size)
-                check(got, lay.g.search_tfidf(qs, k))
+                before = cdb.kernel_launch_count()
+                host = lay.g.search_tfidf(qs, k)
+                assert cdb.kernel_launch_count() - before == device_launches(len(qs), lay.shard_rows(), h.size)
+                check(got, host)
                 check(got, lay.whole.batch_search(qs, k))
     # vocab[0]: df past N in the whole index after the later-version deletes
     df, _, n_docs = lay.whole.term_stats(vocab[:1])
@@ -198,7 +198,10 @@ def test_device_form_over_two_group_chunks():
         before = cdb.kernel_launch_count()
         got = device_search(lay.g, qs, k)
         assert cdb.kernel_launch_count() - before == device_launches(len(qs), lay.shard_rows(), h.size)
-        check(got, lay.g.search_tfidf(qs, k))
+        before = cdb.kernel_launch_count()
+        host = lay.g.search_tfidf(qs, k)
+        assert cdb.kernel_launch_count() - before == device_launches(len(qs), lay.shard_rows(), h.size)
+        check(got, host)
         check(got, lay.whole.batch_search(qs, k))
     lay.close()
 

@@ -142,5 +142,15 @@ def tfidf_group_launches(nq, shard_tiles):
     return total
 
 
+def tfidf_group_search_launches(nq, shard_tiles, n_hashes, loopback):
+    """one sharded TF-IDF search, host or device form: a statistics kernel per local slot, the idf kernel (when the batch
+    has a query term) on every local slot, or on slot 0 alone in a loopback group, then tfidf_group_launches; nothing for
+    an empty batch"""
+    if nq == 0:
+        return 0
+    n = len(shard_tiles)
+    return n + (0 if not n_hashes else 1 if loopback else n) + tfidf_group_launches(nq, shard_tiles)
+
+
 def n_tiles(n_rows):
     return ceil_div(n_rows, TILE_ROWS)
