@@ -175,6 +175,48 @@ class HybridGroupSources(C.Structure):
     ]
 
 
+HYBRID_DENSE_SPARSE, HYBRID_DENSE_TFIDF, HYBRID_SPARSE_TFIDF = 0, 1, 2   # CDB_HYBRID_*: a mixed batch's kinds
+
+
+class HybridMixedSources(C.Structure):
+    _fields_ = [
+        ("kinds", C.c_void_p),
+        ("n_dense", C.c_uint32),
+        ("n_sparse", C.c_uint32),
+        ("n_tfidf", C.c_uint32),
+        ("dense", C.c_void_p),
+        ("dense_queries", C.c_void_p),
+        ("dense_params", SearchParams),
+        ("sparse", C.c_void_p),
+        ("sparse_offsets", C.c_void_p),
+        ("sparse_dims", C.c_void_p),
+        ("sparse_values", C.c_void_p),
+        ("sparse_params", SparseSearchParams),
+        ("tfidf", C.c_void_p),
+        ("tfidf_offsets", C.c_void_p),
+        ("tfidf_hashes", C.c_void_p),
+    ]
+
+
+class HybridGroupMixedSources(C.Structure):
+    _fields_ = [
+        ("kinds", C.c_void_p),
+        ("n_dense", C.c_uint32),
+        ("n_sparse", C.c_uint32),
+        ("n_tfidf", C.c_uint32),
+        ("dense_queries", C.c_void_p),
+        ("dense_params", SearchParams),
+        ("dense_id_stride", C.c_uint32),
+        ("sparse_offsets", C.c_void_p),
+        ("sparse_dims", C.c_void_p),
+        ("sparse_values", C.c_void_p),
+        ("sparse_params", SparseSearchParams),
+        ("tfidf_offsets", C.c_void_p),
+        ("tfidf_hashes", C.c_void_p),
+        ("n_tfidf_hashes", C.c_uint64),
+    ]
+
+
 # symbol -> (restype, argtypes); must list every function of include/cosdata_b200.h
 PROTOTYPES = {
     "cdb_abi_version": (C.c_int32, []),
@@ -316,6 +358,14 @@ PROTOTYPES = {
                                                     c_vp, c_vp, c_vp]),
     "cdb_hybrid_search_batch_sharded_device": (C.c_int32, [C.c_void_p, C.POINTER(HybridGroupSources), C.c_uint32, C.c_uint32, C.c_float,
                                                            c_vp, c_vp, c_vp, c_vp, C.c_void_p]),
+    "cdb_hybrid_search_batch_mixed": (C.c_int32, [C.POINTER(HybridMixedSources), C.c_uint32, C.c_uint32, C.c_float, c_u32p, c_f32p,
+                                                  c_u32p, c_u8p]),
+    "cdb_hybrid_search_batch_mixed_device": (C.c_int32, [C.POINTER(HybridMixedSources), C.c_uint32, C.c_uint32, C.c_float, c_u32p,
+                                                         c_f32p, c_u32p, c_u8p, C.c_void_p]),
+    "cdb_hybrid_search_batch_mixed_sharded": (C.c_int32, [C.c_void_p, C.POINTER(HybridGroupMixedSources), C.c_uint32, C.c_uint32,
+                                                          C.c_float, c_vp, c_vp, c_vp, c_vp]),
+    "cdb_hybrid_search_batch_mixed_sharded_device": (C.c_int32, [C.c_void_p, C.POINTER(HybridGroupMixedSources), C.c_uint32,
+                                                                 C.c_uint32, C.c_float, c_vp, c_vp, c_vp, c_vp, C.c_void_p]),
 }
 
 _lib = None

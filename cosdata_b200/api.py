@@ -1255,3 +1255,69 @@ def hybrid_batch_search(top_k=10, fusion_constant_k=60.0, dense=None, sparse=Non
     _check(_lib.load().cdb_hybrid_search_batch(C.byref(src), nq, int(top_k), float(fusion_constant_k), _ptr(ids), _ptr(scores),
                                                _ptr(counts), _ptr(err)))
     return ids[:nq, :w], scores[:nq, :w], counts[:nq], err[:nq]
+
+
+# which sources each kind of a mixed batch names (CDB_HYBRID_DENSE_SPARSE, _DENSE_TFIDF, _SPARSE_TFIDF), first list first
+HYBRID_KIND_SOURCES = (("dense", "sparse"), ("dense", "tfidf"), ("sparse", "tfidf"))
+
+
+def split_mixed(kinds, dense=None, sparse=None, tfidf=None):
+    """batch_hybrid_search's query_mapping: per-query inputs (row or entry q is query q's input for that source; entries of
+    queries whose kind does not name the source are ignored and may be None) -> (kinds u8[B], {source: its queries in
+    request order}), dense as f32[n, dim], sparse and tfidf as lists"""
+    kinds = np.ascontiguousarray(kinds, dtype=np.uint8).reshape(-1)
+    if kinds.size and int(kinds.max()) > 2:
+        raise ValueError("a kind is 0 (dense + sparse), 1 (dense + tfidf) or 2 (sparse + tfidf)")
+    given = {"dense": dense, "sparse": sparse, "tfidf": tfidf}
+    out = {}
+    for name, q in given.items():
+        rows = [i for i, k in enumerate(kinds.tolist()) if name in HYBRID_KIND_SOURCES[k]]
+        if not rows:
+            continue
+        if q is None:
+            raise ValueError(f"queries of kinds that name {name} need {name} inputs")
+        if len(q) != kinds.size:
+            raise ValueError(f"{name}: one input per query ({kinds.size})")
+        out[name] = np.stack([np.asarray(q[i], np.float32) for i in rows]) if name == "dense" else [q[i] for i in rows]
+    return kinds, out
+
+
+def hybrid_batch_search_mixed(kinds, top_k=10, fusion_constant_k=60.0, dense=None, sparse=None, tfidf=None):
+    """batch_hybrid_search over a batch that mixes kinds (cdb_hybrid_search_batch_mixed): kinds[q] names query q's pair
+    (CDB_HYBRID_*: 0 dense + sparse, 1 dense + tfidf, 2 sparse + tfidf); dense = (DenseIndex, per-query vectors [B][dim],
+    DenseIndex.params keywords or None), sparse = (SparseIndex, per-query sparse queries [B], SparseSearchOptions or None),
+    tfidf = (TfIdfIndex, per-query hash lists [B]); entries of queries whose kind does not name the source are ignored.
+    Each source is searched once over the queries that name it.  -> ids u32[B, 6 * top_k], scores f32[B, 6 * top_k],
+    counts u32[B] (the whole fused union), err u8[B] (the dense search's flags; 0 for sparse + tfidf queries)"""
+    ins = {n: (tuple(x) + (None,))[:3] for n, x in (("dense", dense), ("sparse", sparse), ("tfidf", tfidf)) if x is not None}
+    kinds, batches = split_mixed(kinds, *(ins[n][1] if n in ins else None for n in ("dense", "sparse", "tfidf")))
+    nq = kinds.size
+    src, keep = _lib.HybridMixedSources(), [kinds]
+    src.kinds = _ptr(kinds)
+    if "dense" in ins:
+        ix, _, opts = ins["dense"]
+        src.dense, src.dense_params = ix._h, ix.params(0, **(opts or {}))
+    if "sparse" in ins:
+        src.sparse, src.sparse_params = ins["sparse"][0].h, (ins["sparse"][2] or SparseSearchOptions(0)).params()
+    if "tfidf" in ins:
+        src.tfidf = ins["tfidf"][0].h
+    if "dense" in batches:
+        q = np.ascontiguousarray(batches["dense"], dtype=np.float32)
+        src.n_dense, src.dense_queries = q.shape[0], _ptr(q)
+        keep.append(q)
+    if "sparse" in batches:
+        o, d, v = sparse_csr(batches["sparse"])
+        src.n_sparse, src.sparse_offsets, src.sparse_dims, src.sparse_values = len(o) - 1, _ptr(o), _ptr(d), _ptr(v)
+        keep += [o, d, v]
+    if "tfidf" in batches:
+        o, h = _query_csr(batches["tfidf"])
+        src.n_tfidf, src.tfidf_offsets, src.tfidf_hashes = len(o) - 1, _ptr(o), _ptr(h)
+        keep += [o, h]
+    w = 6 * int(top_k)
+    ids = np.zeros((max(nq, 1), max(w, 1)), np.uint32)
+    scores = np.zeros((max(nq, 1), max(w, 1)), np.float32)
+    counts = np.zeros(max(nq, 1), np.uint32)
+    err = np.zeros(max(nq, 1), np.uint8)
+    _check(_lib.load().cdb_hybrid_search_batch_mixed(C.byref(src), nq, int(top_k), float(fusion_constant_k), _ptr(ids), _ptr(scores),
+                                                     _ptr(counts), _ptr(err)))
+    return ids[:nq, :w], scores[:nq, :w], counts[:nq], err[:nq]

@@ -82,11 +82,37 @@ struct RrfList {
     const uint32_t *ids;      // [B][ld]
     const uint32_t *counts;   // [B]
     uint32_t ld, stride;
+    const uint32_t *rows = nullptr;   // device, [n]: the list row fused into row i (null: row i)
+};
+// a mixed batch's fusion: fused row i lands in output row rows[i] (null: row i); with err, err[rows[i]] = err_in[first
+// list's row] (null err_in: 0)
+struct RrfRows {
+    const uint32_t *rows = nullptr;
+    const uint8_t *err_in = nullptr;
+    uint8_t *err = nullptr;
 };
 cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t ld_out, const void *ids_a, const void *cnt_a,
                            const void *ids_b, const void *cnt_b, const void *out_ids, const void *out_scores, const void *out_counts);
 cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k, uint32_t ld_out, uint32_t *d_ids, float *d_scores,
-                       uint32_t *d_counts, cudaStream_t s);
+                       uint32_t *d_counts, cudaStream_t s, const RrfRows &o = RrfRows{});
+
+// a mixed hybrid batch (cdb_hybrid_search_batch_mixed*): each query's kind names two of the sources dense (0), sparse (1)
+// and TF-IDF (2), first list first; a source's batch holds the queries whose kind names it, in request order
+constexpr int HYB_KIND_SRC[3][2] = {{0, 1}, {0, 2}, {1, 2}};
+// request positions [q0, q1): rows [row0[j], row0[j] + rows[j]) of source j's batch, n[c] queries of kind c, whose maps
+// sit at map[c] in the map array: output rows (from q0), first-list rows, second-list rows (from each source's row0)
+struct MixedChunk {
+    uint32_t q0, q1, row0[3], rows[3], n[3];
+    size_t map[3];
+};
+// kinds non-null when nq > 0, every kind <= 2, and the per-source counts those kinds give
+cdb_status check_kinds(const uint8_t *kinds, uint32_t nq, const uint32_t n_src[3]);
+// chunks of at most `chunk` request positions, and their maps (3 * nq u32)
+void mixed_chunks(const uint8_t *kinds, uint32_t nq, uint32_t chunk, std::vector<MixedChunk> *chunks, std::vector<uint32_t> *maps);
+// one fusion launch per kind present in the chunk: lists[j] holds source j's rows of the chunk (rows unset), d_maps the map
+// array on the device, d_err_dense the dense search's error bytes of the chunk; the outputs start at the chunk's q0
+cdb_status mixed_fuse(const MixedChunk &c, const RrfList lists[3], const uint32_t *d_maps, const uint8_t *d_err_dense, float k,
+                      uint32_t ld_out, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s);
 
 // ---- pairs.cu
 cdb_status distance_pairs_device(int metric, int st, uint32_t dim, const uint8_t *d_x, const float *d_xm,

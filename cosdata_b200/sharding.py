@@ -452,6 +452,71 @@ class ShardGroup:
         _check(self._lib.cdb_hybrid_search_batch_sharded_device(self._h, C.byref(src), nq, int(top_k), float(fusion_constant_k), d_ids,
                                                                 d_scores, d_counts, d_err, C.c_void_p(stream_ptr) if stream_ptr else None))
 
+    def _mixed_sources(self, kinds, dense, sparse, tfidf, dense_id_stride):
+        """cdb_hybrid_group_mixed_sources of kinds (host) and every source's params; queries are set by the caller"""
+        from . import _lib
+        from .api import HYBRID_KIND_SOURCES, SparseSearchOptions, _ptr
+        kinds = np.ascontiguousarray(kinds, dtype=np.uint8).reshape(-1)
+        src = _lib.HybridGroupMixedSources()
+        src.kinds = _ptr(kinds)
+        src.n_dense, src.n_sparse, src.n_tfidf = (sum(name in HYBRID_KIND_SOURCES[k] for k in kinds.tolist() if k <= 2)
+                                                  for name in ("dense", "sparse", "tfidf"))
+        if dense is not None:
+            src.dense_params = self._shards[0].params(0, **((tuple(dense) + (None,))[1] or {}))
+        if sparse is not None:
+            src.sparse_params = ((tuple(sparse) + (None,))[1] or SparseSearchOptions(0)).params()
+        src.dense_id_stride = int(dense_id_stride)
+        return src, kinds
+
+    def hybrid_search_mixed(self, kinds, top_k=10, fusion_constant_k=60.0, dense=None, sparse=None, tfidf=None, dense_id_stride=1):
+        """batch_hybrid_search over a batch that mixes kinds (cdb_hybrid_search_batch_mixed_sharded): kinds[q] names query q's
+        pair (0 dense + sparse, 1 dense + tfidf, 2 sparse + tfidf); dense = (per-query vectors [B][dim], DenseIndex.params
+        keywords), sparse = (per-query sparse queries [B], SparseSearchOptions), tfidf = per-query hash lists [B]; entries of
+        queries whose kind does not name the source are ignored.  -> ids u32[B, 6 * top_k], scores, counts u32[B], err u8[B]
+        (the dense search's flags OR-ed over the ranks; 0 for sparse + tfidf queries)"""
+        from .api import _check, _ptr, _query_csr, sparse_csr, split_mixed
+        kinds, batches = split_mixed(kinds, None if dense is None else tuple(dense)[0], None if sparse is None else tuple(sparse)[0], tfidf)
+        src, kinds = self._mixed_sources(kinds, dense, sparse, tfidf, dense_id_stride)
+        keep = [kinds]
+        if "dense" in batches:
+            q = np.ascontiguousarray(batches["dense"], dtype=np.float32)
+            src.dense_queries = _ptr(q)
+            keep.append(q)
+        if "sparse" in batches:
+            q = sparse_csr(batches["sparse"])
+            src.sparse_offsets, src.sparse_dims, src.sparse_values = [_ptr(a) for a in q]
+            keep += list(q)
+        if "tfidf" in batches:
+            q = _query_csr(batches["tfidf"])
+            src.tfidf_offsets, src.tfidf_hashes = [_ptr(a) for a in q]
+            src.n_tfidf_hashes = int(q[0][-1])
+            keep += list(q)
+        nq, w = kinds.size, 6 * int(top_k)
+        ids = np.zeros((max(nq, 1), max(w, 1)), np.uint32)
+        scores = np.zeros((max(nq, 1), max(w, 1)), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        err = np.zeros(max(nq, 1), np.uint8)
+        _check(self._lib.cdb_hybrid_search_batch_mixed_sharded(self._h, C.byref(src), nq, int(top_k), float(fusion_constant_k), _ptr(ids),
+                                                               _ptr(scores), _ptr(counts), _ptr(err)))
+        return ids[:nq, :w], scores[:nq, :w], counts[:nq], err[:nq]
+
+    def hybrid_search_mixed_device(self, kinds, d_ids, d_scores, d_counts, d_err=None, stream_ptr=None, top_k=10, fusion_constant_k=60.0,
+                                   dense=None, sparse=None, tfidf=None, dense_id_stride=1):
+        """groups of one local slot: hybrid_search_mixed on device pointers (ints), asynchronous on the stream.  kinds stays
+        a host array; each source's queries are already its batch in request order, on the device: dense = (d_queries,
+        kw), sparse = ((d_offsets, d_dims, d_values), options), tfidf = (d_offsets, d_hashes, n_hashes)."""
+        from .api import _check
+        src, kinds = self._mixed_sources(kinds, dense, sparse, tfidf, dense_id_stride)
+        if dense is not None:
+            src.dense_queries = tuple(dense)[0]
+        if sparse is not None:
+            src.sparse_offsets, src.sparse_dims, src.sparse_values = tuple(sparse)[0]
+        if tfidf is not None:
+            src.tfidf_offsets, src.tfidf_hashes, src.n_tfidf_hashes = tfidf
+        _check(self._lib.cdb_hybrid_search_batch_mixed_sharded_device(self._h, C.byref(src), kinds.size, int(top_k), float(fusion_constant_k),
+                                                                      d_ids, d_scores, d_counts, d_err,
+                                                                      C.c_void_p(stream_ptr) if stream_ptr else None))
+
     def close(self):
         if self._h:
             self._lib.cdb_shard_group_destroy(self._h)

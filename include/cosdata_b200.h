@@ -981,8 +981,8 @@ cdb_status cdb_sparse_search_batch_all_sharded(cdb_shard_group *group, const uin
  * k's payload and the quiet bit set (0xFFA00001 -> 0xFFE00001), as x86 SSE propagates it.  No other NaN or -inf arises.
  * Threshold.  batch_hybrid_search searches the sparse side with early_terminate_threshold None (the config value) where
  * hybrid_search passes the request's; here it is sparse_params.early_terminate_threshold, one value per call -- a single
- * request is a batch of 1.  A batch that mixes kinds of request is split by kind pair by the caller (queries are
- * independent, so the results do not change). */
+ * request is a batch of 1.  A batch that mixes kinds of request goes to cdb_hybrid_search_batch_mixed[_sharded][_device]
+ * below, which searches each source once for every query that names it. */
 
 /* Generic fusion of two ranked id lists per query: ids [B][ld], counts [B] (entries below min(count, ld) are taken as
  * given, CDB_INVALID_ID included), id_stride per list as above.  out_ids / out_scores [B][ld_out], out_counts [B].
@@ -1081,6 +1081,91 @@ cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *group, const cdb_hyb
 cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *group, const cdb_hybrid_group_sources *sources,
                                                   uint32_t n_queries, uint32_t top_k, float fusion_constant_k, uint32_t *d_ids,
                                                   float *d_scores, uint32_t *d_counts, uint8_t *d_err_flags, void *stream);
+
+/* ------------------------------------------------ hybrid search over mixed batches
+ * batch_hybrid_search (repo.rs:343-555) takes a batch in which each query names its own pair of sources.  kinds[q] is
+ * query q's pair: the first list is the source the kind names first. */
+enum { CDB_HYBRID_DENSE_SPARSE = 0, CDB_HYBRID_DENSE_TFIDF = 1, CDB_HYBRID_SPARSE_TFIDF = 2 };
+
+/* A mixed batch of B queries.  kinds [B] is HOST memory in both forms (request metadata, read to plan the call).  A source's
+ * queries are those whose kind names it, in request order (the reference's dense_queries, sparse_queries and
+ * tfidf_queries): n_dense = the DENSE_SPARSE and DENSE_TFIDF queries, n_sparse = the DENSE_SPARSE and SPARSE_TFIDF ones,
+ * n_tfidf = the DENSE_TFIDF and SPARSE_TFIDF ones (host counts).  A source with a count of 0 is not searched and its
+ * handle and queries may be NULL.  Queries are host arrays for cdb_hybrid_search_batch_mixed and device arrays for the
+ * device form; the k of each params struct is ignored, as above. */
+typedef struct {
+    const uint8_t *kinds;                     /* [B] CDB_HYBRID_*, host memory */
+    uint32_t n_dense, n_sparse, n_tfidf;
+    cdb_index *dense;
+    const float *dense_queries;               /* [n_dense][dim] raw f32 */
+    cdb_search_params dense_params;
+    cdb_sparse_index *sparse;
+    const uint64_t *sparse_offsets;           /* CSR [n_sparse + 1] */
+    const uint32_t *sparse_dims;
+    const float *sparse_values;
+    cdb_sparse_search_params sparse_params;
+    cdb_tfidf_index *tfidf;
+    const uint64_t *tfidf_offsets;            /* CSR [n_tfidf + 1] of term hashes */
+    const uint32_t *tfidf_hashes;
+} cdb_hybrid_mixed_sources;
+
+/* Hybrid search over a mixed batch (DESIGN.md section 8i).  Row q is, bit for bit in ids, counts and score bits, the row
+ * cdb_hybrid_search_batch returns for query q when the batch is split by kind (queries are independent): every source
+ * with queries is searched ONCE, at k = 3 * top_k (TF-IDF: min(3 * top_k, 512) results), the first on the caller's stream
+ * and the others on side streams forked from and joined back to it, then each kind present is fused with one launch
+ * straight into its queries' rows.  out_ids / out_scores [B][6 * top_k], out_counts [B]; err_flags [B] (may be NULL)
+ * receives the dense search's flags of each query that names the dense source and 0 for SPARSE_TFIDF queries.
+ * sparse_params is one value per call: the batch form passes early_terminate_threshold None (the config value) and
+ * ignores the per-query thresholds, as the reference does.  Locks and snapshots as cdb_hybrid_search_batch.
+ * CDB_INVALID_PARAMS, before any copy or launch: null sources or output; top_k > 341; null kinds with B > 0; a kind above 2;
+ * counts that disagree with kinds; CDB_SEARCH_ALL_CANDIDATES with dense queries; a null handle or null queries of a source
+ * with queries; sparse rerank with 3 * top_k * reranking_factor > 5120; malformed host query CSR (host form); handles of
+ * the searched sources on different devices.  CDB_UNSUPPORTED: a dense handle with graph metadata (use a one-slot shard
+ * group and cdb_hybrid_search_batch_mixed_sharded).  B = 0 or top_k = 0: counts zeroed, no kernel launched. */
+cdb_status cdb_hybrid_search_batch_mixed(const cdb_hybrid_mixed_sources *sources, uint32_t n_queries, uint32_t top_k,
+                                         float fusion_constant_k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts,
+                                         uint8_t *err_flags);
+cdb_status cdb_hybrid_search_batch_mixed_device(const cdb_hybrid_mixed_sources *sources, uint32_t n_queries, uint32_t top_k,
+                                                float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
+                                                uint8_t *d_err_flags, void *stream);
+
+/* A mixed batch over a shard group: the fields of cdb_hybrid_mixed_sources with the group's shards in place of handles (a
+ * source with queries needs a shard of its kind in every local slot).  dense_id_stride is the dense list's id_stride, as in
+ * cdb_hybrid_group_sources.  n_tfidf_hashes is the term count of the TF-IDF CSR (tfidf_offsets[n_tfidf]): the device form
+ * sizes the group's idf exchange by it (the host form reads it from the offsets and ignores the field). */
+typedef struct {
+    const uint8_t *kinds;                     /* [B] CDB_HYBRID_*, host memory */
+    uint32_t n_dense, n_sparse, n_tfidf;
+    const float *dense_queries;               /* [n_dense][dim] raw f32 */
+    cdb_search_params dense_params;
+    uint32_t dense_id_stride;
+    const uint64_t *sparse_offsets;           /* CSR [n_sparse + 1] */
+    const uint32_t *sparse_dims;
+    const float *sparse_values;
+    cdb_sparse_search_params sparse_params;
+    const uint64_t *tfidf_offsets;            /* CSR [n_tfidf + 1] of term hashes */
+    const uint32_t *tfidf_hashes;
+    uint64_t n_tfidf_hashes;
+} cdb_hybrid_group_mixed_sources;
+
+/* The contract of cdb_hybrid_search_batch_mixed over the group: row q is the row cdb_hybrid_search_batch_sharded returns
+ * for query q when the batch is split by kind, and err_flags are OR-ed over the ranks.  Under one hold of the group's lock
+ * the sources with queries run one after the other in the order dense, sparse, TF-IDF; a source without queries issues no
+ * collective.  Every rank passes the same kinds, so every rank issues the same collectives.  The TF-IDF idf step runs once
+ * per call over the TF-IDF queries.  Request positions are taken in chunks that keep the intermediate lists within 256 MB;
+ * a chunk is one contiguous range of each source's queries, each sub-search takes its range and the fusion the chunk.
+ * The host form stages each source's queries once per local device.  The device form serves groups of one local slot and
+ * takes device arrays, TF-IDF included, asynchronously on `stream` (NULL = the legacy default stream).
+ * CDB_INVALID_PARAMS, before any copy or launch: the refusals of cdb_hybrid_search_batch_mixed that need no handle, n_tfidf_hashes
+ * >= 2^31, then under the group's lock those of cdb_hybrid_search_batch_sharded: a local slot without a shard of a searched
+ * kind, local dense shards of which some have graph metadata and some do not (or a mode other than CDB_MODE_HNSW on
+ * metadata shards), world * 3 * top_k * 8 > 200 KB (the dense merge).  B = 0 or top_k = 0: counts zeroed, nothing launched. */
+cdb_status cdb_hybrid_search_batch_mixed_sharded(cdb_shard_group *group, const cdb_hybrid_group_mixed_sources *sources,
+                                                 uint32_t n_queries, uint32_t top_k, float fusion_constant_k, uint32_t *out_ids,
+                                                 float *out_scores, uint32_t *out_counts, uint8_t *err_flags);
+cdb_status cdb_hybrid_search_batch_mixed_sharded_device(cdb_shard_group *group, const cdb_hybrid_group_mixed_sources *sources,
+                                                        uint32_t n_queries, uint32_t top_k, float fusion_constant_k, uint32_t *d_ids,
+                                                        float *d_scores, uint32_t *d_counts, uint8_t *d_err_flags, void *stream);
 
 #ifdef __cplusplus
 }

@@ -295,6 +295,20 @@ class ShardGroup {
                                               r.err.data()));
         return r;
     }
+    // batch_hybrid_search over a batch that mixes kinds (host arrays in `sources`, kinds[b] naming each query's pair): each
+    // source searched once, rows as hybrid_search, err = the dense search's flags (0 for SPARSE_TFIDF queries)
+    SearchResults hybrid_search_mixed(const cdb_hybrid_group_mixed_sources &sources, uint32_t b, uint32_t top_k = 10,
+                                      float fusion_constant_k = 60.0f) const {
+        SearchResults r;
+        r.k = 6 * top_k;
+        r.ids.resize((size_t)b * r.k);
+        r.scores.resize((size_t)b * r.k);
+        r.counts.resize(b);
+        r.err.resize(b);
+        check(cdb_hybrid_search_batch_mixed_sharded(g_, &sources, b, top_k, fusion_constant_k, r.ids.data(), r.scores.data(),
+                                                    r.counts.data(), r.err.data()));
+        return r;
+    }
 
   private:
     cdb_shard_group *g_ = nullptr;
