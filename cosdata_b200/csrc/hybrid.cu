@@ -1,8 +1,8 @@
 // hybrid.cu -- hybrid search (hybrid_search / batch_hybrid_search, src/api/vectordb/search/repo.rs:168-555): reciprocal-rank
-// fusion of two ranked lists per query, and the composed search that runs two of the dense, sparse and TF-IDF searches and
-// fuses their results on the device.  The contract is the header comment of cdb_rrf_fuse (DESIGN.md section 8e).
-// check_fuse_args and fuse_launch also serve a shard group's hybrid search (shard_group.cu, DESIGN.md section 8h).  A mixed
-// batch (each query names its own pair, DESIGN.md section 8i) searches each source once and fuses each kind through row maps.
+// fusion of two ranked lists per query, and the composed search that runs the dense, sparse and TF-IDF searches a batch
+// names and fuses their results on the device.  The contract is the header comment of cdb_rrf_fuse (DESIGN.md section 8e).
+// Each query of a batch names its own pair of sources (DESIGN.md section 8i); a two-source call is a batch of one kind.
+// The request check, the chunks and the fusion also serve a shard group's hybrid search (shard_group.cu, DESIGN.md 8h).
 //
 // rrf_fuse_kernel: one CTA per query.  Every live entry becomes (key << 32 | list << 31 | rank) in shared memory; a bitonic
 // sort groups each key's entries, first list before second, each in rank order; the head of every run folds it (first
@@ -20,7 +20,6 @@ namespace cdb {
 namespace {
 
 constexpr uint32_t RRF_MAX = 2048;      // entries of both lists of one query
-constexpr uint32_t TF_RESULTS = 512;    // TF-IDF's bucket count: its searches return at most 512 results
 
 // 1.0 / (rank as f32 + k + f32::EPSILON): one rounding per operation, left to right, no FMA, no approximate reciprocal
 __device__ __forceinline__ float rrf_contribution(uint32_t rank, float k) {
@@ -94,8 +93,6 @@ __global__ void __launch_bounds__(1024) rrf_fuse_kernel(RrfList a, RrfList b, fl
     if (tid == 0) out_counts[q] = cnt;
 }
 
-}  // namespace
-
 cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t ld_out, const void *ids_a, const void *cnt_a,
                            const void *ids_b, const void *cnt_b, const void *out_ids, const void *out_scores, const void *out_counts) {
     CDB_REQUIRE((uint64_t)ld_a + ld_b <= RRF_MAX, "ld_first + ld_second must be <= 2048");
@@ -105,6 +102,8 @@ cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t l
     CDB_REQUIRE(!nq || !ld_out || (out_ids && out_scores), "null output");
     return CDB_OK;
 }
+
+}  // namespace
 
 cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k, uint32_t ld_out, uint32_t *d_ids, float *d_scores,
                        uint32_t *d_counts, cudaStream_t s, const RrfRows &o) {
@@ -117,6 +116,9 @@ cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k,
     return CDB_OK;
 }
 
+namespace {
+
+// kinds non-null when nq > 0, every kind <= 2, and the per-source counts those kinds give
 cdb_status check_kinds(const uint8_t *kinds, uint32_t nq, const uint32_t n_src[3]) {
     CDB_REQUIRE(kinds || !nq, "null kinds");
     uint32_t n[3] = {0, 0, 0};
@@ -133,8 +135,89 @@ cdb_status check_kinds(const uint8_t *kinds, uint32_t nq, const uint32_t n_src[3
     return CDB_OK;
 }
 
-void mixed_chunks(const uint8_t *kinds, uint32_t nq, uint32_t chunk, std::vector<MixedChunk> *chunks, std::vector<uint32_t> *maps) {
-    maps->assign((size_t)3 * nq, 0);
+// the fields of a request that the single index's and the group's sources share
+struct Request {
+    const uint8_t *kinds;
+    uint32_t n[3];
+    const void *const *handle;   // the single index's handles; null for a group, whose slots are checked under its lock
+    const float *dense_queries;
+    cdb_search_params dense_params;
+    const uint64_t *sparse_offsets;
+    const uint32_t *sparse_dims;
+    const float *sparse_values;
+    cdb_sparse_search_params sparse_params;
+    const uint64_t *tfidf_offsets;
+    const uint32_t *tfidf_hashes;
+    bool host;                   // the query arrays are host memory
+};
+
+template <class S> Request request_of(const S &s, const void *const *handle, bool host) {
+    return Request{s.kinds, {s.n_dense, s.n_sparse, s.n_tfidf}, handle, s.dense_queries, s.dense_params, s.sparse_offsets,
+                   s.sparse_dims, s.sparse_values, s.sparse_params, s.tfidf_offsets, s.tfidf_hashes, host};
+}
+
+// r null: the caller passed no sources
+cdb_status check_request(const Request *r, uint32_t nq, uint32_t top_k) {
+    CDB_REQUIRE(r, "null sources");
+    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
+    if (cdb_status rc = check_kinds(r->kinds, nq, r->n)) return rc;
+    const uint32_t nd = r->n[HYB_DENSE], ns = r->n[HYB_SPARSE], nt = r->n[HYB_TFIDF];
+    // the reference's dense sub-search always has Some(3 * top_k): top_k None has no hybrid form
+    CDB_REQUIRE(!nd || !(r->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
+                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
+    if (r->handle) {
+        CDB_REQUIRE(!nd || r->handle[HYB_DENSE], "null dense handle");
+        CDB_REQUIRE(!ns || r->handle[HYB_SPARSE], "null sparse handle");
+        CDB_REQUIRE(!nt || r->handle[HYB_TFIDF], "null tf-idf handle");
+    }
+    CDB_REQUIRE(!nd || r->dense_queries, "null dense queries");
+    CDB_REQUIRE(!ns || r->sparse_offsets, "null sparse query offsets");
+    CDB_REQUIRE(!nt || r->tfidf_offsets, "null tf-idf query offsets");
+    if (ns && r->sparse_params.rerank)
+        CDB_REQUIRE(r->sparse_params.reranking_factor >= 1 && (uint64_t)3 * top_k * r->sparse_params.reranking_factor <= 5120,
+                    "3 * top_k * reranking_factor must be in 1..5120");
+    if (r->host && ns) {
+        if (cdb_status rc = check_csr(r->sparse_offsets, ns, "sparse_offsets")) return rc;
+        CDB_REQUIRE((r->sparse_dims && r->sparse_values) || !r->sparse_offsets[ns], "null sparse query pairs");
+    }
+    if (r->host && nt) {
+        if (cdb_status rc = check_csr(r->tfidf_offsets, nt, "tfidf_offsets")) return rc;
+        CDB_REQUIRE(r->tfidf_hashes || !r->tfidf_offsets[nt], "null tf-idf query hashes");
+    }
+    return CDB_OK;
+}
+
+}  // namespace
+
+cdb_status hybrid_pair_kinds(bool dense, bool sparse, bool tfidf, uint32_t nq, std::vector<uint8_t> *kinds) {
+    CDB_REQUIRE(dense + sparse + tfidf == 2, "a hybrid search takes exactly two sources");
+    kinds->assign(nq, !dense ? CDB_HYBRID_SPARSE_TFIDF : sparse ? CDB_HYBRID_DENSE_SPARSE : CDB_HYBRID_DENSE_TFIDF);
+    return CDB_OK;
+}
+
+cdb_status check_hybrid_request(const cdb_hybrid_mixed_sources *m, uint32_t nq, uint32_t top_k, bool host) {
+    if (!m) return check_request(nullptr, nq, top_k);
+    const void *const handle[3] = {m->dense, m->sparse, m->tfidf};
+    const Request r = request_of(*m, handle, host);
+    return check_request(&r, nq, top_k);
+}
+
+cdb_status check_hybrid_request(const cdb_hybrid_group_mixed_sources *h, uint32_t nq, uint32_t top_k, bool host) {
+    if (!h) return check_request(nullptr, nq, top_k);
+    const Request r = request_of(*h, nullptr, host);
+    return check_request(&r, nq, top_k);
+}
+
+void mixed_chunks(const uint8_t *kinds, uint32_t nq, const uint32_t ld[3], size_t budget, std::vector<MixedChunk> *chunks,
+                  std::vector<uint32_t> *maps) {
+    bool present[3] = {false, false, false};
+    for (uint32_t q = 0; q < nq; ++q) present[kinds[q]] = true;
+    const bool one_kind = present[0] + present[1] + present[2] == 1;
+    size_t per_q = 0;   // bytes of one request position
+    for (int kd = 0; kd < 3; ++kd)
+        if (present[kd]) per_q = std::max(per_q, ((size_t)ld[HYB_KIND_SRC[kd][0]] + ld[HYB_KIND_SRC[kd][1]]) * 8 + (one_kind ? 8 : 9));
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nq, budget / per_q));
+    maps->assign(one_kind ? 0 : (size_t)3 * nq, 0);
     uint32_t next[3] = {0, 0, 0};   // each source's next row
     size_t at = 0;
     for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
@@ -150,11 +233,15 @@ void mixed_chunks(const uint8_t *kinds, uint32_t nq, uint32_t chunk, std::vector
         uint32_t fill[3] = {0, 0, 0};
         for (uint32_t q = c.q0; q < c.q1; ++q) {
             const int kd = kinds[q], f = HYB_KIND_SRC[kd][0], s = HYB_KIND_SRC[kd][1];
-            uint32_t *m = maps->data() + c.map[kd];
-            const uint32_t i = fill[kd]++;
-            m[i] = q - c.q0;
-            m[c.n[kd] + i] = next[f]++ - c.row0[f];
-            m[2 * (size_t)c.n[kd] + i] = next[s]++ - c.row0[s];
+            if (!one_kind) {
+                uint32_t *m = maps->data() + c.map[kd];
+                const uint32_t i = fill[kd]++;
+                m[i] = q - c.q0;
+                m[c.n[kd] + i] = next[f] - c.row0[f];
+                m[2 * (size_t)c.n[kd] + i] = next[s] - c.row0[s];
+            }
+            ++next[f];
+            ++next[s];
         }
         for (int j = 0; j < 3; ++j) c.rows[j] = next[j] - c.row0[j];
         chunks->push_back(c);
@@ -166,11 +253,15 @@ cdb_status mixed_fuse(const MixedChunk &c, const RrfList lists[3], const uint32_
     for (int kd = 0; kd < 3; ++kd) {
         if (!c.n[kd]) continue;
         const int f = HYB_KIND_SRC[kd][0];
-        const uint32_t *m = d_maps + c.map[kd];
         RrfList a = lists[f], b = lists[HYB_KIND_SRC[kd][1]];
-        a.rows = m + c.n[kd];
-        b.rows = m + 2 * (size_t)c.n[kd];
-        const RrfRows o{m, f == 0 ? d_err_dense : nullptr, d_err};
+        // without maps a dense search wrote its error bytes in place
+        RrfRows o{nullptr, nullptr, f == HYB_DENSE ? nullptr : d_err};
+        if (d_maps) {
+            const uint32_t *m = d_maps + c.map[kd];
+            a.rows = m + c.n[kd];
+            b.rows = m + 2 * (size_t)c.n[kd];
+            o = RrfRows{m, f == HYB_DENSE ? d_err_dense : nullptr, d_err};
+        }
         if (cdb_status rc = fuse_launch(a, b, c.n[kd], k, ld_out, d_ids, d_scores, d_counts, s, o)) return rc;
     }
     return CDB_OK;
@@ -178,167 +269,95 @@ cdb_status mixed_fuse(const MixedChunk &c, const RrfList lists[3], const uint32_
 
 namespace {
 
-enum Source { SRC_DENSE = 0, SRC_SPARSE = 1, SRC_TFIDF = 2 };
-
-// The sources a call searches, in list order (a pair: first, second; a mixed batch: dense, sparse, TF-IDF, those with
-// queries), each over its own batch of nq[i] queries, and the fusions of their lists.
-struct Plan {
-    int n = 0;
-    Source src[3];
-    uint32_t nq[3];
-    uint32_t ld[3];       // columns of each intermediate list
-    int device = -1;
-};
-
-uint32_t source_ld(Source s, uint32_t top_k) { return s == SRC_TFIDF ? std::min(3 * top_k, TF_RESULTS) : 3 * top_k; }
-
-int source_device(const cdb_hybrid_sources *h, Source s) {
-    return s == SRC_DENSE ? index_device(h->dense) : s == SRC_SPARSE ? sparse_index_device(h->sparse) : tfidf_index_device(h->tfidf);
-}
-
-// the refusals shared by both forms of sources after the source list: sparse rerank bound, one device, no graph metadata
-cdb_status plan_sources(const cdb_hybrid_sources *h, uint32_t top_k, Plan *p) {
-    const uint32_t k3 = 3 * top_k;
-    bool sparse = false;
-    for (int j = 0; j < p->n; ++j) sparse |= p->src[j] == SRC_SPARSE;
-    if (sparse && h->sparse_params.rerank)
-        CDB_REQUIRE(h->sparse_params.reranking_factor >= 1 && (uint64_t)k3 * h->sparse_params.reranking_factor <= 5120,
-                   "3 * top_k * reranking_factor must be in 1..5120");
-    // the handles' devices (immutable after create)
-    for (int j = 0; j < p->n; ++j) {
-        const int d = source_device(h, p->src[j]);
-        CDB_REQUIRE(!j || d == p->device, "the handles live on different devices");
-        p->device = d;
+// the request's refusals, then its handles (immutable after create): the sources with queries live on one device, and
+// the dense one has no graph metadata
+cdb_status check_single(const cdb_hybrid_mixed_sources *m, uint32_t nq, uint32_t top_k, bool host, int *device) {
+    if (cdb_status rc = check_hybrid_request(m, nq, top_k, host)) return rc;
+    const int dev[3] = {m->n_dense ? index_device(m->dense) : -1, m->n_sparse ? sparse_index_device(m->sparse) : -1,
+                        m->n_tfidf ? tfidf_index_device(m->tfidf) : -1};
+    for (int j = 0; j < 3; ++j) {
+        CDB_REQUIRE(dev[j] < 0 || *device < 0 || dev[j] == *device, "the handles live on different devices");
+        if (dev[j] >= 0) *device = dev[j];
     }
-    for (int j = 0; j < p->n; ++j)
-        if (p->src[j] == SRC_DENSE && index_has_graph_metadata(h->dense)) {
-            set_error("a dense handle with graph metadata searches through cdb_search_batch_filtered: fuse with cdb_rrf_fuse");
-            return CDB_UNSUPPORTED;
-        }
+    if (m->n_dense && index_has_graph_metadata(m->dense)) {
+        set_error("a dense handle with graph metadata searches through cdb_search_batch_filtered: fuse with cdb_rrf_fuse");
+        return CDB_UNSUPPORTED;
+    }
     return CDB_OK;
 }
 
-// every refusal that needs no device: the handles are read only after the request itself is well-formed
-cdb_status make_plan(const cdb_hybrid_sources *h, uint32_t nq, uint32_t top_k, Plan *p) {
+// a two-source call as a batch of one kind: both named sources take every query
+cdb_status pair_as_batch(const cdb_hybrid_sources *h, uint32_t nq, std::vector<uint8_t> *kinds, cdb_hybrid_mixed_sources *m) {
     CDB_REQUIRE(h, "null sources");
-    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
-    const int n_src = (h->dense != nullptr) + (h->sparse != nullptr) + (h->tfidf != nullptr);
-    CDB_REQUIRE(n_src == 2, "a hybrid search takes exactly two sources");
-    // the reference's dense sub-search always has Some(3 * top_k): top_k None has no hybrid form
-    CDB_REQUIRE(!h->dense || !(h->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
-                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
-    if (h->dense) p->src[p->n++] = SRC_DENSE;
-    if (h->sparse) p->src[p->n++] = SRC_SPARSE;
-    if (h->tfidf) p->src[p->n++] = SRC_TFIDF;
-    for (int j = 0; j < p->n; ++j) {
-        p->nq[j] = nq;
-        p->ld[j] = source_ld(p->src[j], top_k);
-    }
-    CDB_REQUIRE(!h->dense || h->dense_queries || !nq, "null dense queries");
-    CDB_REQUIRE(!h->sparse || h->sparse_offsets || !nq, "null sparse query offsets");
-    CDB_REQUIRE(!h->tfidf || h->tfidf_offsets || !nq, "null tf-idf query offsets");
-    return plan_sources(h, top_k, p);
+    if (cdb_status rc = hybrid_pair_kinds(h->dense, h->sparse, h->tfidf, nq, kinds)) return rc;
+    *m = cdb_hybrid_mixed_sources{kinds->data(), h->dense ? nq : 0, h->sparse ? nq : 0, h->tfidf ? nq : 0, h->dense,
+                                  h->dense_queries, h->dense_params, h->sparse, h->sparse_offsets, h->sparse_dims,
+                                  h->sparse_values, h->sparse_params, h->tfidf, h->tfidf_offsets, h->tfidf_hashes};
+    return CDB_OK;
 }
 
-// a mixed batch's sources as cdb_hybrid_sources, and its plan: the sources with queries, in the order dense, sparse, TF-IDF.
-// host: the query CSRs are host arrays, checked too.  Every refusal of the request comes before a handle is read.
-cdb_status make_mixed_plan(const cdb_hybrid_mixed_sources *m, uint32_t nq, uint32_t top_k, bool host, cdb_hybrid_sources *h, Plan *p) {
-    CDB_REQUIRE(m, "null sources");
-    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
-    const uint32_t n_src[3] = {m->n_dense, m->n_sparse, m->n_tfidf};
-    if (cdb_status rc = check_kinds(m->kinds, nq, n_src)) return rc;
-    CDB_REQUIRE(!m->n_dense || !(m->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
-                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
-    CDB_REQUIRE(!m->n_dense || m->dense, "null dense handle");
-    CDB_REQUIRE(!m->n_sparse || m->sparse, "null sparse handle");
-    CDB_REQUIRE(!m->n_tfidf || m->tfidf, "null tf-idf handle");
-    CDB_REQUIRE(!m->n_dense || m->dense_queries, "null dense queries");
-    CDB_REQUIRE(!m->n_sparse || m->sparse_offsets, "null sparse query offsets");
-    CDB_REQUIRE(!m->n_tfidf || m->tfidf_offsets, "null tf-idf query offsets");
-    if (m->n_sparse && m->sparse_params.rerank)
-        CDB_REQUIRE(m->sparse_params.reranking_factor >= 1 && (uint64_t)3 * top_k * m->sparse_params.reranking_factor <= 5120,
-                   "3 * top_k * reranking_factor must be in 1..5120");
-    if (host && m->n_sparse) {
-        if (cdb_status rc = check_csr(m->sparse_offsets, m->n_sparse, "sparse_offsets")) return rc;
-        CDB_REQUIRE((m->sparse_dims && m->sparse_values) || !m->sparse_offsets[m->n_sparse], "null sparse query pairs");
-    }
-    if (host && m->n_tfidf) {
-        if (cdb_status rc = check_csr(m->tfidf_offsets, m->n_tfidf, "tfidf_offsets")) return rc;
-        CDB_REQUIRE(m->tfidf_hashes || !m->tfidf_offsets[m->n_tfidf], "null tf-idf query hashes");
-    }
-    *h = cdb_hybrid_sources{m->dense, m->dense_queries, m->dense_params, m->sparse, m->sparse_offsets, m->sparse_dims,
-                            m->sparse_values, m->sparse_params, m->tfidf, m->tfidf_offsets, m->tfidf_hashes};
-    for (int j = 0; j < 3; ++j)
-        if (n_src[j]) {
-            p->src[p->n] = (Source)j;
-            p->nq[p->n] = n_src[j];
-            p->ld[p->n++] = source_ld((Source)j, top_k);
-        }
-    return plan_sources(h, top_k, p);
-}
-
-cdb_status run_source(const cdb_hybrid_sources *h, Source src, uint32_t nq, uint32_t k3, uint32_t *ids, float *scores,
+cdb_status run_source(const cdb_hybrid_mixed_sources &m, int src, uint32_t nq, uint32_t k3, uint32_t *ids, float *scores,
                       uint32_t *counts, uint8_t *d_err, cudaStream_t s) {
     switch (src) {
-    case SRC_DENSE: {
-        cdb_search_params p = h->dense_params;
+    case HYB_DENSE: {
+        cdb_search_params p = m.dense_params;
         p.k = k3;
-        return cdb_search_batch_device(h->dense, h->dense_queries, nq, &p, ids, scores, counts, d_err, s);
+        return cdb_search_batch_device(m.dense, m.dense_queries, nq, &p, ids, scores, counts, d_err, s);
     }
-    case SRC_SPARSE: {
-        cdb_sparse_search_params p = h->sparse_params;
+    case HYB_SPARSE: {
+        cdb_sparse_search_params p = m.sparse_params;
         p.k = k3;
-        return cdb_sparse_search_batch_device(h->sparse, h->sparse_offsets, h->sparse_dims, h->sparse_values, nq, &p, ids, scores,
+        return cdb_sparse_search_batch_device(m.sparse, m.sparse_offsets, m.sparse_dims, m.sparse_values, nq, &p, ids, scores,
                                               counts, s);
     }
     default:
-        return cdb_tfidf_search_batch_device(h->tfidf, h->tfidf_offsets, h->tfidf_hashes, nq, k3, ids, scores, counts, s);
+        return cdb_tfidf_search_batch_device(m.tfidf, m.tfidf_offsets, m.tfidf_hashes, nq, k3, ids, scores, counts, s);
     }
 }
 
-// The composed search on `s` after make_plan / make_mixed_plan and cudaSetDevice; top_k >= 1, at least one source with
-// queries.  Every source runs once: the first on the caller's stream, the others on side streams forked from it and joined
-// back, so they overlap.  A pair (kinds null) fuses its two lists row by row, the dense search writing d_err itself; a mixed
-// batch (kinds [nq]) fuses each kind present with one launch through its row maps, which also scatters the dense error
-// bytes.  The lists, the maps and the dense error bytes live in one stream-ordered block, freed behind the last fusion.
-cdb_status hybrid_device(const cdb_hybrid_sources *h, const Plan &p, const uint8_t *kinds, uint32_t nq, uint32_t top_k, float k,
-                         uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s) {
-    const uint32_t k3 = 3 * top_k;
+// The search on `s` after check_single and cudaSetDevice; nq >= 1, top_k >= 1, queries in device memory.  Every source
+// with queries runs once: the first on the caller's stream, the others on side streams forked from it and joined back, so
+// they overlap.  Then each kind present is fused with one launch straight into the caller's rows (mixed_fuse).  The lists,
+// the row maps and the dense error bytes live in one stream-ordered block, freed behind the last fusion.
+cdb_status hybrid_device(const cdb_hybrid_mixed_sources &m, uint32_t nq, uint32_t top_k, float k, uint32_t *d_ids,
+                         float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s) {
+    const uint32_t n[3] = {m.n_dense, m.n_sparse, m.n_tfidf};
+    uint32_t ld[3];
+    int src[3], ns = 0;   // the sources with queries, in the order dense, sparse, TF-IDF
+    for (int j = 0; j < 3; ++j) {
+        ld[j] = hyb_list_ld(j, top_k);
+        if (n[j]) src[ns++] = j;
+    }
     std::vector<MixedChunk> chunks;
     std::vector<uint32_t> maps;
-    if (kinds) mixed_chunks(kinds, nq, std::max<uint32_t>(nq, 1), &chunks, &maps);
-    size_t bytes = maps.size() * 4;
-    uint32_t n_dense = 0;
-    for (int j = 0; j < p.n; ++j) {
-        bytes += (size_t)p.nq[j] * ((size_t)p.ld[j] * 8 + 4);
-        if (p.src[j] == SRC_DENSE) n_dense = p.nq[j];
-    }
-    const bool err_scratch = kinds && d_err && n_dense;
-    if (err_scratch) bytes += n_dense;
+    mixed_chunks(m.kinds, nq, ld, SIZE_MAX, &chunks, &maps);   // one chunk
+    const bool err_scratch = !maps.empty() && d_err && n[HYB_DENSE];
+    size_t bytes = maps.size() * 4 + (err_scratch ? n[HYB_DENSE] : 0);
+    for (int j = 0; j < 3; ++j) bytes += (size_t)n[j] * ((size_t)ld[j] * 8 + 4);
     uint8_t *buf = nullptr;
     CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
-    // per list: ids, scores, counts; then the maps and the dense error bytes
+    // per source: ids, scores, counts; then the maps and the dense error bytes
     uint32_t *ids[3], *counts[3];
     float *scores[3];
     uint8_t *at = buf;
-    for (int j = 0; j < p.n; ++j) {
+    for (int j = 0; j < 3; ++j) {
         ids[j] = reinterpret_cast<uint32_t *>(at);
-        scores[j] = reinterpret_cast<float *>(ids[j] + (size_t)p.nq[j] * p.ld[j]);
-        counts[j] = reinterpret_cast<uint32_t *>(scores[j] + (size_t)p.nq[j] * p.ld[j]);
-        at = reinterpret_cast<uint8_t *>(counts[j] + p.nq[j]);
+        scores[j] = reinterpret_cast<float *>(ids[j] + (size_t)n[j] * ld[j]);
+        counts[j] = reinterpret_cast<uint32_t *>(scores[j] + (size_t)n[j] * ld[j]);
+        at = reinterpret_cast<uint8_t *>(counts[j] + n[j]);
     }
-    uint32_t *d_maps = reinterpret_cast<uint32_t *>(at);
-    uint8_t *err_dense = err_scratch ? reinterpret_cast<uint8_t *>(d_maps + maps.size()) : nullptr;
+    uint32_t *d_maps = maps.empty() ? nullptr : reinterpret_cast<uint32_t *>(at);
+    uint8_t *err_dense = err_scratch ? at + maps.size() * 4 : nullptr;
     cudaStream_t side[2] = {nullptr, nullptr};
     cudaEvent_t fork = nullptr, join[2] = {nullptr, nullptr};
     cudaError_t e = cudaSuccess;
-    if (!maps.empty()) e = cudaMemcpyAsync(d_maps, maps.data(), maps.size() * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess && p.n > 1) e = cudaEventCreateWithFlags(&fork, cudaEventDisableTiming);
-    if (e == cudaSuccess && p.n > 1) e = cudaEventRecord(fork, s);
-    for (int j = 1; j < p.n && e == cudaSuccess; ++j) {
-        e = cudaStreamCreateWithFlags(&side[j - 1], cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&join[j - 1], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(side[j - 1], fork, 0);
+    if (d_maps) e = cudaMemcpyAsync(d_maps, maps.data(), maps.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && ns > 1) e = cudaEventCreateWithFlags(&fork, cudaEventDisableTiming);
+    if (e == cudaSuccess && ns > 1) e = cudaEventRecord(fork, s);
+    for (int i = 1; i < ns && e == cudaSuccess; ++i) {
+        e = cudaStreamCreateWithFlags(&side[i - 1], cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&join[i - 1], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(side[i - 1], fork, 0);
     }
     cdb_status rc = CDB_OK;
     if (e != cudaSuccess) {
@@ -346,9 +365,10 @@ cdb_status hybrid_device(const cdb_hybrid_sources *h, const Plan &p, const uint8
         rc = CDB_CUDA_ERROR;
     }
     // the first list on the caller's stream, the others on the side streams: the searches overlap
-    for (int j = 0; j < p.n && !rc; ++j) {
-        uint8_t *err = p.src[j] != SRC_DENSE ? nullptr : kinds ? err_dense : d_err;
-        rc = run_source(h, p.src[j], p.nq[j], k3, ids[j], scores[j], counts[j], err, j ? side[j - 1] : s);
+    for (int i = 0; i < ns && !rc; ++i) {
+        const int j = src[i];
+        uint8_t *err = j != HYB_DENSE ? nullptr : err_dense ? err_dense : d_err;
+        rc = run_source(m, j, n[j], 3 * top_k, ids[j], scores[j], counts[j], err, i ? side[i - 1] : s);
     }
     // joined whatever happened, so that the scratch is freed behind everything that was enqueued
     for (int j = 0; j < 2; ++j) {
@@ -367,12 +387,9 @@ cdb_status hybrid_device(const cdb_hybrid_sources *h, const Plan &p, const uint8
             }
         }
     }
-    if (!rc && !kinds) {
-        const RrfList a{ids[0], counts[0], p.ld[0], 1}, b{ids[1], counts[1], p.ld[1], 1};
-        rc = fuse_launch(a, b, nq, k, 6 * top_k, d_ids, d_scores, d_counts, s);
-    } else if (!rc) {
-        RrfList lists[3] = {};
-        for (int j = 0; j < p.n; ++j) lists[p.src[j]] = RrfList{ids[j], counts[j], p.ld[j], 1};
+    if (!rc) {
+        RrfList lists[3];
+        for (int j = 0; j < 3; ++j) lists[j] = RrfList{ids[j], counts[j], ld[j], 1};
         rc = mixed_fuse(chunks[0], lists, d_maps, err_dense, k, 6 * top_k, d_ids, d_scores, d_counts, d_err, s);
     }
     cudaFreeAsync(buf, s);
@@ -443,131 +460,54 @@ cdb_status cdb_rrf_fuse(int32_t device, const uint32_t *first_ids, const uint32_
     return rc;
 }
 
+// err_flags is written only when a dense source is named
 cdb_status cdb_hybrid_search_batch_device(const cdb_hybrid_sources *sources, uint32_t nq, uint32_t top_k, float fusion_constant_k,
                                           uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err_flags, void *stream) {
-    CDB_REQUIRE(!nq || !top_k || (d_ids && d_scores && d_counts), "null output");
-    Plan p;
-    cdb_status rc = make_plan(sources, nq, top_k, &p);
-    if (rc) return rc;
-    CDB_CUDA_TRY(cudaSetDevice(p.device));
-    if (!nq) return CDB_OK;
-    cudaStream_t s = stream ? (cudaStream_t)stream : cudaStreamLegacy;
-    if (!top_k) {
-        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
-        return CDB_OK;
-    }
-    return hybrid_device(sources, p, nullptr, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, d_err_flags, s);
+    std::vector<uint8_t> kinds;
+    cdb_hybrid_mixed_sources m;
+    if (cdb_status rc = pair_as_batch(sources, nq, &kinds, &m)) return rc;
+    return cdb_hybrid_search_batch_mixed_device(&m, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts,
+                                                sources->dense ? d_err_flags : nullptr, stream);
 }
 
 cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t nq, uint32_t top_k, float fusion_constant_k,
                                    uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
-    CDB_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
-    Plan p;
-    cdb_status rc = make_plan(sources, nq, top_k, &p);
-    if (rc) return rc;
-    const cdb_hybrid_sources &h = *sources;
-    uint64_t sp_pairs = 0, tf_hashes = 0;
-    if (nq && h.sparse) {
-        if ((rc = check_csr(h.sparse_offsets, nq, "sparse_offsets"))) return rc;
-        sp_pairs = h.sparse_offsets[nq];
-        CDB_REQUIRE((h.sparse_dims && h.sparse_values) || !sp_pairs, "null sparse query pairs");
-    }
-    if (nq && h.tfidf) {
-        if ((rc = check_csr(h.tfidf_offsets, nq, "tfidf_offsets"))) return rc;
-        tf_hashes = h.tfidf_offsets[nq];
-        CDB_REQUIRE(h.tfidf_hashes || !tf_hashes, "null tf-idf query hashes");
-    }
-    CDB_CUDA_TRY(cudaSetDevice(p.device));
-    if (!nq) return CDB_OK;
-    if (!top_k) {
-        memset(out_counts, 0, (size_t)nq * 4);
-        return CDB_OK;
-    }
-    StreamGuard sg;
-    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-    cudaStream_t s = sg.s;
-    // one buffer: dense queries, sparse CSR, tf-idf CSR, then the outputs (8-byte parts first)
-    const size_t dq = h.dense ? (size_t)nq * index_dim(h.dense) : 0;
-    const size_t ld_out = 6 * (size_t)top_k, no = (size_t)nq * ld_out;
-    const size_t n_sp_off = h.sparse ? nq + 1 : 0, n_tf_off = h.tfidf ? nq + 1 : 0;
-    const size_t bytes = (n_sp_off + n_tf_off) * 8 + (dq + 2 * sp_pairs + tf_hashes + 2 * no + nq) * 4 + nq;
-    uint8_t *buf = nullptr;
-    CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
-    cdb_hybrid_sources d = h;
-    uint64_t *sp_off = reinterpret_cast<uint64_t *>(buf), *tf_off = sp_off + n_sp_off;
-    float *dense_q = reinterpret_cast<float *>(tf_off + n_tf_off);
-    uint32_t *sp_dims = reinterpret_cast<uint32_t *>(dense_q + dq);
-    float *sp_vals = reinterpret_cast<float *>(sp_dims + sp_pairs);
-    uint32_t *tf_h = reinterpret_cast<uint32_t *>(sp_vals + sp_pairs);
-    uint32_t *d_ids = tf_h + tf_hashes;
-    float *d_scores = reinterpret_cast<float *>(d_ids + no);
-    uint32_t *d_counts = reinterpret_cast<uint32_t *>(d_scores + no);
-    uint8_t *d_err = reinterpret_cast<uint8_t *>(d_counts + nq);
-    cudaError_t e = cudaSuccess;
-    if (h.dense) {
-        e = cudaMemcpyAsync(dense_q, h.dense_queries, dq * 4, cudaMemcpyHostToDevice, s);
-        d.dense_queries = dense_q;
-    }
-    if (h.sparse) {
-        if (e == cudaSuccess) e = cudaMemcpyAsync(sp_off, h.sparse_offsets, n_sp_off * 8, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && sp_pairs) e = cudaMemcpyAsync(sp_dims, h.sparse_dims, sp_pairs * 4, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && sp_pairs) e = cudaMemcpyAsync(sp_vals, h.sparse_values, sp_pairs * 4, cudaMemcpyHostToDevice, s);
-        d.sparse_offsets = sp_off;
-        d.sparse_dims = sp_dims;
-        d.sparse_values = sp_vals;
-    }
-    if (h.tfidf) {
-        if (e == cudaSuccess) e = cudaMemcpyAsync(tf_off, h.tfidf_offsets, n_tf_off * 8, cudaMemcpyHostToDevice, s);
-        if (e == cudaSuccess && tf_hashes) e = cudaMemcpyAsync(tf_h, h.tfidf_hashes, tf_hashes * 4, cudaMemcpyHostToDevice, s);
-        d.tfidf_offsets = tf_off;
-        d.tfidf_hashes = tf_h;
-    }
-    if (e != cudaSuccess) { set_error(std::string("hybrid search: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
-    if (!rc) rc = hybrid_device(&d, p, nullptr, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, d_err, s);
-    if (!rc) {
-        e = cudaMemcpyAsync(out_ids, d_ids, no * 4, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, d_scores, no * 4, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_counts, d_counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && err_flags && h.dense) e = cudaMemcpyAsync(err_flags, d_err, nq, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) { set_error(std::string("hybrid search: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
-    }
-    cudaFreeAsync(buf, s);
-    return rc;
+    std::vector<uint8_t> kinds;
+    cdb_hybrid_mixed_sources m;
+    if (cdb_status rc = pair_as_batch(sources, nq, &kinds, &m)) return rc;
+    return cdb_hybrid_search_batch_mixed(&m, nq, top_k, fusion_constant_k, out_ids, out_scores, out_counts,
+                                         sources->dense ? err_flags : nullptr);
 }
 
 cdb_status cdb_hybrid_search_batch_mixed_device(const cdb_hybrid_mixed_sources *sources, uint32_t nq, uint32_t top_k,
                                                 float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
                                                 uint8_t *d_err_flags, void *stream) {
     CDB_REQUIRE(!nq || (d_counts && (!top_k || (d_ids && d_scores))), "null output");
-    Plan p;
-    cdb_hybrid_sources h;
-    cdb_status rc = make_mixed_plan(sources, nq, top_k, false, &h, &p);
+    int device = -1;
+    cdb_status rc = check_single(sources, nq, top_k, false, &device);
     if (rc || !nq) return rc;
-    CDB_CUDA_TRY(cudaSetDevice(p.device));
+    CDB_CUDA_TRY(cudaSetDevice(device));
     cudaStream_t s = stream ? (cudaStream_t)stream : cudaStreamLegacy;
     if (!top_k) {
         CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
         return CDB_OK;
     }
-    return hybrid_device(&h, p, sources->kinds, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, d_err_flags, s);
+    return hybrid_device(*sources, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, d_err_flags, s);
 }
 
 cdb_status cdb_hybrid_search_batch_mixed(const cdb_hybrid_mixed_sources *sources, uint32_t nq, uint32_t top_k, float fusion_constant_k,
                                          uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags) {
     CDB_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
-    Plan p;
-    cdb_hybrid_sources h;
-    cdb_status rc = make_mixed_plan(sources, nq, top_k, true, &h, &p);
-    if (rc) return rc;
-    const cdb_hybrid_mixed_sources &m = *sources;
-    const uint64_t sp_pairs = m.n_sparse ? m.sparse_offsets[m.n_sparse] : 0, tf_hashes = m.n_tfidf ? m.tfidf_offsets[m.n_tfidf] : 0;
-    if (!nq) return CDB_OK;
+    int device = -1;
+    cdb_status rc = check_single(sources, nq, top_k, true, &device);
+    if (rc || !nq) return rc;
     if (!top_k) {
         memset(out_counts, 0, (size_t)nq * 4);
         return CDB_OK;
     }
-    CDB_CUDA_TRY(cudaSetDevice(p.device));
+    const cdb_hybrid_mixed_sources &m = *sources;
+    const uint64_t sp_pairs = m.n_sparse ? m.sparse_offsets[m.n_sparse] : 0, tf_hashes = m.n_tfidf ? m.tfidf_offsets[m.n_tfidf] : 0;
+    CDB_CUDA_TRY(cudaSetDevice(device));
     StreamGuard sg;
     CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
     cudaStream_t s = sg.s;
@@ -594,14 +534,15 @@ cdb_status cdb_hybrid_search_batch_mixed(const cdb_hybrid_mixed_sources *sources
     if (e == cudaSuccess && sp_pairs) e = cudaMemcpyAsync(sp_vals, m.sparse_values, sp_pairs * 4, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess && n_tf_off) e = cudaMemcpyAsync(tf_off, m.tfidf_offsets, n_tf_off * 8, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess && tf_hashes) e = cudaMemcpyAsync(tf_h, m.tfidf_hashes, tf_hashes * 4, cudaMemcpyHostToDevice, s);
-    h.dense_queries = dense_q;
-    h.sparse_offsets = sp_off;
-    h.sparse_dims = sp_dims;
-    h.sparse_values = sp_vals;
-    h.tfidf_offsets = tf_off;
-    h.tfidf_hashes = tf_h;
+    cdb_hybrid_mixed_sources d = m;
+    d.dense_queries = dense_q;
+    d.sparse_offsets = sp_off;
+    d.sparse_dims = sp_dims;
+    d.sparse_values = sp_vals;
+    d.tfidf_offsets = tf_off;
+    d.tfidf_hashes = tf_h;
     if (e != cudaSuccess) { set_error(std::string("hybrid search: ") + cudaGetErrorString(e)); rc = CDB_CUDA_ERROR; }
-    if (!rc) rc = hybrid_device(&h, p, m.kinds, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, err_flags ? d_err : nullptr, s);
+    if (!rc) rc = hybrid_device(d, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, err_flags ? d_err : nullptr, s);
     if (!rc) {
         e = cudaMemcpyAsync(out_ids, d_ids, no * 4, cudaMemcpyDeviceToHost, s);
         if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, d_scores, no * 4, cudaMemcpyDeviceToHost, s);

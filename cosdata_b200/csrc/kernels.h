@@ -1,5 +1,6 @@
 // kernels.h -- internal launch wrappers shared between the .cu files.
 #pragma once
+#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -76,41 +77,54 @@ uint32_t index_dim(const cdb_index *ix);
 // graph metadata attached (results carry replica ids); read under the handle's shared lock
 bool index_has_graph_metadata(cdb_index *ix);
 
-// ---- hybrid.cu: the fusion of two ranked lists per query (cdb_rrf_fuse's kernel), shared with the shard group's hybrid search
+// ---- hybrid.cu: the fusion of two ranked lists per query (cdb_rrf_fuse's kernel), and the request check, chunks and
+// fusion of a hybrid batch, shared with the shard group's hybrid search
 constexpr uint32_t HYB_MAX_TOP_K = 341;   // 3 * top_k <= 1024, the dense and sparse searches' k limit
+enum HybSource { HYB_DENSE = 0, HYB_SPARSE = 1, HYB_TFIDF = 2 };
+// columns of a source's intermediate list: 3 * top_k, TF-IDF at most its 512 buckets
+inline uint32_t hyb_list_ld(int src, uint32_t top_k) { return std::min(3 * top_k, src == HYB_TFIDF ? 512u : 3 * top_k); }
 struct RrfList {
     const uint32_t *ids;      // [B][ld]
     const uint32_t *counts;   // [B]
     uint32_t ld, stride;
     const uint32_t *rows = nullptr;   // device, [n]: the list row fused into row i (null: row i)
 };
-// a mixed batch's fusion: fused row i lands in output row rows[i] (null: row i); with err, err[rows[i]] = err_in[first
+// where a fusion writes: fused row i lands in output row rows[i] (null: row i); with err, err[rows[i]] = err_in[first
 // list's row] (null err_in: 0)
 struct RrfRows {
     const uint32_t *rows = nullptr;
     const uint8_t *err_in = nullptr;
     uint8_t *err = nullptr;
 };
-cdb_status check_fuse_args(uint32_t ld_a, uint32_t ld_b, uint32_t nq, uint32_t ld_out, const void *ids_a, const void *cnt_a,
-                           const void *ids_b, const void *cnt_b, const void *out_ids, const void *out_scores, const void *out_counts);
 cdb_status fuse_launch(const RrfList &a, const RrfList &b, uint32_t nq, float k, uint32_t ld_out, uint32_t *d_ids, float *d_scores,
                        uint32_t *d_counts, cudaStream_t s, const RrfRows &o = RrfRows{});
 
-// a mixed hybrid batch (cdb_hybrid_search_batch_mixed*): each query's kind names two of the sources dense (0), sparse (1)
-// and TF-IDF (2), first list first; a source's batch holds the queries whose kind names it, in request order
+// a hybrid batch (cdb_hybrid_search_batch*): each query's kind names two of the sources dense (0), sparse (1) and TF-IDF
+// (2), first list first; a source's batch holds the queries whose kind names it, in request order.  A two-source call is
+// a batch of one kind.
 constexpr int HYB_KIND_SRC[3][2] = {{0, 1}, {0, 2}, {1, 2}};
+// "exactly two sources", then the kinds of a two-source call: nq copies of its pair's kind
+cdb_status hybrid_pair_kinds(bool dense, bool sparse, bool tfidf, uint32_t nq, std::vector<uint8_t> *kinds);
+// The refusals of a request that read no handle and no group, in this order: null sources; top_k > 341; null kinds, a
+// kind above 2 or counts that disagree with the kinds; CDB_SEARCH_ALL_CANDIDATES with dense queries; a null handle (single
+// index) or null queries of a source with queries; the sparse re-rank bound; malformed query CSR (host: host arrays).
+cdb_status check_hybrid_request(const cdb_hybrid_mixed_sources *m, uint32_t nq, uint32_t top_k, bool host);
+cdb_status check_hybrid_request(const cdb_hybrid_group_mixed_sources *h, uint32_t nq, uint32_t top_k, bool host);
 // request positions [q0, q1): rows [row0[j], row0[j] + rows[j]) of source j's batch, n[c] queries of kind c, whose maps
 // sit at map[c] in the map array: output rows (from q0), first-list rows, second-list rows (from each source's row0)
 struct MixedChunk {
     uint32_t q0, q1, row0[3], rows[3], n[3];
     size_t map[3];
 };
-// kinds non-null when nq > 0, every kind <= 2, and the per-source counts those kinds give
-cdb_status check_kinds(const uint8_t *kinds, uint32_t nq, const uint32_t n_src[3]);
-// chunks of at most `chunk` request positions, and their maps (3 * nq u32)
-void mixed_chunks(const uint8_t *kinds, uint32_t nq, uint32_t chunk, std::vector<MixedChunk> *chunks, std::vector<uint32_t> *maps);
+// Chunks of request positions (nq >= 1) whose lists, ld[j] columns for source j, fit in `budget` bytes, and their maps.
+// A batch of one kind gets no maps: query q is row q of both its sources' batches, so the dense search writes its error
+// bytes in place, and a position costs two lists and two counts.  Otherwise the maps take 3 * nq u32 and a position costs
+// the widest kind present and the dense error byte.
+void mixed_chunks(const uint8_t *kinds, uint32_t nq, const uint32_t ld[3], size_t budget, std::vector<MixedChunk> *chunks,
+                  std::vector<uint32_t> *maps);
 // one fusion launch per kind present in the chunk: lists[j] holds source j's rows of the chunk (rows unset), d_maps the map
-// array on the device, d_err_dense the dense search's error bytes of the chunk; the outputs start at the chunk's q0
+// array on the device (null: no maps, rows in place), d_err_dense the dense search's error bytes of the chunk when there
+// are maps; the outputs start at the chunk's q0, and d_err gets 0 at SPARSE_TFIDF queries
 cdb_status mixed_fuse(const MixedChunk &c, const RrfList lists[3], const uint32_t *d_maps, const uint8_t *d_err_dense, float k,
                       uint32_t ld_out, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t s);
 

@@ -1179,11 +1179,8 @@ cdb_status cdb_tfidf_search_batch_sharded_device(cdb_shard_group *g, const uint6
 
 // ---------------------------------------------------------------- hybrid search over the group (DESIGN.md section 8h)
 
-enum HybSource { HYB_DENSE = 0, HYB_SPARSE = 1, HYB_TFIDF = 2 };
-
 struct HybPlan {
-    bool use[3] = {false, false, false};   // the sources searched, always in the order dense, sparse, TF-IDF
-    uint32_t nq[3] = {0, 0, 0};            // each searched source's queries
+    uint32_t nq[3] = {0, 0, 0};            // each source's queries (0: not searched), in the order dense, sparse, TF-IDF
     uint32_t ld[3] = {0, 0, 0};            // columns of each source's intermediate list
     cdb_search_params dense;               // at k = 3 * top_k
     cdb_sparse_search_params sparse;
@@ -1191,73 +1188,21 @@ struct HybPlan {
     bool md = false;                       // the dense shards have graph metadata: the filtered path, no filter
 };
 
-// the refusals after the source list: the sparse rerank bound, then the sub-searches' own parameter checks at k = 3 * top_k
-static cdb_status hyb_params(const cdb_search_params &dense, const cdb_sparse_search_params &sparse, uint32_t top_k, HybPlan *p) {
-    const uint32_t k3 = 3 * top_k;
-    for (int j = 0; j < 3; ++j) p->ld[j] = j == HYB_TFIDF ? std::min(k3, 512u) : k3;
-    if (p->use[HYB_SPARSE] && sparse.rerank)
-        CDB_REQUIRE(sparse.reranking_factor >= 1 && (uint64_t)k3 * sparse.reranking_factor <= 5120,
-                    "3 * top_k * reranking_factor must be in 1..5120");
-    p->dense = dense;
-    p->dense.k = k3;
-    p->sparse = sparse;
-    p->sparse.k = k3;
-    if (top_k && p->use[HYB_DENSE])
-        if (cdb_status rc = check_search_k(&p->dense)) return rc;
-    if (top_k && p->use[HYB_SPARSE])
-        if (cdb_status rc = sparse_check_params(&p->sparse, &p->m)) return rc;
-    return CDB_OK;
-}
-
-// the refusals that need no group, in the order of cdb_hybrid_search_batch's (make_plan in hybrid.cu), then hyb_params
-static cdb_status hyb_plan(const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k, HybPlan *p) {
-    CDB_REQUIRE(h, "null sources");
-    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
-    CDB_REQUIRE((h->use_dense != 0) + (h->use_sparse != 0) + (h->use_tfidf != 0) == 2, "a hybrid search takes exactly two sources");
-    CDB_REQUIRE(!h->use_dense || !(h->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
-                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
-    p->use[HYB_DENSE] = h->use_dense;
-    p->use[HYB_SPARSE] = h->use_sparse;
-    p->use[HYB_TFIDF] = h->use_tfidf;
-    for (int j = 0; j < 3; ++j) p->nq[j] = p->use[j] ? nq : 0;
-    CDB_REQUIRE(!h->use_dense || h->dense_queries || !nq, "null dense queries");
-    CDB_REQUIRE(!h->use_sparse || h->sparse_offsets || !nq, "null sparse query offsets");
-    CDB_REQUIRE(!h->use_tfidf || h->tfidf_offsets || !nq, "null tf-idf query offsets");
-    return hyb_params(h->dense_params, h->sparse_params, top_k, p);
-}
-
-// a mixed batch's refusals that need no group, in the order of cdb_hybrid_search_batch_mixed's: the sources searched are
-// those with queries
-static cdb_status hyb_mixed_plan(const cdb_hybrid_group_mixed_sources *h, uint32_t nq, uint32_t top_k, HybPlan *p) {
-    CDB_REQUIRE(h, "null sources");
-    CDB_REQUIRE(top_k <= HYB_MAX_TOP_K, "top_k must be <= 341 (each sub-search takes 3 * top_k <= 1024)");
-    const uint32_t n_src[3] = {h->n_dense, h->n_sparse, h->n_tfidf};
-    if (cdb_status rc = check_kinds(h->kinds, nq, n_src)) return rc;
-    CDB_REQUIRE(!h->n_dense || !(h->dense_params.flags & CDB_SEARCH_ALL_CANDIDATES),
-                "CDB_SEARCH_ALL_CANDIDATES (top_k None) has no hybrid form: the dense sub-search takes k = 3 * top_k");
+// after check_hybrid_request: the plan, and the sub-searches' own parameter checks at k = 3 * top_k
+static cdb_status hyb_params(const cdb_hybrid_group_mixed_sources &h, uint32_t top_k, HybPlan *p) {
+    const uint32_t n[3] = {h.n_dense, h.n_sparse, h.n_tfidf};
     for (int j = 0; j < 3; ++j) {
-        p->use[j] = n_src[j] != 0;
-        p->nq[j] = n_src[j];
+        p->nq[j] = n[j];
+        p->ld[j] = hyb_list_ld(j, top_k);
     }
-    CDB_REQUIRE(!h->n_dense || h->dense_queries, "null dense queries");
-    CDB_REQUIRE(!h->n_sparse || h->sparse_offsets, "null sparse query offsets");
-    CDB_REQUIRE(!h->n_tfidf || h->tfidf_offsets, "null tf-idf query offsets");
-    return hyb_params(h->dense_params, h->sparse_params, top_k, p);
-}
-
-// the host form's query CSRs, before the group is locked: n_sp / n_tf queries of each searched text source
-static cdb_status hyb_check_csr(const uint64_t *sp_off, const uint32_t *sp_dims, const float *sp_vals, uint32_t n_sp,
-                                const uint64_t *tf_off, const uint32_t *tf_hashes, uint32_t n_tf) {
-    cdb_status rc;
-    if (n_sp) {
-        if ((rc = check_csr(sp_off, n_sp, "sparse_offsets"))) return rc;
-        CDB_REQUIRE((sp_dims && sp_vals) || !sp_off[n_sp], "null sparse query pairs");
-    }
-    if (n_tf) {
-        if ((rc = check_csr(tf_off, n_tf, "tfidf_offsets"))) return rc;
-        CDB_REQUIRE(tf_hashes || !tf_off[n_tf], "null tf-idf query hashes");
-        CDB_REQUIRE(tf_off[n_tf] < (1ull << 31), "a batch of 2^31 query terms or more");
-    }
+    p->dense = h.dense_params;
+    p->dense.k = 3 * top_k;
+    p->sparse = h.sparse_params;
+    p->sparse.k = 3 * top_k;
+    if (top_k && p->nq[HYB_DENSE])
+        if (cdb_status rc = check_search_k(&p->dense)) return rc;
+    if (top_k && p->nq[HYB_SPARSE])
+        if (cdb_status rc = sparse_check_params(&p->sparse, &p->m)) return rc;
     return CDB_OK;
 }
 
@@ -1266,11 +1211,11 @@ static cdb_status hyb_check_csr(const uint64_t *sp_off, const uint32_t *sp_dims,
 static cdb_status hyb_group_check(const cdb_shard_group *g, HybPlan *p) {
     const size_t nl = g->dev.size();
     for (size_t i = 0; i < nl; ++i) {
-        CDB_REQUIRE(!p->use[HYB_DENSE] || g->shard[i], "a group slot has no shard attached");
-        CDB_REQUIRE(!p->use[HYB_SPARSE] || g->sparse[i], "a group slot has no sparse shard attached");
-        CDB_REQUIRE(!p->use[HYB_TFIDF] || g->tfidf[i], "a group slot has no tf-idf shard attached");
+        CDB_REQUIRE(!p->nq[HYB_DENSE] || g->shard[i], "a group slot has no shard attached");
+        CDB_REQUIRE(!p->nq[HYB_SPARSE] || g->sparse[i], "a group slot has no sparse shard attached");
+        CDB_REQUIRE(!p->nq[HYB_TFIDF] || g->tfidf[i], "a group slot has no tf-idf shard attached");
     }
-    if (!p->use[HYB_DENSE]) return CDB_OK;
+    if (!p->nq[HYB_DENSE]) return CDB_OK;
     size_t with_md = 0;
     for (size_t i = 0; i < nl; ++i) with_md += index_md_dims(g->shard[i]) != 0;
     CDB_REQUIRE(with_md == 0 || with_md == nl,
@@ -1283,57 +1228,30 @@ static cdb_status hyb_group_check(const cdb_shard_group *g, HybPlan *p) {
     return merge_check(g, &p->dense);
 }
 
-// The sub-searches and the fusion, per chunk of request positions, under g->mu and every searched text shard's reader lock.
-// dq / sq / tq: each local slot's dense queries, sparse CSR and TF-IDF CSR on its device (nqh: the TF-IDF batch's term
-// count).  A pair (kinds null) searches both sources over the chunk's queries and fuses them row by row, the dense search
-// writing d_err; a mixed batch (kinds [nq], host) searches each source over its range of the chunk and fuses each kind
-// present through its row maps, which scatter the dense error bytes.  A TF-IDF source's idf step runs once, over its whole
-// batch, before the chunks.  The sub-searches run one after the other in the order dense, sparse, TF-IDF, each on the
-// streams its public entry point uses, so every rank issues the same collectives in the same order, and a source with no
-// queries in a chunk issues none; each one's merged list lands in this call's scratch on slot 0, where the fusion writes
-// rows q0.. of the output.  Nothing here waits for the device.
+// The sub-searches and the fusion, per chunk of request positions (mixed_chunks), under g->mu and every searched text
+// shard's reader lock.  dq / sq / tq: each local slot's dense queries, sparse CSR and TF-IDF CSR on its device (nqh: the
+// TF-IDF batch's term count).  A TF-IDF source's idf step runs once, over its whole batch, before the chunks.  In each
+// chunk every source with queries there is searched over its range of them, one after the other in the order dense,
+// sparse, TF-IDF, each on the streams its public entry point uses, so every rank issues the same collectives in the same
+// order; each one's merged list lands in this call's scratch on slot 0, where each kind present is fused into rows q0.. of
+// the output (mixed_fuse).  Nothing here waits for the device.
 static cdb_status hybrid_group_run(cdb_shard_group *g, const HybPlan &p, const uint8_t *kinds, uint32_t nq, uint32_t top_k,
                                    float fusion_k, uint32_t dense_id_stride, const std::vector<const float *> &dq,
                                    const std::vector<SparseQueries> &sq, const std::vector<TfQueries> &tq, uint64_t nqh, uint32_t *d_ids,
                                    float *d_scores, uint32_t *d_counts, uint8_t *d_err, cudaStream_t out_stream) {
     const size_t nl = g->dev.size();
     const uint32_t k3 = 3 * top_k, ld_out = 6 * top_k;
-    // bytes of one request position: ids and scores of its two lists, two counts (a mixed batch: the widest kind present,
-    // and the dense error byte)
-    size_t per_q = 0;
-    if (!kinds) {
-        for (int j = 0; j < 3; ++j) per_q += p.use[j] ? (size_t)p.ld[j] * 8 + 4 : 0;
-    } else {
-        bool present[3] = {false, false, false};
-        for (uint32_t q = 0; q < nq; ++q) present[kinds[q]] = true;
-        for (int kd = 0; kd < 3; ++kd)
-            if (present[kd]) per_q = std::max(per_q, ((size_t)p.ld[HYB_KIND_SRC[kd][0]] + p.ld[HYB_KIND_SRC[kd][1]]) * 8 + 9);
-    }
-    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nq, GROUP_GATHER_BUDGET / per_q));
     std::vector<MixedChunk> chunks;
     std::vector<uint32_t> maps;
-    if (kinds) {
-        mixed_chunks(kinds, nq, chunk, &chunks, &maps);
-    } else {
-        for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
-            MixedChunk c{};
-            c.q0 = q0;
-            c.q1 = std::min(nq, q0 + chunk);
-            for (int j = 0; j < 3; ++j) {
-                c.row0[j] = q0;
-                c.rows[j] = p.use[j] ? c.q1 - q0 : 0;
-            }
-            chunks.push_back(c);
-        }
-    }
+    mixed_chunks(kinds, nq, p.ld, GROUP_GATHER_BUDGET, &chunks, &maps);
     uint32_t rmax[3] = {0, 0, 0};
     for (const MixedChunk &c : chunks)
         for (int j = 0; j < 3; ++j) rmax[j] = std::max(rmax[j], c.rows[j]);
     // per source: ids, scores, counts of a chunk's rows; then the maps and the dense error bytes
-    const bool err_scratch = kinds && d_err && rmax[HYB_DENSE];
+    const bool err_scratch = !maps.empty() && d_err && rmax[HYB_DENSE];
     size_t bytes = maps.size() * 4 + (err_scratch ? rmax[HYB_DENSE] : 0);
     for (int j = 0; j < 3; ++j) bytes += (size_t)rmax[j] * ((size_t)p.ld[j] * 8 + 4);
-    const uint32_t dim = p.use[HYB_DENSE] ? index_dim(g->shard[0]) : 0;
+    const uint32_t dim = p.nq[HYB_DENSE] ? index_dim(g->shard[0]) : 0;
     CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
     const cudaStream_t s0 = slot_stream(g, 0, out_stream);
     uint8_t *buf = nullptr;
@@ -1347,16 +1265,16 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const HybPlan &p, const u
         counts[j] = reinterpret_cast<uint32_t *>(scores[j] + (size_t)rmax[j] * p.ld[j]);
         at = reinterpret_cast<uint8_t *>(counts[j] + rmax[j]);
     }
-    uint32_t *d_maps = reinterpret_cast<uint32_t *>(at);
-    uint8_t *err_dense = err_scratch ? reinterpret_cast<uint8_t *>(d_maps + maps.size()) : nullptr;
+    uint32_t *d_maps = maps.empty() ? nullptr : reinterpret_cast<uint32_t *>(at);
+    uint8_t *err_dense = err_scratch ? at + maps.size() * 4 : nullptr;
     cdb_status rc = CDB_OK;
-    if (!maps.empty() && cudaMemcpyAsync(d_maps, maps.data(), maps.size() * 4, cudaMemcpyHostToDevice, s0) != cudaSuccess) {
+    if (d_maps && cudaMemcpyAsync(d_maps, maps.data(), maps.size() * 4, cudaMemcpyHostToDevice, s0) != cudaSuccess) {
         set_error("hybrid search: copying the row maps failed");
         rc = CDB_CUDA_ERROR;
     }
     const std::vector<ShardFilters> no_filters(nl, ShardFilters{nullptr, nullptr, 0, nullptr});
     std::vector<float *> idf;
-    if (!rc && p.use[HYB_TFIDF]) rc = tfidf_idf_enqueue(g, tq, p.nq[HYB_TFIDF], nqh, &idf, out_stream);
+    if (!rc && p.nq[HYB_TFIDF]) rc = tfidf_idf_enqueue(g, tq, p.nq[HYB_TFIDF], nqh, &idf, out_stream);
     bool first = true;
     for (size_t ci = 0; ci < chunks.size() && !rc; ++ci) {
         const MixedChunk &c = chunks[ci];
@@ -1369,7 +1287,7 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const HybPlan &p, const u
             if (j == HYB_DENSE) {
                 std::vector<const float *> q(nl);
                 for (size_t i = 0; i < nl; ++i) q[i] = dq[i] + (size_t)r0 * dim;
-                uint8_t *err = kinds ? err_dense : d_err ? d_err + c.q0 : nullptr;
+                uint8_t *err = err_dense ? err_dense : d_err ? d_err + c.q0 : nullptr;
                 rc = sharded_enqueue(g, n, &p.dense, q, p.md ? &no_filters : nullptr, ids[j], scores[j], counts[j], err, out_stream);
             } else if (j == HYB_SPARSE) {
                 std::vector<SparseQueries> q(nl);
@@ -1383,17 +1301,8 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const HybPlan &p, const u
         CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
         RrfList lists[3];
         for (int j = 0; j < 3; ++j) lists[j] = RrfList{ids[j], counts[j], p.ld[j], j == HYB_DENSE ? dense_id_stride : 1u};
-        uint32_t *o_ids = d_ids + (size_t)c.q0 * ld_out, *o_counts = d_counts + c.q0;
-        float *o_scores = d_scores + (size_t)c.q0 * ld_out;
-        if (kinds) {
-            rc = mixed_fuse(c, lists, d_maps, err_dense, fusion_k, ld_out, o_ids, o_scores, o_counts, d_err ? d_err + c.q0 : nullptr, s0);
-        } else {
-            const int f = p.use[HYB_DENSE] ? HYB_DENSE : HYB_SPARSE, s = p.use[HYB_TFIDF] ? HYB_TFIDF : HYB_SPARSE;
-            const RrfList &a = lists[f], &b = lists[s];
-            const uint32_t n = c.q1 - c.q0;
-            if (!(rc = check_fuse_args(a.ld, b.ld, n, ld_out, a.ids, a.counts, b.ids, b.counts, o_ids, o_scores, o_counts)))
-                rc = fuse_launch(a, b, n, fusion_k, ld_out, o_ids, o_scores, o_counts, s0);
-        }
+        rc = mixed_fuse(c, lists, d_maps, err_dense, fusion_k, ld_out, d_ids + (size_t)c.q0 * ld_out, d_scores + (size_t)c.q0 * ld_out,
+                        d_counts + c.q0, d_err ? d_err + c.q0 : nullptr, s0);
     }
     // freed behind everything enqueued on slot 0's stream, which every slot's last work joined (collective or loopback copy)
     tfidf_idf_free(g, idf, out_stream);
@@ -1402,77 +1311,88 @@ static cdb_status hybrid_group_run(cdb_shard_group *g, const HybPlan &p, const u
     return rc;
 }
 
+// a two-source call as a batch of one kind: both named sources take every query
+static cdb_status hyb_pair_batch(const cdb_hybrid_group_sources *h, uint32_t nq, std::vector<uint8_t> *kinds,
+                                 cdb_hybrid_group_mixed_sources *m) {
+    CDB_REQUIRE(h, "null sources");
+    if (cdb_status rc = hybrid_pair_kinds(h->use_dense, h->use_sparse, h->use_tfidf, nq, kinds)) return rc;
+    *m = cdb_hybrid_group_mixed_sources{kinds->data(), h->use_dense ? nq : 0, h->use_sparse ? nq : 0, h->use_tfidf ? nq : 0,
+                                        h->dense_queries, h->dense_params, h->dense_id_stride, h->sparse_offsets, h->sparse_dims,
+                                        h->sparse_values, h->sparse_params, h->tfidf_offsets, h->tfidf_hashes, 0};
+    return CDB_OK;
+}
+
+// the device form's refusals that read nothing of the group
+static cdb_status hyb_device_request(const cdb_shard_group *g, const cdb_hybrid_group_mixed_sources *h, uint32_t nq, uint32_t top_k,
+                                     const void *d_ids, const void *d_scores, const void *d_counts, HybPlan *p) {
+    CDB_REQUIRE(!nq || (d_counts && (!top_k || (d_ids && d_scores))), "null output");
+    CDB_REQUIRE(g, "null group");
+    cdb_status rc = check_hybrid_request(h, nq, top_k, false);
+    if (rc || (rc = hyb_params(*h, top_k, p))) return rc;
+    CDB_REQUIRE(!h->n_tfidf || h->tfidf_hashes || !h->n_tfidf_hashes, "null tf-idf query hashes");
+    CDB_REQUIRE(h->n_tfidf_hashes < (1ull << 31), "a batch of 2^31 query terms or more");
+    return CDB_OK;
+}
+
+// the device form after hyb_device_request: the group's work follows what the caller's stream held, and the caller's later
+// work follows it
+static cdb_status hyb_device_run(cdb_shard_group *g, const cdb_hybrid_group_mixed_sources &h, HybPlan *p, uint32_t nq, uint32_t top_k,
+                                 float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, uint8_t *d_err_flags,
+                                 void *stream) {
+    CDB_REQUIRE(g->dev.size() == 1, "the device form serves groups of one local slot (cdb_shard_group_create_rank, or one device)");
+    std::lock_guard<std::mutex> lock(g->mu);
+    cdb_status rc = hyb_group_check(g, p);
+    if (rc || !nq) return rc;
+    const cudaStream_t out = (cudaStream_t)stream, s = slot_stream(g, 0, out);
+    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+    if (s != out) {
+        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], out));
+        CDB_CUDA_TRY(cudaStreamWaitEvent(s, g->ev[0], 0));
+    }
+    if (!top_k) {
+        rc = cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s) == cudaSuccess ? CDB_OK : CDB_CUDA_ERROR;
+        if (rc) set_error("hybrid search: cudaMemsetAsync failed");
+    } else {
+        std::vector<std::shared_lock<std::shared_mutex>> locks;
+        if (p->nq[HYB_SPARSE]) locks.emplace_back(sparse_index_mutex(g->sparse[0]));
+        if (p->nq[HYB_TFIDF]) locks.emplace_back(tfidf_index_mutex(g->tfidf[0]));
+        rc = hybrid_group_run(g, *p, h.kinds, nq, top_k, fusion_constant_k, h.dense_id_stride, {h.dense_queries},
+                              {SparseQueries{h.sparse_offsets, h.sparse_dims, h.sparse_values}},
+                              {TfQueries{h.tfidf_offsets, h.tfidf_hashes}}, h.n_tfidf_hashes, d_ids, d_scores, d_counts, d_err_flags, out);
+    }
+    if (s != out) {
+        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
+        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], s));
+        CDB_CUDA_TRY(cudaStreamWaitEvent(out, g->ev[0], 0));
+    }
+    return rc;
+}
+
 cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *g, const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k,
                                            float fusion_constant_k, uint32_t *out_ids, float *out_scores, uint32_t *out_counts,
                                            uint8_t *err_flags) {
-    CDB_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
-    CDB_REQUIRE(g, "null group");
-    HybPlan p;
-    cdb_status rc = hyb_plan(h, nq, top_k, &p);
-    if (rc || (rc = hyb_check_csr(h->sparse_offsets, h->sparse_dims, h->sparse_values, p.nq[HYB_SPARSE], h->tfidf_offsets,
-                                  h->tfidf_hashes, p.nq[HYB_TFIDF])))
-        return rc;
-    std::lock_guard<std::mutex> lock(g->mu);
-    if ((rc = hyb_group_check(g, &p))) return rc;
-    if (!nq) return CDB_OK;
-    if (!top_k) {
-        memset(out_counts, 0, (size_t)nq * 4);
-        return CDB_OK;
-    }
-    const size_t nl = g->dev.size();
-    std::vector<std::shared_lock<std::shared_mutex>> locks;
-    for (size_t i = 0; i < nl; ++i) {
-        if (h->use_sparse) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
-        if (h->use_tfidf) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
-    }
-    // the dense batch, the sparse CSR and the TF-IDF CSR of the named sources to every local device
-    const uint32_t dim = h->use_dense ? index_dim(g->shard[0]) : 0;
-    const uint64_t nqp = h->use_sparse ? h->sparse_offsets[nq] : 0, nqh = h->use_tfidf ? h->tfidf_offsets[nq] : 0;
-    const size_t off_bytes = ((size_t)nq + 1) * 8;
-    Staged st;
-    HostRows r;
-    if (!(rc = stage_queries(g, {{h->dense_queries, (size_t)nq * dim * 4}, {h->sparse_offsets, h->use_sparse ? off_bytes : 0},
-                                 {h->sparse_dims, nqp * 4}, {h->sparse_values, nqp * 4}, {h->tfidf_offsets, h->use_tfidf ? off_bytes : 0},
-                                 {h->tfidf_hashes, nqh * 4}}, &st)) &&
-        !(rc = host_rows(g, nq, 6 * top_k, out_ids, out_scores, out_counts, h->use_dense ? err_flags : nullptr, &r))) {
-        std::vector<const float *> dq(nl);
-        for (size_t i = 0; i < nl; ++i) dq[i] = st.at<float>(i, 0);
-        rc = hybrid_group_run(g, p, nullptr, nq, top_k, fusion_constant_k, h->dense_id_stride, dq, staged_sparse(st, 1), staged_tfidf(st, 4),
-                              nqh, r.ids, r.scores, r.counts, h->use_dense ? r.err : nullptr, nullptr);
-    }
-    return host_finish(g, rc, &r);
+    std::vector<uint8_t> kinds;
+    cdb_hybrid_group_mixed_sources m;
+    if (cdb_status rc = hyb_pair_batch(h, nq, &kinds, &m)) return rc;
+    return cdb_hybrid_search_batch_mixed_sharded(g, &m, nq, top_k, fusion_constant_k, out_ids, out_scores, out_counts,
+                                                 h->use_dense ? err_flags : nullptr);
 }
 
 cdb_status cdb_hybrid_search_batch_sharded_device(cdb_shard_group *g, const cdb_hybrid_group_sources *h, uint32_t nq, uint32_t top_k,
                                                   float fusion_constant_k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
                                                   uint8_t *d_err_flags, void *stream) {
-    CDB_REQUIRE(!nq || !top_k || (d_ids && d_scores && d_counts), "null output");
-    CDB_REQUIRE(!nq || d_counts, "null output");
-    CDB_REQUIRE(g, "null group");
+    std::vector<uint8_t> kinds;
+    cdb_hybrid_group_mixed_sources m;
     HybPlan p;
-    cdb_status rc = hyb_plan(h, nq, top_k, &p);
-    if (rc) return rc;
+    cdb_status rc = hyb_pair_batch(h, nq, &kinds, &m);
+    if (rc || (rc = hyb_device_request(g, &m, nq, top_k, d_ids, d_scores, d_counts, &p))) return rc;
     if (h->use_tfidf) {
         set_error("the hybrid device form has no TF-IDF sub-search (the host sizes its idf exchange by the batch's term count, "
                   "which cdb_hybrid_group_sources does not carry): use cdb_hybrid_search_batch_sharded");
         return CDB_UNSUPPORTED;
     }
-    CDB_REQUIRE(g->dev.size() == 1, "the device form serves groups of one local slot (cdb_shard_group_create_rank, or one device)");
-    std::lock_guard<std::mutex> lock(g->mu);
-    if ((rc = hyb_group_check(g, &p))) return rc;
-    if (!nq) return CDB_OK;
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    const cudaStream_t s = slot_stream(g, 0, (cudaStream_t)stream);
-    if (!top_k) {
-        CDB_CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s));
-        return CDB_OK;
-    }
-    std::unique_ptr<std::shared_lock<std::shared_mutex>> shard_lock;
-    if (h->use_sparse) shard_lock.reset(new std::shared_lock<std::shared_mutex>(sparse_index_mutex(g->sparse[0])));
-    const std::vector<const float *> dq(1, h->dense_queries);
-    const std::vector<SparseQueries> sq(1, SparseQueries{h->sparse_offsets, h->sparse_dims, h->sparse_values});
-    return hybrid_group_run(g, p, nullptr, nq, top_k, fusion_constant_k, h->dense_id_stride, dq, sq, {}, 0, d_ids, d_scores, d_counts,
-                            h->use_dense ? d_err_flags : nullptr, (cudaStream_t)stream);
+    return hyb_device_run(g, m, &p, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, h->use_dense ? d_err_flags : nullptr,
+                          stream);
 }
 
 cdb_status cdb_hybrid_search_batch_mixed_sharded(cdb_shard_group *g, const cdb_hybrid_group_mixed_sources *h, uint32_t nq, uint32_t top_k,
@@ -1481,10 +1401,9 @@ cdb_status cdb_hybrid_search_batch_mixed_sharded(cdb_shard_group *g, const cdb_h
     CDB_REQUIRE(!nq || (out_counts && (!top_k || (out_ids && out_scores))), "null output");
     CDB_REQUIRE(g, "null group");
     HybPlan p;
-    cdb_status rc = hyb_mixed_plan(h, nq, top_k, &p);
-    if (rc || (rc = hyb_check_csr(h->sparse_offsets, h->sparse_dims, h->sparse_values, h->n_sparse, h->tfidf_offsets, h->tfidf_hashes,
-                                  h->n_tfidf)))
-        return rc;
+    cdb_status rc = check_hybrid_request(h, nq, top_k, true);
+    if (rc || (rc = hyb_params(*h, top_k, &p))) return rc;
+    CDB_REQUIRE(!h->n_tfidf || h->tfidf_offsets[h->n_tfidf] < (1ull << 31), "a batch of 2^31 query terms or more");
     std::lock_guard<std::mutex> lock(g->mu);
     if ((rc = hyb_group_check(g, &p))) return rc;
     if (!nq) return CDB_OK;
@@ -1495,11 +1414,11 @@ cdb_status cdb_hybrid_search_batch_mixed_sharded(cdb_shard_group *g, const cdb_h
     const size_t nl = g->dev.size();
     std::vector<std::shared_lock<std::shared_mutex>> locks;
     for (size_t i = 0; i < nl; ++i) {
-        if (p.use[HYB_SPARSE]) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
-        if (p.use[HYB_TFIDF]) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
+        if (p.nq[HYB_SPARSE]) locks.emplace_back(sparse_index_mutex(g->sparse[i]));
+        if (p.nq[HYB_TFIDF]) locks.emplace_back(tfidf_index_mutex(g->tfidf[i]));
     }
     // each source's batch to every local device, once
-    const uint32_t dim = p.use[HYB_DENSE] ? index_dim(g->shard[0]) : 0;
+    const uint32_t dim = p.nq[HYB_DENSE] ? index_dim(g->shard[0]) : 0;
     const uint64_t nqp = h->n_sparse ? h->sparse_offsets[h->n_sparse] : 0, nqh = h->n_tfidf ? h->tfidf_offsets[h->n_tfidf] : 0;
     Staged st;
     HostRows r;
@@ -1519,41 +1438,9 @@ cdb_status cdb_hybrid_search_batch_mixed_sharded(cdb_shard_group *g, const cdb_h
 cdb_status cdb_hybrid_search_batch_mixed_sharded_device(cdb_shard_group *g, const cdb_hybrid_group_mixed_sources *h, uint32_t nq,
                                                         uint32_t top_k, float fusion_constant_k, uint32_t *d_ids, float *d_scores,
                                                         uint32_t *d_counts, uint8_t *d_err_flags, void *stream) {
-    CDB_REQUIRE(!nq || (d_counts && (!top_k || (d_ids && d_scores))), "null output");
-    CDB_REQUIRE(g, "null group");
     HybPlan p;
-    cdb_status rc = hyb_mixed_plan(h, nq, top_k, &p);
-    if (rc) return rc;
-    CDB_REQUIRE(!h->n_tfidf || h->tfidf_hashes || !h->n_tfidf_hashes, "null tf-idf query hashes");
-    CDB_REQUIRE(h->n_tfidf_hashes < (1ull << 31), "a batch of 2^31 query terms or more");
-    CDB_REQUIRE(g->dev.size() == 1, "the device form serves groups of one local slot (cdb_shard_group_create_rank, or one device)");
-    std::lock_guard<std::mutex> lock(g->mu);
-    if ((rc = hyb_group_check(g, &p))) return rc;
-    if (!nq) return CDB_OK;
-    // the group's work follows what the caller's stream held, and the caller's later work follows it
-    const cudaStream_t out = (cudaStream_t)stream, s = slot_stream(g, 0, out);
-    CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-    if (s != out) {
-        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], out));
-        CDB_CUDA_TRY(cudaStreamWaitEvent(s, g->ev[0], 0));
-    }
-    if (!top_k) {
-        rc = cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, s) == cudaSuccess ? CDB_OK : CDB_CUDA_ERROR;
-        if (rc) set_error("hybrid search: cudaMemsetAsync failed");
-    } else {
-        std::vector<std::shared_lock<std::shared_mutex>> locks;
-        if (p.use[HYB_SPARSE]) locks.emplace_back(sparse_index_mutex(g->sparse[0]));
-        if (p.use[HYB_TFIDF]) locks.emplace_back(tfidf_index_mutex(g->tfidf[0]));
-        rc = hybrid_group_run(g, p, h->kinds, nq, top_k, fusion_constant_k, h->dense_id_stride, {h->dense_queries},
-                              {SparseQueries{h->sparse_offsets, h->sparse_dims, h->sparse_values}},
-                              {TfQueries{h->tfidf_offsets, h->tfidf_hashes}}, h->n_tfidf_hashes, d_ids, d_scores, d_counts, d_err_flags, out);
-    }
-    if (s != out) {
-        CDB_CUDA_TRY(cudaSetDevice(g->dev[0]));
-        CDB_CUDA_TRY(cudaEventRecord(g->ev[0], s));
-        CDB_CUDA_TRY(cudaStreamWaitEvent(out, g->ev[0], 0));
-    }
-    return rc;
+    cdb_status rc = hyb_device_request(g, h, nq, top_k, d_ids, d_scores, d_counts, &p);
+    return rc ? rc : hyb_device_run(g, *h, &p, nq, top_k, fusion_constant_k, d_ids, d_scores, d_counts, d_err_flags, stream);
 }
 
 }  // extern "C"

@@ -1016,20 +1016,23 @@ typedef struct {
     const uint32_t *tfidf_hashes;
 } cdb_hybrid_sources;
 
-/* Composed hybrid search: both sub-searches through their public *_search_batch_device entry points, the second on a side
- * stream forked from and joined back to the caller's stream (the device form's `stream`; NULL = the legacy default stream)
- * so the two overlap, then the fusion on the caller's stream;
- * intermediate lists live in stream-ordered scratch, and no stream, event or allocation outlives the call's work.
+/* Composed hybrid search: the batch of one kind of cdb_hybrid_search_batch_mixed[_device] (below) in which every query
+ * names the two given sources.  Both sub-searches run through their public *_search_batch_device entry points, the second
+ * on a side stream forked from and joined back to the caller's stream (the device form's `stream`; NULL = the legacy
+ * default stream) so the two overlap, then one fusion on the caller's stream; intermediate lists live in stream-ordered
+ * scratch, and no stream, event or allocation outlives the call's work.
  * out_ids / out_scores [B][6 * top_k], out_counts [B]; err_flags [B] (may be NULL) receives the dense search's flags and
  * is written only when a dense source is given.
  * Each sub-search takes its own handle's shared lock and sees that handle as of its own enqueue; there is no snapshot
  * across the two handles (the reference takes none either).  Appends and deletes keep their contracts: they wait for the
  * searches already enqueued on the device.
- * CDB_INVALID_PARAMS: top_k > 341 (the dense and sparse searches take k <= 1024), a sparse source with rerank and
- * 3 * top_k * reranking_factor > 5120, a source count other than two, null queries, handles on different devices.
+ * CDB_INVALID_PARAMS: null sources or a source count other than two, then the refusals of the mixed form: top_k > 341 (the
+ * dense and sparse searches take k <= 1024), CDB_SEARCH_ALL_CANDIDATES, null queries, a sparse source with rerank and
+ * 3 * top_k * reranking_factor > 5120, malformed host query CSR, handles on different devices.
  * CDB_UNSUPPORTED: a dense handle with graph metadata (its HNSW searches go through cdb_search_batch_filtered[_device];
  * attach it to a one-slot shard group and use cdb_hybrid_search_batch_sharded, below).  Refusals of a sub-search's own parameter
- * checks are returned as that search returns them.  top_k = 0: empty results (out_counts zeroed), no kernel launched. */
+ * checks are returned as that search returns them.  B = 0 or top_k = 0: empty results (out_counts zeroed), no kernel
+ * launched. */
 cdb_status cdb_hybrid_search_batch(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k, float fusion_constant_k,
                                    uint32_t *out_ids, float *out_scores, uint32_t *out_counts, uint8_t *err_flags);
 cdb_status cdb_hybrid_search_batch_device(const cdb_hybrid_sources *sources, uint32_t n_queries, uint32_t top_k,
@@ -1061,20 +1064,22 @@ typedef struct {
  * dense_id_stride = max_replica_per_node); when none has, the path of cdb_search_batch_sharded in any mode.  A group of
  * one local slot (cdb_shard_group_create with one device) is a real group, so a single index with graph metadata gets its
  * hybrid search here, which cdb_hybrid_search_batch refuses.
- * Both sub-searches run under one hold of the group's lock, one after the other in list order on the group's streams (the
- * caller's stream in the device form), so every rank issues the same collectives in the same order; the first list lives
- * in scratch of this call until the fusion on local slot 0 (this rank's device in a per-rank group), which every rank
- * runs and so ends with the same rows.  Queries are fused in chunks that keep both intermediate lists within 256 MB.  The
- * host form copies nothing back but the fused ids, scores, counts and error bytes.
- * CDB_INVALID_PARAMS, before any copy or launch: a null group, sources or output; a source count other than two;
- * top_k > 341; sparse rerank with 3 * top_k * reranking_factor > 5120 (and the sparse search's other parameter checks);
- * CDB_SEARCH_ALL_CANDIDATES in dense_params; null queries of a named source; malformed query CSR (host form); a local
- * slot without a shard of a named kind; local dense shards of which some have graph metadata and some do not, or a
- * mode other than CDB_MODE_HNSW on metadata shards; world * 3 * top_k * 8 > 200 KB (the dense merge).  top_k = 0: counts
- * zeroed, nothing launched.
+ * The call is the batch of one kind of cdb_hybrid_search_batch_mixed_sharded[_device] (below) in which every query names
+ * the two given sources.  Both sub-searches run under one hold of the group's lock, one after the other in list order on
+ * the group's streams (the caller's stream in the device form), so every rank issues the same collectives in the same
+ * order; the first list lives in scratch of this call until the fusion on local slot 0 (this rank's device in a per-rank
+ * group), which every rank runs and so ends with the same rows.  Queries are fused in chunks that keep both intermediate
+ * lists within 256 MB.  The host form copies nothing back but the fused ids, scores, counts and error bytes.
+ * CDB_INVALID_PARAMS, before any copy or launch: null sources or a source count other than two, then the refusals of the
+ * mixed form: a null output or group; top_k > 341; CDB_SEARCH_ALL_CANDIDATES in dense_params; null queries of a named
+ * source; sparse rerank with 3 * top_k * reranking_factor > 5120; malformed query CSR (host form); the sparse search's
+ * other parameter checks; a local slot without a shard of a named kind; local dense shards of which some have graph
+ * metadata and some do not, or a mode other than CDB_MODE_HNSW on metadata shards; world * 3 * top_k * 8 > 200 KB (the
+ * dense merge).  B = 0 or top_k = 0: counts zeroed, nothing launched.
  * The device form serves groups of one local slot (per-rank groups and one-device local groups), takes device arrays and
- * is asynchronous on `stream`.  It refuses a TF-IDF source with CDB_UNSUPPORTED: the host sizes the TF-IDF idf exchange by
- * the batch's term count, and cdb_hybrid_group_sources carries none. */
+ * is asynchronous on `stream` (NULL = the legacy default stream): its work follows what `stream` held, and the caller's
+ * later work on `stream` follows it.  It refuses a TF-IDF source with CDB_UNSUPPORTED, before the group is read: the host
+ * sizes the TF-IDF idf exchange by the batch's term count, and cdb_hybrid_group_sources carries none. */
 cdb_status cdb_hybrid_search_batch_sharded(cdb_shard_group *group, const cdb_hybrid_group_sources *sources, uint32_t n_queries,
                                            uint32_t top_k, float fusion_constant_k, uint32_t *out_ids, float *out_scores,
                                            uint32_t *out_counts, uint8_t *err_flags);

@@ -3,7 +3,7 @@ and score bits): the fusion kernel on random and adversarial lists (empty, one-s
 ids, id strides, ids near 2^32 - 2, up to 1023 entries per list, batch 1 and 1024) under fusion constants from 60 to NaN;
 the composed search for each pairing against the fusion of the two handles' own results at k = 3 * top_k (HNSW on a
 GPU-built graph, brute force on the tensor-core path, sparse with and without re-rank, deleted rows in every handle);
-replica-id dense results fused with id_stride; the device form on a side stream, 8 host threads, and appends and deletes
+replica-id dense results fused with id_stride; error bytes written only with a dense source; the device form on a side stream, 8 host threads, and appends and deletes
 queued behind hybrid searches.  The tests without the gpu mark check the refusals that come before any device work."""
 import concurrent.futures
 import ctypes as C
@@ -372,6 +372,34 @@ def test_device_form_on_a_side_stream_and_threads(world, pair):
     with concurrent.futures.ThreadPoolExecutor(8) as ex:
         for got in ex.map(lambda _: cdb.hybrid_batch_search(10, 60.0, **kw), range(16)):
             check(got, want)
+
+
+@gpu
+@pytest.mark.parametrize("pair", PAIRS, ids="-".join)
+def test_error_bytes_only_with_a_dense_source(world, pair):
+    """0xEE-filled err_flags get the dense search's bytes with a dense source and stay untouched without one, in the host
+    and the device form"""
+    import torch
+    from cosdata_b200.api import hybrid_sources
+    dev = torch.device("cuda", 0)
+    kw, _ = sources(world, pair)
+    want = world["hn"].batch_search(world["dq"], 30, **DENSE_HNSW)[3] if "dense" in pair else np.full(B, 0xEE, np.uint8)
+    src, keep, _ = hybrid_sources(**kw)
+    ids, sc = np.zeros((B, 60), np.uint32), np.zeros((B, 60), np.float32)
+    cnt, err = np.zeros(B, np.uint32), np.full(B, 0xEE, np.uint8)
+    assert _lib.load().cdb_hybrid_search_batch(C.byref(src), B, 10, 60.0, ids.ctypes.data, sc.ctypes.data, cnt.ctypes.data,
+                                               err.ctypes.data) == 0
+    assert np.array_equal(err, want)
+    src, alive = device_sources(world, pair, dev)
+    ids = torch.zeros((B, 60), dtype=torch.int32, device=dev)
+    sc = torch.zeros((B, 60), dtype=torch.float32, device=dev)
+    cnt = torch.zeros(B, dtype=torch.int32, device=dev)
+    err = torch.full((B,), 0xEE, dtype=torch.uint8, device=dev)
+    torch.cuda.synchronize(dev)
+    assert _lib.load().cdb_hybrid_search_batch_device(C.byref(src), B, 10, 60.0, ids.data_ptr(), sc.data_ptr(), cnt.data_ptr(),
+                                                      err.data_ptr(), None) == 0
+    torch.cuda.synchronize(dev)
+    assert np.array_equal(err.cpu().numpy(), want)
 
 
 @gpu

@@ -182,7 +182,9 @@ def test_single_index_mixed_equals_the_split_by_kind(single, dense_key, case, b,
 
 def test_error_bytes_land_at_the_dense_queries():
     """a u8 cosine index with all-zero rows: every dense search sets CDB_ERRFLAG_CALCULATION (cosine.rs:230-231), so the
-    error bytes of a shuffled batch are 1 exactly where the query names dense, on the single index and a one-slot group"""
+    error bytes of a shuffled batch are 1 exactly where the query names dense, on the single index and a one-slot group.
+    A batch of one kind gets them from the dense search in place; the split-by-kind call of such a batch is the two-source
+    entry point on the same batch."""
     c = Corpus(seed=35)
     vecs = c.vecs.copy()
     vecs[[7, 9000]] = -1.0
@@ -198,8 +200,8 @@ def test_error_bytes_land_at_the_dense_queries():
     g.attach_sparse(0, sp)
     g.attach_tfidf(0, tf)
     opts = {"mode": cdb.SearchMode.BRUTE_CODES}
-    for b in (1, 64, 200):
-        kinds = kinds_of("012", b, seed=4)
+    for case, b in (("012", 1), ("012", 64), ("012", 200), ("0", 64), ("1", 64), ("2", 64)):
+        kinds = kinds_of(case, b, seed=4)
         dq, sq, tq = c.inputs(b)
         names_dense = np.isin(kinds, (0, 1)).astype(np.uint8)
         got = cdb.hybrid_batch_search_mixed(kinds, 10, 60.0, dense=(ix, dq, opts), sparse=(sp, sq, SP_OPTS), tfidf=(tf, tq))
@@ -236,6 +238,16 @@ def test_single_index_searches_each_source_once(single):
     n0 = cdb.kernel_launch_count()
     got = cdb.hybrid_batch_search_mixed(kinds, 0, 60.0, **kw)
     assert cdb.kernel_launch_count() == n0 and not got[2].any()
+    # a two-source call over the whole batch: its two sub-searches and one fusion
+    qs = {"dense": dq, "sparse": sq, "tfidf": tq}
+    for pair in KIND_SOURCES:
+        n0 = cdb.kernel_launch_count()
+        for name in pair:
+            run[name](qs[name])
+        sub = cdb.kernel_launch_count() - n0
+        n0 = cdb.kernel_launch_count()
+        cdb.hybrid_batch_search(top_k, 60.0, **{name: kw[name] for name in pair})
+        assert cdb.kernel_launch_count() - n0 == sub + 1
 
 
 def torch_of(a, dev):
