@@ -346,6 +346,11 @@ PROTOTYPES = {
     "cdb_tfidf_search_batch": (C.c_int32, [C.c_void_p, c_vp, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p]),
     "cdb_tfidf_search_batch_device": (C.c_int32, [C.c_void_p, c_vp, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_f32p, c_u32p,
                                                   C.c_void_p]),
+    "cdb_tfidf_files_open": (C.c_int32, [C.c_char_p, C.POINTER(C.c_void_p)]),
+    "cdb_tfidf_files_close": (C.c_int32, [C.c_void_p]),
+    "cdb_tfidf_files_info": (C.c_int32, [C.c_void_p, c_vp]),
+    "cdb_tfidf_files_read": (C.c_int32, [C.c_void_p, c_u32p, c_u32p, c_vp, c_u32p, c_f32p, c_u32p]),
+    "cdb_tfidf_index_load_files": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_uint64, c_u8p, C.c_int32]),
     "cdb_rrf_fuse": (C.c_int32, [C.c_int32, c_u32p, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_u32p, C.c_uint32, C.c_uint32,
                                  C.c_uint32, C.c_float, C.c_uint32, c_u32p, c_f32p, c_u32p]),
     "cdb_rrf_fuse_device": (C.c_int32, [C.c_int32, c_u32p, c_u32p, C.c_uint32, C.c_uint32, c_u32p, c_u32p, C.c_uint32,

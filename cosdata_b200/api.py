@@ -1178,11 +1178,57 @@ class TfIdfIndex:
         _check(_lib.load().cdb_tfidf_search_batch(self.h, _ptr(o), _ptr(h), nq, k, _ptr(ids), _ptr(scores), _ptr(counts)))
         return ids[:nq], scores[:nq], counts[:nq]
 
+    def load_files(self, files, n_rows, counted=None, carry_stats=True):
+        """cdb_tfidf_index_load_files: the live words of a TfIdfFiles whose ids are in [id_base, id_base + n_rows) into this
+        empty index, as TFIDFIndexRoot::deserialize left them.  counted: per-row flags that also count empty rows (documents
+        whose text was all stopwords); name only live documents, never deleted ones.  carry_stats=False: N 0 and df 0, for every shard of a group but one."""
+        c = None if counted is None else np.ascontiguousarray(counted, dtype=np.uint8)
+        if c is not None and c.size < n_rows:
+            raise ValueError("counted needs n_rows flags")
+        _check(_lib.load().cdb_tfidf_index_load_files(self.h, files.h, int(n_rows), _ptr(c), 1 if carry_stats else 0))
+
     def search(self, query, top_k=None):
         """-> [(id, score)] best first (search_internal's result order)"""
         ids, scores, counts = self.batch_search([list(query)], top_k)
         c = int(counts[0])
         return list(zip(ids[0, :c].tolist(), scores[0, :c].tolist()))
+
+
+class TfIdfFiles:
+    """the reference's TF-IDF index files (<collection>/tf_idf_index: index-tree.dim, <version>.idat) as
+    TFIDFIndexRoot::deserialize reads them.  .info = dict(n_docs, terms, records, live, id_end, max_version)"""
+
+    INFO = ("n_docs", "terms", "records", "live", "id_end", "max_version")
+
+    def __init__(self, tf_idf_index_dir):
+        h = C.c_void_p()
+        _check(_lib.load().cdb_tfidf_files_open(os.fsencode(tf_idf_index_dir), C.byref(h)))
+        self.h = h
+        info = np.zeros(6, np.uint64)
+        _check(_lib.load().cdb_tfidf_files_info(self.h, _ptr(info)))
+        self.info = dict(zip(self.INFO, (int(x) for x in info)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            _lib.load().cdb_tfidf_files_close(self.h)
+            self.h = None
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def read(self):
+        """-> (hashes u32[T] ascending, df u32[T], offsets u64[T+1], doc_ids u32[L], tfs f32[L], versions u32[L]): each term's
+        live words in list order"""
+        t, n = self.info["terms"], self.info["live"]
+        hs, df, off = np.zeros(max(t, 1), np.uint32), np.zeros(max(t, 1), np.uint32), np.zeros(t + 1, np.uint64)
+        ids, tfs, ver = np.zeros(max(n, 1), np.uint32), np.zeros(max(n, 1), np.float32), np.zeros(max(n, 1), np.uint32)
+        _check(_lib.load().cdb_tfidf_files_read(self.h, _ptr(hs), _ptr(df), _ptr(off), _ptr(ids), _ptr(tfs), _ptr(ver)))
+        return hs[:t], df[:t], off, ids[:n], tfs[:n], ver[:n]
 
 
 # ---------------------------------------------------------------- hybrid search (reciprocal-rank fusion)

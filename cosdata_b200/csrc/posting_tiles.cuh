@@ -213,7 +213,31 @@ struct PostingTiles : PostingStore {
         }
         return rc;
     }
+
+    // A load into an empty store: rows [0, row_off.size() - 1) whose pairs the caller has written to d_keys / d_vals and whose
+    // offsets (row_off, host) it has written to d_row_off.  The rows become the store's and every tile is built; if that
+    // fails the store is empty again and the error stays.  b must fit the largest tile.
+    cdb_status load_rows(std::vector<uint64_t> row_off, BuildBufs &b, cudaStream_t s) {
+        h_row_off = std::move(row_off);
+        n_rows = h_row_off.size() - 1;
+        n_pairs = h_row_off.back();
+        const cdb_status rc = build_tiles(0, (n_rows + TILE_ROWS - 1) >> TILE_SHIFT, b, s);
+        if (rc) {
+            const std::string msg = cdb_last_error_string();
+            restore_rows(0, b, s);
+            set_error(msg);
+        }
+        return rc;
+    }
 };
+
+// the most pairs one row tile of the CSR offsets row_off holds
+inline uint64_t max_tile_pairs(const std::vector<uint64_t> &row_off) {
+    const uint64_t n = row_off.size() - 1;
+    uint64_t m = 0;
+    for (uint64_t r0 = 0; r0 < n; r0 += TILE_ROWS) m = std::max(m, row_off[std::min(n, r0 + TILE_ROWS)] - row_off[r0]);
+    return m;
+}
 
 // the result of a search of an index without tiles: ids CDB_INVALID_ID, scores 0, counts 0
 cdb_status fill_empty_results(uint32_t nq, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts, cudaStream_t s);

@@ -21,6 +21,7 @@
 #include "bm25_idf.h"
 #include "kernels.h"
 #include "posting_tiles.cuh"
+#include "tfidf_file.h"
 
 namespace cdb {
 namespace {
@@ -259,6 +260,66 @@ __global__ void __launch_bounds__(TF_THREADS, 1) tf_group_finalize_kernel(const 
     tf_sort_winners(make_uint2(bid, __float_as_uint(best)), kout, out_ids + (size_t)qi * kout, out_scores + (size_t)qi * kout, out_counts + qi);
 }
 
+// ---------------------------------------------------------------- load from the reference's files (cdb_tfidf_index_load_files)
+// One staged chunk of the files' record words, positions pos0 .. pos0 + n of their concatenation (marked words already
+// u64::MAX): every live word whose id is in [id_base, id_base + n_rows), as the sort key row << 32 | hash and the value
+// version << 32 | tf bits, compacted at *count with one atomic per warp (the order is settled by the sort that follows, whose
+// keys are unique unless a row repeats a hash).  Nothing is written at or past cap.  rec_base / rec_meta: each record's
+// first position and (hash, version), ascending positions.
+__global__ void tf_load_decode_kernel(const uint64_t *__restrict__ words, uint64_t n, uint64_t pos0, const uint64_t *__restrict__ rec_base,
+                                      const uint2 *__restrict__ rec_meta, uint32_t n_recs, uint32_t id_base, uint64_t n_rows, uint64_t cap,
+                                      unsigned long long *__restrict__ count, uint64_t *__restrict__ keys, uint64_t *__restrict__ vals) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint64_t w = ~0ull, row = 0;
+        bool take = false;
+        if (i < n) {
+            w = words[i];
+            row = (uint64_t)(uint32_t)(w >> 32) - id_base;   // wraps past n_rows below id_base
+            take = w != ~0ull && !(w >> 63) && row < n_rows;
+        }
+        const uint32_t m = __ballot_sync(0xFFFFFFFFu, take);
+        if (!m) continue;
+        const int leader = __ffs(m) - 1;
+        unsigned long long at = 0;
+        if (lane == (uint32_t)leader) at = atomicAdd(count, (unsigned long long)__popc(m));
+        at = __shfl_sync(0xFFFFFFFFu, at, leader) + __popc(m & ((1u << lane) - 1));
+        if (!take || at >= cap) continue;
+        // the record holding position pos0 + i: the last one starting at or before it
+        const uint64_t pos = pos0 + i;
+        uint32_t lo = 0, hi = n_recs;
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (rec_base[mid] <= pos) lo = mid + 1; else hi = mid; }
+        const uint2 meta = rec_meta[lo - 1];
+        keys[at] = row << 32 | meta.x;
+        vals[at] = (uint64_t)meta.y << 32 | (uint32_t)w;
+    }
+}
+
+// row_off[r], r in [0, n_rows]: the first of the n sorted keys whose row is r or more
+__global__ void tf_load_offsets_kernel(const uint64_t *__restrict__ keys, uint64_t n, uint64_t n_rows, uint64_t *__restrict__ row_off) {
+    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r > n_rows) return;
+    uint64_t lo = 0, hi = n;
+    while (lo < hi) { const uint64_t mid = (lo + hi) >> 1; if ((keys[mid] >> 32) < r) lo = mid + 1; else hi = mid; }
+    row_off[r] = lo;
+}
+
+// the sorted pairs into the store's hashes and tf values, the version of each row's first pair into row_version, and
+// *mixed = 1 when a row's pairs carry two versions
+__global__ void tf_load_rows_kernel(const uint64_t *__restrict__ keys, const uint64_t *__restrict__ vals, uint64_t n,
+                                    uint32_t *__restrict__ out_hashes, float *__restrict__ out_tfs, uint32_t *__restrict__ row_version,
+                                    uint32_t *__restrict__ mixed) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t k = keys[i], v = vals[i];
+    out_hashes[i] = (uint32_t)k;
+    out_tfs[i] = __uint_as_float((uint32_t)v);
+    if (i == 0 || (keys[i - 1] >> 32) != (k >> 32)) row_version[k >> 32] = (uint32_t)(v >> 32);
+    else if ((vals[i - 1] >> 32) != (v >> 32)) *mixed = 1u;
+}
+
 }  // namespace
 }  // namespace cdb
 
@@ -323,6 +384,38 @@ cdb_status upload_terms(cdb_tfidf_index *ix, const std::vector<uint32_t> &terms,
     return CDB_OK;
 }
 
+// the distinct hashes of d_hashes[0..np) ascending into uniq, and how many pairs hold each into cnt, then a drain of s.  b's
+// scratch must hold np pairs: sorted hashes -> b.vals_out, distinct -> b.flags, counts -> b.vals_in, their number -> b.pos
+cudaError_t distinct_hashes(const uint32_t *d_hashes, uint64_t np, BuildBufs &b, cudaStream_t s, std::vector<uint32_t> &uniq,
+                            std::vector<uint32_t> &cnt) {
+    cudaError_t e = cudaSuccess;
+    if (np) {
+        uint32_t *runs = b.pos;
+        size_t t_sort = 0, t_rle = 0;
+        e = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d_hashes, b.vals_out, (int)np, 0, 32, s);
+        if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
+        const size_t need = std::max(t_sort, t_rle);
+        void *tmp = b.tmp;
+        if (e == cudaSuccess && need > b.tmp_bytes) e = cudaMallocAsync(&tmp, need, s);
+        size_t tb = need;
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp, tb, d_hashes, b.vals_out, (int)np, 0, 32, s);
+        tb = need;
+        if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(tmp, tb, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
+        uint32_t n_runs = 0;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&n_runs, runs, 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess) {
+            uniq.resize(n_runs);
+            cnt.resize(n_runs);
+            e = cudaMemcpyAsync(uniq.data(), b.flags, n_runs * 4ull, cudaMemcpyDeviceToHost, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(cnt.data(), b.vals_in, n_runs * 4ull, cudaMemcpyDeviceToHost, s);
+        }
+        if (tmp != b.tmp) cudaFreeAsync(tmp, s);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return e;
+}
+
 uint32_t out_cols(uint32_t k) { return (k == 0 || k > TF_BUCKETS) ? TF_BUCKETS : k; }
 
 // the scoring kernel's arguments for queries [q0, q0 + chunk); q_idf as TfSearch::q_idf
@@ -367,6 +460,150 @@ cdb_status search_locked(cdb_tfidf_index *ix, const uint64_t *d_qoff, const uint
     }
     cudaFreeAsync(win, s);
     return rc;
+}
+
+constexpr uint64_t TF_LOAD_STAGE_WORDS = (128ull << 20) / 8;   // two pinned staging buffers of 128 MB each
+
+// cdb_tfidf_index_load_files past its checks, on an empty index held exclusively, with the device drained.  The caller
+// empties the store again if this fails.
+cdb_status load_locked(cdb_tfidf_index *ix, const cdb_tfidf_files *f, uint64_t n_rows, const uint8_t *counted, bool carry, cudaStream_t s) {
+    PostingTiles<TfCodec> &st = ix->st;
+    const uint64_t n_recs = f->recs.size(), n_words = f->n_words;
+    CDB_REQUIRE(n_recs < (1ull << 32), "tf-idf load: the files hold 2^32 list records or more");
+    const uint64_t cap = std::min<uint64_t>(f->n_live, st.capacity_pairs);
+    const uint64_t stage = std::min<uint64_t>(n_words, TF_LOAD_STAGE_WORDS);
+    int sms = 0;
+    CDB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ix->desc.device));
+    // device scratch: record table, two sort buffers of cap keys and values, staging, the count, the row versions, the flag
+    const size_t bytes = n_recs * 16 + cap * 32 + 2 * stage * 8 + 8 + n_rows * 4 + 4;
+    uint8_t *buf = nullptr;
+    CDB_CUDA_TRY(cudaMallocAsync(&buf, bytes, s));
+    uint64_t *rec_base = reinterpret_cast<uint64_t *>(buf);
+    uint2 *rec_meta = reinterpret_cast<uint2 *>(rec_base + n_recs);
+    uint64_t *k0 = reinterpret_cast<uint64_t *>(rec_meta + n_recs), *k1 = k0 + cap, *v0 = k1 + cap, *v1 = v0 + cap;
+    uint64_t *d_stage = v1 + cap;
+    unsigned long long *d_count = reinterpret_cast<unsigned long long *>(d_stage + 2 * stage);
+    uint32_t *row_version = reinterpret_cast<uint32_t *>(d_count + 1);
+    uint32_t *d_mixed = row_version + n_rows;
+    uint64_t *h_stage = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    void *tmp = nullptr;
+    auto done = [&](cudaError_t e) -> cdb_status {
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (tmp) cudaFreeAsync(tmp, s);
+        cudaFreeAsync(buf, s);
+        cudaStreamSynchronize(s);
+        if (h_stage) cudaFreeHost(h_stage);
+        for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
+        if (e != cudaSuccess) { set_error(std::string("tf-idf load: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
+        return CDB_OK;
+    };
+    // the record table, then the words in chunks: copied into pinned memory record by record, the marked words overwritten
+    // with u64::MAX, uploaded and decoded while the host fills the other buffer
+    std::vector<uint64_t> hb(n_recs);
+    std::vector<uint2> hm(n_recs);
+    for (uint64_t r = 0; r < n_recs; ++r) { hb[r] = f->recs[r].base; hm[r] = make_uint2(f->hashes[f->recs[r].term], f->recs[r].version); }
+    cudaError_t e = cudaMemsetAsync(d_count, 0, 8, s);
+    if (e == cudaSuccess && n_recs) e = cudaMemcpyAsync(rec_base, hb.data(), n_recs * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && n_recs) e = cudaMemcpyAsync(rec_meta, hm.data(), n_recs * 8, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && stage) e = cudaHostAlloc(&h_stage, 2 * stage * 8, cudaHostAllocDefault);
+    for (int i = 0; i < 2 && e == cudaSuccess && stage; ++i) e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming);
+    uint64_t ri = 0, within = 0;
+    size_t k = 0;
+    for (uint64_t c0 = 0, it = 0; c0 < n_words && e == cudaSuccess; c0 += stage, ++it) {
+        const uint64_t nw = std::min(stage, n_words - c0);
+        const int half = (int)(it & 1);
+        uint64_t *h = h_stage + half * stage;
+        if (it >= 2 && (e = cudaEventSynchronize(ev[half])) != cudaSuccess) break;
+        for (uint64_t filled = 0; filled < nw;) {
+            const TfIdfFileRecord &r = f->recs[ri];
+            const uint64_t take = std::min<uint64_t>(r.len - within, nw - filled);
+            memcpy(h + filled, r.words + 8 * within, take * 8);
+            filled += take;
+            within += take;
+            if (within == r.len) { ++ri; within = 0; }
+        }
+        for (; k < f->killed.size() && f->killed[k] < c0 + nw; ++k) h[f->killed[k] - c0] = ~0ull;
+        e = cudaMemcpyAsync(d_stage + half * stage, h, nw * 8, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaEventRecord(ev[half], s);
+        if (e != cudaSuccess) break;
+        const uint32_t blocks = (uint32_t)std::min<uint64_t>((nw + 255) / 256, (uint64_t)sms * 16);   // grid-stride
+        tf_load_decode_kernel<<<blocks, 256, 0, s>>>(d_stage + half * stage, nw, c0, rec_base, rec_meta, (uint32_t)n_recs, ix->desc.id_base,
+                                                      n_rows, cap, d_count, k0, v0);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        e = cudaGetLastError();
+    }
+    unsigned long long np = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&np, d_count, 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) return done(e);
+    if (np > st.capacity_pairs || np >= (1ull << 31)) {
+        done(cudaSuccess);
+        set_error("tf-idf load: the files hold " + std::to_string(np) + " live pairs for these rows, more than capacity_pairs or 2^31 - 1");
+        return CDB_INVALID_PARAMS;
+    }
+    // rows: the pairs sorted on row << 32 | hash (each row ascending by hash), the offsets, the store's pairs, the versions
+    const int end_bit = 32 + (n_rows > 1 ? 64 - __builtin_clzll(n_rows - 1) : 0);
+    if (np) {
+        size_t tb = 0;
+        e = cub::DeviceRadixSort::SortPairs(nullptr, tb, k0, k1, v0, v1, (int)np, 0, end_bit, s);
+        if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tb, s);
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp, tb, k0, k1, v0, v1, (int)np, 0, end_bit, s);
+    }
+    if (e == cudaSuccess && n_rows) e = cudaMemsetAsync(row_version, 0, n_rows * 4, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_mixed, 0, 4, s);
+    if (e == cudaSuccess) {
+        tf_load_offsets_kernel<<<(uint32_t)((n_rows + 256) / 256), 256, 0, s>>>(k1, np, n_rows, st.d_row_off);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && np) {
+        tf_load_rows_kernel<<<(uint32_t)((np + 255) / 256), 256, 0, s>>>(k1, v1, np, st.d_keys, st.d_vals, row_version, d_mixed);
+        g_launch_count.fetch_add(1, std::memory_order_relaxed);
+        e = cudaGetLastError();
+    }
+    std::vector<uint64_t> row_off(n_rows + 1);
+    std::vector<uint32_t> h_version(n_rows);
+    uint32_t mixed = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(row_off.data(), st.d_row_off, (n_rows + 1) * 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && n_rows) e = cudaMemcpyAsync(h_version.data(), row_version, n_rows * 4, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&mixed, d_mixed, 4, cudaMemcpyDeviceToHost, s);
+    cdb_status rc = done(e);
+    if (rc) return rc;
+    CDB_REQUIRE(!mixed, "tf-idf load: a row's words carry two versions");
+    // per-row state: a row with a live word counts, and so does a row the mask names; a 0 in the mask on such a row is refused
+    std::vector<uint8_t> h_counted(n_rows);
+    for (uint64_t r = 0; r < n_rows; ++r) {
+        const bool words = row_off[r + 1] > row_off[r];
+        CDB_REQUIRE(!counted || counted[r] || !words, "tf-idf load: counted is 0 for a row with live words");
+        h_counted[r] = words || (counted && counted[r]) ? 1 : 0;
+    }
+    // the tiles; then the term table: the files' terms and df with carry_stats, else the hashes of the loaded pairs with df 0
+    BuildBufs b;
+    rc = b.alloc(std::max<uint64_t>(max_tile_pairs(row_off), carry ? 0 : np), TfCodec::END_BIT, s);
+    if (!rc) rc = st.load_rows(std::move(row_off), b, s);
+    if (rc) return rc;
+    std::vector<uint32_t> terms, df;
+    if (carry) {
+        terms = f->hashes;
+        df = f->df;
+    } else {
+        std::vector<uint32_t> cnt;
+        if ((e = distinct_hashes(st.d_keys, np, b, s, terms, cnt)) != cudaSuccess) {
+            set_error(std::string("tf-idf load: ") + cudaGetErrorString(e));
+            return CDB_CUDA_ERROR;
+        }
+        df.assign(terms.size(), 0u);
+    }
+    const uint32_t docs = carry ? f->n_docs : 0u;
+    if ((rc = upload_terms(ix, terms, df, docs, true, s))) return rc;
+    ix->h_terms.swap(terms);
+    ix->h_df.swap(df);
+    ix->documents = docs;
+    ix->version = f->max_version;
+    ix->h_counted.swap(h_counted);
+    ix->h_version.swap(h_version);
+    return CDB_OK;
 }
 
 }  // namespace
@@ -482,33 +719,9 @@ cdb_status cdb_tfidf_index_append(cdb_tfidf_index *ix, const uint64_t *row_offse
     const cudaStream_t s = a.sg.s;
     BuildBufs &b = a.b;
     const uint32_t *d_hashes = ix->st.d_keys + a.p_old;
-    cudaError_t e = cudaSuccess;
     // df increments: the distinct hashes of the appended pairs and how many rows hold each (rows never repeat a hash)
     std::vector<uint32_t> uniq, cnt;
-    if (np) {
-        uint32_t *runs = b.pos;   // scratch: sorted hashes -> b.vals_out, unique -> b.flags, counts -> b.vals_in, runs -> pos
-        size_t t_sort = 0, t_rle = 0;
-        e = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, d_hashes, b.vals_out, (int)np, 0, 32, s);
-        if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
-        const size_t need = std::max(t_sort, t_rle);
-        void *tmp = b.tmp;
-        if (e == cudaSuccess && need > b.tmp_bytes) e = cudaMallocAsync(&tmp, need, s);
-        size_t tb = need;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortKeys(tmp, tb, d_hashes, b.vals_out, (int)np, 0, 32, s);
-        tb = need;
-        if (e == cudaSuccess) e = cub::DeviceRunLengthEncode::Encode(tmp, tb, b.vals_out, b.flags, b.vals_in, runs, (int)np, s);
-        uint32_t n_runs = 0;
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&n_runs, runs, 4, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e == cudaSuccess) {
-            uniq.resize(n_runs);
-            cnt.resize(n_runs);
-            e = cudaMemcpyAsync(uniq.data(), b.flags, n_runs * 4ull, cudaMemcpyDeviceToHost, s);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(cnt.data(), b.vals_in, n_runs * 4ull, cudaMemcpyDeviceToHost, s);
-        }
-        if (tmp != b.tmp) cudaFreeAsync(tmp, s);
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    const cudaError_t e = distinct_hashes(d_hashes, np, b, s, uniq, cnt);
     if (e != cudaSuccess) { set_error(std::string("tf-idf append: ") + cudaGetErrorString(e)); return CDB_CUDA_ERROR; }
     // the merged term table
     std::vector<uint32_t> terms, df;
@@ -540,6 +753,28 @@ cdb_status cdb_tfidf_index_append(cdb_tfidf_index *ix, const uint64_t *row_offse
     for (uint64_t r = 0; r < n; ++r) ix->h_counted.push_back(!counted || counted[r] ? 1 : 0);
     ix->h_version.resize(a.r_new, version);
     return CDB_OK;
+}
+
+cdb_status cdb_tfidf_index_load_files(cdb_tfidf_index *ix, const cdb_tfidf_files *files, uint64_t n_rows, const uint8_t *counted,
+                                      int32_t carry_stats) {
+    CDB_REQUIRE(ix && files, "null argument");
+    std::unique_lock<std::shared_mutex> lock(ix->rw);
+    CDB_REQUIRE(ix->st.n_rows == 0 && ix->h_terms.empty() && ix->documents == 0, "load_files needs an empty index");
+    CDB_REQUIRE(n_rows <= ix->desc.capacity_rows, "n_rows exceeds capacity_rows");
+    CDB_CUDA_TRY(cudaSetDevice(ix->desc.device));
+    // searches already enqueued on other streams finish first
+    CDB_CUDA_TRY(cudaDeviceSynchronize());
+    StreamGuard sg;
+    CDB_CUDA_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+    const cdb_status rc = load_locked(ix, files, n_rows, counted, carry_stats != 0, sg.s);
+    if (rc && ix->st.n_rows) {
+        const std::string msg = cdb_last_error_string();
+        BuildBufs none;   // dropping every row builds no tile
+        ix->st.restore_rows(0, none, sg.s);
+        cudaStreamSynchronize(sg.s);
+        set_error(msg);
+    }
+    return rc;
 }
 
 cdb_status cdb_tfidf_index_delete_rows(cdb_tfidf_index *ix, const uint32_t *rows, uint64_t n, uint32_t version) {

@@ -880,6 +880,50 @@ cdb_status cdb_tfidf_search_batch_device(cdb_tfidf_index *index, const uint64_t 
                                          uint32_t n_queries, uint32_t k, uint32_t *d_ids, float *d_scores, uint32_t *d_counts,
                                          void *stream);
 
+/* ---- the reference's TF-IDF index files (<collection>/tf_idf_index: index-tree.dim and <version>.idat, written by
+ * TFIDFIndexRoot::serialize and the serializers in src/models/serializer/tf_idf), read as TFIDFIndexRoot::deserialize reads them
+ * (src/models/tf_idf_index.rs:369-401).  Host-side, no GPU work.  Format and rules: DESIGN.md section 8d.
+ *   open   walks the tree (node dims checked against their tree position, child-offset cycles refused), reads every term
+ *          slot (a later slot of a quotient replaces an earlier one; hash = quotient << 16 | dim), walks each list's record
+ *          chain (offset and version cycles refused; a list without a record of its slot's version refused) and applies
+ *          the tombstones.  A missing file, a truncated node or record, an offset past a file's end, a cycle or a wrong dim
+ *          is CDB_INVALID_PARAMS with a message.  The files stay mapped until close.
+ *   info   info[6] = {N (total_documents_count), terms, list records kept, live words, largest live id + 1 (0 if none),
+ *          largest version of a kept record}
+ *   read   terms ascending by hash: hashes[terms], df[terms] (VersionedVec::len after deserialize: every word of the kept
+ *          records, marked and tombstone words included), offsets[terms + 1] (CSR into the live words, offsets[0] = 0) and
+ *          per live word in list order doc_ids, tfs and versions (of the record holding it).  A live word is neither
+ *          u64::MAX, nor marked by a tombstone, nor a tombstone (bit 63), so its id is below 2^31.  Any pointer but files
+ *          may be NULL. */
+typedef struct cdb_tfidf_files cdb_tfidf_files; /* opaque */
+cdb_status cdb_tfidf_files_open(const char *tf_idf_index_dir, cdb_tfidf_files **out);
+cdb_status cdb_tfidf_files_close(cdb_tfidf_files *files);
+cdb_status cdb_tfidf_files_info(const cdb_tfidf_files *files, uint64_t *info);
+cdb_status cdb_tfidf_files_read(const cdb_tfidf_files *files, uint32_t *hashes, uint32_t *df, uint64_t *offsets, uint32_t *doc_ids,
+                                float *tfs, uint32_t *versions);
+/* Loads the files into an EMPTY index (no row, no term, N = 0): the state the reference serves after deserialize, so that
+ * searches, term_stats and every later append and delete under the rules above equal the reference's.
+ *   rows      row r (id id_base + r, r < n_rows <= capacity_rows) holds the live words whose id is id_base + r, ascending by
+ *             hash.  Words of ids outside [id_base, id_base + n_rows) are skipped (another shard's).  A row is counted when
+ *             it has a live word or counted[r] = 1 (a document whose text was all stopwords); counted[r] = 0 on a row with a
+ *             live word is refused; counted = NULL marks nothing more.  A row's insert version is that of the record
+ *             holding its words; a row whose words carry two versions is refused, and so is one repeating a hash.  A row
+ *             deleted before the files were written comes back empty and not deleted.  counted must name only live
+ *             documents with text: a deleted document's row is not in the tombstone bitmap, so with counted[r] = 1 it
+ *             would count, and a later delete of it would lower N again.
+ *   stats     carry_stats = 1: N is the files' N and every term of the files is known with its file df.  carry_stats = 0:
+ *             N = 0 and the hashes of the loaded rows are known with df 0.  The index's version is the files' largest.
+ *   groups    a shard group sums N and df over its shards in wrapping u32, so load exactly one shard of a group with
+ *             carry_stats = 1 and the others with 0, each over its own id range: group searches, and later appends and
+ *             deletes on any shard, then equal the one index loaded with the stats.  A shard loaded without them serves
+ *             only group searches (its own N and df are not the corpus's).
+ *   limits    more live pairs for the rows than capacity_pairs (or 2^31 or more) is CDB_INVALID_PARAMS.
+ * The device decodes, sorts and scatters the words; the host only copies the records into pinned staging memory (at most
+ * 256 MB) and marks the tombstoned positions.  The handle is held exclusively, as by an append, after the searches already
+ * enqueued have drained.  A load that fails leaves the index empty and usable. */
+cdb_status cdb_tfidf_index_load_files(cdb_tfidf_index *index, const cdb_tfidf_files *files, uint64_t n_rows, const uint8_t *counted,
+                                      int32_t carry_stats);
+
 /* ------------------------------------------------ multi-GPU: row-sharded sparse and TF-IDF search
  * The sparse and TF-IDF indexes of a collection split over the slots of a cdb_shard_group, next to (or without) its dense
  * shards: a slot holds at most one dense, one sparse and one TF-IDF shard, and one group and one communicator serve all

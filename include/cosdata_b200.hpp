@@ -8,6 +8,7 @@
 //   finalize_ann_results                src/vector_store.rs:404-445
 // Nothing is computed here: every method is one call into libcosdata_b200.so.
 #pragma once
+#include <array>
 #include <cstdint>
 #include <stdexcept>
 #include <string>
@@ -312,6 +313,47 @@ class ShardGroup {
 
   private:
     cdb_shard_group *g_ = nullptr;
+};
+
+// the reference's TF-IDF index files (<collection>/tf_idf_index) as TFIDFIndexRoot::deserialize reads them
+class TfIdfFiles {
+  public:
+    explicit TfIdfFiles(const std::string &dir) { check(cdb_tfidf_files_open(dir.c_str(), &f_)); }
+    ~TfIdfFiles() { cdb_tfidf_files_close(f_); }
+    TfIdfFiles(const TfIdfFiles &) = delete;
+    TfIdfFiles &operator=(const TfIdfFiles &) = delete;
+    // {N, terms, records, live words, largest live id + 1, largest version}
+    std::array<uint64_t, 6> info() const {
+        std::array<uint64_t, 6> i{};
+        check(cdb_tfidf_files_info(f_, i.data()));
+        return i;
+    }
+    const cdb_tfidf_files *handle() const { return f_; }
+
+  private:
+    cdb_tfidf_files *f_ = nullptr;
+};
+
+// TFIDFIndex on one GPU (cdb_tfidf_index): row r has id id_base + r
+class TfIdfIndex {
+  public:
+    TfIdfIndex(uint64_t capacity_rows, uint64_t capacity_pairs, uint32_t id_base = 0, int32_t device = 0) {
+        cdb_tfidf_index_desc d{device, capacity_rows, capacity_pairs, id_base};
+        check(cdb_tfidf_index_create(&d, &ix_));
+    }
+    ~TfIdfIndex() { cdb_tfidf_index_destroy(ix_); }
+    TfIdfIndex(const TfIdfIndex &) = delete;
+    TfIdfIndex &operator=(const TfIdfIndex &) = delete;
+    uint64_t size() const { return cdb_tfidf_index_size(ix_); }
+    // the restart: the live words of rows [0, n_rows) from the files into this empty index; counted (n_rows flags, or
+    // null; live documents only) also counts rows without words; carry_stats false for every shard of a group but one
+    void load_files(const TfIdfFiles &files, uint64_t n_rows, const uint8_t *counted = nullptr, bool carry_stats = true) {
+        check(cdb_tfidf_index_load_files(ix_, files.handle(), n_rows, counted, carry_stats ? 1 : 0));
+    }
+    cdb_tfidf_index *handle() const { return ix_; }
+
+  private:
+    cdb_tfidf_index *ix_ = nullptr;
 };
 
 }  // namespace cosdata

@@ -10,6 +10,7 @@
 //!   hotpath_ref_v1.cdbf   quantize / dot_product_* / DistanceMetric::calculate / PerformantFixedSet results
 //!   prop.data             write_prop_value_to_file records (file_persist.rs:70-90)
 //!   itoe.dim, itoe.0.data TreeMap<InternalId, RawVectorEmbedding> (collection.rs:149-164)
+//!   tf_idf_index/         index-tree.dim and <version>.idat of a TFIDFIndexRoot (tf_idf_index.rs), 3 versions
 //! for the same inputs as tests/golden/make_golden.py.  tests/test_golden.py and the reader tests of
 //! cosdata-b200 pick the files up when present and compare them with the oracle, the committed
 //! golden vectors and the CUDA path.
@@ -31,6 +32,7 @@ use cosdata::models::dot_product::{
 };
 use cosdata::models::file_persist::{write_prop_metadata_to_file, write_prop_value_to_file};
 use cosdata::models::fixedset::PerformantFixedSet;
+use cosdata::models::tf_idf_index::TFIDFIndexRoot;
 use cosdata::models::tree_map::TreeMap;
 use cosdata::models::types::{DistanceMetric, InternalId, Metadata, VectorData, VectorId};
 use cosdata::models::versioning::VersionNumber;
@@ -348,4 +350,65 @@ fn dump_hot_path_fixtures() {
     }
     let _ = std::panic::take_hook();
     println!("fixtures written to {}", dir.display());
+}
+
+// ---------------------------------------------------------------- TF-IDF index files
+// tests/tfidf_files.py::reference_fixture_script restates this script; keep the two identical.
+fn tfidf_hashes() -> Vec<u32> {
+    let mut h = Vec::new();
+    for dim in [0u32, 1, 5, 21, 4096, 65535] {
+        for q in [0u32, 1, 2, 3, 4, 5, 0x7FFF, 0xFFFF] {
+            h.push(q << 16 | dim);
+        }
+    }
+    h
+}
+
+fn tfidf_doc(doc: u32, hashes: &[u32]) -> Vec<(u32, f32)> {
+    let mut pairs = Vec::new();
+    for (j, &h) in hashes.iter().enumerate() {
+        if (doc as usize + j) % 3 == 0 {
+            let tf = if (doc as usize + j) % 7 == 0 { -0.0f32 } else { ((doc as usize * 7 + j) % 13) as f32 * 0.25 };
+            pairs.push((h, tf));
+        }
+    }
+    pairs
+}
+
+#[test]
+fn dump_tfidf_fixtures() {
+    let dir = PathBuf::from(std::env::var("CDB_FIXTURE_DIR").expect("set CDB_FIXTURE_DIR")).join("tf_idf_index");
+    let _ = std::fs::remove_dir_all(&dir);
+    std::fs::create_dir_all(&dir).unwrap();
+    let work = std::env::temp_dir().join(format!("cdb_tfidf_fixture_{}", std::process::id()));
+    let _ = std::fs::remove_dir_all(&work);
+    std::fs::create_dir_all(&work).unwrap();
+    let hashes = tfidf_hashes();
+    let root = TFIDFIndexRoot::new(work.clone()).unwrap();
+    // (version, first document, end document, deleted documents): each version inserts, then deletes, then serializes
+    let script: [(u32, u32, u32, &[u32]); 3] = [(1, 0, 8, &[2]), (2, 8, 14, &[4, 9]), (3, 14, 18, &[10, 15, 0])];
+    for (v, d0, d1, deletes) in script {
+        let version = VersionNumber::from(v);
+        for doc in d0..d1 {
+            for (h, tf) in tfidf_doc(doc, &hashes) {
+                root.insert(h, tf, doc, version).unwrap();
+            }
+            root.total_documents_count.fetch_add(1, std::sync::atomic::Ordering::Relaxed);
+        }
+        for &doc in deletes {
+            for (h, _) in tfidf_doc(doc, &hashes) {
+                root.delete(h, doc, version).unwrap();
+            }
+            root.total_documents_count.fetch_sub(1, std::sync::atomic::Ordering::Relaxed);
+        }
+        root.serialize().unwrap();
+        root.cache.flush_all().unwrap();
+    }
+    drop(root);
+    for entry in std::fs::read_dir(&work).unwrap() {
+        let p = entry.unwrap().path();
+        std::fs::copy(&p, dir.join(p.file_name().unwrap())).unwrap();
+    }
+    let _ = std::fs::remove_dir_all(&work);
+    println!("tf_idf_index fixtures written to {}", dir.display());
 }
